@@ -48,7 +48,8 @@ SYMBOLS = ["balm_last_error", "balm_version", "balm_create", "balm_destroy", "ba
            "balm_default_lm_opts", "balm_comm_unique_id", "balm_comm_init", "balm_get_timings",
            "balm_reset_counters", "balm_sync", "balm_timer_begin", "balm_timer_end", "balm_device_views", "balm_debug_dag_trace", "balm_synth_virtual",
            "balm_download_voxels", "balm_download_voxel_range", "balm_num_obs", "balm_default_assoc_opts", "balm_cut_voxels", "balm_pose_covariance", "balm_marginalize", "balm_download_fix", "balm_append_scan",
-           "balm_download_keys"]
+           "balm_download_keys", "balm_window_reset", "balm_window_cut", "balm_window_recut", "balm_window_marginalize",
+           "balm_window_push"]
 
 
 def lib():
@@ -93,6 +94,11 @@ def lib():
         L.balm_append_scan.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int, C.POINTER(C.c_int64),
                                        C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
         L.balm_download_keys.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+        L.balm_window_reset.argtypes = [C.c_void_p, C.POINTER(AssocOpts)]
+        L.balm_window_cut.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int]
+        L.balm_window_recut.argtypes = [C.c_void_p, C.c_int]
+        L.balm_window_marginalize.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int]
+        L.balm_window_push.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
         _lib = L
     return _lib
 

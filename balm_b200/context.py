@@ -147,6 +147,34 @@ class Context:
         L.check(L.lib().balm_download_fix(self._h, _p(fix)))
         return fix
 
+    # ---- persistent sliding-window octree ----
+    def window_reset(self, voxel_size=2.0, layer_limit=2, min_ps=15, eigen_value_array=(1.0 / 16, 1.0 / 16, 1.0 / 9)):
+        """Empty window map (the reference's surf_map) with these association parameters."""
+        o = L.AssocOpts(float(voxel_size), int(layer_limit), int(min_ps), (C.c_double * 3)(*eigen_value_array))
+        L.check(L.lib().balm_window_reset(self._h, C.byref(o)))
+
+    def window_cut(self, xyz, pose12, slot):
+        """cut_voxel: a scan's body-frame points, at pose12, into window slot `slot`."""
+        xyz = np.ascontiguousarray(xyz, dtype=np.float32).reshape(-1, 3)
+        pose12 = np.ascontiguousarray(pose12, dtype=np.float64).reshape(12)
+        L.check(L.lib().balm_window_cut(self._h, len(xyz), _p(xyz), _p(pose12), int(slot)))
+
+    def window_recut(self, win_count):
+        """recut(win_count) on every root."""
+        L.check(L.lib().balm_window_recut(self._h, int(win_count)))
+
+    def window_marginalize(self, mg_size, poses12, win_count):
+        """marginalize(mg_size, x_poses, win_count) on every root; poses12: N x 12 (the window's optimised poses) or None."""
+        p = None if poses12 is None else np.ascontiguousarray(poses12, dtype=np.float64).reshape(self.N, 12)
+        L.check(L.lib().balm_window_marginalize(self._h, int(mg_size), _p(p), int(win_count)))
+
+    def window_push(self, win_count):
+        """tras_opt(win_count): registers the pushed nodes as the voxel set -> (n_voxels, n_obs)."""
+        M, K = C.c_int64(), C.c_int64()
+        L.check(L.lib().balm_window_push(self._h, int(win_count), C.byref(M), C.byref(K)))
+        self.M = M.value
+        return M.value, K.value
+
     def pose_covariance(self, poses12, point_noise=0.0, c_cov=None, include_fix=False, want_raw=True, want_cov=True):
         """left_jacobian_point / multi_second / H^-1 Rcov H^-T (BAs_left.hpp:342-473, 995-1023, 1089-1096).
         -> (Rcov_raw, Rcov); c_cov: K x 9 x 9 per-observation cluster covariances, or None for isotropic point noise."""

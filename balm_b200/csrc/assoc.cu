@@ -132,6 +132,16 @@ __global__ void node_flag_kernel(const unsigned long long *seg_key, int nseg, in
   const int s = blockIdx.x * blockDim.x + threadIdx.x;
   if (s < nseg) flag[s] = (s == 0 || seg_key[s] != seg_key[s - 1]) ? 1 : 0;
 }
+// judge_eigen (bavoxel.hpp:654-699) on a world-frame cluster: lambda0 / lambda1 of its covariance below the layer's
+// threshold (decision < eigen_value_array[layer], :665,697)
+__device__ __forceinline__ bool cluster_planar(const double *W, double eig_thr) {
+  const double inv = 1.0 / W[9];
+  const double c0 = W[6] * inv, c1 = W[7] * inv, c2 = W[8] * inv;
+  double lam[3], u0[3], u1[3], u2[3];
+  eig3_jacobi(W[0] * inv - c0 * c0, W[1] * inv - c0 * c1, W[2] * inv - c0 * c2, W[3] * inv - c1 * c1,
+              W[4] * inv - c1 * c2, W[5] * inv - c2 * c2, lam, u0, u1, u2);
+  return lam[0] / lam[1] < eig_thr;
+}
 // One thread per node: total world moments over its frames -> judge_eigen (bavoxel.hpp:654-699)
 __global__ void node_judge_kernel(const double *segW, const unsigned long long *seg_key, const int *node_start, int nnode,
                                   int nseg, double eig_thr, unsigned long long *node_key, int *node_size,
@@ -143,14 +153,9 @@ __global__ void node_judge_kernel(const double *segW, const unsigned long long *
   for (int s = a; s < b; s++)
 #pragma unroll
     for (int c = 0; c < 10; c++) W[c] += segW[(size_t)c * nseg + s];
-  const double inv = 1.0 / W[9];
-  const double c0 = W[6] * inv, c1 = W[7] * inv, c2 = W[8] * inv;
-  double lam[3], u0[3], u1[3], u2[3];
-  eig3_jacobi(W[0] * inv - c0 * c0, W[1] * inv - c0 * c1, W[2] * inv - c0 * c2, W[3] * inv - c1 * c1,
-              W[4] * inv - c1 * c2, W[5] * inv - c2 * c2, lam, u0, u1, u2);
   node_key[v] = seg_key[a];
   node_size[v] = (int)(W[9] + 0.5);
-  node_planar[v] = (lam[0] / lam[1] < eig_thr) ? 1 : 0;  // decision < eigen_value_array[layer]  (:665,697)
+  node_planar[v] = cluster_planar(W, eig_thr) ? 1 : 0;
   node_nframes[v] = b - a;
 }
 
@@ -817,4 +822,648 @@ int append_scan_build(balm_ctx *c, int64_t n, const float *xyz_h, const double *
   const bool any_fix = c->fix != nullptr;
   ATRY(reg(c, Mout, (const int64_t *)rp, pi, ob, any_fix ? fx : nullptr, co, Kout));
   return install_keys(c, keys_out, layers_out, Mout, true);
+}
+
+
+// ---------------------------------------------------------------------------------------------------------------------
+// The persistent sliding-window octree in HBM (SURVEY.md 8f row N2): the reference's surf_map of OCTO_TREE_ROOTs kept
+// across window shifts and driven by its four operations
+//   cut_voxel                                    bavoxel.hpp:1170-1223
+//   OCTO_TREE_NODE::recut / judge_eigen / cut_func                :737-776, 654-699, 700-735
+//   OCTO_TREE_ROOT::marginalize -> OCTO_TREE_NODE::to_margi       :948-963, 778-816
+//   OCTO_TREE_NODE::tras_opt -> VOX_HESS::push_voxel              :908-929, 30-51
+// State (all device arrays, grown by doubling, nothing is ever deleted from the node table):
+//   node table, append-only (a node's id never changes): 63-bit key, layer, split flag (octo_state), push_state,
+//     fix_point [10], and per window slot the clusters sig_orig / sig_tran [N][10]. A per-layer table of (key, id)
+//     sorted by key finds a node (a key digit 7 is both "not split" and octant 7, so keys are only unique per layer).
+//   point store: body xyz (vec_orig, float as given), world xyz (vec_tran, fp64), slot, node id and an order stamp.
+//     The stamp orders the points of one (node, slot) list as the reference's vector holds them: a cut stamps
+//     (op << 32 | input index), a move into a child restamps the moved points (op << 32 | rank in stamp order), so
+//     they land after the child's earlier points and keep their parent's order.
+// Clusters are accumulated point by point in that order, exactly as PointCluster::push runs, so sums of the device
+// and of the reference round alike. Split nodes keep whatever points are left in them (slots the recut did not move);
+// nothing reads them unless a later recut(win_count) with win_count - 1 == that slot moves them, as in the reference.
+namespace {
+struct WinLookup {
+  int n = 0;
+  unsigned long long *key = nullptr;
+  int *id = nullptr;
+};
+}  // namespace
+
+struct WindowState {
+  AssocParams P;
+  int N = 0;
+  unsigned long long op = 1;  // stamp counter
+  // nodes
+  int nn = 0, ncap = 0;
+  unsigned long long *nkey = nullptr;
+  int *nlayer = nullptr, *nsplit = nullptr, *npush = nullptr, *naction = nullptr;
+  double *nfix = nullptr;          // [ncap][10]
+  double *sig_o = nullptr, *sig_t = nullptr;  // [ncap][N][10]
+  WinLookup look[3];
+  // points
+  int64_t np = 0, pcap = 0;
+  float *pxyz = nullptr;
+  double *ptran = nullptr;
+  int *pslot = nullptr, *pnode = nullptr;
+  unsigned long long *pstamp = nullptr;
+  ~WindowState() {
+    void *ps[] = {nkey, nlayer, nsplit, npush, naction, nfix, sig_o, sig_t, pxyz, ptran, pslot, pnode, pstamp,
+                  look[0].key, look[0].id, look[1].key, look[1].id, look[2].key, look[2].id};
+    for (void *q : ps) cudaFree(q);
+  }
+};
+
+namespace {
+template <typename T>
+int grow_array(T **p, size_t used, size_t cap) {  // new buffer of `cap` elements holding the first `used` ones
+  T *q = nullptr;
+  CUDA_TRY(cudaMalloc((void **)&q, sizeof(T) * (cap ? cap : 1)));
+  if (used) {
+    const cudaError_t e = cudaMemcpy(q, *p, sizeof(T) * used, cudaMemcpyDeviceToDevice);
+    if (e != cudaSuccess) { cudaFree(q); CUDA_TRY(e); }
+  }
+  cudaFree(*p);
+  *p = q;
+  return BALM_OK;
+}
+
+int win_reserve_nodes(WindowState &w, int need) {
+  if (need <= w.ncap) return BALM_OK;
+  int cap = std::max(need, std::max(1024, 2 * w.ncap));
+  const size_t nn = (size_t)w.nn, c = (size_t)cap, NS = (size_t)w.N * 10;
+  ATRY(grow_array(&w.nkey, nn, c)); ATRY(grow_array(&w.nlayer, nn, c)); ATRY(grow_array(&w.nsplit, nn, c));
+  ATRY(grow_array(&w.npush, nn, c)); ATRY(grow_array(&w.naction, nn, c)); ATRY(grow_array(&w.nfix, nn * 10, c * 10));
+  ATRY(grow_array(&w.sig_o, nn * NS, c * NS)); ATRY(grow_array(&w.sig_t, nn * NS, c * NS));
+  w.ncap = cap;
+  return BALM_OK;
+}
+int win_reserve_points(WindowState &w, int64_t need) {
+  if (need <= w.pcap) return BALM_OK;
+  if (need >= (1ll << 31)) { balm_set_error("balm_window_cut: more than 2^31 points in the window"); return BALM_ERR_UNSUPPORTED; }
+  int64_t cap = std::max<int64_t>(need, std::max<int64_t>(1 << 16, 2 * w.pcap));
+  cap = std::min<int64_t>(cap, (1ll << 31) - 1);
+  const size_t n = (size_t)w.np, c = (size_t)cap;
+  ATRY(grow_array(&w.pxyz, 3 * n, 3 * c)); ATRY(grow_array(&w.ptran, 3 * n, 3 * c)); ATRY(grow_array(&w.pslot, n, c));
+  ATRY(grow_array(&w.pnode, n, c)); ATRY(grow_array(&w.pstamp, n, c));
+  w.pcap = cap;
+  return BALM_OK;
+}
+
+// cub temporary storage from the pool
+struct CubTmp {
+  ScratchPool &pool;
+  char *p = nullptr;
+  size_t bytes = 0;
+  int need(size_t b) {
+    if (b <= bytes) return BALM_OK;
+    pool.drop(p);
+    p = nullptr;
+    bytes = b;
+    return pool.get(&p, bytes);
+  }
+};
+
+__global__ void win_iota_kernel(int *v, int64_t n, int base) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) v[i] = base + (int)i;
+}
+__global__ void win_missing_kernel(const unsigned long long *keys, int m, const unsigned long long *look, int nlook,
+                                   int *miss) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < m) miss[i] = find_key(look, nlook, keys[i]) < 0 ? 1 : 0;
+}
+__global__ void win_init_nodes_kernel(const unsigned long long *keys, int m, int base, int layer, unsigned long long *nkey,
+                                      int *nlayer, int *nsplit, int *npush, double *nfix) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= m) return;
+  const int v = base + i;
+  nkey[v] = keys[i]; nlayer[v] = layer; nsplit[v] = 0; npush[v] = 0;
+#pragma unroll
+  for (int q = 0; q < 10; q++) nfix[(size_t)v * 10 + q] = 0.0;
+}
+// node id of every key (the key is in the layer's table)
+__global__ void win_find_kernel(const unsigned long long *keys, const int *sel, int m, const unsigned long long *look,
+                                const int *look_id, int nlook, int *node_out /*indexed by sel[i] or i*/) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= m) return;
+  node_out[sel ? sel[i] : i] = look_id[find_key(look, nlook, keys[i])];
+}
+
+// the layer-L nodes that `keys` (m keys, any order, duplicates allowed) name and that do not exist yet are appended to
+// the node table in ascending key order, and the layer's lookup table is rebuilt
+int win_add_nodes(WindowState &w, ScratchPool &pool, CubTmp &tmp, cudaStream_t st, const unsigned long long *keys, int m,
+                  int L) {
+  if (m < 1) return BALM_OK;
+  WinLookup &lk = w.look[L];
+  int *miss = nullptr, *nsel = nullptr;
+  unsigned long long *sel = nullptr, *sorted = nullptr, *uniq = nullptr;
+  ATRY(pool.get(&miss, m)); ATRY(pool.get(&nsel, 1)); ATRY(pool.get(&sel, m)); ATRY(pool.get(&sorted, m)); ATRY(pool.get(&uniq, m));
+  win_missing_kernel<<<(m + 255) / 256, 256, 0, st>>>(keys, m, lk.key, lk.n, miss);
+  size_t b1 = 0, b2 = 0, b3 = 0;
+  cub::DeviceSelect::Flagged(nullptr, b1, keys, miss, sel, nsel, m, st);
+  cub::DeviceRadixSort::SortKeys(nullptr, b2, sel, sorted, m, 0, 64, st);
+  cub::DeviceSelect::Unique(nullptr, b3, sorted, uniq, nsel, m, st);
+  ATRY(tmp.need(std::max(b1, std::max(b2, b3))));
+  CUDA_TRY(cub::DeviceSelect::Flagged(tmp.p, tmp.bytes, keys, miss, sel, nsel, m, st));
+  int nmiss = 0;
+  CUDA_TRY(cudaMemcpyAsync(&nmiss, nsel, sizeof(int), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  if (nmiss == 0) return BALM_OK;
+  CUDA_TRY(cub::DeviceRadixSort::SortKeys(tmp.p, tmp.bytes, sel, sorted, nmiss, 0, 64, st));
+  CUDA_TRY(cub::DeviceSelect::Unique(tmp.p, tmp.bytes, sorted, uniq, nsel, nmiss, st));
+  int nnew = 0;
+  CUDA_TRY(cudaMemcpyAsync(&nnew, nsel, sizeof(int), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  if ((int64_t)w.nn + nnew >= (1ll << 31) / std::max(1, 10 * w.N)) {
+    balm_set_error("balm_window: node table too large");
+    return BALM_ERR_UNSUPPORTED;
+  }
+  ATRY(win_reserve_nodes(w, w.nn + nnew));
+  const int base = w.nn;
+  win_init_nodes_kernel<<<(nnew + 255) / 256, 256, 0, st>>>(uniq, nnew, base, L, w.nkey, w.nlayer, w.nsplit, w.npush, w.nfix);
+  CUDA_TRY(cudaMemsetAsync(w.sig_o + (size_t)base * w.N * 10, 0, sizeof(double) * (size_t)nnew * w.N * 10, st));
+  CUDA_TRY(cudaMemsetAsync(w.sig_t + (size_t)base * w.N * 10, 0, sizeof(double) * (size_t)nnew * w.N * 10, st));
+  // lookup: old (key, id) pairs + the new ones, sorted by key
+  const int nl = lk.n + nnew;
+  unsigned long long *k_in = nullptr, *k_out = nullptr;
+  int *i_in = nullptr, *i_out = nullptr;
+  ATRY(pool.get(&k_in, nl)); ATRY(pool.get(&i_in, nl));
+  CUDA_TRY(cudaMalloc((void **)&k_out, sizeof(unsigned long long) * nl));
+  if (cudaMalloc((void **)&i_out, sizeof(int) * nl) != cudaSuccess) { cudaFree(k_out); CUDA_TRY(cudaErrorMemoryAllocation); }
+  if (lk.n) {
+    CUDA_TRY(cudaMemcpyAsync(k_in, lk.key, sizeof(unsigned long long) * lk.n, cudaMemcpyDeviceToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(i_in, lk.id, sizeof(int) * lk.n, cudaMemcpyDeviceToDevice, st));
+  }
+  CUDA_TRY(cudaMemcpyAsync(k_in + lk.n, uniq, sizeof(unsigned long long) * nnew, cudaMemcpyDeviceToDevice, st));
+  win_iota_kernel<<<(nnew + 255) / 256, 256, 0, st>>>(i_in + lk.n, nnew, base);
+  size_t b4 = 0;
+  cub::DeviceRadixSort::SortPairs(nullptr, b4, k_in, k_out, i_in, i_out, nl, 0, 64, st);
+  ATRY(tmp.need(b4));
+  CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp.p, tmp.bytes, k_in, k_out, i_in, i_out, nl, 0, 64, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  cudaFree(lk.key);
+  cudaFree(lk.id);
+  lk.key = k_out; lk.id = i_out; lk.n = nl;
+  w.nn += nnew;
+  return BALM_OK;
+}
+
+// One thread per (node, slot) segment of points given in push order: sig_orig / sig_tran .push of every point, in order
+// (PointCluster::push, tools.hpp:311-316), on top of what the node already holds.
+__global__ void win_push_kernel(const int *order, const int *seg_start, int nseg, int m, const float *pxyz,
+                                const double *ptran, const int *pnode, const int *pslot, int N, double *sig_o,
+                                double *sig_t) {
+  const int s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= nseg) return;
+  const int a = seg_start[s], b = (s + 1 < nseg) ? seg_start[s + 1] : m;
+  const int j0 = order[a];
+  double *so = sig_o + ((size_t)pnode[j0] * N + pslot[j0]) * 10;
+  double *stt = sig_t + ((size_t)pnode[j0] * N + pslot[j0]) * 10;
+  double B[10], W[10];
+#pragma unroll
+  for (int q = 0; q < 10; q++) { B[q] = so[q]; W[q] = stt[q]; }
+  for (int i = a; i < b; i++) {
+    const int j = order[i];
+    const double x = pxyz[3 * j], y = pxyz[3 * j + 1], z = pxyz[3 * j + 2];
+    B[0] += x * x; B[1] += x * y; B[2] += x * z; B[3] += y * y; B[4] += y * z; B[5] += z * z;
+    B[6] += x; B[7] += y; B[8] += z; B[9] += 1.0;
+    const double wx = ptran[3 * j], wy = ptran[3 * j + 1], wz = ptran[3 * j + 2];
+    W[0] += wx * wx; W[1] += wx * wy; W[2] += wx * wz; W[3] += wy * wy; W[4] += wy * wz; W[5] += wz * wz;
+    W[6] += wx; W[7] += wy; W[8] += wz; W[9] += 1.0;
+  }
+#pragma unroll
+  for (int q = 0; q < 10; q++) { so[q] = B[q]; stt[q] = W[q]; }
+}
+__global__ void win_seg_key_kernel(const int *order, int m, const int *pnode, const int *pslot, int N,
+                                   unsigned long long *ck) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < m) ck[i] = (unsigned long long)pnode[order[i]] * (unsigned long long)N + (unsigned long long)pslot[order[i]];
+}
+__global__ void win_seg_flag_kernel(const unsigned long long *ck, int m, int *flag) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < m) flag[i] = (i == 0 || ck[i] != ck[i - 1]) ? 1 : 0;
+}
+
+// pushes the m points `order` (point ids, in push order) into the clusters of their (node, slot)
+int win_push_points(WindowState &w, ScratchPool &pool, CubTmp &tmp, cudaStream_t st, const int *order, int m) {
+  if (m < 1) return BALM_OK;
+  unsigned long long *ck = nullptr, *ck2 = nullptr;
+  int *ord2 = nullptr, *flag = nullptr, *iota = nullptr, *seg = nullptr, *nsel = nullptr;
+  ATRY(pool.get(&ck, m)); ATRY(pool.get(&ck2, m)); ATRY(pool.get(&ord2, m)); ATRY(pool.get(&flag, m));
+  ATRY(pool.get(&iota, m)); ATRY(pool.get(&seg, m)); ATRY(pool.get(&nsel, 1));
+  const unsigned g = (unsigned)((m + 255) / 256);
+  win_seg_key_kernel<<<g, 256, 0, st>>>(order, m, w.pnode, w.pslot, w.N, ck);
+  int bits = 1;
+  while (bits < 64 && ((unsigned long long)w.nn * (unsigned long long)w.N) >> bits) bits++;
+  size_t b1 = 0, b2 = 0;
+  cub::DeviceRadixSort::SortPairs(nullptr, b1, ck, ck2, order, ord2, m, 0, bits, st);
+  cub::DeviceSelect::Flagged(nullptr, b2, iota, flag, seg, nsel, m, st);
+  ATRY(tmp.need(std::max(b1, b2)));
+  CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp.p, tmp.bytes, ck, ck2, order, ord2, m, 0, bits, st));  // stable
+  win_seg_flag_kernel<<<g, 256, 0, st>>>(ck2, m, flag);
+  win_iota_kernel<<<g, 256, 0, st>>>(iota, m, 0);
+  CUDA_TRY(cub::DeviceSelect::Flagged(tmp.p, tmp.bytes, iota, flag, seg, nsel, m, st));
+  int nseg = 0;
+  CUDA_TRY(cudaMemcpyAsync(&nseg, nsel, sizeof(int), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  win_push_kernel<<<(nseg + 127) / 128, 128, 0, st>>>(ord2, seg, nseg, m, w.pxyz, w.ptran, w.pnode, w.pslot, w.N, w.sig_o,
+                                                      w.sig_t);
+  CUDA_TRY(cudaGetLastError());
+  return BALM_OK;
+}
+
+// cut_voxel: world coordinate R p + t (fp64) and root key of every point of the scan
+__global__ void win_cut_kernel(const float *xyz, const double *pose12, int n, AssocParams p, double *tran,
+                               unsigned long long *rkey, int *bad) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  double r[9], t[3];
+  load_pose(pose12, r, t);
+  const double b[3] = {(double)xyz[3 * i], (double)xyz[3 * i + 1], (double)xyz[3 * i + 2]};
+  double wp[3];
+#pragma unroll
+  for (int a = 0; a < 3; a++) wp[a] = r[a * 3] * b[0] + r[a * 3 + 1] * b[1] + r[a * 3 + 2] * b[2] + t[a];
+#pragma unroll
+  for (int a = 0; a < 3; a++) tran[3 * i + a] = wp[a];
+  rkey[i] = world_point_key(wp, p, bad) | 63ull;
+}
+__global__ void win_stamp_kernel(int *pslot, unsigned long long *pstamp, int n, int slot, unsigned long long op) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  pslot[i] = slot;
+  pstamp[i] = (op << 32) | (unsigned long long)i;
+}
+
+// recut, one layer: judge every node of layer L that is not split (recut :739-768); 1 = split earlier (only slot
+// win_count-1 moves, :770), 2 = split now (every slot < win_count moves, :766-767), 0 = no points move
+__global__ void win_judge_kernel(int nn, int L, int N, int w, AssocParams p, const int *nlayer, int *nsplit, int *npush,
+                                 const double *nfix, const double *sig_o, const double *sig_t, int *action) {
+  const int v = blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= nn || nlayer[v] != L) return;
+  if (nsplit[v]) { action[v] = 1; return; }
+  action[v] = 0;
+  npush[v] = 0;
+  const double *f = nfix + (size_t)v * 10;
+  double ps = f[9];
+  for (int i = 0; i < w; i++) ps += sig_o[((size_t)v * N + i) * 10 + 9];
+  if ((int)ps <= p.min_ps) return;                                     // point_size <= min_ps (:748)
+  double W[10];
+#pragma unroll
+  for (int q = 0; q < 10; q++) W[q] = f[q];
+  for (int i = 0; i < w; i++)                                          // covMat = fix_point + sum sig_tran (:656-658)
+#pragma unroll
+    for (int q = 0; q < 10; q++) W[q] += sig_t[((size_t)v * N + i) * 10 + q];
+  if (cluster_planar(W, p.eig[L])) {
+    npush[v] = ((int)(ps - f[9]) > p.min_ps) ? 1 : 0;                  // :752-757
+    return;
+  }
+  if (L == p.layer_limit) return;                                      // :759-760
+  nsplit[v] = 1;
+  action[v] = 2;
+}
+// cut_func: the octant of every moving point around its node's float centre, and the child's key
+__global__ void win_move_kernel(int64_t np, int w, AssocParams p, const int *pnode, const int *pslot, const double *ptran,
+                                const int *action, const unsigned long long *nkey, const int *nlayer,
+                                unsigned long long *ckey, int *flag) {
+  const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= np) return;
+  const int v = pnode[j], a = action[v], s = pslot[j];
+  const bool mv = (a == 2 && s < w) || (a == 1 && s == w - 1);
+  flag[j] = mv ? 1 : 0;
+  if (!mv) return;
+  const unsigned long long k = nkey[v];
+  const int L = nlayer[v];
+  const float quater = (float)(p.voxel_size / 4.0);
+  int oct = 0;
+#pragma unroll
+  for (int ax = 0; ax < 3; ax++) {
+    const long long idx = (long long)((k >> (6 + ROOT_BITS * (2 - ax))) & ((1ull << ROOT_BITS) - 1)) - ROOT_BIAS;
+    float c = (float)((0.5 + (double)idx) * p.voxel_size);             // root centre (:1213-1215)
+    if (L == 1) c = c + (float)(2 * (int)((k >> (3 + 2 - ax)) & 1) - 1) * quater;  // child centre (:717-719)
+    oct = (oct << 1) | (ptran[3 * j + ax] > (double)c ? 1 : 0);        // :709-712
+  }
+  ckey[j] = L == 0 ? ((k & ~63ull) | ((unsigned long long)oct << 3) | 7ull) : ((k & ~7ull) | (unsigned long long)oct);
+}
+__global__ void win_gather_u64_kernel(const unsigned long long *src, const int *idx, int m, unsigned long long *dst) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < m) dst[i] = src[idx[i]];
+}
+__global__ void win_restamp_kernel(const int *order, int m, unsigned long long op, unsigned long long *pstamp) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < m) pstamp[order[i]] = (op << 32) | (unsigned long long)i;
+}
+
+// to_margi (:778-816) on every node that is not split
+__global__ void win_margi_node_kernel(int nn, int N, int mg, int w, const double *poses, const int *nsplit,
+                                      const int *npush, double *nfix, double *sig_o, double *sig_t) {
+  const int v = blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= nn || nsplit[v]) return;
+  double *so = sig_o + (size_t)v * N * 10, *stt = sig_t + (size_t)v * N * 10;
+  if (poses)
+    for (int i = 0; i < w; i++) {                                      // sig_tran[i].transform(sig_orig[i], x_poses[i])
+      double r[9], t[3];
+      load_pose(poses + 12 * i, r, t);
+      const WC c = world_cluster(so + i * 10, r, t);
+      double *d = stt + i * 10;
+      d[0] = c.p00; d[1] = c.p01; d[2] = c.p02; d[3] = c.p11; d[4] = c.p12; d[5] = c.p22;
+      d[6] = c.v0; d[7] = c.v1; d[8] = c.v2; d[9] = c.n;
+    }
+  double *f = nfix + (size_t)v * 10;
+  if (f[9] < 50 && npush[v] == 1)                                      // :790-795
+    for (int i = 0; i < mg; i++)
+#pragma unroll
+      for (int q = 0; q < 10; q++) f[q] += stt[i * 10 + q];
+  for (int i = mg; i < w; i++)                                         // :797-803
+    for (int q = 0; q < 10; q++) { so[(i - mg) * 10 + q] = so[i * 10 + q]; stt[(i - mg) * 10 + q] = stt[i * 10 + q]; }
+  for (int i = w - mg; i < w; i++)                                     // :805-811
+    for (int q = 0; q < 10; q++) { so[i * 10 + q] = 0.0; stt[i * 10 + q] = 0.0; }
+}
+// ... and on their points: re-transform (plvec_trans), drop the retired slots, shift the rest
+__global__ void win_margi_point_kernel(int64_t np, int mg, int w, const double *poses, const int *nsplit, const int *pnode,
+                                       int *pslot, const float *pxyz, double *ptran, int *keep) {
+  const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= np) return;
+  const int s = pslot[j];
+  if (nsplit[pnode[j]] || s >= w) { keep[j] = 1; return; }
+  if (poses) {
+    double r[9], t[3];
+    load_pose(poses + 12 * s, r, t);
+    const double b[3] = {(double)pxyz[3 * j], (double)pxyz[3 * j + 1], (double)pxyz[3 * j + 2]};
+#pragma unroll
+    for (int a = 0; a < 3; a++) ptran[3 * j + a] = r[a * 3] * b[0] + r[a * 3 + 1] * b[1] + r[a * 3 + 2] * b[2] + t[a];
+  }
+  keep[j] = s >= mg ? 1 : 0;
+  if (s >= mg) pslot[j] = s - mg;
+}
+__global__ void win_compact_kernel(const int *sel, int m, const float *xyz, const double *tran, const int *slot,
+                                   const int *node, const unsigned long long *stamp, float *xyz2, double *tran2,
+                                   int *slot2, int *node2, unsigned long long *stamp2) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= m) return;
+  const int j = sel[i];
+#pragma unroll
+  for (int a = 0; a < 3; a++) { xyz2[3 * i + a] = xyz[3 * j + a]; tran2[3 * i + a] = tran[3 * j + a]; }
+  slot2[i] = slot[j]; node2[i] = node[j]; stamp2[i] = stamp[j];
+}
+
+// tras_opt (:908-929) + push_voxel (:30-51)
+__global__ void win_push_flag_kernel(int nn, int N, int w, int min_ps, const int *nsplit, const int *npush,
+                                     const double *sig_o, int *flag) {
+  const int v = blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= nn) return;
+  flag[v] = 0;
+  if (nsplit[v] || npush[v] != 1) return;
+  double pts = 0;
+  for (int i = 0; i < w; i++) pts += sig_o[((size_t)v * N + i) * 10 + 9];
+  if ((int)pts < min_ps) return;
+  int k = 0;
+  for (int i = 0; i < N; i++) k += sig_o[((size_t)v * N + i) * 10 + 9] != 0.0 ? 1 : 0;
+  flag[v] = k >= 2 ? 1 : 0;
+}
+__global__ void win_obs_count_kernel(const int *ids, int M, int N, const double *sig_o, int *cnt) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= M) return;
+  int k = 0;
+  for (int s = 0; s < N; s++) k += sig_o[((size_t)ids[i] * N + s) * 10 + 9] != 0.0 ? 1 : 0;
+  cnt[i] = k;
+}
+__global__ void win_emit_kernel(const int *ids, const int *ostart, int M, int64_t K, int N, const double *sig_o,
+                                const double *nfix, const unsigned long long *nkey, const int *nlayer, long long *row_ptr,
+                                int *pose_idx, double *obs10, double *fix10, double *coe, unsigned long long *key_out,
+                                int *layer_out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i == 0) row_ptr[M] = K;
+  if (i >= M) return;
+  const int v = ids[i];
+  long long o = ostart[i];
+  row_ptr[i] = o;
+  double pts = 0;
+  for (int s = 0; s < N; s++) {
+    const double *c = sig_o + ((size_t)v * N + s) * 10;
+    if (c[9] == 0.0) continue;
+    for (int q = 0; q < 10; q++) obs10[o * 10 + q] = c[q];
+    pose_idx[o] = s;
+    pts += c[9];
+    o++;
+  }
+  for (int q = 0; q < 10; q++) fix10[(size_t)i * 10 + q] = nfix[(size_t)v * 10 + q];
+  coe[i] = pts;                                                        // coe = sum of N (:42-44)
+  key_out[i] = nkey[v];
+  layer_out[i] = nlayer[v];
+}
+}  // namespace
+
+void window_free(WindowState *w) { delete w; }
+
+int window_reset_build(balm_ctx *c, WindowState **ws, double voxel_size, int layer_limit, int min_ps, const double *eig3) {
+  if (layer_limit < 0 || layer_limit > 2) { balm_set_error("balm_window_reset: layer_limit must be in 0..2"); return BALM_ERR_INVALID; }
+  WindowState *w = new WindowState();
+  w->P = AssocParams{voxel_size, layer_limit, min_ps, {eig3[0], eig3[1], eig3[2]}};
+  w->N = c->N;
+  delete *ws;
+  *ws = w;
+  return BALM_OK;
+}
+
+int window_cut_build(balm_ctx *c, WindowState &w, int64_t n, const float *xyz_h, const double *pose12_h, int slot) {
+  if (n == 0) return BALM_OK;
+  if (n < 0 || w.np + n >= (1ll << 31)) { balm_set_error("balm_window_cut: bad point count (the window holds < 2^31 points)"); return BALM_ERR_INVALID; }
+  cudaStream_t st = c->stream;
+  ScratchPool pool;
+  CubTmp tmp{pool};
+  const int m = (int)n;
+  float *xyz = nullptr;
+  double *pose = nullptr, *tran = nullptr;
+  unsigned long long *rkey = nullptr;
+  int *bad = nullptr, *order = nullptr;
+  ATRY(pool.get(&xyz, 3 * (size_t)m)); ATRY(pool.get(&pose, 12)); ATRY(pool.get(&tran, 3 * (size_t)m));
+  ATRY(pool.get(&rkey, m)); ATRY(pool.get(&bad, 1)); ATRY(pool.get(&order, m));
+  CUDA_TRY(cudaMemcpyAsync(xyz, xyz_h, sizeof(float) * 3 * m, cudaMemcpyHostToDevice, st));
+  CUDA_TRY(cudaMemcpyAsync(pose, pose12_h, sizeof(double) * 12, cudaMemcpyHostToDevice, st));
+  CUDA_TRY(cudaMemsetAsync(bad, 0, sizeof(int), st));
+  const unsigned g = (unsigned)((m + 255) / 256);
+  win_cut_kernel<<<g, 256, 0, st>>>(xyz, pose, m, w.P, tran, rkey, bad);
+  int h_bad = 0;
+  CUDA_TRY(cudaMemcpyAsync(&h_bad, bad, sizeof(int), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  if (h_bad) { balm_set_error("balm_window_cut: a point lies outside the +-2^18 root-voxel range"); return BALM_ERR_INVALID; }
+  // nothing was changed so far; from here on the scan is committed
+  ATRY(win_add_nodes(w, pool, tmp, st, rkey, m, 0));
+  ATRY(win_reserve_points(w, w.np + m));
+  const int64_t b = w.np;
+  CUDA_TRY(cudaMemcpyAsync(w.pxyz + 3 * b, xyz, sizeof(float) * 3 * m, cudaMemcpyDeviceToDevice, st));
+  CUDA_TRY(cudaMemcpyAsync(w.ptran + 3 * b, tran, sizeof(double) * 3 * m, cudaMemcpyDeviceToDevice, st));
+  win_stamp_kernel<<<g, 256, 0, st>>>(w.pslot + b, w.pstamp + b, m, slot, w.op++);
+  win_find_kernel<<<g, 256, 0, st>>>(rkey, nullptr, m, w.look[0].key, w.look[0].id, w.look[0].n, w.pnode + b);
+  win_iota_kernel<<<g, 256, 0, st>>>(order, m, (int)b);
+  w.np += m;
+  ATRY(win_push_points(w, pool, tmp, st, order, m));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  c->launches += 10;
+  return BALM_OK;
+}
+
+int window_recut_build(balm_ctx *c, WindowState &w, int win_count) {
+  cudaStream_t st = c->stream;
+  for (int L = 0; L <= w.P.layer_limit; L++) {
+    ScratchPool pool;
+    CubTmp tmp{pool};
+    if (w.nn == 0) return BALM_OK;
+    CUDA_TRY(cudaMemsetAsync(w.naction, 0, sizeof(int) * w.nn, st));
+    win_judge_kernel<<<(w.nn + 127) / 128, 128, 0, st>>>(w.nn, L, w.N, win_count, w.P, w.nlayer, w.nsplit, w.npush, w.nfix,
+                                                         w.sig_o, w.sig_t, w.naction);
+    c->launches += 1;
+    if (L == w.P.layer_limit || w.np == 0) break;
+    const int np = (int)w.np;
+    unsigned long long *ckey = nullptr, *mkey = nullptr, *stamp = nullptr, *stamp2 = nullptr;
+    int *flag = nullptr, *iota = nullptr, *mv = nullptr, *mv2 = nullptr, *nsel = nullptr;
+    ATRY(pool.get(&ckey, np)); ATRY(pool.get(&flag, np)); ATRY(pool.get(&iota, np)); ATRY(pool.get(&mv, np));
+    ATRY(pool.get(&nsel, 1));
+    const unsigned g = (unsigned)((np + 255) / 256);
+    win_move_kernel<<<g, 256, 0, st>>>(w.np, win_count, w.P, w.pnode, w.pslot, w.ptran, w.naction, w.nkey, w.nlayer, ckey, flag);
+    win_iota_kernel<<<g, 256, 0, st>>>(iota, np, 0);
+    size_t b1 = 0;
+    cub::DeviceSelect::Flagged(nullptr, b1, iota, flag, mv, nsel, np, st);
+    ATRY(tmp.need(b1));
+    CUDA_TRY(cub::DeviceSelect::Flagged(tmp.p, tmp.bytes, iota, flag, mv, nsel, np, st));
+    int m = 0;
+    CUDA_TRY(cudaMemcpyAsync(&m, nsel, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    c->launches += 3;
+    if (m == 0) continue;
+    ATRY(pool.get(&mkey, m)); ATRY(pool.get(&stamp, m)); ATRY(pool.get(&stamp2, m)); ATRY(pool.get(&mv2, m));
+    const unsigned gm = (unsigned)((m + 255) / 256);
+    win_gather_u64_kernel<<<gm, 256, 0, st>>>(ckey, mv, m, mkey);
+    ATRY(win_add_nodes(w, pool, tmp, st, mkey, m, L + 1));              // children created on first use (:714-720)
+    win_find_kernel<<<gm, 256, 0, st>>>(mkey, mv, m, w.look[L + 1].key, w.look[L + 1].id, w.look[L + 1].n, w.pnode);
+    // the moved points in the order the parents' lists hold them, appended after the children's earlier points
+    win_gather_u64_kernel<<<gm, 256, 0, st>>>(w.pstamp, mv, m, stamp);
+    size_t b2 = 0;
+    cub::DeviceRadixSort::SortPairs(nullptr, b2, stamp, stamp2, mv, mv2, m, 0, 64, st);
+    ATRY(tmp.need(b2));
+    CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp.p, tmp.bytes, stamp, stamp2, mv, mv2, m, 0, 64, st));
+    win_restamp_kernel<<<gm, 256, 0, st>>>(mv2, m, w.op++, w.pstamp);
+    ATRY(win_push_points(w, pool, tmp, st, mv2, m));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    c->launches += 9;
+  }
+  CUDA_TRY(cudaStreamSynchronize(st));
+  CUDA_TRY(cudaGetLastError());
+  return BALM_OK;
+}
+
+int window_marginalize_build(balm_ctx *c, WindowState &w, int mg, const double *poses_h, int win_count) {
+  cudaStream_t st = c->stream;
+  ScratchPool pool;
+  CubTmp tmp{pool};
+  double *poses = nullptr;
+  if (poses_h) {
+    ATRY(pool.get(&poses, 12 * (size_t)w.N));
+    CUDA_TRY(cudaMemcpyAsync(poses, poses_h, sizeof(double) * 12 * w.N, cudaMemcpyHostToDevice, st));
+  }
+  if (w.nn == 0) return BALM_OK;
+  // the points first: they read the node's split flag only, and the slot before the shift
+  if (w.np > 0) {
+    const int np = (int)w.np;
+    int *keep = nullptr, *iota = nullptr, *sel = nullptr, *nsel = nullptr;
+    ATRY(pool.get(&keep, np)); ATRY(pool.get(&iota, np)); ATRY(pool.get(&sel, np)); ATRY(pool.get(&nsel, 1));
+    const unsigned g = (unsigned)((np + 255) / 256);
+    win_margi_point_kernel<<<g, 256, 0, st>>>(w.np, mg, win_count, poses, w.nsplit, w.pnode, w.pslot, w.pxyz, w.ptran, keep);
+    win_iota_kernel<<<g, 256, 0, st>>>(iota, np, 0);
+    size_t b1 = 0;
+    cub::DeviceSelect::Flagged(nullptr, b1, iota, keep, sel, nsel, np, st);
+    ATRY(tmp.need(b1));
+    CUDA_TRY(cub::DeviceSelect::Flagged(tmp.p, tmp.bytes, iota, keep, sel, nsel, np, st));
+    int m = 0;
+    CUDA_TRY(cudaMemcpyAsync(&m, nsel, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    if (m < np) {  // compact the point store (same capacity, order kept)
+      float *xyz2 = nullptr;
+      double *tran2 = nullptr;
+      int *slot2 = nullptr, *node2 = nullptr;
+      unsigned long long *stamp2 = nullptr;
+      const size_t cap = (size_t)w.pcap;
+      CUDA_TRY(cudaMalloc((void **)&xyz2, sizeof(float) * 3 * cap));
+      CUDA_TRY(cudaMalloc((void **)&tran2, sizeof(double) * 3 * cap));
+      CUDA_TRY(cudaMalloc((void **)&slot2, sizeof(int) * cap));
+      CUDA_TRY(cudaMalloc((void **)&node2, sizeof(int) * cap));
+      CUDA_TRY(cudaMalloc((void **)&stamp2, sizeof(unsigned long long) * cap));
+      if (m > 0)
+        win_compact_kernel<<<(m + 255) / 256, 256, 0, st>>>(sel, m, w.pxyz, w.ptran, w.pslot, w.pnode, w.pstamp, xyz2, tran2,
+                                                            slot2, node2, stamp2);
+      CUDA_TRY(cudaStreamSynchronize(st));
+      cudaFree(w.pxyz); cudaFree(w.ptran); cudaFree(w.pslot); cudaFree(w.pnode); cudaFree(w.pstamp);
+      w.pxyz = xyz2; w.ptran = tran2; w.pslot = slot2; w.pnode = node2; w.pstamp = stamp2;
+      w.np = m;
+    }
+    c->launches += 3;
+  }
+  win_margi_node_kernel<<<(w.nn + 127) / 128, 128, 0, st>>>(w.nn, w.N, mg, win_count, poses, w.nsplit, w.npush, w.nfix,
+                                                            w.sig_o, w.sig_t);
+  CUDA_TRY(cudaStreamSynchronize(st));
+  CUDA_TRY(cudaGetLastError());
+  c->launches += 1;
+  return BALM_OK;
+}
+
+int window_push_build(balm_ctx *c, WindowState &w, int win_count, int64_t *M_out, int64_t *K_out,
+                      int (*reg)(balm_ctx *, int64_t, const int64_t *, const int32_t *, const double *, const double *,
+                                 const double *, int64_t)) {
+  *M_out = 0;
+  *K_out = 0;
+  if (w.nn == 0) return BALM_OK;
+  cudaStream_t st = c->stream;
+  ScratchPool pool;
+  CubTmp tmp{pool};
+  const int nn = w.nn;
+  int *flag = nullptr, *iota = nullptr, *sel = nullptr, *nsel = nullptr;
+  ATRY(pool.get(&flag, nn)); ATRY(pool.get(&iota, nn)); ATRY(pool.get(&sel, nn)); ATRY(pool.get(&nsel, 1));
+  const unsigned g = (unsigned)((nn + 127) / 128);
+  win_push_flag_kernel<<<g, 128, 0, st>>>(nn, w.N, win_count, w.P.min_ps, w.nsplit, w.npush, w.sig_o, flag);
+  win_iota_kernel<<<g, 128, 0, st>>>(iota, nn, 0);
+  size_t b1 = 0;
+  cub::DeviceSelect::Flagged(nullptr, b1, iota, flag, sel, nsel, nn, st);
+  ATRY(tmp.need(b1));
+  CUDA_TRY(cub::DeviceSelect::Flagged(tmp.p, tmp.bytes, iota, flag, sel, nsel, nn, st));
+  int M = 0;
+  CUDA_TRY(cudaMemcpyAsync(&M, nsel, sizeof(int), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  c->launches += 3;
+  if (M == 0) return BALM_OK;
+  // ascending node key (unique among pushed nodes: a pushed node is not split, so none of its ancestors is pushed)
+  unsigned long long *k = nullptr, *k2 = nullptr;
+  int *ids = nullptr, *cnt = nullptr, *ostart = nullptr;
+  ATRY(pool.get(&k, M)); ATRY(pool.get(&k2, M)); ATRY(pool.get(&ids, M)); ATRY(pool.get(&cnt, M)); ATRY(pool.get(&ostart, M));
+  const unsigned gm = (unsigned)((M + 127) / 128);
+  win_gather_u64_kernel<<<gm, 128, 0, st>>>(w.nkey, sel, M, k);
+  size_t b2 = 0, b3 = 0;
+  cub::DeviceRadixSort::SortPairs(nullptr, b2, k, k2, sel, ids, M, 0, 64, st);
+  cub::DeviceScan::ExclusiveSum(nullptr, b3, cnt, ostart, M, st);
+  ATRY(tmp.need(std::max(b2, b3)));
+  CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp.p, tmp.bytes, k, k2, sel, ids, M, 0, 64, st));
+  win_obs_count_kernel<<<gm, 128, 0, st>>>(ids, M, w.N, w.sig_o, cnt);
+  CUDA_TRY(cub::DeviceScan::ExclusiveSum(tmp.p, tmp.bytes, cnt, ostart, M, st));
+  int last[2] = {0, 0};
+  CUDA_TRY(cudaMemcpyAsync(&last[0], cnt + M - 1, sizeof(int), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaMemcpyAsync(&last[1], ostart + M - 1, sizeof(int), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  const int64_t K = (int64_t)last[0] + last[1];
+  long long *rp = nullptr;
+  int *pi = nullptr, *lay = nullptr;
+  double *ob = nullptr, *fx = nullptr, *co = nullptr;
+  unsigned long long *keys_out = nullptr;
+  ATRY(pool.get(&rp, (size_t)M + 1)); ATRY(pool.get(&pi, (size_t)K)); ATRY(pool.get(&ob, (size_t)K * 10));
+  ATRY(pool.get(&fx, (size_t)M * 10)); ATRY(pool.get(&co, (size_t)M)); ATRY(pool.get(&keys_out, (size_t)M));
+  ATRY(pool.get(&lay, (size_t)M));
+  win_emit_kernel<<<gm, 128, 0, st>>>(ids, ostart, M, K, w.N, w.sig_o, w.nfix, w.nkey, w.nlayer, rp, pi, ob, fx, co, keys_out,
+                                      lay);
+  CUDA_TRY(cudaStreamSynchronize(st));
+  CUDA_TRY(cudaGetLastError());
+  c->launches += 6;
+  *M_out = M;
+  *K_out = K;
+  ATRY(reg(c, M, (const int64_t *)rp, pi, ob, fx, co, K));
+  return install_keys(c, keys_out, lay, M, true);
 }

@@ -216,6 +216,7 @@ extern "C" int balm_destroy(balm_ctx *c) {
   cudaSetDevice(c->device);
   cudaStreamSynchronize(c->stream);
   free_problem(c);
+  window_free(c->win);
   if (c->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(c->comm);
   cudaFree(c->poses); cudaFree(c->poses_trial); cudaFree(c->H); cudaFree(c->A); cudaFree(c->W);
   cudaFree(c->dx); cudaFree(c->dvec); cudaFree(c->scal); cudaFree(c->flags); cudaFree(c->accum); cudaFree(c->accum_batch);
@@ -874,6 +875,65 @@ extern "C" int balm_download_fix(balm_ctx *c, double *fix10) {
   if (c->fix) CUDA_TRY(cudaMemcpy(soa.data(), c->fix, sizeof(double) * 10 * c->M, cudaMemcpyDeviceToHost));
   for (int64_t v = 0; v < c->M; v++)
     for (int q = 0; q < 10; q++) fix10[v * 10 + q] = soa[(size_t)q * c->M + v];
+  return BALM_OK;
+}
+
+// ---------------- persistent sliding-window octree (assoc.cu) ----------------
+int window_reset_build(balm_ctx *c, WindowState **ws, double voxel_size, int layer_limit, int min_ps, const double *eig3);
+int window_cut_build(balm_ctx *c, WindowState &w, int64_t n, const float *xyz_h, const double *pose12_h, int slot);
+int window_recut_build(balm_ctx *c, WindowState &w, int win_count);
+int window_marginalize_build(balm_ctx *c, WindowState &w, int mg, const double *poses_h, int win_count);
+int window_push_build(balm_ctx *c, WindowState &w, int win_count, int64_t *M_out, int64_t *K_out,
+                      int (*reg)(balm_ctx *, int64_t, const int64_t *, const int32_t *, const double *, const double *,
+                                 const double *, int64_t));
+static int window_check(balm_ctx *c, const char *fn, int win_count) {
+  if (!c) { balm_set_error(std::string(fn) + ": bad arguments"); return BALM_ERR_INVALID; }
+  if (!c->win) { balm_set_error(std::string(fn) + ": call balm_window_reset first"); return BALM_ERR_INVALID; }
+  if (win_count < 1 || win_count > c->N) { balm_set_error(std::string(fn) + ": win_count must be in [1, N]"); return BALM_ERR_INVALID; }
+  return BALM_OK;
+}
+extern "C" int balm_window_reset(balm_ctx *c, const balm_assoc_opts *opts) {
+  if (!c) { balm_set_error("balm_window_reset: bad arguments"); return BALM_ERR_INVALID; }
+  CUDA_TRY(cudaSetDevice(c->device));
+  balm_assoc_opts o;
+  if (opts) o = *opts; else balm_default_assoc_opts(&o);
+  for (double &e : o.eigen_value_array) e = (double)(float)e;  // `float eigen_value_array[]` (bavoxel.hpp:11)
+  return window_reset_build(c, &c->win, o.voxel_size, o.layer_limit, o.min_ps, o.eigen_value_array);
+}
+extern "C" int balm_window_cut(balm_ctx *c, int64_t n_points, const float *xyz, const double *pose12, int slot) {
+  TRY(window_check(c, "balm_window_cut", 1));
+  if ((n_points > 0 && !xyz) || !pose12 || n_points < 0 || slot < 0 || slot >= c->N) {
+    balm_set_error("balm_window_cut: bad arguments (slot must be in [0, N))");
+    return BALM_ERR_INVALID;
+  }
+  CUDA_TRY(cudaSetDevice(c->device));
+  return window_cut_build(c, *c->win, n_points, xyz, pose12, slot);
+}
+extern "C" int balm_window_recut(balm_ctx *c, int win_count) {
+  TRY(window_check(c, "balm_window_recut", win_count));
+  CUDA_TRY(cudaSetDevice(c->device));
+  return window_recut_build(c, *c->win, win_count);
+}
+extern "C" int balm_window_marginalize(balm_ctx *c, int mg_size, const double *poses12, int win_count) {
+  TRY(window_check(c, "balm_window_marginalize", win_count));
+  if (mg_size < 1 || mg_size >= win_count) {
+    balm_set_error("balm_window_marginalize: mg_size must be in [1, win_count)");
+    return BALM_ERR_INVALID;
+  }
+  CUDA_TRY(cudaSetDevice(c->device));
+  return window_marginalize_build(c, *c->win, mg_size, poses12, win_count);
+}
+extern "C" int balm_window_push(balm_ctx *c, int win_count, int64_t *n_voxels_out, int64_t *n_obs_out) {
+  TRY(window_check(c, "balm_window_push", win_count));
+  CUDA_TRY(cudaSetDevice(c->device));
+  int64_t M = 0, K = 0;
+  TRY(window_push_build(c, *c->win, win_count, &M, &K, balm_set_voxels_dev));
+  if (M == 0) {  // nothing pushed: an empty voxel set
+    drop_keys(c);
+    TRY(register_empty(c));
+  }
+  if (n_voxels_out) *n_voxels_out = M;
+  if (n_obs_out) *n_obs_out = K;
   return BALM_OK;
 }
 

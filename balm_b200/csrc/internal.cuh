@@ -18,6 +18,8 @@
 #define BALM_SYRK_TILE 128
 
 void balm_set_error(const std::string &s);
+struct WindowState;  // the persistent sliding-window octree (assoc.cu)
+void window_free(WindowState *w);
 
 #define CUDA_TRY(expr)                                                                        \
   do {                                                                                        \
@@ -68,6 +70,7 @@ struct balm_ctx {
   double assoc_voxel_size = 1.0;  // association parameters of that call
   int assoc_layer_limit = 2, assoc_min_ps = 15;
   double assoc_eig[3] = {1.0 / 16, 1.0 / 16, 1.0 / 16};
+  WindowState *win = nullptr;     // balm_window_* state (independent of the registered voxel set)
 
   // ---- optimiser state (device) ----
   double *poses = nullptr, *poses_trial = nullptr;  // [12N]

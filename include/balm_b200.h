@@ -162,6 +162,39 @@ int balm_append_scan(balm_ctx *ctx, int64_t n_points, const float *xyz, const do
                      int64_t *n_voxels_out, int64_t *n_obs_out, int64_t *n_matched_out);
 int balm_download_keys(balm_ctx *ctx, uint64_t *keys, int32_t *layers);
 
+/* Persistent sliding-window octree in HBM = the reference's surf_map of OCTO_TREE_ROOTs kept across window shifts
+ * (consistency.cpp / benchmark_realworld.cpp driver loops). Window slots are the ctx's N pose slots. Unlike
+ * balm_append_scan / balm_marginalize, which work on the flattened voxel set, the window keeps every node the reference
+ * keeps: points outside the known planes grow new roots and leaves, a leaf that stops being planar is split further, and
+ * a leaf that is not pushed stays in the map, dormant, with its fix cluster until later scans hit it again. Nodes are
+ * never deleted (the reference never deletes them either): the map grows with the trajectory, by 104 + 160 * N bytes
+ * per node (key, flags, fix cluster, and sig_orig + sig_tran for every slot), plus 52 bytes per point held.
+ * The window is independent of the registered voxel set: balm_set_voxels, balm_cut_voxels, balm_append_scan,
+ * balm_marginalize and balm_synth_virtual do not touch it; balm_destroy frees it. A rejected call (BALM_ERR_INVALID:
+ * slot outside [0, N), win_count outside [1, N], mg_size outside [1, win_count), no balm_window_reset before) leaves the
+ * window unchanged. */
+int balm_window_reset(balm_ctx *ctx, const balm_assoc_opts *opts);
+/* empty map with these association parameters (opts NULL = balm_default_assoc_opts; eigen ratios rounded to float) */
+int balm_window_cut(balm_ctx *ctx, int64_t n_points, const float *xyz, const double *pose12, int slot);
+/* cut_voxel(surf_map, scan, x, slot) (bavoxel.hpp:1170-1223): xyz n_points x 3 float32 in the body frame, pose12 the
+ * scan's pose; every point's world coordinate R p + t (fp64) picks its root voxel (created on first use), and the point
+ * is pushed into that root's slot `slot` -- also when the root is already split: such points wait for the next recut. */
+int balm_window_recut(balm_ctx *ctx, int win_count);
+/* OCTO_TREE_NODE::recut(win_count) on every root (bavoxel.hpp:737-776, judge_eigen :654-699, cut_func :700-735): a node
+ * that is not split is judged from fix_point + sig_tran of the slots < win_count (push_state = 1 when planar with more
+ * than min_ps window points); a node that is not planar below layer_limit is split for good and the points of its slots
+ * < win_count move to the octant children; a node split earlier moves the points of slot win_count - 1 only. */
+int balm_window_marginalize(balm_ctx *ctx, int mg_size, const double *poses12 /* N x 12 or NULL */, int win_count);
+/* OCTO_TREE_ROOT::marginalize(mg_size, x_poses, win_count) (bavoxel.hpp:948-963, to_margi :778-816) on every node that
+ * is not split: with poses12, sig_tran and vec_tran of the slots < win_count are re-transformed by them; a node with
+ * push_state 1 and fewer than 50 fix points adds sig_tran of the slots < mg_size to its fix cluster; slots mg_size ..
+ * win_count - 1 shift down by mg_size and the top mg_size slots are cleared (their points are gone). */
+int balm_window_push(balm_ctx *ctx, int win_count, int64_t *n_voxels_out, int64_t *n_obs_out);
+/* tras_opt(voxhess, win_count) on every root (bavoxel.hpp:908-929, push_voxel :30-51): every node that is not split,
+ * has push_state 1, at least min_ps points in the slots < win_count and at least two non-empty slots is registered in
+ * the ctx as balm_set_voxels would (rows = its non-empty sig_orig slots, fix cluster = its fix_point, coe = its points),
+ * in ascending node key; balm_download_keys / balm_download_fix read them back. No such node -> an empty voxel set. */
+
 /* Pose-covariance propagation of the consistency experiment (SURVEY.md section 8f, row N3):
  *   Rcov_raw = sum over observations of  Ls c_cov Ls^T      -- VOX_HESS::left_jacobian_point + BALM2::multi_second
  *                                                              (src/simulation/BAs_left.hpp:342-473, 995-1023)
