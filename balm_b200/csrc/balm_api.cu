@@ -82,8 +82,7 @@ static void drop_keys(balm_ctx *c) {  // a voxel set registered from arrays carr
 static int alloc_problem_arrays(balm_ctx *c, int64_t M, int64_t K, bool with_fix) {
   // A window of the same shape as the previous one (the common case when BA runs scan after scan, and what every
   // repetition of a benchmark does) keeps every device buffer: cudaFree/cudaMalloc of several GB cost milliseconds.
-  c->reuse_ws = c->obs && c->stats && c->M == M && c->K == K && (c->fix != nullptr) == with_fix &&
-                !getenv("BALM_NO_BUFFER_REUSE");
+  c->reuse_ws = c->obs && c->stats && c->M == M && c->K == K && (c->fix != nullptr) == with_fix;
   if (c->reuse_ws) {
     cudaFree(c->csc_ptr); cudaFree(c->csc_obs); cudaFree(c->csc_vox); cudaFree(c->csc_lo); cudaFree(c->csc_hi);
     c->csc_ptr = c->csc_obs = c->csc_vox = c->csc_lo = c->csc_hi = nullptr;
@@ -114,8 +113,8 @@ static int alloc_workspaces(balm_ctx *c) {
   if (vb < 1) vb = 1;
   c->VB = vb;
   TRY(dev_alloc(&c->stats, (size_t)vb * BALM_STATS_STRIDE));
-  if (vb == c->M && !getenv("BALM_NO_STATS_CACHE")) TRY(dev_alloc(&c->stats_trial, (size_t)vb * BALM_STATS_STRIDE));
-  if (!getenv("BALM_NO_STATS_SPLIT")) TRY(dev_alloc(&c->vsums, (size_t)vb * 10));
+  if (vb == c->M) TRY(dev_alloc(&c->stats_trial, (size_t)vb * BALM_STATS_STRIDE));
+  TRY(dev_alloc(&c->vsums, (size_t)vb * 10));
   if (c->prec == BALM_PREC_FP64) {  // the tensor path writes int8 digit planes directly and never stores fp64 G'
     TRY(dev_alloc(&c->G, (size_t)3 * vb * c->ldg));
     CUDA_TRY(cudaMemsetAsync(c->G, 0, sizeof(double) * (size_t)3 * vb * c->ldg, c->stream));  // zero the column padding
@@ -153,7 +152,6 @@ static int alloc_workspaces(balm_ctx *c) {
       best = s;
     }
   }
-  if (const char *e = getenv("BALM_SYRK_SPLITS")) best = std::max(1, std::min(atoi(e), max_splits));  // tuning knob
   c->syrk_splits = best;
   TRY(dev_alloc(&c->syrk_part, (size_t)best * c->syrk_tiles * BALM_SYRK_TILE * BALM_SYRK_TILE));
   if (c->prec == BALM_PREC_TENSOR) TRY(tensor_syrk_init(c));
@@ -181,8 +179,6 @@ extern "C" int balm_create(balm_ctx **out, int n_poses, int device, int precisio
   int prio_least = 0, prio_greatest = 0;
   CUDA_TRY(cudaDeviceGetStreamPriorityRange(&prio_least, &prio_greatest));
   CUDA_TRY(cudaStreamCreateWithPriority(&c->stream, cudaStreamNonBlocking, prio_greatest));
-  CUDA_TRY(cudaStreamCreateWithPriority(&c->stream2, cudaStreamNonBlocking, prio_least));
-  for (auto &e : c->sev) CUDA_TRY(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
   TRY(factor_kernels_setup());
   TRY(syrk_f64_setup());
   TRY(ldlt_setup());
@@ -193,7 +189,6 @@ extern "C" int balm_create(balm_ctx **out, int n_poses, int device, int precisio
   TRY(dev_alloc(&c->H, n * n + n + 8));
   c->g = c->H + n * n;
   TRY(dev_alloc(&c->A, n * n));
-  TRY(dev_alloc(&c->W, 2 * n * BALM_NB));
   TRY(dev_alloc(&c->dx, n));
   TRY(dev_alloc(&c->dvec, n));
   TRY(dev_alloc(&c->scal, 32));
@@ -201,7 +196,9 @@ extern "C" int balm_create(balm_ctx **out, int n_poses, int device, int precisio
   TRY(dev_alloc(&c->planes, 2 * (size_t)c->N));
   TRY(dev_alloc(&c->accum, (size_t)BALM_ACC * c->Np));
   TRY(dev_alloc(&c->accum_batch, (size_t)BALM_ACC * c->Np));
-  c->res_blocks = c->sm_count * 24;  // residual partials: one per warp of the stats kernel (3 CTAs x 8 warps per SM)
+  // stats pass grids: voxel_sums_kernel up to 3 CTAs x 8 warps per SM, voxel_eig_kernel up to res_blocks CTAs (one
+  // residual partial each)
+  c->res_blocks = c->sm_count * 24;
   TRY(dev_alloc(&c->res_part, (size_t)c->res_blocks));
   CUDA_TRY(cudaMallocHost((void **)&c->h_scal, 16 * sizeof(double)));
   CUDA_TRY(cudaMallocHost((void **)&c->h_flags, 8 * sizeof(int)));
@@ -218,15 +215,12 @@ extern "C" int balm_destroy(balm_ctx *c) {
   free_problem(c);
   window_free(c->win);
   if (c->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(c->comm);
-  cudaFree(c->poses); cudaFree(c->poses_trial); cudaFree(c->H); cudaFree(c->A); cudaFree(c->W);
+  cudaFree(c->poses); cudaFree(c->poses_trial); cudaFree(c->H); cudaFree(c->A);
   cudaFree(c->dx); cudaFree(c->dvec); cudaFree(c->scal); cudaFree(c->flags); cudaFree(c->accum); cudaFree(c->accum_batch);
   cudaFree(c->vox_key); cudaFree(c->vox_layer); cudaFree(c->res_part); cudaFree(c->planes); cudaFree(c->Xinv); cudaFree(c->dinv); cudaFree(c->sol); cudaFree(c->ysol);
   cudaFree(c->Hpack); cudaFree(c->dval); cudaFree(c->rres); cudaFree(c->rdelta); cudaFree(c->dag_flags);
-  if (c->solve_graph) cudaGraphExecDestroy((cudaGraphExec_t)c->solve_graph);
   cudaFreeHost(c->h_scal); cudaFreeHost(c->h_flags);
   for (auto &e : c->ev) if (e) cudaEventDestroy(e);
-  for (auto &e : c->sev) if (e) cudaEventDestroy(e);
-  if (c->stream2) cudaStreamDestroy(c->stream2);
   cudaStreamDestroy(c->stream);
   delete c;
   return BALM_OK;

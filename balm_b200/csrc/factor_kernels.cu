@@ -1,6 +1,6 @@
 // factor_kernels.cu -- the O(K) streaming passes of the eigen-factor evaluation (HBM-bound kernels K1-K3).
 //
-//   voxel_sums_kernel + voxel_eig_kernel (default) / voxel_stats_kernel (single-kernel form):
+//   voxel_sums_kernel + voxel_eig_kernel:
 //                        per voxel  C = sum_i T_i C_i T_i^T (+fix), v_bar, eig(A)  -> residual (+ stats table)
 //                        = VOX_HESS::evaluate_only_residual (bavoxel.hpp:428-470) and phase 1 of
 //                          left_evaluate_acc2 (bavoxel.hpp:322-360)
@@ -24,19 +24,15 @@ struct StatsArgs {
   int64_t Kp;
   const int *pose_idx;
   const long long *row_ptr;
-  const double *coe;
   const double *fix;  // SoA [10][M] or null
   int64_t M;
   const double *poses;
   int N;
   int64_t v0, v1;
-  double *stats;      // [v1-v0][20] or null
-  double *res_part;   // [gridDim.x]
 };
 
-// One WARP per voxel: no block barriers, every warp is an independent stream of (loads -> shuffle reduce -> eig),
-// so the serial eigen-solve of one voxel overlaps the loads of the others. Lanes stride over the voxel's
-// observations with two observations (20 independent 8-byte loads) in flight per lane.
+// voxel_sums_kernel: one WARP per voxel, no block barriers. Lanes stride over the voxel's observations with two
+// observations (20 independent 8-byte loads) in flight per lane.
 constexpr int STATS_WARPS = STATS_THREADS / 32;
 // The stats row of one voxel: [0..19] eigen data, [20..39] the observation sweep's record with every per-voxel factor
 // folded into the vectors it multiplies (so the sweep spends no instruction on them):
@@ -70,67 +66,11 @@ __device__ __forceinline__ void store_stats_row(double *row, double vb0, double 
   st[19] = make_double2(f, vb0 * u0[0] + vb1 * u0[1] + vb2 * u0[2]);
 }
 
-template <bool STORE, bool SMEM_POSES>
-__global__ void __launch_bounds__(STATS_THREADS, 3) voxel_stats_kernel(StatsArgs a) {
-  extern __shared__ double s_poses[];  // [12 * N] pose table (R column-major, p): 96 B per pose, read per observation
-  if (SMEM_POSES) {
-    for (int e = threadIdx.x; e < 12 * a.N; e += STATS_THREADS) s_poses[e] = a.poses[e];
-    __syncthreads();
-  }
-  const double *ptab = SMEM_POSES ? s_poses : a.poses;
-  const int lane = threadIdx.x & 31;
-  const int64_t gw = (int64_t)blockIdx.x * STATS_WARPS + (threadIdx.x >> 5);
-  const int64_t nw = (int64_t)gridDim.x * STATS_WARPS;
-  double res_acc = 0.0;
-
-  for (int64_t v = a.v0 + gw; v < a.v1; v += nw) {
-    const long long s0 = a.row_ptr[v];
-    const int k = (int)(a.row_ptr[v + 1] - s0);
-    double acc[10];
-#pragma unroll
-    for (int c = 0; c < 10; c++) acc[c] = 0.0;
-    for (int j = lane; j < k; j += 64) {
-      const long long sA = s0 + j;
-      const bool hasB = j + 32 < k;
-      const long long sB = hasB ? sA + 32 : sA;
-      double oa[10], ob[10];
-#pragma unroll
-      for (int c = 0; c < 10; c++) { oa[c] = ld_stream(a.obs + c * a.Kp + sA); ob[c] = ld_stream(a.obs + c * a.Kp + sB); }
-      const int pa = __ldg(a.pose_idx + sA), pb = __ldg(a.pose_idx + sB);
-      double r[9], p[3];
-      load_pose_any<SMEM_POSES>(ptab + 12 * pa, r, p);
-      WC w = world_cluster(oa, r, p);
-      acc[0] += w.p00; acc[1] += w.p01; acc[2] += w.p02; acc[3] += w.p11; acc[4] += w.p12;
-      acc[5] += w.p22; acc[6] += w.v0;  acc[7] += w.v1;  acc[8] += w.v2;  acc[9] += w.n;
-      if (hasB) {
-        load_pose_any<SMEM_POSES>(ptab + 12 * pb, r, p);
-        w = world_cluster(ob, r, p);
-        acc[0] += w.p00; acc[1] += w.p01; acc[2] += w.p02; acc[3] += w.p11; acc[4] += w.p12;
-        acc[5] += w.p22; acc[6] += w.v0;  acc[7] += w.v1;  acc[8] += w.v2;  acc[9] += w.n;
-      }
-    }
-#pragma unroll
-    for (int c = 0; c < 10; c++) {
-      acc[c] = warp_sum(acc[c]);
-      if (a.fix) acc[c] += __ldg(a.fix + c * a.M + v);
-    }
-    const double inv = 1.0 / acc[9];
-    const double vb0 = acc[6] * inv, vb1 = acc[7] * inv, vb2 = acc[8] * inv;
-    double lam[3], u0[3], u1[3], u2[3];
-    eig3_jacobi(acc[0] * inv - vb0 * vb0, acc[1] * inv - vb0 * vb1, acc[2] * inv - vb0 * vb2,
-                acc[3] * inv - vb1 * vb1, acc[4] * inv - vb1 * vb2, acc[5] * inv - vb2 * vb2, lam, u0, u1, u2);
-    const double coe = __ldg(a.coe + v);
-    res_acc += coe * lam[0];
-    if (STORE && lane == 0) store_stats_row(a.stats + (v - a.v0) * BALM_STATS_STRIDE, vb0, vb1, vb2, u0, u1, u2, inv, coe, lam);
-  }
-  if (lane == 0) a.res_part[gw] = res_acc;
-}
-
-// ---- the default form of the stats / residual pass: the streaming half and the eigen half as two kernels ----
-// (BALM_NO_STATS_SPLIT=1 selects the single voxel_stats_kernel above; measured at C3: 0.916 -> 0.831 ms)
-// voxel_sums_kernel: the same warp-per-voxel stream as above, but the warp only reduces the ten cluster sums and
-// moves on -- no serial eigen-solve between two voxels' loads. voxel_eig_kernel: one THREAD per voxel does the
-// eigen-solve (M independent chains instead of M x 32 redundant ones), the residual term and the stats record.
+// ---- the stats / residual pass: the streaming half and the eigen half as two kernels ----
+// (one kernel doing both, the eigen-solve in every lane of the voxel's warp, measured at C3: 0.916 -> 0.831 ms)
+// voxel_sums_kernel: the warp only reduces the ten cluster sums and moves on -- no serial eigen-solve between two
+// voxels' loads. voxel_eig_kernel: one THREAD per voxel does the eigen-solve (M independent chains instead of M x 32
+// redundant ones), the residual term and the stats record.
 template <bool SMEM_POSES>
 __global__ void __launch_bounds__(STATS_THREADS, 3) voxel_sums_kernel(StatsArgs a, double *sums /*[v1-v0][10]*/) {
   extern __shared__ double s_poses[];
@@ -534,31 +474,17 @@ int launch_voxel_stats(balm_ctx *c, const double *poses, int64_t v0, int64_t v1,
   const int64_t want = (nv + STATS_WARPS - 1) / STATS_WARPS;
   const int max_blocks = c->res_blocks / STATS_WARPS;
   int blocks = (int)(want < (int64_t)max_blocks ? want : max_blocks);
-  StatsArgs a{c->obs, c->Kp, c->pose_idx, c->row_ptr, c->coe, use_fix ? c->fix : nullptr, c->M, poses, c->N, v0, v1,
-              stats_out, c->res_part};
+  StatsArgs a{c->obs, c->Kp, c->pose_idx, c->row_ptr, use_fix ? c->fix : nullptr, c->M, poses, c->N, v0, v1};
   const int psmem = 12 * c->N * (int)sizeof(double);
   const bool in_smem = psmem <= 64 * 1024;  // up to 682 poses; larger windows read the table through L1
-  if (c->vsums) {  // default: streaming kernel + one eigen-solve per thread (BALM_NO_STATS_SPLIT: single kernel below)
-    if (in_smem) voxel_sums_kernel<true><<<blocks, STATS_THREADS, psmem, c->stream>>>(a, c->vsums);
-    else voxel_sums_kernel<false><<<blocks, STATS_THREADS, 0, c->stream>>>(a, c->vsums);
-    const int64_t wantb = (nv + 127) / 128;
-    const int eb = (int)(wantb < (int64_t)c->res_blocks ? wantb : c->res_blocks);
-    if (store_stats) voxel_eig_kernel<true><<<eb, 128, 0, c->stream>>>(c->vsums, c->coe, v0, v1, stats_out, c->res_part);
-    else voxel_eig_kernel<false><<<eb, 128, 0, c->stream>>>(c->vsums, c->coe, v0, v1, nullptr, c->res_part);
-    residual_reduce_kernel<<<1, 32, 0, c->stream>>>(c->res_part, eb, residual_out_dev, 1);
-    c->launches += 3;
-    CUDA_TRY(cudaGetLastError());
-    return BALM_OK;
-  }
-  if (in_smem) {
-    if (store_stats) voxel_stats_kernel<true, true><<<blocks, STATS_THREADS, psmem, c->stream>>>(a);
-    else voxel_stats_kernel<false, true><<<blocks, STATS_THREADS, psmem, c->stream>>>(a);
-  } else {
-    if (store_stats) voxel_stats_kernel<true, false><<<blocks, STATS_THREADS, 0, c->stream>>>(a);
-    else voxel_stats_kernel<false, false><<<blocks, STATS_THREADS, 0, c->stream>>>(a);
-  }
-  residual_reduce_kernel<<<1, 32, 0, c->stream>>>(c->res_part, blocks * STATS_WARPS, residual_out_dev, 1);
-  c->launches += 2;
+  if (in_smem) voxel_sums_kernel<true><<<blocks, STATS_THREADS, psmem, c->stream>>>(a, c->vsums);
+  else voxel_sums_kernel<false><<<blocks, STATS_THREADS, 0, c->stream>>>(a, c->vsums);
+  const int64_t wantb = (nv + 127) / 128;
+  const int eb = (int)(wantb < (int64_t)c->res_blocks ? wantb : c->res_blocks);
+  if (store_stats) voxel_eig_kernel<true><<<eb, 128, 0, c->stream>>>(c->vsums, c->coe, v0, v1, stats_out, c->res_part);
+  else voxel_eig_kernel<false><<<eb, 128, 0, c->stream>>>(c->vsums, c->coe, v0, v1, nullptr, c->res_part);
+  residual_reduce_kernel<<<1, 32, 0, c->stream>>>(c->res_part, eb, residual_out_dev, 1);
+  c->launches += 3;
   CUDA_TRY(cudaGetLastError());
   return BALM_OK;
 }
@@ -672,8 +598,6 @@ int launch_obs_int8(balm_ctx *c, const double *poses, int64_t v0, int64_t v1, bo
 
 // Kernel attributes are per device: set once per context (a process may drive several GPUs).
 int factor_kernels_setup() {
-  CUDA_TRY(cudaFuncSetAttribute(voxel_stats_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
-  CUDA_TRY(cudaFuncSetAttribute(voxel_stats_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
   CUDA_TRY(cudaFuncSetAttribute(voxel_sums_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
   return BALM_OK;
 }

@@ -36,9 +36,6 @@ void window_free(WindowState *w);
 struct balm_ctx {
   int N = 0, n = 0, ldg = 0, Np = 0, device = 0, prec = 0;
   cudaStream_t stream = nullptr;
-  cudaStream_t stream2 = nullptr;  // side stream of the solve's look-ahead (lower priority)
-  cudaEvent_t sev[3] = {nullptr, nullptr, nullptr};  // panel done / rest done (two parities)
-  bool solve_lookahead = true;
   double *ysol = nullptr;          // [n] forward-substitution result y (kept apart from the running rhs `sol`)
   bool lm_active = false;     // inside balm_damping_iter (scale speculation and stats hand-over are loop-local)
   bool reuse_ws = false;      // the registration in progress has the shape of the previous one: buffers are kept
@@ -76,7 +73,6 @@ struct balm_ctx {
   double *poses = nullptr, *poses_trial = nullptr;  // [12N]
   double *H = nullptr, *g = nullptr;                // [n*n + n + 8] contiguous: H | g | r  (one all-reduce)
   double *A = nullptr;                              // [n*n] factor workspace
-  double *W = nullptr;                              // [2][n*NB] panel * D (double-buffered by step parity)
   double *dx = nullptr;                             // [n]
   double *dvec = nullptr;                           // [n] diag(H)
   double *Xinv = nullptr;                           // [panels][64*64] inverses of the unit-lower diagonal blocks
@@ -86,11 +82,7 @@ struct balm_ctx {
   double *rres = nullptr;                           // [n] residual b - A x of the last solve (backward-error check)
   double *rdelta = nullptr;                         // [n] refinement correction
   int *dag_flags = nullptr;                         // tile-DAG dependency counters: upd | pdone [nt*nt], xdone | rhs_cnt [nt]
-  bool solve_dag = true;                            // persistent tile-DAG factorisation (BALM_SOLVE_MULTIKERNEL=1: old path)
-  int dag_grid = 0, dag_near = 0;
   unsigned long long *dag_trace = nullptr;          // BALM_DAG_TRACE: device timestamps of the last factorisation
-  void *solve_graph = nullptr;                      // cudaGraphExec_t of the solve sequence
-  int solve_launches = 0;
   double *scal = nullptr;                           // device scalars [32]: 0 r(eval) 1 q1 2 r(residual) 3 u 4..15 gauge
                                                     // snapshot, 16/17 this rank's residual at the current / trial poses
   double *h_scal = nullptr;                         // pinned host mirror [16]
@@ -271,6 +263,19 @@ __device__ __forceinline__ double warp_sum(double v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
+}
+
+// 16-byte global -> shared copy through L2 (cp.async.cg)
+__device__ __forceinline__ void cp_async16(void *smem, const void *gmem) {
+  unsigned sa = (unsigned)__cvta_generic_to_shared(smem);
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(sa), "l"(gmem));
+}
+
+// fp64 tensor-core MMA (DMMA): 8x8 C fragment (c0, c1) += 8x4 A fragment (a) * 4x8 B fragment (b)
+__device__ __forceinline__ void dmma_8x8x4(double &c0, double &c1, double a, double b) {
+  asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};\n"
+               : "+d"(c0), "+d"(c1)
+               : "d"(a), "d"(b));
 }
 
 #endif  // __CUDACC__

@@ -12,7 +12,6 @@
 //
 // A is column-major n x n; only the lower triangle is read/written. Panel width NB = 64.
 #include <stdlib.h>
-#include <algorithm>
 #include "internal.cuh"
 #define TRY_LAUNCH(x) do { int _s = (x); if (_s != BALM_OK) return _s; } while (0)
 
@@ -31,17 +30,6 @@ __global__ void damp_copy_kernel(const double *H, double *A, double *dvec, int n
     h += u * h;
   }
   A[(size_t)j * n + i] = h;
-}
-
-// ---- panel step j0: three kernels ------------------------------------------------------------------------
-// (1) ldl_diag_kernel: one CTA factors the 64x64 diagonal block in REGISTERS (16x16 threads, 4x4 each), one
-//     __syncthreads per column (double-buffered column broadcast). The same sweep builds X = L11^-1 (forward
-//     substitution on the identity), so the panel below needs a GEMM instead of a sequential TRSM, and applies
-//     it to the right-hand side: y_j = L11^-1 b_j (forward substitution fused into the factorisation).
-// (2) ldl_panel_kernel: W = A21 X^T (64x64x64 GEMM per 64-row tile), L21 = W d^-1, b_rows -= L21 y_j.
-// (3) ldl_update_kernel: A22 -= L21 W^T on 128x128 tiles of the lower triangle.
-__device__ __forceinline__ void bar_sync_named(int id, int nthreads) {
-  asm volatile("bar.sync %0, %1;\n" ::"r"(id), "r"(nthreads) : "memory");
 }
 
 // The 64x64 diagonal block is factored in four 16-column sub-panels. The serial chain of the whole solve is n = 6N column
@@ -196,222 +184,9 @@ __device__ __forceinline__ bool diag_factor(double (*S)[NB + 1], double (*Xs)[NB
   return bad;
 }
 
-// Diagonal step: factor, write L11/d back, X, 1/d, y_j = X b_j (y goes to `ysol`; `sol` keeps the running rhs).
-// (Factoring the block redundantly inside every panel CTA, to drop this kernel boundary from the critical path, was
-// measured and is NOT faster: 2.81 vs 2.72 ms at n = 3000.)
-__global__ void __launch_bounds__(256) ldl_diag_kernel(double *A, int n, int j0, int nbw, double *Xcm, double *dinv_all,
-                                                       const double *sol, double *ysol, int *flags) {
-  extern __shared__ double dyn_smem[];
-  double (*S)[NB + 1] = reinterpret_cast<double (*)[NB + 1]>(dyn_smem);                   // the block (lower) -> L, d
-  double (*Xs)[NB + 1] = reinterpret_cast<double (*)[NB + 1]>(dyn_smem + NB * (NB + 1));  // L11^-1
-  double (*Wp)[17] = reinterpret_cast<double (*)[17]>(dyn_smem + 2 * NB * (NB + 1));     // current sub-panel times d
-  double (*col16)[16] = reinterpret_cast<double (*)[16]>(dyn_smem + 2 * NB * (NB + 1) + NB * 17);
-  double *bvec = dyn_smem + 2 * NB * (NB + 1) + NB * 17 + 32;
-  const int tid = threadIdx.x;
-  {
-    double ld[16];  // all 16 global loads of this thread in flight together (the kernel is pure latency)
-#pragma unroll
-    for (int it = 0; it < 16; it++) {
-      const int e = tid + it * 256, r = e & (NB - 1), c = e >> 6;
-      double v = (r == c) ? 1.0 : 0.0;  // rows/cols of a short last panel act as identity
-      if (r < nbw && c < nbw && r >= c) v = A[(size_t)(j0 + c) * n + j0 + r];
-      ld[it] = v;
-    }
-    const double bv = (tid < nbw) ? sol[j0 + tid] : 0.0;
-#pragma unroll
-    for (int it = 0; it < 16; it++) {
-      const int e = tid + it * 256, r = e & (NB - 1), c = e >> 6;
-      S[r][c] = ld[it];
-      Xs[r][c] = 0.0;
-    }
-    if (tid < NB) bvec[tid] = bv;
-  }
-  __syncthreads();
-  const bool bad = diag_factor(S, Xs, Wp, col16);
-  if (bad && tid == 0) atomicOr(&flags[0], 1);
-  // ---- write back L11 / d, X (column-major), 1/d, and y_j = X b_j ----
-#pragma unroll 4
-  for (int e = tid; e < NB * NB; e += 256) {
-    const int r = e & (NB - 1), c = e >> 6;
-    if (r < nbw && c < nbw && r >= c) A[(size_t)(j0 + c) * n + j0 + r] = S[r][c];
-    Xcm[c * NB + r] = (r >= c) ? Xs[r][c] : 0.0;
-  }
-  if (tid < nbw) dinv_all[j0 + tid] = 1.0 / S[tid][tid];
-  if (tid < NB) {
-    double sacc = 0.0;
-    for (int c = 0; c <= tid; c++) sacc += Xs[tid][c] * bvec[c];
-    if (tid < nbw) ysol[j0 + tid] = sacc;
-  }
-}
-
-__global__ void __launch_bounds__(256) ldl_panel_kernel(double *A, double *W, int n, int j0, int nbw, const double *Xcm,
-                                                        const double *dinv_all, double *sol, const double *ysol) {
-  extern __shared__ double dyn_smem[];
-  double (*sA)[NB + 4] = reinterpret_cast<double (*)[NB + 4]>(dyn_smem);                  // [k][row]
-  double (*sX)[NB + 4] = reinterpret_cast<double (*)[NB + 4]>(dyn_smem + NB * (NB + 4));  // [k][col] = X[col][k]
-  __shared__ double yj[NB], dv[NB];
-  const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
-  const int i0 = j0 + nbw + blockIdx.x * NB;
-  {
-    // all 32 loads of this thread are issued before the first shared-memory store (latency paid once)
-    double ra[16], rx[16];
-#pragma unroll
-    for (int it = 0; it < 16; it++) {
-      const int e = tid + it * 256, r = e & (NB - 1), k = e >> 6;
-      ra[it] = (k < nbw && i0 + r < n) ? A[(size_t)(j0 + k) * n + i0 + r] : 0.0;
-      rx[it] = Xcm[k * NB + r];  // X[r][k]
-    }
-#pragma unroll
-    for (int it = 0; it < 16; it++) {
-      const int e = tid + it * 256, r = e & (NB - 1), k = e >> 6;
-      sA[k][r] = ra[it];
-      sX[k][r] = rx[it];
-    }
-  }
-  if (tid < NB) {
-    yj[tid] = tid < nbw ? ysol[j0 + tid] : 0.0;
-    dv[tid] = tid < nbw ? dinv_all[j0 + tid] : 0.0;
-  }
-  __syncthreads();
-  double acc[4][4] = {};
-#pragma unroll 8
-  for (int k = 0; k < NB; k++) {
-    double av[4], xv[4];
-#pragma unroll
-    for (int p = 0; p < 4; p++) { av[p] = sA[k][4 * tx + p]; xv[p] = sX[k][4 * ty + p]; }
-#pragma unroll
-    for (int p = 0; p < 4; p++)
-#pragma unroll
-      for (int q = 0; q < 4; q++) acc[p][q] += av[p] * xv[q];
-  }
-  __syncthreads();
-#pragma unroll
-  for (int q = 0; q < 4; q++) {
-    const int c = 4 * ty + q;
-#pragma unroll
-    for (int p = 0; p < 4; p++) {
-      const int r = 4 * tx + p, i = i0 + r;
-      const double l = acc[p][q] * dv[c];
-      sA[c][r] = l;  // reuse as L21 tile [c][r] for the right-hand-side update
-      if (c < nbw && i < n) {
-        W[(size_t)c * n + i] = acc[p][q];
-        A[(size_t)(j0 + c) * n + i] = l;
-      }
-    }
-  }
-  __syncthreads();
-  if (tid < NB && i0 + tid < n) {
-    double s = 0.0;
-#pragma unroll 8
-    for (int c = 0; c < NB; c++) s += sA[c][tid] * yj[c];
-    sol[i0 + tid] -= s;
-  }
-}
-
-__device__ __forceinline__ void cp_async16(void *smem, const void *gmem) {
-  unsigned sa = (unsigned)__cvta_generic_to_shared(smem);
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(sa), "l"(gmem));
-}
-
-constexpr int UT = 128;   // update tile
-constexpr int UKB = 64;   // k rows per stage: the whole panel width in one shot (one global round trip)
-constexpr int ULDS = UT + 4;  // padded smem row (doubles): conflict-free DMMA fragment loads (see syrk_f64.cu)
-constexpr int USTAGE = 2 * UKB * ULDS;  // 135 KB: one CTA per SM
-
-__device__ __forceinline__ void dmma_8x8x4(double &c0, double &c1, double a, double b) {
-  asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};\n"
-               : "+d"(c0), "+d"(c1)
-               : "d"(a), "d"(b));
-}
-
-// Trailing update A22 -= L21 * W^T on 128x128 tiles of the lower triangle with fp64 tensor-core MMAs
-// (mma.sync.m8n8k4.f64, 8 warps x (64x32) warp tiles, the whole 64-wide k slab staged by one cp.async round).
-// The update of a panel step is issued in two parts (look-ahead): the STRIP (strip = 1: the NB columns of the next
-// panel, one tile per 128 rows, stores masked to col < base + NB) stays on the critical path; the REST (strip = 0,
-// base moved past the strip) runs on the side stream while the next diagonal block and panel are factored.
-__global__ void __launch_bounds__(256) ldl_update_kernel(double *A, const double *W, int n, int j0, int nbw, int base,
-                                                         int strip) {
-  extern __shared__ __align__(16) double dyn_smem[];
-  int t = blockIdx.x, tr = 0;
-  if (strip) { tr = t; t = 0; }
-  else while (t >= tr + 1) { t -= tr + 1; tr++; }
-  const int tc = t;  // tc <= tr
-  const int r0 = base + tr * UT, c0 = base + tc * UT;
-  const int climit = strip ? base + NB : n;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int wm = warp >> 2, wn = warp & 3, fr = lane >> 2, fk = lane & 3;
-  double acc[8][4][2];
-#pragma unroll
-  for (int i = 0; i < 8; i++)
-#pragma unroll
-    for (int j = 0; j < 4; j++) acc[i][j][0] = acc[i][j][1] = 0.0;
-  const int nsteps = (nbw + UKB - 1) / UKB;
-  auto load_stage = [&](int stage, int step) {
-    double *sL = dyn_smem + stage * USTAGE;
-    double *sW = sL + UKB * ULDS;
-    const int k0 = step * UKB;
-    // 16-byte pieces; n, r0, c0 are even so a pair is entirely inside or outside the matrix
-#pragma unroll 4
-    for (int e = tid; e < UKB * (UT / 2); e += 256) {
-      const int k = e >> 6, rr = (e & 63) * 2;
-      const bool kv = k0 + k < nbw;
-      if (kv && r0 + rr < n) cp_async16(sL + k * ULDS + rr, A + (size_t)(j0 + k0 + k) * n + r0 + rr);
-      else *reinterpret_cast<double2 *>(sL + k * ULDS + rr) = make_double2(0.0, 0.0);
-      if (kv && c0 + rr < climit) cp_async16(sW + k * ULDS + rr, W + (size_t)(k0 + k) * n + c0 + rr);
-      else *reinterpret_cast<double2 *>(sW + k * ULDS + rr) = make_double2(0.0, 0.0);
-    }
-  };
-  load_stage(0, 0);
-  asm volatile("cp.async.commit_group;\n" ::);
-  for (int step = 0; step < nsteps; step++) {
-    if (step + 1 < nsteps) {
-      load_stage((step + 1) & 1, step + 1);
-      asm volatile("cp.async.commit_group;\n" ::);
-      asm volatile("cp.async.wait_group 1;\n" ::);
-    } else {
-      asm volatile("cp.async.wait_group 0;\n" ::);
-    }
-    __syncthreads();
-    const double *sL = dyn_smem + (step & 1) * USTAGE;
-    const double *sW = sL + UKB * ULDS;
-#pragma unroll
-    for (int kk = 0; kk < UKB; kk += 4) {
-      double af[8], bf[4];
-#pragma unroll
-      for (int i = 0; i < 8; i++) af[i] = sL[(kk + fk) * ULDS + wm * 64 + i * 8 + fr];
-#pragma unroll
-      for (int j = 0; j < 4; j++) bf[j] = sW[(kk + fk) * ULDS + wn * 32 + j * 8 + fr];
-#pragma unroll
-      for (int i = 0; i < 8; i++)
-#pragma unroll
-        for (int j = 0; j < 4; j++) dmma_8x8x4(acc[i][j][0], acc[i][j][1], af[i], bf[j]);
-    }
-    __syncthreads();
-  }
-  // read-modify-write of the C tile: all loads of a row group are issued before the first store, otherwise every
-  // "-=" serialises a full L2 round trip (64 of them per thread)
-#pragma unroll
-  for (int i = 0; i < 8; i++) {
-    const int row = r0 + wm * 64 + i * 8 + fr;
-    double cv[4][2];
-#pragma unroll
-    for (int j = 0; j < 4; j++) {
-      const int col = c0 + wn * 32 + j * 8 + 2 * fk;
-      cv[j][0] = (row < n && col < climit && row >= col) ? A[(size_t)col * n + row] : 0.0;
-      cv[j][1] = (row < n && col + 1 < climit && row >= col + 1) ? A[(size_t)(col + 1) * n + row] : 0.0;
-    }
-#pragma unroll
-    for (int j = 0; j < 4; j++) {
-      const int col = c0 + wn * 32 + j * 8 + 2 * fk;
-      if (row < n && col < climit && row >= col) A[(size_t)col * n + row] = cv[j][0] - acc[i][j][0];
-      if (row < n && col + 1 < climit && row >= col + 1) A[(size_t)(col + 1) * n + row] = cv[j][1] - acc[i][j][1];
-    }
-  }
-}
-
 
 // =====================================================================================================================
-// Persistent tile-DAG factorisation (default).  ONE cooperative launch factors the whole matrix; 64 x 64 tiles, the
+// Persistent tile-DAG factorisation.  ONE cooperative launch factors the whole matrix; 64 x 64 tiles, the
 // dependencies between tile tasks are counters in global memory instead of kernel boundaries:
 //   chain CTA (block 0)  for k = 0 .. nt-1: D'(k) = [mini-panel L_{k,k-1} = A_{k,k-1} X_{k-1}^T d^-1, mini-update
 //                        A_kk -= L W^T, both in shared memory] + the 64 x 64 factorisation (diag_factor) + y_k.
@@ -861,7 +636,7 @@ __global__ void copy_kernel(double *dst, const double *src, int n) {
   if (i < n) dst[i] = src[i];
 }
 
-// rhs = -g (start of the forward substitution, fused into the factorisation kernels)
+// rhs = -g (start of the forward substitution, fused into the factorisation)
 __global__ void rhs_init_kernel(const double *g, double *sol, int n) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) sol[i] = -g[i];
@@ -994,74 +769,6 @@ __global__ void gauge_kernel(double *poses, const double *pose0_snapshot, int N,
 
 }  // namespace
 
-constexpr int DIAG_SMEM = (2 * NB * (NB + 1) + NB * 17 + 32 + NB) * (int)sizeof(double);
-
-// The factorisation loop with look-ahead. Main stream (high priority): diag(k) -> panel(k) -> strip(k) -> diag(k+1);
-// side stream: rest(k) after panel(k). Hazards: strip(k) and rest(k-1) both update the columns of panel k+1, and
-// panel(k+1) overwrites the W buffer rest(k-1) reads (W is double-buffered by step parity) -> strip(k) waits for
-// rest(k-1). rest(k) touches only columns right of panel k+1, which diag/panel(k+1) never access.
-static int enqueue_solve(balm_ctx *c) {
-  const int n = c->n;
-  cudaStream_t st = c->stream, side = c->stream2;
-  dim3 g1((n + 255) / 256, n);
-  damp_copy_kernel<<<g1, 256, 0, st>>>(c->H, c->A, c->dvec, n, c->scal + 3);
-  rhs_init_kernel<<<(n + 255) / 256, 256, 0, st>>>(c->g, c->sol, n);
-  const int panel_smem = 2 * NB * (NB + 4) * (int)sizeof(double);
-  const int update_smem = USTAGE * (int)sizeof(double);
-  int launches = 2;
-  int pending_rest = -1;  // parity of the side-stream event still to be waited for
-  for (int j0 = 0, pi = 0; j0 < n; j0 += NB, pi++) {
-    const int nbw = (n - j0 < NB) ? n - j0 : NB;
-    double *X = c->Xinv + (size_t)pi * NB * NB;
-    double *W = c->W + (size_t)(pi & 1) * n * NB;
-    const int m = n - j0 - nbw;
-    const int mt = (m + NB - 1) / NB, mu = (m + UT - 1) / UT;
-    ldl_diag_kernel<<<1, 256, DIAG_SMEM, st>>>(c->A, n, j0, nbw, X, c->dinv, c->sol, c->ysol, c->flags);
-    launches++;
-    if (m > 0) {
-      ldl_panel_kernel<<<mt, 256, panel_smem, st>>>(c->A, W, n, j0, nbw, X, c->dinv, c->sol, c->ysol);
-      launches++;
-      const int base = j0 + nbw;
-      if (!c->solve_lookahead) {
-        ldl_update_kernel<<<mu * (mu + 1) / 2, 256, update_smem, st>>>(c->A, W, n, j0, nbw, base, 0);
-        launches++;
-        continue;
-      }
-      CUDA_TRY(cudaEventRecord(c->sev[0], st));
-      if (pending_rest >= 0) CUDA_TRY(cudaStreamWaitEvent(st, c->sev[1 + pending_rest], 0));
-      pending_rest = -1;
-      ldl_update_kernel<<<mu, 256, update_smem, st>>>(c->A, W, n, j0, nbw, base, 1);
-      launches++;
-      const int m2 = m - NB;
-      if (m2 > 0) {
-        const int mu2 = (m2 + UT - 1) / UT;
-        CUDA_TRY(cudaStreamWaitEvent(side, c->sev[0], 0));
-        ldl_update_kernel<<<mu2 * (mu2 + 1) / 2, 256, update_smem, side>>>(c->A, W, n, j0, nbw, base + NB, 0);
-        launches++;
-        CUDA_TRY(cudaEventRecord(c->sev[1 + (pi & 1)], side));
-        pending_rest = pi & 1;
-      }
-    }
-  }
-  if (pending_rest >= 0) CUDA_TRY(cudaStreamWaitEvent(st, c->sev[1 + pending_rest], 0));
-  scale_rhs_kernel<<<(n + 255) / 256, 256, 0, st>>>(c->sol, c->ysol, c->dinv, n);
-  launches++;
-  const int npan = (n + NB - 1) / NB;
-  for (int hi = npan - 1; hi >= 0; hi -= BACK_GROUP) {
-    const int lo = hi - BACK_GROUP + 1 > 0 ? hi - BACK_GROUP + 1 : 0;
-    const int g_lo = lo * NB;
-    const int g_hi = (hi + 1) * NB < n ? (hi + 1) * NB : n;
-    const int blocks = g_lo > 0 ? (g_lo + 31) / 32 : 1;
-    ldl_back_kernel<<<blocks, 256, 0, st>>>(c->A, n, g_lo, g_hi - g_lo, c->Xinv + (size_t)lo * NB * NB, c->sol, c->dx);
-    launches++;
-  }
-  q1_kernel<<<1, 1024, 0, st>>>(c->dx, c->g, c->dvec, n, c->scal + 3, c->scal);
-  launches++;
-  c->solve_launches = launches;
-  return BALM_OK;
-}
-
-
 constexpr double SOLVE_OMEGA_TOL = 1e-12;  // componentwise backward error accepted without refinement
 
 // omega of the current c->dx (+ the residual vector in c->rres); flags[4] raised when omega > tol. scal[20] = omega.
@@ -1132,7 +839,7 @@ static int enqueue_back_substitution(balm_ctx *c, const double *rhs_g, double *x
   return BALM_OK;
 }
 
-// Persistent tile-DAG path: damp/copy + rhs, ONE cooperative launch for the factorisation and forward substitution,
+// The damped solve: damp/copy + rhs, ONE cooperative launch for the factorisation and forward substitution,
 // then the grouped backward substitution, q1 and the backward-error check.
 static int enqueue_solve_dag(balm_ctx *c) {
   const int n = c->n, nt = (n + NB - 1) / NB;
@@ -1145,9 +852,10 @@ static int enqueue_solve_dag(balm_ctx *c) {
   a.A = c->A; a.n = n; a.nt = nt; a.Xinv = c->Xinv; a.dinv = c->dinv; a.dval = c->dval; a.sol = c->sol; a.ysol = c->ysol;
   a.flags = c->flags; a.upd = c->dag_flags; a.pdone = c->dag_flags + (size_t)nt * nt;
   a.xdone = c->dag_flags + 2 * (size_t)nt * nt; a.rhs_cnt = a.xdone + nt;
-  int grid = nt < 2 ? 1 : c->dag_grid;
+  // one CTA per SM (216 KB of shared memory each); a grid that cannot be co-resident makes the cooperative launch fail
+  const int grid = nt < 2 ? 1 : c->sm_count;
   const int workers = grid - 1;
-  a.near_ctas = workers >= 16 ? c->dag_near : 0;
+  a.near_ctas = workers >= 16 ? 8 : 0;
   a.trace = c->dag_trace;
   void *params[] = {&a};
   CUDA_TRY(cudaLaunchCooperativeKernel((const void *)dag::ldl_dag_kernel, dim3(grid), dim3(256), params,
@@ -1168,50 +876,17 @@ int launch_ldlt_solve(balm_ctx *c, double u) {
     CUDA_TRY(cudaMalloc((void **)&c->rres, sizeof(double) * n));
     CUDA_TRY(cudaMalloc((void **)&c->rdelta, sizeof(double) * n));
     CUDA_TRY(cudaMalloc((void **)&c->dag_flags, sizeof(int) * (2 * (size_t)npan * npan + 2 * npan)));
-    c->solve_lookahead = getenv("BALM_NO_LOOKAHEAD") == nullptr;
-    // the persistent factorisation needs every CTA resident at once: one CTA per SM (216 KB of shared memory each)
-    int per_sm = 0;
-    CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, dag::ldl_dag_kernel, 256,
-                                                           dag::SMEM_DOUBLES * sizeof(double)));
-    c->solve_dag = per_sm >= 1 && getenv("BALM_SOLVE_MULTIKERNEL") == nullptr;
-    c->dag_grid = c->sm_count;
-    if (const char *e = getenv("BALM_DAG_GRID")) c->dag_grid = std::max(2, std::min(atoi(e), c->sm_count));
     if (getenv("BALM_DAG_TRACE")) {
       CUDA_TRY(cudaMalloc((void **)&c->dag_trace, sizeof(unsigned long long) * (4 * (size_t)npan + 8 * 1024)));
       CUDA_TRY(cudaMemset(c->dag_trace, 0, sizeof(unsigned long long) * (4 * (size_t)npan + 8 * 1024)));
     }
-    c->dag_near = 8;
-    if (const char *e = getenv("BALM_DAG_NEAR")) c->dag_near = std::max(0, std::min(atoi(e), c->dag_grid - 2));
   }
-  c->h_scal[3] = u;  // pinned; the kernels read the damping factor from device memory so the graph is reusable
+  c->h_scal[3] = u;  // pinned; the kernels read the damping factor from device memory
   CUDA_TRY(cudaMemcpyAsync(c->scal + 3, c->h_scal + 3, sizeof(double), cudaMemcpyHostToDevice, c->stream));
   CUDA_TRY(cudaMemsetAsync(c->flags, 0, sizeof(int) * 8, c->stream));
-  if (c->solve_dag) {
-    TRY_LAUNCH(enqueue_solve_dag(c));
-    TRY_LAUNCH(enqueue_solve_check(c));
-    CUDA_TRY(cudaGetLastError());
-    return BALM_OK;
-  }
-  static const bool use_graph = getenv("BALM_NO_GRAPH") == nullptr;
-  if (!use_graph) {
-    TRY_LAUNCH(enqueue_solve(c));
-    c->launches += c->solve_launches;
-    TRY_LAUNCH(enqueue_solve_check(c));
-    CUDA_TRY(cudaGetLastError());
-    return BALM_OK;
-  }
-  if (!c->solve_graph) {  // capture the ~190-launch sequence once, replay it with one launch afterwards
-    cudaGraph_t graph;
-    CUDA_TRY(cudaStreamBeginCapture(c->stream, cudaStreamCaptureModeThreadLocal));
-    const int rc = enqueue_solve(c);
-    CUDA_TRY(cudaStreamEndCapture(c->stream, &graph));
-    if (rc != BALM_OK) return rc;
-    CUDA_TRY(cudaGraphInstantiate((cudaGraphExec_t *)&c->solve_graph, graph, 0));
-    CUDA_TRY(cudaGraphDestroy(graph));
-  }
-  CUDA_TRY(cudaGraphLaunch((cudaGraphExec_t)c->solve_graph, c->stream));
-  c->launches += c->solve_launches;
+  TRY_LAUNCH(enqueue_solve_dag(c));
   TRY_LAUNCH(enqueue_solve_check(c));
+  CUDA_TRY(cudaGetLastError());
   return BALM_OK;
 }
 
@@ -1232,11 +907,6 @@ int launch_gauge(balm_ctx *c, double *poses, int mode) {
 }
 
 int ldlt_setup() {
-  CUDA_TRY(cudaFuncSetAttribute(ldl_panel_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                2 * NB * (NB + 4) * (int)sizeof(double)));
-  CUDA_TRY(cudaFuncSetAttribute(ldl_update_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                USTAGE * (int)sizeof(double)));
-  CUDA_TRY(cudaFuncSetAttribute(ldl_diag_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, DIAG_SMEM));
   CUDA_TRY(cudaFuncSetAttribute(dag::ldl_dag_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                 dag::SMEM_DOUBLES * (int)sizeof(double)));
   return BALM_OK;

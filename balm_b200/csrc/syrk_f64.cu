@@ -20,20 +20,10 @@ constexpr int LDS = TILE + 4;         // padded smem row (doubles): conflict-fre
 constexpr int SYRK_THREADS = 256;
 constexpr int STAGE_DOUBLES = 2 * KB * LDS;
 
-__device__ __forceinline__ void cp_async16(void *smem, const void *gmem) {
-  unsigned sa = (unsigned)__cvta_generic_to_shared(smem);
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(sa), "l"(gmem));
-}
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::); }
 template <int N>
 __device__ __forceinline__ void cp_async_wait() {
   asm volatile("cp.async.wait_group %0;\n" ::"n"(N));
-}
-
-__device__ __forceinline__ void dmma_8x8x4(double &c0, double &c1, double a, double b) {
-  asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};\n"
-               : "+d"(c0), "+d"(c1)
-               : "d"(a), "d"(b));
 }
 
 struct SyrkArgs {

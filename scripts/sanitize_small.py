@@ -1,6 +1,5 @@
 """Small end-to-end run for compute-sanitizer (memcheck / racecheck): both precision modes, dense + sparse; the persistent
-tile-DAG factorisation with several 64-column steps (n = 240: chain + near/far workers), the multi-kernel fallback, the
-sliding-window marginalisation, the pose-covariance propagation, a multi-batch sparse evaluation, and the device
+tile-DAG factorisation with several 64-column steps (n = 240: chain + near/far workers), the sliding-window marginalisation, the pose-covariance propagation, a multi-batch sparse evaluation, and the device
 association chain balm_cut_voxels -> balm_marginalize -> balm_append_scan (octree keys + layers)."""
 import os, sys
 import numpy as np
