@@ -49,7 +49,8 @@ SYMBOLS = ["balm_last_error", "balm_version", "balm_create", "balm_destroy", "ba
            "balm_reset_counters", "balm_sync", "balm_timer_begin", "balm_timer_end", "balm_device_views", "balm_debug_dag_trace", "balm_synth_virtual",
            "balm_download_voxels", "balm_download_voxel_range", "balm_num_obs", "balm_default_assoc_opts", "balm_cut_voxels", "balm_pose_covariance", "balm_marginalize", "balm_download_fix", "balm_append_scan",
            "balm_download_keys", "balm_window_reset", "balm_window_cut", "balm_window_recut", "balm_window_marginalize",
-           "balm_window_push"]
+           "balm_window_push", "balm_batch_create", "balm_batch_destroy", "balm_batch_set_voxels", "balm_batch_evaluate",
+           "balm_batch_damping_iter"]
 
 
 def lib():
@@ -99,6 +100,12 @@ def lib():
         L.balm_window_recut.argtypes = [C.c_void_p, C.c_int]
         L.balm_window_marginalize.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int]
         L.balm_window_push.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
+        L.balm_batch_create.argtypes = [C.POINTER(C.c_void_p), C.c_int]
+        L.balm_batch_destroy.argtypes = [C.c_void_p]
+        L.balm_batch_set_voxels.argtypes = [C.c_void_p, C.c_int] + [C.c_void_p] * 7
+        L.balm_batch_evaluate.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.balm_batch_damping_iter.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(LmOpts), C.c_void_p, C.c_void_p,
+                                              C.c_void_p, C.c_void_p]
         _lib = L
     return _lib
 

@@ -216,3 +216,96 @@ class Context:
 
     def sync(self):
         L.check(L.lib().balm_sync(self._h))
+
+
+class Batch:
+    """One GPU, B independent small problems (at most 32 poses each) registered together; evaluation and LM run for all
+    of them at once, each problem with its own damping, accept / reject and stopping (include/balm_b200.h, balm_batch_*)."""
+
+    def __init__(self, device=0):
+        self._h = C.c_void_p()
+        self.n_poses = []
+        L.check(L.lib().balm_batch_create(C.byref(self._h), int(device)))
+
+    def close(self):
+        if self._h:
+            L.lib().balm_batch_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def set_problems(self, problems):
+        """problems: list of dicts with n_poses and the arrays Context.set_voxels takes (row_ptr, pose_idx, obs10, coe,
+        optional fix10). Problems without fix clusters get zero fix rows when others have them."""
+        n_poses = [int(p["n_poses"]) for p in problems]
+        row_ptrs = [np.asarray(p["row_ptr"], dtype=np.int64) for p in problems]
+        n_vox = [len(rp) - 1 for rp in row_ptrs]
+        pose_ptr = np.concatenate([[0], np.cumsum(n_poses)]).astype(np.int64)
+        voxel_ptr = np.concatenate([[0], np.cumsum(n_vox)]).astype(np.int64)
+        row_ptr, base = [np.zeros(1, dtype=np.int64)], 0
+        for rp in row_ptrs:
+            row_ptr.append(rp[1:] + base)
+            base += int(rp[-1])
+        row_ptr = np.ascontiguousarray(np.concatenate(row_ptr), dtype=np.int64)
+        pose_idx = np.ascontiguousarray(np.concatenate([np.asarray(p["pose_idx"], dtype=np.int32).ravel()
+                                                        for p in problems]), dtype=np.int32)
+        obs10 = np.ascontiguousarray(np.concatenate([np.asarray(p["obs10"], dtype=np.float64).reshape(-1, 10)
+                                                     for p in problems]), dtype=np.float64)
+        coe = np.ascontiguousarray(np.concatenate([np.asarray(p["coe"], dtype=np.float64).ravel() for p in problems]),
+                                   dtype=np.float64)
+        fix10 = None
+        if any(p.get("fix10") is not None for p in problems):
+            fix10 = np.ascontiguousarray(np.concatenate([
+                np.zeros((m, 10)) if p.get("fix10") is None else np.asarray(p["fix10"], dtype=np.float64).reshape(-1, 10)
+                for p, m in zip(problems, n_vox)]), dtype=np.float64)
+        L.check(L.lib().balm_batch_set_voxels(self._h, len(problems), _p(pose_ptr), _p(voxel_ptr), _p(row_ptr),
+                                              _p(pose_idx), _p(obs10), _p(fix10), _p(coe)))
+        self.n_poses = n_poses
+        self._pose_ptr = pose_ptr
+
+    def _concat(self, poses_list):
+        assert len(poses_list) == len(self.n_poses)
+        return np.ascontiguousarray(np.concatenate([np.asarray(p, dtype=np.float64).reshape(n, 12)
+                                                    for p, n in zip(poses_list, self.n_poses)]), dtype=np.float64)
+
+    def evaluate(self, poses_list, include_fix=False):
+        """left_evaluate_acc2 per problem -> list of (H, g, r)."""
+        poses = self._concat(poses_list)
+        ns = [6 * n for n in self.n_poses]
+        H = np.zeros(sum(n * n for n in ns))
+        g = np.zeros(6 * len(poses))
+        r = np.zeros(len(ns))
+        L.check(L.lib().balm_batch_evaluate(self._h, _p(poses), int(include_fix), _p(H), _p(g), _p(r)))
+        out, ho = [], 0
+        for b, n in enumerate(ns):
+            g0 = 6 * int(self._pose_ptr[b])
+            out.append((H[ho:ho + n * n].reshape(n, n, order="F"), g[g0:g0 + n].copy(), float(r[b])))
+            ho += n * n
+        return out
+
+    def damping_iter(self, poses_list, max_iter=10, u0=0.01, v0=2.0, rel_tol=1e-6, hess_includes_fix=False,
+                     gauge_mode=0, min_planes_per_pose=20, verbose=False, want_per_iter=False, force_hess=False):
+        """damping_iter per problem, all advanced together -> list of (status, poses, trace, per_iter)."""
+        poses = self._concat(poses_list)
+        B, P = len(self.n_poses), len(poses)
+        opts = L.LmOpts(max_iter, u0, v0, rel_tol, int(hess_includes_fix), gauge_mode, min_planes_per_pose,
+                        int(verbose), int(force_hess))
+        status = np.zeros(B, dtype=np.int32)
+        n_it = np.zeros(B, dtype=np.int32)
+        trace = (L.Trace * (B * max(1, max_iter)))()
+        per_iter = np.zeros((max_iter, P, 12)) if want_per_iter else None
+        L.check(L.lib().balm_batch_damping_iter(self._h, _p(poses), C.byref(opts), _p(status), _p(n_it), trace,
+                                                _p(per_iter)))
+        out = []
+        for b in range(B):
+            p0, p1 = int(self._pose_ptr[b]), int(self._pose_ptr[b + 1])
+            tr = [dict(r1=t.r1, r2=t.r2, u=t.u, v=t.v, q=t.q, q1=t.q1, accepted=bool(t.accepted),
+                       recomputed_hess=bool(t.recomputed_hess), not_pd=bool(t.not_pd))
+                  for t in trace[b * max_iter:b * max_iter + int(n_it[b])]]
+            out.append((int(status[b]), poses[p0:p1].copy(), tr,
+                        per_iter[:int(n_it[b]), p0:p1].copy() if want_per_iter else None))
+        return out

@@ -1,0 +1,821 @@
+// batch.cu -- batched bundle adjustment: B independent small problems (at most BALM_BATCH_MAX_POSES poses each),
+// registered once and optimised together, each with its own LM state (include/balm_b200.h, balm_batch_*).
+//
+// Per LM iteration, enqueued back to back on the batch's stream, every kernel masked per problem:
+//   batch_stats_kernel<true>   per voxel: cluster sums, eigen-decomposition, stats row, residual term (= the stats pass)
+//   batch_residual_kernel      per problem: fixed-order sum of its voxels' residual terms -> r1
+//   batch_obs_kernel           per 32-voxel chunk of one problem: G' rows (fp64, dense per problem) and the per-pose
+//                              gradient / diagonal-block partials (obs_terms, shared with obs_pass_kernel)
+//   batch_syrk_kernel          per (problem, 64x64 upper tile, 768-row chunk): DMMA partial of G'^T G'
+//   batch_assemble_kernel      per (problem, 64-column block): H = -sum of partials + blockdiag, g
+//   batch_solve_kernel         per problem, one CTA: unpivoted LDL^T of H + uD in shared memory, backward error, up to
+//                              3 rounds of refinement, q1, trial poses
+//   batch_stats_kernel<false> + batch_residual_kernel at the trial poses -> r2
+//   batch_lm_kernel            one thread per problem: accept / reject, u, v, trace, stop
+// The host waits once per iteration, for the number of problems still active. Every split of work depends on the
+// problem alone and every sum runs in a fixed order (no floating-point atomics), so a problem's results do not depend on
+// the other problems of the batch or on its position in it.
+#include <math.h>
+#include <string.h>
+#include <algorithm>
+#include <vector>
+#include "internal.cuh"
+
+namespace {
+
+constexpr int CHUNK = 32;                      // voxels per warp of the observation sweep
+constexpr int ROWS = 768;                      // G' rows (256 voxels) per SYRK work item
+constexpr int TILE = 64;                       // SYRK output tile
+constexpr int KB = 16;                         // G' rows per shared-memory stage of the SYRK
+constexpr int LDS = TILE + 4;
+constexpr int MAXN = 6 * BALM_BATCH_MAX_POSES;  // 192 unknowns
+constexpr int SOLVE_THREADS = 256;
+constexpr double OMEGA_TOL = 1e-12;            // componentwise backward error accepted without refinement (ldlt.cu)
+constexpr int SOLVE_SMEM = (MAXN * (MAXN + 1) / 2 + 5 * MAXN) * (int)sizeof(double);
+
+struct Prob {                  // layout of one problem, built on the host at registration
+  int pose_base, np, n, ldp;   // first pose in the concatenated array, poses, 6 np, G' row stride (n rounded up to 64)
+  int ochunk_base, n_ochunks;  // its observation-sweep chunks
+  int item_base, n_rchunks;    // its SYRK items: tile t, row chunk c -> item_base + t * n_rchunks + c
+  long long vox_base, nvox;    // its voxels
+  long long goff, hoff;        // offsets of its G' and H
+};
+
+struct Dev {  // what the kernels read
+  const Prob *prob;
+  const int *vox_prob;
+  const long long *row_ptr;
+  const int *pose_idx;
+  const double *obs;  // AoS [K][10]
+  const double *fix;  // AoS [M][10] or null
+  const double *coe;
+  int64_t M, K;
+};
+
+// ---- per voxel: the world-frame cluster sum over its observations (+ fix), eig, residual term, stats row ----
+template <bool STORE>
+__global__ void __launch_bounds__(256) batch_stats_kernel(Dev d, const double *poses, const int *mask, int use_fix,
+                                                          double *stats, double *res_v) {
+  const int lane = threadIdx.x & 31;
+  const int64_t nw = (int64_t)gridDim.x * 8;
+  for (int64_t v = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5); v < d.M; v += nw) {
+    const int b = d.vox_prob[v];
+    if (!mask[b]) continue;
+    const double *pz = poses + 12 * (size_t)d.prob[b].pose_base;
+    const long long s0 = d.row_ptr[v];
+    const int k = (int)(d.row_ptr[v + 1] - s0);  // <= BALM_BATCH_MAX_POSES (checked at registration)
+    double acc[10];
+#pragma unroll
+    for (int c = 0; c < 10; c++) acc[c] = 0.0;
+    if (lane < k) {
+      const double *o = d.obs + (size_t)(s0 + lane) * 10;
+      double r[9], p[3];
+      load_pose(pz + 12 * d.pose_idx[s0 + lane], r, p);
+      const WC w = world_cluster(o, r, p);
+      acc[0] = w.p00; acc[1] = w.p01; acc[2] = w.p02; acc[3] = w.p11; acc[4] = w.p12;
+      acc[5] = w.p22; acc[6] = w.v0;  acc[7] = w.v1;  acc[8] = w.v2;  acc[9] = w.n;
+    }
+#pragma unroll
+    for (int c = 0; c < 10; c++) {
+      acc[c] = warp_sum(acc[c]);
+      if (use_fix && d.fix) acc[c] += d.fix[(size_t)v * 10 + c];
+    }
+    if (lane == 0) {
+      const double inv = 1.0 / acc[9];
+      const double vb0 = acc[6] * inv, vb1 = acc[7] * inv, vb2 = acc[8] * inv;
+      double lam[3], u0[3], u1[3], u2[3];
+      eig3_jacobi(acc[0] * inv - vb0 * vb0, acc[1] * inv - vb0 * vb1, acc[2] * inv - vb0 * vb2,
+                  acc[3] * inv - vb1 * vb1, acc[4] * inv - vb1 * vb2, acc[5] * inv - vb2 * vb2, lam, u0, u1, u2);
+      const double coe = d.coe[v];
+      res_v[v] = coe * lam[0];
+      if (STORE) store_stats_row(stats + (size_t)v * BALM_STATS_STRIDE, vb0, vb1, vb2, u0, u1, u2, inv, coe, lam);
+    }
+  }
+}
+
+// ---- per problem: fixed-order sum of its voxels' residual terms ----
+__global__ void __launch_bounds__(128) batch_residual_kernel(const Prob *prob, const int *mask, const double *res_v,
+                                                             double *out) {
+  __shared__ double red[4];
+  const int b = blockIdx.x;
+  if (!mask[b]) return;
+  const Prob pr = prob[b];
+  double s = 0.0;
+  for (long long v = threadIdx.x; v < pr.nvox; v += 128) s += res_v[pr.vox_base + v];
+  s = warp_sum(s);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
+  __syncthreads();
+  if (threadIdx.x == 0) out[b] = (red[0] + red[1]) + (red[2] + red[3]);
+}
+
+// ---- per chunk of CHUNK voxels of one problem, one warp, lane = problem-local pose ----
+__global__ void __launch_bounds__(128) batch_obs_kernel(Dev d, const double *poses, const int *mask,
+                                                        const int *ochunk_prob, int n_ochunks, const double *stats,
+                                                        double *G, double *opart) {
+  __shared__ int slot_of[4][32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int c = blockIdx.x * 4 + warp;
+  if (c >= n_ochunks) return;
+  const int b = ochunk_prob[c];
+  if (!mask[b]) return;
+  const Prob pr = d.prob[b];
+  const bool active = lane < pr.np;
+  double r[9], p[3];
+  if (active) load_pose(poses + 12 * (size_t)(pr.pose_base + lane), r, p);
+  double acc[27];
+#pragma unroll
+  for (int q = 0; q < 27; q++) acc[q] = 0.0;
+  const long long v0 = pr.vox_base + (long long)(c - pr.ochunk_base) * CHUNK;
+  const long long v1 = v0 + CHUNK < pr.vox_base + pr.nvox ? v0 + CHUNK : pr.vox_base + pr.nvox;
+  for (long long v = v0; v < v1; v++) {
+    const long long s0 = d.row_ptr[v];
+    const int k = (int)(d.row_ptr[v + 1] - s0);
+    slot_of[warp][lane] = -1;
+    __syncwarp();
+    if (lane < k) slot_of[warp][d.pose_idx[s0 + lane]] = lane;  // pose_idx < np <= 32 (checked at registration)
+    __syncwarp();
+    const int slot = slot_of[warp][lane];
+    __syncwarp();
+    if (slot < 0) continue;
+    double o[10], st[BALM_SWEEP_WORDS];
+    const double2 *o2 = reinterpret_cast<const double2 *>(d.obs + (size_t)(s0 + slot) * 10);
+    const double2 *st2 = reinterpret_cast<const double2 *>(stats + (size_t)v * BALM_STATS_STRIDE + BALM_SWEEP_OFF);
+#pragma unroll
+    for (int q = 0; q < 5; q++) {
+      const double2 x = __ldg(o2 + q);
+      o[2 * q] = x.x;
+      o[2 * q + 1] = x.y;
+    }
+#pragma unroll
+    for (int q = 0; q < BALM_SWEEP_WORDS / 2; q++) {
+      const double2 x = __ldg(st2 + q);
+      st[2 * q] = x.x;
+      st[2 * q + 1] = x.y;
+    }
+    double *g0 = G + pr.goff + (size_t)(3 * (v - pr.vox_base)) * pr.ldp + 6 * lane;
+    obs_terms<true>(o, r, p, st, acc, [&](const double (&gv)[3][6]) {
+#pragma unroll
+      for (int rr = 0; rr < 3; rr++) {
+        double2 *qd = reinterpret_cast<double2 *>(g0 + (size_t)rr * pr.ldp);
+#pragma unroll
+        for (int h = 0; h < 3; h++) qd[h] = make_double2(gv[rr][2 * h], gv[rr][2 * h + 1]);
+      }
+    });
+  }
+  if (active) {
+    double *pp = opart + (size_t)c * 27 * 32 + lane;
+#pragma unroll
+    for (int q = 0; q < 27; q++) pp[q * 32] = acc[q];
+  }
+}
+
+// ---- per (problem, upper 64x64 tile, 768-row chunk): partial of G'^T G' with DMMA, 2 x 2 warps of 32 x 32 ----
+__global__ void __launch_bounds__(128) batch_syrk_kernel(const Prob *prob, const int *mask, const int4 *items,
+                                                         const double *G, double *spart) {
+  __shared__ __align__(16) double sA[KB][LDS], sB[KB][LDS];
+  const int4 it = items[blockIdx.x];  // (problem, tile row, tile column, row chunk)
+  if (!mask[it.x]) return;
+  const Prob pr = prob[it.x];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int wm = warp >> 1, wn = warp & 1, fr = lane >> 2, fk = lane & 3;
+  const long long rows = 3 * pr.nvox, k_begin = (long long)it.w * ROWS;
+  const long long k_end = k_begin + ROWS < rows ? k_begin + ROWS : rows;
+  const double *gA = G + pr.goff + it.y * TILE, *gB = G + pr.goff + it.z * TILE;
+  double acc[4][4][2];
+#pragma unroll
+  for (int i = 0; i < 4; i++)
+#pragma unroll
+    for (int j = 0; j < 4; j++) acc[i][j][0] = acc[i][j][1] = 0.0;
+  for (long long k0 = k_begin; k0 < k_end; k0 += KB) {
+    for (int e = tid; e < KB * TILE / 2; e += 128) {
+      const int rr = e / (TILE / 2), cc = (e % (TILE / 2)) * 2;
+      const long long kr = k0 + rr;
+      double2 va = make_double2(0.0, 0.0), vb = va;
+      if (kr < k_end) {
+        va = *reinterpret_cast<const double2 *>(gA + (size_t)kr * pr.ldp + cc);
+        vb = *reinterpret_cast<const double2 *>(gB + (size_t)kr * pr.ldp + cc);
+      }
+      *reinterpret_cast<double2 *>(&sA[rr][cc]) = va;
+      *reinterpret_cast<double2 *>(&sB[rr][cc]) = vb;
+    }
+    __syncthreads();
+#pragma unroll
+    for (int kk = 0; kk < KB; kk += 4) {
+      double af[4], bf[4];
+#pragma unroll
+      for (int i = 0; i < 4; i++) af[i] = sA[kk + fk][wm * 32 + i * 8 + fr];
+#pragma unroll
+      for (int j = 0; j < 4; j++) bf[j] = sB[kk + fk][wn * 32 + j * 8 + fr];
+#pragma unroll
+      for (int i = 0; i < 4; i++)
+#pragma unroll
+        for (int j = 0; j < 4; j++) dmma_8x8x4(acc[i][j][0], acc[i][j][1], af[i], bf[j]);
+    }
+    __syncthreads();
+  }
+  double *out = spart + (size_t)blockIdx.x * TILE * TILE;
+#pragma unroll
+  for (int i = 0; i < 4; i++)
+#pragma unroll
+    for (int j = 0; j < 4; j++) {
+      const int row = wm * 32 + i * 8 + fr, col = wn * 32 + j * 8 + 2 * fk;
+      *reinterpret_cast<double2 *>(out + row * TILE + col) = make_double2(acc[i][j][0], acc[i][j][1]);
+    }
+}
+
+// ---- per (problem, 64-column block): H = -sum over row chunks of the SYRK partials + blockdiag, g ----
+// Element (i, j) and (j, i) are computed from the same upper partial, so H is exactly symmetric.
+__global__ void __launch_bounds__(256) batch_assemble_kernel(const Prob *prob, const int *mask, const double *opart,
+                                                             const double *spart, double *H, double *g) {
+  __shared__ double accs[27][32];
+  const int b = blockIdx.x;
+  if (!mask[b]) return;
+  const Prob pr = prob[b];
+  const int n = pr.n, nt = pr.ldp / TILE;
+  if (blockIdx.y * TILE >= n) return;
+  for (int e = threadIdx.x; e < 27 * pr.np; e += 256) {
+    const int q = e / pr.np, i = e % pr.np;
+    double s = 0.0;
+    for (int c = 0; c < pr.n_ochunks; c++) s += opart[((size_t)(pr.ochunk_base + c) * 27 + q) * 32 + i];
+    accs[q][i] = s;
+  }
+  __syncthreads();
+  double *Hb = H + pr.hoff;
+  const int j_end = (blockIdx.y + 1) * TILE < n ? (blockIdx.y + 1) * TILE : n;
+  for (int j = blockIdx.y * TILE; j < j_end; j++) {
+    for (int i = threadIdx.x; i < n; i += 256) {
+      const int rr = i < j ? i : j, cc = i < j ? j : i;
+      const int bi = rr / TILE, bj = cc / TILE;
+      const int t = bi * nt - bi * (bi - 1) / 2 + (bj - bi);
+      const double *src = spart + (size_t)(pr.item_base + t * pr.n_rchunks) * TILE * TILE + (rr % TILE) * TILE + cc % TILE;
+      double s = 0.0;
+      for (int c = 0; c < pr.n_rchunks; c++) s += src[(size_t)c * TILE * TILE];
+      double h = -s;
+      const int pi = rr / 6;
+      if (pi == cc / 6) {
+        const int r6 = rr % 6, c6 = cc % 6;
+        h += accs[6 + r6 * 6 - r6 * (r6 - 1) / 2 + (c6 - r6)][pi];
+      }
+      Hb[(size_t)j * n + i] = h;
+    }
+  }
+  if (blockIdx.y == 0)
+    for (int i = threadIdx.x; i < n; i += 256) g[6 * (size_t)pr.pose_base + i] = accs[i % 6][i / 6];
+}
+
+// ---- damped solve, one CTA per problem, the packed lower triangle of H + uD in shared memory ----
+__device__ __forceinline__ int tri_idx(int i, int j, int n) { return j * n - j * (j - 1) / 2 + (i - j); }  // i >= j
+
+// w <- (L D L^T)^-1 w with the factors in A (unit-lower L below the diagonal, D on it)
+__device__ void ldl_apply(const double *A, int n, double *w) {
+  for (int k = 0; k < n; k++) {  // L y = w
+    const double wk = w[k];
+    for (int i = k + 1 + threadIdx.x; i < n; i += SOLVE_THREADS) w[i] -= A[tri_idx(i, k, n)] * wk;
+    __syncthreads();
+  }
+  for (int i = threadIdx.x; i < n; i += SOLVE_THREADS) w[i] /= A[tri_idx(i, i, n)];
+  __syncthreads();
+  for (int k = n - 1; k >= 0; k--) {  // L^T x = y
+    const double xk = w[k];
+    for (int i = threadIdx.x; i < k; i += SOLVE_THREADS) w[i] -= A[tri_idx(k, i, n)] * xk;
+    __syncthreads();
+  }
+}
+
+// componentwise backward error of x for (H + uD) x = -g, computed from H (Oettli-Prager, as solve_residual_kernel):
+// rres = b - A x; returns whether it exceeds OMEGA_TOL anywhere
+__device__ bool backward_error(const double *Hb, const double *gb, int n, double u, const double *x, double *rres) {
+  bool bad = false;
+  const int i = threadIdx.x;
+  if (i < n) {
+    double s = 0.0, sa = 0.0;
+    for (int j = 0; j < n; j++) {  // H exactly symmetric: row i = column i
+      double h = Hb[(size_t)j * n + i];
+      if (j == i) h += u * h;
+      const double t = h * x[j];
+      s += t;
+      sa += fabs(t);
+    }
+    const double b = -gb[i], r = b - s, den = sa + fabs(b);
+    rres[i] = r;
+    const double om = den > 0.0 ? fabs(r) / den : 0.0;
+    bad = !(om <= OMEGA_TOL);
+  }
+  return __syncthreads_or(bad) != 0;
+}
+
+// q1 = 0.5 dx.(u D dx - g)  (bavoxel.hpp:1127), block-wide, fixed order
+__device__ double damped_q1(const double *x, const double *D, const double *gb, int n, double u, double *red) {
+  const int tid = threadIdx.x;
+  double part = tid < n ? x[tid] * (u * D[tid] * x[tid] - gb[tid]) : 0.0;
+  part = warp_sum(part);
+  if ((tid & 31) == 0) red[tid >> 5] = part;
+  __syncthreads();
+  double s = 0.0;
+#pragma unroll
+  for (int q = 0; q < SOLVE_THREADS / 32; q++) s += red[q];
+  __syncthreads();
+  return 0.5 * s;
+}
+
+__global__ void __launch_bounds__(SOLVE_THREADS) batch_solve_kernel(const Prob *prob, const int *active, const double *H,
+                                                                    const double *g, const double *uvec,
+                                                                    const double *poses, double *trial, double *q1_out,
+                                                                    int *notpd_out) {
+  extern __shared__ double sm[];
+  __shared__ double red[SOLVE_THREADS / 32];
+  const int b = blockIdx.x;
+  if (!active[b]) return;
+  const Prob pr = prob[b];
+  const int n = pr.n, tid = threadIdx.x;
+  double *A = sm, *D = A + n * (n + 1) / 2, *x = D + MAXN, *w = x + MAXN, *rres = w + MAXN, *col = rres + MAXN;
+  const double *Hb = H + pr.hoff, *gb = g + 6 * (size_t)pr.pose_base;
+  const double u = uvec[b];
+  for (int e = tid; e < n * n; e += SOLVE_THREADS) {  // A = H + u diag(H), as damp_copy_kernel
+    const int j = e / n, i = e % n;
+    if (i < j) continue;
+    double h = Hb[e];
+    if (i == j) {
+      D[i] = h;
+      h += u * h;
+    }
+    A[tri_idx(i, j, n)] = h;
+  }
+  for (int i = tid; i < n; i += SOLVE_THREADS) x[i] = -gb[i];
+  __syncthreads();
+  // unpivoted right-looking LDL^T; a zero / tiny / non-finite pivot (ldlt.cu's criterion) makes the step not_pd
+  bool pivot_bad = false;
+  for (int k = 0; k < n; k++) {
+    const int kk = tri_idx(k, k, n);
+    const double dk = A[kk];
+    if (!(fabs(dk) > 1e-290 && fabs(dk) < 1e300)) { pivot_bad = true; break; }
+    for (int i = k + 1 + tid; i < n; i += SOLVE_THREADS) {
+      const double t = A[kk + i - k];
+      col[i] = t;
+      A[kk + i - k] = t / dk;
+    }
+    __syncthreads();
+    const int lane = tid & 31, warp = tid >> 5;
+    for (int j = k + 1 + warp; j < n; j += SOLVE_THREADS / 32) {
+      const double cj = col[j];
+      double *Aj = A + tri_idx(j, j, n);
+      for (int i = j + lane; i < n; i += 32) Aj[i - j] -= A[kk + i - k] * cj;
+    }
+    __syncthreads();
+  }
+  int not_pd = pivot_bad ? 1 : 0;
+  double q1 = 0.0;
+  if (!pivot_bad) {
+    ldl_apply(A, n, x);
+    bool omega_bad = backward_error(Hb, gb, n, u, x, rres);
+    q1 = damped_q1(x, D, gb, n, u, red);
+    not_pd = isfinite(q1) ? 0 : 1;
+    if (!not_pd && omega_bad) {  // fp64 iterative refinement with the same factors (refine_solution)
+      for (int round = 0; round < 3 && omega_bad; round++) {
+        for (int i = tid; i < n; i += SOLVE_THREADS) w[i] = rres[i];
+        __syncthreads();
+        ldl_apply(A, n, w);
+        for (int i = tid; i < n; i += SOLVE_THREADS) x[i] += w[i];
+        __syncthreads();
+        omega_bad = backward_error(Hb, gb, n, u, x, rres);
+      }
+      q1 = damped_q1(x, D, gb, n, u, red);
+      if (omega_bad || !isfinite(q1)) not_pd = 1;
+    }
+  } else {
+    for (int i = tid; i < n; i += SOLVE_THREADS) x[i] = 0.0;
+    __syncthreads();
+  }
+  if (tid < pr.np) {
+    const size_t o = 12 * (size_t)(pr.pose_base + tid);
+    pose_update_one(poses + o, x + 6 * tid, trial + o);
+  }
+  if (tid == 0) {
+    q1_out[b] = q1;
+    notpd_out[b] = not_pd;
+  }
+}
+
+struct LmArgs {
+  const Prob *prob;
+  int B, it, max_iter, force_hess;
+  double rel_tol;
+  const double *r_eval, *r2, *q1;
+  const int *notpd;
+  double *r1, *u, *v;
+  int *active, *calc, *evalm, *n_iters, *n_active;
+  double *poses;
+  const double *trial;
+  balm_trace *trace;  // [B][max_iter]
+};
+
+// ---- LM control, one thread per problem: the host loop of balm_damping_iter (bavoxel.hpp:1129-1155) ----
+__global__ void batch_lm_kernel(LmArgs a) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= a.B || !a.active[b]) return;
+  const int calc = a.calc[b];
+  const double r1 = calc ? a.r_eval[b] : a.r1[b], r2 = a.r2[b], q1 = a.q1[b];
+  const int not_pd = a.notpd[b];
+  double u = a.u[b], v = a.v[b];
+  double q = r1 - r2;
+  if (not_pd || !isfinite(r2)) q = -1.0;  // unusable step -> rejected, u *= v
+  balm_trace t{r1, r2, u, v, q, q1, 0, calc, not_pd};
+  int next_calc;
+  if (q > 0) {  // bavoxel.hpp:1134-1143
+    const Prob pr = a.prob[b];
+    for (int e = 0; e < 12 * pr.np; e++) a.poses[12 * (size_t)pr.pose_base + e] = a.trial[12 * (size_t)pr.pose_base + e];
+    const double rho = q / q1;
+    v = 2;
+    const double f = 1 - pow(2 * rho - 1, 3.0);
+    u *= (f < (1.0 / 3.0) ? (1.0 / 3.0) : f);
+    next_calc = 1;
+    t.accepted = 1;
+  } else {  // bavoxel.hpp:1144-1149
+    u = u * v;
+    v = 2 * v;
+    next_calc = a.force_hess;
+  }
+  a.trace[(size_t)b * a.max_iter + a.it] = t;
+  a.n_iters[b] = a.it + 1;
+  a.r1[b] = r1;
+  a.u[b] = u;
+  a.v[b] = v;
+  a.calc[b] = next_calc;
+  const bool stop = (a.rel_tol >= 0 && fabs(r1 - r2) / r1 < a.rel_tol) || a.it + 1 >= a.max_iter;  // bavoxel.hpp:1155
+  a.evalm[b] = stop ? 0 : next_calc;
+  if (stop) a.active[b] = 0;
+  else atomicAdd(a.n_active, 1);
+}
+
+// ---- gauge step per pose, pose 0 of each problem read from a snapshot ----
+__global__ void batch_gauge_kernel(const Prob *prob, const int *pose_prob, const int *status, int P, double *poses,
+                                   const double *snapshot, int mode) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= P) return;
+  const int b = pose_prob[j];
+  if (status[b] != BALM_OK) return;
+  const int base = prob[b].pose_base;
+  gauge_one(poses + 12 * (size_t)j, snapshot + 12 * (size_t)base, mode == 1 && j == base);
+}
+
+// ---- registration: per voxel, the CSR invariants and the per-pose voxel counts ----
+__global__ void batch_check_kernel(Dev d, int *bad, int *planes) {
+  const int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= d.M) return;
+  const Prob pr = d.prob[d.vox_prob[v]];
+  const long long s0 = d.row_ptr[v], s1 = d.row_ptr[v + 1];
+  if (s0 < 0 || s1 < s0 || s1 > d.K || s1 - s0 > pr.np) { atomicOr(bad, 1); return; }
+  int prev = -1;
+  for (long long s = s0; s < s1; s++) {
+    const int p = d.pose_idx[s];
+    if (p <= prev || p >= pr.np) { atomicOr(bad, 1); return; }
+    prev = p;
+  }
+  for (long long s = s0; s < s1; s++) atomicAdd(&planes[pr.pose_base + d.pose_idx[s]], 1);
+}
+
+__global__ void batch_init_kernel(int B, const int *status, int max_iter, double u0, double v0, double *u, double *v,
+                                  int *active, int *calc, int *evalm, int *n_iters) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  const int on = status[b] == BALM_OK && max_iter > 0;
+  u[b] = u0; v[b] = v0; active[b] = on; calc[b] = 1; evalm[b] = on; n_iters[b] = 0;
+}
+
+__global__ void fill_kernel(int *p, int n, int val) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) p[i] = val;
+}
+
+}  // namespace
+
+// One registration: the problems, their voxels and every workspace sized for them. A new registration is built and
+// checked completely before it replaces the previous one.
+struct BatchReg {
+  int B = 0, P = 0, n_ochunks = 0, n_items = 0;
+  int64_t M = 0, K = 0;
+  std::vector<Prob> hprob;
+  std::vector<int> min_planes;  // per problem: the fewest voxels observing one of its poses
+  size_t H_size = 0, G_size = 0;
+  Prob *prob = nullptr;
+  int *vox_prob = nullptr, *pose_prob = nullptr, *ochunk_prob = nullptr;
+  int4 *items = nullptr;
+  long long *row_ptr = nullptr;
+  int *pose_idx = nullptr;
+  double *obs = nullptr, *fix = nullptr, *coe = nullptr;
+  double *G = nullptr, *stats = nullptr, *res_v = nullptr, *opart = nullptr, *spart = nullptr, *H = nullptr, *g = nullptr;
+  double *poses = nullptr, *trial = nullptr;
+  double *r_eval = nullptr, *r2 = nullptr, *r1 = nullptr, *q1 = nullptr, *u = nullptr, *v = nullptr;
+  int *ints = nullptr;  // [7][B]: notpd, active, calc, evalm, n_iters, status, ones; then n_active
+  int *notpd() { return ints; }
+  int *active() { return ints + B; }
+  int *calc() { return ints + 2 * B; }
+  int *evalm() { return ints + 3 * B; }
+  int *n_iters() { return ints + 4 * B; }
+  int *status() { return ints + 5 * B; }
+  int *ones() { return ints + 6 * B; }
+  int *n_active() { return ints + 7 * B; }
+  Dev dev() const { return Dev{prob, vox_prob, row_ptr, pose_idx, obs, fix, coe, M, K}; }
+  ~BatchReg() {
+    void *ptrs[] = {prob, vox_prob, pose_prob, ochunk_prob, items, row_ptr, pose_idx, obs, fix, coe, G, stats, res_v,
+                    opart, spart, H, g, poses, trial, r_eval, r2, r1, q1, u, v, ints};
+    for (void *p : ptrs) cudaFree(p);
+  }
+};
+
+struct balm_batch {
+  int device = 0, sm_count = 132;
+  cudaStream_t stream = nullptr;
+  BatchReg *reg = nullptr;
+  int *h_count = nullptr;  // pinned: problems still active after an iteration
+};
+
+namespace {
+
+template <typename T>
+int dalloc(T **p, size_t count) {
+  CUDA_TRY(cudaMalloc((void **)p, sizeof(T) * (count ? count : 1)));
+  return BALM_OK;
+}
+template <typename T>
+int upload(T **p, const T *src, size_t count, cudaStream_t st) {
+  const int rc = dalloc(p, count);
+  if (rc != BALM_OK) return rc;
+  if (count) CUDA_TRY(cudaMemcpyAsync(*p, src, sizeof(T) * count, cudaMemcpyHostToDevice, st));
+  return BALM_OK;
+}
+#define BTRY(x)                     \
+  do {                              \
+    const int _s = (x);             \
+    if (_s != BALM_OK) return _s;   \
+  } while (0)
+
+int invalid(const char *msg) {
+  balm_set_error(msg);
+  return BALM_ERR_INVALID;
+}
+
+// The evaluation of every problem with mask[b] != 0 at r->poses: r_eval, H, g.
+int enqueue_eval(balm_batch *bt, BatchReg *r, const int *mask, bool use_fix) {
+  cudaStream_t st = bt->stream;
+  const Dev d = r->dev();
+  if (r->M > 0) {
+    const int blocks = (int)std::min<int64_t>((r->M + 7) / 8, (int64_t)bt->sm_count * 8);
+    batch_stats_kernel<true><<<blocks, 256, 0, st>>>(d, r->poses, mask, use_fix ? 1 : 0, r->stats, r->res_v);
+  }
+  batch_residual_kernel<<<r->B, 128, 0, st>>>(r->prob, mask, r->res_v, r->r_eval);
+  if (r->n_ochunks > 0)
+    batch_obs_kernel<<<(r->n_ochunks + 3) / 4, 128, 0, st>>>(d, r->poses, mask, r->ochunk_prob, r->n_ochunks, r->stats,
+                                                             r->G, r->opart);
+  if (r->n_items > 0) batch_syrk_kernel<<<r->n_items, 128, 0, st>>>(r->prob, mask, r->items, r->G, r->spart);
+  batch_assemble_kernel<<<dim3(r->B, MAXN / TILE), 256, 0, st>>>(r->prob, mask, r->opart, r->spart, r->H, r->g);
+  CUDA_TRY(cudaGetLastError());
+  return BALM_OK;
+}
+
+// The residual (fix clusters included, as evaluate_only_residual) at the trial poses of every active problem: r2.
+int enqueue_trial_residual(balm_batch *bt, BatchReg *r) {
+  cudaStream_t st = bt->stream;
+  if (r->M > 0) {
+    const int blocks = (int)std::min<int64_t>((r->M + 7) / 8, (int64_t)bt->sm_count * 8);
+    batch_stats_kernel<false><<<blocks, 256, 0, st>>>(r->dev(), r->trial, r->active(), 1, nullptr, r->res_v);
+  }
+  batch_residual_kernel<<<r->B, 128, 0, st>>>(r->prob, r->active(), r->res_v, r->r2);
+  CUDA_TRY(cudaGetLastError());
+  return BALM_OK;
+}
+
+}  // namespace
+
+extern "C" int balm_batch_create(balm_batch **out, int device) {
+  if (!out) return invalid("balm_batch_create: bad arguments");
+  int ndev = 0;
+  CUDA_TRY(cudaGetDeviceCount(&ndev));
+  if (device < 0 || device >= ndev) { balm_set_error("balm_batch_create: no such CUDA device"); return BALM_ERR_CUDA; }
+  CUDA_TRY(cudaSetDevice(device));
+  cudaDeviceProp prop;
+  CUDA_TRY(cudaGetDeviceProperties(&prop, device));
+  CUDA_TRY(cudaFuncSetAttribute(batch_solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SOLVE_SMEM));
+  balm_batch *b = new balm_batch();
+  b->device = device;
+  b->sm_count = prop.multiProcessorCount;
+  if (cudaStreamCreateWithFlags(&b->stream, cudaStreamNonBlocking) != cudaSuccess ||
+      cudaMallocHost((void **)&b->h_count, sizeof(int)) != cudaSuccess) {
+    balm_set_error("balm_batch_create: stream / pinned buffer allocation failed");
+    if (b->stream) cudaStreamDestroy(b->stream);
+    delete b;
+    return BALM_ERR_CUDA;
+  }
+  *out = b;
+  return BALM_OK;
+}
+
+extern "C" int balm_batch_destroy(balm_batch *b) {
+  if (!b) return BALM_OK;
+  cudaSetDevice(b->device);
+  cudaStreamSynchronize(b->stream);
+  delete b->reg;
+  cudaFreeHost(b->h_count);
+  cudaStreamDestroy(b->stream);
+  delete b;
+  return BALM_OK;
+}
+
+static int build_registration(balm_batch *bt, BatchReg *r, int B, const int64_t *pose_ptr, const int64_t *voxel_ptr,
+                              const int64_t *row_ptr, const int32_t *pose_idx, const double *obs10,
+                              const double *fix10, const double *coe) {
+  cudaStream_t st = bt->stream;
+  r->B = B;
+  r->P = (int)pose_ptr[B];
+  r->M = voxel_ptr[B];
+  r->K = row_ptr[r->M];
+  // host-side layout: problems, observation-sweep chunks, SYRK items, voxel -> problem, pose -> problem
+  std::vector<int> vox_prob((size_t)r->M), pose_prob((size_t)r->P), ochunk_prob;
+  std::vector<int4> items;
+  r->hprob.resize(B);
+  long long goff = 0, hoff = 0;
+  for (int b = 0; b < B; b++) {
+    Prob &p = r->hprob[b];
+    p.pose_base = (int)pose_ptr[b];
+    p.np = (int)(pose_ptr[b + 1] - pose_ptr[b]);
+    p.n = 6 * p.np;
+    p.ldp = (p.n + TILE - 1) / TILE * TILE;
+    p.vox_base = voxel_ptr[b];
+    p.nvox = voxel_ptr[b + 1] - voxel_ptr[b];
+    p.ochunk_base = (int)ochunk_prob.size();
+    p.n_ochunks = (int)((p.nvox + CHUNK - 1) / CHUNK);
+    ochunk_prob.insert(ochunk_prob.end(), (size_t)p.n_ochunks, b);
+    p.item_base = (int)items.size();
+    p.n_rchunks = (int)((3 * p.nvox + ROWS - 1) / ROWS);
+    const int nt = p.ldp / TILE;
+    for (int ti = 0; ti < nt; ti++)
+      for (int tj = ti; tj < nt; tj++)
+        for (int c = 0; c < p.n_rchunks; c++) items.push_back(make_int4(b, ti, tj, c));
+    p.goff = goff;
+    p.hoff = hoff;
+    goff += 3 * p.nvox * p.ldp;
+    hoff += (long long)p.n * p.n;
+    std::fill(vox_prob.begin() + p.vox_base, vox_prob.begin() + p.vox_base + p.nvox, b);
+    std::fill(pose_prob.begin() + p.pose_base, pose_prob.begin() + p.pose_base + p.np, b);
+  }
+  r->n_ochunks = (int)ochunk_prob.size();
+  r->n_items = (int)items.size();
+  r->G_size = (size_t)goff;
+  r->H_size = (size_t)hoff;
+  BTRY(upload(&r->prob, r->hprob.data(), (size_t)B, st));
+  BTRY(upload(&r->vox_prob, vox_prob.data(), vox_prob.size(), st));
+  BTRY(upload(&r->pose_prob, pose_prob.data(), pose_prob.size(), st));
+  BTRY(upload(&r->ochunk_prob, ochunk_prob.data(), ochunk_prob.size(), st));
+  BTRY(upload(&r->items, items.data(), items.size(), st));
+  BTRY(upload(&r->row_ptr, reinterpret_cast<const long long *>(row_ptr), (size_t)r->M + 1, st));
+  BTRY(upload(&r->pose_idx, pose_idx, (size_t)r->K, st));
+  BTRY(upload(&r->obs, obs10, (size_t)r->K * 10, st));
+  if (fix10) BTRY(upload(&r->fix, fix10, (size_t)r->M * 10, st));
+  BTRY(upload(&r->coe, coe, (size_t)r->M, st));
+  BTRY(dalloc(&r->ints, 7 * (size_t)B + 1));
+  int *d_planes = nullptr;
+  BTRY(dalloc(&d_planes, (size_t)r->P));
+  CUDA_TRY(cudaMemsetAsync(d_planes, 0, sizeof(int) * r->P, st));
+  CUDA_TRY(cudaMemsetAsync(r->n_active(), 0, sizeof(int), st));  // serves as the check's error flag here
+  if (r->M > 0) batch_check_kernel<<<(unsigned)((r->M + 127) / 128), 128, 0, st>>>(r->dev(), r->n_active(), d_planes);
+  std::vector<int> planes((size_t)r->P);
+  int bad = 0;
+  CUDA_TRY(cudaMemcpyAsync(&bad, r->n_active(), sizeof(int), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaMemcpyAsync(planes.data(), d_planes, sizeof(int) * r->P, cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  cudaFree(d_planes);
+  if (bad) return invalid("balm_batch_set_voxels: inside a voxel, pose_idx must be ascending and in [0, N_p) of its problem");
+  r->min_planes.resize(B);
+  for (int b = 0; b < B; b++) {
+    const Prob &p = r->hprob[b];
+    r->min_planes[b] = *std::min_element(planes.begin() + p.pose_base, planes.begin() + p.pose_base + p.np);
+  }
+  // workspaces
+  BTRY(dalloc(&r->G, r->G_size));
+  CUDA_TRY(cudaMemsetAsync(r->G, 0, sizeof(double) * r->G_size, st));  // columns of non-observing poses stay zero
+  BTRY(dalloc(&r->stats, (size_t)r->M * BALM_STATS_STRIDE));
+  BTRY(dalloc(&r->res_v, (size_t)r->M));
+  BTRY(dalloc(&r->opart, (size_t)r->n_ochunks * 27 * 32));
+  BTRY(dalloc(&r->spart, (size_t)r->n_items * TILE * TILE));
+  BTRY(dalloc(&r->H, r->H_size));
+  BTRY(dalloc(&r->g, 6 * (size_t)r->P));
+  BTRY(dalloc(&r->poses, 12 * (size_t)r->P));
+  BTRY(dalloc(&r->trial, 12 * (size_t)r->P));
+  double **scal[] = {&r->r_eval, &r->r2, &r->r1, &r->q1, &r->u, &r->v};
+  for (double **p : scal) BTRY(dalloc(p, (size_t)B));
+  fill_kernel<<<(B + 127) / 128, 128, 0, st>>>(r->ones(), B, 1);
+  CUDA_TRY(cudaGetLastError());
+  CUDA_TRY(cudaStreamSynchronize(st));
+  return BALM_OK;
+}
+
+extern "C" int balm_batch_set_voxels(balm_batch *bt, int n_problems, const int64_t *pose_ptr, const int64_t *voxel_ptr,
+                                     const int64_t *row_ptr, const int32_t *pose_idx, const double *obs10,
+                                     const double *fix10, const double *coe) {
+  if (!bt || !pose_ptr || !voxel_ptr || !row_ptr) return invalid("balm_batch_set_voxels: bad arguments");
+  if (n_problems < 1) return invalid("balm_batch_set_voxels: n_problems must be >= 1");
+  if (pose_ptr[0] != 0 || voxel_ptr[0] != 0) return invalid("balm_batch_set_voxels: pose_ptr[0] and voxel_ptr[0] must be 0");
+  for (int b = 0; b < n_problems; b++) {
+    const int64_t np = pose_ptr[b + 1] - pose_ptr[b];
+    if (np < 1 || np > BALM_BATCH_MAX_POSES)
+      return invalid("balm_batch_set_voxels: every problem needs 1 .. BALM_BATCH_MAX_POSES poses (pose_ptr ascending)");
+    if (voxel_ptr[b + 1] < voxel_ptr[b]) return invalid("balm_batch_set_voxels: voxel_ptr must be ascending");
+  }
+  const int64_t M = voxel_ptr[n_problems];
+  if (row_ptr[0] != 0) return invalid("balm_batch_set_voxels: row_ptr[0] must be 0");
+  const int64_t K = row_ptr[M];
+  if (K < 0 || (K > 0 && (!pose_idx || !obs10)) || (M > 0 && !coe)) return invalid("balm_batch_set_voxels: bad arguments");
+  if (K >= ((int64_t)1 << 31) || pose_ptr[n_problems] >= ((int64_t)1 << 31)) {
+    balm_set_error("balm_batch_set_voxels: more than 2^31 observations or poses");
+    return BALM_ERR_UNSUPPORTED;
+  }
+  CUDA_TRY(cudaSetDevice(bt->device));
+  CUDA_TRY(cudaStreamSynchronize(bt->stream));
+  BatchReg *r = new BatchReg();
+  const int rc = build_registration(bt, r, n_problems, pose_ptr, voxel_ptr, row_ptr, pose_idx, obs10, fix10, coe);
+  if (rc != BALM_OK) {  // the previous registration stays in place
+    cudaStreamSynchronize(bt->stream);
+    delete r;
+    return rc;
+  }
+  delete bt->reg;
+  bt->reg = r;
+  return BALM_OK;
+}
+
+extern "C" int balm_batch_evaluate(balm_batch *bt, const double *poses12, int include_fix, double *H, double *g,
+                                   double *residual) {
+  if (!bt || !poses12 || !residual) return invalid("balm_batch_evaluate: bad arguments");
+  BatchReg *r = bt->reg;
+  if (!r) return invalid("balm_batch_evaluate: no problems registered");
+  CUDA_TRY(cudaSetDevice(bt->device));
+  cudaStream_t st = bt->stream;
+  CUDA_TRY(cudaMemcpyAsync(r->poses, poses12, sizeof(double) * 12 * r->P, cudaMemcpyHostToDevice, st));
+  BTRY(enqueue_eval(bt, r, r->ones(), include_fix != 0));
+  if (H) CUDA_TRY(cudaMemcpyAsync(H, r->H, sizeof(double) * r->H_size, cudaMemcpyDeviceToHost, st));
+  if (g) CUDA_TRY(cudaMemcpyAsync(g, r->g, sizeof(double) * 6 * r->P, cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaMemcpyAsync(residual, r->r_eval, sizeof(double) * r->B, cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  return BALM_OK;
+}
+
+extern "C" int balm_batch_damping_iter(balm_batch *bt, double *poses12, const balm_lm_opts *o, int *status,
+                                       int *n_iters, balm_trace *trace, double *poses_per_iter) {
+  if (!bt || !poses12 || !o || !status || !n_iters) return invalid("balm_batch_damping_iter: bad arguments");
+  if (o->verbose != 0) return invalid("balm_batch_damping_iter: verbose is not supported (the traces are returned)");
+  BatchReg *r = bt->reg;
+  if (!r) return invalid("balm_batch_damping_iter: no problems registered");
+  CUDA_TRY(cudaSetDevice(bt->device));
+  cudaStream_t st = bt->stream;
+  const int B = r->B, max_iter = o->max_iter > 0 ? o->max_iter : 0;
+  for (int b = 0; b < B; b++) {  // bavoxel.hpp:1071-1085, per problem
+    status[b] = (o->min_planes_per_pose > 0 && r->min_planes[b] < o->min_planes_per_pose) ? BALM_ERR_TOO_FEW_PLANES : BALM_OK;
+    n_iters[b] = 0;
+  }
+  balm_trace *d_trace = nullptr;
+  BTRY(dalloc(&d_trace, (size_t)B * std::max(1, max_iter)));
+  struct Free {
+    balm_trace *p;
+    ~Free() { cudaFree(p); }
+  } free_trace{d_trace};
+  const size_t pbytes = sizeof(double) * 12 * r->P;
+  CUDA_TRY(cudaMemcpyAsync(r->poses, poses12, pbytes, cudaMemcpyHostToDevice, st));
+  CUDA_TRY(cudaMemcpyAsync(r->status(), status, sizeof(int) * B, cudaMemcpyHostToDevice, st));
+  CUDA_TRY(cudaMemsetAsync(d_trace, 0, sizeof(balm_trace) * B * std::max(1, max_iter), st));
+  batch_init_kernel<<<(B + 127) / 128, 128, 0, st>>>(B, r->status(), max_iter, o->u0, o->v0, r->u, r->v, r->active(),
+                                                     r->calc(), r->evalm(), r->n_iters());
+  CUDA_TRY(cudaGetLastError());
+  bool any = false;
+  for (int b = 0; b < B; b++) any = any || status[b] == BALM_OK;
+  LmArgs a{r->prob, B, 0, max_iter, o->force_hess != 0 ? 1 : 0, o->rel_tol, r->r_eval, r->r2, r->q1, r->notpd(),
+           r->r1, r->u, r->v, r->active(), r->calc(), r->evalm(), r->n_iters(), r->n_active(), r->poses, r->trial,
+           d_trace};
+  for (int it = 0; any && it < max_iter; it++) {
+    BTRY(enqueue_eval(bt, r, r->evalm(), o->hess_includes_fix != 0));
+    batch_solve_kernel<<<B, SOLVE_THREADS, SOLVE_SMEM, st>>>(r->prob, r->active(), r->H, r->g, r->u, r->poses,
+                                                             r->trial, r->q1, r->notpd());
+    CUDA_TRY(cudaGetLastError());
+    BTRY(enqueue_trial_residual(bt, r));
+    CUDA_TRY(cudaMemsetAsync(r->n_active(), 0, sizeof(int), st));
+    a.it = it;
+    batch_lm_kernel<<<(B + 127) / 128, 128, 0, st>>>(a);
+    CUDA_TRY(cudaGetLastError());
+    if (poses_per_iter)
+      CUDA_TRY(cudaMemcpyAsync(poses_per_iter + (size_t)it * 12 * r->P, r->poses, pbytes, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(bt->h_count, r->n_active(), sizeof(int), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    any = *bt->h_count > 0;
+  }
+  if (o->gauge_mode == 0 || o->gauge_mode == 1) {
+    CUDA_TRY(cudaMemcpyAsync(r->trial, r->poses, pbytes, cudaMemcpyDeviceToDevice, st));  // pose-0 snapshots
+    batch_gauge_kernel<<<(r->P + 127) / 128, 128, 0, st>>>(r->prob, r->pose_prob, r->status(), r->P, r->poses, r->trial,
+                                                           o->gauge_mode);
+    CUDA_TRY(cudaGetLastError());
+  }
+  CUDA_TRY(cudaMemcpyAsync(poses12, r->poses, pbytes, cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaMemcpyAsync(n_iters, r->n_iters(), sizeof(int) * B, cudaMemcpyDeviceToHost, st));
+  if (trace && max_iter > 0)
+    CUDA_TRY(cudaMemcpyAsync(trace, d_trace, sizeof(balm_trace) * B * max_iter, cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  return BALM_OK;
+}

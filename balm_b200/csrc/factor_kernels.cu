@@ -34,37 +34,6 @@ struct StatsArgs {
 // voxel_sums_kernel: one WARP per voxel, no block barriers. Lanes stride over the voxel's observations with two
 // observations (20 independent 8-byte loads) in flight per lane.
 constexpr int STATS_WARPS = STATS_THREADS / 32;
-// The stats row of one voxel: [0..19] eigen data, [20..39] the observation sweep's record with every per-voxel factor
-// folded into the vectors it multiplies (so the sweep spends no instruction on them):
-//   vb, u0, a_k = sqrt(coe |w_k|)/NN u_k (k = 1,2; w_k = 2/(l0 - l_k), bavoxel.hpp:392), ug = 2 coe/NN u0,
-//   uh = sqrt(coe |w_0|) u0 (w_0 = -2/NN^2, bavoxel.hpp:385), f = 2 coe/NN, s0 = vb . u0
-__device__ __forceinline__ void store_stats_row(double *row, double vb0, double vb1, double vb2, const double *u0,
-                                                const double *u1, const double *u2, double inv, double coe,
-                                                const double *lam) {
-  const double c0 = sqrt(2.0 * coe) * inv, c1 = sqrt(2.0 * coe / (lam[1] - lam[0])), c2 = sqrt(2.0 * coe / (lam[2] - lam[0]));
-  double2 *st = reinterpret_cast<double2 *>(row);
-  st[0] = make_double2(vb0, vb1);
-  st[1] = make_double2(vb2, u0[0]);
-  st[2] = make_double2(u0[1], u0[2]);
-  st[3] = make_double2(u1[0], u1[1]);
-  st[4] = make_double2(u1[2], u2[0]);
-  st[5] = make_double2(u2[1], u2[2]);
-  st[6] = make_double2(inv, c0);
-  st[7] = make_double2(c1, c2);
-  st[8] = make_double2(coe, lam[0]);
-  st[9] = make_double2(lam[1], lam[2]);
-  const double f = 2.0 * coe * inv, k1 = c1 * inv, k2 = c2 * inv;
-  st[10] = make_double2(vb0, vb1);
-  st[11] = make_double2(vb2, u0[0]);
-  st[12] = make_double2(u0[1], u0[2]);
-  st[13] = make_double2(k1 * u1[0], k1 * u1[1]);
-  st[14] = make_double2(k1 * u1[2], k2 * u2[0]);
-  st[15] = make_double2(k2 * u2[1], k2 * u2[2]);
-  st[16] = make_double2(f * u0[0], f * u0[1]);
-  st[17] = make_double2(f * u0[2], c0 * u0[0]);
-  st[18] = make_double2(c0 * u0[1], c0 * u0[2]);
-  st[19] = make_double2(f, vb0 * u0[0] + vb1 * u0[1] + vb2 * u0[2]);
-}
 
 // ---- the stats / residual pass: the streaming half and the eigen half as two kernels ----
 // (one kernel doing both, the eigen-solve in every lane of the voxel's warp, measured at C3: 0.916 -> 0.831 ms)
@@ -302,67 +271,9 @@ __global__ void __launch_bounds__(WPC * 32, MINB) obs_pass_kernel(ObsArgs a) {
         st[2 * c + 1] = x.y;
       }
     }
-    // ---- per-voxel sweep record (written by the eigen half of the stats pass, words 20..39 of the stats row) ----
-    //   vb = mean, u0 = plane normal, a_k = sqrt(coe |w_k|)/NN u_k (k = 1, 2: the G' rows come out scaled),
-    //   ug = 2 coe/NN u0, uh = sqrt(2 coe)/NN u0, f = 2 coe/NN, s0 = vb . u0
-    const double *vb = st, *u0 = st + 3, *a1 = st + 6, *a2 = st + 9, *ug = st + 12, *uh = st + 15;
-    const double f = st[18], s0 = st[19];
-    // ---- world-frame cluster (PointCluster::transform, tools.hpp:333-339): P' = R P R^T + v' p^T + p (R v)^T ----
-    const double rv0 = r[0] * o[6] + r[1] * o[7] + r[2] * o[8];
-    const double rv1 = r[3] * o[6] + r[4] * o[7] + r[5] * o[8];
-    const double rv2 = r[6] * o[6] + r[7] * o[7] + r[8] * o[8];
-    const double n = o[9];
-    const double vw[3] = {rv0 + n * p[0], rv1 + n * p[1], rv2 + n * p[2]};
-    double p00, p01, p02, p11, p12, p22;
-    {
-      const double x00 = r[0] * o[0] + r[1] * o[1] + r[2] * o[2];
-      const double x01 = r[0] * o[1] + r[1] * o[3] + r[2] * o[4];
-      const double x02 = r[0] * o[2] + r[1] * o[4] + r[2] * o[5];
-      const double x10 = r[3] * o[0] + r[4] * o[1] + r[5] * o[2];
-      const double x11 = r[3] * o[1] + r[4] * o[3] + r[5] * o[4];
-      const double x12 = r[3] * o[2] + r[4] * o[4] + r[5] * o[5];
-      const double x20 = r[6] * o[0] + r[7] * o[1] + r[8] * o[2];
-      const double x21 = r[6] * o[1] + r[7] * o[3] + r[8] * o[4];
-      const double x22 = r[6] * o[2] + r[7] * o[4] + r[8] * o[5];
-      p00 = x00 * r[0] + x01 * r[1] + x02 * r[2] + vw[0] * p[0] + p[0] * rv0;
-      p01 = x00 * r[3] + x01 * r[4] + x02 * r[5] + vw[0] * p[1] + p[0] * rv1;
-      p02 = x00 * r[6] + x01 * r[7] + x02 * r[8] + vw[0] * p[2] + p[0] * rv2;
-      p11 = x10 * r[3] + x11 * r[4] + x12 * r[5] + vw[1] * p[1] + p[1] * rv1;
-      p12 = x10 * r[6] + x11 * r[7] + x12 * r[8] + vw[1] * p[2] + p[1] * rv2;
-      p22 = x20 * r[6] + x21 * r[7] + x22 * r[8] + vw[2] * p[2] + p[2] * rv2;
-    }
-    // M = [P' - v' vb^T ; (v' - n vb)^T]  (= TC_i * [R_i | p_i - vb]^T, bavoxel.hpp:368-370)
-    const double m00 = p00 - vw[0] * vb[0], m01 = p01 - vw[0] * vb[1], m02 = p02 - vw[0] * vb[2];
-    const double m10 = p01 - vw[1] * vb[0], m11 = p11 - vw[1] * vb[1], m12 = p12 - vw[1] * vb[2];
-    const double m20 = p02 - vw[2] * vb[0], m21 = p12 - vw[2] * vb[1], m22 = p22 - vw[2] * vb[2];
-    const double mb[3] = {vw[0] - n * vb[0], vw[1] - n * vb[1], vw[2] - n * vb[2]};
-    const double t0[3] = {m00 * u0[0] + m01 * u0[1] + m02 * u0[2], m10 * u0[0] + m11 * u0[1] + m12 * u0[2],
-                          m20 * u0[0] + m21 * u0[1] + m22 * u0[2]};
-    const double s0p = mb[0] * u0[0] + mb[1] * u0[1] + mb[2] * u0[2];
-
-    // ---- G' rows (3 per voxel), 6 contiguous values per pose:  row 0 = sqrt(coe|w0|) a_i, a_i = [-u0 x v' ; n u0]
-    // (bavoxel.hpp:380,385); rows k = 1,2 = sqrt(coe|w_k|) g_k^i, g_k^i = (U_k M u_0 + U_0 M u_k)/NN with
-    // U_k = [hat(-u_k) 0; 0 u_k] (bavoxel.hpp:371-378,392) -- the scale factors ride on the record's vectors ----
-    {
-      double gv[3][6];
-      gv[0][0] = vw[1] * uh[2] - vw[2] * uh[1];
-      gv[0][1] = vw[2] * uh[0] - vw[0] * uh[2];
-      gv[0][2] = vw[0] * uh[1] - vw[1] * uh[0];
-      gv[0][3] = n * uh[0]; gv[0][4] = n * uh[1]; gv[0][5] = n * uh[2];
-#pragma unroll
-      for (int k = 1; k < 3; k++) {
-        const double *ak = k == 1 ? a1 : a2;
-        const double ma[3] = {m00 * ak[0] + m01 * ak[1] + m02 * ak[2], m10 * ak[0] + m11 * ak[1] + m12 * ak[2],
-                              m20 * ak[0] + m21 * ak[1] + m22 * ak[2]};
-        const double sa = mb[0] * ak[0] + mb[1] * ak[1] + mb[2] * ak[2];
-        // -(a_k x t0 + u0 x (M a_k)) = t0 x a_k + (M a_k) x u0
-        gv[k][0] = t0[1] * ak[2] - t0[2] * ak[1] + ma[1] * u0[2] - ma[2] * u0[1];
-        gv[k][1] = t0[2] * ak[0] - t0[0] * ak[2] + ma[2] * u0[0] - ma[0] * u0[2];
-        gv[k][2] = t0[0] * ak[1] - t0[1] * ak[0] + ma[0] * u0[1] - ma[1] * u0[0];
-        gv[k][3] = ak[0] * s0p + u0[0] * sa;
-        gv[k][4] = ak[1] * s0p + u0[1] * sa;
-        gv[k][5] = ak[2] * s0p + u0[2] * sa;
-      }
+    // ---- G' rows of this observation (emitted as fp64 / digit planes / column maxima), then its gradient and
+    // diagonal-block terms (obs_terms) ----
+    obs_terms<MODE != OBS_INT8>(o, r, p, st, acc, [&](const double (&gv)[3][6]) {
       if (MODE == OBS_FP64) {
         double *g0 = a.G + (size_t)(3 * (v - a.v0)) * a.ldg + 6 * i;
 #pragma unroll
@@ -405,41 +316,7 @@ __global__ void __launch_bounds__(WPC * 32, MINB) obs_pass_kernel(ObsArgs a) {
           acc[27 + q] += gv[0][q] * gv[0][q] + gv[1][q] * gv[1][q] + gv[2][q] * gv[2][q];
         }
       }
-    }
-    if (MODE == OBS_INT8) continue;  // gradient and diagonal blocks were accumulated by the first sweep
-    // ---- gradient: coe g_0^i = [t0 x ug ; ug (mb . u0)]  (bavoxel.hpp:381) ----
-    acc[0] += t0[1] * ug[2] - t0[2] * ug[1];
-    acc[1] += t0[2] * ug[0] - t0[0] * ug[2];
-    acc[2] += t0[0] * ug[1] - t0[1] * ug[0];
-    acc[3] += ug[0] * s0p; acc[4] += ug[1] * s0p; acc[5] += ug[2] * s0p;
-    // ---- diagonal block coe*( 2/NN * U0 TCT U0^T + [[Ell+Ell^T,0],[0,0]] )  (bavoxel.hpp:387-388,397-402), upper
-    // triangle in row-major order acc[6..26]. Columns 3..5: f a_i u0^T. Top-left 3x3: with |u0| = 1,
-    //   hat(u0) P' hat(u0)^T = -P' + u0 q^T + q u0^T - tr(P') u0 u0^T + (tr(P') - u0.q) I,  q = P' u0 = t0 + s0 v',
-    // and Ell + Ell^T = (u0 t0^T + t0 u0^T - 2 (t0.u0) I)/NN, so the block is
-    //   -f P' + ug z^T + z ug^T + f kappa I,  z = 1.5 t0 + s0 v' - tr(P')/2 u0,  kappa = tr(P') - 2 u0.t0 - s0 u0.v' ----
-    {
-      const double ag[6] = {vw[1] * ug[2] - vw[2] * ug[1], vw[2] * ug[0] - vw[0] * ug[2], vw[0] * ug[1] - vw[1] * ug[0],
-                            n * ug[0], n * ug[1], n * ug[2]};
-      const double trp = p00 + p11 + p22, hh = 0.5 * trp;
-      const double z[3] = {1.5 * t0[0] + s0 * vw[0] - hh * u0[0], 1.5 * t0[1] + s0 * vw[1] - hh * u0[1],
-                           1.5 * t0[2] + s0 * vw[2] - hh * u0[2]};
-      const double ut = u0[0] * t0[0] + u0[1] * t0[1] + u0[2] * t0[2];
-      const double uv = u0[0] * vw[0] + u0[1] * vw[1] + u0[2] * vw[2];
-      const double fk = f * (trp - 2.0 * ut - s0 * uv);
-      // rows 0..2: [ TL(rr, rr..2) | ag[rr] u0^T ]; rows 3..5: ag[rr] u0[rr-3 ..]
-      acc[6]  += fk - f * p00 + 2.0 * (ug[0] * z[0]);
-      acc[7]  += ug[0] * z[1] + z[0] * ug[1] - f * p01;
-      acc[8]  += ug[0] * z[2] + z[0] * ug[2] - f * p02;
-      acc[9]  += ag[0] * u0[0]; acc[10] += ag[0] * u0[1]; acc[11] += ag[0] * u0[2];
-      acc[12] += fk - f * p11 + 2.0 * (ug[1] * z[1]);
-      acc[13] += ug[1] * z[2] + z[1] * ug[2] - f * p12;
-      acc[14] += ag[1] * u0[0]; acc[15] += ag[1] * u0[1]; acc[16] += ag[1] * u0[2];
-      acc[17] += fk - f * p22 + 2.0 * (ug[2] * z[2]);
-      acc[18] += ag[2] * u0[0]; acc[19] += ag[2] * u0[1]; acc[20] += ag[2] * u0[2];
-      acc[21] += ag[3] * u0[0]; acc[22] += ag[3] * u0[1]; acc[23] += ag[3] * u0[2];
-      acc[24] += ag[4] * u0[1]; acc[25] += ag[4] * u0[2];
-      acc[26] += ag[5] * u0[2];
-    }
+    });
   }
   if (MODE != OBS_INT8 && active && a.colmax) {
 #pragma unroll

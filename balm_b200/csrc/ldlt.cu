@@ -723,21 +723,7 @@ __global__ void __launch_bounds__(1024) q1_kernel(const double *x, const double 
 __global__ void pose_update_kernel(const double *pin, const double *dx, double *pout, int N) {
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= N) return;
-  double dR[9], r[9], p[3];
-  exp_so3(dx + 6 * j, dR);
-  load_pose(pin + 12 * j, r, p);
-  double rn[9], pn[3];
-#pragma unroll
-  for (int a = 0; a < 3; a++) {
-#pragma unroll
-    for (int b = 0; b < 3; b++) rn[a * 3 + b] = dR[a * 3] * r[b] + dR[a * 3 + 1] * r[3 + b] + dR[a * 3 + 2] * r[6 + b];
-    pn[a] = dR[a * 3] * p[0] + dR[a * 3 + 1] * p[1] + dR[a * 3 + 2] * p[2] + dx[6 * j + 3 + a];
-  }
-#pragma unroll
-  for (int c = 0; c < 3; c++)
-#pragma unroll
-    for (int a = 0; a < 3; a++) pout[12 * j + c * 3 + a] = rn[a * 3 + c];
-  pout[12 * j + 9] = pn[0]; pout[12 * j + 10] = pn[1]; pout[12 * j + 11] = pn[2];
+  pose_update_one(pin + 12 * j, dx + 6 * j, pout + 12 * j);
 }
 
 // x_i <- T_0^-1 x_i (bavoxel.hpp:1159-1164); mode 1 also forces pose 0 to the exact identity
@@ -745,26 +731,7 @@ __global__ void pose_update_kernel(const double *pin, const double *dx, double *
 __global__ void gauge_kernel(double *poses, const double *pose0_snapshot, int N, int mode) {
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= N) return;
-  double r0[9], p0[3], r[9], p[3];
-  load_pose(pose0_snapshot, r0, p0);
-  load_pose(poses + 12 * j, r, p);
-  double rn[9], pn[3];
-  const double d[3] = {p[0] - p0[0], p[1] - p0[1], p[2] - p0[2]};
-#pragma unroll
-  for (int a = 0; a < 3; a++) {
-    pn[a] = r0[a] * d[0] + r0[3 + a] * d[1] + r0[6 + a] * d[2];
-#pragma unroll
-    for (int b = 0; b < 3; b++) rn[a * 3 + b] = r0[a] * r[b] + r0[3 + a] * r[3 + b] + r0[6 + a] * r[6 + b];
-  }
-  if (mode == 1 && j == 0) {
-    rn[0] = 1; rn[1] = 0; rn[2] = 0; rn[3] = 0; rn[4] = 1; rn[5] = 0; rn[6] = 0; rn[7] = 0; rn[8] = 1;
-    pn[0] = pn[1] = pn[2] = 0;
-  }
-#pragma unroll
-  for (int c = 0; c < 3; c++)
-#pragma unroll
-    for (int a = 0; a < 3; a++) poses[12 * j + c * 3 + a] = rn[a * 3 + c];
-  poses[12 * j + 9] = pn[0]; poses[12 * j + 10] = pn[1]; poses[12 * j + 11] = pn[2];
+  gauge_one(poses + 12 * j, pose0_snapshot, mode == 1 && j == 0);
 }
 
 }  // namespace

@@ -195,6 +195,38 @@ int balm_window_push(balm_ctx *ctx, int win_count, int64_t *n_voxels_out, int64_
  * the ctx as balm_set_voxels would (rows = its non-empty sig_orig slots, fix cluster = its fix_point, coe = its points),
  * in ascending node key; balm_download_keys / balm_download_fix read them back. No such node -> an empty voxel set. */
 
+/* Batched bundle adjustment: B independent small problems (an HBA bottom layer of short windows, one BALM2 per window)
+ * registered once and optimised together on one GPU. A batch has its own handle and stream: it does not allocate the
+ * dense n x n buffers of a balm_ctx, so a batch of 400 problems of 10 poses pays for 400 blocks of 60 x 60, not for one
+ * matrix of 24 000^2. fp64 arithmetic throughout (the BALM_PREC_FP64 contract); no tensor path, no communicator.
+ * Problem p owns the poses [pose_ptr[p], pose_ptr[p+1]) of the concatenated pose array (1 <= count <=
+ * BALM_BATCH_MAX_POSES) and the voxels [voxel_ptr[p], voxel_ptr[p+1]) (may be empty). row_ptr / obs10 / coe / fix10 as
+ * balm_set_voxels, over all voxels (fix10: every voxel or NULL; all-zero rows for problems without fix clusters).
+ * pose_idx is problem-local (0 .. N_p - 1), ascending inside a voxel. Host arrays, copied. A malformed registration
+ * (n_problems < 1; a problem with 0 or more than BALM_BATCH_MAX_POSES poses; pose_ptr / voxel_ptr / row_ptr not starting
+ * at 0 or not ascending; pose_idx out of its problem's range or not ascending inside a voxel -- checked on the device)
+ * returns BALM_ERR_INVALID and leaves the previous registration in place. */
+#define BALM_BATCH_MAX_POSES 32   /* per problem: 6N <= 192 unknowns */
+typedef struct balm_batch balm_batch;
+int balm_batch_create(balm_batch **out, int device);
+int balm_batch_destroy(balm_batch *b);
+int balm_batch_set_voxels(balm_batch *b, int n_problems, const int64_t *pose_ptr, const int64_t *voxel_ptr,
+                          const int64_t *row_ptr, const int32_t *pose_idx, const double *obs10,
+                          const double *fix10, const double *coe);
+/* left_evaluate_acc2 per problem, at poses12 (P x 12, P = pose_ptr[B]). H: the problems' full column-major (6N_p)^2
+ * blocks one after the other, g: 6P, residual: B. H, g may be NULL. */
+int balm_batch_evaluate(balm_batch *b, const double *poses12, int include_fix, double *H, double *g, double *residual);
+/* balm_damping_iter per problem, all problems advanced together: each problem's iterations are exactly those of
+ * balm_damping_iter on a BALM_PREC_FP64 context holding only that problem (precheck, u0 / v0, accept rule, reused H after a
+ * rejected step unless force_hess, rel_tol exit, hess_includes_fix, gauge_mode on the problem's own pose 0). A converged
+ * problem stops; the others go on. poses12: P x 12, updated in place for problems with status BALM_OK.
+ * status[B]: BALM_OK or BALM_ERR_TOO_FEW_PLANES (that problem is left untouched, n_iters 0). n_iters[B].
+ * trace: [B][max_iter] or NULL (entries past a problem's n_iters are zero); poses_per_iter: [max_iter][P][12] or NULL
+ * (a problem's rows past its n_iters repeat its last poses; rows past the batch's last iteration are not written). opts->verbose != 0 is rejected (BALM_ERR_INVALID): the traces are
+ * returned instead of printed. The host waits once per iteration. */
+int balm_batch_damping_iter(balm_batch *b, double *poses12, const balm_lm_opts *opts, int *status, int *n_iters,
+                            balm_trace *trace, double *poses_per_iter);
+
 /* Pose-covariance propagation of the consistency experiment (SURVEY.md section 8f, row N3):
  *   Rcov_raw = sum over observations of  Ls c_cov Ls^T      -- VOX_HESS::left_jacobian_point + BALM2::multi_second
  *                                                              (src/simulation/BAs_left.hpp:342-473, 995-1023)

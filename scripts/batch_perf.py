@@ -1,0 +1,134 @@
+"""Device time of the batched bundle adjustment (balm_b200.Batch) next to what a caller does without it: one Context per
+pose count and, for every window, set_voxels + damping_iter, on the fp64 and on the tensor path.
+
+Workloads (HBA's bottom layer splits a trajectory into many short windows): (a) 256 windows x 10 poses x 1 000 planes,
+(b) 32 windows x 32 poses x 5 000 planes. Every window is generated on the GPU by Context.synth_virtual (its own seed) and
+read back with download_voxels, so the batch and the loop run on the same host arrays. Two option sets: fixed work
+(force_hess, rel_tol < 0, 10 iterations: every LM iteration does the same work) and the defaults. The batch, the fp64 loop
+and the tensor loop alternate --repeats times in one process; every call ends in a device synchronisation, so a host clock
+around it measures the device work. Registration (set_problems / set_voxels) is timed apart from the LM calls.
+A separate torch.profiler run of one fixed-work batch call gives the device time per kernel.
+Prints one JSON line; --out FILE also writes it there."""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path[:0] = [ROOT, os.path.join(ROOT, "tests")]
+
+
+def gpu_info():
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                           capture_output=True, text=True, timeout=30).stdout.strip()
+    except Exception as e:  # the numbers are still valid, but say where they came from
+        q = f"nvidia-smi unavailable: {e}"
+    return q
+
+
+def make_windows(n_windows, n_poses, n_planes, seed0):
+    import balm_b200
+    c = balm_b200.Context(n_poses, 0, balm_b200.PREC_FP64)
+    probs, init = [], []
+    for w in range(n_windows):
+        _, x0 = c.synth_virtual(n_planes, seed=seed0 + w)
+        row_ptr, pose_idx, obs10, coe = c.download_voxels()
+        probs.append(dict(n_poses=n_poses, row_ptr=row_ptr, pose_idx=pose_idx, obs10=obs10, coe=coe))
+        init.append(x0)
+    c.close()
+    return probs, init
+
+
+def run_workload(name, n_windows, n_poses, n_planes, repeats, seed0):
+    import balm_b200
+    probs, init = make_windows(n_windows, n_poses, n_planes, seed0)
+    options = {"fixed": dict(max_iter=10, force_hess=True, rel_tol=-1.0, gauge_mode=2),
+               "default": dict()}
+    batch = balm_b200.Batch(0)
+    ctx = {p: balm_b200.Context(n_poses, 0, p) for p in (balm_b200.PREC_FP64, balm_b200.PREC_TENSOR)}
+    out = dict(windows=n_windows, poses=n_poses, planes=n_planes)
+
+    def clock(f):
+        t0 = time.perf_counter()
+        r = f()
+        return r, 1e3 * (time.perf_counter() - t0)
+
+    def loop(c, kw):
+        poses, reg, lm, iters = [], 0.0, 0.0, []
+        for pr, x0 in zip(probs, init):
+            _, t = clock(lambda: c.set_voxels(pr["row_ptr"], pr["pose_idx"], pr["obs10"], pr["coe"]))
+            reg += t
+            (p, tr, _), t = clock(lambda: c.damping_iter(x0, **kw))
+            lm += t
+            poses.append(p)
+            iters.append(len(tr))
+        return poses, reg, lm, iters
+
+    for key, kw in options.items():
+        ms = {k: [] for k in ("batch_register", "batch_lm", "fp64_register", "fp64_lm", "tensor_register", "tensor_lm")}
+        for rep in range(repeats + 1):  # the first round warms up every shape
+            _, t_reg = clock(lambda: batch.set_problems(probs))
+            res, t_lm = clock(lambda: batch.damping_iter(init, **kw))
+            p64, r64, l64, it64 = loop(ctx[balm_b200.PREC_FP64], kw)
+            ptc, rtc, ltc, _ = loop(ctx[balm_b200.PREC_TENSOR], kw)
+            if rep == 0:
+                continue
+            for k, v in (("batch_register", t_reg), ("batch_lm", t_lm), ("fp64_register", r64), ("fp64_lm", l64),
+                         ("tensor_register", rtc), ("tensor_lm", ltc)):
+                ms[k].append(v)
+        dpose = max(float(np.abs(r[1] - p).max()) for r, p in zip(res, p64))
+        iters = [len(r[2]) for r in res]
+        out[key] = dict(ms=ms, ms_median={k: float(np.median(v)) for k, v in ms.items()},
+                        batch_iters_total=int(sum(iters)), loop_iters_total=int(sum(it64)),
+                        max_pose_diff_batch_vs_fp64_loop=dpose,
+                        same_iteration_counts=bool(iters == it64))
+    # one profiled fixed-work call of its own: device time per kernel, summed over the call
+    try:
+        import torch
+        from torch.profiler import ProfilerActivity, profile
+        batch.set_problems(probs)
+        batch.damping_iter(init, **options["fixed"])
+        torch.cuda.synchronize()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            batch.damping_iter(init, **options["fixed"])
+            torch.cuda.synchronize()
+        per = {}
+        for e in prof.key_averages():
+            t = getattr(e, "device_time_total", None)
+            if t is None:
+                t = e.cuda_time_total
+            if t > 0:
+                per[e.key] = dict(ms=t / 1e3, calls=e.count)
+        out["profile_fixed_ms_per_kernel"] = per
+    except Exception as e:  # the end-to-end numbers above stand on their own
+        out["profile_fixed_ms_per_kernel"] = f"profiler failed: {e}"
+    batch.close()
+    for c in ctx.values():
+        c.close()
+    return out
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--repeats", type=int, default=3)
+    ap.add_argument("--workloads", default="a,b")
+    ap.add_argument("--out", default=None, help="also write the result to this JSON file")
+    a = ap.parse_args()
+    shapes = {"a": (256, 10, 1000, 100), "b": (32, 32, 5000, 900)}
+    res = dict(gpu=gpu_info(), repeats=a.repeats)
+    for w in a.workloads.split(","):
+        res[w] = run_workload(w, *shapes[w][:3], a.repeats, shapes[w][3])
+    if a.out:
+        os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
+        with open(a.out, "w") as f:
+            json.dump(res, f, indent=1)
+    print(json.dumps(res))
+
+
+if __name__ == "__main__":
+    main()

@@ -1,6 +1,7 @@
 """Small end-to-end run for compute-sanitizer (memcheck / racecheck): both precision modes, dense + sparse; the persistent
-tile-DAG factorisation with several 64-column steps (n = 240: chain + near/far workers), the sliding-window marginalisation, the pose-covariance propagation, a multi-batch sparse evaluation, and the device
-association chain balm_cut_voxels -> balm_marginalize -> balm_append_scan (octree keys + layers)."""
+tile-DAG factorisation with several 64-column steps (n = 240: chain + near/far workers), the sliding-window marginalisation, the pose-covariance propagation, a multi-batch sparse evaluation, the device
+association chain balm_cut_voxels -> balm_marginalize -> balm_append_scan (octree keys + layers), and a batch of
+independent problems (balm_batch_*: a dense one with fix clusters, a sparse one of 32 poses, an empty one)."""
 import os, sys
 import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -41,4 +42,17 @@ M2, K2, matched = c.append_scan(pts[frs == N].astype(np.float32), shifted, N - m
 keys, layers = c.download_keys(with_layers=True)
 print("assoc chain", (M0, K0), (M1, K1), (M2, K2), "matched", matched, "layers", np.bincount(layers, minlength=3), flush=True)
 c.close()
+scs = [scenes.make_scene(n_poses=6, n_planes=30, seed=5, pts_size=6, with_fix=True),
+       scenes.make_scene(n_poses=32, n_planes=40, seed=6, drop=0.4, pts_size=6)]
+probs = [dict(n_poses=s["n_poses"], row_ptr=s["row_ptr"], pose_idx=s["pose_idx"], obs10=s["obs10"], coe=s["coe"],
+              fix10=s["fix10"]) for s in scs]
+probs.append(dict(n_poses=2, row_ptr=np.zeros(1, dtype=np.int64), pose_idx=np.zeros(0, dtype=np.int32),
+                  obs10=np.zeros((0, 10)), coe=np.zeros(0)))
+b = balm_b200.Batch(0)
+b.set_problems(probs)
+x = [s["poses_init"] for s in scs] + [np.tile([1, 0, 0, 0, 1, 0, 0, 0, 1, 0, 0, 0.0], (2, 1))]
+print("batch r", [r for _, _, r in b.evaluate(x, include_fix=True)], flush=True)
+res = b.damping_iter(x, max_iter=2, min_planes_per_pose=0, hess_includes_fix=True, want_per_iter=True)
+print("batch iters", [len(tr) for _, _, tr, _ in res], flush=True)
+b.close()
 print("SANITIZE_DONE")
