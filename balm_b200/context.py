@@ -267,6 +267,55 @@ class Batch:
         self.n_poses = n_poses
         self._pose_ptr = pose_ptr
 
+    def cut_scans(self, scans, windows, poses_list, voxel_size=2.0, layer_limit=2, min_ps=15,
+                  eigen_value_array=(1.0 / 16, 1.0 / 16, 1.0 / 9)):
+        """Association for every window on the device (include/balm_b200.h, balm_batch_cut_voxels). scans: list of
+        (n_s x 3) body-frame points, each uploaded once; windows: per problem the scan indices of its slots (1 .. 32);
+        poses_list: per window its N_w x 12 initial poses. Window w gets what Context(N_w).cut_voxels registers on its
+        scans' points with frame = slot. A window without a plane voxel is registered empty. -> per window (M, K)."""
+        scans = [np.asarray(s, dtype=np.float32).reshape(-1, 3) for s in scans]
+        n_poses = [len(w) for w in windows]
+        scan_ptr = np.concatenate([[0], np.cumsum([len(s) for s in scans])]).astype(np.int64)
+        pose_ptr = np.concatenate([[0], np.cumsum(n_poses)]).astype(np.int64)
+        pose_scan = np.ascontiguousarray(np.concatenate([np.asarray(w, dtype=np.int64).ravel() for w in windows]),
+                                         dtype=np.int32)
+        xyz = np.ascontiguousarray(np.concatenate(scans) if scans else np.zeros((0, 3)), dtype=np.float32)
+        poses = np.ascontiguousarray(np.concatenate([np.asarray(p, dtype=np.float64).reshape(n, 12)
+                                                     for p, n in zip(poses_list, n_poses)]), dtype=np.float64)
+        o = L.AssocOpts(float(voxel_size), int(layer_limit), int(min_ps), (C.c_double * 3)(*eigen_value_array))
+        M = np.zeros(len(windows), dtype=np.int64)
+        K = np.zeros(len(windows), dtype=np.int64)
+        L.check(L.lib().balm_batch_cut_voxels(self._h, len(windows), _p(pose_ptr), _p(pose_scan), len(scans),
+                                              _p(scan_ptr), _p(xyz), _p(poses), C.byref(o), _p(M), _p(K)))
+        self.n_poses = n_poses
+        self._pose_ptr = pose_ptr
+        return [(int(m), int(k)) for m, k in zip(M, K)]
+
+    def download_voxels(self, with_keys=False):
+        """The current registration, per problem a dict set_problems accepts (row_ptr re-based to 0); with_keys adds
+        keys and layers (only after cut_scans)."""
+        B, P, M, K = C.c_int(), C.c_int64(), C.c_int64(), C.c_int64()
+        L.check(L.lib().balm_batch_sizes(self._h, C.byref(B), C.byref(P), C.byref(M), C.byref(K)))
+        voxel_ptr = np.zeros(B.value + 1, dtype=np.int64)
+        row_ptr = np.zeros(M.value + 1, dtype=np.int64)
+        pose_idx = np.zeros(K.value, dtype=np.int32)
+        obs10 = np.zeros((K.value, 10))
+        coe = np.zeros(M.value)
+        keys = np.zeros(M.value, dtype=np.uint64) if with_keys else None
+        layers = np.zeros(M.value, dtype=np.int32) if with_keys else None
+        L.check(L.lib().balm_batch_download_voxels(self._h, _p(voxel_ptr), _p(row_ptr), _p(pose_idx), _p(obs10), _p(coe),
+                                                   _p(keys), _p(layers)))
+        out = []
+        for b in range(B.value):
+            v0, v1 = int(voxel_ptr[b]), int(voxel_ptr[b + 1])
+            s0, s1 = int(row_ptr[v0]), int(row_ptr[v1])
+            d = dict(n_poses=int(self._pose_ptr[b + 1] - self._pose_ptr[b]), row_ptr=row_ptr[v0:v1 + 1] - s0,
+                     pose_idx=pose_idx[s0:s1].copy(), obs10=obs10[s0:s1].copy(), coe=coe[v0:v1].copy())
+            if with_keys:
+                d.update(keys=keys[v0:v1].copy(), layers=layers[v0:v1].copy())
+            out.append(d)
+        return out
+
     def _concat(self, poses_list):
         assert len(poses_list) == len(self.n_poses)
         return np.ascontiguousarray(np.concatenate([np.asarray(p, dtype=np.float64).reshape(n, 12)

@@ -14,6 +14,12 @@
 // planar, has more than min_ps points and at least two observing frames, and every ancestor was large enough and NOT
 // planar. All reductions run in a fixed order: the result is deterministic. Output order: ascending node key
 // (digit 7 = "not split at this layer"), the order tests/assoc_ref.py uses.
+//
+// The same level loop serves a batch of independent problems (balm_batch_cut_voxels). Its items are the points of every
+// problem in (problem, slot, point) order -- an index into the points uploaded once plus a pose row -- so a scan shared
+// by two windows is read twice but stored once. Every sort is stable and ordered by (problem, key): each (problem, node,
+// slot) segment is summed in the order a context holding only that problem would sum it, so each problem's voxels are
+// bitwise those of balm_cut_voxels on its own points. One problem with rows = frames is balm_cut_voxels itself.
 #include <cub/cub.cuh>
 #include <algorithm>
 #include <vector>
@@ -39,15 +45,17 @@ __device__ __forceinline__ long long ref_voxel_index(double w, double vs) {
 // 63-bit key of a world point: root voxel (cut_voxel) + the octants cut_func would choose at layers 1 and 2
 __device__ __forceinline__ unsigned long long world_point_key(const double *w, const AssocParams &p, int *bad);
 
-__global__ void point_key_kernel(const float *xyz, const int *frame, const double *poses, int n_poses, int64_t n,
-                                 AssocParams p, unsigned long long *key, int *bad) {
+// key of every item: its point (src) in the world frame of its pose row
+__global__ void item_key_kernel(const float *xyz, const int *src, const int *row, const double *poses, int n_rows,
+                                int64_t n, AssocParams p, unsigned long long *key, int *bad) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  int f = frame[i];
-  if (f < 0 || f >= n_poses) { atomicOr(bad, 2); f = 0; }
+  int f = row[i];
+  if (f < 0 || f >= n_rows) { atomicOr(bad, 2); f = 0; }
   double r[9], t[3];
   load_pose(poses + 12 * f, r, t);
-  const double b[3] = {(double)xyz[3 * i], (double)xyz[3 * i + 1], (double)xyz[3 * i + 2]};
+  const int64_t j = src[i];
+  const double b[3] = {(double)xyz[3 * j], (double)xyz[3 * j + 1], (double)xyz[3 * j + 2]};
   double w[3];
 #pragma unroll
   for (int a = 0; a < 3; a++) w[a] = r[a * 3] * b[0] + r[a * 3 + 1] * b[1] + r[a * 3 + 2] * b[2] + t[a];
@@ -77,43 +85,52 @@ __global__ void iota_kernel(int *v, int64_t n) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) v[i] = (int)i;
 }
-__global__ void gather_frame_kernel(const int *frame, const int *idx, unsigned *out, int64_t n) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) out[i] = (unsigned)frame[idx[i]];
+// batch items: one CTA per pose row j, whose items [item_ptr[j], item_ptr[j+1]) are the points of its scan
+__global__ void expand_rows_kernel(const long long *item_ptr, const long long *src_base, int *src, int *row) {
+  const int j = blockIdx.x;
+  const long long a = item_ptr[j], b = item_ptr[j + 1], s = src_base[j];
+  for (long long e = a + threadIdx.x; e < b; e += blockDim.x) {
+    src[e] = (int)(s + (e - a));
+    row[e] = j;
+  }
 }
-// key of layer L: digits below L forced to 7 ("not split")
-__global__ void level_key_kernel(const unsigned long long *key, const int *idx, unsigned long long *out, int64_t n, int L) {
+// digits below layer L forced to 7 ("not split")
+__device__ __forceinline__ unsigned long long level_key(unsigned long long k, int L) {
+  return L == 0 ? k | 63ull : (L == 1 ? k | 7ull : k);
+}
+__global__ void level_key_kernel(const unsigned long long *key, unsigned long long *out, int64_t n, int L) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) out[i] = level_key(key[i], L);
+}
+__global__ void gather_prob_kernel(const int *idx, const int *row, const int *row_prob, unsigned *out, int64_t n) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) out[i] = (unsigned)row_prob[row[idx[i]]];
+}
+// a (problem, node, slot) segment starts where the level key or the pose row changes (rows belong to one problem)
+__global__ void seg_flag_kernel(const unsigned long long *key, const int *idx, const int *row, int64_t n, int L, int *flag) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  unsigned long long k = key[idx[i]];
-  if (L == 0) k |= 63ull;
-  else if (L == 1) k |= 7ull;
-  out[i] = k;
-}
-__global__ void seg_flag_kernel(const unsigned long long *keyL, const int *idx, const int *frame, int64_t n, int *flag) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  flag[i] = (i == 0 || keyL[i] != keyL[i - 1] || frame[idx[i]] != frame[idx[i - 1]]) ? 1 : 0;
+  flag[i] = (i == 0 || level_key(key[idx[i]], L) != level_key(key[idx[i - 1]], L) || row[idx[i]] != row[idx[i - 1]]) ? 1 : 0;
 }
 __global__ void seg_start_kernel(const int *flag, const int *scan, int64_t n, int *seg_start) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n && flag[i]) seg_start[scan[i]] = (int)i;
 }
 
-// One thread per (node, frame) segment: body-frame cluster (PointCluster::push, tools.hpp:311-316) and world-frame
-// moments, accumulated in sorted order.
-__global__ void seg_reduce_kernel(const float *xyz, const int *frame, const double *poses, const int *idx,
-                                  const unsigned long long *keyL, const int *seg_start, int nseg, int64_t n,
-                                  double *segB, double *segW, int *seg_frame, unsigned long long *seg_key) {
+// One thread per (problem, node, slot) segment: body-frame cluster (PointCluster::push, tools.hpp:311-316) and
+// world-frame moments, accumulated in sorted order.
+__global__ void seg_reduce_kernel(const float *xyz, const int *src, const int *row, const double *poses, const int *idx,
+                                  const unsigned long long *key, int L, const int *seg_start, int nseg, int64_t n,
+                                  double *segB, double *segW, int *seg_row, unsigned long long *seg_key) {
   const int s = blockIdx.x * blockDim.x + threadIdx.x;
   if (s >= nseg) return;
   const int64_t a = seg_start[s], b = (s + 1 < nseg) ? seg_start[s + 1] : n;
-  const int f = frame[idx[a]];
+  const int f = row[idx[a]];
   double r[9], t[3];
   load_pose(poses + 12 * f, r, t);
   double B[10] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0}, W[10] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
   for (int64_t i = a; i < b; i++) {
-    const int j = idx[i];
+    const int64_t j = src[idx[i]];
     const double x = xyz[3 * j], y = xyz[3 * j + 1], z = xyz[3 * j + 2];
     B[0] += x * x; B[1] += x * y; B[2] += x * z; B[3] += y * y; B[4] += y * z; B[5] += z * z;
     B[6] += x; B[7] += y; B[8] += z; B[9] += 1.0;
@@ -125,12 +142,14 @@ __global__ void seg_reduce_kernel(const float *xyz, const int *frame, const doub
   }
 #pragma unroll
   for (int c = 0; c < 10; c++) { segB[(size_t)c * nseg + s] = B[c]; segW[(size_t)c * nseg + s] = W[c]; }
-  seg_frame[s] = f;
-  seg_key[s] = keyL[a];
+  seg_row[s] = f;
+  seg_key[s] = level_key(key[idx[a]], L);
 }
-__global__ void node_flag_kernel(const unsigned long long *seg_key, int nseg, int *flag) {
+__global__ void node_flag_kernel(const unsigned long long *seg_key, const int *seg_row, const int *row_prob, int nseg,
+                                 int *flag) {
   const int s = blockIdx.x * blockDim.x + threadIdx.x;
-  if (s < nseg) flag[s] = (s == 0 || seg_key[s] != seg_key[s - 1]) ? 1 : 0;
+  if (s < nseg)
+    flag[s] = (s == 0 || seg_key[s] != seg_key[s - 1] || row_prob[seg_row[s]] != row_prob[seg_row[s - 1]]) ? 1 : 0;
 }
 // judge_eigen (bavoxel.hpp:654-699) on a world-frame cluster: lambda0 / lambda1 of its covariance below the layer's
 // threshold (decision < eigen_value_array[layer], :665,697)
@@ -142,10 +161,11 @@ __device__ __forceinline__ bool cluster_planar(const double *W, double eig_thr) 
               W[4] * inv - c1 * c2, W[5] * inv - c2 * c2, lam, u0, u1, u2);
   return lam[0] / lam[1] < eig_thr;
 }
-// One thread per node: total world moments over its frames -> judge_eigen (bavoxel.hpp:654-699)
-__global__ void node_judge_kernel(const double *segW, const unsigned long long *seg_key, const int *node_start, int nnode,
-                                  int nseg, double eig_thr, unsigned long long *node_key, int *node_size,
-                                  int *node_planar, int *node_nframes) {
+// One thread per (problem, node): total world moments over its slots -> judge_eigen (bavoxel.hpp:654-699)
+__global__ void node_judge_kernel(const double *segW, const unsigned long long *seg_key, const int *seg_row,
+                                  const int *row_prob, const int *node_start, int nnode, int nseg, double eig_thr,
+                                  unsigned long long *node_key, int *node_prob, int *node_size, int *node_planar,
+                                  int *node_nframes) {
   const int v = blockIdx.x * blockDim.x + threadIdx.x;
   if (v >= nnode) return;
   const int a = node_start[v], b = (v + 1 < nnode) ? node_start[v + 1] : nseg;
@@ -154,18 +174,19 @@ __global__ void node_judge_kernel(const double *segW, const unsigned long long *
 #pragma unroll
     for (int c = 0; c < 10; c++) W[c] += segW[(size_t)c * nseg + s];
   node_key[v] = seg_key[a];
+  node_prob[v] = row_prob[seg_row[a]];
   node_size[v] = (int)(W[9] + 0.5);
   node_planar[v] = cluster_planar(W, eig_thr) ? 1 : 0;
   node_nframes[v] = b - a;
 }
 
-struct LevelTables {  // device arrays of one layer
+struct LevelTables {  // device arrays of one layer, nodes in ascending (problem, key)
   int nseg = 0, nnode = 0;
   double *segB = nullptr;          // [10][nseg] body-frame clusters
-  int *seg_frame = nullptr;
+  int *seg_row = nullptr;          // [nseg] pose row
   int *node_start = nullptr;       // [nnode] first segment
   unsigned long long *node_key = nullptr;
-  int *node_size = nullptr, *node_planar = nullptr, *node_nframes = nullptr, *node_leaf = nullptr;
+  int *node_prob = nullptr, *node_size = nullptr, *node_planar = nullptr, *node_nframes = nullptr, *node_leaf = nullptr;
 };
 
 __device__ __forceinline__ int find_key(const unsigned long long *keys, int n, unsigned long long k) {
@@ -178,24 +199,42 @@ __device__ __forceinline__ int find_key(const unsigned long long *keys, int n, u
   }
   return -1;
 }
+// the same search on a table sorted by (problem, key)
+__device__ __forceinline__ int find_node(const int *probs, const unsigned long long *keys, int n, int p,
+                                         unsigned long long k) {
+  int lo = 0, hi = n - 1;
+  while (lo <= hi) {
+    const int mid = (lo + hi) >> 1;
+    const int q = probs[mid];
+    const unsigned long long v = keys[mid];
+    if (q == p && v == k) return mid;
+    if (q < p || (q == p && v < k)) lo = mid + 1; else hi = mid - 1;
+  }
+  return -1;
+}
+
+struct AncestorTable {
+  const unsigned long long *key;
+  const int *prob, *size, *planar;
+  int n;
+};
 
 // recut (bavoxel.hpp:737-776) evaluated per node: a node is reached iff every ancestor had more than min_ps points and
 // failed the planarity test; it becomes a plane voxel iff it is planar with more than min_ps points (push_state = 1)
-// and at least two frames observe it (push_voxel :37).
-__global__ void leaf_decide_kernel(int L, int nnode, const unsigned long long *key, const int *size, const int *planar,
-                                   const int *nframes, const unsigned long long *key0, const int *size0,
-                                   const int *planar0, int n0, const unsigned long long *key1, const int *size1,
-                                   const int *planar1, int n1, int min_ps, int layer_limit, int *leaf) {
+// and at least two frames observe it (push_voxel :37). Ancestors are looked up in the node's own problem.
+__global__ void leaf_decide_kernel(int L, int nnode, const unsigned long long *key, const int *prob, const int *size,
+                                   const int *planar, const int *nframes, AncestorTable t0, AncestorTable t1,
+                                   int min_ps, int layer_limit, int *leaf) {
   const int v = blockIdx.x * blockDim.x + threadIdx.x;
   if (v >= nnode) return;
   bool reached = L <= layer_limit;
   if (reached && L >= 1) {
-    const int r = find_key(key0, n0, key[v] | 63ull);
-    reached = r >= 0 && size0[r] > min_ps && !planar0[r];
+    const int r = find_node(t0.prob, t0.key, t0.n, prob[v], key[v] | 63ull);
+    reached = r >= 0 && t0.size[r] > min_ps && !t0.planar[r];
   }
   if (reached && L >= 2) {
-    const int r = find_key(key1, n1, key[v] | 7ull);
-    reached = r >= 0 && size1[r] > min_ps && !planar1[r];
+    const int r = find_node(t1.prob, t1.key, t1.n, prob[v], key[v] | 7ull);
+    reached = r >= 0 && t1.size[r] > min_ps && !t1.planar[r];
   }
   leaf[v] = (reached && size[v] > min_ps && planar[v] && nframes[v] >= 2) ? 1 : 0;
 }
@@ -208,42 +247,55 @@ __global__ void leaf_collect_kernel(int L, int nnode, const int *leaf, const int
   out_key[o] = key[v];
   out_ref[o] = (L << 28) | v;  // layer and node id
 }
-__global__ void leaf_count_kernel(const int *ref, int nleaf, const int *nf0, const int *nf1, const int *nf2, int *cnt) {
+// out[i] = the node table entry of leaf i (layer and node id in ref[i])
+template <typename T>
+__global__ void leaf_gather_kernel(const int *ref, int nleaf, const int *t0, const int *t1, const int *t2, T *out) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= nleaf) return;
   const int L = ref[i] >> 28, v = ref[i] & 0x0FFFFFFF;
-  cnt[i] = (L == 0 ? nf0 : (L == 1 ? nf1 : nf2))[v];
+  out[i] = (T)(L == 0 ? t0 : (L == 1 ? t1 : t2))[v];
 }
-__global__ void leaf_layer_kernel(const int *ref, int nleaf, int *layer) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < nleaf) layer[i] = ref[i] >> 28;
+// per problem b in [0, B]: its first leaf (leaves sorted by problem) and first observation
+__global__ void prob_ptr_kernel(const unsigned *lprob, const int *cnt, const int *obs_start, int nleaf, int B,
+                                long long *voxel_ptr, long long *obs_ptr) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b > B) return;
+  int lo = 0, hi = nleaf;
+  while (lo < hi) { const int m = (lo + hi) >> 1; if ((int)lprob[m] < b) lo = m + 1; else hi = m; }
+  voxel_ptr[b] = lo;
+  obs_ptr[b] = lo < nleaf ? obs_start[lo] : (long long)obs_start[nleaf - 1] + cnt[nleaf - 1];
 }
 struct EmitLevel {
   const double *segB;
-  const int *seg_frame, *node_start, *node_size;
+  const int *seg_row, *node_start, *node_size;
+  const unsigned long long *node_key;
   int nseg;
 };
+// One CTA per plane voxel: its observations (slot = row_slot of the segment's pose row) into the registration's layout
 __global__ void emit_kernel(const int *ref, const int *obs_start, int nleaf, EmitLevel e0, EmitLevel e1, EmitLevel e2,
-                            const int *cnt, double *obs, int64_t Kp, int *pose_idx, long long *row_ptr, double *coe) {
-  const int i = blockIdx.x;  // one CTA per plane voxel
+                            const int *cnt, const int *row_slot, AssocEmit out) {
+  const int i = blockIdx.x;
   if (i >= nleaf) return;
   const int L = ref[i] >> 28, v = ref[i] & 0x0FFFFFFF;
   const EmitLevel e = L == 0 ? e0 : (L == 1 ? e1 : e2);
   const int s0 = e.node_start[v], k = cnt[i], o0 = obs_start[i];
   for (int j = threadIdx.x; j < k; j += blockDim.x) {
 #pragma unroll
-    for (int c = 0; c < 10; c++) obs[(size_t)c * Kp + o0 + j] = e.segB[(size_t)c * e.nseg + s0 + j];
-    pose_idx[o0 + j] = e.seg_frame[s0 + j];
+    for (int c = 0; c < 10; c++)
+      out.obs[(size_t)c * out.obs_cstride + (size_t)(o0 + j) * out.obs_ostride] = e.segB[(size_t)c * e.nseg + s0 + j];
+    out.pose_idx[o0 + j] = row_slot[e.seg_row[s0 + j]];
   }
   if (threadIdx.x == 0) {
-    row_ptr[i] = o0;
-    coe[i] = (double)e.node_size[v];  // coe = sum of N over the window (bavoxel.hpp:42-44)
-    if (i == nleaf - 1) row_ptr[nleaf] = o0 + k;
+    out.row_ptr[i] = o0;
+    out.coe[i] = (double)e.node_size[v];  // coe = sum of N over the window (bavoxel.hpp:42-44)
+    out.key[i] = e.node_key[v];
+    out.layer[i] = L;
+    if (i == nleaf - 1) out.row_ptr[nleaf] = o0 + k;
   }
 }
 
-// Every scratch buffer of assoc_build lives in a pool that frees what is left on ANY exit path (the early returns of
-// ATRY / CUDA_TRY, "no plane voxels found", a bad frame index ...), so a failed call leaks nothing.
+// Every scratch buffer of assoc_cut lives in a pool that frees what is left on ANY exit path (the early returns of
+// ATRY / CUDA_TRY, a rejected registration, a bad frame index ...), so a failed call leaks nothing.
 struct ScratchPool {
   std::vector<void *> ptrs;
   ~ScratchPool() { for (void *q : ptrs) cudaFree(q); }
@@ -264,54 +316,89 @@ struct ScratchPool {
 
 }  // namespace
 
-// Builds the plane voxels of `ctx` from raw scans. xyz (n x 3 float32, body frame) and frame (n) are HOST arrays,
-// poses12 the initial poses. On success the voxels are registered exactly as balm_set_voxels would have done.
-int assoc_build(balm_ctx *c, int64_t n, const float *xyz_h, const int *frame_h, const double *poses12_h,
-                double voxel_size, int layer_limit, int min_ps, const double *eig3, int64_t *M_out, int64_t *K_out,
-                int (*register_csr)(balm_ctx *, int64_t, int64_t)) {
-  if (n < 1 || n >= (1ll << 31) || layer_limit < 0 || layer_limit > 2) {
-    balm_set_error("balm_cut_voxels: bad arguments (n < 2^31, layer_limit in 0..2)");
-    return BALM_ERR_INVALID;
-  }
-  cudaStream_t st = c->stream;
+int assoc_cut(cudaStream_t st, const AssocInput &in, const balm_assoc_opts &o, const AssocRegister &reg,
+              long long *launches) {
+  const bool one = in.frame != nullptr;  // balm_cut_voxels: one problem, rows = frames
+  const int B = one ? 1 : in.n_problems, n_rows = one ? in.n_rows : (int)in.pose_ptr[in.n_problems];
+  const int64_t n = one ? in.n_points : in.n_items;
   ScratchPool pool;
-  AssocParams P{voxel_size, layer_limit, min_ps, {eig3[0], eig3[1], eig3[2]}};
+  AssocParams P{o.voxel_size, o.layer_limit, o.min_ps, {o.eigen_value_array[0], o.eigen_value_array[1], o.eigen_value_array[2]}};
   float *xyz = nullptr;
-  int *frame = nullptr, *idx = nullptr, *idx2 = nullptr, *flag = nullptr, *scan = nullptr, *seg_start = nullptr, *bad = nullptr;
-  unsigned *fkey = nullptr, *fkey2 = nullptr;
-  unsigned long long *key = nullptr, *keyL = nullptr, *keyL2 = nullptr;
   double *poses = nullptr;
-  ATRY(pool.get(&xyz, (size_t)3 * n)); ATRY(pool.get(&frame, (size_t)n)); ATRY(pool.get(&idx, (size_t)n)); ATRY(pool.get(&idx2, (size_t)n));
-  ATRY(pool.get(&flag, (size_t)n)); ATRY(pool.get(&scan, (size_t)n)); ATRY(pool.get(&seg_start, (size_t)n)); ATRY(pool.get(&bad, 1));
-  ATRY(pool.get(&fkey, (size_t)n)); ATRY(pool.get(&fkey2, (size_t)n));
-  ATRY(pool.get(&key, (size_t)n)); ATRY(pool.get(&keyL, (size_t)n)); ATRY(pool.get(&keyL2, (size_t)n));
-  ATRY(pool.get(&poses, (size_t)12 * c->N));
-  CUDA_TRY(cudaMemcpyAsync(xyz, xyz_h, sizeof(float) * 3 * n, cudaMemcpyHostToDevice, st));
-  CUDA_TRY(cudaMemcpyAsync(frame, frame_h, sizeof(int) * n, cudaMemcpyHostToDevice, st));
-  CUDA_TRY(cudaMemcpyAsync(poses, poses12_h, sizeof(double) * 12 * c->N, cudaMemcpyHostToDevice, st));
+  int *src = nullptr, *row = nullptr, *row_slot = nullptr, *row_prob = nullptr, *bad = nullptr;
+  ATRY(pool.get(&xyz, (size_t)3 * in.n_points)); ATRY(pool.get(&poses, (size_t)12 * n_rows));
+  ATRY(pool.get(&src, (size_t)n)); ATRY(pool.get(&row, (size_t)n)); ATRY(pool.get(&bad, 1));
+  ATRY(pool.get(&row_slot, (size_t)2 * n_rows));
+  row_prob = row_slot + n_rows;
+  std::vector<int> hrow((size_t)2 * n_rows, 0);  // per pose row: slot in its problem, problem
+  for (int p = 0; p < B; p++)
+    for (int j = one ? 0 : (int)in.pose_ptr[p]; j < (one ? n_rows : (int)in.pose_ptr[p + 1]); j++) {
+      hrow[j] = one ? j : j - (int)in.pose_ptr[p];
+      hrow[(size_t)n_rows + j] = p;
+    }
+  if (in.n_points) CUDA_TRY(cudaMemcpyAsync(xyz, in.xyz, sizeof(float) * 3 * in.n_points, cudaMemcpyHostToDevice, st));
+  CUDA_TRY(cudaMemcpyAsync(poses, in.poses12, sizeof(double) * 12 * n_rows, cudaMemcpyHostToDevice, st));
+  CUDA_TRY(cudaMemcpyAsync(row_slot, hrow.data(), sizeof(int) * 2 * n_rows, cudaMemcpyHostToDevice, st));
   CUDA_TRY(cudaMemsetAsync(bad, 0, sizeof(int), st));
-  const unsigned gb = (unsigned)((n + 255) / 256);
-  point_key_kernel<<<gb, 256, 0, st>>>(xyz, frame, poses, c->N, n, P, key, bad);
-  // stable order by frame first, so that every later stable sort keeps the frames ascending inside a node
-  iota_kernel<<<gb, 256, 0, st>>>(idx, n);
-  gather_frame_kernel<<<gb, 256, 0, st>>>(frame, idx, fkey, n);
-  size_t tmp_bytes = 0, tb2 = 0, tb3 = 0;
-  cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, fkey, fkey2, idx, idx2, (int)n, 0, 32, st);
-  cub::DeviceRadixSort::SortPairs(nullptr, tb2, keyL, keyL2, idx, idx2, (int)n, 0, 63, st);
-  cub::DeviceScan::ExclusiveSum(nullptr, tb3, flag, scan, (int)n, st);
-  tmp_bytes = std::max(tmp_bytes, std::max(tb2, tb3));
+  int *flag = nullptr, *scan = nullptr, *seg_start = nullptr, *idx = nullptr, *work = nullptr, *work2 = nullptr;
+  unsigned *pk = nullptr, *pk2 = nullptr;
+  unsigned long long *key = nullptr, *keyL = nullptr, *keyL2 = nullptr;
   char *tmp = nullptr;
-  ATRY(pool.get(&tmp, tmp_bytes));
-  CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, fkey, fkey2, idx, idx2, (int)n, 0, 32, st));
-  int *order = idx2;   // frame-sorted point order
-  int *work = idx;     // per-level sorted order
-  c->launches += 4;
+  size_t tmp_bytes = 0;
+  const unsigned gb = (unsigned)((n + 255) / 256);
+  int pbits = 1;
+  while ((1 << pbits) < B) pbits++;
+  if (n > 0) {
+    ATRY(pool.get(&flag, (size_t)n)); ATRY(pool.get(&scan, (size_t)n)); ATRY(pool.get(&seg_start, (size_t)n));
+    ATRY(pool.get(&idx, (size_t)n)); ATRY(pool.get(&work, (size_t)n)); ATRY(pool.get(&work2, (size_t)n));
+    ATRY(pool.get(&pk, (size_t)n)); ATRY(pool.get(&pk2, (size_t)n));
+    ATRY(pool.get(&key, (size_t)n)); ATRY(pool.get(&keyL, (size_t)n)); ATRY(pool.get(&keyL2, (size_t)n));
+    size_t tb1 = 0, tb2 = 0, tb3 = 0;
+    cub::DeviceRadixSort::SortPairs(nullptr, tb1, pk, pk2, idx, work, (int)n, 0, 32, st);
+    cub::DeviceRadixSort::SortPairs(nullptr, tb2, keyL, keyL2, idx, work, (int)n, 0, 63, st);
+    cub::DeviceScan::ExclusiveSum(nullptr, tb3, flag, scan, (int)n, st);
+    tmp_bytes = std::max(tb1, std::max(tb2, tb3));
+    ATRY(pool.get(&tmp, tmp_bytes));
+    if (one) {
+      // items = the points in a stable order by frame, so that every later stable sort keeps the frames ascending
+      // inside a node
+      CUDA_TRY(cudaMemcpyAsync(pk, in.frame, sizeof(int) * n, cudaMemcpyHostToDevice, st));
+      iota_kernel<<<gb, 256, 0, st>>>(idx, n);
+      CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, pk, reinterpret_cast<unsigned *>(row), idx, src, (int)n,
+                                               0, 32, st));
+      *launches += 2;
+    } else {
+      // items in (problem, slot, point) order: frames are already ascending inside every problem
+      std::vector<long long> tab((size_t)2 * n_rows + 1);  // item_ptr [n_rows + 1], then the first point of each row
+      tab[0] = 0;
+      for (int j = 0; j < n_rows; j++) {
+        const int s = in.pose_scan[j];
+        tab[j + 1] = tab[j] + (in.scan_ptr[s + 1] - in.scan_ptr[s]);
+        tab[(size_t)n_rows + 1 + j] = in.scan_ptr[s];
+      }
+      long long *dtab = nullptr;
+      ATRY(pool.get(&dtab, tab.size()));
+      CUDA_TRY(cudaMemcpyAsync(dtab, tab.data(), sizeof(long long) * tab.size(), cudaMemcpyHostToDevice, st));
+      expand_rows_kernel<<<n_rows, 256, 0, st>>>(dtab, dtab + n_rows + 1, src, row);
+      *launches += 1;
+    }
+    item_key_kernel<<<gb, 256, 0, st>>>(xyz, src, row, poses, n_rows, n, P, key, bad);
+    *launches += 1;
+  }
 
   LevelTables T[3];
-  for (int L = 0; L <= layer_limit; L++) {
-    level_key_kernel<<<gb, 256, 0, st>>>(key, order, keyL, n, L);
-    CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, keyL, keyL2, order, work, (int)n, 0, 63, st));
-    seg_flag_kernel<<<gb, 256, 0, st>>>(keyL2, work, frame, n, flag);
+  for (int L = 0; n > 0 && L <= o.layer_limit; L++) {
+    // stable sort of the items by (problem, level key): by key, then by problem
+    level_key_kernel<<<gb, 256, 0, st>>>(key, keyL, n, L);
+    iota_kernel<<<gb, 256, 0, st>>>(idx, n);
+    CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, keyL, keyL2, idx, work, (int)n, 0, 63, st));
+    if (B > 1) {
+      gather_prob_kernel<<<gb, 256, 0, st>>>(work, row, row_prob, pk, n);
+      CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, pk, pk2, work, work2, (int)n, 0, pbits, st));
+      std::swap(work, work2);
+      *launches += 2;
+    }
+    seg_flag_kernel<<<gb, 256, 0, st>>>(key, work, row, n, L, flag);
     CUDA_TRY(cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, flag, scan, (int)n, st));
     int last_flag = 0, last_scan = 0;
     CUDA_TRY(cudaMemcpyAsync(&last_flag, flag + n - 1, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -324,11 +411,12 @@ int assoc_build(balm_ctx *c, int64_t n, const float *xyz_h, const int *frame_h, 
     double *segW = nullptr;
     unsigned long long *seg_key = nullptr;
     int *nflag = nullptr, *nscan = nullptr;
-    ATRY(pool.get(&t.segB, (size_t)10 * nseg)); ATRY(pool.get(&segW, (size_t)10 * nseg)); ATRY(pool.get(&t.seg_frame, (size_t)nseg));
+    ATRY(pool.get(&t.segB, (size_t)10 * nseg)); ATRY(pool.get(&segW, (size_t)10 * nseg)); ATRY(pool.get(&t.seg_row, (size_t)nseg));
     ATRY(pool.get(&seg_key, (size_t)nseg)); ATRY(pool.get(&nflag, (size_t)nseg)); ATRY(pool.get(&nscan, (size_t)nseg));
     const unsigned gs = (unsigned)((nseg + 127) / 128);
-    seg_reduce_kernel<<<gs, 128, 0, st>>>(xyz, frame, poses, work, keyL2, seg_start, nseg, n, t.segB, segW, t.seg_frame, seg_key);
-    node_flag_kernel<<<gs, 128, 0, st>>>(seg_key, nseg, nflag);
+    seg_reduce_kernel<<<gs, 128, 0, st>>>(xyz, src, row, poses, work, key, L, seg_start, nseg, n, t.segB, segW, t.seg_row,
+                                          seg_key);
+    node_flag_kernel<<<gs, 128, 0, st>>>(seg_key, t.seg_row, row_prob, nseg, nflag);
     size_t tb = 0;
     cub::DeviceScan::ExclusiveSum(nullptr, tb, nflag, nscan, nseg, st);
     if (tb > tmp_bytes) { pool.drop(tmp); tmp = nullptr; tmp_bytes = tb; ATRY(pool.get(&tmp, tmp_bytes)); }
@@ -338,31 +426,35 @@ int assoc_build(balm_ctx *c, int64_t n, const float *xyz_h, const int *frame_h, 
     CUDA_TRY(cudaStreamSynchronize(st));
     t.nnode = last_scan + last_flag;
     ATRY(pool.get(&t.node_start, (size_t)t.nnode)); ATRY(pool.get(&t.node_key, (size_t)t.nnode));
-    ATRY(pool.get(&t.node_size, (size_t)t.nnode)); ATRY(pool.get(&t.node_planar, (size_t)t.nnode));
-    ATRY(pool.get(&t.node_nframes, (size_t)t.nnode)); ATRY(pool.get(&t.node_leaf, (size_t)t.nnode));
+    ATRY(pool.get(&t.node_prob, (size_t)t.nnode)); ATRY(pool.get(&t.node_size, (size_t)t.nnode));
+    ATRY(pool.get(&t.node_planar, (size_t)t.nnode)); ATRY(pool.get(&t.node_nframes, (size_t)t.nnode));
+    ATRY(pool.get(&t.node_leaf, (size_t)t.nnode));
     seg_start_kernel<<<gs, 128, 0, st>>>(nflag, nscan, nseg, t.node_start);
-    node_judge_kernel<<<(unsigned)((t.nnode + 127) / 128), 128, 0, st>>>(segW, seg_key, t.node_start, t.nnode, nseg, P.eig[L],
-                                                                        t.node_key, t.node_size, t.node_planar, t.node_nframes);
+    node_judge_kernel<<<(unsigned)((t.nnode + 127) / 128), 128, 0, st>>>(
+        segW, seg_key, t.seg_row, row_prob, t.node_start, t.nnode, nseg, P.eig[L], t.node_key, t.node_prob, t.node_size,
+        t.node_planar, t.node_nframes);
     CUDA_TRY(cudaStreamSynchronize(st));
     pool.drop(segW); pool.drop(seg_key); pool.drop(nflag); pool.drop(nscan);
-    c->launches += 9;
+    *launches += 10;
   }
   int h_bad = 0;
   CUDA_TRY(cudaMemcpy(&h_bad, bad, sizeof(int), cudaMemcpyDeviceToHost));
   if (h_bad) {
-    balm_set_error(h_bad & 2 ? "balm_cut_voxels: frame index outside [0, n_poses)"
-                             : "balm_cut_voxels: a point lies outside the +-2^18 root-voxel range");
+    balm_set_error(std::string(in.who) + (h_bad & 2 ? ": frame index outside [0, n_poses)"
+                                                    : ": a point lies outside the +-2^18 root-voxel range"));
     return BALM_ERR_INVALID;
   }
 
-  // ---- leaves of every layer, merged in key order ----
+  // ---- leaves of every layer, merged in (problem, key) order ----
   int nleaf_L[3] = {0, 0, 0};
   int *lscan[3] = {nullptr, nullptr, nullptr};
-  for (int L = 0; L <= layer_limit; L++) {
+  const AncestorTable a0{T[0].node_key, T[0].node_prob, T[0].node_size, T[0].node_planar, T[0].nnode};
+  const AncestorTable a1{T[1].node_key, T[1].node_prob, T[1].node_size, T[1].node_planar, T[1].nnode};
+  for (int L = 0; n > 0 && L <= o.layer_limit; L++) {
     LevelTables &t = T[L];
     leaf_decide_kernel<<<(unsigned)((t.nnode + 127) / 128), 128, 0, st>>>(
-        L, t.nnode, t.node_key, t.node_size, t.node_planar, t.node_nframes, T[0].node_key, T[0].node_size, T[0].node_planar,
-        T[0].nnode, T[1].node_key, T[1].node_size, T[1].node_planar, T[1].nnode, min_ps, layer_limit, t.node_leaf);
+        L, t.nnode, t.node_key, t.node_prob, t.node_size, t.node_planar, t.node_nframes, a0, a1, o.min_ps, o.layer_limit,
+        t.node_leaf);
     ATRY(pool.get(&lscan[L], (size_t)t.nnode));
     size_t tb = 0;
     cub::DeviceScan::ExclusiveSum(nullptr, tb, t.node_leaf, lscan[L], t.nnode, st);
@@ -375,60 +467,61 @@ int assoc_build(balm_ctx *c, int64_t n, const float *xyz_h, const int *frame_h, 
     nleaf_L[L] = a + b;
   }
   const int nleaf = nleaf_L[0] + nleaf_L[1] + nleaf_L[2];
-  if (nleaf < 1) { balm_set_error("balm_cut_voxels: no plane voxels found"); return BALM_ERR_INVALID; }
-  unsigned long long *lkey = nullptr, *lkey2 = nullptr;
-  int *lref = nullptr, *lref2 = nullptr, *lcnt = nullptr, *lobs = nullptr;
-  ATRY(pool.get(&lkey, (size_t)nleaf)); ATRY(pool.get(&lkey2, (size_t)nleaf)); ATRY(pool.get(&lref, (size_t)nleaf));
-  ATRY(pool.get(&lref2, (size_t)nleaf)); ATRY(pool.get(&lcnt, (size_t)nleaf)); ATRY(pool.get(&lobs, (size_t)nleaf));
-  int base = 0;
-  for (int L = 0; L <= layer_limit; L++) {
-    leaf_collect_kernel<<<(unsigned)((T[L].nnode + 127) / 128), 128, 0, st>>>(L, T[L].nnode, T[L].node_leaf, lscan[L],
-                                                                             T[L].node_key, lkey, lref, base);
-    base += nleaf_L[L];
-  }
-  {
-    size_t tb = 0;
+  std::vector<long long> hptr((size_t)2 * (B + 1), 0);  // voxel_ptr [B + 1], then obs_ptr [B + 1]
+  int *lref = nullptr, *lcnt = nullptr, *lobs = nullptr;
+  if (nleaf > 0) {
+    unsigned long long *lkey = nullptr, *lkey2 = nullptr;
+    int *lref2 = nullptr;
+    long long *dptr = nullptr;
+    ATRY(pool.get(&lkey, (size_t)nleaf)); ATRY(pool.get(&lkey2, (size_t)nleaf)); ATRY(pool.get(&lref, (size_t)nleaf));
+    ATRY(pool.get(&lref2, (size_t)nleaf)); ATRY(pool.get(&lcnt, (size_t)nleaf)); ATRY(pool.get(&lobs, (size_t)nleaf));
+    ATRY(pool.get(&dptr, hptr.size()));
+    int base = 0;
+    for (int L = 0; L <= o.layer_limit; L++) {
+      leaf_collect_kernel<<<(unsigned)((T[L].nnode + 127) / 128), 128, 0, st>>>(L, T[L].nnode, T[L].node_leaf, lscan[L],
+                                                                               T[L].node_key, lkey, lref, base);
+      base += nleaf_L[L];
+    }
+    const unsigned gl = (unsigned)((nleaf + 127) / 128);
+    unsigned *lprob = pk, *lprob2 = pk2;  // the items' problem keys are free now (nleaf <= n)
+    size_t tb = 0, tb2 = 0, tb3 = 0;
     cub::DeviceRadixSort::SortPairs(nullptr, tb, lkey, lkey2, lref, lref2, nleaf, 0, 63, st);
+    cub::DeviceRadixSort::SortPairs(nullptr, tb2, lprob, lprob2, lref, lref2, nleaf, 0, pbits, st);
+    cub::DeviceScan::ExclusiveSum(nullptr, tb3, lcnt, lobs, nleaf, st);
+    tb = std::max(tb, std::max(tb2, tb3));
     if (tb > tmp_bytes) { pool.drop(tmp); tmp = nullptr; tmp_bytes = tb; ATRY(pool.get(&tmp, tmp_bytes)); }
     CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, lkey, lkey2, lref, lref2, nleaf, 0, 63, st));
-  }
-  leaf_count_kernel<<<(unsigned)((nleaf + 127) / 128), 128, 0, st>>>(lref2, nleaf, T[0].node_nframes, T[1].node_nframes,
-                                                                    T[2].node_nframes, lcnt);
-  {
-    size_t tb = 0;
-    cub::DeviceScan::ExclusiveSum(nullptr, tb, lcnt, lobs, nleaf, st);
-    if (tb > tmp_bytes) { pool.drop(tmp); tmp = nullptr; tmp_bytes = tb; ATRY(pool.get(&tmp, tmp_bytes)); }
+    std::swap(lref, lref2);
+    leaf_gather_kernel<unsigned><<<gl, 128, 0, st>>>(lref, nleaf, T[0].node_prob, T[1].node_prob, T[2].node_prob, lprob);
+    if (B > 1) {
+      CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, lprob, lprob2, lref, lref2, nleaf, 0, pbits, st));
+      std::swap(lref, lref2);
+      std::swap(lprob, lprob2);
+    }
+    leaf_gather_kernel<int><<<gl, 128, 0, st>>>(lref, nleaf, T[0].node_nframes, T[1].node_nframes, T[2].node_nframes, lcnt);
     CUDA_TRY(cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, lcnt, lobs, nleaf, st));
+    prob_ptr_kernel<<<(B + 128) / 128, 128, 0, st>>>(lprob, lcnt, lobs, nleaf, B, dptr, dptr + B + 1);
+    CUDA_TRY(cudaMemcpyAsync(hptr.data(), dptr, sizeof(long long) * hptr.size(), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    *launches += 5 + 2 * (o.layer_limit + 1) + (B > 1 ? 1 : 0);
   }
-  int a = 0, b = 0;
-  CUDA_TRY(cudaMemcpyAsync(&a, lcnt + nleaf - 1, sizeof(int), cudaMemcpyDeviceToHost, st));
-  CUDA_TRY(cudaMemcpyAsync(&b, lobs + nleaf - 1, sizeof(int), cudaMemcpyDeviceToHost, st));
-  CUDA_TRY(cudaStreamSynchronize(st));
-  const int64_t K = (int64_t)a + b;
-  // ---- register: allocate the problem arrays of the context and emit straight into them ----
-  ATRY(register_csr(c, nleaf, K));
-  EmitLevel e[3];
-  for (int L = 0; L < 3; L++) e[L] = EmitLevel{T[L].segB, T[L].seg_frame, T[L].node_start, T[L].node_size, T[L].nseg};
-  emit_kernel<<<nleaf, 64, 0, st>>>(lref2, lobs, nleaf, e[0], e[1], e[2], lcnt, c->obs, c->Kp, c->pose_idx, c->row_ptr, c->coe);
+  const int64_t K = hptr[2 * (size_t)B + 1];
+  // ---- register: the caller allocates its arrays for M voxels and K observations; emit straight into them ----
+  AssocEmit out{};
+  ATRY(reg(nleaf, K, reinterpret_cast<const int64_t *>(hptr.data()), reinterpret_cast<const int64_t *>(hptr.data() + B + 1),
+           &out));
+  if (nleaf > 0) {
+    EmitLevel e[3];
+    for (int L = 0; L < 3; L++)
+      e[L] = EmitLevel{T[L].segB, T[L].seg_row, T[L].node_start, T[L].node_size, T[L].node_key, T[L].nseg};
+    emit_kernel<<<nleaf, 64, 0, st>>>(lref, lobs, nleaf, e[0], e[1], e[2], lcnt, row_slot, out);
+    *launches += 1;
+  } else {
+    CUDA_TRY(cudaMemsetAsync(out.row_ptr, 0, sizeof(long long), st));
+  }
   CUDA_TRY(cudaStreamSynchronize(st));
   CUDA_TRY(cudaGetLastError());
-  c->launches += 12;
-  // the voxel keys (ascending) and the parameters stay with the context: balm_append_scan / balm_marginalize need them
-  cudaFree(c->vox_key);
-  c->vox_key = nullptr;
-  CUDA_TRY(cudaMalloc((void **)&c->vox_key, sizeof(unsigned long long) * (size_t)nleaf));
-  CUDA_TRY(cudaMemcpy(c->vox_key, lkey2, sizeof(unsigned long long) * (size_t)nleaf, cudaMemcpyDeviceToDevice));
-  cudaFree(c->vox_layer);
-  c->vox_layer = nullptr;
-  CUDA_TRY(cudaMalloc((void **)&c->vox_layer, sizeof(int) * (size_t)nleaf));
-  leaf_layer_kernel<<<(unsigned)((nleaf + 127) / 128), 128, 0, st>>>(lref2, nleaf, c->vox_layer);
-  CUDA_TRY(cudaStreamSynchronize(st));
-  c->has_keys = true;
-  c->assoc_voxel_size = voxel_size; c->assoc_layer_limit = layer_limit; c->assoc_min_ps = min_ps;
-  for (int q = 0; q < 3; q++) c->assoc_eig[q] = eig3[q];
   // the pool's destructor frees every scratch buffer (level tables included)
-  *M_out = nleaf;
-  *K_out = K;
   return BALM_OK;
 }
 

@@ -397,32 +397,49 @@ extern "C" int balm_set_voxels_dev(balm_ctx *c, int64_t M, const int64_t *row_pt
 extern "C" int64_t balm_num_obs(balm_ctx *c) { return c ? c->K : 0; }
 
 // ---------------- association on the GPU (assoc.cu) ----------------
-int assoc_build(balm_ctx *c, int64_t n, const float *xyz_h, const int *frame_h, const double *poses12_h,
-                double voxel_size, int layer_limit, int min_ps, const double *eig3, int64_t *M_out, int64_t *K_out,
-                int (*register_csr)(balm_ctx *, int64_t, int64_t));
-
-static int assoc_register(balm_ctx *c, int64_t M, int64_t K) { return alloc_problem_arrays(c, M, K, false); }
-
 extern "C" void balm_default_assoc_opts(balm_assoc_opts *o) {
   o->voxel_size = 1.0; o->layer_limit = 2; o->min_ps = 15;
   o->eigen_value_array[0] = o->eigen_value_array[1] = o->eigen_value_array[2] = 1.0 / 16;
+}
+
+// opts or the defaults, with the planarity thresholds rounded as the reference stores them: it keeps them in a
+// `float eigen_value_array[]` (bavoxel.hpp:11) and compares the double ratio with the promoted float (bavoxel.hpp:697),
+// so 1/9 is (double)(float)(1.0/9), not the double 1/9
+balm_assoc_opts resolve_assoc_opts(const balm_assoc_opts *opts) {
+  balm_assoc_opts o;
+  if (opts) o = *opts; else balm_default_assoc_opts(&o);
+  for (double &e : o.eigen_value_array) e = (double)(float)e;
+  return o;
 }
 
 extern "C" int balm_cut_voxels(balm_ctx *c, int64_t n_points, const float *xyz, const int32_t *frame,
                                const double *poses12, const balm_assoc_opts *opts, int64_t *n_voxels_out,
                                int64_t *n_obs_out) {
   if (!c || !xyz || !frame || !poses12) { balm_set_error("balm_cut_voxels: bad arguments"); return BALM_ERR_INVALID; }
+  const balm_assoc_opts o = resolve_assoc_opts(opts);
+  if (n_points < 1 || n_points >= (1ll << 31) || o.layer_limit < 0 || o.layer_limit > 2) {
+    balm_set_error("balm_cut_voxels: bad arguments (n < 2^31, layer_limit in 0..2)");
+    return BALM_ERR_INVALID;
+  }
   CUDA_TRY(cudaSetDevice(c->device));
-  balm_assoc_opts o;
-  if (opts) o = *opts; else balm_default_assoc_opts(&o);
-  // the reference keeps the planarity thresholds in a `float eigen_value_array[]` (bavoxel.hpp:11) and compares the
-  // double ratio with the promoted float (bavoxel.hpp:697): 1/9 is (double)(float)(1.0/9), not the double 1/9
-  for (double &e : o.eigen_value_array) e = (double)(float)e;
-  int64_t M = 0, K = 0;
-  TRY(assoc_build(c, n_points, xyz, frame, poses12, o.voxel_size, o.layer_limit, o.min_ps, o.eigen_value_array, &M, &K,
-                  assoc_register));
-  if (n_voxels_out) *n_voxels_out = M;
-  if (n_obs_out) *n_obs_out = K;
+  AssocInput in{"balm_cut_voxels", n_points, xyz, c->N, poses12, frame, 1, nullptr, nullptr, nullptr, n_points};
+  // register: allocate the problem arrays of the context and the voxel keys, which stay with it (balm_append_scan /
+  // balm_marginalize need them)
+  const AssocRegister reg = [c](int64_t M, int64_t K, const int64_t *, const int64_t *, AssocEmit *out) {
+    if (M < 1) { balm_set_error("balm_cut_voxels: no plane voxels found"); return (int)BALM_ERR_INVALID; }
+    TRY(alloc_problem_arrays(c, M, K, false));
+    drop_keys(c);
+    TRY(dev_alloc(&c->vox_key, (size_t)M));
+    TRY(dev_alloc(&c->vox_layer, (size_t)M));
+    *out = AssocEmit{c->obs, c->Kp, 1, c->pose_idx, c->row_ptr, c->coe, c->vox_key, c->vox_layer};
+    return (int)BALM_OK;
+  };
+  TRY(assoc_cut(c->stream, in, o, reg, &c->launches));
+  c->has_keys = true;
+  c->assoc_voxel_size = o.voxel_size; c->assoc_layer_limit = o.layer_limit; c->assoc_min_ps = o.min_ps;
+  for (int q = 0; q < 3; q++) c->assoc_eig[q] = o.eigen_value_array[q];
+  if (n_voxels_out) *n_voxels_out = c->M;
+  if (n_obs_out) *n_obs_out = c->K;
   return finish_registration(c);
 }
 
@@ -889,9 +906,7 @@ static int window_check(balm_ctx *c, const char *fn, int win_count) {
 extern "C" int balm_window_reset(balm_ctx *c, const balm_assoc_opts *opts) {
   if (!c) { balm_set_error("balm_window_reset: bad arguments"); return BALM_ERR_INVALID; }
   CUDA_TRY(cudaSetDevice(c->device));
-  balm_assoc_opts o;
-  if (opts) o = *opts; else balm_default_assoc_opts(&o);
-  for (double &e : o.eigen_value_array) e = (double)(float)e;  // `float eigen_value_array[]` (bavoxel.hpp:11)
+  const balm_assoc_opts o = resolve_assoc_opts(opts);
   return window_reset_build(c, &c->win, o.voxel_size, o.layer_limit, o.min_ps, o.eigen_value_array);
 }
 extern "C" int balm_window_cut(balm_ctx *c, int64_t n_points, const float *xyz, const double *pose12, int slot) {

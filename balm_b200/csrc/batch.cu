@@ -503,6 +503,8 @@ struct BatchReg {
   long long *row_ptr = nullptr;
   int *pose_idx = nullptr;
   double *obs = nullptr, *fix = nullptr, *coe = nullptr;
+  unsigned long long *key = nullptr;  // [M] octree keys and layers when the voxels were cut from scans, else null
+  int *layer = nullptr;
   double *G = nullptr, *stats = nullptr, *res_v = nullptr, *opart = nullptr, *spart = nullptr, *H = nullptr, *g = nullptr;
   double *poses = nullptr, *trial = nullptr;
   double *r_eval = nullptr, *r2 = nullptr, *r1 = nullptr, *q1 = nullptr, *u = nullptr, *v = nullptr;
@@ -517,7 +519,7 @@ struct BatchReg {
   int *n_active() { return ints + 7 * B; }
   Dev dev() const { return Dev{prob, vox_prob, row_ptr, pose_idx, obs, fix, coe, M, K}; }
   ~BatchReg() {
-    void *ptrs[] = {prob, vox_prob, pose_prob, ochunk_prob, items, row_ptr, pose_idx, obs, fix, coe, G, stats, res_v,
+    void *ptrs[] = {prob, vox_prob, pose_prob, ochunk_prob, items, row_ptr, pose_idx, obs, fix, coe, key, layer, G, stats, res_v,
                     opart, spart, H, g, poses, trial, r_eval, r2, r1, q1, u, v, ints};
     for (void *p : ptrs) cudaFree(p);
   }
@@ -621,15 +623,14 @@ extern "C" int balm_batch_destroy(balm_batch *b) {
   return BALM_OK;
 }
 
-static int build_registration(balm_batch *bt, BatchReg *r, int B, const int64_t *pose_ptr, const int64_t *voxel_ptr,
-                              const int64_t *row_ptr, const int32_t *pose_idx, const double *obs10,
-                              const double *fix10, const double *coe) {
+// Host-side layout of a registration of M = voxel_ptr[B] voxels and K observations: problems, observation-sweep chunks,
+// SYRK items, voxel -> problem, pose -> problem.
+static int reg_layout(balm_batch *bt, BatchReg *r, int B, const int64_t *pose_ptr, const int64_t *voxel_ptr, int64_t K) {
   cudaStream_t st = bt->stream;
   r->B = B;
   r->P = (int)pose_ptr[B];
   r->M = voxel_ptr[B];
-  r->K = row_ptr[r->M];
-  // host-side layout: problems, observation-sweep chunks, SYRK items, voxel -> problem, pose -> problem
+  r->K = K;
   std::vector<int> vox_prob((size_t)r->M), pose_prob((size_t)r->P), ochunk_prob;
   std::vector<int4> items;
   r->hprob.resize(B);
@@ -667,11 +668,14 @@ static int build_registration(balm_batch *bt, BatchReg *r, int B, const int64_t 
   BTRY(upload(&r->pose_prob, pose_prob.data(), pose_prob.size(), st));
   BTRY(upload(&r->ochunk_prob, ochunk_prob.data(), ochunk_prob.size(), st));
   BTRY(upload(&r->items, items.data(), items.size(), st));
-  BTRY(upload(&r->row_ptr, reinterpret_cast<const long long *>(row_ptr), (size_t)r->M + 1, st));
-  BTRY(upload(&r->pose_idx, pose_idx, (size_t)r->K, st));
-  BTRY(upload(&r->obs, obs10, (size_t)r->K * 10, st));
-  if (fix10) BTRY(upload(&r->fix, fix10, (size_t)r->M * 10, st));
-  BTRY(upload(&r->coe, coe, (size_t)r->M, st));
+  return BALM_OK;
+}
+
+// With row_ptr / pose_idx / obs / coe (/ fix) in place: the per-voxel checks on the device, the per-pose plane counts
+// of the precheck, and the workspaces.
+static int reg_finish(balm_batch *bt, BatchReg *r) {
+  cudaStream_t st = bt->stream;
+  const int B = r->B;
   BTRY(dalloc(&r->ints, 7 * (size_t)B + 1));
   int *d_planes = nullptr;
   BTRY(dalloc(&d_planes, (size_t)r->P));
@@ -709,6 +713,31 @@ static int build_registration(balm_batch *bt, BatchReg *r, int B, const int64_t 
   return BALM_OK;
 }
 
+static int build_registration(balm_batch *bt, BatchReg *r, int B, const int64_t *pose_ptr, const int64_t *voxel_ptr,
+                              const int64_t *row_ptr, const int32_t *pose_idx, const double *obs10,
+                              const double *fix10, const double *coe) {
+  cudaStream_t st = bt->stream;
+  BTRY(reg_layout(bt, r, B, pose_ptr, voxel_ptr, row_ptr[voxel_ptr[B]]));
+  BTRY(upload(&r->row_ptr, reinterpret_cast<const long long *>(row_ptr), (size_t)r->M + 1, st));
+  BTRY(upload(&r->pose_idx, pose_idx, (size_t)r->K, st));
+  BTRY(upload(&r->obs, obs10, (size_t)r->K * 10, st));
+  if (fix10) BTRY(upload(&r->fix, fix10, (size_t)r->M * 10, st));
+  BTRY(upload(&r->coe, coe, (size_t)r->M, st));
+  return reg_finish(bt, r);
+}
+
+// Replaces the registration with r once r is complete; otherwise deletes r and keeps the previous one.
+static int install(balm_batch *bt, BatchReg *r, int rc) {
+  if (rc != BALM_OK) {
+    cudaStreamSynchronize(bt->stream);
+    delete r;
+    return rc;
+  }
+  delete bt->reg;
+  bt->reg = r;
+  return BALM_OK;
+}
+
 extern "C" int balm_batch_set_voxels(balm_batch *bt, int n_problems, const int64_t *pose_ptr, const int64_t *voxel_ptr,
                                      const int64_t *row_ptr, const int32_t *pose_idx, const double *obs10,
                                      const double *fix10, const double *coe) {
@@ -732,14 +761,98 @@ extern "C" int balm_batch_set_voxels(balm_batch *bt, int n_problems, const int64
   CUDA_TRY(cudaSetDevice(bt->device));
   CUDA_TRY(cudaStreamSynchronize(bt->stream));
   BatchReg *r = new BatchReg();
-  const int rc = build_registration(bt, r, n_problems, pose_ptr, voxel_ptr, row_ptr, pose_idx, obs10, fix10, coe);
-  if (rc != BALM_OK) {  // the previous registration stays in place
-    cudaStreamSynchronize(bt->stream);
-    delete r;
-    return rc;
+  return install(bt, r, build_registration(bt, r, n_problems, pose_ptr, voxel_ptr, row_ptr, pose_idx, obs10, fix10, coe));
+}
+
+extern "C" int balm_batch_cut_voxels(balm_batch *bt, int n_problems, const int64_t *pose_ptr, const int32_t *pose_scan,
+                                     int n_scans, const int64_t *scan_ptr, const float *xyz, const double *poses12,
+                                     const balm_assoc_opts *opts, int64_t *n_voxels_out, int64_t *n_obs_out) {
+  if (!bt || !pose_ptr || !pose_scan || !scan_ptr || !poses12 || n_scans < 1)
+    return invalid("balm_batch_cut_voxels: bad arguments");
+  if (n_problems < 1) return invalid("balm_batch_cut_voxels: n_problems must be >= 1");
+  if (pose_ptr[0] != 0) return invalid("balm_batch_cut_voxels: pose_ptr[0] must be 0");
+  for (int b = 0; b < n_problems; b++) {
+    const int64_t np = pose_ptr[b + 1] - pose_ptr[b];
+    if (np < 1 || np > BALM_BATCH_MAX_POSES)
+      return invalid("balm_batch_cut_voxels: every problem needs 1 .. BALM_BATCH_MAX_POSES poses (pose_ptr ascending)");
   }
-  delete bt->reg;
-  bt->reg = r;
+  if (scan_ptr[0] != 0) return invalid("balm_batch_cut_voxels: scan_ptr[0] must be 0");
+  for (int s = 0; s < n_scans; s++)
+    if (scan_ptr[s + 1] < scan_ptr[s]) return invalid("balm_batch_cut_voxels: scan_ptr must be ascending");
+  const balm_assoc_opts o = resolve_assoc_opts(opts);
+  if (o.layer_limit < 0 || o.layer_limit > 2) return invalid("balm_batch_cut_voxels: layer_limit must be in 0..2");
+  const int64_t P = pose_ptr[n_problems], n_points = scan_ptr[n_scans];
+  int64_t n_items = 0;  // points replicated over the windows that use them
+  for (int64_t j = 0; j < P; j++) {
+    const int s = pose_scan[j];
+    if (s < 0 || s >= n_scans) return invalid("balm_batch_cut_voxels: pose_scan entry outside [0, n_scans)");
+    n_items += scan_ptr[s + 1] - scan_ptr[s];
+  }
+  if (n_points > 0 && !xyz) return invalid("balm_batch_cut_voxels: bad arguments");
+  if (n_items >= ((int64_t)1 << 31) || n_points >= ((int64_t)1 << 31)) {
+    balm_set_error("balm_batch_cut_voxels: 2^31 or more points, counted once per pose row that uses them");
+    return BALM_ERR_UNSUPPORTED;
+  }
+  CUDA_TRY(cudaSetDevice(bt->device));
+  CUDA_TRY(cudaStreamSynchronize(bt->stream));
+  BatchReg *r = new BatchReg();
+  std::vector<int64_t> obs_ptr;
+  const AssocInput in{"balm_batch_cut_voxels", n_points, xyz, (int)P, poses12, nullptr, n_problems, pose_ptr, pose_scan,
+                      scan_ptr, n_items};
+  const AssocRegister reg = [&](int64_t M, int64_t K, const int64_t *voxel_ptr, const int64_t *optr, AssocEmit *out) {
+    BTRY(reg_layout(bt, r, n_problems, pose_ptr, voxel_ptr, K));
+    BTRY(dalloc(&r->row_ptr, (size_t)M + 1));
+    BTRY(dalloc(&r->pose_idx, (size_t)K));
+    BTRY(dalloc(&r->obs, (size_t)K * 10));
+    BTRY(dalloc(&r->coe, (size_t)M));
+    BTRY(dalloc(&r->key, (size_t)M));
+    BTRY(dalloc(&r->layer, (size_t)M));
+    *out = AssocEmit{r->obs, 1, 10, r->pose_idx, r->row_ptr, r->coe, r->key, r->layer};
+    obs_ptr.assign(optr, optr + n_problems + 1);
+    return (int)BALM_OK;
+  };
+  long long launches = 0;
+  int rc = assoc_cut(bt->stream, in, o, reg, &launches);
+  if (rc == BALM_OK) rc = reg_finish(bt, r);
+  if (rc == BALM_OK)
+    for (int b = 0; b < n_problems; b++) {
+      if (n_voxels_out) n_voxels_out[b] = r->hprob[b].nvox;
+      if (n_obs_out) n_obs_out[b] = obs_ptr[b + 1] - obs_ptr[b];
+    }
+  return install(bt, r, rc);
+}
+
+extern "C" int balm_batch_sizes(balm_batch *bt, int *n_problems, int64_t *n_poses, int64_t *n_voxels, int64_t *n_obs) {
+  if (!bt) return invalid("balm_batch_sizes: bad arguments");
+  const BatchReg *r = bt->reg;
+  if (!r) return invalid("balm_batch_sizes: no problems registered");
+  if (n_problems) *n_problems = r->B;
+  if (n_poses) *n_poses = r->P;
+  if (n_voxels) *n_voxels = r->M;
+  if (n_obs) *n_obs = r->K;
+  return BALM_OK;
+}
+
+extern "C" int balm_batch_download_voxels(balm_batch *bt, int64_t *voxel_ptr, int64_t *row_ptr, int32_t *pose_idx,
+                                          double *obs10, double *coe, uint64_t *keys, int32_t *layers) {
+  if (!bt) return invalid("balm_batch_download_voxels: bad arguments");
+  const BatchReg *r = bt->reg;
+  if (!r) return invalid("balm_batch_download_voxels: no problems registered");
+  if ((keys || layers) && !r->key)
+    return invalid("balm_batch_download_voxels: keys and layers exist only after balm_batch_cut_voxels");
+  CUDA_TRY(cudaSetDevice(bt->device));
+  cudaStream_t st = bt->stream;
+  if (voxel_ptr) {
+    for (int b = 0; b < r->B; b++) voxel_ptr[b] = r->hprob[b].vox_base;
+    voxel_ptr[r->B] = r->M;
+  }
+  if (row_ptr) CUDA_TRY(cudaMemcpyAsync(row_ptr, r->row_ptr, sizeof(int64_t) * (r->M + 1), cudaMemcpyDeviceToHost, st));
+  if (pose_idx && r->K) CUDA_TRY(cudaMemcpyAsync(pose_idx, r->pose_idx, sizeof(int32_t) * r->K, cudaMemcpyDeviceToHost, st));
+  if (obs10 && r->K) CUDA_TRY(cudaMemcpyAsync(obs10, r->obs, sizeof(double) * 10 * r->K, cudaMemcpyDeviceToHost, st));
+  if (coe && r->M) CUDA_TRY(cudaMemcpyAsync(coe, r->coe, sizeof(double) * r->M, cudaMemcpyDeviceToHost, st));
+  if (keys && r->M) CUDA_TRY(cudaMemcpyAsync(keys, r->key, sizeof(uint64_t) * r->M, cudaMemcpyDeviceToHost, st));
+  if (layers && r->M) CUDA_TRY(cudaMemcpyAsync(layers, r->layer, sizeof(int32_t) * r->M, cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
   return BALM_OK;
 }
 

@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
+#include <functional>
 #include <string>
 #include "../../include/balm_b200.h"
 
@@ -490,3 +491,42 @@ int tensor_syrk_check(balm_ctx *c);
 int tensor_syrk_check_enqueue(balm_ctx *c);
 int tensor_syrk_check_finish(balm_ctx *c);
 void tensor_syrk_new_problem(balm_ctx *c);
+
+// ---------------- association (assoc.cu) ----------------
+// The plane voxels of one or more problems cut from raw scans. Host arrays; xyz (n_points x 3 float32, body frame) and
+// poses12 are uploaded once. Either frame != NULL: one problem whose pose rows are its frames (balm_cut_voxels; the
+// points of frame f are in slot f), or a problem table: problem p owns the rows [pose_ptr[p], pose_ptr[p+1]) and row j
+// is the scan pose_scan[j] = points [scan_ptr[s], scan_ptr[s+1]) in slot j - pose_ptr[p]; n_items = the sum of the
+// rows' point counts (< 2^31, checked by the caller).
+struct AssocInput {
+  const char *who;  // prefix of error messages
+  int64_t n_points;
+  const float *xyz;
+  int n_rows;  // pose rows when frame != NULL
+  const double *poses12;
+  const int32_t *frame;
+  int n_problems;
+  const int64_t *pose_ptr;
+  const int32_t *pose_scan;
+  const int64_t *scan_ptr;
+  int64_t n_items;
+};
+// Where the voxels are emitted (device arrays): observation o, column c at obs[c * obs_cstride + o * obs_ostride]
+// (SoA of a context or AoS of a batch), pose_idx = slot, row_ptr [M + 1], coe, key and layer [M].
+struct AssocEmit {
+  double *obs;
+  int64_t obs_cstride, obs_ostride;
+  int *pose_idx;
+  long long *row_ptr;
+  double *coe;
+  unsigned long long *key;
+  int *layer;
+};
+// Called once the sizes are known: M voxels, K observations, per problem voxel_ptr / obs_ptr [B + 1]. Allocates the
+// destination and fills *out, or returns an error that ends the call.
+using AssocRegister = std::function<int(int64_t M, int64_t K, const int64_t *voxel_ptr, const int64_t *obs_ptr,
+                                        AssocEmit *out)>;
+balm_assoc_opts resolve_assoc_opts(const balm_assoc_opts *opts);  // opts or the defaults, eigen ratios rounded to float
+// opts: from resolve_assoc_opts, layer_limit in 0..2 (checked by the caller)
+int assoc_cut(cudaStream_t st, const AssocInput &in, const balm_assoc_opts &opts, const AssocRegister &reg,
+              long long *launches);

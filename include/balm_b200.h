@@ -226,6 +226,32 @@ int balm_batch_evaluate(balm_batch *b, const double *poses12, int include_fix, d
  * returned instead of printed. The host waits once per iteration. */
 int balm_batch_damping_iter(balm_batch *b, double *poses12, const balm_lm_opts *opts, int *status, int *n_iters,
                             balm_trace *trace, double *poses_per_iter);
+/* Association for a batch: the plane voxels of every problem cut from raw scans on the device and registered as
+ * balm_batch_set_voxels would register them. Scans are given once: scan s is xyz[scan_ptr[s] .. scan_ptr[s+1]) (float32,
+ * body frame). Problem p owns the pose rows [pose_ptr[p], pose_ptr[p+1]) of poses12 (P x 12, the initial poses, the
+ * same array later passed to balm_batch_damping_iter); pose row j is scan pose_scan[j] in slot j - pose_ptr[p].
+ * Windows may share scans (HBA windows overlap by half); each problem sees only its own slots.
+ * Problem p's voxels are bitwise those balm_cut_voxels registers on a context of N_p poses given the points of its scans
+ * concatenated in slot order, frame = slot, and its pose rows (ascending node key; row_ptr, pose_idx = slot, obs10, coe,
+ * keys, layers). opts as balm_cut_voxels (NULL: the defaults; eigen ratios rounded to float). A problem without a plane
+ * voxel gets an empty voxel range; balm_batch_damping_iter then reports BALM_ERR_TOO_FEW_PLANES for it unless
+ * min_planes_per_pose is 0. No fix clusters. A problem's result depends on nothing else in the batch; two calls are
+ * bitwise equal. Points are uploaded once; host synchronisations and allocations are a fixed number per octree layer,
+ * whatever the number of problems. BALM_ERR_INVALID (the previous registration stays in place): the problem-table checks
+ * of balm_batch_set_voxels, scan_ptr not starting at 0 or not ascending, a pose_scan entry outside [0, n_scans),
+ * layer_limit outside 0..2, a point outside the +-2^18 root-voxel range. BALM_ERR_UNSUPPORTED, before anything is
+ * allocated: 2^31 or more points, counted once per pose row that uses them (or in xyz). n_voxels_out / n_obs_out: [B]
+ * or NULL. */
+int balm_batch_cut_voxels(balm_batch *b, int n_problems, const int64_t *pose_ptr, const int32_t *pose_scan,
+                          int n_scans, const int64_t *scan_ptr, const float *xyz, const double *poses12,
+                          const balm_assoc_opts *opts, int64_t *n_voxels_out, int64_t *n_obs_out);
+/* Sizes of the current registration, then a copy of it (any pointer may be NULL): voxel_ptr [B + 1], row_ptr [M + 1]
+ * (over all voxels), pose_idx [K] (problem-local), obs10 [K x 10], coe [M]; keys / layers [M] as balm_download_keys, per
+ * problem in ascending key, only after balm_batch_cut_voxels (non-NULL otherwise -> BALM_ERR_INVALID). Fix clusters
+ * are not copied. No registration -> BALM_ERR_INVALID. */
+int balm_batch_sizes(balm_batch *b, int *n_problems, int64_t *n_poses, int64_t *n_voxels, int64_t *n_obs);
+int balm_batch_download_voxels(balm_batch *b, int64_t *voxel_ptr, int64_t *row_ptr, int32_t *pose_idx, double *obs10,
+                               double *coe, uint64_t *keys, int32_t *layers);
 
 /* Pose-covariance propagation of the consistency experiment (SURVEY.md section 8f, row N3):
  *   Rcov_raw = sum over observations of  Ls c_cov Ls^T      -- VOX_HESS::left_jacobian_point + BALM2::multi_second

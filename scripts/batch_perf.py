@@ -2,7 +2,9 @@
 pose count and, for every window, set_voxels + damping_iter, on the fp64 and on the tensor path.
 
 Workloads (HBA's bottom layer splits a trajectory into many short windows): (a) 256 windows x 10 poses x 1 000 planes,
-(b) 32 windows x 32 poses x 5 000 planes. Every window is generated on the GPU by Context.synth_virtual (its own seed) and
+(b) 32 windows x 32 poses x 5 000 planes, and (c) one bottom layer from raw scans: 160 synthetic scans of 20 000
+points (assoc_ref.synthetic_scans, room 12), windows of 10 scans every 5 scans (31 windows), associated per window and as
+one batch (see run_from_scans). For (a) and (b) every window is generated on the GPU by Context.synth_virtual (its own seed) and
 read back with download_voxels, so the batch and the loop run on the same host arrays. Two option sets: fixed work
 (force_hess, rel_tol < 0, 10 iterations: every LM iteration does the same work) and the defaults. The batch, the fp64 loop
 and the tensor loop alternate --repeats times in one process; every call ends in a device synchronisation, so a host clock
@@ -113,16 +115,112 @@ def run_workload(name, n_windows, n_poses, n_planes, repeats, seed0):
     return out
 
 
+def layer_windows(n, length=10, stride=5):
+    out, s = [], 0
+    while True:
+        out.append(list(range(s, min(s + length, n))))
+        if s + length >= n:
+            return out
+        s += stride
+
+
+def run_from_scans(n_scans, pts_per_scan, room, repeats):
+    """Workload (c), one HBA bottom layer from raw scans: (i) a Context per window, cut_voxels + damping_iter; (ii) per
+    window cut_voxels + download_voxels, then Batch.set_problems + damping_iter; (iii) Batch.cut_scans + damping_iter.
+    Association + registration and LM are timed apart."""
+    import assoc_ref
+    import scenes
+    import balm_b200
+    pts, frs, poses = assoc_ref.synthetic_scans(n_poses=n_scans, pts_per_scan=pts_per_scan, room=room)
+    scans = [pts[frs == i].astype(np.float32) for i in range(n_scans)]
+    p12 = scenes.pack_poses([r for r, _ in poses], [p for _, p in poses])
+    windows = layer_windows(n_scans)
+    wposes = [p12[w] for w in windows]
+    wpts = [np.concatenate([scans[s] for s in w]) for w in windows]
+    wfr = [np.concatenate([np.full(len(scans[s]), k, dtype=np.int32) for k, s in enumerate(w)]) for w in windows]
+    kwc = dict(voxel_size=2.0, eigen_value_array=(1 / 16, 1 / 16, 1 / 9))
+    options = {"fixed": dict(max_iter=10, force_hess=True, rel_tol=-1.0, gauge_mode=2, min_planes_per_pose=0),
+               "default": dict(min_planes_per_pose=0)}
+    ctx = {n: balm_b200.Context(n, 0, balm_b200.PREC_FP64) for n in {len(w) for w in windows}}
+    batch = balm_b200.Batch(0)
+    out = dict(scans=n_scans, pts_per_scan=pts_per_scan, windows=len(windows), window=10, stride=5,
+               points_replicated=int(sum(len(x) for x in wpts)))
+
+    def clock(f):
+        t0 = time.perf_counter()
+        r = f()
+        return r, 1e3 * (time.perf_counter() - t0)
+
+    for key, kw in options.items():
+        ms = {k: [] for k in ("i_assoc", "i_lm", "ii_assoc_register", "ii_lm", "iii_cut", "iii_lm")}
+        for rep in range(repeats + 1):  # the first round warms up every shape
+            ta = tl = 0.0
+            p_i = []
+            for w, x0 in enumerate(wposes):
+                c = ctx[len(windows[w])]
+                _, t = clock(lambda: c.cut_voxels(wpts[w], wfr[w], x0, **kwc))
+                ta += t
+                (p, _, _), t = clock(lambda: c.damping_iter(x0, **kw))
+                tl += t
+                p_i.append(p)
+
+            def per_window():
+                probs = []
+                for w, x0 in enumerate(wposes):
+                    c = ctx[len(windows[w])]
+                    c.cut_voxels(wpts[w], wfr[w], x0, **kwc)
+                    rp, pi, ob, co = c.download_voxels()
+                    probs.append(dict(n_poses=len(windows[w]), row_ptr=rp, pose_idx=pi, obs10=ob, coe=co))
+                batch.set_problems(probs)
+            _, t_ii = clock(per_window)
+            r_ii, l_ii = clock(lambda: batch.damping_iter(wposes, **kw))
+            _, t_iii = clock(lambda: batch.cut_scans(scans, windows, wposes, **kwc))
+            r_iii, l_iii = clock(lambda: batch.damping_iter(wposes, **kw))
+            if rep == 0:
+                continue
+            for k, v in (("i_assoc", ta), ("i_lm", tl), ("ii_assoc_register", t_ii), ("ii_lm", l_ii), ("iii_cut", t_iii),
+                         ("iii_lm", l_iii)):
+                ms[k].append(v)
+        out[key] = dict(ms=ms, ms_median={k: float(np.median(v)) for k, v in ms.items()},
+                        ii_iii_poses_bitwise_equal=bool(all(np.array_equal(a[1], b[1]) for a, b in zip(r_ii, r_iii))),
+                        max_pose_diff_iii_vs_i=max(float(np.abs(a[1] - b).max()) for a, b in zip(r_iii, p_i)),
+                        iters_iii=[len(r[2]) for r in r_iii])
+    try:  # one profiled cut_scans call of its own: device time per kernel
+        import torch
+        from torch.profiler import ProfilerActivity, profile
+        torch.cuda.synchronize()
+        with profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
+            batch.cut_scans(scans, windows, wposes, **kwc)
+            torch.cuda.synchronize()
+        per = {}
+        for e in prof.key_averages():
+            t = getattr(e, "device_time_total", None)
+            if t is None:
+                t = e.cuda_time_total
+            if t > 0 or "cuda" in e.key.lower():
+                per[e.key] = dict(device_ms=t / 1e3, host_ms=e.cpu_time_total / 1e3, calls=e.count)
+        out["profile_cut_scans"] = per
+    except Exception as e:
+        out["profile_cut_scans"] = f"profiler failed: {e}"
+    batch.close()
+    for c in ctx.values():
+        c.close()
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--repeats", type=int, default=3)
-    ap.add_argument("--workloads", default="a,b")
+    ap.add_argument("--workloads", default="a,b,c")
     ap.add_argument("--out", default=None, help="also write the result to this JSON file")
     a = ap.parse_args()
     shapes = {"a": (256, 10, 1000, 100), "b": (32, 32, 5000, 900)}
     res = dict(gpu=gpu_info(), repeats=a.repeats)
     for w in a.workloads.split(","):
-        res[w] = run_workload(w, *shapes[w][:3], a.repeats, shapes[w][3])
+        if w == "c":
+            res[w] = run_from_scans(160, 20000, 12.0, a.repeats)
+        else:
+            res[w] = run_workload(w, *shapes[w][:3], a.repeats, shapes[w][3])
     if a.out:
         os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
         with open(a.out, "w") as f:

@@ -1,7 +1,8 @@
 """Small end-to-end run for compute-sanitizer (memcheck / racecheck): both precision modes, dense + sparse; the persistent
 tile-DAG factorisation with several 64-column steps (n = 240: chain + near/far workers), the sliding-window marginalisation, the pose-covariance propagation, a multi-batch sparse evaluation, the device
 association chain balm_cut_voxels -> balm_marginalize -> balm_append_scan (octree keys + layers), and a batch of
-independent problems (balm_batch_*: a dense one with fix clusters, a sparse one of 32 poses, an empty one)."""
+independent problems (balm_batch_*: a dense one with fix clusters, a sparse one of 32 poses, an empty one), and a batch
+association of overlapping windows with one empty window (balm_batch_cut_voxels)."""
 import os, sys
 import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -54,5 +55,15 @@ x = [s["poses_init"] for s in scs] + [np.tile([1, 0, 0, 0, 1, 0, 0, 0, 1, 0, 0, 
 print("batch r", [r for _, _, r in b.evaluate(x, include_fix=True)], flush=True)
 res = b.damping_iter(x, max_iter=2, min_planes_per_pose=0, hess_includes_fix=True, want_per_iter=True)
 print("batch iters", [len(tr) for _, _, tr, _ in res], flush=True)
+b.close()
+# batch association: overlapping windows (2 and 4 scans sharing scans) and one empty window (a single scan)
+pts, frs, poses = assoc_ref.synthetic_scans(n_poses=6, pts_per_scan=1500, seed=14)
+p12 = scenes.pack_poses([r for r, _ in poses], [p for _, p in poses])
+scans = [pts[frs == i] for i in range(6)]
+windows = [[0, 1, 2, 3], [2, 3, 4, 5], [4]]
+b = balm_b200.Batch(0)
+mk = b.cut_scans(scans, windows, [p12[w] for w in windows])
+res = b.damping_iter([p12[w] for w in windows], max_iter=2, min_planes_per_pose=0)
+print("batch cut", mk, "iters", [len(tr) for _, _, tr, _ in res], flush=True)
 b.close()
 print("SANITIZE_DONE")
