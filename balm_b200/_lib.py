@@ -50,7 +50,8 @@ SYMBOLS = ["balm_last_error", "balm_version", "balm_create", "balm_destroy", "ba
            "balm_download_voxels", "balm_download_voxel_range", "balm_num_obs", "balm_default_assoc_opts", "balm_cut_voxels", "balm_pose_covariance", "balm_marginalize", "balm_download_fix", "balm_append_scan",
            "balm_download_keys", "balm_window_reset", "balm_window_cut", "balm_window_recut", "balm_window_marginalize",
            "balm_window_push", "balm_batch_create", "balm_batch_destroy", "balm_batch_set_voxels", "balm_batch_evaluate",
-           "balm_batch_damping_iter", "balm_batch_cut_voxels", "balm_batch_sizes", "balm_batch_download_voxels"]
+           "balm_batch_damping_iter", "balm_batch_cut_voxels", "balm_batch_sizes", "balm_batch_download_voxels",
+           "balm_batch_pose_covariance"]
 
 
 def lib():
@@ -110,6 +111,8 @@ def lib():
                                            [C.POINTER(AssocOpts), C.c_void_p, C.c_void_p]
         L.balm_batch_sizes.argtypes = [C.c_void_p, C.POINTER(C.c_int)] + [C.POINTER(C.c_int64)] * 3
         L.balm_batch_download_voxels.argtypes = [C.c_void_p] + [C.c_void_p] * 7
+        L.balm_batch_pose_covariance.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_double, C.c_int] + \
+                                                [C.c_void_p] * 3
         _lib = L
     return _lib
 

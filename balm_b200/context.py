@@ -358,3 +358,31 @@ class Batch:
             out.append((int(status[b]), poses[p0:p1].copy(), tr,
                         per_iter[:int(n_it[b]), p0:p1].copy() if want_per_iter else None))
         return out
+
+    def pose_covariance(self, poses_list, point_noise=0.0, c_cov=None, include_fix=False, want_raw=True, want_cov=True):
+        """Context.pose_covariance per problem, all in one call (include/balm_b200.h, balm_batch_pose_covariance) -> per
+        problem (status, Rcov_raw, Rcov). c_cov: per problem a K_p x 9 x 9 array of its observations' cluster
+        covariances (concatenated as set_problems concatenates obs10), or None for isotropic point noise. status is
+        ERR_NOT_PD (Rcov zero) where H is singular, e.g. without fix clusters; always OK with want_cov=False."""
+        poses = self._concat(poses_list)
+        ns = [6 * n for n in self.n_poses]
+        cc = None
+        if c_cov is not None:
+            cc = np.ascontiguousarray(np.concatenate([np.asarray(c, dtype=np.float64).reshape(-1, 81) for c in c_cov]),
+                                      dtype=np.float64)
+            K = C.c_int64()
+            L.check(L.lib().balm_batch_sizes(self._h, None, None, None, C.byref(K)))
+            if len(cc) != K.value:
+                raise ValueError(f"c_cov has {len(cc)} observations, the registration {K.value}")
+        size = sum(n * n for n in ns)
+        raw = np.zeros(size) if want_raw else None
+        cov = np.zeros(size) if want_cov else None
+        status = np.zeros(len(ns), dtype=np.int32)
+        L.check(L.lib().balm_batch_pose_covariance(self._h, _p(poses), _p(cc), float(point_noise), int(include_fix),
+                                                   _p(status), _p(raw), _p(cov)))
+        out, o = [], 0
+        for b, n in enumerate(ns):
+            out.append((int(status[b]), raw[o:o + n * n].reshape(n, n, order="F") if want_raw else None,
+                        cov[o:o + n * n].reshape(n, n, order="F") if want_cov else None))
+            o += n * n
+        return out

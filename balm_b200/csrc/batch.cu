@@ -15,6 +15,14 @@
 // The host waits once per iteration, for the number of problems still active. Every split of work depends on the
 // problem alone and every sum runs in a fixed order (no floating-point atomics), so a problem's results do not depend on
 // the other problems of the batch or on its position in it.
+//
+// The pose covariance (balm_batch_pose_covariance) follows the same rules, with the per-observation terms of covariance.cu:
+//   batch_stats_kernel<true>    (inside enqueue_eval when Rcov is wanted, which also gives H) at the given poses
+//   batch_cov_rows_kernel       per voxel: Wz, the eight rows c2 Q^T | c2 V^T (8 M_p x ldp per problem), c2^2 D per obs
+//   batch_cov_diag_kernel       per 32-voxel chunk: per-pose partial sums of the c2^2 D blocks
+//   batch_syrk_kernel<8, 4>     per (problem, tile, 768-row chunk): partial of Q V^T + V Q^T (A = partner row ^ 4)
+//   batch_cov_assemble_kernel   per (problem, 64-column block): Rcov_raw = + sum of partials + blockdiag
+//   batch_cov_solve_kernel      per problem, one CTA: LDL^T of H, singularity test, H^-1 Rcov_raw H^-1, symmetrised
 #include <math.h>
 #include <string.h>
 #include <algorithm>
@@ -169,7 +177,12 @@ __global__ void __launch_bounds__(128) batch_obs_kernel(Dev d, const double *pos
   }
 }
 
-// ---- per (problem, upper 64x64 tile, 768-row chunk): partial of G'^T G' with DMMA, 2 x 2 warps of 32 x 32 ----
+// ---- per (problem, upper 64x64 tile, 768-row chunk): partial of A^T G with DMMA, 2 x 2 warps of 32 x 32 ----
+// RPV rows per voxel, problem p's rows at G + goff_p / 3 * RPV (the layout of G', 3 rows per voxel, with RPV rows).
+// A is G (XOR = 0: the Hessian's G'^T G') or G with every row replaced by its partner row ^ XOR (XOR = 4: the eight
+// covariance rows c2 Q^T | c2 V^T of a voxel give Q V^T + V Q^T). ROWS is a multiple of 8, so a partner never
+// straddles a chunk.
+template <int RPV, int XOR>
 __global__ void __launch_bounds__(128) batch_syrk_kernel(const Prob *prob, const int *mask, const int4 *items,
                                                          const double *G, double *spart) {
   __shared__ __align__(16) double sA[KB][LDS], sB[KB][LDS];
@@ -178,9 +191,10 @@ __global__ void __launch_bounds__(128) batch_syrk_kernel(const Prob *prob, const
   const Prob pr = prob[it.x];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int wm = warp >> 1, wn = warp & 1, fr = lane >> 2, fk = lane & 3;
-  const long long rows = 3 * pr.nvox, k_begin = (long long)it.w * ROWS;
+  const long long rows = RPV * pr.nvox, k_begin = (long long)it.w * ROWS;
   const long long k_end = k_begin + ROWS < rows ? k_begin + ROWS : rows;
-  const double *gA = G + pr.goff + it.y * TILE, *gB = G + pr.goff + it.z * TILE;
+  const double *G0 = G + (RPV == 3 ? pr.goff : pr.goff / 3 * RPV);
+  const double *gA = G0 + it.y * TILE, *gB = G0 + it.z * TILE;
   double acc[4][4][2];
 #pragma unroll
   for (int i = 0; i < 4; i++)
@@ -192,7 +206,7 @@ __global__ void __launch_bounds__(128) batch_syrk_kernel(const Prob *prob, const
       const long long kr = k0 + rr;
       double2 va = make_double2(0.0, 0.0), vb = va;
       if (kr < k_end) {
-        va = *reinterpret_cast<const double2 *>(gA + (size_t)kr * pr.ldp + cc);
+        va = *reinterpret_cast<const double2 *>(gA + (size_t)(kr ^ XOR) * pr.ldp + cc);
         vb = *reinterpret_cast<const double2 *>(gB + (size_t)kr * pr.ldp + cc);
       }
       *reinterpret_cast<double2 *>(&sA[rr][cc]) = va;
@@ -318,6 +332,32 @@ __device__ double damped_q1(const double *x, const double *D, const double *gb, 
   return 0.5 * s;
 }
 
+// Unpivoted right-looking LDL^T of the packed lower triangle in A, in place (unit-lower L below the diagonal, D on it);
+// col: n doubles of scratch. Stops at a zero / tiny / non-finite pivot (ldlt.cu's criterion) and returns true then.
+// Block-wide; the result is the same in every thread.
+__device__ __forceinline__ bool ldl_factor(double *A, int n, double *col) {
+  const int tid = threadIdx.x;
+  for (int k = 0; k < n; k++) {
+    const int kk = tri_idx(k, k, n);
+    const double dk = A[kk];
+    if (!(fabs(dk) > 1e-290 && fabs(dk) < 1e300)) return true;
+    for (int i = k + 1 + tid; i < n; i += SOLVE_THREADS) {
+      const double t = A[kk + i - k];
+      col[i] = t;
+      A[kk + i - k] = t / dk;
+    }
+    __syncthreads();
+    const int lane = tid & 31, warp = tid >> 5;
+    for (int j = k + 1 + warp; j < n; j += SOLVE_THREADS / 32) {
+      const double cj = col[j];
+      double *Aj = A + tri_idx(j, j, n);
+      for (int i = j + lane; i < n; i += 32) Aj[i - j] -= A[kk + i - k] * cj;
+    }
+    __syncthreads();
+  }
+  return false;
+}
+
 __global__ void __launch_bounds__(SOLVE_THREADS) batch_solve_kernel(const Prob *prob, const int *active, const double *H,
                                                                     const double *g, const double *uvec,
                                                                     const double *poses, double *trial, double *q1_out,
@@ -343,26 +383,8 @@ __global__ void __launch_bounds__(SOLVE_THREADS) batch_solve_kernel(const Prob *
   }
   for (int i = tid; i < n; i += SOLVE_THREADS) x[i] = -gb[i];
   __syncthreads();
-  // unpivoted right-looking LDL^T; a zero / tiny / non-finite pivot (ldlt.cu's criterion) makes the step not_pd
-  bool pivot_bad = false;
-  for (int k = 0; k < n; k++) {
-    const int kk = tri_idx(k, k, n);
-    const double dk = A[kk];
-    if (!(fabs(dk) > 1e-290 && fabs(dk) < 1e300)) { pivot_bad = true; break; }
-    for (int i = k + 1 + tid; i < n; i += SOLVE_THREADS) {
-      const double t = A[kk + i - k];
-      col[i] = t;
-      A[kk + i - k] = t / dk;
-    }
-    __syncthreads();
-    const int lane = tid & 31, warp = tid >> 5;
-    for (int j = k + 1 + warp; j < n; j += SOLVE_THREADS / 32) {
-      const double cj = col[j];
-      double *Aj = A + tri_idx(j, j, n);
-      for (int i = j + lane; i < n; i += 32) Aj[i - j] -= A[kk + i - k] * cj;
-    }
-    __syncthreads();
-  }
+  // a zero / tiny / non-finite pivot makes the step not_pd
+  const bool pivot_bad = ldl_factor(A, n, col);
   int not_pd = pivot_bad ? 1 : 0;
   double q1 = 0.0;
   if (!pivot_bad) {
@@ -487,6 +509,206 @@ __global__ void fill_kernel(int *p, int n, int val) {
   if (i < n) p[i] = val;
 }
 
+// ---------------- pose covariance (balm_batch_pose_covariance; the mathematics is covariance.cu's) ----------------
+// Per lane of the rows kernel, in shared memory: its CovTerms (padded by one double: a stride of 115 doubles leaves at
+// most two lanes on a bank) and its 9 x 9 c_cov. In registers they would not fit next to E c.
+constexpr int COV_TSTRIDE = (int)(sizeof(CovTerms) / sizeof(double)) + 1;
+constexpr int COV_SMEM = 32 * (COV_TSTRIDE + 81) * (int)sizeof(double);
+
+// ---- per voxel, a CTA of one warp, lane = observation (k <= 32): Wz = sum_j Z_j c_j Z_j^T (fixed-order shuffle reduction),
+// then the voxel's eight rows c2 Q^T | c2 V^T into the problem's row buffer and every observation's c2^2 D block ----
+__global__ void __launch_bounds__(32) batch_cov_rows_kernel(Dev d, const double *poses, const double *stats,
+                                                            const double *ccov, double pn2, double *rows, double *Dobs) {
+  extern __shared__ double cov_sm[];
+  __shared__ double Wz[4][4];  // the voxel's, the same in every lane
+  const int lane = threadIdx.x;
+  CovTerms &t = *reinterpret_cast<CovTerms *>(cov_sm + lane * COV_TSTRIDE);
+  double *C = cov_sm + 32 * COV_TSTRIDE + lane * 81;
+  const int64_t v = blockIdx.x;
+  const Prob pr = d.prob[d.vox_prob[v]];
+  const long long s0 = d.row_ptr[v];
+  const int k = (int)(d.row_ptr[v + 1] - s0);
+  const long long s = s0 + lane;
+  const double *st = stats + (size_t)v * BALM_STATS_STRIDE;
+  double acc[10];
+#pragma unroll
+  for (int e = 0; e < 10; e++) acc[e] = 0.0;
+  const int p = lane < k ? d.pose_idx[s] : 0;
+  if (lane < k) {
+    double o[10];
+#pragma unroll
+    for (int c = 0; c < 10; c++) o[c] = d.obs[(size_t)s * 10 + c];
+    if (ccov) {
+      for (int e = 0; e < 81; e++) C[e] = ccov[(size_t)s * 81 + e];
+    } else {
+      cluster_cov_iso(o, pn2, C);
+    }
+    cov_terms(o, poses + 12 * (size_t)(pr.pose_base + p), st, t);
+    cov_wz_add(t, C, acc);
+  }
+#pragma unroll
+  for (int e = 0; e < 10; e++) acc[e] = warp_sum(acc[e]);
+  if (lane == 0) {
+    int q = 0;
+    for (int i = 0; i < 4; i++)
+      for (int j = i; j < 4; j++) { Wz[i][j] = acc[q]; Wz[j][i] = acc[q]; q++; }
+  }
+  __syncwarp();
+  if (lane < k) {
+    const double c2 = st[16] * 2.0 * st[12];  // coe * 2 / NN
+    double *g = rows + pr.goff / 3 * 8 + (size_t)(8 * (v - pr.vox_base)) * pr.ldp + 6 * p;
+    cov_obs_rows(t, C, Wz, c2, g, pr.ldp, Dobs + (size_t)s * 21);
+  }
+}
+
+// ---- per chunk of CHUNK voxels of one problem, one warp, lane = problem-local pose: the sum of the pose's c2^2 D
+// blocks over the chunk's voxels in ascending order ----
+__global__ void __launch_bounds__(128) batch_cov_diag_kernel(Dev d, const int *ochunk_prob, int n_ochunks,
+                                                             const double *Dobs, double *dpart) {
+  __shared__ int slot_of[4][32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int c = blockIdx.x * 4 + warp;
+  if (c >= n_ochunks) return;
+  const Prob pr = d.prob[ochunk_prob[c]];
+  double acc[21];
+#pragma unroll
+  for (int q = 0; q < 21; q++) acc[q] = 0.0;
+  const long long v0 = pr.vox_base + (long long)(c - pr.ochunk_base) * CHUNK;
+  const long long v1 = v0 + CHUNK < pr.vox_base + pr.nvox ? v0 + CHUNK : pr.vox_base + pr.nvox;
+  for (long long v = v0; v < v1; v++) {
+    const long long s0 = d.row_ptr[v];
+    const int k = (int)(d.row_ptr[v + 1] - s0);
+    slot_of[warp][lane] = -1;
+    __syncwarp();
+    if (lane < k) slot_of[warp][d.pose_idx[s0 + lane]] = lane;
+    __syncwarp();
+    const int slot = slot_of[warp][lane];
+    __syncwarp();
+    if (slot < 0) continue;
+    const double *dd = Dobs + (size_t)(s0 + slot) * 21;
+#pragma unroll
+    for (int q = 0; q < 21; q++) acc[q] += dd[q];
+  }
+  if (lane < pr.np) {
+    double *pp = dpart + (size_t)c * 21 * 32 + lane;
+#pragma unroll
+    for (int q = 0; q < 21; q++) pp[q * 32] = acc[q];
+  }
+}
+
+// ---- per (problem, 64-column block): Rcov_raw = + sum over row chunks of the SYRK partials + blockdiag(D), the
+// Hessian assembly with the opposite sign and no gradient. cit[p] = (first SYRK item, row chunks) of problem p. ----
+__global__ void __launch_bounds__(256) batch_cov_assemble_kernel(const Prob *prob, const int2 *cit, const double *dpart,
+                                                                 const double *spart, double *R) {
+  __shared__ double accs[21][32];
+  const int b = blockIdx.x;
+  const Prob pr = prob[b];
+  const int n = pr.n, nt = pr.ldp / TILE;
+  if (blockIdx.y * TILE >= n) return;
+  const int2 ci = cit[b];
+  for (int e = threadIdx.x; e < 21 * pr.np; e += 256) {
+    const int q = e / pr.np, i = e % pr.np;
+    double s = 0.0;
+    for (int c = 0; c < pr.n_ochunks; c++) s += dpart[((size_t)(pr.ochunk_base + c) * 21 + q) * 32 + i];
+    accs[q][i] = s;
+  }
+  __syncthreads();
+  double *Rb = R + pr.hoff;
+  const int j_end = (blockIdx.y + 1) * TILE < n ? (blockIdx.y + 1) * TILE : n;
+  for (int j = blockIdx.y * TILE; j < j_end; j++) {
+    for (int i = threadIdx.x; i < n; i += 256) {
+      const int rr = i < j ? i : j, cc = i < j ? j : i;
+      const int bi = rr / TILE, bj = cc / TILE;
+      const int t = bi * nt - bi * (bi - 1) / 2 + (bj - bi);
+      const double *src = spart + (size_t)(ci.x + t * ci.y) * TILE * TILE + (rr % TILE) * TILE + cc % TILE;
+      double s = 0.0;
+      for (int c = 0; c < ci.y; c++) s += src[(size_t)c * TILE * TILE];
+      const int pi = rr / 6;
+      if (pi == cc / 6) {
+        const int r6 = rr % 6, c6 = cc % 6;
+        s += accs[r6 * 6 - r6 * (r6 - 1) / 2 + (c6 - r6)][pi];
+      }
+      Rb[(size_t)j * n + i] = s;
+    }
+  }
+}
+
+// ---- per problem, one CTA: undamped LDL^T of H in shared memory, the singularity test of pose_covariance_dev, then
+// Rcov = H^-1 R H^-1 as two sweeps over n right-hand sides, thread t owning right-hand side t (R and the result in
+// global memory, n^2 doubles being too many for shared memory; every access below is coalesced across threads).
+// The result is made exactly symmetric by copying its upper triangle to the lower one. ----
+// x <- (L D L^T)^-1 x for the vector x[i * n] (i = 0 .. n-1), the factors in A; one thread
+__device__ __forceinline__ void ldl_apply_strided(const double *A, int n, double *x) {
+  for (int i = 0; i < n; i++) {  // L y = x
+    double s = x[(size_t)i * n];
+    for (int k = 0; k < i; k++) s -= A[tri_idx(i, k, n)] * x[(size_t)k * n];
+    x[(size_t)i * n] = s;
+  }
+  for (int i = n - 1; i >= 0; i--) {  // L^T x = D^-1 y
+    double s = x[(size_t)i * n] / A[tri_idx(i, i, n)];
+    for (int k = n - 1; k > i; k--) s -= A[tri_idx(k, i, n)] * x[(size_t)k * n];
+    x[(size_t)i * n] = s;
+  }
+}
+
+__global__ void __launch_bounds__(SOLVE_THREADS) batch_cov_solve_kernel(const Prob *prob, const double *H,
+                                                                        const double *Rraw, double *Rcov, int *status) {
+  extern __shared__ double sm[];
+  __shared__ int singular;
+  const int b = blockIdx.x;
+  const Prob pr = prob[b];
+  const int n = pr.n, tid = threadIdx.x;
+  double *A = sm, *col = A + n * (n + 1) / 2;
+  const double *Hb = H + pr.hoff, *Rb = Rraw + pr.hoff;
+  double *X = Rcov + pr.hoff;
+  for (int e = tid; e < n * n; e += SOLVE_THREADS) {
+    const int j = e / n, i = e % n;
+    if (i >= j) A[tri_idx(i, j, n)] = Hb[e];
+  }
+  __syncthreads();
+  const bool pivot_bad = ldl_factor(A, n, col);
+  if (tid == 0) {
+    // a singular H (free gauge) pivots at rounding level relative to the others rather than at zero
+    double dmin = 1e300, dmax = 0.0;
+    for (int i = 0; i < n && !pivot_bad; i++) {
+      const double dd = fabs(A[tri_idx(i, i, n)]);
+      dmin = fmin(dmin, dd);
+      dmax = fmax(dmax, dd);
+    }
+    singular = pivot_bad || !(dmin > 1e-11 * dmax);
+    status[b] = singular ? BALM_ERR_NOT_PD : BALM_OK;
+  }
+  __syncthreads();
+  if (singular) {
+    for (int e = tid; e < n * n; e += SOLVE_THREADS) X[e] = 0.0;
+    return;
+  }
+  // X[t + i n] = (H^-1 R)(i, t): right-hand side t is column t of R, read as row t (R is exactly symmetric)
+  if (tid < n) {
+    for (int i = 0; i < n; i++) X[tid + (size_t)i * n] = Rb[tid + (size_t)i * n];
+    ldl_apply_strided(A, n, X + tid);
+  }
+  __syncthreads();
+  // transpose in place: X[t + i n] = (H^-1 R)(t, i), so right-hand side t of the second sweep is row t of H^-1 R
+  for (int e = tid; e < n * n; e += SOLVE_THREADS) {
+    const int i = e % n, j = e / n;
+    if (i < j) {
+      const double a = X[e], c = X[j + (size_t)i * n];
+      X[e] = c;
+      X[j + (size_t)i * n] = a;
+    }
+  }
+  __syncthreads();
+  // X[t + i n] = (H^-1 (H^-1 R)^T)(i, t) = (H^-1 R H^-1)(i, t): column-major, X holds the transpose of the result,
+  // which is the result up to rounding; its upper triangle is kept
+  if (tid < n) ldl_apply_strided(A, n, X + tid);
+  __syncthreads();
+  for (int e = tid; e < n * n; e += SOLVE_THREADS) {
+    const int i = e % n, j = e / n;
+    if (i > j) X[e] = X[j + (size_t)i * n];
+  }
+}
+
 }  // namespace
 
 // One registration: the problems, their voxels and every workspace sized for them. A new registration is built and
@@ -569,7 +791,7 @@ int enqueue_eval(balm_batch *bt, BatchReg *r, const int *mask, bool use_fix) {
   if (r->n_ochunks > 0)
     batch_obs_kernel<<<(r->n_ochunks + 3) / 4, 128, 0, st>>>(d, r->poses, mask, r->ochunk_prob, r->n_ochunks, r->stats,
                                                              r->G, r->opart);
-  if (r->n_items > 0) batch_syrk_kernel<<<r->n_items, 128, 0, st>>>(r->prob, mask, r->items, r->G, r->spart);
+  if (r->n_items > 0) batch_syrk_kernel<3, 0><<<r->n_items, 128, 0, st>>>(r->prob, mask, r->items, r->G, r->spart);
   batch_assemble_kernel<<<dim3(r->B, MAXN / TILE), 256, 0, st>>>(r->prob, mask, r->opart, r->spart, r->H, r->g);
   CUDA_TRY(cudaGetLastError());
   return BALM_OK;
@@ -598,6 +820,8 @@ extern "C" int balm_batch_create(balm_batch **out, int device) {
   cudaDeviceProp prop;
   CUDA_TRY(cudaGetDeviceProperties(&prop, device));
   CUDA_TRY(cudaFuncSetAttribute(batch_solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SOLVE_SMEM));
+  CUDA_TRY(cudaFuncSetAttribute(batch_cov_solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SOLVE_SMEM));
+  CUDA_TRY(cudaFuncSetAttribute(batch_cov_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, COV_SMEM));
   balm_batch *b = new balm_batch();
   b->device = device;
   b->sm_count = prop.multiProcessorCount;
@@ -930,5 +1154,91 @@ extern "C" int balm_batch_damping_iter(balm_batch *bt, double *poses12, const ba
   if (trace && max_iter > 0)
     CUDA_TRY(cudaMemcpyAsync(trace, d_trace, sizeof(balm_trace) * B * max_iter, cudaMemcpyDeviceToHost, st));
   CUDA_TRY(cudaStreamSynchronize(st));
+  return BALM_OK;
+}
+
+extern "C" int balm_batch_pose_covariance(balm_batch *bt, const double *poses12, const double *c_cov81, double point_noise,
+                                          int include_fix, int *status, double *Rcov_raw, double *Rcov) {
+  if (!bt || !poses12) return invalid("balm_batch_pose_covariance: bad arguments");
+  BatchReg *r = bt->reg;
+  if (!r) return invalid("balm_batch_pose_covariance: no problems registered");
+  if (r->M >= ((int64_t)1 << 31)) {
+    balm_set_error("balm_batch_pose_covariance: 2^31 or more voxels");
+    return BALM_ERR_UNSUPPORTED;
+  }
+  CUDA_TRY(cudaSetDevice(bt->device));
+  cudaStream_t st = bt->stream;
+  const int B = r->B;
+  // the covariance SYRK's items: per problem its upper tiles x chunks of ROWS of its 8 M_p rows
+  std::vector<int4> items;
+  std::vector<int2> cit((size_t)B);
+  for (int b = 0; b < B; b++) {
+    const Prob &p = r->hprob[b];
+    const int nt = p.ldp / TILE, nrc = (int)((8 * p.nvox + ROWS - 1) / ROWS);
+    cit[b] = make_int2((int)items.size(), nrc);
+    for (int ti = 0; ti < nt; ti++)
+      for (int tj = ti; tj < nt; tj++)
+        for (int c = 0; c < nrc; c++) items.push_back(make_int4(b, ti, tj, c));
+  }
+  struct Scratch {  // device scratch of one call, freed on every exit path
+    std::vector<void *> p;
+    ~Scratch() { for (void *q : p) cudaFree(q); }
+  } pool;
+  auto get = [&](auto **out, size_t count) {
+    const int rc = dalloc(out, count);
+    if (rc == BALM_OK) pool.p.push_back((void *)*out);
+    return rc;
+  };
+  double *rows = nullptr, *Dobs = nullptr, *dpart = nullptr, *spart = nullptr, *raw = nullptr, *cov = nullptr,
+         *ccov = nullptr;
+  int4 *d_items = nullptr;
+  int2 *d_cit = nullptr;
+  int *d_status = nullptr;
+  const size_t n_rows = r->G_size / 3 * 8;
+  BTRY(get(&rows, n_rows));
+  BTRY(get(&Dobs, (size_t)r->K * 21));
+  BTRY(get(&dpart, (size_t)r->n_ochunks * 21 * 32));
+  BTRY(get(&spart, items.size() * TILE * TILE));
+  BTRY(get(&raw, r->H_size));
+  BTRY(get(&d_items, items.size()));
+  BTRY(get(&d_cit, (size_t)B));
+  if (Rcov) {
+    BTRY(get(&cov, r->H_size));
+    BTRY(get(&d_status, (size_t)B));
+  }
+  if (c_cov81) {
+    BTRY(get(&ccov, (size_t)r->K * 81));
+    if (r->K) CUDA_TRY(cudaMemcpyAsync(ccov, c_cov81, sizeof(double) * 81 * r->K, cudaMemcpyHostToDevice, st));
+  }
+  if (!items.empty())
+    CUDA_TRY(cudaMemcpyAsync(d_items, items.data(), sizeof(int4) * items.size(), cudaMemcpyHostToDevice, st));
+  CUDA_TRY(cudaMemcpyAsync(d_cit, cit.data(), sizeof(int2) * B, cudaMemcpyHostToDevice, st));
+  CUDA_TRY(cudaMemcpyAsync(r->poses, poses12, sizeof(double) * 12 * r->P, cudaMemcpyHostToDevice, st));
+  const Dev d = r->dev();
+  // the voxel statistics at these poses (fix clusters as include_fix): with Rcov, the evaluation of H computes them
+  if (Rcov) {
+    BTRY(enqueue_eval(bt, r, r->ones(), include_fix != 0));
+  } else if (r->M > 0) {
+    const int blocks = (int)std::min<int64_t>((r->M + 7) / 8, (int64_t)bt->sm_count * 8);
+    batch_stats_kernel<true><<<blocks, 256, 0, st>>>(d, r->poses, r->ones(), include_fix != 0 ? 1 : 0, r->stats, r->res_v);
+  }
+  CUDA_TRY(cudaMemsetAsync(rows, 0, sizeof(double) * n_rows, st));  // columns of non-observing poses stay zero
+  if (r->M > 0) {  // one CTA per voxel: a grid-stride loop would cost the kernel a spill
+    batch_cov_rows_kernel<<<(unsigned)r->M, 32, COV_SMEM, st>>>(d, r->poses, r->stats, ccov, point_noise * point_noise, rows,
+                                                        Dobs);
+  }
+  if (r->n_ochunks > 0)
+    batch_cov_diag_kernel<<<(r->n_ochunks + 3) / 4, 128, 0, st>>>(d, r->ochunk_prob, r->n_ochunks, Dobs, dpart);
+  if (!items.empty())
+    batch_syrk_kernel<8, 4><<<(unsigned)items.size(), 128, 0, st>>>(r->prob, r->ones(), d_items, rows, spart);
+  batch_cov_assemble_kernel<<<dim3(B, MAXN / TILE), 256, 0, st>>>(r->prob, d_cit, dpart, spart, raw);
+  if (Rcov) batch_cov_solve_kernel<<<B, SOLVE_THREADS, SOLVE_SMEM, st>>>(r->prob, r->H, raw, cov, d_status);
+  CUDA_TRY(cudaGetLastError());
+  if (Rcov_raw) CUDA_TRY(cudaMemcpyAsync(Rcov_raw, raw, sizeof(double) * r->H_size, cudaMemcpyDeviceToHost, st));
+  if (Rcov) CUDA_TRY(cudaMemcpyAsync(Rcov, cov, sizeof(double) * r->H_size, cudaMemcpyDeviceToHost, st));
+  if (Rcov && status) CUDA_TRY(cudaMemcpyAsync(status, d_status, sizeof(int) * B, cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  if (!Rcov && status)
+    for (int b = 0; b < B; b++) status[b] = BALM_OK;
   return BALM_OK;
 }

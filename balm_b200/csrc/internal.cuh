@@ -383,6 +383,165 @@ __device__ __forceinline__ void cross3(const double *a, const double *b, double 
   c[2] = a[0] * b[1] - a[1] * b[0];
 }
 
+// ---- pose-covariance propagation (covariance.cu, batch.cu): the per-observation terms of left_jacobian_point ----
+__device__ __forceinline__ void hat3(const double *v, double *M /*3x3 row-major*/) {
+  M[0] = 0; M[1] = -v[2]; M[2] = v[1];
+  M[3] = v[2]; M[4] = 0; M[5] = -v[0];
+  M[6] = -v[1]; M[7] = v[0]; M[8] = 0;
+}
+// g1(w): 4 x 9 (BAs_left.hpp:321-331), row-major
+__device__ __forceinline__ void g1_mat(const double *w, double *X /*[4][9]*/) {
+#pragma unroll
+  for (int e = 0; e < 36; e++) X[e] = 0.0;
+  X[0] = w[0]; X[1] = w[1]; X[2] = w[2]; X[6] = w[3];
+  X[9 + 1] = w[0]; X[9 + 3] = w[1]; X[9 + 4] = w[2]; X[9 + 7] = w[3];
+  X[18 + 2] = w[0]; X[18 + 4] = w[1]; X[18 + 5] = w[2]; X[18 + 8] = w[3];
+  X[27 + 6] = w[0]; X[27 + 7] = w[1]; X[27 + 8] = w[2];
+}
+
+// c_cov (9x9, row-major) of a cluster under isotropic point noise, from its moments (toolss.hpp:311-343):
+// Bi = x Ex + y Ey + z Ez  ->  sum Bf Bf^T = [[sum_kl P_kl E_k E_l^T, sum_k v_k E_k], [sym, N I]]
+__device__ __forceinline__ void cluster_cov_iso(const double *o, double pn2, double *C /*[81]*/) {
+  const double P[3][3] = {{o[0], o[1], o[2]}, {o[1], o[3], o[4]}, {o[2], o[4], o[5]}};
+  // E_k as (row, col, value) triplets: Ex: (0,0,2) (1,1,1) (2,2,1); Ey: (1,0,1) (3,1,2) (4,2,1); Ez: (2,0,1) (4,1,1) (5,2,2)
+  const int Er[3][3] = {{0, 1, 2}, {1, 3, 4}, {2, 4, 5}};
+  const double Ev[3][3] = {{2, 1, 1}, {1, 2, 1}, {1, 1, 2}};
+#pragma unroll
+  for (int e = 0; e < 81; e++) C[e] = 0.0;
+  for (int k = 0; k < 3; k++)
+    for (int l = 0; l < 3; l++)
+      for (int cc = 0; cc < 3; cc++)  // (E_k E_l^T)[r1][r2] = sum_c E_k[r1][c] E_l[r2][c]; column c holds one entry per E
+        C[Er[k][cc] * 9 + Er[l][cc]] += P[k][l] * Ev[k][cc] * Ev[l][cc];
+  for (int k = 0; k < 3; k++)
+    for (int cc = 0; cc < 3; cc++) {
+      C[Er[k][cc] * 9 + 6 + cc] += o[6 + k] * Ev[k][cc];
+      C[(6 + cc) * 9 + Er[k][cc]] += o[6 + k] * Ev[k][cc];
+    }
+  for (int d = 0; d < 3; d++) C[(6 + d) * 9 + 6 + d] = o[9];
+#pragma unroll
+  for (int e = 0; e < 81; e++) C[e] *= pn2;
+}
+
+// Everything one observation contributes to the covariance sum (covariance.cu explains the factorisation).
+struct CovTerms {
+  double Z[4][9];   // [G_j ; -h_j^T / NN]
+  double E[6][9];
+  double Q[6][4];   // [A_p | a_p]
+};
+
+// o: the observation, pose12: its pose, st: the voxel's stats row (store_stats_row: vb, u0..u2, 1/NN, coe, lambda)
+__device__ __forceinline__ void cov_terms(const double *o, const double *pose12, const double *st, CovTerms &t) {
+  double r[9], p[3];
+  load_pose(pose12, r, p);  // row-major R
+  const double *vb = st, *u0 = st + 3, *u1 = st + 6, *u2 = st + 9;
+  const double inv = st[12];
+  const double lam0 = st[17], lam1 = st[18], lam2 = st[19];
+  const WC w = world_cluster(o, r, p);
+  // m = P' - v' vb^T, mb = v' - n vb  (= TC [R | p - vb]^T, as in the observation sweep)
+  const double m[3][3] = {{w.p00 - w.v0 * vb[0], w.p01 - w.v0 * vb[1], w.p02 - w.v0 * vb[2]},
+                          {w.p01 - w.v1 * vb[0], w.p11 - w.v1 * vb[1], w.p12 - w.v1 * vb[2]},
+                          {w.p02 - w.v2 * vb[0], w.p12 - w.v2 * vb[1], w.p22 - w.v2 * vb[2]}};
+  const double mb[3] = {w.v0 - w.n * vb[0], w.v1 - w.n * vb[1], w.v2 - w.n * vb[2]};
+  double t0[3], s0 = 0.0;
+  for (int a = 0; a < 3; a++) { t0[a] = m[a][0] * u0[0] + m[a][1] * u0[1] + m[a][2] * u0[2]; s0 += mb[a] * u0[a]; }
+  // A_p = [hat(t0) - hat(u0) m ; s0 I + u0 mb^T]
+  double Ht[9], Hu[9];
+  hat3(t0, Ht);
+  hat3(u0, Hu);
+  for (int a = 0; a < 3; a++)
+    for (int b = 0; b < 3; b++) {
+      t.Q[a][b] = Ht[a * 3 + b] - (Hu[a * 3] * m[0][b] + Hu[a * 3 + 1] * m[1][b] + Hu[a * 3 + 2] * m[2][b]);
+      t.Q[3 + a][b] = (a == b ? s0 : 0.0) + u0[a] * mb[b];
+    }
+  // a_p = [-u0 x v' ; n u0]
+  const double vw[3] = {w.v0, w.v1, w.v2};
+  double cuv[3];
+  cross3(u0, vw, cuv);
+  for (int a = 0; a < 3; a++) { t.Q[a][3] = -cuv[a]; t.Q[3 + a][3] = w.n * u0[a]; }
+  // ub = R^T u0, w4 = [ub ; p.u0], w5 = [ub ; (p - vb).u0]
+  double ub[3];
+  for (int a = 0; a < 3; a++) ub[a] = r[a] * u0[0] + r[3 + a] * u0[1] + r[6 + a] * u0[2];
+  const double pu = p[0] * u0[0] + p[1] * u0[1] + p[2] * u0[2];
+  const double vu = vb[0] * u0[0] + vb[1] * u0[1] + vb[2] * u0[2];
+  const double w4[4] = {ub[0], ub[1], ub[2], pu}, w5[4] = {ub[0], ub[1], ub[2], pu - vu};
+  double X[36];
+  // B_j = [R | p - vb] g1(w4) - (vb.u0) [0 | R]   (3 x 9)
+  g1_mat(w4, X);
+  double B[3][9];
+  for (int a = 0; a < 3; a++)
+    for (int e = 0; e < 9; e++)
+      B[a][e] = r[a * 3] * X[e] + r[a * 3 + 1] * X[9 + e] + r[a * 3 + 2] * X[18 + e] + (p[a] - vb[a]) * X[27 + e];
+  for (int a = 0; a < 3; a++)
+    for (int b = 0; b < 3; b++) B[a][6 + b] -= vu * r[a * 3 + b];
+  // G_j = Mk B_j / NN,  Mk = sum_{k=1,2} u_k u_k^T / (lam0 - lam_k)
+  const double f1 = 1.0 / (lam0 - lam1), f2 = 1.0 / (lam0 - lam2);
+  for (int e = 0; e < 9; e++) {
+    const double d1 = u1[0] * B[0][e] + u1[1] * B[1][e] + u1[2] * B[2][e];
+    const double d2 = u2[0] * B[0][e] + u2[1] * B[1][e] + u2[2] * B[2][e];
+    for (int a = 0; a < 3; a++) t.Z[a][e] = (f1 * u1[a] * d1 + f2 * u2[a] * d2) * inv;
+    t.Z[3][e] = 0.0;
+  }
+  for (int b = 0; b < 3; b++) t.Z[3][6 + b] = -ub[b] * inv;  // -h_j^T / NN, h_j = [0_6, R^T u0]
+  // E_p = U_l T g1(w5): top = -hat(u0) (R X03 + p X3), bottom = u0 X3
+  g1_mat(w5, X);
+  for (int e = 0; e < 9; e++) {
+    double y[3];
+    for (int a = 0; a < 3; a++) y[a] = r[a * 3] * X[e] + r[a * 3 + 1] * X[9 + e] + r[a * 3 + 2] * X[18 + e] + p[a] * X[27 + e];
+    double cy[3];
+    cross3(u0, y, cy);
+    for (int a = 0; a < 3; a++) { t.E[a][e] = -cy[a]; t.E[3 + a][e] = u0[a] * X[27 + e]; }
+  }
+}
+
+// acc[0..9] += upper triangle of Z c Z^T (4x4), row-major: one observation's part of the voxel's Wz
+__device__ __forceinline__ void cov_wz_add(const CovTerms &t, const double *C, double *acc) {
+  double ZC[4][9];
+  for (int i = 0; i < 4; i++)
+    for (int e = 0; e < 9; e++) {
+      double x = 0.0;
+      for (int f = 0; f < 9; f++) x += t.Z[i][f] * C[f * 9 + e];
+      ZC[i][e] = x;
+    }
+  int q = 0;
+  for (int i = 0; i < 4; i++)
+    for (int j = i; j < 4; j++) {
+      double x = 0.0;
+      for (int e = 0; e < 9; e++) x += ZC[i][e] * t.Z[j][e];
+      acc[q++] += x;
+    }
+}
+
+// One observation's six columns of its voxel's eight rows (c2 Q^T | c2 V^T): g[m * ld + i], m = 0..7, i = 0..5 (g points
+// at column 6 p of the voxel's first row), and its diagonal block c2^2 D = c2^2 E c E^T, upper triangle row-major -> d[21]
+__device__ __forceinline__ void cov_obs_rows(const CovTerms &t, const double *C, const double (&Wz)[4][4], double c2,
+                                             double *g, int ld, double *d) {
+  // EC = E c (6x9);  Y^T = E c Z^T (6x4);  D = E c E^T (6x6)
+  double EC[6][9];
+  for (int i = 0; i < 6; i++)
+    for (int e = 0; e < 9; e++) {
+      double x = 0.0;
+      for (int f = 0; f < 9; f++) x += t.E[i][f] * C[f * 9 + e];
+      EC[i][e] = x;
+    }
+  for (int i = 0; i < 6; i++) {
+    for (int mcol = 0; mcol < 4; mcol++) {
+      double yt = 0.0;
+      for (int e = 0; e < 9; e++) yt += EC[i][e] * t.Z[mcol][e];
+      double qw = 0.0;
+      for (int f = 0; f < 4; f++) qw += t.Q[i][f] * Wz[f][mcol];
+      g[(size_t)mcol * ld + i] = c2 * t.Q[i][mcol];
+      g[(size_t)(4 + mcol) * ld + i] = c2 * (0.5 * qw + yt);
+    }
+  }
+  int q = 0;
+  for (int i = 0; i < 6; i++)
+    for (int j = i; j < 6; j++) {
+      double x = 0.0;
+      for (int e = 0; e < 9; e++) x += EC[i][e] * t.E[j][e];
+      d[q++] = c2 * c2 * x;
+    }
+}
+
 // Exp (tools.hpp:56-71), row-major output
 __device__ __forceinline__ void exp_so3(const double *phi, double *R) {
   const double nrm = sqrt(phi[0] * phi[0] + phi[1] * phi[1] + phi[2] * phi[2]);

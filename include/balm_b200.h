@@ -252,6 +252,26 @@ int balm_batch_cut_voxels(balm_batch *b, int n_problems, const int64_t *pose_ptr
 int balm_batch_sizes(balm_batch *b, int *n_problems, int64_t *n_poses, int64_t *n_voxels, int64_t *n_obs);
 int balm_batch_download_voxels(balm_batch *b, int64_t *voxel_ptr, int64_t *row_ptr, int32_t *pose_idx, double *obs10,
                                double *coe, uint64_t *keys, int32_t *layers);
+/* balm_pose_covariance per problem, all problems in one call: problem p's results are those of balm_pose_covariance on
+ * a BALM_PREC_FP64 context holding only problem p, at its rows of poses12 (P x 12, read only). c_cov81: K x 81 in
+ * registration order (the order of obs10), or NULL for isotropic point noise of standard deviation point_noise.
+ * include_fix as balm_pose_covariance. Outputs, each may be NULL: Rcov_raw and Rcov hold the problems' (6N_p)^2
+ * column-major blocks one after the other (the layout of balm_batch_evaluate's H); status[B].
+ * Rcov_p = H_p^-1 Rcov_raw_p H_p^-1 with H_p evaluated at the poses (fix clusters as include_fix) and factored without
+ * damping or pivoting; it is made exactly symmetric by copying its upper triangle to the lower one. status[p] is BALM_OK,
+ * or BALM_ERR_NOT_PD when H_p is singular under balm_pose_covariance's criterion (a zero / tiny / non-finite LDL^T pivot,
+ * or min |d| <= 1e-11 max |d|): that problem's Rcov block is zero, its Rcov_raw block is still valid. A problem without
+ * voxels has a zero Rcov_raw and BALM_ERR_NOT_PD. Registrations from balm_batch_cut_voxels have no fix clusters, so every
+ * problem's H is singular (free gauge) and reports BALM_ERR_NOT_PD; their Rcov_raw is valid. With Rcov == NULL, H is
+ * neither evaluated nor factored and every status is BALM_OK. The call returns BALM_OK when it ran, whatever the
+ * statuses; BALM_ERR_INVALID without a registration. A problem's results do not depend on the rest of the batch; two
+ * calls are bitwise equal. The host waits once. Device scratch allocated and freed by one call, in doubles:
+ *   sum_p 8 M_p ldp_p (rows; ldp_p = 6 N_p rounded up to 64) + 21 K (per-observation diagonal blocks)
+ *   + 672 sum_p ceil(M_p / 32) (per-chunk diagonal partials) + 4096 sum_p T_p (T_p + 1) / 2 ceil(8 M_p / 768)
+ *   (SYRK partials, T_p = ldp_p / 64) + sum_p (6 N_p)^2 (Rcov_raw), + sum_p (6 N_p)^2 more with Rcov, + 81 K with c_cov81;
+ *   plus 16 bytes per SYRK item, 8 bytes per problem and, with Rcov, 4 bytes per problem. */
+int balm_batch_pose_covariance(balm_batch *b, const double *poses12, const double *c_cov81, double point_noise,
+                               int include_fix, int *status, double *Rcov_raw, double *Rcov);
 
 /* Pose-covariance propagation of the consistency experiment (SURVEY.md section 8f, row N3):
  *   Rcov_raw = sum over observations of  Ls c_cov Ls^T      -- VOX_HESS::left_jacobian_point + BALM2::multi_second

@@ -4,7 +4,8 @@ pose count and, for every window, set_voxels + damping_iter, on the fp64 and on 
 Workloads (HBA's bottom layer splits a trajectory into many short windows): (a) 256 windows x 10 poses x 1 000 planes,
 (b) 32 windows x 32 poses x 5 000 planes, and (c) one bottom layer from raw scans: 160 synthetic scans of 20 000
 points (assoc_ref.synthetic_scans, room 12), windows of 10 scans every 5 scans (31 windows), associated per window and as
-one batch (see run_from_scans). For (a) and (b) every window is generated on the GPU by Context.synth_virtual (its own seed) and
+one batch (see run_from_scans), and (d) the pose covariance of the windows of (a) and (b) with fix clusters (see
+run_covariance). For (a) and (b) every window is generated on the GPU by Context.synth_virtual (its own seed) and
 read back with download_voxels, so the batch and the loop run on the same host arrays. Two option sets: fixed work
 (force_hess, rel_tol < 0, 10 iterations: every LM iteration does the same work) and the defaults. The batch, the fp64 loop
 and the tensor loop alternate --repeats times in one process; every call ends in a device synchronisation, so a host clock
@@ -115,6 +116,89 @@ def run_workload(name, n_windows, n_poses, n_planes, repeats, seed0):
     return out
 
 
+def world_cluster(o10, p12):
+    """An observation's cluster moved to the world frame by its pose (PointCluster::transform)."""
+    R, t = p12[:9].reshape(3, 3).T, p12[9:]
+    P = np.array([[o10[0], o10[1], o10[2]], [o10[1], o10[3], o10[4]], [o10[2], o10[4], o10[5]]])
+    v, n = o10[6:9], o10[9]
+    Rv = R @ v
+    Pw = R @ P @ R.T + np.outer(Rv, t) + np.outer(t, Rv) + n * np.outer(t, t)
+    vw = Rv + n * t
+    return np.array([Pw[0, 0], Pw[0, 1], Pw[0, 2], Pw[1, 1], Pw[1, 2], Pw[2, 2], vw[0], vw[1], vw[2], n])
+
+
+def run_covariance(name, n_windows, n_poses, n_planes, repeats, seed0):
+    """Workload (d): the windows of (a) or (b), each voxel given a fix cluster (its pose-0 observation in the world
+    frame at the true poses, what marginalising that scan leaves behind), optimised by one Batch.damping_iter; then
+    the pose covariance at the optimum, isotropic point noise 0.01, fix clusters included: (i) a Context (fp64) per
+    window, pose_covariance only (set_voxels done beforehand), (ii) the same with set_voxels inside the timed loop,
+    (iii) one Batch.pose_covariance. Medians over the repeats, after one warm-up round."""
+    import balm_b200
+    c = balm_b200.Context(n_poses, 0, balm_b200.PREC_FP64)
+    probs, init = [], []
+    for w in range(n_windows):
+        gt, x0 = c.synth_virtual(n_planes, seed=seed0 + w)
+        row_ptr, pose_idx, obs10, coe = c.download_voxels()
+        fix10 = np.stack([world_cluster(obs10[row_ptr[v]], gt[pose_idx[row_ptr[v]]]) for v in range(len(coe))])
+        probs.append(dict(n_poses=n_poses, row_ptr=row_ptr, pose_idx=pose_idx, obs10=obs10, coe=coe, fix10=fix10))
+        init.append(x0)
+    c.close()
+    batch = balm_b200.Batch(0)
+    batch.set_problems(probs)
+    res = batch.damping_iter(init, hess_includes_fix=True, gauge_mode=2)
+    poses = [r[1] for r in res]
+    ctx = balm_b200.Context(n_poses, 0, balm_b200.PREC_FP64)
+    kw = dict(point_noise=0.01, include_fix=True)
+
+    def clock(f):
+        t0 = time.perf_counter()
+        r = f()
+        return r, 1e3 * (time.perf_counter() - t0)
+
+    def loop(register_inside):
+        out, t = [], 0.0
+        for pr, x in zip(probs, poses):
+            if register_inside:
+                (raw, cov), dt = clock(lambda: (ctx.set_voxels(pr["row_ptr"], pr["pose_idx"], pr["obs10"], pr["coe"],
+                                                               pr["fix10"]), ctx.pose_covariance(x, **kw))[1])
+            else:
+                ctx.set_voxels(pr["row_ptr"], pr["pose_idx"], pr["obs10"], pr["coe"], pr["fix10"])
+                (raw, cov), dt = clock(lambda: ctx.pose_covariance(x, **kw))
+            t += dt
+            out.append((raw, cov))
+        return out, t
+
+    ms = {k: [] for k in ("i_context_cov", "ii_context_register_and_cov", "iii_batch_cov")}
+    for rep in range(repeats + 1):
+        ref, t_i = loop(False)
+        _, t_ii = loop(True)
+        got, t_iii = clock(lambda: batch.pose_covariance(poses, **kw))
+        if rep == 0:
+            continue
+        for k, v in zip(ms, (t_i, t_ii, t_iii)):
+            ms[k].append(v)
+    rel = lambda a, b: float(np.abs(a - b).max() / np.abs(b).max())
+    out = dict(windows=n_windows, poses=n_poses, planes=n_planes, ms=ms,
+               ms_median={k: float(np.median(v)) for k, v in ms.items()},
+               statuses=sorted({g[0] for g in got}),
+               max_rel_diff_raw_batch_vs_context=max(rel(g[1], r[0]) for g, r in zip(got, ref)),
+               max_rel_diff_cov_batch_vs_context=max(rel(g[2], r[1]) for g, r in zip(got, ref)))
+    try:  # one profiled batch call of its own: device time per kernel
+        import torch
+        from torch.profiler import ProfilerActivity, profile
+        torch.cuda.synchronize()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            batch.pose_covariance(poses, **kw)
+            torch.cuda.synchronize()
+        out["profile_ms_per_kernel"] = {e.key: dict(ms=getattr(e, "device_time_total", 0) / 1e3, calls=e.count)
+                                        for e in prof.key_averages() if getattr(e, "device_time_total", 0) > 0}
+    except Exception as e:
+        out["profile_ms_per_kernel"] = f"profiler failed: {e}"
+    batch.close()
+    ctx.close()
+    return out
+
+
 def layer_windows(n, length=10, stride=5):
     out, s = [], 0
     while True:
@@ -219,6 +303,8 @@ def main():
     for w in a.workloads.split(","):
         if w == "c":
             res[w] = run_from_scans(160, 20000, 12.0, a.repeats)
+        elif w == "d":
+            res[w] = {k: run_covariance(k, *shapes[k][:3], a.repeats, shapes[k][3]) for k in ("a", "b")}
         else:
             res[w] = run_workload(w, *shapes[w][:3], a.repeats, shapes[w][3])
     if a.out:

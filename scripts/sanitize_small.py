@@ -2,7 +2,8 @@
 tile-DAG factorisation with several 64-column steps (n = 240: chain + near/far workers), the sliding-window marginalisation, the pose-covariance propagation, a multi-batch sparse evaluation, the device
 association chain balm_cut_voxels -> balm_marginalize -> balm_append_scan (octree keys + layers), and a batch of
 independent problems (balm_batch_*: a dense one with fix clusters, a sparse one of 32 poses, an empty one), and a batch
-association of overlapping windows with one empty window (balm_batch_cut_voxels)."""
+association of overlapping windows with one empty window (balm_batch_cut_voxels), and the batch pose covariance of
+an anchored, a free and an empty problem (balm_batch_pose_covariance)."""
 import os, sys
 import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -55,6 +56,8 @@ x = [s["poses_init"] for s in scs] + [np.tile([1, 0, 0, 0, 1, 0, 0, 0, 1, 0, 0, 
 print("batch r", [r for _, _, r in b.evaluate(x, include_fix=True)], flush=True)
 res = b.damping_iter(x, max_iter=2, min_planes_per_pose=0, hess_includes_fix=True, want_per_iter=True)
 print("batch iters", [len(tr) for _, _, tr, _ in res], flush=True)
+cov = b.pose_covariance([r[1] for r in res], point_noise=0.01, include_fix=True)
+print("batch covariance", [(st, float(np.trace(raw)), float(np.trace(c))) for st, raw, c in cov], flush=True)
 b.close()
 # batch association: overlapping windows (2 and 4 scans sharing scans) and one empty window (a single scan)
 pts, frs, poses = assoc_ref.synthetic_scans(n_poses=6, pts_per_scan=1500, seed=14)
