@@ -10,6 +10,12 @@ def _p(a):
     return a.ctypes.data_as(C.c_void_p) if a is not None else None
 
 
+def _trace_dicts(trace):
+    """balm_trace records -> one dict per LM iteration."""
+    return [dict(r1=t.r1, r2=t.r2, u=t.u, v=t.v, q=t.q, q1=t.q1, accepted=bool(t.accepted),
+                 recomputed_hess=bool(t.recomputed_hess), not_pd=bool(t.not_pd)) for t in trace]
+
+
 class Context:
     """One GPU, one registered set of plane voxels, N poses."""
 
@@ -114,9 +120,7 @@ class Context:
         n_it = C.c_int()
         per_iter = np.zeros((max_iter, self.N, 12)) if want_per_iter else None
         L.check(L.lib().balm_damping_iter(self._h, _p(poses), C.byref(opts), trace, C.byref(n_it), _p(per_iter)))
-        tr = [dict(r1=t.r1, r2=t.r2, u=t.u, v=t.v, q=t.q, q1=t.q1, accepted=bool(t.accepted),
-                   recomputed_hess=bool(t.recomputed_hess), not_pd=bool(t.not_pd)) for t in trace[:n_it.value]]
-        return poses, tr, (per_iter[:n_it.value] if want_per_iter else None)
+        return poses, _trace_dicts(trace[:n_it.value]), (per_iter[:n_it.value] if want_per_iter else None)
 
     def marginalize(self, mg_size, poses12, min_ps=15):
         """OCTO_TREE_ROOT::marginalize on the registered voxel set (bavoxel.hpp:948-963, 778-816) -> (n_voxels, n_obs)."""
@@ -352,9 +356,7 @@ class Batch:
         out = []
         for b in range(B):
             p0, p1 = int(self._pose_ptr[b]), int(self._pose_ptr[b + 1])
-            tr = [dict(r1=t.r1, r2=t.r2, u=t.u, v=t.v, q=t.q, q1=t.q1, accepted=bool(t.accepted),
-                       recomputed_hess=bool(t.recomputed_hess), not_pd=bool(t.not_pd))
-                  for t in trace[b * max_iter:b * max_iter + int(n_it[b])]]
+            tr = _trace_dicts(trace[b * max_iter:b * max_iter + int(n_it[b])])
             out.append((int(status[b]), poses[p0:p1].copy(), tr,
                         per_iter[:int(n_it[b]), p0:p1].copy() if want_per_iter else None))
         return out

@@ -294,26 +294,6 @@ __global__ void emit_kernel(const int *ref, const int *obs_start, int nleaf, Emi
   }
 }
 
-// Every scratch buffer of assoc_cut lives in a pool that frees what is left on ANY exit path (the early returns of
-// ATRY / CUDA_TRY, a rejected registration, a bad frame index ...), so a failed call leaks nothing.
-struct ScratchPool {
-  std::vector<void *> ptrs;
-  ~ScratchPool() { for (void *q : ptrs) cudaFree(q); }
-  template <typename T>
-  int get(T **p, size_t n) {
-    CUDA_TRY(cudaMalloc((void **)p, sizeof(T) * (n ? n : 1)));
-    ptrs.push_back((void *)*p);
-    return BALM_OK;
-  }
-  void drop(void *q) {
-    if (!q) return;
-    for (size_t i = 0; i < ptrs.size(); i++)
-      if (ptrs[i] == q) { ptrs[i] = ptrs.back(); ptrs.pop_back(); break; }
-    cudaFree(q);
-  }
-};
-#define ATRY(x) do { int _s = (x); if (_s != BALM_OK) return _s; } while (0)
-
 }  // namespace
 
 int assoc_cut(cudaStream_t st, const AssocInput &in, const balm_assoc_opts &o, const AssocRegister &reg,
@@ -326,9 +306,9 @@ int assoc_cut(cudaStream_t st, const AssocInput &in, const balm_assoc_opts &o, c
   float *xyz = nullptr;
   double *poses = nullptr;
   int *src = nullptr, *row = nullptr, *row_slot = nullptr, *row_prob = nullptr, *bad = nullptr;
-  ATRY(pool.get(&xyz, (size_t)3 * in.n_points)); ATRY(pool.get(&poses, (size_t)12 * n_rows));
-  ATRY(pool.get(&src, (size_t)n)); ATRY(pool.get(&row, (size_t)n)); ATRY(pool.get(&bad, 1));
-  ATRY(pool.get(&row_slot, (size_t)2 * n_rows));
+  TRY(pool.get(&xyz, (size_t)3 * in.n_points)); TRY(pool.get(&poses, (size_t)12 * n_rows));
+  TRY(pool.get(&src, (size_t)n)); TRY(pool.get(&row, (size_t)n)); TRY(pool.get(&bad, 1));
+  TRY(pool.get(&row_slot, (size_t)2 * n_rows));
   row_prob = row_slot + n_rows;
   std::vector<int> hrow((size_t)2 * n_rows, 0);  // per pose row: slot in its problem, problem
   for (int p = 0; p < B; p++)
@@ -349,16 +329,16 @@ int assoc_cut(cudaStream_t st, const AssocInput &in, const balm_assoc_opts &o, c
   int pbits = 1;
   while ((1 << pbits) < B) pbits++;
   if (n > 0) {
-    ATRY(pool.get(&flag, (size_t)n)); ATRY(pool.get(&scan, (size_t)n)); ATRY(pool.get(&seg_start, (size_t)n));
-    ATRY(pool.get(&idx, (size_t)n)); ATRY(pool.get(&work, (size_t)n)); ATRY(pool.get(&work2, (size_t)n));
-    ATRY(pool.get(&pk, (size_t)n)); ATRY(pool.get(&pk2, (size_t)n));
-    ATRY(pool.get(&key, (size_t)n)); ATRY(pool.get(&keyL, (size_t)n)); ATRY(pool.get(&keyL2, (size_t)n));
+    TRY(pool.get(&flag, (size_t)n)); TRY(pool.get(&scan, (size_t)n)); TRY(pool.get(&seg_start, (size_t)n));
+    TRY(pool.get(&idx, (size_t)n)); TRY(pool.get(&work, (size_t)n)); TRY(pool.get(&work2, (size_t)n));
+    TRY(pool.get(&pk, (size_t)n)); TRY(pool.get(&pk2, (size_t)n));
+    TRY(pool.get(&key, (size_t)n)); TRY(pool.get(&keyL, (size_t)n)); TRY(pool.get(&keyL2, (size_t)n));
     size_t tb1 = 0, tb2 = 0, tb3 = 0;
     cub::DeviceRadixSort::SortPairs(nullptr, tb1, pk, pk2, idx, work, (int)n, 0, 32, st);
     cub::DeviceRadixSort::SortPairs(nullptr, tb2, keyL, keyL2, idx, work, (int)n, 0, 63, st);
     cub::DeviceScan::ExclusiveSum(nullptr, tb3, flag, scan, (int)n, st);
     tmp_bytes = std::max(tb1, std::max(tb2, tb3));
-    ATRY(pool.get(&tmp, tmp_bytes));
+    TRY(pool.get(&tmp, tmp_bytes));
     if (one) {
       // items = the points in a stable order by frame, so that every later stable sort keeps the frames ascending
       // inside a node
@@ -377,7 +357,7 @@ int assoc_cut(cudaStream_t st, const AssocInput &in, const balm_assoc_opts &o, c
         tab[(size_t)n_rows + 1 + j] = in.scan_ptr[s];
       }
       long long *dtab = nullptr;
-      ATRY(pool.get(&dtab, tab.size()));
+      TRY(pool.get(&dtab, tab.size()));
       CUDA_TRY(cudaMemcpyAsync(dtab, tab.data(), sizeof(long long) * tab.size(), cudaMemcpyHostToDevice, st));
       expand_rows_kernel<<<n_rows, 256, 0, st>>>(dtab, dtab + n_rows + 1, src, row);
       *launches += 1;
@@ -411,24 +391,24 @@ int assoc_cut(cudaStream_t st, const AssocInput &in, const balm_assoc_opts &o, c
     double *segW = nullptr;
     unsigned long long *seg_key = nullptr;
     int *nflag = nullptr, *nscan = nullptr;
-    ATRY(pool.get(&t.segB, (size_t)10 * nseg)); ATRY(pool.get(&segW, (size_t)10 * nseg)); ATRY(pool.get(&t.seg_row, (size_t)nseg));
-    ATRY(pool.get(&seg_key, (size_t)nseg)); ATRY(pool.get(&nflag, (size_t)nseg)); ATRY(pool.get(&nscan, (size_t)nseg));
+    TRY(pool.get(&t.segB, (size_t)10 * nseg)); TRY(pool.get(&segW, (size_t)10 * nseg)); TRY(pool.get(&t.seg_row, (size_t)nseg));
+    TRY(pool.get(&seg_key, (size_t)nseg)); TRY(pool.get(&nflag, (size_t)nseg)); TRY(pool.get(&nscan, (size_t)nseg));
     const unsigned gs = (unsigned)((nseg + 127) / 128);
     seg_reduce_kernel<<<gs, 128, 0, st>>>(xyz, src, row, poses, work, key, L, seg_start, nseg, n, t.segB, segW, t.seg_row,
                                           seg_key);
     node_flag_kernel<<<gs, 128, 0, st>>>(seg_key, t.seg_row, row_prob, nseg, nflag);
     size_t tb = 0;
     cub::DeviceScan::ExclusiveSum(nullptr, tb, nflag, nscan, nseg, st);
-    if (tb > tmp_bytes) { pool.drop(tmp); tmp = nullptr; tmp_bytes = tb; ATRY(pool.get(&tmp, tmp_bytes)); }
+    if (tb > tmp_bytes) { pool.drop(tmp); tmp = nullptr; tmp_bytes = tb; TRY(pool.get(&tmp, tmp_bytes)); }
     CUDA_TRY(cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, nflag, nscan, nseg, st));
     CUDA_TRY(cudaMemcpyAsync(&last_flag, nflag + nseg - 1, sizeof(int), cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaMemcpyAsync(&last_scan, nscan + nseg - 1, sizeof(int), cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
     t.nnode = last_scan + last_flag;
-    ATRY(pool.get(&t.node_start, (size_t)t.nnode)); ATRY(pool.get(&t.node_key, (size_t)t.nnode));
-    ATRY(pool.get(&t.node_prob, (size_t)t.nnode)); ATRY(pool.get(&t.node_size, (size_t)t.nnode));
-    ATRY(pool.get(&t.node_planar, (size_t)t.nnode)); ATRY(pool.get(&t.node_nframes, (size_t)t.nnode));
-    ATRY(pool.get(&t.node_leaf, (size_t)t.nnode));
+    TRY(pool.get(&t.node_start, (size_t)t.nnode)); TRY(pool.get(&t.node_key, (size_t)t.nnode));
+    TRY(pool.get(&t.node_prob, (size_t)t.nnode)); TRY(pool.get(&t.node_size, (size_t)t.nnode));
+    TRY(pool.get(&t.node_planar, (size_t)t.nnode)); TRY(pool.get(&t.node_nframes, (size_t)t.nnode));
+    TRY(pool.get(&t.node_leaf, (size_t)t.nnode));
     seg_start_kernel<<<gs, 128, 0, st>>>(nflag, nscan, nseg, t.node_start);
     node_judge_kernel<<<(unsigned)((t.nnode + 127) / 128), 128, 0, st>>>(
         segW, seg_key, t.seg_row, row_prob, t.node_start, t.nnode, nseg, P.eig[L], t.node_key, t.node_prob, t.node_size,
@@ -455,10 +435,10 @@ int assoc_cut(cudaStream_t st, const AssocInput &in, const balm_assoc_opts &o, c
     leaf_decide_kernel<<<(unsigned)((t.nnode + 127) / 128), 128, 0, st>>>(
         L, t.nnode, t.node_key, t.node_prob, t.node_size, t.node_planar, t.node_nframes, a0, a1, o.min_ps, o.layer_limit,
         t.node_leaf);
-    ATRY(pool.get(&lscan[L], (size_t)t.nnode));
+    TRY(pool.get(&lscan[L], (size_t)t.nnode));
     size_t tb = 0;
     cub::DeviceScan::ExclusiveSum(nullptr, tb, t.node_leaf, lscan[L], t.nnode, st);
-    if (tb > tmp_bytes) { pool.drop(tmp); tmp = nullptr; tmp_bytes = tb; ATRY(pool.get(&tmp, tmp_bytes)); }
+    if (tb > tmp_bytes) { pool.drop(tmp); tmp = nullptr; tmp_bytes = tb; TRY(pool.get(&tmp, tmp_bytes)); }
     CUDA_TRY(cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, t.node_leaf, lscan[L], t.nnode, st));
     int a = 0, b = 0;
     CUDA_TRY(cudaMemcpyAsync(&a, t.node_leaf + t.nnode - 1, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -473,9 +453,9 @@ int assoc_cut(cudaStream_t st, const AssocInput &in, const balm_assoc_opts &o, c
     unsigned long long *lkey = nullptr, *lkey2 = nullptr;
     int *lref2 = nullptr;
     long long *dptr = nullptr;
-    ATRY(pool.get(&lkey, (size_t)nleaf)); ATRY(pool.get(&lkey2, (size_t)nleaf)); ATRY(pool.get(&lref, (size_t)nleaf));
-    ATRY(pool.get(&lref2, (size_t)nleaf)); ATRY(pool.get(&lcnt, (size_t)nleaf)); ATRY(pool.get(&lobs, (size_t)nleaf));
-    ATRY(pool.get(&dptr, hptr.size()));
+    TRY(pool.get(&lkey, (size_t)nleaf)); TRY(pool.get(&lkey2, (size_t)nleaf)); TRY(pool.get(&lref, (size_t)nleaf));
+    TRY(pool.get(&lref2, (size_t)nleaf)); TRY(pool.get(&lcnt, (size_t)nleaf)); TRY(pool.get(&lobs, (size_t)nleaf));
+    TRY(pool.get(&dptr, hptr.size()));
     int base = 0;
     for (int L = 0; L <= o.layer_limit; L++) {
       leaf_collect_kernel<<<(unsigned)((T[L].nnode + 127) / 128), 128, 0, st>>>(L, T[L].nnode, T[L].node_leaf, lscan[L],
@@ -489,7 +469,7 @@ int assoc_cut(cudaStream_t st, const AssocInput &in, const balm_assoc_opts &o, c
     cub::DeviceRadixSort::SortPairs(nullptr, tb2, lprob, lprob2, lref, lref2, nleaf, 0, pbits, st);
     cub::DeviceScan::ExclusiveSum(nullptr, tb3, lcnt, lobs, nleaf, st);
     tb = std::max(tb, std::max(tb2, tb3));
-    if (tb > tmp_bytes) { pool.drop(tmp); tmp = nullptr; tmp_bytes = tb; ATRY(pool.get(&tmp, tmp_bytes)); }
+    if (tb > tmp_bytes) { pool.drop(tmp); tmp = nullptr; tmp_bytes = tb; TRY(pool.get(&tmp, tmp_bytes)); }
     CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, lkey, lkey2, lref, lref2, nleaf, 0, 63, st));
     std::swap(lref, lref2);
     leaf_gather_kernel<unsigned><<<gl, 128, 0, st>>>(lref, nleaf, T[0].node_prob, T[1].node_prob, T[2].node_prob, lprob);
@@ -508,7 +488,7 @@ int assoc_cut(cudaStream_t st, const AssocInput &in, const balm_assoc_opts &o, c
   const int64_t K = hptr[2 * (size_t)B + 1];
   // ---- register: the caller allocates its arrays for M voxels and K observations; emit straight into them ----
   AssocEmit out{};
-  ATRY(reg(nleaf, K, reinterpret_cast<const int64_t *>(hptr.data()), reinterpret_cast<const int64_t *>(hptr.data() + B + 1),
+  TRY(reg(nleaf, K, reinterpret_cast<const int64_t *>(hptr.data()), reinterpret_cast<const int64_t *>(hptr.data() + B + 1),
            &out));
   if (nleaf > 0) {
     EmitLevel e[3];
@@ -572,7 +552,7 @@ int build_pose_major_lists(balm_ctx *c, const int *planes_host) {
   CUDA_TRY(cudaMalloc((void **)&c->csc_hi, sizeof(int) * (size_t)N));
   CUDA_TRY(cudaMemcpyAsync(c->csc_ptr, ptr.data(), sizeof(int) * ((size_t)N + 1), cudaMemcpyHostToDevice, st));
   int *vox = nullptr, *idx = nullptr, *keys = nullptr, *keys2 = nullptr;
-  ATRY(pool.get(&vox, (size_t)K)); ATRY(pool.get(&idx, (size_t)K)); ATRY(pool.get(&keys, (size_t)K)); ATRY(pool.get(&keys2, (size_t)K));
+  TRY(pool.get(&vox, (size_t)K)); TRY(pool.get(&idx, (size_t)K)); TRY(pool.get(&keys, (size_t)K)); TRY(pool.get(&keys2, (size_t)K));
   obs_voxel_kernel<<<(unsigned)((M + 127) / 128), 128, 0, st>>>(c->row_ptr, M, vox);
   iota_kernel<<<(unsigned)((K + 255) / 256), 256, 0, st>>>(idx, K);
   CUDA_TRY(cudaMemcpyAsync(keys, c->pose_idx, sizeof(int) * (size_t)K, cudaMemcpyDeviceToDevice, st));
@@ -581,7 +561,7 @@ int build_pose_major_lists(balm_ctx *c, const int *planes_host) {
   size_t tb = 0;
   cub::DeviceRadixSort::SortPairs(nullptr, tb, keys, keys2, idx, c->csc_obs, (int)K, 0, bits, st);
   char *tmp = nullptr;
-  ATRY(pool.get(&tmp, tb));
+  TRY(pool.get(&tmp, tb));
   CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, tb, keys, keys2, idx, c->csc_obs, (int)K, 0, bits, st));
   gather_int_kernel<<<(unsigned)((K + 255) / 256), 256, 0, st>>>(vox, c->csc_obs, c->csc_vox, K);
   CUDA_TRY(cudaStreamSynchronize(st));
@@ -685,13 +665,13 @@ int marginalize_build(balm_ctx *c, int mg, const double *poses_dev, int min_ps, 
   cudaStream_t st = c->stream;
   ScratchPool pool;
   int *keep = nullptr, *cnt = nullptr, *vscan = nullptr, *oscan = nullptr;
-  ATRY(pool.get(&keep, (size_t)M)); ATRY(pool.get(&cnt, (size_t)M)); ATRY(pool.get(&vscan, (size_t)M)); ATRY(pool.get(&oscan, (size_t)M));
+  TRY(pool.get(&keep, (size_t)M)); TRY(pool.get(&cnt, (size_t)M)); TRY(pool.get(&vscan, (size_t)M)); TRY(pool.get(&oscan, (size_t)M));
   const unsigned gb = (unsigned)((M + 127) / 128);
   marg_count_kernel<<<gb, 128, 0, st>>>(c->row_ptr, c->pose_idx, c->obs, c->Kp, M, mg, min_ps, keep, cnt);
   size_t tb = 0;
   cub::DeviceScan::ExclusiveSum(nullptr, tb, keep, vscan, (int)M, st);
   char *tmp = nullptr;
-  ATRY(pool.get(&tmp, tb));
+  TRY(pool.get(&tmp, tb));
   CUDA_TRY(cub::DeviceScan::ExclusiveSum(tmp, tb, keep, vscan, (int)M, st));
   CUDA_TRY(cub::DeviceScan::ExclusiveSum(tmp, tb, cnt, oscan, (int)M, st));
   int last[4] = {0, 0, 0, 0};
@@ -706,12 +686,12 @@ int marginalize_build(balm_ctx *c, int mg, const double *poses_dev, int min_ps, 
   long long *rp = nullptr;
   int *pi = nullptr;
   double *ob = nullptr, *fx = nullptr, *co = nullptr;
-  ATRY(pool.get(&rp, (size_t)Mout + 1)); ATRY(pool.get(&pi, (size_t)Kout)); ATRY(pool.get(&ob, (size_t)Kout * 10));
-  ATRY(pool.get(&fx, (size_t)Mout * 10)); ATRY(pool.get(&co, (size_t)Mout));
+  TRY(pool.get(&rp, (size_t)Mout + 1)); TRY(pool.get(&pi, (size_t)Kout)); TRY(pool.get(&ob, (size_t)Kout * 10));
+  TRY(pool.get(&fx, (size_t)Mout * 10)); TRY(pool.get(&co, (size_t)Mout));
   unsigned long long *keys_out = nullptr;
   int *layers_out = nullptr;
   const bool had_keys = c->has_keys && c->vox_key;
-  if (had_keys) { ATRY(pool.get(&keys_out, (size_t)Mout)); ATRY(pool.get(&layers_out, (size_t)Mout)); }
+  if (had_keys) { TRY(pool.get(&keys_out, (size_t)Mout)); TRY(pool.get(&layers_out, (size_t)Mout)); }
   marg_emit_kernel<<<gb, 128, 0, st>>>(c->row_ptr, c->pose_idx, c->obs, c->Kp, c->fix, M, poses_dev, mg, keep, vscan, oscan, rp,
                                        pi, ob, fx, co, Mout, Kout, had_keys ? c->vox_key : nullptr, keys_out, c->vox_layer,
                                        layers_out);
@@ -720,7 +700,7 @@ int marginalize_build(balm_ctx *c, int mg, const double *poses_dev, int min_ps, 
   c->launches += 4;
   if (Mout < 1) { balm_set_error("balm_marginalize: no voxel is left with two observing scans"); return BALM_ERR_INVALID; }
   // re-register from the device arrays (copies them, transposes the observations, rebuilds the pose-major lists)
-  ATRY(reg(c, Mout, (const int64_t *)rp, pi, ob, fx, co, Kout));
+  TRY(reg(c, Mout, (const int64_t *)rp, pi, ob, fx, co, Kout));
   return install_keys(c, keys_out, layers_out, Mout, had_keys);
 }
 
@@ -859,10 +839,10 @@ int append_scan_build(balm_ctx *c, int64_t n, const float *xyz_h, const double *
   unsigned *vid = nullptr, *vid2 = nullptr;
   int *idx = nullptr, *idx2 = nullptr, *keep = nullptr, *cnt = nullptr, *vscan = nullptr, *oscan = nullptr, *bad = nullptr;
   double *newobs = nullptr;
-  ATRY(pool.get(&xyz, (size_t)3 * n)); ATRY(pool.get(&vid, (size_t)n)); ATRY(pool.get(&vid2, (size_t)n));
-  ATRY(pool.get(&idx, (size_t)n)); ATRY(pool.get(&idx2, (size_t)n)); ATRY(pool.get(&newobs, (size_t)M * 10));
-  ATRY(pool.get(&keep, (size_t)M)); ATRY(pool.get(&cnt, (size_t)M)); ATRY(pool.get(&vscan, (size_t)M)); ATRY(pool.get(&oscan, (size_t)M));
-  ATRY(pool.get(&bad, 1));
+  TRY(pool.get(&xyz, (size_t)3 * n)); TRY(pool.get(&vid, (size_t)n)); TRY(pool.get(&vid2, (size_t)n));
+  TRY(pool.get(&idx, (size_t)n)); TRY(pool.get(&idx2, (size_t)n)); TRY(pool.get(&newobs, (size_t)M * 10));
+  TRY(pool.get(&keep, (size_t)M)); TRY(pool.get(&cnt, (size_t)M)); TRY(pool.get(&vscan, (size_t)M)); TRY(pool.get(&oscan, (size_t)M));
+  TRY(pool.get(&bad, 1));
   CUDA_TRY(cudaMemcpyAsync(xyz, xyz_h, sizeof(float) * 3 * n, cudaMemcpyHostToDevice, st));
   CUDA_TRY(cudaMemsetAsync(bad, 0, sizeof(int), st));
   const unsigned gp = (unsigned)((n + 255) / 256), gv = (unsigned)((M + 127) / 128);
@@ -875,7 +855,7 @@ int append_scan_build(balm_ctx *c, int64_t n, const float *xyz_h, const double *
   cub::DeviceScan::ExclusiveSum(nullptr, tb2, keep, vscan, (int)M, st);
   tb = std::max(tb, tb2);
   char *tmp = nullptr;
-  ATRY(pool.get(&tmp, tb));
+  TRY(pool.get(&tmp, tb));
   CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, tb, vid, vid2, idx, idx2, (int)n, 0, bits, st));  // stable: point order kept
   append_cluster_kernel<<<gv, 128, 0, st>>>(xyz, vid2, idx2, n, (int)M, newobs);
   append_judge_kernel<<<gv, 128, 0, st>>>(c->row_ptr, c->pose_idx, c->obs, c->Kp, c->fix, M, poses_dev, newobs, slot, c->vox_layer, P,
@@ -902,9 +882,9 @@ int append_scan_build(balm_ctx *c, int64_t n, const float *xyz_h, const double *
   double *ob = nullptr, *fx = nullptr, *co = nullptr;
   unsigned long long *keys_out = nullptr;
   int *layers_out = nullptr;
-  ATRY(pool.get(&rp, (size_t)Mout + 1)); ATRY(pool.get(&pi, (size_t)Kout)); ATRY(pool.get(&ob, (size_t)Kout * 10));
-  ATRY(pool.get(&fx, (size_t)Mout * 10)); ATRY(pool.get(&co, (size_t)Mout)); ATRY(pool.get(&keys_out, (size_t)Mout));
-  ATRY(pool.get(&layers_out, (size_t)Mout));
+  TRY(pool.get(&rp, (size_t)Mout + 1)); TRY(pool.get(&pi, (size_t)Kout)); TRY(pool.get(&ob, (size_t)Kout * 10));
+  TRY(pool.get(&fx, (size_t)Mout * 10)); TRY(pool.get(&co, (size_t)Mout)); TRY(pool.get(&keys_out, (size_t)Mout));
+  TRY(pool.get(&layers_out, (size_t)Mout));
   append_emit_kernel<<<gv, 128, 0, st>>>(c->row_ptr, c->pose_idx, c->obs, c->Kp, c->fix, c->coe, M, newobs, slot, keep, vscan, oscan,
                                          c->vox_key, c->vox_layer, rp, pi, ob, fx, co, keys_out, layers_out, Mout, Kout);
   CUDA_TRY(cudaStreamSynchronize(st));
@@ -913,7 +893,7 @@ int append_scan_build(balm_ctx *c, int64_t n, const float *xyz_h, const double *
   *M_out = Mout;
   *K_out = Kout;
   const bool any_fix = c->fix != nullptr;
-  ATRY(reg(c, Mout, (const int64_t *)rp, pi, ob, any_fix ? fx : nullptr, co, Kout));
+  TRY(reg(c, Mout, (const int64_t *)rp, pi, ob, any_fix ? fx : nullptr, co, Kout));
   return install_keys(c, keys_out, layers_out, Mout, true);
 }
 
@@ -986,9 +966,9 @@ int win_reserve_nodes(WindowState &w, int need) {
   if (need <= w.ncap) return BALM_OK;
   int cap = std::max(need, std::max(1024, 2 * w.ncap));
   const size_t nn = (size_t)w.nn, c = (size_t)cap, NS = (size_t)w.N * 10;
-  ATRY(grow_array(&w.nkey, nn, c)); ATRY(grow_array(&w.nlayer, nn, c)); ATRY(grow_array(&w.nsplit, nn, c));
-  ATRY(grow_array(&w.npush, nn, c)); ATRY(grow_array(&w.naction, nn, c)); ATRY(grow_array(&w.nfix, nn * 10, c * 10));
-  ATRY(grow_array(&w.sig_o, nn * NS, c * NS)); ATRY(grow_array(&w.sig_t, nn * NS, c * NS));
+  TRY(grow_array(&w.nkey, nn, c)); TRY(grow_array(&w.nlayer, nn, c)); TRY(grow_array(&w.nsplit, nn, c));
+  TRY(grow_array(&w.npush, nn, c)); TRY(grow_array(&w.naction, nn, c)); TRY(grow_array(&w.nfix, nn * 10, c * 10));
+  TRY(grow_array(&w.sig_o, nn * NS, c * NS)); TRY(grow_array(&w.sig_t, nn * NS, c * NS));
   w.ncap = cap;
   return BALM_OK;
 }
@@ -998,8 +978,8 @@ int win_reserve_points(WindowState &w, int64_t need) {
   int64_t cap = std::max<int64_t>(need, std::max<int64_t>(1 << 16, 2 * w.pcap));
   cap = std::min<int64_t>(cap, (1ll << 31) - 1);
   const size_t n = (size_t)w.np, c = (size_t)cap;
-  ATRY(grow_array(&w.pxyz, 3 * n, 3 * c)); ATRY(grow_array(&w.ptran, 3 * n, 3 * c)); ATRY(grow_array(&w.pslot, n, c));
-  ATRY(grow_array(&w.pnode, n, c)); ATRY(grow_array(&w.pstamp, n, c));
+  TRY(grow_array(&w.pxyz, 3 * n, 3 * c)); TRY(grow_array(&w.ptran, 3 * n, 3 * c)); TRY(grow_array(&w.pslot, n, c));
+  TRY(grow_array(&w.pnode, n, c)); TRY(grow_array(&w.pstamp, n, c));
   w.pcap = cap;
   return BALM_OK;
 }
@@ -1052,13 +1032,13 @@ int win_add_nodes(WindowState &w, ScratchPool &pool, CubTmp &tmp, cudaStream_t s
   WinLookup &lk = w.look[L];
   int *miss = nullptr, *nsel = nullptr;
   unsigned long long *sel = nullptr, *sorted = nullptr, *uniq = nullptr;
-  ATRY(pool.get(&miss, m)); ATRY(pool.get(&nsel, 1)); ATRY(pool.get(&sel, m)); ATRY(pool.get(&sorted, m)); ATRY(pool.get(&uniq, m));
+  TRY(pool.get(&miss, m)); TRY(pool.get(&nsel, 1)); TRY(pool.get(&sel, m)); TRY(pool.get(&sorted, m)); TRY(pool.get(&uniq, m));
   win_missing_kernel<<<(m + 255) / 256, 256, 0, st>>>(keys, m, lk.key, lk.n, miss);
   size_t b1 = 0, b2 = 0, b3 = 0;
   cub::DeviceSelect::Flagged(nullptr, b1, keys, miss, sel, nsel, m, st);
   cub::DeviceRadixSort::SortKeys(nullptr, b2, sel, sorted, m, 0, 64, st);
   cub::DeviceSelect::Unique(nullptr, b3, sorted, uniq, nsel, m, st);
-  ATRY(tmp.need(std::max(b1, std::max(b2, b3))));
+  TRY(tmp.need(std::max(b1, std::max(b2, b3))));
   CUDA_TRY(cub::DeviceSelect::Flagged(tmp.p, tmp.bytes, keys, miss, sel, nsel, m, st));
   int nmiss = 0;
   CUDA_TRY(cudaMemcpyAsync(&nmiss, nsel, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -1073,7 +1053,7 @@ int win_add_nodes(WindowState &w, ScratchPool &pool, CubTmp &tmp, cudaStream_t s
     balm_set_error("balm_window: node table too large");
     return BALM_ERR_UNSUPPORTED;
   }
-  ATRY(win_reserve_nodes(w, w.nn + nnew));
+  TRY(win_reserve_nodes(w, w.nn + nnew));
   const int base = w.nn;
   win_init_nodes_kernel<<<(nnew + 255) / 256, 256, 0, st>>>(uniq, nnew, base, L, w.nkey, w.nlayer, w.nsplit, w.npush, w.nfix);
   CUDA_TRY(cudaMemsetAsync(w.sig_o + (size_t)base * w.N * 10, 0, sizeof(double) * (size_t)nnew * w.N * 10, st));
@@ -1082,7 +1062,7 @@ int win_add_nodes(WindowState &w, ScratchPool &pool, CubTmp &tmp, cudaStream_t s
   const int nl = lk.n + nnew;
   unsigned long long *k_in = nullptr, *k_out = nullptr;
   int *i_in = nullptr, *i_out = nullptr;
-  ATRY(pool.get(&k_in, nl)); ATRY(pool.get(&i_in, nl));
+  TRY(pool.get(&k_in, nl)); TRY(pool.get(&i_in, nl));
   CUDA_TRY(cudaMalloc((void **)&k_out, sizeof(unsigned long long) * nl));
   if (cudaMalloc((void **)&i_out, sizeof(int) * nl) != cudaSuccess) { cudaFree(k_out); CUDA_TRY(cudaErrorMemoryAllocation); }
   if (lk.n) {
@@ -1093,7 +1073,7 @@ int win_add_nodes(WindowState &w, ScratchPool &pool, CubTmp &tmp, cudaStream_t s
   win_iota_kernel<<<(nnew + 255) / 256, 256, 0, st>>>(i_in + lk.n, nnew, base);
   size_t b4 = 0;
   cub::DeviceRadixSort::SortPairs(nullptr, b4, k_in, k_out, i_in, i_out, nl, 0, 64, st);
-  ATRY(tmp.need(b4));
+  TRY(tmp.need(b4));
   CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp.p, tmp.bytes, k_in, k_out, i_in, i_out, nl, 0, 64, st));
   CUDA_TRY(cudaStreamSynchronize(st));
   cudaFree(lk.key);
@@ -1144,8 +1124,8 @@ int win_push_points(WindowState &w, ScratchPool &pool, CubTmp &tmp, cudaStream_t
   if (m < 1) return BALM_OK;
   unsigned long long *ck = nullptr, *ck2 = nullptr;
   int *ord2 = nullptr, *flag = nullptr, *iota = nullptr, *seg = nullptr, *nsel = nullptr;
-  ATRY(pool.get(&ck, m)); ATRY(pool.get(&ck2, m)); ATRY(pool.get(&ord2, m)); ATRY(pool.get(&flag, m));
-  ATRY(pool.get(&iota, m)); ATRY(pool.get(&seg, m)); ATRY(pool.get(&nsel, 1));
+  TRY(pool.get(&ck, m)); TRY(pool.get(&ck2, m)); TRY(pool.get(&ord2, m)); TRY(pool.get(&flag, m));
+  TRY(pool.get(&iota, m)); TRY(pool.get(&seg, m)); TRY(pool.get(&nsel, 1));
   const unsigned g = (unsigned)((m + 255) / 256);
   win_seg_key_kernel<<<g, 256, 0, st>>>(order, m, w.pnode, w.pslot, w.N, ck);
   int bits = 1;
@@ -1153,7 +1133,7 @@ int win_push_points(WindowState &w, ScratchPool &pool, CubTmp &tmp, cudaStream_t
   size_t b1 = 0, b2 = 0;
   cub::DeviceRadixSort::SortPairs(nullptr, b1, ck, ck2, order, ord2, m, 0, bits, st);
   cub::DeviceSelect::Flagged(nullptr, b2, iota, flag, seg, nsel, m, st);
-  ATRY(tmp.need(std::max(b1, b2)));
+  TRY(tmp.need(std::max(b1, b2)));
   CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp.p, tmp.bytes, ck, ck2, order, ord2, m, 0, bits, st));  // stable
   win_seg_flag_kernel<<<g, 256, 0, st>>>(ck2, m, flag);
   win_iota_kernel<<<g, 256, 0, st>>>(iota, m, 0);
@@ -1371,8 +1351,8 @@ int window_cut_build(balm_ctx *c, WindowState &w, int64_t n, const float *xyz_h,
   double *pose = nullptr, *tran = nullptr;
   unsigned long long *rkey = nullptr;
   int *bad = nullptr, *order = nullptr;
-  ATRY(pool.get(&xyz, 3 * (size_t)m)); ATRY(pool.get(&pose, 12)); ATRY(pool.get(&tran, 3 * (size_t)m));
-  ATRY(pool.get(&rkey, m)); ATRY(pool.get(&bad, 1)); ATRY(pool.get(&order, m));
+  TRY(pool.get(&xyz, 3 * (size_t)m)); TRY(pool.get(&pose, 12)); TRY(pool.get(&tran, 3 * (size_t)m));
+  TRY(pool.get(&rkey, m)); TRY(pool.get(&bad, 1)); TRY(pool.get(&order, m));
   CUDA_TRY(cudaMemcpyAsync(xyz, xyz_h, sizeof(float) * 3 * m, cudaMemcpyHostToDevice, st));
   CUDA_TRY(cudaMemcpyAsync(pose, pose12_h, sizeof(double) * 12, cudaMemcpyHostToDevice, st));
   CUDA_TRY(cudaMemsetAsync(bad, 0, sizeof(int), st));
@@ -1383,8 +1363,8 @@ int window_cut_build(balm_ctx *c, WindowState &w, int64_t n, const float *xyz_h,
   CUDA_TRY(cudaStreamSynchronize(st));
   if (h_bad) { balm_set_error("balm_window_cut: a point lies outside the +-2^18 root-voxel range"); return BALM_ERR_INVALID; }
   // nothing was changed so far; from here on the scan is committed
-  ATRY(win_add_nodes(w, pool, tmp, st, rkey, m, 0));
-  ATRY(win_reserve_points(w, w.np + m));
+  TRY(win_add_nodes(w, pool, tmp, st, rkey, m, 0));
+  TRY(win_reserve_points(w, w.np + m));
   const int64_t b = w.np;
   CUDA_TRY(cudaMemcpyAsync(w.pxyz + 3 * b, xyz, sizeof(float) * 3 * m, cudaMemcpyDeviceToDevice, st));
   CUDA_TRY(cudaMemcpyAsync(w.ptran + 3 * b, tran, sizeof(double) * 3 * m, cudaMemcpyDeviceToDevice, st));
@@ -1392,7 +1372,7 @@ int window_cut_build(balm_ctx *c, WindowState &w, int64_t n, const float *xyz_h,
   win_find_kernel<<<g, 256, 0, st>>>(rkey, nullptr, m, w.look[0].key, w.look[0].id, w.look[0].n, w.pnode + b);
   win_iota_kernel<<<g, 256, 0, st>>>(order, m, (int)b);
   w.np += m;
-  ATRY(win_push_points(w, pool, tmp, st, order, m));
+  TRY(win_push_points(w, pool, tmp, st, order, m));
   CUDA_TRY(cudaStreamSynchronize(st));
   c->launches += 10;
   return BALM_OK;
@@ -1412,33 +1392,33 @@ int window_recut_build(balm_ctx *c, WindowState &w, int win_count) {
     const int np = (int)w.np;
     unsigned long long *ckey = nullptr, *mkey = nullptr, *stamp = nullptr, *stamp2 = nullptr;
     int *flag = nullptr, *iota = nullptr, *mv = nullptr, *mv2 = nullptr, *nsel = nullptr;
-    ATRY(pool.get(&ckey, np)); ATRY(pool.get(&flag, np)); ATRY(pool.get(&iota, np)); ATRY(pool.get(&mv, np));
-    ATRY(pool.get(&nsel, 1));
+    TRY(pool.get(&ckey, np)); TRY(pool.get(&flag, np)); TRY(pool.get(&iota, np)); TRY(pool.get(&mv, np));
+    TRY(pool.get(&nsel, 1));
     const unsigned g = (unsigned)((np + 255) / 256);
     win_move_kernel<<<g, 256, 0, st>>>(w.np, win_count, w.P, w.pnode, w.pslot, w.ptran, w.naction, w.nkey, w.nlayer, ckey, flag);
     win_iota_kernel<<<g, 256, 0, st>>>(iota, np, 0);
     size_t b1 = 0;
     cub::DeviceSelect::Flagged(nullptr, b1, iota, flag, mv, nsel, np, st);
-    ATRY(tmp.need(b1));
+    TRY(tmp.need(b1));
     CUDA_TRY(cub::DeviceSelect::Flagged(tmp.p, tmp.bytes, iota, flag, mv, nsel, np, st));
     int m = 0;
     CUDA_TRY(cudaMemcpyAsync(&m, nsel, sizeof(int), cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
     c->launches += 3;
     if (m == 0) continue;
-    ATRY(pool.get(&mkey, m)); ATRY(pool.get(&stamp, m)); ATRY(pool.get(&stamp2, m)); ATRY(pool.get(&mv2, m));
+    TRY(pool.get(&mkey, m)); TRY(pool.get(&stamp, m)); TRY(pool.get(&stamp2, m)); TRY(pool.get(&mv2, m));
     const unsigned gm = (unsigned)((m + 255) / 256);
     win_gather_u64_kernel<<<gm, 256, 0, st>>>(ckey, mv, m, mkey);
-    ATRY(win_add_nodes(w, pool, tmp, st, mkey, m, L + 1));              // children created on first use (:714-720)
+    TRY(win_add_nodes(w, pool, tmp, st, mkey, m, L + 1));              // children created on first use (:714-720)
     win_find_kernel<<<gm, 256, 0, st>>>(mkey, mv, m, w.look[L + 1].key, w.look[L + 1].id, w.look[L + 1].n, w.pnode);
     // the moved points in the order the parents' lists hold them, appended after the children's earlier points
     win_gather_u64_kernel<<<gm, 256, 0, st>>>(w.pstamp, mv, m, stamp);
     size_t b2 = 0;
     cub::DeviceRadixSort::SortPairs(nullptr, b2, stamp, stamp2, mv, mv2, m, 0, 64, st);
-    ATRY(tmp.need(b2));
+    TRY(tmp.need(b2));
     CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp.p, tmp.bytes, stamp, stamp2, mv, mv2, m, 0, 64, st));
     win_restamp_kernel<<<gm, 256, 0, st>>>(mv2, m, w.op++, w.pstamp);
-    ATRY(win_push_points(w, pool, tmp, st, mv2, m));
+    TRY(win_push_points(w, pool, tmp, st, mv2, m));
     CUDA_TRY(cudaStreamSynchronize(st));
     c->launches += 9;
   }
@@ -1453,7 +1433,7 @@ int window_marginalize_build(balm_ctx *c, WindowState &w, int mg, const double *
   CubTmp tmp{pool};
   double *poses = nullptr;
   if (poses_h) {
-    ATRY(pool.get(&poses, 12 * (size_t)w.N));
+    TRY(pool.get(&poses, 12 * (size_t)w.N));
     CUDA_TRY(cudaMemcpyAsync(poses, poses_h, sizeof(double) * 12 * w.N, cudaMemcpyHostToDevice, st));
   }
   if (w.nn == 0) return BALM_OK;
@@ -1461,13 +1441,13 @@ int window_marginalize_build(balm_ctx *c, WindowState &w, int mg, const double *
   if (w.np > 0) {
     const int np = (int)w.np;
     int *keep = nullptr, *iota = nullptr, *sel = nullptr, *nsel = nullptr;
-    ATRY(pool.get(&keep, np)); ATRY(pool.get(&iota, np)); ATRY(pool.get(&sel, np)); ATRY(pool.get(&nsel, 1));
+    TRY(pool.get(&keep, np)); TRY(pool.get(&iota, np)); TRY(pool.get(&sel, np)); TRY(pool.get(&nsel, 1));
     const unsigned g = (unsigned)((np + 255) / 256);
     win_margi_point_kernel<<<g, 256, 0, st>>>(w.np, mg, win_count, poses, w.nsplit, w.pnode, w.pslot, w.pxyz, w.ptran, keep);
     win_iota_kernel<<<g, 256, 0, st>>>(iota, np, 0);
     size_t b1 = 0;
     cub::DeviceSelect::Flagged(nullptr, b1, iota, keep, sel, nsel, np, st);
-    ATRY(tmp.need(b1));
+    TRY(tmp.need(b1));
     CUDA_TRY(cub::DeviceSelect::Flagged(tmp.p, tmp.bytes, iota, keep, sel, nsel, np, st));
     int m = 0;
     CUDA_TRY(cudaMemcpyAsync(&m, nsel, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -1512,13 +1492,13 @@ int window_push_build(balm_ctx *c, WindowState &w, int win_count, int64_t *M_out
   CubTmp tmp{pool};
   const int nn = w.nn;
   int *flag = nullptr, *iota = nullptr, *sel = nullptr, *nsel = nullptr;
-  ATRY(pool.get(&flag, nn)); ATRY(pool.get(&iota, nn)); ATRY(pool.get(&sel, nn)); ATRY(pool.get(&nsel, 1));
+  TRY(pool.get(&flag, nn)); TRY(pool.get(&iota, nn)); TRY(pool.get(&sel, nn)); TRY(pool.get(&nsel, 1));
   const unsigned g = (unsigned)((nn + 127) / 128);
   win_push_flag_kernel<<<g, 128, 0, st>>>(nn, w.N, win_count, w.P.min_ps, w.nsplit, w.npush, w.sig_o, flag);
   win_iota_kernel<<<g, 128, 0, st>>>(iota, nn, 0);
   size_t b1 = 0;
   cub::DeviceSelect::Flagged(nullptr, b1, iota, flag, sel, nsel, nn, st);
-  ATRY(tmp.need(b1));
+  TRY(tmp.need(b1));
   CUDA_TRY(cub::DeviceSelect::Flagged(tmp.p, tmp.bytes, iota, flag, sel, nsel, nn, st));
   int M = 0;
   CUDA_TRY(cudaMemcpyAsync(&M, nsel, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -1528,13 +1508,13 @@ int window_push_build(balm_ctx *c, WindowState &w, int win_count, int64_t *M_out
   // ascending node key (unique among pushed nodes: a pushed node is not split, so none of its ancestors is pushed)
   unsigned long long *k = nullptr, *k2 = nullptr;
   int *ids = nullptr, *cnt = nullptr, *ostart = nullptr;
-  ATRY(pool.get(&k, M)); ATRY(pool.get(&k2, M)); ATRY(pool.get(&ids, M)); ATRY(pool.get(&cnt, M)); ATRY(pool.get(&ostart, M));
+  TRY(pool.get(&k, M)); TRY(pool.get(&k2, M)); TRY(pool.get(&ids, M)); TRY(pool.get(&cnt, M)); TRY(pool.get(&ostart, M));
   const unsigned gm = (unsigned)((M + 127) / 128);
   win_gather_u64_kernel<<<gm, 128, 0, st>>>(w.nkey, sel, M, k);
   size_t b2 = 0, b3 = 0;
   cub::DeviceRadixSort::SortPairs(nullptr, b2, k, k2, sel, ids, M, 0, 64, st);
   cub::DeviceScan::ExclusiveSum(nullptr, b3, cnt, ostart, M, st);
-  ATRY(tmp.need(std::max(b2, b3)));
+  TRY(tmp.need(std::max(b2, b3)));
   CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp.p, tmp.bytes, k, k2, sel, ids, M, 0, 64, st));
   win_obs_count_kernel<<<gm, 128, 0, st>>>(ids, M, w.N, w.sig_o, cnt);
   CUDA_TRY(cub::DeviceScan::ExclusiveSum(tmp.p, tmp.bytes, cnt, ostart, M, st));
@@ -1547,9 +1527,9 @@ int window_push_build(balm_ctx *c, WindowState &w, int win_count, int64_t *M_out
   int *pi = nullptr, *lay = nullptr;
   double *ob = nullptr, *fx = nullptr, *co = nullptr;
   unsigned long long *keys_out = nullptr;
-  ATRY(pool.get(&rp, (size_t)M + 1)); ATRY(pool.get(&pi, (size_t)K)); ATRY(pool.get(&ob, (size_t)K * 10));
-  ATRY(pool.get(&fx, (size_t)M * 10)); ATRY(pool.get(&co, (size_t)M)); ATRY(pool.get(&keys_out, (size_t)M));
-  ATRY(pool.get(&lay, (size_t)M));
+  TRY(pool.get(&rp, (size_t)M + 1)); TRY(pool.get(&pi, (size_t)K)); TRY(pool.get(&ob, (size_t)K * 10));
+  TRY(pool.get(&fx, (size_t)M * 10)); TRY(pool.get(&co, (size_t)M)); TRY(pool.get(&keys_out, (size_t)M));
+  TRY(pool.get(&lay, (size_t)M));
   win_emit_kernel<<<gm, 128, 0, st>>>(ids, ostart, M, K, w.N, w.sig_o, w.nfix, w.nkey, w.nlayer, rp, pi, ob, fx, co, keys_out,
                                       lay);
   CUDA_TRY(cudaStreamSynchronize(st));
@@ -1557,6 +1537,6 @@ int window_push_build(balm_ctx *c, WindowState &w, int win_count, int64_t *M_out
   c->launches += 6;
   *M_out = M;
   *K_out = K;
-  ATRY(reg(c, M, (const int64_t *)rp, pi, ob, fx, co, K));
+  TRY(reg(c, M, (const int64_t *)rp, pi, ob, fx, co, K));
   return install_keys(c, keys_out, lay, M, true);
 }

@@ -47,17 +47,6 @@ struct NcclDyn {
 static NcclDyn g_nccl;
 
 // ---------------- helpers ----------------
-template <typename T>
-static int dev_alloc(T **p, size_t count) {
-  CUDA_TRY(cudaMalloc((void **)p, sizeof(T) * (count ? count : 1)));
-  return BALM_OK;
-}
-#define TRY(x)                \
-  do {                        \
-    int _s = (x);             \
-    if (_s != BALM_OK) return _s; \
-  } while (0)
-
 static void free_problem(balm_ctx *c) {
   cudaFree(c->obs); cudaFree(c->pose_idx); cudaFree(c->row_ptr); cudaFree(c->coe); cudaFree(c->fix);
   cudaFree(c->csc_ptr); cudaFree(c->csc_obs); cudaFree(c->csc_vox); cudaFree(c->csc_lo); cudaFree(c->csc_hi);

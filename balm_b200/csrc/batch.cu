@@ -4,10 +4,10 @@
 // Per LM iteration, enqueued back to back on the batch's stream, every kernel masked per problem:
 //   batch_stats_kernel<true>   per voxel: cluster sums, eigen-decomposition, stats row, residual term (= the stats pass)
 //   batch_residual_kernel      per problem: fixed-order sum of its voxels' residual terms -> r1
-//   batch_obs_kernel           per 32-voxel chunk of one problem: G' rows (fp64, dense per problem) and the per-pose
-//                              gradient / diagonal-block partials (obs_terms, shared with obs_pass_kernel)
-//   batch_syrk_kernel          per (problem, 64x64 upper tile, 768-row chunk): DMMA partial of G'^T G'
-//   batch_assemble_kernel      per (problem, 64-column block): H = -sum of partials + blockdiag, g
+//   batch_obs_kernel           per 32-voxel chunk of one problem (chunk_walk): G' rows (fp64, dense per problem) and the
+//                              per-pose gradient / diagonal-block partials (obs_terms, shared with obs_pass_kernel)
+//   batch_syrk_kernel<3, 0>    per (problem, 64x64 upper tile, 768-row chunk): DMMA partial of G'^T G'
+//   batch_assemble_kernel<27, 6, true, true>  per (problem, 64-column block): H = -sum of partials + blockdiag, g
 //   batch_solve_kernel         per problem, one CTA: unpivoted LDL^T of H + uD in shared memory, backward error, up to
 //                              3 rounds of refinement, q1, trial poses
 //   batch_stats_kernel<false> + batch_residual_kernel at the trial poses -> r2
@@ -19,9 +19,9 @@
 // The pose covariance (balm_batch_pose_covariance) follows the same rules, with the per-observation terms of covariance.cu:
 //   batch_stats_kernel<true>    (inside enqueue_eval when Rcov is wanted, which also gives H) at the given poses
 //   batch_cov_rows_kernel       per voxel: Wz, the eight rows c2 Q^T | c2 V^T (8 M_p x ldp per problem), c2^2 D per obs
-//   batch_cov_diag_kernel       per 32-voxel chunk: per-pose partial sums of the c2^2 D blocks
+//   batch_cov_diag_kernel       per 32-voxel chunk (chunk_walk): per-pose partial sums of the c2^2 D blocks
 //   batch_syrk_kernel<8, 4>     per (problem, tile, 768-row chunk): partial of Q V^T + V Q^T (A = partner row ^ 4)
-//   batch_cov_assemble_kernel   per (problem, 64-column block): Rcov_raw = + sum of partials + blockdiag
+//   batch_assemble_kernel<21, 0, false, false>  per (problem, 64-column block): Rcov_raw = + sum of partials + blockdiag
 //   batch_cov_solve_kernel      per problem, one CTA: LDL^T of H, singularity test, H^-1 Rcov_raw H^-1, symmetrised
 #include <math.h>
 #include <string.h>
@@ -44,7 +44,6 @@ constexpr int SOLVE_SMEM = (MAXN * (MAXN + 1) / 2 + 5 * MAXN) * (int)sizeof(doub
 struct Prob {                  // layout of one problem, built on the host at registration
   int pose_base, np, n, ldp;   // first pose in the concatenated array, poses, 6 np, G' row stride (n rounded up to 64)
   int ochunk_base, n_ochunks;  // its observation-sweep chunks
-  int item_base, n_rchunks;    // its SYRK items: tile t, row chunk c -> item_base + t * n_rchunks + c
   long long vox_base, nvox;    // its voxels
   long long goff, hoff;        // offsets of its G' and H
 };
@@ -116,6 +115,26 @@ __global__ void __launch_bounds__(128) batch_residual_kernel(const Prob *prob, c
   if (threadIdx.x == 0) out[b] = (red[0] + red[1]) + (red[2] + red[3]);
 }
 
+// ---- the voxels of chunk c (of CHUNK voxels) of problem pr in ascending order, one warp, lane = problem-local pose:
+// f(v, s) for every voxel v that the lane's pose observes, s its observation. slot_of: 32 ints of the warp's own ----
+template <typename F>
+__device__ __forceinline__ void chunk_walk(const Dev &d, const Prob &pr, int c, int *slot_of, F f) {
+  const int lane = threadIdx.x & 31;
+  const long long v0 = pr.vox_base + (long long)(c - pr.ochunk_base) * CHUNK;
+  const long long v1 = v0 + CHUNK < pr.vox_base + pr.nvox ? v0 + CHUNK : pr.vox_base + pr.nvox;
+  for (long long v = v0; v < v1; v++) {
+    const long long s0 = d.row_ptr[v];
+    const int k = (int)(d.row_ptr[v + 1] - s0);
+    slot_of[lane] = -1;
+    __syncwarp();
+    if (lane < k) slot_of[d.pose_idx[s0 + lane]] = lane;  // pose_idx < np <= 32 (checked at registration)
+    __syncwarp();
+    const int slot = slot_of[lane];
+    __syncwarp();
+    if (slot >= 0) f(v, s0 + slot);
+  }
+}
+
 // ---- per chunk of CHUNK voxels of one problem, one warp, lane = problem-local pose ----
 __global__ void __launch_bounds__(128) batch_obs_kernel(Dev d, const double *poses, const int *mask,
                                                         const int *ochunk_prob, int n_ochunks, const double *stats,
@@ -133,20 +152,9 @@ __global__ void __launch_bounds__(128) batch_obs_kernel(Dev d, const double *pos
   double acc[27];
 #pragma unroll
   for (int q = 0; q < 27; q++) acc[q] = 0.0;
-  const long long v0 = pr.vox_base + (long long)(c - pr.ochunk_base) * CHUNK;
-  const long long v1 = v0 + CHUNK < pr.vox_base + pr.nvox ? v0 + CHUNK : pr.vox_base + pr.nvox;
-  for (long long v = v0; v < v1; v++) {
-    const long long s0 = d.row_ptr[v];
-    const int k = (int)(d.row_ptr[v + 1] - s0);
-    slot_of[warp][lane] = -1;
-    __syncwarp();
-    if (lane < k) slot_of[warp][d.pose_idx[s0 + lane]] = lane;  // pose_idx < np <= 32 (checked at registration)
-    __syncwarp();
-    const int slot = slot_of[warp][lane];
-    __syncwarp();
-    if (slot < 0) continue;
+  chunk_walk(d, pr, c, slot_of[warp], [&](long long v, long long s) {
     double o[10], st[BALM_SWEEP_WORDS];
-    const double2 *o2 = reinterpret_cast<const double2 *>(d.obs + (size_t)(s0 + slot) * 10);
+    const double2 *o2 = reinterpret_cast<const double2 *>(d.obs + (size_t)s * 10);
     const double2 *st2 = reinterpret_cast<const double2 *>(stats + (size_t)v * BALM_STATS_STRIDE + BALM_SWEEP_OFF);
 #pragma unroll
     for (int q = 0; q < 5; q++) {
@@ -169,7 +177,7 @@ __global__ void __launch_bounds__(128) batch_obs_kernel(Dev d, const double *pos
         for (int h = 0; h < 3; h++) qd[h] = make_double2(gv[rr][2 * h], gv[rr][2 * h + 1]);
       }
     });
-  }
+  });
   if (active) {
     double *pp = opart + (size_t)c * 27 * 32 + lane;
 #pragma unroll
@@ -237,20 +245,26 @@ __global__ void __launch_bounds__(128) batch_syrk_kernel(const Prob *prob, const
     }
 }
 
-// ---- per (problem, 64-column block): H = -sum over row chunks of the SYRK partials + blockdiag, g ----
-// Element (i, j) and (j, i) are computed from the same upper partial, so H is exactly symmetric.
-__global__ void __launch_bounds__(256) batch_assemble_kernel(const Prob *prob, const int *mask, const double *opart,
-                                                             const double *spart, double *H, double *g) {
-  __shared__ double accs[27][32];
+// ---- per (problem, 64-column block): H = -sum (NEG) or +sum over row chunks of the SYRK partials, then + blockdiag;
+// the diagonal blocks are the chunk-ordered sums of the problem's per-chunk partials (W words per pose, the block's
+// upper triangle row-major from word OFF), and with GRAD words 0..5 are the gradient, written to g.
+// range[p] = (first SYRK item, row chunks) of problem p. Element (i, j) and (j, i) are computed from the same upper
+// partial, so H is exactly symmetric. The Hessian is <27, 6, true, true>, Rcov_raw <21, 0, false, false>. ----
+template <int W, int OFF, bool NEG, bool GRAD>
+__global__ void __launch_bounds__(256) batch_assemble_kernel(const Prob *prob, const int *mask, const int2 *range,
+                                                             const double *part, const double *spart, double *H,
+                                                             double *g) {
+  __shared__ double accs[W][32];
   const int b = blockIdx.x;
   if (!mask[b]) return;
   const Prob pr = prob[b];
   const int n = pr.n, nt = pr.ldp / TILE;
   if (blockIdx.y * TILE >= n) return;
-  for (int e = threadIdx.x; e < 27 * pr.np; e += 256) {
+  const int2 ir = range[b];
+  for (int e = threadIdx.x; e < W * pr.np; e += 256) {
     const int q = e / pr.np, i = e % pr.np;
     double s = 0.0;
-    for (int c = 0; c < pr.n_ochunks; c++) s += opart[((size_t)(pr.ochunk_base + c) * 27 + q) * 32 + i];
+    for (int c = 0; c < pr.n_ochunks; c++) s += part[((size_t)(pr.ochunk_base + c) * W + q) * 32 + i];
     accs[q][i] = s;
   }
   __syncthreads();
@@ -261,19 +275,19 @@ __global__ void __launch_bounds__(256) batch_assemble_kernel(const Prob *prob, c
       const int rr = i < j ? i : j, cc = i < j ? j : i;
       const int bi = rr / TILE, bj = cc / TILE;
       const int t = bi * nt - bi * (bi - 1) / 2 + (bj - bi);
-      const double *src = spart + (size_t)(pr.item_base + t * pr.n_rchunks) * TILE * TILE + (rr % TILE) * TILE + cc % TILE;
+      const double *src = spart + (size_t)(ir.x + t * ir.y) * TILE * TILE + (rr % TILE) * TILE + cc % TILE;
       double s = 0.0;
-      for (int c = 0; c < pr.n_rchunks; c++) s += src[(size_t)c * TILE * TILE];
-      double h = -s;
+      for (int c = 0; c < ir.y; c++) s += src[(size_t)c * TILE * TILE];
+      double h = NEG ? -s : s;
       const int pi = rr / 6;
       if (pi == cc / 6) {
         const int r6 = rr % 6, c6 = cc % 6;
-        h += accs[6 + r6 * 6 - r6 * (r6 - 1) / 2 + (c6 - r6)][pi];
+        h += accs[OFF + r6 * 6 - r6 * (r6 - 1) / 2 + (c6 - r6)][pi];
       }
       Hb[(size_t)j * n + i] = h;
     }
   }
-  if (blockIdx.y == 0)
+  if (GRAD && blockIdx.y == 0)
     for (int i = threadIdx.x; i < n; i += 256) g[6 * (size_t)pr.pose_base + i] = accs[i % 6][i / 6];
 }
 
@@ -573,63 +587,15 @@ __global__ void __launch_bounds__(128) batch_cov_diag_kernel(Dev d, const int *o
   double acc[21];
 #pragma unroll
   for (int q = 0; q < 21; q++) acc[q] = 0.0;
-  const long long v0 = pr.vox_base + (long long)(c - pr.ochunk_base) * CHUNK;
-  const long long v1 = v0 + CHUNK < pr.vox_base + pr.nvox ? v0 + CHUNK : pr.vox_base + pr.nvox;
-  for (long long v = v0; v < v1; v++) {
-    const long long s0 = d.row_ptr[v];
-    const int k = (int)(d.row_ptr[v + 1] - s0);
-    slot_of[warp][lane] = -1;
-    __syncwarp();
-    if (lane < k) slot_of[warp][d.pose_idx[s0 + lane]] = lane;
-    __syncwarp();
-    const int slot = slot_of[warp][lane];
-    __syncwarp();
-    if (slot < 0) continue;
-    const double *dd = Dobs + (size_t)(s0 + slot) * 21;
+  chunk_walk(d, pr, c, slot_of[warp], [&](long long, long long s) {
+    const double *dd = Dobs + (size_t)s * 21;
 #pragma unroll
     for (int q = 0; q < 21; q++) acc[q] += dd[q];
-  }
+  });
   if (lane < pr.np) {
     double *pp = dpart + (size_t)c * 21 * 32 + lane;
 #pragma unroll
     for (int q = 0; q < 21; q++) pp[q * 32] = acc[q];
-  }
-}
-
-// ---- per (problem, 64-column block): Rcov_raw = + sum over row chunks of the SYRK partials + blockdiag(D), the
-// Hessian assembly with the opposite sign and no gradient. cit[p] = (first SYRK item, row chunks) of problem p. ----
-__global__ void __launch_bounds__(256) batch_cov_assemble_kernel(const Prob *prob, const int2 *cit, const double *dpart,
-                                                                 const double *spart, double *R) {
-  __shared__ double accs[21][32];
-  const int b = blockIdx.x;
-  const Prob pr = prob[b];
-  const int n = pr.n, nt = pr.ldp / TILE;
-  if (blockIdx.y * TILE >= n) return;
-  const int2 ci = cit[b];
-  for (int e = threadIdx.x; e < 21 * pr.np; e += 256) {
-    const int q = e / pr.np, i = e % pr.np;
-    double s = 0.0;
-    for (int c = 0; c < pr.n_ochunks; c++) s += dpart[((size_t)(pr.ochunk_base + c) * 21 + q) * 32 + i];
-    accs[q][i] = s;
-  }
-  __syncthreads();
-  double *Rb = R + pr.hoff;
-  const int j_end = (blockIdx.y + 1) * TILE < n ? (blockIdx.y + 1) * TILE : n;
-  for (int j = blockIdx.y * TILE; j < j_end; j++) {
-    for (int i = threadIdx.x; i < n; i += 256) {
-      const int rr = i < j ? i : j, cc = i < j ? j : i;
-      const int bi = rr / TILE, bj = cc / TILE;
-      const int t = bi * nt - bi * (bi - 1) / 2 + (bj - bi);
-      const double *src = spart + (size_t)(ci.x + t * ci.y) * TILE * TILE + (rr % TILE) * TILE + cc % TILE;
-      double s = 0.0;
-      for (int c = 0; c < ci.y; c++) s += src[(size_t)c * TILE * TILE];
-      const int pi = rr / 6;
-      if (pi == cc / 6) {
-        const int r6 = rr % 6, c6 = cc % 6;
-        s += accs[r6 * 6 - r6 * (r6 - 1) / 2 + (c6 - r6)][pi];
-      }
-      Rb[(size_t)j * n + i] = s;
-    }
   }
 }
 
@@ -721,7 +687,8 @@ struct BatchReg {
   size_t H_size = 0, G_size = 0;
   Prob *prob = nullptr;
   int *vox_prob = nullptr, *pose_prob = nullptr, *ochunk_prob = nullptr;
-  int4 *items = nullptr;
+  int4 *items = nullptr;       // the Hessian SYRK's (syrk_items)
+  int2 *item_range = nullptr;
   long long *row_ptr = nullptr;
   int *pose_idx = nullptr;
   double *obs = nullptr, *fix = nullptr, *coe = nullptr;
@@ -741,8 +708,8 @@ struct BatchReg {
   int *n_active() { return ints + 7 * B; }
   Dev dev() const { return Dev{prob, vox_prob, row_ptr, pose_idx, obs, fix, coe, M, K}; }
   ~BatchReg() {
-    void *ptrs[] = {prob, vox_prob, pose_prob, ochunk_prob, items, row_ptr, pose_idx, obs, fix, coe, key, layer, G, stats, res_v,
-                    opart, spart, H, g, poses, trial, r_eval, r2, r1, q1, u, v, ints};
+    void *ptrs[] = {prob, vox_prob, pose_prob, ochunk_prob, items, item_range, row_ptr, pose_idx, obs, fix, coe, key, layer, G,
+                    stats, res_v, opart, spart, H, g, poses, trial, r_eval, r2, r1, q1, u, v, ints};
     for (void *p : ptrs) cudaFree(p);
   }
 };
@@ -757,54 +724,74 @@ struct balm_batch {
 namespace {
 
 template <typename T>
-int dalloc(T **p, size_t count) {
-  CUDA_TRY(cudaMalloc((void **)p, sizeof(T) * (count ? count : 1)));
-  return BALM_OK;
-}
-template <typename T>
 int upload(T **p, const T *src, size_t count, cudaStream_t st) {
-  const int rc = dalloc(p, count);
-  if (rc != BALM_OK) return rc;
+  TRY(dev_alloc(p, count));
   if (count) CUDA_TRY(cudaMemcpyAsync(*p, src, sizeof(T) * count, cudaMemcpyHostToDevice, st));
   return BALM_OK;
 }
-#define BTRY(x)                     \
-  do {                              \
-    const int _s = (x);             \
-    if (_s != BALM_OK) return _s;   \
-  } while (0)
-
-int invalid(const char *msg) {
+int invalid(const std::string &msg) {
   balm_set_error(msg);
   return BALM_ERR_INVALID;
+}
+
+// The problem table of a registration: n_problems >= 1, pose_ptr[0] = 0 and 1 .. BALM_BATCH_MAX_POSES poses each.
+int check_pose_ptr(const char *who, int n_problems, const int64_t *pose_ptr) {
+  const std::string w = who;
+  if (n_problems < 1) return invalid(w + ": n_problems must be >= 1");
+  if (pose_ptr[0] != 0) return invalid(w + ": pose_ptr[0] must be 0");
+  for (int b = 0; b < n_problems; b++) {
+    const int64_t np = pose_ptr[b + 1] - pose_ptr[b];
+    if (np < 1 || np > BALM_BATCH_MAX_POSES)
+      return invalid(w + ": every problem needs 1 .. BALM_BATCH_MAX_POSES poses (pose_ptr ascending)");
+  }
+  return BALM_OK;
+}
+
+// The SYRK items of every problem for rpv rows per voxel (3: G', 8: the covariance rows): per problem its upper tiles x
+// chunks of ROWS rows, item (problem, tile row, tile column, row chunk); range[p] = (first item, row chunks) of problem p.
+void syrk_items(const std::vector<Prob> &hprob, int rpv, std::vector<int4> &items, std::vector<int2> &range) {
+  items.clear();
+  range.resize(hprob.size());
+  for (size_t b = 0; b < hprob.size(); b++) {
+    const Prob &p = hprob[b];
+    const int nt = p.ldp / TILE, nrc = (int)((rpv * p.nvox + ROWS - 1) / ROWS);
+    range[b] = make_int2((int)items.size(), nrc);
+    for (int ti = 0; ti < nt; ti++)
+      for (int tj = ti; tj < nt; tj++)
+        for (int c = 0; c < nrc; c++) items.push_back(make_int4((int)b, ti, tj, c));
+  }
+}
+
+// batch_stats_kernel at poses for every problem with mask[b] != 0: the residual terms, and with stats non-null the
+// stats rows.
+void enqueue_stats(balm_batch *bt, BatchReg *r, const double *poses, const int *mask, bool use_fix, double *stats) {
+  if (r->M == 0) return;
+  const int blocks = (int)std::min<int64_t>((r->M + 7) / 8, (int64_t)bt->sm_count * 8);
+  if (stats)
+    batch_stats_kernel<true><<<blocks, 256, 0, bt->stream>>>(r->dev(), poses, mask, use_fix ? 1 : 0, stats, r->res_v);
+  else
+    batch_stats_kernel<false><<<blocks, 256, 0, bt->stream>>>(r->dev(), poses, mask, use_fix ? 1 : 0, nullptr, r->res_v);
 }
 
 // The evaluation of every problem with mask[b] != 0 at r->poses: r_eval, H, g.
 int enqueue_eval(balm_batch *bt, BatchReg *r, const int *mask, bool use_fix) {
   cudaStream_t st = bt->stream;
-  const Dev d = r->dev();
-  if (r->M > 0) {
-    const int blocks = (int)std::min<int64_t>((r->M + 7) / 8, (int64_t)bt->sm_count * 8);
-    batch_stats_kernel<true><<<blocks, 256, 0, st>>>(d, r->poses, mask, use_fix ? 1 : 0, r->stats, r->res_v);
-  }
+  enqueue_stats(bt, r, r->poses, mask, use_fix, r->stats);
   batch_residual_kernel<<<r->B, 128, 0, st>>>(r->prob, mask, r->res_v, r->r_eval);
   if (r->n_ochunks > 0)
-    batch_obs_kernel<<<(r->n_ochunks + 3) / 4, 128, 0, st>>>(d, r->poses, mask, r->ochunk_prob, r->n_ochunks, r->stats,
-                                                             r->G, r->opart);
+    batch_obs_kernel<<<(r->n_ochunks + 3) / 4, 128, 0, st>>>(r->dev(), r->poses, mask, r->ochunk_prob, r->n_ochunks,
+                                                             r->stats, r->G, r->opart);
   if (r->n_items > 0) batch_syrk_kernel<3, 0><<<r->n_items, 128, 0, st>>>(r->prob, mask, r->items, r->G, r->spart);
-  batch_assemble_kernel<<<dim3(r->B, MAXN / TILE), 256, 0, st>>>(r->prob, mask, r->opart, r->spart, r->H, r->g);
+  batch_assemble_kernel<27, 6, true, true><<<dim3(r->B, MAXN / TILE), 256, 0, st>>>(r->prob, mask, r->item_range, r->opart,
+                                                                                    r->spart, r->H, r->g);
   CUDA_TRY(cudaGetLastError());
   return BALM_OK;
 }
 
 // The residual (fix clusters included, as evaluate_only_residual) at the trial poses of every active problem: r2.
 int enqueue_trial_residual(balm_batch *bt, BatchReg *r) {
-  cudaStream_t st = bt->stream;
-  if (r->M > 0) {
-    const int blocks = (int)std::min<int64_t>((r->M + 7) / 8, (int64_t)bt->sm_count * 8);
-    batch_stats_kernel<false><<<blocks, 256, 0, st>>>(r->dev(), r->trial, r->active(), 1, nullptr, r->res_v);
-  }
-  batch_residual_kernel<<<r->B, 128, 0, st>>>(r->prob, r->active(), r->res_v, r->r2);
+  enqueue_stats(bt, r, r->trial, r->active(), true, nullptr);
+  batch_residual_kernel<<<r->B, 128, 0, bt->stream>>>(r->prob, r->active(), r->res_v, r->r2);
   CUDA_TRY(cudaGetLastError());
   return BALM_OK;
 }
@@ -856,7 +843,6 @@ static int reg_layout(balm_batch *bt, BatchReg *r, int B, const int64_t *pose_pt
   r->M = voxel_ptr[B];
   r->K = K;
   std::vector<int> vox_prob((size_t)r->M), pose_prob((size_t)r->P), ochunk_prob;
-  std::vector<int4> items;
   r->hprob.resize(B);
   long long goff = 0, hoff = 0;
   for (int b = 0; b < B; b++) {
@@ -870,12 +856,6 @@ static int reg_layout(balm_batch *bt, BatchReg *r, int B, const int64_t *pose_pt
     p.ochunk_base = (int)ochunk_prob.size();
     p.n_ochunks = (int)((p.nvox + CHUNK - 1) / CHUNK);
     ochunk_prob.insert(ochunk_prob.end(), (size_t)p.n_ochunks, b);
-    p.item_base = (int)items.size();
-    p.n_rchunks = (int)((3 * p.nvox + ROWS - 1) / ROWS);
-    const int nt = p.ldp / TILE;
-    for (int ti = 0; ti < nt; ti++)
-      for (int tj = ti; tj < nt; tj++)
-        for (int c = 0; c < p.n_rchunks; c++) items.push_back(make_int4(b, ti, tj, c));
     p.goff = goff;
     p.hoff = hoff;
     goff += 3 * p.nvox * p.ldp;
@@ -883,15 +863,19 @@ static int reg_layout(balm_batch *bt, BatchReg *r, int B, const int64_t *pose_pt
     std::fill(vox_prob.begin() + p.vox_base, vox_prob.begin() + p.vox_base + p.nvox, b);
     std::fill(pose_prob.begin() + p.pose_base, pose_prob.begin() + p.pose_base + p.np, b);
   }
+  std::vector<int4> items;
+  std::vector<int2> range;
+  syrk_items(r->hprob, 3, items, range);
   r->n_ochunks = (int)ochunk_prob.size();
   r->n_items = (int)items.size();
   r->G_size = (size_t)goff;
   r->H_size = (size_t)hoff;
-  BTRY(upload(&r->prob, r->hprob.data(), (size_t)B, st));
-  BTRY(upload(&r->vox_prob, vox_prob.data(), vox_prob.size(), st));
-  BTRY(upload(&r->pose_prob, pose_prob.data(), pose_prob.size(), st));
-  BTRY(upload(&r->ochunk_prob, ochunk_prob.data(), ochunk_prob.size(), st));
-  BTRY(upload(&r->items, items.data(), items.size(), st));
+  TRY(upload(&r->prob, r->hprob.data(), (size_t)B, st));
+  TRY(upload(&r->vox_prob, vox_prob.data(), vox_prob.size(), st));
+  TRY(upload(&r->pose_prob, pose_prob.data(), pose_prob.size(), st));
+  TRY(upload(&r->ochunk_prob, ochunk_prob.data(), ochunk_prob.size(), st));
+  TRY(upload(&r->items, items.data(), items.size(), st));
+  TRY(upload(&r->item_range, range.data(), range.size(), st));
   return BALM_OK;
 }
 
@@ -900,9 +884,9 @@ static int reg_layout(balm_batch *bt, BatchReg *r, int B, const int64_t *pose_pt
 static int reg_finish(balm_batch *bt, BatchReg *r) {
   cudaStream_t st = bt->stream;
   const int B = r->B;
-  BTRY(dalloc(&r->ints, 7 * (size_t)B + 1));
+  TRY(dev_alloc(&r->ints, 7 * (size_t)B + 1));
   int *d_planes = nullptr;
-  BTRY(dalloc(&d_planes, (size_t)r->P));
+  TRY(dev_alloc(&d_planes, (size_t)r->P));
   CUDA_TRY(cudaMemsetAsync(d_planes, 0, sizeof(int) * r->P, st));
   CUDA_TRY(cudaMemsetAsync(r->n_active(), 0, sizeof(int), st));  // serves as the check's error flag here
   if (r->M > 0) batch_check_kernel<<<(unsigned)((r->M + 127) / 128), 128, 0, st>>>(r->dev(), r->n_active(), d_planes);
@@ -919,18 +903,18 @@ static int reg_finish(balm_batch *bt, BatchReg *r) {
     r->min_planes[b] = *std::min_element(planes.begin() + p.pose_base, planes.begin() + p.pose_base + p.np);
   }
   // workspaces
-  BTRY(dalloc(&r->G, r->G_size));
+  TRY(dev_alloc(&r->G, r->G_size));
   CUDA_TRY(cudaMemsetAsync(r->G, 0, sizeof(double) * r->G_size, st));  // columns of non-observing poses stay zero
-  BTRY(dalloc(&r->stats, (size_t)r->M * BALM_STATS_STRIDE));
-  BTRY(dalloc(&r->res_v, (size_t)r->M));
-  BTRY(dalloc(&r->opart, (size_t)r->n_ochunks * 27 * 32));
-  BTRY(dalloc(&r->spart, (size_t)r->n_items * TILE * TILE));
-  BTRY(dalloc(&r->H, r->H_size));
-  BTRY(dalloc(&r->g, 6 * (size_t)r->P));
-  BTRY(dalloc(&r->poses, 12 * (size_t)r->P));
-  BTRY(dalloc(&r->trial, 12 * (size_t)r->P));
+  TRY(dev_alloc(&r->stats, (size_t)r->M * BALM_STATS_STRIDE));
+  TRY(dev_alloc(&r->res_v, (size_t)r->M));
+  TRY(dev_alloc(&r->opart, (size_t)r->n_ochunks * 27 * 32));
+  TRY(dev_alloc(&r->spart, (size_t)r->n_items * TILE * TILE));
+  TRY(dev_alloc(&r->H, r->H_size));
+  TRY(dev_alloc(&r->g, 6 * (size_t)r->P));
+  TRY(dev_alloc(&r->poses, 12 * (size_t)r->P));
+  TRY(dev_alloc(&r->trial, 12 * (size_t)r->P));
   double **scal[] = {&r->r_eval, &r->r2, &r->r1, &r->q1, &r->u, &r->v};
-  for (double **p : scal) BTRY(dalloc(p, (size_t)B));
+  for (double **p : scal) TRY(dev_alloc(p, (size_t)B));
   fill_kernel<<<(B + 127) / 128, 128, 0, st>>>(r->ones(), B, 1);
   CUDA_TRY(cudaGetLastError());
   CUDA_TRY(cudaStreamSynchronize(st));
@@ -941,12 +925,12 @@ static int build_registration(balm_batch *bt, BatchReg *r, int B, const int64_t 
                               const int64_t *row_ptr, const int32_t *pose_idx, const double *obs10,
                               const double *fix10, const double *coe) {
   cudaStream_t st = bt->stream;
-  BTRY(reg_layout(bt, r, B, pose_ptr, voxel_ptr, row_ptr[voxel_ptr[B]]));
-  BTRY(upload(&r->row_ptr, reinterpret_cast<const long long *>(row_ptr), (size_t)r->M + 1, st));
-  BTRY(upload(&r->pose_idx, pose_idx, (size_t)r->K, st));
-  BTRY(upload(&r->obs, obs10, (size_t)r->K * 10, st));
-  if (fix10) BTRY(upload(&r->fix, fix10, (size_t)r->M * 10, st));
-  BTRY(upload(&r->coe, coe, (size_t)r->M, st));
+  TRY(reg_layout(bt, r, B, pose_ptr, voxel_ptr, row_ptr[voxel_ptr[B]]));
+  TRY(upload(&r->row_ptr, reinterpret_cast<const long long *>(row_ptr), (size_t)r->M + 1, st));
+  TRY(upload(&r->pose_idx, pose_idx, (size_t)r->K, st));
+  TRY(upload(&r->obs, obs10, (size_t)r->K * 10, st));
+  if (fix10) TRY(upload(&r->fix, fix10, (size_t)r->M * 10, st));
+  TRY(upload(&r->coe, coe, (size_t)r->M, st));
   return reg_finish(bt, r);
 }
 
@@ -966,14 +950,10 @@ extern "C" int balm_batch_set_voxels(balm_batch *bt, int n_problems, const int64
                                      const int64_t *row_ptr, const int32_t *pose_idx, const double *obs10,
                                      const double *fix10, const double *coe) {
   if (!bt || !pose_ptr || !voxel_ptr || !row_ptr) return invalid("balm_batch_set_voxels: bad arguments");
-  if (n_problems < 1) return invalid("balm_batch_set_voxels: n_problems must be >= 1");
-  if (pose_ptr[0] != 0 || voxel_ptr[0] != 0) return invalid("balm_batch_set_voxels: pose_ptr[0] and voxel_ptr[0] must be 0");
-  for (int b = 0; b < n_problems; b++) {
-    const int64_t np = pose_ptr[b + 1] - pose_ptr[b];
-    if (np < 1 || np > BALM_BATCH_MAX_POSES)
-      return invalid("balm_batch_set_voxels: every problem needs 1 .. BALM_BATCH_MAX_POSES poses (pose_ptr ascending)");
+  TRY(check_pose_ptr("balm_batch_set_voxels", n_problems, pose_ptr));
+  if (voxel_ptr[0] != 0) return invalid("balm_batch_set_voxels: voxel_ptr[0] must be 0");
+  for (int b = 0; b < n_problems; b++)
     if (voxel_ptr[b + 1] < voxel_ptr[b]) return invalid("balm_batch_set_voxels: voxel_ptr must be ascending");
-  }
   const int64_t M = voxel_ptr[n_problems];
   if (row_ptr[0] != 0) return invalid("balm_batch_set_voxels: row_ptr[0] must be 0");
   const int64_t K = row_ptr[M];
@@ -993,13 +973,7 @@ extern "C" int balm_batch_cut_voxels(balm_batch *bt, int n_problems, const int64
                                      const balm_assoc_opts *opts, int64_t *n_voxels_out, int64_t *n_obs_out) {
   if (!bt || !pose_ptr || !pose_scan || !scan_ptr || !poses12 || n_scans < 1)
     return invalid("balm_batch_cut_voxels: bad arguments");
-  if (n_problems < 1) return invalid("balm_batch_cut_voxels: n_problems must be >= 1");
-  if (pose_ptr[0] != 0) return invalid("balm_batch_cut_voxels: pose_ptr[0] must be 0");
-  for (int b = 0; b < n_problems; b++) {
-    const int64_t np = pose_ptr[b + 1] - pose_ptr[b];
-    if (np < 1 || np > BALM_BATCH_MAX_POSES)
-      return invalid("balm_batch_cut_voxels: every problem needs 1 .. BALM_BATCH_MAX_POSES poses (pose_ptr ascending)");
-  }
+  TRY(check_pose_ptr("balm_batch_cut_voxels", n_problems, pose_ptr));
   if (scan_ptr[0] != 0) return invalid("balm_batch_cut_voxels: scan_ptr[0] must be 0");
   for (int s = 0; s < n_scans; s++)
     if (scan_ptr[s + 1] < scan_ptr[s]) return invalid("balm_batch_cut_voxels: scan_ptr must be ascending");
@@ -1024,13 +998,13 @@ extern "C" int balm_batch_cut_voxels(balm_batch *bt, int n_problems, const int64
   const AssocInput in{"balm_batch_cut_voxels", n_points, xyz, (int)P, poses12, nullptr, n_problems, pose_ptr, pose_scan,
                       scan_ptr, n_items};
   const AssocRegister reg = [&](int64_t M, int64_t K, const int64_t *voxel_ptr, const int64_t *optr, AssocEmit *out) {
-    BTRY(reg_layout(bt, r, n_problems, pose_ptr, voxel_ptr, K));
-    BTRY(dalloc(&r->row_ptr, (size_t)M + 1));
-    BTRY(dalloc(&r->pose_idx, (size_t)K));
-    BTRY(dalloc(&r->obs, (size_t)K * 10));
-    BTRY(dalloc(&r->coe, (size_t)M));
-    BTRY(dalloc(&r->key, (size_t)M));
-    BTRY(dalloc(&r->layer, (size_t)M));
+    TRY(reg_layout(bt, r, n_problems, pose_ptr, voxel_ptr, K));
+    TRY(dev_alloc(&r->row_ptr, (size_t)M + 1));
+    TRY(dev_alloc(&r->pose_idx, (size_t)K));
+    TRY(dev_alloc(&r->obs, (size_t)K * 10));
+    TRY(dev_alloc(&r->coe, (size_t)M));
+    TRY(dev_alloc(&r->key, (size_t)M));
+    TRY(dev_alloc(&r->layer, (size_t)M));
     *out = AssocEmit{r->obs, 1, 10, r->pose_idx, r->row_ptr, r->coe, r->key, r->layer};
     obs_ptr.assign(optr, optr + n_problems + 1);
     return (int)BALM_OK;
@@ -1088,7 +1062,7 @@ extern "C" int balm_batch_evaluate(balm_batch *bt, const double *poses12, int in
   CUDA_TRY(cudaSetDevice(bt->device));
   cudaStream_t st = bt->stream;
   CUDA_TRY(cudaMemcpyAsync(r->poses, poses12, sizeof(double) * 12 * r->P, cudaMemcpyHostToDevice, st));
-  BTRY(enqueue_eval(bt, r, r->ones(), include_fix != 0));
+  TRY(enqueue_eval(bt, r, r->ones(), include_fix != 0));
   if (H) CUDA_TRY(cudaMemcpyAsync(H, r->H, sizeof(double) * r->H_size, cudaMemcpyDeviceToHost, st));
   if (g) CUDA_TRY(cudaMemcpyAsync(g, r->g, sizeof(double) * 6 * r->P, cudaMemcpyDeviceToHost, st));
   CUDA_TRY(cudaMemcpyAsync(residual, r->r_eval, sizeof(double) * r->B, cudaMemcpyDeviceToHost, st));
@@ -1109,12 +1083,9 @@ extern "C" int balm_batch_damping_iter(balm_batch *bt, double *poses12, const ba
     status[b] = (o->min_planes_per_pose > 0 && r->min_planes[b] < o->min_planes_per_pose) ? BALM_ERR_TOO_FEW_PLANES : BALM_OK;
     n_iters[b] = 0;
   }
+  ScratchPool pool;
   balm_trace *d_trace = nullptr;
-  BTRY(dalloc(&d_trace, (size_t)B * std::max(1, max_iter)));
-  struct Free {
-    balm_trace *p;
-    ~Free() { cudaFree(p); }
-  } free_trace{d_trace};
+  TRY(pool.get(&d_trace, (size_t)B * std::max(1, max_iter)));
   const size_t pbytes = sizeof(double) * 12 * r->P;
   CUDA_TRY(cudaMemcpyAsync(r->poses, poses12, pbytes, cudaMemcpyHostToDevice, st));
   CUDA_TRY(cudaMemcpyAsync(r->status(), status, sizeof(int) * B, cudaMemcpyHostToDevice, st));
@@ -1128,11 +1099,11 @@ extern "C" int balm_batch_damping_iter(balm_batch *bt, double *poses12, const ba
            r->r1, r->u, r->v, r->active(), r->calc(), r->evalm(), r->n_iters(), r->n_active(), r->poses, r->trial,
            d_trace};
   for (int it = 0; any && it < max_iter; it++) {
-    BTRY(enqueue_eval(bt, r, r->evalm(), o->hess_includes_fix != 0));
+    TRY(enqueue_eval(bt, r, r->evalm(), o->hess_includes_fix != 0));
     batch_solve_kernel<<<B, SOLVE_THREADS, SOLVE_SMEM, st>>>(r->prob, r->active(), r->H, r->g, r->u, r->poses,
                                                              r->trial, r->q1, r->notpd());
     CUDA_TRY(cudaGetLastError());
-    BTRY(enqueue_trial_residual(bt, r));
+    TRY(enqueue_trial_residual(bt, r));
     CUDA_TRY(cudaMemsetAsync(r->n_active(), 0, sizeof(int), st));
     a.it = it;
     batch_lm_kernel<<<(B + 127) / 128, 128, 0, st>>>(a);
@@ -1169,59 +1140,39 @@ extern "C" int balm_batch_pose_covariance(balm_batch *bt, const double *poses12,
   CUDA_TRY(cudaSetDevice(bt->device));
   cudaStream_t st = bt->stream;
   const int B = r->B;
-  // the covariance SYRK's items: per problem its upper tiles x chunks of ROWS of its 8 M_p rows
-  std::vector<int4> items;
-  std::vector<int2> cit((size_t)B);
-  for (int b = 0; b < B; b++) {
-    const Prob &p = r->hprob[b];
-    const int nt = p.ldp / TILE, nrc = (int)((8 * p.nvox + ROWS - 1) / ROWS);
-    cit[b] = make_int2((int)items.size(), nrc);
-    for (int ti = 0; ti < nt; ti++)
-      for (int tj = ti; tj < nt; tj++)
-        for (int c = 0; c < nrc; c++) items.push_back(make_int4(b, ti, tj, c));
-  }
-  struct Scratch {  // device scratch of one call, freed on every exit path
-    std::vector<void *> p;
-    ~Scratch() { for (void *q : p) cudaFree(q); }
-  } pool;
-  auto get = [&](auto **out, size_t count) {
-    const int rc = dalloc(out, count);
-    if (rc == BALM_OK) pool.p.push_back((void *)*out);
-    return rc;
-  };
+  std::vector<int4> items;  // the covariance SYRK's: 8 rows per voxel
+  std::vector<int2> range;
+  syrk_items(r->hprob, 8, items, range);
+  ScratchPool pool;
   double *rows = nullptr, *Dobs = nullptr, *dpart = nullptr, *spart = nullptr, *raw = nullptr, *cov = nullptr,
          *ccov = nullptr;
   int4 *d_items = nullptr;
-  int2 *d_cit = nullptr;
+  int2 *d_range = nullptr;
   int *d_status = nullptr;
   const size_t n_rows = r->G_size / 3 * 8;
-  BTRY(get(&rows, n_rows));
-  BTRY(get(&Dobs, (size_t)r->K * 21));
-  BTRY(get(&dpart, (size_t)r->n_ochunks * 21 * 32));
-  BTRY(get(&spart, items.size() * TILE * TILE));
-  BTRY(get(&raw, r->H_size));
-  BTRY(get(&d_items, items.size()));
-  BTRY(get(&d_cit, (size_t)B));
+  TRY(pool.get(&rows, n_rows));
+  TRY(pool.get(&Dobs, (size_t)r->K * 21));
+  TRY(pool.get(&dpart, (size_t)r->n_ochunks * 21 * 32));
+  TRY(pool.get(&spart, items.size() * TILE * TILE));
+  TRY(pool.get(&raw, r->H_size));
+  TRY(pool.get(&d_items, items.size()));
+  TRY(pool.get(&d_range, (size_t)B));
   if (Rcov) {
-    BTRY(get(&cov, r->H_size));
-    BTRY(get(&d_status, (size_t)B));
+    TRY(pool.get(&cov, r->H_size));
+    TRY(pool.get(&d_status, (size_t)B));
   }
   if (c_cov81) {
-    BTRY(get(&ccov, (size_t)r->K * 81));
+    TRY(pool.get(&ccov, (size_t)r->K * 81));
     if (r->K) CUDA_TRY(cudaMemcpyAsync(ccov, c_cov81, sizeof(double) * 81 * r->K, cudaMemcpyHostToDevice, st));
   }
   if (!items.empty())
     CUDA_TRY(cudaMemcpyAsync(d_items, items.data(), sizeof(int4) * items.size(), cudaMemcpyHostToDevice, st));
-  CUDA_TRY(cudaMemcpyAsync(d_cit, cit.data(), sizeof(int2) * B, cudaMemcpyHostToDevice, st));
+  CUDA_TRY(cudaMemcpyAsync(d_range, range.data(), sizeof(int2) * B, cudaMemcpyHostToDevice, st));
   CUDA_TRY(cudaMemcpyAsync(r->poses, poses12, sizeof(double) * 12 * r->P, cudaMemcpyHostToDevice, st));
   const Dev d = r->dev();
   // the voxel statistics at these poses (fix clusters as include_fix): with Rcov, the evaluation of H computes them
-  if (Rcov) {
-    BTRY(enqueue_eval(bt, r, r->ones(), include_fix != 0));
-  } else if (r->M > 0) {
-    const int blocks = (int)std::min<int64_t>((r->M + 7) / 8, (int64_t)bt->sm_count * 8);
-    batch_stats_kernel<true><<<blocks, 256, 0, st>>>(d, r->poses, r->ones(), include_fix != 0 ? 1 : 0, r->stats, r->res_v);
-  }
+  if (Rcov) TRY(enqueue_eval(bt, r, r->ones(), include_fix != 0));
+  else enqueue_stats(bt, r, r->poses, r->ones(), include_fix != 0, r->stats);
   CUDA_TRY(cudaMemsetAsync(rows, 0, sizeof(double) * n_rows, st));  // columns of non-observing poses stay zero
   if (r->M > 0) {  // one CTA per voxel: a grid-stride loop would cost the kernel a spill
     batch_cov_rows_kernel<<<(unsigned)r->M, 32, COV_SMEM, st>>>(d, r->poses, r->stats, ccov, point_noise * point_noise, rows,
@@ -1231,7 +1182,8 @@ extern "C" int balm_batch_pose_covariance(balm_batch *bt, const double *poses12,
     batch_cov_diag_kernel<<<(r->n_ochunks + 3) / 4, 128, 0, st>>>(d, r->ochunk_prob, r->n_ochunks, Dobs, dpart);
   if (!items.empty())
     batch_syrk_kernel<8, 4><<<(unsigned)items.size(), 128, 0, st>>>(r->prob, r->ones(), d_items, rows, spart);
-  batch_cov_assemble_kernel<<<dim3(B, MAXN / TILE), 256, 0, st>>>(r->prob, d_cit, dpart, spart, raw);
+  batch_assemble_kernel<21, 0, false, false><<<dim3(B, MAXN / TILE), 256, 0, st>>>(r->prob, r->ones(), d_range, dpart,
+                                                                                    spart, raw, nullptr);
   if (Rcov) batch_cov_solve_kernel<<<B, SOLVE_THREADS, SOLVE_SMEM, st>>>(r->prob, r->H, raw, cov, d_status);
   CUDA_TRY(cudaGetLastError());
   if (Rcov_raw) CUDA_TRY(cudaMemcpyAsync(Rcov_raw, raw, sizeof(double) * r->H_size, cudaMemcpyDeviceToHost, st));

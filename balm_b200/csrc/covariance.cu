@@ -23,8 +23,6 @@
 #include <vector>
 #include "internal.cuh"
 
-#define CTRY(x) do { int _s = (x); if (_s != BALM_OK) return _s; } while (0)
-
 int launch_syrk_f64_on(balm_ctx *c, const double *G, int64_t rows, bool first_batch, int row_xor);
 
 namespace {
@@ -118,30 +116,6 @@ __global__ void cov_diag_reduce_kernel(const double *Dobs, int N, int64_t M, int
     for (int t = csc_lo[p]; t < csc_hi[p]; t++) s += Dobs[(size_t)csc_obs[t] * 21 + q];
   }
   Dacc[(size_t)q * N + p] = add ? Dacc[(size_t)q * N + p] + s : s;
-}
-
-// Rcov_raw = + sum_splits S + blockdiag(D), mirrored (the Hessian assembly with the opposite sign and no gradient)
-__global__ void __launch_bounds__(1024) cov_assemble_kernel(const double *part, int splits, int tiles, int nb, const double *Dacc,
-                                                            int N, int n, double *R) {
-  constexpr int TILE = BALM_SYRK_TILE;
-  const int bx = blockIdx.x, by = blockIdx.y;
-  if (by < bx) return;
-  const int tx = threadIdx.x, ty = threadIdx.y;
-  const int r = bx * 32 + ty, c = by * 32 + tx;
-  if (r >= n || c >= n) return;
-  const int rr = r < c ? r : c, cc = r < c ? c : r;
-  const int bi = rr / TILE, bj = cc / TILE;
-  const int t = bi * nb - bi * (bi - 1) / 2 + (bj - bi);
-  const size_t off = (size_t)t * (TILE * TILE) + (size_t)(rr % TILE) * TILE + (cc % TILE);
-  double s = 0.0;
-  for (int sp = 0; sp < splits; sp++) s += part[(size_t)sp * tiles * (TILE * TILE) + off];
-  if (rr / 6 == cc / 6) {
-    const int r6 = rr % 6, c6 = cc % 6;
-    const int q = r6 * 6 - r6 * (r6 - 1) / 2 + (c6 - r6);
-    s += Dacc[(size_t)q * N + rr / 6];
-  }
-  R[(size_t)r * n + c] = s;
-  R[(size_t)c * n + r] = s;
 }
 
 // ---- n right-hand sides through the LDL^T factors of the solve (A: L below the diagonal, Xinv: L_jj^-1, dinv) ----
@@ -270,16 +244,6 @@ int covariance_setup() {
   return BALM_OK;
 }
 
-struct DevPool {  // device scratch of one call, freed on every exit path
-  std::vector<void *> p;
-  ~DevPool() { for (void *q : p) cudaFree(q); }
-  template <typename T> int get(T **out, size_t count) {
-    CUDA_TRY(cudaMalloc((void **)out, sizeof(T) * (count ? count : 1)));
-    p.push_back((void *)*out);
-    return BALM_OK;
-  }
-};
-
 // Defined in balm_api.cu
 int balm_cov_evaluate_hessian(balm_ctx *c, const double *poses_dev, bool include_fix);
 
@@ -289,29 +253,29 @@ int pose_covariance_dev(balm_ctx *c, const double *poses_dev, const double *ccov
   const int64_t M = c->M, K = c->K;
   cudaStream_t st = c->stream;
   if (M < 1) { balm_set_error("balm_pose_covariance: no voxels registered"); return BALM_ERR_INVALID; }
-  DevPool pool;
+  ScratchPool pool;
   // voxels per batch: the stats table holds VB voxels; the row buffer gets its own budget
   size_t budget = (size_t)4 << 30;
   if (const char *e = getenv("BALM_COV_BUDGET_MB")) budget = (size_t)atoll(e) << 20;
   int64_t vb = std::min<int64_t>(c->VB, (int64_t)(budget / ((size_t)8 * c->ldg * sizeof(double))));
   vb = std::max<int64_t>(1, std::min<int64_t>(vb, M));
   double *G = nullptr, *Wz = nullptr, *Dobs = nullptr, *Dacc = nullptr, *R = nullptr, *ccov = nullptr;
-  CTRY(pool.get(&G, (size_t)8 * vb * c->ldg));
-  CTRY(pool.get(&Wz, (size_t)vb * 10));
-  CTRY(pool.get(&Dobs, (size_t)K * 21));
-  CTRY(pool.get(&Dacc, (size_t)21 * N));
-  CTRY(pool.get(&R, (size_t)n * n));
+  TRY(pool.get(&G, (size_t)8 * vb * c->ldg));
+  TRY(pool.get(&Wz, (size_t)vb * 10));
+  TRY(pool.get(&Dobs, (size_t)K * 21));
+  TRY(pool.get(&Dacc, (size_t)21 * N));
+  TRY(pool.get(&R, (size_t)n * n));
   if (ccov_host) {
-    CTRY(pool.get(&ccov, (size_t)K * 81));
+    TRY(pool.get(&ccov, (size_t)K * 81));
     CUDA_TRY(cudaMemcpyAsync(ccov, ccov_host, sizeof(double) * (size_t)K * 81, cudaMemcpyHostToDevice, st));
   }
   bool first = true;
   for (int64_t v0 = 0; v0 < M; v0 += vb) {
     const int64_t v1 = std::min(M, v0 + vb), nv = v1 - v0;
-    CTRY(launch_csc_batch(c, v0, v1));
+    TRY(launch_csc_batch(c, v0, v1));
     double *rdummy = c->scal + 21;
     CUDA_TRY(cudaMemsetAsync(rdummy, 0, sizeof(double), st));
-    CTRY(launch_voxel_stats(c, poses_dev, v0, v1, c->stats, include_fix, rdummy));
+    TRY(launch_voxel_stats(c, poses_dev, v0, v1, c->stats, include_fix, rdummy));
     CUDA_TRY(cudaMemsetAsync(G, 0, sizeof(double) * (size_t)8 * nv * c->ldg, st));
     CovArgs a{c->obs, c->Kp, c->pose_idx, c->row_ptr, poses_dev, c->stats, ccov, point_noise * point_noise, v0, v1, N,
               c->ldg, Wz, G, Dobs};
@@ -321,20 +285,16 @@ int pose_covariance_dev(balm_ctx *c, const double *poses_dev, const double *ccov
     cov_diag_reduce_kernel<<<N, 32, 0, st>>>(Dobs, N, M, c->dense ? 1 : 0, c->csc_ptr, c->csc_obs, Dacc, first ? 0 : 1, v0,
                                              v1, c->csc_lo, c->csc_hi);
     c->launches += 3;
-    CTRY(launch_syrk_f64_on(c, G, 8 * nv, first, /*row_xor=*/4));
+    TRY(launch_syrk_f64_on(c, G, 8 * nv, first, /*row_xor=*/4));
     first = false;
   }
-  CTRY(launch_csc_batch(c, 0, M));
-  const int nbb = (n + 31) / 32;
-  cov_assemble_kernel<<<dim3(nbb, nbb), dim3(32, 32), 0, st>>>(c->syrk_part, c->syrk_splits, c->syrk_tiles, c->syrk_nb, Dacc, N,
-                                                             n, R);
-  c->launches += 1;
-  CUDA_TRY(cudaGetLastError());
+  TRY(launch_csc_batch(c, 0, M));
+  TRY(launch_assemble(c, Dacc, R));
   if (Rraw_host) CUDA_TRY(cudaMemcpyAsync(Rraw_host, R, sizeof(double) * (size_t)n * n, cudaMemcpyDeviceToHost, st));
   if (Rcov_host) {
     // H at these poses (divide_thread, BAs_left.hpp:1091), factored without damping, then H^-1 R H^-T
-    CTRY(balm_cov_evaluate_hessian(c, poses_dev, include_fix));
-    CTRY(launch_ldlt_solve(c, 0.0));
+    TRY(balm_cov_evaluate_hessian(c, poses_dev, include_fix));
+    TRY(launch_ldlt_solve(c, 0.0));
     CUDA_TRY(cudaMemcpyAsync(c->h_flags, c->flags, sizeof(int), cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
     // a singular H (free gauge: no fix clusters in it) does not produce an exact zero pivot in floating point but
@@ -347,9 +307,9 @@ int pose_covariance_dev(balm_ctx *c, const double *poses_dev, const double *ccov
       balm_set_error("balm_pose_covariance: H is singular (gauge freedom not fixed: no fix clusters in the Hessian)");
       return BALM_ERR_NOT_PD;
     }
-    CTRY(solve_many(c, R));                                   // H^-1 R
+    TRY(solve_many(c, R));                                   // H^-1 R
     transpose_inplace_kernel<<<dim3((n + 31) / 32, (n + 31) / 32), dim3(32, 32), 0, st>>>(R, n);
-    CTRY(solve_many(c, R));                                   // H^-1 (H^-1 R)^T = H^-1 R H^-T
+    TRY(solve_many(c, R));                                   // H^-1 (H^-1 R)^T = H^-1 R H^-T
     c->launches += 1;
     CUDA_TRY(cudaMemcpyAsync(Rcov_host, R, sizeof(double) * (size_t)n * n, cudaMemcpyDeviceToHost, st));
   }

@@ -5,6 +5,7 @@
 #include <stdio.h>
 #include <functional>
 #include <string>
+#include <vector>
 #include "../../include/balm_b200.h"
 
 #define BALM_SCAL_RCUR 16
@@ -33,6 +34,38 @@ void window_free(WindowState *w);
     }                                                                                         \
   } while (0)
 
+// ---------------- host helpers ----------------
+// returns the status of x from the calling function unless it is BALM_OK
+#define TRY(x)                      \
+  do {                              \
+    const int _s = (x);             \
+    if (_s != BALM_OK) return _s;   \
+  } while (0)
+
+template <typename T>
+int dev_alloc(T **p, size_t count) {  // count elements of T (at least one, so that the pointer is never null)
+  CUDA_TRY(cudaMalloc((void **)p, sizeof(T) * (count ? count : 1)));
+  return BALM_OK;
+}
+
+// Device scratch of one call: every buffer taken from the pool is freed on ANY exit path (the early returns of TRY /
+// CUDA_TRY, a rejected registration, a bad frame index ...), so a failed call leaks nothing. drop frees one early.
+struct ScratchPool {
+  std::vector<void *> ptrs;
+  ~ScratchPool() { for (void *q : ptrs) cudaFree(q); }
+  template <typename T>
+  int get(T **p, size_t n) {
+    TRY(dev_alloc(p, n));
+    ptrs.push_back((void *)*p);
+    return BALM_OK;
+  }
+  void drop(void *q) {
+    if (!q) return;
+    for (size_t i = 0; i < ptrs.size(); i++)
+      if (ptrs[i] == q) { ptrs[i] = ptrs.back(); ptrs.pop_back(); break; }
+    cudaFree(q);
+  }
+};
 
 struct balm_ctx {
   int N = 0, n = 0, ldg = 0, Np = 0, device = 0, prec = 0;
@@ -631,7 +664,10 @@ int launch_obs_int8(balm_ctx *c, const double *poses, int64_t v0, int64_t v1, bo
                     const int *skip, int wpc = 4);
 int tensor_obs_and_syrk(balm_ctx *c, const double *poses, int64_t v0, int64_t v1, bool first_batch);
 int launch_syrk_f64(balm_ctx *c, int64_t rows, bool first_batch);
-int launch_assemble(balm_ctx *c);
+// Dacc null: the Hessian, H = -S + blockdiag(accum rows 6..26) and g, into c->H / c->g (or the all-reduce pack).
+// Else R = +S + blockdiag(Dacc), Dacc [21][N]: Rcov_raw of covariance.cu, whose rows always go through the fp64 SYRK.
+// S: the SYRK partials in c->syrk_part, summed over the splits in ascending order.
+int launch_assemble(balm_ctx *c, const double *Dacc = nullptr, double *R = nullptr);
 int build_pose_major_lists(balm_ctx *c, const int *planes_host);
 int launch_csc_batch(balm_ctx *c, int64_t v0, int64_t v1);
 int launch_ldlt_solve(balm_ctx *c, double u);

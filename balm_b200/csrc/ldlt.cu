@@ -13,7 +13,6 @@
 // A is column-major n x n; only the lower triangle is read/written. Panel width NB = 64.
 #include <stdlib.h>
 #include "internal.cuh"
-#define TRY_LAUNCH(x) do { int _s = (x); if (_s != BALM_OK) return _s; } while (0)
 
 namespace {
 
@@ -768,12 +767,12 @@ int refine_solution(balm_ctx *c, int *still_bad) {
       launches++;
     }
     c->launches += launches;
-    TRY_LAUNCH(enqueue_back_substitution(c, c->g, c->rdelta, false));
+    TRY(enqueue_back_substitution(c, c->g, c->rdelta, false));
     axpy_kernel<<<(n + 255) / 256, 256, 0, st>>>(c->dx, c->rdelta, n);
     q1_kernel<<<1, 1024, 0, st>>>(c->dx, c->g, c->dvec, n, c->scal + 3, c->scal);
     c->launches += 2;
     CUDA_TRY(cudaMemsetAsync(c->flags + 4, 0, sizeof(int), st));
-    TRY_LAUNCH(enqueue_solve_check(c));
+    TRY(enqueue_solve_check(c));
     CUDA_TRY(cudaMemcpyAsync(c->h_flags + 4, c->flags + 4, sizeof(int), cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaMemcpyAsync(c->h_scal + 1, c->scal + 1, sizeof(double), cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
@@ -851,8 +850,8 @@ int launch_ldlt_solve(balm_ctx *c, double u) {
   c->h_scal[3] = u;  // pinned; the kernels read the damping factor from device memory
   CUDA_TRY(cudaMemcpyAsync(c->scal + 3, c->h_scal + 3, sizeof(double), cudaMemcpyHostToDevice, c->stream));
   CUDA_TRY(cudaMemsetAsync(c->flags, 0, sizeof(int) * 8, c->stream));
-  TRY_LAUNCH(enqueue_solve_dag(c));
-  TRY_LAUNCH(enqueue_solve_check(c));
+  TRY(enqueue_solve_dag(c));
+  TRY(enqueue_solve_check(c));
   CUDA_TRY(cudaGetLastError());
   return BALM_OK;
 }

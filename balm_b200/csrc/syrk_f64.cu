@@ -141,18 +141,22 @@ __global__ void __launch_bounds__(SYRK_THREADS, 1) syrk_f64_kernel(SyrkArgs a) {
 struct AsmArgs {
   const double *part;
   int splits, tiles, nb;
-  const double *accum;  // [BALM_ACC][Np]
-  int N, Np, n;
+  const double *accum;  // [BALM_ACC][Np]: g and the exact diagonal (read only with g / exact_diag)
+  int Np, n;
+  const double *dblk;   // upper triangles of the 6x6 diagonal blocks, element q of pose i at dblk[q * ldd + i]
+  int ldd;
   int exact_diag;       // take the diagonal of G'^T G' from the fp64 sums of squares (tensor path)
   double *H;            // n x n
-  double *g;            // n
+  double *g;            // n, or null
   double *pack;         // multi-GPU: write the lower triangle | g straight into the all-reduce buffer instead of H (or null)
 };
 
-// H(i,j) = -sum_splits S(i,j) (+ D block on the diagonal); lower triangle mirrored from the upper tiles.
+// H(i,j) = -sum_splits S(i,j) (NEG, the Hessian) or +sum_splits S(i,j) (the covariance's Rcov_raw), splits in ascending
+// order, then + the D block on the diagonal; lower triangle mirrored from the upper tiles.
 // One CTA per 32x32 block of the upper triangle: the partial tiles are read coalesced (column index fastest), the
 // mirrored (lower) element is written straight away (coalesced in the same index) and the upper element goes through
 // a shared-memory transpose so that its column-major store is coalesced too.
+template <bool NEG>
 __global__ void __launch_bounds__(1024) assemble_kernel(AsmArgs a) {
   __shared__ double tile[32][33];
   const int bx = blockIdx.x, by = blockIdx.y;  // block row bx, block column by (by >= bx)
@@ -167,13 +171,13 @@ __global__ void __launch_bounds__(1024) assemble_kernel(AsmArgs a) {
     const size_t off = (size_t)t * (TILE * TILE) + (size_t)(rr % TILE) * TILE + (cc % TILE);
     double s = 0.0;
     for (int sp = 0; sp < a.splits; sp++) s += a.part[(size_t)sp * a.tiles * (TILE * TILE) + off];
-    h = -s;
+    h = NEG ? -s : s;
     const int pi = rr / 6, pj = cc / 6;
     if (a.exact_diag && rr == cc) h = -a.accum[(size_t)(27 + rr % 6) * a.Np + pi];
     if (pi == pj) {
       const int r6 = rr % 6, c6 = cc % 6;  // r6 <= c6
-      const int q = 6 + r6 * 6 - r6 * (r6 - 1) / 2 + (c6 - r6);
-      h += a.accum[(size_t)q * a.Np + pi];
+      const int q = r6 * 6 - r6 * (r6 - 1) / 2 + (c6 - r6);
+      h += a.dblk[(size_t)q * a.ldd + pi];
     }
     // element (row c, col r): the mirrored (lower) one, coalesced in c -- into H, or into column r of the packed triangle
     if (a.pack) { if (c >= r) a.pack[(size_t)r * a.n - (size_t)r * (r - 1) / 2 + (c - r)] = h; }
@@ -189,7 +193,7 @@ __global__ void __launch_bounds__(1024) assemble_kernel(AsmArgs a) {
     const int r2 = bx * 32 + tx, c2 = by * 32 + ty;
     if (r2 < a.n && c2 < a.n) a.H[(size_t)c2 * a.n + r2] = tile[tx][ty];
   }
-  if (bx == 0 && ty == 0 && c < a.n) a.g[c] = a.accum[(size_t)(c % 6) * a.Np + c / 6];
+  if (a.g && bx == 0 && ty == 0 && c < a.n) a.g[c] = a.accum[(size_t)(c % 6) * a.Np + c / 6];
 }
 
 }  // namespace
@@ -208,12 +212,18 @@ int launch_syrk_f64_on(balm_ctx *c, const double *G, int64_t rows, bool first_ba
   return BALM_OK;
 }
 
-int launch_assemble(balm_ctx *c) {
-  AsmArgs a{c->syrk_part, c->syrk_splits, c->syrk_tiles, c->syrk_nb, c->accum, c->N, c->Np, c->n,
-            c->prec == BALM_PREC_TENSOR ? 1 : 0, c->H, c->g, (c->world > 1 && c->comm) ? c->Hpack : nullptr};
+int launch_assemble(balm_ctx *c, const double *Dacc, double *R) {
   const int nbb = (c->n + 31) / 32;
   dim3 block(32, 32), grid(nbb, nbb);
-  assemble_kernel<<<grid, block, 0, c->stream>>>(a);
+  if (!Dacc) {
+    const AsmArgs a{c->syrk_part, c->syrk_splits, c->syrk_tiles, c->syrk_nb, c->accum, c->Np, c->n, c->accum + 6 * c->Np,
+                    c->Np, c->prec == BALM_PREC_TENSOR ? 1 : 0, c->H, c->g, (c->world > 1 && c->comm) ? c->Hpack : nullptr};
+    assemble_kernel<true><<<grid, block, 0, c->stream>>>(a);
+  } else {
+    const AsmArgs a{c->syrk_part, c->syrk_splits, c->syrk_tiles, c->syrk_nb, nullptr, c->Np, c->n, Dacc, c->N, 0, R,
+                    nullptr, nullptr};
+    assemble_kernel<false><<<grid, block, 0, c->stream>>>(a);
+  }
   c->launches += 1;
   CUDA_TRY(cudaGetLastError());
   return BALM_OK;
