@@ -295,9 +295,37 @@ class Batch:
         self._pose_ptr = pose_ptr
         return [(int(m), int(k)) for m, k in zip(M, K)]
 
-    def download_voxels(self, with_keys=False):
+    def marginalize(self, mg_sizes, poses_list, min_ps=15):
+        """Context.marginalize per problem, all in one call (include/balm_b200.h, balm_batch_marginalize): the oldest
+        mg_sizes[p] scans of problem p folded into its fix clusters at its poses; 0 leaves a problem unchanged. A problem
+        left without a voxel is registered empty. -> per problem (M, K)."""
+        mg = np.ascontiguousarray(mg_sizes, dtype=np.int32)
+        poses = self._concat(poses_list)
+        M = np.zeros(len(self.n_poses), dtype=np.int64)
+        K = np.zeros(len(self.n_poses), dtype=np.int64)
+        L.check(L.lib().balm_batch_marginalize(self._h, _p(mg), _p(poses), int(min_ps), _p(M), _p(K)))
+        return [(int(m), int(k)) for m, k in zip(M, K)]
+
+    def append_scans(self, scans, scan_of, slots, poses_list):
+        """Context.append_scan per problem, all in one call (include/balm_b200.h, balm_batch_append_scan). scans: list
+        of (n_s x 3) body-frame points, each uploaded once; scan_of[p]: the scan problem p takes in slot slots[p], or -1
+        (problem unchanged). Needs a registration from cut_scans. A problem left without voxels is registered empty,
+        with 0 points matched. -> per problem (M, K, points matched)."""
+        scans = [np.asarray(s, dtype=np.float32).reshape(-1, 3) for s in scans]
+        scan_ptr = np.concatenate([[0], np.cumsum([len(s) for s in scans])]).astype(np.int64)
+        xyz = np.ascontiguousarray(np.concatenate(scans) if scans else np.zeros((0, 3)), dtype=np.float32)
+        scan_of = np.ascontiguousarray(scan_of, dtype=np.int32)
+        slots = np.ascontiguousarray(slots, dtype=np.int32)
+        poses = self._concat(poses_list)
+        B = len(self.n_poses)
+        M, K, m = (np.zeros(B, dtype=np.int64) for _ in range(3))
+        L.check(L.lib().balm_batch_append_scan(self._h, _p(scan_of), _p(slots), len(scans), _p(scan_ptr), _p(xyz),
+                                               _p(poses), _p(M), _p(K), _p(m)))
+        return [(int(a), int(b), int(c)) for a, b, c in zip(M, K, m)]
+
+    def download_voxels(self, with_keys=False, with_fix=False):
         """The current registration, per problem a dict set_problems accepts (row_ptr re-based to 0); with_keys adds
-        keys and layers (only after cut_scans)."""
+        keys and layers (only after cut_scans), with_fix the fix clusters fix10 (zero rows where a voxel has none)."""
         B, P, M, K = C.c_int(), C.c_int64(), C.c_int64(), C.c_int64()
         L.check(L.lib().balm_batch_sizes(self._h, C.byref(B), C.byref(P), C.byref(M), C.byref(K)))
         voxel_ptr = np.zeros(B.value + 1, dtype=np.int64)
@@ -309,6 +337,10 @@ class Batch:
         layers = np.zeros(M.value, dtype=np.int32) if with_keys else None
         L.check(L.lib().balm_batch_download_voxels(self._h, _p(voxel_ptr), _p(row_ptr), _p(pose_idx), _p(obs10), _p(coe),
                                                    _p(keys), _p(layers)))
+        fix10 = None
+        if with_fix:
+            fix10 = np.zeros((M.value, 10))
+            L.check(L.lib().balm_batch_download_fix(self._h, _p(fix10)))
         out = []
         for b in range(B.value):
             v0, v1 = int(voxel_ptr[b]), int(voxel_ptr[b + 1])
@@ -317,6 +349,8 @@ class Batch:
                      pose_idx=pose_idx[s0:s1].copy(), obs10=obs10[s0:s1].copy(), coe=coe[v0:v1].copy())
             if with_keys:
                 d.update(keys=keys[v0:v1].copy(), layers=layers[v0:v1].copy())
+            if with_fix:
+                d.update(fix10=fix10[v0:v1].copy())
             out.append(d)
         return out
 

@@ -588,16 +588,68 @@ int launch_csc_batch(balm_ctx *c, int64_t v0, int64_t v1) {
 //   coe = number of points left, :42-44).
 // The flattened voxel set has no octree any more, so a leaf that is not pushed is dropped together with its fix cluster
 // (in the reference it stays in the map for later scans); documented in DESIGN.md.
+//
+// The per-voxel rules of marginalisation and of appending a scan are device functions shared by a context's kernels
+// (observations SoA [10][Kp], fix SoA [10][M]) and the batch's (balm_batch_marginalize / balm_batch_append_scan,
+// observations and fix AoS [n][10]): both run the same arithmetic in the same order, so a batch problem is bitwise what
+// a context holding it alone computes.
 namespace {
+struct Strided {  // column c of row s at p[c * cs + s * rs]; p may be null (a missing fix set reads as zeros)
+  const double *p;
+  int64_t cs, rs;
+  __device__ __forceinline__ double operator()(int64_t s, int c) const { return p ? p[c * cs + s * rs] : 0.0; }
+};
+__device__ __forceinline__ void add_world(double *f, const double *ob, const double *pose12) {
+  double r[9], t[3];
+  load_pose(pose12, r, t);
+  const WC w = world_cluster(ob, r, t);
+  f[0] += w.p00; f[1] += w.p01; f[2] += w.p02; f[3] += w.p11; f[4] += w.p12; f[5] += w.p22;
+  f[6] += w.v0; f[7] += w.v1; f[8] += w.v2; f[9] += w.n;
+}
+
+// keep rule of marginalisation (tras_opt / push_voxel after to_margi): the voxel's observations of slots >= mg must hold
+// at least min_ps points and come from at least two scans; *k = their number
+__device__ __forceinline__ int marg_keep(const long long *row_ptr, const int *pose_idx, Strided obs, int64_t v, int mg,
+                                         int min_ps, int *k) {
+  int n = 0;
+  double pts = 0.0;
+  for (long long s = row_ptr[v]; s < row_ptr[v + 1]; s++)
+    if (pose_idx[s] >= mg) { n++; pts += obs(s, 9); }
+  *k = n;
+  return ((int)pts >= min_ps && n >= 2) ? 1 : 0;
+}
+// to_margi on a kept voxel: observations of slots < mg folded into the fix cluster (written to fix_out[10]) unless it
+// already holds 50 points, the others moved to rows o.. with their slots shifted down by mg. Returns the points left.
+__device__ __forceinline__ double marg_emit(const long long *row_ptr, const int *pose_idx, Strided obs, Strided fix,
+                                            int64_t v, const double *poses, int mg, long long o, int *pose_idx_out,
+                                            double *obs10_out, double *fix_out) {
+  double f[10];
+  for (int c = 0; c < 10; c++) f[c] = fix(v, c);
+  const bool absorb = (int)f[9] < 50;  // fix_point.N < 50 (bavoxel.hpp:790; push_state == 1 for a registered plane leaf)
+  double pts = 0.0;
+  for (long long s = row_ptr[v]; s < row_ptr[v + 1]; s++) {
+    double ob[10];
+    for (int c = 0; c < 10; c++) ob[c] = obs(s, c);
+    const int p = pose_idx[s];
+    if (p < mg) {
+      if (absorb) add_world(f, ob, poses + 12 * p);  // fix_point += sig_tran[i]  (transform: tools.hpp:333-339)
+    } else {
+      for (int c = 0; c < 10; c++) obs10_out[o * 10 + c] = ob[c];
+      pose_idx_out[o] = p - mg;
+      pts += ob[9];
+      o++;
+    }
+  }
+  for (int c = 0; c < 10; c++) fix_out[c] = f[c];
+  return pts;
+}
+
 __global__ void marg_count_kernel(const long long *row_ptr, const int *pose_idx, const double *obs, int64_t Kp, int64_t M,
                                   int mg, int min_ps, int *keep, int *cnt) {
   const int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (v >= M) return;
   int k = 0;
-  double pts = 0.0;
-  for (long long s = row_ptr[v]; s < row_ptr[v + 1]; s++)
-    if (pose_idx[s] >= mg) { k++; pts += obs[9 * Kp + s]; }
-  const int kp = ((int)pts >= min_ps && k >= 2) ? 1 : 0;
+  const int kp = marg_keep(row_ptr, pose_idx, Strided{obs, Kp, 1}, v, mg, min_ps, &k);
   keep[v] = kp;
   cnt[v] = kp ? k : 0;
 }
@@ -612,33 +664,10 @@ __global__ void marg_emit_kernel(const long long *row_ptr, const int *pose_idx, 
   if (v >= M || !keep[v]) return;
   const int nv = vscan[v];
   if (key_in) { key_out[nv] = key_in[v]; layer_out[nv] = layer_in[v]; }
-  long long o = oscan[v];
+  const long long o = oscan[v];
   row_ptr_out[nv] = o;
-  double f[10];
-  for (int c = 0; c < 10; c++) f[c] = fix ? fix[c * M + v] : 0.0;
-  const bool absorb = (int)f[9] < 50;  // fix_point.N < 50 (bavoxel.hpp:790; push_state == 1 for a registered plane leaf)
-  double pts = 0.0;
-  for (long long s = row_ptr[v]; s < row_ptr[v + 1]; s++) {
-    double ob[10];
-    for (int c = 0; c < 10; c++) ob[c] = obs[c * Kp + s];
-    const int p = pose_idx[s];
-    if (p < mg) {
-      if (absorb) {  // fix_point += sig_tran[i]  (transform: tools.hpp:333-339)
-        double r[9], t[3];
-        load_pose(poses + 12 * p, r, t);
-        const WC w = world_cluster(ob, r, t);
-        f[0] += w.p00; f[1] += w.p01; f[2] += w.p02; f[3] += w.p11; f[4] += w.p12; f[5] += w.p22;
-        f[6] += w.v0; f[7] += w.v1; f[8] += w.v2; f[9] += w.n;
-      }
-    } else {
-      for (int c = 0; c < 10; c++) obs10_out[o * 10 + c] = ob[c];
-      pose_idx_out[o] = p - mg;
-      pts += ob[9];
-      o++;
-    }
-  }
-  for (int c = 0; c < 10; c++) fix10_out[(size_t)nv * 10 + c] = f[c];
-  coe_out[nv] = pts;
+  coe_out[nv] = marg_emit(row_ptr, pose_idx, Strided{obs, Kp, 1}, Strided{fix, M, 1}, v, poses, mg, o, pose_idx_out,
+                          obs10_out, fix10_out + (size_t)nv * 10);
 }
 }  // namespace
 
@@ -717,11 +746,9 @@ int marginalize_build(balm_ctx *c, int mg, const double *poses_dev, int min_ps, 
 // roots / new leaves from points that fall outside the existing planes, and re-splitting a leaf that stopped being planar
 // -- both appear at the next full balm_cut_voxels.
 namespace {
-__global__ void append_match_kernel(const float *xyz, const double *pose12, int64_t n, AssocParams p,
-                                    const unsigned long long *vox_key, const int *vox_layer, int M, unsigned *vid1,
-                                    int *bad) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
+// the registered voxel (index into keys[0 .. n), ascending) a body-frame point falls into at pose12, or -1
+__device__ __forceinline__ int append_match(const float *xyz, int64_t i, const double *pose12, const AssocParams &p,
+                                            const unsigned long long *vox_key, const int *vox_layer, int n) {
   double r[9], t[3];
   load_pose(pose12, r, t);
   const double b[3] = {(double)xyz[3 * i], (double)xyz[3 * i + 1], (double)xyz[3 * i + 2]};
@@ -729,62 +756,51 @@ __global__ void append_match_kernel(const float *xyz, const double *pose12, int6
 #pragma unroll
   for (int a = 0; a < 3; a++) w[a] = r[a * 3] * b[0] + r[a * 3 + 1] * b[1] + r[a * 3 + 2] * b[2] + t[a];
   int dummy = 0;
-  (void)bad;
   const unsigned long long k = world_point_key(w, p, &dummy);
   // a key digit 7 means "not split" AND is octant 7, so a hit only counts when the voxel's layer agrees
-  int v = find_key(vox_key, M, k | 63ull);            // a layer-0 leaf (the whole root voxel is one plane)
+  int v = find_key(vox_key, n, k | 63ull);            // a layer-0 leaf (the whole root voxel is one plane)
   if (v >= 0 && vox_layer[v] != 0) v = -1;
-  if (v < 0) { v = find_key(vox_key, M, k | 7ull); if (v >= 0 && vox_layer[v] != 1) v = -1; }   // a layer-1 leaf
-  if (v < 0) { v = find_key(vox_key, M, k); if (v >= 0 && vox_layer[v] != 2) v = -1; }          // a layer-2 leaf
-  vid1[i] = (unsigned)(v + 1);                        // 0 = the point falls into no registered plane voxel
+  if (v < 0) { v = find_key(vox_key, n, k | 7ull); if (v >= 0 && vox_layer[v] != 1) v = -1; }   // a layer-1 leaf
+  if (v < 0) { v = find_key(vox_key, n, k); if (v >= 0 && vox_layer[v] != 2) v = -1; }          // a layer-2 leaf
+  return v;
 }
-// one thread per voxel: the new scan's body-frame cluster (points in their original order)
-__global__ void append_cluster_kernel(const float *xyz, const unsigned *vid_sorted, const int *idx_sorted, int64_t n, int M,
-                                      double *newobs /*[M][10]*/) {
-  const int v = blockIdx.x * blockDim.x + threadIdx.x;
-  if (v >= M) return;
-  const unsigned want = (unsigned)(v + 1);
+// the new scan's body-frame cluster of the voxel whose points have id `want` in vid_sorted (stable-sorted, so the
+// points sum in their original order; pt_sorted: their indices into xyz)
+__device__ __forceinline__ void append_cluster(const float *xyz, const unsigned *vid_sorted, const int *pt_sorted,
+                                               int64_t n, unsigned want, double *out10) {
   int64_t lo = 0, hi = n;
   while (lo < hi) { const int64_t m = (lo + hi) >> 1; if (vid_sorted[m] < want) lo = m + 1; else hi = m; }
   double B[10] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
   for (int64_t i = lo; i < n && vid_sorted[i] == want; i++) {
-    const int j = idx_sorted[i];
+    const int64_t j = pt_sorted[i];  // 3 j overflows 32 bits beyond 715 827 882 points (a batch's scan pool)
     const double x = xyz[3 * j], y = xyz[3 * j + 1], z = xyz[3 * j + 2];
     B[0] += x * x; B[1] += x * y; B[2] += x * z; B[3] += y * y; B[4] += y * z; B[5] += z * z;
     B[6] += x; B[7] += y; B[8] += z; B[9] += 1.0;
   }
 #pragma unroll
-  for (int q = 0; q < 10; q++) newobs[(size_t)v * 10 + q] = B[q];
+  for (int q = 0; q < 10; q++) out10[q] = B[q];
 }
-// one thread per voxel: judge_eigen on fix + every window cluster (old ones and the new one) at the current poses
-__global__ void append_judge_kernel(const long long *row_ptr, const int *pose_idx, const double *obs, int64_t Kp,
-                                    const double *fix, int64_t M, const double *poses, const double *newobs, int slot,
-                                    const int *vox_layer, AssocParams p, int *keep, int *cnt, int *bad) {
-  const int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (v >= M) return;
+// recut's re-judgement of a voxel: judge_eigen on fix + every window cluster (old ones and the new one nb) at the
+// current poses; keep iff planar, more than min_ps window points and at least two scans (*k of them). *slot_bad: a scan
+// already in the voxel does not lie below `slot`.
+__device__ __forceinline__ int append_judge(const long long *row_ptr, const int *pose_idx, Strided obs, Strided fix,
+                                            int64_t v, const double *poses, const double *nb, int slot, int layer,
+                                            const AssocParams &p, int *k_out, bool *slot_bad) {
   double W[10];
-  for (int q = 0; q < 10; q++) W[q] = fix ? fix[q * M + v] : 0.0;
+  for (int q = 0; q < 10; q++) W[q] = fix(v, q);
   double pts = 0.0;
   int k = 0;
+  bool bad = false;
   for (long long s = row_ptr[v]; s < row_ptr[v + 1]; s++) {
     double ob[10];
-    for (int q = 0; q < 10; q++) ob[q] = obs[q * Kp + s];
-    double r[9], t[3];
-    load_pose(poses + 12 * pose_idx[s], r, t);
-    const WC w = world_cluster(ob, r, t);
-    W[0] += w.p00; W[1] += w.p01; W[2] += w.p02; W[3] += w.p11; W[4] += w.p12; W[5] += w.p22;
-    W[6] += w.v0; W[7] += w.v1; W[8] += w.v2; W[9] += w.n;
+    for (int q = 0; q < 10; q++) ob[q] = obs(s, q);
+    add_world(W, ob, poses + 12 * pose_idx[s]);
     pts += ob[9];
     k++;
-    if (pose_idx[s] >= slot) atomicOr(bad, 1);  // the new scan must take a slot above every scan already in the voxel
+    bad |= pose_idx[s] >= slot;  // the new scan must take a slot above every scan already in the voxel
   }
-  const double *nb = newobs + (size_t)v * 10;
   if (nb[9] > 0.0) {
-    double r[9], t[3];
-    load_pose(poses + 12 * slot, r, t);
-    const WC w = world_cluster(nb, r, t);
-    W[0] += w.p00; W[1] += w.p01; W[2] += w.p02; W[3] += w.p11; W[4] += w.p12; W[5] += w.p22;
-    W[6] += w.v0; W[7] += w.v1; W[8] += w.v2; W[9] += w.n;
+    add_world(W, nb, poses + 12 * slot);
     pts += nb[9];
     k++;
   }
@@ -793,9 +809,53 @@ __global__ void append_judge_kernel(const long long *row_ptr, const int *pose_id
   double lam[3], u0[3], u1[3], u2[3];
   eig3_jacobi(W[0] * inv - c0 * c0, W[1] * inv - c0 * c1, W[2] * inv - c0 * c2, W[3] * inv - c1 * c1,
               W[4] * inv - c1 * c2, W[5] * inv - c2 * c2, lam, u0, u1, u2);
-  const int layer = vox_layer[v];
   const bool planar = lam[0] / lam[1] < p.eig[layer];                     // judge_eigen (:665,697)
-  const int kp = (planar && (int)pts > p.min_ps && k >= 2) ? 1 : 0;       // recut :755-757, push_voxel :37
+  *k_out = k;
+  *slot_bad = bad;
+  return (planar && (int)pts > p.min_ps && k >= 2) ? 1 : 0;              // recut :755-757, push_voxel :37
+}
+// a kept voxel with its new observation nb (if any points) in slot `slot`, from row o on; fix row copied (unless fix_out
+// is null), coe grown
+__device__ __forceinline__ void append_emit(const long long *row_ptr, const int *pose_idx, Strided obs, Strided fix,
+                                            const double *coe, int64_t v, const double *nb, int slot, long long o,
+                                            int *pose_idx_out, double *obs10_out, double *fix_out, double *coe_out) {
+  for (long long s = row_ptr[v]; s < row_ptr[v + 1]; s++, o++) {
+    for (int q = 0; q < 10; q++) obs10_out[o * 10 + q] = obs(s, q);
+    pose_idx_out[o] = pose_idx[s];
+  }
+  if (nb[9] > 0.0) {
+    for (int q = 0; q < 10; q++) obs10_out[o * 10 + q] = nb[q];
+    pose_idx_out[o] = slot;
+  }
+  if (fix_out)
+    for (int q = 0; q < 10; q++) fix_out[q] = fix(v, q);
+  *coe_out = coe[v] + nb[9];  // push_voxel: coe = sum of N over the window (:42-44)
+}
+
+__global__ void append_match_kernel(const float *xyz, const double *pose12, int64_t n, AssocParams p,
+                                    const unsigned long long *vox_key, const int *vox_layer, int M, unsigned *vid1) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  vid1[i] = (unsigned)(append_match(xyz, i, pose12, p, vox_key, vox_layer, M) + 1);  // 0 = in no registered voxel
+}
+// one thread per voxel: the new scan's body-frame cluster (points in their original order)
+__global__ void append_cluster_kernel(const float *xyz, const unsigned *vid_sorted, const int *idx_sorted, int64_t n, int M,
+                                      double *newobs /*[M][10]*/) {
+  const int v = blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= M) return;
+  append_cluster(xyz, vid_sorted, idx_sorted, n, (unsigned)(v + 1), newobs + (size_t)v * 10);
+}
+// one thread per voxel: judge_eigen on fix + every window cluster (old ones and the new one) at the current poses
+__global__ void append_judge_kernel(const long long *row_ptr, const int *pose_idx, const double *obs, int64_t Kp,
+                                    const double *fix, int64_t M, const double *poses, const double *newobs, int slot,
+                                    const int *vox_layer, AssocParams p, int *keep, int *cnt, int *bad) {
+  const int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= M) return;
+  int k = 0;
+  bool slot_bad = false;
+  const int kp = append_judge(row_ptr, pose_idx, Strided{obs, Kp, 1}, Strided{fix, M, 1}, v, poses,
+                              newobs + (size_t)v * 10, slot, vox_layer[v], p, &k, &slot_bad);
+  if (slot_bad) atomicOr(bad, 1);
   keep[v] = kp;
   cnt[v] = kp ? k : 0;
 }
@@ -809,21 +869,12 @@ __global__ void append_emit_kernel(const long long *row_ptr, const int *pose_idx
   if (v == 0) row_ptr_out[Mout] = Kout;
   if (v >= M || !keep[v]) return;
   const int nv = vscan[v];
-  long long o = oscan[v];
+  const long long o = oscan[v];
   row_ptr_out[nv] = o;
   key_out[nv] = key_in[v];
   layer_out[nv] = layer_in[v];
-  for (long long s = row_ptr[v]; s < row_ptr[v + 1]; s++, o++) {
-    for (int q = 0; q < 10; q++) obs10_out[o * 10 + q] = obs[q * Kp + s];
-    pose_idx_out[o] = pose_idx[s];
-  }
-  const double *nb = newobs + (size_t)v * 10;
-  if (nb[9] > 0.0) {
-    for (int q = 0; q < 10; q++) obs10_out[o * 10 + q] = nb[q];
-    pose_idx_out[o] = slot;
-  }
-  for (int q = 0; q < 10; q++) fix10_out[(size_t)nv * 10 + q] = fix ? fix[q * M + v] : 0.0;
-  coe_out[nv] = coe[v] + nb[9];  // push_voxel: coe = sum of N over the window (:42-44)
+  append_emit(row_ptr, pose_idx, Strided{obs, Kp, 1}, Strided{fix, M, 1}, coe, v, newobs + (size_t)v * 10, slot, o,
+              pose_idx_out, obs10_out, fix10_out + (size_t)nv * 10, coe_out + nv);
 }
 }  // namespace
 
@@ -846,7 +897,7 @@ int append_scan_build(balm_ctx *c, int64_t n, const float *xyz_h, const double *
   CUDA_TRY(cudaMemcpyAsync(xyz, xyz_h, sizeof(float) * 3 * n, cudaMemcpyHostToDevice, st));
   CUDA_TRY(cudaMemsetAsync(bad, 0, sizeof(int), st));
   const unsigned gp = (unsigned)((n + 255) / 256), gv = (unsigned)((M + 127) / 128);
-  append_match_kernel<<<gp, 256, 0, st>>>(xyz, poses_dev + 12 * slot, n, P, c->vox_key, c->vox_layer, (int)M, vid, bad);
+  append_match_kernel<<<gp, 256, 0, st>>>(xyz, poses_dev + 12 * slot, n, P, c->vox_key, c->vox_layer, (int)M, vid);
   iota_kernel<<<gp, 256, 0, st>>>(idx, n);
   int bits = 1;
   while ((1ll << bits) <= M) bits++;
@@ -895,6 +946,243 @@ int append_scan_build(balm_ctx *c, int64_t n, const float *xyz_h, const double *
   const bool any_fix = c->fix != nullptr;
   TRY(reg(c, Mout, (const int64_t *)rp, pi, ob, any_fix ? fx : nullptr, co, Kout));
   return install_keys(c, keys_out, layers_out, Mout, true);
+}
+
+
+// ---------------------------------------------------------------------------------------------------------------------
+// The same two steps for every problem of a batch in one call (balm_batch_marginalize / balm_batch_append_scan). One
+// thread per voxel of the whole registration finds its problem through vox_prob and runs the context's rule (the device
+// functions above) on the problem's poses, mg_size or slot; a problem whose argument is 0 (marginalise) or -1 (append)
+// keeps every voxel unchanged. Voxels are grouped by problem, so the global exclusive scans of the keep flags and of the
+// kept observation counts give every problem a contiguous range of the new registration, and batch_window_ptr_kernel
+// reads the per-problem offsets off them. Appending: the (problem, point) items of the new scans are expanded as the cut
+// expands its rows, every point is looked up among its own problem's keys only, and a stable radix sort by global voxel
+// id + 1 keeps the points of one voxel in scan order, so its new cluster sums as the context's does.
+namespace {
+__global__ void batch_marg_count_kernel(const long long *row_ptr, const int *pose_idx, const double *obs,
+                                        const int *vox_prob, int64_t M, const int *mg, int min_ps, int *keep, int *cnt) {
+  const int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= M) return;
+  const int m = mg[vox_prob[v]];
+  int k = (int)(row_ptr[v + 1] - row_ptr[v]), kp = 1;
+  if (m > 0) kp = marg_keep(row_ptr, pose_idx, Strided{obs, 1, 10}, v, m, min_ps, &k);
+  keep[v] = kp;
+  cnt[v] = kp ? k : 0;
+}
+__global__ void batch_marg_emit_kernel(const long long *row_ptr, const int *pose_idx, const double *obs, const double *fix,
+                                       const double *coe, const unsigned long long *key, const int *layer,
+                                       const int *vox_prob, int64_t M, const int *pose_base, const int *mg,
+                                       const double *poses, const int *keep, const int *vscan, const int *oscan,
+                                       WindowEmit out, int64_t Mout, int64_t Kout) {
+  const int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (v == 0) out.row_ptr[Mout] = Kout;
+  if (v >= M || !keep[v]) return;
+  const int b = vox_prob[v], m = mg[b], nv = vscan[v];
+  const long long o = oscan[v];
+  out.row_ptr[nv] = o;
+  if (key) { out.key[nv] = key[v]; out.layer[nv] = layer[v]; }
+  const double pts = marg_emit(row_ptr, pose_idx, Strided{obs, 1, 10}, Strided{fix, 1, 10}, v, poses + 12 * (size_t)pose_base[b],
+                               m, o, out.pose_idx, out.obs, out.fix + (size_t)nv * 10);
+  out.coe[nv] = m > 0 ? pts : coe[v];
+}
+__global__ void batch_append_match_kernel(const float *xyz, const int *src, const int *prob, int64_t n,
+                                          const double *poses, const long long *vptr, const int *pose_base,
+                                          const int *slot, AssocParams p, const unsigned long long *key,
+                                          const int *layer, unsigned *vid1) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int b = prob[i];
+  const long long v0 = vptr[b];
+  const int v = append_match(xyz, src[i], poses + 12 * (size_t)(pose_base[b] + slot[b]), p, key + v0, layer + v0,
+                             (int)(vptr[b + 1] - v0));
+  vid1[i] = v < 0 ? 0u : (unsigned)(v0 + v + 1);  // 0 = in no voxel of its problem
+}
+__global__ void batch_append_judge_kernel(const long long *row_ptr, const int *pose_idx, const double *obs,
+                                          const double *fix, const int *vox_prob, int64_t M, const int *pose_base,
+                                          const int *slot, const double *poses, const double *newobs, const int *layer,
+                                          AssocParams p, int *keep, int *cnt, int *bad) {
+  const int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= M) return;
+  const int b = vox_prob[v], s = slot[b];
+  int k = (int)(row_ptr[v + 1] - row_ptr[v]), kp = 1;
+  if (s >= 0) {
+    bool slot_bad = false;
+    kp = append_judge(row_ptr, pose_idx, Strided{obs, 1, 10}, Strided{fix, 1, 10}, v, poses + 12 * (size_t)pose_base[b],
+                      newobs + (size_t)v * 10, s, layer[v], p, &k, &slot_bad);
+    if (slot_bad) atomicMin(bad, b);  // the lowest such problem is reported
+  }
+  keep[v] = kp;
+  cnt[v] = kp ? k : 0;
+}
+__global__ void batch_append_emit_kernel(const long long *row_ptr, const int *pose_idx, const double *obs, const double *fix,
+                                         const double *coe, const unsigned long long *key, const int *layer,
+                                         const int *vox_prob, int64_t M, const int *slot, const double *newobs,
+                                         const int *keep, const int *vscan, const int *oscan, WindowEmit out,
+                                         int64_t Mout, int64_t Kout) {
+  const int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (v == 0) out.row_ptr[Mout] = Kout;
+  if (v >= M || !keep[v]) return;
+  const int nv = vscan[v];
+  const long long o = oscan[v];
+  out.row_ptr[nv] = o;
+  out.key[nv] = key[v];
+  out.layer[nv] = layer[v];
+  append_emit(row_ptr, pose_idx, Strided{obs, 1, 10}, Strided{fix, 1, 10}, coe, v, newobs + (size_t)v * 10,
+              slot[vox_prob[v]], o, out.pose_idx, out.obs, out.fix ? out.fix + (size_t)nv * 10 : nullptr, out.coe + nv);
+}
+// per problem b in [0, B]: its first voxel and first observation in the new registration ([0][B + 1], [1][B + 1]); with
+// vid_sorted, for b < B the points of its new scan that fell into one of its voxels ([2][B])
+__global__ void batch_window_ptr_kernel(const long long *vptr, int B, int64_t M, const int *keep, const int *vscan,
+                                        const int *cnt, const int *oscan, const unsigned *vid_sorted, int64_t n,
+                                        long long *out) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b > B) return;
+  const long long v0 = vptr[b];
+  out[b] = v0 < M ? vscan[v0] : (long long)vscan[M - 1] + keep[M - 1];
+  out[B + 1 + b] = v0 < M ? oscan[v0] : (long long)oscan[M - 1] + cnt[M - 1];
+  if (!vid_sorted || b == B) return;
+  int64_t lim[2];
+  for (int e = 0; e < 2; e++) {  // first point with vid >= v0 + 1, first with vid >= v1 + 1
+    const unsigned want = (unsigned)(vptr[b + e] + 1);
+    int64_t lo = 0, hi = n;
+    while (lo < hi) { const int64_t m = (lo + hi) >> 1; if (vid_sorted[m] < want) lo = m + 1; else hi = m; }
+    lim[e] = lo;
+  }
+  out[2 * (B + 1) + b] = lim[1] - lim[0];
+}
+
+// per-problem device table: voxel_ptr [B + 1], then (pose_base, arg) [2][B]; and the poses
+int window_tables(cudaStream_t st, ScratchPool &pool, const BatchVoxels &in, const int *arg, double **poses,
+                  long long **vptr, int **pinfo) {
+  const int B = in.B, P = (int)in.pose_ptr[B];
+  std::vector<int> h((size_t)2 * B);
+  for (int b = 0; b < B; b++) { h[b] = (int)in.pose_ptr[b]; h[(size_t)B + b] = arg[b]; }
+  TRY(pool.get(poses, (size_t)12 * P)); TRY(pool.get(vptr, (size_t)B + 1)); TRY(pool.get(pinfo, h.size()));
+  CUDA_TRY(cudaMemcpyAsync(*poses, in.poses12, sizeof(double) * 12 * P, cudaMemcpyHostToDevice, st));
+  CUDA_TRY(cudaMemcpyAsync(*vptr, in.voxel_ptr, sizeof(long long) * (B + 1), cudaMemcpyHostToDevice, st));
+  CUDA_TRY(cudaMemcpyAsync(*pinfo, h.data(), sizeof(int) * h.size(), cudaMemcpyHostToDevice, st));
+  return BALM_OK;
+}
+// with keep / cnt of the in.M voxels: their exclusive scans and the per-problem offsets (+ matched counts) on the host
+int window_offsets(cudaStream_t st, ScratchPool &pool, const BatchVoxels &in, const long long *vptr, const int *keep,
+                   const int *cnt, int *vscan, int *oscan, const unsigned *vid_sorted, int64_t n, int *bad,
+                   std::vector<long long> &h, int *h_bad) {
+  const int B = in.B;
+  size_t tb = 0;
+  cub::DeviceScan::ExclusiveSum(nullptr, tb, keep, vscan, (int)in.M, st);
+  char *tmp = nullptr;
+  long long *dptr = nullptr;
+  TRY(pool.get(&tmp, tb)); TRY(pool.get(&dptr, h.size()));
+  CUDA_TRY(cub::DeviceScan::ExclusiveSum(tmp, tb, keep, vscan, (int)in.M, st));
+  CUDA_TRY(cub::DeviceScan::ExclusiveSum(tmp, tb, cnt, oscan, (int)in.M, st));
+  batch_window_ptr_kernel<<<(B + 128) / 128, 128, 0, st>>>(vptr, B, in.M, keep, vscan, cnt, oscan, vid_sorted, n, dptr);
+  CUDA_TRY(cudaMemcpyAsync(h.data(), dptr, sizeof(long long) * h.size(), cudaMemcpyDeviceToHost, st));
+  if (bad) CUDA_TRY(cudaMemcpyAsync(h_bad, bad, sizeof(int), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  return BALM_OK;
+}
+}  // namespace
+
+int batch_marginalize_build(cudaStream_t st, const BatchVoxels &in, const int *mg_size, int min_ps,
+                            const WindowRegister &reg) {
+  const int B = in.B;
+  const int64_t M = in.M;
+  ScratchPool pool;
+  double *poses = nullptr;
+  long long *vptr = nullptr;
+  int *pinfo = nullptr, *keep = nullptr, *cnt = nullptr, *vscan = nullptr, *oscan = nullptr;
+  TRY(window_tables(st, pool, in, mg_size, &poses, &vptr, &pinfo));
+  std::vector<long long> h((size_t)2 * (B + 1), 0);  // new voxel_ptr [B + 1], obs_ptr [B + 1]
+  const unsigned gv = (unsigned)((M + 127) / 128);
+  if (M > 0) {
+    TRY(pool.get(&keep, (size_t)M)); TRY(pool.get(&cnt, (size_t)M)); TRY(pool.get(&vscan, (size_t)M)); TRY(pool.get(&oscan, (size_t)M));
+    batch_marg_count_kernel<<<gv, 128, 0, st>>>(in.row_ptr, in.pose_idx, in.obs, in.vox_prob, M, pinfo + B, min_ps, keep, cnt);
+    TRY(window_offsets(st, pool, in, vptr, keep, cnt, vscan, oscan, nullptr, 0, nullptr, h, nullptr));
+  }
+  WindowEmit out{};
+  TRY(reg(reinterpret_cast<const int64_t *>(h.data()), reinterpret_cast<const int64_t *>(h.data() + B + 1), &out));
+  if (M > 0)
+    batch_marg_emit_kernel<<<gv, 128, 0, st>>>(in.row_ptr, in.pose_idx, in.obs, in.fix, in.coe, in.key, in.layer,
+                                               in.vox_prob, M, pinfo, pinfo + B, poses, keep, vscan, oscan, out, h[B],
+                                               h[2 * (size_t)B + 1]);
+  else
+    CUDA_TRY(cudaMemsetAsync(out.row_ptr, 0, sizeof(long long), st));
+  CUDA_TRY(cudaGetLastError());
+  CUDA_TRY(cudaStreamSynchronize(st));
+  return BALM_OK;
+}
+
+int batch_append_build(cudaStream_t st, const BatchVoxels &in, const balm_assoc_opts &o, const int32_t *scan_of,
+                       const int *slot, const int64_t *scan_ptr, const float *xyz, int64_t n_points,
+                       const WindowRegister &reg, int64_t *n_matched) {
+  const int B = in.B;
+  const int64_t M = in.M;
+  ScratchPool pool;
+  AssocParams P{o.voxel_size, o.layer_limit, o.min_ps, {o.eigen_value_array[0], o.eigen_value_array[1], o.eigen_value_array[2]}};
+  std::vector<int> arg(B);
+  std::vector<long long> tab((size_t)2 * B + 1, 0);  // item_ptr [B + 1], then the first point of each problem's scan
+  for (int b = 0; b < B; b++) {
+    const int s = scan_of[b];
+    arg[b] = s >= 0 ? slot[b] : -1;
+    tab[b + 1] = tab[b] + (s >= 0 ? scan_ptr[s + 1] - scan_ptr[s] : 0);
+    tab[(size_t)B + 1 + b] = s >= 0 ? scan_ptr[s] : 0;
+  }
+  const int64_t n = tab[B];
+  double *poses = nullptr, *newobs = nullptr;
+  long long *vptr = nullptr, *dtab = nullptr;
+  int *pinfo = nullptr, *keep = nullptr, *cnt = nullptr, *vscan = nullptr, *oscan = nullptr, *bad = nullptr;
+  int *src = nullptr, *src2 = nullptr, *prob = nullptr;
+  unsigned *vid = nullptr, *vid2 = nullptr;
+  float *dxyz = nullptr;
+  TRY(window_tables(st, pool, in, arg.data(), &poses, &vptr, &pinfo));
+  std::vector<long long> h((size_t)3 * B + 2, 0);  // new voxel_ptr [B + 1], obs_ptr [B + 1], matched points [B]
+  int h_bad = 0x7f7f7f7f;
+  const unsigned gv = (unsigned)((M + 127) / 128);
+  if (M > 0) {
+    if (n > 0) {
+      TRY(pool.get(&dxyz, (size_t)3 * n_points)); TRY(pool.get(&dtab, tab.size()));
+      TRY(pool.get(&src, (size_t)n)); TRY(pool.get(&src2, (size_t)n)); TRY(pool.get(&prob, (size_t)n));
+      TRY(pool.get(&vid, (size_t)n)); TRY(pool.get(&vid2, (size_t)n));
+      CUDA_TRY(cudaMemcpyAsync(dxyz, xyz, sizeof(float) * 3 * n_points, cudaMemcpyHostToDevice, st));
+      CUDA_TRY(cudaMemcpyAsync(dtab, tab.data(), sizeof(long long) * tab.size(), cudaMemcpyHostToDevice, st));
+      expand_rows_kernel<<<B, 256, 0, st>>>(dtab, dtab + B + 1, src, prob);
+      batch_append_match_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(dxyz, src, prob, n, poses, vptr, pinfo,
+                                                                             pinfo + B, P, in.key, in.layer, vid);
+      int bits = 1;
+      while ((1ll << bits) <= M) bits++;
+      size_t tb = 0;
+      cub::DeviceRadixSort::SortPairs(nullptr, tb, vid, vid2, src, src2, (int)n, 0, bits, st);
+      char *tmp = nullptr;
+      TRY(pool.get(&tmp, tb));
+      CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, tb, vid, vid2, src, src2, (int)n, 0, bits, st));  // stable
+    }
+    TRY(pool.get(&newobs, (size_t)M * 10));
+    TRY(pool.get(&keep, (size_t)M)); TRY(pool.get(&cnt, (size_t)M)); TRY(pool.get(&vscan, (size_t)M)); TRY(pool.get(&oscan, (size_t)M));
+    TRY(pool.get(&bad, 1));
+    CUDA_TRY(cudaMemsetAsync(bad, 0x7f, sizeof(int), st));
+    append_cluster_kernel<<<gv, 128, 0, st>>>(dxyz, vid2, src2, n, (int)M, newobs);
+    batch_append_judge_kernel<<<gv, 128, 0, st>>>(in.row_ptr, in.pose_idx, in.obs, in.fix, in.vox_prob, M, pinfo,
+                                                  pinfo + B, poses, newobs, in.layer, P, keep, cnt, bad);
+    TRY(window_offsets(st, pool, in, vptr, keep, cnt, vscan, oscan, vid2, n, bad, h, &h_bad));
+  }
+  if (h_bad != 0x7f7f7f7f) {
+    balm_set_error("balm_batch_append_scan: problem " + std::to_string(h_bad) +
+                   ": `slot` must be above every scan already observing its voxels");
+    return BALM_ERR_INVALID;
+  }
+  WindowEmit out{};
+  TRY(reg(reinterpret_cast<const int64_t *>(h.data()), reinterpret_cast<const int64_t *>(h.data() + B + 1), &out));
+  if (M > 0)
+    batch_append_emit_kernel<<<gv, 128, 0, st>>>(in.row_ptr, in.pose_idx, in.obs, in.fix, in.coe, in.key, in.layer,
+                                                 in.vox_prob, M, pinfo + B, newobs, keep, vscan, oscan, out, h[B],
+                                                 h[2 * (size_t)B + 1]);
+  else
+    CUDA_TRY(cudaMemsetAsync(out.row_ptr, 0, sizeof(long long), st));
+  CUDA_TRY(cudaGetLastError());
+  CUDA_TRY(cudaStreamSynchronize(st));
+  // a problem left without voxels (where the context call fails) matched nothing that stays registered
+  for (int b = 0; b < B; b++) n_matched[b] = h[b + 1] > h[b] ? h[2 * (size_t)(B + 1) + b] : 0;
+  return BALM_OK;
 }
 
 

@@ -694,6 +694,7 @@ struct BatchReg {
   double *obs = nullptr, *fix = nullptr, *coe = nullptr;
   unsigned long long *key = nullptr;  // [M] octree keys and layers when the voxels were cut from scans, else null
   int *layer = nullptr;
+  balm_assoc_opts assoc{};            // with keys: the options of that cut (balm_batch_append_scan judges with them)
   double *G = nullptr, *stats = nullptr, *res_v = nullptr, *opart = nullptr, *spart = nullptr, *H = nullptr, *g = nullptr;
   double *poses = nullptr, *trial = nullptr;
   double *r_eval = nullptr, *r2 = nullptr, *r1 = nullptr, *q1 = nullptr, *u = nullptr, *v = nullptr;
@@ -1006,6 +1007,7 @@ extern "C" int balm_batch_cut_voxels(balm_batch *bt, int n_problems, const int64
     TRY(dev_alloc(&r->key, (size_t)M));
     TRY(dev_alloc(&r->layer, (size_t)M));
     *out = AssocEmit{r->obs, 1, 10, r->pose_idx, r->row_ptr, r->coe, r->key, r->layer};
+    r->assoc = o;
     obs_ptr.assign(optr, optr + n_problems + 1);
     return (int)BALM_OK;
   };
@@ -1018,6 +1020,130 @@ extern "C" int balm_batch_cut_voxels(balm_batch *bt, int n_problems, const int64
       if (n_obs_out) n_obs_out[b] = obs_ptr[b + 1] - obs_ptr[b];
     }
   return install(bt, r, rc);
+}
+
+// ---- sliding window (assoc.cu: batch_marginalize_build / batch_append_build) ----
+// The registration as those steps read it; pose_ptr / voxel_ptr receive the host tables it points into.
+static BatchVoxels window_input(const BatchReg *r, const double *poses12, std::vector<int64_t> &pose_ptr,
+                                std::vector<int64_t> &voxel_ptr) {
+  pose_ptr.resize((size_t)r->B + 1);
+  voxel_ptr.resize((size_t)r->B + 1);
+  for (int b = 0; b < r->B; b++) {
+    pose_ptr[b] = r->hprob[b].pose_base;
+    voxel_ptr[b] = r->hprob[b].vox_base;
+  }
+  pose_ptr[r->B] = r->P;
+  voxel_ptr[r->B] = r->M;
+  return BatchVoxels{r->B, r->M, r->K, pose_ptr.data(), voxel_ptr.data(), r->vox_prob, r->row_ptr, r->pose_idx,
+                     r->obs, r->fix, r->coe, r->key, r->layer, poses12};
+}
+
+// The new registration r of old's problems with the sizes the step found: layout, then the arrays it emits into (fix
+// clusters when `fix`, keys and layers when old has them, and old's association options).
+static int window_register(balm_batch *bt, const BatchReg *old, BatchReg *r, const int64_t *pose_ptr,
+                           const int64_t *voxel_ptr, const int64_t *obs_ptr, bool fix, WindowEmit *out) {
+  const int64_t M = voxel_ptr[old->B], K = obs_ptr[old->B];
+  TRY(reg_layout(bt, r, old->B, pose_ptr, voxel_ptr, K));
+  TRY(dev_alloc(&r->row_ptr, (size_t)M + 1));
+  TRY(dev_alloc(&r->pose_idx, (size_t)K));
+  TRY(dev_alloc(&r->obs, (size_t)K * 10));
+  TRY(dev_alloc(&r->coe, (size_t)M));
+  if (fix) TRY(dev_alloc(&r->fix, (size_t)M * 10));
+  if (old->key) {
+    TRY(dev_alloc(&r->key, (size_t)M));
+    TRY(dev_alloc(&r->layer, (size_t)M));
+  }
+  r->assoc = old->assoc;
+  *out = WindowEmit{r->row_ptr, r->pose_idx, r->obs, r->fix, r->coe, r->key, r->layer};
+  return BALM_OK;
+}
+
+extern "C" int balm_batch_marginalize(balm_batch *bt, const int *mg_size, const double *poses12, int min_ps,
+                                      int64_t *n_voxels_out, int64_t *n_obs_out) {
+  if (!bt || !mg_size || !poses12) return invalid("balm_batch_marginalize: bad arguments");
+  const BatchReg *old = bt->reg;
+  if (!old) return invalid("balm_batch_marginalize: no problems registered");
+  for (int b = 0; b < old->B; b++)
+    if (mg_size[b] < 0 || mg_size[b] >= old->hprob[b].np)
+      return invalid("balm_batch_marginalize: problem " + std::to_string(b) + ": mg_size must be 0 or in [1, N_p)");
+  CUDA_TRY(cudaSetDevice(bt->device));
+  CUDA_TRY(cudaStreamSynchronize(bt->stream));
+  std::vector<int64_t> pose_ptr, voxel_ptr, obs_ptr;
+  const BatchVoxels in = window_input(old, poses12, pose_ptr, voxel_ptr);
+  BatchReg *r = new BatchReg();
+  const WindowRegister reg = [&](const int64_t *vp, const int64_t *op, WindowEmit *out) {
+    obs_ptr.assign(op, op + old->B + 1);
+    return window_register(bt, old, r, pose_ptr.data(), vp, op, true, out);
+  };
+  int rc = batch_marginalize_build(bt->stream, in, mg_size, min_ps, reg);
+  if (rc == BALM_OK) rc = reg_finish(bt, r);
+  if (rc == BALM_OK)
+    for (int b = 0; b < old->B; b++) {
+      if (n_voxels_out) n_voxels_out[b] = r->hprob[b].nvox;
+      if (n_obs_out) n_obs_out[b] = obs_ptr[b + 1] - obs_ptr[b];
+    }
+  return install(bt, r, rc);
+}
+
+extern "C" int balm_batch_append_scan(balm_batch *bt, const int32_t *scan_of, const int *slot, int n_scans,
+                                      const int64_t *scan_ptr, const float *xyz, const double *poses12,
+                                      int64_t *n_voxels_out, int64_t *n_obs_out, int64_t *n_matched_out) {
+  if (!bt || !scan_of || !slot || !scan_ptr || !poses12 || n_scans < 1)
+    return invalid("balm_batch_append_scan: bad arguments");
+  const BatchReg *old = bt->reg;
+  if (!old) return invalid("balm_batch_append_scan: no problems registered");
+  if (!old->key) return invalid("balm_batch_append_scan: needs a registration from balm_batch_cut_voxels (octree keys)");
+  if (scan_ptr[0] != 0) return invalid("balm_batch_append_scan: scan_ptr[0] must be 0");
+  for (int s = 0; s < n_scans; s++)
+    if (scan_ptr[s + 1] < scan_ptr[s]) return invalid("balm_batch_append_scan: scan_ptr must be ascending");
+  int64_t n_items = 0;  // points replicated over the problems that take them
+  for (int b = 0; b < old->B; b++) {
+    const std::string w = "balm_batch_append_scan: problem " + std::to_string(b);
+    const int s = scan_of[b];
+    if (s == -1) continue;
+    if (s < 0 || s >= n_scans) return invalid(w + ": scan index outside [0, n_scans)");
+    if (slot[b] < 0 || slot[b] >= old->hprob[b].np) return invalid(w + ": slot outside [0, N_p)");
+    if (scan_ptr[s + 1] - scan_ptr[s] < 1) return invalid(w + ": empty scan");
+    n_items += scan_ptr[s + 1] - scan_ptr[s];
+  }
+  const int64_t n_points = scan_ptr[n_scans];
+  if (n_points > 0 && !xyz) return invalid("balm_batch_append_scan: bad arguments");
+  if (n_items >= ((int64_t)1 << 31) || n_points >= ((int64_t)1 << 31)) {
+    balm_set_error("balm_batch_append_scan: 2^31 or more points, counted once per problem that takes them (or in xyz)");
+    return BALM_ERR_UNSUPPORTED;
+  }
+  CUDA_TRY(cudaSetDevice(bt->device));
+  CUDA_TRY(cudaStreamSynchronize(bt->stream));
+  std::vector<int64_t> pose_ptr, voxel_ptr, obs_ptr, matched((size_t)old->B);
+  const BatchVoxels in = window_input(old, poses12, pose_ptr, voxel_ptr);
+  BatchReg *r = new BatchReg();
+  const WindowRegister reg = [&](const int64_t *vp, const int64_t *op, WindowEmit *out) {
+    obs_ptr.assign(op, op + old->B + 1);
+    return window_register(bt, old, r, pose_ptr.data(), vp, op, old->fix != nullptr, out);
+  };
+  int rc = batch_append_build(bt->stream, in, old->assoc, scan_of, slot, scan_ptr, xyz, n_points, reg, matched.data());
+  if (rc == BALM_OK) rc = reg_finish(bt, r);
+  if (rc == BALM_OK)
+    for (int b = 0; b < old->B; b++) {
+      if (n_voxels_out) n_voxels_out[b] = r->hprob[b].nvox;
+      if (n_obs_out) n_obs_out[b] = obs_ptr[b + 1] - obs_ptr[b];
+      if (n_matched_out) n_matched_out[b] = matched[b];
+    }
+  return install(bt, r, rc);
+}
+
+extern "C" int balm_batch_download_fix(balm_batch *bt, double *fix10) {
+  if (!bt || !fix10) return invalid("balm_batch_download_fix: bad arguments");
+  const BatchReg *r = bt->reg;
+  if (!r) return invalid("balm_batch_download_fix: no problems registered");
+  CUDA_TRY(cudaSetDevice(bt->device));
+  if (!r->fix) {
+    memset(fix10, 0, sizeof(double) * 10 * (size_t)r->M);
+    return BALM_OK;
+  }
+  if (r->M) CUDA_TRY(cudaMemcpyAsync(fix10, r->fix, sizeof(double) * 10 * r->M, cudaMemcpyDeviceToHost, bt->stream));
+  CUDA_TRY(cudaStreamSynchronize(bt->stream));
+  return BALM_OK;
 }
 
 extern "C" int balm_batch_sizes(balm_batch *bt, int *n_problems, int64_t *n_poses, int64_t *n_voxels, int64_t *n_obs) {

@@ -725,3 +725,42 @@ balm_assoc_opts resolve_assoc_opts(const balm_assoc_opts *opts);  // opts or the
 // opts: from resolve_assoc_opts, layer_limit in 0..2 (checked by the caller)
 int assoc_cut(cudaStream_t st, const AssocInput &in, const balm_assoc_opts &opts, const AssocRegister &reg,
               long long *launches);
+
+// The sliding-window steps of a batch (balm_batch_marginalize / balm_batch_append_scan). The registration they read:
+// problem p owns the pose rows [pose_ptr[p], pose_ptr[p+1]) and the voxels [voxel_ptr[p], voxel_ptr[p+1]) (host tables
+// [B + 1]); device arrays vox_prob [M], row_ptr [M + 1], pose_idx [K] (problem-local), obs [K][10], fix [M][10] or null,
+// coe [M], key / layer [M] (null: not carried; appending needs them). poses12: the host's P x 12 poses.
+struct BatchVoxels {
+  int B;
+  int64_t M, K;
+  const int64_t *pose_ptr, *voxel_ptr;
+  const int *vox_prob;
+  const long long *row_ptr;
+  const int *pose_idx;
+  const double *obs, *fix, *coe;
+  const unsigned long long *key;
+  const int *layer;
+  const double *poses12;
+};
+// Where the new registration is emitted (device arrays, AoS): row_ptr [M + 1], pose_idx / obs [K], fix / coe / key /
+// layer [M]; fix is always written by marginalisation, by appending only when the input has one; key / layer when the
+// input has them.
+struct WindowEmit {
+  long long *row_ptr;
+  int *pose_idx;
+  double *obs, *fix, *coe;
+  unsigned long long *key;
+  int *layer;
+};
+// Called once the sizes are known: per problem voxel_ptr / obs_ptr [B + 1] of the new registration. Allocates the
+// destination and fills *out, or returns an error that ends the call.
+using WindowRegister = std::function<int(const int64_t *voxel_ptr, const int64_t *obs_ptr, WindowEmit *out)>;
+// mg_size [B]: 0 (problem copied unchanged) or in [1, N_p) (checked by the caller)
+int batch_marginalize_build(cudaStream_t st, const BatchVoxels &in, const int *mg_size, int min_ps,
+                            const WindowRegister &reg);
+// scan_of [B] (-1: problem copied unchanged) and slot [B] checked by the caller; scan s = xyz[scan_ptr[s] ..
+// scan_ptr[s+1]) of n_points; n_matched [B]. BALM_ERR_INVALID names the lowest problem whose slot is not above every
+// scan already observing one of its voxels.
+int batch_append_build(cudaStream_t st, const BatchVoxels &in, const balm_assoc_opts &o, const int32_t *scan_of,
+                       const int *slot, const int64_t *scan_ptr, const float *xyz, int64_t n_points,
+                       const WindowRegister &reg, int64_t *n_matched);

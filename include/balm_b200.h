@@ -235,7 +235,7 @@ int balm_batch_damping_iter(balm_batch *b, double *poses12, const balm_lm_opts *
  * concatenated in slot order, frame = slot, and its pose rows (ascending node key; row_ptr, pose_idx = slot, obs10, coe,
  * keys, layers). opts as balm_cut_voxels (NULL: the defaults; eigen ratios rounded to float). A problem without a plane
  * voxel gets an empty voxel range; balm_batch_damping_iter then reports BALM_ERR_TOO_FEW_PLANES for it unless
- * min_planes_per_pose is 0. No fix clusters. A problem's result depends on nothing else in the batch; two calls are
+ * min_planes_per_pose is 0. No fix clusters (balm_batch_marginalize adds them). A problem's result depends on nothing else in the batch; two calls are
  * bitwise equal. Points are uploaded once; host synchronisations and allocations are a fixed number per octree layer,
  * whatever the number of problems. BALM_ERR_INVALID (the previous registration stays in place): the problem-table checks
  * of balm_batch_set_voxels, scan_ptr not starting at 0 or not ascending, a pose_scan entry outside [0, n_scans),
@@ -248,10 +248,44 @@ int balm_batch_cut_voxels(balm_batch *b, int n_problems, const int64_t *pose_ptr
 /* Sizes of the current registration, then a copy of it (any pointer may be NULL): voxel_ptr [B + 1], row_ptr [M + 1]
  * (over all voxels), pose_idx [K] (problem-local), obs10 [K x 10], coe [M]; keys / layers [M] as balm_download_keys, per
  * problem in ascending key, only after balm_batch_cut_voxels (non-NULL otherwise -> BALM_ERR_INVALID). Fix clusters
- * are not copied. No registration -> BALM_ERR_INVALID. */
+ * are not copied (balm_batch_download_fix below). No registration -> BALM_ERR_INVALID. */
 int balm_batch_sizes(balm_batch *b, int *n_problems, int64_t *n_poses, int64_t *n_voxels, int64_t *n_obs);
 int balm_batch_download_voxels(balm_batch *b, int64_t *voxel_ptr, int64_t *row_ptr, int32_t *pose_idx, double *obs10,
                                double *coe, uint64_t *keys, int32_t *layers);
+/* The sliding-window step for a batch (balm_marginalize + balm_append_scan per problem, all problems in one call each).
+ * poses12: P x 12, the problems' pose rows as balm_batch_damping_iter returns them (read only); N_p does not change.
+ * balm_batch_marginalize: problem p with mg_size[p] in [1, N_p) gets exactly what balm_marginalize(ctx_p, mg_size[p],
+ * its pose rows, min_ps) registers on a BALM_PREC_FP64 context holding only problem p: row_ptr, pose_idx shifted down by
+ * mg_size[p], obs10 moved (not recomputed), fix clusters (a fix cluster of 50 or more points absorbs nothing, :790), coe,
+ * and keys and layers compacted when the registration carries them. mg_size[p] == 0 leaves problem p bitwise untouched.
+ * Where the context call would fail (no voxel is left with two observing scans) or the problem has no voxels, the problem
+ * gets an empty voxel range (n_voxels_out[p] = 0). Afterwards the registration holds fix clusters for every voxel (zero
+ * rows for untouched problems that had none). n_voxels_out / n_obs_out: [B] or NULL.
+ * balm_batch_append_scan: scans are given once, as in balm_batch_cut_voxels (scan s = xyz[scan_ptr[s] .. scan_ptr[s+1]),
+ * float32, body frame); one scan may serve several problems. Problem p with scan_of[p] >= 0 gets exactly what
+ * balm_append_scan(ctx_p, that scan, its pose rows, slot[p]) registers: keys, layers, row_ptr, pose_idx, obs10, fix
+ * clusters (kept only if the registration has them), coe and n_matched_out[p]. scan_of[p] == -1 leaves problem p bitwise
+ * untouched. The registration must carry keys (balm_batch_cut_voxels, possibly followed by these two calls): the leaves
+ * are found and re-judged with the association options of that cut. Where the context call would fail (no plane voxel
+ * survives) the problem gets an empty voxel range and n_matched_out[p] = 0. n_voxels_out / n_obs_out / n_matched_out:
+ * [B] or NULL.
+ * Both: BALM_ERR_INVALID leaves the previous registration in place: no registration; mg_size outside {0} and [1, N_p);
+ * scan_of outside -1 and [0, n_scans); slot outside [0, N_p); an empty scan; scan_ptr not starting at 0 or not
+ * ascending; a registration without keys (append); a slot not above every scan already observing one of the problem's
+ * voxels (checked on the device; the message names the lowest such problem). BALM_ERR_UNSUPPORTED, before anything is
+ * allocated: 2^31 or more points, counted once per problem that takes them (or in xyz). A problem's result depends on
+ * nothing else in the batch; two calls are bitwise equal. Host waits and allocations are a fixed number per call,
+ * whatever B: 5 stream synchronisations in each call (entry, per-problem offsets, emission, and the registration's check
+ * and workspaces as in balm_batch_set_voxels), and about 40 (marginalise) or 50 (append) device allocations, most of
+ * them the new registration's arrays and workspaces.
+ * balm_batch_download_fix: the registration's fix clusters, M x 10 (zero rows where a voxel has none, all zero when the
+ * registration has no fix clusters). */
+int balm_batch_marginalize(balm_batch *b, const int *mg_size, const double *poses12, int min_ps, int64_t *n_voxels_out,
+                           int64_t *n_obs_out);
+int balm_batch_append_scan(balm_batch *b, const int32_t *scan_of, const int *slot, int n_scans, const int64_t *scan_ptr,
+                           const float *xyz, const double *poses12, int64_t *n_voxels_out, int64_t *n_obs_out,
+                           int64_t *n_matched_out);
+int balm_batch_download_fix(balm_batch *b, double *fix10);
 /* balm_pose_covariance per problem, all problems in one call: problem p's results are those of balm_pose_covariance on
  * a BALM_PREC_FP64 context holding only problem p, at its rows of poses12 (P x 12, read only). c_cov81: K x 81 in
  * registration order (the order of obs10), or NULL for isotropic point noise of standard deviation point_noise.
@@ -262,7 +296,8 @@ int balm_batch_download_voxels(balm_batch *b, int64_t *voxel_ptr, int64_t *row_p
  * or BALM_ERR_NOT_PD when H_p is singular under balm_pose_covariance's criterion (a zero / tiny / non-finite LDL^T pivot,
  * or min |d| <= 1e-11 max |d|): that problem's Rcov block is zero, its Rcov_raw block is still valid. A problem without
  * voxels has a zero Rcov_raw and BALM_ERR_NOT_PD. Registrations from balm_batch_cut_voxels have no fix clusters, so every
- * problem's H is singular (free gauge) and reports BALM_ERR_NOT_PD; their Rcov_raw is valid. With Rcov == NULL, H is
+ * problem's H is singular (free gauge) and reports BALM_ERR_NOT_PD; their Rcov_raw is valid. balm_batch_marginalize
+ * gives them fix clusters that anchor the gauge (include_fix = 1). With Rcov == NULL, H is
  * neither evaluated nor factored and every status is BALM_OK. The call returns BALM_OK when it ran, whatever the
  * statuses; BALM_ERR_INVALID without a registration. A problem's results do not depend on the rest of the batch; two
  * calls are bitwise equal. The host waits once. Device scratch allocated and freed by one call, in doubles:

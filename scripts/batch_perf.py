@@ -4,8 +4,8 @@ pose count and, for every window, set_voxels + damping_iter, on the fp64 and on 
 Workloads (HBA's bottom layer splits a trajectory into many short windows): (a) 256 windows x 10 poses x 1 000 planes,
 (b) 32 windows x 32 poses x 5 000 planes, and (c) one bottom layer from raw scans: 160 synthetic scans of 20 000
 points (assoc_ref.synthetic_scans, room 12), windows of 10 scans every 5 scans (31 windows), associated per window and as
-one batch (see run_from_scans), and (d) the pose covariance of the windows of (a) and (b) with fix clusters (see
-run_covariance). For (a) and (b) every window is generated on the GPU by Context.synth_virtual (its own seed) and
+one batch (see run_from_scans), (d) the pose covariance of the windows of (a) and (b) with fix clusters (see
+run_covariance), and (e) a Monte Carlo sliding window of 64 sequences (see run_sliding_window). For (a) and (b) every window is generated on the GPU by Context.synth_virtual (its own seed) and
 read back with download_voxels, so the batch and the loop run on the same host arrays. Two option sets: fixed work
 (force_hess, rel_tol < 0, 10 iterations: every LM iteration does the same work) and the defaults. The batch, the fp64 loop
 and the tensor loop alternate --repeats times in one process; every call ends in a device synchronisation, so a host clock
@@ -292,6 +292,103 @@ def run_from_scans(n_scans, pts_per_scan, room, repeats):
     return out
 
 
+def run_sliding_window(n_seq, window, mg, shifts, pts_per_scan, room):
+    """Workload (e), a Monte Carlo sliding window: n_seq independent sequences (assoc_ref.synthetic_scans, one seed
+    each), a window of `window` scans cut and optimised once, then `shifts` window shifts, each marginalising the mg
+    oldest scans, appending mg new ones, optimising with the fix clusters and propagating the pose covariance:
+    (i) a Context (fp64) per sequence, marginalize + mg x append_scan + damping_iter + pose_covariance;
+    (ii) one Batch doing the same calls for every sequence. Per shift, the context route marginalises and appends at the
+    poses of the batch route, so their registrations must be bitwise equal (checked after every shift, outside the
+    timed calls); each route then optimises and propagates on its own. Time per shift for each route."""
+    import assoc_ref
+    import scenes
+    import balm_b200
+    n_scans = window + mg * shifts
+    scans, windows, init, new_pose = [], [], [], []
+    for q in range(n_seq):
+        pts, frs, poses = assoc_ref.synthetic_scans(n_poses=n_scans, pts_per_scan=pts_per_scan, seed=100 + q, room=room)
+        p12 = scenes.pack_poses([r for r, _ in poses], [p for _, p in poses])
+        base = len(scans)
+        scans += [pts[frs == i].astype(np.float32) for i in range(n_scans)]
+        windows.append(list(range(base, base + window)))
+        init.append(p12[:window])
+        new_pose.append(p12)
+    kwc = dict(voxel_size=2.0, eigen_value_array=(1 / 16, 1 / 16, 1 / 9))
+    lm_kw = dict(gauge_mode=2, min_planes_per_pose=0)
+    cov_kw = dict(point_noise=0.01, include_fix=True)
+    batch = balm_b200.Batch(0)
+    batch.cut_scans(scans, windows, init, **kwc)
+    x_b = [r[1] for r in batch.damping_iter(init, **lm_kw)]
+    ctx = []
+    for win, x0 in zip(windows, init):
+        c = balm_b200.Context(window, 0, balm_b200.PREC_FP64)
+        c.cut_voxels(np.concatenate([scans[s] for s in win]),
+                     np.concatenate([np.full(len(scans[s]), k, dtype=np.int32) for k, s in enumerate(win)]), x0, **kwc)
+        c.damping_iter(x0, **lm_kw)
+        ctx.append(c)
+
+    def clock(f):
+        t0 = time.perf_counter()
+        r = f()
+        return r, 1e3 * (time.perf_counter() - t0)
+
+    parts = ("marginalize", "append", "lm", "cov")
+    ms = {"i_context": [], "ii_batch": []}
+    ms_part = {r: {k: [] for k in parts} for r in ms}  # per shift, the route's time in each kind of call
+    bitwise, dpose, dcov, statuses = True, 0.0, 0.0, set()
+    for k in range(shifts):
+        new = [[windows[q][0] + window + mg * k + j for q in range(n_seq)] for j in range(mg)]
+        shifted = [np.vstack([x[mg:], new_pose[q][window + mg * k:window + mg * (k + 1)]]) for q, x in enumerate(x_b)]
+        slots = [window - mg + j for j in range(mg)]
+        tb = dict.fromkeys(parts, 0.0)
+        _, tb["marginalize"] = clock(lambda: batch.marginalize([mg] * n_seq, x_b))
+        for j in range(mg):  # only the scans this call appends: sequence q takes scan q of the list
+            _, t = clock(lambda: batch.append_scans([scans[s] for s in new[j]], list(range(n_seq)), [slots[j]] * n_seq,
+                                                    shifted))
+            tb["append"] += t
+        reg = batch.download_voxels(with_keys=True, with_fix=True)  # for the check, not part of the route
+        lm, tb["lm"] = clock(lambda: batch.damping_iter(shifted, hess_includes_fix=True, **lm_kw))
+        cov, tb["cov"] = clock(lambda: batch.pose_covariance([r[1] for r in lm], **cov_kw))
+        tc = dict.fromkeys(parts, 0.0)
+        ref = []
+        for q, c in enumerate(ctx):
+            _, t = clock(lambda: c.marginalize(mg, x_b[q]))
+            tc["marginalize"] += t
+            for j in range(mg):
+                _, t = clock(lambda: c.append_scan(scans[new[j][q]], shifted[q], slots[j]))
+                tc["append"] += t
+            (p, _, _), t = clock(lambda: c.damping_iter(shifted[q], hess_includes_fix=True, **lm_kw))
+            tc["lm"] += t
+            (_, cv), t = clock(lambda: c.pose_covariance(p, **cov_kw))
+            tc["cov"] += t
+            ref.append((p, cv))
+        for route, tt in (("ii_batch", tb), ("i_context", tc)):
+            ms[route].append(sum(tt.values()))
+            for key in parts:
+                ms_part[route][key].append(tt[key])
+        for c, d in zip(ctx, reg):
+            rp, pi, ob, co = c.download_voxels()
+            keys, layers = c.download_keys(with_layers=True)
+            same = (np.array_equal(rp, d["row_ptr"]) and np.array_equal(pi, d["pose_idx"]) and
+                    np.array_equal(ob, d["obs10"]) and np.array_equal(co, d["coe"]) and
+                    np.array_equal(c.download_fix(), d["fix10"]) and np.array_equal(keys, d["keys"]) and
+                    np.array_equal(layers, d["layers"]))
+            bitwise = bitwise and same
+        for (st, p, _, _), (cst, _, cv), (pc, cvc) in zip(lm, cov, ref):
+            statuses.add(cst)
+            dpose = max(dpose, float(np.abs(p - pc).max()))
+            dcov = max(dcov, float(np.abs(cv - cvc).max() / np.abs(cvc).max()))
+        x_b = [r[1] for r in lm]
+    batch.close()
+    for c in ctx:
+        c.close()
+    return dict(sequences=n_seq, window=window, mg=mg, shifts=shifts, pts_per_scan=pts_per_scan, room=room, ms=ms,
+                ms_median_per_shift={k: float(np.median(v)) for k, v in ms.items()}, ms_per_call_kind=ms_part,
+                ms_per_call_kind_median={r: {k: float(np.median(v)) for k, v in d.items()} for r, d in ms_part.items()},
+                registrations_bitwise_equal=bool(bitwise), max_pose_diff_ii_vs_i=dpose,
+                max_rel_cov_diff_ii_vs_i=dcov, batch_cov_statuses=sorted(statuses))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--repeats", type=int, default=3)
@@ -303,6 +400,8 @@ def main():
     for w in a.workloads.split(","):
         if w == "c":
             res[w] = run_from_scans(160, 20000, 12.0, a.repeats)
+        elif w == "e":
+            res[w] = run_sliding_window(64, 10, 2, 5, 20000, 12.0)
         elif w == "d":
             res[w] = {k: run_covariance(k, *shapes[k][:3], a.repeats, shapes[k][3]) for k in ("a", "b")}
         else:

@@ -2,8 +2,9 @@
 tile-DAG factorisation with several 64-column steps (n = 240: chain + near/far workers), the sliding-window marginalisation, the pose-covariance propagation, a multi-batch sparse evaluation, the device
 association chain balm_cut_voxels -> balm_marginalize -> balm_append_scan (octree keys + layers), and a batch of
 independent problems (balm_batch_*: a dense one with fix clusters, a sparse one of 32 poses, an empty one), and a batch
-association of overlapping windows with one empty window (balm_batch_cut_voxels), and the batch pose covariance of
-an anchored, a free and an empty problem (balm_batch_pose_covariance)."""
+association of overlapping windows with one empty window (balm_batch_cut_voxels), the batch pose covariance of
+an anchored, a free and an empty problem (balm_batch_pose_covariance), and the batched marginalise + append of those
+windows, the empty one included (balm_batch_marginalize / balm_batch_append_scan)."""
 import os, sys
 import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -68,5 +69,11 @@ b = balm_b200.Batch(0)
 mk = b.cut_scans(scans, windows, [p12[w] for w in windows])
 res = b.damping_iter([p12[w] for w in windows], max_iter=2, min_planes_per_pose=0)
 print("batch cut", mk, "iters", [len(tr) for _, _, tr, _ in res], flush=True)
+# batch sliding window on that registration: marginalise the first two windows (the empty one untouched), then append
+# the shared scan 5 to both in the slot that frees
+x = [r[1] for r in res]
+mm = b.marginalize([1, 1, 0], x)
+ma = b.append_scans(scans, [5, 5, -1], [3, 3, 0], x)
+print("batch marginalise", mm, "append", ma, "fix rows", len(b.download_voxels(with_fix=True)[0]["fix10"]), flush=True)
 b.close()
 print("SANITIZE_DONE")
