@@ -12,19 +12,22 @@
 // result does not depend on tile order, k-splits or the number of GPUs.
 //
 // Kernel anatomy (syrk_tc_kernel; one CTA per SM, persistent over (tile, column half, k-split) items, 384 threads):
-//   warp 8   : TMA producer (warps 9-11 idle: registers go to the consumers by setmaxnreg) -- cp.async.bulk.tensor.3d of the S int8 planes of the A block (128 columns bi, 128B
-//              swizzle) and of the B half block (64 columns of bj, 64B swizzle), KS = 64 contraction rows per stage,
-//              into a 192 KB shared-memory ring of 4-8 stages (mbarrier full/empty)
-//   warps 0-7: consumers    -- mma.sync m16n8k32 s8 x s8 -> s32, a 4 x 2 grid of 32 x 32 warp tiles over the
-//              128 x 64 output half tile, S(S+1)/2 digit-pair products per k step into S register accumulators;
-//              then the epilogue: fp64 Horner combine, column scales, fp64 partial tile to global (same partial
-//              layout as the fp64 path -> same assemble kernel)
-// The register accumulators (S * 128 x 64 int32 = 128 registers per consumer thread at S = 4) are what bounds the
-// output tile to 128 x 64. The digit planes are stored MN-major (pose index contiguous, as the observation sweep
-// writes them coalesced) while the s8 MMA wants K-contiguous fragments, so every consumer thread reads 4 x 4 byte
-// blocks (four 32-bit loads from four contraction rows) and transposes them with byte permutes. Contraction rows and
-// output rows / columns are assigned to fragment positions such that the loads are free of bank conflicts under the
-// TMA swizzle; the epilogue maps fragment positions back (frag_row / frag_col below).
+//   warp 8    : TMA producer -- cp.async.bulk.tensor.3d of the S int8 planes of the A block (128 columns bi, 128B
+//               swizzle) and of the B half block (64 columns of bj, 64B swizzle), KS = 64 contraction rows per stage,
+//               into a 192 KB shared-memory ring of 3-6 stages (mbarrier full/empty)
+//   warps 9-11: B transposers -- copy the S B half planes of each landed stage into K-major core matrices beside it
+//               in the same stage (mbarrier tfull)
+//   warps 0-7 : consumers, two warpgroups of 64 output rows each -- wgmma m64n64k32 s8 x s8 -> s32 with A from
+//               registers and B from the K-major copy, S(S+1)/2 digit-pair products per k32 step into S register
+//               accumulators; then the epilogue: fp64 Horner combine, column scales, fp64 partial tile to global
+//               (same partial layout as the fp64 path -> same assemble kernel)
+// The register accumulators (S * 64 x 64 int32 per warpgroup = 128 registers per consumer thread at S = 4) are what
+// bounds the output tile to 128 x 64. The digit planes are stored MN-major (pose index contiguous, as the observation
+// sweep writes them coalesced) while s8 wgmma reads shared-memory operands K-major only. So A is transposed on its way
+// into registers (ldmatrix.trans of 16-bit pairs, then byte permutes), once per plane and k32 step, and feeds all the
+// S - s products of its plane; B is transposed once per stage by the transposer warps. Both sides assign the same
+// contraction row to each k position of the MMA (the k position map below), so the integer sums are those of the plain
+// product, bit for bit.
 #include <cuda.h>
 #include <vector>
 #include <algorithm>
@@ -38,18 +41,22 @@ constexpr int SMAX = 4;               // digit planes
 constexpr int KS = 64;                // contraction rows per pipeline stage
 constexpr int A_PLANE_BYTES = KS * TILE;  // 8192: one plane of the A block, one stage (128-byte rows)
 constexpr int B_PLANE_BYTES = KS * HALF;  // 4096: one plane of the B half block, one stage (64-byte rows)
+constexpr int BT_PLANE_BYTES = KS * HALF; // 4096: the same plane K-major (wgmma core matrices, see bt_offset)
 constexpr int RING_BYTES = 196608;        // stage ring (the rest of the 227 KB per block is left to L1)
 constexpr int MAX_STAGES = 8;
-// a stage holds S planes of the A block and S planes of the B half block: 4 stages for S = 4, 5 for S = 3, 8 for S = 2
-__host__ __device__ constexpr int stage_bytes_for(int S) { return S * (A_PLANE_BYTES + B_PLANE_BYTES); }
+// a stage holds S planes of the A block, S planes of the B half block and their K-major copies:
+// 3 stages for S = 4, 4 for S = 3, 6 for S = 2
+__host__ __device__ constexpr int stage_bytes_for(int S) { return S * (A_PLANE_BYTES + B_PLANE_BYTES + BT_PLANE_BYTES); }
 __host__ __device__ constexpr int stages_for(int S) {
   return RING_BYTES / stage_bytes_for(S) > MAX_STAGES ? MAX_STAGES : RING_BYTES / stage_bytes_for(S);
 }
 constexpr int CONSUMER_WARPS = 8;
+constexpr int TRANSPOSE_WARPS = 3;                      // warps 9-11
 constexpr int TC_THREADS = 32 * (CONSUMER_WARPS + 4);   // two consumer warpgroups + one producer warpgroup
-// register split (setmaxnreg): the producer warpgroup gives registers up so the consumers can hold their accumulators;
-// 2 * 128 * 232 + 128 * 40 <= 65536
-constexpr int CONSUMER_REGS = 232, PRODUCER_REGS = 40;
+// register split (setmaxnreg): the producer warpgroup gives registers up so the consumers can hold their accumulators
+// (S * 32 + 2 * S * 4 A-fragment registers). The pool is what the launch allocated, 384 threads x 168 registers, and
+// setmaxnreg.inc waits until the registers are free: 2 * 128 * 224 + 128 * 56 <= 384 * 168
+constexpr int CONSUMER_REGS = 224, PRODUCER_REGS = 56;
 constexpr int TC_SMEM = RING_BYTES + 1024 + 256;        // ring + alignment slack + barriers
 constexpr int MAX_ROWS_PER_ITEM = 32576;                // S * rows * 2^14 < 2^31 with the 64-row rounding of the k-split
 
@@ -91,38 +98,71 @@ __device__ __forceinline__ void tma_load_3d(void *dst, const CUtensorMap *map, u
       : "memory");
 }
 
-__device__ __forceinline__ uint32_t lds32(const uint8_t *p) { return *reinterpret_cast<const uint32_t *>(p); }
+// Four 8 x 8 matrices of 16-bit pairs, transposed: lane 8q + i gives the address of row i of matrix q; thread
+// (g = lane/4, t = lane%4) receives in r[q] the pair g of row 2t (low half) and of row 2t + 1 (high half).
+__device__ __forceinline__ void ldsm_x4_trans(uint32_t addr, uint32_t *r) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];\n"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(addr)
+               : "memory");
+}
 
-__device__ __forceinline__ void mma_s8(int32_t *d, const uint32_t *a, const uint32_t *b) {
+// Contraction rows and k positions. A k32 step covers 32 contraction rows: four groups of 8, one ldmatrix matrix each.
+// Thread t's two rows 2t, 2t + 1 of groups q and q + 1 go to the four k positions 4t..4t+3 (q = 0) and 16+4t..16+4t+3
+// (q = 2) of the MMA: k position 16 h + 4 t + j holds contraction row 16 h + 2 t + (j & 1) + 8 (j >> 1). A (in
+// registers) and B (in the K-major copy) use the same map; as it is a bijection, the products are those of the plain
+// contraction.
+// From the ldmatrix.trans result of pairs (c, c + 1) at the rows of groups q, q + 1: the 4 k positions of column c
+// (0x6420, even bytes) or c + 1 (0x7531, odd bytes).
+constexpr uint32_t PERM_EVEN = 0x6420, PERM_ODD = 0x7531;
+
+// K-major copy of one B plane, one stage: wgmma core matrices of 8 columns x 16 k bytes (128 contiguous bytes,
+// no swizzle); k32 step c at c * 2048, column group n / 8 at (n / 8) * 256 (SBO), k half at 128 (LBO).
+constexpr int BT_LBO = 128, BT_SBO = 256, BT_CHUNK = 2048;
+__device__ __forceinline__ int bt_offset(int c, int n, int kword) {  // kword = k position / 4 in 0..7
+  return c * BT_CHUNK + (n >> 3) * BT_SBO + (kword >> 2) * BT_LBO + (n & 7) * 16 + 4 * (kword & 3);
+}
+__device__ __forceinline__ uint64_t bt_desc(uint32_t saddr) {  // wgmma matrix descriptor, no swizzle
+  return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)(BT_LBO >> 4) << 16) | ((uint64_t)(BT_SBO >> 4) << 32);
+}
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;\n" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator accesses across the asynchronous MMAs
+__device__ __forceinline__ void fence_acc(int32_t (&d)[32]) {
+#pragma unroll
+  for (int i = 0; i < 32; i++) asm volatile("" : "+r"(d[i])::"memory");
+}
+
+// D (64 x 64 s32, accumulated) += A (64 x 32 s8, registers) * B (32 x 64 s8, K-major shared memory)
+__device__ __forceinline__ void wgmma_s8(int32_t (&d)[32], const uint32_t (&a)[4], uint64_t desc_b) {
   asm volatile(
-      "mma.sync.aligned.m16n8k32.row.col.s32.s8.s8.s32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
-      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
+      "wgmma.mma_async.sync.aligned.m64n64k32.s32.s8.s8 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, {%32,%33,%34,%35}, %36, 1;\n"
+      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]),
+        "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]),
+        "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]),
+        "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b)
+      : "memory");
 }
 
-// 4 x 4 byte transpose: byte j of out[m] = byte m of in[j]
-__device__ __forceinline__ void transpose4x4(const uint32_t *in, uint32_t *out) {
-  const uint32_t t0 = __byte_perm(in[0], in[1], 0x5140), t1 = __byte_perm(in[2], in[3], 0x5140);
-  const uint32_t t2 = __byte_perm(in[0], in[1], 0x7362), t3 = __byte_perm(in[2], in[3], 0x7362);
-  out[0] = __byte_perm(t0, t1, 0x5410);
-  out[1] = __byte_perm(t0, t1, 0x7632);
-  out[2] = __byte_perm(t2, t3, 0x5410);
-  out[3] = __byte_perm(t2, t3, 0x7632);
+// true iff every thread of the calling warpgroup (named barrier id, 128 threads) passes ok = true
+__device__ __forceinline__ bool warpgroup_all(bool ok, int id) {
+  uint32_t r;
+  asm volatile(
+      "{\n\t.reg .pred p, q;\n\t"
+      "setp.ne.u32 p, %1, 0;\n\t"
+      "bar.red.and.pred q, %2, 128, p;\n\t"
+      "selp.u32 %0, 1, 0, q;\n\t}\n"
+      : "=r"(r)
+      : "r"((uint32_t)ok), "r"(id)
+      : "memory");
+  return r != 0;
 }
-
-// Fragment layout. In a k32 step, thread (g = lane/4, t = lane%4) holds the k indices 4t..4t+3 and 16+4t..16+4t+3 of
-// the MMA; they are mapped to the contraction rows t+4j and 16+t+4j (j = 0..3) of the 32-row chunk. The thread loads
-// 32-bit word wa (4 consecutive output rows) of the A block and word wb (4 consecutive columns) of the B half block at
-// those rows, both independent of t, so the four lanes of a fragment row / column see the same output index:
-//   A (128-byte rows, 128B swizzle: 16-byte chunk q of row r sits at q ^ (r & 7)):  wa = 4 wm + (g & 3) + 16 (g >> 2)
-//   B ( 64-byte rows,  64B swizzle: 16-byte chunk q of row r sits at q ^ ((r >> 1) & 3)): wb = 4 wn + (g & 3) + 8 (g >> 2)
-// With these words the 32 lanes of every load hit 32 different banks.
-__device__ __forceinline__ int word_a(int wm, int g) { return 4 * wm + (g & 3) + 16 * (g >> 2); }
-__device__ __forceinline__ int word_b(int wn, int g) { return 4 * wn + (g & 3) + 8 * (g >> 2); }
-// MMA tile mt (0,1) of a warp: fragment row g -> output row 4 wa(g) + 2 mt, row g + 8 -> 4 wa(g) + 2 mt + 1;
-// MMA tile nt (0..3): fragment column c -> output column 4 wb(c) + nt of the half tile.
-__device__ __forceinline__ int frag_row(int wm, int g, int mt, int upper) { return 4 * word_a(wm, g) + 2 * mt + upper; }
-__device__ __forceinline__ int frag_col(int wn, int c, int nt) { return 4 * word_b(wn, c) + nt; }
 
 struct TcArgs {
   int64_t rows;       // contraction rows of this batch (3 per voxel)
@@ -161,114 +201,137 @@ __device__ __forceinline__ ItemInfo decode_item(const TcArgs &a, int work, int64
   return it;
 }
 
-// One consumer warp: 32 x 32 of the 128 x 64 half tile, all items of this CTA.
+// One consumer warpgroup (wg = 0, 1): output rows 64 wg .. 64 wg + 63 of the 128 x 64 half tile, all items of this
+// CTA. Warp w (0..7) holds the 16 rows of 16-byte chunk w of the A block: fragment row g is output row 16 w + 2 g,
+// fragment row g + 8 is output row 16 w + 2 g + 1; fragment column n is column n of the half tile.
 template <int S>
 __device__ __forceinline__ void consumer_loop(const TcArgs &a, uint8_t *stage_base, uint64_t *full_bar,
-                                              uint64_t *empty_bar, int n_items, int64_t per, int first, int stride) {
+                                              uint64_t *tfull_bar, uint64_t *empty_bar, int n_items, int64_t per,
+                                              int first, int stride) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int g = lane >> 2, t = lane & 3;
-  const int wm = warp & 3, wn = warp >> 2;
+  const int g = lane >> 2, t = lane & 3, i = lane & 7, wg = warp >> 2;
   constexpr int nst = stages_for(S), sbytes = stage_bytes_for(S);
-  // byte offsets inside one plane of rows t+4j (the +16 rows and the second k32 chunk add constants)
-  uint32_t offa[4], offb[4];
-  {
-    const int qa = word_a(wm, g) >> 2, qb = word_b(wn, g) >> 2;
-#pragma unroll
-    for (int j = 0; j < 4; j++) {
-      const int r = t + 4 * j;
-      offa[j] = r * TILE + ((qa ^ (r & 7)) << 4) + 4 * (g & 3);
-      offb[j] = r * HALF + ((qb ^ ((r >> 1) & 3)) << 4) + 4 * (g & 3);
-    }
-  }
+  const uint32_t ring = smem_u32(stage_base);
+  // ldmatrix row of this lane: contraction row 8 (lane / 8) + i of a k32 step, chunk `warp` under the 128B swizzle;
+  // the 8 rows of each matrix sit in 8 different chunks, so the loads are free of bank conflicts
+  const uint32_t lda = ring + ((lane >> 3) * 8 + i) * TILE + ((warp ^ i) << 4);
   const double inv256 = 1.0 / 256.0;
   int st = 0;
   uint32_t ph = 0;
   for (int item = first; item < n_items; item += stride) {
     const ItemInfo info = decode_item(a, item, per);
-    int32_t acc[S][2][4][4];
+    int32_t acc[S][32];
 #pragma unroll
     for (int d = 0; d < S; d++)
 #pragma unroll
-      for (int mt = 0; mt < 2; mt++)
-#pragma unroll
-        for (int nt = 0; nt < 4; nt++)
-#pragma unroll
-          for (int q = 0; q < 4; q++) acc[d][mt][nt][q] = 0;
+      for (int q = 0; q < 32; q++) acc[d][q] = 0;
+    uint32_t af[2][S][4];  // A fragments of every plane, one set per k32 step of a stage (the other may be in flight)
     bool alive = true;
+    int prev = -1;  // the stage whose MMAs may still be in flight
     for (int ks = 0; ks < info.nsteps; ks++) {
-      if (!__all_sync(0xffffffffu, mbar_wait(&full_bar[st], ph, a.err))) { alive = false; break; }  // the warp leaves together
-      const uint8_t *pa = stage_base + st * sbytes, *pb = pa + S * A_PLANE_BYTES;
+      const bool ok = mbar_wait(&full_bar[st], ph, a.err) && mbar_wait(&tfull_bar[st], ph, a.err);
+      if (!warpgroup_all(ok, 1 + wg)) { alive = false; break; }  // the warpgroup leaves together (wgmma is .aligned)
+      const uint32_t sa = lda + st * sbytes;
+      const uint64_t sdesc = bt_desc(ring + S * (A_PLANE_BYTES + B_PLANE_BYTES) + st * sbytes);
 #pragma unroll
       for (int c = 0; c < KS / 32; c++) {
-        uint32_t bf[S][4][2];  // B fragments of every plane: [plane][n tile][k half]
-#pragma unroll
-        for (int tt = 0; tt < S; tt++) {
-          uint32_t lo[4], hi[4], x[4];
-          const uint8_t *base = pb + tt * B_PLANE_BYTES + c * 32 * HALF;
-#pragma unroll
-          for (int j = 0; j < 4; j++) x[j] = lds32(base + offb[j]);
-          transpose4x4(x, lo);
-#pragma unroll
-          for (int j = 0; j < 4; j++) x[j] = lds32(base + 16 * HALF + offb[j]);
-          transpose4x4(x, hi);
-#pragma unroll
-          for (int nt = 0; nt < 4; nt++) { bf[tt][nt][0] = lo[nt]; bf[tt][nt][1] = hi[nt]; }
-        }
 #pragma unroll
         for (int s = 0; s < S; s++) {
-          uint32_t lo[4], hi[4], x[4];
-          const uint8_t *base = pa + s * A_PLANE_BYTES + c * 32 * TILE;
+          uint32_t m[4];
+          ldsm_x4_trans(sa + s * A_PLANE_BYTES + c * 32 * TILE, m);
+          af[c][s][0] = __byte_perm(m[0], m[1], PERM_EVEN);
+          af[c][s][1] = __byte_perm(m[0], m[1], PERM_ODD);
+          af[c][s][2] = __byte_perm(m[2], m[3], PERM_EVEN);
+          af[c][s][3] = __byte_perm(m[2], m[3], PERM_ODD);
+        }
+        wgmma_fence();
 #pragma unroll
-          for (int j = 0; j < 4; j++) x[j] = lds32(base + offa[j]);
-          transpose4x4(x, lo);
-#pragma unroll
-          for (int j = 0; j < 4; j++) x[j] = lds32(base + 16 * TILE + offa[j]);
-          transpose4x4(x, hi);
-          uint32_t af[2][4];
-#pragma unroll
-          for (int mt = 0; mt < 2; mt++) {
-            af[mt][0] = lo[2 * mt];
-            af[mt][1] = lo[2 * mt + 1];
-            af[mt][2] = hi[2 * mt];
-            af[mt][3] = hi[2 * mt + 1];
-          }
+        for (int s = 0; s < S; s++)
 #pragma unroll
           for (int tt = 0; tt + s < S; tt++)
-#pragma unroll
-            for (int mt = 0; mt < 2; mt++)
-#pragma unroll
-              for (int nt = 0; nt < 4; nt++) mma_s8(acc[s + tt][mt][nt], af[mt], bf[tt][nt]);
+            wgmma_s8(acc[s + tt], af[c][s], sdesc + ((tt * BT_PLANE_BYTES + c * BT_CHUNK) >> 4));
+        wgmma_commit();
+        // every group but this one has retired: after the first k32 step that frees the previous stage, after the
+        // second the A fragments of the first
+        wgmma_wait<1>();
+        if (c == 0 && prev >= 0) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&empty_bar[prev]);
         }
       }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&empty_bar[st]);  // this warp has read the stage
+      prev = st;
       if (++st == nst) { st = 0; ph ^= 1; }
     }
+    wgmma_wait<0>();
+#pragma unroll
+    for (int d = 0; d < S; d++) fence_acc(acc[d]);
     if (!alive) break;
+    if (prev >= 0) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[prev]);
+    }
     // ---- epilogue: Horner over the digit-pair order d = S-1 .. 0, column scales, fp64 partial tile ----
     double *tile_out = a.part + ((size_t)info.sp * a.tiles + info.t) * (TILE * TILE);
 #pragma unroll
-    for (int mt = 0; mt < 2; mt++) {
+    for (int up = 0; up < 2; up++) {
+      const int row = 16 * warp + 2 * g + up;
+      const double isc_row = __ldg(a.isc + info.bi * TILE + row);
+      double *out = tile_out + (size_t)row * TILE + info.h * HALF;
 #pragma unroll
-      for (int up = 0; up < 2; up++) {
-        const int row = frag_row(wm, g, mt, up);
-        const double isc_row = __ldg(a.isc + info.bi * TILE + row);
-        double *out = tile_out + (size_t)row * TILE + info.h * HALF;
+      for (int j = 0; j < HALF / 8; j++) {
 #pragma unroll
-        for (int nt = 0; nt < 4; nt++) {
+        for (int e = 0; e < 2; e++) {
+          const int q = 4 * j + 2 * up + e;
+          const int col = 8 * j + 2 * t + e;
+          double val = (double)acc[S - 1][q];
 #pragma unroll
-          for (int e = 0; e < 2; e++) {
-            const int q = 2 * up + e;
-            const int col = frag_col(wn, 2 * t + e, nt);
-            double val = (double)acc[S - 1][mt][nt][q];
-#pragma unroll
-            for (int d = S - 2; d >= 0; d--) val = val * inv256 + (double)acc[d][mt][nt][q];
-            double w = val * isc_row * __ldg(a.isc + info.bj * TILE + info.h * HALF + col);
-            if (a.accumulate) w += out[col];
-            out[col] = w;
-          }
+          for (int d = S - 2; d >= 0; d--) val = val * inv256 + (double)acc[d][q];
+          double w = val * isc_row * __ldg(a.isc + info.bj * TILE + info.h * HALF + col);
+          if (a.accumulate) w += out[col];
+          out[col] = w;
         }
       }
+    }
+  }
+}
+
+// One transposer warp (tw = 0..2): the K-major copies of the B half planes of every stage this CTA consumes. Work unit
+// u = (plane, k32 step c, 16-column chunk q) of a stage: one ldmatrix.trans of its 4 x 8 contraction rows gives thread
+// (g, t) the k positions 4t..4t+3 and 16+4t..16+4t+3 of columns 16 q + 2 g and 16 q + 2 g + 1.
+__device__ __forceinline__ void transpose_loop(const TcArgs &a, uint8_t *stage_base, uint64_t *full_bar,
+                                               uint64_t *tfull_bar, int S, int n_items, int64_t per, int first,
+                                               int stride, int tw) {
+  const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3, i = lane & 7;
+  const int nst = stages_for(S), sbytes = stage_bytes_for(S);
+  // source row of this lane: contraction row 8 (lane / 8) + i of a k32 step; 64-byte rows under the 64B swizzle
+  // (chunk q of row r at q ^ ((r >> 1) & 3)), so the 8 rows of each matrix hit 8 different 16-byte bank groups
+  const uint32_t src = smem_u32(stage_base) + S * A_PLANE_BYTES + ((lane >> 3) * 8 + i) * HALF;
+  uint8_t *dst = stage_base + S * (A_PLANE_BYTES + B_PLANE_BYTES);
+  // lanes g >= 4 store column 2g + 1 before 2g: the 32 lanes of every store then hit 32 different banks
+  const int flip = g >> 2;
+  const uint32_t perm0 = flip ? PERM_ODD : PERM_EVEN, perm1 = flip ? PERM_EVEN : PERM_ODD;
+  int st = 0;
+  uint32_t ph = 0;
+  bool alive = true;
+  for (int item = first; alive && item < n_items; item += stride) {
+    const ItemInfo info = decode_item(a, item, per);
+    for (int ks = 0; ks < info.nsteps; ks++) {
+      if (!__all_sync(0xffffffffu, mbar_wait(&full_bar[st], ph, a.err))) { alive = false; break; }
+      for (int u = tw; u < 8 * S; u += TRANSPOSE_WARPS) {
+        const int p = u >> 3, c = (u >> 2) & 1, q = u & 3;
+        uint32_t m[4];
+        ldsm_x4_trans(src + st * sbytes + p * B_PLANE_BYTES + c * 32 * HALF + ((q ^ (i >> 1)) << 4), m);
+        uint8_t *d = dst + st * sbytes + p * BT_PLANE_BYTES;
+        const int n0 = 16 * q + 2 * g + flip, n1 = n0 ^ 1;
+        *reinterpret_cast<uint32_t *>(d + bt_offset(c, n0, t)) = __byte_perm(m[0], m[1], perm0);
+        *reinterpret_cast<uint32_t *>(d + bt_offset(c, n1, t)) = __byte_perm(m[0], m[1], perm1);
+        *reinterpret_cast<uint32_t *>(d + bt_offset(c, n0, 4 + t)) = __byte_perm(m[2], m[3], perm0);
+        *reinterpret_cast<uint32_t *>(d + bt_offset(c, n1, 4 + t)) = __byte_perm(m[2], m[3], perm1);
+      }
+      asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");  // the copy is read by wgmma (async proxy)
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&tfull_bar[st]);
+      if (++st == nst) { st = 0; ph ^= 1; }
     }
   }
 }
@@ -280,12 +343,17 @@ __global__ void __launch_bounds__(TC_THREADS, 1) syrk_tc_kernel(const __grid_con
   uint8_t *stage_base = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t *full_bar = reinterpret_cast<uint64_t *>(stage_base + RING_BYTES);
   uint64_t *empty_bar = full_bar + MAX_STAGES;
+  uint64_t *tfull_bar = empty_bar + MAX_STAGES;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int S = *a.S_dev;
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < MAX_STAGES; i++) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], CONSUMER_WARPS); }
+    for (int i = 0; i < MAX_STAGES; i++) {
+      mbar_init(&full_bar[i], 1);
+      mbar_init(&empty_bar[i], CONSUMER_WARPS);
+      mbar_init(&tfull_bar[i], TRANSPOSE_WARPS);
+    }
     asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
   }
   __syncthreads();
@@ -295,9 +363,12 @@ __global__ void __launch_bounds__(TC_THREADS, 1) syrk_tc_kernel(const __grid_con
   const int64_t per = ((a.rows + a.splits - 1) / a.splits + KS - 1) / KS * KS;
 
   if (warp >= CONSUMER_WARPS) {
-    // ===================== TMA producer =====================
     asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;\n" ::"n"(PRODUCER_REGS));
-    if (warp == CONSUMER_WARPS && lane == 0) {
+    if (warp > CONSUMER_WARPS) {
+      // ===================== B transposers =====================
+      transpose_loop(a, stage_base, full_bar, tfull_bar, S, n_items, per, first, stride, warp - CONSUMER_WARPS - 1);
+    } else if (lane == 0) {
+      // ===================== TMA producer =====================
       asm volatile("prefetch.tensormap [%0];\n" ::"l"(&tmap_a) : "memory");
       asm volatile("prefetch.tensormap [%0];\n" ::"l"(&tmap_b) : "memory");
       const int nst = stages_for(S), sbytes = stage_bytes_for(S);
@@ -309,7 +380,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) syrk_tc_kernel(const __grid_con
         for (int ks = 0; ks < info.nsteps; ks++) {
           if (!mbar_wait(&empty_bar[st], ph ^ 1, a.err)) { alive = false; break; }
           uint8_t *sb = stage_base + st * sbytes;
-          mbar_expect_tx(&full_bar[st], sbytes);
+          mbar_expect_tx(&full_bar[st], S * (A_PLANE_BYTES + B_PLANE_BYTES));
           const int krow = (int)(info.k_begin + (int64_t)ks * KS);
           for (int s = 0; s < S; s++) {
             tma_load_3d(sb + s * A_PLANE_BYTES, &tmap_a, &full_bar[st], info.bi * TILE, krow, s);
@@ -321,11 +392,11 @@ __global__ void __launch_bounds__(TC_THREADS, 1) syrk_tc_kernel(const __grid_con
       }
     }
   } else {
-    // ===================== MMA + epilogue =====================
+    // ===================== wgmma + epilogue =====================
     asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;\n" ::"n"(CONSUMER_REGS));
-    if (S == 4) consumer_loop<4>(a, stage_base, full_bar, empty_bar, n_items, per, first, stride);
-    else if (S == 3) consumer_loop<3>(a, stage_base, full_bar, empty_bar, n_items, per, first, stride);
-    else consumer_loop<2>(a, stage_base, full_bar, empty_bar, n_items, per, first, stride);
+    if (S == 4) consumer_loop<4>(a, stage_base, full_bar, tfull_bar, empty_bar, n_items, per, first, stride);
+    else if (S == 3) consumer_loop<3>(a, stage_base, full_bar, tfull_bar, empty_bar, n_items, per, first, stride);
+    else consumer_loop<2>(a, stage_base, full_bar, tfull_bar, empty_bar, n_items, per, first, stride);
   }
 }
 
