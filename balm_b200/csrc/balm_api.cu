@@ -125,9 +125,11 @@ static int alloc_workspaces(balm_ctx *c) {
   double best_eff = 0;
   // every split costs one fp64 partial tile per output tile (written by the SYRK epilogue, read by the assembly):
   // the tensor path (the faster SYRK, where the partial tiles weigh more) takes the SMALLEST split count that keeps the
-  // last wave >= 95 % full and respects the int32 exactness bound (<= 32704 contraction rows per item); the fp64 path
-  // maximises balance.
-  const int min_splits = c->prec == BALM_PREC_TENSOR ? (int)((rows + 32575) / 32576) : 1;  // per-item rows (rounded up to 64) stay <= 32640
+  // last wave >= 95 % full and respects the int32 exactness bound (<= BALM_TC_MAX_ROWS_PER_ITEM = 32704 contraction
+  // rows per item); the fp64 path maximises balance. As 32704 is a multiple of 64, s >= rows / 32704 splits keep every
+  // item's rows, ceil(rows rounded up to 64 / s) rounded up to 64, within the bound.
+  const int min_splits = c->prec == BALM_PREC_TENSOR
+                             ? (int)((rows + BALM_TC_MAX_ROWS_PER_ITEM - 1) / BALM_TC_MAX_ROWS_PER_ITEM) : 1;
   const int items_per_tile = c->prec == BALM_PREC_TENSOR ? 2 : 1;  // the tensor SYRK computes a tile in two column halves
   for (int s = std::min(min_splits, max_splits); s <= max_splits; s++) {
     const int items = c->syrk_tiles * items_per_tile * s;

@@ -18,6 +18,9 @@
                               // + exact fp64 sums of squares of the 6 G' columns (diagonal of G'^T G')
 #define BALM_NB 64            // LDL^T panel width
 #define BALM_SYRK_TILE 128
+// int32 exactness bound of the tensor SYRK: contraction rows of one (tile, k-split) item, a multiple of 64.
+// A digit-pair sum T_d adds at most 4 * rows products of magnitude <= 2^14: 4 * 32704 * 2^14 < 2^31.
+#define BALM_TC_MAX_ROWS_PER_ITEM 32704
 
 void balm_set_error(const std::string &s);
 struct WindowState;  // the persistent sliding-window octree (assoc.cu)

@@ -58,7 +58,8 @@ constexpr int TC_THREADS = 32 * (CONSUMER_WARPS + 4);   // two consumer warpgrou
 // setmaxnreg.inc waits until the registers are free: 2 * 128 * 224 + 128 * 56 <= 384 * 168
 constexpr int CONSUMER_REGS = 224, PRODUCER_REGS = 56;
 constexpr int TC_SMEM = RING_BYTES + 1024 + 256;        // ring + alignment slack + barriers
-constexpr int MAX_ROWS_PER_ITEM = 32576;                // S * rows * 2^14 < 2^31 with the 64-row rounding of the k-split
+constexpr int MAX_ROWS_PER_ITEM = BALM_TC_MAX_ROWS_PER_ITEM;  // 32704: 4 * rows * 2^14 < 2^31 (a multiple of KS)
+static_assert(MAX_ROWS_PER_ITEM % KS == 0 && 4ll * MAX_ROWS_PER_ITEM * (1 << 14) < (1ll << 31), "int32 exactness bound");
 
 // ---------------- PTX wrappers ----------------
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -511,7 +512,52 @@ struct TcState {
   int forced_S = 0;      // BALM_TC_SLICES override (0 = decided on the device per batch)
   int *S_dev = nullptr;  // [1]
   int last_S = 0;        // read back with the error flag (instrumentation)
+  int64_t last_rows_padded = 0;  // contraction rows of the last batch's SYRK (0: none since the registration)
 };
+
+// The two tensor maps of a digit-plane buffer [SMAX][rows_alloc][ldq] (int8, column index fastest): the A block
+// (box {128, KS, 1}, 128-byte swizzle) and one column half of the B block (box {64, KS, 1}, 64-byte swizzle).
+int encode_tc_maps(int8_t *planes, int ldq, int64_t rows_alloc, CUtensorMap *map_a, CUtensorMap *map_b) {
+  EncodeTiledFn encode = nullptr;
+  cudaDriverEntryPointQueryResult qres;
+  CUDA_TRY(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", (void **)&encode, cudaEnableDefault, &qres));
+  if (!encode || qres != cudaDriverEntryPointSuccess) {
+    balm_set_error("cuTensorMapEncodeTiled not available from the driver");
+    return BALM_ERR_CUDA;
+  }
+  const cuuint64_t dims[3] = {(cuuint64_t)ldq, (cuuint64_t)rows_alloc, (cuuint64_t)SMAX};
+  const cuuint64_t strides[2] = {(cuuint64_t)ldq, (cuuint64_t)ldq * rows_alloc};
+  const cuuint32_t estr[3] = {1, 1, 1};
+  const cuuint32_t box_a[3] = {TILE, KS, 1};
+  if (encode(map_a, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, planes, dims, strides, box_a, estr,
+             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS) {
+    balm_set_error("cuTensorMapEncodeTiled (A block) failed");
+    return BALM_ERR_CUDA;
+  }
+  const cuuint32_t box_b[3] = {HALF, KS, 1};
+  if (encode(map_b, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, planes, dims, strides, box_b, estr,
+             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS) {
+    balm_set_error("cuTensorMapEncodeTiled (B half block) failed");
+    return BALM_ERR_CUDA;
+  }
+  return BALM_OK;
+}
+
+// One syrk_tc_kernel launch on c's stream: rows_padded (a multiple of KS) contraction rows of the planes behind the
+// maps, nb x nb blocks of 128 columns, `splits` k-splits; one CTA per item up to one per SM.
+int launch_syrk_tc(balm_ctx *c, const CUtensorMap &map_a, const CUtensorMap &map_b, int64_t rows_padded, int nb,
+                   int tiles, int splits, const int *S_dev, const double *isc, double *part, bool accumulate, int *err) {
+  TcArgs a{rows_padded, nb, tiles, splits, S_dev, isc, part, accumulate ? 1 : 0, err};
+  const int items = a.tiles * 2 * a.splits;
+  const int grid = items < c->sm_count ? items : c->sm_count;
+  syrk_tc_kernel<<<grid, TC_THREADS, TC_SMEM, c->stream>>>(map_a, map_b, a);
+  CUDA_TRY(cudaGetLastError());
+  return BALM_OK;
+}
+
+const char *const TC_TIMEOUT_MSG = "tensor-core SYRK pipeline timed out (mbarrier wait bound exceeded)";
 
 }  // namespace
 
@@ -543,30 +589,7 @@ int tensor_syrk_init(balm_ctx *c) {
   CUDA_TRY(cudaMemset(st->err, 0, sizeof(int)));
   c->colmax = st->colmax;  // the observation pass writes the column maxima here
 
-  EncodeTiledFn encode = nullptr;
-  cudaDriverEntryPointQueryResult qres;
-  CUDA_TRY(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", (void **)&encode, cudaEnableDefault, &qres));
-  if (!encode || qres != cudaDriverEntryPointSuccess) {
-    balm_set_error("cuTensorMapEncodeTiled not available from the driver");
-    return BALM_ERR_CUDA;
-  }
-  const cuuint64_t dims[3] = {(cuuint64_t)ldq, (cuuint64_t)st->rows_alloc, (cuuint64_t)SMAX};
-  const cuuint64_t strides[2] = {(cuuint64_t)ldq, (cuuint64_t)ldq * st->rows_alloc};
-  const cuuint32_t estr[3] = {1, 1, 1};
-  const cuuint32_t box_a[3] = {TILE, KS, 1};
-  if (encode(&st->map_a, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, c->Gq, dims, strides, box_a, estr,
-             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS) {
-    balm_set_error("cuTensorMapEncodeTiled (A block) failed");
-    return BALM_ERR_CUDA;
-  }
-  const cuuint32_t box_b[3] = {HALF, KS, 1};
-  if (encode(&st->map_b, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, c->Gq, dims, strides, box_b, estr,
-             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS) {
-    balm_set_error("cuTensorMapEncodeTiled (B half block) failed");
-    return BALM_ERR_CUDA;
-  }
+  TRY(encode_tc_maps(c->Gq, ldq, st->rows_alloc, &st->map_a, &st->map_b));
   // int32 exactness bound: every (tile, split) item contracts at most MAX_ROWS_PER_ITEM rows
   const int64_t rows = 3 * c->VB;
   const int min_splits = (int)((rows + MAX_ROWS_PER_ITEM - 1) / MAX_ROWS_PER_ITEM);
@@ -627,15 +650,11 @@ int tensor_obs_and_syrk(balm_ctx *c, const double *poses, int64_t v0, int64_t v1
   if (rc != BALM_OK) return rc;
   if (full) st->spec_ready = true;
   st->last_spec = spec;
+  st->last_rows_padded = rows_padded;
   CUDA_TRY(cudaEventRecord(c->ev[2], c->stream));
-  TcArgs a{rows_padded, c->syrk_nb, c->syrk_tiles, c->syrk_splits, st->S_dev, st->isc, c->syrk_part,
-           first_batch ? 0 : 1, st->err};
-  const int items = a.tiles * 2 * a.splits;
-  const int grid = items < c->sm_count ? items : c->sm_count;
-  syrk_tc_kernel<<<grid, TC_THREADS, TC_SMEM, c->stream>>>(st->map_a, st->map_b, a);
   c->launches += 2;
-  CUDA_TRY(cudaGetLastError());
-  return BALM_OK;
+  return launch_syrk_tc(c, st->map_a, st->map_b, rows_padded, c->syrk_nb, c->syrk_tiles, c->syrk_splits, st->S_dev,
+                        st->isc, c->syrk_part, !first_batch, st->err);
 }
 
 // The SYRK's error flag, the digit-plane count and the speculation verdict of the batch in flight: the copies are
@@ -656,7 +675,7 @@ int tensor_syrk_check_finish(balm_ctx *c) {  // after the stream has been synchr
   c->tm.digit_planes = st->last_S;
   if (st->last_spec) (c->h_flags[3] ? c->tm.single_sweeps : c->tm.redone_sweeps) += 1;
   if (c->h_flags[1] != 0) {
-    balm_set_error("tensor-core SYRK pipeline timed out (mbarrier wait bound exceeded)");
+    balm_set_error(TC_TIMEOUT_MSG);
     return BALM_ERR_CUDA;
   }
   return BALM_OK;
@@ -669,7 +688,83 @@ int tensor_syrk_check(balm_ctx *c) {
   return tensor_syrk_check_finish(c);
 }
 
-void tensor_syrk_new_problem(balm_ctx *c) {  // same-shape re-registration: the workspaces stay, the speculation does not
+// same-shape re-registration: the workspaces stay; the speculation and the record of the last batch (its planes now
+// describe other voxels) do not
+void tensor_syrk_new_problem(balm_ctx *c) {
   TcState *st = static_cast<TcState *>(c->tmap);
-  if (st) st->spec_ready = false;
+  if (st) {
+    st->spec_ready = false;
+    st->last_rows_padded = 0;
+  }
+}
+
+// ---------------- debug hooks (include/balm_b200.h): the SYRK alone, and what it consumed ----------------
+extern "C" int balm_debug_syrk_tc(balm_ctx *c, const int8_t *planes, int S, int64_t rows, const double *isc, int splits,
+                                  int accumulate, double *part) {
+  if (!c || !planes || !isc || !part) { balm_set_error("balm_debug_syrk_tc: bad arguments"); return BALM_ERR_INVALID; }
+  if (S < 2 || S > SMAX || rows < 1 || rows > ((int64_t)1 << 30) || splits < 1) {
+    balm_set_error("balm_debug_syrk_tc: S must be 2..4, rows 1..2^30 and splits >= 1");
+    return BALM_ERR_INVALID;
+  }
+  const int ldq = c->ldg, nb = ldq / TILE, tiles = nb * (nb + 1) / 2;
+  const int64_t rows_padded = (rows + KS - 1) / KS * KS;
+  const int64_t per = ((rows_padded + splits - 1) / splits + KS - 1) / KS * KS;  // as syrk_tc_kernel splits them
+  if (per > MAX_ROWS_PER_ITEM || (int64_t)tiles * 2 * splits > (1 << 30)) {
+    balm_set_error("balm_debug_syrk_tc: more than 32704 contraction rows per item (int32 exactness bound)");
+    return BALM_ERR_INVALID;
+  }
+  CUDA_TRY(cudaSetDevice(c->device));
+  const size_t plane = (size_t)rows_padded * ldq, count = (size_t)splits * tiles * TILE * TILE;
+  ScratchPool pool;
+  int8_t *d_planes;
+  double *d_isc, *d_part;
+  int *d_S, *d_err;
+  TRY(pool.get(&d_planes, SMAX * plane));
+  TRY(pool.get(&d_isc, (size_t)ldq));
+  TRY(pool.get(&d_part, count));
+  TRY(pool.get(&d_S, 1));
+  TRY(pool.get(&d_err, 1));
+  CUDA_TRY(cudaMemsetAsync(d_planes, 0, SMAX * plane, c->stream));  // K padding rows and unused planes
+  for (int s = 0; s < S; s++)
+    CUDA_TRY(cudaMemcpyAsync(d_planes + s * plane, planes + (size_t)s * rows * ldq, (size_t)rows * ldq,
+                             cudaMemcpyHostToDevice, c->stream));
+  CUDA_TRY(cudaMemcpyAsync(d_isc, isc, sizeof(double) * ldq, cudaMemcpyHostToDevice, c->stream));
+  CUDA_TRY(cudaMemcpyAsync(d_part, part, sizeof(double) * count, cudaMemcpyHostToDevice, c->stream));
+  CUDA_TRY(cudaMemcpyAsync(d_S, &S, sizeof(int), cudaMemcpyHostToDevice, c->stream));
+  CUDA_TRY(cudaMemsetAsync(d_err, 0, sizeof(int), c->stream));
+  CUtensorMap map_a, map_b;
+  TRY(encode_tc_maps(d_planes, ldq, rows_padded, &map_a, &map_b));
+  CUDA_TRY(cudaFuncSetAttribute(syrk_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM));
+  TRY(launch_syrk_tc(c, map_a, map_b, rows_padded, nb, tiles, splits, d_S, d_isc, d_part, accumulate != 0, d_err));
+  int err = 0;
+  CUDA_TRY(cudaMemcpyAsync(&err, d_err, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+  CUDA_TRY(cudaMemcpyAsync(part, d_part, sizeof(double) * count, cudaMemcpyDeviceToHost, c->stream));
+  CUDA_TRY(cudaStreamSynchronize(c->stream));
+  if (err != 0) {
+    balm_set_error(TC_TIMEOUT_MSG);
+    return BALM_ERR_CUDA;
+  }
+  return BALM_OK;
+}
+
+extern "C" int balm_debug_tc_planes(balm_ctx *c, int8_t *planes, double *isc, int *S, int64_t *rows_padded,
+                                    int *splits) {
+  TcState *st = (c && c->prec == BALM_PREC_TENSOR) ? static_cast<TcState *>(c->tmap) : nullptr;
+  if (!st || st->last_rows_padded == 0) {
+    balm_set_error("balm_debug_tc_planes: no tensor-path evaluation of the registered voxels");
+    return BALM_ERR_INVALID;
+  }
+  CUDA_TRY(cudaSetDevice(c->device));
+  CUDA_TRY(cudaStreamSynchronize(c->stream));
+  int s = 0;
+  CUDA_TRY(cudaMemcpy(&s, st->S_dev, sizeof(int), cudaMemcpyDeviceToHost));
+  const size_t plane = (size_t)st->last_rows_padded * c->ldg;
+  if (planes)
+    for (int q = 0; q < s; q++)
+      CUDA_TRY(cudaMemcpy(planes + q * plane, c->Gq + (size_t)q * st->rows_alloc * c->ldg, plane, cudaMemcpyDeviceToHost));
+  if (isc) CUDA_TRY(cudaMemcpy(isc, st->isc, sizeof(double) * c->ldg, cudaMemcpyDeviceToHost));
+  if (S) *S = s;
+  if (rows_padded) *rows_padded = st->last_rows_padded;
+  if (splits) *splits = c->syrk_splits;
+  return BALM_OK;
 }

@@ -337,6 +337,23 @@ int balm_timer_end(balm_ctx *ctx, float *ms);
 /* Debug aid: with BALM_DAG_TRACE=1 in the environment, device timestamps (ns) of the last factorisation: 4 per 64-column
  * step of the chain, then 3 per CTA (start, end, tasks executed). */
 int balm_debug_dag_trace(balm_ctx *ctx, unsigned long long *out, int max_entries);
+/* Debug aid: the tensor path's SYRK kernel alone, on caller-supplied digit planes, so that its fp64 partial tiles can be
+ * compared bit for bit with an exact integer reference. Uses ctx's device, stream and column count ldg = 6N rounded up
+ * to 128 (tiles = T (T + 1) / 2 upper-triangle tiles of 128 x 128, T = ldg / 128); neither needs nor touches a
+ * registration or an evaluation. planes: S (2..4) int8 planes of rows x ldg, plane 0 the most significant digit, column
+ * index fastest; rows are padded to a multiple of 64 with zeros. isc: ldg column factors. part (in/out):
+ * splits x tiles x 128 x 128 doubles, tile t of split sp at (sp * tiles + t) * 16384, row-major; accumulate = 0
+ * overwrites it, 1 adds to it. The rows go to `splits` k-split items of per = ceil(padded rows / splits) rounded up to
+ * 64 rows each; BALM_ERR_INVALID before any launch for S outside 2..4, rows outside 1..2^30, splits < 1 or per > 32704
+ * (the int32 exactness bound: 4 * 32704 * 2^14 < 2^31). A pipeline timeout is BALM_ERR_CUDA. Device scratch is
+ * allocated and freed by the call. */
+int balm_debug_syrk_tc(balm_ctx *ctx, const int8_t *planes, int S, int64_t rows, const double *isc, int splits,
+                       int accumulate, double *part);
+/* Debug aid: after a tensor-path evaluation, what the SYRK consumed in its last voxel batch: the S digit planes (their
+ * first rows_padded rows, S x rows_padded x ldg int8, layout as above), the ldg column factors isc, S and the context's
+ * k-split count. NULL arrays are not written, so a first call sizes the buffers. BALM_ERR_INVALID on an fp64 context or
+ * before any evaluation of the registered voxels. */
+int balm_debug_tc_planes(balm_ctx *ctx, int8_t *planes, double *isc, int *S, int64_t *rows_padded, int *splits);
 /* Device pointers of the last evaluation's H (n*n col-major), g (n) -- for zero-copy consumers. */
 int balm_device_views(balm_ctx *ctx, double **H_dev, double **g_dev);
 
