@@ -167,6 +167,8 @@ extern "C" int balm_create(balm_ctx **out, int n_poses, int device, int precisio
   cudaDeviceProp prop;
   CUDA_TRY(cudaGetDeviceProperties(&prop, device));
   c->sm_count = prop.multiProcessorCount;
+  if (precision == BALM_PREC_TENSOR && getenv("BALM_TC_TRACE"))
+    TRY(dev_alloc(&c->tc_trace, (size_t)c->sm_count * BALM_TC_TRACE_WORDS));
   int prio_least = 0, prio_greatest = 0;
   CUDA_TRY(cudaDeviceGetStreamPriorityRange(&prio_least, &prio_greatest));
   CUDA_TRY(cudaStreamCreateWithPriority(&c->stream, cudaStreamNonBlocking, prio_greatest));
@@ -210,6 +212,7 @@ extern "C" int balm_destroy(balm_ctx *c) {
   cudaFree(c->dx); cudaFree(c->dvec); cudaFree(c->scal); cudaFree(c->flags); cudaFree(c->accum); cudaFree(c->accum_batch);
   cudaFree(c->vox_key); cudaFree(c->vox_layer); cudaFree(c->res_part); cudaFree(c->planes); cudaFree(c->Xinv); cudaFree(c->dinv); cudaFree(c->sol); cudaFree(c->ysol);
   cudaFree(c->Hpack); cudaFree(c->dval); cudaFree(c->rres); cudaFree(c->rdelta); cudaFree(c->dag_flags);
+  cudaFree(c->tc_trace);
   cudaFreeHost(c->h_scal); cudaFreeHost(c->h_flags);
   for (auto &e : c->ev) if (e) cudaEventDestroy(e);
   cudaStreamDestroy(c->stream);

@@ -435,7 +435,7 @@ int launch_obs_colmax(balm_ctx *c, const double *poses, int64_t v0, int64_t v1, 
 // accumulators AND digit planes with the previous evaluation's scales); `skip`: device flag that disarms sweep 2.
 int launch_obs_int8(balm_ctx *c, const double *poses, int64_t v0, int64_t v1, bool first_batch, const double *sc,
                     int8_t *Gq, int64_t plane_stride, const int *S_dev, int S_alloc, int64_t rows_padded, bool fused,
-                    const int *skip, int wpc) {
+                    const int *skip) {
   const int64_t nv = v1 - v0;
   if (nv <= 0) return BALM_OK;
   ObsArgs a;
@@ -455,10 +455,7 @@ int launch_obs_int8(balm_ctx *c, const double *poses, int64_t v0, int64_t v1, bo
     }
   }
   if (fused) {
-    if (c->dense && wpc == 3) {  // 96-thread CTAs: one of them fits next to a resident SYRK CTA (register file)
-      grid.y = ((c->N + 31) / 32 + 2) / 3;
-      obs_pass_kernel<true, OBS_FUSED, 3><<<grid, 96, 0, c->stream>>>(a);
-    } else if (c->dense) obs_pass_kernel<true, OBS_FUSED><<<grid, 128, 0, c->stream>>>(a);
+    if (c->dense) obs_pass_kernel<true, OBS_FUSED><<<grid, 128, 0, c->stream>>>(a);
     else obs_pass_kernel<false, OBS_FUSED><<<grid, 128, 0, c->stream>>>(a);
     const int total = BALM_ACC * c->Np;
     obs_reduce_kernel<<<(total + 255) / 256, 256, 0, c->stream>>>(c->obs_part, chunks, total, c->accum,

@@ -21,6 +21,8 @@
 // int32 exactness bound of the tensor SYRK: contraction rows of one (tile, k-split) item, a multiple of 64.
 // A digit-pair sum T_d adds at most 4 * rows products of magnitude <= 2^14: 4 * 32704 * 2^14 < 2^31.
 #define BALM_TC_MAX_ROWS_PER_ITEM 32704
+// BALM_TC_TRACE: words per CTA of the tensor SYRK's per-role clock trace (layout: balm_debug_tc_trace)
+#define BALM_TC_TRACE_WORDS 18
 
 void balm_set_error(const std::string &s);
 struct WindowState;  // the persistent sliding-window octree (assoc.cu)
@@ -120,6 +122,7 @@ struct balm_ctx {
   double *rdelta = nullptr;                         // [n] refinement correction
   int *dag_flags = nullptr;                         // tile-DAG dependency counters: upd | pdone [nt*nt], xdone | rhs_cnt [nt]
   unsigned long long *dag_trace = nullptr;          // BALM_DAG_TRACE: device timestamps of the last factorisation
+  unsigned long long *tc_trace = nullptr;           // BALM_TC_TRACE: per-CTA clocks of the last tensor SYRK launch
   double *scal = nullptr;                           // device scalars [32]: 0 r(eval) 1 q1 2 r(residual) 3 u 4..15 gauge
                                                     // snapshot, 16/17 this rank's residual at the current / trial poses
   double *h_scal = nullptr;                         // pinned host mirror [16]
@@ -664,7 +667,7 @@ int launch_obs_pass(balm_ctx *c, const double *poses, int64_t v0, int64_t v1, bo
 int launch_obs_colmax(balm_ctx *c, const double *poses, int64_t v0, int64_t v1, bool first_batch);
 int launch_obs_int8(balm_ctx *c, const double *poses, int64_t v0, int64_t v1, bool first_batch, const double *sc,
                     int8_t *Gq, int64_t plane_stride, const int *S_dev, int S_alloc, int64_t rows_padded, bool fused,
-                    const int *skip, int wpc = 4);
+                    const int *skip);
 int tensor_obs_and_syrk(balm_ctx *c, const double *poses, int64_t v0, int64_t v1, bool first_batch);
 int launch_syrk_f64(balm_ctx *c, int64_t rows, bool first_batch);
 // Dacc null: the Hessian, H = -S + blockdiag(accum rows 6..26) and g, into c->H / c->g (or the all-reduce pack).

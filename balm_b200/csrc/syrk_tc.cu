@@ -14,9 +14,9 @@
 // Kernel anatomy (syrk_tc_kernel; one CTA per SM, persistent over (tile, column half, k-split) items, 384 threads):
 //   warp 8    : TMA producer -- cp.async.bulk.tensor.3d of the S int8 planes of the A block (128 columns bi, 128B
 //               swizzle) and of the B half block (64 columns of bj, 64B swizzle), KS = 64 contraction rows per stage,
-//               into a 192 KB shared-memory ring of 3-6 stages (mbarrier full/empty)
-//   warps 9-11: B transposers -- copy the S B half planes of each landed stage into K-major core matrices beside it
-//               in the same stage (mbarrier tfull)
+//               into the A and B rings (see Rings: 160-224 KB of shared memory in all, mbarrier full/empty per slot)
+//   warps 9-11: B transposers -- load each landed B slot into registers, free it, and store the K-major core
+//               matrices into a slot of the BT ring
 //   warps 0-7 : consumers, two warpgroups of 64 output rows each -- wgmma m64n64k32 s8 x s8 -> s32 with A from
 //               registers and B from the K-major copy, S(S+1)/2 digit-pair products per k32 step into S register
 //               accumulators; then the epilogue: fp64 Horner combine, column scales, fp64 partial tile to global
@@ -42,22 +42,44 @@ constexpr int KS = 64;                // contraction rows per pipeline stage
 constexpr int A_PLANE_BYTES = KS * TILE;  // 8192: one plane of the A block, one stage (128-byte rows)
 constexpr int B_PLANE_BYTES = KS * HALF;  // 4096: one plane of the B half block, one stage (64-byte rows)
 constexpr int BT_PLANE_BYTES = KS * HALF; // 4096: the same plane K-major (wgmma core matrices, see bt_offset)
-constexpr int RING_BYTES = 196608;        // stage ring (the rest of the 227 KB per block is left to L1)
-constexpr int MAX_STAGES = 8;
-// a stage holds S planes of the A block, S planes of the B half block and their K-major copies:
-// 3 stages for S = 4, 4 for S = 3, 6 for S = 2
-__host__ __device__ constexpr int stage_bytes_for(int S) { return S * (A_PLANE_BYTES + B_PLANE_BYTES + BT_PLANE_BYTES); }
-__host__ __device__ constexpr int stages_for(int S) {
-  return RING_BYTES / stage_bytes_for(S) > MAX_STAGES ? MAX_STAGES : RING_BYTES / stage_bytes_for(S);
-}
+constexpr int MAX_SLOTS = 8;             // barriers per ring
+constexpr int BAR_BYTES = 6 * MAX_SLOTS * 8;
+constexpr int RING_BYTES = 227 * 1024 - 1024 - BAR_BYTES;  // the block's whole shared memory but alignment slack, barriers
+// Three rings, one slot per 64-row stage each, all advancing by one slot per stage: A (S planes of the A block, TMA),
+// B (S planes of the B half block as TMA lands them, MN-major) and BT (their K-major copies). A slot of B is free again
+// as soon as the transposers have loaded it into registers, a slot of BT once the consumers' MMAs on it retired, so
+// neither the in-flight loads nor the MMAs hold a copy they do not use. Depths per S (A x B x BT slots), chosen with
+// the BALM_TC_TRACE per-role clocks and the benchmark at its C3 shape (S = 3): with two BT slots the transposers run
+// only one stage ahead of the consumers, whose waits on BT then dominate; deeper A or B rings than below measured no
+// faster:
+//   S = 2: 6 x 16 KB + 4 x 8 KB + 4 x 8 KB = 160 KB; S = 3: 4 x 24 + 4 x 12 + 4 x 12 = 192 KB;
+//   S = 4: 4 x 32 + 2 x 16 + 4 x 16 = 224 KB
+template <int S>
+struct Rings {
+  static constexpr int DA = S == 2 ? 6 : 4, DB = S == 4 ? 2 : 4, DT = 4;
+  static constexpr int A_SLOT = S * A_PLANE_BYTES, B_SLOT = S * B_PLANE_BYTES, T_SLOT = S * BT_PLANE_BYTES;
+  static constexpr int B_OFF = DA * A_SLOT, T_OFF = B_OFF + DB * B_SLOT, BYTES = T_OFF + DT * T_SLOT;
+  static_assert(BYTES <= RING_BYTES && DA <= MAX_SLOTS && DB <= MAX_SLOTS && DT <= MAX_SLOTS, "ring layout");
+  static_assert(A_SLOT % 1024 == 0 && B_SLOT % 1024 == 0 && T_SLOT % 1024 == 0, "swizzle alignment");
+};
+// slot and phase of a ring of D slots
+template <int D>
+struct RingPos {
+  int slot = 0;
+  uint32_t ph = 0;
+  __device__ __forceinline__ void next() {
+    if (++slot == D) { slot = 0; ph ^= 1; }
+  }
+};
 constexpr int CONSUMER_WARPS = 8;
 constexpr int TRANSPOSE_WARPS = 3;                      // warps 9-11
 constexpr int TC_THREADS = 32 * (CONSUMER_WARPS + 4);   // two consumer warpgroups + one producer warpgroup
 // register split (setmaxnreg): the producer warpgroup gives registers up so the consumers can hold their accumulators
-// (S * 32 + 2 * S * 4 A-fragment registers). The pool is what the launch allocated, 384 threads x 168 registers, and
-// setmaxnreg.inc waits until the registers are free: 2 * 128 * 224 + 128 * 56 <= 384 * 168
-constexpr int CONSUMER_REGS = 224, PRODUCER_REGS = 56;
-constexpr int TC_SMEM = RING_BYTES + 1024 + 256;        // ring + alignment slack + barriers
+// (S * 32 + 2 * S * 4 A-fragment registers); the transposers keep a whole stage of their ldmatrix results (up to 44
+// registers at S = 4). The pool is what the launch allocated, 384 threads x 168 registers, and setmaxnreg.inc waits
+// until the registers are free: 2 * 128 * 216 + 128 * 72 <= 384 * 168
+constexpr int CONSUMER_REGS = 216, PRODUCER_REGS = 72;
+constexpr int TC_SMEM = RING_BYTES + 1024 + BAR_BYTES;  // rings + alignment slack + barriers
 constexpr int MAX_ROWS_PER_ITEM = BALM_TC_MAX_ROWS_PER_ITEM;  // 32704: 4 * rows * 2^14 < 2^31 (a multiple of KS)
 static_assert(MAX_ROWS_PER_ITEM % KS == 0 && 4ll * MAX_ROWS_PER_ITEM * (1 << 14) < (1ll << 31), "int32 exactness bound");
 
@@ -92,6 +114,22 @@ __device__ __forceinline__ bool mbar_wait(uint64_t *bar, uint32_t parity, int *e
   return false;
 }
 
+__device__ __forceinline__ unsigned long long globaltimer_ns() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;\n" : "=l"(t));
+  return t;
+}
+// BALM_TC_TRACE (balm_debug_tc_trace): per-CTA word offsets of the stage count, the consumer warp 0 globaltimer pair and
+// the clock64 sums of the consumer warps 0 and 4 (5 each), of transposer warp 9 (3) and of the producer (2)
+constexpr int TR_STAGES = 0, TR_NS = 1, TR_CONS = 3, TR_XPOSE = 13, TR_PROD = 16, TR_WORDS = BALM_TC_TRACE_WORDS;
+static_assert(TR_PROD + 2 == TR_WORDS, "trace layout");
+// clock64 in the traced instantiation; the untraced one reads no clock
+template <bool TRACE>
+__device__ __forceinline__ long long tclock() {
+  if constexpr (TRACE) return clock64();
+  else return 0;
+}
+
 __device__ __forceinline__ void tma_load_3d(void *dst, const CUtensorMap *map, uint64_t *bar, int c0, int c1, int c2) {
   asm volatile(
       "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];\n"
@@ -118,11 +156,10 @@ __device__ __forceinline__ void ldsm_x4_trans(uint32_t addr, uint32_t *r) {
 constexpr uint32_t PERM_EVEN = 0x6420, PERM_ODD = 0x7531;
 
 // K-major copy of one B plane, one stage: wgmma core matrices of 8 columns x 16 k bytes (128 contiguous bytes,
-// no swizzle); k32 step c at c * 2048, column group n / 8 at (n / 8) * 256 (SBO), k half at 128 (LBO).
+// no swizzle); k32 step c at c * 2048, column group n / 8 at (n / 8) * 256 (SBO), k half at 128 (LBO). The 4 k positions
+// 4 kword .. 4 kword + 3 (kword in 0..7) of column n are the word at
+//   bt_offset(c, n, kword) = c * BT_CHUNK + (n >> 3) * BT_SBO + (kword >> 2) * BT_LBO + (n & 7) * 16 + 4 * (kword & 3).
 constexpr int BT_LBO = 128, BT_SBO = 256, BT_CHUNK = 2048;
-__device__ __forceinline__ int bt_offset(int c, int n, int kword) {  // kword = k position / 4 in 0..7
-  return c * BT_CHUNK + (n >> 3) * BT_SBO + (kword >> 2) * BT_LBO + (n & 7) * 16 + 4 * (kword & 3);
-}
 __device__ __forceinline__ uint64_t bt_desc(uint32_t saddr) {  // wgmma matrix descriptor, no swizzle
   return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)(BT_LBO >> 4) << 16) | ((uint64_t)(BT_SBO >> 4) << 32);
 }
@@ -173,6 +210,7 @@ struct TcArgs {
   double *part;       // [splits][tiles][128*128]
   int accumulate;
   int *err;
+  unsigned long long *trace;  // [gridDim.x][TR_WORDS], written by the traced instantiation only
 };
 
 struct ItemInfo {
@@ -186,6 +224,13 @@ __device__ __forceinline__ void tile_coords_tc(int t, int nb, int &bi, int &bj) 
   while (rem >= nb - r) { rem -= nb - r; r++; }
   bi = r;
   bj = r + rem;
+}
+
+// Items are distributed round robin over the CTAs: item blockIdx.x, blockIdx.x + gridDim.x, ...
+__device__ __forceinline__ int n_items(const TcArgs &a) { return a.tiles * 2 * a.splits; }
+// contraction rows of a k-split item: ceil(rows / splits) rounded up to KS
+__device__ __forceinline__ int64_t rows_per_item(const TcArgs &a) {
+  return ((a.rows + a.splits - 1) / a.splits + KS - 1) / KS * KS;
 }
 
 // work = (sp * tiles + t) * 2 + h: the two column halves of a tile run on neighbouring CTAs and share the A block in L2
@@ -202,24 +247,30 @@ __device__ __forceinline__ ItemInfo decode_item(const TcArgs &a, int work, int64
   return it;
 }
 
+// Shared-memory barriers of the three rings (MAX_SLOTS each): full = the slot holds its stage, empty = it may be refilled
+struct RingBars {
+  uint64_t *full_a, *empty_a, *full_b, *empty_b, *full_t, *empty_t;
+};
+
 // One consumer warpgroup (wg = 0, 1): output rows 64 wg .. 64 wg + 63 of the 128 x 64 half tile, all items of this
 // CTA. Warp w (0..7) holds the 16 rows of 16-byte chunk w of the A block: fragment row g is output row 16 w + 2 g,
 // fragment row g + 8 is output row 16 w + 2 g + 1; fragment column n is column n of the half tile.
-template <int S>
-__device__ __forceinline__ void consumer_loop(const TcArgs &a, uint8_t *stage_base, uint64_t *full_bar,
-                                              uint64_t *tfull_bar, uint64_t *empty_bar, int n_items, int64_t per,
-                                              int first, int stride) {
+template <int S, bool TRACE>
+__device__ __forceinline__ void consumer_loop(const TcArgs &a, uint32_t ring, const RingBars &bar) {
+  using R = Rings<S>;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int g = lane >> 2, t = lane & 3, i = lane & 7, wg = warp >> 2;
-  constexpr int nst = stages_for(S), sbytes = stage_bytes_for(S);
-  const uint32_t ring = smem_u32(stage_base);
   // ldmatrix row of this lane: contraction row 8 (lane / 8) + i of a k32 step, chunk `warp` under the 128B swizzle;
   // the 8 rows of each matrix sit in 8 different chunks, so the loads are free of bank conflicts
   const uint32_t lda = ring + ((lane >> 3) * 8 + i) * TILE + ((warp ^ i) << 4);
+  const uint32_t bt_ring = ring + R::T_OFF;
   const double inv256 = 1.0 / 256.0;
-  int st = 0;
-  uint32_t ph = 0;
-  for (int item = first; item < n_items; item += stride) {
+  long long tr[4] = {0, 0, 0, 0};  // trace: wait A full, wait BT full, wgmma.wait_group, epilogue
+  const long long t_start = tclock<TRACE>();
+  const unsigned long long ns_start = TRACE ? globaltimer_ns() : 0;
+  int k = 0;  // stages consumed so far: stage k sits in slot k % D of a ring of D slots, phase (k / D) & 1
+  const int64_t per = rows_per_item(a);
+  for (int item = blockIdx.x; item < n_items(a); item += gridDim.x) {
     const ItemInfo info = decode_item(a, item, per);
     int32_t acc[S][32];
 #pragma unroll
@@ -228,12 +279,16 @@ __device__ __forceinline__ void consumer_loop(const TcArgs &a, uint8_t *stage_ba
       for (int q = 0; q < 32; q++) acc[d][q] = 0;
     uint32_t af[2][S][4];  // A fragments of every plane, one set per k32 step of a stage (the other may be in flight)
     bool alive = true;
-    int prev = -1;  // the stage whose MMAs may still be in flight
-    for (int ks = 0; ks < info.nsteps; ks++) {
-      const bool ok = mbar_wait(&full_bar[st], ph, a.err) && mbar_wait(&tfull_bar[st], ph, a.err);
-      if (!warpgroup_all(ok, 1 + wg)) { alive = false; break; }  // the warpgroup leaves together (wgmma is .aligned)
-      const uint32_t sa = lda + st * sbytes;
-      const uint64_t sdesc = bt_desc(ring + S * (A_PLANE_BYTES + B_PLANE_BYTES) + st * sbytes);
+    for (int ks = 0; ks < info.nsteps; ks++, k++) {
+      const int sla = k % R::DA, slt = k % R::DT;
+      const long long t0 = tclock<TRACE>();
+      const bool ok_a = mbar_wait(&bar.full_a[sla], (k / R::DA) & 1, a.err);
+      const long long t1 = tclock<TRACE>();
+      const bool ok = warpgroup_all(ok_a && mbar_wait(&bar.full_t[slt], (k / R::DT) & 1, a.err), 1 + wg);
+      if constexpr (TRACE) { tr[0] += t1 - t0; tr[1] += clock64() - t1; }
+      if (!ok) { alive = false; break; }  // the warpgroup leaves together (wgmma is .aligned)
+      const uint32_t sa = lda + sla * R::A_SLOT;
+      const uint64_t sdesc = bt_desc(bt_ring + slt * R::T_SLOT);
 #pragma unroll
       for (int c = 0; c < KS / 32; c++) {
 #pragma unroll
@@ -254,22 +309,31 @@ __device__ __forceinline__ void consumer_loop(const TcArgs &a, uint8_t *stage_ba
         wgmma_commit();
         // every group but this one has retired: after the first k32 step that frees the previous stage, after the
         // second the A fragments of the first
+        const long long t2 = tclock<TRACE>();
         wgmma_wait<1>();
-        if (c == 0 && prev >= 0) {
+        if constexpr (TRACE) tr[2] += clock64() - t2;
+        if (c == 0 && ks > 0) {  // the previous stage's MMAs have retired: free its A and BT slots
           __syncwarp();
-          if (lane == 0) mbar_arrive(&empty_bar[prev]);
+          if (lane == 0) {
+            mbar_arrive(&bar.empty_a[(k - 1) % R::DA]);
+            mbar_arrive(&bar.empty_t[(k - 1) % R::DT]);
+          }
         }
       }
-      prev = st;
-      if (++st == nst) { st = 0; ph ^= 1; }
     }
+    const long long t3 = tclock<TRACE>();
     wgmma_wait<0>();
 #pragma unroll
     for (int d = 0; d < S; d++) fence_acc(acc[d]);
+    const long long t4 = tclock<TRACE>();
+    if constexpr (TRACE) tr[2] += t4 - t3;
     if (!alive) break;
-    if (prev >= 0) {
+    if (info.nsteps > 0) {
       __syncwarp();
-      if (lane == 0) mbar_arrive(&empty_bar[prev]);
+      if (lane == 0) {
+        mbar_arrive(&bar.empty_a[(k - 1) % R::DA]);
+        mbar_arrive(&bar.empty_t[(k - 1) % R::DT]);
+      }
     }
     // ---- epilogue: Horner over the digit-pair order d = S-1 .. 0, column scales, fp64 partial tile ----
     double *tile_out = a.part + ((size_t)info.sp * a.tiles + info.t) * (TILE * TILE);
@@ -293,112 +357,193 @@ __device__ __forceinline__ void consumer_loop(const TcArgs &a, uint8_t *stage_ba
         }
       }
     }
+    if constexpr (TRACE) tr[3] += clock64() - t4;
   }
-}
-
-// One transposer warp (tw = 0..2): the K-major copies of the B half planes of every stage this CTA consumes. Work unit
-// u = (plane, k32 step c, 16-column chunk q) of a stage: one ldmatrix.trans of its 4 x 8 contraction rows gives thread
-// (g, t) the k positions 4t..4t+3 and 16+4t..16+4t+3 of columns 16 q + 2 g and 16 q + 2 g + 1.
-__device__ __forceinline__ void transpose_loop(const TcArgs &a, uint8_t *stage_base, uint64_t *full_bar,
-                                               uint64_t *tfull_bar, int S, int n_items, int64_t per, int first,
-                                               int stride, int tw) {
-  const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3, i = lane & 7;
-  const int nst = stages_for(S), sbytes = stage_bytes_for(S);
-  // source row of this lane: contraction row 8 (lane / 8) + i of a k32 step; 64-byte rows under the 64B swizzle
-  // (chunk q of row r at q ^ ((r >> 1) & 3)), so the 8 rows of each matrix hit 8 different 16-byte bank groups
-  const uint32_t src = smem_u32(stage_base) + S * A_PLANE_BYTES + ((lane >> 3) * 8 + i) * HALF;
-  uint8_t *dst = stage_base + S * (A_PLANE_BYTES + B_PLANE_BYTES);
-  // lanes g >= 4 store column 2g + 1 before 2g: the 32 lanes of every store then hit 32 different banks
-  const int flip = g >> 2;
-  const uint32_t perm0 = flip ? PERM_ODD : PERM_EVEN, perm1 = flip ? PERM_EVEN : PERM_ODD;
-  int st = 0;
-  uint32_t ph = 0;
-  bool alive = true;
-  for (int item = first; alive && item < n_items; item += stride) {
-    const ItemInfo info = decode_item(a, item, per);
-    for (int ks = 0; ks < info.nsteps; ks++) {
-      if (!__all_sync(0xffffffffu, mbar_wait(&full_bar[st], ph, a.err))) { alive = false; break; }
-      for (int u = tw; u < 8 * S; u += TRANSPOSE_WARPS) {
-        const int p = u >> 3, c = (u >> 2) & 1, q = u & 3;
-        uint32_t m[4];
-        ldsm_x4_trans(src + st * sbytes + p * B_PLANE_BYTES + c * 32 * HALF + ((q ^ (i >> 1)) << 4), m);
-        uint8_t *d = dst + st * sbytes + p * BT_PLANE_BYTES;
-        const int n0 = 16 * q + 2 * g + flip, n1 = n0 ^ 1;
-        *reinterpret_cast<uint32_t *>(d + bt_offset(c, n0, t)) = __byte_perm(m[0], m[1], perm0);
-        *reinterpret_cast<uint32_t *>(d + bt_offset(c, n1, t)) = __byte_perm(m[0], m[1], perm1);
-        *reinterpret_cast<uint32_t *>(d + bt_offset(c, n0, 4 + t)) = __byte_perm(m[2], m[3], perm0);
-        *reinterpret_cast<uint32_t *>(d + bt_offset(c, n1, 4 + t)) = __byte_perm(m[2], m[3], perm1);
+  if constexpr (TRACE) {
+    if ((warp & 3) == 0 && lane == 0) {
+      unsigned long long *o = a.trace + (size_t)blockIdx.x * TR_WORDS;
+      const long long total = clock64() - t_start;
+#pragma unroll
+      for (int w = 0; w < 4; w++) o[TR_CONS + 5 * wg + w] = tr[w];
+      o[TR_CONS + 5 * wg + 4] = total;
+      if (wg == 0) {
+        o[TR_STAGES] = k;
+        o[TR_NS] = ns_start;
+        o[TR_NS + 1] = globaltimer_ns();
       }
-      asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");  // the copy is read by wgmma (async proxy)
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tfull_bar[st]);
-      if (++st == nst) { st = 0; ph ^= 1; }
     }
   }
 }
 
+__device__ __forceinline__ void sts_u32(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.u32 [%0], %1;\n" ::"r"(addr), "r"(v) : "memory");
+}
+
+// One transposer warp (TW = 0..2): the K-major copies of the B half planes of every stage this CTA consumes. Work unit
+// u = (plane p, k32 step c, 16-column chunk q) = 8 p + 4 c + q of a stage; warp TW takes u = TW, TW + 3, ... One
+// ldmatrix.trans of a unit's 4 x 8 contraction rows gives thread (g, t) the k positions 4t..4t+3 and 16+4t..16+4t+3 of
+// columns 16 q + 2 g and 16 q + 2 g + 1. A stage: wait for its B slot, issue all of the warp's ldmatrix loads and
+// release the B slot, wait for a free BT slot, permute and store, publish the BT slot.
+template <int S, int TW, bool TRACE>
+__device__ __forceinline__ void transpose_loop(const TcArgs &a, uint32_t ring, const RingBars &bar) {
+  using R = Rings<S>;
+  constexpr int J = (8 * S - TW + 2) / 3;  // units of this warp per stage, all loaded before any store (4 J <= 44
+                                          // registers of the producer warpgroup's PRODUCER_REGS)
+  const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3, i = lane & 7;
+  // source row of this lane: contraction row 8 (lane / 8) + i of a k32 step; 64-byte rows under the 64B swizzle
+  // (chunk q of row r at q ^ ((r >> 1) & 3)), so the 8 rows of each matrix hit 8 different 16-byte bank groups. The row
+  // offset is a multiple of 64, so chunk q of a unit is at (src + slot, plane and step offsets) ^ (q << 4).
+  const uint32_t src = ring + R::B_OFF + ((lane >> 3) * 8 + i) * HALF + ((i >> 1) << 4);
+  // lanes g >= 4 store column 2g + 1 before 2g: the 32 lanes of every store then hit 32 different banks.
+  // bt_offset(c, 16 q + n, kw) for this lane's column n = 2g + flip: c * BT_CHUNK + q * 2 BT_SBO + dst0 (kw = t) or
+  // + BT_LBO (kw = 4 + t); its neighbour n ^ 1 sits at dst0 ^ 16
+  const int flip = g >> 2, n = 2 * g + flip;
+  const uint32_t perm0 = flip ? PERM_ODD : PERM_EVEN, perm1 = flip ? PERM_EVEN : PERM_ODD;
+  const uint32_t dst = ring + R::T_OFF + (n >> 3) * BT_SBO + (n & 7) * 16 + 4 * t;
+  long long tr[3] = {0, 0, 0};  // trace: wait B full, wait BT empty, total
+  RingPos<R::DB> pb;
+  RingPos<R::DT> pt;
+  bool alive = true;
+  const int64_t per = rows_per_item(a);
+  for (int item = blockIdx.x; alive && item < n_items(a); item += gridDim.x) {
+    const ItemInfo info = decode_item(a, item, per);
+    for (int ks = 0; ks < info.nsteps; ks++) {
+      const long long t0 = tclock<TRACE>();
+      const bool ok = __all_sync(0xffffffffu, mbar_wait(&bar.full_b[pb.slot], pb.ph, a.err));
+      if constexpr (TRACE) tr[0] += clock64() - t0;
+      if (!ok) { alive = false; break; }
+      const uint32_t sb = src + pb.slot * R::B_SLOT, db = dst + pt.slot * R::T_SLOT;
+      uint32_t m[J][4];
+#pragma unroll
+      for (int j = 0; j < J; j++) {
+        const int u = TW + 3 * j, p = u >> 3, c = (u >> 2) & 1, q = u & 3;
+        ldsm_x4_trans((sb + p * B_PLANE_BYTES + c * 32 * HALF) ^ (q << 4), m[j]);
+      }
+      // the slot is refilled by TMA (async proxy) once released: the proxy fence orders these generic-proxy reads
+      // before that write. Without it the arrive does not wait for the ldmatrix data, and the refill can overwrite the
+      // slot before it is read.
+      asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&bar.empty_b[pb.slot]);
+      const long long t1 = tclock<TRACE>();
+      const bool free_t = __all_sync(0xffffffffu, mbar_wait(&bar.empty_t[pt.slot], pt.ph ^ 1, a.err));
+      if constexpr (TRACE) tr[1] += clock64() - t1;
+      if (!free_t) { alive = false; break; }
+#pragma unroll
+      for (int j = 0; j < J; j++) {
+        const int u = TW + 3 * j, p = u >> 3, c = (u >> 2) & 1, q = u & 3;
+        const uint32_t d = db + p * BT_PLANE_BYTES + c * BT_CHUNK + q * 2 * BT_SBO;
+        sts_u32(d, __byte_perm(m[j][0], m[j][1], perm0));
+        sts_u32(d ^ 16, __byte_perm(m[j][0], m[j][1], perm1));
+        sts_u32(d + BT_LBO, __byte_perm(m[j][2], m[j][3], perm0));
+        sts_u32((d + BT_LBO) ^ 16, __byte_perm(m[j][2], m[j][3], perm1));
+      }
+      asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");  // the copy is read by wgmma (async proxy)
+      __syncwarp();
+      if (lane == 0) {
+        mbar_arrive(&bar.full_t[pt.slot]);
+      }
+      pb.next();
+      pt.next();
+      if constexpr (TRACE) tr[2] += clock64() - t0;
+    }
+  }
+  if constexpr (TRACE) {
+    if (TW == 0 && lane == 0) {
+      unsigned long long *o = a.trace + (size_t)blockIdx.x * TR_WORDS;
+      o[TR_XPOSE] = tr[0];
+      o[TR_XPOSE + 1] = tr[1];
+      o[TR_XPOSE + 2] = tr[2] - tr[0] - tr[1];  // busy
+    }
+  }
+}
+
+// The TMA producer (one thread): per stage, the S planes of the B half block into the B ring first (they still have to
+// be transposed), then the S planes of the A block into the A ring.
+template <int S, bool TRACE>
+__device__ __forceinline__ void producer_loop(const TcArgs &a, const CUtensorMap *tmap_a, const CUtensorMap *tmap_b,
+                                              uint8_t *ring, const RingBars &bar) {
+  using R = Rings<S>;
+  asm volatile("prefetch.tensormap [%0];\n" ::"l"(tmap_a) : "memory");
+  asm volatile("prefetch.tensormap [%0];\n" ::"l"(tmap_b) : "memory");
+  long long tr[2] = {0, 0};  // trace: wait A empty, wait B empty
+  RingPos<R::DA> pa;
+  RingPos<R::DB> pb;
+  bool alive = true;
+  const int64_t per = rows_per_item(a);
+  for (int item = blockIdx.x; alive && item < n_items(a); item += gridDim.x) {
+    const ItemInfo info = decode_item(a, item, per);
+    for (int ks = 0; ks < info.nsteps; ks++) {
+      const int krow = (int)(info.k_begin + (int64_t)ks * KS);
+      const long long t0 = tclock<TRACE>();
+      if (!mbar_wait(&bar.empty_b[pb.slot], pb.ph ^ 1, a.err)) { alive = false; break; }
+      const long long t1 = tclock<TRACE>();
+      uint8_t *sb = ring + R::B_OFF + pb.slot * R::B_SLOT;
+      mbar_expect_tx(&bar.full_b[pb.slot], S * B_PLANE_BYTES);
+      for (int s = 0; s < S; s++)
+        tma_load_3d(sb + s * B_PLANE_BYTES, tmap_b, &bar.full_b[pb.slot], info.bj * TILE + info.h * HALF, krow, s);
+      const long long t2 = tclock<TRACE>();
+      if (!mbar_wait(&bar.empty_a[pa.slot], pa.ph ^ 1, a.err)) { alive = false; break; }
+      if constexpr (TRACE) { tr[0] += clock64() - t2; tr[1] += t1 - t0; }
+      uint8_t *sa = ring + pa.slot * R::A_SLOT;
+      mbar_expect_tx(&bar.full_a[pa.slot], S * A_PLANE_BYTES);
+      for (int s = 0; s < S; s++) tma_load_3d(sa + s * A_PLANE_BYTES, tmap_a, &bar.full_a[pa.slot], info.bi * TILE, krow, s);
+      pa.next();
+      pb.next();
+    }
+  }
+  if constexpr (TRACE) {
+    unsigned long long *o = a.trace + (size_t)blockIdx.x * TR_WORDS;
+    o[TR_PROD] = tr[0];
+    o[TR_PROD + 1] = tr[1];
+  }
+}
+
+template <int S, bool TRACE>
+__device__ __forceinline__ void syrk_tc_cta(const CUtensorMap *tmap_a, const CUtensorMap *tmap_b, const TcArgs &a,
+                                            uint8_t *ring, const RingBars &bar) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const uint32_t ring_u32 = smem_u32(ring);
+  if (warp >= CONSUMER_WARPS) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;\n" ::"n"(PRODUCER_REGS));
+    // ===================== B transposers (warps 9-11) =====================
+    if (warp == CONSUMER_WARPS + 1) transpose_loop<S, 0, TRACE>(a, ring_u32, bar);
+    else if (warp == CONSUMER_WARPS + 2) transpose_loop<S, 1, TRACE>(a, ring_u32, bar);
+    else if (warp == CONSUMER_WARPS + 3) transpose_loop<S, 2, TRACE>(a, ring_u32, bar);
+    // ===================== TMA producer (warp 8, one thread) =====================
+    else if (lane == 0) producer_loop<S, TRACE>(a, tmap_a, tmap_b, ring, bar);
+  } else {
+    // ===================== wgmma + epilogue =====================
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;\n" ::"n"(CONSUMER_REGS));
+    consumer_loop<S, TRACE>(a, ring_u32, bar);
+  }
+}
+
+template <bool TRACE>
 __global__ void __launch_bounds__(TC_THREADS, 1) syrk_tc_kernel(const __grid_constant__ CUtensorMap tmap_a,
                                                                 const __grid_constant__ CUtensorMap tmap_b, TcArgs a) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  // 1024-byte aligned stage ring (the swizzle patterns are functions of the shared-memory address), then barriers
-  uint8_t *stage_base = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t *full_bar = reinterpret_cast<uint64_t *>(stage_base + RING_BYTES);
-  uint64_t *empty_bar = full_bar + MAX_STAGES;
-  uint64_t *tfull_bar = empty_bar + MAX_STAGES;
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int S = *a.S_dev;
-
+  // 1024-byte aligned rings (the swizzle patterns are functions of the shared-memory address), then barriers
+  uint8_t *ring = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint64_t *bars = reinterpret_cast<uint64_t *>(ring + RING_BYTES);
+  const RingBars bar{bars, bars + MAX_SLOTS, bars + 2 * MAX_SLOTS, bars + 3 * MAX_SLOTS, bars + 4 * MAX_SLOTS,
+                     bars + 5 * MAX_SLOTS};
   if (threadIdx.x == 0) {
-    for (int i = 0; i < MAX_STAGES; i++) {
-      mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], CONSUMER_WARPS);
-      mbar_init(&tfull_bar[i], TRANSPOSE_WARPS);
+    for (int i = 0; i < MAX_SLOTS; i++) {
+      mbar_init(&bar.full_a[i], 1);
+      mbar_init(&bar.empty_a[i], CONSUMER_WARPS);
+      mbar_init(&bar.full_b[i], 1);
+      mbar_init(&bar.empty_b[i], TRANSPOSE_WARPS);
+      mbar_init(&bar.full_t[i], TRANSPOSE_WARPS);
+      mbar_init(&bar.empty_t[i], CONSUMER_WARPS);
     }
     asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
   }
   __syncthreads();
-
-  const int n_items = a.tiles * 2 * a.splits;
-  const int first = (int)blockIdx.x, stride = (int)gridDim.x;
-  const int64_t per = ((a.rows + a.splits - 1) / a.splits + KS - 1) / KS * KS;
-
-  if (warp >= CONSUMER_WARPS) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;\n" ::"n"(PRODUCER_REGS));
-    if (warp > CONSUMER_WARPS) {
-      // ===================== B transposers =====================
-      transpose_loop(a, stage_base, full_bar, tfull_bar, S, n_items, per, first, stride, warp - CONSUMER_WARPS - 1);
-    } else if (lane == 0) {
-      // ===================== TMA producer =====================
-      asm volatile("prefetch.tensormap [%0];\n" ::"l"(&tmap_a) : "memory");
-      asm volatile("prefetch.tensormap [%0];\n" ::"l"(&tmap_b) : "memory");
-      const int nst = stages_for(S), sbytes = stage_bytes_for(S);
-      int st = 0;
-      uint32_t ph = 0;
-      bool alive = true;
-      for (int item = first; alive && item < n_items; item += stride) {
-        const ItemInfo info = decode_item(a, item, per);
-        for (int ks = 0; ks < info.nsteps; ks++) {
-          if (!mbar_wait(&empty_bar[st], ph ^ 1, a.err)) { alive = false; break; }
-          uint8_t *sb = stage_base + st * sbytes;
-          mbar_expect_tx(&full_bar[st], S * (A_PLANE_BYTES + B_PLANE_BYTES));
-          const int krow = (int)(info.k_begin + (int64_t)ks * KS);
-          for (int s = 0; s < S; s++) {
-            tma_load_3d(sb + s * A_PLANE_BYTES, &tmap_a, &full_bar[st], info.bi * TILE, krow, s);
-            tma_load_3d(sb + S * A_PLANE_BYTES + s * B_PLANE_BYTES, &tmap_b, &full_bar[st],
-                        info.bj * TILE + info.h * HALF, krow, s);
-          }
-          if (++st == nst) { st = 0; ph ^= 1; }
-        }
-      }
-    }
-  } else {
-    // ===================== wgmma + epilogue =====================
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;\n" ::"n"(CONSUMER_REGS));
-    if (S == 4) consumer_loop<4>(a, stage_base, full_bar, tfull_bar, empty_bar, n_items, per, first, stride);
-    else if (S == 3) consumer_loop<3>(a, stage_base, full_bar, tfull_bar, empty_bar, n_items, per, first, stride);
-    else consumer_loop<2>(a, stage_base, full_bar, tfull_bar, empty_bar, n_items, per, first, stride);
-  }
+  const int S = *a.S_dev;
+  if (S == 4) syrk_tc_cta<4, TRACE>(&tmap_a, &tmap_b, a, ring, bar);
+  else if (S == 3) syrk_tc_cta<3, TRACE>(&tmap_a, &tmap_b, a, ring, bar);
+  else syrk_tc_cta<2, TRACE>(&tmap_a, &tmap_b, a, ring, bar);
 }
 
 // Column scales and digit-plane count of one batch, decided ON THE DEVICE from the column maxima and sums of squares
@@ -547,13 +692,25 @@ int encode_tc_maps(int8_t *planes, int ldq, int64_t rows_alloc, CUtensorMap *map
 
 // One syrk_tc_kernel launch on c's stream: rows_padded (a multiple of KS) contraction rows of the planes behind the
 // maps, nb x nb blocks of 128 columns, `splits` k-splits; one CTA per item up to one per SM.
+// With c->tc_trace (BALM_TC_TRACE) the traced instantiation runs and records the launch.
 int launch_syrk_tc(balm_ctx *c, const CUtensorMap &map_a, const CUtensorMap &map_b, int64_t rows_padded, int nb,
                    int tiles, int splits, const int *S_dev, const double *isc, double *part, bool accumulate, int *err) {
-  TcArgs a{rows_padded, nb, tiles, splits, S_dev, isc, part, accumulate ? 1 : 0, err};
+  TcArgs a{rows_padded, nb, tiles, splits, S_dev, isc, part, accumulate ? 1 : 0, err, c->tc_trace};
   const int items = a.tiles * 2 * a.splits;
   const int grid = items < c->sm_count ? items : c->sm_count;
-  syrk_tc_kernel<<<grid, TC_THREADS, TC_SMEM, c->stream>>>(map_a, map_b, a);
+  if (c->tc_trace) {
+    CUDA_TRY(cudaMemsetAsync(c->tc_trace, 0, sizeof(unsigned long long) * c->sm_count * TR_WORDS, c->stream));
+    syrk_tc_kernel<true><<<grid, TC_THREADS, TC_SMEM, c->stream>>>(map_a, map_b, a);
+  } else {
+    syrk_tc_kernel<false><<<grid, TC_THREADS, TC_SMEM, c->stream>>>(map_a, map_b, a);
+  }
   CUDA_TRY(cudaGetLastError());
+  return BALM_OK;
+}
+
+int syrk_tc_set_smem() {
+  CUDA_TRY(cudaFuncSetAttribute(syrk_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM));
+  CUDA_TRY(cudaFuncSetAttribute(syrk_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM));
   return BALM_OK;
 }
 
@@ -599,7 +756,7 @@ int tensor_syrk_init(balm_ctx *c) {
     CUDA_TRY(cudaMalloc((void **)&c->syrk_part,
                         sizeof(double) * (size_t)c->syrk_splits * c->syrk_tiles * TILE * TILE));
   }
-  CUDA_TRY(cudaFuncSetAttribute(syrk_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM));
+  TRY(syrk_tc_set_smem());
   return BALM_OK;
 }
 
@@ -734,7 +891,7 @@ extern "C" int balm_debug_syrk_tc(balm_ctx *c, const int8_t *planes, int S, int6
   CUDA_TRY(cudaMemsetAsync(d_err, 0, sizeof(int), c->stream));
   CUtensorMap map_a, map_b;
   TRY(encode_tc_maps(d_planes, ldq, rows_padded, &map_a, &map_b));
-  CUDA_TRY(cudaFuncSetAttribute(syrk_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM));
+  TRY(syrk_tc_set_smem());
   TRY(launch_syrk_tc(c, map_a, map_b, rows_padded, nb, tiles, splits, d_S, d_isc, d_part, accumulate != 0, d_err));
   int err = 0;
   CUDA_TRY(cudaMemcpyAsync(&err, d_err, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
@@ -766,5 +923,17 @@ extern "C" int balm_debug_tc_planes(balm_ctx *c, int8_t *planes, double *isc, in
   if (S) *S = s;
   if (rows_padded) *rows_padded = st->last_rows_padded;
   if (splits) *splits = c->syrk_splits;
+  return BALM_OK;
+}
+
+extern "C" int balm_debug_tc_trace(balm_ctx *c, unsigned long long *out, int max_entries) {
+  if (!c || !out || !c->tc_trace || max_entries < 0) {
+    balm_set_error("balm_debug_tc_trace: no trace (BALM_TC_TRACE=1 at the creation of a tensor-precision context)");
+    return BALM_ERR_INVALID;
+  }
+  CUDA_TRY(cudaSetDevice(c->device));
+  CUDA_TRY(cudaStreamSynchronize(c->stream));
+  const size_t total = std::min<size_t>((size_t)max_entries, (size_t)c->sm_count * TR_WORDS);
+  CUDA_TRY(cudaMemcpy(out, c->tc_trace, sizeof(unsigned long long) * total, cudaMemcpyDeviceToHost));
   return BALM_OK;
 }
