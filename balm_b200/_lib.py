@@ -52,7 +52,9 @@ SYMBOLS = ["balm_last_error", "balm_version", "balm_create", "balm_destroy", "ba
            "balm_download_keys", "balm_window_reset", "balm_window_cut", "balm_window_recut", "balm_window_marginalize",
            "balm_window_push", "balm_batch_create", "balm_batch_destroy", "balm_batch_set_voxels", "balm_batch_evaluate",
            "balm_batch_damping_iter", "balm_batch_cut_voxels", "balm_batch_sizes", "balm_batch_download_voxels",
-           "balm_batch_pose_covariance", "balm_batch_marginalize", "balm_batch_append_scan", "balm_batch_download_fix"]
+           "balm_batch_pose_covariance", "balm_batch_marginalize", "balm_batch_append_scan", "balm_batch_download_fix",
+           "balm_batch_window_reset", "balm_batch_window_cut", "balm_batch_window_recut", "balm_batch_window_marginalize",
+           "balm_batch_window_push"]
 
 
 def lib():
@@ -122,6 +124,11 @@ def lib():
         L.balm_batch_marginalize.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
         L.balm_batch_append_scan.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int] + [C.c_void_p] * 6
         L.balm_batch_download_fix.argtypes = [C.c_void_p, C.c_void_p]
+        L.balm_batch_window_reset.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.POINTER(AssocOpts)]
+        L.balm_batch_window_cut.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int] + [C.c_void_p] * 3
+        L.balm_batch_window_recut.argtypes = [C.c_void_p, C.c_void_p]
+        L.balm_batch_window_marginalize.argtypes = [C.c_void_p] + [C.c_void_p] * 3
+        L.balm_batch_window_push.argtypes = [C.c_void_p] + [C.c_void_p] * 3
         _lib = L
     return _lib
 

@@ -229,6 +229,7 @@ class Batch:
     def __init__(self, device=0):
         self._h = C.c_void_p()
         self.n_poses = []
+        self._win_slots = None
         L.check(L.lib().balm_batch_create(C.byref(self._h), int(device)))
 
     def close(self):
@@ -322,6 +323,61 @@ class Batch:
         L.check(L.lib().balm_batch_append_scan(self._h, _p(scan_of), _p(slots), len(scans), _p(scan_ptr), _p(xyz),
                                                _p(poses), _p(M), _p(K), _p(m)))
         return [(int(a), int(b), int(c)) for a, b, c in zip(M, K, m)]
+
+    # ---- persistent sliding-window octrees, one per problem ----
+    def window_reset(self, n_slots, voxel_size=2.0, layer_limit=2, min_ps=15,
+                     eigen_value_array=(1.0 / 16, 1.0 / 16, 1.0 / 9)):
+        """Empty window maps (include/balm_b200.h, balm_batch_window_*): problem p gets n_slots[p] (1 .. 32) slots, every
+        problem these association parameters. Problem p is a Context(n_slots[p]) window driven by the same calls."""
+        ns = np.ascontiguousarray([int(n) for n in n_slots], dtype=np.int32)
+        o = L.AssocOpts(float(voxel_size), int(layer_limit), int(min_ps), (C.c_double * 3)(*eigen_value_array))
+        L.check(L.lib().balm_batch_window_reset(self._h, len(ns), _p(ns), C.byref(o)))
+        self._win_slots = [int(n) for n in ns]
+
+    def _win_poses(self, poses_list):
+        if self._win_slots is None:  # no window_reset yet: the library refuses the call
+            return np.zeros((1, 12))
+        assert len(poses_list) == len(self._win_slots)
+        return np.ascontiguousarray(np.concatenate([np.asarray(p, dtype=np.float64).reshape(n, 12)
+                                                    for p, n in zip(poses_list, self._win_slots)]), dtype=np.float64)
+
+    def window_cut(self, scans, scan_of, slots, poses_list):
+        """Context.window_cut per problem, all in one call. scans: list of (n_s x 3) body-frame points, each uploaded once;
+        scan_of[p]: the scan problem p takes into slot slots[p] at its pose poses_list[p][slots[p]], or -1 (map left
+        alone); poses_list: per problem its n_slots[p] x 12 poses."""
+        scans = [np.asarray(s, dtype=np.float32).reshape(-1, 3) for s in scans]
+        scan_ptr = np.concatenate([[0], np.cumsum([len(s) for s in scans])]).astype(np.int64)
+        xyz = np.ascontiguousarray(np.concatenate(scans) if scans else np.zeros((0, 3)), dtype=np.float32)
+        scan_of = np.ascontiguousarray(scan_of, dtype=np.int32)
+        slots = np.ascontiguousarray(slots, dtype=np.int32)
+        poses = self._win_poses(poses_list)
+        L.check(L.lib().balm_batch_window_cut(self._h, _p(scan_of), _p(slots), len(scans), _p(scan_ptr), _p(xyz),
+                                              _p(poses)))
+
+    def window_recut(self, win_counts):
+        """Context.window_recut(win_counts[p]) per problem; 0 leaves a map alone."""
+        w = np.ascontiguousarray(win_counts, dtype=np.int32)
+        L.check(L.lib().balm_batch_window_recut(self._h, _p(w)))
+
+    def window_marginalize(self, mg_sizes, poses_list, win_counts):
+        """Context.window_marginalize(mg_sizes[p], poses_list[p], win_counts[p]) per problem; mg 0 leaves a map alone.
+        poses_list: per problem n_slots[p] x 12 poses, or None (no re-transform)."""
+        mg = np.ascontiguousarray(mg_sizes, dtype=np.int32)
+        w = np.ascontiguousarray(win_counts, dtype=np.int32)
+        poses = None if poses_list is None else self._win_poses(poses_list)
+        L.check(L.lib().balm_batch_window_marginalize(self._h, _p(mg), _p(poses), _p(w)))
+
+    def window_push(self, win_counts):
+        """Context.window_push(win_counts[p]) per problem, registered as the batch's problems (n_poses = n_slots, fix
+        clusters, keys); win_counts[p] == 0 gives problem p an empty voxel range. -> per problem (M, K)."""
+        w = np.ascontiguousarray(win_counts, dtype=np.int32)
+        B = len(self._win_slots or [])
+        M = np.zeros(B, dtype=np.int64)
+        K = np.zeros(B, dtype=np.int64)
+        L.check(L.lib().balm_batch_window_push(self._h, _p(w), _p(M), _p(K)))
+        self.n_poses = list(self._win_slots)
+        self._pose_ptr = np.concatenate([[0], np.cumsum(self.n_poses)]).astype(np.int64)
+        return [(int(m), int(k)) for m, k in zip(M, K)]
 
     def download_voxels(self, with_keys=False, with_fix=False):
         """The current registration, per problem a dict set_problems accepts (row_ptr re-based to 0); with_keys adds

@@ -1193,33 +1193,52 @@ int batch_append_build(cudaStream_t st, const BatchVoxels &in, const balm_assoc_
 //   OCTO_TREE_NODE::recut / judge_eigen / cut_func                :737-776, 654-699, 700-735
 //   OCTO_TREE_ROOT::marginalize -> OCTO_TREE_NODE::to_margi       :948-963, 778-816
 //   OCTO_TREE_NODE::tras_opt -> VOX_HESS::push_voxel              :908-929, 30-51
+// One state holds the maps of B independent problems (balm_batch_window_*); a context's balm_window_* is the case B = 1.
 // State (all device arrays, grown by doubling, nothing is ever deleted from the node table):
-//   node table, append-only (a node's id never changes): 63-bit key, layer, split flag (octo_state), push_state,
-//     fix_point [10], and per window slot the clusters sig_orig / sig_tran [N][10]. A per-layer table of (key, id)
-//     sorted by key finds a node (a key digit 7 is both "not split" and octant 7, so keys are only unique per layer).
-//   point store: body xyz (vec_orig, float as given), world xyz (vec_tran, fp64), slot, node id and an order stamp.
-//     The stamp orders the points of one (node, slot) list as the reference's vector holds them: a cut stamps
-//     (op << 32 | input index), a move into a child restamps the moved points (op << 32 | rank in stamp order), so
-//     they land after the child's earlier points and keep their parent's order.
+//   node table, append-only (a node's id never changes): 63-bit key, problem, layer, split flag (octo_state),
+//     push_state, fix_point [10], and per window slot the clusters sig_orig / sig_tran [N][10], N = the largest slot
+//     count of the problems. A per-layer table of node ids sorted by (problem, key), with per-problem offsets, finds a
+//     node inside its problem's range (a key digit 7 is both "not split" and octant 7, so keys are only unique per
+//     layer and problem).
+//   point store: body xyz (vec_orig, float as given), world xyz (vec_tran, fp64), slot, problem, node id and an order
+//     stamp. The stamp orders the points of one (node, slot) list as the reference's vector holds them: a cut stamps
+//     (op << 32 | rank of the point among the call's items), a move into a child restamps the moved points (op << 32 |
+//     rank in stamp order), so they land after the child's earlier points and keep their parent's order. A cut's items
+//     are the points of every problem in (problem, scan point) order, so within one problem the stamps order its points
+//     as a context holding that problem alone orders them.
+//   per-problem table (WinProb): slot count and first pose row, and the call's win_count / mg_size, 0 = problem left
+//     alone by this call.
 // Clusters are accumulated point by point in that order, exactly as PointCluster::push runs, so sums of the device
-// and of the reference round alike. Split nodes keep whatever points are left in them (slots the recut did not move);
-// nothing reads them unless a later recut(win_count) with win_count - 1 == that slot moves them, as in the reference.
+// and of the reference round alike; a (node, slot) belongs to one problem, so a problem's sums do not depend on the
+// rest of the batch, and node ids never reach the output. Split nodes keep whatever points are left in them (slots
+// the recut did not move); nothing reads them unless a later recut(win_count) with win_count - 1 == that slot moves
+// them, as in the reference.
 namespace {
+struct WinProb {
+  int n_slots, pose_base;
+  int w, mg;  // of the current call
+};
 struct WinLookup {
   int n = 0;
-  unsigned long long *key = nullptr;
-  int *id = nullptr;
+  unsigned long long *key = nullptr;  // [n] sorted by (problem, key)
+  int *id = nullptr;                  // [n]
+  int *off = nullptr;                 // [B + 1] the range of each problem
 };
 }  // namespace
 
 struct WindowState {
   AssocParams P;
-  int N = 0;
-  unsigned long long op = 1;  // stamp counter
+  balm_assoc_opts opts;
+  bool batch = false;              // balm_batch_window_*: errors name the problem, too many points is UNSUPPORTED
+  int B = 0, N = 0;                // problems, slot stride (max n_slots)
+  std::vector<WinProb> hprob;
+  std::vector<int> n_slots;
+  WinProb *prob = nullptr;         // device [B]
+  unsigned long long op = 1;       // stamp counter
   // nodes
   int nn = 0, ncap = 0;
   unsigned long long *nkey = nullptr;
-  int *nlayer = nullptr, *nsplit = nullptr, *npush = nullptr, *naction = nullptr;
+  int *nprob = nullptr, *nlayer = nullptr, *nsplit = nullptr, *npush = nullptr, *naction = nullptr;
   double *nfix = nullptr;          // [ncap][10]
   double *sig_o = nullptr, *sig_t = nullptr;  // [ncap][N][10]
   WinLookup look[3];
@@ -1227,12 +1246,13 @@ struct WindowState {
   int64_t np = 0, pcap = 0;
   float *pxyz = nullptr;
   double *ptran = nullptr;
-  int *pslot = nullptr, *pnode = nullptr;
+  int *pslot = nullptr, *pprob = nullptr, *pnode = nullptr;
   unsigned long long *pstamp = nullptr;
   ~WindowState() {
-    void *ps[] = {nkey, nlayer, nsplit, npush, naction, nfix, sig_o, sig_t, pxyz, ptran, pslot, pnode, pstamp,
-                  look[0].key, look[0].id, look[1].key, look[1].id, look[2].key, look[2].id};
+    void *ps[] = {prob, nkey, nprob, nlayer, nsplit, npush, naction, nfix, sig_o, sig_t, pxyz, ptran, pslot, pprob, pnode,
+                  pstamp};
     for (void *q : ps) cudaFree(q);
+    for (WinLookup &l : look) { cudaFree(l.key); cudaFree(l.id); cudaFree(l.off); }
   }
 };
 
@@ -1254,22 +1274,38 @@ int win_reserve_nodes(WindowState &w, int need) {
   if (need <= w.ncap) return BALM_OK;
   int cap = std::max(need, std::max(1024, 2 * w.ncap));
   const size_t nn = (size_t)w.nn, c = (size_t)cap, NS = (size_t)w.N * 10;
-  TRY(grow_array(&w.nkey, nn, c)); TRY(grow_array(&w.nlayer, nn, c)); TRY(grow_array(&w.nsplit, nn, c));
-  TRY(grow_array(&w.npush, nn, c)); TRY(grow_array(&w.naction, nn, c)); TRY(grow_array(&w.nfix, nn * 10, c * 10));
+  TRY(grow_array(&w.nkey, nn, c)); TRY(grow_array(&w.nprob, nn, c)); TRY(grow_array(&w.nlayer, nn, c));
+  TRY(grow_array(&w.nsplit, nn, c)); TRY(grow_array(&w.npush, nn, c)); TRY(grow_array(&w.naction, nn, c));
+  TRY(grow_array(&w.nfix, nn * 10, c * 10));
   TRY(grow_array(&w.sig_o, nn * NS, c * NS)); TRY(grow_array(&w.sig_t, nn * NS, c * NS));
   w.ncap = cap;
   return BALM_OK;
 }
 int win_reserve_points(WindowState &w, int64_t need) {
   if (need <= w.pcap) return BALM_OK;
-  if (need >= (1ll << 31)) { balm_set_error("balm_window_cut: more than 2^31 points in the window"); return BALM_ERR_UNSUPPORTED; }
   int64_t cap = std::max<int64_t>(need, std::max<int64_t>(1 << 16, 2 * w.pcap));
   cap = std::min<int64_t>(cap, (1ll << 31) - 1);
   const size_t n = (size_t)w.np, c = (size_t)cap;
   TRY(grow_array(&w.pxyz, 3 * n, 3 * c)); TRY(grow_array(&w.ptran, 3 * n, 3 * c)); TRY(grow_array(&w.pslot, n, c));
-  TRY(grow_array(&w.pnode, n, c)); TRY(grow_array(&w.pstamp, n, c));
+  TRY(grow_array(&w.pprob, n, c)); TRY(grow_array(&w.pnode, n, c)); TRY(grow_array(&w.pstamp, n, c));
   w.pcap = cap;
   return BALM_OK;
+}
+
+// the call's win_count / mg_size per problem (null: 0) into the device table
+int win_upload(WindowState &w, cudaStream_t st, const int *wc, const int *mg) {
+  for (int p = 0; p < w.B; p++) {
+    w.hprob[p].w = wc ? wc[p] : 0;
+    w.hprob[p].mg = mg ? mg[p] : 0;
+  }
+  CUDA_TRY(cudaMemcpyAsync(w.prob, w.hprob.data(), sizeof(WinProb) * w.B, cudaMemcpyHostToDevice, st));
+  return BALM_OK;
+}
+
+int radix_bits(unsigned long long maxval) {  // bits that hold every value in [0, maxval]
+  int bits = 1;
+  while (bits < 64 && (maxval >> bits)) bits++;
+  return bits;
 }
 
 // cub temporary storage from the pool
@@ -1286,54 +1322,132 @@ struct CubTmp {
   }
 };
 
+// index of key k among problem p's entries of a lookup table, or -1
+__device__ __forceinline__ int look_find(const unsigned long long *key, const int *off, int p, unsigned long long k) {
+  const int a = off[p];
+  const int i = find_key(key + a, off[p + 1] - a, k);
+  return i < 0 ? -1 : a + i;
+}
+
 __global__ void win_iota_kernel(int *v, int64_t n, int base) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) v[i] = base + (int)i;
 }
-__global__ void win_missing_kernel(const unsigned long long *keys, int m, const unsigned long long *look, int nlook,
-                                   int *miss) {
+__global__ void win_missing_kernel(const unsigned long long *keys, const int *probs, int m, const unsigned long long *look,
+                                   const int *off, int *miss) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < m) miss[i] = find_key(look, nlook, keys[i]) < 0 ? 1 : 0;
+  if (i < m) miss[i] = look_find(look, off, probs[i], keys[i]) < 0 ? 1 : 0;
 }
-__global__ void win_init_nodes_kernel(const unsigned long long *keys, int m, int base, int layer, unsigned long long *nkey,
-                                      int *nlayer, int *nsplit, int *npush, double *nfix) {
+// first of every (problem, key) run of a sorted list
+__global__ void win_unique_flag_kernel(const unsigned long long *keys, const int *probs, int m, int *flag) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < m) flag[i] = (i == 0 || keys[i] != keys[i - 1] || probs[i] != probs[i - 1]) ? 1 : 0;
+}
+__global__ void win_init_nodes_kernel(const unsigned long long *keys, const int *probs, int m, int base, int layer,
+                                      unsigned long long *nkey, int *nprob, int *nlayer, int *nsplit, int *npush,
+                                      double *nfix) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= m) return;
   const int v = base + i;
-  nkey[v] = keys[i]; nlayer[v] = layer; nsplit[v] = 0; npush[v] = 0;
+  nkey[v] = keys[i]; nprob[v] = probs[i]; nlayer[v] = layer; nsplit[v] = 0; npush[v] = 0;
 #pragma unroll
   for (int q = 0; q < 10; q++) nfix[(size_t)v * 10 + q] = 0.0;
 }
-// node id of every key (the key is in the layer's table)
-__global__ void win_find_kernel(const unsigned long long *keys, const int *sel, int m, const unsigned long long *look,
-                                const int *look_id, int nlook, int *node_out /*indexed by sel[i] or i*/) {
+// node id of every key (the key is in its problem's range of the layer's table)
+__global__ void win_find_kernel(const unsigned long long *keys, const int *probs, const int *sel, int m,
+                                const unsigned long long *look, const int *look_id, const int *off,
+                                int *node_out /*indexed by sel[i] or i*/) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= m) return;
-  node_out[sel ? sel[i] : i] = look_id[find_key(look, nlook, keys[i])];
+  node_out[sel ? sel[i] : i] = look_id[look_find(look, off, probs[i], keys[i])];
+}
+__global__ void win_gather_i32_kernel(const int *src, const int *idx, int m, int *dst) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < m) dst[i] = src[idx[i]];
+}
+__global__ void win_gather_u64_kernel(const unsigned long long *src, const int *idx, int m, unsigned long long *dst) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < m) dst[i] = src[idx[i]];
+}
+// off[p] = first entry of problem p (and off[B] = n) in a list of node ids sorted by problem
+__global__ void win_offsets_kernel(const int *ids, int n, const int *nprob, int B, int *off) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p > B) return;
+  int lo = 0, hi = n;
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (nprob[ids[mid]] < p) lo = mid + 1; else hi = mid;
+  }
+  off[p] = lo;
 }
 
-// the layer-L nodes that `keys` (m keys, any order, duplicates allowed) name and that do not exist yet are appended to
-// the node table in ascending key order, and the layer's lookup table is rebuilt
-int win_add_nodes(WindowState &w, ScratchPool &pool, CubTmp &tmp, cudaStream_t st, const unsigned long long *keys, int m,
-                  int L) {
+// node ids in ascending (problem, key): sorted by key (64 bits), then stably by problem when there is more than one.
+// ids / keys: n entries, permuted in place through the scratch buffers ids2 / keys2 (n each).
+int win_sort_ids(WindowState &w, ScratchPool &pool, CubTmp &tmp, cudaStream_t st, unsigned long long *&keys, int *&ids,
+                 unsigned long long *&keys2, int *&ids2, int n) {
+  size_t b1 = 0;
+  cub::DeviceRadixSort::SortPairs(nullptr, b1, keys, keys2, ids, ids2, n, 0, 64, st);
+  TRY(tmp.need(b1));
+  CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp.p, tmp.bytes, keys, keys2, ids, ids2, n, 0, 64, st));
+  std::swap(keys, keys2);
+  std::swap(ids, ids2);
+  if (w.B == 1) return BALM_OK;
+  int *pr = nullptr, *pr2 = nullptr;
+  TRY(pool.get(&pr, n)); TRY(pool.get(&pr2, n));
+  const unsigned g = (unsigned)((n + 255) / 256);
+  win_gather_i32_kernel<<<g, 256, 0, st>>>(w.nprob, ids, n, pr);
+  const int bits = radix_bits((unsigned long long)(w.B - 1));
+  size_t b2 = 0;
+  cub::DeviceRadixSort::SortPairs(nullptr, b2, pr, pr2, ids, ids2, n, 0, bits, st);
+  TRY(tmp.need(b2));
+  CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp.p, tmp.bytes, pr, pr2, ids, ids2, n, 0, bits, st));  // stable
+  std::swap(ids, ids2);
+  win_gather_u64_kernel<<<g, 256, 0, st>>>(w.nkey, ids, n, keys);
+  return BALM_OK;
+}
+
+// the layer-L nodes that (keys, probs) (m entries, any order, duplicates allowed) name and that do not exist yet are
+// appended to the node table in ascending (problem, key) order, and the layer's lookup table is rebuilt
+int win_add_nodes(WindowState &w, ScratchPool &pool, CubTmp &tmp, cudaStream_t st, const unsigned long long *keys,
+                  const int *probs, int m, int L) {
   if (m < 1) return BALM_OK;
   WinLookup &lk = w.look[L];
-  int *miss = nullptr, *nsel = nullptr;
+  int *miss = nullptr, *nsel = nullptr, *selp = nullptr, *sp = nullptr, *flag = nullptr, *up = nullptr;
   unsigned long long *sel = nullptr, *sorted = nullptr, *uniq = nullptr;
-  TRY(pool.get(&miss, m)); TRY(pool.get(&nsel, 1)); TRY(pool.get(&sel, m)); TRY(pool.get(&sorted, m)); TRY(pool.get(&uniq, m));
-  win_missing_kernel<<<(m + 255) / 256, 256, 0, st>>>(keys, m, lk.key, lk.n, miss);
-  size_t b1 = 0, b2 = 0, b3 = 0;
+  TRY(pool.get(&miss, m)); TRY(pool.get(&nsel, 1)); TRY(pool.get(&sel, m)); TRY(pool.get(&sorted, m));
+  TRY(pool.get(&uniq, m)); TRY(pool.get(&selp, m)); TRY(pool.get(&sp, m)); TRY(pool.get(&flag, m)); TRY(pool.get(&up, m));
+  win_missing_kernel<<<(m + 255) / 256, 256, 0, st>>>(keys, probs, m, lk.key, lk.off, miss);
+  size_t b1 = 0, b2 = 0;
   cub::DeviceSelect::Flagged(nullptr, b1, keys, miss, sel, nsel, m, st);
-  cub::DeviceRadixSort::SortKeys(nullptr, b2, sel, sorted, m, 0, 64, st);
-  cub::DeviceSelect::Unique(nullptr, b3, sorted, uniq, nsel, m, st);
-  TRY(tmp.need(std::max(b1, std::max(b2, b3))));
+  cub::DeviceSelect::Flagged(nullptr, b2, probs, miss, selp, nsel, m, st);
+  TRY(tmp.need(std::max(b1, b2)));
+  CUDA_TRY(cub::DeviceSelect::Flagged(tmp.p, tmp.bytes, probs, miss, selp, nsel, m, st));
   CUDA_TRY(cub::DeviceSelect::Flagged(tmp.p, tmp.bytes, keys, miss, sel, nsel, m, st));
   int nmiss = 0;
   CUDA_TRY(cudaMemcpyAsync(&nmiss, nsel, sizeof(int), cudaMemcpyDeviceToHost, st));
   CUDA_TRY(cudaStreamSynchronize(st));
   if (nmiss == 0) return BALM_OK;
-  CUDA_TRY(cub::DeviceRadixSort::SortKeys(tmp.p, tmp.bytes, sel, sorted, nmiss, 0, 64, st));
-  CUDA_TRY(cub::DeviceSelect::Unique(tmp.p, tmp.bytes, sorted, uniq, nsel, nmiss, st));
+  // (problem, key) of the missing entries in ascending order: by key, then stably by problem
+  size_t b3 = 0;
+  cub::DeviceRadixSort::SortPairs(nullptr, b3, sel, sorted, selp, sp, nmiss, 0, 64, st);
+  TRY(tmp.need(b3));
+  CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp.p, tmp.bytes, sel, sorted, selp, sp, nmiss, 0, 64, st));
+  if (w.B > 1) {
+    const int bits = radix_bits((unsigned long long)(w.B - 1));
+    size_t b4 = 0;
+    cub::DeviceRadixSort::SortPairs(nullptr, b4, sp, selp, sorted, sel, nmiss, 0, bits, st);
+    TRY(tmp.need(b4));
+    CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp.p, tmp.bytes, sp, selp, sorted, sel, nmiss, 0, bits, st));
+    std::swap(sp, selp);
+    std::swap(sorted, sel);
+  }
+  win_unique_flag_kernel<<<(nmiss + 255) / 256, 256, 0, st>>>(sorted, sp, nmiss, flag);
+  size_t b5 = 0, b6 = 0;
+  cub::DeviceSelect::Flagged(nullptr, b5, sorted, flag, uniq, nsel, nmiss, st);
+  cub::DeviceSelect::Flagged(nullptr, b6, sp, flag, up, nsel, nmiss, st);
+  TRY(tmp.need(std::max(b5, b6)));
+  CUDA_TRY(cub::DeviceSelect::Flagged(tmp.p, tmp.bytes, sp, flag, up, nsel, nmiss, st));
+  CUDA_TRY(cub::DeviceSelect::Flagged(tmp.p, tmp.bytes, sorted, flag, uniq, nsel, nmiss, st));
   int nnew = 0;
   CUDA_TRY(cudaMemcpyAsync(&nnew, nsel, sizeof(int), cudaMemcpyDeviceToHost, st));
   CUDA_TRY(cudaStreamSynchronize(st));
@@ -1343,30 +1457,38 @@ int win_add_nodes(WindowState &w, ScratchPool &pool, CubTmp &tmp, cudaStream_t s
   }
   TRY(win_reserve_nodes(w, w.nn + nnew));
   const int base = w.nn;
-  win_init_nodes_kernel<<<(nnew + 255) / 256, 256, 0, st>>>(uniq, nnew, base, L, w.nkey, w.nlayer, w.nsplit, w.npush, w.nfix);
+  win_init_nodes_kernel<<<(nnew + 255) / 256, 256, 0, st>>>(uniq, up, nnew, base, L, w.nkey, w.nprob, w.nlayer, w.nsplit,
+                                                            w.npush, w.nfix);
   CUDA_TRY(cudaMemsetAsync(w.sig_o + (size_t)base * w.N * 10, 0, sizeof(double) * (size_t)nnew * w.N * 10, st));
   CUDA_TRY(cudaMemsetAsync(w.sig_t + (size_t)base * w.N * 10, 0, sizeof(double) * (size_t)nnew * w.N * 10, st));
-  // lookup: old (key, id) pairs + the new ones, sorted by key
+  // lookup: old (key, id) pairs + the new ones, sorted by (problem, key)
   const int nl = lk.n + nnew;
-  unsigned long long *k_in = nullptr, *k_out = nullptr;
-  int *i_in = nullptr, *i_out = nullptr;
-  TRY(pool.get(&k_in, nl)); TRY(pool.get(&i_in, nl));
-  CUDA_TRY(cudaMalloc((void **)&k_out, sizeof(unsigned long long) * nl));
-  if (cudaMalloc((void **)&i_out, sizeof(int) * nl) != cudaSuccess) { cudaFree(k_out); CUDA_TRY(cudaErrorMemoryAllocation); }
+  unsigned long long *k_in = nullptr, *k2 = nullptr;
+  int *i_in = nullptr, *i2 = nullptr;
+  TRY(pool.get(&k_in, nl)); TRY(pool.get(&i_in, nl)); TRY(pool.get(&k2, nl)); TRY(pool.get(&i2, nl));
   if (lk.n) {
     CUDA_TRY(cudaMemcpyAsync(k_in, lk.key, sizeof(unsigned long long) * lk.n, cudaMemcpyDeviceToDevice, st));
     CUDA_TRY(cudaMemcpyAsync(i_in, lk.id, sizeof(int) * lk.n, cudaMemcpyDeviceToDevice, st));
   }
   CUDA_TRY(cudaMemcpyAsync(k_in + lk.n, uniq, sizeof(unsigned long long) * nnew, cudaMemcpyDeviceToDevice, st));
   win_iota_kernel<<<(nnew + 255) / 256, 256, 0, st>>>(i_in + lk.n, nnew, base);
-  size_t b4 = 0;
-  cub::DeviceRadixSort::SortPairs(nullptr, b4, k_in, k_out, i_in, i_out, nl, 0, 64, st);
-  TRY(tmp.need(b4));
-  CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp.p, tmp.bytes, k_in, k_out, i_in, i_out, nl, 0, 64, st));
+  TRY(win_sort_ids(w, pool, tmp, st, k_in, i_in, k2, i2, nl));
+  unsigned long long *k_out = nullptr;
+  int *i_out = nullptr, *o_out = nullptr;
+  if (cudaMalloc((void **)&k_out, sizeof(unsigned long long) * nl) != cudaSuccess ||
+      cudaMalloc((void **)&i_out, sizeof(int) * nl) != cudaSuccess ||
+      cudaMalloc((void **)&o_out, sizeof(int) * (w.B + 1)) != cudaSuccess) {
+    cudaFree(k_out); cudaFree(i_out); cudaFree(o_out);
+    CUDA_TRY(cudaErrorMemoryAllocation);
+  }
+  CUDA_TRY(cudaMemcpyAsync(k_out, k_in, sizeof(unsigned long long) * nl, cudaMemcpyDeviceToDevice, st));
+  CUDA_TRY(cudaMemcpyAsync(i_out, i_in, sizeof(int) * nl, cudaMemcpyDeviceToDevice, st));
+  win_offsets_kernel<<<(w.B + 128) / 128, 128, 0, st>>>(i_out, nl, w.nprob, w.B, o_out);
   CUDA_TRY(cudaStreamSynchronize(st));
   cudaFree(lk.key);
   cudaFree(lk.id);
-  lk.key = k_out; lk.id = i_out; lk.n = nl;
+  cudaFree(lk.off);
+  lk.key = k_out; lk.id = i_out; lk.off = o_out; lk.n = nl;
   w.nn += nnew;
   return BALM_OK;
 }
@@ -1416,8 +1538,7 @@ int win_push_points(WindowState &w, ScratchPool &pool, CubTmp &tmp, cudaStream_t
   TRY(pool.get(&iota, m)); TRY(pool.get(&seg, m)); TRY(pool.get(&nsel, 1));
   const unsigned g = (unsigned)((m + 255) / 256);
   win_seg_key_kernel<<<g, 256, 0, st>>>(order, m, w.pnode, w.pslot, w.N, ck);
-  int bits = 1;
-  while (bits < 64 && ((unsigned long long)w.nn * (unsigned long long)w.N) >> bits) bits++;
+  const int bits = radix_bits((unsigned long long)w.nn * (unsigned long long)w.N);
   size_t b1 = 0, b2 = 0;
   cub::DeviceRadixSort::SortPairs(nullptr, b1, ck, ck2, order, ord2, m, 0, bits, st);
   cub::DeviceSelect::Flagged(nullptr, b2, iota, flag, seg, nsel, m, st);
@@ -1435,34 +1556,49 @@ int win_push_points(WindowState &w, ScratchPool &pool, CubTmp &tmp, cudaStream_t
   return BALM_OK;
 }
 
-// cut_voxel: world coordinate R p + t (fp64) and root key of every point of the scan
-__global__ void win_cut_kernel(const float *xyz, const double *pose12, int n, AssocParams p, double *tran,
-                               unsigned long long *rkey, int *bad) {
+// cut_voxel: world coordinate R p + t (fp64) and root key of every item (point src[i] of entry row[i] = (problem,
+// pose row, slot)); a point outside the root range flags its problem
+__global__ void win_cut_kernel(const float *xyz, const int *src, const int *row, const int4 *ent, const double *poses,
+                               int n, AssocParams p, double *tran, unsigned long long *rkey, int *iprob, int *bad) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
+  const int4 e = ent[row[i]];
   double r[9], t[3];
-  load_pose(pose12, r, t);
-  const double b[3] = {(double)xyz[3 * i], (double)xyz[3 * i + 1], (double)xyz[3 * i + 2]};
+  load_pose(poses + 12 * (size_t)e.y, r, t);
+  const int64_t j = src[i];
+  const double b[3] = {(double)xyz[3 * j], (double)xyz[3 * j + 1], (double)xyz[3 * j + 2]};
   double wp[3];
 #pragma unroll
   for (int a = 0; a < 3; a++) wp[a] = r[a * 3] * b[0] + r[a * 3 + 1] * b[1] + r[a * 3 + 2] * b[2] + t[a];
 #pragma unroll
   for (int a = 0; a < 3; a++) tran[3 * i + a] = wp[a];
-  rkey[i] = world_point_key(wp, p, bad) | 63ull;
+  rkey[i] = world_point_key(wp, p, bad + e.x) | 63ull;
+  iprob[i] = e.x;
 }
-__global__ void win_stamp_kernel(int *pslot, unsigned long long *pstamp, int n, int slot, unsigned long long op) {
+// the items into the point store from index 0 of the given arrays: body xyz, slot, problem, stamp (op << 32 | item)
+__global__ void win_store_kernel(const float *xyz, const int *src, const int *row, const int4 *ent, int n,
+                                 unsigned long long op, float *pxyz, int *pslot, int *pprob, unsigned long long *pstamp) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  pslot[i] = slot;
+  const int4 e = ent[row[i]];
+  const int64_t j = src[i];
+#pragma unroll
+  for (int a = 0; a < 3; a++) pxyz[3 * i + a] = xyz[3 * j + a];
+  pslot[i] = e.z;
+  pprob[i] = e.x;
   pstamp[i] = (op << 32) | (unsigned long long)i;
 }
 
-// recut, one layer: judge every node of layer L that is not split (recut :739-768); 1 = split earlier (only slot
-// win_count-1 moves, :770), 2 = split now (every slot < win_count moves, :766-767), 0 = no points move
-__global__ void win_judge_kernel(int nn, int L, int N, int w, AssocParams p, const int *nlayer, int *nsplit, int *npush,
-                                 const double *nfix, const double *sig_o, const double *sig_t, int *action) {
+// recut, one layer: judge every node of layer L that is not split (recut :739-768) in a problem this call recuts
+// (w = its win_count > 0); 1 = split earlier (only slot w-1 moves, :770), 2 = split now (every slot < w moves,
+// :766-767), 0 = no points move
+__global__ void win_judge_kernel(int nn, int L, int N, AssocParams p, const WinProb *prob, const int *nprob,
+                                 const int *nlayer, int *nsplit, int *npush, const double *nfix, const double *sig_o,
+                                 const double *sig_t, int *action) {
   const int v = blockIdx.x * blockDim.x + threadIdx.x;
   if (v >= nn || nlayer[v] != L) return;
+  const int w = prob[nprob[v]].w;
+  if (w == 0) return;
   if (nsplit[v]) { action[v] = 1; return; }
   action[v] = 0;
   npush[v] = 0;
@@ -1485,12 +1621,12 @@ __global__ void win_judge_kernel(int nn, int L, int N, int w, AssocParams p, con
   action[v] = 2;
 }
 // cut_func: the octant of every moving point around its node's float centre, and the child's key
-__global__ void win_move_kernel(int64_t np, int w, AssocParams p, const int *pnode, const int *pslot, const double *ptran,
-                                const int *action, const unsigned long long *nkey, const int *nlayer,
-                                unsigned long long *ckey, int *flag) {
+__global__ void win_move_kernel(int64_t np, AssocParams p, const WinProb *prob, const int *pprob, const int *pnode,
+                                const int *pslot, const double *ptran, const int *action, const unsigned long long *nkey,
+                                const int *nlayer, unsigned long long *ckey, int *flag) {
   const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= np) return;
-  const int v = pnode[j], a = action[v], s = pslot[j];
+  const int v = pnode[j], a = action[v], s = pslot[j], w = prob[pprob[j]].w;
   const bool mv = (a == 2 && s < w) || (a == 1 && s == w - 1);
   flag[j] = mv ? 1 : 0;
   if (!mv) return;
@@ -1507,25 +1643,25 @@ __global__ void win_move_kernel(int64_t np, int w, AssocParams p, const int *pno
   }
   ckey[j] = L == 0 ? ((k & ~63ull) | ((unsigned long long)oct << 3) | 7ull) : ((k & ~7ull) | (unsigned long long)oct);
 }
-__global__ void win_gather_u64_kernel(const unsigned long long *src, const int *idx, int m, unsigned long long *dst) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < m) dst[i] = src[idx[i]];
-}
 __global__ void win_restamp_kernel(const int *order, int m, unsigned long long op, unsigned long long *pstamp) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < m) pstamp[order[i]] = (op << 32) | (unsigned long long)i;
 }
 
-// to_margi (:778-816) on every node that is not split
-__global__ void win_margi_node_kernel(int nn, int N, int mg, int w, const double *poses, const int *nsplit,
-                                      const int *npush, double *nfix, double *sig_o, double *sig_t) {
+// to_margi (:778-816) on every node that is not split, in a problem this call marginalises (mg > 0); poses: the
+// problems' pose rows or null
+__global__ void win_margi_node_kernel(int nn, int N, const WinProb *prob, const int *nprob, const double *poses,
+                                      const int *nsplit, const int *npush, double *nfix, double *sig_o, double *sig_t) {
   const int v = blockIdx.x * blockDim.x + threadIdx.x;
   if (v >= nn || nsplit[v]) return;
+  const WinProb pr = prob[nprob[v]];
+  const int mg = pr.mg, w = pr.w;
+  if (mg == 0) return;
   double *so = sig_o + (size_t)v * N * 10, *stt = sig_t + (size_t)v * N * 10;
   if (poses)
     for (int i = 0; i < w; i++) {                                      // sig_tran[i].transform(sig_orig[i], x_poses[i])
       double r[9], t[3];
-      load_pose(poses + 12 * i, r, t);
+      load_pose(poses + 12 * ((size_t)pr.pose_base + i), r, t);
       const WC c = world_cluster(so + i * 10, r, t);
       double *d = stt + i * 10;
       d[0] = c.p00; d[1] = c.p01; d[2] = c.p02; d[3] = c.p11; d[4] = c.p12; d[5] = c.p22;
@@ -1542,15 +1678,17 @@ __global__ void win_margi_node_kernel(int nn, int N, int mg, int w, const double
     for (int q = 0; q < 10; q++) { so[i * 10 + q] = 0.0; stt[i * 10 + q] = 0.0; }
 }
 // ... and on their points: re-transform (plvec_trans), drop the retired slots, shift the rest
-__global__ void win_margi_point_kernel(int64_t np, int mg, int w, const double *poses, const int *nsplit, const int *pnode,
-                                       int *pslot, const float *pxyz, double *ptran, int *keep) {
+__global__ void win_margi_point_kernel(int64_t np, const WinProb *prob, const int *pprob, const double *poses,
+                                       const int *nsplit, const int *pnode, int *pslot, const float *pxyz, double *ptran,
+                                       int *keep) {
   const int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= np) return;
-  const int s = pslot[j];
-  if (nsplit[pnode[j]] || s >= w) { keep[j] = 1; return; }
+  const WinProb pr = prob[pprob[j]];
+  const int s = pslot[j], mg = pr.mg;
+  if (mg == 0 || nsplit[pnode[j]] || s >= pr.w) { keep[j] = 1; return; }
   if (poses) {
     double r[9], t[3];
-    load_pose(poses + 12 * s, r, t);
+    load_pose(poses + 12 * ((size_t)pr.pose_base + s), r, t);
     const double b[3] = {(double)pxyz[3 * j], (double)pxyz[3 * j + 1], (double)pxyz[3 * j + 2]};
 #pragma unroll
     for (int a = 0; a < 3; a++) ptran[3 * j + a] = r[a * 3] * b[0] + r[a * 3 + 1] * b[1] + r[a * 3 + 2] * b[2] + t[a];
@@ -1559,131 +1697,196 @@ __global__ void win_margi_point_kernel(int64_t np, int mg, int w, const double *
   if (s >= mg) pslot[j] = s - mg;
 }
 __global__ void win_compact_kernel(const int *sel, int m, const float *xyz, const double *tran, const int *slot,
-                                   const int *node, const unsigned long long *stamp, float *xyz2, double *tran2,
-                                   int *slot2, int *node2, unsigned long long *stamp2) {
+                                   const int *prb, const int *node, const unsigned long long *stamp, float *xyz2,
+                                   double *tran2, int *slot2, int *prb2, int *node2, unsigned long long *stamp2) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= m) return;
   const int j = sel[i];
 #pragma unroll
   for (int a = 0; a < 3; a++) { xyz2[3 * i + a] = xyz[3 * j + a]; tran2[3 * i + a] = tran[3 * j + a]; }
-  slot2[i] = slot[j]; node2[i] = node[j]; stamp2[i] = stamp[j];
+  slot2[i] = slot[j]; prb2[i] = prb[j]; node2[i] = node[j]; stamp2[i] = stamp[j];
 }
 
-// tras_opt (:908-929) + push_voxel (:30-51)
-__global__ void win_push_flag_kernel(int nn, int N, int w, int min_ps, const int *nsplit, const int *npush,
-                                     const double *sig_o, int *flag) {
+// tras_opt (:908-929) + push_voxel (:30-51), in a problem this call pushes (w > 0)
+__global__ void win_push_flag_kernel(int nn, int N, int min_ps, const WinProb *prob, const int *nprob, const int *nsplit,
+                                     const int *npush, const double *sig_o, int *flag) {
   const int v = blockIdx.x * blockDim.x + threadIdx.x;
   if (v >= nn) return;
   flag[v] = 0;
-  if (nsplit[v] || npush[v] != 1) return;
+  const WinProb pr = prob[nprob[v]];
+  if (pr.w == 0 || nsplit[v] || npush[v] != 1) return;
   double pts = 0;
-  for (int i = 0; i < w; i++) pts += sig_o[((size_t)v * N + i) * 10 + 9];
+  for (int i = 0; i < pr.w; i++) pts += sig_o[((size_t)v * N + i) * 10 + 9];
   if ((int)pts < min_ps) return;
   int k = 0;
-  for (int i = 0; i < N; i++) k += sig_o[((size_t)v * N + i) * 10 + 9] != 0.0 ? 1 : 0;
+  for (int i = 0; i < pr.n_slots; i++) k += sig_o[((size_t)v * N + i) * 10 + 9] != 0.0 ? 1 : 0;
   flag[v] = k >= 2 ? 1 : 0;
 }
-__global__ void win_obs_count_kernel(const int *ids, int M, int N, const double *sig_o, int *cnt) {
+__global__ void win_obs_count_kernel(const int *ids, int M, int N, const WinProb *prob, const int *nprob,
+                                     const double *sig_o, int *cnt) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= M) return;
+  const int v = ids[i], ns = prob[nprob[v]].n_slots;
   int k = 0;
-  for (int s = 0; s < N; s++) k += sig_o[((size_t)ids[i] * N + s) * 10 + 9] != 0.0 ? 1 : 0;
+  for (int s = 0; s < ns; s++) k += sig_o[((size_t)v * N + s) * 10 + 9] != 0.0 ? 1 : 0;
   cnt[i] = k;
 }
-__global__ void win_emit_kernel(const int *ids, const int *ostart, int M, int64_t K, int N, const double *sig_o,
-                                const double *nfix, const unsigned long long *nkey, const int *nlayer, long long *row_ptr,
-                                int *pose_idx, double *obs10, double *fix10, double *coe, unsigned long long *key_out,
-                                int *layer_out) {
+// per problem p: its first pushed voxel vptr[p] (vptr[B] = M) and first observation optr[p] (optr[B] = K)
+__global__ void win_push_ptr_kernel(const int *ids, int M, const int *nprob, const int *cnt, const int *ostart, int B,
+                                    long long *vptr, long long *optr) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p > B) return;
+  int lo = 0, hi = M;
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (nprob[ids[mid]] < p) lo = mid + 1; else hi = mid;
+  }
+  vptr[p] = lo;
+  optr[p] = lo < M ? (long long)ostart[lo] : (long long)ostart[M - 1] + cnt[M - 1];
+}
+__global__ void win_emit_kernel(const int *ids, const int *ostart, int M, int64_t K, int N, const WinProb *prob,
+                                const int *nprob, const double *sig_o, const double *nfix, const unsigned long long *nkey,
+                                const int *nlayer, WindowEmit out) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i == 0) row_ptr[M] = K;
+  if (i == 0) out.row_ptr[M] = K;
   if (i >= M) return;
-  const int v = ids[i];
+  const int v = ids[i], ns = prob[nprob[v]].n_slots;
   long long o = ostart[i];
-  row_ptr[i] = o;
+  out.row_ptr[i] = o;
   double pts = 0;
-  for (int s = 0; s < N; s++) {
+  for (int s = 0; s < ns; s++) {
     const double *c = sig_o + ((size_t)v * N + s) * 10;
     if (c[9] == 0.0) continue;
-    for (int q = 0; q < 10; q++) obs10[o * 10 + q] = c[q];
-    pose_idx[o] = s;
+    for (int q = 0; q < 10; q++) out.obs[o * 10 + q] = c[q];
+    out.pose_idx[o] = s;
     pts += c[9];
     o++;
   }
-  for (int q = 0; q < 10; q++) fix10[(size_t)i * 10 + q] = nfix[(size_t)v * 10 + q];
-  coe[i] = pts;                                                        // coe = sum of N (:42-44)
-  key_out[i] = nkey[v];
-  layer_out[i] = nlayer[v];
+  for (int q = 0; q < 10; q++) out.fix[(size_t)i * 10 + q] = nfix[(size_t)v * 10 + q];
+  out.coe[i] = pts;                                                    // coe = sum of N (:42-44)
+  out.key[i] = nkey[v];
+  out.layer[i] = nlayer[v];
 }
 }  // namespace
 
 void window_free(WindowState *w) { delete w; }
+const std::vector<int> &window_slots(const WindowState *w) { return w->n_slots; }
+const balm_assoc_opts &window_opts(const WindowState *w) { return w->opts; }
 
-int window_reset_build(balm_ctx *c, WindowState **ws, double voxel_size, int layer_limit, int min_ps, const double *eig3) {
-  if (layer_limit < 0 || layer_limit > 2) { balm_set_error("balm_window_reset: layer_limit must be in 0..2"); return BALM_ERR_INVALID; }
+int window_reset_build(WindowState **ws, const char *who, int B, const int *n_slots, const balm_assoc_opts &o, bool batch) {
+  if (o.layer_limit < 0 || o.layer_limit > 2) { balm_set_error(std::string(who) + ": layer_limit must be in 0..2"); return BALM_ERR_INVALID; }
   WindowState *w = new WindowState();
-  w->P = AssocParams{voxel_size, layer_limit, min_ps, {eig3[0], eig3[1], eig3[2]}};
-  w->N = c->N;
+  w->P = AssocParams{o.voxel_size, o.layer_limit, o.min_ps, {o.eigen_value_array[0], o.eigen_value_array[1], o.eigen_value_array[2]}};
+  w->opts = o;
+  w->batch = batch;
+  w->B = B;
+  w->n_slots.assign(n_slots, n_slots + B);
+  w->hprob.resize(B);
+  int base = 0;
+  for (int p = 0; p < B; p++) {
+    w->hprob[p] = WinProb{n_slots[p], base, 0, 0};
+    base += n_slots[p];
+    w->N = std::max(w->N, n_slots[p]);
+  }
+  cudaError_t e = cudaMalloc((void **)&w->prob, sizeof(WinProb) * B);
+  for (WinLookup &l : w->look)
+    if (e == cudaSuccess && (e = cudaMalloc((void **)&l.off, sizeof(int) * (B + 1))) == cudaSuccess)
+      e = cudaMemset(l.off, 0, sizeof(int) * (B + 1));
+  if (e != cudaSuccess) {
+    delete w;
+    CUDA_TRY(e);
+  }
   delete *ws;
   *ws = w;
   return BALM_OK;
 }
 
-int window_cut_build(balm_ctx *c, WindowState &w, int64_t n, const float *xyz_h, const double *pose12_h, int slot) {
+int window_cut_build(cudaStream_t st, WindowState &w, const char *who, const int32_t *scan_of, const int *slot,
+                     int n_scans, const int64_t *scan_ptr, const float *xyz_h, const double *poses12_h,
+                     long long *launches) {
+  // entries: the problems that take a non-empty scan, in problem order; their items are that scan's points in order
+  std::vector<long long> item_ptr(1, 0), src_base;
+  std::vector<int4> ent;
+  for (int p = 0; p < w.B; p++) {
+    const int s = scan_of[p];
+    if (s < 0 || scan_ptr[s + 1] == scan_ptr[s]) continue;
+    ent.push_back(make_int4(p, w.hprob[p].pose_base + slot[p], slot[p], 0));
+    src_base.push_back(scan_ptr[s]);
+    item_ptr.push_back(item_ptr.back() + (scan_ptr[s + 1] - scan_ptr[s]));
+  }
+  const int64_t n = item_ptr.back();
   if (n == 0) return BALM_OK;
-  if (n < 0 || w.np + n >= (1ll << 31)) { balm_set_error("balm_window_cut: bad point count (the window holds < 2^31 points)"); return BALM_ERR_INVALID; }
-  cudaStream_t st = c->stream;
+  if (w.np + n >= (1ll << 31)) {
+    balm_set_error(std::string(who) + ": 2^31 or more points in the window");
+    return w.batch ? BALM_ERR_UNSUPPORTED : BALM_ERR_INVALID;
+  }
+  const int E = (int)ent.size(), m = (int)n, P = w.hprob.back().pose_base + w.hprob.back().n_slots;
+  const int64_t n_points = scan_ptr[n_scans];
   ScratchPool pool;
   CubTmp tmp{pool};
-  const int m = (int)n;
   float *xyz = nullptr;
-  double *pose = nullptr, *tran = nullptr;
+  double *poses = nullptr, *tran = nullptr;
   unsigned long long *rkey = nullptr;
-  int *bad = nullptr, *order = nullptr;
-  TRY(pool.get(&xyz, 3 * (size_t)m)); TRY(pool.get(&pose, 12)); TRY(pool.get(&tran, 3 * (size_t)m));
-  TRY(pool.get(&rkey, m)); TRY(pool.get(&bad, 1)); TRY(pool.get(&order, m));
-  CUDA_TRY(cudaMemcpyAsync(xyz, xyz_h, sizeof(float) * 3 * m, cudaMemcpyHostToDevice, st));
-  CUDA_TRY(cudaMemcpyAsync(pose, pose12_h, sizeof(double) * 12, cudaMemcpyHostToDevice, st));
-  CUDA_TRY(cudaMemsetAsync(bad, 0, sizeof(int), st));
+  long long *d_iptr = nullptr, *d_sbase = nullptr;
+  int4 *d_ent = nullptr;
+  int *bad = nullptr, *order = nullptr, *src = nullptr, *row = nullptr, *iprob = nullptr;
+  TRY(pool.get(&xyz, 3 * (size_t)n_points)); TRY(pool.get(&poses, 12 * (size_t)P)); TRY(pool.get(&tran, 3 * (size_t)m));
+  TRY(pool.get(&rkey, m)); TRY(pool.get(&bad, w.B)); TRY(pool.get(&order, m)); TRY(pool.get(&src, m));
+  TRY(pool.get(&row, m)); TRY(pool.get(&iprob, m)); TRY(pool.get(&d_iptr, E + 1)); TRY(pool.get(&d_sbase, E));
+  TRY(pool.get(&d_ent, E));
+  CUDA_TRY(cudaMemcpyAsync(xyz, xyz_h, sizeof(float) * 3 * n_points, cudaMemcpyHostToDevice, st));
+  CUDA_TRY(cudaMemcpyAsync(poses, poses12_h, sizeof(double) * 12 * P, cudaMemcpyHostToDevice, st));
+  CUDA_TRY(cudaMemcpyAsync(d_iptr, item_ptr.data(), sizeof(long long) * (E + 1), cudaMemcpyHostToDevice, st));
+  CUDA_TRY(cudaMemcpyAsync(d_sbase, src_base.data(), sizeof(long long) * E, cudaMemcpyHostToDevice, st));
+  CUDA_TRY(cudaMemcpyAsync(d_ent, ent.data(), sizeof(int4) * E, cudaMemcpyHostToDevice, st));
+  CUDA_TRY(cudaMemsetAsync(bad, 0, sizeof(int) * w.B, st));
   const unsigned g = (unsigned)((m + 255) / 256);
-  win_cut_kernel<<<g, 256, 0, st>>>(xyz, pose, m, w.P, tran, rkey, bad);
-  int h_bad = 0;
-  CUDA_TRY(cudaMemcpyAsync(&h_bad, bad, sizeof(int), cudaMemcpyDeviceToHost, st));
+  expand_rows_kernel<<<E, 256, 0, st>>>(d_iptr, d_sbase, src, row);
+  win_cut_kernel<<<g, 256, 0, st>>>(xyz, src, row, d_ent, poses, m, w.P, tran, rkey, iprob, bad);
+  std::vector<int> h_bad(w.B);
+  CUDA_TRY(cudaMemcpyAsync(h_bad.data(), bad, sizeof(int) * w.B, cudaMemcpyDeviceToHost, st));
   CUDA_TRY(cudaStreamSynchronize(st));
-  if (h_bad) { balm_set_error("balm_window_cut: a point lies outside the +-2^18 root-voxel range"); return BALM_ERR_INVALID; }
-  // nothing was changed so far; from here on the scan is committed
-  TRY(win_add_nodes(w, pool, tmp, st, rkey, m, 0));
+  for (int p = 0; p < w.B; p++)
+    if (h_bad[p]) {
+      balm_set_error(std::string(who) + (w.batch ? ": problem " + std::to_string(p) : std::string()) +
+                     ": a point lies outside the +-2^18 root-voxel range");
+      return BALM_ERR_INVALID;
+    }
+  // nothing was changed so far; from here on the scans are committed
+  TRY(win_add_nodes(w, pool, tmp, st, rkey, iprob, m, 0));
   TRY(win_reserve_points(w, w.np + m));
   const int64_t b = w.np;
-  CUDA_TRY(cudaMemcpyAsync(w.pxyz + 3 * b, xyz, sizeof(float) * 3 * m, cudaMemcpyDeviceToDevice, st));
   CUDA_TRY(cudaMemcpyAsync(w.ptran + 3 * b, tran, sizeof(double) * 3 * m, cudaMemcpyDeviceToDevice, st));
-  win_stamp_kernel<<<g, 256, 0, st>>>(w.pslot + b, w.pstamp + b, m, slot, w.op++);
-  win_find_kernel<<<g, 256, 0, st>>>(rkey, nullptr, m, w.look[0].key, w.look[0].id, w.look[0].n, w.pnode + b);
+  win_store_kernel<<<g, 256, 0, st>>>(xyz, src, row, d_ent, m, w.op++, w.pxyz + 3 * b, w.pslot + b, w.pprob + b,
+                                      w.pstamp + b);
+  win_find_kernel<<<g, 256, 0, st>>>(rkey, iprob, nullptr, m, w.look[0].key, w.look[0].id, w.look[0].off, w.pnode + b);
   win_iota_kernel<<<g, 256, 0, st>>>(order, m, (int)b);
   w.np += m;
   TRY(win_push_points(w, pool, tmp, st, order, m));
   CUDA_TRY(cudaStreamSynchronize(st));
-  c->launches += 10;
+  *launches += 12;
   return BALM_OK;
 }
 
-int window_recut_build(balm_ctx *c, WindowState &w, int win_count) {
-  cudaStream_t st = c->stream;
+int window_recut_build(cudaStream_t st, WindowState &w, const int *win_count, long long *launches) {
+  TRY(win_upload(w, st, win_count, nullptr));
   for (int L = 0; L <= w.P.layer_limit; L++) {
     ScratchPool pool;
     CubTmp tmp{pool};
     if (w.nn == 0) return BALM_OK;
     CUDA_TRY(cudaMemsetAsync(w.naction, 0, sizeof(int) * w.nn, st));
-    win_judge_kernel<<<(w.nn + 127) / 128, 128, 0, st>>>(w.nn, L, w.N, win_count, w.P, w.nlayer, w.nsplit, w.npush, w.nfix,
-                                                         w.sig_o, w.sig_t, w.naction);
-    c->launches += 1;
+    win_judge_kernel<<<(w.nn + 127) / 128, 128, 0, st>>>(w.nn, L, w.N, w.P, w.prob, w.nprob, w.nlayer, w.nsplit, w.npush,
+                                                         w.nfix, w.sig_o, w.sig_t, w.naction);
+    *launches += 1;
     if (L == w.P.layer_limit || w.np == 0) break;
     const int np = (int)w.np;
     unsigned long long *ckey = nullptr, *mkey = nullptr, *stamp = nullptr, *stamp2 = nullptr;
-    int *flag = nullptr, *iota = nullptr, *mv = nullptr, *mv2 = nullptr, *nsel = nullptr;
+    int *flag = nullptr, *iota = nullptr, *mv = nullptr, *mv2 = nullptr, *mprob = nullptr, *nsel = nullptr;
     TRY(pool.get(&ckey, np)); TRY(pool.get(&flag, np)); TRY(pool.get(&iota, np)); TRY(pool.get(&mv, np));
     TRY(pool.get(&nsel, 1));
     const unsigned g = (unsigned)((np + 255) / 256);
-    win_move_kernel<<<g, 256, 0, st>>>(w.np, win_count, w.P, w.pnode, w.pslot, w.ptran, w.naction, w.nkey, w.nlayer, ckey, flag);
+    win_move_kernel<<<g, 256, 0, st>>>(w.np, w.P, w.prob, w.pprob, w.pnode, w.pslot, w.ptran, w.naction, w.nkey, w.nlayer,
+                                       ckey, flag);
     win_iota_kernel<<<g, 256, 0, st>>>(iota, np, 0);
     size_t b1 = 0;
     cub::DeviceSelect::Flagged(nullptr, b1, iota, flag, mv, nsel, np, st);
@@ -1692,13 +1895,16 @@ int window_recut_build(balm_ctx *c, WindowState &w, int win_count) {
     int m = 0;
     CUDA_TRY(cudaMemcpyAsync(&m, nsel, sizeof(int), cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
-    c->launches += 3;
+    *launches += 3;
     if (m == 0) continue;
     TRY(pool.get(&mkey, m)); TRY(pool.get(&stamp, m)); TRY(pool.get(&stamp2, m)); TRY(pool.get(&mv2, m));
+    TRY(pool.get(&mprob, m));
     const unsigned gm = (unsigned)((m + 255) / 256);
     win_gather_u64_kernel<<<gm, 256, 0, st>>>(ckey, mv, m, mkey);
-    TRY(win_add_nodes(w, pool, tmp, st, mkey, m, L + 1));              // children created on first use (:714-720)
-    win_find_kernel<<<gm, 256, 0, st>>>(mkey, mv, m, w.look[L + 1].key, w.look[L + 1].id, w.look[L + 1].n, w.pnode);
+    win_gather_i32_kernel<<<gm, 256, 0, st>>>(w.pprob, mv, m, mprob);
+    TRY(win_add_nodes(w, pool, tmp, st, mkey, mprob, m, L + 1));       // children created on first use (:714-720)
+    const WinLookup &lk = w.look[L + 1];
+    win_find_kernel<<<gm, 256, 0, st>>>(mkey, mprob, mv, m, lk.key, lk.id, lk.off, w.pnode);
     // the moved points in the order the parents' lists hold them, appended after the children's earlier points
     win_gather_u64_kernel<<<gm, 256, 0, st>>>(w.pstamp, mv, m, stamp);
     size_t b2 = 0;
@@ -1708,21 +1914,23 @@ int window_recut_build(balm_ctx *c, WindowState &w, int win_count) {
     win_restamp_kernel<<<gm, 256, 0, st>>>(mv2, m, w.op++, w.pstamp);
     TRY(win_push_points(w, pool, tmp, st, mv2, m));
     CUDA_TRY(cudaStreamSynchronize(st));
-    c->launches += 9;
+    *launches += 10;
   }
   CUDA_TRY(cudaStreamSynchronize(st));
   CUDA_TRY(cudaGetLastError());
   return BALM_OK;
 }
 
-int window_marginalize_build(balm_ctx *c, WindowState &w, int mg, const double *poses_h, int win_count) {
-  cudaStream_t st = c->stream;
+int window_marginalize_build(cudaStream_t st, WindowState &w, const int *mg, const double *poses_h, const int *win_count,
+                             long long *launches) {
   ScratchPool pool;
   CubTmp tmp{pool};
+  TRY(win_upload(w, st, win_count, mg));
   double *poses = nullptr;
   if (poses_h) {
-    TRY(pool.get(&poses, 12 * (size_t)w.N));
-    CUDA_TRY(cudaMemcpyAsync(poses, poses_h, sizeof(double) * 12 * w.N, cudaMemcpyHostToDevice, st));
+    const size_t P = (size_t)w.hprob.back().pose_base + w.hprob.back().n_slots;
+    TRY(pool.get(&poses, 12 * P));
+    CUDA_TRY(cudaMemcpyAsync(poses, poses_h, sizeof(double) * 12 * P, cudaMemcpyHostToDevice, st));
   }
   if (w.nn == 0) return BALM_OK;
   // the points first: they read the node's split flag only, and the slot before the shift
@@ -1731,7 +1939,8 @@ int window_marginalize_build(balm_ctx *c, WindowState &w, int mg, const double *
     int *keep = nullptr, *iota = nullptr, *sel = nullptr, *nsel = nullptr;
     TRY(pool.get(&keep, np)); TRY(pool.get(&iota, np)); TRY(pool.get(&sel, np)); TRY(pool.get(&nsel, 1));
     const unsigned g = (unsigned)((np + 255) / 256);
-    win_margi_point_kernel<<<g, 256, 0, st>>>(w.np, mg, win_count, poses, w.nsplit, w.pnode, w.pslot, w.pxyz, w.ptran, keep);
+    win_margi_point_kernel<<<g, 256, 0, st>>>(w.np, w.prob, w.pprob, poses, w.nsplit, w.pnode, w.pslot, w.pxyz, w.ptran,
+                                              keep);
     win_iota_kernel<<<g, 256, 0, st>>>(iota, np, 0);
     size_t b1 = 0;
     cub::DeviceSelect::Flagged(nullptr, b1, iota, keep, sel, nsel, np, st);
@@ -1743,88 +1952,113 @@ int window_marginalize_build(balm_ctx *c, WindowState &w, int mg, const double *
     if (m < np) {  // compact the point store (same capacity, order kept)
       float *xyz2 = nullptr;
       double *tran2 = nullptr;
-      int *slot2 = nullptr, *node2 = nullptr;
+      int *slot2 = nullptr, *prob2 = nullptr, *node2 = nullptr;
       unsigned long long *stamp2 = nullptr;
       const size_t cap = (size_t)w.pcap;
-      CUDA_TRY(cudaMalloc((void **)&xyz2, sizeof(float) * 3 * cap));
-      CUDA_TRY(cudaMalloc((void **)&tran2, sizeof(double) * 3 * cap));
-      CUDA_TRY(cudaMalloc((void **)&slot2, sizeof(int) * cap));
-      CUDA_TRY(cudaMalloc((void **)&node2, sizeof(int) * cap));
-      CUDA_TRY(cudaMalloc((void **)&stamp2, sizeof(unsigned long long) * cap));
+      if (cudaMalloc((void **)&xyz2, sizeof(float) * 3 * cap) != cudaSuccess ||
+          cudaMalloc((void **)&tran2, sizeof(double) * 3 * cap) != cudaSuccess ||
+          cudaMalloc((void **)&slot2, sizeof(int) * cap) != cudaSuccess ||
+          cudaMalloc((void **)&prob2, sizeof(int) * cap) != cudaSuccess ||
+          cudaMalloc((void **)&node2, sizeof(int) * cap) != cudaSuccess ||
+          cudaMalloc((void **)&stamp2, sizeof(unsigned long long) * cap) != cudaSuccess) {
+        cudaFree(xyz2); cudaFree(tran2); cudaFree(slot2); cudaFree(prob2); cudaFree(node2); cudaFree(stamp2);
+        CUDA_TRY(cudaErrorMemoryAllocation);
+      }
       if (m > 0)
-        win_compact_kernel<<<(m + 255) / 256, 256, 0, st>>>(sel, m, w.pxyz, w.ptran, w.pslot, w.pnode, w.pstamp, xyz2, tran2,
-                                                            slot2, node2, stamp2);
+        win_compact_kernel<<<(m + 255) / 256, 256, 0, st>>>(sel, m, w.pxyz, w.ptran, w.pslot, w.pprob, w.pnode, w.pstamp,
+                                                            xyz2, tran2, slot2, prob2, node2, stamp2);
       CUDA_TRY(cudaStreamSynchronize(st));
-      cudaFree(w.pxyz); cudaFree(w.ptran); cudaFree(w.pslot); cudaFree(w.pnode); cudaFree(w.pstamp);
-      w.pxyz = xyz2; w.ptran = tran2; w.pslot = slot2; w.pnode = node2; w.pstamp = stamp2;
+      cudaFree(w.pxyz); cudaFree(w.ptran); cudaFree(w.pslot); cudaFree(w.pprob); cudaFree(w.pnode); cudaFree(w.pstamp);
+      w.pxyz = xyz2; w.ptran = tran2; w.pslot = slot2; w.pprob = prob2; w.pnode = node2; w.pstamp = stamp2;
       w.np = m;
     }
-    c->launches += 3;
+    *launches += 3;
   }
-  win_margi_node_kernel<<<(w.nn + 127) / 128, 128, 0, st>>>(w.nn, w.N, mg, win_count, poses, w.nsplit, w.npush, w.nfix,
+  win_margi_node_kernel<<<(w.nn + 127) / 128, 128, 0, st>>>(w.nn, w.N, w.prob, w.nprob, poses, w.nsplit, w.npush, w.nfix,
                                                             w.sig_o, w.sig_t);
   CUDA_TRY(cudaStreamSynchronize(st));
   CUDA_TRY(cudaGetLastError());
-  c->launches += 1;
+  *launches += 1;
   return BALM_OK;
 }
 
-int window_push_build(balm_ctx *c, WindowState &w, int win_count, int64_t *M_out, int64_t *K_out,
-                      int (*reg)(balm_ctx *, int64_t, const int64_t *, const int32_t *, const double *, const double *,
-                                 const double *, int64_t)) {
-  *M_out = 0;
-  *K_out = 0;
-  if (w.nn == 0) return BALM_OK;
-  cudaStream_t st = c->stream;
+int window_push_build(cudaStream_t st, WindowState &w, const int *win_count, const WindowRegister &reg,
+                      long long *launches) {
   ScratchPool pool;
   CubTmp tmp{pool};
-  const int nn = w.nn;
-  int *flag = nullptr, *iota = nullptr, *sel = nullptr, *nsel = nullptr;
-  TRY(pool.get(&flag, nn)); TRY(pool.get(&iota, nn)); TRY(pool.get(&sel, nn)); TRY(pool.get(&nsel, 1));
-  const unsigned g = (unsigned)((nn + 127) / 128);
-  win_push_flag_kernel<<<g, 128, 0, st>>>(nn, w.N, win_count, w.P.min_ps, w.nsplit, w.npush, w.sig_o, flag);
-  win_iota_kernel<<<g, 128, 0, st>>>(iota, nn, 0);
-  size_t b1 = 0;
-  cub::DeviceSelect::Flagged(nullptr, b1, iota, flag, sel, nsel, nn, st);
-  TRY(tmp.need(b1));
-  CUDA_TRY(cub::DeviceSelect::Flagged(tmp.p, tmp.bytes, iota, flag, sel, nsel, nn, st));
+  TRY(win_upload(w, st, win_count, nullptr));
+  const int nn = w.nn, B = w.B;
   int M = 0;
-  CUDA_TRY(cudaMemcpyAsync(&M, nsel, sizeof(int), cudaMemcpyDeviceToHost, st));
-  CUDA_TRY(cudaStreamSynchronize(st));
-  c->launches += 3;
-  if (M == 0) return BALM_OK;
-  // ascending node key (unique among pushed nodes: a pushed node is not split, so none of its ancestors is pushed)
+  int *flag = nullptr, *iota = nullptr, *sel = nullptr, *nsel = nullptr;
+  if (nn > 0) {
+    TRY(pool.get(&flag, nn)); TRY(pool.get(&iota, nn)); TRY(pool.get(&sel, nn)); TRY(pool.get(&nsel, 1));
+    const unsigned g = (unsigned)((nn + 127) / 128);
+    win_push_flag_kernel<<<g, 128, 0, st>>>(nn, w.N, w.P.min_ps, w.prob, w.nprob, w.nsplit, w.npush, w.sig_o, flag);
+    win_iota_kernel<<<g, 128, 0, st>>>(iota, nn, 0);
+    size_t b1 = 0;
+    cub::DeviceSelect::Flagged(nullptr, b1, iota, flag, sel, nsel, nn, st);
+    TRY(tmp.need(b1));
+    CUDA_TRY(cub::DeviceSelect::Flagged(tmp.p, tmp.bytes, iota, flag, sel, nsel, nn, st));
+    CUDA_TRY(cudaMemcpyAsync(&M, nsel, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    *launches += 3;
+  }
+  std::vector<int64_t> h((size_t)2 * (B + 1), 0);  // voxel_ptr | obs_ptr
+  WindowEmit out{};
+  if (M == 0) {
+    TRY(reg(h.data(), h.data() + B + 1, &out));
+    CUDA_TRY(cudaMemsetAsync(out.row_ptr, 0, sizeof(long long), st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    return BALM_OK;
+  }
+  // ascending (problem, key) (unique among one problem's pushed nodes: a pushed node is not split, so none of its
+  // ancestors is pushed)
   unsigned long long *k = nullptr, *k2 = nullptr;
-  int *ids = nullptr, *cnt = nullptr, *ostart = nullptr;
-  TRY(pool.get(&k, M)); TRY(pool.get(&k2, M)); TRY(pool.get(&ids, M)); TRY(pool.get(&cnt, M)); TRY(pool.get(&ostart, M));
+  int *ids = nullptr, *ids2 = nullptr, *cnt = nullptr, *ostart = nullptr;
+  long long *ptrs = nullptr;
+  TRY(pool.get(&k, M)); TRY(pool.get(&k2, M)); TRY(pool.get(&ids2, M)); TRY(pool.get(&cnt, M)); TRY(pool.get(&ostart, M));
+  TRY(pool.get(&ptrs, 2 * ((size_t)B + 1)));
   const unsigned gm = (unsigned)((M + 127) / 128);
-  win_gather_u64_kernel<<<gm, 128, 0, st>>>(w.nkey, sel, M, k);
-  size_t b2 = 0, b3 = 0;
-  cub::DeviceRadixSort::SortPairs(nullptr, b2, k, k2, sel, ids, M, 0, 64, st);
+  ids = sel;
+  win_gather_u64_kernel<<<gm, 128, 0, st>>>(w.nkey, ids, M, k);
+  TRY(win_sort_ids(w, pool, tmp, st, k, ids, k2, ids2, M));
+  win_obs_count_kernel<<<gm, 128, 0, st>>>(ids, M, w.N, w.prob, w.nprob, w.sig_o, cnt);
+  size_t b3 = 0;
   cub::DeviceScan::ExclusiveSum(nullptr, b3, cnt, ostart, M, st);
-  TRY(tmp.need(std::max(b2, b3)));
-  CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp.p, tmp.bytes, k, k2, sel, ids, M, 0, 64, st));
-  win_obs_count_kernel<<<gm, 128, 0, st>>>(ids, M, w.N, w.sig_o, cnt);
+  TRY(tmp.need(b3));
   CUDA_TRY(cub::DeviceScan::ExclusiveSum(tmp.p, tmp.bytes, cnt, ostart, M, st));
-  int last[2] = {0, 0};
-  CUDA_TRY(cudaMemcpyAsync(&last[0], cnt + M - 1, sizeof(int), cudaMemcpyDeviceToHost, st));
-  CUDA_TRY(cudaMemcpyAsync(&last[1], ostart + M - 1, sizeof(int), cudaMemcpyDeviceToHost, st));
+  win_push_ptr_kernel<<<(B + 128) / 128, 128, 0, st>>>(ids, M, w.nprob, cnt, ostart, B, ptrs, ptrs + B + 1);
+  CUDA_TRY(cudaMemcpyAsync(h.data(), ptrs, sizeof(long long) * 2 * (B + 1), cudaMemcpyDeviceToHost, st));
   CUDA_TRY(cudaStreamSynchronize(st));
-  const int64_t K = (int64_t)last[0] + last[1];
-  long long *rp = nullptr;
-  int *pi = nullptr, *lay = nullptr;
-  double *ob = nullptr, *fx = nullptr, *co = nullptr;
-  unsigned long long *keys_out = nullptr;
-  TRY(pool.get(&rp, (size_t)M + 1)); TRY(pool.get(&pi, (size_t)K)); TRY(pool.get(&ob, (size_t)K * 10));
-  TRY(pool.get(&fx, (size_t)M * 10)); TRY(pool.get(&co, (size_t)M)); TRY(pool.get(&keys_out, (size_t)M));
-  TRY(pool.get(&lay, (size_t)M));
-  win_emit_kernel<<<gm, 128, 0, st>>>(ids, ostart, M, K, w.N, w.sig_o, w.nfix, w.nkey, w.nlayer, rp, pi, ob, fx, co, keys_out,
-                                      lay);
+  const int64_t K = h[2 * (size_t)B + 1];
+  TRY(reg(h.data(), h.data() + B + 1, &out));
+  win_emit_kernel<<<gm, 128, 0, st>>>(ids, ostart, M, K, w.N, w.prob, w.nprob, w.sig_o, w.nfix, w.nkey, w.nlayer, out);
   CUDA_TRY(cudaStreamSynchronize(st));
   CUDA_TRY(cudaGetLastError());
-  c->launches += 6;
+  *launches += 8;
+  return BALM_OK;
+}
+
+// balm_window_push: the one-problem push into pool buffers, then registered as the context's voxel set with its keys
+int window_push_ctx(balm_ctx *c, WindowState &w, int win_count, int64_t *M_out, int64_t *K_out,
+                    int (*reg)(balm_ctx *, int64_t, const int64_t *, const int32_t *, const double *, const double *,
+                               const double *, int64_t)) {
+  ScratchPool pool;
+  int64_t M = 0, K = 0;
+  WindowEmit dst{};
+  const WindowRegister to_pool = [&](const int64_t *vp, const int64_t *op, WindowEmit *out) {
+    M = vp[1];
+    K = op[1];
+    TRY(pool.get(&dst.row_ptr, (size_t)M + 1)); TRY(pool.get(&dst.pose_idx, (size_t)K));
+    TRY(pool.get(&dst.obs, (size_t)K * 10)); TRY(pool.get(&dst.fix, (size_t)M * 10)); TRY(pool.get(&dst.coe, (size_t)M));
+    TRY(pool.get(&dst.key, (size_t)M)); TRY(pool.get(&dst.layer, (size_t)M));
+    *out = dst;
+    return (int)BALM_OK;
+  };
+  TRY(window_push_build(c->stream, w, &win_count, to_pool, &c->launches));
   *M_out = M;
   *K_out = K;
-  TRY(reg(c, M, (const int64_t *)rp, pi, ob, fx, co, K));
-  return install_keys(c, keys_out, lay, M, true);
+  if (M == 0) return BALM_OK;
+  TRY(reg(c, M, (const int64_t *)dst.row_ptr, dst.pose_idx, dst.obs, dst.fix, dst.coe, K));
+  return install_keys(c, dst.key, dst.layer, M, true);
 }

@@ -884,13 +884,10 @@ extern "C" int balm_download_fix(balm_ctx *c, double *fix10) {
 }
 
 // ---------------- persistent sliding-window octree (assoc.cu) ----------------
-int window_reset_build(balm_ctx *c, WindowState **ws, double voxel_size, int layer_limit, int min_ps, const double *eig3);
-int window_cut_build(balm_ctx *c, WindowState &w, int64_t n, const float *xyz_h, const double *pose12_h, int slot);
-int window_recut_build(balm_ctx *c, WindowState &w, int win_count);
-int window_marginalize_build(balm_ctx *c, WindowState &w, int mg, const double *poses_h, int win_count);
-int window_push_build(balm_ctx *c, WindowState &w, int win_count, int64_t *M_out, int64_t *K_out,
-                      int (*reg)(balm_ctx *, int64_t, const int64_t *, const int32_t *, const double *, const double *,
-                                 const double *, int64_t));
+// the one-problem case of the batch's window (window_*_build, internal.cuh)
+int window_push_ctx(balm_ctx *c, WindowState &w, int win_count, int64_t *M_out, int64_t *K_out,
+                    int (*reg)(balm_ctx *, int64_t, const int64_t *, const int32_t *, const double *, const double *,
+                               const double *, int64_t));
 static int window_check(balm_ctx *c, const char *fn, int win_count) {
   if (!c) { balm_set_error(std::string(fn) + ": bad arguments"); return BALM_ERR_INVALID; }
   if (!c->win) { balm_set_error(std::string(fn) + ": call balm_window_reset first"); return BALM_ERR_INVALID; }
@@ -901,7 +898,7 @@ extern "C" int balm_window_reset(balm_ctx *c, const balm_assoc_opts *opts) {
   if (!c) { balm_set_error("balm_window_reset: bad arguments"); return BALM_ERR_INVALID; }
   CUDA_TRY(cudaSetDevice(c->device));
   const balm_assoc_opts o = resolve_assoc_opts(opts);
-  return window_reset_build(c, &c->win, o.voxel_size, o.layer_limit, o.min_ps, o.eigen_value_array);
+  return window_reset_build(&c->win, "balm_window_reset", 1, &c->N, o, false);
 }
 extern "C" int balm_window_cut(balm_ctx *c, int64_t n_points, const float *xyz, const double *pose12, int slot) {
   TRY(window_check(c, "balm_window_cut", 1));
@@ -909,13 +906,22 @@ extern "C" int balm_window_cut(balm_ctx *c, int64_t n_points, const float *xyz, 
     balm_set_error("balm_window_cut: bad arguments (slot must be in [0, N))");
     return BALM_ERR_INVALID;
   }
+  if (n_points >= (1ll << 31)) {
+    balm_set_error("balm_window_cut: bad point count (the window holds < 2^31 points)");
+    return BALM_ERR_INVALID;
+  }
   CUDA_TRY(cudaSetDevice(c->device));
-  return window_cut_build(c, *c->win, n_points, xyz, pose12, slot);
+  std::vector<double> poses((size_t)12 * c->N, 0.0);  // the scan's pose in row `slot`
+  std::copy(pose12, pose12 + 12, poses.begin() + 12 * (size_t)slot);
+  const int32_t scan = 0;
+  const int64_t scan_ptr[2] = {0, n_points};
+  return window_cut_build(c->stream, *c->win, "balm_window_cut", &scan, &slot, 1, scan_ptr, xyz, poses.data(),
+                          &c->launches);
 }
 extern "C" int balm_window_recut(balm_ctx *c, int win_count) {
   TRY(window_check(c, "balm_window_recut", win_count));
   CUDA_TRY(cudaSetDevice(c->device));
-  return window_recut_build(c, *c->win, win_count);
+  return window_recut_build(c->stream, *c->win, &win_count, &c->launches);
 }
 extern "C" int balm_window_marginalize(balm_ctx *c, int mg_size, const double *poses12, int win_count) {
   TRY(window_check(c, "balm_window_marginalize", win_count));
@@ -924,13 +930,13 @@ extern "C" int balm_window_marginalize(balm_ctx *c, int mg_size, const double *p
     return BALM_ERR_INVALID;
   }
   CUDA_TRY(cudaSetDevice(c->device));
-  return window_marginalize_build(c, *c->win, mg_size, poses12, win_count);
+  return window_marginalize_build(c->stream, *c->win, &mg_size, poses12, &win_count, &c->launches);
 }
 extern "C" int balm_window_push(balm_ctx *c, int win_count, int64_t *n_voxels_out, int64_t *n_obs_out) {
   TRY(window_check(c, "balm_window_push", win_count));
   CUDA_TRY(cudaSetDevice(c->device));
   int64_t M = 0, K = 0;
-  TRY(window_push_build(c, *c->win, win_count, &M, &K, balm_set_voxels_dev));
+  TRY(window_push_ctx(c, *c->win, win_count, &M, &K, balm_set_voxels_dev));
   if (M == 0) {  // nothing pushed: an empty voxel set
     drop_keys(c);
     TRY(register_empty(c));

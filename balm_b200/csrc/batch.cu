@@ -23,6 +23,9 @@
 //   batch_syrk_kernel<8, 4>     per (problem, tile, 768-row chunk): partial of Q V^T + V Q^T (A = partner row ^ 4)
 //   batch_assemble_kernel<21, 0, false, false>  per (problem, 64-column block): Rcov_raw = + sum of partials + blockdiag
 //   batch_cov_solve_kernel      per problem, one CTA: LDL^T of H, singularity test, H^-1 Rcov_raw H^-1, symmetrised
+//
+// The batch's persistent window maps (balm_batch_window_*) live in assoc.cu's WindowState, one state for every problem;
+// balm_batch_window_push emits the pushed nodes straight into a new registration (reg_layout / reg_finish / install).
 #include <math.h>
 #include <string.h>
 #include <algorithm>
@@ -719,6 +722,7 @@ struct balm_batch {
   int device = 0, sm_count = 132;
   cudaStream_t stream = nullptr;
   BatchReg *reg = nullptr;
+  WindowState *win = nullptr;  // balm_batch_window_* maps (independent of the registration)
   int *h_count = nullptr;  // pinned: problems still active after an iteration
 };
 
@@ -829,6 +833,7 @@ extern "C" int balm_batch_destroy(balm_batch *b) {
   cudaSetDevice(b->device);
   cudaStreamSynchronize(b->stream);
   delete b->reg;
+  window_free(b->win);
   cudaFreeHost(b->h_count);
   cudaStreamDestroy(b->stream);
   delete b;
@@ -1128,6 +1133,122 @@ extern "C" int balm_batch_append_scan(balm_batch *bt, const int32_t *scan_of, co
       if (n_voxels_out) n_voxels_out[b] = r->hprob[b].nvox;
       if (n_obs_out) n_obs_out[b] = obs_ptr[b + 1] - obs_ptr[b];
       if (n_matched_out) n_matched_out[b] = matched[b];
+    }
+  return install(bt, r, rc);
+}
+
+// ---- persistent sliding-window octree (assoc.cu: window_*_build, the maps of every problem in one state) ----
+// The window's problems and per-problem counts (win_count / mg_size: 0 or in [lo, hi_p]) checked before anything runs.
+static int window_ready(balm_batch *bt, const char *who) {
+  if (!bt) return invalid(std::string(who) + ": bad arguments");
+  if (!bt->win) return invalid(std::string(who) + ": call balm_batch_window_reset first");
+  return BALM_OK;
+}
+static int check_win_count(const char *who, const std::vector<int> &ns, const int *win_count) {
+  if (!win_count) return invalid(std::string(who) + ": bad arguments");
+  for (size_t b = 0; b < ns.size(); b++)
+    if (win_count[b] < 0 || win_count[b] > ns[b])
+      return invalid(std::string(who) + ": problem " + std::to_string(b) + ": win_count must be 0 or in [1, n_slots]");
+  return BALM_OK;
+}
+
+extern "C" int balm_batch_window_reset(balm_batch *bt, int n_problems, const int *n_slots, const balm_assoc_opts *opts) {
+  if (!bt || !n_slots || n_problems < 1) return invalid("balm_batch_window_reset: bad arguments");
+  for (int b = 0; b < n_problems; b++)
+    if (n_slots[b] < 1 || n_slots[b] > BALM_BATCH_MAX_POSES)
+      return invalid("balm_batch_window_reset: problem " + std::to_string(b) + ": n_slots must be in 1 .. BALM_BATCH_MAX_POSES");
+  CUDA_TRY(cudaSetDevice(bt->device));
+  CUDA_TRY(cudaStreamSynchronize(bt->stream));
+  return window_reset_build(&bt->win, "balm_batch_window_reset", n_problems, n_slots, resolve_assoc_opts(opts), true);
+}
+
+extern "C" int balm_batch_window_cut(balm_batch *bt, const int32_t *scan_of, const int *slot, int n_scans,
+                                     const int64_t *scan_ptr, const float *xyz, const double *poses12) {
+  const char *who = "balm_batch_window_cut";
+  TRY(window_ready(bt, who));
+  if (!scan_of || !slot || !scan_ptr || !poses12 || n_scans < 1) return invalid("balm_batch_window_cut: bad arguments");
+  if (scan_ptr[0] != 0) return invalid("balm_batch_window_cut: scan_ptr[0] must be 0");
+  for (int s = 0; s < n_scans; s++)
+    if (scan_ptr[s + 1] < scan_ptr[s]) return invalid("balm_batch_window_cut: scan_ptr must be ascending");
+  const std::vector<int> &ns = window_slots(bt->win);
+  int64_t n_items = 0;  // points replicated over the problems that take them
+  for (size_t b = 0; b < ns.size(); b++) {
+    const std::string w = "balm_batch_window_cut: problem " + std::to_string(b);
+    const int s = scan_of[b];
+    if (s == -1) continue;
+    if (s < 0 || s >= n_scans) return invalid(w + ": scan index outside [0, n_scans)");
+    if (slot[b] < 0 || slot[b] >= ns[b]) return invalid(w + ": slot outside [0, n_slots)");
+    n_items += scan_ptr[s + 1] - scan_ptr[s];
+  }
+  const int64_t n_points = scan_ptr[n_scans];
+  if (n_points > 0 && !xyz) return invalid("balm_batch_window_cut: bad arguments");
+  if (n_items >= ((int64_t)1 << 31) || n_points >= ((int64_t)1 << 31)) {
+    balm_set_error("balm_batch_window_cut: 2^31 or more points, counted once per problem that takes them (or in xyz)");
+    return BALM_ERR_UNSUPPORTED;
+  }
+  CUDA_TRY(cudaSetDevice(bt->device));
+  CUDA_TRY(cudaStreamSynchronize(bt->stream));
+  long long launches = 0;
+  return window_cut_build(bt->stream, *bt->win, who, scan_of, slot, n_scans, scan_ptr, xyz, poses12, &launches);
+}
+
+extern "C" int balm_batch_window_recut(balm_batch *bt, const int *win_count) {
+  TRY(window_ready(bt, "balm_batch_window_recut"));
+  TRY(check_win_count("balm_batch_window_recut", window_slots(bt->win), win_count));
+  CUDA_TRY(cudaSetDevice(bt->device));
+  CUDA_TRY(cudaStreamSynchronize(bt->stream));
+  long long launches = 0;
+  return window_recut_build(bt->stream, *bt->win, win_count, &launches);
+}
+
+extern "C" int balm_batch_window_marginalize(balm_batch *bt, const int *mg_size, const double *poses12,
+                                             const int *win_count) {
+  TRY(window_ready(bt, "balm_batch_window_marginalize"));
+  const std::vector<int> &ns = window_slots(bt->win);
+  TRY(check_win_count("balm_batch_window_marginalize", ns, win_count));
+  if (!mg_size) return invalid("balm_batch_window_marginalize: bad arguments");
+  for (size_t b = 0; b < ns.size(); b++)
+    if (mg_size[b] != 0 && (mg_size[b] < 1 || mg_size[b] >= win_count[b]))
+      return invalid("balm_batch_window_marginalize: problem " + std::to_string(b) +
+                     ": mg_size must be 0 or in [1, win_count)");
+  CUDA_TRY(cudaSetDevice(bt->device));
+  CUDA_TRY(cudaStreamSynchronize(bt->stream));
+  long long launches = 0;
+  return window_marginalize_build(bt->stream, *bt->win, mg_size, poses12, win_count, &launches);
+}
+
+extern "C" int balm_batch_window_push(balm_batch *bt, const int *win_count, int64_t *n_voxels_out, int64_t *n_obs_out) {
+  TRY(window_ready(bt, "balm_batch_window_push"));
+  const std::vector<int> &ns = window_slots(bt->win);
+  TRY(check_win_count("balm_batch_window_push", ns, win_count));
+  CUDA_TRY(cudaSetDevice(bt->device));
+  CUDA_TRY(cudaStreamSynchronize(bt->stream));
+  const int B = (int)ns.size();
+  std::vector<int64_t> pose_ptr((size_t)B + 1, 0), obs_ptr;
+  for (int b = 0; b < B; b++) pose_ptr[b + 1] = pose_ptr[b] + ns[b];
+  BatchReg *r = new BatchReg();
+  const WindowRegister reg = [&](const int64_t *vp, const int64_t *op, WindowEmit *out) {
+    const int64_t M = vp[B], K = op[B];
+    obs_ptr.assign(op, op + B + 1);
+    TRY(reg_layout(bt, r, B, pose_ptr.data(), vp, K));
+    TRY(dev_alloc(&r->row_ptr, (size_t)M + 1));
+    TRY(dev_alloc(&r->pose_idx, (size_t)K));
+    TRY(dev_alloc(&r->obs, (size_t)K * 10));
+    TRY(dev_alloc(&r->coe, (size_t)M));
+    TRY(dev_alloc(&r->fix, (size_t)M * 10));
+    TRY(dev_alloc(&r->key, (size_t)M));
+    TRY(dev_alloc(&r->layer, (size_t)M));
+    r->assoc = window_opts(bt->win);
+    *out = WindowEmit{r->row_ptr, r->pose_idx, r->obs, r->fix, r->coe, r->key, r->layer};
+    return (int)BALM_OK;
+  };
+  long long launches = 0;
+  int rc = window_push_build(bt->stream, *bt->win, win_count, reg, &launches);
+  if (rc == BALM_OK) rc = reg_finish(bt, r);
+  if (rc == BALM_OK)
+    for (int b = 0; b < B; b++) {
+      if (n_voxels_out) n_voxels_out[b] = r->hprob[b].nvox;
+      if (n_obs_out) n_obs_out[b] = obs_ptr[b + 1] - obs_ptr[b];
     }
   return install(bt, r, rc);
 }

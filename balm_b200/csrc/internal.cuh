@@ -770,3 +770,23 @@ int batch_marginalize_build(cudaStream_t st, const BatchVoxels &in, const int *m
 int batch_append_build(cudaStream_t st, const BatchVoxels &in, const balm_assoc_opts &o, const int32_t *scan_of,
                        const int *slot, const int64_t *scan_ptr, const float *xyz, int64_t n_points,
                        const WindowRegister &reg, int64_t *n_matched);
+
+// The persistent sliding-window octree of B problems (balm_window_* with B = 1, balm_batch_window_*). Problem p has
+// n_slots[p] slots and owns the pose rows [sum_{q<p} n_slots[q], ...) of every poses12 (host, P x 12). Arguments are
+// checked by the callers (who: prefix of error messages); per-problem arrays have B entries, 0 / -1 = problem left
+// alone. A rejected call (BALM_ERR_INVALID / UNSUPPORTED before anything changed) leaves the window as it was.
+// reset: o from resolve_assoc_opts, replaces *ws; batch: errors name the problem, 2^31 points are UNSUPPORTED.
+int window_reset_build(WindowState **ws, const char *who, int B, const int *n_slots, const balm_assoc_opts &o, bool batch);
+const std::vector<int> &window_slots(const WindowState *w);
+const balm_assoc_opts &window_opts(const WindowState *w);
+// cut: problem p takes scan scan_of[p] (xyz[scan_ptr[s] .. scan_ptr[s+1]) of the n_scans) into slot slot[p], at pose
+// row pose_base[p] + slot[p]
+int window_cut_build(cudaStream_t st, WindowState &w, const char *who, const int32_t *scan_of, const int *slot,
+                     int n_scans, const int64_t *scan_ptr, const float *xyz, const double *poses12, long long *launches);
+int window_recut_build(cudaStream_t st, WindowState &w, const int *win_count, long long *launches);
+// poses12 may be null (no re-transform)
+int window_marginalize_build(cudaStream_t st, WindowState &w, const int *mg, const double *poses12, const int *win_count,
+                             long long *launches);
+// the pushed nodes of every problem in ascending (problem, key), emitted where reg says (fix, key and layer always)
+int window_push_build(cudaStream_t st, WindowState &w, const int *win_count, const WindowRegister &reg,
+                      long long *launches);

@@ -167,8 +167,9 @@ int balm_download_keys(balm_ctx *ctx, uint64_t *keys, int32_t *layers);
  * balm_append_scan / balm_marginalize, which work on the flattened voxel set, the window keeps every node the reference
  * keeps: points outside the known planes grow new roots and leaves, a leaf that stops being planar is split further, and
  * a leaf that is not pushed stays in the map, dormant, with its fix cluster until later scans hit it again. Nodes are
- * never deleted (the reference never deletes them either): the map grows with the trajectory, by 104 + 160 * N bytes
- * per node (key, flags, fix cluster, and sig_orig + sig_tran for every slot), plus 52 bytes per point held.
+ * never deleted (the reference never deletes them either): the map grows with the trajectory, by 120 + 160 * N bytes
+ * per node (key, problem, flags, fix cluster, lookup entry, and sig_orig + sig_tran for every slot), plus 56 bytes per
+ * point held. This is the one-problem case of balm_batch_window_* below.
  * The window is independent of the registered voxel set: balm_set_voxels, balm_cut_voxels, balm_append_scan,
  * balm_marginalize and balm_synth_virtual do not touch it; balm_destroy frees it. A rejected call (BALM_ERR_INVALID:
  * slot outside [0, N), win_count outside [1, N], mg_size outside [1, win_count), no balm_window_reset before) leaves the
@@ -286,6 +287,39 @@ int balm_batch_append_scan(balm_batch *b, const int32_t *scan_of, const int *slo
                            const float *xyz, const double *poses12, int64_t *n_voxels_out, int64_t *n_obs_out,
                            int64_t *n_matched_out);
 int balm_batch_download_fix(balm_batch *b, double *fix10);
+/* Persistent sliding-window octrees for a batch: B independent window maps (balm_window_* above), one per problem, kept
+ * in HBM across shifts and driven together; balm_batch_window_push turns them into the batch's registration, so
+ * balm_batch_damping_iter, balm_batch_pose_covariance, balm_batch_marginalize and balm_batch_append_scan run on it.
+ * balm_batch_window_reset: problem p gets n_slots[p] (1 .. BALM_BATCH_MAX_POSES) window slots and owns the pose rows
+ * [sum_{q<p} n_slots[q], ...) of every poses12 (P x 12, P = sum n_slots), laid out as in the other batch calls; opts as
+ * balm_window_reset (NULL = defaults), the same for every problem. Replaces any earlier window maps.
+ * balm_batch_window_cut: scans are given once (scan s = xyz[scan_ptr[s] .. scan_ptr[s+1]), float32, body frame); one scan
+ * may serve several problems, at different poses and slots. Problem p with scan_of[p] >= 0 takes that scan into slot
+ * slot[p] at pose row pose_base[p] + slot[p]; scan_of[p] == -1 leaves its map alone.
+ * balm_batch_window_recut / marginalize / push: win_count[p] (and mg_size[p]) as the balm_window_* call of that name;
+ * win_count[p] == 0 (marginalize: mg_size[p] == 0) leaves problem p's map alone, and push gives it an empty voxel range.
+ * After any sequence of these calls, problem p's push is bitwise what balm_window_push registers on a context of
+ * n_slots[p] poses reset with the same opts and driven by the same calls on its scans, pose rows, slots and counts (a
+ * skipped problem = a call not made): keys, layers, row_ptr, pose_idx, obs10, fix clusters, coe, M and K. A problem's
+ * result does not depend on the rest of the batch or on its position in it; two identical call sequences are bitwise
+ * equal. Push replaces the registration (N_p = n_slots[p], fix clusters always present, keys, layers and the association
+ * options carried); n_voxels_out / n_obs_out: [B] or NULL. The window maps are independent of the registration:
+ * balm_batch_set_voxels, cut_voxels, marginalize and append_scan do not touch them; balm_batch_destroy frees them.
+ * Memory: 120 + 160 * max n_slots bytes per node and 56 bytes per point held, summed over the problems. Host waits per
+ * call are a fixed number whatever B (recut: a fixed number per octree layer).
+ * BALM_ERR_INVALID leaves both the window maps and the registration unchanged: no balm_batch_window_reset before;
+ * n_problems < 1 or n_slots outside 1 .. BALM_BATCH_MAX_POSES; scan_of outside -1 and [0, n_scans); slot outside
+ * [0, n_slots[p]); scan_ptr not starting at 0 or not ascending; win_count outside 0 and [1, n_slots[p]]; mg_size outside
+ * 0 and [1, win_count[p]); a point outside the +-2^18 root-voxel range (checked on the device before any map changes).
+ * BALM_ERR_UNSUPPORTED, before anything is allocated: 2^31 or more points, counted once per problem that takes them (or
+ * in xyz, or in the maps). Messages name the lowest offending problem. */
+int balm_batch_window_reset(balm_batch *b, int n_problems, const int *n_slots, const balm_assoc_opts *opts);
+int balm_batch_window_cut(balm_batch *b, const int32_t *scan_of, const int *slot, int n_scans, const int64_t *scan_ptr,
+                          const float *xyz, const double *poses12);
+int balm_batch_window_recut(balm_batch *b, const int *win_count);
+int balm_batch_window_marginalize(balm_batch *b, const int *mg_size, const double *poses12 /* P x 12 or NULL */,
+                                  const int *win_count);
+int balm_batch_window_push(balm_batch *b, const int *win_count, int64_t *n_voxels_out, int64_t *n_obs_out);
 /* balm_pose_covariance per problem, all problems in one call: problem p's results are those of balm_pose_covariance on
  * a BALM_PREC_FP64 context holding only problem p, at its rows of poses12 (P x 12, read only). c_cov81: K x 81 in
  * registration order (the order of obs10), or NULL for isotropic point noise of standard deviation point_noise.

@@ -5,7 +5,8 @@ Workloads (HBA's bottom layer splits a trajectory into many short windows): (a) 
 (b) 32 windows x 32 poses x 5 000 planes, and (c) one bottom layer from raw scans: 160 synthetic scans of 20 000
 points (assoc_ref.synthetic_scans, room 12), windows of 10 scans every 5 scans (31 windows), associated per window and as
 one batch (see run_from_scans), (d) the pose covariance of the windows of (a) and (b) with fix clusters (see
-run_covariance), and (e) a Monte Carlo sliding window of 64 sequences (see run_sliding_window). For (a) and (b) every window is generated on the GPU by Context.synth_virtual (its own seed) and
+run_covariance), (e) a Monte Carlo sliding window of 64 sequences (see run_sliding_window), (f) the same on the persistent window
+maps (see run_persistent_window). For (a) and (b) every window is generated on the GPU by Context.synth_virtual (its own seed) and
 read back with download_voxels, so the batch and the loop run on the same host arrays. Two option sets: fixed work
 (force_hess, rel_tol < 0, 10 iterations: every LM iteration does the same work) and the defaults. The batch, the fp64 loop
 and the tensor loop alternate --repeats times in one process; every call ends in a device synchronisation, so a host clock
@@ -389,6 +390,145 @@ def run_sliding_window(n_seq, window, mg, shifts, pts_per_scan, room):
                 max_rel_cov_diff_ii_vs_i=dcov, batch_cov_statuses=sorted(statuses))
 
 
+def run_persistent_window(n_seq, window, mg, shifts, pts_per_scan):
+    """Workload (f), workload (e) on the persistent window maps: n_seq independent sequences of window_ref.growth_scans
+    (one seed and step each, scans that keep reaching new space), a window of `window` scans cut, recut, pushed and
+    optimised once, then `shifts` window shifts, each marginalising the mg oldest scans at the optimised poses, cutting
+    and recutting mg new ones, pushing, optimising with the fix clusters and propagating the pose covariance:
+    (i) a Context window (fp64) per sequence; (ii) one Batch window for all of them (balm_batch_window_*). The context
+    route marginalises at the batch route's poses, so their pushes must be bitwise equal (checked after every shift,
+    outside the timed calls). Also counts, per shift, the voxels the reduced batch path (cut_scans, then marginalize +
+    append_scans, workload (e)'s calls) keeps on the same stream."""
+    import scenes
+    import window_ref
+    import balm_b200
+    n_scans = window + mg * shifts
+    seqs = []
+    for q in range(n_seq):
+        pts, frs, noisy, _ = window_ref.growth_scans(n_scans=n_scans, pts_per_scan=pts_per_scan, seed=200 + q,
+                                                     step=0.3 + 0.01 * (q % 30))
+        p12 = scenes.pack_poses([r for r, _ in noisy], [p for _, p in noisy])
+        seqs.append(([pts[frs == i].astype(np.float32) for i in range(n_scans)], p12))
+    kwc = dict(voxel_size=2.0, layer_limit=2, min_ps=15, eigen_value_array=(1 / 16, 1 / 16, 1 / 9))
+    lm_kw = dict(gauge_mode=2, min_planes_per_pose=0)
+    cov_kw = dict(point_noise=0.01, include_fix=True)
+    B = n_seq
+
+    def clock(f):
+        t0 = time.perf_counter()
+        r = f()
+        return r, 1e3 * (time.perf_counter() - t0)
+
+    def poses_at(q, slot_scans):
+        x = np.zeros((window, 12))
+        x[:len(slot_scans)] = seqs[q][1][slot_scans]
+        return x
+
+    batch = balm_b200.Batch(0)
+    batch.window_reset([window] * B, **kwc)
+    ctx = [balm_b200.Context(window, 0, balm_b200.PREC_FP64) for _ in range(B)]
+    for c in ctx:
+        c.window_reset(**kwc)
+    init = [poses_at(q, list(range(window))) for q in range(B)]
+    for s in range(window):  # fill
+        batch.window_cut([seqs[q][0][s] for q in range(B)], list(range(B)), [s] * B, init)
+        batch.window_recut([s + 1] * B)
+        for q, c in enumerate(ctx):
+            c.window_cut(seqs[q][0][s], init[q][s], s)
+            c.window_recut(s + 1)
+    first_push = batch.window_push([window] * B)
+    for c in ctx:
+        c.window_push(window)
+    x_b = [r[1] for r in batch.damping_iter(init, **lm_kw)]
+    for q, c in enumerate(ctx):
+        c.damping_iter(init[q], **lm_kw)
+    # the reduced path on the same stream, for its voxel counts only
+    red = balm_b200.Batch(0)
+    cut = red.cut_scans([sc for q in range(B) for sc in seqs[q][0][:window]],
+                        [list(range(q * window, (q + 1) * window)) for q in range(B)], init, **kwc)
+    x_r = [r[1] for r in red.damping_iter(init, **lm_kw)]
+    red_vox = [int(sum(m for m, _ in cut))]
+
+    parts = ("marginalize", "cut", "recut", "push", "lm", "cov")
+    ms = {"i_context": [], "ii_batch": []}
+    ms_part = {r: {k: [] for k in parts} for r in ms}
+    vox = [int(sum(m for m, _ in first_push))]
+    bitwise, dpose, statuses, ctx_statuses = True, 0.0, set(), set()
+    for k in range(shifts):
+        new = [window + mg * k + j for j in range(mg)]
+        shifted = [np.vstack([x_b[q][mg:], seqs[q][1][new]]) for q in range(B)]
+        tb = dict.fromkeys(parts, 0.0)
+        _, tb["marginalize"] = clock(lambda: batch.window_marginalize([mg] * B, x_b, [window] * B))
+        for j in range(mg):
+            slot = window - mg + j
+            _, t = clock(lambda: batch.window_cut([seqs[q][0][new[j]] for q in range(B)], list(range(B)), [slot] * B,
+                                                  shifted))
+            tb["cut"] += t
+            _, t = clock(lambda: batch.window_recut([slot + 1] * B))
+            tb["recut"] += t
+        pushed, tb["push"] = clock(lambda: batch.window_push([window] * B))
+        reg = batch.download_voxels(with_keys=True, with_fix=True)  # for the check, not part of the route
+        lm, tb["lm"] = clock(lambda: batch.damping_iter(shifted, hess_includes_fix=True, **lm_kw))
+        cov, tb["cov"] = clock(lambda: batch.pose_covariance([r[1] for r in lm], **cov_kw))
+        tc = dict.fromkeys(parts, 0.0)
+        ref = []
+        for q, c in enumerate(ctx):
+            _, t = clock(lambda: c.window_marginalize(mg, x_b[q], window))
+            tc["marginalize"] += t
+            for j in range(mg):
+                slot = window - mg + j
+                _, t = clock(lambda: c.window_cut(seqs[q][0][new[j]], shifted[q][slot], slot))
+                tc["cut"] += t
+                _, t = clock(lambda: c.window_recut(slot + 1))
+                tc["recut"] += t
+            _, t = clock(lambda: c.window_push(window))
+            tc["push"] += t
+            rp, pi, ob, co = c.download_voxels()
+            keys, layers = c.download_keys(with_layers=True)
+            d = reg[q]
+            bitwise = bitwise and (np.array_equal(rp, d["row_ptr"]) and np.array_equal(pi, d["pose_idx"]) and
+                                   np.array_equal(ob, d["obs10"]) and np.array_equal(co, d["coe"]) and
+                                   np.array_equal(c.download_fix(), d["fix10"]) and np.array_equal(keys, d["keys"]) and
+                                   np.array_equal(layers, d["layers"]))
+            (p, _, _), t = clock(lambda: c.damping_iter(shifted[q], hess_includes_fix=True, **lm_kw))
+            tc["lm"] += t
+            t0 = time.perf_counter()
+            try:  # the context reports a singular H (a weakly observed direction) as an error, the batch as a status
+                c.pose_covariance(p, **cov_kw)
+                ctx_statuses.add(0)  # BALM_OK
+            except balm_b200.BalmError as e:
+                ctx_statuses.add(e.status)
+            tc["cov"] += 1e3 * (time.perf_counter() - t0)
+            ref.append(p)
+        for route, tt in (("ii_batch", tb), ("i_context", tc)):
+            ms[route].append(sum(tt.values()))
+            for key in parts:
+                ms_part[route][key].append(tt[key])
+        for (st, p, _, _), (cst, _, _), pc in zip(lm, cov, ref):
+            statuses.add(cst)
+            dpose = max(dpose, float(np.abs(p - pc).max()))
+        x_b = [r[1] for r in lm]
+        vox.append(int(sum(m for m, _ in pushed)))
+        # the reduced path: marginalise at its own optimised poses, append the same scans, optimise
+        red.marginalize([mg] * B, x_r)
+        shifted_r = [np.vstack([x_r[q][mg:], seqs[q][1][new]]) for q in range(B)]
+        for j in range(mg):
+            app = red.append_scans([seqs[q][0][new[j]] for q in range(B)], list(range(B)), [window - mg + j] * B,
+                                   shifted_r)
+        red_vox.append(int(sum(m for m, _, _ in app)))
+        x_r = [r[1] for r in red.damping_iter(shifted_r, hess_includes_fix=True, **lm_kw)]
+    batch.close()
+    red.close()
+    for c in ctx:
+        c.close()
+    return dict(sequences=n_seq, window=window, mg=mg, shifts=shifts, pts_per_scan=pts_per_scan, ms=ms,
+                ms_median_per_shift={k: float(np.median(v)) for k, v in ms.items()}, ms_per_call_kind=ms_part,
+                ms_per_call_kind_median={r: {k: float(np.median(v)) for k, v in d.items()} for r, d in ms_part.items()},
+                voxels_per_shift_persistent=vox, voxels_per_shift_reduced=red_vox,
+                pushes_bitwise_equal=bool(bitwise), max_pose_diff_ii_vs_i=dpose, batch_cov_statuses=sorted(statuses),
+                context_cov_statuses=sorted(ctx_statuses))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--repeats", type=int, default=3)
@@ -402,6 +542,8 @@ def main():
             res[w] = run_from_scans(160, 20000, 12.0, a.repeats)
         elif w == "e":
             res[w] = run_sliding_window(64, 10, 2, 5, 20000, 12.0)
+        elif w == "f":
+            res[w] = run_persistent_window(64, 10, 2, 10, 20000)
         elif w == "d":
             res[w] = {k: run_covariance(k, *shapes[k][:3], a.repeats, shapes[k][3]) for k in ("a", "b")}
         else:

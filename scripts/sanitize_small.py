@@ -4,7 +4,8 @@ association chain balm_cut_voxels -> balm_marginalize -> balm_append_scan (octre
 independent problems (balm_batch_*: a dense one with fix clusters, a sparse one of 32 poses, an empty one), and a batch
 association of overlapping windows with one empty window (balm_batch_cut_voxels), the batch pose covariance of
 an anchored, a free and an empty problem (balm_batch_pose_covariance), and the batched marginalise + append of those
-windows, the empty one included (balm_batch_marginalize / balm_batch_append_scan)."""
+windows, the empty one included (balm_batch_marginalize / balm_batch_append_scan), and the batch's persistent window maps
+(balm_batch_window_*)."""
 import os, sys
 import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -75,5 +76,20 @@ x = [r[1] for r in res]
 mm = b.marginalize([1, 1, 0], x)
 ma = b.append_scans(scans, [5, 5, -1], [3, 3, 0], x)
 print("batch marginalise", mm, "append", ma, "fix rows", len(b.download_voxels(with_fix=True)[0]["fix10"]), flush=True)
+b.close()
+# persistent window maps of a batch: 4 and 3 slots, the shared scan 2 cut into both, one problem skipped in each call,
+# a shift of the first problem, a push with one empty range
+b = balm_b200.Batch(0)
+b.window_reset([4, 3], layer_limit=2)
+wx = [p12[:4], p12[2:5]]
+for s in range(3):
+    b.window_cut(scans, [s, 2 + s], [s, s], wx)
+    b.window_recut([s + 1, s + 1])
+b.window_cut(scans, [3, -1], [3, 0], wx)
+b.window_recut([4, 0])
+b.window_marginalize([2, 0], wx, [4, 0])
+b.window_cut(scans, [4, -1], [2, 0], [p12[2:6], wx[1]])
+b.window_recut([3, 0])
+print("batch window push", b.window_push([3, 0]), b.window_push([3, 3]), flush=True)
 b.close()
 print("SANITIZE_DONE")
