@@ -54,7 +54,7 @@ SYMBOLS = ["balm_last_error", "balm_version", "balm_create", "balm_destroy", "ba
            "balm_batch_damping_iter", "balm_batch_cut_voxels", "balm_batch_sizes", "balm_batch_download_voxels",
            "balm_batch_pose_covariance", "balm_batch_marginalize", "balm_batch_append_scan", "balm_batch_download_fix",
            "balm_batch_window_reset", "balm_batch_window_cut", "balm_batch_window_recut", "balm_batch_window_marginalize",
-           "balm_batch_window_push"]
+           "balm_batch_window_push", "balm_batch_merge_scans"]
 
 
 def lib():
@@ -117,6 +117,8 @@ def lib():
                                               C.c_void_p, C.c_void_p]
         L.balm_batch_cut_voxels.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int] + [C.c_void_p] * 3 + \
                                            [C.POINTER(AssocOpts), C.c_void_p, C.c_void_p]
+        L.balm_batch_merge_scans.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int] + [C.c_void_p] * 3 + \
+                                            [C.c_double, C.c_void_p, C.c_void_p]
         L.balm_batch_sizes.argtypes = [C.c_void_p, C.POINTER(C.c_int)] + [C.POINTER(C.c_int64)] * 3
         L.balm_batch_download_voxels.argtypes = [C.c_void_p] + [C.c_void_p] * 7
         L.balm_batch_pose_covariance.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_double, C.c_int] + \

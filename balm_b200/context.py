@@ -296,6 +296,26 @@ class Batch:
         self._pose_ptr = pose_ptr
         return [(int(m), int(k)) for m, k in zip(M, K)]
 
+    def merge_scans(self, scans, windows, poses_list, voxel_size):
+        """Keyframes on the device (include/balm_b200.h, balm_batch_merge_scans): per window, its scans' points in the
+        body frame of its slot 0 at poses_list[w], down-sampled at voxel_size (< 0.001: not reduced). scans / windows as
+        cut_scans. Leaves the registration alone. -> per window an (n_w x 3) float32 cloud, voxels in ascending order."""
+        scans = [np.asarray(s, dtype=np.float32).reshape(-1, 3) for s in scans]
+        n_poses = [len(w) for w in windows]
+        scan_ptr = np.concatenate([[0], np.cumsum([len(s) for s in scans])]).astype(np.int64)
+        pose_ptr = np.concatenate([[0], np.cumsum(n_poses)]).astype(np.int64)
+        pose_scan = np.ascontiguousarray(np.concatenate([np.asarray(w, dtype=np.int64).ravel() for w in windows]),
+                                         dtype=np.int32)
+        xyz = np.ascontiguousarray(np.concatenate(scans) if scans else np.zeros((0, 3)), dtype=np.float32)
+        poses = np.ascontiguousarray(np.concatenate([np.asarray(p, dtype=np.float64).reshape(n, 12)
+                                                     for p, n in zip(poses_list, n_poses)]), dtype=np.float64)
+        n_items = int(sum(scan_ptr[s + 1] - scan_ptr[s] for s in pose_scan))
+        kf_ptr = np.zeros(len(windows) + 1, dtype=np.int64)
+        kf = np.zeros((n_items, 3), dtype=np.float32)
+        L.check(L.lib().balm_batch_merge_scans(self._h, len(windows), _p(pose_ptr), _p(pose_scan), len(scans),
+                                               _p(scan_ptr), _p(xyz), _p(poses), float(voxel_size), _p(kf_ptr), _p(kf)))
+        return [kf[kf_ptr[w]:kf_ptr[w + 1]].copy() for w in range(len(windows))]
+
     def marginalize(self, mg_sizes, poses_list, min_ps=15):
         """Context.marginalize per problem, all in one call (include/balm_b200.h, balm_batch_marginalize): the oldest
         mg_sizes[p] scans of problem p folded into its fix clusters at its poses; 0 leaves a problem unchanged. A problem

@@ -505,6 +505,196 @@ int assoc_cut(cudaStream_t st, const AssocInput &in, const balm_assoc_opts &o, c
   return BALM_OK;
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// Keyframe merge of a batch (balm_batch_merge_scans): the items of the cut, (problem, slot, point), are moved into the
+// body frame of their problem's slot 0 and reduced by down_sampling_voxel (tools.hpp:203-242) with a deterministic mean.
+// Items are sorted stably by the 63-bit key [ix | iy | iz] (21 bits each, biased by 2^20), then stably by problem, so
+// that a voxel's points keep their item order and every problem's voxels come out in ascending (ix, iy, iz).
+namespace {
+
+constexpr int KF_BITS = 21;
+constexpr long long KF_BIAS = 1ll << 20;
+
+// q = R_a^T (R_k b + t_k - t_a), every operation correctly rounded in this order (no contraction), rounded to float;
+// with reduce, the down-sampling key of q, and the lowest problem with an index outside +-2^20 in *bad.
+__global__ void merge_item_kernel(const float *xyz, const int *src, const int *row, const int *row_prob,
+                                  const long long *pose_ptr, const double *poses, int64_t n, bool reduce, float vs,
+                                  float *q, unsigned long long *key, int *bad) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int f = row[i], p = row_prob[f];
+  double r[9], t[3], ra[9], ta[3];
+  load_pose(poses + 12 * (size_t)f, r, t);
+  load_pose(poses + 12 * (size_t)pose_ptr[p], ra, ta);
+  const int64_t j = src[i];
+  const double b[3] = {(double)xyz[3 * j], (double)xyz[3 * j + 1], (double)xyz[3 * j + 2]};
+  double d[3];
+#pragma unroll
+  for (int a = 0; a < 3; a++) {
+    const double w = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(r[a * 3], b[0]), __dmul_rn(r[a * 3 + 1], b[1])),
+                                         __dmul_rn(r[a * 3 + 2], b[2])), t[a]);
+    d[a] = __dsub_rn(w, ta[a]);
+  }
+  unsigned long long k = 0;
+  bool out = false;
+#pragma unroll
+  for (int a = 0; a < 3; a++) {
+    const float qa = __double2float_rn(__dadd_rn(__dadd_rn(__dmul_rn(ra[a], d[0]), __dmul_rn(ra[3 + a], d[1])),
+                                                 __dmul_rn(ra[6 + a], d[2])));
+    q[3 * i + a] = qa;
+    float loc = __fdiv_rn(qa, vs);  // the float32 quotient of tools.hpp:215-217, "-1 for negatives", truncated
+    if (loc < 0) loc -= 1.0f;
+    out |= !(loc > -(float)(KF_BIAS + 1) && loc < (float)KF_BIAS);  // catches NaN too
+    const long long idx = out ? 0 : (long long)loc;
+    k = (k << KF_BITS) | (unsigned long long)(idx + KF_BIAS);
+  }
+  if (!reduce) return;
+  if (out) atomicMin(bad, p);
+  key[i] = k;
+}
+// a (problem, voxel) segment starts where the key or the problem changes
+__global__ void merge_flag_kernel(const unsigned long long *key, const int *idx, const int *row, const int *row_prob,
+                                  int64_t n, int *flag) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  flag[i] = (i == 0 || key[idx[i]] != key[idx[i - 1]] || row_prob[row[idx[i]]] != row_prob[row[idx[i - 1]]]) ? 1 : 0;
+}
+// kf_ptr[p] = voxels of the problems below p: the voxel count before the first sorted item of a problem >= p (sorted
+// problem ids in sprob; null when B = 1)
+__global__ void merge_offsets_kernel(const unsigned *sprob, const int *flag, const int *scan, int64_t n, int B,
+                                     long long *kf_ptr) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p > B) return;
+  int64_t lo = 0, hi = n;  // first position whose problem is >= p
+  if (sprob) {
+    while (lo < hi) {
+      const int64_t m = (lo + hi) / 2;
+      if ((int)sprob[m] < p) lo = m + 1; else hi = m;
+    }
+  } else {
+    lo = p == 0 ? 0 : n;
+  }
+  kf_ptr[p] = lo < n ? scan[lo] : scan[n - 1] + flag[n - 1];
+}
+// one thread per (problem, voxel): the fp64 sum of its points in item order over the count, rounded to float
+__global__ void merge_reduce_kernel(const float *q, const int *idx, const int *vstart, int nvox, int64_t n, float *out) {
+  const int v = blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= nvox) return;
+  const int64_t a = vstart[v], b = v + 1 < nvox ? vstart[v + 1] : n;
+  double s[3] = {0.0, 0.0, 0.0};
+  for (int64_t e = a; e < b; e++) {
+    const int64_t j = idx[e];
+#pragma unroll
+    for (int c = 0; c < 3; c++) s[c] = __dadd_rn(s[c], (double)q[3 * j + c]);
+  }
+#pragma unroll
+  for (int c = 0; c < 3; c++) out[3 * (int64_t)v + c] = __double2float_rn(__ddiv_rn(s[c], (double)(b - a)));
+}
+
+}  // namespace
+
+int merge_scans_build(cudaStream_t st, const MergeInput &in, int64_t *kf_ptr, float *kf_xyz, long long *launches) {
+  const int B = in.n_problems, n_rows = (int)in.pose_ptr[B];
+  const int64_t n = in.n_items;
+  const bool reduce = in.voxel_size >= 0.001;
+  std::vector<long long> tab((size_t)2 * n_rows + 1);  // item_ptr [n_rows + 1], then the first point of each row
+  std::vector<int> hprob((size_t)n_rows);
+  tab[0] = 0;
+  for (int p = 0; p < B; p++)
+    for (int64_t j = in.pose_ptr[p]; j < in.pose_ptr[p + 1]; j++) {
+      const int s = in.pose_scan[j];
+      tab[j + 1] = tab[j] + (in.scan_ptr[s + 1] - in.scan_ptr[s]);
+      tab[(size_t)n_rows + 1 + j] = in.scan_ptr[s];
+      hprob[j] = p;
+    }
+  std::vector<long long> hptr((size_t)B + 1);
+  if (!reduce)  // no reduction: keyframe p is its items, in (slot, point) order
+    for (int p = 0; p <= B; p++) hptr[p] = tab[in.pose_ptr[p]];
+  if (n == 0) {
+    if (reduce) std::fill(hptr.begin(), hptr.end(), 0ll);
+    for (int p = 0; p <= B; p++) kf_ptr[p] = hptr[p];
+    return BALM_OK;
+  }
+  ScratchPool pool;
+  float *xyz = nullptr, *q = nullptr;
+  double *poses = nullptr;
+  long long *dtab = nullptr, *dpose_ptr = nullptr;
+  int *src = nullptr, *row = nullptr, *row_prob = nullptr, *bad = nullptr;
+  unsigned long long *key = nullptr;
+  TRY(pool.get(&xyz, (size_t)3 * in.n_points)); TRY(pool.get(&poses, (size_t)12 * n_rows));
+  TRY(pool.get(&dtab, tab.size())); TRY(pool.get(&dpose_ptr, (size_t)B + 1)); TRY(pool.get(&row_prob, (size_t)n_rows));
+  TRY(pool.get(&src, (size_t)n)); TRY(pool.get(&row, (size_t)n)); TRY(pool.get(&q, (size_t)3 * n));
+  TRY(pool.get(&bad, 1));
+  if (reduce) TRY(pool.get(&key, (size_t)n));
+  CUDA_TRY(cudaMemcpyAsync(xyz, in.xyz, sizeof(float) * 3 * in.n_points, cudaMemcpyHostToDevice, st));
+  CUDA_TRY(cudaMemcpyAsync(poses, in.poses12, sizeof(double) * 12 * n_rows, cudaMemcpyHostToDevice, st));
+  CUDA_TRY(cudaMemcpyAsync(dtab, tab.data(), sizeof(long long) * tab.size(), cudaMemcpyHostToDevice, st));
+  CUDA_TRY(cudaMemcpyAsync(dpose_ptr, in.pose_ptr, sizeof(long long) * (B + 1), cudaMemcpyHostToDevice, st));
+  CUDA_TRY(cudaMemcpyAsync(row_prob, hprob.data(), sizeof(int) * n_rows, cudaMemcpyHostToDevice, st));
+  CUDA_TRY(cudaMemsetAsync(bad, 0x7f, sizeof(int), st));  // 0x7f7f7f7f: no problem is that large
+  const unsigned gb = (unsigned)((n + 255) / 256);
+  expand_rows_kernel<<<n_rows, 256, 0, st>>>(dtab, dtab + n_rows + 1, src, row);
+  merge_item_kernel<<<gb, 256, 0, st>>>(xyz, src, row, row_prob, dpose_ptr, poses, n, reduce, (float)in.voxel_size, q,
+                                        key, bad);
+  *launches += 2;
+  if (!reduce) {
+    CUDA_TRY(cudaMemcpyAsync(kf_xyz, q, sizeof(float) * 3 * n, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    CUDA_TRY(cudaGetLastError());
+    for (int p = 0; p <= B; p++) kf_ptr[p] = hptr[p];
+    return BALM_OK;
+  }
+  int *idx = nullptr, *work = nullptr, *work2 = nullptr, *flag = nullptr, *scan = nullptr;
+  unsigned *pk = nullptr, *pk2 = nullptr;
+  unsigned long long *key2 = nullptr;
+  long long *dkf = nullptr;
+  TRY(pool.get(&idx, (size_t)n)); TRY(pool.get(&work, (size_t)n)); TRY(pool.get(&work2, (size_t)n));
+  TRY(pool.get(&flag, (size_t)n)); TRY(pool.get(&scan, (size_t)n)); TRY(pool.get(&key2, (size_t)n));
+  TRY(pool.get(&pk, (size_t)n)); TRY(pool.get(&pk2, (size_t)n)); TRY(pool.get(&dkf, (size_t)B + 1));
+  int pbits = 1;
+  while ((1 << pbits) < B) pbits++;
+  size_t tb1 = 0, tb2 = 0, tb3 = 0;
+  cub::DeviceRadixSort::SortPairs(nullptr, tb1, key, key2, idx, work, (int)n, 0, 3 * KF_BITS, st);
+  cub::DeviceRadixSort::SortPairs(nullptr, tb2, pk, pk2, work, work2, (int)n, 0, pbits, st);
+  cub::DeviceScan::ExclusiveSum(nullptr, tb3, flag, scan, (int)n, st);
+  size_t tmp_bytes = std::max(tb1, std::max(tb2, tb3));
+  char *tmp = nullptr;
+  TRY(pool.get(&tmp, tmp_bytes));
+  iota_kernel<<<gb, 256, 0, st>>>(idx, n);
+  CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, key, key2, idx, work, (int)n, 0, 3 * KF_BITS, st));
+  if (B > 1) {
+    gather_prob_kernel<<<gb, 256, 0, st>>>(work, row, row_prob, pk, n);
+    CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, pk, pk2, work, work2, (int)n, 0, pbits, st));
+    std::swap(work, work2);
+    *launches += 2;
+  }
+  merge_flag_kernel<<<gb, 256, 0, st>>>(key, work, row, row_prob, n, flag);
+  CUDA_TRY(cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, flag, scan, (int)n, st));
+  int *vstart = work2;  // free after the sorts (n >= the voxel count)
+  seg_start_kernel<<<gb, 256, 0, st>>>(flag, scan, n, vstart);
+  merge_offsets_kernel<<<(B + 128) / 128, 128, 0, st>>>(B > 1 ? pk2 : nullptr, flag, scan, n, B, dkf);
+  int h_bad = 0;
+  CUDA_TRY(cudaMemcpyAsync(hptr.data(), dkf, sizeof(long long) * (B + 1), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaMemcpyAsync(&h_bad, bad, sizeof(int), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  *launches += 6;
+  if (h_bad != 0x7f7f7f7f) {
+    balm_set_error(std::string(in.who) + ": problem " + std::to_string(h_bad) +
+                   ": a point's voxel index lies outside +-2^20 at this voxel_size");
+    return BALM_ERR_INVALID;
+  }
+  const int nvox = (int)hptr[B];
+  float *out = nullptr;
+  TRY(pool.get(&out, (size_t)3 * nvox));
+  merge_reduce_kernel<<<(unsigned)((nvox + 127) / 128), 128, 0, st>>>(q, work, vstart, nvox, n, out);
+  *launches += 1;
+  CUDA_TRY(cudaMemcpyAsync(kf_xyz, out, sizeof(float) * 3 * nvox, cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  CUDA_TRY(cudaGetLastError());
+  for (int p = 0; p <= B; p++) kf_ptr[p] = hptr[p];
+  return BALM_OK;
+}
+
 
 // ---------------------------------------------------------------------------------------------------------------------
 // Pose-major observation lists of a sparse co-visibility problem (the reference walks a voxel's win_size slots and

@@ -1027,6 +1027,38 @@ extern "C" int balm_batch_cut_voxels(balm_batch *bt, int n_problems, const int64
   return install(bt, r, rc);
 }
 
+extern "C" int balm_batch_merge_scans(balm_batch *bt, int n_problems, const int64_t *pose_ptr, const int32_t *pose_scan,
+                                      int n_scans, const int64_t *scan_ptr, const float *xyz, const double *poses12,
+                                      double voxel_size, int64_t *kf_ptr, float *kf_xyz) {
+  if (!bt || !pose_ptr || !pose_scan || !scan_ptr || !poses12 || !kf_ptr || n_scans < 1)
+    return invalid("balm_batch_merge_scans: bad arguments");
+  TRY(check_pose_ptr("balm_batch_merge_scans", n_problems, pose_ptr));
+  if (scan_ptr[0] != 0) return invalid("balm_batch_merge_scans: scan_ptr[0] must be 0");
+  for (int s = 0; s < n_scans; s++)
+    if (scan_ptr[s + 1] < scan_ptr[s]) return invalid("balm_batch_merge_scans: scan_ptr must be ascending");
+  if (!std::isfinite(voxel_size)) return invalid("balm_batch_merge_scans: voxel_size must be finite");
+  const int64_t P = pose_ptr[n_problems], n_points = scan_ptr[n_scans];
+  int64_t n_items = 0;
+  for (int64_t j = 0; j < P; j++) {
+    const int s = pose_scan[j];
+    if (s < 0 || s >= n_scans) return invalid("balm_batch_merge_scans: pose_scan entry outside [0, n_scans)");
+    n_items += scan_ptr[s + 1] - scan_ptr[s];
+  }
+  if ((n_points > 0 && !xyz) || (n_items > 0 && !kf_xyz)) return invalid("balm_batch_merge_scans: bad arguments");
+  if (n_items >= ((int64_t)1 << 31) || n_points >= ((int64_t)1 << 31)) {
+    balm_set_error("balm_batch_merge_scans: 2^31 or more points, counted once per pose row that uses them");
+    return BALM_ERR_UNSUPPORTED;
+  }
+  CUDA_TRY(cudaSetDevice(bt->device));
+  CUDA_TRY(cudaStreamSynchronize(bt->stream));
+  const MergeInput in{"balm_batch_merge_scans", n_problems, pose_ptr, pose_scan, scan_ptr, n_points, xyz, poses12,
+                      voxel_size, n_items};
+  long long launches = 0;
+  const int rc = merge_scans_build(bt->stream, in, kf_ptr, kf_xyz, &launches);
+  if (rc != BALM_OK) cudaStreamSynchronize(bt->stream);
+  return rc;
+}
+
 // ---- sliding window (assoc.cu: batch_marginalize_build / batch_append_build) ----
 // The registration as those steps read it; pose_ptr / voxel_ptr receive the host tables it points into.
 static BatchVoxels window_input(const BatchReg *r, const double *poses12, std::vector<int64_t> &pose_ptr,

@@ -731,6 +731,22 @@ balm_assoc_opts resolve_assoc_opts(const balm_assoc_opts *opts);  // opts or the
 // opts: from resolve_assoc_opts, layer_limit in 0..2 (checked by the caller)
 int assoc_cut(cudaStream_t st, const AssocInput &in, const balm_assoc_opts &opts, const AssocRegister &reg,
               long long *launches);
+// Keyframes of a batch (balm_batch_merge_scans): the problem table and scan pool of AssocInput's batch form, checked by
+// the caller; n_items (< 2^31) = the rows' point counts summed. Writes kf_ptr [B + 1] and kf_xyz (host) only on success;
+// BALM_ERR_INVALID names the lowest problem with a voxel index outside +-2^20.
+struct MergeInput {
+  const char *who;
+  int n_problems;
+  const int64_t *pose_ptr;
+  const int32_t *pose_scan;
+  const int64_t *scan_ptr;
+  int64_t n_points;
+  const float *xyz;
+  const double *poses12;
+  double voxel_size;
+  int64_t n_items;
+};
+int merge_scans_build(cudaStream_t st, const MergeInput &in, int64_t *kf_ptr, float *kf_xyz, long long *launches);
 
 // The sliding-window steps of a batch (balm_batch_marginalize / balm_batch_append_scan). The registration they read:
 // problem p owns the pose rows [pose_ptr[p], pose_ptr[p+1]) and the voxels [voxel_ptr[p], voxel_ptr[p+1]) (host tables

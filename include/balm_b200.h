@@ -246,6 +246,32 @@ int balm_batch_damping_iter(balm_batch *b, double *poses12, const balm_lm_opts *
 int balm_batch_cut_voxels(balm_batch *b, int n_problems, const int64_t *pose_ptr, const int32_t *pose_scan,
                           int n_scans, const int64_t *scan_ptr, const float *xyz, const double *poses12,
                           const balm_assoc_opts *opts, int64_t *n_voxels_out, int64_t *n_obs_out);
+/* Keyframes of a batch, the step between two layers of hierarchical BA: every window's scans merged into one down-sampled
+ * cloud in the body frame of its slot 0, on the device. The problem table and scan pool have the meaning they have in
+ * balm_batch_cut_voxels (scans given once, windows may share scans, pose row j is scan pose_scan[j] in slot
+ * j - pose_ptr[p]); poses12 holds the rows as balm_batch_damping_iter returns them (P x 12, read only).
+ * Keyframe p: every point b of every slot k, expressed in the body frame of the problem's anchor a = slot 0,
+ *   q = R_a^T (R_k b + t_k - t_a),
+ * reduced by down_sampling_voxel (tools.hpp:203-242) at voxel_size: one point per occupied voxel, the mean of its points.
+ * It is kf_xyz[kf_ptr[p] .. kf_ptr[p+1]) (float32 x 3), voxels in ascending (ix, iy, iz). kf_ptr: [B + 1]; the caller
+ * sizes kf_xyz for n_items = sum_j |scan pose_scan[j]| points (it may be NULL when that is 0). voxel_size < 0.001: no
+ * reduction, as in the reference: keyframe p is its transformed points in (slot, point) order.
+ * The arithmetic is fixed so that a numpy restatement reproduces it bit for bit: the transform in fp64, each operation
+ * correctly rounded in the order written, without contraction: ((r0 b0 + r1 b1) + r2 b2) + t, then - t_a, then R_a^T in
+ * the same form, rounded to float32; voxel index = the float32 quotient q / (float)voxel_size, minus 1 if negative,
+ * truncated; mean = the fp64 sum of a voxel's float32 points in item order (slot, then point) over their count, rounded
+ * to float32. The reference keeps a float32 running mean in hash-map order instead; this deterministic mean is the one
+ * balm_b200.drivers.down_sampling_voxel takes. A problem's keyframe does not depend on the rest of the batch or on its
+ * position in it; two calls are bitwise equal. The registration and the window maps are not touched.
+ * Host waits: 3 stream synchronisations (entry, the B + 1 offsets, the keyframes; 2 without reduction); about 20 device
+ * allocations, freed by the call, whatever B. BALM_ERR_INVALID leaves kf_ptr and kf_xyz unwritten: the problem-table
+ * checks of balm_batch_set_voxels, scan_ptr not starting at 0 or not ascending, a pose_scan entry outside [0, n_scans),
+ * a non-finite voxel_size, a voxel index outside +-2^20 (checked on the device; the message names the lowest such
+ * problem). BALM_ERR_UNSUPPORTED, before anything is allocated: 2^31 or more points, counted once per pose row that uses
+ * them (or in xyz). */
+int balm_batch_merge_scans(balm_batch *b, int n_problems, const int64_t *pose_ptr, const int32_t *pose_scan,
+                           int n_scans, const int64_t *scan_ptr, const float *xyz, const double *poses12,
+                           double voxel_size, int64_t *kf_ptr, float *kf_xyz);
 /* Sizes of the current registration, then a copy of it (any pointer may be NULL): voxel_ptr [B + 1], row_ptr [M + 1]
  * (over all voxels), pose_idx [K] (problem-local), obs10 [K x 10], coe [M]; keys / layers [M] as balm_download_keys, per
  * problem in ascending key, only after balm_batch_cut_voxels (non-NULL otherwise -> BALM_ERR_INVALID). Fix clusters

@@ -4,8 +4,9 @@ association chain balm_cut_voxels -> balm_marginalize -> balm_append_scan (octre
 independent problems (balm_batch_*: a dense one with fix clusters, a sparse one of 32 poses, an empty one), and a batch
 association of overlapping windows with one empty window (balm_batch_cut_voxels), the batch pose covariance of
 an anchored, a free and an empty problem (balm_batch_pose_covariance), and the batched marginalise + append of those
-windows, the empty one included (balm_batch_marginalize / balm_batch_append_scan), and the batch's persistent window maps
-(balm_batch_window_*)."""
+windows, the empty one included (balm_batch_marginalize / balm_batch_append_scan), the batch's persistent window maps
+(balm_batch_window_*), and the keyframe merge of overlapping windows with an empty scan and an empty window at voxel
+sizes 0 and 0.2 (balm_batch_merge_scans)."""
 import os, sys
 import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -91,5 +92,12 @@ b.window_marginalize([2, 0], wx, [4, 0])
 b.window_cut(scans, [4, -1], [2, 0], [p12[2:6], wx[1]])
 b.window_recut([3, 0])
 print("batch window push", b.window_push([3, 0]), b.window_push([3, 3]), flush=True)
+b.close()
+# keyframe merge: overlapping windows, an empty scan inside one of them, an all-empty window, voxel_size 0 and 0.2
+b = balm_b200.Batch(0)
+mscans = scans + [np.zeros((0, 3), np.float32)]
+mwin = [[0, 1, 6, 2], [2, 3, 4], [6]]
+mx = [p12[[0, 1, 1, 2]], p12[2:5], p12[:1]]
+print("batch merge", [[len(k) for k in b.merge_scans(mscans, mwin, mx, vs)] for vs in (0.0, 0.2)], flush=True)
 b.close()
 print("SANITIZE_DONE")
