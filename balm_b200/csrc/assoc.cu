@@ -85,6 +85,10 @@ __global__ void iota_kernel(int *v, int64_t n) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) v[i] = (int)i;
 }
+__global__ void win_iota_kernel(int *v, int64_t n, int base) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) v[i] = base + (int)i;
+}
 // batch items: one CTA per pose row j, whose items [item_ptr[j], item_ptr[j+1]) are the points of its scan
 __global__ void expand_rows_kernel(const long long *item_ptr, const long long *src_base, int *src, int *row) {
   const int j = blockIdx.x;
@@ -779,10 +783,11 @@ int launch_csc_batch(balm_ctx *c, int64_t v0, int64_t v1) {
 // The flattened voxel set has no octree any more, so a leaf that is not pushed is dropped together with its fix cluster
 // (in the reference it stays in the map for later scans); documented in DESIGN.md.
 //
-// The per-voxel rules of marginalisation and of appending a scan are device functions shared by a context's kernels
-// (observations SoA [10][Kp], fix SoA [10][M]) and the batch's (balm_batch_marginalize / balm_batch_append_scan,
-// observations and fix AoS [n][10]): both run the same arithmetic in the same order, so a batch problem is bitwise what
-// a context holding it alone computes.
+// Both steps have one implementation, batch_marginalize_build / batch_append_build below, for the B problems of a batch
+// (balm_batch_marginalize / balm_batch_append_scan, observations and fix AoS [n][10]); a context's balm_marginalize /
+// balm_append_scan is its one-problem case (observations SoA [10][Kp], fix SoA [10][M]). The kernels read either layout
+// through a Strided view and run the same arithmetic in the same order, so a batch problem is bitwise what a context
+// holding it alone computes.
 namespace {
 struct Strided {  // column c of row s at p[c * cs + s * rs]; p may be null (a missing fix set reads as zeros)
   const double *p;
@@ -833,95 +838,7 @@ __device__ __forceinline__ double marg_emit(const long long *row_ptr, const int 
   for (int c = 0; c < 10; c++) fix_out[c] = f[c];
   return pts;
 }
-
-__global__ void marg_count_kernel(const long long *row_ptr, const int *pose_idx, const double *obs, int64_t Kp, int64_t M,
-                                  int mg, int min_ps, int *keep, int *cnt) {
-  const int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (v >= M) return;
-  int k = 0;
-  const int kp = marg_keep(row_ptr, pose_idx, Strided{obs, Kp, 1}, v, mg, min_ps, &k);
-  keep[v] = kp;
-  cnt[v] = kp ? k : 0;
-}
-__global__ void marg_emit_kernel(const long long *row_ptr, const int *pose_idx, const double *obs, int64_t Kp,
-                                 const double *fix /*SoA [10][M] or null*/, int64_t M, const double *poses, int mg,
-                                 const int *keep, const int *vscan, const int *oscan, long long *row_ptr_out,
-                                 int *pose_idx_out, double *obs10_out, double *fix10_out, double *coe_out, int64_t Mout,
-                                 int64_t Kout, const unsigned long long *key_in, unsigned long long *key_out,
-                                 const int *layer_in, int *layer_out) {
-  const int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (v == 0) row_ptr_out[Mout] = Kout;
-  if (v >= M || !keep[v]) return;
-  const int nv = vscan[v];
-  if (key_in) { key_out[nv] = key_in[v]; layer_out[nv] = layer_in[v]; }
-  const long long o = oscan[v];
-  row_ptr_out[nv] = o;
-  coe_out[nv] = marg_emit(row_ptr, pose_idx, Strided{obs, Kp, 1}, Strided{fix, M, 1}, v, poses, mg, o, pose_idx_out,
-                          obs10_out, fix10_out + (size_t)nv * 10);
-}
 }  // namespace
-
-// after a re-registration: the compacted keys of the new voxel set (or none)
-static int install_keys(balm_ctx *c, const unsigned long long *keys_dev, const int *layers_dev, int64_t M, bool have) {
-  cudaFree(c->vox_key);
-  cudaFree(c->vox_layer);
-  c->vox_key = nullptr;
-  c->vox_layer = nullptr;
-  c->has_keys = false;
-  if (!have) return BALM_OK;
-  CUDA_TRY(cudaMalloc((void **)&c->vox_key, sizeof(unsigned long long) * (size_t)M));
-  CUDA_TRY(cudaMalloc((void **)&c->vox_layer, sizeof(int) * (size_t)M));
-  CUDA_TRY(cudaMemcpy(c->vox_key, keys_dev, sizeof(unsigned long long) * (size_t)M, cudaMemcpyDeviceToDevice));
-  CUDA_TRY(cudaMemcpy(c->vox_layer, layers_dev, sizeof(int) * (size_t)M, cudaMemcpyDeviceToDevice));
-  c->has_keys = true;
-  return BALM_OK;
-}
-
-int marginalize_build(balm_ctx *c, int mg, const double *poses_dev, int min_ps, int64_t *M_out, int64_t *K_out,
-                      int (*reg)(balm_ctx *, int64_t, const int64_t *, const int32_t *, const double *, const double *,
-                                 const double *, int64_t)) {
-  const int64_t M = c->M;
-  cudaStream_t st = c->stream;
-  ScratchPool pool;
-  int *keep = nullptr, *cnt = nullptr, *vscan = nullptr, *oscan = nullptr;
-  TRY(pool.get(&keep, (size_t)M)); TRY(pool.get(&cnt, (size_t)M)); TRY(pool.get(&vscan, (size_t)M)); TRY(pool.get(&oscan, (size_t)M));
-  const unsigned gb = (unsigned)((M + 127) / 128);
-  marg_count_kernel<<<gb, 128, 0, st>>>(c->row_ptr, c->pose_idx, c->obs, c->Kp, M, mg, min_ps, keep, cnt);
-  size_t tb = 0;
-  cub::DeviceScan::ExclusiveSum(nullptr, tb, keep, vscan, (int)M, st);
-  char *tmp = nullptr;
-  TRY(pool.get(&tmp, tb));
-  CUDA_TRY(cub::DeviceScan::ExclusiveSum(tmp, tb, keep, vscan, (int)M, st));
-  CUDA_TRY(cub::DeviceScan::ExclusiveSum(tmp, tb, cnt, oscan, (int)M, st));
-  int last[4] = {0, 0, 0, 0};
-  CUDA_TRY(cudaMemcpyAsync(&last[0], keep + M - 1, sizeof(int), cudaMemcpyDeviceToHost, st));
-  CUDA_TRY(cudaMemcpyAsync(&last[1], vscan + M - 1, sizeof(int), cudaMemcpyDeviceToHost, st));
-  CUDA_TRY(cudaMemcpyAsync(&last[2], cnt + M - 1, sizeof(int), cudaMemcpyDeviceToHost, st));
-  CUDA_TRY(cudaMemcpyAsync(&last[3], oscan + M - 1, sizeof(int), cudaMemcpyDeviceToHost, st));
-  CUDA_TRY(cudaStreamSynchronize(st));
-  const int64_t Mout = (int64_t)last[0] + last[1], Kout = (int64_t)last[2] + last[3];
-  *M_out = Mout;
-  *K_out = Kout;
-  long long *rp = nullptr;
-  int *pi = nullptr;
-  double *ob = nullptr, *fx = nullptr, *co = nullptr;
-  TRY(pool.get(&rp, (size_t)Mout + 1)); TRY(pool.get(&pi, (size_t)Kout)); TRY(pool.get(&ob, (size_t)Kout * 10));
-  TRY(pool.get(&fx, (size_t)Mout * 10)); TRY(pool.get(&co, (size_t)Mout));
-  unsigned long long *keys_out = nullptr;
-  int *layers_out = nullptr;
-  const bool had_keys = c->has_keys && c->vox_key;
-  if (had_keys) { TRY(pool.get(&keys_out, (size_t)Mout)); TRY(pool.get(&layers_out, (size_t)Mout)); }
-  marg_emit_kernel<<<gb, 128, 0, st>>>(c->row_ptr, c->pose_idx, c->obs, c->Kp, c->fix, M, poses_dev, mg, keep, vscan, oscan, rp,
-                                       pi, ob, fx, co, Mout, Kout, had_keys ? c->vox_key : nullptr, keys_out, c->vox_layer,
-                                       layers_out);
-  CUDA_TRY(cudaStreamSynchronize(st));
-  CUDA_TRY(cudaGetLastError());
-  c->launches += 4;
-  if (Mout < 1) { balm_set_error("balm_marginalize: no voxel is left with two observing scans"); return BALM_ERR_INVALID; }
-  // re-register from the device arrays (copies them, transposes the observations, rebuilds the pose-major lists)
-  TRY(reg(c, Mout, (const int64_t *)rp, pi, ob, fx, co, Kout));
-  return install_keys(c, keys_out, layers_out, Mout, had_keys);
-}
 
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -1022,12 +939,6 @@ __device__ __forceinline__ void append_emit(const long long *row_ptr, const int 
   *coe_out = coe[v] + nb[9];  // push_voxel: coe = sum of N over the window (:42-44)
 }
 
-__global__ void append_match_kernel(const float *xyz, const double *pose12, int64_t n, AssocParams p,
-                                    const unsigned long long *vox_key, const int *vox_layer, int M, unsigned *vid1) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  vid1[i] = (unsigned)(append_match(xyz, i, pose12, p, vox_key, vox_layer, M) + 1);  // 0 = in no registered voxel
-}
 // one thread per voxel: the new scan's body-frame cluster (points in their original order)
 __global__ void append_cluster_kernel(const float *xyz, const unsigned *vid_sorted, const int *idx_sorted, int64_t n, int M,
                                       double *newobs /*[M][10]*/) {
@@ -1035,131 +946,31 @@ __global__ void append_cluster_kernel(const float *xyz, const unsigned *vid_sort
   if (v >= M) return;
   append_cluster(xyz, vid_sorted, idx_sorted, n, (unsigned)(v + 1), newobs + (size_t)v * 10);
 }
-// one thread per voxel: judge_eigen on fix + every window cluster (old ones and the new one) at the current poses
-__global__ void append_judge_kernel(const long long *row_ptr, const int *pose_idx, const double *obs, int64_t Kp,
-                                    const double *fix, int64_t M, const double *poses, const double *newobs, int slot,
-                                    const int *vox_layer, AssocParams p, int *keep, int *cnt, int *bad) {
-  const int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (v >= M) return;
-  int k = 0;
-  bool slot_bad = false;
-  const int kp = append_judge(row_ptr, pose_idx, Strided{obs, Kp, 1}, Strided{fix, M, 1}, v, poses,
-                              newobs + (size_t)v * 10, slot, vox_layer[v], p, &k, &slot_bad);
-  if (slot_bad) atomicOr(bad, 1);
-  keep[v] = kp;
-  cnt[v] = kp ? k : 0;
-}
-__global__ void append_emit_kernel(const long long *row_ptr, const int *pose_idx, const double *obs, int64_t Kp,
-                                   const double *fix, const double *coe, int64_t M, const double *newobs, int slot,
-                                   const int *keep, const int *vscan, const int *oscan, const unsigned long long *key_in,
-                                   const int *layer_in, long long *row_ptr_out, int *pose_idx_out, double *obs10_out,
-                                   double *fix10_out, double *coe_out, unsigned long long *key_out, int *layer_out,
-                                   int64_t Mout, int64_t Kout) {
-  const int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (v == 0) row_ptr_out[Mout] = Kout;
-  if (v >= M || !keep[v]) return;
-  const int nv = vscan[v];
-  const long long o = oscan[v];
-  row_ptr_out[nv] = o;
-  key_out[nv] = key_in[v];
-  layer_out[nv] = layer_in[v];
-  append_emit(row_ptr, pose_idx, Strided{obs, Kp, 1}, Strided{fix, M, 1}, coe, v, newobs + (size_t)v * 10, slot, o,
-              pose_idx_out, obs10_out, fix10_out + (size_t)nv * 10, coe_out + nv);
-}
 }  // namespace
-
-int append_scan_build(balm_ctx *c, int64_t n, const float *xyz_h, const double *poses_dev, int slot, int64_t *M_out,
-                      int64_t *K_out, int64_t *matched_out,
-                      int (*reg)(balm_ctx *, int64_t, const int64_t *, const int32_t *, const double *, const double *,
-                                 const double *, int64_t)) {
-  const int64_t M = c->M;
-  cudaStream_t st = c->stream;
-  ScratchPool pool;
-  AssocParams P{c->assoc_voxel_size, c->assoc_layer_limit, c->assoc_min_ps, {c->assoc_eig[0], c->assoc_eig[1], c->assoc_eig[2]}};
-  float *xyz = nullptr;
-  unsigned *vid = nullptr, *vid2 = nullptr;
-  int *idx = nullptr, *idx2 = nullptr, *keep = nullptr, *cnt = nullptr, *vscan = nullptr, *oscan = nullptr, *bad = nullptr;
-  double *newobs = nullptr;
-  TRY(pool.get(&xyz, (size_t)3 * n)); TRY(pool.get(&vid, (size_t)n)); TRY(pool.get(&vid2, (size_t)n));
-  TRY(pool.get(&idx, (size_t)n)); TRY(pool.get(&idx2, (size_t)n)); TRY(pool.get(&newobs, (size_t)M * 10));
-  TRY(pool.get(&keep, (size_t)M)); TRY(pool.get(&cnt, (size_t)M)); TRY(pool.get(&vscan, (size_t)M)); TRY(pool.get(&oscan, (size_t)M));
-  TRY(pool.get(&bad, 1));
-  CUDA_TRY(cudaMemcpyAsync(xyz, xyz_h, sizeof(float) * 3 * n, cudaMemcpyHostToDevice, st));
-  CUDA_TRY(cudaMemsetAsync(bad, 0, sizeof(int), st));
-  const unsigned gp = (unsigned)((n + 255) / 256), gv = (unsigned)((M + 127) / 128);
-  append_match_kernel<<<gp, 256, 0, st>>>(xyz, poses_dev + 12 * slot, n, P, c->vox_key, c->vox_layer, (int)M, vid);
-  iota_kernel<<<gp, 256, 0, st>>>(idx, n);
-  int bits = 1;
-  while ((1ll << bits) <= M) bits++;
-  size_t tb = 0, tb2 = 0;
-  cub::DeviceRadixSort::SortPairs(nullptr, tb, vid, vid2, idx, idx2, (int)n, 0, bits, st);
-  cub::DeviceScan::ExclusiveSum(nullptr, tb2, keep, vscan, (int)M, st);
-  tb = std::max(tb, tb2);
-  char *tmp = nullptr;
-  TRY(pool.get(&tmp, tb));
-  CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, tb, vid, vid2, idx, idx2, (int)n, 0, bits, st));  // stable: point order kept
-  append_cluster_kernel<<<gv, 128, 0, st>>>(xyz, vid2, idx2, n, (int)M, newobs);
-  append_judge_kernel<<<gv, 128, 0, st>>>(c->row_ptr, c->pose_idx, c->obs, c->Kp, c->fix, M, poses_dev, newobs, slot, c->vox_layer, P,
-                                          keep, cnt, bad);
-  CUDA_TRY(cub::DeviceScan::ExclusiveSum(tmp, tb, keep, vscan, (int)M, st));
-  CUDA_TRY(cub::DeviceScan::ExclusiveSum(tmp, tb, cnt, oscan, (int)M, st));
-  int last[5] = {0, 0, 0, 0, 0};
-  CUDA_TRY(cudaMemcpyAsync(&last[0], keep + M - 1, sizeof(int), cudaMemcpyDeviceToHost, st));
-  CUDA_TRY(cudaMemcpyAsync(&last[1], vscan + M - 1, sizeof(int), cudaMemcpyDeviceToHost, st));
-  CUDA_TRY(cudaMemcpyAsync(&last[2], cnt + M - 1, sizeof(int), cudaMemcpyDeviceToHost, st));
-  CUDA_TRY(cudaMemcpyAsync(&last[3], oscan + M - 1, sizeof(int), cudaMemcpyDeviceToHost, st));
-  CUDA_TRY(cudaMemcpyAsync(&last[4], bad, sizeof(int), cudaMemcpyDeviceToHost, st));
-  CUDA_TRY(cudaStreamSynchronize(st));
-  if (last[4]) { balm_set_error("balm_append_scan: `slot` must be above every scan already observing the voxels"); return BALM_ERR_INVALID; }
-  const int64_t Mout = (int64_t)last[0] + last[1], Kout = (int64_t)last[2] + last[3];
-  if (Mout < 1) { balm_set_error("balm_append_scan: no plane voxel survives the re-judgement"); return BALM_ERR_INVALID; }
-  if (matched_out) {  // points that fell into a registered voxel: n minus the leading zeros of the sorted ids
-    std::vector<unsigned> h((size_t)n);
-    CUDA_TRY(cudaMemcpy(h.data(), vid2, sizeof(unsigned) * (size_t)n, cudaMemcpyDeviceToHost));
-    *matched_out = n - (std::upper_bound(h.begin(), h.end(), 0u) - h.begin());
-  }
-  long long *rp = nullptr;
-  int *pi = nullptr;
-  double *ob = nullptr, *fx = nullptr, *co = nullptr;
-  unsigned long long *keys_out = nullptr;
-  int *layers_out = nullptr;
-  TRY(pool.get(&rp, (size_t)Mout + 1)); TRY(pool.get(&pi, (size_t)Kout)); TRY(pool.get(&ob, (size_t)Kout * 10));
-  TRY(pool.get(&fx, (size_t)Mout * 10)); TRY(pool.get(&co, (size_t)Mout)); TRY(pool.get(&keys_out, (size_t)Mout));
-  TRY(pool.get(&layers_out, (size_t)Mout));
-  append_emit_kernel<<<gv, 128, 0, st>>>(c->row_ptr, c->pose_idx, c->obs, c->Kp, c->fix, c->coe, M, newobs, slot, keep, vscan, oscan,
-                                         c->vox_key, c->vox_layer, rp, pi, ob, fx, co, keys_out, layers_out, Mout, Kout);
-  CUDA_TRY(cudaStreamSynchronize(st));
-  CUDA_TRY(cudaGetLastError());
-  c->launches += 8;
-  *M_out = Mout;
-  *K_out = Kout;
-  const bool any_fix = c->fix != nullptr;
-  TRY(reg(c, Mout, (const int64_t *)rp, pi, ob, any_fix ? fx : nullptr, co, Kout));
-  return install_keys(c, keys_out, layers_out, Mout, true);
-}
 
 
 // ---------------------------------------------------------------------------------------------------------------------
-// The same two steps for every problem of a batch in one call (balm_batch_marginalize / balm_batch_append_scan). One
-// thread per voxel of the whole registration finds its problem through vox_prob and runs the context's rule (the device
-// functions above) on the problem's poses, mg_size or slot; a problem whose argument is 0 (marginalise) or -1 (append)
-// keeps every voxel unchanged. Voxels are grouped by problem, so the global exclusive scans of the keep flags and of the
-// kept observation counts give every problem a contiguous range of the new registration, and batch_window_ptr_kernel
-// reads the per-problem offsets off them. Appending: the (problem, point) items of the new scans are expanded as the cut
-// expands its rows, every point is looked up among its own problem's keys only, and a stable radix sort by global voxel
-// id + 1 keeps the points of one voxel in scan order, so its new cluster sums as the context's does.
+// Both steps for every problem of a batch in one call. One thread per voxel of the whole registration finds its problem
+// through vox_prob (null: one problem) and runs the rule (the device functions above) on the problem's poses, mg_size or
+// slot; a problem whose argument is 0 (marginalise) or -1 (append) keeps every voxel unchanged. Voxels are grouped by
+// problem, so the global exclusive scans of the keep flags and of the kept observation counts give every problem a
+// contiguous range of the new registration, and batch_window_ptr_kernel reads the per-problem offsets off them.
+// Appending: the (problem, point) items of the new scans are expanded as the cut expands its rows, every point is looked
+// up among its own problem's keys only, and a stable radix sort by global voxel id + 1 keeps the points of one voxel in
+// scan order, so its new cluster sums in the order of the scan's points.
 namespace {
-__global__ void batch_marg_count_kernel(const long long *row_ptr, const int *pose_idx, const double *obs,
-                                        const int *vox_prob, int64_t M, const int *mg, int min_ps, int *keep, int *cnt) {
+__device__ __forceinline__ int prob_of(const int *prob, int64_t i) { return prob ? prob[i] : 0; }
+__global__ void batch_marg_count_kernel(const long long *row_ptr, const int *pose_idx, Strided obs, const int *vox_prob,
+                                        int64_t M, const int *mg, int min_ps, int *keep, int *cnt) {
   const int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (v >= M) return;
-  const int m = mg[vox_prob[v]];
+  const int m = mg[prob_of(vox_prob, v)];
   int k = (int)(row_ptr[v + 1] - row_ptr[v]), kp = 1;
-  if (m > 0) kp = marg_keep(row_ptr, pose_idx, Strided{obs, 1, 10}, v, m, min_ps, &k);
+  if (m > 0) kp = marg_keep(row_ptr, pose_idx, obs, v, m, min_ps, &k);
   keep[v] = kp;
   cnt[v] = kp ? k : 0;
 }
-__global__ void batch_marg_emit_kernel(const long long *row_ptr, const int *pose_idx, const double *obs, const double *fix,
+__global__ void batch_marg_emit_kernel(const long long *row_ptr, const int *pose_idx, Strided obs, Strided fix,
                                        const double *coe, const unsigned long long *key, const int *layer,
                                        const int *vox_prob, int64_t M, const int *pose_base, const int *mg,
                                        const double *poses, const int *keep, const int *vscan, const int *oscan,
@@ -1167,12 +978,12 @@ __global__ void batch_marg_emit_kernel(const long long *row_ptr, const int *pose
   const int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (v == 0) out.row_ptr[Mout] = Kout;
   if (v >= M || !keep[v]) return;
-  const int b = vox_prob[v], m = mg[b], nv = vscan[v];
+  const int b = prob_of(vox_prob, v), m = mg[b], nv = vscan[v];
   const long long o = oscan[v];
   out.row_ptr[nv] = o;
   if (key) { out.key[nv] = key[v]; out.layer[nv] = layer[v]; }
-  const double pts = marg_emit(row_ptr, pose_idx, Strided{obs, 1, 10}, Strided{fix, 1, 10}, v, poses + 12 * (size_t)pose_base[b],
-                               m, o, out.pose_idx, out.obs, out.fix + (size_t)nv * 10);
+  const double pts = marg_emit(row_ptr, pose_idx, obs, fix, v, poses + 12 * (size_t)pose_base[b], m, o, out.pose_idx,
+                               out.obs, out.fix + (size_t)nv * 10);
   out.coe[nv] = m > 0 ? pts : coe[v];
 }
 __global__ void batch_append_match_kernel(const float *xyz, const int *src, const int *prob, int64_t n,
@@ -1181,30 +992,30 @@ __global__ void batch_append_match_kernel(const float *xyz, const int *src, cons
                                           const int *layer, unsigned *vid1) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  const int b = prob[i];
+  const int b = prob_of(prob, i);
   const long long v0 = vptr[b];
   const int v = append_match(xyz, src[i], poses + 12 * (size_t)(pose_base[b] + slot[b]), p, key + v0, layer + v0,
                              (int)(vptr[b + 1] - v0));
   vid1[i] = v < 0 ? 0u : (unsigned)(v0 + v + 1);  // 0 = in no voxel of its problem
 }
-__global__ void batch_append_judge_kernel(const long long *row_ptr, const int *pose_idx, const double *obs,
-                                          const double *fix, const int *vox_prob, int64_t M, const int *pose_base,
-                                          const int *slot, const double *poses, const double *newobs, const int *layer,
-                                          AssocParams p, int *keep, int *cnt, int *bad) {
+__global__ void batch_append_judge_kernel(const long long *row_ptr, const int *pose_idx, Strided obs, Strided fix,
+                                          const int *vox_prob, int64_t M, const int *pose_base, const int *slot,
+                                          const double *poses, const double *newobs, const int *layer, AssocParams p,
+                                          int *keep, int *cnt, int *bad) {
   const int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (v >= M) return;
-  const int b = vox_prob[v], s = slot[b];
+  const int b = prob_of(vox_prob, v), s = slot[b];
   int k = (int)(row_ptr[v + 1] - row_ptr[v]), kp = 1;
   if (s >= 0) {
     bool slot_bad = false;
-    kp = append_judge(row_ptr, pose_idx, Strided{obs, 1, 10}, Strided{fix, 1, 10}, v, poses + 12 * (size_t)pose_base[b],
-                      newobs + (size_t)v * 10, s, layer[v], p, &k, &slot_bad);
+    kp = append_judge(row_ptr, pose_idx, obs, fix, v, poses + 12 * (size_t)pose_base[b], newobs + (size_t)v * 10, s,
+                      layer[v], p, &k, &slot_bad);
     if (slot_bad) atomicMin(bad, b);  // the lowest such problem is reported
   }
   keep[v] = kp;
   cnt[v] = kp ? k : 0;
 }
-__global__ void batch_append_emit_kernel(const long long *row_ptr, const int *pose_idx, const double *obs, const double *fix,
+__global__ void batch_append_emit_kernel(const long long *row_ptr, const int *pose_idx, Strided obs, Strided fix,
                                          const double *coe, const unsigned long long *key, const int *layer,
                                          const int *vox_prob, int64_t M, const int *slot, const double *newobs,
                                          const int *keep, const int *vscan, const int *oscan, WindowEmit out,
@@ -1217,8 +1028,8 @@ __global__ void batch_append_emit_kernel(const long long *row_ptr, const int *po
   out.row_ptr[nv] = o;
   out.key[nv] = key[v];
   out.layer[nv] = layer[v];
-  append_emit(row_ptr, pose_idx, Strided{obs, 1, 10}, Strided{fix, 1, 10}, coe, v, newobs + (size_t)v * 10,
-              slot[vox_prob[v]], o, out.pose_idx, out.obs, out.fix ? out.fix + (size_t)nv * 10 : nullptr, out.coe + nv);
+  append_emit(row_ptr, pose_idx, obs, fix, coe, v, newobs + (size_t)v * 10, slot[prob_of(vox_prob, v)], o,
+              out.pose_idx, out.obs, out.fix ? out.fix + (size_t)nv * 10 : nullptr, out.coe + nv);
 }
 // per problem b in [0, B]: its first voxel and first observation in the new registration ([0][B + 1], [1][B + 1]); with
 // vid_sorted, for b < B the points of its new scan that fell into one of its voxels ([2][B])
@@ -1241,16 +1052,23 @@ __global__ void batch_window_ptr_kernel(const long long *vptr, int B, int64_t M,
   out[2 * (B + 1) + b] = lim[1] - lim[0];
 }
 
-// per-problem device table: voxel_ptr [B + 1], then (pose_base, arg) [2][B]; and the poses
+// the poses [12 P], per-problem device table voxel_ptr [B + 1], then (pose_base, arg) [2][B]: one buffer, one copy (a
+// context's call is the case B = 1, where allocations and copies dominate)
 int window_tables(cudaStream_t st, ScratchPool &pool, const BatchVoxels &in, const int *arg, double **poses,
                   long long **vptr, int **pinfo) {
-  const int B = in.B, P = (int)in.pose_ptr[B];
-  std::vector<int> h((size_t)2 * B);
-  for (int b = 0; b < B; b++) { h[b] = (int)in.pose_ptr[b]; h[(size_t)B + b] = arg[b]; }
-  TRY(pool.get(poses, (size_t)12 * P)); TRY(pool.get(vptr, (size_t)B + 1)); TRY(pool.get(pinfo, h.size()));
-  CUDA_TRY(cudaMemcpyAsync(*poses, in.poses12, sizeof(double) * 12 * P, cudaMemcpyHostToDevice, st));
-  CUDA_TRY(cudaMemcpyAsync(*vptr, in.voxel_ptr, sizeof(long long) * (B + 1), cudaMemcpyHostToDevice, st));
-  CUDA_TRY(cudaMemcpyAsync(*pinfo, h.data(), sizeof(int) * h.size(), cudaMemcpyHostToDevice, st));
+  const int B = in.B;
+  const size_t np = (size_t)12 * in.pose_ptr[B], nw = np + (size_t)B + 1;  // 8-byte words before the int table
+  std::vector<long long> h(nw + B);
+  std::copy(in.poses12, in.poses12 + np, reinterpret_cast<double *>(h.data()));
+  std::copy(in.voxel_ptr, in.voxel_ptr + B + 1, h.begin() + np);
+  int *info = reinterpret_cast<int *>(h.data() + nw);
+  for (int b = 0; b < B; b++) { info[b] = (int)in.pose_ptr[b]; info[B + b] = arg[b]; }
+  long long *d = nullptr;
+  TRY(pool.get(&d, h.size()));
+  CUDA_TRY(cudaMemcpyAsync(d, h.data(), sizeof(long long) * h.size(), cudaMemcpyHostToDevice, st));
+  *poses = reinterpret_cast<double *>(d);
+  *vptr = d + np;
+  *pinfo = reinterpret_cast<int *>(d + nw);
   return BALM_OK;
 }
 // with keep / cnt of the in.M voxels: their exclusive scans and the per-problem offsets (+ matched counts) on the host
@@ -1274,9 +1092,10 @@ int window_offsets(cudaStream_t st, ScratchPool &pool, const BatchVoxels &in, co
 }  // namespace
 
 int batch_marginalize_build(cudaStream_t st, const BatchVoxels &in, const int *mg_size, int min_ps,
-                            const WindowRegister &reg) {
+                            const WindowRegister &reg, long long *launches) {
   const int B = in.B;
   const int64_t M = in.M;
+  const Strided obs{in.obs, in.obs_cstride, in.obs_ostride}, fix{in.fix, in.fix_cstride, in.fix_vstride};
   ScratchPool pool;
   double *poses = nullptr;
   long long *vptr = nullptr;
@@ -1285,18 +1104,22 @@ int batch_marginalize_build(cudaStream_t st, const BatchVoxels &in, const int *m
   std::vector<long long> h((size_t)2 * (B + 1), 0);  // new voxel_ptr [B + 1], obs_ptr [B + 1]
   const unsigned gv = (unsigned)((M + 127) / 128);
   if (M > 0) {
-    TRY(pool.get(&keep, (size_t)M)); TRY(pool.get(&cnt, (size_t)M)); TRY(pool.get(&vscan, (size_t)M)); TRY(pool.get(&oscan, (size_t)M));
-    batch_marg_count_kernel<<<gv, 128, 0, st>>>(in.row_ptr, in.pose_idx, in.obs, in.vox_prob, M, pinfo + B, min_ps, keep, cnt);
+    TRY(pool.get(&keep, (size_t)4 * M));
+    cnt = keep + M; vscan = keep + 2 * M; oscan = keep + 3 * M;
+    batch_marg_count_kernel<<<gv, 128, 0, st>>>(in.row_ptr, in.pose_idx, obs, in.vox_prob, M, pinfo + B, min_ps, keep, cnt);
     TRY(window_offsets(st, pool, in, vptr, keep, cnt, vscan, oscan, nullptr, 0, nullptr, h, nullptr));
+    *launches += 4;
   }
   WindowEmit out{};
   TRY(reg(reinterpret_cast<const int64_t *>(h.data()), reinterpret_cast<const int64_t *>(h.data() + B + 1), &out));
-  if (M > 0)
-    batch_marg_emit_kernel<<<gv, 128, 0, st>>>(in.row_ptr, in.pose_idx, in.obs, in.fix, in.coe, in.key, in.layer,
-                                               in.vox_prob, M, pinfo, pinfo + B, poses, keep, vscan, oscan, out, h[B],
+  if (M > 0) {
+    batch_marg_emit_kernel<<<gv, 128, 0, st>>>(in.row_ptr, in.pose_idx, obs, fix, in.coe, in.key, in.layer, in.vox_prob, M,
+                                               pinfo, pinfo + B, poses, keep, vscan, oscan, out, h[B],
                                                h[2 * (size_t)B + 1]);
-  else
+    *launches += 1;
+  } else {
     CUDA_TRY(cudaMemsetAsync(out.row_ptr, 0, sizeof(long long), st));
+  }
   CUDA_TRY(cudaGetLastError());
   CUDA_TRY(cudaStreamSynchronize(st));
   return BALM_OK;
@@ -1304,9 +1127,10 @@ int batch_marginalize_build(cudaStream_t st, const BatchVoxels &in, const int *m
 
 int batch_append_build(cudaStream_t st, const BatchVoxels &in, const balm_assoc_opts &o, const int32_t *scan_of,
                        const int *slot, const int64_t *scan_ptr, const float *xyz, int64_t n_points,
-                       const WindowRegister &reg, int64_t *n_matched) {
+                       const WindowRegister &reg, int64_t *n_matched, bool batch, long long *launches) {
   const int B = in.B;
   const int64_t M = in.M;
+  const Strided obs{in.obs, in.obs_cstride, in.obs_ostride}, fix{in.fix, in.fix_cstride, in.fix_vstride};
   ScratchPool pool;
   AssocParams P{o.voxel_size, o.layer_limit, o.min_ps, {o.eigen_value_array[0], o.eigen_value_array[1], o.eigen_value_array[2]}};
   std::vector<int> arg(B);
@@ -1330,14 +1154,19 @@ int batch_append_build(cudaStream_t st, const BatchVoxels &in, const balm_assoc_
   const unsigned gv = (unsigned)((M + 127) / 128);
   if (M > 0) {
     if (n > 0) {
-      TRY(pool.get(&dxyz, (size_t)3 * n_points)); TRY(pool.get(&dtab, tab.size()));
-      TRY(pool.get(&src, (size_t)n)); TRY(pool.get(&src2, (size_t)n)); TRY(pool.get(&prob, (size_t)n));
+      const unsigned gp = (unsigned)((n + 255) / 256);
+      TRY(pool.get(&dxyz, (size_t)3 * n_points)); TRY(pool.get(&src, (size_t)n)); TRY(pool.get(&src2, (size_t)n));
       TRY(pool.get(&vid, (size_t)n)); TRY(pool.get(&vid2, (size_t)n));
       CUDA_TRY(cudaMemcpyAsync(dxyz, xyz, sizeof(float) * 3 * n_points, cudaMemcpyHostToDevice, st));
-      CUDA_TRY(cudaMemcpyAsync(dtab, tab.data(), sizeof(long long) * tab.size(), cudaMemcpyHostToDevice, st));
-      expand_rows_kernel<<<B, 256, 0, st>>>(dtab, dtab + B + 1, src, prob);
-      batch_append_match_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(dxyz, src, prob, n, poses, vptr, pinfo,
-                                                                             pinfo + B, P, in.key, in.layer, vid);
+      if (B == 1) {  // one problem: its scan's points in order over a full grid (prob stays null: problem 0)
+        win_iota_kernel<<<gp, 256, 0, st>>>(src, n, (int)tab[2]);
+      } else {
+        TRY(pool.get(&dtab, tab.size())); TRY(pool.get(&prob, (size_t)n));
+        CUDA_TRY(cudaMemcpyAsync(dtab, tab.data(), sizeof(long long) * tab.size(), cudaMemcpyHostToDevice, st));
+        expand_rows_kernel<<<B, 256, 0, st>>>(dtab, dtab + B + 1, src, prob);
+      }
+      batch_append_match_kernel<<<gp, 256, 0, st>>>(dxyz, src, prob, n, poses, vptr, pinfo, pinfo + B, P, in.key,
+                                                    in.layer, vid);
       int bits = 1;
       while ((1ll << bits) <= M) bits++;
       size_t tb = 0;
@@ -1345,29 +1174,37 @@ int batch_append_build(cudaStream_t st, const BatchVoxels &in, const balm_assoc_
       char *tmp = nullptr;
       TRY(pool.get(&tmp, tb));
       CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, tb, vid, vid2, src, src2, (int)n, 0, bits, st));  // stable
+      *launches += 3;
     }
     TRY(pool.get(&newobs, (size_t)M * 10));
-    TRY(pool.get(&keep, (size_t)M)); TRY(pool.get(&cnt, (size_t)M)); TRY(pool.get(&vscan, (size_t)M)); TRY(pool.get(&oscan, (size_t)M));
+    TRY(pool.get(&keep, (size_t)4 * M));
+    cnt = keep + M; vscan = keep + 2 * M; oscan = keep + 3 * M;
     TRY(pool.get(&bad, 1));
     CUDA_TRY(cudaMemsetAsync(bad, 0x7f, sizeof(int), st));
     append_cluster_kernel<<<gv, 128, 0, st>>>(dxyz, vid2, src2, n, (int)M, newobs);
-    batch_append_judge_kernel<<<gv, 128, 0, st>>>(in.row_ptr, in.pose_idx, in.obs, in.fix, in.vox_prob, M, pinfo,
-                                                  pinfo + B, poses, newobs, in.layer, P, keep, cnt, bad);
+    batch_append_judge_kernel<<<gv, 128, 0, st>>>(in.row_ptr, in.pose_idx, obs, fix, in.vox_prob, M, pinfo, pinfo + B,
+                                                  poses, newobs, in.layer, P, keep, cnt, bad);
     TRY(window_offsets(st, pool, in, vptr, keep, cnt, vscan, oscan, vid2, n, bad, h, &h_bad));
+    *launches += 5;
   }
   if (h_bad != 0x7f7f7f7f) {
-    balm_set_error("balm_batch_append_scan: problem " + std::to_string(h_bad) +
-                   ": `slot` must be above every scan already observing its voxels");
+    if (batch)
+      balm_set_error("balm_batch_append_scan: problem " + std::to_string(h_bad) +
+                     ": `slot` must be above every scan already observing its voxels");
+    else
+      balm_set_error("balm_append_scan: `slot` must be above every scan already observing the voxels");
     return BALM_ERR_INVALID;
   }
   WindowEmit out{};
   TRY(reg(reinterpret_cast<const int64_t *>(h.data()), reinterpret_cast<const int64_t *>(h.data() + B + 1), &out));
-  if (M > 0)
-    batch_append_emit_kernel<<<gv, 128, 0, st>>>(in.row_ptr, in.pose_idx, in.obs, in.fix, in.coe, in.key, in.layer,
-                                                 in.vox_prob, M, pinfo + B, newobs, keep, vscan, oscan, out, h[B],
+  if (M > 0) {
+    batch_append_emit_kernel<<<gv, 128, 0, st>>>(in.row_ptr, in.pose_idx, obs, fix, in.coe, in.key, in.layer, in.vox_prob,
+                                                 M, pinfo + B, newobs, keep, vscan, oscan, out, h[B],
                                                  h[2 * (size_t)B + 1]);
-  else
+    *launches += 1;
+  } else {
     CUDA_TRY(cudaMemsetAsync(out.row_ptr, 0, sizeof(long long), st));
+  }
   CUDA_TRY(cudaGetLastError());
   CUDA_TRY(cudaStreamSynchronize(st));
   // a problem left without voxels (where the context call fails) matched nothing that stays registered
@@ -1519,10 +1356,6 @@ __device__ __forceinline__ int look_find(const unsigned long long *key, const in
   return i < 0 ? -1 : a + i;
 }
 
-__global__ void win_iota_kernel(int *v, int64_t n, int base) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) v[i] = base + (int)i;
-}
 __global__ void win_missing_kernel(const unsigned long long *keys, const int *probs, int m, const unsigned long long *look,
                                    const int *off, int *miss) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -2227,28 +2060,4 @@ int window_push_build(cudaStream_t st, WindowState &w, const int *win_count, con
   CUDA_TRY(cudaGetLastError());
   *launches += 8;
   return BALM_OK;
-}
-
-// balm_window_push: the one-problem push into pool buffers, then registered as the context's voxel set with its keys
-int window_push_ctx(balm_ctx *c, WindowState &w, int win_count, int64_t *M_out, int64_t *K_out,
-                    int (*reg)(balm_ctx *, int64_t, const int64_t *, const int32_t *, const double *, const double *,
-                               const double *, int64_t)) {
-  ScratchPool pool;
-  int64_t M = 0, K = 0;
-  WindowEmit dst{};
-  const WindowRegister to_pool = [&](const int64_t *vp, const int64_t *op, WindowEmit *out) {
-    M = vp[1];
-    K = op[1];
-    TRY(pool.get(&dst.row_ptr, (size_t)M + 1)); TRY(pool.get(&dst.pose_idx, (size_t)K));
-    TRY(pool.get(&dst.obs, (size_t)K * 10)); TRY(pool.get(&dst.fix, (size_t)M * 10)); TRY(pool.get(&dst.coe, (size_t)M));
-    TRY(pool.get(&dst.key, (size_t)M)); TRY(pool.get(&dst.layer, (size_t)M));
-    *out = dst;
-    return (int)BALM_OK;
-  };
-  TRY(window_push_build(c->stream, w, &win_count, to_pool, &c->launches));
-  *M_out = M;
-  *K_out = K;
-  if (M == 0) return BALM_OK;
-  TRY(reg(c, M, (const int64_t *)dst.row_ptr, dst.pose_idx, dst.obs, dst.fix, dst.coe, K));
-  return install_keys(c, dst.key, dst.layer, M, true);
 }

@@ -430,8 +430,7 @@ extern "C" int balm_cut_voxels(balm_ctx *c, int64_t n_points, const float *xyz, 
   };
   TRY(assoc_cut(c->stream, in, o, reg, &c->launches));
   c->has_keys = true;
-  c->assoc_voxel_size = o.voxel_size; c->assoc_layer_limit = o.layer_limit; c->assoc_min_ps = o.min_ps;
-  for (int q = 0; q < 3; q++) c->assoc_eig[q] = o.eigen_value_array[q];
+  c->assoc = o;
   if (n_voxels_out) *n_voxels_out = c->M;
   if (n_obs_out) *n_obs_out = c->K;
   return finish_registration(c);
@@ -828,26 +827,71 @@ extern "C" int balm_damping_iter(balm_ctx *c, double *poses12, const balm_lm_opt
   return BALM_OK;
 }
 
-// ---------------- sliding-window marginalisation (assoc.cu) ----------------
-int marginalize_build(balm_ctx *c, int mg, const double *poses_dev, int min_ps, int64_t *M_out, int64_t *K_out,
-                      int (*reg)(balm_ctx *, int64_t, const int64_t *, const int32_t *, const double *, const double *,
-                                 const double *, int64_t));
+// ---------------- sliding window on the registered voxel set (assoc.cu) ----------------
+// A sliding-window build of the batch (batch_marginalize_build, batch_append_build, window_push_build) run as its
+// one-problem case into scratch buffers, then registered as the context's voxel set, with fix clusters when `fix` and
+// octree keys when `keys`. An empty result is registered as an empty set when `empty` is null; otherwise the call is
+// rejected with that message before anything is emitted, and the context keeps its registration.
+static int ctx_window_step(balm_ctx *c, bool fix, bool keys, const char *empty,
+                           const std::function<int(const WindowRegister &)> &build, int64_t *M_out, int64_t *K_out) {
+  ScratchPool pool;
+  int64_t M = 0, K = 0;
+  WindowEmit dst{};
+  const WindowRegister to_pool = [&](const int64_t *vp, const int64_t *op, WindowEmit *out) {
+    M = vp[1];
+    K = op[1];
+    if (M == 0 && empty) { balm_set_error(empty); return (int)BALM_ERR_INVALID; }
+    TRY(pool.get(&dst.row_ptr, (size_t)M + 1)); TRY(pool.get(&dst.pose_idx, (size_t)K));
+    TRY(pool.get(&dst.obs, (size_t)K * 10)); TRY(pool.get(&dst.coe, (size_t)M));
+    if (fix) TRY(pool.get(&dst.fix, (size_t)M * 10));
+    if (keys) { TRY(pool.get(&dst.key, (size_t)M)); TRY(pool.get(&dst.layer, (size_t)M)); }
+    *out = dst;
+    return (int)BALM_OK;
+  };
+  TRY(build(to_pool));
+  if (M == 0) {
+    drop_keys(c);
+    TRY(register_empty(c));
+  } else {
+    TRY(balm_set_voxels_dev(c, M, (const int64_t *)dst.row_ptr, dst.pose_idx, dst.obs, dst.fix, dst.coe, K));
+    if (keys) {  // balm_set_voxels_dev dropped the previous ones
+      TRY(dev_alloc(&c->vox_key, (size_t)M));
+      TRY(dev_alloc(&c->vox_layer, (size_t)M));
+      CUDA_TRY(cudaMemcpy(c->vox_key, dst.key, sizeof(unsigned long long) * M, cudaMemcpyDeviceToDevice));
+      CUDA_TRY(cudaMemcpy(c->vox_layer, dst.layer, sizeof(int) * M, cudaMemcpyDeviceToDevice));
+      c->has_keys = true;
+    }
+  }
+  if (M_out) *M_out = M;
+  if (K_out) *K_out = K;
+  return BALM_OK;
+}
+
+// The context's registration as the sliding-window builds read it: one problem, observations SoA [10][Kp], fix SoA
+// [10][M]. pose_ptr / voxel_ptr [2] receive the host tables it points into.
+static BatchVoxels ctx_voxels(const balm_ctx *c, const double *poses12, int64_t *pose_ptr, int64_t *voxel_ptr) {
+  pose_ptr[0] = voxel_ptr[0] = 0;
+  pose_ptr[1] = c->N;
+  voxel_ptr[1] = c->M;
+  const bool keys = c->has_keys;
+  return BatchVoxels{1, c->M, pose_ptr, voxel_ptr, nullptr, c->row_ptr, c->pose_idx, c->obs, c->Kp, 1, c->fix, c->M, 1,
+                     c->coe, keys ? c->vox_key : nullptr, keys ? c->vox_layer : nullptr, poses12};
+}
+
 extern "C" int balm_marginalize(balm_ctx *c, int mg_size, const double *poses12, int min_ps, int64_t *n_voxels_out,
                                 int64_t *n_obs_out) {
   if (!c || !poses12 || mg_size < 1 || mg_size >= c->N) { balm_set_error("balm_marginalize: bad arguments"); return BALM_ERR_INVALID; }
   if (!c->registered || c->M < 1) { balm_set_error("balm_marginalize: no voxels registered"); return BALM_ERR_INVALID; }
   CUDA_TRY(cudaSetDevice(c->device));
   CUDA_TRY(cudaMemcpyAsync(c->poses, poses12, sizeof(double) * 12 * c->N, cudaMemcpyHostToDevice, c->stream));
-  int64_t M = 0, K = 0;
-  TRY(marginalize_build(c, mg_size, c->poses, min_ps, &M, &K, balm_set_voxels_dev));
-  if (n_voxels_out) *n_voxels_out = M;
-  if (n_obs_out) *n_obs_out = K;
-  return BALM_OK;
+  int64_t pose_ptr[2], voxel_ptr[2];
+  const BatchVoxels in = ctx_voxels(c, poses12, pose_ptr, voxel_ptr);
+  return ctx_window_step(c, true, c->has_keys, "balm_marginalize: no voxel is left with two observing scans",
+                         [&](const WindowRegister &reg) {
+                           return batch_marginalize_build(c->stream, in, &mg_size, min_ps, reg, &c->launches);
+                         },
+                         n_voxels_out, n_obs_out);
 }
-int append_scan_build(balm_ctx *c, int64_t n, const float *xyz_h, const double *poses_dev, int slot, int64_t *M_out,
-                      int64_t *K_out, int64_t *matched_out,
-                      int (*reg)(balm_ctx *, int64_t, const int64_t *, const int32_t *, const double *, const double *,
-                                 const double *, int64_t));
 extern "C" int balm_append_scan(balm_ctx *c, int64_t n_points, const float *xyz, const double *poses12, int slot,
                                 int64_t *n_voxels_out, int64_t *n_obs_out, int64_t *n_matched_out) {
   if (!c || !xyz || !poses12 || n_points < 1 || n_points >= (1ll << 31) || slot < 0 || slot >= c->N) {
@@ -860,10 +904,17 @@ extern "C" int balm_append_scan(balm_ctx *c, int64_t n_points, const float *xyz,
   }
   CUDA_TRY(cudaSetDevice(c->device));
   CUDA_TRY(cudaMemcpyAsync(c->poses, poses12, sizeof(double) * 12 * c->N, cudaMemcpyHostToDevice, c->stream));
-  int64_t M = 0, K = 0;
-  TRY(append_scan_build(c, n_points, xyz, c->poses, slot, &M, &K, n_matched_out, balm_set_voxels_dev));
-  if (n_voxels_out) *n_voxels_out = M;
-  if (n_obs_out) *n_obs_out = K;
+  int64_t pose_ptr[2], voxel_ptr[2], matched = 0;
+  const BatchVoxels in = ctx_voxels(c, poses12, pose_ptr, voxel_ptr);
+  const int32_t scan = 0;
+  const int64_t scan_ptr[2] = {0, n_points};
+  TRY(ctx_window_step(c, c->fix != nullptr, true, "balm_append_scan: no plane voxel survives the re-judgement",
+                      [&](const WindowRegister &reg) {
+                        return batch_append_build(c->stream, in, c->assoc, &scan, &slot, scan_ptr, xyz, n_points, reg,
+                                                  &matched, false, &c->launches);
+                      },
+                      n_voxels_out, n_obs_out));
+  if (n_matched_out) *n_matched_out = matched;
   return BALM_OK;
 }
 extern "C" int balm_download_keys(balm_ctx *c, uint64_t *keys, int32_t *layers) {
@@ -885,9 +936,6 @@ extern "C" int balm_download_fix(balm_ctx *c, double *fix10) {
 
 // ---------------- persistent sliding-window octree (assoc.cu) ----------------
 // the one-problem case of the batch's window (window_*_build, internal.cuh)
-int window_push_ctx(balm_ctx *c, WindowState &w, int win_count, int64_t *M_out, int64_t *K_out,
-                    int (*reg)(balm_ctx *, int64_t, const int64_t *, const int32_t *, const double *, const double *,
-                               const double *, int64_t));
 static int window_check(balm_ctx *c, const char *fn, int win_count) {
   if (!c) { balm_set_error(std::string(fn) + ": bad arguments"); return BALM_ERR_INVALID; }
   if (!c->win) { balm_set_error(std::string(fn) + ": call balm_window_reset first"); return BALM_ERR_INVALID; }
@@ -935,15 +983,11 @@ extern "C" int balm_window_marginalize(balm_ctx *c, int mg_size, const double *p
 extern "C" int balm_window_push(balm_ctx *c, int win_count, int64_t *n_voxels_out, int64_t *n_obs_out) {
   TRY(window_check(c, "balm_window_push", win_count));
   CUDA_TRY(cudaSetDevice(c->device));
-  int64_t M = 0, K = 0;
-  TRY(window_push_ctx(c, *c->win, win_count, &M, &K, balm_set_voxels_dev));
-  if (M == 0) {  // nothing pushed: an empty voxel set
-    drop_keys(c);
-    TRY(register_empty(c));
-  }
-  if (n_voxels_out) *n_voxels_out = M;
-  if (n_obs_out) *n_obs_out = K;
-  return BALM_OK;
+  return ctx_window_step(c, true, true, nullptr,
+                         [&](const WindowRegister &reg) {
+                           return window_push_build(c->stream, *c->win, &win_count, reg, &c->launches);
+                         },
+                         n_voxels_out, n_obs_out);
 }
 
 // ---------------- pose covariance (covariance.cu) ----------------

@@ -1071,8 +1071,8 @@ static BatchVoxels window_input(const BatchReg *r, const double *poses12, std::v
   }
   pose_ptr[r->B] = r->P;
   voxel_ptr[r->B] = r->M;
-  return BatchVoxels{r->B, r->M, r->K, pose_ptr.data(), voxel_ptr.data(), r->vox_prob, r->row_ptr, r->pose_idx,
-                     r->obs, r->fix, r->coe, r->key, r->layer, poses12};
+  return BatchVoxels{r->B, r->M, pose_ptr.data(), voxel_ptr.data(), r->vox_prob, r->row_ptr, r->pose_idx, r->obs, 1, 10,
+                     r->fix, 1, 10, r->coe, r->key, r->layer, poses12};
 }
 
 // The new registration r of old's problems with the sizes the step found: layout, then the arrays it emits into (fix
@@ -1112,7 +1112,8 @@ extern "C" int balm_batch_marginalize(balm_batch *bt, const int *mg_size, const 
     obs_ptr.assign(op, op + old->B + 1);
     return window_register(bt, old, r, pose_ptr.data(), vp, op, true, out);
   };
-  int rc = batch_marginalize_build(bt->stream, in, mg_size, min_ps, reg);
+  long long launches = 0;
+  int rc = batch_marginalize_build(bt->stream, in, mg_size, min_ps, reg, &launches);
   if (rc == BALM_OK) rc = reg_finish(bt, r);
   if (rc == BALM_OK)
     for (int b = 0; b < old->B; b++) {
@@ -1158,7 +1159,9 @@ extern "C" int balm_batch_append_scan(balm_batch *bt, const int32_t *scan_of, co
     obs_ptr.assign(op, op + old->B + 1);
     return window_register(bt, old, r, pose_ptr.data(), vp, op, old->fix != nullptr, out);
   };
-  int rc = batch_append_build(bt->stream, in, old->assoc, scan_of, slot, scan_ptr, xyz, n_points, reg, matched.data());
+  long long launches = 0;
+  int rc = batch_append_build(bt->stream, in, old->assoc, scan_of, slot, scan_ptr, xyz, n_points, reg, matched.data(),
+                              true, &launches);
   if (rc == BALM_OK) rc = reg_finish(bt, r);
   if (rc == BALM_OK)
     for (int b = 0; b < old->B; b++) {

@@ -103,9 +103,7 @@ struct balm_ctx {
   int *vox_layer = nullptr;       // [M] octree layer of every voxel (a key digit 7 is BOTH octant 7 and "not split":
                                   // the layer says which)
   bool has_keys = false;
-  double assoc_voxel_size = 1.0;  // association parameters of that call
-  int assoc_layer_limit = 2, assoc_min_ps = 15;
-  double assoc_eig[3] = {1.0 / 16, 1.0 / 16, 1.0 / 16};
+  balm_assoc_opts assoc{1.0, 2, 15, {1.0 / 16, 1.0 / 16, 1.0 / 16}};  // association options of that call
   WindowState *win = nullptr;     // balm_window_* state (independent of the registered voxel set)
 
   // ---- optimiser state (device) ----
@@ -748,18 +746,24 @@ struct MergeInput {
 };
 int merge_scans_build(cudaStream_t st, const MergeInput &in, int64_t *kf_ptr, float *kf_xyz, long long *launches);
 
-// The sliding-window steps of a batch (balm_batch_marginalize / balm_batch_append_scan). The registration they read:
-// problem p owns the pose rows [pose_ptr[p], pose_ptr[p+1]) and the voxels [voxel_ptr[p], voxel_ptr[p+1]) (host tables
-// [B + 1]); device arrays vox_prob [M], row_ptr [M + 1], pose_idx [K] (problem-local), obs [K][10], fix [M][10] or null,
-// coe [M], key / layer [M] (null: not carried; appending needs them). poses12: the host's P x 12 poses.
+// The sliding-window steps of a batch (balm_batch_marginalize / balm_batch_append_scan) and of a context, its one-problem
+// case (balm_marginalize / balm_append_scan). The registration they read: problem p owns the pose rows [pose_ptr[p],
+// pose_ptr[p+1]) and the voxels [voxel_ptr[p], voxel_ptr[p+1]) (host tables [B + 1]); device arrays vox_prob [M] (null:
+// every voxel is problem 0, B = 1), row_ptr [M + 1], pose_idx [K] (problem-local), obs: column c of observation o at
+// obs[c * obs_cstride + o * obs_ostride] (AoS [K][10] of a batch, SoA [10][Kp] of a context), fix likewise per voxel or
+// null, coe [M], key / layer [M] (null: not carried; appending needs them). poses12: the host's P x 12 poses.
 struct BatchVoxels {
   int B;
-  int64_t M, K;
+  int64_t M;
   const int64_t *pose_ptr, *voxel_ptr;
   const int *vox_prob;
   const long long *row_ptr;
   const int *pose_idx;
-  const double *obs, *fix, *coe;
+  const double *obs;
+  int64_t obs_cstride, obs_ostride;
+  const double *fix;
+  int64_t fix_cstride, fix_vstride;
+  const double *coe;
   const unsigned long long *key;
   const int *layer;
   const double *poses12;
@@ -779,13 +783,14 @@ struct WindowEmit {
 using WindowRegister = std::function<int(const int64_t *voxel_ptr, const int64_t *obs_ptr, WindowEmit *out)>;
 // mg_size [B]: 0 (problem copied unchanged) or in [1, N_p) (checked by the caller)
 int batch_marginalize_build(cudaStream_t st, const BatchVoxels &in, const int *mg_size, int min_ps,
-                            const WindowRegister &reg);
+                            const WindowRegister &reg, long long *launches);
 // scan_of [B] (-1: problem copied unchanged) and slot [B] checked by the caller; scan s = xyz[scan_ptr[s] ..
-// scan_ptr[s+1]) of n_points; n_matched [B]. BALM_ERR_INVALID names the lowest problem whose slot is not above every
-// scan already observing one of its voxels.
+// scan_ptr[s+1]) of n_points; n_matched [B]. BALM_ERR_INVALID, before reg is called, when a slot is not above every scan
+// already observing one of its problem's voxels: batch, the message of balm_batch_append_scan naming the lowest such
+// problem, else that of balm_append_scan.
 int batch_append_build(cudaStream_t st, const BatchVoxels &in, const balm_assoc_opts &o, const int32_t *scan_of,
                        const int *slot, const int64_t *scan_ptr, const float *xyz, int64_t n_points,
-                       const WindowRegister &reg, int64_t *n_matched);
+                       const WindowRegister &reg, int64_t *n_matched, bool batch, long long *launches);
 
 // The persistent sliding-window octree of B problems (balm_window_* with B = 1, balm_batch_window_*). Problem p has
 // n_slots[p] slots and owns the pose rows [sum_{q<p} n_slots[q], ...) of every poses12 (host, P x 12). Arguments are
