@@ -54,7 +54,8 @@ SYMBOLS = ["balm_last_error", "balm_version", "balm_create", "balm_destroy", "ba
            "balm_batch_damping_iter", "balm_batch_cut_voxels", "balm_batch_sizes", "balm_batch_download_voxels",
            "balm_batch_pose_covariance", "balm_batch_marginalize", "balm_batch_append_scan", "balm_batch_download_fix",
            "balm_batch_window_reset", "balm_batch_window_cut", "balm_batch_window_recut", "balm_batch_window_marginalize",
-           "balm_batch_window_push", "balm_batch_merge_scans"]
+           "balm_batch_window_push", "balm_batch_merge_scans", "balm_set_pose_factors", "balm_pose_graph_evaluate",
+           "balm_pose_graph_iter"]
 
 
 def lib():
@@ -131,6 +132,10 @@ def lib():
         L.balm_batch_window_recut.argtypes = [C.c_void_p, C.c_void_p]
         L.balm_batch_window_marginalize.argtypes = [C.c_void_p] + [C.c_void_p] * 3
         L.balm_batch_window_push.argtypes = [C.c_void_p] + [C.c_void_p] * 3
+        L.balm_set_pose_factors.argtypes = [C.c_void_p, C.c_int] + [C.c_void_p] * 5
+        L.balm_pose_graph_evaluate.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_double)]
+        L.balm_pose_graph_iter.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(LmOpts), C.c_void_p, C.POINTER(C.c_int),
+                                           C.c_void_p]
         _lib = L
     return _lib
 

@@ -190,6 +190,53 @@ class Context:
                                              _p(cov)))
         return raw, cov
 
+    # ---- pose graph ----
+    def set_pose_factors(self, factors):
+        """Window factors (include/balm_b200.h, balm_set_pose_factors): list of dict(poses = N_f distinct global pose
+        indices, poses_hat = N_f x 12 refined window poses, H = (6 N_f)^2 window BA Hessian). Replaces the previous factor
+        set; a rejected call keeps it. -> per factor OK or ERR_NOT_PD (left out of the cost)."""
+        idx = [np.asarray(f["poses"], dtype=np.int64).ravel() for f in factors]
+        hat, Hs = [], []
+        for f, i in zip(factors, idx):
+            n = 6 * len(i)
+            hat.append(np.asarray(f["poses_hat"], dtype=np.float64).reshape(len(i), 12))
+            H = np.asarray(f["H"], dtype=np.float64)
+            if H.shape != (n, n):
+                raise ValueError(f"set_pose_factors: H of a {len(i)}-pose factor must be {n} x {n}, got {H.shape}")
+            Hs.append(H.ravel(order="F"))
+        ptr = np.concatenate([[0], np.cumsum([len(i) for i in idx])]).astype(np.int64)
+        pose = np.ascontiguousarray(np.concatenate(idx) if idx else np.zeros(0), dtype=np.int32)
+        hat = np.ascontiguousarray(np.concatenate(hat) if hat else np.zeros((0, 12)), dtype=np.float64)
+        Hc = np.ascontiguousarray(np.concatenate(Hs) if Hs else np.zeros(0), dtype=np.float64)
+        status = np.zeros(len(factors), dtype=np.int32)
+        L.check(L.lib().balm_set_pose_factors(self._h, len(factors), _p(ptr), _p(pose), _p(hat), _p(Hc), _p(status)))
+        return [int(s) for s in status]
+
+    def pose_graph_evaluate(self, poses12, want_H=True):
+        """-> (H, g, cost) of the registered factors at poses12 (H dense n x n, None with want_H=False)."""
+        poses12 = np.ascontiguousarray(poses12, dtype=np.float64)
+        H = np.zeros((self.n, self.n), order="F") if want_H else None
+        g = np.zeros(self.n)
+        r = C.c_double()
+        L.check(L.lib().balm_pose_graph_evaluate(self._h, _p(poses12), _p(H), _p(g), C.byref(r)))
+        return H, g, r.value
+
+    def pose_graph_iter(self, poses12, max_iter=10, u0=0.01, v0=2.0, rel_tol=1e-6, gauge_mode=0, verbose=False,
+                        want_per_iter=False, force_hess=False):
+        """damping_iter's LM on the pose-graph cost -> (poses, trace); with want_per_iter every trace record also holds
+        the accepted poses after its iteration under "poses"."""
+        poses = np.array(poses12, dtype=np.float64, order="C", copy=True)
+        opts = L.LmOpts(max_iter, u0, v0, rel_tol, 0, gauge_mode, 0, int(verbose), int(force_hess))
+        trace = (L.Trace * max(1, max_iter))()
+        n_it = C.c_int()
+        per_iter = np.zeros((max_iter, self.N, 12)) if want_per_iter else None
+        L.check(L.lib().balm_pose_graph_iter(self._h, _p(poses), C.byref(opts), trace, C.byref(n_it), _p(per_iter)))
+        tr = _trace_dicts(trace[:n_it.value])
+        if want_per_iter:
+            for t, p in zip(tr, per_iter):
+                t["poses"] = p
+        return poses, tr
+
     # ---- multi-GPU ----
     @staticmethod
     def comm_unique_id():

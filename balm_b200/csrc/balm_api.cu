@@ -176,6 +176,7 @@ extern "C" int balm_create(balm_ctx **out, int n_poses, int device, int precisio
   TRY(syrk_f64_setup());
   TRY(ldlt_setup());
   TRY(covariance_setup());
+  TRY(pose_graph_setup());
   const size_t n = c->n;
   TRY(dev_alloc(&c->poses, 12 * (size_t)c->N));
   TRY(dev_alloc(&c->poses_trial, 12 * (size_t)c->N));
@@ -207,6 +208,7 @@ extern "C" int balm_destroy(balm_ctx *c) {
   cudaStreamSynchronize(c->stream);
   free_problem(c);
   window_free(c->win);
+  pose_graph_free(c->pg);
   if (c->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(c->comm);
   cudaFree(c->poses); cudaFree(c->poses_trial); cudaFree(c->H); cudaFree(c->A);
   cudaFree(c->dx); cudaFree(c->dvec); cudaFree(c->scal); cudaFree(c->flags); cudaFree(c->accum); cudaFree(c->accum_batch);
@@ -722,6 +724,30 @@ extern "C" void balm_default_lm_opts(balm_lm_opts *o) {
   o->min_planes_per_pose = 20; o->verbose = 0; o->force_hess = 0;
 }
 
+// The accept rule of BALM2::damping_iter (bavoxel.hpp:1127-1149), shared by balm_damping_iter and balm_pose_graph_iter:
+// q = r1 - r2 (-1 for an unusable step, which is then rejected), the reference's trace line, and u, v updated: on
+// acceptance (q > 0) u *= max(1/3, 1 - (2 rho - 1)^3) with rho = q / q1 and v = 2, else u *= v and v *= 2.
+// *t receives the iteration's trace record; returns whether the step is accepted.
+static bool lm_rule(const balm_lm_opts *o, int it, double r1, double r2, double q1, int not_pd, bool calc_hess, double *u,
+                    double *v, balm_trace *t) {
+  double q = r1 - r2;
+  if (not_pd || !std::isfinite(r2)) q = -1.0;
+  if (o->verbose)  // the reference's trace line (bavoxel.hpp:1132)
+    printf("iter%d: (%lf %lf) u: %lf v: %.1lf q: %.3lf %lf %lf\n", it, r1, r2, *u, *v, q / q1, q1, q);
+  *t = balm_trace{r1, r2, *u, *v, q, q1, 0, calc_hess ? 1 : 0, not_pd};
+  if (q > 0) {  // bavoxel.hpp:1134-1143
+    const double rho = q / q1;
+    *v = 2;
+    const double f = 1 - pow(2 * rho - 1, 3);
+    *u *= (f < (1.0 / 3.0) ? (1.0 / 3.0) : f);
+    t->accepted = 1;
+    return true;
+  }
+  *u = *u * *v;  // bavoxel.hpp:1144-1149
+  *v = 2 * *v;
+  return false;
+}
+
 extern "C" int balm_damping_iter(balm_ctx *c, double *poses12, const balm_lm_opts *o, balm_trace *trace, int *n_iters,
                                  double *poses_per_iter) {
   if (!c || !poses12 || !o) { balm_set_error("balm_damping_iter: bad arguments"); return BALM_ERR_INVALID; }
@@ -791,27 +817,16 @@ extern "C" int balm_damping_iter(balm_ctx *c, double *poses12, const balm_lm_opt
       }
     }
     if (calc_hess) r1 = c->h_scal[0];
-    double q = r1 - r2;
-    if (not_pd || !std::isfinite(r2)) q = -1.0;  // unusable step -> rejected, u *= v
-    if (o->verbose)  // the reference's trace line (bavoxel.hpp:1132)
-      printf("iter%d: (%lf %lf) u: %lf v: %.1lf q: %.3lf %lf %lf\n", it, r1, r2, u, v, q / q1, q1, q);
-    balm_trace t{r1, r2, u, v, q, q1, 0, calc_hess ? 1 : 0, not_pd};
-    if (q > 0) {  // bavoxel.hpp:1134-1143
+    balm_trace t;
+    if (lm_rule(o, it, r1, r2, q1, not_pd, calc_hess, &u, &v, &t)) {
       std::swap(c->poses, c->poses_trial);
       if (hand_over) {
         std::swap(c->stats, c->stats_trial);
         CUDA_TRY(cudaMemcpyAsync(c->scal + BALM_SCAL_RCUR, c->scal + BALM_SCAL_RTRIAL, sizeof(double), cudaMemcpyDeviceToDevice, c->stream));
       }
       stats_cached = hand_over;
-      const double rho = q / q1;
-      v = 2;
-      const double f = 1 - pow(2 * rho - 1, 3);
-      u *= (f < (1.0 / 3.0) ? (1.0 / 3.0) : f);
       calc_hess = true;
-      t.accepted = 1;
-    } else {  // bavoxel.hpp:1144-1149
-      u = u * v;
-      v = 2 * v;
+    } else {
       calc_hess = o->force_hess != 0;
       stats_cached = c->stats_trial != nullptr;  // c->stats still describes c->poses (single batch)
     }
@@ -820,6 +835,129 @@ extern "C" int balm_damping_iter(balm_ctx *c, double *poses12, const balm_lm_opt
       CUDA_TRY(cudaMemcpyAsync(poses_per_iter + (size_t)it * 12 * c->N, c->poses, pbytes, cudaMemcpyDeviceToHost, c->stream));
     if (n_iters) *n_iters = it + 1;
     if (o->rel_tol >= 0 && fabs(r1 - r2) / r1 < o->rel_tol) break;  // bavoxel.hpp:1155
+  }
+  if (o->gauge_mode == 0 || o->gauge_mode == 1) TRY(launch_gauge(c, c->poses, o->gauge_mode));
+  CUDA_TRY(cudaMemcpyAsync(poses12, c->poses, pbytes, cudaMemcpyDeviceToHost, c->stream));
+  CUDA_TRY(cudaStreamSynchronize(c->stream));
+  return BALM_OK;
+}
+
+// ---------------- pose graph (pose_graph.cu) ----------------
+extern "C" int balm_set_pose_factors(balm_ctx *c, int n_factors, const int64_t *factor_ptr, const int32_t *factor_pose,
+                                     const double *poses_hat12, const double *H, int32_t *status_out) {
+  if (!c || n_factors < 1 || !factor_ptr || !factor_pose || !poses_hat12 || !H) {
+    balm_set_error("balm_set_pose_factors: bad arguments");
+    return BALM_ERR_INVALID;
+  }
+  if (factor_ptr[0] != 0) { balm_set_error("balm_set_pose_factors: factor_ptr[0] must be 0"); return BALM_ERR_INVALID; }
+  int64_t hsize = 0;
+  std::vector<char> seen((size_t)c->N, 0);
+  for (int f = 0; f < n_factors; f++) {
+    const int64_t N = factor_ptr[f + 1] - factor_ptr[f];
+    if (N < 2 || N > BALM_BATCH_MAX_POSES) {
+      balm_set_error("balm_set_pose_factors: factor " + std::to_string(f) + " has " + std::to_string(N) +
+                     " poses (2 .. 32 allowed)");
+      return BALM_ERR_INVALID;
+    }
+    const int32_t *idx = factor_pose + factor_ptr[f];
+    bool ok = true;
+    for (int64_t k = 0; k < N && ok; k++) {
+      ok = idx[k] >= 0 && idx[k] < c->N && !seen[idx[k]];
+      if (ok) seen[idx[k]] = 1;
+    }
+    for (int64_t k = 0; k < N; k++)
+      if (idx[k] >= 0 && idx[k] < c->N) seen[idx[k]] = 0;
+    if (!ok) {
+      balm_set_error("balm_set_pose_factors: factor " + std::to_string(f) +
+                     " needs distinct pose indices in [0, n_poses)");
+      return BALM_ERR_INVALID;
+    }
+    hsize += 36 * N * N;
+  }
+  const int64_t S = factor_ptr[n_factors];
+  for (int64_t e = 0; e < 12 * S; e++)
+    if (!std::isfinite(poses_hat12[e])) { balm_set_error("balm_set_pose_factors: non-finite poses_hat12"); return BALM_ERR_INVALID; }
+  for (int64_t e = 0; e < hsize; e++)
+    if (!std::isfinite(H[e])) { balm_set_error("balm_set_pose_factors: non-finite H"); return BALM_ERR_INVALID; }
+  CUDA_TRY(cudaSetDevice(c->device));
+  return pose_graph_set(c, n_factors, factor_ptr, factor_pose, poses_hat12, H, status_out);
+}
+
+extern "C" int balm_pose_graph_evaluate(balm_ctx *c, const double *poses12, double *H, double *g, double *cost) {
+  if (!c || !poses12) { balm_set_error("balm_pose_graph_evaluate: bad arguments"); return BALM_ERR_INVALID; }
+  if (!c->pg) { balm_set_error("balm_pose_graph_evaluate: no pose factors registered"); return BALM_ERR_INVALID; }
+  CUDA_TRY(cudaSetDevice(c->device));
+  CUDA_TRY(cudaMemcpyAsync(c->poses, poses12, sizeof(double) * 12 * c->N, cudaMemcpyHostToDevice, c->stream));
+  TRY(pose_graph_eval(c, c->poses));
+  const size_t n = c->n;
+  if (H) CUDA_TRY(cudaMemcpyAsync(H, c->H, sizeof(double) * n * n, cudaMemcpyDeviceToHost, c->stream));
+  if (g) CUDA_TRY(cudaMemcpyAsync(g, c->g, sizeof(double) * n, cudaMemcpyDeviceToHost, c->stream));
+  CUDA_TRY(cudaMemcpyAsync(c->h_scal, c->scal, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+  CUDA_TRY(cudaStreamSynchronize(c->stream));
+  if (cost) *cost = c->h_scal[0];
+  return BALM_OK;
+}
+
+// the pose-graph cost at c->poses_trial -> *r2 (waits for the stream)
+static int pose_graph_trial_cost(balm_ctx *c, double *r2) {
+  TRY(pose_graph_cost(c, c->poses_trial, c->scal + 2));
+  CUDA_TRY(cudaMemcpyAsync(c->h_scal + 2, c->scal + 2, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+  CUDA_TRY(cudaStreamSynchronize(c->stream));
+  *r2 = c->h_scal[2];
+  return BALM_OK;
+}
+
+extern "C" int balm_pose_graph_iter(balm_ctx *c, double *poses12, const balm_lm_opts *o, balm_trace *trace, int *n_iters,
+                                    double *poses_per_iter) {
+  if (!c || !poses12 || !o) { balm_set_error("balm_pose_graph_iter: bad arguments"); return BALM_ERR_INVALID; }
+  if (n_iters) *n_iters = 0;
+  if (c->world > 1 || c->comm) { balm_set_error("balm_pose_graph_iter: single-GPU contexts only"); return BALM_ERR_INVALID; }
+  if (!c->pg) { balm_set_error("balm_pose_graph_iter: no pose factors registered"); return BALM_ERR_INVALID; }
+  CUDA_TRY(cudaSetDevice(c->device));
+  const size_t pbytes = sizeof(double) * 12 * c->N;
+  CUDA_TRY(cudaMemcpyAsync(c->poses, poses12, pbytes, cudaMemcpyHostToDevice, c->stream));
+  double u = o->u0, v = o->v0, r1 = 0, r2 = 0;
+  bool calc_hess = true;
+  struct DeferScope {
+    balm_ctx *c;
+    ~DeferScope() { c->defer = false; }
+  } scope{c};
+  for (int it = 0; it < o->max_iter; it++) {
+    // evaluation -> solve -> pose update -> trial cost enqueued back to back, one wait at the end
+    c->defer = true;
+    int rc = BALM_OK;
+    if (calc_hess) {
+      rc = pose_graph_eval(c, c->poses);
+      if (rc == BALM_OK && cudaMemcpyAsync(c->h_scal, c->scal, sizeof(double), cudaMemcpyDeviceToHost, c->stream) != cudaSuccess)
+        rc = BALM_ERR_CUDA;
+    }
+    double q1 = 0;
+    int not_pd = 0;
+    if (rc == BALM_OK) rc = solve_dev(c, u, &q1, &not_pd);
+    if (rc == BALM_OK) rc = launch_pose_update(c, c->poses, c->dx, c->poses_trial);
+    if (rc == BALM_OK) rc = pose_graph_trial_cost(c, &r2);
+    c->defer = false;
+    if (rc != BALM_OK) return rc;
+    TRY(collect_solve(c, &q1, &not_pd));
+    int refined = 0;
+    TRY(maybe_refine(c, &q1, &not_pd, &refined));
+    if (refined && !not_pd) {  // dx changed: the trial poses and their cost again
+      TRY(launch_pose_update(c, c->poses, c->dx, c->poses_trial));
+      TRY(pose_graph_trial_cost(c, &r2));
+    }
+    if (calc_hess) r1 = c->h_scal[0];
+    balm_trace t;
+    if (lm_rule(o, it, r1, r2, q1, not_pd, calc_hess, &u, &v, &t)) {
+      std::swap(c->poses, c->poses_trial);
+      calc_hess = true;
+    } else {
+      calc_hess = o->force_hess != 0;  // H and g at c->poses are still in place
+    }
+    if (trace) trace[it] = t;
+    if (poses_per_iter)
+      CUDA_TRY(cudaMemcpyAsync(poses_per_iter + (size_t)it * 12 * c->N, c->poses, pbytes, cudaMemcpyDeviceToHost, c->stream));
+    if (n_iters) *n_iters = it + 1;
+    if (o->rel_tol >= 0 && fabs(r1 - r2) / r1 < o->rel_tol) break;
   }
   if (o->gauge_mode == 0 || o->gauge_mode == 1) TRY(launch_gauge(c, c->poses, o->gauge_mode));
   CUDA_TRY(cudaMemcpyAsync(poses12, c->poses, pbytes, cudaMemcpyDeviceToHost, c->stream));

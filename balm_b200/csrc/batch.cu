@@ -294,10 +294,9 @@ __global__ void __launch_bounds__(256) batch_assemble_kernel(const Prob *prob, c
     for (int i = threadIdx.x; i < n; i += 256) g[6 * (size_t)pr.pose_base + i] = accs[i % 6][i / 6];
 }
 
-// ---- damped solve, one CTA per problem, the packed lower triangle of H + uD in shared memory ----
-__device__ __forceinline__ int tri_idx(int i, int j, int n) { return j * n - j * (j - 1) / 2 + (i - j); }  // i >= j
-
-// w <- (L D L^T)^-1 w with the factors in A (unit-lower L below the diagonal, D on it)
+// ---- damped solve, one CTA per problem, the packed lower triangle of H + uD in shared memory (tri_idx, ldl_factor:
+// internal.cuh) ----
+// w <-(L D L^T)^-1 w with the factors in A (unit-lower L below the diagonal, D on it)
 __device__ void ldl_apply(const double *A, int n, double *w) {
   for (int k = 0; k < n; k++) {  // L y = w
     const double wk = w[k];
@@ -349,32 +348,6 @@ __device__ double damped_q1(const double *x, const double *D, const double *gb, 
   return 0.5 * s;
 }
 
-// Unpivoted right-looking LDL^T of the packed lower triangle in A, in place (unit-lower L below the diagonal, D on it);
-// col: n doubles of scratch. Stops at a zero / tiny / non-finite pivot (ldlt.cu's criterion) and returns true then.
-// Block-wide; the result is the same in every thread.
-__device__ __forceinline__ bool ldl_factor(double *A, int n, double *col) {
-  const int tid = threadIdx.x;
-  for (int k = 0; k < n; k++) {
-    const int kk = tri_idx(k, k, n);
-    const double dk = A[kk];
-    if (!(fabs(dk) > 1e-290 && fabs(dk) < 1e300)) return true;
-    for (int i = k + 1 + tid; i < n; i += SOLVE_THREADS) {
-      const double t = A[kk + i - k];
-      col[i] = t;
-      A[kk + i - k] = t / dk;
-    }
-    __syncthreads();
-    const int lane = tid & 31, warp = tid >> 5;
-    for (int j = k + 1 + warp; j < n; j += SOLVE_THREADS / 32) {
-      const double cj = col[j];
-      double *Aj = A + tri_idx(j, j, n);
-      for (int i = j + lane; i < n; i += 32) Aj[i - j] -= A[kk + i - k] * cj;
-    }
-    __syncthreads();
-  }
-  return false;
-}
-
 __global__ void __launch_bounds__(SOLVE_THREADS) batch_solve_kernel(const Prob *prob, const int *active, const double *H,
                                                                     const double *g, const double *uvec,
                                                                     const double *poses, double *trial, double *q1_out,
@@ -401,7 +374,7 @@ __global__ void __launch_bounds__(SOLVE_THREADS) batch_solve_kernel(const Prob *
   for (int i = tid; i < n; i += SOLVE_THREADS) x[i] = -gb[i];
   __syncthreads();
   // a zero / tiny / non-finite pivot makes the step not_pd
-  const bool pivot_bad = ldl_factor(A, n, col);
+  const bool pivot_bad = ldl_factor<SOLVE_THREADS>(A, n, col);
   int not_pd = pivot_bad ? 1 : 0;
   double q1 = 0.0;
   if (!pivot_bad) {
@@ -635,7 +608,7 @@ __global__ void __launch_bounds__(SOLVE_THREADS) batch_cov_solve_kernel(const Pr
     if (i >= j) A[tri_idx(i, j, n)] = Hb[e];
   }
   __syncthreads();
-  const bool pivot_bad = ldl_factor(A, n, col);
+  const bool pivot_bad = ldl_factor<SOLVE_THREADS>(A, n, col);
   if (tid == 0) {
     // a singular H (free gauge) pivots at rounding level relative to the others rather than at zero
     double dmin = 1e300, dmax = 0.0;

@@ -27,6 +27,8 @@
 void balm_set_error(const std::string &s);
 struct WindowState;  // the persistent sliding-window octree (assoc.cu)
 void window_free(WindowState *w);
+struct PoseGraph;    // the registered window factors (pose_graph.cu)
+void pose_graph_free(PoseGraph *p);
 
 #define CUDA_TRY(expr)                                                                        \
   do {                                                                                        \
@@ -105,6 +107,7 @@ struct balm_ctx {
   bool has_keys = false;
   balm_assoc_opts assoc{1.0, 2, 15, {1.0 / 16, 1.0 / 16, 1.0 / 16}};  // association options of that call
   WindowState *win = nullptr;     // balm_window_* state (independent of the registered voxel set)
+  PoseGraph *pg = nullptr;        // balm_set_pose_factors' window factors (independent of the registered voxel set)
 
   // ---- optimiser state (device) ----
   double *poses = nullptr, *poses_trial = nullptr;  // [12N]
@@ -637,6 +640,36 @@ __device__ __forceinline__ void gauge_one(double *pose, const double *pose0, boo
   pose[9] = pn[0]; pose[10] = pn[1]; pose[11] = pn[2];
 }
 
+// ---- packed lower-triangle LDL^T of a small system in shared memory (batch.cu's solves, pose_graph.cu's check) ----
+__device__ __forceinline__ int tri_idx(int i, int j, int n) { return j * n - j * (j - 1) / 2 + (i - j); }  // i >= j
+
+// Unpivoted right-looking LDL^T of the packed lower triangle in A, in place (unit-lower L below the diagonal, D on it);
+// col: n doubles of scratch. Stops at a zero / tiny / non-finite pivot (ldlt.cu's criterion) and returns true then.
+// Block-wide over THREADS threads; the result is the same in every thread.
+template <int THREADS>
+__device__ __forceinline__ bool ldl_factor(double *A, int n, double *col) {
+  const int tid = threadIdx.x;
+  for (int k = 0; k < n; k++) {
+    const int kk = tri_idx(k, k, n);
+    const double dk = A[kk];
+    if (!(fabs(dk) > 1e-290 && fabs(dk) < 1e300)) return true;
+    for (int i = k + 1 + tid; i < n; i += THREADS) {
+      const double t = A[kk + i - k];
+      col[i] = t;
+      A[kk + i - k] = t / dk;
+    }
+    __syncthreads();
+    const int lane = tid & 31, warp = tid >> 5;
+    for (int j = k + 1 + warp; j < n; j += THREADS / 32) {
+      const double cj = col[j];
+      double *Aj = A + tri_idx(j, j, n);
+      for (int i = j + lane; i < n; i += 32) Aj[i - j] -= A[kk + i - k] * cj;
+    }
+    __syncthreads();
+  }
+  return false;
+}
+
 __device__ __forceinline__ double warp_sum(double v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -684,12 +717,23 @@ int factor_kernels_setup();
 int syrk_f64_setup();
 int ldlt_setup();
 int covariance_setup();
+int pose_graph_setup();
 int tensor_syrk_init(balm_ctx *c);
 void tensor_syrk_free(balm_ctx *c);
 int tensor_syrk_check(balm_ctx *c);
 int tensor_syrk_check_enqueue(balm_ctx *c);
 int tensor_syrk_check_finish(balm_ctx *c);
 void tensor_syrk_new_problem(balm_ctx *c);
+
+// ---------------- pose graph (pose_graph.cu) ----------------
+// balm_set_pose_factors after its argument checks: uploads the factors, runs the PD check (status_out [n_factors]) and
+// builds the assembly tables; replaces c->pg only on success.
+int pose_graph_set(balm_ctx *c, int n_factors, const int64_t *factor_ptr, const int32_t *factor_pose,
+                   const double *poses_hat12, const double *H, int32_t *status_out);
+// H | g | scal[0] of the registered factors at the device poses (enqueued, no wait)
+int pose_graph_eval(balm_ctx *c, const double *poses);
+// the cost at the device poses into the device scalar *out (enqueued, no wait)
+int pose_graph_cost(balm_ctx *c, const double *poses, double *out);
 
 // ---------------- association (assoc.cu) ----------------
 // The plane voxels of one or more problems cut from raw scans. Host arrays; xyz (n_points x 3 float32, body frame) and

@@ -1,0 +1,424 @@
+// pose_graph.cu -- the pose graph of hierarchical BA's top-down step (include/balm_b200.h, balm_set_pose_factors,
+// balm_pose_graph_evaluate, balm_pose_graph_iter; DESIGN.md "Pose graph"). A window factor f holds N_f (2..32) global
+// pose indices idx, the window's refined poses T^_k and its BA Hessian H_f; with A = T_idx[0] T^_0^-1
+//     e_k = c(A^-1 T_idx[k], T^_k)  (e_0 = 0),   c(T, T^) = (Log(R R^^T), p - R R^^T p^),
+//     cost_f = 1/2 sum_{k,l >= 1} e_k^T H_f[k,l] e_l.
+// fp64 throughout; every sum runs in a fixed order and there are no floating-point atomics, so results repeat bit for bit.
+//   pg_check_kernel      per factor, one CTA: LDL^T of H_f restricted to slots >= 1 in shared memory -> status
+//   pg_linearise_kernel  per active factor, one CTA: e_k, J_k (shared), M = E^T H~ E and b = E^T H~ e -> staging
+//   pg_assemble_kernel   per (global 6x6 block pair i <= j, entry): the pair's (factor, slot, slot) terms in factor order
+//                        -> H (i, j) and (j, i) from one sum; per gradient entry: the pose's slots in factor order -> g
+//   pg_cost_kernel       per active factor, one CTA: cost_f
+//   pg_sum_kernel        one CTA: the factors' costs in factor order -> a device scalar
+#include <math.h>
+#include <algorithm>
+#include <memory>
+#include <vector>
+#include "internal.cuh"
+
+namespace {
+
+constexpr int PG_THREADS = 256;
+constexpr int PG_MAXN = BALM_BATCH_MAX_POSES;  // poses per factor
+constexpr int PG_MAXM = 6 * (PG_MAXN - 1);     // unknowns of H~ (slots >= 1)
+constexpr int CHECK_SMEM = (PG_MAXM * (PG_MAXM + 1) / 2 + PG_MAXM) * (int)sizeof(double);
+
+// Log of a rotation (row-major): theta = atan2(|v|, (tr - 1)/2), v = vee(R - R^T)/2; below 90 degrees phi = theta/|v| v,
+// else the axis from the symmetric part (R + R^T)/2 - cos(theta) I = (1 - cos(theta)) a a^T, signed by v
+__device__ __forceinline__ void log_so3(const double *R, double *phi) {
+  const double v[3] = {0.5 * (R[7] - R[5]), 0.5 * (R[2] - R[6]), 0.5 * (R[3] - R[1])};
+  const double c = 0.5 * (R[0] + R[4] + R[8] - 1.0);
+  const double s = sqrt(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]);
+  const double th = atan2(s, c);
+  if (c > 0.0) {
+    const double f = s == 0.0 ? 0.0 : th / s;
+    for (int a = 0; a < 3; a++) phi[a] = f * v[a];
+    return;
+  }
+  double B[9];
+  for (int a = 0; a < 3; a++)
+    for (int b = 0; b < 3; b++) B[a * 3 + b] = 0.5 * (R[a * 3 + b] + R[b * 3 + a]) - (a == b ? c : 0.0);
+  int i = 0;
+  if (B[4] > B[0]) i = 1;
+  if (B[8] > B[i * 4]) i = 2;
+  const double den = sqrt(B[i * 4] * (1.0 - c));
+  double ax[3] = {B[i] / den, B[3 + i] / den, B[6 + i] / den};
+  const double sg = ax[0] * v[0] + ax[1] * v[1] + ax[2] * v[2] < 0.0 ? -th : th;
+  for (int a = 0; a < 3; a++) phi[a] = sg * ax[a];
+}
+
+// e (6) and, when J is not null, J = de/d(delta_k) (row-major 6 x 6) of slot k >= 1: T0 / Tk the current poses of the
+// factor's slots 0 and k, h0 / hk its T^_0 and T^_k (pose12 layout). With Q = R^_0 R_0^T and phi = e[0..2]:
+//   J = [[Jl^-1(phi) Q, 0], [-Q hat(p_k - R_k R^_k^T p^_k), Q]].
+// Not inlined, so that the linearisation and the cost pass compute bitwise the same e.
+__device__ __noinline__ void pg_residual(const double *T0, const double *Tk, const double *h0, const double *hk,
+                                         double *e, double *J) {
+  double r0[9], p0[3], rk[9], pk[3], rh0[9], ph0[3], rhk[9], phk[3];
+  load_pose(T0, r0, p0);
+  load_pose(Tk, rk, pk);
+  load_pose(h0, rh0, ph0);
+  load_pose(hk, rhk, phk);
+  double Q[9], Rs[9], D[9], ps[3];
+  for (int a = 0; a < 3; a++)
+    for (int b = 0; b < 3; b++) Q[a * 3 + b] = rh0[a * 3] * r0[b * 3] + rh0[a * 3 + 1] * r0[b * 3 + 1] + rh0[a * 3 + 2] * r0[b * 3 + 2];
+  const double dp[3] = {pk[0] - p0[0], pk[1] - p0[1], pk[2] - p0[2]};
+  for (int a = 0; a < 3; a++) {
+    for (int b = 0; b < 3; b++) Rs[a * 3 + b] = Q[a * 3] * rk[b] + Q[a * 3 + 1] * rk[3 + b] + Q[a * 3 + 2] * rk[6 + b];
+    ps[a] = Q[a * 3] * dp[0] + Q[a * 3 + 1] * dp[1] + Q[a * 3 + 2] * dp[2] + ph0[a];
+  }
+  for (int a = 0; a < 3; a++)
+    for (int b = 0; b < 3; b++) D[a * 3 + b] = Rs[a * 3] * rhk[b * 3] + Rs[a * 3 + 1] * rhk[b * 3 + 1] + Rs[a * 3 + 2] * rhk[b * 3 + 2];
+  log_so3(D, e);
+  for (int a = 0; a < 3; a++) e[3 + a] = ps[a] - (D[a * 3] * phk[0] + D[a * 3 + 1] * phk[1] + D[a * 3 + 2] * phk[2]);
+  if (!J) return;
+  double w[3];  // p_k - R_k R^_k^T p^_k
+  for (int a = 0; a < 3; a++) {
+    double m[3];
+    for (int b = 0; b < 3; b++) m[b] = rk[a * 3] * rhk[b * 3] + rk[a * 3 + 1] * rhk[b * 3 + 1] + rk[a * 3 + 2] * rhk[b * 3 + 2];
+    w[a] = pk[a] - (m[0] * phk[0] + m[1] * phk[1] + m[2] * phk[2]);
+  }
+  // Jl^-1(phi) = I - 1/2 hat(phi) + c2 hat(phi)^2, c2 = (1 - (th/2) cot(th/2)) / th^2 (series below th = 0.1)
+  const double t2 = e[0] * e[0] + e[1] * e[1] + e[2] * e[2], th = sqrt(t2);
+  double c2;
+  if (th < 0.1) {
+    c2 = 1.0 / 12 + t2 * (1.0 / 720 + t2 * (1.0 / 30240 + t2 / 1209600));
+  } else {
+    const double h = 0.5 * th;
+    c2 = (1.0 - h * cos(h) / sin(h)) / t2;
+  }
+  const double K[9] = {0, -e[2], e[1], e[2], 0, -e[0], -e[1], e[0], 0};
+  const double W[9] = {0, -w[2], w[1], w[2], 0, -w[0], -w[1], w[0], 0};
+  double Ji[9];
+  for (int a = 0; a < 3; a++)
+    for (int b = 0; b < 3; b++)
+      Ji[a * 3 + b] = (a == b ? 1.0 : 0.0) - 0.5 * K[a * 3 + b] + c2 * (e[a] * e[b] - (a == b ? t2 : 0.0));
+  for (int a = 0; a < 3; a++)
+    for (int b = 0; b < 3; b++) {
+      J[a * 6 + b] = Ji[a * 3] * Q[b] + Ji[a * 3 + 1] * Q[3 + b] + Ji[a * 3 + 2] * Q[6 + b];
+      J[a * 6 + 3 + b] = 0.0;
+      J[(3 + a) * 6 + b] = -(Q[a * 3] * W[b] + Q[a * 3 + 1] * W[3 + b] + Q[a * 3 + 2] * W[6 + b]);
+      J[(3 + a) * 6 + 3 + b] = Q[a * 3 + b];
+    }
+}
+
+// ---- registration: H~ = H_f restricted to slots >= 1 must be positive definite. The pivot test of
+// batch_cov_solve_kernel (zero / tiny / non-finite pivot, or min |d| <= 1e-11 max |d|), and every pivot positive ----
+__global__ void __launch_bounds__(PG_THREADS) pg_check_kernel(const long long *fptr, const long long *hoff,
+                                                              const double *H, int *status) {
+  extern __shared__ double sm[];
+  const int f = blockIdx.x, tid = threadIdx.x;
+  const int n6 = 6 * (int)(fptr[f + 1] - fptr[f]), n = n6 - 6;
+  double *A = sm, *col = A + n * (n + 1) / 2;
+  const double *Hf = H + hoff[f];
+  for (int e = tid; e < n * n; e += PG_THREADS) {
+    const int j = e / n, i = e % n;
+    if (i >= j) A[tri_idx(i, j, n)] = Hf[(size_t)(j + 6) * n6 + i + 6];
+  }
+  __syncthreads();
+  const bool pivot_bad = ldl_factor<PG_THREADS>(A, n, col);
+  if (tid == 0) {
+    double dmin = 1e300, dmax = 0.0;
+    bool neg = false;
+    for (int i = 0; i < n && !pivot_bad; i++) {
+      const double d = A[tri_idx(i, i, n)];
+      neg = neg || !(d > 0.0);
+      dmin = fmin(dmin, fabs(d));
+      dmax = fmax(dmax, fabs(d));
+    }
+    status[f] = pivot_bad || neg || !(dmin > 1e-11 * dmax) ? BALM_ERR_NOT_PD : BALM_OK;
+  }
+}
+
+struct FactorView {  // one factor as the per-factor kernels read it
+  const long long *fptr, *hoff;
+  const int *pose;    // [S] global pose index of every slot
+  const double *hat;  // [S][12] T^
+  const double *H;    // per factor (6N)^2, column-major
+};
+
+// e_k (and J_k) of slots 1..N-1 of factor f into shared memory, threads 1..N-1
+__device__ __forceinline__ void factor_residuals(const FactorView &fv, int f, const double *poses, double (*se)[6],
+                                                 double (*sJ)[36]) {
+  const long long s0 = fv.fptr[f];
+  const int N = (int)(fv.fptr[f + 1] - s0), k = threadIdx.x;
+  if (k > 0 && k < N)
+    pg_residual(poses + 12 * (size_t)fv.pose[s0], poses + 12 * (size_t)fv.pose[s0 + k], fv.hat + 12 * s0,
+                fv.hat + 12 * (s0 + k), se[k], sJ ? sJ[k] : nullptr);
+  __syncthreads();
+}
+
+// ---- per active factor: M (6N x 6N, column-major, at the factor's H offset) and b (6 per slot) ----
+__global__ void __launch_bounds__(PG_THREADS) pg_linearise_kernel(FactorView fv, const int *act, const double *poses,
+                                                                  double *M, double *b) {
+  __shared__ double se[PG_MAXN][6], sJ[PG_MAXN][36];
+  const int f = act[blockIdx.x], tid = threadIdx.x;
+  const long long s0 = fv.fptr[f];
+  const int N = (int)(fv.fptr[f + 1] - s0), n6 = 6 * N, nb = N - 1;
+  const double *Hf = fv.H + fv.hoff[f];
+  double *Mf = M + fv.hoff[f], *bf = b + 6 * s0;
+  factor_residuals(fv, f, poses, se, sJ);
+  // k, l >= 1: M[k,l] = J_k^T H_f[k,l] J_l, b_k = J_k^T sum_l H_f[k,l] e_l
+  const int nm = nb * nb * 36;
+  for (int q = tid; q < nm + nb * 6; q += PG_THREADS) {
+    if (q < nm) {
+      const int a = q % 6, c6 = (q / 6) % 6, blk = q / 36, k = 1 + blk % nb, l = 1 + blk / nb;
+      const double *Hkl = Hf + (size_t)(6 * l) * n6 + 6 * k;  // H_f[6k + c, 6l + d] = Hkl[d n6 + c]
+      double s = 0.0;
+      for (int d = 0; d < 6; d++) {
+        double t = 0.0;
+        for (int c = 0; c < 6; c++) t += sJ[k][c * 6 + a] * Hkl[(size_t)d * n6 + c];
+        s += t * sJ[l][d * 6 + c6];
+      }
+      Mf[(size_t)(6 * l + c6) * n6 + 6 * k + a] = s;
+    } else {
+      const int r = q - nm, a = r % 6, k = 1 + r / 6;
+      double s = 0.0;
+      for (int c = 0; c < 6; c++) {
+        double t = 0.0;
+        for (int l = 1; l < N; l++)
+          for (int d = 0; d < 6; d++) t += Hf[(size_t)(6 * l + d) * n6 + 6 * k + c] * se[l][d];
+        s += sJ[k][c * 6 + a] * t;
+      }
+      bf[6 * k + a] = s;
+    }
+  }
+  __syncthreads();  // the block's global writes above are visible to it from here on
+  // slot 0 by the invariance to a common left transform (k, l >= 1, ascending): M[0,m] = -sum_k M[k,m],
+  // M[m,0] = -sum_l M[m,l], M[0,0] = sum_l sum_k M[k,l], b_0 = -sum_k b_k
+  for (int q = tid; q < 2 * nb * 36 + 36 + 6; q += PG_THREADS) {
+    if (q < 2 * nb * 36) {
+      const int a = q % 6, c6 = (q / 6) % 6, m = 1 + (q / 36) % nb;
+      double s = 0.0;
+      if (q < nb * 36) {
+        for (int k = 1; k < N; k++) s += Mf[(size_t)(6 * m + c6) * n6 + 6 * k + a];
+        Mf[(size_t)(6 * m + c6) * n6 + a] = -s;
+      } else {
+        for (int l = 1; l < N; l++) s += Mf[(size_t)(6 * l + c6) * n6 + 6 * m + a];
+        Mf[(size_t)c6 * n6 + 6 * m + a] = -s;
+      }
+    } else if (q < 2 * nb * 36 + 36) {
+      const int r = q - 2 * nb * 36, a = r % 6, c6 = r / 6;
+      double s = 0.0;
+      for (int l = 1; l < N; l++)
+        for (int k = 1; k < N; k++) s += Mf[(size_t)(6 * l + c6) * n6 + 6 * k + a];
+      Mf[(size_t)c6 * n6 + a] = s;
+    } else {
+      const int a = q - 2 * nb * 36 - 36;
+      double s = 0.0;
+      for (int k = 1; k < N; k++) s += bf[6 * k + a];
+      bf[a] = -s;
+    }
+  }
+}
+
+// ---- dense H and g: one thread per (block pair, entry), then one per gradient entry. H is zeroed beforehand. ----
+__global__ void __launch_bounds__(PG_THREADS) pg_assemble_kernel(const long long *fptr, const long long *hoff,
+                                                                 const int2 *pair, const int *pair_ptr, const int3 *term,
+                                                                 long long n_pairs, const double *M, const int *gp_ptr,
+                                                                 const long long *gp_slot, const double *b, int P,
+                                                                 double *H, double *g) {
+  const long long t = (long long)blockIdx.x * PG_THREADS + threadIdx.x;
+  const size_t n = 6 * (size_t)P;
+  if (t < 36 * n_pairs) {
+    const long long p = t / 36;
+    const int e = (int)(t % 36), a = e % 6, c6 = e / 6;
+    const int2 ij = pair[p];
+    // a diagonal pair sums its lower entries for both (a, c6) and (c6, a): the block comes out exactly symmetric
+    const int ra = ij.x == ij.y ? max(a, c6) : a, rc = ij.x == ij.y ? min(a, c6) : c6;
+    double s = 0.0;
+    for (int q = pair_ptr[p]; q < pair_ptr[p + 1]; q++) {
+      const int3 fkl = term[q];
+      const int n6 = 6 * (int)(fptr[fkl.x + 1] - fptr[fkl.x]);
+      s += M[hoff[fkl.x] + (size_t)(6 * fkl.z + rc) * n6 + 6 * fkl.y + ra];
+    }
+    H[(6 * (size_t)ij.y + c6) * n + 6 * (size_t)ij.x + a] = s;
+    if (ij.x != ij.y) H[(6 * (size_t)ij.x + a) * n + 6 * (size_t)ij.y + c6] = s;
+  } else if (t < 36 * n_pairs + 6 * (long long)P) {
+    const long long r = t - 36 * n_pairs;
+    const int i = (int)(r / 6), a = (int)(r % 6);
+    double s = 0.0;
+    for (int q = gp_ptr[i]; q < gp_ptr[i + 1]; q++) s += b[6 * gp_slot[q] + a];
+    g[6 * (size_t)i + a] = s;
+  }
+}
+
+// ---- per active factor: cost_f = 1/2 e~^T H~ e~, thread r owning row 6 + r of H~ ----
+__global__ void __launch_bounds__(PG_THREADS) pg_cost_kernel(FactorView fv, const int *act, const double *poses,
+                                                             double *cost_part) {
+  __shared__ double se[PG_MAXN][6];
+  __shared__ double red[PG_THREADS / 32];
+  const int f = act[blockIdx.x], tid = threadIdx.x;
+  const int N = (int)(fv.fptr[f + 1] - fv.fptr[f]), n6 = 6 * N;
+  const double *Hf = fv.H + fv.hoff[f];
+  factor_residuals(fv, f, poses, se, nullptr);
+  const double *ef = &se[0][0];
+  double part = 0.0;
+  if (tid < n6 - 6) {
+    const int r = 6 + tid;
+    double t = 0.0;
+    for (int c = 6; c < n6; c++) t += Hf[(size_t)c * n6 + r] * ef[c];
+    part = ef[r] * t;
+  }
+  part = warp_sum(part);
+  if ((tid & 31) == 0) red[tid >> 5] = part;
+  __syncthreads();
+  if (tid == 0) {
+    double s = 0.0;
+    for (int q = 0; q < PG_THREADS / 32; q++) s += red[q];
+    cost_part[blockIdx.x] = 0.5 * s;
+  }
+}
+
+__global__ void __launch_bounds__(PG_THREADS) pg_sum_kernel(const double *part, int n, double *out) {
+  __shared__ double red[PG_THREADS / 32];
+  const int tid = threadIdx.x;
+  double s = 0.0;
+  for (int i = tid; i < n; i += PG_THREADS) s += part[i];
+  s = warp_sum(s);
+  if ((tid & 31) == 0) red[tid >> 5] = s;
+  __syncthreads();
+  if (tid == 0) {
+    double r = 0.0;
+    for (int q = 0; q < PG_THREADS / 32; q++) r += red[q];
+    *out = r;
+  }
+}
+
+}  // namespace
+
+// The registered factor set (device). Factor f owns slots [fptr[f], fptr[f+1]) and the (6N_f)^2 doubles at hoff[f] of
+// H and of the staging M.
+struct PoseGraph {
+  int F = 0, n_act = 0, P = 0;
+  long long S = 0, HS = 0, n_pairs = 0;
+  long long *fptr = nullptr, *hoff = nullptr, *gp_slot = nullptr;
+  int *pose = nullptr, *act = nullptr, *pair_ptr = nullptr, *gp_ptr = nullptr, *status = nullptr;
+  int2 *pair = nullptr;
+  int3 *term = nullptr;
+  double *hat = nullptr, *H = nullptr, *M = nullptr, *b = nullptr, *cost_part = nullptr;
+  ~PoseGraph() {
+    cudaFree(fptr); cudaFree(hoff); cudaFree(gp_slot); cudaFree(pose); cudaFree(act); cudaFree(pair_ptr);
+    cudaFree(gp_ptr); cudaFree(status); cudaFree(pair); cudaFree(term); cudaFree(hat); cudaFree(H); cudaFree(M);
+    cudaFree(b); cudaFree(cost_part);
+  }
+  FactorView view() const { return FactorView{fptr, hoff, pose, hat, H}; }
+};
+
+void pose_graph_free(PoseGraph *p) { delete p; }
+
+int pose_graph_setup() {
+  CUDA_TRY(cudaFuncSetAttribute(pg_check_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, CHECK_SMEM));
+  return BALM_OK;
+}
+
+template <typename T>
+static int upload(T **dst, const T *src, size_t count, cudaStream_t st) {
+  TRY(dev_alloc(dst, count));
+  if (count) CUDA_TRY(cudaMemcpyAsync(*dst, src, sizeof(T) * count, cudaMemcpyHostToDevice, st));
+  return BALM_OK;
+}
+
+int pose_graph_set(balm_ctx *c, int n_factors, const int64_t *factor_ptr, const int32_t *factor_pose,
+                   const double *poses_hat12, const double *H, int32_t *status_out) {
+  cudaStream_t st = c->stream;
+  std::unique_ptr<PoseGraph> p(new PoseGraph());
+  const int F = n_factors;
+  p->F = F;
+  p->P = c->N;
+  p->S = factor_ptr[F];
+  std::vector<long long> fptr(factor_ptr, factor_ptr + F + 1), hoff(F + 1, 0);
+  for (int f = 0; f < F; f++) {
+    const long long N = fptr[f + 1] - fptr[f];
+    hoff[f + 1] = hoff[f] + 36 * N * N;
+  }
+  p->HS = hoff[F];
+  TRY(upload(&p->fptr, fptr.data(), F + 1, st));
+  TRY(upload(&p->hoff, hoff.data(), F + 1, st));
+  TRY(upload(&p->pose, factor_pose, (size_t)p->S, st));
+  TRY(upload(&p->hat, poses_hat12, 12 * (size_t)p->S, st));
+  TRY(upload(&p->H, H, (size_t)p->HS, st));
+  TRY(dev_alloc(&p->status, F));
+  pg_check_kernel<<<F, PG_THREADS, CHECK_SMEM, st>>>(p->fptr, p->hoff, p->H, p->status);
+  c->launches += 1;
+  CUDA_TRY(cudaGetLastError());
+  std::vector<int> status(F);
+  CUDA_TRY(cudaMemcpyAsync(status.data(), p->status, sizeof(int) * F, cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  // assembly tables: the terms of every block pair i <= j and the slots of every pose, each in factor order
+  std::vector<int> act;
+  struct Term { long long key; int f, k, l; };
+  std::vector<Term> terms;
+  std::vector<std::pair<int, long long>> slots;  // (pose, global slot)
+  for (int f = 0; f < F; f++) {
+    if (status[f] != BALM_OK) continue;
+    act.push_back(f);
+    const int N = (int)(fptr[f + 1] - fptr[f]);
+    const int32_t *idx = factor_pose + fptr[f];
+    for (int l = 0; l < N; l++) {
+      slots.push_back({idx[l], fptr[f] + l});
+      for (int k = 0; k < N; k++)
+        if (idx[k] <= idx[l]) terms.push_back({(long long)idx[k] * c->N + idx[l], f, k, l});
+    }
+  }
+  std::stable_sort(terms.begin(), terms.end(), [](const Term &a, const Term &b) { return a.key < b.key; });
+  std::stable_sort(slots.begin(), slots.end(), [](const std::pair<int, long long> &a, const std::pair<int, long long> &b) {
+    return a.first < b.first;
+  });
+  if (terms.size() >= ((size_t)1 << 31)) { balm_set_error("balm_set_pose_factors: too many factor terms"); return BALM_ERR_UNSUPPORTED; }
+  std::vector<int2> pair;
+  std::vector<int> pair_ptr;
+  std::vector<int3> term(terms.size());
+  for (size_t q = 0; q < terms.size(); q++) {
+    if (q == 0 || terms[q].key != terms[q - 1].key) {
+      pair.push_back(make_int2((int)(terms[q].key / c->N), (int)(terms[q].key % c->N)));
+      pair_ptr.push_back((int)q);
+    }
+    term[q] = make_int3(terms[q].f, terms[q].k, terms[q].l);
+  }
+  pair_ptr.push_back((int)terms.size());
+  std::vector<int> gp_ptr(c->N + 1, 0);
+  std::vector<long long> gp_slot(slots.size());
+  for (size_t q = 0; q < slots.size(); q++) {
+    gp_ptr[slots[q].first + 1]++;
+    gp_slot[q] = slots[q].second;
+  }
+  for (int i = 0; i < c->N; i++) gp_ptr[i + 1] += gp_ptr[i];
+  p->n_act = (int)act.size();
+  p->n_pairs = (long long)pair.size();
+  TRY(upload(&p->act, act.data(), act.size(), st));
+  TRY(upload(&p->pair, pair.data(), pair.size(), st));
+  TRY(upload(&p->pair_ptr, pair_ptr.data(), pair_ptr.size(), st));
+  TRY(upload(&p->term, term.data(), term.size(), st));
+  TRY(upload(&p->gp_ptr, gp_ptr.data(), gp_ptr.size(), st));
+  TRY(upload(&p->gp_slot, gp_slot.data(), gp_slot.size(), st));
+  TRY(dev_alloc(&p->M, (size_t)p->HS));
+  TRY(dev_alloc(&p->b, 6 * (size_t)p->S));
+  TRY(dev_alloc(&p->cost_part, (size_t)std::max(1, p->n_act)));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  if (status_out) std::copy(status.begin(), status.end(), status_out);
+  pose_graph_free(c->pg);
+  c->pg = p.release();
+  return BALM_OK;
+}
+
+int pose_graph_cost(balm_ctx *c, const double *poses, double *out) {
+  const PoseGraph &p = *c->pg;
+  if (p.n_act) pg_cost_kernel<<<p.n_act, PG_THREADS, 0, c->stream>>>(p.view(), p.act, poses, p.cost_part);
+  pg_sum_kernel<<<1, PG_THREADS, 0, c->stream>>>(p.cost_part, p.n_act, out);
+  c->launches += p.n_act ? 2 : 1;
+  CUDA_TRY(cudaGetLastError());
+  return BALM_OK;
+}
+
+int pose_graph_eval(balm_ctx *c, const double *poses) {
+  const PoseGraph &p = *c->pg;
+  const size_t n = c->n;
+  if (p.n_act) pg_linearise_kernel<<<p.n_act, PG_THREADS, 0, c->stream>>>(p.view(), p.act, poses, p.M, p.b);
+  CUDA_TRY(cudaMemsetAsync(c->H, 0, sizeof(double) * n * n, c->stream));
+  const long long threads = 36 * p.n_pairs + 6 * (long long)p.P;
+  pg_assemble_kernel<<<(unsigned)((threads + PG_THREADS - 1) / PG_THREADS), PG_THREADS, 0, c->stream>>>(
+      p.fptr, p.hoff, p.pair, p.pair_ptr, p.term, p.n_pairs, p.M, p.gp_ptr, p.gp_slot, p.b, p.P, c->H, c->g);
+  c->launches += p.n_act ? 2 : 1;
+  CUDA_TRY(cudaGetLastError());
+  return pose_graph_cost(c, poses, c->scal);
+}

@@ -13,6 +13,11 @@ with w the lowest-index window containing i, T that window's refined poses (its 
 BALM_OK) and F_w the final pose of keyframe w. The top's F is the input pose of its slot 0, so the result is in the
 input's world frame.
 
+With pose_graph=True the placement above is only the start: every converged window of every layer becomes a factor over
+the scans its items stand for (its relative poses, weighted by its BA Hessian; include/balm_b200.h,
+balm_set_pose_factors), and one LM solve over all scans (Context.pose_graph_iter) fuses them into one trajectory,
+re-anchored so that scan 0 keeps its input pose.
+
 python -m balm_b200.hba --file_path DIR [--out refined.csv] runs it on a benchmark_realworld directory."""
 import argparse
 import sys
@@ -22,7 +27,7 @@ import numpy as np
 
 from . import _lib as L
 from . import drivers, io
-from .context import Batch
+from .context import Batch, Context
 
 MAX_POSES = 32  # BALM_BATCH_MAX_POSES
 DEFAULT_ASSOC = dict(voxel_size=2.0, layer_limit=2, min_ps=15, eigen_value_array=(1.0 / 16, 1.0 / 16, 1.0 / 9))
@@ -74,13 +79,30 @@ def propagate(layers):
     return np.array(F)
 
 
-def hba(scans, poses12, length=10, stride=5, downsample=0.1, assoc=None, device=0, top_size=MAX_POSES, **lm_opts):
+def fuse_windows(poses_in, poses0, factors, device=0):
+    """Context.pose_graph_iter (gauge_mode 2) over all scans from poses0, then re-anchored so that scan 0 keeps its
+    input pose poses_in[0] -> (poses, dict(status, trace, n_factors, ms))."""
+    t0 = time.perf_counter()
+    c = Context(len(poses0), device)
+    try:
+        status = c.set_pose_factors(factors)
+        x, trace = c.pose_graph_iter(poses0, gauge_mode=2)
+    finally:
+        c.close()
+    x = np.array([relative_chain(poses_in[0], x[0], p) for p in x])
+    return x, dict(status=status, trace=trace, n_factors=len(factors), ms=1e3 * (time.perf_counter() - t0))
+
+
+def hba(scans, poses12, length=10, stride=5, downsample=0.1, assoc=None, device=0, top_size=MAX_POSES,
+        pose_graph=False, **lm_opts):
     """scans: list of (n_s x 3) body-frame points; poses12: P x 12 initial poses. downsample: the keyframes' voxel edge
     (< 0.001: keyframes keep every point); assoc: cut_scans options (DEFAULT_ASSOC when None); lm_opts: damping_iter
     options of every window. Layers are built while more than top_size (<= 32) items remain.
     -> dict(poses = P x 12 final poses, layers = per layer, bottom first and the top last: windows, status, n_iters,
     n_voxels, poses_in (the items' input poses), poses (per window the poses carried down), kf_sizes (None at the top)
-    and ms (wall times of cut, lm and merge))."""
+    and ms (wall times of cut, lm and merge)). pose_graph: the final poses come from the pose graph over every converged
+    window with at least 2 items, started from the propagated ones; the result then also holds pose_graph = dict(status
+    per factor, trace, n_factors, ms)."""
     if not (2 <= length <= MAX_POSES and 1 <= stride <= length and 1 <= top_size <= MAX_POSES):
         raise ValueError("hba: needs 2 <= length <= 32, 1 <= stride <= length and 1 <= top_size <= 32")
     poses12 = np.asarray(poses12, dtype=np.float64).reshape(-1, 12)
@@ -88,7 +110,8 @@ def hba(scans, poses12, length=10, stride=5, downsample=0.1, assoc=None, device=
         raise ValueError("hba: one pose per scan, at least one scan")
     assoc = dict(DEFAULT_ASSOC if assoc is None else assoc)
     items, x = list(scans), poses12
-    layers = []
+    scan_of = list(range(len(scans)))  # the bottom scan every item stands for: keyframe w is window w's slot 0
+    layers, factors = [], []
     b = Batch(device)
     try:
         while True:
@@ -105,15 +128,26 @@ def hba(scans, poses12, length=10, stride=5, downsample=0.1, assoc=None, device=
                        n_voxels=[m for m, _ in mk], poses_in=x, poses=T, kf_sizes=None,
                        ms=dict(cut=1e3 * (t1 - t0), lm=1e3 * (t2 - t1), merge=0.0))
             layers.append(lay)
+            if pose_graph:
+                for win, st, (H, _, _), Tw in zip(windows, lay["status"], b.evaluate(T), T):
+                    if st == L.OK and len(win) >= 2:
+                        factors.append(dict(poses=[scan_of[i] for i in win], poses_hat=Tw, H=H))
             if top:
                 break
             kfs = b.merge_scans(items, windows, T, downsample)
             lay["ms"]["merge"] = 1e3 * (time.perf_counter() - t2)
             lay["kf_sizes"] = [len(k) for k in kfs]
             items, x = kfs, np.array([wp[0] for wp in wposes])
+            scan_of = [scan_of[w[0]] for w in windows]
     finally:
         b.close()
-    return dict(poses=propagate(layers), layers=layers)
+    res = dict(poses=propagate(layers), layers=layers)
+    if pose_graph:
+        if factors:
+            res["poses"], res["pose_graph"] = fuse_windows(poses12, res["poses"], factors, device)
+        else:
+            res["pose_graph"] = dict(status=[], trace=[], n_factors=0, ms=0.0)
+    return res
 
 
 def main(argv=None):
@@ -127,6 +161,7 @@ def main(argv=None):
     ap.add_argument("--device", type=int, default=0)
     ap.add_argument("--max_scans", type=int, default=None, help="use only the first scans")
     ap.add_argument("--out", default=None, help="write the refined poses in alidarPose.csv format")
+    ap.add_argument("--pose_graph", action="store_true", help="fuse every window's relative poses in a pose graph")
     a = ap.parse_args(argv)
     R, p, _, scans = io.read_realworld_dir(a.file_path, a.max_scans)
     if len(R) == 0:
@@ -136,7 +171,8 @@ def main(argv=None):
     R = np.einsum("ji,njk->nik", R0, R)
     print("The size of poses: %d" % len(R))
     assoc = dict(DEFAULT_ASSOC, voxel_size=a.voxel_size)
-    res = hba(scans, drivers.pack_poses(R, p), a.length, a.stride, a.downsample, assoc, a.device, a.top_size)
+    res = hba(scans, drivers.pack_poses(R, p), a.length, a.stride, a.downsample, assoc, a.device, a.top_size,
+              pose_graph=a.pose_graph)
     for li, lay in enumerate(res["layers"]):
         guard = sum(st == L.ERR_TOO_FEW_PLANES for st in lay["status"])
         print("layer %d: %d windows, %d iterations, voxels %d, keyframe points %s, cut %.1f ms, LM %.1f ms, merge %.1f ms"
@@ -146,6 +182,12 @@ def main(argv=None):
         if guard:  # bavoxel.hpp:1079-1085, per window: that window keeps its input poses
             print("%d windows: Initial error too large." % guard)
             print("Please loose plane determination criteria for more planes.")
+    if a.pose_graph:
+        pg = res["pose_graph"]
+        tr = pg["trace"]
+        final = "-" if not tr else "%.6g -> %.6g" % (tr[0]["r1"], tr[-1]["r2"] if tr[-1]["accepted"] else tr[-1]["r1"])
+        print("pose graph: %d factors (%d not positive definite), %d iterations, cost %s, %.1f ms"
+              % (pg["n_factors"], sum(st == L.ERR_NOT_PD for st in pg["status"]), len(tr), final, pg["ms"]))
     if a.out:
         Rf, pf = drivers.unpack_poses(res["poses"])
         io.write_pose_csv(a.out, Rf, pf)

@@ -6,7 +6,9 @@ Workload: 177 synthetic scans of 75 000 points (assoc_ref.synthetic_scans, room 
 windows of 10 scans every 5, keyframes down-sampled at 0.1 m: 35 windows, then 6, then a top window of 6. Both routes
 run in one process, device first (once to warm up every shape, then --repeats times), then the host route; every batch
 call ends in a device synchronisation, so the host clock around a call measures its device work. The two routes must
-give bitwise-equal poses, statuses and keyframe sizes. Prints one JSON line; --out FILE also writes it there."""
+give bitwise-equal poses, statuses and keyframe sizes. Then the device route again with the pose graph
+(hba(pose_graph=True)): its total, the pose graph's own wall time, factor count and LM iterations. Prints one JSON line;
+--out FILE also writes it there."""
 import argparse
 import json
 import os
@@ -34,14 +36,14 @@ def host_merge(self, scans, windows, poses_list, voxel_size):
     return [hba_ref.keyframe_ref(scans, w, p, voxel_size) for w, p in zip(windows, poses_list)]
 
 
-def run(scans, poses, host):
+def run(scans, poses, host, pose_graph=False):
     from balm_b200 import Batch, hba
     device_merge = Batch.merge_scans
     if host:
         Batch.merge_scans = host_merge
     try:
         t0 = time.perf_counter()
-        res = hba.hba(scans, poses, downsample=0.1)
+        res = hba.hba(scans, poses, downsample=0.1, pose_graph=pose_graph)
         total = 1e3 * (time.perf_counter() - t0)
     finally:
         Batch.merge_scans = device_merge
@@ -78,6 +80,12 @@ def main():
     out["bitwise_equal"] = bool(np.array_equal(r0["poses"], h0["poses"]) and all(
         x["status"] == y["status"] and x["kf_sizes"] == y["kf_sizes"] for x, y in zip(r0["layers"], h0["layers"])))
     out["device_runs_bitwise_equal"] = bool(all(np.array_equal(r["poses"], r0["poses"]) for r, _ in dev))
+    pgr = [run(scans, p12, host=False, pose_graph=True) for _ in range(a.repeats)]
+    out["pose_graph"] = dict(total_ms=[t for _, t in pgr], pose_graph_ms=[r["pose_graph"]["ms"] for r, _ in pgr],
+                             factors=pgr[0][0]["pose_graph"]["n_factors"],
+                             not_pd=int(sum(s != 0 for s in pgr[0][0]["pose_graph"]["status"])),
+                             iters=len(pgr[0][0]["pose_graph"]["trace"]),
+                             runs_bitwise_equal=bool(all(np.array_equal(r["poses"], pgr[0][0]["poses"]) for r, _ in pgr)))
     s = json.dumps(out)
     if a.out:
         os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
