@@ -6,12 +6,12 @@ package does not load it, using any class does, and fails loudly if the library 
 """
 from . import _lib
 from ._lib import PREC_FP64, PREC_TENSOR, BalmError
-from .context import Batch, Context
+from .context import Batch, Context, PoseGraph
 from . import bavoxel
 from . import shard
 from . import io
 from . import drivers
 from .bavoxel import BALM2, IMUST, VOX_HESS, PointCluster
 
-__all__ = ["Context", "Batch", "BALM2", "VOX_HESS", "IMUST", "PointCluster", "PREC_FP64", "PREC_TENSOR", "BalmError",
+__all__ = ["Context", "Batch", "PoseGraph", "BALM2", "VOX_HESS", "IMUST", "PointCluster", "PREC_FP64", "PREC_TENSOR", "BalmError",
            "bavoxel", "shard", "io", "drivers"]

@@ -55,7 +55,8 @@ SYMBOLS = ["balm_last_error", "balm_version", "balm_create", "balm_destroy", "ba
            "balm_batch_pose_covariance", "balm_batch_marginalize", "balm_batch_append_scan", "balm_batch_download_fix",
            "balm_batch_window_reset", "balm_batch_window_cut", "balm_batch_window_recut", "balm_batch_window_marginalize",
            "balm_batch_window_push", "balm_batch_merge_scans", "balm_set_pose_factors", "balm_pose_graph_evaluate",
-           "balm_pose_graph_iter"]
+           "balm_pose_graph_iter", "balm_spg_create", "balm_spg_destroy", "balm_spg_set_factors", "balm_spg_structure",
+           "balm_spg_evaluate", "balm_spg_iter"]
 
 
 def lib():
@@ -136,6 +137,13 @@ def lib():
         L.balm_pose_graph_evaluate.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_double)]
         L.balm_pose_graph_iter.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(LmOpts), C.c_void_p, C.POINTER(C.c_int),
                                            C.c_void_p]
+        L.balm_spg_create.argtypes = [C.POINTER(C.c_void_p), C.c_int, C.c_int]
+        L.balm_spg_destroy.argtypes = [C.c_void_p]
+        L.balm_spg_destroy.restype = None
+        L.balm_spg_set_factors.argtypes = [C.c_void_p, C.c_int] + [C.c_void_p] * 5
+        L.balm_spg_structure.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+        L.balm_spg_evaluate.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_double)]
+        L.balm_spg_iter.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(LmOpts), C.c_void_p, C.POINTER(C.c_int), C.c_void_p]
         _lib = L
     return _lib
 

@@ -16,6 +16,41 @@ def _trace_dicts(trace):
                  recomputed_hess=bool(t.recomputed_hess), not_pd=bool(t.not_pd)) for t in trace]
 
 
+def _set_pose_factors(fn, handle, factors):
+    """Marshal window factors for balm_set_pose_factors / balm_spg_set_factors -> per factor status."""
+    idx = [np.asarray(f["poses"], dtype=np.int64).ravel() for f in factors]
+    hat, Hs = [], []
+    for f, i in zip(factors, idx):
+        n = 6 * len(i)
+        hat.append(np.asarray(f["poses_hat"], dtype=np.float64).reshape(len(i), 12))
+        H = np.asarray(f["H"], dtype=np.float64)
+        if H.shape != (n, n):
+            raise ValueError(f"set_pose_factors: H of a {len(i)}-pose factor must be {n} x {n}, got {H.shape}")
+        Hs.append(H.ravel(order="F"))
+    ptr = np.concatenate([[0], np.cumsum([len(i) for i in idx])]).astype(np.int64)
+    pose = np.ascontiguousarray(np.concatenate(idx) if idx else np.zeros(0), dtype=np.int32)
+    hat = np.ascontiguousarray(np.concatenate(hat) if hat else np.zeros((0, 12)), dtype=np.float64)
+    Hc = np.ascontiguousarray(np.concatenate(Hs) if Hs else np.zeros(0), dtype=np.float64)
+    status = np.zeros(len(factors), dtype=np.int32)
+    L.check(fn(handle, len(factors), _p(ptr), _p(pose), _p(hat), _p(Hc), _p(status)))
+    return [int(s) for s in status]
+
+
+def _pose_graph_iter(fn, handle, N, poses12, max_iter, u0, v0, rel_tol, gauge_mode, verbose, want_per_iter, force_hess):
+    """balm_pose_graph_iter / balm_spg_iter -> (poses, trace dicts)."""
+    poses = np.array(poses12, dtype=np.float64, order="C", copy=True)
+    opts = L.LmOpts(max_iter, u0, v0, rel_tol, 0, gauge_mode, 0, int(verbose), int(force_hess))
+    trace = (L.Trace * max(1, max_iter))()
+    n_it = C.c_int()
+    per_iter = np.zeros((max_iter, N, 12)) if want_per_iter else None
+    L.check(fn(handle, _p(poses), C.byref(opts), trace, C.byref(n_it), _p(per_iter)))
+    tr = _trace_dicts(trace[:n_it.value])
+    if want_per_iter:
+        for t, p in zip(tr, per_iter):
+            t["poses"] = p
+    return poses, tr
+
+
 class Context:
     """One GPU, one registered set of plane voxels, N poses."""
 
@@ -195,22 +230,7 @@ class Context:
         """Window factors (include/balm_b200.h, balm_set_pose_factors): list of dict(poses = N_f distinct global pose
         indices, poses_hat = N_f x 12 refined window poses, H = (6 N_f)^2 window BA Hessian). Replaces the previous factor
         set; a rejected call keeps it. -> per factor OK or ERR_NOT_PD (left out of the cost)."""
-        idx = [np.asarray(f["poses"], dtype=np.int64).ravel() for f in factors]
-        hat, Hs = [], []
-        for f, i in zip(factors, idx):
-            n = 6 * len(i)
-            hat.append(np.asarray(f["poses_hat"], dtype=np.float64).reshape(len(i), 12))
-            H = np.asarray(f["H"], dtype=np.float64)
-            if H.shape != (n, n):
-                raise ValueError(f"set_pose_factors: H of a {len(i)}-pose factor must be {n} x {n}, got {H.shape}")
-            Hs.append(H.ravel(order="F"))
-        ptr = np.concatenate([[0], np.cumsum([len(i) for i in idx])]).astype(np.int64)
-        pose = np.ascontiguousarray(np.concatenate(idx) if idx else np.zeros(0), dtype=np.int32)
-        hat = np.ascontiguousarray(np.concatenate(hat) if hat else np.zeros((0, 12)), dtype=np.float64)
-        Hc = np.ascontiguousarray(np.concatenate(Hs) if Hs else np.zeros(0), dtype=np.float64)
-        status = np.zeros(len(factors), dtype=np.int32)
-        L.check(L.lib().balm_set_pose_factors(self._h, len(factors), _p(ptr), _p(pose), _p(hat), _p(Hc), _p(status)))
-        return [int(s) for s in status]
+        return _set_pose_factors(L.lib().balm_set_pose_factors, self._h, factors)
 
     def pose_graph_evaluate(self, poses12, want_H=True):
         """-> (H, g, cost) of the registered factors at poses12 (H dense n x n, None with want_H=False)."""
@@ -225,17 +245,8 @@ class Context:
                         want_per_iter=False, force_hess=False):
         """damping_iter's LM on the pose-graph cost -> (poses, trace); with want_per_iter every trace record also holds
         the accepted poses after its iteration under "poses"."""
-        poses = np.array(poses12, dtype=np.float64, order="C", copy=True)
-        opts = L.LmOpts(max_iter, u0, v0, rel_tol, 0, gauge_mode, 0, int(verbose), int(force_hess))
-        trace = (L.Trace * max(1, max_iter))()
-        n_it = C.c_int()
-        per_iter = np.zeros((max_iter, self.N, 12)) if want_per_iter else None
-        L.check(L.lib().balm_pose_graph_iter(self._h, _p(poses), C.byref(opts), trace, C.byref(n_it), _p(per_iter)))
-        tr = _trace_dicts(trace[:n_it.value])
-        if want_per_iter:
-            for t, p in zip(tr, per_iter):
-                t["poses"] = p
-        return poses, tr
+        return _pose_graph_iter(L.lib().balm_pose_graph_iter, self._h, self.N, poses12, max_iter, u0, v0, rel_tol,
+                                gauge_mode, verbose, want_per_iter, force_hess)
 
     # ---- multi-GPU ----
     @staticmethod
@@ -545,3 +556,56 @@ class Batch:
                         cov[o:o + n * n].reshape(n, n, order="F") if want_cov else None))
             o += n * n
         return out
+
+
+class PoseGraph:
+    """The pose graph of Context.set_pose_factors for trajectories of any length (include/balm_b200.h, balm_spg_*): H is
+    kept as its nonzero 6x6 blocks and the damped system is solved by a block-sparse LDL^T, so memory grows with the
+    number of blocks rather than with (6 n_poses)^2."""
+
+    def __init__(self, n_poses, device=0):
+        self._h = C.c_void_p()
+        self.N = int(n_poses)
+        self.n = 6 * self.N
+        L.check(L.lib().balm_spg_create(C.byref(self._h), self.N, int(device)))
+
+    def close(self):
+        if self._h:
+            L.lib().balm_spg_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def set_pose_factors(self, factors):
+        """Context.set_pose_factors' factors, checks and result; also orders the poses and factors the pattern."""
+        return _set_pose_factors(L.lib().balm_spg_set_factors, self._h, factors)
+
+    def structure(self):
+        """-> dict(pairs, l_blocks, levels, device_bytes): nonzero block pairs of H, blocks of the factor L, levels of
+        its elimination tree and the device memory the handle holds."""
+        st = np.zeros(4, dtype=np.int64)
+        L.check(L.lib().balm_spg_structure(self._h, _p(st), None))
+        return dict(pairs=int(st[0]), l_blocks=int(st[1]), levels=int(st[2]), device_bytes=int(st[3]))
+
+    def pose_graph_evaluate(self, poses12):
+        """-> (pairs [n_pairs, 2] (i <= j), blocks [n_pairs, 6, 6] (H rows of pose i, columns of pose j), g, cost)."""
+        poses12 = np.ascontiguousarray(poses12, dtype=np.float64)
+        st = np.zeros(4, dtype=np.int64)
+        L.check(L.lib().balm_spg_structure(self._h, _p(st), None))
+        pairs = np.zeros((int(st[0]), 2), dtype=np.int32)
+        L.check(L.lib().balm_spg_structure(self._h, _p(st), _p(pairs)))
+        blocks = np.zeros((len(pairs), 36))
+        g = np.zeros(self.n)
+        r = C.c_double()
+        L.check(L.lib().balm_spg_evaluate(self._h, _p(poses12), _p(blocks), _p(g), C.byref(r)))
+        return pairs, blocks.reshape(-1, 6, 6).transpose(0, 2, 1), g, r.value
+
+    def pose_graph_iter(self, poses12, max_iter=10, u0=0.01, v0=2.0, rel_tol=1e-6, gauge_mode=0, verbose=False,
+                        want_per_iter=False, force_hess=False):
+        """Context.pose_graph_iter on the sparse solve: same arguments, poses and trace dicts."""
+        return _pose_graph_iter(L.lib().balm_spg_iter, self._h, self.N, poses12, max_iter, u0, v0, rel_tol, gauge_mode,
+                                verbose, want_per_iter, force_hess)

@@ -8,6 +8,8 @@
 #include <stdlib.h>
 #include <string.h>
 #include <algorithm>
+#include <climits>
+#include <memory>
 #include <vector>
 #include <time.h>
 #include "internal.cuh"
@@ -842,43 +844,50 @@ extern "C" int balm_damping_iter(balm_ctx *c, double *poses12, const balm_lm_opt
   return BALM_OK;
 }
 
-// ---------------- pose graph (pose_graph.cu) ----------------
-extern "C" int balm_set_pose_factors(balm_ctx *c, int n_factors, const int64_t *factor_ptr, const int32_t *factor_pose,
-                                     const double *poses_hat12, const double *H, int32_t *status_out) {
-  if (!c || n_factors < 1 || !factor_ptr || !factor_pose || !poses_hat12 || !H) {
-    balm_set_error("balm_set_pose_factors: bad arguments");
+// ---------------- pose graph (pose_graph.cu, pose_graph_sparse.cu) ----------------
+// The argument checks of balm_set_pose_factors and balm_spg_set_factors over P poses; `who` prefixes the messages.
+static int pose_factors_check(const char *who, int P, int n_factors, const int64_t *factor_ptr,
+                              const int32_t *factor_pose, const double *poses_hat12, const double *H) {
+  const std::string w = std::string(who) + ": ";
+  if (n_factors < 1 || !factor_ptr || !factor_pose || !poses_hat12 || !H) {
+    balm_set_error(w + "bad arguments");
     return BALM_ERR_INVALID;
   }
-  if (factor_ptr[0] != 0) { balm_set_error("balm_set_pose_factors: factor_ptr[0] must be 0"); return BALM_ERR_INVALID; }
+  if (factor_ptr[0] != 0) { balm_set_error(w + "factor_ptr[0] must be 0"); return BALM_ERR_INVALID; }
   int64_t hsize = 0;
-  std::vector<char> seen((size_t)c->N, 0);
+  std::vector<char> seen((size_t)P, 0);
   for (int f = 0; f < n_factors; f++) {
     const int64_t N = factor_ptr[f + 1] - factor_ptr[f];
     if (N < 2 || N > BALM_BATCH_MAX_POSES) {
-      balm_set_error("balm_set_pose_factors: factor " + std::to_string(f) + " has " + std::to_string(N) +
-                     " poses (2 .. 32 allowed)");
+      balm_set_error(w + "factor " + std::to_string(f) + " has " + std::to_string(N) + " poses (2 .. 32 allowed)");
       return BALM_ERR_INVALID;
     }
     const int32_t *idx = factor_pose + factor_ptr[f];
     bool ok = true;
     for (int64_t k = 0; k < N && ok; k++) {
-      ok = idx[k] >= 0 && idx[k] < c->N && !seen[idx[k]];
+      ok = idx[k] >= 0 && idx[k] < P && !seen[idx[k]];
       if (ok) seen[idx[k]] = 1;
     }
     for (int64_t k = 0; k < N; k++)
-      if (idx[k] >= 0 && idx[k] < c->N) seen[idx[k]] = 0;
+      if (idx[k] >= 0 && idx[k] < P) seen[idx[k]] = 0;
     if (!ok) {
-      balm_set_error("balm_set_pose_factors: factor " + std::to_string(f) +
-                     " needs distinct pose indices in [0, n_poses)");
+      balm_set_error(w + "factor " + std::to_string(f) + " needs distinct pose indices in [0, n_poses)");
       return BALM_ERR_INVALID;
     }
     hsize += 36 * N * N;
   }
   const int64_t S = factor_ptr[n_factors];
   for (int64_t e = 0; e < 12 * S; e++)
-    if (!std::isfinite(poses_hat12[e])) { balm_set_error("balm_set_pose_factors: non-finite poses_hat12"); return BALM_ERR_INVALID; }
+    if (!std::isfinite(poses_hat12[e])) { balm_set_error(w + "non-finite poses_hat12"); return BALM_ERR_INVALID; }
   for (int64_t e = 0; e < hsize; e++)
-    if (!std::isfinite(H[e])) { balm_set_error("balm_set_pose_factors: non-finite H"); return BALM_ERR_INVALID; }
+    if (!std::isfinite(H[e])) { balm_set_error(w + "non-finite H"); return BALM_ERR_INVALID; }
+  return BALM_OK;
+}
+
+extern "C" int balm_set_pose_factors(balm_ctx *c, int n_factors, const int64_t *factor_ptr, const int32_t *factor_pose,
+                                     const double *poses_hat12, const double *H, int32_t *status_out) {
+  if (!c) { balm_set_error("balm_set_pose_factors: bad arguments"); return BALM_ERR_INVALID; }
+  TRY(pose_factors_check("balm_set_pose_factors", c->N, n_factors, factor_ptr, factor_pose, poses_hat12, H));
   CUDA_TRY(cudaSetDevice(c->device));
   return pose_graph_set(c, n_factors, factor_ptr, factor_pose, poses_hat12, H, status_out);
 }
@@ -898,12 +907,82 @@ extern "C" int balm_pose_graph_evaluate(balm_ctx *c, const double *poses12, doub
   return BALM_OK;
 }
 
-// the pose-graph cost at c->poses_trial -> *r2 (waits for the stream)
-static int pose_graph_trial_cost(balm_ctx *c, double *r2) {
-  TRY(pose_graph_cost(c, c->poses_trial, c->scal + 2));
-  CUDA_TRY(cudaMemcpyAsync(c->h_scal + 2, c->scal + 2, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
-  CUDA_TRY(cudaStreamSynchronize(c->stream));
-  *r2 = c->h_scal[2];
+// The LM loop of balm_pose_graph_iter and balm_spg_iter: damping_iter's rule on the pose-graph cost. The two hold and
+// solve H differently: `eval` leaves H, g and the cost (scal[0]) at the given poses, `solve` dx, q1 (scal[1]) and the
+// flags for the damping u, both enqueued; `finish` reads q1 and not_pd after the iteration's wait and refines dx when
+// the backward-error check failed (*refined = 1: dx changed).
+struct PoseGraphLm {
+  cudaStream_t st;
+  int N;
+  const PoseGraph *pg;
+  double **poses, **poses_trial;  // the owner's [12N] buffers, swapped on acceptance
+  double *dx, *scal, *h_scal;     // scal: device [32] (3 u, 4..15 gauge snapshot), h_scal: pinned host [16]
+  long long *launches;
+  std::function<int(const double *poses)> eval;
+  std::function<int(double u)> solve;
+  std::function<int(double *q1, int *not_pd, int *refined)> finish;
+};
+
+// the pose-graph cost at the trial poses -> *r2 (waits for the stream)
+static int pose_graph_trial_cost(const PoseGraphLm &s, double *r2) {
+  TRY(pose_graph_cost(s.pg, s.st, *s.poses_trial, s.scal + 2, s.launches));
+  CUDA_TRY(cudaMemcpyAsync(s.h_scal + 2, s.scal + 2, sizeof(double), cudaMemcpyDeviceToHost, s.st));
+  CUDA_TRY(cudaStreamSynchronize(s.st));
+  *r2 = s.h_scal[2];
+  return BALM_OK;
+}
+
+static int trial_poses(const PoseGraphLm &s) {
+  *s.launches += 1;
+  return launch_pose_update(s.st, s.N, *s.poses, s.dx, *s.poses_trial);
+}
+
+static int pose_graph_lm(const PoseGraphLm &s, double *poses12, const balm_lm_opts *o, balm_trace *trace, int *n_iters,
+                         double *poses_per_iter) {
+  const size_t pbytes = sizeof(double) * 12 * s.N;
+  CUDA_TRY(cudaMemcpyAsync(*s.poses, poses12, pbytes, cudaMemcpyHostToDevice, s.st));
+  double u = o->u0, v = o->v0, r1 = 0, r2 = 0;
+  bool calc_hess = true;
+  for (int it = 0; it < o->max_iter; it++) {
+    // evaluation -> solve -> pose update -> trial cost enqueued back to back, one wait at the end
+    int rc = BALM_OK;
+    if (calc_hess) {
+      rc = s.eval(*s.poses);
+      if (rc == BALM_OK && cudaMemcpyAsync(s.h_scal, s.scal, sizeof(double), cudaMemcpyDeviceToHost, s.st) != cudaSuccess)
+        rc = BALM_ERR_CUDA;
+    }
+    double q1 = 0;
+    int not_pd = 0;
+    if (rc == BALM_OK) rc = s.solve(u);
+    if (rc == BALM_OK) rc = trial_poses(s);
+    if (rc == BALM_OK) rc = pose_graph_trial_cost(s, &r2);
+    if (rc != BALM_OK) return rc;
+    int refined = 0;
+    TRY(s.finish(&q1, &not_pd, &refined));
+    if (refined && !not_pd) {  // dx changed: the trial poses and their cost again
+      TRY(trial_poses(s));
+      TRY(pose_graph_trial_cost(s, &r2));
+    }
+    if (calc_hess) r1 = s.h_scal[0];
+    balm_trace t;
+    if (lm_rule(o, it, r1, r2, q1, not_pd, calc_hess, &u, &v, &t)) {
+      std::swap(*s.poses, *s.poses_trial);
+      calc_hess = true;
+    } else {
+      calc_hess = o->force_hess != 0;  // H and g at the current poses are still in place
+    }
+    if (trace) trace[it] = t;
+    if (poses_per_iter)
+      CUDA_TRY(cudaMemcpyAsync(poses_per_iter + (size_t)it * 12 * s.N, *s.poses, pbytes, cudaMemcpyDeviceToHost, s.st));
+    if (n_iters) *n_iters = it + 1;
+    if (o->rel_tol >= 0 && fabs(r1 - r2) / r1 < o->rel_tol) break;
+  }
+  if (o->gauge_mode == 0 || o->gauge_mode == 1) {
+    *s.launches += 1;
+    TRY(launch_gauge(s.st, s.N, *s.poses, s.scal + 4, o->gauge_mode));
+  }
+  CUDA_TRY(cudaMemcpyAsync(poses12, *s.poses, pbytes, cudaMemcpyDeviceToHost, s.st));
+  CUDA_TRY(cudaStreamSynchronize(s.st));
   return BALM_OK;
 }
 
@@ -914,55 +993,165 @@ extern "C" int balm_pose_graph_iter(balm_ctx *c, double *poses12, const balm_lm_
   if (c->world > 1 || c->comm) { balm_set_error("balm_pose_graph_iter: single-GPU contexts only"); return BALM_ERR_INVALID; }
   if (!c->pg) { balm_set_error("balm_pose_graph_iter: no pose factors registered"); return BALM_ERR_INVALID; }
   CUDA_TRY(cudaSetDevice(c->device));
-  const size_t pbytes = sizeof(double) * 12 * c->N;
-  CUDA_TRY(cudaMemcpyAsync(c->poses, poses12, pbytes, cudaMemcpyHostToDevice, c->stream));
-  double u = o->u0, v = o->v0, r1 = 0, r2 = 0;
-  bool calc_hess = true;
-  struct DeferScope {
-    balm_ctx *c;
-    ~DeferScope() { c->defer = false; }
-  } scope{c};
-  for (int it = 0; it < o->max_iter; it++) {
-    // evaluation -> solve -> pose update -> trial cost enqueued back to back, one wait at the end
-    c->defer = true;
-    int rc = BALM_OK;
-    if (calc_hess) {
-      rc = pose_graph_eval(c, c->poses);
-      if (rc == BALM_OK && cudaMemcpyAsync(c->h_scal, c->scal, sizeof(double), cudaMemcpyDeviceToHost, c->stream) != cudaSuccess)
-        rc = BALM_ERR_CUDA;
-    }
+  PoseGraphLm s{c->stream, c->N, c->pg, &c->poses, &c->poses_trial, c->dx, c->scal, c->h_scal, &c->launches};
+  s.eval = [c](const double *poses) -> int { return pose_graph_eval(c, poses); };
+  s.solve = [c](double u) -> int {  // deferred: q1 and the flags are read by finish()
     double q1 = 0;
     int not_pd = 0;
-    if (rc == BALM_OK) rc = solve_dev(c, u, &q1, &not_pd);
-    if (rc == BALM_OK) rc = launch_pose_update(c, c->poses, c->dx, c->poses_trial);
-    if (rc == BALM_OK) rc = pose_graph_trial_cost(c, &r2);
+    c->defer = true;
+    const int rc = solve_dev(c, u, &q1, &not_pd);
     c->defer = false;
-    if (rc != BALM_OK) return rc;
-    TRY(collect_solve(c, &q1, &not_pd));
-    int refined = 0;
-    TRY(maybe_refine(c, &q1, &not_pd, &refined));
-    if (refined && !not_pd) {  // dx changed: the trial poses and their cost again
-      TRY(launch_pose_update(c, c->poses, c->dx, c->poses_trial));
-      TRY(pose_graph_trial_cost(c, &r2));
-    }
-    if (calc_hess) r1 = c->h_scal[0];
-    balm_trace t;
-    if (lm_rule(o, it, r1, r2, q1, not_pd, calc_hess, &u, &v, &t)) {
-      std::swap(c->poses, c->poses_trial);
-      calc_hess = true;
-    } else {
-      calc_hess = o->force_hess != 0;  // H and g at c->poses are still in place
-    }
-    if (trace) trace[it] = t;
-    if (poses_per_iter)
-      CUDA_TRY(cudaMemcpyAsync(poses_per_iter + (size_t)it * 12 * c->N, c->poses, pbytes, cudaMemcpyDeviceToHost, c->stream));
-    if (n_iters) *n_iters = it + 1;
-    if (o->rel_tol >= 0 && fabs(r1 - r2) / r1 < o->rel_tol) break;
+    return rc;
+  };
+  s.finish = [c](double *q1, int *not_pd, int *refined) -> int {
+    TRY(collect_solve(c, q1, not_pd));
+    return maybe_refine(c, q1, not_pd, refined);
+  };
+  return pose_graph_lm(s, poses12, o, trace, n_iters, poses_per_iter);
+}
+
+// ---------------- sparse pose graph (pose_graph.cu, pose_graph_sparse.cu) ----------------
+struct balm_spg {
+  int N = 0, device = 0;
+  cudaStream_t stream = nullptr;
+  PoseGraph *pg = nullptr;          // the registered factors (null before the first registration)
+  SparseSolver *solver = nullptr;   // their ordering, symbolic factorisation and captured solve
+  double *blocks = nullptr;         // [pairs][36] H
+  double *poses = nullptr, *poses_trial = nullptr;  // [12N]
+  double *g = nullptr, *dx = nullptr, *dvec = nullptr;  // [6N]
+  double *scal = nullptr;           // device scalars [32], laid out as balm_ctx::scal
+  int *flags = nullptr;             // device flags [8] (0: bad pivot, 4: backward-error check failed)
+  double *h_scal = nullptr;         // pinned [16]
+  int *h_flags = nullptr;           // pinned [8]
+  long long launches = 0;
+  ~balm_spg() {
+    sparse_solver_free(solver);
+    pose_graph_free(pg);
+    cudaFree(blocks); cudaFree(poses); cudaFree(poses_trial); cudaFree(g); cudaFree(dx); cudaFree(dvec); cudaFree(scal);
+    cudaFree(flags);
+    cudaFreeHost(h_scal);
+    cudaFreeHost(h_flags);
+    if (stream) cudaStreamDestroy(stream);
   }
-  if (o->gauge_mode == 0 || o->gauge_mode == 1) TRY(launch_gauge(c, c->poses, o->gauge_mode));
-  CUDA_TRY(cudaMemcpyAsync(poses12, c->poses, pbytes, cudaMemcpyDeviceToHost, c->stream));
-  CUDA_TRY(cudaStreamSynchronize(c->stream));
+};
+
+extern "C" int balm_spg_create(balm_spg **out, int n_poses, int device) {
+  if (!out || n_poses < 1 || n_poses > (INT_MAX / 6 - 1)) { balm_set_error("balm_spg_create: bad arguments"); return BALM_ERR_INVALID; }
+  *out = nullptr;
+  CUDA_TRY(cudaSetDevice(device));
+  TRY(pose_graph_setup());
+  std::unique_ptr<balm_spg> s(new balm_spg());
+  s->N = n_poses;
+  s->device = device;
+  const size_t n = 6 * (size_t)n_poses;
+  CUDA_TRY(cudaStreamCreateWithFlags(&s->stream, cudaStreamNonBlocking));
+  TRY(dev_alloc(&s->poses, 12 * (size_t)n_poses));
+  TRY(dev_alloc(&s->poses_trial, 12 * (size_t)n_poses));
+  TRY(dev_alloc(&s->g, n));
+  TRY(dev_alloc(&s->dx, n));
+  TRY(dev_alloc(&s->dvec, n));
+  TRY(dev_alloc(&s->scal, 32));
+  TRY(dev_alloc(&s->flags, 8));
+  CUDA_TRY(cudaMallocHost((void **)&s->h_scal, sizeof(double) * 16));
+  CUDA_TRY(cudaMallocHost((void **)&s->h_flags, sizeof(int) * 8));
+  CUDA_TRY(cudaMemset(s->scal, 0, sizeof(double) * 32));
+  CUDA_TRY(cudaMemset(s->flags, 0, sizeof(int) * 8));
+  *out = s.release();
   return BALM_OK;
+}
+
+extern "C" void balm_spg_destroy(balm_spg *s) {
+  if (!s) return;
+  cudaSetDevice(s->device);
+  cudaStreamSynchronize(s->stream);
+  delete s;
+}
+
+extern "C" int balm_spg_set_factors(balm_spg *s, int n_factors, const int64_t *factor_ptr, const int32_t *factor_pose,
+                                    const double *poses_hat12, const double *H, int32_t *status_out) {
+  if (!s) { balm_set_error("balm_spg_set_factors: bad arguments"); return BALM_ERR_INVALID; }
+  TRY(pose_factors_check("balm_spg_set_factors", s->N, n_factors, factor_ptr, factor_pose, poses_hat12, H));
+  CUDA_TRY(cudaSetDevice(s->device));
+  PoseGraph *pg = nullptr;
+  std::vector<int> status;
+  TRY(pose_graph_build(s->stream, s->N, n_factors, factor_ptr, factor_pose, poses_hat12, H, &status, &pg, &s->launches));
+  std::unique_ptr<PoseGraph, void (*)(PoseGraph *)> pg_own(pg, pose_graph_free);
+  const std::vector<int2> &pairs = pose_graph_pairs(pg);
+  double *blocks = nullptr;
+  TRY(dev_alloc(&blocks, 36 * pairs.size()));
+  std::unique_ptr<double, cudaError_t (*)(void *)> blocks_own(blocks, cudaFree);
+  SparseSolver *solver = nullptr;
+  TRY(sparse_solver_build(s->stream, s->N, pairs, blocks, s->g, s->dvec, s->dx, s->scal, s->flags, &solver));
+  if (status_out) std::copy(status.begin(), status.end(), status_out);
+  sparse_solver_free(s->solver);
+  pose_graph_free(s->pg);
+  cudaFree(s->blocks);
+  s->solver = solver;
+  s->pg = pg_own.release();
+  s->blocks = blocks_own.release();
+  return BALM_OK;
+}
+
+extern "C" int balm_spg_structure(balm_spg *s, int64_t stats[4], int32_t *pairs) {
+  if (!s || !stats) { balm_set_error("balm_spg_structure: bad arguments"); return BALM_ERR_INVALID; }
+  if (!s->pg) { balm_set_error("balm_spg_structure: no pose factors registered"); return BALM_ERR_INVALID; }
+  const std::vector<int2> &pr = pose_graph_pairs(s->pg);
+  stats[0] = (int64_t)pr.size();
+  sparse_solver_stats(s->solver, &stats[1], &stats[2], &stats[3]);
+  stats[3] += (int64_t)(sizeof(double) * (36 * pr.size() + 2 * 12 * (size_t)s->N + 3 * 6 * (size_t)s->N + 32) +
+                        sizeof(int) * 8) + pose_graph_bytes(s->pg);
+  if (pairs)
+    for (size_t p = 0; p < pr.size(); p++) { pairs[2 * p] = pr[p].x; pairs[2 * p + 1] = pr[p].y; }
+  return BALM_OK;
+}
+
+extern "C" int balm_spg_evaluate(balm_spg *s, const double *poses12, double *blocks, double *g, double *cost) {
+  if (!s || !poses12) { balm_set_error("balm_spg_evaluate: bad arguments"); return BALM_ERR_INVALID; }
+  if (!s->pg) { balm_set_error("balm_spg_evaluate: no pose factors registered"); return BALM_ERR_INVALID; }
+  CUDA_TRY(cudaSetDevice(s->device));
+  CUDA_TRY(cudaMemcpyAsync(s->poses, poses12, sizeof(double) * 12 * s->N, cudaMemcpyHostToDevice, s->stream));
+  TRY(pose_graph_eval_blocks(s->pg, s->stream, s->poses, s->blocks, s->g, s->scal, &s->launches));
+  const size_t nbl = 36 * pose_graph_pairs(s->pg).size();
+  if (blocks && nbl) CUDA_TRY(cudaMemcpyAsync(blocks, s->blocks, sizeof(double) * nbl, cudaMemcpyDeviceToHost, s->stream));
+  if (g) CUDA_TRY(cudaMemcpyAsync(g, s->g, sizeof(double) * 6 * s->N, cudaMemcpyDeviceToHost, s->stream));
+  CUDA_TRY(cudaMemcpyAsync(s->h_scal, s->scal, sizeof(double), cudaMemcpyDeviceToHost, s->stream));
+  CUDA_TRY(cudaStreamSynchronize(s->stream));
+  if (cost) *cost = s->h_scal[0];
+  return BALM_OK;
+}
+
+extern "C" int balm_spg_iter(balm_spg *sp, double *poses12, const balm_lm_opts *o, balm_trace *trace, int *n_iters,
+                             double *poses_per_iter) {
+  if (!sp || !poses12 || !o) { balm_set_error("balm_spg_iter: bad arguments"); return BALM_ERR_INVALID; }
+  if (n_iters) *n_iters = 0;
+  if (!sp->pg) { balm_set_error("balm_spg_iter: no pose factors registered"); return BALM_ERR_INVALID; }
+  CUDA_TRY(cudaSetDevice(sp->device));
+  PoseGraphLm s{sp->stream, sp->N, sp->pg, &sp->poses, &sp->poses_trial, sp->dx, sp->scal, sp->h_scal, &sp->launches};
+  s.eval = [sp](const double *poses) -> int {
+    return pose_graph_eval_blocks(sp->pg, sp->stream, poses, sp->blocks, sp->g, sp->scal, &sp->launches);
+  };
+  s.solve = [sp](double u) -> int {
+    sp->h_scal[3] = u;  // pinned; the kernels read the damping factor from device memory
+    CUDA_TRY(cudaMemcpyAsync(sp->scal + 3, sp->h_scal + 3, sizeof(double), cudaMemcpyHostToDevice, sp->stream));
+    TRY(sparse_solve(sp->solver, sp->stream));
+    sp->launches += 1;
+    CUDA_TRY(cudaMemcpyAsync(sp->h_scal + 1, sp->scal + 1, sizeof(double), cudaMemcpyDeviceToHost, sp->stream));
+    CUDA_TRY(cudaMemcpyAsync(sp->h_flags, sp->flags, sizeof(int) * 8, cudaMemcpyDeviceToHost, sp->stream));
+    return BALM_OK;
+  };
+  s.finish = [sp](double *q1, int *not_pd, int *refined) -> int {  // collect_solve and maybe_refine of the context
+    *q1 = sp->h_scal[1];
+    *not_pd = sp->h_flags[0] != 0 || !std::isfinite(*q1);
+    *refined = 0;
+    if (sp->h_flags[4] == 0 || *not_pd) return BALM_OK;
+    int still_bad = 0;
+    TRY(sparse_refine(sp->solver, sp->stream, sp->h_flags, sp->h_scal, &still_bad));
+    *q1 = sp->h_scal[1];
+    *refined = 1;
+    if (still_bad || !std::isfinite(*q1)) *not_pd = 1;
+    return BALM_OK;
+  };
+  return pose_graph_lm(s, poses12, o, trace, n_iters, poses_per_iter);
 }
 
 // ---------------- sliding window on the registered voxel set (assoc.cu) ----------------

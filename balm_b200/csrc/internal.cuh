@@ -17,6 +17,7 @@
 #define BALM_ACC 33           // per-pose accumulators of the observation pass: g(6) + sym 6x6 diag block (21)
                               // + exact fp64 sums of squares of the 6 G' columns (diagonal of G'^T G')
 #define BALM_NB 64            // LDL^T panel width
+constexpr double SOLVE_OMEGA_TOL = 1e-12;  // componentwise backward error of a damped solve accepted without refinement
 #define BALM_SYRK_TILE 128
 // int32 exactness bound of the tensor SYRK: contraction rows of one (tile, k-split) item, a multiple of 64.
 // A digit-pair sum T_d adds at most 4 * rows products of magnitude <= 2^14: 4 * 32704 * 2^14 < 2^31.
@@ -710,7 +711,13 @@ int launch_csc_batch(balm_ctx *c, int64_t v0, int64_t v1);
 int launch_ldlt_solve(balm_ctx *c, double u);
 int refine_solution(balm_ctx *c, int *still_bad);
 int launch_pose_update(balm_ctx *c, const double *poses_in, const double *dx, double *poses_out);
+int launch_pose_update(cudaStream_t st, int N, const double *poses_in, const double *dx, double *poses_out);
 int launch_gauge(balm_ctx *c, double *poses, int mode);
+// snap: 12 doubles of device scratch for pose 0
+int launch_gauge(cudaStream_t st, int N, double *poses, double *snap, int mode);
+// q1 = 1/2 x.(u D x - g) -> scal[1], u = *u_dev
+int launch_q1(cudaStream_t st, const double *x, const double *g, const double *dvec, int n, const double *u_dev,
+              double *scal);
 int launch_synth(balm_ctx *c, int64_t n_voxels, int64_t first_voxel, int pts, double noise, double range,
                  uint64_t seed, const double *poses_gt_dev);
 int factor_kernels_setup();
@@ -726,14 +733,40 @@ int tensor_syrk_check_finish(balm_ctx *c);
 void tensor_syrk_new_problem(balm_ctx *c);
 
 // ---------------- pose graph (pose_graph.cu) ----------------
-// balm_set_pose_factors after its argument checks: uploads the factors, runs the PD check (status_out [n_factors]) and
-// builds the assembly tables; replaces c->pg only on success.
+// After those checks: uploads the factors on st, runs the PD check (per factor status) and builds the assembly tables
+// -> a new set in *out (the caller replaces its own with it).
+int pose_graph_build(cudaStream_t st, int P, int n_factors, const int64_t *factor_ptr, const int32_t *factor_pose,
+                     const double *poses_hat12, const double *H, std::vector<int> *status, PoseGraph **out,
+                     long long *launches);
+// balm_set_pose_factors after its argument checks: pose_graph_build, status_out [n_factors]; replaces c->pg on success.
 int pose_graph_set(balm_ctx *c, int n_factors, const int64_t *factor_ptr, const int32_t *factor_pose,
                    const double *poses_hat12, const double *H, int32_t *status_out);
 // H | g | scal[0] of the registered factors at the device poses (enqueued, no wait)
 int pose_graph_eval(balm_ctx *c, const double *poses);
+// the same sums with one 6x6 block per pair (column-major, in pose_graph_pairs order) instead of dense H (enqueued)
+int pose_graph_eval_blocks(const PoseGraph *p, cudaStream_t st, const double *poses, double *blocks, double *g,
+                           double *cost, long long *launches);
 // the cost at the device poses into the device scalar *out (enqueued, no wait)
-int pose_graph_cost(balm_ctx *c, const double *poses, double *out);
+int pose_graph_cost(const PoseGraph *p, cudaStream_t st, const double *poses, double *out, long long *launches);
+// the (i, j), i <= j, of every nonzero 6x6 block pair of H, ascending in (i, j)
+const std::vector<int2> &pose_graph_pairs(const PoseGraph *p);
+// device bytes the registered set holds (factors, staging, tables)
+long long pose_graph_bytes(const PoseGraph *p);
+
+// ---------------- sparse pose graph (pose_graph_sparse.cu) ----------------
+struct SparseSolver;  // nested-dissection ordering, symbolic factorisation and the per-solve CUDA graph
+void sparse_solver_free(SparseSolver *s);
+// Symbolic factorisation of the pairs' block pattern over P poses (host), device tables and the captured solve on st.
+// dvec, dx, scal and flags are the handle's buffers the solve reads and writes (as the context's launch_ldlt_solve).
+int sparse_solver_build(cudaStream_t st, int P, const std::vector<int2> &pairs, const double *blocks, const double *g,
+                        double *dvec, double *dx, double *scal, int *flags, SparseSolver **out);
+// blocks of L, elimination-tree levels and device bytes held
+void sparse_solver_stats(const SparseSolver *s, int64_t *l_blocks, int64_t *levels, int64_t *bytes);
+// (H + u diag(H)) dx = -g with u in scal[3]: damped copy, factorisation, substitutions, q1 -> scal[1], the backward-error
+// check (flags[0] bad pivot, flags[4] check failed, scal[20] omega); one graph launch, enqueued
+int sparse_solve(SparseSolver *s, cudaStream_t st);
+// refine_solution's rounds with the same factors; *still_bad when omega stayed above the tolerance (waits)
+int sparse_refine(SparseSolver *s, cudaStream_t st, int *h_flags, double *h_scal, int *still_bad);
 
 // ---------------- association (assoc.cu) ----------------
 // The plane voxels of one or more problems cut from raw scans. Host arrays; xyz (n_points x 3 float32, body frame) and

@@ -735,8 +735,6 @@ __global__ void gauge_kernel(double *poses, const double *pose0_snapshot, int N,
 
 }  // namespace
 
-constexpr double SOLVE_OMEGA_TOL = 1e-12;  // componentwise backward error accepted without refinement
-
 // omega of the current c->dx (+ the residual vector in c->rres); flags[4] raised when omega > tol. scal[20] = omega.
 static int enqueue_solve_check(balm_ctx *c) {
   const int n = c->n;
@@ -856,19 +854,32 @@ int launch_ldlt_solve(balm_ctx *c, double u) {
   return BALM_OK;
 }
 
+int launch_pose_update(cudaStream_t st, int N, const double *poses_in, const double *dx, double *poses_out) {
+  pose_update_kernel<<<(N + 127) / 128, 128, 0, st>>>(poses_in, dx, poses_out, N);
+  CUDA_TRY(cudaGetLastError());
+  return BALM_OK;
+}
+
 int launch_pose_update(balm_ctx *c, const double *poses_in, const double *dx, double *poses_out) {
-  pose_update_kernel<<<(c->N + 127) / 128, 128, 0, c->stream>>>(poses_in, dx, poses_out, c->N);
   c->launches += 1;
+  return launch_pose_update(c->stream, c->N, poses_in, dx, poses_out);
+}
+
+int launch_gauge(cudaStream_t st, int N, double *poses, double *snap, int mode) {
+  CUDA_TRY(cudaMemcpyAsync(snap, poses, 12 * sizeof(double), cudaMemcpyDeviceToDevice, st));
+  gauge_kernel<<<(N + 127) / 128, 128, 0, st>>>(poses, snap, N, mode);
   CUDA_TRY(cudaGetLastError());
   return BALM_OK;
 }
 
 int launch_gauge(balm_ctx *c, double *poses, int mode) {
-  // snapshot pose 0 into scal[4..15]
-  CUDA_TRY(cudaMemcpyAsync(c->scal + 4, poses, 12 * sizeof(double), cudaMemcpyDeviceToDevice, c->stream));
-  gauge_kernel<<<(c->N + 127) / 128, 128, 0, c->stream>>>(poses, c->scal + 4, c->N, mode);
   c->launches += 1;
-  CUDA_TRY(cudaGetLastError());
+  return launch_gauge(c->stream, c->N, poses, c->scal + 4, mode);  // snapshot pose 0 into scal[4..15]
+}
+
+int launch_q1(cudaStream_t st, const double *x, const double *g, const double *dvec, int n, const double *u_dev,
+              double *scal) {
+  q1_kernel<<<1, 1024, 0, st>>>(x, g, dvec, n, u_dev, scal);
   return BALM_OK;
 }
 

@@ -211,12 +211,28 @@ __global__ void __launch_bounds__(PG_THREADS) pg_linearise_kernel(FactorView fv,
   }
 }
 
-// ---- dense H and g: one thread per (block pair, entry), then one per gradient entry. H is zeroed beforehand. ----
+// ---- H and g: one thread per (block pair, entry), then one per gradient entry. The pair sums go to `out`: dense H
+// (zeroed beforehand) for the context, one 6x6 block per pair for the sparse pose graph. ----
+struct DenseH {  // H (6P)^2 column-major: entry (a, c6) of pair (i, j) at (6i + a, 6j + c6) and its transpose
+  double *H;
+  __device__ __forceinline__ void operator()(size_t n, long long p, int2 ij, int a, int c6, double s) const {
+    H[(6 * (size_t)ij.y + c6) * n + 6 * (size_t)ij.x + a] = s;
+    if (ij.x != ij.y) H[(6 * (size_t)ij.x + a) * n + 6 * (size_t)ij.y + c6] = s;
+  }
+};
+struct PairBlocks {  // block p (36, column-major) = H rows 6i.., columns 6j..
+  double *B;
+  __device__ __forceinline__ void operator()(size_t, long long p, int2, int a, int c6, double s) const {
+    B[36 * p + 6 * c6 + a] = s;
+  }
+};
+
+template <typename Out>
 __global__ void __launch_bounds__(PG_THREADS) pg_assemble_kernel(const long long *fptr, const long long *hoff,
                                                                  const int2 *pair, const int *pair_ptr, const int3 *term,
                                                                  long long n_pairs, const double *M, const int *gp_ptr,
                                                                  const long long *gp_slot, const double *b, int P,
-                                                                 double *H, double *g) {
+                                                                 Out out, double *g) {
   const long long t = (long long)blockIdx.x * PG_THREADS + threadIdx.x;
   const size_t n = 6 * (size_t)P;
   if (t < 36 * n_pairs) {
@@ -231,8 +247,7 @@ __global__ void __launch_bounds__(PG_THREADS) pg_assemble_kernel(const long long
       const int n6 = 6 * (int)(fptr[fkl.x + 1] - fptr[fkl.x]);
       s += M[hoff[fkl.x] + (size_t)(6 * fkl.z + rc) * n6 + 6 * fkl.y + ra];
     }
-    H[(6 * (size_t)ij.y + c6) * n + 6 * (size_t)ij.x + a] = s;
-    if (ij.x != ij.y) H[(6 * (size_t)ij.x + a) * n + 6 * (size_t)ij.y + c6] = s;
+    out(n, p, ij, a, c6, s);
   } else if (t < 36 * n_pairs + 6 * (long long)P) {
     const long long r = t - 36 * n_pairs;
     const int i = (int)(r / 6), a = (int)(r % 6);
@@ -296,6 +311,8 @@ struct PoseGraph {
   int2 *pair = nullptr;
   int3 *term = nullptr;
   double *hat = nullptr, *H = nullptr, *M = nullptr, *b = nullptr, *cost_part = nullptr;
+  std::vector<int2> pair_h;  // host copy of `pair`
+  long long bytes = 0;       // device memory held
   ~PoseGraph() {
     cudaFree(fptr); cudaFree(hoff); cudaFree(gp_slot); cudaFree(pose); cudaFree(act); cudaFree(pair_ptr);
     cudaFree(gp_ptr); cudaFree(status); cudaFree(pair); cudaFree(term); cudaFree(hat); cudaFree(H); cudaFree(M);
@@ -318,13 +335,13 @@ static int upload(T **dst, const T *src, size_t count, cudaStream_t st) {
   return BALM_OK;
 }
 
-int pose_graph_set(balm_ctx *c, int n_factors, const int64_t *factor_ptr, const int32_t *factor_pose,
-                   const double *poses_hat12, const double *H, int32_t *status_out) {
-  cudaStream_t st = c->stream;
+int pose_graph_build(cudaStream_t st, int P, int n_factors, const int64_t *factor_ptr, const int32_t *factor_pose,
+                     const double *poses_hat12, const double *H, std::vector<int> *status_out, PoseGraph **out,
+                     long long *launches) {
   std::unique_ptr<PoseGraph> p(new PoseGraph());
   const int F = n_factors;
   p->F = F;
-  p->P = c->N;
+  p->P = P;
   p->S = factor_ptr[F];
   std::vector<long long> fptr(factor_ptr, factor_ptr + F + 1), hoff(F + 1, 0);
   for (int f = 0; f < F; f++) {
@@ -339,7 +356,7 @@ int pose_graph_set(balm_ctx *c, int n_factors, const int64_t *factor_ptr, const 
   TRY(upload(&p->H, H, (size_t)p->HS, st));
   TRY(dev_alloc(&p->status, F));
   pg_check_kernel<<<F, PG_THREADS, CHECK_SMEM, st>>>(p->fptr, p->hoff, p->H, p->status);
-  c->launches += 1;
+  *launches += 1;
   CUDA_TRY(cudaGetLastError());
   std::vector<int> status(F);
   CUDA_TRY(cudaMemcpyAsync(status.data(), p->status, sizeof(int) * F, cudaMemcpyDeviceToHost, st));
@@ -357,7 +374,7 @@ int pose_graph_set(balm_ctx *c, int n_factors, const int64_t *factor_ptr, const 
     for (int l = 0; l < N; l++) {
       slots.push_back({idx[l], fptr[f] + l});
       for (int k = 0; k < N; k++)
-        if (idx[k] <= idx[l]) terms.push_back({(long long)idx[k] * c->N + idx[l], f, k, l});
+        if (idx[k] <= idx[l]) terms.push_back({(long long)idx[k] * P + idx[l], f, k, l});
     }
   }
   std::stable_sort(terms.begin(), terms.end(), [](const Term &a, const Term &b) { return a.key < b.key; });
@@ -370,19 +387,19 @@ int pose_graph_set(balm_ctx *c, int n_factors, const int64_t *factor_ptr, const 
   std::vector<int3> term(terms.size());
   for (size_t q = 0; q < terms.size(); q++) {
     if (q == 0 || terms[q].key != terms[q - 1].key) {
-      pair.push_back(make_int2((int)(terms[q].key / c->N), (int)(terms[q].key % c->N)));
+      pair.push_back(make_int2((int)(terms[q].key / P), (int)(terms[q].key % P)));
       pair_ptr.push_back((int)q);
     }
     term[q] = make_int3(terms[q].f, terms[q].k, terms[q].l);
   }
   pair_ptr.push_back((int)terms.size());
-  std::vector<int> gp_ptr(c->N + 1, 0);
+  std::vector<int> gp_ptr(P + 1, 0);
   std::vector<long long> gp_slot(slots.size());
   for (size_t q = 0; q < slots.size(); q++) {
     gp_ptr[slots[q].first + 1]++;
     gp_slot[q] = slots[q].second;
   }
-  for (int i = 0; i < c->N; i++) gp_ptr[i + 1] += gp_ptr[i];
+  for (int i = 0; i < P; i++) gp_ptr[i + 1] += gp_ptr[i];
   p->n_act = (int)act.size();
   p->n_pairs = (long long)pair.size();
   TRY(upload(&p->act, act.data(), act.size(), st));
@@ -395,30 +412,60 @@ int pose_graph_set(balm_ctx *c, int n_factors, const int64_t *factor_ptr, const 
   TRY(dev_alloc(&p->b, 6 * (size_t)p->S));
   TRY(dev_alloc(&p->cost_part, (size_t)std::max(1, p->n_act)));
   CUDA_TRY(cudaStreamSynchronize(st));
-  if (status_out) std::copy(status.begin(), status.end(), status_out);
-  pose_graph_free(c->pg);
-  c->pg = p.release();
+  p->bytes = (long long)(sizeof(long long) * (2 * (F + 1) + gp_slot.size()) +
+                         sizeof(int) * (p->S + act.size() + pair_ptr.size() + gp_ptr.size() + F) +
+                         sizeof(int2) * pair.size() + sizeof(int3) * term.size() +
+                         sizeof(double) * (12 * p->S + 2 * p->HS + 6 * p->S + std::max(1, p->n_act)));
+  p->pair_h = std::move(pair);
+  *status_out = std::move(status);
+  *out = p.release();
   return BALM_OK;
 }
 
-int pose_graph_cost(balm_ctx *c, const double *poses, double *out) {
-  const PoseGraph &p = *c->pg;
-  if (p.n_act) pg_cost_kernel<<<p.n_act, PG_THREADS, 0, c->stream>>>(p.view(), p.act, poses, p.cost_part);
-  pg_sum_kernel<<<1, PG_THREADS, 0, c->stream>>>(p.cost_part, p.n_act, out);
-  c->launches += p.n_act ? 2 : 1;
+int pose_graph_set(balm_ctx *c, int n_factors, const int64_t *factor_ptr, const int32_t *factor_pose,
+                   const double *poses_hat12, const double *H, int32_t *status_out) {
+  PoseGraph *p = nullptr;
+  std::vector<int> status;
+  TRY(pose_graph_build(c->stream, c->N, n_factors, factor_ptr, factor_pose, poses_hat12, H, &status, &p, &c->launches));
+  if (status_out) std::copy(status.begin(), status.end(), status_out);
+  pose_graph_free(c->pg);
+  c->pg = p;
+  return BALM_OK;
+}
+
+const std::vector<int2> &pose_graph_pairs(const PoseGraph *p) { return p->pair_h; }
+long long pose_graph_bytes(const PoseGraph *p) { return p->bytes; }
+
+int pose_graph_cost(const PoseGraph *pg, cudaStream_t st, const double *poses, double *out, long long *launches) {
+  const PoseGraph &p = *pg;
+  if (p.n_act) pg_cost_kernel<<<p.n_act, PG_THREADS, 0, st>>>(p.view(), p.act, poses, p.cost_part);
+  pg_sum_kernel<<<1, PG_THREADS, 0, st>>>(p.cost_part, p.n_act, out);
+  *launches += p.n_act ? 2 : 1;
+  CUDA_TRY(cudaGetLastError());
+  return BALM_OK;
+}
+
+template <typename Out>
+static int pose_graph_assemble(const PoseGraph &p, cudaStream_t st, const double *poses, Out out, double *g,
+                               long long *launches) {
+  if (p.n_act) pg_linearise_kernel<<<p.n_act, PG_THREADS, 0, st>>>(p.view(), p.act, poses, p.M, p.b);
+  const long long threads = 36 * p.n_pairs + 6 * (long long)p.P;
+  pg_assemble_kernel<<<(unsigned)((threads + PG_THREADS - 1) / PG_THREADS), PG_THREADS, 0, st>>>(
+      p.fptr, p.hoff, p.pair, p.pair_ptr, p.term, p.n_pairs, p.M, p.gp_ptr, p.gp_slot, p.b, p.P, out, g);
+  *launches += p.n_act ? 2 : 1;
   CUDA_TRY(cudaGetLastError());
   return BALM_OK;
 }
 
 int pose_graph_eval(balm_ctx *c, const double *poses) {
-  const PoseGraph &p = *c->pg;
   const size_t n = c->n;
-  if (p.n_act) pg_linearise_kernel<<<p.n_act, PG_THREADS, 0, c->stream>>>(p.view(), p.act, poses, p.M, p.b);
   CUDA_TRY(cudaMemsetAsync(c->H, 0, sizeof(double) * n * n, c->stream));
-  const long long threads = 36 * p.n_pairs + 6 * (long long)p.P;
-  pg_assemble_kernel<<<(unsigned)((threads + PG_THREADS - 1) / PG_THREADS), PG_THREADS, 0, c->stream>>>(
-      p.fptr, p.hoff, p.pair, p.pair_ptr, p.term, p.n_pairs, p.M, p.gp_ptr, p.gp_slot, p.b, p.P, c->H, c->g);
-  c->launches += p.n_act ? 2 : 1;
-  CUDA_TRY(cudaGetLastError());
-  return pose_graph_cost(c, poses, c->scal);
+  TRY(pose_graph_assemble(*c->pg, c->stream, poses, DenseH{c->H}, c->g, &c->launches));
+  return pose_graph_cost(c->pg, c->stream, poses, c->scal, &c->launches);
+}
+
+int pose_graph_eval_blocks(const PoseGraph *p, cudaStream_t st, const double *poses, double *blocks, double *g,
+                           double *cost, long long *launches) {
+  TRY(pose_graph_assemble(*p, st, poses, PairBlocks{blocks}, g, launches));
+  return pose_graph_cost(p, st, poses, cost, launches);
 }

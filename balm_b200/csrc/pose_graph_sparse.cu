@@ -1,0 +1,526 @@
+// pose_graph_sparse.cu -- the block-sparse damped solve of the sparse pose graph (include/balm_b200.h, balm_spg_*;
+// DESIGN.md "Pose graph", "Sparse solve"). A = H + u diag(H) over P poses, H the pose graph's 6x6 block pattern, is
+// factored as P L D P^T (unit-lower L of 6x6 blocks, diagonal D, no pivoting) in a nested-dissection order, and
+// (H + u diag(H)) dx = -g solved with it. Nothing of size (6P)^2 exists.
+// Registration (host, once per factor set): the ordering, the elimination tree and its levels, every column's block
+// rows, every block's update terms and every row's blocks; then the per-solve launch sequence is captured in a CUDA
+// graph. fp64 throughout; every sum runs in a fixed order and there are no floating-point atomics, so solves repeat bit
+// for bit.
+//   spg_damp_kernel      per (block of L, entry): the pair's block of H (transposed when the order swaps it) or a
+//                        zero fill block; diagonal blocks add u diag(H) and write diag(H)
+//   spg_factor_kernel    per column of one elimination-tree level, one CTA: the column's blocks minus their update
+//                        terms (a warp per block), the diagonal block's 6x6 LDL^T, the off-diagonal blocks scaled, then
+//                        the column's forward substitution (FACTOR = false: the substitution only, for refinement)
+//   spg_back_kernel      per column of one level, top level first, one warp: D^-1 and the backward substitution
+//   spg_check_kernel     per row: r = -g - A dx over the pose's pairs in ascending order, the componentwise backward
+//                        error omega (the dense solve's check, same tolerance)
+#include <math.h>
+#include <algorithm>
+#include <memory>
+#include <queue>
+#include <vector>
+#include "internal.cuh"
+
+namespace {
+
+constexpr int SP_THREADS = 512;
+constexpr int ND_LEAF = 32;  // nested dissection stops at this many poses; a leaf keeps index order
+
+struct SpView {      // L and D as the level kernels read them
+  const int *colptr;  // [P+1] blocks of column j: colptr[j] (the diagonal) .. colptr[j+1], rows ascending
+  const int *rowidx;  // [nb] block row
+  const int *lcol;    // [nb] block column
+  const long long *tptr;  // [nb+1] update terms of every block
+  const int2 *term;   // (position of L_ik, position of L_jk), ascending k
+  const int *rptr, *rpos;  // [P+1] / [nb - P] off-diagonal blocks of every row, ascending column
+  const int *perm;    // [P] pose of column j
+  double *Lx;         // [nb][36] column-major blocks
+  double *D;          // [6P]
+  int *flags;
+};
+
+__device__ __forceinline__ bool bad_pivot(double d) { return !(fabs(d) > 1e-290 && fabs(d) < 1e300); }  // as ldlt.cu
+
+__global__ void __launch_bounds__(256) spg_damp_kernel(const double *Hb, const int *lsrc, SpView v, long long nb,
+                                                       const double *u_dev, double *dvec) {
+  const long long t = (long long)blockIdx.x * 256 + threadIdx.x;
+  if (t >= 36 * nb) return;
+  const long long b = t / 36;
+  const int e = (int)(t % 36), a = e % 6, c = e / 6;
+  const int s = lsrc[b];  // 2 pair + transposed, or -1
+  double h = 0.0;
+  if (s >= 0) h = Hb[36 * (size_t)(s >> 1) + ((s & 1) ? 6 * a + c : 6 * c + a)];
+  const int j = v.lcol[b];
+  if (b == v.colptr[j] && a == c) {
+    dvec[6 * (size_t)v.perm[j] + a] = h;
+    h += *u_dev * h;
+  }
+  v.Lx[t] = h;
+}
+
+// One CTA per column j of a level: every column L_jk it depends on belongs to a lower level (k is a descendant of j).
+template <bool FACTOR>
+__global__ void __launch_bounds__(SP_THREADS) spg_factor_kernel(SpView v, const int *cols, const double *rhs, double sgn,
+                                                                double *y) {
+  __shared__ double W[36], d[6], yj[6];
+  const int j = cols[blockIdx.x], tid = threadIdx.x;
+  const int b0 = v.colptr[j], b1 = v.colptr[j + 1];
+  double *Ljj = v.Lx + 36 * (size_t)b0;
+  if (FACTOR) {
+    // W_ij = A_ij - sum_k L_ik D_k L_jk^T: one warp per block, lane l summing the terms l, l + 32, ... in ascending k,
+    // then the lanes' sums in a fixed butterfly
+    const int lane = tid & 31;
+    for (int b = b0 + (tid >> 5); b < b1; b += SP_THREADS / 32) {
+      double acc[36];
+#pragma unroll
+      for (int e = 0; e < 36; e++) acc[e] = 0.0;
+      for (long long t = v.tptr[b] + lane; t < v.tptr[b + 1]; t += 32) {
+        const int2 tk = v.term[t];
+        const double *Li = v.Lx + 36 * (size_t)tk.x, *Lj = v.Lx + 36 * (size_t)tk.y, *Dk = v.D + 6 * (size_t)v.lcol[tk.x];
+#pragma unroll
+        for (int m = 0; m < 6; m++) {
+          double li[6], lj[6];
+          const double dk = Dk[m];
+#pragma unroll
+          for (int a = 0; a < 6; a++) {
+            li[a] = Li[6 * m + a] * dk;
+            lj[a] = Lj[6 * m + a];
+          }
+#pragma unroll
+          for (int c = 0; c < 6; c++)
+#pragma unroll
+            for (int a = 0; a < 6; a++) acc[6 * c + a] = fma(li[a], lj[c], acc[6 * c + a]);
+        }
+      }
+      double *Lb = v.Lx + 36 * (size_t)b;
+#pragma unroll
+      for (int e = 0; e < 36; e++) {
+        const double s = Lb[e] - warp_sum(acc[e]);
+        if (lane == (e & 31)) {
+          if (b == b0) W[e] = s;
+          else Lb[e] = s;
+        }
+      }
+    }
+    __syncthreads();
+    if (tid == 0) {  // W_jj = L_jj D_j L_jj^T from its lower triangle, column by column
+      bool bad = false;
+      for (int m = 0; m < 6; m++) {
+        double dm = W[7 * m];
+        for (int p = 0; p < m; p++) dm -= W[6 * p + m] * W[6 * p + m] * d[p];
+        bad = bad || bad_pivot(dm);
+        d[m] = dm;
+        for (int r = m + 1; r < 6; r++) {
+          double s = W[6 * m + r];
+          for (int p = 0; p < m; p++) s -= W[6 * p + r] * W[6 * p + m] * d[p];
+          W[6 * m + r] = s / dm;
+        }
+      }
+      for (int m = 0; m < 6; m++) {
+        v.D[6 * (size_t)j + m] = d[m];
+        for (int r = 0; r < 6; r++) Ljj[6 * m + r] = r == m ? 1.0 : r > m ? W[6 * m + r] : 0.0;
+      }
+      if (bad) atomicOr(&v.flags[0], 1);
+    }
+    __syncthreads();
+    // L_ij D_j L_jj^T = W_ij, one thread per row of an off-diagonal block
+    for (int q = tid; q < 6 * (b1 - b0 - 1); q += SP_THREADS) {
+      double *B = v.Lx + 36 * (size_t)(b0 + 1 + q / 6);
+      const int a = q % 6;
+      double yr[6];
+      for (int m = 0; m < 6; m++) {
+        double s = B[6 * m + a];
+        for (int p = 0; p < m; p++) s -= yr[p] * W[6 * p + m];
+        yr[m] = s;
+      }
+      for (int m = 0; m < 6; m++) B[6 * m + a] = yr[m] / d[m];
+    }
+  }
+  // y_j = L_jj^-1 (b_j - sum_k L_jk y_k), b = sgn rhs in pose order
+  if (tid < 6) {
+    double s = sgn * rhs[6 * (size_t)v.perm[j] + tid];
+    for (int q = v.rptr[j]; q < v.rptr[j + 1]; q++) {
+      const int p = v.rpos[q];
+      const double *B = v.Lx + 36 * (size_t)p, *yk = y + 6 * (size_t)v.lcol[p];
+      for (int m = 0; m < 6; m++) s -= B[6 * m + tid] * yk[m];
+    }
+    yj[tid] = s;
+  }
+  __syncthreads();
+  if (tid == 0) {
+    for (int m = 0; m < 6; m++) {
+      double s = yj[m];
+      for (int p = 0; p < m; p++) s -= Ljj[6 * p + m] * yj[p];
+      yj[m] = s;
+      y[6 * (size_t)j + m] = s;
+    }
+  }
+}
+
+// x_j = L_jj^-T (D_j^-1 y_j - sum_i L_ij^T x_i) over the column's off-diagonal blocks in ascending row order; x in
+// column order, and into out in pose order (ACCUM: out += x, the refinement's correction)
+template <bool ACCUM>
+__global__ void __launch_bounds__(32) spg_back_kernel(SpView v, const int *cols, const double *y, double *x,
+                                                      double *out) {
+  __shared__ double z[6];
+  const int j = cols[blockIdx.x], tid = threadIdx.x;
+  const int b0 = v.colptr[j], b1 = v.colptr[j + 1];
+  if (tid < 6) {
+    double s = y[6 * (size_t)j + tid] / v.D[6 * (size_t)j + tid];
+    for (int b = b0 + 1; b < b1; b++) {
+      const double *B = v.Lx + 36 * (size_t)b, *xi = x + 6 * (size_t)v.rowidx[b];
+      for (int c = 0; c < 6; c++) s -= B[6 * tid + c] * xi[c];
+    }
+    z[tid] = s;
+  }
+  __syncwarp();
+  if (tid == 0) {
+    const double *Ljj = v.Lx + 36 * (size_t)b0;
+    const size_t o = 6 * (size_t)v.perm[j];
+    for (int m = 5; m >= 0; m--) {
+      double s = z[m];
+      for (int p = m + 1; p < 6; p++) s -= Ljj[6 * m + p] * z[p];
+      z[m] = s;
+      x[6 * (size_t)j + m] = s;
+      if (ACCUM) out[o + m] += s;
+      else out[o + m] = s;
+    }
+  }
+}
+
+// the backward error of dx: row 6i + a of A dx over pose i's pairs (2 pair + transposed, other pose) in ascending order
+__global__ void __launch_bounds__(256) spg_check_kernel(const double *Hb, const int *pp_ptr, const int2 *pp,
+                                                        const double *g, const double *x, int P, const double *u_dev,
+                                                        double tol, double *rres, int *flags, double *omega_out) {
+  const int r = blockIdx.x * 256 + threadIdx.x;
+  if (r >= 6 * P) return;
+  const int i = r / 6, a = r % 6;
+  const double u = *u_dev;
+  double s = 0.0, sa = 0.0;
+  for (int q = pp_ptr[i]; q < pp_ptr[i + 1]; q++) {
+    const int2 e = pp[q];
+    const double *B = Hb + 36 * (size_t)(e.x >> 1);
+    for (int c = 0; c < 6; c++) {
+      double h = B[(e.x & 1) ? 6 * a + c : 6 * c + a];
+      if (e.y == i && c == a) h += u * h;
+      const double t = h * x[6 * (size_t)e.y + c];
+      s += t;
+      sa += fabs(t);
+    }
+  }
+  const double b = -g[r], res = b - s, den = sa + fabs(b);
+  rres[r] = res;
+  const double om = den > 0.0 ? fabs(res) / den : 0.0;
+  if (!(om <= tol)) atomicOr(&flags[4], 1);
+  atomicMax(reinterpret_cast<unsigned long long *>(omega_out), (unsigned long long)__double_as_longlong(om));
+}
+
+// ---- ordering: nested dissection of the pose graph (xadj / adj: CSR of every pose's neighbours) ----
+// A vertex set (ascending pose index) of more than ND_LEAF poses is cut at its median index; the separator is a greedy
+// vertex cover of the crossing edges (most uncovered crossing edges first, the lower index on a tie). The two halves
+// without it are ordered recursively, then the separator in ascending index.
+void nd_order(const std::vector<int> &V, const std::vector<long long> &xadj, const std::vector<int> &adj,
+              std::vector<int> &side, std::vector<int> &cnt, std::vector<int> &order) {
+  if ((int)V.size() <= ND_LEAF) {
+    order.insert(order.end(), V.begin(), V.end());
+    return;
+  }
+  const size_t h = V.size() / 2;
+  for (size_t q = 0; q < V.size(); q++) side[V[q]] = q < h ? 1 : 2;
+  std::priority_queue<std::pair<int, int>> heap;  // (crossing edges, -pose)
+  for (int v : V) {
+    int n = 0;
+    for (long long q = xadj[v]; q < xadj[v + 1]; q++) n += side[adj[q]] == 3 - side[v];
+    cnt[v] = n;
+    if (n) heap.push({n, -v});
+  }
+  std::vector<int> sep;
+  while (!heap.empty()) {
+    const int n = heap.top().first, v = -heap.top().second;
+    heap.pop();
+    if (side[v] == 0 || cnt[v] == 0) continue;
+    if (n != cnt[v]) { heap.push({cnt[v], -v}); continue; }
+    const int sv = side[v];
+    side[v] = 0;  // separator
+    sep.push_back(v);
+    for (long long q = xadj[v]; q < xadj[v + 1]; q++)
+      if (side[adj[q]] == 3 - sv) cnt[adj[q]]--;
+  }
+  std::vector<int> left, right;
+  for (int v : V) {
+    if (side[v] == 1) left.push_back(v);
+    else if (side[v] == 2) right.push_back(v);
+    side[v] = -1;
+  }
+  std::sort(sep.begin(), sep.end());
+  nd_order(left, xadj, adj, side, cnt, order);
+  nd_order(right, xadj, adj, side, cnt, order);
+  order.insert(order.end(), sep.begin(), sep.end());
+}
+
+}  // namespace
+
+struct SparseSolver {
+  int P = 0;
+  long long nb = 0, nterm = 0, bytes = 0;
+  std::vector<int> lev_ptr;  // host: level l's columns are levcols[lev_ptr[l] .. lev_ptr[l+1])
+  int *perm = nullptr, *colptr = nullptr, *rowidx = nullptr, *lcol = nullptr, *lsrc = nullptr, *rptr = nullptr,
+      *rpos = nullptr, *levcols = nullptr, *pp_ptr = nullptr;
+  long long *tptr = nullptr;
+  int2 *term = nullptr, *pp = nullptr;
+  double *Lx = nullptr, *D = nullptr, *y = nullptr, *xs = nullptr, *rres = nullptr;
+  const double *Hb = nullptr, *g = nullptr;
+  double *dvec = nullptr, *dx = nullptr, *scal = nullptr;
+  int *flags = nullptr;
+  cudaGraphExec_t exec = nullptr;
+  ~SparseSolver() {
+    if (exec) cudaGraphExecDestroy(exec);
+    cudaFree(perm); cudaFree(colptr); cudaFree(rowidx); cudaFree(lcol); cudaFree(lsrc); cudaFree(rptr); cudaFree(rpos);
+    cudaFree(levcols); cudaFree(pp_ptr); cudaFree(tptr); cudaFree(term); cudaFree(pp); cudaFree(Lx); cudaFree(D);
+    cudaFree(y); cudaFree(xs); cudaFree(rres);
+  }
+  SpView view() const { return SpView{colptr, rowidx, lcol, tptr, term, rptr, rpos, perm, Lx, D, flags}; }
+  template <typename T>
+  int alloc(T **p, size_t count) {
+    TRY(dev_alloc(p, count));
+    bytes += (long long)(sizeof(T) * (count ? count : 1));
+    return BALM_OK;
+  }
+  template <typename T>
+  int put(T **p, const std::vector<T> &h, cudaStream_t st) {
+    TRY(alloc(p, h.size()));
+    if (!h.empty()) CUDA_TRY(cudaMemcpyAsync(*p, h.data(), sizeof(T) * h.size(), cudaMemcpyHostToDevice, st));
+    return BALM_OK;
+  }
+};
+
+void sparse_solver_free(SparseSolver *s) { delete s; }
+
+void sparse_solver_stats(const SparseSolver *s, int64_t *l_blocks, int64_t *levels, int64_t *bytes) {
+  *l_blocks = s->nb;
+  *levels = (int64_t)s->lev_ptr.size() - 1;
+  *bytes = s->bytes;
+}
+
+static int too_large(const char *what) {
+  balm_set_error(std::string("balm_spg_set_factors: ") + what);
+  return BALM_ERR_UNSUPPORTED;
+}
+
+// The forward sweep over the levels upwards, then the backward sweep downwards (enqueued).
+template <bool REFINE>
+static int enqueue_substitutions(SparseSolver &s, cudaStream_t st, const double *rhs, double sgn, double *out) {
+  const SpView v = s.view();
+  const int nlev = (int)s.lev_ptr.size() - 1;
+  for (int l = 0; l < nlev; l++)
+    spg_factor_kernel<!REFINE><<<s.lev_ptr[l + 1] - s.lev_ptr[l], SP_THREADS, 0, st>>>(v, s.levcols + s.lev_ptr[l], rhs,
+                                                                                       sgn, s.y);
+  for (int l = nlev - 1; l >= 0; l--)
+    spg_back_kernel<REFINE><<<s.lev_ptr[l + 1] - s.lev_ptr[l], 32, 0, st>>>(v, s.levcols + s.lev_ptr[l], s.y, s.xs, out);
+  CUDA_TRY(cudaGetLastError());
+  return BALM_OK;
+}
+
+static int enqueue_check(SparseSolver &s, cudaStream_t st) {
+  CUDA_TRY(cudaMemsetAsync(s.scal + 20, 0, sizeof(double), st));
+  spg_check_kernel<<<(6 * s.P + 255) / 256, 256, 0, st>>>(s.Hb, s.pp_ptr, s.pp, s.g, s.dx, s.P, s.scal + 3,
+                                                          SOLVE_OMEGA_TOL, s.rres, s.flags, s.scal + 20);
+  CUDA_TRY(cudaGetLastError());
+  return BALM_OK;
+}
+
+int sparse_solver_build(cudaStream_t st, int P, const std::vector<int2> &pairs, const double *blocks, const double *g,
+                        double *dvec, double *dx, double *scal, int *flags, SparseSolver **out) {
+  std::unique_ptr<SparseSolver> s(new SparseSolver());
+  s->P = P;
+  const long long npairs = (long long)pairs.size();
+  if (npairs >= (1LL << 30)) return too_large("too many block pairs");
+  // the pose graph's adjacency
+  std::vector<long long> xadj(P + 1, 0);
+  for (const int2 &p : pairs)
+    if (p.x != p.y) { xadj[p.x + 1]++; xadj[p.y + 1]++; }
+  for (int i = 0; i < P; i++) xadj[i + 1] += xadj[i];
+  std::vector<int> adj(xadj[P]);
+  {
+    std::vector<long long> fill(xadj.begin(), xadj.end() - 1);
+    for (const int2 &p : pairs)
+      if (p.x != p.y) { adj[fill[p.x]++] = p.y; adj[fill[p.y]++] = p.x; }
+  }
+  // ordering: order[k] = the pose of column k
+  std::vector<int> order, iperm(P), V(P), side(P, -1), cnt(P, 0);
+  order.reserve(P);
+  for (int i = 0; i < P; i++) V[i] = i;
+  nd_order(V, xadj, adj, side, cnt, order);
+  for (int k = 0; k < P; k++) iperm[order[k]] = k;
+  // symbolic factorisation: struct(j) = {i > j : A_ij != 0} united with struct(c) \ {j} of j's children c
+  std::vector<std::vector<int>> cstruct(P), children(P);
+  std::vector<int> mark(P, -1), level(P, 0);
+  for (int j = 0; j < P; j++) {
+    std::vector<int> &rows = cstruct[j];
+    const int pj = order[j];
+    for (long long q = xadj[pj]; q < xadj[pj + 1]; q++) {
+      const int i = iperm[adj[q]];
+      if (i > j && mark[i] != j) { mark[i] = j; rows.push_back(i); }
+    }
+    for (int c : children[j]) {
+      level[j] = std::max(level[j], level[c] + 1);
+      for (int i : cstruct[c])
+        if (i > j && mark[i] != j) { mark[i] = j; rows.push_back(i); }
+    }
+    std::sort(rows.begin(), rows.end());
+    if (!rows.empty()) children[rows[0]].push_back(j);  // the elimination tree's parent
+  }
+  // L's blocks: column j holds its diagonal block, then struct(j) ascending
+  std::vector<int> colptr(P + 1, 0);
+  for (int j = 0; j < P; j++) {
+    const long long n = (long long)colptr[j] + 1 + (long long)cstruct[j].size();
+    if (n >= (1LL << 31) / 36) return too_large("too many blocks of L");
+    colptr[j + 1] = (int)n;
+  }
+  const long long nb = colptr[P];
+  s->nb = nb;
+  std::vector<int> rowidx(nb), lcol(nb), lsrc(nb, -1), rcnt(P + 1, 0);
+  for (int j = 0; j < P; j++) {
+    rowidx[colptr[j]] = j;
+    lcol[colptr[j]] = j;
+    for (size_t q = 0; q < cstruct[j].size(); q++) {
+      rowidx[colptr[j] + 1 + q] = cstruct[j][q];
+      lcol[colptr[j] + 1 + q] = j;
+      rcnt[cstruct[j][q] + 1]++;
+    }
+  }
+  // where every pair of H lands in L: block (max, min) of its two columns, transposed when the pair's first pose comes
+  // later in the order
+  for (long long p = 0; p < npairs; p++) {
+    const int a = iperm[pairs[p].x], b = iperm[pairs[p].y];
+    const int col = std::min(a, b), row = std::max(a, b);
+    const int *r0 = rowidx.data() + colptr[col], *r1 = rowidx.data() + colptr[col + 1];
+    const int pos = (int)(std::lower_bound(r0, r1, row) - rowidx.data());
+    lsrc[pos] = (int)(2 * p + (a < b ? 1 : 0));
+  }
+  // every row's off-diagonal blocks, ascending column
+  std::vector<int> rptr(P + 1, 0), rpos(nb - P);
+  for (int i = 0; i < P; i++) rptr[i + 1] = rptr[i] + rcnt[i + 1];
+  {
+    std::vector<int> fill(rptr.begin(), rptr.end() - 1);
+    for (int k = 0; k < P; k++)
+      for (int b = colptr[k] + 1; b < colptr[k + 1]; b++) rpos[fill[rowidx[b]]++] = b;
+  }
+  // update terms: column k contributes L_ik D_k L_jk^T to block (i, j) for every i >= j in struct(k); struct(k) above j
+  // lies in column j's rows (the elimination tree), so one merge walk finds every block. Two passes: count, fill, both
+  // over k ascending, so that every block's terms are in ascending k.
+  std::vector<long long> tptr(nb + 1, 0);
+  for (int pass = 0; pass < 2; pass++) {
+    std::vector<long long> fill;
+    std::vector<int2> term;
+    if (pass == 1) {
+      for (long long b = 0; b < nb; b++) tptr[b + 1] += tptr[b];
+      s->nterm = tptr[nb];
+      fill.assign(tptr.begin(), tptr.end() - 1);
+      term.resize(s->nterm);
+    }
+    for (int k = 0; k < P; k++) {
+      const int k0 = colptr[k] + 1, m = colptr[k + 1] - k0;
+      for (int u = 0; u < m; u++) {
+        const int j = rowidx[k0 + u];
+        int q = colptr[j];
+        for (int t = u; t < m; t++) {
+          const int i = rowidx[k0 + t];
+          while (rowidx[q] != i) q++;
+          if (pass == 0) tptr[q + 1]++;
+          else term[fill[q]++] = make_int2(k0 + t, k0 + u);
+        }
+      }
+    }
+    if (pass == 1) TRY(s->put(&s->term, term, st));
+  }
+  // the levels, columns ascending inside a level
+  const int nlev = P ? 1 + *std::max_element(level.begin(), level.end()) : 0;
+  std::vector<int> lev_ptr(nlev + 1, 0), levcols(P);
+  for (int j = 0; j < P; j++) lev_ptr[level[j] + 1]++;
+  for (int l = 0; l < nlev; l++) lev_ptr[l + 1] += lev_ptr[l];
+  {
+    std::vector<int> fill(lev_ptr.begin(), lev_ptr.end() - 1);
+    for (int j = 0; j < P; j++) levcols[fill[level[j]]++] = j;
+  }
+  s->lev_ptr = lev_ptr;
+  // every pose's pairs for the residual check, ascending in the other pose
+  std::vector<int> pp_ptr(P + 1, 0);
+  for (const int2 &p : pairs) {
+    pp_ptr[p.x + 1]++;
+    if (p.x != p.y) pp_ptr[p.y + 1]++;
+  }
+  for (int i = 0; i < P; i++) pp_ptr[i + 1] += pp_ptr[i];
+  std::vector<int2> pp(pp_ptr[P]);
+  {
+    std::vector<int> fill(pp_ptr.begin(), pp_ptr.end() - 1);
+    for (long long p = 0; p < npairs; p++) {
+      pp[fill[pairs[p].x]++] = make_int2((int)(2 * p), pairs[p].y);
+      if (pairs[p].x != pairs[p].y) pp[fill[pairs[p].y]++] = make_int2((int)(2 * p + 1), pairs[p].x);
+    }
+    for (int i = 0; i < P; i++)
+      std::sort(pp.begin() + pp_ptr[i], pp.begin() + pp_ptr[i + 1], [](const int2 &a, const int2 &b) { return a.y < b.y; });
+  }
+  TRY(s->put(&s->perm, order, st));
+  TRY(s->put(&s->colptr, colptr, st));
+  TRY(s->put(&s->rowidx, rowidx, st));
+  TRY(s->put(&s->lcol, lcol, st));
+  TRY(s->put(&s->lsrc, lsrc, st));
+  TRY(s->put(&s->tptr, tptr, st));
+  TRY(s->put(&s->rptr, rptr, st));
+  TRY(s->put(&s->rpos, rpos, st));
+  TRY(s->put(&s->levcols, levcols, st));
+  TRY(s->put(&s->pp_ptr, pp_ptr, st));
+  TRY(s->put(&s->pp, pp, st));
+  TRY(s->alloc(&s->Lx, 36 * (size_t)nb));
+  TRY(s->alloc(&s->D, 6 * (size_t)P));
+  TRY(s->alloc(&s->y, 6 * (size_t)P));
+  TRY(s->alloc(&s->xs, 6 * (size_t)P));
+  TRY(s->alloc(&s->rres, 6 * (size_t)P));
+  CUDA_TRY(cudaStreamSynchronize(st));  // the host tables above are freed on return
+  s->Hb = blocks;
+  s->g = g;
+  s->dvec = dvec;
+  s->dx = dx;
+  s->scal = scal;
+  s->flags = flags;
+  // the per-solve launch sequence as one graph: 2 levels + 4 launches and 3 memsets per solve
+  cudaGraph_t graph = nullptr;
+  CUDA_TRY(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
+  int rc = BALM_OK;
+  if (cudaMemsetAsync(flags, 0, sizeof(int) * 8, st) != cudaSuccess) rc = BALM_ERR_CUDA;
+  if (rc == BALM_OK && nb)
+    spg_damp_kernel<<<(unsigned)((36 * nb + 255) / 256), 256, 0, st>>>(blocks, s->lsrc, s->view(), nb, scal + 3, dvec);
+  if (rc == BALM_OK) rc = enqueue_substitutions<false>(*s, st, g, -1.0, dx);
+  if (rc == BALM_OK) rc = launch_q1(st, dx, g, dvec, 6 * P, scal + 3, scal);
+  if (rc == BALM_OK) rc = enqueue_check(*s, st);
+  const cudaError_t ce = cudaStreamEndCapture(st, &graph);
+  if (rc != BALM_OK) { if (graph) cudaGraphDestroy(graph); return rc; }
+  CUDA_TRY(ce);
+  const cudaError_t ie = cudaGraphInstantiate(&s->exec, graph, 0);
+  cudaGraphDestroy(graph);
+  CUDA_TRY(ie);
+  *out = s.release();
+  return BALM_OK;
+}
+
+int sparse_solve(SparseSolver *s, cudaStream_t st) {
+  CUDA_TRY(cudaGraphLaunch(s->exec, st));
+  return BALM_OK;
+}
+
+int sparse_refine(SparseSolver *s, cudaStream_t st, int *h_flags, double *h_scal, int *still_bad) {
+  *still_bad = 1;
+  for (int round = 0; round < 3; round++) {
+    // A delta = r with the same factors, dx += delta
+    TRY(enqueue_substitutions<true>(*s, st, s->rres, 1.0, s->dx));
+    TRY(launch_q1(st, s->dx, s->g, s->dvec, 6 * s->P, s->scal + 3, s->scal));
+    CUDA_TRY(cudaMemsetAsync(s->flags + 4, 0, sizeof(int), st));
+    TRY(enqueue_check(*s, st));
+    CUDA_TRY(cudaMemcpyAsync(h_flags + 4, s->flags + 4, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(h_scal + 1, s->scal + 1, sizeof(double), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    if (h_flags[4] == 0) { *still_bad = 0; break; }
+  }
+  return BALM_OK;
+}

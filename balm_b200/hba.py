@@ -15,8 +15,9 @@ input's world frame.
 
 With pose_graph=True the placement above is only the start: every converged window of every layer becomes a factor over
 the scans its items stand for (its relative poses, weighted by its BA Hessian; include/balm_b200.h,
-balm_set_pose_factors), and one LM solve over all scans (Context.pose_graph_iter) fuses them into one trajectory,
-re-anchored so that scan 0 keeps its input pose.
+balm_set_pose_factors), and one LM solve over all scans fuses them into one trajectory, re-anchored so that scan 0 keeps
+its input pose. That solve is dense (Context.pose_graph_iter) for short trajectories and block-sparse (PoseGraph) from
+PG_SPARSE_MIN_POSES scans on, so that trajectories of any length fit on the device.
 
 python -m balm_b200.hba --file_path DIR [--out refined.csv] runs it on a benchmark_realworld directory."""
 import argparse
@@ -27,9 +28,12 @@ import numpy as np
 
 from . import _lib as L
 from . import drivers, io
-from .context import Batch, Context
+from .context import Batch, Context, PoseGraph
 
 MAX_POSES = 32  # BALM_BATCH_MAX_POSES
+# fuse_windows' crossover from the context's dense pose-graph solve to the sparse one (DESIGN.md "Pose graph",
+# scripts/pose_graph_perf.py): measured on an H100, the sparse iteration is faster from here on.
+PG_SPARSE_MIN_POSES = 1000
 DEFAULT_ASSOC = dict(voxel_size=2.0, layer_limit=2, min_ps=15, eigen_value_array=(1.0 / 16, 1.0 / 16, 1.0 / 9))
 
 
@@ -80,10 +84,11 @@ def propagate(layers):
 
 
 def fuse_windows(poses_in, poses0, factors, device=0):
-    """Context.pose_graph_iter (gauge_mode 2) over all scans from poses0, then re-anchored so that scan 0 keeps its
-    input pose poses_in[0] -> (poses, dict(status, trace, n_factors, ms))."""
+    """The pose graph's LM (gauge_mode 2) over all scans from poses0, then re-anchored so that scan 0 keeps its input
+    pose poses_in[0] -> (poses, dict(status, trace, n_factors, ms)). From PG_SPARSE_MIN_POSES scans on it runs on the
+    sparse solve (PoseGraph), below on the context's dense one."""
     t0 = time.perf_counter()
-    c = Context(len(poses0), device)
+    c = PoseGraph(len(poses0), device) if len(poses0) >= PG_SPARSE_MIN_POSES else Context(len(poses0), device)
     try:
         status = c.set_pose_factors(factors)
         x, trace = c.pose_graph_iter(poses0, gauge_mode=2)

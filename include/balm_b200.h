@@ -405,6 +405,32 @@ int balm_pose_graph_evaluate(balm_ctx *ctx, const double *poses12, double *H, do
 int balm_pose_graph_iter(balm_ctx *ctx, double *poses12, const balm_lm_opts *opts, balm_trace *trace, int *n_iters,
                          double *poses_per_iter);
 
+/* Sparse pose graph (DESIGN.md "Pose graph", "Sparse solve"): the same factors, cost and LM as balm_set_pose_factors /
+ * balm_pose_graph_iter, with H held as its nonzero 6x6 blocks and the damped system solved by a block LDL^T in a
+ * nested-dissection order. Device memory grows with the number of blocks, not with (6P)^2, so trajectories of any
+ * length fit; the context's dense pose graph is the faster choice for short ones. A balm_spg is a handle of its own:
+ * it holds no voxels and takes no balm_ctx call.
+ * balm_spg_create: n_poses >= 1 poses on `device`; allocates O(n_poses) device memory only. */
+typedef struct balm_spg balm_spg;
+int balm_spg_create(balm_spg **out, int n_poses, int device);
+void balm_spg_destroy(balm_spg *spg);
+/* balm_set_pose_factors' arguments, checks, messages, NOT_PD status and rejection rule (a rejected call keeps the
+ * previous set). A registration also orders the poses, builds the symbolic factorisation and captures the per-solve
+ * launches in a CUDA graph; BALM_ERR_UNSUPPORTED (previous set kept) when the pattern is too large to index. */
+int balm_spg_set_factors(balm_spg *spg, int n_factors, const int64_t *factor_ptr, const int32_t *factor_pose,
+                         const double *poses_hat12, const double *H, int32_t *status_out);
+/* stats: [0] nonzero block pairs (i <= j) of H, [1] blocks of L, [2] elimination-tree levels, [3] device bytes the
+ * handle holds (factors and their staging, tables, L, vectors).
+ * pairs (may be NULL, so that a first call can size it): 2 int32 (i, j) per block pair, ascending in (i, j). */
+int balm_spg_structure(balm_spg *spg, int64_t stats[4], int32_t *pairs);
+/* balm_pose_graph_evaluate with H as blocks: 36 doubles per block pair (rows of pose i, columns of pose j,
+ * column-major) in balm_spg_structure's order, bitwise the context's dense entries. blocks and g may be NULL. */
+int balm_spg_evaluate(balm_spg *spg, const double *poses12, double *blocks, double *g, double *cost);
+/* balm_pose_graph_iter's contract (LM rule, force_hess, rel_tol, gauge_mode, trace records, refinement and not_pd
+ * rules) on the sparse solve. */
+int balm_spg_iter(balm_spg *spg, double *poses12, const balm_lm_opts *opts, balm_trace *trace, int *n_iters,
+                  double *poses_per_iter);
+
 /* Multi-GPU: voxels are sharded across ranks by the caller (each rank registers its own shard); the library
  * all-reduces [H | g | r] with NCCL after every evaluation and the scalar after every residual pass.
  * unique_id: 128 bytes from balm_comm_unique_id() on rank 0, broadcast by the caller (torch.distributed, MPI). */

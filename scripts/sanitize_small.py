@@ -6,7 +6,8 @@ association of overlapping windows with one empty window (balm_batch_cut_voxels)
 an anchored, a free and an empty problem (balm_batch_pose_covariance), and the batched marginalise + append of those
 windows, the empty one included (balm_batch_marginalize / balm_batch_append_scan), the batch's persistent window maps
 (balm_batch_window_*), and the keyframe merge of overlapping windows with an empty scan and an empty window at voxel
-sizes 0 and 0.2 (balm_batch_merge_scans)."""
+sizes 0 and 0.2 (balm_batch_merge_scans), and the sparse pose graph (balm_spg_*) on a small pyramid with a long-range
+factor, a factor that is not positive definite and a pose in no factor."""
 import os, sys
 import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -100,4 +101,17 @@ mwin = [[0, 1, 6, 2], [2, 3, 4], [6]]
 mx = [p12[[0, 1, 1, 2]], p12[2:5], p12[:1]]
 print("batch merge", [[len(k) for k in b.merge_scans(mscans, mwin, mx, vs)] for vs in (0.0, 0.2)], flush=True)
 b.close()
+# sparse pose graph: registration, evaluation, LM with refinement checks; then a pose in no factor (not_pd steps)
+import pose_graph_ref as pgr
+rng = np.random.default_rng(15)
+truth = np.array([pgr.random_pose(rng, 0.5, 3.0) for _ in range(81)])
+fs = [pgr.make_factor(rng, truth, w, noise=0.01) for w in pgr.pyramid_factor_poses(80, top=8) + [[2, 77]]]
+fs.append(dict(fs[0], H=-fs[0]["H"]))
+s = balm_b200.PoseGraph(81)
+print("sparse pose graph status", s.set_pose_factors(fs).count(0), s.structure(), flush=True)
+print("  cost", s.pose_graph_evaluate(pgr.perturb(rng, truth, 0.05, 0.2))[3], flush=True)
+print("  not_pd", [t["not_pd"] for t in s.pose_graph_iter(truth, max_iter=2)[1]], flush=True)
+s.set_pose_factors(fs[:-1])
+print("  iters", len(s.pose_graph_iter(pgr.perturb(rng, truth, 0.05, 0.2), max_iter=3)[1]), flush=True)
+s.close()
 print("SANITIZE_DONE")
