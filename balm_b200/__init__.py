@@ -5,7 +5,7 @@ The arithmetic lives in libbalm_b200.so (hand-written CUDA, C ABI in include/bal
 package does not load it, using any class does, and fails loudly if the library has not been built.
 """
 from . import _lib
-from ._lib import PREC_FP64, PREC_TENSOR, BalmError
+from ._lib import PREC_BLOCKS, PREC_FP64, PREC_TENSOR, BalmError
 from .context import Batch, Context, PoseGraph
 from . import bavoxel
 from . import shard
@@ -13,5 +13,6 @@ from . import io
 from . import drivers
 from .bavoxel import BALM2, IMUST, VOX_HESS, PointCluster
 
-__all__ = ["Context", "Batch", "PoseGraph", "BALM2", "VOX_HESS", "IMUST", "PointCluster", "PREC_FP64", "PREC_TENSOR", "BalmError",
+__all__ = ["Context", "Batch", "PoseGraph", "BALM2", "VOX_HESS", "IMUST", "PointCluster", "PREC_FP64", "PREC_TENSOR", "PREC_BLOCKS",
+           "BalmError",
            "bavoxel", "shard", "io", "drivers"]

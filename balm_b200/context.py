@@ -139,6 +139,27 @@ class Context:
         L.check(L.lib().balm_residual(self._h, _p(poses12), C.byref(r)))
         return r.value
 
+    def block_structure(self, want_pairs=False):
+        """PREC_BLOCKS contexts: -> dict(pairs, l_blocks, levels, device_bytes): block pairs (i <= j) of H, blocks of the
+        factor L, levels of its elimination tree and the device memory the context holds; with want_pairs also
+        "pair_list", the (pairs, 2) int32 array of (i, j), ascending."""
+        st = np.zeros(4, dtype=np.int64)
+        L.check(L.lib().balm_block_structure(self._h, _p(st), None))
+        out = dict(pairs=int(st[0]), l_blocks=int(st[1]), levels=int(st[2]), device_bytes=int(st[3]))
+        if want_pairs:
+            pr = np.zeros((out["pairs"], 2), dtype=np.int32)
+            L.check(L.lib().balm_block_structure(self._h, _p(st), _p(pr)))
+            out["pair_list"] = pr
+        return out
+
+    def download_blocks(self):
+        """PREC_BLOCKS contexts: the last evaluation's blocks, (pairs, 6, 6) with [p, a, c] = H[6 i + a, 6 j + c] of
+        pair p = (i, j) in block_structure's order."""
+        npairs = self.block_structure()["pairs"]
+        b = np.zeros((npairs, 36))
+        L.check(L.lib().balm_download_blocks(self._h, _p(b)))
+        return b.reshape(npairs, 6, 6).transpose(0, 2, 1).copy()
+
     def solve(self, u):
         dx = np.zeros(self.n)
         q1 = C.c_double()

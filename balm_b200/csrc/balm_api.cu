@@ -59,6 +59,8 @@ static void free_problem(balm_ctx *c) {
   cudaFree(c->stats); cudaFree(c->stats_trial); cudaFree(c->G); cudaFree(c->obs_part); cudaFree(c->syrk_part);
   c->stats = c->stats_trial = c->G = c->obs_part = c->syrk_part = nullptr;
   tensor_syrk_free(c);
+  block_hessian_free(c->bh);
+  c->bh = nullptr;
   c->M = c->K = c->Kp = 0;
   c->registered = false;
 }
@@ -73,7 +75,9 @@ static void drop_keys(balm_ctx *c) {  // a voxel set registered from arrays carr
 static int alloc_problem_arrays(balm_ctx *c, int64_t M, int64_t K, bool with_fix) {
   // A window of the same shape as the previous one (the common case when BA runs scan after scan, and what every
   // repetition of a benchmark does) keeps every device buffer: cudaFree/cudaMalloc of several GB cost milliseconds.
-  c->reuse_ws = c->obs && c->stats && c->M == M && c->K == K && (c->fix != nullptr) == with_fix;
+  // A blocks context rebuilds its pattern on every registration: equal M and K do not mean equal co-visibility.
+  c->reuse_ws = c->prec != BALM_PREC_BLOCKS && c->obs && c->stats && c->M == M && c->K == K &&
+                (c->fix != nullptr) == with_fix;
   if (c->reuse_ws) {
     cudaFree(c->csc_ptr); cudaFree(c->csc_obs); cudaFree(c->csc_vox); cudaFree(c->csc_lo); cudaFree(c->csc_hi);
     c->csc_ptr = c->csc_obs = c->csc_vox = c->csc_lo = c->csc_hi = nullptr;
@@ -90,8 +94,8 @@ static int alloc_problem_arrays(balm_ctx *c, int64_t M, int64_t K, bool with_fix
   return BALM_OK;
 }
 
-// Workspaces that depend on the registered problem (batch size, split counts).
-static int alloc_workspaces(balm_ctx *c) {
+// Workspaces that depend on the registered problem (batch size, split counts; the block pattern of a blocks context).
+static int alloc_workspaces_of(balm_ctx *c) {
   if (c->reuse_ws) {  // same shape: batch size, split counts, tensor maps and digit-plane buffers are all unchanged
     c->reuse_ws = false;
     tensor_syrk_new_problem(c);
@@ -99,7 +103,13 @@ static int alloc_workspaces(balm_ctx *c) {
   }
   size_t g_budget = (size_t)16 << 30;  // bytes for the fp64 G' batch
   if (const char *e = getenv("BALM_G_BUDGET_MB")) g_budget = (size_t)atoll(e) << 20;  // tests: force batching
-  int64_t vb = (int64_t)(g_budget / ((size_t)3 * c->ldg * sizeof(double)));
+  const bool blocks = c->prec == BALM_PREC_BLOCKS;
+  if (blocks && (size_t)18 * sizeof(double) * c->K > g_budget) {  // single batch: every observation's G' rows at once
+    free_problem(c);
+    balm_set_error("blocks registration: the per-observation G' rows (144 B per observation) exceed the G' budget");
+    return BALM_ERR_UNSUPPORTED;
+  }
+  int64_t vb = blocks ? c->M : (int64_t)(g_budget / ((size_t)3 * c->ldg * sizeof(double)));
   if (vb > c->M) vb = c->M;
   if (vb < 1) vb = 1;
   c->VB = vb;
@@ -110,11 +120,13 @@ static int alloc_workspaces(balm_ctx *c) {
     TRY(dev_alloc(&c->G, (size_t)3 * vb * c->ldg));
     CUDA_TRY(cudaMemsetAsync(c->G, 0, sizeof(double) * (size_t)3 * vb * c->ldg, c->stream));  // zero the column padding
   }
+  if (blocks) TRY(dev_alloc(&c->G, (size_t)18 * c->K));
   const int tiles_p = (c->N + 31) / 32;
   c->obs_chunks = std::max(1, (c->sm_count * 16 + tiles_p - 1) / tiles_p);
   if (c->obs_chunks > 4096) c->obs_chunks = 4096;
   TRY(dev_alloc(&c->obs_part, (size_t)c->obs_chunks * BALM_ACC * c->Np));
   CUDA_TRY(cudaMemsetAsync(c->obs_part, 0, sizeof(double) * (size_t)c->obs_chunks * BALM_ACC * c->Np, c->stream));
+  if (blocks) return block_hessian_build(c, "blocks registration");
   // SYRK work decomposition: (tile, k-split) items, sized so the last wave is nearly full
   c->syrk_nb = c->ldg / BALM_SYRK_TILE;
   c->syrk_tiles = c->syrk_nb * (c->syrk_nb + 1) / 2;
@@ -151,10 +163,17 @@ static int alloc_workspaces(balm_ctx *c) {
   return BALM_OK;
 }
 
+// A blocks context whose workspaces or pattern could not be built is left without a registration.
+static int alloc_workspaces(balm_ctx *c) {
+  const int rc = alloc_workspaces_of(c);
+  if (rc != BALM_OK && c->prec == BALM_PREC_BLOCKS) free_problem(c);
+  return rc;
+}
+
 // ---------------- ctx ----------------
 extern "C" int balm_create(balm_ctx **out, int n_poses, int device, int precision) {
   if (!out || n_poses < 1) { balm_set_error("balm_create: bad arguments"); return BALM_ERR_INVALID; }
-  if (precision != BALM_PREC_FP64 && precision != BALM_PREC_TENSOR) {
+  if (precision != BALM_PREC_FP64 && precision != BALM_PREC_TENSOR && precision != BALM_PREC_BLOCKS) {
     balm_set_error("balm_create: unknown precision mode");
     return BALM_ERR_INVALID;
   }
@@ -182,9 +201,13 @@ extern "C" int balm_create(balm_ctx **out, int n_poses, int device, int precisio
   const size_t n = c->n;
   TRY(dev_alloc(&c->poses, 12 * (size_t)c->N));
   TRY(dev_alloc(&c->poses_trial, 12 * (size_t)c->N));
-  TRY(dev_alloc(&c->H, n * n + n + 8));
-  c->g = c->H + n * n;
-  TRY(dev_alloc(&c->A, n * n));
+  if (precision == BALM_PREC_BLOCKS) {  // nothing of size n^2
+    TRY(dev_alloc(&c->g, n + 8));
+  } else {
+    TRY(dev_alloc(&c->H, n * n + n + 8));
+    c->g = c->H + n * n;
+    TRY(dev_alloc(&c->A, n * n));
+  }
   TRY(dev_alloc(&c->dx, n));
   TRY(dev_alloc(&c->dvec, n));
   TRY(dev_alloc(&c->scal, 32));
@@ -212,6 +235,7 @@ extern "C" int balm_destroy(balm_ctx *c) {
   window_free(c->win);
   pose_graph_free(c->pg);
   if (c->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(c->comm);
+  if (c->prec == BALM_PREC_BLOCKS) cudaFree(c->g);
   cudaFree(c->poses); cudaFree(c->poses_trial); cudaFree(c->H); cudaFree(c->A);
   cudaFree(c->dx); cudaFree(c->dvec); cudaFree(c->scal); cudaFree(c->flags); cudaFree(c->accum); cudaFree(c->accum_batch);
   cudaFree(c->vox_key); cudaFree(c->vox_layer); cudaFree(c->res_part); cudaFree(c->planes); cudaFree(c->Xinv); cudaFree(c->dinv); cudaFree(c->sol); cudaFree(c->ysol);
@@ -264,6 +288,8 @@ static int finish_registration(balm_ctx *c) {
   CUDA_TRY(cudaMemsetAsync(d_out, 0, sizeof(int) * 4, c->stream));
   CUDA_TRY(cudaMemsetAsync(d_planes, 0, sizeof(int) * N, c->stream));
   csr_check_kernel<<<(unsigned)((M + 127) / 128), 128, 0, c->stream>>>(c->row_ptr, c->pose_idx, M, N, d_out);
+  if (sizeof(int) * N > 48 * 1024)  // a blocks context can hold more poses than the default shared-memory limit covers
+    CUDA_TRY(cudaFuncSetAttribute(pose_hist_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(int) * N));
   pose_hist_kernel<<<c->sm_count * 4, 256, sizeof(int) * N, c->stream>>>(c->pose_idx, c->K, N, d_planes);
   c->launches += 2;
   int h_out[4];
@@ -324,6 +350,7 @@ static int register_empty(balm_ctx *c) {
   free_problem(c);
   CUDA_TRY(cudaMemsetAsync(c->planes, 0, sizeof(int) * c->N, c->stream));
   c->dense = true; c->max_k = 0; c->min_planes = 0; c->VB = 0;
+  if (c->prec == BALM_PREC_BLOCKS) TRY(block_hessian_build(c, "blocks registration"));  // every diagonal pair, no term
   c->registered = true;
   return BALM_OK;
 }
@@ -556,7 +583,12 @@ static int evaluate_dev(balm_ctx *c, const double *poses, int64_t head, int64_t 
   c->pending_stats_cached = stats_cached;
   if (head == end) {  // empty range (or an empty shard): this rank contributes H = 0, g = 0, r = 0 -- and still enters
     // the all-reduce below, which the other ranks of a multi-GPU job are waiting in
-    CUDA_TRY(cudaMemsetAsync(c->H, 0, sizeof(double) * ((size_t)c->n * c->n + c->n + 1), c->stream));
+    if (c->prec == BALM_PREC_BLOCKS) {
+      TRY(blocks_zero(c));
+      CUDA_TRY(cudaMemsetAsync(c->g, 0, sizeof(double) * ((size_t)c->n + 1), c->stream));
+    } else {
+      CUDA_TRY(cudaMemsetAsync(c->H, 0, sizeof(double) * ((size_t)c->n * c->n + c->n + 1), c->stream));
+    }
     for (int e = 0; e <= 5; e++) CUDA_TRY(cudaEventRecord(c->ev[e], c->stream));
   }
   for (int64_t v0 = head; v0 < end; v0 += c->VB) {
@@ -571,7 +603,8 @@ static int evaluate_dev(balm_ctx *c, const double *poses, int64_t head, int64_t 
     } else {
       TRY(launch_obs_pass(c, poses, v0, v1, first));
       CUDA_TRY(cudaEventRecord(c->ev[2], c->stream));
-      TRY(launch_syrk_f64(c, 3 * (v1 - v0), first));
+      if (c->prec == BALM_PREC_BLOCKS) TRY(launch_blocks(c, v0, v1));  // single batch: the blocks and g, no assembly
+      else TRY(launch_syrk_f64(c, 3 * (v1 - v0), first));
     }
     CUDA_TRY(cudaEventRecord(c->ev[3], c->stream));
     if (deferred) {
@@ -589,7 +622,7 @@ static int evaluate_dev(balm_ctx *c, const double *poses, int64_t head, int64_t 
   CUDA_TRY(cudaMemcpyAsync(c->scal + BALM_SCAL_RCUR, r_dev, sizeof(double), cudaMemcpyDeviceToDevice, c->stream));  // local, pre all-reduce
   if (end > head) {
     CUDA_TRY(cudaEventRecord(c->ev[4], c->stream));
-    TRY(launch_assemble(c));
+    if (c->prec != BALM_PREC_BLOCKS) TRY(launch_assemble(c));
     CUDA_TRY(cudaEventRecord(c->ev[5], c->stream));
   }
   if (c->world > 1 && c->comm) {  // the assembly wrote the lower triangle | g into c->Hpack (an empty range: zeros)
@@ -608,7 +641,8 @@ static int evaluate_dev(balm_ctx *c, const double *poses, int64_t head, int64_t 
     return BALM_OK;
   }
   CUDA_TRY(cudaEventSynchronize(c->ev[6]));
-  cudaEventElapsedTime(&ms, c->ev[4], c->ev[5]); c->tm.ms_assemble += ms;
+  cudaEventElapsedTime(&ms, c->ev[4], c->ev[5]);
+  if (c->prec != BALM_PREC_BLOCKS) c->tm.ms_assemble += ms;
   cudaEventElapsedTime(&ms, c->ev[5], c->ev[6]); c->tm.ms_allreduce += ms;
   c->tm.n_eval += 1;
   return BALM_OK;
@@ -623,7 +657,8 @@ static int collect_eval(balm_ctx *c) {
   if (!c->pending_stats_cached) { c->tm.ms_stats += ms; c->tm.n_stats += 1; }
   cudaEventElapsedTime(&ms, c->ev[1], c->ev[2]); c->tm.ms_obs += ms;
   cudaEventElapsedTime(&ms, c->ev[2], c->ev[3]); c->tm.ms_syrk += ms;
-  cudaEventElapsedTime(&ms, c->ev[4], c->ev[5]); c->tm.ms_assemble += ms;
+  cudaEventElapsedTime(&ms, c->ev[4], c->ev[5]);
+  if (c->prec != BALM_PREC_BLOCKS) c->tm.ms_assemble += ms;
   cudaEventElapsedTime(&ms, c->ev[5], c->ev[6]); c->tm.ms_allreduce += ms;
   c->tm.n_eval += 1;
   if (c->prec == BALM_PREC_TENSOR) return tensor_syrk_check_finish(c);
@@ -649,6 +684,25 @@ static int residual_dev(balm_ctx *c, const double *poses, double *host_out, bool
   return BALM_OK;
 }
 
+// A blocks context's H as the dense column-major n x n matrix of its blocks (zeros elsewhere), on the host (waits).
+static int blocks_to_dense(balm_ctx *c, double *H) {
+  const std::vector<int2> &pr = blocks_pairs(c->bh);
+  std::vector<double> b(36 * pr.size());
+  CUDA_TRY(cudaMemcpyAsync(b.data(), blocks_device(c->bh), sizeof(double) * b.size(), cudaMemcpyDeviceToHost, c->stream));
+  CUDA_TRY(cudaStreamSynchronize(c->stream));
+  const size_t n = c->n;
+  std::fill(H, H + n * n, 0.0);
+  for (size_t p = 0; p < pr.size(); p++)
+    for (int col = 0; col < 6; col++)
+      for (int row = 0; row < 6; row++) {
+        const double h = b[36 * p + 6 * col + row];
+        const size_t r = 6 * (size_t)pr[p].x + row, cc = 6 * (size_t)pr[p].y + col;
+        H[cc * n + r] = h;
+        H[r * n + cc] = h;
+      }
+  return BALM_OK;
+}
+
 extern "C" int balm_evaluate(balm_ctx *c, const double *poses12, int64_t head, int64_t end, int include_fix,
                              double *H, double *g, double *residual) {
   if (!c || !poses12) { balm_set_error("balm_evaluate: bad arguments"); return BALM_ERR_INVALID; }
@@ -656,7 +710,8 @@ extern "C" int balm_evaluate(balm_ctx *c, const double *poses12, int64_t head, i
   CUDA_TRY(cudaMemcpyAsync(c->poses, poses12, sizeof(double) * 12 * c->N, cudaMemcpyHostToDevice, c->stream));
   TRY(evaluate_dev(c, c->poses, head, end, include_fix != 0));
   const size_t n = c->n;
-  if (H) CUDA_TRY(cudaMemcpyAsync(H, c->H, sizeof(double) * n * n, cudaMemcpyDeviceToHost, c->stream));
+  if (H && c->prec == BALM_PREC_BLOCKS) TRY(blocks_to_dense(c, H));
+  else if (H) CUDA_TRY(cudaMemcpyAsync(H, c->H, sizeof(double) * n * n, cudaMemcpyDeviceToHost, c->stream));
   if (g) CUDA_TRY(cudaMemcpyAsync(g, c->g, sizeof(double) * n, cudaMemcpyDeviceToHost, c->stream));
   CUDA_TRY(cudaMemcpyAsync(c->h_scal, c->scal, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
   CUDA_TRY(cudaStreamSynchronize(c->stream));
@@ -688,7 +743,8 @@ static int maybe_refine(balm_ctx *c, double *q1, int *not_pd, int *refined) {
   *refined = 0;
   if (c->h_flags[4] == 0 || *not_pd) return BALM_OK;
   int still_bad = 0;
-  TRY(refine_solution(c, &still_bad));
+  if (c->prec == BALM_PREC_BLOCKS) TRY(blocks_refine(c, &still_bad));
+  else TRY(refine_solution(c, &still_bad));
   *q1 = c->h_scal[1];
   *refined = 1;
   if (still_bad || !std::isfinite(*q1)) *not_pd = 1;
@@ -697,7 +753,8 @@ static int maybe_refine(balm_ctx *c, double *q1, int *not_pd, int *refined) {
 
 static int solve_dev(balm_ctx *c, double u, double *q1, int *not_pd) {
   CUDA_TRY(cudaEventRecord(c->ev[9], c->stream));
-  TRY(launch_ldlt_solve(c, u));
+  if (c->prec == BALM_PREC_BLOCKS) TRY(blocks_solve(c, u));
+  else TRY(launch_ldlt_solve(c, u));
   CUDA_TRY(cudaEventRecord(c->ev[10], c->stream));
   CUDA_TRY(cudaMemcpyAsync(c->h_scal + 1, c->scal + 1, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
   CUDA_TRY(cudaMemcpyAsync(c->h_flags, c->flags, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
@@ -887,6 +944,7 @@ static int pose_factors_check(const char *who, int P, int n_factors, const int64
 extern "C" int balm_set_pose_factors(balm_ctx *c, int n_factors, const int64_t *factor_ptr, const int32_t *factor_pose,
                                      const double *poses_hat12, const double *H, int32_t *status_out) {
   if (!c) { balm_set_error("balm_set_pose_factors: bad arguments"); return BALM_ERR_INVALID; }
+  TRY(refuse_blocks(c, "balm_set_pose_factors"));
   TRY(pose_factors_check("balm_set_pose_factors", c->N, n_factors, factor_ptr, factor_pose, poses_hat12, H));
   CUDA_TRY(cudaSetDevice(c->device));
   return pose_graph_set(c, n_factors, factor_ptr, factor_pose, poses_hat12, H, status_out);
@@ -894,6 +952,7 @@ extern "C" int balm_set_pose_factors(balm_ctx *c, int n_factors, const int64_t *
 
 extern "C" int balm_pose_graph_evaluate(balm_ctx *c, const double *poses12, double *H, double *g, double *cost) {
   if (!c || !poses12) { balm_set_error("balm_pose_graph_evaluate: bad arguments"); return BALM_ERR_INVALID; }
+  TRY(refuse_blocks(c, "balm_pose_graph_evaluate"));
   if (!c->pg) { balm_set_error("balm_pose_graph_evaluate: no pose factors registered"); return BALM_ERR_INVALID; }
   CUDA_TRY(cudaSetDevice(c->device));
   CUDA_TRY(cudaMemcpyAsync(c->poses, poses12, sizeof(double) * 12 * c->N, cudaMemcpyHostToDevice, c->stream));
@@ -989,6 +1048,7 @@ static int pose_graph_lm(const PoseGraphLm &s, double *poses12, const balm_lm_op
 extern "C" int balm_pose_graph_iter(balm_ctx *c, double *poses12, const balm_lm_opts *o, balm_trace *trace, int *n_iters,
                                     double *poses_per_iter) {
   if (!c || !poses12 || !o) { balm_set_error("balm_pose_graph_iter: bad arguments"); return BALM_ERR_INVALID; }
+  TRY(refuse_blocks(c, "balm_pose_graph_iter"));
   if (n_iters) *n_iters = 0;
   if (c->world > 1 || c->comm) { balm_set_error("balm_pose_graph_iter: single-GPU contexts only"); return BALM_ERR_INVALID; }
   if (!c->pg) { balm_set_error("balm_pose_graph_iter: no pose factors registered"); return BALM_ERR_INVALID; }
@@ -1081,7 +1141,8 @@ extern "C" int balm_spg_set_factors(balm_spg *s, int n_factors, const int64_t *f
   TRY(dev_alloc(&blocks, 36 * pairs.size()));
   std::unique_ptr<double, cudaError_t (*)(void *)> blocks_own(blocks, cudaFree);
   SparseSolver *solver = nullptr;
-  TRY(sparse_solver_build(s->stream, s->N, pairs, blocks, s->g, s->dvec, s->dx, s->scal, s->flags, &solver));
+  TRY(sparse_solver_build(s->stream, s->N, pairs, blocks, s->g, s->dvec, s->dx, s->scal, s->flags, "balm_spg_set_factors",
+                          &solver));
   if (status_out) std::copy(status.begin(), status.end(), status_out);
   sparse_solver_free(s->solver);
   pose_graph_free(s->pg);
@@ -1326,6 +1387,7 @@ int balm_cov_evaluate_hessian(balm_ctx *c, const double *poses_dev, bool include
 extern "C" int balm_pose_covariance(balm_ctx *c, const double *poses12, const double *c_cov81, double point_noise,
                                     int include_fix, double *Rcov_raw, double *Rcov) {
   if (!c || !poses12 || (!Rcov_raw && !Rcov)) { balm_set_error("balm_pose_covariance: bad arguments"); return BALM_ERR_INVALID; }
+  TRY(refuse_blocks(c, "balm_pose_covariance"));
   if (!c->registered || c->M < 1) { balm_set_error("balm_pose_covariance: no voxels registered"); return BALM_ERR_INVALID; }
   if (c->world > 1) { balm_set_error("balm_pose_covariance: single-GPU contexts only"); return BALM_ERR_UNSUPPORTED; }
   CUDA_TRY(cudaSetDevice(c->device));
@@ -1346,6 +1408,7 @@ extern "C" int balm_comm_unique_id(void *out128) {
 
 extern "C" int balm_comm_init(balm_ctx *c, int rank, int world, const void *unique_id128) {
   if (!c || world < 1 || rank < 0 || rank >= world) { balm_set_error("balm_comm_init: bad arguments"); return BALM_ERR_INVALID; }
+  TRY(refuse_blocks(c, "balm_comm_init"));
   c->rank = rank; c->world = world;
   if (world == 1) return BALM_OK;
   if (!unique_id128) { balm_set_error("balm_comm_init: unique id required"); return BALM_ERR_INVALID; }
@@ -1410,7 +1473,40 @@ extern "C" int balm_debug_dag_trace(balm_ctx *c, unsigned long long *out, int ma
 
 extern "C" int balm_device_views(balm_ctx *c, double **H_dev, double **g_dev) {
   if (!c) return BALM_ERR_INVALID;
+  TRY(refuse_blocks(c, "balm_device_views"));
   if (H_dev) *H_dev = c->H;
   if (g_dev) *g_dev = c->g;
+  return BALM_OK;
+}
+
+// ---------------- block-sparse Hessian (blocks.cu) ----------------
+extern "C" int balm_block_structure(balm_ctx *c, int64_t stats[4], int32_t *pairs) {
+  if (!c || !stats) { balm_set_error("balm_block_structure: bad arguments"); return BALM_ERR_INVALID; }
+  if (c->prec != BALM_PREC_BLOCKS || !c->bh) {
+    balm_set_error("balm_block_structure: no voxels registered on a BALM_PREC_BLOCKS context");
+    return BALM_ERR_INVALID;
+  }
+  const std::vector<int2> &pr = blocks_pairs(c->bh);
+  stats[0] = (int64_t)pr.size();
+  const size_t N = c->N, n = c->n, K = c->K, M = c->M;
+  const size_t dbl = 18 * K + 10 * (size_t)c->Kp + (c->fix ? 10 * M : 0) + M + 2 * M * BALM_STATS_STRIDE + 10 * M +
+                     (size_t)(c->obs_chunks + 2) * BALM_ACC * c->Np + 24 * N + 3 * n + 8 + 32 + c->res_blocks;
+  const size_t ints = K + (M + 1) * 2 + 2 * N + 8 + (c->csc_ptr ? 2 * K + 3 * N + 1 : 0);
+  stats[3] = blocks_bytes(c->bh, &stats[1], &stats[2]) + (int64_t)(sizeof(double) * dbl + sizeof(int) * ints);
+  if (pairs)
+    for (size_t p = 0; p < pr.size(); p++) { pairs[2 * p] = pr[p].x; pairs[2 * p + 1] = pr[p].y; }
+  return BALM_OK;
+}
+
+extern "C" int balm_download_blocks(balm_ctx *c, double *blocks) {
+  if (!c || !blocks) { balm_set_error("balm_download_blocks: bad arguments"); return BALM_ERR_INVALID; }
+  if (c->prec != BALM_PREC_BLOCKS || !c->bh) {
+    balm_set_error("balm_download_blocks: no voxels registered on a BALM_PREC_BLOCKS context");
+    return BALM_ERR_INVALID;
+  }
+  CUDA_TRY(cudaSetDevice(c->device));
+  const size_t nbl = 36 * blocks_pairs(c->bh).size();
+  CUDA_TRY(cudaMemcpyAsync(blocks, blocks_device(c->bh), sizeof(double) * nbl, cudaMemcpyDeviceToHost, c->stream));
+  CUDA_TRY(cudaStreamSynchronize(c->stream));
   return BALM_OK;
 }

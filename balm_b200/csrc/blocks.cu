@@ -1,0 +1,259 @@
+// blocks.cu -- the block-sparse Hessian of a BALM_PREC_BLOCKS context (DESIGN.md "Block-sparse voxel BA").
+// H is held as the 6x6 blocks of the pose pairs (i <= j) that share at least one voxel, plus every diagonal pair (i, i);
+// the damped system is solved by the sparse pose graph's nested-dissection block LDL^T (pose_graph_sparse.cu).
+// Nothing of size (6N)^2 exists.
+//   Registration (block_hessian_build, every registration route ends here): every voxel emits its k(k+1)/2 observation
+//   pairs keyed by their pose pair; one stable radix sort by key gives the unique pose pairs (run-length encoding) and,
+//   for each, its update terms in ascending voxel order -- the fixed summation order of the evaluation.
+//   Evaluation: the observation sweep (obs_pass_kernel<..., OBS_BLOCKS>) stores every observation's three scaled G' rows
+//   (18 doubles) instead of the dense G'; blocks_kernel sums, per pair, the terms' outer products, one warp per pair,
+//   lane l taking the terms l, l + 32, ... and the lanes' sums meeting in warp_sum's fixed butterfly. The block is minus
+//   that sum, plus the observation sweep's diagonal block on a diagonal pair. fp64 throughout, no floating-point atomics.
+#include <cub/cub.cuh>
+#include <algorithm>
+#include <memory>
+#include <vector>
+#include "internal.cuh"
+
+struct BlockHessian {
+  std::vector<int2> pairs;           // host: (i, j), i <= j, ascending
+  long long nterm = 0, bytes = 0;
+  int2 *pair_dev = nullptr;          // [pairs]
+  long long *tptr = nullptr;         // [pairs + 1] terms of pair p: term[tptr[p] .. tptr[p+1])
+  unsigned long long *term = nullptr;  // [nterm] observation of pose i (low word) | of pose j (high word), voxel-ascending
+  double *blocks = nullptr;          // [pairs][36] column-major, rows of pose i
+  SparseSolver *solver = nullptr;
+  ~BlockHessian() {
+    sparse_solver_free(solver);
+    cudaFree(pair_dev); cudaFree(tptr); cudaFree(term); cudaFree(blocks);
+  }
+};
+
+void block_hessian_free(BlockHessian *b) { delete b; }
+
+namespace {
+
+__global__ void pair_count_kernel(const long long *row_ptr, int64_t M, long long *cnt) {
+  const int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (v > M) return;
+  const long long k = v < M ? row_ptr[v + 1] - row_ptr[v] : 0;
+  cnt[v] = k * (k + 1) / 2;
+}
+
+// one warp per voxel: the pairs (a, b), a <= b, of its observations, a-major, at the voxel's offset
+__global__ void pair_emit_kernel(const long long *row_ptr, const int *pose_idx, int64_t M, int N, const long long *off,
+                                 unsigned long long *key, unsigned long long *val) {
+  const int64_t v = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (v >= M) return;
+  const long long s0 = row_ptr[v];
+  const int k = (int)(row_ptr[v + 1] - s0);
+  long long o = off[v];
+  for (int a = 0; a < k; a++) {
+    const int pa = pose_idx[s0 + a];
+    for (int b = a + lane; b < k; b += 32) {
+      key[o + b - a] = (unsigned long long)pa * N + pose_idx[s0 + b];
+      val[o + b - a] = (unsigned long long)(unsigned)(s0 + a) | ((unsigned long long)(unsigned)(s0 + b) << 32);
+    }
+    o += k - a;
+  }
+}
+
+// One warp per pair: block = -sum_terms sum_rr Gs[s_i][rr] Gs[s_j][rr]^T (+ the diagonal block D_i on a diagonal pair),
+// terms restricted to the observations [row_ptr[head], row_ptr[end]) (voxels [head, end)). Threads t < n also copy g.
+__global__ void __launch_bounds__(256) blocks_kernel(const int2 *pairs, const long long *tptr,
+                                                     const unsigned long long *term, long long npairs, const double *Gs,
+                                                     const long long *row_ptr, int64_t head, int64_t end,
+                                                     const double *accum, int Np, int n, double *blocks, double *g) {
+  const long long gt = (long long)blockIdx.x * 256 + threadIdx.x;
+  if (gt < n) g[gt] = accum[(size_t)(gt % 6) * Np + gt / 6];
+  const long long p = gt >> 5;
+  const int lane = threadIdx.x & 31;
+  if (p >= npairs) return;
+  const unsigned lo = (unsigned)row_ptr[head], hi = (unsigned)row_ptr[end];
+  // the pair's terms are voxel-ascending, so their first observation index is too: [t0, t1) = those inside the range
+  long long t0 = tptr[p], t1 = tptr[p + 1];
+  {
+    long long l = t0, h = t1;
+    while (l < h) { const long long m = (l + h) >> 1; if ((unsigned)term[m] < lo) l = m + 1; else h = m; }
+    t0 = l;
+    h = t1;
+    while (l < h) { const long long m = (l + h) >> 1; if ((unsigned)term[m] < hi) l = m + 1; else h = m; }
+    t1 = l;
+  }
+  double acc[36];
+#pragma unroll
+  for (int e = 0; e < 36; e++) acc[e] = 0.0;
+  for (long long t = t0 + lane; t < t1; t += 32) {
+    const unsigned long long w = term[t];
+    const double2 *gi = reinterpret_cast<const double2 *>(Gs + 18 * (size_t)(unsigned)w);
+    const double2 *gj = reinterpret_cast<const double2 *>(Gs + 18 * (size_t)(unsigned)(w >> 32));
+#pragma unroll
+    for (int rr = 0; rr < 3; rr++) {
+      double a[6], b[6];
+#pragma unroll
+      for (int h = 0; h < 3; h++) {
+        const double2 x = __ldg(gi + 3 * rr + h), y = __ldg(gj + 3 * rr + h);
+        a[2 * h] = x.x; a[2 * h + 1] = x.y;
+        b[2 * h] = y.x; b[2 * h + 1] = y.y;
+      }
+#pragma unroll
+      for (int c = 0; c < 6; c++)
+#pragma unroll
+        for (int r = 0; r < 6; r++) acc[6 * c + r] = fma(a[r], b[c], acc[6 * c + r]);
+    }
+  }
+  const int2 pr = pairs[p];
+  double *B = blocks + 36 * (size_t)p;
+#pragma unroll
+  for (int e = 0; e < 36; e++) {
+    double h = -warp_sum(acc[e]);
+    if (lane == (e & 31)) {
+      if (pr.x == pr.y) {  // assemble_kernel's D block: upper triangle, row-major, index q of (min, max)
+        const int r = e % 6, c = e / 6, r6 = r < c ? r : c, c6 = r < c ? c : r;
+        const int q = r6 * 6 - r6 * (r6 - 1) / 2 + (c6 - r6);
+        h += accum[(size_t)(6 + q) * Np + pr.x];
+      }
+      B[e] = h;
+    }
+  }
+}
+
+}  // namespace
+
+int block_hessian_build(balm_ctx *c, const char *who) {
+  const int N = c->N;
+  const int64_t M = c->M;
+  cudaStream_t st = c->stream;
+  ScratchPool pool;
+  std::unique_ptr<BlockHessian> bh(new BlockHessian());
+  auto refuse = [&](const char *what) {
+    balm_set_error(std::string(who) + ": " + what);
+    return (int)BALM_ERR_UNSUPPORTED;
+  };
+  std::vector<unsigned long long> ukey;
+  std::vector<int> ucnt;
+  if (M > 0) {
+    long long *cnt = nullptr, *off = nullptr;
+    TRY(pool.get(&cnt, (size_t)M + 1));
+    TRY(pool.get(&off, (size_t)M + 1));
+    pair_count_kernel<<<(unsigned)((M + 1 + 255) / 256), 256, 0, st>>>(c->row_ptr, M, cnt);
+    size_t tb = 0;
+    CUDA_TRY(cub::DeviceScan::ExclusiveSum(nullptr, tb, cnt, off, M + 1, st));
+    char *tmp = nullptr;
+    TRY(pool.get(&tmp, tb));
+    CUDA_TRY(cub::DeviceScan::ExclusiveSum(tmp, tb, cnt, off, M + 1, st));
+    long long nterm = 0;
+    CUDA_TRY(cudaMemcpyAsync(&nterm, off + M, sizeof(long long), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    pool.drop(tmp);
+    pool.drop(cnt);
+    if (nterm >= (1LL << 31)) return refuse("2^31 or more observation pairs (block update terms)");
+    bh->nterm = nterm;
+    // key: pose pair i * N + j, value: the two observations; one stable sort by key
+    unsigned long long *k0 = nullptr, *k1 = nullptr, *v0 = nullptr, *v1 = nullptr;
+    TRY(pool.get(&k0, (size_t)nterm)); TRY(pool.get(&k1, (size_t)nterm));
+    TRY(pool.get(&v0, (size_t)nterm)); TRY(pool.get(&v1, (size_t)nterm));
+    pair_emit_kernel<<<(unsigned)((M * 32 + 255) / 256), 256, 0, st>>>(c->row_ptr, c->pose_idx, M, N, off, k0, v0);
+    int bits = 1;
+    while (bits < 64 && ((unsigned long long)1 << bits) < (unsigned long long)N * N) bits++;
+    cub::DoubleBuffer<unsigned long long> dk(k0, k1), dv(v0, v1);
+    tb = 0;
+    CUDA_TRY(cub::DeviceRadixSort::SortPairs(nullptr, tb, dk, dv, (int)nterm, 0, bits, st));
+    TRY(pool.get(&tmp, tb));
+    CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, tb, dk, dv, (int)nterm, 0, bits, st));
+    pool.drop(tmp);
+    // unique pose pairs and their term counts, into the sort's spare buffers
+    unsigned long long *uk = dk.Alternate();
+    int *uc = reinterpret_cast<int *>(dv.Alternate()), *nruns = nullptr;
+    TRY(pool.get(&nruns, 1));
+    tb = 0;
+    CUDA_TRY(cub::DeviceRunLengthEncode::Encode(nullptr, tb, dk.Current(), uk, uc, nruns, (int)nterm, st));
+    TRY(pool.get(&tmp, tb));
+    CUDA_TRY(cub::DeviceRunLengthEncode::Encode(tmp, tb, dk.Current(), uk, uc, nruns, (int)nterm, st));
+    int nr = 0;
+    CUDA_TRY(cudaMemcpyAsync(&nr, nruns, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    if (nr + (long long)N >= (1LL << 30)) return refuse("2^30 or more block pairs");
+    ukey.resize(nr);
+    ucnt.resize(nr);
+    CUDA_TRY(cudaMemcpyAsync(ukey.data(), uk, sizeof(unsigned long long) * nr, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(ucnt.data(), uc, sizeof(int) * nr, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    CUDA_TRY(cudaGetLastError());
+    c->launches += 5;
+    // keep the sorted terms, free everything else
+    bh->term = dv.Current();
+    pool.release(bh->term);
+  }
+  // the pairs with every diagonal pair added (a pose in no voxel gets a zero block, hence a zero pivot)
+  std::vector<long long> tptr;
+  bh->pairs.reserve(ukey.size() + N);
+  tptr.reserve(ukey.size() + N + 1);
+  tptr.push_back(0);
+  size_t q = 0;
+  for (int i = 0; i < N; i++) {
+    const unsigned long long diag = (unsigned long long)i * N + i;
+    if (q == ukey.size() || ukey[q] != diag) {
+      bh->pairs.push_back(make_int2(i, i));
+      tptr.push_back(tptr.back());
+    }
+    for (; q < ukey.size() && ukey[q] < (unsigned long long)(i + 1) * N; q++) {
+      bh->pairs.push_back(make_int2(i, (int)(ukey[q] - (unsigned long long)i * N)));
+      tptr.push_back(tptr.back() + ucnt[q]);
+    }
+  }
+  const size_t np = bh->pairs.size();
+  TRY(dev_alloc(&bh->pair_dev, np));
+  TRY(dev_alloc(&bh->tptr, np + 1));
+  TRY(dev_alloc(&bh->blocks, 36 * np));
+  CUDA_TRY(cudaMemcpyAsync(bh->pair_dev, bh->pairs.data(), sizeof(int2) * np, cudaMemcpyHostToDevice, st));
+  CUDA_TRY(cudaMemcpyAsync(bh->tptr, tptr.data(), sizeof(long long) * (np + 1), cudaMemcpyHostToDevice, st));
+  CUDA_TRY(cudaMemsetAsync(bh->blocks, 0, sizeof(double) * 36 * np, st));
+  TRY(sparse_solver_build(st, N, bh->pairs, bh->blocks, c->g, c->dvec, c->dx, c->scal, c->flags, who, &bh->solver));
+  bh->bytes = (long long)(np * (sizeof(int2) + sizeof(long long) + 36 * sizeof(double)) + sizeof(long long) +
+                          sizeof(unsigned long long) * bh->nterm);
+  block_hessian_free(c->bh);
+  c->bh = bh.release();
+  return BALM_OK;
+}
+
+int launch_blocks(balm_ctx *c, int64_t head, int64_t end) {
+  const BlockHessian *b = c->bh;
+  const long long np = (long long)b->pairs.size();
+  const long long threads = std::max<long long>(32 * np, c->n);
+  blocks_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, c->stream>>>(b->pair_dev, b->tptr, b->term, np, c->G,
+                                                                          c->row_ptr, head, end, c->accum, c->Np, c->n,
+                                                                          b->blocks, c->g);
+  c->launches += 1;
+  CUDA_TRY(cudaGetLastError());
+  return BALM_OK;
+}
+
+int blocks_zero(balm_ctx *c) {
+  CUDA_TRY(cudaMemsetAsync(c->bh->blocks, 0, sizeof(double) * 36 * c->bh->pairs.size(), c->stream));
+  return BALM_OK;
+}
+
+int blocks_solve(balm_ctx *c, double u) {
+  c->h_scal[3] = u;  // pinned; the kernels read the damping factor from device memory
+  CUDA_TRY(cudaMemcpyAsync(c->scal + 3, c->h_scal + 3, sizeof(double), cudaMemcpyHostToDevice, c->stream));
+  TRY(sparse_solve(c->bh->solver, c->stream));
+  c->launches += 1;
+  return BALM_OK;
+}
+
+int blocks_refine(balm_ctx *c, int *still_bad) {
+  TRY(sparse_refine(c->bh->solver, c->stream, c->h_flags, c->h_scal, still_bad));
+  c->tm.refinements += 1;
+  return BALM_OK;
+}
+
+const std::vector<int2> &blocks_pairs(const BlockHessian *b) { return b->pairs; }
+const double *blocks_device(const BlockHessian *b) { return b->blocks; }
+
+long long blocks_bytes(const BlockHessian *b, int64_t *l_blocks, int64_t *levels) {
+  int64_t sb = 0;
+  sparse_solver_stats(b->solver, l_blocks, levels, &sb);
+  return b->bytes + sb;
+}

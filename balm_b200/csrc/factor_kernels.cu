@@ -151,7 +151,7 @@ struct ObsArgs {
 
 // One lane = one pose; a warp covers 32 consecutive poses and walks a chunk of voxels, so the observation
 // loads of a dense scene (slot j == pose j) are coalesced and the 27 accumulators stay in registers.
-enum { OBS_FP64 = 0, OBS_MAXONLY = 1, OBS_INT8 = 2, OBS_FUSED = 3 };
+enum { OBS_FP64 = 0, OBS_MAXONLY = 1, OBS_INT8 = 2, OBS_FUSED = 3, OBS_BLOCKS = 4 };
 constexpr int OBS_STAGES = 4;  // cp.async ring depth of the dense sweep (iterations in flight per warp)
 // MODE: OBS_FP64    writes fp64 G' + gradient / diagonal blocks                          [fp64 SYRK path]
 //       OBS_MAXONLY first sweep of the tensor path: column maxima of G' (-> power-of-two column scales) and the
@@ -162,6 +162,8 @@ constexpr int OBS_STAGES = 4;  // cp.async ring depth of the dense sweep (iterat
 //                   step moves the column maxima by far less than the factor 2 of headroom a balanced top digit
 //                   has); tc_scale_kernel checks the new maxima against the scales used and, if a column overflowed
 //                   or lost precision, re-arms the OBS_INT8 sweep (which otherwise returns at once)
+//       OBS_BLOCKS  the three scaled G' rows of every observation into a.G[s][18] (s: the observation's CSR index) +
+//                   gradient / diagonal blocks                                        [block-sparse path, blocks.cu]
 template <bool DENSE, int MODE, int WPC = 4, int MINB = 2>
 __global__ void __launch_bounds__(WPC * 32, MINB) obs_pass_kernel(ObsArgs a) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -271,8 +273,17 @@ __global__ void __launch_bounds__(WPC * 32, MINB) obs_pass_kernel(ObsArgs a) {
         st[2 * c + 1] = x.y;
       }
     }
-    // ---- G' rows of this observation (emitted as fp64 / digit planes / column maxima), then its gradient and
-    // diagonal-block terms (obs_terms) ----
+    // ---- G' rows of this observation (emitted as fp64 / digit planes / column maxima / per-observation rows), then its
+    // gradient and diagonal-block terms (obs_terms) ----
+    if constexpr (MODE == OBS_BLOCKS) {
+      double2 *qd = reinterpret_cast<double2 *>(a.G + 18 * (size_t)(DENSE ? v * a.N + i : a.csc_obs[t]));
+      obs_terms<true>(o, r, p, st, acc, [&](const double (&gv)[3][6]) {
+#pragma unroll
+        for (int rr = 0; rr < 3; rr++)
+#pragma unroll
+          for (int h = 0; h < 3; h++) qd[3 * rr + h] = make_double2(gv[rr][2 * h], gv[rr][2 * h + 1]);
+      });
+    } else {
     obs_terms<MODE != OBS_INT8>(o, r, p, st, acc, [&](const double (&gv)[3][6]) {
       if (MODE == OBS_FP64) {
         double *g0 = a.G + (size_t)(3 * (v - a.v0)) * a.ldg + 6 * i;
@@ -317,6 +328,7 @@ __global__ void __launch_bounds__(WPC * 32, MINB) obs_pass_kernel(ObsArgs a) {
         }
       }
     });
+    }
   }
   if (MODE != OBS_INT8 && active && a.colmax) {
 #pragma unroll
@@ -392,7 +404,7 @@ static void obs_fill(balm_ctx *c, ObsArgs &a, const double *poses, int64_t v0, i
   a.colmax = c->colmax;
 }
 
-// fp64 SYRK path: one sweep writing fp64 G' (+ gradient / diagonal blocks).
+// fp64 SYRK path: one sweep writing fp64 G' (+ gradient / diagonal blocks); block-sparse path: the per-observation rows.
 int launch_obs_pass(balm_ctx *c, const double *poses, int64_t v0, int64_t v1, bool first_batch) {
   const int64_t nv = v1 - v0;
   if (nv <= 0) return BALM_OK;
@@ -401,10 +413,15 @@ int launch_obs_pass(balm_ctx *c, const double *poses, int64_t v0, int64_t v1, bo
   a.colmax = nullptr;
   dim3 grid;
   const int chunks = obs_grid(c, a, nv, grid);
-  if (!c->dense)  // sparse: G' rows of non-observing poses must be zero
-    CUDA_TRY(cudaMemsetAsync(c->G, 0, sizeof(double) * (size_t)3 * nv * c->ldg, c->stream));
-  if (c->dense) obs_pass_kernel<true, OBS_FP64><<<grid, 128, 0, c->stream>>>(a);
-  else obs_pass_kernel<false, OBS_FP64><<<grid, 128, 0, c->stream>>>(a);
+  if (c->prec == BALM_PREC_BLOCKS) {  // per-observation rows: nothing of the dense G' to clear
+    if (c->dense) obs_pass_kernel<true, OBS_BLOCKS><<<grid, 128, 0, c->stream>>>(a);
+    else obs_pass_kernel<false, OBS_BLOCKS><<<grid, 128, 0, c->stream>>>(a);
+  } else {
+    if (!c->dense)  // sparse: G' rows of non-observing poses must be zero
+      CUDA_TRY(cudaMemsetAsync(c->G, 0, sizeof(double) * (size_t)3 * nv * c->ldg, c->stream));
+    if (c->dense) obs_pass_kernel<true, OBS_FP64><<<grid, 128, 0, c->stream>>>(a);
+    else obs_pass_kernel<false, OBS_FP64><<<grid, 128, 0, c->stream>>>(a);
+  }
   const int total = BALM_ACC * c->Np;
   obs_reduce_kernel<<<(total + 255) / 256, 256, 0, c->stream>>>(c->obs_part, chunks, total, c->accum,
                                                                 c->accum_batch, first_batch ? 0 : 1);

@@ -30,6 +30,8 @@ struct WindowState;  // the persistent sliding-window octree (assoc.cu)
 void window_free(WindowState *w);
 struct PoseGraph;    // the registered window factors (pose_graph.cu)
 void pose_graph_free(PoseGraph *p);
+struct BlockHessian;  // the block pattern of a BALM_PREC_BLOCKS context (blocks.cu)
+void block_hessian_free(BlockHessian *b);
 
 #define CUDA_TRY(expr)                                                                        \
   do {                                                                                        \
@@ -68,10 +70,13 @@ struct ScratchPool {
     return BALM_OK;
   }
   void drop(void *q) {
+    release(q);
+    cudaFree(q);
+  }
+  void release(void *q) {  // the caller keeps q: it is no longer freed on exit
     if (!q) return;
     for (size_t i = 0; i < ptrs.size(); i++)
       if (ptrs[i] == q) { ptrs[i] = ptrs.back(); ptrs.pop_back(); break; }
-    cudaFree(q);
   }
 };
 
@@ -109,11 +114,13 @@ struct balm_ctx {
   balm_assoc_opts assoc{1.0, 2, 15, {1.0 / 16, 1.0 / 16, 1.0 / 16}};  // association options of that call
   WindowState *win = nullptr;     // balm_window_* state (independent of the registered voxel set)
   PoseGraph *pg = nullptr;        // balm_set_pose_factors' window factors (independent of the registered voxel set)
+  BlockHessian *bh = nullptr;     // BALM_PREC_BLOCKS: the registered set's block pattern, terms, blocks and solver
 
   // ---- optimiser state (device) ----
   double *poses = nullptr, *poses_trial = nullptr;  // [12N]
-  double *H = nullptr, *g = nullptr;                // [n*n + n + 8] contiguous: H | g | r  (one all-reduce)
-  double *A = nullptr;                              // [n*n] factor workspace
+  double *H = nullptr, *g = nullptr;                // [n*n + n + 8] contiguous: H | g | r  (one all-reduce);
+                                                    // BALM_PREC_BLOCKS: no H, g [n + 8] (g | r)
+  double *A = nullptr;                              // [n*n] factor workspace (none in BALM_PREC_BLOCKS)
   double *dx = nullptr;                             // [n]
   double *dvec = nullptr;                           // [n] diag(H)
   double *Xinv = nullptr;                           // [panels][64*64] inverses of the unit-lower diagonal blocks
@@ -137,7 +144,8 @@ struct balm_ctx {
   double *vsums = nullptr;        // [VB][10] per-voxel cluster sums (stats pass: streaming kernel -> eigen kernel)
   double *stats_trial = nullptr;  // [M][20] stats of the LM trial poses (single-batch problems): an accepted step
                                   // hands them to the next evaluation instead of recomputing them
-  double *G = nullptr;            // [3*VB][ldg] fp64 scaled factor matrix G' (MN-major: pose index contiguous)
+  double *G = nullptr;            // [3*VB][ldg] fp64 scaled factor matrix G' (MN-major: pose index contiguous);
+                                  // BALM_PREC_BLOCKS: [K][18] the three scaled G' rows of every observation (CSR order)
   int obs_chunks = 0;
   double *obs_part = nullptr;     // [obs_chunks][27][Np]
   double *accum = nullptr;        // [BALM_ACC][Np] reduced g / diag-block / sum-of-squares accumulators
@@ -162,6 +170,13 @@ struct balm_ctx {
   cudaEvent_t ev[16] = {};
   long long launches = 0;
 };
+
+// BALM_ERR_UNSUPPORTED for a call that needs the dense H on a BALM_PREC_BLOCKS context (which has none), else BALM_OK
+inline int refuse_blocks(const balm_ctx *c, const char *who) {
+  if (c->prec != BALM_PREC_BLOCKS) return BALM_OK;
+  balm_set_error(std::string(who) + ": not available on a BALM_PREC_BLOCKS context (it holds no dense H)");
+  return BALM_ERR_UNSUPPORTED;
+}
 
 // ---------------- device math ----------------
 #ifdef __CUDACC__
@@ -758,8 +773,9 @@ struct SparseSolver;  // nested-dissection ordering, symbolic factorisation and 
 void sparse_solver_free(SparseSolver *s);
 // Symbolic factorisation of the pairs' block pattern over P poses (host), device tables and the captured solve on st.
 // dvec, dx, scal and flags are the handle's buffers the solve reads and writes (as the context's launch_ldlt_solve).
+// who: prefix of the BALM_ERR_UNSUPPORTED message when the pattern is too large to index.
 int sparse_solver_build(cudaStream_t st, int P, const std::vector<int2> &pairs, const double *blocks, const double *g,
-                        double *dvec, double *dx, double *scal, int *flags, SparseSolver **out);
+                        double *dvec, double *dx, double *scal, int *flags, const char *who, SparseSolver **out);
 // blocks of L, elimination-tree levels and device bytes held
 void sparse_solver_stats(const SparseSolver *s, int64_t *l_blocks, int64_t *levels, int64_t *bytes);
 // (H + u diag(H)) dx = -g with u in scal[3]: damped copy, factorisation, substitutions, q1 -> scal[1], the backward-error
@@ -767,6 +783,21 @@ void sparse_solver_stats(const SparseSolver *s, int64_t *l_blocks, int64_t *leve
 int sparse_solve(SparseSolver *s, cudaStream_t st);
 // refine_solution's rounds with the same factors; *still_bad when omega stayed above the tolerance (waits)
 int sparse_refine(SparseSolver *s, cudaStream_t st, int *h_flags, double *h_scal, int *still_bad);
+
+// ---------------- block-sparse Hessian of a BALM_PREC_BLOCKS context (blocks.cu) ----------------
+// The registered voxels' pair pattern, update terms and symbolic factorisation -> c->bh (replacing the previous one).
+// BALM_ERR_UNSUPPORTED (message prefixed with who) when the terms or pairs are too many to index; c->bh is then kept.
+int block_hessian_build(balm_ctx *c, const char *who);
+// the blocks of voxels [head, end) from c->G (the per-observation store) and the accumulators, g from the accumulators
+int launch_blocks(balm_ctx *c, int64_t head, int64_t end);
+int blocks_zero(balm_ctx *c);
+// the damped solve (u into scal[3]) and its refinement: launch_ldlt_solve / refine_solution of a blocks context
+int blocks_solve(balm_ctx *c, double u);
+int blocks_refine(balm_ctx *c, int *still_bad);
+const std::vector<int2> &blocks_pairs(const BlockHessian *b);
+const double *blocks_device(const BlockHessian *b);
+// device bytes of the pattern, terms, blocks and solver; l_blocks / levels of the factorisation
+long long blocks_bytes(const BlockHessian *b, int64_t *l_blocks, int64_t *levels);
 
 // ---------------- association (assoc.cu) ----------------
 // The plane voxels of one or more problems cut from raw scans. Host arrays; xyz (n_points x 3 float32, body frame) and

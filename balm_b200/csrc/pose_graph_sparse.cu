@@ -302,8 +302,8 @@ void sparse_solver_stats(const SparseSolver *s, int64_t *l_blocks, int64_t *leve
   *bytes = s->bytes;
 }
 
-static int too_large(const char *what) {
-  balm_set_error(std::string("balm_spg_set_factors: ") + what);
+static int too_large(const char *who, const char *what) {
+  balm_set_error(std::string(who) + ": " + what);
   return BALM_ERR_UNSUPPORTED;
 }
 
@@ -330,11 +330,11 @@ static int enqueue_check(SparseSolver &s, cudaStream_t st) {
 }
 
 int sparse_solver_build(cudaStream_t st, int P, const std::vector<int2> &pairs, const double *blocks, const double *g,
-                        double *dvec, double *dx, double *scal, int *flags, SparseSolver **out) {
+                        double *dvec, double *dx, double *scal, int *flags, const char *who, SparseSolver **out) {
   std::unique_ptr<SparseSolver> s(new SparseSolver());
   s->P = P;
   const long long npairs = (long long)pairs.size();
-  if (npairs >= (1LL << 30)) return too_large("too many block pairs");
+  if (npairs >= (1LL << 30)) return too_large(who, "too many block pairs");
   // the pose graph's adjacency
   std::vector<long long> xadj(P + 1, 0);
   for (const int2 &p : pairs)
@@ -374,7 +374,7 @@ int sparse_solver_build(cudaStream_t st, int P, const std::vector<int2> &pairs, 
   std::vector<int> colptr(P + 1, 0);
   for (int j = 0; j < P; j++) {
     const long long n = (long long)colptr[j] + 1 + (long long)cstruct[j].size();
-    if (n >= (1LL << 31) / 36) return too_large("too many blocks of L");
+    if (n >= (1LL << 31) / 36) return too_large(who, "too many blocks of L");
     colptr[j + 1] = (int)n;
   }
   const long long nb = colptr[P];

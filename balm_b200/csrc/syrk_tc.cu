@@ -859,6 +859,7 @@ void tensor_syrk_new_problem(balm_ctx *c) {
 extern "C" int balm_debug_syrk_tc(balm_ctx *c, const int8_t *planes, int S, int64_t rows, const double *isc, int splits,
                                   int accumulate, double *part) {
   if (!c || !planes || !isc || !part) { balm_set_error("balm_debug_syrk_tc: bad arguments"); return BALM_ERR_INVALID; }
+  TRY(refuse_blocks(c, "balm_debug_syrk_tc"));
   if (S < 2 || S > SMAX || rows < 1 || rows > ((int64_t)1 << 30) || splits < 1) {
     balm_set_error("balm_debug_syrk_tc: S must be 2..4, rows 1..2^30 and splits >= 1");
     return BALM_ERR_INVALID;
@@ -906,6 +907,7 @@ extern "C" int balm_debug_syrk_tc(balm_ctx *c, const int8_t *planes, int S, int6
 
 extern "C" int balm_debug_tc_planes(balm_ctx *c, int8_t *planes, double *isc, int *S, int64_t *rows_padded,
                                     int *splits) {
+  if (c) TRY(refuse_blocks(c, "balm_debug_tc_planes"));
   TcState *st = (c && c->prec == BALM_PREC_TENSOR) ? static_cast<TcState *>(c->tmap) : nullptr;
   if (!st || st->last_rows_padded == 0) {
     balm_set_error("balm_debug_tc_planes: no tensor-path evaluation of the registered voxels");
@@ -927,6 +929,7 @@ extern "C" int balm_debug_tc_planes(balm_ctx *c, int8_t *planes, double *isc, in
 }
 
 extern "C" int balm_debug_tc_trace(balm_ctx *c, unsigned long long *out, int max_entries) {
+  if (c) TRY(refuse_blocks(c, "balm_debug_tc_trace"));
   if (!c || !out || !c->tc_trace || max_entries < 0) {
     balm_set_error("balm_debug_tc_trace: no trace (BALM_TC_TRACE=1 at the creation of a tensor-precision context)");
     return BALM_ERR_INVALID;

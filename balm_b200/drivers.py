@@ -17,6 +17,11 @@ from . import _lib as L
 from . import io
 from .context import Context
 
+# benchmark_realworld runs PREC_BLOCKS from this many scans on, whatever `precision` says: a lidar sequence has local
+# co-visibility, and the block-sparse Hessian and solve beat the dense ones there (DESIGN.md "Block-sparse voxel BA").
+# The mode is chosen by pose count because the context, and with it the mode, exists before the association runs.
+BLOCKS_MIN_POSES = 1000
+
 
 def pack_poses(R, p):
     """[n,3,3], [n,3] -> [n,12] (R column-major, then p): the layout of IMUST::R.data() followed by p."""
@@ -108,7 +113,7 @@ def benchmark_realworld(file_path, voxel_size=2.0, device=0, precision=L.PREC_TE
     xyz = np.concatenate(scans).astype(np.float32)
     frame = np.concatenate([np.full(len(s), i, dtype=np.int32) for i, s in enumerate(scans)])
     t_read = time.perf_counter()
-    ctx = Context(win_size, device, precision)
+    ctx = Context(win_size, device, L.PREC_BLOCKS if win_size >= BLOCKS_MIN_POSES else precision)
     try:
         n_vox, n_obs = ctx.cut_voxels(xyz, frame, poses_init, voxel_size=voxel_size, layer_limit=2, min_ps=15,
                                       eigen_value_array=(1.0 / 16, 1.0 / 16, 1.0 / 9))  # :183-185, bavoxel.hpp:8-19

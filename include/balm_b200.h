@@ -45,7 +45,17 @@ typedef enum {
 /* Arithmetic of the rank-3M Hessian accumulation  H -= G' G'^T  (bavoxel.hpp:385,392,410-416). */
 typedef enum {
   BALM_PREC_FP64 = 0,   /* fp64 DMMA accumulation (BASELINE config C2, "fp64 accumulation") */
-  BALM_PREC_TENSOR = 1  /* int8 tensor-core split-integer (Ozaki) accumulation, exact int32 sums, fp64 result */
+  BALM_PREC_TENSOR = 1, /* int8 tensor-core split-integer (Ozaki) accumulation, exact int32 sums, fp64 result */
+  BALM_PREC_BLOCKS = 2  /* fp64, H held as the 6x6 blocks of the pose pairs sharing a voxel (plus every diagonal pair)
+                           and the damped system solved by the sparse pose graph's nested-dissection block LDL^T (DESIGN.md
+                           "Block-sparse voxel BA"). Nothing of size (6N)^2 is allocated, so windows of thousands of
+                           scans with local co-visibility fit. g, the residual and the diagonal blocks' sweep terms are
+                           bitwise those of BALM_PREC_FP64. Single batch: 144 B per observation must fit the G' budget
+                           (16 GB, BALM_G_BUDGET_MB), else the registration is BALM_ERR_UNSUPPORTED and leaves the
+                           context without voxels, as do 2^31 observation pairs or 2^30 block pairs. balm_comm_init,
+                           balm_pose_covariance, balm_set_pose_factors, balm_pose_graph_*, balm_device_views and the
+                           tensor debug aids return BALM_ERR_UNSUPPORTED on such a context and change nothing;
+                           balm_evaluate's H (when not NULL) is the dense matrix expanded from the blocks. */
 } balm_precision;
 
 typedef struct {
@@ -430,6 +440,14 @@ int balm_spg_evaluate(balm_spg *spg, const double *poses12, double *blocks, doub
  * rules) on the sparse solve. */
 int balm_spg_iter(balm_spg *spg, double *poses12, const balm_lm_opts *opts, balm_trace *trace, int *n_iters,
                   double *poses_per_iter);
+
+/* Block-sparse Hessian of a BALM_PREC_BLOCKS context (BALM_ERR_INVALID on any other, or before a registration).
+ * stats: [0] block pairs (i <= j) of H, [1] blocks of the factor L, [2] elimination-tree levels, [3] device bytes the
+ * context holds. pairs (may be NULL, so that a first call can size it): 2 int32 (i, j) per block pair, ascending. */
+int balm_block_structure(balm_ctx *ctx, int64_t stats[4], int32_t *pairs);
+/* The last evaluation's blocks, bitwise what the solve consumed: 36 doubles per pair (rows of pose i, columns of pose
+ * j, column-major) in balm_block_structure's order. */
+int balm_download_blocks(balm_ctx *ctx, double *blocks);
 
 /* Multi-GPU: voxels are sharded across ranks by the caller (each rank registers its own shard); the library
  * all-reduces [H | g | r] with NCCL after every evaluation and the scalar after every residual pass.
