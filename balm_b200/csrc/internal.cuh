@@ -159,6 +159,7 @@ struct balm_ctx {
   int8_t *Gq = nullptr;           // [4][rows_alloc][ldg] int8 digit planes of rint(G' * sc) (3 or 4 used per batch)
   unsigned long long *colmax = nullptr;  // [ldg] bit patterns of max |G'[:,j]| of the current batch
   void *tmap = nullptr;           // CUtensorMap storage
+  int tc_tile = 0;                // BALM_TC_TILE: 0 = whole tiles when every SM gets one, 1 = column halves, 2 = whole
 
   // ---- multi-GPU ----
   void *comm = nullptr;

@@ -11,24 +11,26 @@
 // (S = 4) and the dropped digit pairs s+t >= S (same order); integer accumulation is associative, so the
 // result does not depend on tile order, k-splits or the number of GPUs.
 //
-// Kernel anatomy (syrk_tc_kernel; one CTA per SM, persistent over (tile, column half, k-split) items, 384 threads):
-//   warp 8    : TMA producer -- cp.async.bulk.tensor.3d of the S int8 planes of the A block (128 columns bi, 128B
-//               swizzle) and of the B half block (64 columns of bj, 64B swizzle), KS = 64 contraction rows per stage,
-//               into the A and B rings (see Rings: 160-224 KB of shared memory in all, mbarrier full/empty per slot)
-//   warps 9-11: B transposers -- load each landed B slot into registers, free it, and store the K-major core
-//               matrices into a slot of the BT ring
-//   warps 0-7 : consumers, two warpgroups of 64 output rows each -- wgmma m64n64k32 s8 x s8 -> s32 with A from
-//               registers and B from the K-major copy, S(S+1)/2 digit-pair products per k32 step into S register
-//               accumulators; then the epilogue: fp64 Horner combine, column scales, fp64 partial tile to global
-//               (same partial layout as the fp64 path -> same assemble kernel)
-// The register accumulators (S * 64 x 64 int32 per warpgroup = 128 registers per consumer thread at S = 4) are what
-// bounds the output tile to 128 x 64. The digit planes are stored MN-major (pose index contiguous, as the observation
-// sweep writes them coalesced) while s8 wgmma reads shared-memory operands K-major only. So A is transposed on its way
-// into registers (ldmatrix.trans of 16-bit pairs, then byte permutes), once per plane and k32 step, and feeds all the
-// S - s products of its plane; B is transposed once per stage by the transposer warps. Both sides assign the same
-// contraction row to each k position of the MMA (the k position map below), so the integer sums are those of the plain
-// product, bit for bit.
-#include <cuda.h>
+// The observation sweep writes the digit planes MN-major (pose index contiguous, Gq[S][rows][ldg], coalesced), while
+// s8 wgmma reads shared-memory operands K-major only. tc_kmajor_kernel therefore transposes the planes once per SYRK
+// launch into GqT[S][rows / 64][ldg][64]: per 64-row band, every column's 64 contraction rows as one 64-byte row, in the
+// order wgmma reads them from shared memory (64-byte swizzle, see sw64_desc). A 128- or 64-column block of one band is
+// then one contiguous 8 or 4 KB run that a single bulk copy lands ready for the MMAs; the SYRK reads that copy alone.
+//
+// Kernel anatomy (syrk_tc_kernel; one CTA per SM, persistent over its items, 384 threads). An item is a whole 128 x 128
+// output tile (S <= 3 on problems with at least one (tile, k-split) pair per SM, see launch_syrk_tc) or one 128 x 64
+// column half of a tile, times one k-split:
+//   warp 8    : producer (one lane) -- cp.async.bulk of the S K-major planes of the A block (128 columns bi) and of the
+//               B block (128 columns bj, or the 64 of the half), KS = 64 contraction rows per stage, into one ring of
+//               stage slots (see Ring: up to 224 KB of shared memory, mbarrier full/empty per slot); warps 9-11 have
+//               no work
+//   warps 0-7 : consumers, two warpgroups of 64 output rows each -- wgmma m64n128k32 (whole tiles) or m64n64k32 (halves)
+//               s8 x s8 -> s32 with B from the landed stage and A from it too (whole tiles) or from registers
+//               (ldmatrix, halves), S(S+1)/2 digit-pair
+//               products per k32 step into S register accumulators; then the epilogue: fp64 Horner combine, column
+//               scales, fp64 partial tile to global (same partial layout as the fp64 path -> same assemble kernel)
+// The register accumulators (S * 64 x N int32 per warpgroup = S * N / 2 registers per consumer thread) are what bounds
+// the output tile: 192 at S = 3 and N = 128, so S = 4 (which would need 256) keeps 128 x 64 halves.
 #include <vector>
 #include <algorithm>
 #include "internal.cuh"
@@ -36,50 +38,33 @@
 namespace {
 
 constexpr int TILE = BALM_SYRK_TILE;  // 128
-constexpr int HALF = TILE / 2;        // output columns of one item
+constexpr int HALF = TILE / 2;        // output columns of a half-tile item
 constexpr int SMAX = 4;               // digit planes
-constexpr int KS = 64;                // contraction rows per pipeline stage
-constexpr int A_PLANE_BYTES = KS * TILE;  // 8192: one plane of the A block, one stage (128-byte rows)
-constexpr int B_PLANE_BYTES = KS * HALF;  // 4096: one plane of the B half block, one stage (64-byte rows)
-constexpr int BT_PLANE_BYTES = KS * HALF; // 4096: the same plane K-major (wgmma core matrices, see bt_offset)
-constexpr int MAX_SLOTS = 8;             // barriers per ring
-constexpr int BAR_BYTES = 6 * MAX_SLOTS * 8;
+constexpr int KS = 64;                // contraction rows per pipeline stage (= the 64-byte swizzle span of a K-major row)
+constexpr int A_PLANE_BYTES = KS * TILE;  // 8192: one K-major plane of a 128-column block, one stage (64-byte rows)
+constexpr int MAX_SLOTS = 8;             // barriers of the ring
+constexpr int BAR_BYTES = 2 * MAX_SLOTS * 8;
 constexpr int RING_BYTES = 227 * 1024 - 1024 - BAR_BYTES;  // the block's whole shared memory but alignment slack, barriers
-// Three rings, one slot per 64-row stage each, all advancing by one slot per stage: A (S planes of the A block, TMA),
-// B (S planes of the B half block as TMA lands them, MN-major) and BT (their K-major copies). A slot of B is free again
-// as soon as the transposers have loaded it into registers, a slot of BT once the consumers' MMAs on it retired, so
-// neither the in-flight loads nor the MMAs hold a copy they do not use. Depths per S (A x B x BT slots), chosen with
-// the BALM_TC_TRACE per-role clocks and the benchmark at its C3 shape (S = 3): with two BT slots the transposers run
-// only one stage ahead of the consumers, whose waits on BT then dominate; deeper A or B rings than below measured no
-// faster:
-//   S = 2: 6 x 16 KB + 4 x 8 KB + 4 x 8 KB = 160 KB; S = 3: 4 x 24 + 4 x 12 + 4 x 12 = 192 KB;
-//   S = 4: 4 x 32 + 2 x 16 + 4 x 16 = 224 KB
-template <int S>
-struct Rings {
-  static constexpr int DA = S == 2 ? 6 : 4, DB = S == 4 ? 2 : 4, DT = 4;
-  static constexpr int A_SLOT = S * A_PLANE_BYTES, B_SLOT = S * B_PLANE_BYTES, T_SLOT = S * BT_PLANE_BYTES;
-  static constexpr int B_OFF = DA * A_SLOT, T_OFF = B_OFF + DB * B_SLOT, BYTES = T_OFF + DT * T_SLOT;
-  static_assert(BYTES <= RING_BYTES && DA <= MAX_SLOTS && DB <= MAX_SLOTS && DT <= MAX_SLOTS, "ring layout");
-  static_assert(A_SLOT % 1024 == 0 && B_SLOT % 1024 == 0 && T_SLOT % 1024 == 0, "swizzle alignment");
-};
-// slot and phase of a ring of D slots
-template <int D>
-struct RingPos {
-  int slot = 0;
-  uint32_t ph = 0;
-  __device__ __forceinline__ void next() {
-    if (++slot == D) { slot = 0; ph ^= 1; }
-  }
+// One ring of stage slots: a slot holds the S planes of the A block, then the S planes of the B block (128 or 64
+// columns), all landed by bulk copies on the slot's one full barrier and freed together once the consumers' MMAs on it retired.
+// As many slots as fit, at most MAX_SLOTS:
+//   whole tiles: S = 2: 7 x 32 KB, S = 3: 4 x 48 KB;  halves: S = 2: 8 x 24 KB, S = 3: 6 x 36 KB, S = 4: 4 x 48 KB
+template <int S, bool FULL>
+struct Ring {
+  static constexpr int N = FULL ? TILE : HALF;  // output columns of an item
+  static constexpr int B_PLANE = KS * N;
+  static constexpr int B_OFF = S * A_PLANE_BYTES, SLOT = B_OFF + S * B_PLANE;
+  static constexpr int D = RING_BYTES / SLOT < MAX_SLOTS ? RING_BYTES / SLOT : MAX_SLOTS;
+  static_assert(D >= 2 && SLOT % 1024 == 0, "ring layout (the 64-byte swizzle repeats every 512 bytes)");
 };
 constexpr int CONSUMER_WARPS = 8;
-constexpr int TRANSPOSE_WARPS = 3;                      // warps 9-11
 constexpr int TC_THREADS = 32 * (CONSUMER_WARPS + 4);   // two consumer warpgroups + one producer warpgroup
-// register split (setmaxnreg): the producer warpgroup gives registers up so the consumers can hold their accumulators
-// (S * 32 + 2 * S * 4 A-fragment registers); the transposers keep a whole stage of their ldmatrix results (up to 44
-// registers at S = 4). The pool is what the launch allocated, 384 threads x 168 registers, and setmaxnreg.inc waits
-// until the registers are free: 2 * 128 * 216 + 128 * 72 <= 384 * 168
-constexpr int CONSUMER_REGS = 216, PRODUCER_REGS = 72;
-constexpr int TC_SMEM = RING_BYTES + 1024 + BAR_BYTES;  // rings + alignment slack + barriers
+// register split (setmaxnreg): the producer warpgroup (one copying lane) gives nearly all its registers up so the consumers
+// can hold their accumulators (S * N / 2, 192 at S = 3 on whole tiles) and two k32 steps of A fragments (2 * S * 4).
+// The pool is what the launch allocated, 384 threads x 168 registers, and setmaxnreg.inc waits until the registers are
+// free: 2 * 128 * 240 + 128 * 24 = 384 * 168
+constexpr int CONSUMER_REGS = 240, PRODUCER_REGS = 24;
+constexpr int TC_SMEM = RING_BYTES + 1024 + BAR_BYTES;  // ring + alignment slack + barriers
 constexpr int MAX_ROWS_PER_ITEM = BALM_TC_MAX_ROWS_PER_ITEM;  // 32704: 4 * rows * 2^14 < 2^31 (a multiple of KS)
 static_assert(MAX_ROWS_PER_ITEM % KS == 0 && 4ll * MAX_ROWS_PER_ITEM * (1 << 14) < (1ll << 31), "int32 exactness bound");
 
@@ -119,9 +104,10 @@ __device__ __forceinline__ unsigned long long globaltimer_ns() {
   asm volatile("mov.u64 %0, %%globaltimer;\n" : "=l"(t));
   return t;
 }
-// BALM_TC_TRACE (balm_debug_tc_trace): per-CTA word offsets of the stage count, the consumer warp 0 globaltimer pair and
-// the clock64 sums of the consumer warps 0 and 4 (5 each), of transposer warp 9 (3) and of the producer (2)
-constexpr int TR_STAGES = 0, TR_NS = 1, TR_CONS = 3, TR_XPOSE = 13, TR_PROD = 16, TR_WORDS = BALM_TC_TRACE_WORDS;
+// BALM_TC_TRACE (balm_debug_tc_trace): per-CTA word offsets of the stage count (in 128 x 64 half-tile units: a stage of
+// a whole tile counts 2), the consumer warp 0 globaltimer pair, the clock64 sums of the consumer warps 0 and 4 (5 each),
+// three words that stay zero (they held a B transposer's clocks) and the producer's (2)
+constexpr int TR_STAGES = 0, TR_NS = 1, TR_CONS = 3, TR_PROD = 16, TR_WORDS = BALM_TC_TRACE_WORDS;
 static_assert(TR_PROD + 2 == TR_WORDS, "trace layout");
 // clock64 in the traced instantiation; the untraced one reads no clock
 template <bool TRACE>
@@ -130,38 +116,29 @@ __device__ __forceinline__ long long tclock() {
   else return 0;
 }
 
-__device__ __forceinline__ void tma_load_3d(void *dst, const CUtensorMap *map, uint64_t *bar, int c0, int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];\n"
-      ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
+// one contiguous run of global memory into shared memory, completing on the mbarrier's transaction count
+__device__ __forceinline__ void bulk_load(void *dst, const void *src, uint32_t bytes, uint64_t *bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n"
+               ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar))
+               : "memory");
 }
 
-// Four 8 x 8 matrices of 16-bit pairs, transposed: lane 8q + i gives the address of row i of matrix q; thread
-// (g = lane/4, t = lane%4) receives in r[q] the pair g of row 2t (low half) and of row 2t + 1 (high half).
-__device__ __forceinline__ void ldsm_x4_trans(uint32_t addr, uint32_t *r) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];\n"
+// Four 8 x 8 matrices of 16-bit pairs: lane 8q + i gives the address of row i of matrix q; thread (g = lane/4,
+// t = lane%4) receives in r[q] the pair t of row g, i.e. bytes 4t..4t+3 of that 16-byte row.
+__device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t *r) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];\n"
                : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
                : "r"(addr)
                : "memory");
 }
 
-// Contraction rows and k positions. A k32 step covers 32 contraction rows: four groups of 8, one ldmatrix matrix each.
-// Thread t's two rows 2t, 2t + 1 of groups q and q + 1 go to the four k positions 4t..4t+3 (q = 0) and 16+4t..16+4t+3
-// (q = 2) of the MMA: k position 16 h + 4 t + j holds contraction row 16 h + 2 t + (j & 1) + 8 (j >> 1). A (in
-// registers) and B (in the K-major copy) use the same map; as it is a bijection, the products are those of the plain
-// contraction.
-// From the ldmatrix.trans result of pairs (c, c + 1) at the rows of groups q, q + 1: the 4 k positions of column c
-// (0x6420, even bytes) or c + 1 (0x7531, odd bytes).
-constexpr uint32_t PERM_EVEN = 0x6420, PERM_ODD = 0x7531;
-
-// K-major copy of one B plane, one stage: wgmma core matrices of 8 columns x 16 k bytes (128 contiguous bytes,
-// no swizzle); k32 step c at c * 2048, column group n / 8 at (n / 8) * 256 (SBO), k half at 128 (LBO). The 4 k positions
-// 4 kword .. 4 kword + 3 (kword in 0..7) of column n are the word at
-//   bt_offset(c, n, kword) = c * BT_CHUNK + (n >> 3) * BT_SBO + (kword >> 2) * BT_LBO + (n & 7) * 16 + 4 * (kword & 3).
-constexpr int BT_LBO = 128, BT_SBO = 256, BT_CHUNK = 2048;
-__device__ __forceinline__ uint64_t bt_desc(uint32_t saddr) {  // wgmma matrix descriptor, no swizzle
-  return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)(BT_LBO >> 4) << 16) | ((uint64_t)(BT_SBO >> 4) << 32);
+// A K-major plane of a stage as it lands (the layout of GqT): column n of the block is the 64-byte row n (contraction rows 0..63 of the
+// stage), its 16-byte chunk q at (q ^ ((n >> 1) & 3)) under the 64-byte swizzle. wgmma reads it through a descriptor of
+// that swizzle mode (layout type 2): 8-row core-matrix groups SW_SBO = 512 bytes apart, the k32 step c at + 32 c bytes
+// (the swizzle is a function of the address, and every plane starts on a 512-byte boundary).
+constexpr int SW_SBO = 8 * KS;
+__device__ __forceinline__ uint64_t sw64_desc(uint32_t saddr) {
+  return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(SW_SBO >> 4) << 32) | ((uint64_t)2 << 62);
 }
 
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory"); }
@@ -169,9 +146,10 @@ __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_grou
 template <int N>
 __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;\n" ::"n"(N) : "memory"); }
 // keeps the compiler from moving accumulator accesses across the asynchronous MMAs
-__device__ __forceinline__ void fence_acc(int32_t (&d)[32]) {
+template <int R>
+__device__ __forceinline__ void fence_acc(int32_t (&d)[R]) {
 #pragma unroll
-  for (int i = 0; i < 32; i++) asm volatile("" : "+r"(d[i])::"memory");
+  for (int i = 0; i < R; i++) asm volatile("" : "+r"(d[i])::"memory");
 }
 
 // D (64 x 64 s32, accumulated) += A (64 x 32 s8, registers) * B (32 x 64 s8, K-major shared memory)
@@ -185,6 +163,25 @@ __device__ __forceinline__ void wgmma_s8(int32_t (&d)[32], const uint32_t (&a)[4
         "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]),
         "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31])
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b)
+      : "memory");
+}
+// D (64 x 128 s32, accumulated) += A (64 x 32 s8, K-major shared memory) * B (32 x 128 s8, K-major shared memory)
+__device__ __forceinline__ void wgmma_s8_ss(int32_t (&d)[64], uint64_t desc_a, uint64_t desc_b) {
+  asm volatile(
+      "wgmma.mma_async.sync.aligned.m64n128k32.s32.s8.s8 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
+      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
+      "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,"
+      "%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, 1;\n"
+      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]),
+        "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]),
+        "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]),
+        "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]),
+        "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]),
+        "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]),
+        "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]),
+        "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63])
+      : "l"(desc_a), "l"(desc_b)
       : "memory");
 }
 
@@ -203,8 +200,12 @@ __device__ __forceinline__ bool warpgroup_all(bool ok, int id) {
 }
 
 struct TcArgs {
+  const int8_t *planes_t;  // GqT [SMAX][rows / KS][ldq][KS], see tc_kmajor_kernel
+  int64_t plane;      // bytes per plane of planes_t
+  int ldq;
   int64_t rows;       // contraction rows of this batch (3 per voxel)
   int nb, tiles, splits;
+  int full;           // whole 128 x 128 tiles when S <= 3 (launch_syrk_tc decides)
   const int *S_dev;   // digit-plane count chosen by tc_scale_kernel
   const double *isc;  // [ldq]  256^(S-1) / sc_j
   double *part;       // [splits][tiles][128*128]
@@ -227,18 +228,22 @@ __device__ __forceinline__ void tile_coords_tc(int t, int nb, int &bi, int &bj) 
 }
 
 // Items are distributed round robin over the CTAs: item blockIdx.x, blockIdx.x + gridDim.x, ...
-__device__ __forceinline__ int n_items(const TcArgs &a) { return a.tiles * 2 * a.splits; }
+template <bool FULL>
+__device__ __forceinline__ int n_items(const TcArgs &a) { return a.tiles * (FULL ? 1 : 2) * a.splits; }
 // contraction rows of a k-split item: ceil(rows / splits) rounded up to KS
 __device__ __forceinline__ int64_t rows_per_item(const TcArgs &a) {
   return ((a.rows + a.splits - 1) / a.splits + KS - 1) / KS * KS;
 }
 
-// work = (sp * tiles + t) * 2 + h: the two column halves of a tile run on neighbouring CTAs and share the A block in L2
+// whole tiles: work = sp * tiles + t; halves: work = (sp * tiles + t) * 2 + h, the two column halves of a tile run on
+// neighbouring CTAs and share the A block in L2
+template <bool FULL>
 __device__ __forceinline__ ItemInfo decode_item(const TcArgs &a, int work, int64_t per) {
   ItemInfo it;
-  it.h = work & 1;
-  it.t = (work >> 1) % a.tiles;
-  it.sp = (work >> 1) / a.tiles;
+  it.h = FULL ? 0 : (work & 1);
+  const int w = FULL ? work : (work >> 1);
+  it.t = w % a.tiles;
+  it.sp = w / a.tiles;
   tile_coords_tc(it.t, a.nb, it.bi, it.bj);
   it.k_begin = (int64_t)it.sp * per;
   int64_t k_end = it.k_begin + per;
@@ -247,77 +252,73 @@ __device__ __forceinline__ ItemInfo decode_item(const TcArgs &a, int work, int64
   return it;
 }
 
-// Shared-memory barriers of the three rings (MAX_SLOTS each): full = the slot holds its stage, empty = it may be refilled
-struct RingBars {
-  uint64_t *full_a, *empty_a, *full_b, *empty_b, *full_t, *empty_t;
-};
-
-// One consumer warpgroup (wg = 0, 1): output rows 64 wg .. 64 wg + 63 of the 128 x 64 half tile, all items of this
-// CTA. Warp w (0..7) holds the 16 rows of 16-byte chunk w of the A block: fragment row g is output row 16 w + 2 g,
-// fragment row g + 8 is output row 16 w + 2 g + 1; fragment column n is column n of the half tile.
-template <int S, bool TRACE>
-__device__ __forceinline__ void consumer_loop(const TcArgs &a, uint32_t ring, const RingBars &bar) {
-  using R = Rings<S>;
+// One consumer warpgroup (wg = 0, 1): output rows 64 wg .. 64 wg + 63 of the item, all items of this CTA. Warp w (0..7)
+// holds output rows 16 w .. 16 w + 15: fragment row g is output row 16 w + g, fragment row g + 8 is 16 w + g + 8;
+// fragment column n is column n of the item. A stage's slot sits at slot k % D, phase (k / D) & 1, for the k-th stage
+// this CTA consumes.
+template <int S, bool FULL, bool TRACE>
+__device__ __forceinline__ void consumer_loop(const TcArgs &a, uint32_t ring, uint64_t *full, uint64_t *empty) {
+  using R = Ring<S, FULL>;
+  constexpr int NACC = R::N / 2;  // accumulator registers per digit-pair sum
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int g = lane >> 2, t = lane & 3, i = lane & 7, wg = warp >> 2;
-  // ldmatrix row of this lane: contraction row 8 (lane / 8) + i of a k32 step, chunk `warp` under the 128B swizzle;
-  // the 8 rows of each matrix sit in 8 different chunks, so the loads are free of bank conflicts
-  const uint32_t lda = ring + ((lane >> 3) * 8 + i) * TILE + ((warp ^ i) << 4);
-  const uint32_t bt_ring = ring + R::T_OFF;
+  // ldmatrix row of this lane: matrix q = lane / 8 is output rows 16 warp + 8 (q & 1) + 0..7 at 16-byte chunk 2 c + q / 2
+  // of the k32 step c; under the swizzle that chunk sits at ((q / 2) ^ ((i >> 1) & 3)) ^ 2 c. The 8 rows of a matrix
+  // fill the 8 distinct 16-byte positions of two 128-byte lines, free of bank conflicts.
+  const int row = 16 * warp + 8 * ((lane >> 3) & 1) + i;
+  const uint32_t lda = ring + row * KS + ((((lane >> 4) & 1) ^ ((i >> 1) & 3)) << 4);
   const double inv256 = 1.0 / 256.0;
-  long long tr[4] = {0, 0, 0, 0};  // trace: wait A full, wait BT full, wgmma.wait_group, epilogue
+  long long tr[4] = {0, 0, 0, 0};  // trace: wait stage full, warpgroup vote, wgmma.wait_group, epilogue
   const long long t_start = tclock<TRACE>();
   const unsigned long long ns_start = TRACE ? globaltimer_ns() : 0;
-  int k = 0;  // stages consumed so far: stage k sits in slot k % D of a ring of D slots, phase (k / D) & 1
+  int k = 0;  // stages consumed so far
   const int64_t per = rows_per_item(a);
-  for (int item = blockIdx.x; item < n_items(a); item += gridDim.x) {
-    const ItemInfo info = decode_item(a, item, per);
-    int32_t acc[S][32];
+  for (int item = blockIdx.x; item < n_items<FULL>(a); item += gridDim.x) {
+    const ItemInfo info = decode_item<FULL>(a, item, per);
+    int32_t acc[S][NACC];
 #pragma unroll
     for (int d = 0; d < S; d++)
 #pragma unroll
-      for (int q = 0; q < 32; q++) acc[d][q] = 0;
-    uint32_t af[2][S][4];  // A fragments of every plane, one set per k32 step of a stage (the other may be in flight)
+      for (int q = 0; q < NACC; q++) acc[d][q] = 0;
+    // halves: A fragments of every plane, one set per k32 step of a stage (the other may be in flight); whole tiles read
+    // A from shared memory, as the 192 accumulators leave no room for them
+    uint32_t af[2][FULL ? 1 : S][4];
     bool alive = true;
     for (int ks = 0; ks < info.nsteps; ks++, k++) {
-      const int sla = k % R::DA, slt = k % R::DT;
+      const int sl = k % R::D;
       const long long t0 = tclock<TRACE>();
-      const bool ok_a = mbar_wait(&bar.full_a[sla], (k / R::DA) & 1, a.err);
+      const bool ok_s = mbar_wait(&full[sl], (k / R::D) & 1, a.err);
       const long long t1 = tclock<TRACE>();
-      const bool ok = warpgroup_all(ok_a && mbar_wait(&bar.full_t[slt], (k / R::DT) & 1, a.err), 1 + wg);
+      const bool ok = warpgroup_all(ok_s, 1 + wg);
       if constexpr (TRACE) { tr[0] += t1 - t0; tr[1] += clock64() - t1; }
       if (!ok) { alive = false; break; }  // the warpgroup leaves together (wgmma is .aligned)
-      const uint32_t sa = lda + sla * R::A_SLOT;
-      const uint64_t sdesc = bt_desc(bt_ring + slt * R::T_SLOT);
+      const uint32_t sa = lda + sl * R::SLOT;
+      const uint64_t adesc = sw64_desc(ring + sl * R::SLOT + wg * 64 * KS);  // this warpgroup's 64 rows of the A block
+      const uint64_t sdesc = sw64_desc(ring + sl * R::SLOT + R::B_OFF);
 #pragma unroll
       for (int c = 0; c < KS / 32; c++) {
+        if constexpr (!FULL) {
 #pragma unroll
-        for (int s = 0; s < S; s++) {
-          uint32_t m[4];
-          ldsm_x4_trans(sa + s * A_PLANE_BYTES + c * 32 * TILE, m);
-          af[c][s][0] = __byte_perm(m[0], m[1], PERM_EVEN);
-          af[c][s][1] = __byte_perm(m[0], m[1], PERM_ODD);
-          af[c][s][2] = __byte_perm(m[2], m[3], PERM_EVEN);
-          af[c][s][3] = __byte_perm(m[2], m[3], PERM_ODD);
+          for (int s = 0; s < S; s++) ldsm_x4((sa + s * A_PLANE_BYTES) ^ (c << 5), af[c][s]);
         }
         wgmma_fence();
 #pragma unroll
         for (int s = 0; s < S; s++)
 #pragma unroll
-          for (int tt = 0; tt + s < S; tt++)
-            wgmma_s8(acc[s + tt], af[c][s], sdesc + ((tt * BT_PLANE_BYTES + c * BT_CHUNK) >> 4));
+          for (int tt = 0; tt + s < S; tt++) {
+            const uint64_t db = sdesc + ((tt * R::B_PLANE + c * 32) >> 4);
+            if constexpr (FULL) wgmma_s8_ss(acc[s + tt], adesc + ((s * A_PLANE_BYTES + c * 32) >> 4), db);
+            else wgmma_s8(acc[s + tt], af[c][s], db);
+          }
         wgmma_commit();
         // every group but this one has retired: after the first k32 step that frees the previous stage, after the
         // second the A fragments of the first
         const long long t2 = tclock<TRACE>();
         wgmma_wait<1>();
         if constexpr (TRACE) tr[2] += clock64() - t2;
-        if (c == 0 && ks > 0) {  // the previous stage's MMAs have retired: free its A and BT slots
+        if (c == 0 && ks > 0) {  // the previous stage's MMAs have retired: free its slot
           __syncwarp();
-          if (lane == 0) {
-            mbar_arrive(&bar.empty_a[(k - 1) % R::DA]);
-            mbar_arrive(&bar.empty_t[(k - 1) % R::DT]);
-          }
+          if (lane == 0) mbar_arrive(&empty[(k - 1) % R::D]);
         }
       }
     }
@@ -330,20 +331,17 @@ __device__ __forceinline__ void consumer_loop(const TcArgs &a, uint32_t ring, co
     if (!alive) break;
     if (info.nsteps > 0) {
       __syncwarp();
-      if (lane == 0) {
-        mbar_arrive(&bar.empty_a[(k - 1) % R::DA]);
-        mbar_arrive(&bar.empty_t[(k - 1) % R::DT]);
-      }
+      if (lane == 0) mbar_arrive(&empty[(k - 1) % R::D]);
     }
     // ---- epilogue: Horner over the digit-pair order d = S-1 .. 0, column scales, fp64 partial tile ----
     double *tile_out = a.part + ((size_t)info.sp * a.tiles + info.t) * (TILE * TILE);
 #pragma unroll
     for (int up = 0; up < 2; up++) {
-      const int row = 16 * warp + 2 * g + up;
-      const double isc_row = __ldg(a.isc + info.bi * TILE + row);
-      double *out = tile_out + (size_t)row * TILE + info.h * HALF;
+      const int orow = 16 * warp + g + 8 * up;
+      const double isc_row = __ldg(a.isc + info.bi * TILE + orow);
+      double *out = tile_out + (size_t)orow * TILE + info.h * HALF;
 #pragma unroll
-      for (int j = 0; j < HALF / 8; j++) {
+      for (int j = 0; j < R::N / 8; j++) {
 #pragma unroll
         for (int e = 0; e < 2; e++) {
           const int q = 4 * j + 2 * up + e;
@@ -367,7 +365,7 @@ __device__ __forceinline__ void consumer_loop(const TcArgs &a, uint32_t ring, co
       for (int w = 0; w < 4; w++) o[TR_CONS + 5 * wg + w] = tr[w];
       o[TR_CONS + 5 * wg + 4] = total;
       if (wg == 0) {
-        o[TR_STAGES] = k;
+        o[TR_STAGES] = (FULL ? 2 : 1) * k;
         o[TR_NS] = ns_start;
         o[TR_NS + 1] = globaltimer_ns();
       }
@@ -375,175 +373,108 @@ __device__ __forceinline__ void consumer_loop(const TcArgs &a, uint32_t ring, co
   }
 }
 
-__device__ __forceinline__ void sts_u32(uint32_t addr, uint32_t v) {
-  asm volatile("st.shared.u32 [%0], %1;\n" ::"r"(addr), "r"(v) : "memory");
-}
-
-// One transposer warp (TW = 0..2): the K-major copies of the B half planes of every stage this CTA consumes. Work unit
-// u = (plane p, k32 step c, 16-column chunk q) = 8 p + 4 c + q of a stage; warp TW takes u = TW, TW + 3, ... One
-// ldmatrix.trans of a unit's 4 x 8 contraction rows gives thread (g, t) the k positions 4t..4t+3 and 16+4t..16+4t+3 of
-// columns 16 q + 2 g and 16 q + 2 g + 1. A stage: wait for its B slot, issue all of the warp's ldmatrix loads and
-// release the B slot, wait for a free BT slot, permute and store, publish the BT slot.
-template <int S, int TW, bool TRACE>
-__device__ __forceinline__ void transpose_loop(const TcArgs &a, uint32_t ring, const RingBars &bar) {
-  using R = Rings<S>;
-  constexpr int J = (8 * S - TW + 2) / 3;  // units of this warp per stage, all loaded before any store (4 J <= 44
-                                          // registers of the producer warpgroup's PRODUCER_REGS)
-  const int lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3, i = lane & 7;
-  // source row of this lane: contraction row 8 (lane / 8) + i of a k32 step; 64-byte rows under the 64B swizzle
-  // (chunk q of row r at q ^ ((r >> 1) & 3)), so the 8 rows of each matrix hit 8 different 16-byte bank groups. The row
-  // offset is a multiple of 64, so chunk q of a unit is at (src + slot, plane and step offsets) ^ (q << 4).
-  const uint32_t src = ring + R::B_OFF + ((lane >> 3) * 8 + i) * HALF + ((i >> 1) << 4);
-  // lanes g >= 4 store column 2g + 1 before 2g: the 32 lanes of every store then hit 32 different banks.
-  // bt_offset(c, 16 q + n, kw) for this lane's column n = 2g + flip: c * BT_CHUNK + q * 2 BT_SBO + dst0 (kw = t) or
-  // + BT_LBO (kw = 4 + t); its neighbour n ^ 1 sits at dst0 ^ 16
-  const int flip = g >> 2, n = 2 * g + flip;
-  const uint32_t perm0 = flip ? PERM_ODD : PERM_EVEN, perm1 = flip ? PERM_EVEN : PERM_ODD;
-  const uint32_t dst = ring + R::T_OFF + (n >> 3) * BT_SBO + (n & 7) * 16 + 4 * t;
-  long long tr[3] = {0, 0, 0};  // trace: wait B full, wait BT empty, total
-  RingPos<R::DB> pb;
-  RingPos<R::DT> pt;
-  bool alive = true;
+// The producer (one thread): per stage, the S planes of the A block, then the S planes of the B block (or of its column
+// half), all into one slot; each is one contiguous run of GqT.
+template <int S, bool FULL, bool TRACE>
+__device__ __forceinline__ void producer_loop(const TcArgs &a, uint8_t *ring, uint64_t *full, uint64_t *empty) {
+  using R = Ring<S, FULL>;
+  long long tr = 0;  // trace: wait slot empty
+  int sl = 0;
+  uint32_t ph = 0;
   const int64_t per = rows_per_item(a);
-  for (int item = blockIdx.x; alive && item < n_items(a); item += gridDim.x) {
-    const ItemInfo info = decode_item(a, item, per);
+  for (int item = blockIdx.x; item < n_items<FULL>(a); item += gridDim.x) {
+    const ItemInfo info = decode_item<FULL>(a, item, per);
     for (int ks = 0; ks < info.nsteps; ks++) {
+      // band (k_begin / KS + ks) of the planes, then column bi * 128 (A) or bj * 128 + h * 64 (B) within it
+      const int8_t *band = a.planes_t + (info.k_begin + (int64_t)ks * KS) * a.ldq;
+      const int8_t *src_a = band + (int64_t)info.bi * TILE * KS, *src_b = band + (int64_t)(info.bj * TILE + info.h * HALF) * KS;
       const long long t0 = tclock<TRACE>();
-      const bool ok = __all_sync(0xffffffffu, mbar_wait(&bar.full_b[pb.slot], pb.ph, a.err));
-      if constexpr (TRACE) tr[0] += clock64() - t0;
-      if (!ok) { alive = false; break; }
-      const uint32_t sb = src + pb.slot * R::B_SLOT, db = dst + pt.slot * R::T_SLOT;
-      uint32_t m[J][4];
-#pragma unroll
-      for (int j = 0; j < J; j++) {
-        const int u = TW + 3 * j, p = u >> 3, c = (u >> 2) & 1, q = u & 3;
-        ldsm_x4_trans((sb + p * B_PLANE_BYTES + c * 32 * HALF) ^ (q << 4), m[j]);
-      }
-      // the slot is refilled by TMA (async proxy) once released: the proxy fence orders these generic-proxy reads
-      // before that write. Without it the arrive does not wait for the ldmatrix data, and the refill can overwrite the
-      // slot before it is read.
-      asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bar.empty_b[pb.slot]);
-      const long long t1 = tclock<TRACE>();
-      const bool free_t = __all_sync(0xffffffffu, mbar_wait(&bar.empty_t[pt.slot], pt.ph ^ 1, a.err));
-      if constexpr (TRACE) tr[1] += clock64() - t1;
-      if (!free_t) { alive = false; break; }
-#pragma unroll
-      for (int j = 0; j < J; j++) {
-        const int u = TW + 3 * j, p = u >> 3, c = (u >> 2) & 1, q = u & 3;
-        const uint32_t d = db + p * BT_PLANE_BYTES + c * BT_CHUNK + q * 2 * BT_SBO;
-        sts_u32(d, __byte_perm(m[j][0], m[j][1], perm0));
-        sts_u32(d ^ 16, __byte_perm(m[j][0], m[j][1], perm1));
-        sts_u32(d + BT_LBO, __byte_perm(m[j][2], m[j][3], perm0));
-        sts_u32((d + BT_LBO) ^ 16, __byte_perm(m[j][2], m[j][3], perm1));
-      }
-      asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");  // the copy is read by wgmma (async proxy)
-      __syncwarp();
-      if (lane == 0) {
-        mbar_arrive(&bar.full_t[pt.slot]);
-      }
-      pb.next();
-      pt.next();
-      if constexpr (TRACE) tr[2] += clock64() - t0;
+      if (!mbar_wait(&empty[sl], ph ^ 1, a.err)) return;
+      if constexpr (TRACE) tr += clock64() - t0;
+      uint8_t *slot = ring + sl * R::SLOT;
+      mbar_expect_tx(&full[sl], R::SLOT);
+      for (int s = 0; s < S; s++) bulk_load(slot + s * A_PLANE_BYTES, src_a + s * a.plane, A_PLANE_BYTES, &full[sl]);
+      for (int s = 0; s < S; s++) bulk_load(slot + R::B_OFF + s * R::B_PLANE, src_b + s * a.plane, R::B_PLANE, &full[sl]);
+      if (++sl == R::D) { sl = 0; ph ^= 1; }
     }
   }
-  if constexpr (TRACE) {
-    if (TW == 0 && lane == 0) {
-      unsigned long long *o = a.trace + (size_t)blockIdx.x * TR_WORDS;
-      o[TR_XPOSE] = tr[0];
-      o[TR_XPOSE + 1] = tr[1];
-      o[TR_XPOSE + 2] = tr[2] - tr[0] - tr[1];  // busy
-    }
-  }
+  if constexpr (TRACE) a.trace[(size_t)blockIdx.x * TR_WORDS + TR_PROD] = tr;
 }
 
-// The TMA producer (one thread): per stage, the S planes of the B half block into the B ring first (they still have to
-// be transposed), then the S planes of the A block into the A ring.
-template <int S, bool TRACE>
-__device__ __forceinline__ void producer_loop(const TcArgs &a, const CUtensorMap *tmap_a, const CUtensorMap *tmap_b,
-                                              uint8_t *ring, const RingBars &bar) {
-  using R = Rings<S>;
-  asm volatile("prefetch.tensormap [%0];\n" ::"l"(tmap_a) : "memory");
-  asm volatile("prefetch.tensormap [%0];\n" ::"l"(tmap_b) : "memory");
-  long long tr[2] = {0, 0};  // trace: wait A empty, wait B empty
-  RingPos<R::DA> pa;
-  RingPos<R::DB> pb;
-  bool alive = true;
-  const int64_t per = rows_per_item(a);
-  for (int item = blockIdx.x; alive && item < n_items(a); item += gridDim.x) {
-    const ItemInfo info = decode_item(a, item, per);
-    for (int ks = 0; ks < info.nsteps; ks++) {
-      const int krow = (int)(info.k_begin + (int64_t)ks * KS);
-      const long long t0 = tclock<TRACE>();
-      if (!mbar_wait(&bar.empty_b[pb.slot], pb.ph ^ 1, a.err)) { alive = false; break; }
-      const long long t1 = tclock<TRACE>();
-      uint8_t *sb = ring + R::B_OFF + pb.slot * R::B_SLOT;
-      mbar_expect_tx(&bar.full_b[pb.slot], S * B_PLANE_BYTES);
-      for (int s = 0; s < S; s++)
-        tma_load_3d(sb + s * B_PLANE_BYTES, tmap_b, &bar.full_b[pb.slot], info.bj * TILE + info.h * HALF, krow, s);
-      const long long t2 = tclock<TRACE>();
-      if (!mbar_wait(&bar.empty_a[pa.slot], pa.ph ^ 1, a.err)) { alive = false; break; }
-      if constexpr (TRACE) { tr[0] += clock64() - t2; tr[1] += t1 - t0; }
-      uint8_t *sa = ring + pa.slot * R::A_SLOT;
-      mbar_expect_tx(&bar.full_a[pa.slot], S * A_PLANE_BYTES);
-      for (int s = 0; s < S; s++) tma_load_3d(sa + s * A_PLANE_BYTES, tmap_a, &bar.full_a[pa.slot], info.bi * TILE, krow, s);
-      pa.next();
-      pb.next();
-    }
-  }
-  if constexpr (TRACE) {
-    unsigned long long *o = a.trace + (size_t)blockIdx.x * TR_WORDS;
-    o[TR_PROD] = tr[0];
-    o[TR_PROD + 1] = tr[1];
-  }
-}
-
-template <int S, bool TRACE>
-__device__ __forceinline__ void syrk_tc_cta(const CUtensorMap *tmap_a, const CUtensorMap *tmap_b, const TcArgs &a,
-                                            uint8_t *ring, const RingBars &bar) {
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t ring_u32 = smem_u32(ring);
-  if (warp >= CONSUMER_WARPS) {
+template <int S, bool FULL, bool TRACE>
+__device__ __forceinline__ void syrk_tc_cta(const TcArgs &a, uint8_t *ring, uint64_t *full, uint64_t *empty) {
+  if (threadIdx.x >= 32 * CONSUMER_WARPS) {
     asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;\n" ::"n"(PRODUCER_REGS));
-    // ===================== B transposers (warps 9-11) =====================
-    if (warp == CONSUMER_WARPS + 1) transpose_loop<S, 0, TRACE>(a, ring_u32, bar);
-    else if (warp == CONSUMER_WARPS + 2) transpose_loop<S, 1, TRACE>(a, ring_u32, bar);
-    else if (warp == CONSUMER_WARPS + 3) transpose_loop<S, 2, TRACE>(a, ring_u32, bar);
-    // ===================== TMA producer (warp 8, one thread) =====================
-    else if (lane == 0) producer_loop<S, TRACE>(a, tmap_a, tmap_b, ring, bar);
+    // ===================== producer (warp 8, one thread) =====================
+    if (threadIdx.x == 32 * CONSUMER_WARPS) producer_loop<S, FULL, TRACE>(a, ring, full, empty);
   } else {
     // ===================== wgmma + epilogue =====================
     asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;\n" ::"n"(CONSUMER_REGS));
-    consumer_loop<S, TRACE>(a, ring_u32, bar);
+    consumer_loop<S, FULL, TRACE>(a, smem_u32(ring), full, empty);
   }
 }
 
 template <bool TRACE>
-__global__ void __launch_bounds__(TC_THREADS, 1) syrk_tc_kernel(const __grid_constant__ CUtensorMap tmap_a,
-                                                                const __grid_constant__ CUtensorMap tmap_b, TcArgs a) {
+__global__ void __launch_bounds__(TC_THREADS, 1) syrk_tc_kernel(TcArgs a) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  // 1024-byte aligned rings (the swizzle patterns are functions of the shared-memory address), then barriers
+  // 1024-byte aligned ring (the swizzle patterns are functions of the shared-memory address), then barriers
   uint8_t *ring = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t *bars = reinterpret_cast<uint64_t *>(ring + RING_BYTES);
-  const RingBars bar{bars, bars + MAX_SLOTS, bars + 2 * MAX_SLOTS, bars + 3 * MAX_SLOTS, bars + 4 * MAX_SLOTS,
-                     bars + 5 * MAX_SLOTS};
+  uint64_t *full = reinterpret_cast<uint64_t *>(ring + RING_BYTES), *empty = full + MAX_SLOTS;
   if (threadIdx.x == 0) {
     for (int i = 0; i < MAX_SLOTS; i++) {
-      mbar_init(&bar.full_a[i], 1);
-      mbar_init(&bar.empty_a[i], CONSUMER_WARPS);
-      mbar_init(&bar.full_b[i], 1);
-      mbar_init(&bar.empty_b[i], TRANSPOSE_WARPS);
-      mbar_init(&bar.full_t[i], TRANSPOSE_WARPS);
-      mbar_init(&bar.empty_t[i], CONSUMER_WARPS);
+      mbar_init(&full[i], 1);
+      mbar_init(&empty[i], CONSUMER_WARPS);
     }
     asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
   }
   __syncthreads();
   const int S = *a.S_dev;
-  if (S == 4) syrk_tc_cta<4, TRACE>(&tmap_a, &tmap_b, a, ring, bar);
-  else if (S == 3) syrk_tc_cta<3, TRACE>(&tmap_a, &tmap_b, a, ring, bar);
-  else syrk_tc_cta<2, TRACE>(&tmap_a, &tmap_b, a, ring, bar);
+  if (S == 4) syrk_tc_cta<4, false, TRACE>(a, ring, full, empty);
+  else if (S == 3 && a.full) syrk_tc_cta<3, true, TRACE>(a, ring, full, empty);
+  else if (S == 3) syrk_tc_cta<3, false, TRACE>(a, ring, full, empty);
+  else if (a.full) syrk_tc_cta<2, true, TRACE>(a, ring, full, empty);
+  else syrk_tc_cta<2, false, TRACE>(a, ring, full, empty);
+}
+
+// K-major copy of the digit planes for s < *S_dev: band b = row / 64 of plane s of Gq [rows][ldq] becomes the run
+// GqT[s][b][ldq][64], column n's 64 contraction rows as one 64-byte row whose 16-byte chunk q sits at q ^ ((n >> 1) & 3):
+// the shared-memory image wgmma reads (sw64_desc) of every 128- or 64-column block of the band. A block moves a 64-row x
+// 128-column tile through shared memory: coalesced 16-byte loads of the MN-major rows, 4 x 4 byte transposes of words,
+// then the tile's 8 KB output run.
+constexpr int KT_ROWS = KS, KT_COLS = 128, KT_THREADS = 256;
+__global__ void __launch_bounds__(KT_THREADS) tc_kmajor_kernel(const int8_t *__restrict__ Gq, int8_t *__restrict__ GqT,
+                                                               int ldq, int64_t plane, const int *S_dev) {
+  const int s = blockIdx.z;
+  if (s >= *S_dev) return;
+  __shared__ uint32_t tile[KT_ROWS][KT_COLS / 4 + 1];
+  const int64_t r0 = (int64_t)blockIdx.x * KT_ROWS;
+  const int c0 = blockIdx.y * KT_COLS;
+  const int8_t *src = Gq + s * plane + r0 * ldq + c0;
+#pragma unroll
+  for (int p = 0; p < KT_ROWS * KT_COLS / 16 / KT_THREADS; p++) {
+    const int idx = threadIdx.x + p * KT_THREADS, r = idx >> 3, ch = idx & 7;
+    const uint4 v = __ldg(reinterpret_cast<const uint4 *>(src + (int64_t)r * ldq) + ch);
+    tile[r][4 * ch] = v.x;
+    tile[r][4 * ch + 1] = v.y;
+    tile[r][4 * ch + 2] = v.z;
+    tile[r][4 * ch + 3] = v.w;
+  }
+  __syncthreads();
+  int8_t *dst = GqT + s * plane + r0 * ldq + (int64_t)c0 * KS;  // band r0 / 64, column c0
+#pragma unroll
+  for (int p = 0; p < KT_ROWS * KT_COLS / 16 / KT_THREADS; p++) {
+    const int idx = threadIdx.x + p * KT_THREADS, kq = idx & 15, m = idx >> 4;  // rows 4 kq.., columns 4 m..
+    const uint32_t w0 = tile[4 * kq][m], w1 = tile[4 * kq + 1][m], w2 = tile[4 * kq + 2][m], w3 = tile[4 * kq + 3][m];
+    const uint32_t lo01 = __byte_perm(w0, w1, 0x5140), hi01 = __byte_perm(w0, w1, 0x7362);
+    const uint32_t lo23 = __byte_perm(w2, w3, 0x5140), hi23 = __byte_perm(w2, w3, 0x7362);
+    const uint32_t out[4] = {__byte_perm(lo01, lo23, 0x5410), __byte_perm(lo01, lo23, 0x7632),
+                             __byte_perm(hi01, hi23, 0x5410), __byte_perm(hi01, hi23, 0x7632)};
+#pragma unroll
+    for (int j = 0; j < 4; j++) {
+      const int n = 4 * m + j;  // column within the tile (c0 is a multiple of 8: the same swizzle row)
+      *reinterpret_cast<uint32_t *>(dst + n * KS + ((((kq >> 2) ^ (n >> 1)) & 3) << 4) + 4 * (kq & 3)) = out[j];
+    }
+  }
 }
 
 // Column scales and digit-plane count of one batch, decided ON THE DEVICE from the column maxima and sums of squares
@@ -637,13 +568,8 @@ __global__ void tc_adopt_kernel(double *sc, double *isc, int *S_dev, const doubl
 }
 
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
-                                  const cuuint64_t *, const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
 struct TcState {
-  CUtensorMap map_a;        // box {128, KS, 1}, 128-byte swizzle: the A block
-  CUtensorMap map_b;        // box {64, KS, 1}, 64-byte swizzle: one column half of the B block
+  int8_t *GqT = nullptr;    // [SMAX][rows_alloc / KS][ldg][KS] K-major copy of c->Gq (tc_kmajor_kernel)
   double *sc = nullptr, *isc = nullptr;
   double *sc_next = nullptr, *isc_next = nullptr;  // fresh scales of the last full-range evaluation (speculation)
   int *S_next = nullptr, *spec_ok = nullptr;
@@ -660,49 +586,33 @@ struct TcState {
   int64_t last_rows_padded = 0;  // contraction rows of the last batch's SYRK (0: none since the registration)
 };
 
-// The two tensor maps of a digit-plane buffer [SMAX][rows_alloc][ldq] (int8, column index fastest): the A block
-// (box {128, KS, 1}, 128-byte swizzle) and one column half of the B block (box {64, KS, 1}, 64-byte swizzle).
-int encode_tc_maps(int8_t *planes, int ldq, int64_t rows_alloc, CUtensorMap *map_a, CUtensorMap *map_b) {
-  EncodeTiledFn encode = nullptr;
-  cudaDriverEntryPointQueryResult qres;
-  CUDA_TRY(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", (void **)&encode, cudaEnableDefault, &qres));
-  if (!encode || qres != cudaDriverEntryPointSuccess) {
-    balm_set_error("cuTensorMapEncodeTiled not available from the driver");
-    return BALM_ERR_CUDA;
-  }
-  const cuuint64_t dims[3] = {(cuuint64_t)ldq, (cuuint64_t)rows_alloc, (cuuint64_t)SMAX};
-  const cuuint64_t strides[2] = {(cuuint64_t)ldq, (cuuint64_t)ldq * rows_alloc};
-  const cuuint32_t estr[3] = {1, 1, 1};
-  const cuuint32_t box_a[3] = {TILE, KS, 1};
-  if (encode(map_a, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, planes, dims, strides, box_a, estr,
-             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS) {
-    balm_set_error("cuTensorMapEncodeTiled (A block) failed");
-    return BALM_ERR_CUDA;
-  }
-  const cuuint32_t box_b[3] = {HALF, KS, 1};
-  if (encode(map_b, CU_TENSOR_MAP_DATA_TYPE_UINT8, 3, planes, dims, strides, box_b, estr,
-             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS) {
-    balm_set_error("cuTensorMapEncodeTiled (B half block) failed");
-    return BALM_ERR_CUDA;
-  }
+// The K-major copy of the first rows_padded rows of the planes Gq [SMAX][rows_alloc][ldq] into GqT (same plane size),
+// the *S_dev planes in use only.
+int launch_tc_kmajor(balm_ctx *c, const int8_t *Gq, int8_t *GqT, int ldq, int64_t rows_alloc, int64_t rows_padded,
+                     const int *S_dev) {
+  const dim3 grid((unsigned)(rows_padded / KT_ROWS), (unsigned)(ldq / KT_COLS), SMAX);
+  tc_kmajor_kernel<<<grid, KT_THREADS, 0, c->stream>>>(Gq, GqT, ldq, rows_alloc * ldq, S_dev);
+  CUDA_TRY(cudaGetLastError());
+  c->launches += 1;
   return BALM_OK;
 }
 
-// One syrk_tc_kernel launch on c's stream: rows_padded (a multiple of KS) contraction rows of the planes behind the
-// maps, nb x nb blocks of 128 columns, `splits` k-splits; one CTA per item up to one per SM.
+// One syrk_tc_kernel launch on c's stream: rows_padded (a multiple of KS) contraction rows of the K-major planes
+// planes_t (plane stride `plane` bytes), nb x nb blocks of 128 columns, `splits` k-splits; one CTA per item up to one per SM. Whole 128 x 128 tiles
+// (at S <= 3) halve the L2 traffic per MAC but also the item count, so they are taken only when every SM still gets
+// an item (tiles x splits >= SMs); BALM_TC_TILE=half|full (c->tc_tile) overrides the rule.
 // With c->tc_trace (BALM_TC_TRACE) the traced instantiation runs and records the launch.
-int launch_syrk_tc(balm_ctx *c, const CUtensorMap &map_a, const CUtensorMap &map_b, int64_t rows_padded, int nb,
-                   int tiles, int splits, const int *S_dev, const double *isc, double *part, bool accumulate, int *err) {
-  TcArgs a{rows_padded, nb, tiles, splits, S_dev, isc, part, accumulate ? 1 : 0, err, c->tc_trace};
-  const int items = a.tiles * 2 * a.splits;
+int launch_syrk_tc(balm_ctx *c, const int8_t *planes_t, int64_t plane, int64_t rows_padded, int nb, int tiles,
+                   int splits, const int *S_dev, const double *isc, double *part, bool accumulate, int *err) {
+  const bool full = c->tc_tile == 0 ? (int64_t)tiles * splits >= c->sm_count : c->tc_tile == 2;
+  TcArgs a{planes_t, plane, c->ldg, rows_padded, nb, tiles, splits, full ? 1 : 0, S_dev, isc, part, accumulate ? 1 : 0, err, c->tc_trace};
+  const int items = a.tiles * 2 * a.splits;  // half-tile items; the whole-tile count when S <= 3 is not known here
   const int grid = items < c->sm_count ? items : c->sm_count;
   if (c->tc_trace) {
     CUDA_TRY(cudaMemsetAsync(c->tc_trace, 0, sizeof(unsigned long long) * c->sm_count * TR_WORDS, c->stream));
-    syrk_tc_kernel<true><<<grid, TC_THREADS, TC_SMEM, c->stream>>>(map_a, map_b, a);
+    syrk_tc_kernel<true><<<grid, TC_THREADS, TC_SMEM, c->stream>>>(a);
   } else {
-    syrk_tc_kernel<false><<<grid, TC_THREADS, TC_SMEM, c->stream>>>(map_a, map_b, a);
+    syrk_tc_kernel<false><<<grid, TC_THREADS, TC_SMEM, c->stream>>>(a);
   }
   CUDA_TRY(cudaGetLastError());
   return BALM_OK;
@@ -731,6 +641,8 @@ int tensor_syrk_init(balm_ctx *c) {
   st->rows_alloc = (3 * c->VB + KS - 1) / KS * KS;
   CUDA_TRY(cudaMalloc((void **)&c->Gq, (size_t)SMAX * st->rows_alloc * ldq));
   CUDA_TRY(cudaMemset(c->Gq, 0, (size_t)SMAX * st->rows_alloc * ldq));  // column padding [6N, ldg) stays zero
+  CUDA_TRY(cudaMalloc((void **)&st->GqT, (size_t)SMAX * st->rows_alloc * ldq));
+  CUDA_TRY(cudaMemset(st->GqT, 0, (size_t)SMAX * st->rows_alloc * ldq));
   CUDA_TRY(cudaMalloc((void **)&st->S_dev, sizeof(int)));
   CUDA_TRY(cudaMalloc((void **)&st->sc, sizeof(double) * ldq));
   CUDA_TRY(cudaMalloc((void **)&st->isc, sizeof(double) * ldq));
@@ -746,7 +658,6 @@ int tensor_syrk_init(balm_ctx *c) {
   CUDA_TRY(cudaMemset(st->err, 0, sizeof(int)));
   c->colmax = st->colmax;  // the observation pass writes the column maxima here
 
-  TRY(encode_tc_maps(c->Gq, ldq, st->rows_alloc, &st->map_a, &st->map_b));
   // int32 exactness bound: every (tile, split) item contracts at most MAX_ROWS_PER_ITEM rows
   const int64_t rows = 3 * c->VB;
   const int min_splits = (int)((rows + MAX_ROWS_PER_ITEM - 1) / MAX_ROWS_PER_ITEM);
@@ -765,6 +676,7 @@ void tensor_syrk_free(balm_ctx *c) {
     TcState *st = static_cast<TcState *>(c->tmap);
     cudaFree(st->sc_next); cudaFree(st->isc_next); cudaFree(st->S_next); cudaFree(st->spec_ok);
     cudaFree(st->sc); cudaFree(st->isc); cudaFree(st->colmax); cudaFree(st->err); cudaFree(st->S_dev);
+    cudaFree(st->GqT);
     delete st;
     c->tmap = nullptr;
   }
@@ -774,7 +686,8 @@ void tensor_syrk_free(balm_ctx *c) {
 }
 
 // One batch of the tensor path: (1) column maxima of G' -> power-of-two scales, (2) observation sweep writing the
-// int8 digit planes directly, (3) tensor-core SYRK. ev[2] is recorded between the observation sweeps and the SYRK.
+// int8 digit planes directly, (3) their K-major copy and the tensor-core SYRK. ev[2] is recorded between the
+// observation sweeps and the K-major copy, so the SYRK's time includes the copy.
 int tensor_obs_and_syrk(balm_ctx *c, const double *poses, int64_t v0, int64_t v1, bool first_batch) {
   TcState *st = static_cast<TcState *>(c->tmap);
   if (!st) { balm_set_error("tensor path not initialised"); return BALM_ERR_INVALID; }
@@ -810,8 +723,9 @@ int tensor_obs_and_syrk(balm_ctx *c, const double *poses, int64_t v0, int64_t v1
   st->last_rows_padded = rows_padded;
   CUDA_TRY(cudaEventRecord(c->ev[2], c->stream));
   c->launches += 2;
-  return launch_syrk_tc(c, st->map_a, st->map_b, rows_padded, c->syrk_nb, c->syrk_tiles, c->syrk_splits, st->S_dev,
-                        st->isc, c->syrk_part, !first_batch, st->err);
+  TRY(launch_tc_kmajor(c, c->Gq, st->GqT, ldq, st->rows_alloc, rows_padded, st->S_dev));
+  return launch_syrk_tc(c, st->GqT, plane_stride, rows_padded, c->syrk_nb, c->syrk_tiles, c->syrk_splits,
+                        st->S_dev, st->isc, c->syrk_part, !first_batch, st->err);
 }
 
 // The SYRK's error flag, the digit-plane count and the speculation verdict of the batch in flight: the copies are
@@ -874,10 +788,11 @@ extern "C" int balm_debug_syrk_tc(balm_ctx *c, const int8_t *planes, int S, int6
   CUDA_TRY(cudaSetDevice(c->device));
   const size_t plane = (size_t)rows_padded * ldq, count = (size_t)splits * tiles * TILE * TILE;
   ScratchPool pool;
-  int8_t *d_planes;
+  int8_t *d_planes, *d_planes_t;
   double *d_isc, *d_part;
   int *d_S, *d_err;
   TRY(pool.get(&d_planes, SMAX * plane));
+  TRY(pool.get(&d_planes_t, SMAX * plane));
   TRY(pool.get(&d_isc, (size_t)ldq));
   TRY(pool.get(&d_part, count));
   TRY(pool.get(&d_S, 1));
@@ -890,10 +805,10 @@ extern "C" int balm_debug_syrk_tc(balm_ctx *c, const int8_t *planes, int S, int6
   CUDA_TRY(cudaMemcpyAsync(d_part, part, sizeof(double) * count, cudaMemcpyHostToDevice, c->stream));
   CUDA_TRY(cudaMemcpyAsync(d_S, &S, sizeof(int), cudaMemcpyHostToDevice, c->stream));
   CUDA_TRY(cudaMemsetAsync(d_err, 0, sizeof(int), c->stream));
-  CUtensorMap map_a, map_b;
-  TRY(encode_tc_maps(d_planes, ldq, rows_padded, &map_a, &map_b));
   TRY(syrk_tc_set_smem());
-  TRY(launch_syrk_tc(c, map_a, map_b, rows_padded, nb, tiles, splits, d_S, d_isc, d_part, accumulate != 0, d_err));
+  TRY(launch_tc_kmajor(c, d_planes, d_planes_t, ldq, rows_padded, rows_padded, d_S));
+  TRY(launch_syrk_tc(c, d_planes_t, (int64_t)plane, rows_padded, nb, tiles, splits, d_S, d_isc, d_part, accumulate != 0,
+                     d_err));
   int err = 0;
   CUDA_TRY(cudaMemcpyAsync(&err, d_err, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
   CUDA_TRY(cudaMemcpyAsync(part, d_part, sizeof(double) * count, cudaMemcpyDeviceToHost, c->stream));

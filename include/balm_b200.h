@@ -468,14 +468,16 @@ int balm_debug_dag_trace(balm_ctx *ctx, unsigned long long *out, int max_entries
 /* Debug aid: with BALM_TC_TRACE=1 in the environment when a tensor-precision ctx is created, the last tensor SYRK launch
  * (of an evaluation or of balm_debug_syrk_tc) records clock64 sums per role, 18 words per CTA, CTA b at 18 b (CTAs
  * beyond the launch's grid hold zeros):
- *   0 stages (64-row contraction steps) the CTA consumed; 1, 2 %globaltimer (ns) at the start and the end of consumer
- *   warp 0, whose total below spans the same interval;
- *   3..7 consumer warp 0 and 8..12 consumer warp 4 (one per warpgroup): waiting on A full, waiting on the transposed B
- *   full, in wgmma.wait_group, epilogue, total;
- *   13..15 transposer warp 9: waiting on B full, waiting on a free transposed-B slot, busy;
- *   16, 17 TMA producer: waiting on a free A slot, waiting on a free B slot.
+ *   0 stages (64-row contraction steps) the CTA consumed, in 128 x 64 half-tile units (a stage of a whole 128 x 128
+ *   tile counts 2); 1, 2 %globaltimer (ns) at the start and the end of consumer warp 0, whose total below spans the same
+ *   interval;
+ *   3..7 consumer warp 0 and 8..12 consumer warp 4 (one per warpgroup): waiting on the stage full, in the warpgroup's
+ *   vote that it arrived, in wgmma.wait_group, epilogue, total;
+ *   13..15 zero (there is no transposer warp any more);
+ *   16 producer: waiting on a free slot; 17 zero.
  * Copies min(max_entries, 18 x SM count) words; BALM_ERR_INVALID when the ctx records no trace. Without the variable
- * the SYRK runs an instantiation that reads no clock. */
+ * the SYRK runs an instantiation that reads no clock. BALM_TC_TILE=half|full at ctx creation forces the SYRK's item
+ * shape (default: whole tiles at S <= 3 when tiles x k-splits >= the SM count). */
 int balm_debug_tc_trace(balm_ctx *ctx, unsigned long long *out, int max_entries);
 /* Debug aid: the tensor path's SYRK kernel alone, on caller-supplied digit planes, so that its fp64 partial tiles can be
  * compared bit for bit with an exact integer reference. Uses ctx's device, stream and column count ldg = 6N rounded up

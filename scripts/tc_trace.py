@@ -1,8 +1,9 @@
 #!/usr/bin/env python
 """Where a stage of the tensor SYRK (syrk_tc_kernel) spends its clocks, by role (BALM_TC_TRACE=1): the benchmark's C3
 scene (500 poses x 100 000 plane voxels, tensor path), a few evaluations, then the trace of the last SYRK launch.
-Prints clocks per 64-row stage (mean over the CTAs, and over the busiest CTA) of every category of
-balm_debug_tc_trace, the stage count and the SM clock derived from the globaltimer pair.
+Prints clocks per 64-row stage of a 128 x 64 half tile (a whole-tile stage counts as two; mean over the CTAs, and over
+the busiest CTA) of every category of balm_debug_tc_trace, the stage count and the SM clock derived from the globaltimer
+pair. BALM_TC_TILE=half|full in the environment forces the item shape.
 Usage: python scripts/tc_trace.py [N_POSES [N_VOXELS]]"""
 import ctypes as C
 import json
@@ -18,10 +19,9 @@ import balm_b200  # noqa: E402
 from balm_b200 import _lib as L  # noqa: E402
 
 WORDS = 18
-ROLES = [("consumer warp 0", 3, ["wait A full", "wait BT full", "wgmma.wait_group", "epilogue", "total"]),
-         ("consumer warp 4", 8, ["wait A full", "wait BT full", "wgmma.wait_group", "epilogue", "total"]),
-         ("transposer warp 9", 13, ["wait B full", "wait BT empty", "busy"]),
-         ("producer", 16, ["wait A empty", "wait B empty"])]
+ROLES = [("consumer warp 0", 3, ["wait stage full", "warpgroup vote", "wgmma.wait_group", "epilogue", "total"]),
+         ("consumer warp 4", 8, ["wait stage full", "warpgroup vote", "wgmma.wait_group", "epilogue", "total"]),
+         ("producer", 16, ["wait slot empty"])]
 
 N = int(sys.argv[1]) if len(sys.argv) > 1 else 500
 M = int(sys.argv[2]) if len(sys.argv) > 2 else 100000
