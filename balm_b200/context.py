@@ -51,6 +51,14 @@ def _pose_graph_iter(fn, handle, N, poses12, max_iter, u0, v0, rel_tol, gauge_mo
     return poses, tr
 
 
+def _covariance(fn, handle, poses12, n_pairs, *args):
+    """balm_spg_covariance / balm_block_covariance -> [n_pairs, 6, 6] blocks (rows of pose i, columns of pose j)."""
+    poses12 = np.ascontiguousarray(poses12, dtype=np.float64)
+    cov = np.zeros((n_pairs, 36))
+    L.check(fn(handle, _p(poses12), *args, _p(cov)))
+    return cov.reshape(-1, 6, 6).transpose(0, 2, 1)
+
+
 class Context:
     """One GPU, one registered set of plane voxels, N poses."""
 
@@ -159,6 +167,14 @@ class Context:
         b = np.zeros((npairs, 36))
         L.check(L.lib().balm_download_blocks(self._h, _p(b)))
         return b.reshape(npairs, 6, 6).transpose(0, 2, 1).copy()
+
+    def block_covariance(self, poses12, include_fix=False, anchor=0):
+        """PREC_BLOCKS contexts: Sigma = (H without pose anchor's rows and columns)^-1 on H's block pattern, H as
+        evaluate(poses12, include_fix=include_fix) returns it (anchor=-1: nothing deleted; fix clusters must then fix the
+        gauge). -> (pairs [n_pairs, 2] (i <= j), cov [n_pairs, 6, 6]) with cov[p, a, c] = Sigma[6 i + a, 6 j + c]."""
+        pairs = self.block_structure(want_pairs=True)["pair_list"]
+        return pairs, _covariance(L.lib().balm_block_covariance, self._h, poses12, len(pairs), int(include_fix),
+                                  int(anchor))
 
     def solve(self, u):
         dx = np.zeros(self.n)
@@ -624,6 +640,16 @@ class PoseGraph:
         r = C.c_double()
         L.check(L.lib().balm_spg_evaluate(self._h, _p(poses12), _p(blocks), _p(g), C.byref(r)))
         return pairs, blocks.reshape(-1, 6, 6).transpose(0, 2, 1), g, r.value
+
+    def covariance(self, poses12, anchor=0):
+        """Marginal covariances: Sigma = (H without pose anchor's rows and columns)^-1 on H's block pattern, H the
+        Gauss-Newton Hessian at poses12 (anchor=-1: nothing deleted, which leaves the gauge free: ERR_NOT_PD).
+        -> (pairs [n_pairs, 2] (i <= j), cov [n_pairs, 6, 6]) with cov[p, a, c] = Sigma[6 i + a, 6 j + c]."""
+        st = np.zeros(4, dtype=np.int64)
+        L.check(L.lib().balm_spg_structure(self._h, _p(st), None))
+        pairs = np.zeros((int(st[0]), 2), dtype=np.int32)
+        L.check(L.lib().balm_spg_structure(self._h, _p(st), _p(pairs)))
+        return pairs, _covariance(L.lib().balm_spg_covariance, self._h, poses12, len(pairs), int(anchor))
 
     def pose_graph_iter(self, poses12, max_iter=10, u0=0.01, v0=2.0, rel_tol=1e-6, gauge_mode=0, verbose=False,
                         want_per_iter=False, force_hess=False):

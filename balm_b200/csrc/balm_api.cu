@@ -1217,6 +1217,17 @@ extern "C" int balm_spg_iter(balm_spg *sp, double *poses12, const balm_lm_opts *
   return pose_graph_lm(s, poses12, o, trace, n_iters, poses_per_iter);
 }
 
+extern "C" int balm_spg_covariance(balm_spg *s, const double *poses12, int anchor, double *cov) {
+  if (!s || !poses12 || !cov) { balm_set_error("balm_spg_covariance: bad arguments"); return BALM_ERR_INVALID; }
+  if (!s->pg) { balm_set_error("balm_spg_covariance: no pose factors registered"); return BALM_ERR_INVALID; }
+  if (anchor < -1 || anchor >= s->N) { balm_set_error("balm_spg_covariance: anchor outside [-1, N)"); return BALM_ERR_INVALID; }
+  CUDA_TRY(cudaSetDevice(s->device));
+  return sparse_covariance(s->solver, s->stream, anchor, [&]() -> int {
+    CUDA_TRY(cudaMemcpyAsync(s->poses, poses12, sizeof(double) * 12 * s->N, cudaMemcpyHostToDevice, s->stream));
+    return pose_graph_eval_blocks(s->pg, s->stream, s->poses, s->blocks, s->g, s->scal, &s->launches);
+  }, "balm_spg_covariance", cov, &s->launches);
+}
+
 // ---------------- sliding window on the registered voxel set (assoc.cu) ----------------
 // A sliding-window build of the batch (batch_marginalize_build, batch_append_build, window_push_build) run as its
 // one-problem case into scratch buffers, then registered as the context's voxel set, with fix clusters when `fix` and
@@ -1511,4 +1522,25 @@ extern "C" int balm_download_blocks(balm_ctx *c, double *blocks) {
   CUDA_TRY(cudaMemcpyAsync(blocks, blocks_device(c->bh), sizeof(double) * nbl, cudaMemcpyDeviceToHost, c->stream));
   CUDA_TRY(cudaStreamSynchronize(c->stream));
   return BALM_OK;
+}
+
+extern "C" int balm_block_covariance(balm_ctx *c, const double *poses12, int include_fix, int anchor, double *cov) {
+  if (!c || !poses12 || !cov) { balm_set_error("balm_block_covariance: bad arguments"); return BALM_ERR_INVALID; }
+  if (c->prec != BALM_PREC_BLOCKS || !c->bh || !c->registered) {
+    balm_set_error("balm_block_covariance: no voxels registered on a BALM_PREC_BLOCKS context");
+    return BALM_ERR_INVALID;
+  }
+  if (anchor < -1 || anchor >= c->N) { balm_set_error("balm_block_covariance: anchor outside [-1, N)"); return BALM_ERR_INVALID; }
+  CUDA_TRY(cudaSetDevice(c->device));
+  // the evaluation is deferred (its events are read after sparse_covariance's waits), so the call waits twice
+  const int rc = sparse_covariance(blocks_solver(c->bh), c->stream, anchor, [&]() -> int {
+    CUDA_TRY(cudaMemcpyAsync(c->poses, poses12, sizeof(double) * 12 * c->N, cudaMemcpyHostToDevice, c->stream));
+    c->defer = true;
+    const int e = balm_cov_evaluate_hessian(c, c->poses, include_fix != 0);
+    c->defer = false;
+    return e;
+  }, "balm_block_covariance", cov, &c->launches);
+  if (rc == BALM_OK || rc == BALM_ERR_NOT_PD) TRY(collect_eval(c));  // the stream has been synchronised
+  c->pending_eval = false;
+  return rc;
 }

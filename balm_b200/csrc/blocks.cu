@@ -251,6 +251,7 @@ int blocks_refine(balm_ctx *c, int *still_bad) {
 
 const std::vector<int2> &blocks_pairs(const BlockHessian *b) { return b->pairs; }
 const double *blocks_device(const BlockHessian *b) { return b->blocks; }
+SparseSolver *blocks_solver(const BlockHessian *b) { return b->solver; }
 
 long long blocks_bytes(const BlockHessian *b, int64_t *l_blocks, int64_t *levels) {
   int64_t sb = 0;

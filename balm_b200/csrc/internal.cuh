@@ -784,6 +784,14 @@ void sparse_solver_stats(const SparseSolver *s, int64_t *l_blocks, int64_t *leve
 int sparse_solve(SparseSolver *s, cudaStream_t st);
 // refine_solution's rounds with the same factors; *still_bad when omega stayed above the tolerance (waits)
 int sparse_refine(SparseSolver *s, cudaStream_t st, int *h_flags, double *h_scal, int *still_bad);
+// Marginal covariances: cov (host, [pairs][36] in the registration's pair order, rows of pose i, columns of pose j,
+// column-major) = (H without the anchor's rows and columns)^-1 on H's block pattern, 0 on the anchor's blocks (anchor in
+// [-1, P), checked by the caller). The first call builds the selected-inversion tables (BALM_ERR_UNSUPPORTED, before
+// eval and with nothing changed, when too large). eval leaves H in the solver's blocks (enqueued); then the undamped
+// factorisation overwrites L, D, dvec and scal[3], BALM_ERR_NOT_PD (message prefixed with who) when it is singular.
+// Waits twice (pivot test, copy-out), and once more on the first call while it builds the tables.
+int sparse_covariance(SparseSolver *s, cudaStream_t st, int anchor, const std::function<int()> &eval, const char *who,
+                      double *cov, long long *launches);
 
 // ---------------- block-sparse Hessian of a BALM_PREC_BLOCKS context (blocks.cu) ----------------
 // The registered voxels' pair pattern, update terms and symbolic factorisation -> c->bh (replacing the previous one).
@@ -797,6 +805,7 @@ int blocks_solve(balm_ctx *c, double u);
 int blocks_refine(balm_ctx *c, int *still_bad);
 const std::vector<int2> &blocks_pairs(const BlockHessian *b);
 const double *blocks_device(const BlockHessian *b);
+SparseSolver *blocks_solver(const BlockHessian *b);
 // device bytes of the pattern, terms, blocks and solver; l_blocks / levels of the factorisation
 long long blocks_bytes(const BlockHessian *b, int64_t *l_blocks, int64_t *levels);
 

@@ -14,6 +14,12 @@
 //   spg_back_kernel      per column of one level, top level first, one warp: D^-1 and the backward substitution
 //   spg_check_kernel     per row: r = -g - A dx over the pose's pairs in ascending order, the componentwise backward
 //                        error omega (the dense solve's check, same tolerance)
+// Marginal covariances (sparse_covariance; DESIGN.md "Marginal covariances"): H factored undamped with one pose held
+// fixed, then the entries of H^-1 on L's pattern by selected inversion, gathered onto H's pattern.
+//   spg_anchor_kernel    one CTA: the anchor's row and column of L's blocks zeroed, its diagonal block I
+//   spg_selinv_kernel    per column of one level, top level first, one CTA: L^ = L L_jj^-1 in place, the column's Z
+//                        blocks from its ancestors' (a warp per block), then its diagonal block
+//   spg_cov_gather_kernel  per (pair, entry): Z's block of every pair of H
 #include <math.h>
 #include <algorithm>
 #include <memory>
@@ -24,6 +30,7 @@
 namespace {
 
 constexpr int SP_THREADS = 512;
+constexpr int SEL_THREADS = 256;  // spg_selinv_kernel: its 36-entry accumulators need more than 128 registers
 constexpr int ND_LEAF = 32;  // nested dissection stops at this many poses; a leaf keeps index order
 
 struct SpView {      // L and D as the level kernels read them
@@ -215,6 +222,133 @@ __global__ void __launch_bounds__(256) spg_check_kernel(const double *Hb, const 
   atomicMax(reinterpret_cast<unsigned long long *>(omega_out), (unsigned long long)__double_as_longlong(om));
 }
 
+// The covariance's anchored copy: after spg_damp_kernel with u = 0, every block of column ac and of row ac becomes 0 and
+// the diagonal block I, so that the factorisation is that of H without the anchor's rows and columns (one CTA).
+__global__ void __launch_bounds__(256) spg_anchor_kernel(SpView v, int ac) {
+  const int c0 = v.colptr[ac], nc = v.colptr[ac + 1] - c0, r0 = v.rptr[ac], nr = v.rptr[ac + 1] - r0;
+  for (int t = threadIdx.x; t < 36 * (nc + nr); t += 256) {
+    const int q = t / 36, e = t % 36;
+    const int b = q < nc ? c0 + q : v.rpos[r0 + q - nc];
+    v.Lx[36 * (size_t)b + e] = (b == c0 && e % 7 == 0) ? 1.0 : 0.0;
+  }
+}
+
+// Selected inversion (Takahashi), one CTA per column j of a level, top level first: with L^_kj = L_kj L_jj^-1 and
+// S = struct(j),
+//   Z_ij = -sum_{k in S} Z_ik L^_kj   (i in S),      Z_jj = L_jj^-T D_j^-1 L_jj^-1 - sum_{k in S} L^_kj^T Z_kj,
+// where every Z_ik belongs to an ancestor column (S is a clique of L's pattern). Block t of the column's off-diagonal
+// blocks sums the terms sterm[sptr[j] + t m + u], u = 0 .. m - 1 (ascending k = S[u]): 2 position of Z_ik's block
+// (max, min) + transposed; L^_kj is the column's block 1 + u. L_Sj is overwritten with L^_Sj (nothing else reads it
+// before the next factorisation).
+__global__ void __launch_bounds__(SEL_THREADS) spg_selinv_kernel(SpView v, const int *cols, const long long *sptr,
+                                                                const int *sterm, double *Z) {
+  __shared__ double Minv[36], S[36];
+  const int j = cols[blockIdx.x], tid = threadIdx.x, lane = tid & 31;
+  const int b0 = v.colptr[j], m = v.colptr[j + 1] - b0 - 1;
+  const double *Ljj = v.Lx + 36 * (size_t)b0;
+  // L^_kj: x L_jj = b for every row b of an off-diagonal block, one thread per row
+  for (int q = tid; q < 6 * m; q += SEL_THREADS) {
+    double *B = v.Lx + 36 * (size_t)(b0 + 1 + q / 6);
+    const int a = q % 6;
+    double x[6];
+#pragma unroll
+    for (int c = 5; c >= 0; c--) {
+      double s = B[6 * c + a];
+#pragma unroll
+      for (int r = c + 1; r < 6; r++) s -= x[r] * Ljj[6 * c + r];
+      x[c] = s;
+    }
+#pragma unroll
+    for (int c = 0; c < 6; c++) B[6 * c + a] = x[c];
+  }
+  if (tid == SEL_THREADS - 1) {  // L_jj^-1, unit lower, column-major
+    for (int c = 0; c < 6; c++)
+      for (int r = 0; r < 6; r++) {
+        double s = r == c ? 1.0 : 0.0;
+        for (int p = c; p < r; p++) s -= Ljj[6 * p + r] * Minv[6 * c + p];
+        Minv[6 * c + r] = r < c ? 0.0 : s;
+      }
+  }
+  __syncthreads();
+  // Z_ij: one warp per block, lane l summing the terms l, l + 32, ..., then the lanes' sums in a fixed butterfly
+  for (int t = tid >> 5; t < m; t += SEL_THREADS / 32) {
+    double acc[36];
+#pragma unroll
+    for (int e = 0; e < 36; e++) acc[e] = 0.0;
+    const int *w = sterm + sptr[j] + (long long)t * m;
+    for (int u = lane; u < m; u += 32) {
+      const int x = w[u];
+      const double *Zk = Z + 36 * (size_t)(x >> 1), *Lk = v.Lx + 36 * (size_t)(b0 + 1 + u);
+      const int sa = (x & 1) ? 6 : 1, sp = (x & 1) ? 1 : 6;  // Z_ik[a][p] = Zk[sa a + sp p]
+#pragma unroll
+      for (int p = 0; p < 6; p++) {
+        double zi[6], lk[6];
+#pragma unroll
+        for (int a = 0; a < 6; a++) {
+          zi[a] = Zk[sa * a + sp * p];
+          lk[a] = Lk[6 * a + p];
+        }
+#pragma unroll
+        for (int c = 0; c < 6; c++)
+#pragma unroll
+          for (int a = 0; a < 6; a++) acc[6 * c + a] = fma(zi[a], lk[c], acc[6 * c + a]);
+      }
+    }
+    double *Zb = Z + 36 * (size_t)(b0 + 1 + t);
+#pragma unroll
+    for (int e = 0; e < 36; e++) {
+      const double s = -warp_sum(acc[e]);
+      if (lane == (e & 31)) Zb[e] = s;
+    }
+  }
+  __syncthreads();
+  // sum_k L^_kj^T Z_kj over the column's blocks by warp 0, the same lane split and butterfly
+  if (tid < 32) {
+    double acc[36];
+#pragma unroll
+    for (int e = 0; e < 36; e++) acc[e] = 0.0;
+    for (int u = lane; u < m; u += 32) {
+      const double *Lk = v.Lx + 36 * (size_t)(b0 + 1 + u), *Zk = Z + 36 * (size_t)(b0 + 1 + u);
+#pragma unroll
+      for (int p = 0; p < 6; p++) {
+        double lk[6], zk[6];
+#pragma unroll
+        for (int a = 0; a < 6; a++) {
+          lk[a] = Lk[6 * a + p];
+          zk[a] = Zk[6 * a + p];
+        }
+#pragma unroll
+        for (int c = 0; c < 6; c++)
+#pragma unroll
+          for (int a = 0; a < 6; a++) acc[6 * c + a] = fma(lk[a], zk[c], acc[6 * c + a]);
+      }
+    }
+#pragma unroll
+    for (int e = 0; e < 36; e++) {
+      const double s = warp_sum(acc[e]);
+      if (lane == (e & 31)) S[e] = s;
+    }
+  }
+  __syncthreads();
+  if (tid < 36) {  // entry (hi, lo) of the lower triangle into both of its places: exactly symmetric
+    const int a = tid % 6, c = tid / 6, hi = a > c ? a : c, lo = a > c ? c : a;
+    double e = 0.0;
+    for (int r = hi; r < 6; r++) e += Minv[6 * hi + r] * Minv[6 * lo + r] / v.D[6 * (size_t)j + r];
+    Z[36 * (size_t)b0 + tid] = e - S[6 * lo + hi];
+  }
+}
+
+// cov, per (pair, entry): the pair's block of Z (zsrc: 2 position + transposed, the inverse of lsrc); 0 on the anchor
+// column ac's row and column
+__global__ void __launch_bounds__(256) spg_cov_gather_kernel(const double *Z, const int *zsrc, SpView v, long long npairs,
+                                                             int ac, double *cov) {
+  const long long t = (long long)blockIdx.x * 256 + threadIdx.x;
+  if (t >= 36 * npairs) return;
+  const int s = zsrc[t / 36], e = (int)(t % 36), r = e % 6, c = e / 6, pos = s >> 1;
+  const double z = Z[36 * (size_t)pos + ((s & 1) ? 6 * r + c : 6 * c + r)];
+  cov[t] = (v.rowidx[pos] == ac || v.lcol[pos] == ac) ? 0.0 : z;
+}
+
 // ---- ordering: nested dissection of the pose graph (xadj / adj: CSR of every pose's neighbours) ----
 // A vertex set (ascending pose index) of more than ND_LEAF poses is cut at its median index; the separator is a greedy
 // vertex cover of the crossing edges (most uncovered crossing edges first, the lower index on a tie). The two halves
@@ -273,11 +407,18 @@ struct SparseSolver {
   double *dvec = nullptr, *dx = nullptr, *scal = nullptr;
   int *flags = nullptr;
   cudaGraphExec_t exec = nullptr;
+  // selected inversion (sparse_covariance), built by its first call: terms of every column (sptr [P+1], sterm), the
+  // inverse of lsrc (zsrc [pairs]), Z [nb][36], and on the host the column of every pose
+  long long npairs = 0, nsel = 0;
+  long long *sptr = nullptr;
+  int *sterm = nullptr, *zsrc = nullptr;
+  double *Z = nullptr;
+  std::vector<int> col_of;
   ~SparseSolver() {
     if (exec) cudaGraphExecDestroy(exec);
     cudaFree(perm); cudaFree(colptr); cudaFree(rowidx); cudaFree(lcol); cudaFree(lsrc); cudaFree(rptr); cudaFree(rpos);
     cudaFree(levcols); cudaFree(pp_ptr); cudaFree(tptr); cudaFree(term); cudaFree(pp); cudaFree(Lx); cudaFree(D);
-    cudaFree(y); cudaFree(xs); cudaFree(rres);
+    cudaFree(y); cudaFree(xs); cudaFree(rres); cudaFree(sptr); cudaFree(sterm); cudaFree(zsrc); cudaFree(Z);
   }
   SpView view() const { return SpView{colptr, rowidx, lcol, tptr, term, rptr, rpos, perm, Lx, D, flags}; }
   template <typename T>
@@ -334,6 +475,7 @@ int sparse_solver_build(cudaStream_t st, int P, const std::vector<int2> &pairs, 
   std::unique_ptr<SparseSolver> s(new SparseSolver());
   s->P = P;
   const long long npairs = (long long)pairs.size();
+  s->npairs = npairs;
   if (npairs >= (1LL << 30)) return too_large(who, "too many block pairs");
   // the pose graph's adjacency
   std::vector<long long> xadj(P + 1, 0);
@@ -522,5 +664,118 @@ int sparse_refine(SparseSolver *s, cudaStream_t st, int *h_flags, double *h_scal
     CUDA_TRY(cudaStreamSynchronize(st));
     if (h_flags[4] == 0) { *still_bad = 0; break; }
   }
+  return BALM_OK;
+}
+
+// The selected inversion's tables from the registered structure (host, once): column k with S = struct(k), m = |S|,
+// gives its block t the terms u = 0 .. m - 1 at sptr[k] + t m + u: the position of block (S[max(t,u)], S[min(t,u)])
+// (found by the factor table's merge walk down column S[min]) times 2, + 1 when t < u (Z_ik read transposed).
+static int selinv_build(SparseSolver &s, cudaStream_t st, const char *who) {
+  const int P = s.P;
+  const long long nb = s.nb;
+  std::vector<int> colptr(P + 1), rowidx(nb), lsrc(nb), perm(P);
+  CUDA_TRY(cudaMemcpyAsync(colptr.data(), s.colptr, sizeof(int) * (P + 1), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaMemcpyAsync(rowidx.data(), s.rowidx, sizeof(int) * nb, cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaMemcpyAsync(lsrc.data(), s.lsrc, sizeof(int) * nb, cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaMemcpyAsync(perm.data(), s.perm, sizeof(int) * P, cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  std::vector<long long> sptr(P + 1, 0);
+  for (int k = 0; k < P; k++) {
+    const long long m = colptr[k + 1] - colptr[k] - 1;
+    sptr[k + 1] = sptr[k] + m * m;
+  }
+  const long long nsel = sptr[P];
+  // int positions of Z (< 2^31 / 36, packed with the flag) are always in range; the count is what can outgrow a card
+  if (nsel >= (1LL << 33)) return too_large(who, "2^33 or more selected-inversion terms");
+  std::vector<int> sterm(nsel), zsrc(s.npairs);
+  for (int k = 0; k < P; k++) {
+    const int k0 = colptr[k] + 1, m = colptr[k + 1] - k0;
+    int *w = sterm.data() + sptr[k];
+    for (int u = 0; u < m; u++) {
+      int q = colptr[rowidx[k0 + u]];
+      for (int t = u; t < m; t++) {
+        while (rowidx[q] != rowidx[k0 + t]) q++;
+        w[(size_t)t * m + u] = 2 * q;
+        if (t != u) w[(size_t)u * m + t] = 2 * q + 1;
+      }
+    }
+  }
+  for (long long b = 0; b < nb; b++)
+    if (lsrc[b] >= 0) zsrc[lsrc[b] >> 1] = (int)(2 * b + (lsrc[b] & 1));
+  s.col_of.assign(P, 0);
+  for (int j = 0; j < P; j++) s.col_of[perm[j]] = j;
+  ScratchPool pool;  // nothing is kept unless every allocation succeeds
+  long long *d_sptr = nullptr;
+  int *d_sterm = nullptr, *d_zsrc = nullptr;
+  double *d_Z = nullptr;
+  long long bytes = 0;
+  auto get = [&](auto **p, size_t n) {
+    bytes += (long long)(sizeof(**p) * (n ? n : 1));
+    return pool.get(p, n);
+  };
+  TRY(get(&d_sptr, sptr.size()));
+  TRY(get(&d_sterm, sterm.size()));
+  TRY(get(&d_zsrc, zsrc.size()));
+  TRY(get(&d_Z, 36 * (size_t)nb));
+  CUDA_TRY(cudaMemcpyAsync(d_sptr, sptr.data(), sizeof(long long) * sptr.size(), cudaMemcpyHostToDevice, st));
+  if (nsel) CUDA_TRY(cudaMemcpyAsync(d_sterm, sterm.data(), sizeof(int) * nsel, cudaMemcpyHostToDevice, st));
+  if (s.npairs) CUDA_TRY(cudaMemcpyAsync(d_zsrc, zsrc.data(), sizeof(int) * zsrc.size(), cudaMemcpyHostToDevice, st));
+  CUDA_TRY(cudaStreamSynchronize(st));  // the host tables are freed on return
+  for (void *q : {(void *)d_sptr, (void *)d_sterm, (void *)d_zsrc, (void *)d_Z}) pool.release(q);
+  s.sptr = d_sptr;
+  s.sterm = d_sterm;
+  s.zsrc = d_zsrc;
+  s.Z = d_Z;
+  s.nsel = nsel;
+  s.bytes += bytes;
+  return BALM_OK;
+}
+
+int sparse_covariance(SparseSolver *s, cudaStream_t st, int anchor, const std::function<int()> &eval, const char *who,
+                      double *cov, long long *launches) {
+  if (!s->Z) TRY(selinv_build(*s, st, who));
+  TRY(eval());
+  const SpView v = s->view();
+  const int P = s->P, nlev = (int)s->lev_ptr.size() - 1, ac = anchor >= 0 ? s->col_of[anchor] : -1;
+  // the undamped copy (u = 0 in scal[3]; the next solve writes its own), the anchor's blocks, the factorisation (its
+  // forward substitution on g runs into the scratch y)
+  CUDA_TRY(cudaMemsetAsync(s->flags, 0, sizeof(int) * 8, st));
+  CUDA_TRY(cudaMemsetAsync(s->scal + 3, 0, sizeof(double), st));
+  if (s->nb) spg_damp_kernel<<<(unsigned)((36 * s->nb + 255) / 256), 256, 0, st>>>(s->Hb, s->lsrc, v, s->nb, s->scal + 3,
+                                                                                   s->dvec);
+  if (ac >= 0) spg_anchor_kernel<<<1, 256, 0, st>>>(v, ac);
+  for (int l = 0; l < nlev; l++)
+    spg_factor_kernel<true><<<s->lev_ptr[l + 1] - s->lev_ptr[l], SP_THREADS, 0, st>>>(v, s->levcols + s->lev_ptr[l], s->g,
+                                                                                      -1.0, s->y);
+  CUDA_TRY(cudaGetLastError());
+  *launches += 2 + nlev;
+  // singular: a bad pivot, or over every column but the anchor's min d <= 1e-11 max d (balm_pose_covariance's rule
+  // with positive pivots; the anchor's unit pivots would hide the scale of H)
+  std::vector<double> d(6 * (size_t)P);
+  int bad = 0;
+  CUDA_TRY(cudaMemcpyAsync(d.data(), s->D, sizeof(double) * d.size(), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaMemcpyAsync(&bad, s->flags, sizeof(int), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  double dmin = INFINITY, dmax = 0.0;
+  for (int j = 0; j < P; j++)
+    if (j != ac)
+      for (int m = 0; m < 6; m++) {
+        dmin = std::min(dmin, d[6 * (size_t)j + m]);
+        dmax = std::max(dmax, d[6 * (size_t)j + m]);
+      }
+  if (bad || !(dmin > 0.0 && dmin > 1e-11 * dmax && dmax < INFINITY)) {
+    balm_set_error(std::string(who) + ": H with the anchor's rows and columns deleted is singular");
+    return BALM_ERR_NOT_PD;
+  }
+  // Z top level first, then cov gathered into L's storage (no longer needed) and copied out
+  for (int l = nlev - 1; l >= 0; l--)
+    spg_selinv_kernel<<<s->lev_ptr[l + 1] - s->lev_ptr[l], SEL_THREADS, 0, st>>>(v, s->levcols + s->lev_ptr[l], s->sptr,
+                                                                                s->sterm, s->Z);
+  if (s->npairs)
+    spg_cov_gather_kernel<<<(unsigned)((36 * s->npairs + 255) / 256), 256, 0, st>>>(s->Z, s->zsrc, v, s->npairs, ac, s->Lx);
+  CUDA_TRY(cudaGetLastError());
+  *launches += nlev + 1;
+  CUDA_TRY(cudaMemcpyAsync(cov, s->Lx, sizeof(double) * 36 * s->npairs, cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
   return BALM_OK;
 }

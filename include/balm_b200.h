@@ -440,6 +440,25 @@ int balm_spg_evaluate(balm_spg *spg, const double *poses12, double *blocks, doub
  * rules) on the sparse solve. */
 int balm_spg_iter(balm_spg *spg, double *poses12, const balm_lm_opts *opts, balm_trace *trace, int *n_iters,
                   double *poses_per_iter);
+/* Marginal pose covariances (DESIGN.md "Marginal covariances"): H evaluated undamped at poses12, the 6 rows and columns
+ * of pose `anchor` deleted when anchor >= 0 (H~), and Sigma = H~^-1 restricted to H's block pattern: 36 doubles per
+ * block pair (rows of pose i, columns of pose j, column-major) in balm_spg_structure's order, written to cov. Blocks
+ * touching the anchor are 0; diagonal blocks are exactly symmetric. Coordinates are those of the LM pose update,
+ * delta = (dtheta, dp) with T <- (Exp(dtheta) R, Exp(dtheta) p + dp); the factors' H are information matrices, so Sigma
+ * is the Laplace covariance of the estimate. H has the 6-dimensional gauge null space of a common left transform:
+ * anchor = 0 is the normal call. anchor in [-1, N).
+ * BALM_ERR_NOT_PD (cov not written) when H~ is singular: a bad pivot, or over every column but the anchor's the smallest
+ * LDL^T pivot is not > 1e-11 x the largest (e.g. two unconnected components, a pose in no factor, anchor = -1).
+ * BALM_ERR_INVALID for a null argument, no registered factors or an anchor out of range; BALM_ERR_UNSUPPORTED, with
+ * nothing changed, when the selected-inversion tables are too large to index.
+ * The first call after a registration builds those tables (device bytes grow by 288 per block of L, 4 per term with
+ * Sigma_j |struct(j)|^2 terms, 4 per pair and 8 per pose; balm_spg_structure's stats[3] counts them); later calls reuse
+ * them until the next
+ * registration. Afterwards the handle's blocks, g and factor storage hold this call's evaluation (H at poses12, undamped);
+ * the next balm_spg_iter re-evaluates and refactors, so its results are bitwise those without the covariance call.
+ * The call waits for the device twice (the pivot test and the copy-out), the first one also while it builds the
+ * tables. */
+int balm_spg_covariance(balm_spg *spg, const double *poses12, int anchor, double *cov);
 
 /* Block-sparse Hessian of a BALM_PREC_BLOCKS context (BALM_ERR_INVALID on any other, or before a registration).
  * stats: [0] block pairs (i <= j) of H, [1] blocks of the factor L, [2] elimination-tree levels, [3] device bytes the
@@ -448,6 +467,14 @@ int balm_block_structure(balm_ctx *ctx, int64_t stats[4], int32_t *pairs);
 /* The last evaluation's blocks, bitwise what the solve consumed: 36 doubles per pair (rows of pose i, columns of pose
  * j, column-major) in balm_block_structure's order. */
 int balm_download_blocks(balm_ctx *ctx, double *blocks);
+/* balm_spg_covariance's Sigma on a BALM_PREC_BLOCKS context: H~^-1 on H's block pattern, in balm_block_structure's order,
+ * with H as balm_evaluate returns it at poses12 over every voxel (include_fix as in balm_pose_covariance). This is the
+ * inverse of the library's Hessian, not balm_pose_covariance's propagated point noise: scaling it by a point-noise model
+ * is the caller's job. A registration whose fix clusters anchor the gauge can use anchor = -1 with include_fix = 1;
+ * without them anchor = -1 is BALM_ERR_NOT_PD. BALM_ERR_INVALID also on any other kind of context or before a
+ * registration. Tables, errors and side effects as balm_spg_covariance's: afterwards balm_download_blocks returns H at
+ * poses12, and the next balm_damping_iter is bitwise what it would have been without this call. */
+int balm_block_covariance(balm_ctx *ctx, const double *poses12, int include_fix, int anchor, double *cov);
 
 /* Multi-GPU: voxels are sharded across ranks by the caller (each rank registers its own shard); the library
  * all-reduces [H | g | r] with NCCL after every evaluation and the scalar after every residual pass.
