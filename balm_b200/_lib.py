@@ -57,7 +57,7 @@ SYMBOLS = ["balm_last_error", "balm_version", "balm_create", "balm_destroy", "ba
            "balm_batch_window_push", "balm_batch_merge_scans", "balm_set_pose_factors", "balm_pose_graph_evaluate",
            "balm_pose_graph_iter", "balm_spg_create", "balm_spg_destroy", "balm_spg_set_factors", "balm_spg_structure",
            "balm_spg_evaluate", "balm_spg_iter", "balm_spg_covariance", "balm_block_structure", "balm_download_blocks",
-           "balm_block_covariance"]
+           "balm_block_covariance", "balm_block_set_factors"]
 
 
 def lib():
@@ -149,6 +149,7 @@ def lib():
         L.balm_block_structure.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
         L.balm_download_blocks.argtypes = [C.c_void_p, C.c_void_p]
         L.balm_block_covariance.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]
+        L.balm_block_set_factors.argtypes = [C.c_void_p, C.c_int] + [C.c_void_p] * 5
         _lib = L
     return _lib
 

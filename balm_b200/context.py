@@ -176,6 +176,17 @@ class Context:
         return pairs, _covariance(L.lib().balm_block_covariance, self._h, poses12, len(pairs), int(include_fix),
                                   int(anchor))
 
+    def set_block_factors(self, factors):
+        """PREC_BLOCKS contexts: pose factors (set_pose_factors' dicts, e.g. from odometry_factors) in the cost, added to
+        the voxel cost in every evaluation over all voxels, damping_iter, block_covariance (include/balm_b200.h,
+        balm_block_set_factors). Their H must be in the voxel cost's units (points x m^2). min_planes_per_pose still
+        counts voxels only: pass 0 when factors carry scans that see no plane. [] detaches the set; a rejected call
+        keeps the previous one. -> per factor OK or ERR_NOT_PD (left out of the cost)."""
+        if not factors:
+            L.check(L.lib().balm_block_set_factors(self._h, 0, None, None, None, None, None))
+            return []
+        return _set_pose_factors(L.lib().balm_block_set_factors, self._h, factors)
+
     def solve(self, u):
         dx = np.zeros(self.n)
         q1 = C.c_double()

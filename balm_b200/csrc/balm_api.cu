@@ -582,6 +582,8 @@ static int evaluate_dev(balm_ctx *c, const double *poses, int64_t head, int64_t 
   // defer mode (LM loop, whole problem in one batch): nothing is waited for here; collect_eval() reads the events and
   // the tensor path's flags after the iteration's single synchronisation
   const bool deferred = c->defer && head == 0 && end == c->M && c->VB >= c->M && end > head;
+  // a blocks context's pose factors are part of every full-range evaluation (sub-ranges stay voxels only)
+  const bool factors = c->prec == BALM_PREC_BLOCKS && c->pg && head == 0 && end == c->M;
   c->pending_stats_cached = stats_cached;
   if (head == end) {  // empty range (or an empty shard): this rank contributes H = 0, g = 0, r = 0 -- and still enters
     // the all-reduce below, which the other ranks of a multi-GPU job are waiting in
@@ -622,9 +624,10 @@ static int evaluate_dev(balm_ctx *c, const double *poses, int64_t head, int64_t 
     first = false;
   }
   CUDA_TRY(cudaMemcpyAsync(c->scal + BALM_SCAL_RCUR, r_dev, sizeof(double), cudaMemcpyDeviceToDevice, c->stream));  // local, pre all-reduce
-  if (end > head) {
+  if (end > head || factors) {
     CUDA_TRY(cudaEventRecord(c->ev[4], c->stream));
     if (c->prec != BALM_PREC_BLOCKS) TRY(launch_assemble(c));
+    if (factors) TRY(blocks_add_factors(c, poses));  // after the RCUR copy above: the hand-over caches voxels only
     CUDA_TRY(cudaEventRecord(c->ev[5], c->stream));
   }
   if (c->world > 1 && c->comm) {  // the assembly wrote the lower triangle | g into c->Hpack (an empty range: zeros)
@@ -644,7 +647,7 @@ static int evaluate_dev(balm_ctx *c, const double *poses, int64_t head, int64_t 
   }
   CUDA_TRY(cudaEventSynchronize(c->ev[6]));
   cudaEventElapsedTime(&ms, c->ev[4], c->ev[5]);
-  if (c->prec != BALM_PREC_BLOCKS) c->tm.ms_assemble += ms;
+  if (c->prec != BALM_PREC_BLOCKS || factors) c->tm.ms_assemble += ms;
   cudaEventElapsedTime(&ms, c->ev[5], c->ev[6]); c->tm.ms_allreduce += ms;
   c->tm.n_eval += 1;
   return BALM_OK;
@@ -660,7 +663,7 @@ static int collect_eval(balm_ctx *c) {
   cudaEventElapsedTime(&ms, c->ev[1], c->ev[2]); c->tm.ms_obs += ms;
   cudaEventElapsedTime(&ms, c->ev[2], c->ev[3]); c->tm.ms_syrk += ms;
   cudaEventElapsedTime(&ms, c->ev[4], c->ev[5]);
-  if (c->prec != BALM_PREC_BLOCKS) c->tm.ms_assemble += ms;
+  if (c->prec != BALM_PREC_BLOCKS || c->pg) c->tm.ms_assemble += ms;  // deferred: always full range
   cudaEventElapsedTime(&ms, c->ev[5], c->ev[6]); c->tm.ms_allreduce += ms;
   c->tm.n_eval += 1;
   if (c->prec == BALM_PREC_TENSOR) return tensor_syrk_check_finish(c);
@@ -674,6 +677,7 @@ static int residual_dev(balm_ctx *c, const double *poses, double *host_out, bool
   CUDA_TRY(cudaMemsetAsync(r_dev, 0, sizeof(double), c->stream));
   TRY(launch_voxel_stats(c, poses, 0, c->M, keep_stats ? c->stats_trial : nullptr, true, r_dev));
   CUDA_TRY(cudaMemcpyAsync(c->scal + BALM_SCAL_RTRIAL, r_dev, sizeof(double), cudaMemcpyDeviceToDevice, c->stream));  // local, pre all-reduce
+  if (c->prec == BALM_PREC_BLOCKS && c->pg) TRY(blocks_add_factor_cost(c, poses, r_dev));  // after RTRIAL: voxels only
   TRY(allreduce_sum(c, r_dev, 1));
   CUDA_TRY(cudaEventRecord(c->ev[8], c->stream));
   CUDA_TRY(cudaMemcpyAsync(c->h_scal + 2, r_dev, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
@@ -950,6 +954,28 @@ extern "C" int balm_set_pose_factors(balm_ctx *c, int n_factors, const int64_t *
   TRY(pose_factors_check("balm_set_pose_factors", c->N, n_factors, factor_ptr, factor_pose, poses_hat12, H));
   CUDA_TRY(cudaSetDevice(c->device));
   return pose_graph_set(c, n_factors, factor_ptr, factor_pose, poses_hat12, H, status_out);
+}
+
+extern "C" int balm_block_set_factors(balm_ctx *c, int n_factors, const int64_t *factor_ptr, const int32_t *factor_pose,
+                                      const double *poses_hat12, const double *H, int32_t *status_out) {
+  const char *who = "balm_block_set_factors";
+  if (!c) { balm_set_error(std::string(who) + ": bad arguments"); return BALM_ERR_INVALID; }
+  if (c->prec != BALM_PREC_BLOCKS) {
+    balm_set_error(std::string(who) + ": BALM_PREC_BLOCKS contexts only (the dense ones take balm_set_pose_factors)");
+    return BALM_ERR_INVALID;
+  }
+  if (n_factors != 0) TRY(pose_factors_check(who, c->N, n_factors, factor_ptr, factor_pose, poses_hat12, H));
+  CUDA_TRY(cudaSetDevice(c->device));
+  PoseGraph *pg = nullptr;
+  std::vector<int> status;
+  if (n_factors != 0)  // 0 detaches the factor set
+    TRY(pose_graph_build(c->stream, c->N, n_factors, factor_ptr, factor_pose, poses_hat12, H, &status, &pg, &c->launches));
+  std::unique_ptr<PoseGraph, void (*)(PoseGraph *)> pg_own(pg, pose_graph_free);
+  if (c->bh) TRY(blocks_repattern(c, pg, who));  // no voxels registered yet: the next registration builds the union
+  if (status_out) std::copy(status.begin(), status.end(), status_out);
+  pose_graph_free(c->pg);
+  c->pg = pg_own.release();
+  return BALM_OK;
 }
 
 extern "C" int balm_pose_graph_evaluate(balm_ctx *c, const double *poses12, double *H, double *g, double *cost) {
@@ -1505,7 +1531,8 @@ extern "C" int balm_block_structure(balm_ctx *c, int64_t stats[4], int32_t *pair
   const size_t dbl = 18 * K + 10 * (size_t)c->Kp + (c->fix ? 10 * M : 0) + M + 2 * M * BALM_STATS_STRIDE + 10 * M +
                      (size_t)(c->obs_chunks + 2) * BALM_ACC * c->Np + 24 * N + 3 * n + 8 + 32 + c->res_blocks;
   const size_t ints = K + (M + 1) * 2 + 2 * N + 8 + (c->csc_ptr ? 2 * K + 3 * N + 1 : 0);
-  stats[3] = blocks_bytes(c->bh, &stats[1], &stats[2]) + (int64_t)(sizeof(double) * dbl + sizeof(int) * ints);
+  stats[3] = blocks_bytes(c->bh, &stats[1], &stats[2]) + (int64_t)(sizeof(double) * dbl + sizeof(int) * ints) +
+             (c->pg ? pose_graph_bytes(c->pg) : 0);
   if (pairs)
     for (size_t p = 0; p < pr.size(); p++) { pairs[2 * p] = pr[p].x; pairs[2 * p + 1] = pr[p].y; }
   return BALM_OK;

@@ -9,24 +9,41 @@
 //   (18 doubles) instead of the dense G'; blocks_kernel sums, per pair, the terms' outer products, one warp per pair,
 //   lane l taking the terms l, l + 32, ... and the lanes' sums meeting in warp_sum's fixed butterfly. The block is minus
 //   that sum, plus the observation sweep's diagonal block on a diagonal pair. fp64 throughout, no floating-point atomics.
+//   Pose factors (balm_block_set_factors, DESIGN.md "Voxels and pose factors in one cost"): the pattern is the union of
+//   the voxel pairs, the active factors' pairs and the diagonal (block_pattern_build, rebuilt without re-sorting the
+//   voxel terms when only the factors change); a full-range evaluation adds the factor sums of pose_graph.cu onto the
+//   voxel blocks, g and residual, each entry once, in that order.
 #include <cub/cub.cuh>
 #include <algorithm>
 #include <memory>
 #include <vector>
 #include "internal.cuh"
 
-struct BlockHessian {
+// The union pattern: the voxel pairs, the pairs of the context's active pose factors and every diagonal pair (i, i),
+// each pair's voxel terms (none for a pair no voxel gives), the blocks and their solver.
+struct BlockPattern {
   std::vector<int2> pairs;           // host: (i, j), i <= j, ascending
-  long long nterm = 0, bytes = 0;
+  long long bytes = 0;
   int2 *pair_dev = nullptr;          // [pairs]
   long long *tptr = nullptr;         // [pairs + 1] terms of pair p: term[tptr[p] .. tptr[p+1])
-  unsigned long long *term = nullptr;  // [nterm] observation of pose i (low word) | of pose j (high word), voxel-ascending
   double *blocks = nullptr;          // [pairs][36] column-major, rows of pose i
+  int *fmap = nullptr;               // [factor pairs] index in `pairs` of each of pose_graph_pairs (with factors only)
+  double *fgc = nullptr;             // [n + 1] the factors' g and cost before they are added (with factors only)
   SparseSolver *solver = nullptr;
-  ~BlockHessian() {
+  ~BlockPattern() {
     sparse_solver_free(solver);
-    cudaFree(pair_dev); cudaFree(tptr); cudaFree(term); cudaFree(blocks);
+    cudaFree(pair_dev); cudaFree(tptr); cudaFree(blocks); cudaFree(fmap); cudaFree(fgc);
   }
+};
+
+struct BlockHessian {
+  std::vector<unsigned long long> vkey;  // host: pose pair i * N + j (i <= j) of every pair that shares a voxel, ascending
+  std::vector<int> vcnt;                 // host: its number of terms
+  long long nterm = 0;
+  unsigned long long *term = nullptr;  // [nterm] observation of pose i (low word) | of pose j (high word), pair-major,
+                                       // voxel-ascending within a pair
+  std::unique_ptr<BlockPattern> pat;
+  ~BlockHessian() { cudaFree(term); }
 };
 
 void block_hessian_free(BlockHessian *b) { delete b; }
@@ -119,7 +136,70 @@ __global__ void __launch_bounds__(256) blocks_kernel(const int2 *pairs, const lo
   }
 }
 
+// y[t] += x[t]: a blocks context's factor g and cost added onto the voxel ones (one add per entry, fixed order)
+__global__ void add_kernel(const double *x, int n, double *y) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t < n) y[t] += x[t];
+}
+
 }  // namespace
+
+// The union of bh's voxel pairs, pg's pairs (pg may be null) and every diagonal pair, in ascending (i, j): a pair no
+// voxel gives gets an empty term range (a pose in no voxel and no factor gets a zero block, hence a zero pivot). Then
+// the blocks, the factor map and the symbolic factorisation -> *out.
+static int block_pattern_build(balm_ctx *c, const BlockHessian &bh, const PoseGraph *pg, const char *who,
+                               std::unique_ptr<BlockPattern> *out) {
+  const int N = c->N;
+  cudaStream_t st = c->stream;
+  std::unique_ptr<BlockPattern> u(new BlockPattern());
+  static const std::vector<int2> none;
+  const std::vector<int2> &fp = pg ? pose_graph_pairs(pg) : none;
+  std::vector<long long> tptr;
+  std::vector<int> fmap;
+  u->pairs.reserve(bh.vkey.size() + N);
+  tptr.reserve(bh.vkey.size() + N + 1);
+  fmap.reserve(fp.size());
+  tptr.push_back(0);
+  size_t q = 0, r = 0;  // cursors into the voxel and the factor pairs
+  const unsigned long long none_left = ~0ull;
+  for (int i = 0; i < N; i++) {
+    const unsigned long long row_end = (unsigned long long)(i + 1) * N;
+    bool diag = true;  // the diagonal pair is the smallest key of row i
+    for (;;) {
+      const unsigned long long kv = q < bh.vkey.size() && bh.vkey[q] < row_end ? bh.vkey[q] : none_left;
+      const unsigned long long kf = r < fp.size() && fp[r].x == i ? (unsigned long long)i * N + fp[r].y : none_left;
+      const unsigned long long k = diag ? (unsigned long long)i * N + i : std::min(kv, kf);
+      if (k == none_left) break;
+      diag = false;
+      u->pairs.push_back(make_int2(i, (int)(k - (unsigned long long)i * N)));
+      tptr.push_back(tptr.back() + (kv == k ? bh.vcnt[q++] : 0));
+      if (kf == k) { fmap.push_back((int)u->pairs.size() - 1); r++; }
+    }
+  }
+  const size_t np = u->pairs.size();
+  if (np >= ((size_t)1 << 30)) {
+    balm_set_error(std::string(who) + ": 2^30 or more block pairs");
+    return BALM_ERR_UNSUPPORTED;
+  }
+  TRY(dev_alloc(&u->pair_dev, np));
+  TRY(dev_alloc(&u->tptr, np + 1));
+  TRY(dev_alloc(&u->blocks, 36 * np));
+  CUDA_TRY(cudaMemcpyAsync(u->pair_dev, u->pairs.data(), sizeof(int2) * np, cudaMemcpyHostToDevice, st));
+  CUDA_TRY(cudaMemcpyAsync(u->tptr, tptr.data(), sizeof(long long) * (np + 1), cudaMemcpyHostToDevice, st));
+  CUDA_TRY(cudaMemsetAsync(u->blocks, 0, sizeof(double) * 36 * np, st));
+  u->bytes = (long long)(np * (sizeof(int2) + sizeof(long long) + 36 * sizeof(double)) + sizeof(long long));
+  if (pg) {
+    TRY(dev_alloc(&u->fmap, fmap.size()));
+    TRY(dev_alloc(&u->fgc, (size_t)c->n + 1));
+    if (!fmap.empty())
+      CUDA_TRY(cudaMemcpyAsync(u->fmap, fmap.data(), sizeof(int) * fmap.size(), cudaMemcpyHostToDevice, st));
+    u->bytes += (long long)(sizeof(int) * std::max<size_t>(1, fmap.size()) + sizeof(double) * ((size_t)c->n + 1));
+  }
+  TRY(sparse_solver_build(st, N, u->pairs, u->blocks, c->g, c->dvec, c->dx, c->scal, c->flags, who, &u->solver));
+  CUDA_TRY(cudaStreamSynchronize(st));  // the host tables above are freed on return
+  *out = std::move(u);
+  return BALM_OK;
+}
 
 int block_hessian_build(balm_ctx *c, const char *who) {
   const int N = c->N;
@@ -131,8 +211,6 @@ int block_hessian_build(balm_ctx *c, const char *who) {
     balm_set_error(std::string(who) + ": " + what);
     return (int)BALM_ERR_UNSUPPORTED;
   };
-  std::vector<unsigned long long> ukey;
-  std::vector<int> ucnt;
   if (M > 0) {
     long long *cnt = nullptr, *off = nullptr;
     TRY(pool.get(&cnt, (size_t)M + 1));
@@ -175,10 +253,10 @@ int block_hessian_build(balm_ctx *c, const char *who) {
     CUDA_TRY(cudaMemcpyAsync(&nr, nruns, sizeof(int), cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
     if (nr + (long long)N >= (1LL << 30)) return refuse("2^30 or more block pairs");
-    ukey.resize(nr);
-    ucnt.resize(nr);
-    CUDA_TRY(cudaMemcpyAsync(ukey.data(), uk, sizeof(unsigned long long) * nr, cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaMemcpyAsync(ucnt.data(), uc, sizeof(int) * nr, cudaMemcpyDeviceToHost, st));
+    bh->vkey.resize(nr);
+    bh->vcnt.resize(nr);
+    CUDA_TRY(cudaMemcpyAsync(bh->vkey.data(), uk, sizeof(unsigned long long) * nr, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(bh->vcnt.data(), uc, sizeof(int) * nr, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
     CUDA_TRY(cudaGetLastError());
     c->launches += 5;
@@ -186,75 +264,75 @@ int block_hessian_build(balm_ctx *c, const char *who) {
     bh->term = dv.Current();
     pool.release(bh->term);
   }
-  // the pairs with every diagonal pair added (a pose in no voxel gets a zero block, hence a zero pivot)
-  std::vector<long long> tptr;
-  bh->pairs.reserve(ukey.size() + N);
-  tptr.reserve(ukey.size() + N + 1);
-  tptr.push_back(0);
-  size_t q = 0;
-  for (int i = 0; i < N; i++) {
-    const unsigned long long diag = (unsigned long long)i * N + i;
-    if (q == ukey.size() || ukey[q] != diag) {
-      bh->pairs.push_back(make_int2(i, i));
-      tptr.push_back(tptr.back());
-    }
-    for (; q < ukey.size() && ukey[q] < (unsigned long long)(i + 1) * N; q++) {
-      bh->pairs.push_back(make_int2(i, (int)(ukey[q] - (unsigned long long)i * N)));
-      tptr.push_back(tptr.back() + ucnt[q]);
-    }
-  }
-  const size_t np = bh->pairs.size();
-  TRY(dev_alloc(&bh->pair_dev, np));
-  TRY(dev_alloc(&bh->tptr, np + 1));
-  TRY(dev_alloc(&bh->blocks, 36 * np));
-  CUDA_TRY(cudaMemcpyAsync(bh->pair_dev, bh->pairs.data(), sizeof(int2) * np, cudaMemcpyHostToDevice, st));
-  CUDA_TRY(cudaMemcpyAsync(bh->tptr, tptr.data(), sizeof(long long) * (np + 1), cudaMemcpyHostToDevice, st));
-  CUDA_TRY(cudaMemsetAsync(bh->blocks, 0, sizeof(double) * 36 * np, st));
-  TRY(sparse_solver_build(st, N, bh->pairs, bh->blocks, c->g, c->dvec, c->dx, c->scal, c->flags, who, &bh->solver));
-  bh->bytes = (long long)(np * (sizeof(int2) + sizeof(long long) + 36 * sizeof(double)) + sizeof(long long) +
-                          sizeof(unsigned long long) * bh->nterm);
+  TRY(block_pattern_build(c, *bh, c->pg, who, &bh->pat));
   block_hessian_free(c->bh);
   c->bh = bh.release();
   return BALM_OK;
 }
 
+int blocks_repattern(balm_ctx *c, const PoseGraph *pg, const char *who) {
+  std::unique_ptr<BlockPattern> pat;
+  TRY(block_pattern_build(c, *c->bh, pg, who, &pat));
+  c->bh->pat = std::move(pat);
+  return BALM_OK;
+}
+
 int launch_blocks(balm_ctx *c, int64_t head, int64_t end) {
   const BlockHessian *b = c->bh;
-  const long long np = (long long)b->pairs.size();
+  const BlockPattern &u = *b->pat;
+  const long long np = (long long)u.pairs.size();
   const long long threads = std::max<long long>(32 * np, c->n);
-  blocks_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, c->stream>>>(b->pair_dev, b->tptr, b->term, np, c->G,
+  blocks_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, c->stream>>>(u.pair_dev, u.tptr, b->term, np, c->G,
                                                                           c->row_ptr, head, end, c->accum, c->Np, c->n,
-                                                                          b->blocks, c->g);
+                                                                          u.blocks, c->g);
+  c->launches += 1;
+  CUDA_TRY(cudaGetLastError());
+  return BALM_OK;
+}
+
+int blocks_add_factors(balm_ctx *c, const double *poses) {
+  const BlockPattern &u = *c->bh->pat;
+  TRY(pose_graph_add_blocks(c->pg, c->stream, poses, u.blocks, u.fmap, u.fgc, &c->launches));
+  add_kernel<<<(unsigned)((c->n + 1 + 255) / 256), 256, 0, c->stream>>>(u.fgc, c->n + 1, c->g);  // g, then r = g[n]
+  c->launches += 1;
+  CUDA_TRY(cudaGetLastError());
+  return BALM_OK;
+}
+
+int blocks_add_factor_cost(balm_ctx *c, const double *poses, double *r) {
+  const BlockPattern &u = *c->bh->pat;
+  TRY(pose_graph_cost(c->pg, c->stream, poses, u.fgc + c->n, &c->launches));
+  add_kernel<<<1, 32, 0, c->stream>>>(u.fgc + c->n, 1, r);
   c->launches += 1;
   CUDA_TRY(cudaGetLastError());
   return BALM_OK;
 }
 
 int blocks_zero(balm_ctx *c) {
-  CUDA_TRY(cudaMemsetAsync(c->bh->blocks, 0, sizeof(double) * 36 * c->bh->pairs.size(), c->stream));
+  CUDA_TRY(cudaMemsetAsync(c->bh->pat->blocks, 0, sizeof(double) * 36 * c->bh->pat->pairs.size(), c->stream));
   return BALM_OK;
 }
 
 int blocks_solve(balm_ctx *c, double u) {
   c->h_scal[3] = u;  // pinned; the kernels read the damping factor from device memory
   CUDA_TRY(cudaMemcpyAsync(c->scal + 3, c->h_scal + 3, sizeof(double), cudaMemcpyHostToDevice, c->stream));
-  TRY(sparse_solve(c->bh->solver, c->stream));
+  TRY(sparse_solve(c->bh->pat->solver, c->stream));
   c->launches += 1;
   return BALM_OK;
 }
 
 int blocks_refine(balm_ctx *c, int *still_bad) {
-  TRY(sparse_refine(c->bh->solver, c->stream, c->h_flags, c->h_scal, still_bad));
+  TRY(sparse_refine(c->bh->pat->solver, c->stream, c->h_flags, c->h_scal, still_bad));
   c->tm.refinements += 1;
   return BALM_OK;
 }
 
-const std::vector<int2> &blocks_pairs(const BlockHessian *b) { return b->pairs; }
-const double *blocks_device(const BlockHessian *b) { return b->blocks; }
-SparseSolver *blocks_solver(const BlockHessian *b) { return b->solver; }
+const std::vector<int2> &blocks_pairs(const BlockHessian *b) { return b->pat->pairs; }
+const double *blocks_device(const BlockHessian *b) { return b->pat->blocks; }
+SparseSolver *blocks_solver(const BlockHessian *b) { return b->pat->solver; }
 
 long long blocks_bytes(const BlockHessian *b, int64_t *l_blocks, int64_t *levels) {
   int64_t sb = 0;
-  sparse_solver_stats(b->solver, l_blocks, levels, &sb);
-  return b->bytes + sb;
+  sparse_solver_stats(b->pat->solver, l_blocks, levels, &sb);
+  return (long long)sizeof(unsigned long long) * b->nterm + b->pat->bytes + sb;
 }

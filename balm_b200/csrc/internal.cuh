@@ -113,7 +113,8 @@ struct balm_ctx {
   bool has_keys = false;
   balm_assoc_opts assoc{1.0, 2, 15, {1.0 / 16, 1.0 / 16, 1.0 / 16}};  // association options of that call
   WindowState *win = nullptr;     // balm_window_* state (independent of the registered voxel set)
-  PoseGraph *pg = nullptr;        // balm_set_pose_factors' window factors (independent of the registered voxel set)
+  PoseGraph *pg = nullptr;        // balm_set_pose_factors' window factors (independent of the registered voxel set);
+                                  // BALM_PREC_BLOCKS: balm_block_set_factors' factors, part of the cost
   BlockHessian *bh = nullptr;     // BALM_PREC_BLOCKS: the registered set's block pattern, terms, blocks and solver
 
   // ---- optimiser state (device) ----
@@ -762,6 +763,10 @@ int pose_graph_eval(balm_ctx *c, const double *poses);
 // the same sums with one 6x6 block per pair (column-major, in pose_graph_pairs order) instead of dense H (enqueued)
 int pose_graph_eval_blocks(const PoseGraph *p, cudaStream_t st, const double *poses, double *blocks, double *g,
                            double *cost, long long *launches);
+// A blocks context's factor term (enqueued): pair p's sum added onto blocks[map[p]], the factor g into g_cost[0 .. 6P)
+// and the cost into g_cost[6P]
+int pose_graph_add_blocks(const PoseGraph *p, cudaStream_t st, const double *poses, double *blocks, const int *map,
+                          double *g_cost, long long *launches);
 // the cost at the device poses into the device scalar *out (enqueued, no wait)
 int pose_graph_cost(const PoseGraph *p, cudaStream_t st, const double *poses, double *out, long long *launches);
 // the (i, j), i <= j, of every nonzero 6x6 block pair of H, ascending in (i, j)
@@ -794,9 +799,17 @@ int sparse_covariance(SparseSolver *s, cudaStream_t st, int anchor, const std::f
                       double *cov, long long *launches);
 
 // ---------------- block-sparse Hessian of a BALM_PREC_BLOCKS context (blocks.cu) ----------------
-// The registered voxels' pair pattern, update terms and symbolic factorisation -> c->bh (replacing the previous one).
-// BALM_ERR_UNSUPPORTED (message prefixed with who) when the terms or pairs are too many to index; c->bh is then kept.
+// The registered voxels' pair pattern and update terms, then the union pattern with c->pg's factor pairs and its
+// symbolic factorisation -> c->bh (replacing the previous one). BALM_ERR_UNSUPPORTED (message prefixed with who) when
+// the terms or pairs are too many to index; c->bh is then kept.
 int block_hessian_build(balm_ctx *c, const char *who);
+// The union pattern of c->bh's voxel pairs and pg's pairs (pg may be null) replaces c->bh's, the voxel terms kept; on an
+// error c->bh is unchanged.
+int blocks_repattern(balm_ctx *c, const PoseGraph *pg, const char *who);
+// c->pg's factor blocks, g and cost at poses added onto the evaluated blocks, c->g and the residual c->g[n] (enqueued)
+int blocks_add_factors(balm_ctx *c, const double *poses);
+// c->pg's cost at poses added onto the device scalar *r (enqueued)
+int blocks_add_factor_cost(balm_ctx *c, const double *poses, double *r);
 // the blocks of voxels [head, end) from c->G (the per-observation store) and the accumulators, g from the accumulators
 int launch_blocks(balm_ctx *c, int64_t head, int64_t end);
 int blocks_zero(balm_ctx *c);

@@ -8,6 +8,7 @@
 //   pg_linearise_kernel  per active factor, one CTA: e_k, J_k (shared), M = E^T H~ E and b = E^T H~ e -> staging
 //   pg_assemble_kernel   per (global 6x6 block pair i <= j, entry): the pair's (factor, slot, slot) terms in factor order
 //                        -> H (i, j) and (j, i) from one sum; per gradient entry: the pose's slots in factor order -> g
+//                        (outputs: dense H, the sparse pose graph's blocks, or added onto a blocks context's blocks)
 //   pg_cost_kernel       per active factor, one CTA: cost_f
 //   pg_sum_kernel        one CTA: the factors' costs in factor order -> a device scalar
 #include <math.h>
@@ -212,7 +213,8 @@ __global__ void __launch_bounds__(PG_THREADS) pg_linearise_kernel(FactorView fv,
 }
 
 // ---- H and g: one thread per (block pair, entry), then one per gradient entry. The pair sums go to `out`: dense H
-// (zeroed beforehand) for the context, one 6x6 block per pair for the sparse pose graph. ----
+// (zeroed beforehand) for the context, one 6x6 block per pair for the sparse pose graph, or added onto the voxel blocks of
+// a BALM_PREC_BLOCKS context (DESIGN.md "Voxels and pose factors in one cost"). ----
 struct DenseH {  // H (6P)^2 column-major: entry (a, c6) of pair (i, j) at (6i + a, 6j + c6) and its transpose
   double *H;
   __device__ __forceinline__ void operator()(size_t n, long long p, int2 ij, int a, int c6, double s) const {
@@ -224,6 +226,13 @@ struct PairBlocks {  // block p (36, column-major) = H rows 6i.., columns 6j..
   double *B;
   __device__ __forceinline__ void operator()(size_t, long long p, int2, int a, int c6, double s) const {
     B[36 * p + 6 * c6 + a] = s;
+  }
+};
+struct AddBlocks {  // a BALM_PREC_BLOCKS context's union pattern: block map[p] (36, column-major) += pair p's sum
+  double *B;
+  const int *map;
+  __device__ __forceinline__ void operator()(size_t, long long p, int2, int a, int c6, double s) const {
+    B[36 * (size_t)map[p] + 6 * c6 + a] += s;
   }
 };
 
@@ -468,4 +477,10 @@ int pose_graph_eval_blocks(const PoseGraph *p, cudaStream_t st, const double *po
                            double *cost, long long *launches) {
   TRY(pose_graph_assemble(*p, st, poses, PairBlocks{blocks}, g, launches));
   return pose_graph_cost(p, st, poses, cost, launches);
+}
+
+int pose_graph_add_blocks(const PoseGraph *p, cudaStream_t st, const double *poses, double *blocks, const int *map,
+                          double *g_cost, long long *launches) {
+  TRY(pose_graph_assemble(*p, st, poses, AddBlocks{blocks, map}, g_cost, launches));
+  return pose_graph_cost(p, st, poses, g_cost + 6 * (size_t)p->P, launches);
 }

@@ -55,7 +55,8 @@ typedef enum {
                            context without voxels, as do 2^31 observation pairs or 2^30 block pairs. balm_comm_init,
                            balm_pose_covariance, balm_set_pose_factors, balm_pose_graph_*, balm_device_views and the
                            tensor debug aids return BALM_ERR_UNSUPPORTED on such a context and change nothing;
-                           balm_evaluate's H (when not NULL) is the dense matrix expanded from the blocks. */
+                           balm_evaluate's H (when not NULL) is the dense matrix expanded from the blocks. Pose factors
+                           join the voxel cost through balm_block_set_factors. */
 } balm_precision;
 
 typedef struct {
@@ -475,6 +476,23 @@ int balm_download_blocks(balm_ctx *ctx, double *blocks);
  * registration. Tables, errors and side effects as balm_spg_covariance's: afterwards balm_download_blocks returns H at
  * poses12, and the next balm_damping_iter is bitwise what it would have been without this call. */
 int balm_block_covariance(balm_ctx *ctx, const double *poses12, int include_fix, int anchor, double *cov);
+/* Pose factors in the cost of a BALM_PREC_BLOCKS context (DESIGN.md "Voxels and pose factors in one cost"): odometry
+ * between consecutive scans, loop closures, HBA window factors. Arguments, checks, error messages, per-factor status
+ * (BALM_ERR_NOT_PD factors are left out of the pattern and every sum) and factor cost are balm_set_pose_factors'; H_f must
+ * be in the voxel cost's units (coe x lambda: points x m^2, as balm_batch_evaluate's H is). n_factors == 0 (the arrays may
+ * be NULL) detaches the factor set. Once attached, the context's cost is the voxel cost plus the sum of the active
+ * factors' costs in every evaluation over the whole voxel range (head == 0, end == M, also M == 0): balm_evaluate's H, g
+ * and residual, balm_residual, balm_damping_iter, balm_solve, balm_download_blocks and balm_block_covariance. A
+ * sub-range evaluation stays voxels only, bitwise what it is without factors. min_planes_per_pose still counts voxels:
+ * pass 0 when factors carry scans that see no plane. balm_block_structure reports the union pattern (voxel pairs, the
+ * active factors' pairs, every diagonal pair) and counts the factor set's bytes; balm_timings.ms_assemble is the factor
+ * linearisation, assembly and cost time (0 without factors).
+ * The set is independent of the voxel registration: it may be set before one and survives every registration route.
+ * Factor indices are pose slots, so after a window shift re-setting them is the caller's job.
+ * BALM_ERR_INVALID on any other kind of context, with nothing changed; a rejected call (invalid arguments, or
+ * BALM_ERR_UNSUPPORTED when the union pattern is too large to index) keeps the previous set and pattern. */
+int balm_block_set_factors(balm_ctx *ctx, int n_factors, const int64_t *factor_ptr, const int32_t *factor_pose,
+                           const double *poses_hat12, const double *H, int32_t *status_out);
 
 /* Multi-GPU: voxels are sharded across ranks by the caller (each rank registers its own shard); the library
  * all-reduces [H | g | r] with NCCL after every evaluation and the scalar after every residual pass.
