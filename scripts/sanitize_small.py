@@ -7,7 +7,8 @@ an anchored, a free and an empty problem (balm_batch_pose_covariance), and the b
 windows, the empty one included (balm_batch_marginalize / balm_batch_append_scan), the batch's persistent window maps
 (balm_batch_window_*), and the keyframe merge of overlapping windows with an empty scan and an empty window at voxel
 sizes 0 and 0.2 (balm_batch_merge_scans), and the sparse pose graph (balm_spg_*) on a small pyramid with a long-range
-factor, a factor that is not positive definite and a pose in no factor."""
+factor, a factor that is not positive definite and a pose in no factor, and a factor-only PREC_BLOCKS context on an
+87-pose clique (the factor, selected-inversion, anchor and refinement kernels past their wrap edges)."""
 import os, sys
 import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -114,4 +115,17 @@ print("  not_pd", [t["not_pd"] for t in s.pose_graph_iter(truth, max_iter=2)[1]]
 s.set_pose_factors(fs[:-1])
 print("  iters", len(s.pose_graph_iter(pgr.perturb(rng, truth, 0.05, 0.2), max_iter=3)[1]), flush=True)
 s.close()
+# a factor-only blocks context on an 87-pose clique: every loop of the factor and selected-inversion kernels wraps
+# (86 blocks below the first column's diagonal); a solve just past a singular leading minor of H + u diag(H), which
+# refines, one at u = 0.01 and a covariance (anchor kernel, selected inversion, gather)
+import nd_symbolic_ref as nd
+from test_gpu_sparse_ldlt_edges import PATTERNS, _blocks_ctx, _factors, _leading_minor_crossing
+P, fs, x = _factors("clique87", seed=0)
+c = _blocks_ctx(P, fs)
+H = c.evaluate(x)[0]
+u = _leading_minor_crossing(H, nd.symbolic(P, nd.pairs_of(P, PATTERNS["clique87"][1]))["order"], P // 2) * (1 + 1e-8)
+print("clique87 blocks solve at u", u, "not_pd", c.solve(u)[2], "refinements", c.timings()["refinements"], flush=True)
+print("  u 0.01 not_pd", c.solve(0.01)[2], flush=True)
+print("  covariance trace", sum(np.trace(b) for b in c.block_covariance(x, anchor=0)[1]), flush=True)
+c.close()
 print("SANITIZE_DONE")
