@@ -8,6 +8,7 @@ LIB_PATH = os.path.join(_HERE, "libbalm_b200.so")
 
 OK, ERR_INVALID, ERR_CUDA, ERR_NOT_PD, ERR_TOO_FEW_PLANES, ERR_NCCL, ERR_UNSUPPORTED = range(7)
 PREC_FP64, PREC_TENSOR, PREC_BLOCKS = 0, 1, 2
+LOSS_TRIVIAL, LOSS_HUBER, LOSS_CAUCHY = 0, 1, 2
 
 
 class LmOpts(C.Structure):
@@ -57,7 +58,8 @@ SYMBOLS = ["balm_last_error", "balm_version", "balm_create", "balm_destroy", "ba
            "balm_batch_window_push", "balm_batch_merge_scans", "balm_set_pose_factors", "balm_pose_graph_evaluate",
            "balm_pose_graph_iter", "balm_spg_create", "balm_spg_destroy", "balm_spg_set_factors", "balm_spg_structure",
            "balm_spg_evaluate", "balm_spg_iter", "balm_spg_covariance", "balm_block_structure", "balm_download_blocks",
-           "balm_block_covariance", "balm_block_set_factors"]
+           "balm_block_covariance", "balm_block_set_factors", "balm_set_factor_loss", "balm_factor_residuals",
+           "balm_spg_set_factor_loss", "balm_spg_factor_residuals"]
 
 
 def lib():
@@ -150,6 +152,10 @@ def lib():
         L.balm_download_blocks.argtypes = [C.c_void_p, C.c_void_p]
         L.balm_block_covariance.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]
         L.balm_block_set_factors.argtypes = [C.c_void_p, C.c_int] + [C.c_void_p] * 5
+        L.balm_set_factor_loss.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
+        L.balm_factor_residuals.argtypes = [C.c_void_p] + [C.c_void_p] * 3
+        L.balm_spg_set_factor_loss.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
+        L.balm_spg_factor_residuals.argtypes = [C.c_void_p] + [C.c_void_p] * 3
         _lib = L
     return _lib
 

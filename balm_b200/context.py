@@ -36,6 +36,32 @@ def _set_pose_factors(fn, handle, factors):
     return [int(s) for s in status]
 
 
+_LOSS = {"trivial": L.LOSS_TRIVIAL, "huber": L.LOSS_HUBER, "cauchy": L.LOSS_CAUCHY}
+
+
+def _set_factor_loss(fn, handle, n_factors, kind, scale):
+    """balm_set_factor_loss / balm_spg_set_factor_loss: kind a loss name or one per factor, scale a scalar or one per
+    factor (ignored for trivial factors); kind="trivial" resets every factor."""
+    if isinstance(kind, str):
+        if kind == "trivial":
+            L.check(fn(handle, n_factors, None, None))
+            return
+        kind = [kind] * n_factors
+    if any(k not in _LOSS for k in kind):
+        raise ValueError(f"set_factor_loss: kinds must be in {sorted(_LOSS)}, got {sorted(set(kind) - set(_LOSS))}")
+    k = np.array([_LOSS[x] for x in kind], dtype=np.int32)
+    sc = None if scale is None else np.ascontiguousarray(np.broadcast_to(np.asarray(scale, dtype=np.float64), k.shape))
+    L.check(fn(handle, len(k), _p(k), _p(sc)))
+
+
+def _factor_residuals(fn, handle, n_factors, poses12):
+    """balm_factor_residuals / balm_spg_factor_residuals -> (s, w), one entry per factor of the registered set."""
+    poses12 = np.ascontiguousarray(poses12, dtype=np.float64)
+    s, w = np.zeros(n_factors), np.zeros(n_factors)
+    L.check(fn(handle, _p(poses12), _p(s), _p(w)))
+    return s, w
+
+
 def _pose_graph_iter(fn, handle, N, poses12, max_iter, u0, v0, rel_tol, gauge_mode, verbose, want_per_iter, force_hess):
     """balm_pose_graph_iter / balm_spg_iter -> (poses, trace dicts)."""
     poses = np.array(poses12, dtype=np.float64, order="C", copy=True)
@@ -66,6 +92,7 @@ class Context:
         self._h = C.c_void_p()
         self.N = int(n_poses)
         self.n = 6 * self.N
+        self._n_factors = 0  # the registered pose factor set's size
         L.check(L.lib().balm_create(C.byref(self._h), self.N, int(device), int(precision)))
 
     def close(self):
@@ -184,8 +211,24 @@ class Context:
         keeps the previous one. -> per factor OK or ERR_NOT_PD (left out of the cost)."""
         if not factors:
             L.check(L.lib().balm_block_set_factors(self._h, 0, None, None, None, None, None))
+            self._n_factors = 0
             return []
-        return _set_pose_factors(L.lib().balm_block_set_factors, self._h, factors)
+        status = _set_pose_factors(L.lib().balm_block_set_factors, self._h, factors)
+        self._n_factors = len(status)
+        return status
+
+    def set_factor_loss(self, kind, scale=None):
+        """Robust loss of the registered pose factors (set_pose_factors', or set_block_factors' on PREC_BLOCKS contexts;
+        include/balm_b200.h, balm_set_factor_loss): kind "trivial", "huber" or "cauchy", or one of those per factor;
+        scale c (units of sqrt(s), s = e~^T H~ e~) a scalar or one per factor. Every evaluation, LM and covariance of the
+        factors then uses cost 1/2 rho(s), gradient rho'(s) b and the reweighted H rho'(s) M. kind="trivial" resets; a
+        new factor set starts trivial."""
+        _set_factor_loss(L.lib().balm_set_factor_loss, self._h, self._n_factors, kind, scale)
+
+    def factor_residuals(self, poses12):
+        """-> (s, w): s_f = e~^T H~ e~ and w_f = rho'(s_f) of every registered factor at poses12 (0, 0 for a factor left
+        out as ERR_NOT_PD; w = 1 without a loss)."""
+        return _factor_residuals(L.lib().balm_factor_residuals, self._h, self._n_factors, poses12)
 
     def solve(self, u):
         dx = np.zeros(self.n)
@@ -278,7 +321,9 @@ class Context:
         """Window factors (include/balm_b200.h, balm_set_pose_factors): list of dict(poses = N_f distinct global pose
         indices, poses_hat = N_f x 12 refined window poses, H = (6 N_f)^2 window BA Hessian). Replaces the previous factor
         set; a rejected call keeps it. -> per factor OK or ERR_NOT_PD (left out of the cost)."""
-        return _set_pose_factors(L.lib().balm_set_pose_factors, self._h, factors)
+        status = _set_pose_factors(L.lib().balm_set_pose_factors, self._h, factors)
+        self._n_factors = len(status)
+        return status
 
     def pose_graph_evaluate(self, poses12, want_H=True):
         """-> (H, g, cost) of the registered factors at poses12 (H dense n x n, None with want_H=False)."""
@@ -615,6 +660,7 @@ class PoseGraph:
         self._h = C.c_void_p()
         self.N = int(n_poses)
         self.n = 6 * self.N
+        self._n_factors = 0
         L.check(L.lib().balm_spg_create(C.byref(self._h), self.N, int(device)))
 
     def close(self):
@@ -630,7 +676,17 @@ class PoseGraph:
 
     def set_pose_factors(self, factors):
         """Context.set_pose_factors' factors, checks and result; also orders the poses and factors the pattern."""
-        return _set_pose_factors(L.lib().balm_spg_set_factors, self._h, factors)
+        status = _set_pose_factors(L.lib().balm_spg_set_factors, self._h, factors)
+        self._n_factors = len(status)
+        return status
+
+    def set_factor_loss(self, kind, scale=None):
+        """Context.set_factor_loss on this handle's factors (evaluate, iterate and covariance use the robust cost)."""
+        _set_factor_loss(L.lib().balm_spg_set_factor_loss, self._h, self._n_factors, kind, scale)
+
+    def factor_residuals(self, poses12):
+        """Context.factor_residuals on this handle's factors -> (s, w)."""
+        return _factor_residuals(L.lib().balm_spg_factor_residuals, self._h, self._n_factors, poses12)
 
     def structure(self):
         """-> dict(pairs, l_blocks, levels, device_bytes): nonzero block pairs of H, blocks of the factor L, levels of

@@ -978,6 +978,43 @@ extern "C" int balm_block_set_factors(balm_ctx *c, int n_factors, const int64_t 
   return BALM_OK;
 }
 
+// balm_set_factor_loss / balm_spg_set_factor_loss on the factor set pg (null: none registered)
+static int set_factor_loss(const char *who, PoseGraph *pg, cudaStream_t st, int n_factors, const int32_t *kind,
+                           const double *scale) {
+  const std::string w = std::string(who) + ": ";
+  if (!pg) { balm_set_error(w + "no pose factors registered"); return BALM_ERR_INVALID; }
+  if (n_factors != pose_graph_n_factors(pg)) {
+    balm_set_error(w + "n_factors " + std::to_string(n_factors) + " is not the registered count " +
+                   std::to_string(pose_graph_n_factors(pg)));
+    return BALM_ERR_INVALID;
+  }
+  for (int f = 0; kind && f < n_factors; f++) {
+    if (kind[f] != BALM_LOSS_TRIVIAL && kind[f] != BALM_LOSS_HUBER && kind[f] != BALM_LOSS_CAUCHY) {
+      balm_set_error(w + "factor " + std::to_string(f) + " has loss kind " + std::to_string(kind[f]) + " (0, 1, 2 allowed)");
+      return BALM_ERR_INVALID;
+    }
+    if (kind[f] != BALM_LOSS_TRIVIAL && !(scale && std::isfinite(scale[f]) && scale[f] > 0.0)) {
+      balm_set_error(w + "factor " + std::to_string(f) + " needs a finite scale > 0");
+      return BALM_ERR_INVALID;
+    }
+  }
+  return pose_graph_set_loss(pg, st, kind, scale);
+}
+
+extern "C" int balm_set_factor_loss(balm_ctx *c, int n_factors, const int32_t *kind, const double *scale) {
+  if (!c) { balm_set_error("balm_set_factor_loss: bad arguments"); return BALM_ERR_INVALID; }
+  CUDA_TRY(cudaSetDevice(c->device));
+  return set_factor_loss("balm_set_factor_loss", c->pg, c->stream, n_factors, kind, scale);
+}
+
+extern "C" int balm_factor_residuals(balm_ctx *c, const double *poses12, double *s, double *w) {
+  if (!c || !poses12) { balm_set_error("balm_factor_residuals: bad arguments"); return BALM_ERR_INVALID; }
+  if (!c->pg) { balm_set_error("balm_factor_residuals: no pose factors registered"); return BALM_ERR_INVALID; }
+  CUDA_TRY(cudaSetDevice(c->device));
+  CUDA_TRY(cudaMemcpyAsync(c->poses, poses12, sizeof(double) * 12 * c->N, cudaMemcpyHostToDevice, c->stream));
+  return pose_graph_residuals(c->pg, c->stream, c->poses, s, w, &c->launches);
+}
+
 extern "C" int balm_pose_graph_evaluate(balm_ctx *c, const double *poses12, double *H, double *g, double *cost) {
   if (!c || !poses12) { balm_set_error("balm_pose_graph_evaluate: bad arguments"); return BALM_ERR_INVALID; }
   TRY(refuse_blocks(c, "balm_pose_graph_evaluate"));
@@ -1252,6 +1289,20 @@ extern "C" int balm_spg_covariance(balm_spg *s, const double *poses12, int ancho
     CUDA_TRY(cudaMemcpyAsync(s->poses, poses12, sizeof(double) * 12 * s->N, cudaMemcpyHostToDevice, s->stream));
     return pose_graph_eval_blocks(s->pg, s->stream, s->poses, s->blocks, s->g, s->scal, &s->launches);
   }, "balm_spg_covariance", cov, &s->launches);
+}
+
+extern "C" int balm_spg_set_factor_loss(balm_spg *s, int n_factors, const int32_t *kind, const double *scale) {
+  if (!s) { balm_set_error("balm_spg_set_factor_loss: bad arguments"); return BALM_ERR_INVALID; }
+  CUDA_TRY(cudaSetDevice(s->device));
+  return set_factor_loss("balm_spg_set_factor_loss", s->pg, s->stream, n_factors, kind, scale);
+}
+
+extern "C" int balm_spg_factor_residuals(balm_spg *s, const double *poses12, double *sf, double *w) {
+  if (!s || !poses12) { balm_set_error("balm_spg_factor_residuals: bad arguments"); return BALM_ERR_INVALID; }
+  if (!s->pg) { balm_set_error("balm_spg_factor_residuals: no pose factors registered"); return BALM_ERR_INVALID; }
+  CUDA_TRY(cudaSetDevice(s->device));
+  CUDA_TRY(cudaMemcpyAsync(s->poses, poses12, sizeof(double) * 12 * s->N, cudaMemcpyHostToDevice, s->stream));
+  return pose_graph_residuals(s->pg, s->stream, s->poses, sf, w, &s->launches);
 }
 
 // ---------------- sliding window on the registered voxel set (assoc.cu) ----------------

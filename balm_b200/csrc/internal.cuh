@@ -771,8 +771,15 @@ int pose_graph_add_blocks(const PoseGraph *p, cudaStream_t st, const double *pos
 int pose_graph_cost(const PoseGraph *p, cudaStream_t st, const double *poses, double *out, long long *launches);
 // the (i, j), i <= j, of every nonzero 6x6 block pair of H, ascending in (i, j)
 const std::vector<int2> &pose_graph_pairs(const PoseGraph *p);
-// device bytes the registered set holds (factors, staging, tables)
+// device bytes the registered set holds (factors, staging, tables, and the loss arrays while a loss is set)
 long long pose_graph_bytes(const PoseGraph *p);
+int pose_graph_n_factors(const PoseGraph *p);
+// balm_set_factor_loss after its argument checks: kind [F] (null: all trivial) and scale [F]; waits for the upload
+int pose_graph_set_loss(PoseGraph *p, cudaStream_t st, const int32_t *kind, const double *scale);
+// balm_factor_residuals: s_f and rho'(s_f) of every factor at the device poses (0 for inactive factors) into the host
+// arrays s and w [F] (either may be null); enqueues the cost pass and waits once
+int pose_graph_residuals(const PoseGraph *p, cudaStream_t st, const double *poses, double *s, double *w,
+                         long long *launches);
 
 // ---------------- sparse pose graph (pose_graph_sparse.cu) ----------------
 struct SparseSolver;  // nested-dissection ordering, symbolic factorisation and the per-solve CUDA graph

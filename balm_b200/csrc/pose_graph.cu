@@ -11,7 +11,12 @@
 //                        (outputs: dense H, the sparse pose graph's blocks, or added onto a blocks context's blocks)
 //   pg_cost_kernel       per active factor, one CTA: cost_f
 //   pg_sum_kernel        one CTA: the factors' costs in factor order -> a device scalar
+// Robust losses (DESIGN.md "Robust pose factors"): with s_f = e~^T H~ e~ the factor's cost becomes 1/2 rho(s_f), its b
+// rho'(s_f) b and its M rho'(s_f) M (IRLS). The <FactorLoss> instantiations of pg_cost_kernel (writes s_f and
+// w_f = rho'(s_f)) and pg_linearise_kernel (scales M and b by w_f) run only when an active factor has a non-trivial loss;
+// the <NoLoss> ones are the kernels without a loss.
 #include <math.h>
+#include <type_traits>
 #include <algorithm>
 #include <memory>
 #include <vector>
@@ -148,15 +153,27 @@ __device__ __forceinline__ void factor_residuals(const FactorView &fv, int f, co
   __syncthreads();
 }
 
-// ---- per active factor: M (6N x 6N, column-major, at the factor's H offset) and b (6 per slot) ----
+struct NoLoss {};      // the pure quadratic: kernels exactly as without robust losses
+struct FactorLoss {   // per factor: kind (BALM_LOSS_*), scale c, outputs s_f and w_f = rho'(s_f)
+  const int *kind;    // null: every factor trivial
+  const double *scale;
+  double *s, *w;
+};
+
+// ---- per active factor: M (6N x 6N, column-major, at the factor's H offset) and b (6 per slot); with FactorLoss both
+// scaled by w_f, which the cost pass before has written ----
+template <typename Loss>
 __global__ void __launch_bounds__(PG_THREADS) pg_linearise_kernel(FactorView fv, const int *act, const double *poses,
-                                                                  double *M, double *b) {
+                                                                  double *M, double *b, Loss loss) {
+  constexpr bool robust = std::is_same<Loss, FactorLoss>::value;
   __shared__ double se[PG_MAXN][6], sJ[PG_MAXN][36];
   const int f = act[blockIdx.x], tid = threadIdx.x;
   const long long s0 = fv.fptr[f];
   const int N = (int)(fv.fptr[f + 1] - s0), n6 = 6 * N, nb = N - 1;
   const double *Hf = fv.H + fv.hoff[f];
   double *Mf = M + fv.hoff[f], *bf = b + 6 * s0;
+  double wf = 1.0;
+  if constexpr (robust) wf = loss.w[f];
   factor_residuals(fv, f, poses, se, sJ);
   // k, l >= 1: M[k,l] = J_k^T H_f[k,l] J_l, b_k = J_k^T sum_l H_f[k,l] e_l
   const int nm = nb * nb * 36;
@@ -170,6 +187,7 @@ __global__ void __launch_bounds__(PG_THREADS) pg_linearise_kernel(FactorView fv,
         for (int c = 0; c < 6; c++) t += sJ[k][c * 6 + a] * Hkl[(size_t)d * n6 + c];
         s += t * sJ[l][d * 6 + c6];
       }
+      if constexpr (robust) s *= wf;
       Mf[(size_t)(6 * l + c6) * n6 + 6 * k + a] = s;
     } else {
       const int r = q - nm, a = r % 6, k = 1 + r / 6;
@@ -180,6 +198,7 @@ __global__ void __launch_bounds__(PG_THREADS) pg_linearise_kernel(FactorView fv,
           for (int d = 0; d < 6; d++) t += Hf[(size_t)(6 * l + d) * n6 + 6 * k + c] * se[l][d];
         s += sJ[k][c * 6 + a] * t;
       }
+      if constexpr (robust) s *= wf;
       bf[6 * k + a] = s;
     }
   }
@@ -266,9 +285,27 @@ __global__ void __launch_bounds__(PG_THREADS) pg_assemble_kernel(const long long
   }
 }
 
-// ---- per active factor: cost_f = 1/2 e~^T H~ e~, thread r owning row 6 + r of H~ ----
+// rho(s) and rho'(s) of BALM_LOSS_HUBER / BALM_LOSS_CAUCHY at scale c; BALM_LOSS_TRIVIAL: s and 1
+__device__ __forceinline__ void loss_rho(int kind, double c, double s, double *rho, double *drho) {
+  const double c2 = c * c;
+  if (kind == BALM_LOSS_HUBER && s > c2) {
+    const double r = sqrt(s);
+    *rho = 2.0 * c * r - c2;
+    *drho = c / r;
+  } else if (kind == BALM_LOSS_CAUCHY) {
+    *rho = c2 * log1p(s / c2);
+    *drho = 1.0 / (1.0 + s / c2);
+  } else {
+    *rho = s;
+    *drho = 1.0;
+  }
+}
+
+// ---- per active factor: cost_f = 1/2 e~^T H~ e~, thread r owning row 6 + r of H~; with FactorLoss s_f = e~^T H~ e~,
+// cost_f = 1/2 rho(s_f) and s_f, w_f = rho'(s_f) to the loss's outputs ----
+template <typename Loss>
 __global__ void __launch_bounds__(PG_THREADS) pg_cost_kernel(FactorView fv, const int *act, const double *poses,
-                                                             double *cost_part) {
+                                                             double *cost_part, Loss loss) {
   __shared__ double se[PG_MAXN][6];
   __shared__ double red[PG_THREADS / 32];
   const int f = act[blockIdx.x], tid = threadIdx.x;
@@ -289,6 +326,13 @@ __global__ void __launch_bounds__(PG_THREADS) pg_cost_kernel(FactorView fv, cons
   if (tid == 0) {
     double s = 0.0;
     for (int q = 0; q < PG_THREADS / 32; q++) s += red[q];
+    if constexpr (std::is_same<Loss, FactorLoss>::value) {
+      double rho, drho;
+      loss_rho(loss.kind ? loss.kind[f] : BALM_LOSS_TRIVIAL, loss.kind ? loss.scale[f] : 1.0, s, &rho, &drho);
+      loss.s[f] = s;
+      loss.w[f] = drho;
+      s = rho;
+    }
     cost_part[blockIdx.x] = 0.5 * s;
   }
 }
@@ -320,15 +364,29 @@ struct PoseGraph {
   int2 *pair = nullptr;
   int3 *term = nullptr;
   double *hat = nullptr, *H = nullptr, *M = nullptr, *b = nullptr, *cost_part = nullptr;
+  // balm_set_factor_loss: [F] kind, scale, s, w; allocated only while some factor's kind is non-trivial
+  int *loss_kind = nullptr;
+  double *loss_scale = nullptr, *loss_s = nullptr, *loss_w = nullptr;
+  bool robust = false;       // an active factor has a non-trivial kind
   std::vector<int2> pair_h;  // host copy of `pair`
+  std::vector<int> act_h;    // host copy of `act`
   long long bytes = 0;       // device memory held
   ~PoseGraph() {
     cudaFree(fptr); cudaFree(hoff); cudaFree(gp_slot); cudaFree(pose); cudaFree(act); cudaFree(pair_ptr);
     cudaFree(gp_ptr); cudaFree(status); cudaFree(pair); cudaFree(term); cudaFree(hat); cudaFree(H); cudaFree(M);
     cudaFree(b); cudaFree(cost_part);
+    free_loss();
+  }
+  void free_loss() {
+    cudaFree(loss_kind); cudaFree(loss_scale); cudaFree(loss_s); cudaFree(loss_w);
+    loss_kind = nullptr;
+    loss_scale = loss_s = loss_w = nullptr;
   }
   FactorView view() const { return FactorView{fptr, hoff, pose, hat, H}; }
+  FactorLoss loss() const { return FactorLoss{loss_kind, loss_scale, loss_s, loss_w}; }
 };
+
+constexpr long long LOSS_BYTES_PER_FACTOR = sizeof(int) + 3 * sizeof(double);
 
 void pose_graph_free(PoseGraph *p) { delete p; }
 
@@ -426,6 +484,7 @@ int pose_graph_build(cudaStream_t st, int P, int n_factors, const int64_t *facto
                          sizeof(int2) * pair.size() + sizeof(int3) * term.size() +
                          sizeof(double) * (12 * p->S + 2 * p->HS + 6 * p->S + std::max(1, p->n_act)));
   p->pair_h = std::move(pair);
+  p->act_h = std::move(act);
   *status_out = std::move(status);
   *out = p.release();
   return BALM_OK;
@@ -444,43 +503,118 @@ int pose_graph_set(balm_ctx *c, int n_factors, const int64_t *factor_ptr, const 
 
 const std::vector<int2> &pose_graph_pairs(const PoseGraph *p) { return p->pair_h; }
 long long pose_graph_bytes(const PoseGraph *p) { return p->bytes; }
+int pose_graph_n_factors(const PoseGraph *p) { return p->F; }
+
+int pose_graph_set_loss(PoseGraph *p, cudaStream_t st, const int32_t *kind, const double *scale) {
+  const int F = p->F;
+  const bool any = kind && std::any_of(kind, kind + F, [](int32_t k) { return k != BALM_LOSS_TRIVIAL; });
+  if (!any) {  // every factor trivial: no arrays, the kernels without a loss
+    if (p->loss_kind) p->bytes -= LOSS_BYTES_PER_FACTOR * F;
+    p->free_loss();
+    p->robust = false;
+    return BALM_OK;
+  }
+  if (!p->loss_kind) {
+    if (dev_alloc(&p->loss_kind, F) != BALM_OK || dev_alloc(&p->loss_scale, F) != BALM_OK ||
+        dev_alloc(&p->loss_s, F) != BALM_OK || dev_alloc(&p->loss_w, F) != BALM_OK) {
+      p->free_loss();  // still no loss: every factor trivial
+      return BALM_ERR_CUDA;
+    }
+    p->bytes += LOSS_BYTES_PER_FACTOR * F;
+  }
+  std::vector<double> c(F);
+  bool robust = false;
+  for (int f = 0; f < F; f++) c[f] = kind[f] == BALM_LOSS_TRIVIAL ? 1.0 : scale[f];  // a trivial factor's scale is unused
+  for (int f : p->act_h) robust = robust || kind[f] != BALM_LOSS_TRIVIAL;
+  CUDA_TRY(cudaMemcpyAsync(p->loss_kind, kind, sizeof(int) * F, cudaMemcpyHostToDevice, st));
+  CUDA_TRY(cudaMemcpyAsync(p->loss_scale, c.data(), sizeof(double) * F, cudaMemcpyHostToDevice, st));
+  CUDA_TRY(cudaMemsetAsync(p->loss_s, 0, sizeof(double) * F, st));  // inactive factors keep s = w = 0
+  CUDA_TRY(cudaMemsetAsync(p->loss_w, 0, sizeof(double) * F, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  p->robust = robust;
+  return BALM_OK;
+}
+
+// the robust cost pass into cost_part and the loss outputs
+static int robust_cost_pass(const PoseGraph &p, cudaStream_t st, const double *poses, const FactorLoss &loss,
+                            long long *launches) {
+  if (!p.n_act) return BALM_OK;
+  pg_cost_kernel<<<p.n_act, PG_THREADS, 0, st>>>(p.view(), p.act, poses, p.cost_part, loss);
+  *launches += 1;
+  CUDA_TRY(cudaGetLastError());
+  return BALM_OK;
+}
+
+static int sum_pass(const PoseGraph &p, cudaStream_t st, double *out, long long *launches) {
+  pg_sum_kernel<<<1, PG_THREADS, 0, st>>>(p.cost_part, p.n_act, out);
+  *launches += 1;
+  CUDA_TRY(cudaGetLastError());
+  return BALM_OK;
+}
 
 int pose_graph_cost(const PoseGraph *pg, cudaStream_t st, const double *poses, double *out, long long *launches) {
   const PoseGraph &p = *pg;
-  if (p.n_act) pg_cost_kernel<<<p.n_act, PG_THREADS, 0, st>>>(p.view(), p.act, poses, p.cost_part);
+  if (p.robust) {
+    TRY(robust_cost_pass(p, st, poses, p.loss(), launches));
+    return sum_pass(p, st, out, launches);
+  }
+  if (p.n_act) pg_cost_kernel<<<p.n_act, PG_THREADS, 0, st>>>(p.view(), p.act, poses, p.cost_part, NoLoss{});
   pg_sum_kernel<<<1, PG_THREADS, 0, st>>>(p.cost_part, p.n_act, out);
   *launches += p.n_act ? 2 : 1;
   CUDA_TRY(cudaGetLastError());
   return BALM_OK;
 }
 
+int pose_graph_residuals(const PoseGraph *pg, cudaStream_t st, const double *poses, double *s, double *w,
+                         long long *launches) {
+  const PoseGraph &p = *pg;
+  const size_t F = (size_t)p.F;
+  double *tmp = nullptr;  // without a loss: s and w of one call
+  if (!p.loss_kind) {
+    TRY(dev_alloc(&tmp, 2 * F));
+    CUDA_TRY(cudaMemsetAsync(tmp, 0, sizeof(double) * 2 * F, st));
+  }
+  std::unique_ptr<double, cudaError_t (*)(void *)> tmp_own(tmp, cudaFree);
+  const FactorLoss loss = tmp ? FactorLoss{nullptr, nullptr, tmp, tmp + F} : p.loss();
+  TRY(robust_cost_pass(p, st, poses, loss, launches));
+  if (s) CUDA_TRY(cudaMemcpyAsync(s, loss.s, sizeof(double) * F, cudaMemcpyDeviceToHost, st));
+  if (w) CUDA_TRY(cudaMemcpyAsync(w, loss.w, sizeof(double) * F, cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  return BALM_OK;
+}
+
+// H (through `out`), g and the cost at poses. With a loss the cost pass runs first, so that the linearisation can weight
+// M and b, and the evaluation's cost is its sum; without one, today's order.
 template <typename Out>
 static int pose_graph_assemble(const PoseGraph &p, cudaStream_t st, const double *poses, Out out, double *g,
-                               long long *launches) {
-  if (p.n_act) pg_linearise_kernel<<<p.n_act, PG_THREADS, 0, st>>>(p.view(), p.act, poses, p.M, p.b);
+                               double *cost, long long *launches) {
+  if (p.robust) {
+    TRY(robust_cost_pass(p, st, poses, p.loss(), launches));
+    if (p.n_act) pg_linearise_kernel<<<p.n_act, PG_THREADS, 0, st>>>(p.view(), p.act, poses, p.M, p.b, p.loss());
+  } else if (p.n_act) {
+    pg_linearise_kernel<<<p.n_act, PG_THREADS, 0, st>>>(p.view(), p.act, poses, p.M, p.b, NoLoss{});
+  }
   const long long threads = 36 * p.n_pairs + 6 * (long long)p.P;
   pg_assemble_kernel<<<(unsigned)((threads + PG_THREADS - 1) / PG_THREADS), PG_THREADS, 0, st>>>(
       p.fptr, p.hoff, p.pair, p.pair_ptr, p.term, p.n_pairs, p.M, p.gp_ptr, p.gp_slot, p.b, p.P, out, g);
   *launches += p.n_act ? 2 : 1;
   CUDA_TRY(cudaGetLastError());
-  return BALM_OK;
+  if (p.robust) return sum_pass(p, st, cost, launches);
+  return pose_graph_cost(&p, st, poses, cost, launches);
 }
 
 int pose_graph_eval(balm_ctx *c, const double *poses) {
   const size_t n = c->n;
   CUDA_TRY(cudaMemsetAsync(c->H, 0, sizeof(double) * n * n, c->stream));
-  TRY(pose_graph_assemble(*c->pg, c->stream, poses, DenseH{c->H}, c->g, &c->launches));
-  return pose_graph_cost(c->pg, c->stream, poses, c->scal, &c->launches);
+  return pose_graph_assemble(*c->pg, c->stream, poses, DenseH{c->H}, c->g, c->scal, &c->launches);
 }
 
 int pose_graph_eval_blocks(const PoseGraph *p, cudaStream_t st, const double *poses, double *blocks, double *g,
                            double *cost, long long *launches) {
-  TRY(pose_graph_assemble(*p, st, poses, PairBlocks{blocks}, g, launches));
-  return pose_graph_cost(p, st, poses, cost, launches);
+  return pose_graph_assemble(*p, st, poses, PairBlocks{blocks}, g, cost, launches);
 }
 
 int pose_graph_add_blocks(const PoseGraph *p, cudaStream_t st, const double *poses, double *blocks, const int *map,
                           double *g_cost, long long *launches) {
-  TRY(pose_graph_assemble(*p, st, poses, AddBlocks{blocks, map}, g_cost, launches));
-  return pose_graph_cost(p, st, poses, g_cost + 6 * (size_t)p->P, launches);
+  return pose_graph_assemble(*p, st, poses, AddBlocks{blocks, map}, g_cost, g_cost + 6 * (size_t)p->P, launches);
 }

@@ -59,6 +59,13 @@ typedef enum {
                            join the voxel cost through balm_block_set_factors. */
 } balm_precision;
 
+/* Robust losses of pose factors (balm_set_factor_loss), rho of s = e~^T H~ e~ at scale c > 0 (units of sqrt(s)). */
+typedef enum {
+  BALM_LOSS_TRIVIAL = 0, /* rho = s */
+  BALM_LOSS_HUBER = 1,   /* rho = s for s <= c^2, else 2 c sqrt(s) - c^2 */
+  BALM_LOSS_CAUCHY = 2   /* rho = c^2 log(1 + s / c^2) */
+} balm_loss;
+
 typedef struct {
   int max_iter;             /* 10  (bavoxel.hpp:1104); benchmark_virtual twin: 20 (benchmark_virtual.cpp:408) */
   double u0;                /* 0.01 (bavoxel.hpp:1087); twin: 0.1 (benchmark_virtual.cpp:380) */
@@ -460,6 +467,11 @@ int balm_spg_iter(balm_spg *spg, double *poses12, const balm_lm_opts *opts, balm
  * The call waits for the device twice (the pivot test and the copy-out), the first one also while it builds the
  * tables. */
 int balm_spg_covariance(balm_spg *spg, const double *poses12, int anchor, double *cov);
+/* balm_set_factor_loss and balm_factor_residuals on the handle's factor set: same losses, meaning (balm_spg_evaluate,
+ * balm_spg_iter and balm_spg_covariance use the robust cost, gradient and reweighted H), checks and lifetime
+ * (balm_spg_set_factors resets the loss); balm_spg_structure's stats[3] counts the 28 bytes per factor. */
+int balm_spg_set_factor_loss(balm_spg *spg, int n_factors, const int32_t *kind, const double *scale);
+int balm_spg_factor_residuals(balm_spg *spg, const double *poses12, double *s, double *w);
 
 /* Block-sparse Hessian of a BALM_PREC_BLOCKS context (BALM_ERR_INVALID on any other, or before a registration).
  * stats: [0] block pairs (i <= j) of H, [1] blocks of the factor L, [2] elimination-tree levels, [3] device bytes the
@@ -493,6 +505,28 @@ int balm_block_covariance(balm_ctx *ctx, const double *poses12, int include_fix,
  * BALM_ERR_UNSUPPORTED when the union pattern is too large to index) keeps the previous set and pattern. */
 int balm_block_set_factors(balm_ctx *ctx, int n_factors, const int64_t *factor_ptr, const int32_t *factor_pose,
                            const double *poses_hat12, const double *H, int32_t *status_out);
+/* Robust pose factors (DESIGN.md "Robust pose factors"): a loss kind[f] (balm_loss) and scale[f] for every factor of
+ * the context's registered set (balm_set_pose_factors' on FP64 / TENSOR contexts, balm_block_set_factors' on a
+ * BALM_PREC_BLOCKS context). With s_f = e~^T H~ e~ (twice the quadratic cost_f) and w_f = rho'(s_f), factor f then
+ * contributes cost 1/2 rho(s_f), gradient w_f b_f (the exact gradient of that cost) and Hessian w_f M_f, the iteratively
+ * reweighted Gauss-Newton term without the second-order rho'' part, in every call that evaluates the factors:
+ * balm_pose_graph_evaluate / _iter, and on a blocks context balm_evaluate, balm_residual, balm_damping_iter,
+ * balm_solve, balm_download_blocks and balm_block_covariance (whose Sigma is then the inverse of the reweighted H at
+ * poses12). A trivial factor's terms are bitwise those without a loss, also next to robust ones. scale is in units of
+ * sqrt(s): for factors in the voxel cost's units (2 sigma_p^2 x information, see odometry_factors) and a chi-square
+ * gate at probability p, c^2 = 2 sigma_p^2 chi2_6(p). kind == NULL resets every factor to trivial (scale unused).
+ * BALM_ERR_INVALID, the previous loss kept, for a null ctx, no registered factor set (a blocks context with none
+ * attached), n_factors not the registered count, a kind outside BALM_LOSS_*, or a non-trivial kind whose scale is not
+ * finite and > 0 (a trivial factor's scale is ignored; scale may be NULL when every kind is trivial). The loss belongs to
+ * the factor set: registering or detaching a set resets it to trivial; voxel registrations keep it. It changes no
+ * pattern, so nothing is refactored symbolically or re-captured. While a kind is non-trivial the set holds 28 more
+ * device bytes per factor (kind, scale, s_f, w_f), counted in balm_block_structure's stats[3]. */
+int balm_set_factor_loss(balm_ctx *ctx, int n_factors, const int32_t *kind, const double *scale);
+/* s_f and w_f = rho'(s_f) of every factor of the registered set at poses12, into s and w (n_factors each; either may
+ * be NULL). Factors left out as BALM_ERR_NOT_PD report s = w = 0; without a loss w = 1 for the others, which serves
+ * chi-square gating of candidate closures. Enqueues the cost pass only and waits once. BALM_ERR_INVALID for a null ctx
+ * or poses12, or no registered factor set. */
+int balm_factor_residuals(balm_ctx *ctx, const double *poses12, double *s, double *w);
 
 /* Multi-GPU: voxels are sharded across ranks by the caller (each rank registers its own shard); the library
  * all-reduces [H | g | r] with NCCL after every evaluation and the scalar after every residual pass.
