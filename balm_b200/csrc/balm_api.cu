@@ -189,7 +189,7 @@ extern "C" int balm_create(balm_ctx **out, int n_poses, int device, int precisio
   CUDA_TRY(cudaGetDeviceProperties(&prop, device));
   c->sm_count = prop.multiProcessorCount;
   if (precision == BALM_PREC_TENSOR && getenv("BALM_TC_TRACE"))
-    TRY(dev_alloc(&c->tc_trace, (size_t)c->sm_count * BALM_TC_TRACE_WORDS));
+    TRY(dev_alloc(&c->tc_trace, (size_t)c->sm_count * (BALM_TC_TRACE_WORDS + BALM_TC_COPY_TRACE_WORDS)));
   if (const char *e = getenv("BALM_TC_TILE"))  // tensor SYRK items: column halves or whole tiles (launch_syrk_tc)
     c->tc_tile = !strcmp(e, "half") ? 1 : !strcmp(e, "full") ? 2 : 0;
   int prio_least = 0, prio_greatest = 0;

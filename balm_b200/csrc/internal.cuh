@@ -24,6 +24,8 @@ constexpr double SOLVE_OMEGA_TOL = 1e-12;  // componentwise backward error of a 
 #define BALM_TC_MAX_ROWS_PER_ITEM 32704
 // BALM_TC_TRACE: words per CTA of the tensor SYRK's per-role clock trace (layout: balm_debug_tc_trace)
 #define BALM_TC_TRACE_WORDS 18
+// ... and words per CTA of its copier warps' trace, stored after every CTA's role words (balm_debug_tc_copy_trace)
+#define BALM_TC_COPY_TRACE_WORDS 3
 
 void balm_set_error(const std::string &s);
 struct WindowState;  // the persistent sliding-window octree (assoc.cu)

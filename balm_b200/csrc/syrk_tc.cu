@@ -12,18 +12,22 @@
 // result does not depend on tile order, k-splits or the number of GPUs.
 //
 // The observation sweep writes the digit planes MN-major (pose index contiguous, Gq[S][rows][ldg], coalesced), while
-// s8 wgmma reads shared-memory operands K-major only. tc_kmajor_kernel therefore transposes the planes once per SYRK
-// launch into GqT[S][rows / 64][ldg][64]: per 64-row band, every column's 64 contraction rows as one 64-byte row, in the
-// order wgmma reads them from shared memory (64-byte swizzle, see sw64_desc). A 128- or 64-column block of one band is
-// then one contiguous 8 or 4 KB run that a single bulk copy lands ready for the MMAs; the SYRK reads that copy alone.
+// s8 wgmma reads shared-memory operands K-major only. The SYRK kernel therefore transposes the planes itself, into
+// GqT[S][rows / 64][ldg][64]: per 64-row band, every column's 64 contraction rows as one 64-byte row, in the order wgmma
+// reads them from shared memory (64-byte swizzle, see sw64_desc). A 128- or 64-column block of one band is then one
+// contiguous 8 or 4 KB run that a single bulk copy lands ready for the MMAs. The copy is HBM traffic and the SYRK is
+// MMA-bound, so the copy runs in the same launch, a few bands ahead of the MMAs that need it.
 //
-// Kernel anatomy (syrk_tc_kernel; one CTA per SM, persistent over its items, 384 threads). An item is a whole 128 x 128
-// output tile (S <= 3 on problems with at least one (tile, k-split) pair per SM, see launch_syrk_tc) or one 128 x 64
-// column half of a tile, times one k-split:
-//   warp 8    : producer (one lane) -- cp.async.bulk of the S K-major planes of the A block (128 columns bi) and of the
-//               B block (128 columns bj, or the 64 of the half), KS = 64 contraction rows per stage, into one ring of
-//               stage slots (see Ring: up to 224 KB of shared memory, mbarrier full/empty per slot); warps 9-11 have
-//               no work
+// Kernel anatomy (syrk_tc_kernel; one CTA per SM, persistent over its items, 384 threads, a cooperative launch). An item
+// is a whole 128 x 128 output tile (S <= 3 on problems with at least one (tile, k-split) pair per SM, see launch_syrk_tc)
+// or one 128 x 64 column half of a tile, times one k-split:
+//   warps 9-11: copiers -- copy units (64-row band b, 128-column block cb), all S planes, from Gq into GqT, band-major
+//               in ascending band order, dealt round robin over the copier warps of all CTAs; each unit then stamps its
+//               readiness flag with the launch's epoch (see copier_loop). A copier waits on nothing but its own loads.
+//   warp 8    : producer -- acquires the flags of the A and the B blocks of 16 stages at a time, then per stage
+//               cp.async.bulk of the S K-major planes of the A block (128 columns bi) and of the B block (128 columns
+//               bj, or the 64 of the half), KS = 64 contraction rows per stage, into one ring of stage slots (see Ring:
+//               up to 192 KB of shared memory, mbarrier full/empty per slot)
 //   warps 0-7 : consumers, two warpgroups of 64 output rows each -- wgmma m64n128k32 (whole tiles) or m64n64k32 (halves)
 //               s8 x s8 -> s32 with B from the landed stage and A from it too (whole tiles) or from registers
 //               (ldmatrix, halves), S(S+1)/2 digit-pair
@@ -44,11 +48,14 @@ constexpr int KS = 64;                // contraction rows per pipeline stage (= 
 constexpr int A_PLANE_BYTES = KS * TILE;  // 8192: one K-major plane of a 128-column block, one stage (64-byte rows)
 constexpr int MAX_SLOTS = 8;             // barriers of the ring
 constexpr int BAR_BYTES = 2 * MAX_SLOTS * 8;
-constexpr int RING_BYTES = 227 * 1024 - 1024 - BAR_BYTES;  // the block's whole shared memory but alignment slack, barriers
+constexpr int COPIER_WARPS = 3;
+constexpr int STAGING_BYTES = COPIER_WARPS * KS * TILE;  // one MN-major 64 x 128 plane tile per copier warp
+// the block's whole shared memory but alignment slack, the copiers' staging and the barriers
+constexpr int RING_BYTES = 227 * 1024 - 1024 - STAGING_BYTES - BAR_BYTES;
 // One ring of stage slots: a slot holds the S planes of the A block, then the S planes of the B block (128 or 64
 // columns), all landed by bulk copies on the slot's one full barrier and freed together once the consumers' MMAs on it retired.
 // As many slots as fit, at most MAX_SLOTS:
-//   whole tiles: S = 2: 7 x 32 KB, S = 3: 4 x 48 KB;  halves: S = 2: 8 x 24 KB, S = 3: 6 x 36 KB, S = 4: 4 x 48 KB
+//   whole tiles: S = 2: 6 x 32 KB, S = 3: 4 x 48 KB;  halves: S = 2: 8 x 24 KB, S = 3: 5 x 36 KB, S = 4: 4 x 48 KB
 template <int S, bool FULL>
 struct Ring {
   static constexpr int N = FULL ? TILE : HALF;  // output columns of an item
@@ -58,13 +65,13 @@ struct Ring {
   static_assert(D >= 2 && SLOT % 1024 == 0, "ring layout (the 64-byte swizzle repeats every 512 bytes)");
 };
 constexpr int CONSUMER_WARPS = 8;
-constexpr int TC_THREADS = 32 * (CONSUMER_WARPS + 4);   // two consumer warpgroups + one producer warpgroup
-// register split (setmaxnreg): the producer warpgroup (one copying lane) gives nearly all its registers up so the consumers
+constexpr int TC_THREADS = 32 * (CONSUMER_WARPS + 4);   // two consumer warpgroups + the producer / copier warpgroup
+// register split (setmaxnreg): the producer / copier warpgroup gives nearly all its registers up so the consumers
 // can hold their accumulators (S * N / 2, 192 at S = 3 on whole tiles) and two k32 steps of A fragments (2 * S * 4).
 // The pool is what the launch allocated, 384 threads x 168 registers, and setmaxnreg.inc waits until the registers are
-// free: 2 * 128 * 240 + 128 * 24 = 384 * 168
-constexpr int CONSUMER_REGS = 240, PRODUCER_REGS = 24;
-constexpr int TC_SMEM = RING_BYTES + 1024 + BAR_BYTES;  // ring + alignment slack + barriers
+// free: 2 * 128 * 232 + 128 * 40 = 384 * 168. The copiers' transposes need more than 24 registers without spilling.
+constexpr int CONSUMER_REGS = 232, PRODUCER_REGS = 40;
+constexpr int TC_SMEM = RING_BYTES + STAGING_BYTES + 1024 + BAR_BYTES;  // ring + staging + alignment slack + barriers
 constexpr int MAX_ROWS_PER_ITEM = BALM_TC_MAX_ROWS_PER_ITEM;  // 32704: 4 * rows * 2^14 < 2^31 (a multiple of KS)
 static_assert(MAX_ROWS_PER_ITEM % KS == 0 && 4ll * MAX_ROWS_PER_ITEM * (1 << 14) < (1ll << 31), "int32 exactness bound");
 
@@ -106,9 +113,12 @@ __device__ __forceinline__ unsigned long long globaltimer_ns() {
 }
 // BALM_TC_TRACE (balm_debug_tc_trace): per-CTA word offsets of the stage count (in 128 x 64 half-tile units: a stage of
 // a whole tile counts 2), the consumer warp 0 globaltimer pair, the clock64 sums of the consumer warps 0 and 4 (5 each),
-// three words that stay zero (they held a B transposer's clocks) and the producer's (2)
+// three words that stay zero (they held a B transposer's clocks) and the producer's (2: waiting on a free slot, waiting
+// on readiness flags). The copiers' words (balm_debug_tc_copy_trace) follow all CTAs' words: per CTA the clocks its
+// copier warps spent on units, of those the clocks waiting on their loads, and the plane tiles copied.
 constexpr int TR_STAGES = 0, TR_NS = 1, TR_CONS = 3, TR_PROD = 16, TR_WORDS = BALM_TC_TRACE_WORDS;
-static_assert(TR_PROD + 2 == TR_WORDS, "trace layout");
+constexpr int TR_COPY_WORDS = BALM_TC_COPY_TRACE_WORDS;
+static_assert(TR_PROD + 2 == TR_WORDS && TR_COPY_WORDS == 3, "trace layout");
 // clock64 in the traced instantiation; the untraced one reads no clock
 template <bool TRACE>
 __device__ __forceinline__ long long tclock() {
@@ -121,6 +131,34 @@ __device__ __forceinline__ void bulk_load(void *dst, const void *src, uint32_t b
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n"
                ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
+}
+
+// 16 bytes of global memory into shared memory, bypassing L1; cp_async_wait_all waits for all of this thread's
+__device__ __forceinline__ void cp_async16(uint32_t dst, const void *src) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(dst), "l"(src) : "memory");
+}
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;\n" ::: "memory"); }
+__device__ __forceinline__ uint32_t lds32(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.u32 %0, [%1];\n" : "=r"(v) : "r"(addr) : "memory");
+  return v;
+}
+
+// Readiness flags of the copy units (release by the copier warp that wrote the unit, acquire by the producers that read
+// it; see copier_loop and producer_loop for the ordering)
+__device__ __forceinline__ void flag_release(unsigned *f, unsigned v) {
+  asm volatile("st.release.gpu.global.u32 [%0], %1;\n" ::"l"(f), "r"(v) : "memory");
+}
+// Bounded spin, as mbar_wait: true once *f == epoch; false when the error flag is set or the bound is exceeded
+__device__ __forceinline__ bool flag_wait(const unsigned *f, unsigned epoch, int *err) {
+  for (long long it = 0; it < (1ll << 22); it++) {
+    unsigned v;
+    asm volatile("ld.acquire.gpu.global.u32 %0, [%1];\n" : "=r"(v) : "l"(f) : "memory");
+    if (v == epoch) return true;
+    if ((it & 1023) == 1023 && *((volatile int *)err) != 0) return false;
+  }
+  atomicExch(err, 2);
+  return false;
 }
 
 // Four 8 x 8 matrices of 16-bit pairs: lane 8q + i gives the address of row i of matrix q; thread (g = lane/4,
@@ -139,6 +177,20 @@ __device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t *r) {
 constexpr int SW_SBO = 8 * KS;
 __device__ __forceinline__ uint64_t sw64_desc(uint32_t saddr) {
   return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(SW_SBO >> 4) << 32) | ((uint64_t)2 << 62);
+}
+// Byte offset, in a K-major block of GqT, of contraction rows 4 kq .. 4 kq + 3 of column n (n counted from a multiple of
+// 8, which starts the same swizzle row)
+__device__ __forceinline__ int kmajor_offset(int n, int kq) {
+  return n * KS + ((((kq >> 2) ^ (n >> 1)) & 3) << 4) + 4 * (kq & 3);
+}
+// 4 x 4 byte transpose: w[i] holds bytes (row i, columns 0..3); out[j] receives bytes (rows 0..3, column j)
+__device__ __forceinline__ void transpose4x4(const uint32_t (&w)[4], uint32_t (&out)[4]) {
+  const uint32_t lo01 = __byte_perm(w[0], w[1], 0x5140), hi01 = __byte_perm(w[0], w[1], 0x7362);
+  const uint32_t lo23 = __byte_perm(w[2], w[3], 0x5140), hi23 = __byte_perm(w[2], w[3], 0x7362);
+  out[0] = __byte_perm(lo01, lo23, 0x5410);
+  out[1] = __byte_perm(lo01, lo23, 0x7632);
+  out[2] = __byte_perm(hi01, hi23, 0x5410);
+  out[3] = __byte_perm(hi01, hi23, 0x7632);
 }
 
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory"); }
@@ -200,10 +252,13 @@ __device__ __forceinline__ bool warpgroup_all(bool ok, int id) {
 }
 
 struct TcArgs {
-  const int8_t *planes_t;  // GqT [SMAX][rows / KS][ldq][KS], see tc_kmajor_kernel
-  int64_t plane;      // bytes per plane of planes_t
+  const int8_t *planes;    // Gq [SMAX][rows][ldq], the MN-major digit planes the observation sweep wrote
+  int8_t *planes_t;        // GqT [SMAX][rows / KS][ldq][KS], their K-major copy, written by the copiers
+  int64_t plane;      // bytes per plane of planes and planes_t
   int ldq;
-  int64_t rows;       // contraction rows of this batch (3 per voxel)
+  int64_t rows;       // contraction rows of this batch (3 per voxel), padded to a multiple of KS
+  unsigned *flags;    // [rows / KS][nb]: copy unit (band, 128-column block) is in planes_t once it holds epoch
+  unsigned epoch;     // this launch's stamp, never 0 (flags are allocated zeroed)
   int nb, tiles, splits;
   int full;           // whole 128 x 128 tiles when S <= 3 (launch_syrk_tc decides)
   const int *S_dev;   // digit-plane count chosen by tc_scale_kernel
@@ -211,7 +266,8 @@ struct TcArgs {
   double *part;       // [splits][tiles][128*128]
   int accumulate;
   int *err;
-  unsigned long long *trace;  // [gridDim.x][TR_WORDS], written by the traced instantiation only
+  unsigned long long *trace;       // [gridDim.x][TR_WORDS], written by the traced instantiation only
+  unsigned long long *copy_trace;  // [gridDim.x][TR_COPY_WORDS], likewise
 };
 
 struct ItemInfo {
@@ -269,8 +325,10 @@ __device__ __forceinline__ void consumer_loop(const TcArgs &a, uint32_t ring, ui
   const uint32_t lda = ring + row * KS + ((((lane >> 4) & 1) ^ ((i >> 1) & 3)) << 4);
   const double inv256 = 1.0 / 256.0;
   long long tr[4] = {0, 0, 0, 0};  // trace: wait stage full, warpgroup vote, wgmma.wait_group, epilogue
-  const long long t_start = tclock<TRACE>();
-  const unsigned long long ns_start = TRACE ? globaltimer_ns() : 0;
+  // the start clock's low word (a launch spans far fewer than 2^32 clocks) and the start time written at once: at 232
+  // registers, the traced whole tiles would spill more across the items
+  const uint32_t t_start = (uint32_t)tclock<TRACE>();
+  if (TRACE && warp == 0 && lane == 0) a.trace[(size_t)blockIdx.x * TR_WORDS + TR_NS] = globaltimer_ns();
   int k = 0;  // stages consumed so far
   const int64_t per = rows_per_item(a);
   for (int item = blockIdx.x; item < n_items<FULL>(a); item += gridDim.x) {
@@ -360,25 +418,29 @@ __device__ __forceinline__ void consumer_loop(const TcArgs &a, uint32_t ring, ui
   if constexpr (TRACE) {
     if ((warp & 3) == 0 && lane == 0) {
       unsigned long long *o = a.trace + (size_t)blockIdx.x * TR_WORDS;
-      const long long total = clock64() - t_start;
+      const long long total = (uint32_t)((uint32_t)clock64() - t_start);
 #pragma unroll
       for (int w = 0; w < 4; w++) o[TR_CONS + 5 * wg + w] = tr[w];
       o[TR_CONS + 5 * wg + 4] = total;
       if (wg == 0) {
         o[TR_STAGES] = (FULL ? 2 : 1) * k;
-        o[TR_NS] = ns_start;
         o[TR_NS + 1] = globaltimer_ns();
       }
     }
   }
 }
 
-// The producer (one thread): per stage, the S planes of the A block, then the S planes of the B block (or of its column
-// half), all into one slot; each is one contiguous run of GqT.
+// The producer (warp 8): per stage, lane 0 loads the S planes of the A block and the S planes of the B block (or of its
+// column half) into one slot, each one contiguous run of GqT. Before stages ks .. ks + 15 of an item, the warp acquires
+// their copy units' readiness flags in one round trip: lane l < 16 that of the A block of stage ks + l, lane 16 + l
+// that of its B block (a B flag covers a column half too). An acquire and a proxy fence per stage would cost the
+// single issuing thread about as much as the consumers spend on a stage.
+constexpr int FLAG_BATCH = 16;
 template <int S, bool FULL, bool TRACE>
 __device__ __forceinline__ void producer_loop(const TcArgs &a, uint8_t *ring, uint64_t *full, uint64_t *empty) {
   using R = Ring<S, FULL>;
-  long long tr = 0;  // trace: wait slot empty
+  const int lane = threadIdx.x & 31;
+  long long tr = 0, trf = 0;  // trace: wait slot empty, wait readiness flags
   int sl = 0;
   uint32_t ph = 0;
   const int64_t per = rows_per_item(a);
@@ -386,27 +448,108 @@ __device__ __forceinline__ void producer_loop(const TcArgs &a, uint8_t *ring, ui
     const ItemInfo info = decode_item<FULL>(a, item, per);
     for (int ks = 0; ks < info.nsteps; ks++) {
       // band (k_begin / KS + ks) of the planes, then column bi * 128 (A) or bj * 128 + h * 64 (B) within it
-      const int8_t *band = a.planes_t + (info.k_begin + (int64_t)ks * KS) * a.ldq;
-      const int8_t *src_a = band + (int64_t)info.bi * TILE * KS, *src_b = band + (int64_t)(info.bj * TILE + info.h * HALF) * KS;
-      const long long t0 = tclock<TRACE>();
-      if (!mbar_wait(&empty[sl], ph ^ 1, a.err)) return;
-      if constexpr (TRACE) tr += clock64() - t0;
-      uint8_t *slot = ring + sl * R::SLOT;
-      mbar_expect_tx(&full[sl], R::SLOT);
-      for (int s = 0; s < S; s++) bulk_load(slot + s * A_PLANE_BYTES, src_a + s * a.plane, A_PLANE_BYTES, &full[sl]);
-      for (int s = 0; s < S; s++) bulk_load(slot + R::B_OFF + s * R::B_PLANE, src_b + s * a.plane, R::B_PLANE, &full[sl]);
+      const int64_t band = info.k_begin / KS + ks;
+      if (ks % FLAG_BATCH == 0) {
+        // Ordering of the copiers' generic-proxy stores before the bulk copies (async proxy) that read them, PTX ISA,
+        // memory consistency model: a copier's st.release and this ld.acquire (flag_wait) form a release / acquire
+        // pattern, so its stores happen before everything after the acquire in causality order; bar.warp.sync
+        // (__syncwarp) orders every lane's acquire before lane 0's later operations; and as the bulk copies read through
+        // the async proxy, "fence.proxy.async" is required between those generic-proxy writes and async-proxy reads of
+        // the same memory: lane 0 issues fence.proxy.async.global after the acquires and before its cp.async.bulk.
+        const long long t0 = tclock<TRACE>();
+        const int st = ks + (lane & (FLAG_BATCH - 1));
+        const bool ok = st >= info.nsteps ||
+                        flag_wait(a.flags + (band + (lane & (FLAG_BATCH - 1))) * a.nb + (lane < FLAG_BATCH ? info.bi : info.bj),
+                                  a.epoch, a.err);
+        __syncwarp();
+        if (!__all_sync(0xffffffffu, ok)) return;
+        if (lane == 0) asm volatile("fence.proxy.async.global;\n" ::: "memory");
+        if constexpr (TRACE) trf += clock64() - t0;
+      }
+      const long long t1 = tclock<TRACE>();
+      if (!__all_sync(0xffffffffu, mbar_wait(&empty[sl], ph ^ 1, a.err))) return;
+      if constexpr (TRACE) tr += clock64() - t1;
+      if (lane == 0) {
+        const int8_t *src = a.planes_t + band * KS * a.ldq;
+        const int8_t *src_a = src + (int64_t)info.bi * TILE * KS, *src_b = src + (int64_t)(info.bj * TILE + info.h * HALF) * KS;
+        uint8_t *slot = ring + sl * R::SLOT;
+        mbar_expect_tx(&full[sl], R::SLOT);
+        for (int s = 0; s < S; s++) bulk_load(slot + s * A_PLANE_BYTES, src_a + s * a.plane, A_PLANE_BYTES, &full[sl]);
+        for (int s = 0; s < S; s++) bulk_load(slot + R::B_OFF + s * R::B_PLANE, src_b + s * a.plane, R::B_PLANE, &full[sl]);
+      }
       if (++sl == R::D) { sl = 0; ph ^= 1; }
     }
   }
-  if constexpr (TRACE) a.trace[(size_t)blockIdx.x * TR_WORDS + TR_PROD] = tr;
+  if constexpr (TRACE) {
+    if (lane == 0) {
+      a.trace[(size_t)blockIdx.x * TR_WORDS + TR_PROD] = tr;
+      a.trace[(size_t)blockIdx.x * TR_WORDS + TR_PROD + 1] = trf;
+    }
+  }
+}
+
+// One copier warp (cw of ncw over all CTAs): units u = cw, cw + ncw, ... of the (rows / KS) x nb units (band-major, so
+// in ascending band order as the consumers of every k-split need them). Per plane s < S of a unit: the MN-major 64 x 128
+// tile of Gq into this warp's staging buffer (cp.async; the 16-byte chunk ch of row r at chunk ch ^ ((r >> 2) & 7), so
+// that the loads below hit 16 banks, two lanes each), then 4 x 4 byte transposes into GqT: lane (kq = lane % 16,
+// h = lane / 16) takes rows 4 kq .. 4 kq + 3 and in step it the 4 columns of word m = 2 it + h; the four 4-byte stores
+// of a step land, with those of the other lanes of its half-warp, whole 64-byte K-major rows. Then the unit's flag.
+template <int S, bool TRACE>
+__device__ __forceinline__ void copier_loop(const TcArgs &a, uint8_t *staging, int cw, int ncw) {
+  const int lane = threadIdx.x & 31, kq = lane & 15, h = lane >> 4;
+  const uint32_t st = smem_u32(staging), rows = st + 4 * kq * TILE;  // rows 4 kq .. 4 kq + 3 of the staged tile
+  const int units = (int)(a.rows / KS) * a.nb;  // < 2^31 (launch_syrk_tc)
+  for (int u = cw; u < units; u += ncw) {
+    const long long t0 = tclock<TRACE>();
+    const int band = u / a.nb, cb = u - band * a.nb;
+    const int8_t *src = a.planes + (int64_t)band * KS * a.ldq + cb * TILE;
+    int8_t *dst = a.planes_t + (int64_t)band * KS * a.ldq + cb * TILE * KS;
+    for (int s = 0; s < S; s++, src += a.plane, dst += a.plane) {
+#pragma unroll 1
+      for (int p = 0; p < KS * TILE / 16 / 32; p++) {
+        const int idx = lane + 32 * p, r = idx >> 3, ch = idx & 7;
+        cp_async16(st + r * TILE + ((ch ^ ((r >> 2) & 7)) << 4), src + (int64_t)r * a.ldq + 16 * ch);
+      }
+      const long long t1 = tclock<TRACE>();
+      cp_async_wait_all();
+      __syncwarp();
+      if (TRACE && lane == 0) atomicAdd(a.copy_trace + blockIdx.x * TR_COPY_WORDS + 1, (unsigned long long)(clock64() - t1));
+#pragma unroll 4
+      for (int it = 0; it < TILE / 8; it++) {
+        const int m = 2 * it + h;
+        const uint32_t wa = rows + (((m >> 2) ^ (kq & 7)) << 4) + 4 * (m & 3);  // word m of row 4 kq
+        const uint32_t w[4] = {lds32(wa), lds32(wa + TILE), lds32(wa + 2 * TILE), lds32(wa + 3 * TILE)};
+        uint32_t out[4];
+        transpose4x4(w, out);
+#pragma unroll
+        for (int j = 0; j < 4; j++) *reinterpret_cast<uint32_t *>(dst + kmajor_offset(4 * m + j, kq)) = out[j];
+      }
+      __syncwarp();  // every lane has read the staging buffer before the next plane lands in it
+    }
+    // Release pattern (PTX ISA, memory consistency model): the bar.warp.sync (__syncwarp) that ends the last plane orders
+    // every lane's stores before lane 0's st.release, which makes them visible to whoever acquires the flag
+    // (producer_loop). No proxy fence here: these stores are generic-proxy writes, the reader fences its async proxy.
+    if (lane == 0) flag_release(a.flags + u, a.epoch);
+    if (TRACE && lane == 0) {  // the trace's words, added per unit: nothing stays live across units
+      atomicAdd(a.copy_trace + blockIdx.x * TR_COPY_WORDS, (unsigned long long)(clock64() - t0));
+      atomicAdd(a.copy_trace + blockIdx.x * TR_COPY_WORDS + 2, (unsigned long long)S);
+    }
+  }
 }
 
 template <int S, bool FULL, bool TRACE>
-__device__ __forceinline__ void syrk_tc_cta(const TcArgs &a, uint8_t *ring, uint64_t *full, uint64_t *empty) {
+__device__ __forceinline__ void syrk_tc_cta(const TcArgs &a, uint8_t *ring, uint8_t *staging, uint64_t *full,
+                                            uint64_t *empty) {
   if (threadIdx.x >= 32 * CONSUMER_WARPS) {
     asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;\n" ::"n"(PRODUCER_REGS));
-    // ===================== producer (warp 8, one thread) =====================
-    if (threadIdx.x == 32 * CONSUMER_WARPS) producer_loop<S, FULL, TRACE>(a, ring, full, empty);
+    const int w = (threadIdx.x >> 5) - CONSUMER_WARPS - 1;  // copier warp 0..2, or -1 for the producer's warp
+    if (w < 0) {
+      // ===================== producer (warp 8) =====================
+      producer_loop<S, FULL, TRACE>(a, ring, full, empty);
+    } else {
+      // ===================== copiers (warps 9-11) =====================
+      copier_loop<S, TRACE>(a, staging + w * KS * TILE, COPIER_WARPS * blockIdx.x + w, COPIER_WARPS * gridDim.x);
+    }
   } else {
     // ===================== wgmma + epilogue =====================
     asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;\n" ::"n"(CONSUMER_REGS));
@@ -419,7 +562,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) syrk_tc_kernel(TcArgs a) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // 1024-byte aligned ring (the swizzle patterns are functions of the shared-memory address), then barriers
   uint8_t *ring = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t *full = reinterpret_cast<uint64_t *>(ring + RING_BYTES), *empty = full + MAX_SLOTS;
+  uint8_t *staging = ring + RING_BYTES;  // 16-byte aligned (cp.async)
+  uint64_t *full = reinterpret_cast<uint64_t *>(staging + STAGING_BYTES), *empty = full + MAX_SLOTS;
   if (threadIdx.x == 0) {
     for (int i = 0; i < MAX_SLOTS; i++) {
       mbar_init(&full[i], 1);
@@ -429,53 +573,13 @@ __global__ void __launch_bounds__(TC_THREADS, 1) syrk_tc_kernel(TcArgs a) {
   }
   __syncthreads();
   const int S = *a.S_dev;
-  if (S == 4) syrk_tc_cta<4, false, TRACE>(a, ring, full, empty);
-  else if (S == 3 && a.full) syrk_tc_cta<3, true, TRACE>(a, ring, full, empty);
-  else if (S == 3) syrk_tc_cta<3, false, TRACE>(a, ring, full, empty);
-  else if (a.full) syrk_tc_cta<2, true, TRACE>(a, ring, full, empty);
-  else syrk_tc_cta<2, false, TRACE>(a, ring, full, empty);
+  if (S == 4) syrk_tc_cta<4, false, TRACE>(a, ring, staging, full, empty);
+  else if (S == 3 && a.full) syrk_tc_cta<3, true, TRACE>(a, ring, staging, full, empty);
+  else if (S == 3) syrk_tc_cta<3, false, TRACE>(a, ring, staging, full, empty);
+  else if (a.full) syrk_tc_cta<2, true, TRACE>(a, ring, staging, full, empty);
+  else syrk_tc_cta<2, false, TRACE>(a, ring, staging, full, empty);
 }
-
-// K-major copy of the digit planes for s < *S_dev: band b = row / 64 of plane s of Gq [rows][ldq] becomes the run
-// GqT[s][b][ldq][64], column n's 64 contraction rows as one 64-byte row whose 16-byte chunk q sits at q ^ ((n >> 1) & 3):
-// the shared-memory image wgmma reads (sw64_desc) of every 128- or 64-column block of the band. A block moves a 64-row x
-// 128-column tile through shared memory: coalesced 16-byte loads of the MN-major rows, 4 x 4 byte transposes of words,
-// then the tile's 8 KB output run.
-constexpr int KT_ROWS = KS, KT_COLS = 128, KT_THREADS = 256;
-__global__ void __launch_bounds__(KT_THREADS) tc_kmajor_kernel(const int8_t *__restrict__ Gq, int8_t *__restrict__ GqT,
-                                                               int ldq, int64_t plane, const int *S_dev) {
-  const int s = blockIdx.z;
-  if (s >= *S_dev) return;
-  __shared__ uint32_t tile[KT_ROWS][KT_COLS / 4 + 1];
-  const int64_t r0 = (int64_t)blockIdx.x * KT_ROWS;
-  const int c0 = blockIdx.y * KT_COLS;
-  const int8_t *src = Gq + s * plane + r0 * ldq + c0;
-#pragma unroll
-  for (int p = 0; p < KT_ROWS * KT_COLS / 16 / KT_THREADS; p++) {
-    const int idx = threadIdx.x + p * KT_THREADS, r = idx >> 3, ch = idx & 7;
-    const uint4 v = __ldg(reinterpret_cast<const uint4 *>(src + (int64_t)r * ldq) + ch);
-    tile[r][4 * ch] = v.x;
-    tile[r][4 * ch + 1] = v.y;
-    tile[r][4 * ch + 2] = v.z;
-    tile[r][4 * ch + 3] = v.w;
-  }
-  __syncthreads();
-  int8_t *dst = GqT + s * plane + r0 * ldq + (int64_t)c0 * KS;  // band r0 / 64, column c0
-#pragma unroll
-  for (int p = 0; p < KT_ROWS * KT_COLS / 16 / KT_THREADS; p++) {
-    const int idx = threadIdx.x + p * KT_THREADS, kq = idx & 15, m = idx >> 4;  // rows 4 kq.., columns 4 m..
-    const uint32_t w0 = tile[4 * kq][m], w1 = tile[4 * kq + 1][m], w2 = tile[4 * kq + 2][m], w3 = tile[4 * kq + 3][m];
-    const uint32_t lo01 = __byte_perm(w0, w1, 0x5140), hi01 = __byte_perm(w0, w1, 0x7362);
-    const uint32_t lo23 = __byte_perm(w2, w3, 0x5140), hi23 = __byte_perm(w2, w3, 0x7362);
-    const uint32_t out[4] = {__byte_perm(lo01, lo23, 0x5410), __byte_perm(lo01, lo23, 0x7632),
-                             __byte_perm(hi01, hi23, 0x5410), __byte_perm(hi01, hi23, 0x7632)};
-#pragma unroll
-    for (int j = 0; j < 4; j++) {
-      const int n = 4 * m + j;  // column within the tile (c0 is a multiple of 8: the same swizzle row)
-      *reinterpret_cast<uint32_t *>(dst + n * KS + ((((kq >> 2) ^ (n >> 1)) & 3) << 4) + 4 * (kq & 3)) = out[j];
-    }
-  }
-}
+static_assert(RING_BYTES % 16 == 0 && STAGING_BYTES % 16 == 0, "staging and barrier alignment");
 
 // Column scales and digit-plane count of one batch, decided ON THE DEVICE from the column maxima and sums of squares
 // of G' (one block):
@@ -569,7 +673,9 @@ __global__ void tc_adopt_kernel(double *sc, double *isc, int *S_dev, const doubl
 
 
 struct TcState {
-  int8_t *GqT = nullptr;    // [SMAX][rows_alloc / KS][ldg][KS] K-major copy of c->Gq (tc_kmajor_kernel)
+  int8_t *GqT = nullptr;    // [SMAX][rows_alloc / KS][ldg][KS] K-major copy of c->Gq (syrk_tc_kernel's copiers)
+  unsigned *flags = nullptr;  // [rows_alloc / KS][ldg / 128] readiness of its copy units, stamped with epoch
+  unsigned epoch = 0;         // of the last SYRK launch
   double *sc = nullptr, *isc = nullptr;
   double *sc_next = nullptr, *isc_next = nullptr;  // fresh scales of the last full-range evaluation (speculation)
   int *S_next = nullptr, *spec_ok = nullptr;
@@ -586,35 +692,32 @@ struct TcState {
   int64_t last_rows_padded = 0;  // contraction rows of the last batch's SYRK (0: none since the registration)
 };
 
-// The K-major copy of the first rows_padded rows of the planes Gq [SMAX][rows_alloc][ldq] into GqT (same plane size),
-// the *S_dev planes in use only.
-int launch_tc_kmajor(balm_ctx *c, const int8_t *Gq, int8_t *GqT, int ldq, int64_t rows_alloc, int64_t rows_padded,
-                     const int *S_dev) {
-  const dim3 grid((unsigned)(rows_padded / KT_ROWS), (unsigned)(ldq / KT_COLS), SMAX);
-  tc_kmajor_kernel<<<grid, KT_THREADS, 0, c->stream>>>(Gq, GqT, ldq, rows_alloc * ldq, S_dev);
-  CUDA_TRY(cudaGetLastError());
-  c->launches += 1;
-  return BALM_OK;
-}
-
-// One syrk_tc_kernel launch on c's stream: rows_padded (a multiple of KS) contraction rows of the K-major planes
-// planes_t (plane stride `plane` bytes), nb x nb blocks of 128 columns, `splits` k-splits; one CTA per item up to one per SM. Whole 128 x 128 tiles
-// (at S <= 3) halve the L2 traffic per MAC but also the item count, so they are taken only when every SM still gets
-// an item (tiles x splits >= SMs); BALM_TC_TILE=half|full (c->tc_tile) overrides the rule.
+// One syrk_tc_kernel launch on c's stream: rows_padded (a multiple of KS) contraction rows of the MN-major planes
+// `planes`, copied K-major into planes_t by the launch itself (both of plane stride `plane` bytes), nb x nb blocks of 128
+// columns, `splits` k-splits; one CTA per item up to one per SM. Whole 128 x 128 tiles (at S <= 3) halve the L2 traffic
+// per MAC but also the item count, so they are taken only when every SM still gets an item (tiles x splits >= SMs);
+// BALM_TC_TILE=half|full (c->tc_tile) overrides the rule. flags: (rows_padded / KS) x nb words, none equal to epoch.
+// A CTA waits on copy units of other CTAs, so the launch is cooperative: all CTAs are resident, or it fails.
 // With c->tc_trace (BALM_TC_TRACE) the traced instantiation runs and records the launch.
-int launch_syrk_tc(balm_ctx *c, const int8_t *planes_t, int64_t plane, int64_t rows_padded, int nb, int tiles,
-                   int splits, const int *S_dev, const double *isc, double *part, bool accumulate, int *err) {
+int launch_syrk_tc(balm_ctx *c, const int8_t *planes, int8_t *planes_t, int64_t plane, int64_t rows_padded, int nb,
+                   int tiles, int splits, const int *S_dev, const double *isc, double *part, bool accumulate, int *err,
+                   unsigned *flags, unsigned epoch) {
+  if (rows_padded / KS * nb > INT32_MAX) {  // the copiers count units in int
+    balm_set_error("tensor SYRK: more than 2^31 copy units");
+    return BALM_ERR_INVALID;
+  }
   const bool full = c->tc_tile == 0 ? (int64_t)tiles * splits >= c->sm_count : c->tc_tile == 2;
-  TcArgs a{planes_t, plane, c->ldg, rows_padded, nb, tiles, splits, full ? 1 : 0, S_dev, isc, part, accumulate ? 1 : 0, err, c->tc_trace};
+  unsigned long long *copy_trace = c->tc_trace ? c->tc_trace + (size_t)c->sm_count * TR_WORDS : nullptr;
+  TcArgs a{planes, planes_t, plane, c->ldg, rows_padded, flags, epoch, nb, tiles, splits, full ? 1 : 0,
+           S_dev, isc, part, accumulate ? 1 : 0, err, c->tc_trace, copy_trace};
   const int items = a.tiles * 2 * a.splits;  // half-tile items; the whole-tile count when S <= 3 is not known here
   const int grid = items < c->sm_count ? items : c->sm_count;
-  if (c->tc_trace) {
-    CUDA_TRY(cudaMemsetAsync(c->tc_trace, 0, sizeof(unsigned long long) * c->sm_count * TR_WORDS, c->stream));
-    syrk_tc_kernel<true><<<grid, TC_THREADS, TC_SMEM, c->stream>>>(a);
-  } else {
-    syrk_tc_kernel<false><<<grid, TC_THREADS, TC_SMEM, c->stream>>>(a);
-  }
-  CUDA_TRY(cudaGetLastError());
+  void *params[] = {&a};
+  if (c->tc_trace)
+    CUDA_TRY(cudaMemsetAsync(c->tc_trace, 0, sizeof(unsigned long long) * c->sm_count * (TR_WORDS + TR_COPY_WORDS),
+                             c->stream));
+  const void *kernel = c->tc_trace ? (const void *)syrk_tc_kernel<true> : (const void *)syrk_tc_kernel<false>;
+  CUDA_TRY(cudaLaunchCooperativeKernel(kernel, dim3(grid), dim3(TC_THREADS), params, TC_SMEM, c->stream));
   return BALM_OK;
 }
 
@@ -643,6 +746,9 @@ int tensor_syrk_init(balm_ctx *c) {
   CUDA_TRY(cudaMemset(c->Gq, 0, (size_t)SMAX * st->rows_alloc * ldq));  // column padding [6N, ldg) stays zero
   CUDA_TRY(cudaMalloc((void **)&st->GqT, (size_t)SMAX * st->rows_alloc * ldq));
   CUDA_TRY(cudaMemset(st->GqT, 0, (size_t)SMAX * st->rows_alloc * ldq));
+  const size_t n_flags = (size_t)(st->rows_alloc / KS) * (ldq / TILE);
+  CUDA_TRY(cudaMalloc((void **)&st->flags, sizeof(unsigned) * n_flags));
+  CUDA_TRY(cudaMemset(st->flags, 0, sizeof(unsigned) * n_flags));
   CUDA_TRY(cudaMalloc((void **)&st->S_dev, sizeof(int)));
   CUDA_TRY(cudaMalloc((void **)&st->sc, sizeof(double) * ldq));
   CUDA_TRY(cudaMalloc((void **)&st->isc, sizeof(double) * ldq));
@@ -676,7 +782,7 @@ void tensor_syrk_free(balm_ctx *c) {
     TcState *st = static_cast<TcState *>(c->tmap);
     cudaFree(st->sc_next); cudaFree(st->isc_next); cudaFree(st->S_next); cudaFree(st->spec_ok);
     cudaFree(st->sc); cudaFree(st->isc); cudaFree(st->colmax); cudaFree(st->err); cudaFree(st->S_dev);
-    cudaFree(st->GqT);
+    cudaFree(st->GqT); cudaFree(st->flags);
     delete st;
     c->tmap = nullptr;
   }
@@ -686,8 +792,8 @@ void tensor_syrk_free(balm_ctx *c) {
 }
 
 // One batch of the tensor path: (1) column maxima of G' -> power-of-two scales, (2) observation sweep writing the
-// int8 digit planes directly, (3) their K-major copy and the tensor-core SYRK. ev[2] is recorded between the
-// observation sweeps and the K-major copy, so the SYRK's time includes the copy.
+// int8 digit planes directly, (3) the tensor-core SYRK, which makes their K-major copy as it goes. ev[2] is recorded
+// between the observation sweeps and the SYRK.
 int tensor_obs_and_syrk(balm_ctx *c, const double *poses, int64_t v0, int64_t v1, bool first_batch) {
   TcState *st = static_cast<TcState *>(c->tmap);
   if (!st) { balm_set_error("tensor path not initialised"); return BALM_ERR_INVALID; }
@@ -723,9 +829,12 @@ int tensor_obs_and_syrk(balm_ctx *c, const double *poses, int64_t v0, int64_t v1
   st->last_rows_padded = rows_padded;
   CUDA_TRY(cudaEventRecord(c->ev[2], c->stream));
   c->launches += 2;
-  TRY(launch_tc_kmajor(c, c->Gq, st->GqT, ldq, st->rows_alloc, rows_padded, st->S_dev));
-  return launch_syrk_tc(c, st->GqT, plane_stride, rows_padded, c->syrk_nb, c->syrk_tiles, c->syrk_splits,
-                        st->S_dev, st->isc, c->syrk_part, !first_batch, st->err);
+  if (++st->epoch == 0) {  // after 2^32 launches: flags of old launches could hold any stamp
+    CUDA_TRY(cudaMemsetAsync(st->flags, 0, sizeof(unsigned) * (size_t)(st->rows_alloc / KS) * c->syrk_nb, c->stream));
+    st->epoch = 1;
+  }
+  return launch_syrk_tc(c, c->Gq, st->GqT, plane_stride, rows_padded, c->syrk_nb, c->syrk_tiles, c->syrk_splits,
+                        st->S_dev, st->isc, c->syrk_part, !first_batch, st->err, st->flags, st->epoch);
 }
 
 // The SYRK's error flag, the digit-plane count and the speculation verdict of the batch in flight: the copies are
@@ -791,8 +900,11 @@ extern "C" int balm_debug_syrk_tc(balm_ctx *c, const int8_t *planes, int S, int6
   int8_t *d_planes, *d_planes_t;
   double *d_isc, *d_part;
   int *d_S, *d_err;
+  unsigned *d_flags;
+  const size_t n_flags = (size_t)(rows_padded / KS) * nb;
   TRY(pool.get(&d_planes, SMAX * plane));
   TRY(pool.get(&d_planes_t, SMAX * plane));
+  TRY(pool.get(&d_flags, n_flags));
   TRY(pool.get(&d_isc, (size_t)ldq));
   TRY(pool.get(&d_part, count));
   TRY(pool.get(&d_S, 1));
@@ -805,10 +917,10 @@ extern "C" int balm_debug_syrk_tc(balm_ctx *c, const int8_t *planes, int S, int6
   CUDA_TRY(cudaMemcpyAsync(d_part, part, sizeof(double) * count, cudaMemcpyHostToDevice, c->stream));
   CUDA_TRY(cudaMemcpyAsync(d_S, &S, sizeof(int), cudaMemcpyHostToDevice, c->stream));
   CUDA_TRY(cudaMemsetAsync(d_err, 0, sizeof(int), c->stream));
+  CUDA_TRY(cudaMemsetAsync(d_flags, 0, sizeof(unsigned) * n_flags, c->stream));
   TRY(syrk_tc_set_smem());
-  TRY(launch_tc_kmajor(c, d_planes, d_planes_t, ldq, rows_padded, rows_padded, d_S));
-  TRY(launch_syrk_tc(c, d_planes_t, (int64_t)plane, rows_padded, nb, tiles, splits, d_S, d_isc, d_part, accumulate != 0,
-                     d_err));
+  TRY(launch_syrk_tc(c, d_planes, d_planes_t, (int64_t)plane, rows_padded, nb, tiles, splits, d_S, d_isc, d_part,
+                     accumulate != 0, d_err, d_flags, 1));
   int err = 0;
   CUDA_TRY(cudaMemcpyAsync(&err, d_err, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
   CUDA_TRY(cudaMemcpyAsync(part, d_part, sizeof(double) * count, cudaMemcpyDeviceToHost, c->stream));
@@ -853,5 +965,19 @@ extern "C" int balm_debug_tc_trace(balm_ctx *c, unsigned long long *out, int max
   CUDA_TRY(cudaStreamSynchronize(c->stream));
   const size_t total = std::min<size_t>((size_t)max_entries, (size_t)c->sm_count * TR_WORDS);
   CUDA_TRY(cudaMemcpy(out, c->tc_trace, sizeof(unsigned long long) * total, cudaMemcpyDeviceToHost));
+  return BALM_OK;
+}
+
+extern "C" int balm_debug_tc_copy_trace(balm_ctx *c, unsigned long long *out, int max_entries) {
+  if (c) TRY(refuse_blocks(c, "balm_debug_tc_copy_trace"));
+  if (!c || !out || !c->tc_trace || max_entries < 0) {
+    balm_set_error("balm_debug_tc_copy_trace: no trace (BALM_TC_TRACE=1 at the creation of a tensor-precision context)");
+    return BALM_ERR_INVALID;
+  }
+  CUDA_TRY(cudaSetDevice(c->device));
+  CUDA_TRY(cudaStreamSynchronize(c->stream));
+  const size_t total = std::min<size_t>((size_t)max_entries, (size_t)c->sm_count * TR_COPY_WORDS);
+  CUDA_TRY(cudaMemcpy(out, c->tc_trace + (size_t)c->sm_count * TR_WORDS, sizeof(unsigned long long) * total,
+                      cudaMemcpyDeviceToHost));
   return BALM_OK;
 }

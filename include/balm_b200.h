@@ -553,11 +553,16 @@ int balm_debug_dag_trace(balm_ctx *ctx, unsigned long long *out, int max_entries
  *   3..7 consumer warp 0 and 8..12 consumer warp 4 (one per warpgroup): waiting on the stage full, in the warpgroup's
  *   vote that it arrived, in wgmma.wait_group, epilogue, total;
  *   13..15 zero (there is no transposer warp any more);
- *   16 producer: waiting on a free slot; 17 zero.
+ *   16 producer: waiting on a free slot; 17 producer: waiting on the readiness flags of the stage's copy units.
  * Copies min(max_entries, 18 x SM count) words; BALM_ERR_INVALID when the ctx records no trace. Without the variable
  * the SYRK runs an instantiation that reads no clock. BALM_TC_TILE=half|full at ctx creation forces the SYRK's item
  * shape (default: whole tiles at S <= 3 when tiles x k-splits >= the SM count). */
 int balm_debug_tc_trace(balm_ctx *ctx, unsigned long long *out, int max_entries);
+/* Debug aid: the same launch's copier warps (which copy the digit planes K-major, one 64-row x 128-column tile of one
+ * plane at a time), 3 words per CTA, CTA b at 3 b: 0 clock64 sum over its copier warps of the time spent on their copy
+ * units; 1 of that, the time waiting on their loads; 2 plane tiles copied (summed over CTAs: digit planes x
+ * ceil(rows / 64) x ldg / 128). Copies min(max_entries, 3 x SM count) words; BALM_ERR_INVALID as balm_debug_tc_trace. */
+int balm_debug_tc_copy_trace(balm_ctx *ctx, unsigned long long *out, int max_entries);
 /* Debug aid: the tensor path's SYRK kernel alone, on caller-supplied digit planes, so that its fp64 partial tiles can be
  * compared bit for bit with an exact integer reference. Uses ctx's device, stream and column count ldg = 6N rounded up
  * to 128 (tiles = T (T + 1) / 2 upper-triangle tiles of 128 x 128, T = ldg / 128); neither needs nor touches a

@@ -21,7 +21,8 @@ from balm_b200 import _lib as L  # noqa: E402
 WORDS = 18
 ROLES = [("consumer warp 0", 3, ["wait stage full", "warpgroup vote", "wgmma.wait_group", "epilogue", "total"]),
          ("consumer warp 4", 8, ["wait stage full", "warpgroup vote", "wgmma.wait_group", "epilogue", "total"]),
-         ("producer", 16, ["wait slot empty"])]
+         ("producer", 16, ["wait slot empty", "wait flags"])]
+COPY_WORDS = 3
 
 N = int(sys.argv[1]) if len(sys.argv) > 1 else 500
 M = int(sys.argv[2]) if len(sys.argv) > 2 else 100000
@@ -48,5 +49,17 @@ for role, off, cats in ROLES:
         top = float(tr[busiest, off + k] / stages[busiest])
         out[f"{role}/{cat}"] = round(mean, 1)
         print(f"{role:18s} {cat:18s} {mean:15.1f} {top:12.1f}")
+cbuf = np.zeros(COPY_WORDS * 1024, dtype=np.uint64)
+L.check(L.lib().balm_debug_tc_copy_trace(c._h, cbuf.ctypes.data_as(C.c_void_p), len(cbuf)))
+# per CTA: its three copier warps' clocks on their units, of those the clocks waiting on loads, plane tiles copied
+ct = cbuf.reshape(-1, COPY_WORDS).astype(np.int64)
+ct = ct[ct[:, 2] > 0]
+out.update({"copier/plane tiles": int(ct[:, 2].sum()),
+            "copier/clk per plane tile": float((ct[:, 0] / ct[:, 2]).mean()),
+            "copier/busy share of consumer span": float(ct[:, 0].mean() / 3 / tr[:, 7].mean()),
+            "copier/wait share": float(ct[:, 1].sum() / max(ct[:, 0].sum(), 1))})
+print(f"copiers: {out['copier/plane tiles']} plane tiles, {out['copier/clk per plane tile']:.0f} clk per tile and warp, "
+      f"busy {100 * out['copier/busy share of consumer span']:.1f} % of the consumers' span, "
+      f"{100 * out['copier/wait share']:.1f} % of that waiting on loads")
 print(json.dumps(out))
 c.close()
