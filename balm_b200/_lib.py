@@ -46,7 +46,7 @@ _lib = None
 # every symbol include/balm_b200.h declares (tests check that the library exports all of them)
 SYMBOLS = ["balm_last_error", "balm_version", "balm_create", "balm_destroy", "balm_set_voxels",
            "balm_set_voxels_dev", "balm_evaluate", "balm_residual", "balm_solve", "balm_damping_iter",
-           "balm_default_lm_opts", "balm_comm_unique_id", "balm_comm_init", "balm_get_timings",
+           "balm_default_lm_opts", "balm_comm_unique_id", "balm_comm_init", "balm_get_timings", "balm_get_reused_sweeps",
            "balm_reset_counters", "balm_sync", "balm_timer_begin", "balm_timer_end", "balm_device_views", "balm_debug_dag_trace",
            "balm_debug_syrk_tc", "balm_debug_tc_planes", "balm_debug_tc_trace", "balm_debug_tc_copy_trace", "balm_synth_virtual",
            "balm_download_voxels", "balm_download_voxel_range", "balm_num_obs", "balm_default_assoc_opts", "balm_cut_voxels", "balm_pose_covariance", "balm_marginalize", "balm_download_fix", "balm_append_scan",
@@ -86,6 +86,7 @@ def lib():
         L.balm_comm_unique_id.argtypes = [C.c_void_p]
         L.balm_comm_init.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p]
         L.balm_get_timings.argtypes = [C.c_void_p, C.POINTER(Timings)]
+        L.balm_get_reused_sweeps.argtypes = [C.c_void_p, C.POINTER(C.c_int)]
         L.balm_reset_counters.argtypes = [C.c_void_p]
         L.balm_sync.argtypes = [C.c_void_p]
         L.balm_timer_begin.argtypes = [C.c_void_p]

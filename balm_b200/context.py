@@ -356,7 +356,9 @@ class Context:
     def timings(self):
         t = L.Timings()
         L.check(L.lib().balm_get_timings(self._h, C.byref(t)))
-        return {k: getattr(t, k) for k, _ in L.Timings._fields_}
+        reused = C.c_int()
+        L.check(L.lib().balm_get_reused_sweeps(self._h, C.byref(reused)))
+        return {**{k: getattr(t, k) for k, _ in L.Timings._fields_}, "reused_sweeps": reused.value}
 
     def reset_counters(self):
         L.check(L.lib().balm_reset_counters(self._h))

@@ -850,16 +850,19 @@ extern "C" int balm_damping_iter(balm_ctx *c, double *poses12, const balm_lm_opt
   tensor_syrk_new_problem(c);  // nothing speculative is carried over from earlier calls
   struct LmScope {             // lm_active / defer are cleared on every exit path
     balm_ctx *c;
-    ~LmScope() { c->lm_active = false; c->defer = false; c->pending_eval = false; }
+    ~LmScope() { c->lm_active = false; c->defer = false; c->pending_eval = false; c->eval_same_poses = false; }
   } lm_scope{c};
   c->lm_active = true;
+  bool same_poses = false;  // the last step was rejected: c->poses are those of the previous evaluation
   for (int it = 0; it < o->max_iter; it++) {
     // evaluation -> solve -> pose update -> trial residual are enqueued back to back; the host waits once, at the
     // end of residual_dev, and then reads r1, q1, the pivot flag and the phase timers
     c->defer = !getenv("BALM_SYNC_PHASES");
     int rc = BALM_OK;
     if (calc_hess) {
+      c->eval_same_poses = same_poses;
       rc = evaluate_dev(c, c->poses, 0, c->M, o->hess_includes_fix != 0, stats_cached);
+      c->eval_same_poses = false;
       if (rc == BALM_OK && cudaMemcpyAsync(c->h_scal, c->scal, sizeof(double), cudaMemcpyDeviceToHost, c->stream) != cudaSuccess)
         rc = BALM_ERR_CUDA;
     }
@@ -891,9 +894,11 @@ extern "C" int balm_damping_iter(balm_ctx *c, double *poses12, const balm_lm_opt
       }
       stats_cached = hand_over;
       calc_hess = true;
+      same_poses = false;
     } else {
       calc_hess = o->force_hess != 0;
       stats_cached = c->stats_trial != nullptr;  // c->stats still describes c->poses (single batch)
+      same_poses = true;
     }
     if (trace) trace[it] = t;
     if (poses_per_iter)
@@ -1522,9 +1527,15 @@ extern "C" int balm_get_timings(balm_ctx *c, balm_timings *out) {
   out->launches = (int)c->launches;
   return BALM_OK;
 }
+extern "C" int balm_get_reused_sweeps(balm_ctx *c, int *out) {
+  if (!c || !out) return BALM_ERR_INVALID;
+  *out = c->reused_sweeps;
+  return BALM_OK;
+}
 extern "C" int balm_reset_counters(balm_ctx *c) {
   if (!c) return BALM_ERR_INVALID;
   c->launches = 0;
+  c->reused_sweeps = 0;
   c->tm = balm_timings{};
   return BALM_OK;
 }

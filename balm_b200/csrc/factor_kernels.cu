@@ -143,7 +143,8 @@ struct ObsArgs {
   int8_t *Gq;           // [S][rows_alloc][ldg]
   int64_t plane_stride;
   const int *S_dev;     // digit-plane count chosen on the device by tc_scale_kernel
-  const int *skip;      // OBS_INT8: the speculative single sweep was accepted -> nothing to do
+  const int *skip;      // device flag, nonzero -> nothing to do. OBS_INT8: the speculative single sweep was accepted;
+                        // OBS_FUSED: the planes and accumulators of the same poses and scales are still in place
   // csc
   const int *csc_ptr, *csc_obs, *csc_vox;
   const int *csc_lo, *csc_hi;  // [N] this batch's segment of every pose's list
@@ -170,8 +171,8 @@ __global__ void __launch_bounds__(WPC * 32, MINB) obs_pass_kernel(ObsArgs a) {
   const int tile = blockIdx.y * WPC + warp;
   const int i = tile * 32 + lane;
   if (tile * 32 >= a.N) return;
-  if (MODE == OBS_INT8 && a.skip && *a.skip) return;
   constexpr bool EMIT = (MODE == OBS_INT8 || MODE == OBS_FUSED);
+  if (EMIT && a.skip && *a.skip) return;
   const bool active = i < a.N;
   double r[9], p[3];
   if (active) load_pose(a.poses + 12 * i, r, p);
@@ -343,9 +344,9 @@ __global__ void __launch_bounds__(WPC * 32, MINB) obs_pass_kernel(ObsArgs a) {
 }
 
 __global__ void obs_reduce_kernel(const double *part, int chunks, int total, double *accum, double *accum_batch,
-                                  int add) {
+                                  int add, const int *skip = nullptr) {
   const int e = blockIdx.x * blockDim.x + threadIdx.x;
-  if (e >= total) return;
+  if (e >= total || (skip && *skip)) return;
   double s = 0.0;
   for (int c = 0; c < chunks; c++) s += part[(size_t)c * total + e];
   accum[e] = add ? accum[e] + s : s;
@@ -449,7 +450,8 @@ int launch_obs_colmax(balm_ctx *c, const double *poses, int64_t v0, int64_t v1, 
 }
 
 // tensor path, sweep 2: int8 digit planes written directly. `fused`: the single speculative sweep (column maxima,
-// accumulators AND digit planes with the previous evaluation's scales); `skip`: device flag that disarms sweep 2.
+// accumulators AND digit planes with the previous evaluation's scales); `skip`: device flag that disarms sweep 2, or
+// the fused sweep and its reduction (what they would write is already in place).
 int launch_obs_int8(balm_ctx *c, const double *poses, int64_t v0, int64_t v1, bool first_batch, const double *sc,
                     int8_t *Gq, int64_t plane_stride, const int *S_dev, int S_alloc, int64_t rows_padded, bool fused,
                     const int *skip) {
@@ -476,7 +478,7 @@ int launch_obs_int8(balm_ctx *c, const double *poses, int64_t v0, int64_t v1, bo
     else obs_pass_kernel<false, OBS_FUSED><<<grid, 128, 0, c->stream>>>(a);
     const int total = BALM_ACC * c->Np;
     obs_reduce_kernel<<<(total + 255) / 256, 256, 0, c->stream>>>(c->obs_part, chunks, total, c->accum,
-                                                                  c->accum_batch, first_batch ? 0 : 1);
+                                                                  c->accum_batch, first_batch ? 0 : 1, skip);
     c->launches += 2;
   } else {
     if (c->dense) obs_pass_kernel<true, OBS_INT8><<<grid, 128, 0, c->stream>>>(a);

@@ -91,6 +91,7 @@ struct balm_ctx {
   bool defer = false;         // inside balm_damping_iter: phases are enqueued back to back, one host sync per iteration
   bool pending_eval = false;  // an evaluation's events / flags still have to be read (defer mode)
   bool pending_stats_cached = false;
+  bool eval_same_poses = false;  // the evaluation in progress follows a rejected LM step: the previous one had its poses
   int sm_count = 132;
 
   // ---- registered problem (device) ----
@@ -171,6 +172,7 @@ struct balm_ctx {
 
   // ---- instrumentation ----
   balm_timings tm{};
+  int reused_sweeps = 0;  // balm_get_reused_sweeps (kept out of balm_timings, whose layout is fixed)
   cudaEvent_t ev[16] = {};
   long long launches = 0;
 };

@@ -658,17 +658,31 @@ __global__ void __launch_bounds__(1024) tc_scale_kernel(const unsigned long long
   }
 }
 
-// start of a speculative evaluation: the scales found by the previous one become the ones in use
+// start of a speculative evaluation (one block): the scales found by the previous one become the ones in use
 // (skew: test hook BALM_TC_SPEC_SKEW -- the adopted scales are multiplied by 2^skew so that the device-side check
-//  has something to reject; 0 in production)
-__global__ void tc_adopt_kernel(double *sc, double *isc, int *S_dev, const double *sc_next, const double *isc_next,
-                                const int *S_next, int ldq, int skew) {
-  const int j = blockIdx.x * blockDim.x + threadIdx.x;
-  if (j < ldq) {
+//  has something to reject; 0 in production), and the column maxima are cleared for the fused sweep.
+// same_poses: the previous evaluation was at these poses (a rejected LM step). If its planes were written by the
+// fused sweep and kept (*spec_ok, still its verdict) and the adopted scales and plane count equal the ones they were
+// written with, a fused sweep now would write the same planes, column maxima and accumulator partials bit for bit
+// (and the check would keep them again): *reuse = 1 and the sweep, its reduction and the clearing are skipped.
+__global__ void __launch_bounds__(1024) tc_adopt_kernel(double *sc, double *isc, int *S_dev, const double *sc_next,
+                                                        const double *isc_next, const int *S_next, int ldq, int skew,
+                                                        int same_poses, const int *spec_ok, int *reuse,
+                                                        unsigned long long *colmax) {
+  int differ = !same_poses || *spec_ok == 0 || *S_next != *S_dev;
+  if (!differ)
+    for (int j = threadIdx.x; j < ldq; j += blockDim.x)
+      if (ldexp(sc_next[j], skew) != sc[j]) differ = 1;
+  const bool keep = __syncthreads_or(differ) == 0;  // every read of sc / S_dev above precedes the writes below
+  for (int j = threadIdx.x; j < ldq; j += blockDim.x) {
     sc[j] = ldexp(sc_next[j], skew);
     isc[j] = ldexp(isc_next[j], -skew);
+    if (!keep) colmax[j] = 0ull;
   }
-  if (j == 0) *S_dev = *S_next;
+  if (threadIdx.x == 0) {
+    *S_dev = *S_next;
+    *reuse = keep ? 1 : 0;
+  }
 }
 
 
@@ -683,6 +697,8 @@ struct TcState {
   bool spec_enabled = true;                        // BALM_NO_SPEC=1 keeps the two-sweep path
   bool last_spec = false;                          // the batch in flight used the fused sweep
   int spec_skew = 0;                               // BALM_TC_SPEC_SKEW (tests)
+  int *reuse = nullptr;                            // tc_adopt_kernel: the fused sweep of the batch in flight is skipped
+  bool reuse_enabled = true;                       // BALM_NO_SWEEP_REUSE=1 sweeps again after every rejected step
   unsigned long long *colmax = nullptr;
   int *err = nullptr;
   int64_t rows_alloc = 0;
@@ -757,7 +773,10 @@ int tensor_syrk_init(balm_ctx *c) {
   CUDA_TRY(cudaMalloc((void **)&st->S_next, sizeof(int)));
   CUDA_TRY(cudaMalloc((void **)&st->spec_ok, sizeof(int)));
   CUDA_TRY(cudaMemset(st->spec_ok, 0, sizeof(int)));
+  CUDA_TRY(cudaMalloc((void **)&st->reuse, sizeof(int)));
+  CUDA_TRY(cudaMemset(st->reuse, 0, sizeof(int)));
   st->spec_enabled = getenv("BALM_NO_SPEC") == nullptr;
+  st->reuse_enabled = getenv("BALM_NO_SWEEP_REUSE") == nullptr;
   if (const char *e = getenv("BALM_TC_SPEC_SKEW")) st->spec_skew = atoi(e);
   CUDA_TRY(cudaMalloc((void **)&st->colmax, sizeof(unsigned long long) * ldq));
   CUDA_TRY(cudaMalloc((void **)&st->err, sizeof(int)));
@@ -780,7 +799,7 @@ int tensor_syrk_init(balm_ctx *c) {
 void tensor_syrk_free(balm_ctx *c) {
   if (c->tmap) {
     TcState *st = static_cast<TcState *>(c->tmap);
-    cudaFree(st->sc_next); cudaFree(st->isc_next); cudaFree(st->S_next); cudaFree(st->spec_ok);
+    cudaFree(st->sc_next); cudaFree(st->isc_next); cudaFree(st->S_next); cudaFree(st->spec_ok); cudaFree(st->reuse);
     cudaFree(st->sc); cudaFree(st->isc); cudaFree(st->colmax); cudaFree(st->err); cudaFree(st->S_dev);
     cudaFree(st->GqT); cudaFree(st->flags);
     delete st;
@@ -800,7 +819,6 @@ int tensor_obs_and_syrk(balm_ctx *c, const double *poses, int64_t v0, int64_t v1
   const int ldq = c->ldg;
   const int64_t rows = 3 * (v1 - v0);
   const int64_t rows_padded = (rows + KS - 1) / KS * KS;
-  CUDA_TRY(cudaMemsetAsync(st->colmax, 0, sizeof(unsigned long long) * ldq, c->stream));
   // Speculation lives inside one balm_damping_iter call only: its first evaluation sweeps twice, and the public
   // balm_evaluate always does -- so every entry point stays a pure function of its arguments (same inputs, same bits,
   // whatever was evaluated before).
@@ -809,12 +827,16 @@ int tensor_obs_and_syrk(balm_ctx *c, const double *poses, int64_t v0, int64_t v1
   const int64_t plane_stride = (int64_t)st->rows_alloc * ldq;
   int rc;
   if (spec) {  // one sweep with the previous evaluation's scales; sweep 2 below only runs if tc_scale_kernel re-arms it
-    tc_adopt_kernel<<<(ldq + 255) / 256, 256, 0, c->stream>>>(st->sc, st->isc, st->S_dev, st->sc_next, st->isc_next,
-                                                              st->S_next, ldq, st->spec_skew);
+    // (and none at all when a rejected step left the planes of these poses and scales in place: tc_adopt_kernel).
+    // Dense scenes only: a sparse batch's planes are cleared before its sweep.
+    const bool may_reuse = c->eval_same_poses && st->reuse_enabled && c->dense;
+    tc_adopt_kernel<<<1, 1024, 0, c->stream>>>(st->sc, st->isc, st->S_dev, st->sc_next, st->isc_next, st->S_next, ldq,
+                                               st->spec_skew, may_reuse ? 1 : 0, st->spec_ok, st->reuse, st->colmax);
     c->launches += 1;
     rc = launch_obs_int8(c, poses, v0, v1, first_batch, st->sc, c->Gq, plane_stride, st->S_dev, SMAX, rows_padded, true,
-                         nullptr);
+                         may_reuse ? st->reuse : nullptr);
   } else {
+    CUDA_TRY(cudaMemsetAsync(st->colmax, 0, sizeof(unsigned long long) * ldq, c->stream));
     rc = launch_obs_colmax(c, poses, v0, v1, first_batch);
   }
   if (rc != BALM_OK) return rc;
@@ -845,6 +867,7 @@ int tensor_syrk_check_enqueue(balm_ctx *c) {
   CUDA_TRY(cudaMemcpyAsync(c->h_flags + 1, st->err, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
   CUDA_TRY(cudaMemcpyAsync(c->h_flags + 2, st->S_dev, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
   CUDA_TRY(cudaMemcpyAsync(c->h_flags + 3, st->spec_ok, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+  CUDA_TRY(cudaMemcpyAsync(c->h_flags + 5, st->reuse, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
   return BALM_OK;
 }
 
@@ -853,7 +876,10 @@ int tensor_syrk_check_finish(balm_ctx *c) {  // after the stream has been synchr
   if (!st) return BALM_OK;
   st->last_S = c->h_flags[2];
   c->tm.digit_planes = st->last_S;
-  if (st->last_spec) (c->h_flags[3] ? c->tm.single_sweeps : c->tm.redone_sweeps) += 1;
+  if (st->last_spec) {
+    (c->h_flags[3] ? c->tm.single_sweeps : c->tm.redone_sweeps) += 1;
+    if (c->h_flags[5]) c->reused_sweeps += 1;
+  }
   if (c->h_flags[1] != 0) {
     balm_set_error(TC_TIMEOUT_MSG);
     return BALM_ERR_CUDA;

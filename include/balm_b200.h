@@ -536,6 +536,10 @@ int balm_comm_init(balm_ctx *ctx, int rank, int world, const void *unique_id128)
 
 /* Instrumentation */
 int balm_get_timings(balm_ctx *ctx, balm_timings *out);
+/* Tensor path, since balm_reset_counters(): re-evaluations after a rejected step (force_hess) that ran no observation
+ * sweep, because the digit planes and accumulators of the same poses and column scales were still in place. They are
+ * also counted in balm_timings.single_sweeps. */
+int balm_get_reused_sweeps(balm_ctx *ctx, int *out);
 int balm_reset_counters(balm_ctx *ctx);
 int balm_sync(balm_ctx *ctx);
 /* CUDA-event bracket on the ctx stream: begin records, end records + synchronises and returns elapsed ms. */
