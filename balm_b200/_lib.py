@@ -59,7 +59,8 @@ SYMBOLS = ["balm_last_error", "balm_version", "balm_create", "balm_destroy", "ba
            "balm_pose_graph_iter", "balm_spg_create", "balm_spg_destroy", "balm_spg_set_factors", "balm_spg_structure",
            "balm_spg_evaluate", "balm_spg_iter", "balm_spg_covariance", "balm_block_structure", "balm_download_blocks",
            "balm_block_covariance", "balm_block_set_factors", "balm_set_factor_loss", "balm_factor_residuals",
-           "balm_spg_set_factor_loss", "balm_spg_factor_residuals"]
+           "balm_spg_set_factor_loss", "balm_spg_factor_residuals", "balm_set_pose_priors", "balm_prior_residuals",
+           "balm_spg_set_pose_priors", "balm_spg_prior_residuals"]
 
 
 def lib():
@@ -158,6 +159,10 @@ def lib():
         L.balm_factor_residuals.argtypes = [C.c_void_p] + [C.c_void_p] * 3
         L.balm_spg_set_factor_loss.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
         L.balm_spg_factor_residuals.argtypes = [C.c_void_p] + [C.c_void_p] * 3
+        L.balm_set_pose_priors.argtypes = [C.c_void_p, C.c_int] + [C.c_void_p] * 7
+        L.balm_prior_residuals.argtypes = [C.c_void_p] + [C.c_void_p] * 3
+        L.balm_spg_set_pose_priors.argtypes = [C.c_void_p, C.c_int] + [C.c_void_p] * 7
+        L.balm_spg_prior_residuals.argtypes = [C.c_void_p] + [C.c_void_p] * 3
         _lib = L
     return _lib
 

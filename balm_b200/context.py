@@ -62,6 +62,38 @@ def _factor_residuals(fn, handle, n_factors, poses12):
     return s, w
 
 
+def _set_pose_priors(fn, handle, N, priors, kind, scale):
+    """Marshal absolute pose priors for balm_set_pose_priors / balm_spg_set_pose_priors -> per prior status. Each prior
+    is a dict pose, pose_hat (12), H (6 x 6), optional lever_arm (3); kind a loss name or one per prior, scale a scalar
+    or one per prior. [] detaches the set."""
+    n = len(priors)
+    if n == 0:
+        L.check(fn(handle, 0, None, None, None, None, None, None, None))
+        return []
+    pose = np.array([int(p["pose"]) for p in priors], dtype=np.int32)
+    hat = np.ascontiguousarray([np.asarray(p["pose_hat"], dtype=np.float64).reshape(12) for p in priors])
+    Hs = []
+    for p in priors:
+        H = np.asarray(p["H"], dtype=np.float64)
+        if H.shape != (6, 6):
+            raise ValueError(f"set_pose_priors: H must be 6 x 6, got {H.shape}")
+        Hs.append(H.ravel(order="F"))
+    H = np.ascontiguousarray(Hs)
+    lever = None
+    if any(p.get("lever_arm") is not None for p in priors):
+        lever = np.ascontiguousarray([np.zeros(3) if p.get("lever_arm") is None else
+                                      np.asarray(p["lever_arm"], dtype=np.float64).reshape(3) for p in priors])
+    kinds = [kind] * n if isinstance(kind, str) else list(kind)
+    if any(k not in _LOSS for k in kinds):
+        raise ValueError(f"set_pose_priors: kinds must be in {sorted(_LOSS)}, got {sorted(set(kinds) - set(_LOSS))}")
+    k = None if all(x == "trivial" for x in kinds) else np.array([_LOSS[x] for x in kinds], dtype=np.int32)
+    sc = None if k is None or scale is None else \
+        np.ascontiguousarray(np.broadcast_to(np.asarray(scale, dtype=np.float64), (n,)))
+    status = np.zeros(n, dtype=np.int32)
+    L.check(fn(handle, n, _p(pose), _p(hat), _p(lever), _p(H), _p(k), _p(sc), _p(status)))
+    return [int(s) for s in status]
+
+
 def _pose_graph_iter(fn, handle, N, poses12, max_iter, u0, v0, rel_tol, gauge_mode, verbose, want_per_iter, force_hess):
     """balm_pose_graph_iter / balm_spg_iter -> (poses, trace dicts)."""
     poses = np.array(poses12, dtype=np.float64, order="C", copy=True)
@@ -93,6 +125,7 @@ class Context:
         self.N = int(n_poses)
         self.n = 6 * self.N
         self._n_factors = 0  # the registered pose factor set's size
+        self._n_priors = 0   # the registered pose prior set's size
         L.check(L.lib().balm_create(C.byref(self._h), self.N, int(device), int(precision)))
 
     def close(self):
@@ -229,6 +262,22 @@ class Context:
         """-> (s, w): s_f = e~^T H~ e~ and w_f = rho'(s_f) of every registered factor at poses12 (0, 0 for a factor left
         out as ERR_NOT_PD; w = 1 without a loss)."""
         return _factor_residuals(L.lib().balm_factor_residuals, self._h, self._n_factors, poses12)
+
+    def set_pose_priors(self, priors, kind="trivial", scale=None):
+        """Absolute pose priors (include/balm_b200.h, balm_set_pose_priors): list of dict(pose, pose_hat (12), H (6 x 6,
+        (rotation, translation) order, positive semi-definite), optional lever_arm (3, body frame)), e.g. from
+        pose_priors / position_priors. Prior cost 1/2 rho(e^T H e) with e = (Log(R R^^T), R l + p - p^). They join the
+        pose-graph cost (pose_graph_evaluate / pose_graph_iter), and on PREC_BLOCKS contexts every evaluation over all
+        voxels, damping_iter and block_covariance. With an active prior pass gauge_mode=2 and use anchor=-1. kind / scale
+        as set_factor_loss'. [] detaches; the set survives factor and voxel registrations. -> per prior OK or ERR_NOT_PD
+        (left out of the cost)."""
+        status = _set_pose_priors(L.lib().balm_set_pose_priors, self._h, self.N, priors, kind, scale)
+        self._n_priors = len(status)
+        return status
+
+    def prior_residuals(self, poses12):
+        """-> (s, w): s_q = e^T H_q e and w_q = rho'(s_q) of every registered prior at poses12 (0, 0 for NOT_PD ones)."""
+        return _factor_residuals(L.lib().balm_prior_residuals, self._h, self._n_priors, poses12)
 
     def solve(self, u):
         dx = np.zeros(self.n)
@@ -663,6 +712,7 @@ class PoseGraph:
         self.N = int(n_poses)
         self.n = 6 * self.N
         self._n_factors = 0
+        self._n_priors = 0
         L.check(L.lib().balm_spg_create(C.byref(self._h), self.N, int(device)))
 
     def close(self):
@@ -689,6 +739,17 @@ class PoseGraph:
     def factor_residuals(self, poses12):
         """Context.factor_residuals on this handle's factors -> (s, w)."""
         return _factor_residuals(L.lib().balm_spg_factor_residuals, self._h, self._n_factors, poses12)
+
+    def set_pose_priors(self, priors, kind="trivial", scale=None):
+        """Context.set_pose_priors on this handle (evaluate, iterate and covariance include them). A prior on a pose
+        that no factor covers adds that pose's diagonal block to the pattern."""
+        status = _set_pose_priors(L.lib().balm_spg_set_pose_priors, self._h, self.N, priors, kind, scale)
+        self._n_priors = len(status)
+        return status
+
+    def prior_residuals(self, poses12):
+        """Context.prior_residuals on this handle's priors -> (s, w)."""
+        return _factor_residuals(L.lib().balm_spg_prior_residuals, self._h, self._n_priors, poses12)
 
     def structure(self):
         """-> dict(pairs, l_blocks, levels, device_bytes): nonzero block pairs of H, blocks of the factor L, levels of

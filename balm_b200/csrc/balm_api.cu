@@ -236,6 +236,7 @@ extern "C" int balm_destroy(balm_ctx *c) {
   free_problem(c);
   window_free(c->win);
   pose_graph_free(c->pg);
+  prior_set_free(c->pr);
   if (c->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(c->comm);
   if (c->prec == BALM_PREC_BLOCKS) cudaFree(c->g);
   cudaFree(c->poses); cudaFree(c->poses_trial); cudaFree(c->H); cudaFree(c->A);
@@ -584,6 +585,7 @@ static int evaluate_dev(balm_ctx *c, const double *poses, int64_t head, int64_t 
   const bool deferred = c->defer && head == 0 && end == c->M && c->VB >= c->M && end > head;
   // a blocks context's pose factors are part of every full-range evaluation (sub-ranges stay voxels only)
   const bool factors = c->prec == BALM_PREC_BLOCKS && c->pg && head == 0 && end == c->M;
+  const bool priors = c->prec == BALM_PREC_BLOCKS && c->pr && head == 0 && end == c->M;  // so are its pose priors
   c->pending_stats_cached = stats_cached;
   if (head == end) {  // empty range (or an empty shard): this rank contributes H = 0, g = 0, r = 0 -- and still enters
     // the all-reduce below, which the other ranks of a multi-GPU job are waiting in
@@ -624,10 +626,11 @@ static int evaluate_dev(balm_ctx *c, const double *poses, int64_t head, int64_t 
     first = false;
   }
   CUDA_TRY(cudaMemcpyAsync(c->scal + BALM_SCAL_RCUR, r_dev, sizeof(double), cudaMemcpyDeviceToDevice, c->stream));  // local, pre all-reduce
-  if (end > head || factors) {
+  if (end > head || factors || priors) {
     CUDA_TRY(cudaEventRecord(c->ev[4], c->stream));
     if (c->prec != BALM_PREC_BLOCKS) TRY(launch_assemble(c));
     if (factors) TRY(blocks_add_factors(c, poses));  // after the RCUR copy above: the hand-over caches voxels only
+    if (priors) TRY(blocks_add_priors(c, poses));
     CUDA_TRY(cudaEventRecord(c->ev[5], c->stream));
   }
   if (c->world > 1 && c->comm) {  // the assembly wrote the lower triangle | g into c->Hpack (an empty range: zeros)
@@ -647,7 +650,7 @@ static int evaluate_dev(balm_ctx *c, const double *poses, int64_t head, int64_t 
   }
   CUDA_TRY(cudaEventSynchronize(c->ev[6]));
   cudaEventElapsedTime(&ms, c->ev[4], c->ev[5]);
-  if (c->prec != BALM_PREC_BLOCKS || factors) c->tm.ms_assemble += ms;
+  if (c->prec != BALM_PREC_BLOCKS || factors || priors) c->tm.ms_assemble += ms;
   cudaEventElapsedTime(&ms, c->ev[5], c->ev[6]); c->tm.ms_allreduce += ms;
   c->tm.n_eval += 1;
   return BALM_OK;
@@ -663,7 +666,7 @@ static int collect_eval(balm_ctx *c) {
   cudaEventElapsedTime(&ms, c->ev[1], c->ev[2]); c->tm.ms_obs += ms;
   cudaEventElapsedTime(&ms, c->ev[2], c->ev[3]); c->tm.ms_syrk += ms;
   cudaEventElapsedTime(&ms, c->ev[4], c->ev[5]);
-  if (c->prec != BALM_PREC_BLOCKS || c->pg) c->tm.ms_assemble += ms;  // deferred: always full range
+  if (c->prec != BALM_PREC_BLOCKS || c->pg || c->pr) c->tm.ms_assemble += ms;  // deferred: always full range
   cudaEventElapsedTime(&ms, c->ev[5], c->ev[6]); c->tm.ms_allreduce += ms;
   c->tm.n_eval += 1;
   if (c->prec == BALM_PREC_TENSOR) return tensor_syrk_check_finish(c);
@@ -678,6 +681,7 @@ static int residual_dev(balm_ctx *c, const double *poses, double *host_out, bool
   TRY(launch_voxel_stats(c, poses, 0, c->M, keep_stats ? c->stats_trial : nullptr, true, r_dev));
   CUDA_TRY(cudaMemcpyAsync(c->scal + BALM_SCAL_RTRIAL, r_dev, sizeof(double), cudaMemcpyDeviceToDevice, c->stream));  // local, pre all-reduce
   if (c->prec == BALM_PREC_BLOCKS && c->pg) TRY(blocks_add_factor_cost(c, poses, r_dev));  // after RTRIAL: voxels only
+  if (c->prec == BALM_PREC_BLOCKS && c->pr) TRY(prior_add_cost(c->pr, c->stream, poses, r_dev, &c->launches));
   TRY(allreduce_sum(c, r_dev, 1));
   CUDA_TRY(cudaEventRecord(c->ev[8], c->stream));
   CUDA_TRY(cudaMemcpyAsync(c->h_scal + 2, r_dev, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
@@ -813,12 +817,22 @@ static bool lm_rule(const balm_lm_opts *o, int it, double r1, double r2, double 
   return false;
 }
 
+// With an active absolute pose prior the cost has no gauge freedom: re-anchoring to pose 0 would move the result off
+// the priors.
+static int refuse_gauge_with_priors(const char *who, const PriorSet *pr, const balm_lm_opts *o) {
+  if (!prior_set_active(pr) || (o->gauge_mode != 0 && o->gauge_mode != 1)) return BALM_OK;
+  balm_set_error(std::string(who) + ": gauge_mode " + std::to_string(o->gauge_mode) +
+                 " re-anchors to pose 0, which moves the result off the pose priors; pass gauge_mode 2");
+  return BALM_ERR_INVALID;
+}
+
 extern "C" int balm_damping_iter(balm_ctx *c, double *poses12, const balm_lm_opts *o, balm_trace *trace, int *n_iters,
                                  double *poses_per_iter) {
   if (!c || !poses12 || !o) { balm_set_error("balm_damping_iter: bad arguments"); return BALM_ERR_INVALID; }
   CUDA_TRY(cudaSetDevice(c->device));
   if (n_iters) *n_iters = 0;
   if (!c->registered) { balm_set_error("no voxels registered"); return BALM_ERR_INVALID; }
+  if (c->prec == BALM_PREC_BLOCKS) TRY(refuse_gauge_with_priors("balm_damping_iter", c->pr, o));
   if (o->min_planes_per_pose > 0) {  // bavoxel.hpp:1071-1085 (the shim reproduces the printf + exit(0))
     // The guard is on the GLOBAL count of voxels seeing each pose. With several ranks every rank all-reduces the
     // per-pose histogram of its shard first, so all ranks take the same branch (a rank returning alone would leave
@@ -1047,6 +1061,7 @@ struct PoseGraphLm {
   double **poses, **poses_trial;  // the owner's [12N] buffers, swapped on acceptance
   double *dx, *scal, *h_scal;     // scal: device [32] (3 u, 4..15 gauge snapshot), h_scal: pinned host [16]
   long long *launches;
+  const PriorSet *pr = nullptr;   // the owner's pose priors (their cost joins the trial cost)
   std::function<int(const double *poses)> eval;
   std::function<int(double u)> solve;
   std::function<int(double *q1, int *not_pd, int *refined)> finish;
@@ -1055,6 +1070,7 @@ struct PoseGraphLm {
 // the pose-graph cost at the trial poses -> *r2 (waits for the stream)
 static int pose_graph_trial_cost(const PoseGraphLm &s, double *r2) {
   TRY(pose_graph_cost(s.pg, s.st, *s.poses_trial, s.scal + 2, s.launches));
+  if (s.pr) TRY(prior_add_cost(s.pr, s.st, *s.poses_trial, s.scal + 2, s.launches));
   CUDA_TRY(cudaMemcpyAsync(s.h_scal + 2, s.scal + 2, sizeof(double), cudaMemcpyDeviceToHost, s.st));
   CUDA_TRY(cudaStreamSynchronize(s.st));
   *r2 = s.h_scal[2];
@@ -1122,8 +1138,10 @@ extern "C" int balm_pose_graph_iter(balm_ctx *c, double *poses12, const balm_lm_
   if (n_iters) *n_iters = 0;
   if (c->world > 1 || c->comm) { balm_set_error("balm_pose_graph_iter: single-GPU contexts only"); return BALM_ERR_INVALID; }
   if (!c->pg) { balm_set_error("balm_pose_graph_iter: no pose factors registered"); return BALM_ERR_INVALID; }
+  TRY(refuse_gauge_with_priors("balm_pose_graph_iter", c->pr, o));
   CUDA_TRY(cudaSetDevice(c->device));
   PoseGraphLm s{c->stream, c->N, c->pg, &c->poses, &c->poses_trial, c->dx, c->scal, c->h_scal, &c->launches};
+  s.pr = c->pr;
   s.eval = [c](const double *poses) -> int { return pose_graph_eval(c, poses); };
   s.solve = [c](double u) -> int {  // deferred: q1 and the flags are read by finish()
     double q1 = 0;
@@ -1145,8 +1163,13 @@ struct balm_spg {
   int N = 0, device = 0;
   cudaStream_t stream = nullptr;
   PoseGraph *pg = nullptr;          // the registered factors (null before the first registration)
+  PriorSet *pr = nullptr;           // the registered pose priors (null: none)
   SparseSolver *solver = nullptr;   // their ordering, symbolic factorisation and captured solve
   double *blocks = nullptr;         // [pairs][36] H
+  // Only while a prior sits on a pose that no active factor covers: the pattern is the factor pairs united with those
+  // poses' diagonal pairs (upairs), and the factor sums go to blocks[fmap[p]]; otherwise the pattern is the factors'.
+  std::vector<int2> upairs;
+  int *fmap = nullptr;
   double *poses = nullptr, *poses_trial = nullptr;  // [12N]
   double *g = nullptr, *dx = nullptr, *dvec = nullptr;  // [6N]
   double *scal = nullptr;           // device scalars [32], laid out as balm_ctx::scal
@@ -1157,6 +1180,8 @@ struct balm_spg {
   ~balm_spg() {
     sparse_solver_free(solver);
     pose_graph_free(pg);
+    prior_set_free(pr);
+    cudaFree(fmap);
     cudaFree(blocks); cudaFree(poses); cudaFree(poses_trial); cudaFree(g); cudaFree(dx); cudaFree(dvec); cudaFree(scal);
     cudaFree(flags);
     cudaFreeHost(h_scal);
@@ -1197,6 +1222,67 @@ extern "C" void balm_spg_destroy(balm_spg *s) {
   delete s;
 }
 
+// A sparse pose graph's block pattern for the factor set pg and the priors pr (either may hold nothing active): the
+// factor pairs, united with the diagonal pair of every pose with an active prior that no factor pair covers. Only such
+// a pose makes the union differ from the factor pattern (grown). Blocks and solver are built here; commit() hands them
+// to the handle.
+struct SpgPattern {
+  bool grown = false;
+  std::vector<int2> upairs;
+  int *fmap = nullptr;
+  double *blocks = nullptr;
+  SparseSolver *solver = nullptr;
+  ~SpgPattern() { sparse_solver_free(solver); cudaFree(fmap); cudaFree(blocks); }
+  const std::vector<int2> &pairs(const PoseGraph *pg) const { return grown ? upairs : pose_graph_pairs(pg); }
+  void commit(balm_spg *s) {
+    sparse_solver_free(s->solver);
+    cudaFree(s->fmap);
+    cudaFree(s->blocks);
+    s->solver = solver;
+    s->fmap = fmap;
+    s->blocks = blocks;
+    s->upairs = std::move(upairs);
+    solver = nullptr;
+    fmap = nullptr;
+    blocks = nullptr;
+  }
+};
+
+static bool pair_less(const int2 &a, const int2 &b) { return a.x < b.x || (a.x == b.x && a.y < b.y); }
+
+// the union's pairs only (no device work): false when the factor pattern already holds every prior pose's diagonal
+static bool spg_union(const PoseGraph *pg, const PriorSet *pr, std::vector<int2> *up, std::vector<int> *fmap) {
+  const std::vector<int2> &fp = pose_graph_pairs(pg);
+  std::vector<int2> extra;
+  if (prior_set_active(pr))
+    for (int i : prior_set_poses(pr))
+      if (!std::binary_search(fp.begin(), fp.end(), make_int2(i, i), pair_less)) extra.push_back(make_int2(i, i));
+  if (extra.empty()) return false;
+  up->resize(fp.size() + extra.size());
+  std::merge(fp.begin(), fp.end(), extra.begin(), extra.end(), up->begin(), pair_less);
+  fmap->resize(fp.size());
+  for (size_t p = 0, q = 0; p < fp.size(); p++) {
+    while ((*up)[q].x != fp[p].x || (*up)[q].y != fp[p].y) q++;
+    (*fmap)[p] = (int)q++;
+  }
+  return true;
+}
+
+static int spg_pattern(balm_spg *s, const PoseGraph *pg, const PriorSet *pr, const char *who, SpgPattern *out) {
+  std::vector<int> fmap;
+  out->grown = spg_union(pg, pr, &out->upairs, &fmap);
+  const std::vector<int2> &pairs = out->pairs(pg);
+  TRY(dev_alloc(&out->blocks, 36 * pairs.size()));
+  if (out->grown) {
+    TRY(dev_alloc(&out->fmap, fmap.size()));
+    CUDA_TRY(cudaMemcpyAsync(out->fmap, fmap.data(), sizeof(int) * fmap.size(), cudaMemcpyHostToDevice, s->stream));
+  }
+  TRY(sparse_solver_build(s->stream, s->N, pairs, out->blocks, s->g, s->dvec, s->dx, s->scal, s->flags, who,
+                          &out->solver));
+  CUDA_TRY(cudaStreamSynchronize(s->stream));
+  return BALM_OK;
+}
+
 extern "C" int balm_spg_set_factors(balm_spg *s, int n_factors, const int64_t *factor_ptr, const int32_t *factor_pose,
                                     const double *poses_hat12, const double *H, int32_t *status_out) {
   if (!s) { balm_set_error("balm_spg_set_factors: bad arguments"); return BALM_ERR_INVALID; }
@@ -1206,31 +1292,40 @@ extern "C" int balm_spg_set_factors(balm_spg *s, int n_factors, const int64_t *f
   std::vector<int> status;
   TRY(pose_graph_build(s->stream, s->N, n_factors, factor_ptr, factor_pose, poses_hat12, H, &status, &pg, &s->launches));
   std::unique_ptr<PoseGraph, void (*)(PoseGraph *)> pg_own(pg, pose_graph_free);
-  const std::vector<int2> &pairs = pose_graph_pairs(pg);
-  double *blocks = nullptr;
-  TRY(dev_alloc(&blocks, 36 * pairs.size()));
-  std::unique_ptr<double, cudaError_t (*)(void *)> blocks_own(blocks, cudaFree);
-  SparseSolver *solver = nullptr;
-  TRY(sparse_solver_build(s->stream, s->N, pairs, blocks, s->g, s->dvec, s->dx, s->scal, s->flags, "balm_spg_set_factors",
-                          &solver));
+  SpgPattern pat;
+  TRY(spg_pattern(s, pg, s->pr, "balm_spg_set_factors", &pat));
+  if (s->pr) TRY(prior_set_map(s->pr, s->stream, pat.pairs(pg)));
   if (status_out) std::copy(status.begin(), status.end(), status_out);
-  sparse_solver_free(s->solver);
+  pat.commit(s);
   pose_graph_free(s->pg);
-  cudaFree(s->blocks);
-  s->solver = solver;
   s->pg = pg_own.release();
-  s->blocks = blocks_own.release();
   return BALM_OK;
 }
+
+// H, g and the cost of the factors and then the priors at the device poses into s->blocks, s->g, s->scal[0] (enqueued)
+static int spg_eval(balm_spg *s, const double *poses) {
+  if (s->fmap) {
+    CUDA_TRY(cudaMemsetAsync(s->blocks, 0, sizeof(double) * 36 * s->upairs.size(), s->stream));
+    TRY(pose_graph_add_blocks(s->pg, s->stream, poses, s->blocks, s->fmap, s->g, s->scal, &s->launches));
+  } else {
+    TRY(pose_graph_eval_blocks(s->pg, s->stream, poses, s->blocks, s->g, s->scal, &s->launches));
+  }
+  if (s->pr) TRY(prior_add_blocks(s->pr, s->stream, poses, s->blocks, s->g, s->scal, &s->launches));
+  return BALM_OK;
+}
+
+static const std::vector<int2> &spg_pairs(const balm_spg *s) { return s->fmap ? s->upairs : pose_graph_pairs(s->pg); }
 
 extern "C" int balm_spg_structure(balm_spg *s, int64_t stats[4], int32_t *pairs) {
   if (!s || !stats) { balm_set_error("balm_spg_structure: bad arguments"); return BALM_ERR_INVALID; }
   if (!s->pg) { balm_set_error("balm_spg_structure: no pose factors registered"); return BALM_ERR_INVALID; }
-  const std::vector<int2> &pr = pose_graph_pairs(s->pg);
+  const std::vector<int2> &pr = spg_pairs(s);
   stats[0] = (int64_t)pr.size();
   sparse_solver_stats(s->solver, &stats[1], &stats[2], &stats[3]);
   stats[3] += (int64_t)(sizeof(double) * (36 * pr.size() + 2 * 12 * (size_t)s->N + 3 * 6 * (size_t)s->N + 32) +
                         sizeof(int) * 8) + pose_graph_bytes(s->pg);
+  if (s->fmap) stats[3] += (int64_t)(sizeof(int) * pose_graph_pairs(s->pg).size());
+  if (s->pr) stats[3] += prior_set_bytes(s->pr);
   if (pairs)
     for (size_t p = 0; p < pr.size(); p++) { pairs[2 * p] = pr[p].x; pairs[2 * p + 1] = pr[p].y; }
   return BALM_OK;
@@ -1241,8 +1336,8 @@ extern "C" int balm_spg_evaluate(balm_spg *s, const double *poses12, double *blo
   if (!s->pg) { balm_set_error("balm_spg_evaluate: no pose factors registered"); return BALM_ERR_INVALID; }
   CUDA_TRY(cudaSetDevice(s->device));
   CUDA_TRY(cudaMemcpyAsync(s->poses, poses12, sizeof(double) * 12 * s->N, cudaMemcpyHostToDevice, s->stream));
-  TRY(pose_graph_eval_blocks(s->pg, s->stream, s->poses, s->blocks, s->g, s->scal, &s->launches));
-  const size_t nbl = 36 * pose_graph_pairs(s->pg).size();
+  TRY(spg_eval(s, s->poses));
+  const size_t nbl = 36 * spg_pairs(s).size();
   if (blocks && nbl) CUDA_TRY(cudaMemcpyAsync(blocks, s->blocks, sizeof(double) * nbl, cudaMemcpyDeviceToHost, s->stream));
   if (g) CUDA_TRY(cudaMemcpyAsync(g, s->g, sizeof(double) * 6 * s->N, cudaMemcpyDeviceToHost, s->stream));
   CUDA_TRY(cudaMemcpyAsync(s->h_scal, s->scal, sizeof(double), cudaMemcpyDeviceToHost, s->stream));
@@ -1256,11 +1351,11 @@ extern "C" int balm_spg_iter(balm_spg *sp, double *poses12, const balm_lm_opts *
   if (!sp || !poses12 || !o) { balm_set_error("balm_spg_iter: bad arguments"); return BALM_ERR_INVALID; }
   if (n_iters) *n_iters = 0;
   if (!sp->pg) { balm_set_error("balm_spg_iter: no pose factors registered"); return BALM_ERR_INVALID; }
+  TRY(refuse_gauge_with_priors("balm_spg_iter", sp->pr, o));
   CUDA_TRY(cudaSetDevice(sp->device));
   PoseGraphLm s{sp->stream, sp->N, sp->pg, &sp->poses, &sp->poses_trial, sp->dx, sp->scal, sp->h_scal, &sp->launches};
-  s.eval = [sp](const double *poses) -> int {
-    return pose_graph_eval_blocks(sp->pg, sp->stream, poses, sp->blocks, sp->g, sp->scal, &sp->launches);
-  };
+  s.pr = sp->pr;
+  s.eval = [sp](const double *poses) -> int { return spg_eval(sp, poses); };
   s.solve = [sp](double u) -> int {
     sp->h_scal[3] = u;  // pinned; the kernels read the damping factor from device memory
     CUDA_TRY(cudaMemcpyAsync(sp->scal + 3, sp->h_scal + 3, sizeof(double), cudaMemcpyHostToDevice, sp->stream));
@@ -1292,7 +1387,7 @@ extern "C" int balm_spg_covariance(balm_spg *s, const double *poses12, int ancho
   CUDA_TRY(cudaSetDevice(s->device));
   return sparse_covariance(s->solver, s->stream, anchor, [&]() -> int {
     CUDA_TRY(cudaMemcpyAsync(s->poses, poses12, sizeof(double) * 12 * s->N, cudaMemcpyHostToDevice, s->stream));
-    return pose_graph_eval_blocks(s->pg, s->stream, s->poses, s->blocks, s->g, s->scal, &s->launches);
+    return spg_eval(s, s->poses);
   }, "balm_spg_covariance", cov, &s->launches);
 }
 
@@ -1308,6 +1403,106 @@ extern "C" int balm_spg_factor_residuals(balm_spg *s, const double *poses12, dou
   CUDA_TRY(cudaSetDevice(s->device));
   CUDA_TRY(cudaMemcpyAsync(s->poses, poses12, sizeof(double) * 12 * s->N, cudaMemcpyHostToDevice, s->stream));
   return pose_graph_residuals(s->pg, s->stream, s->poses, sf, w, &s->launches);
+}
+
+// ---------------- absolute pose priors (pose_graph.cu) ----------------
+// The argument checks of balm_set_pose_priors and balm_spg_set_pose_priors over P poses (n_priors >= 1)
+static int pose_priors_check(const char *who, int P, int n, const int32_t *pose, const double *hat12,
+                             const double *lever3, const double *H36, const int32_t *kind, const double *scale) {
+  const std::string w = std::string(who) + ": ";
+  if (n < 0 || (n > 0 && (!pose || !hat12 || !H36))) { balm_set_error(w + "bad arguments"); return BALM_ERR_INVALID; }
+  for (int q = 0; q < n; q++) {
+    const std::string pq = w + "prior " + std::to_string(q);
+    if (pose[q] < 0 || pose[q] >= P) { balm_set_error(pq + " names a pose outside [0, n_poses)"); return BALM_ERR_INVALID; }
+    bool finite = true;
+    for (int e = 0; e < 12; e++) finite = finite && std::isfinite(hat12[12 * (size_t)q + e]);
+    for (int e = 0; lever3 && e < 3; e++) finite = finite && std::isfinite(lever3[3 * (size_t)q + e]);
+    const double *Hq = H36 + 36 * (size_t)q;
+    double hmax = 0.0;
+    for (int e = 0; e < 36; e++) { finite = finite && std::isfinite(Hq[e]); hmax = std::max(hmax, fabs(Hq[e])); }
+    if (!finite) { balm_set_error(pq + " has a non-finite pose_hat, lever arm or H"); return BALM_ERR_INVALID; }
+    for (int a = 0; a < 6; a++)
+      for (int c = 0; c < a; c++)
+        if (fabs(Hq[6 * c + a] - Hq[6 * a + c]) > 1e-12 * hmax) {
+          balm_set_error(pq + " has an H that is not symmetric");
+          return BALM_ERR_INVALID;
+        }
+    if (kind && kind[q] != BALM_LOSS_TRIVIAL && kind[q] != BALM_LOSS_HUBER && kind[q] != BALM_LOSS_CAUCHY) {
+      balm_set_error(pq + " has loss kind " + std::to_string(kind[q]) + " (0, 1, 2 allowed)");
+      return BALM_ERR_INVALID;
+    }
+    if (kind && kind[q] != BALM_LOSS_TRIVIAL && !(scale && std::isfinite(scale[q]) && scale[q] > 0.0)) {
+      balm_set_error(pq + " needs a finite scale > 0");
+      return BALM_ERR_INVALID;
+    }
+  }
+  return BALM_OK;
+}
+
+extern "C" int balm_set_pose_priors(balm_ctx *c, int n_priors, const int32_t *pose, const double *poses_hat12,
+                                    const double *lever3, const double *H36, const int32_t *kind, const double *scale,
+                                    int32_t *status_out) {
+  const char *who = "balm_set_pose_priors";
+  if (!c) { balm_set_error(std::string(who) + ": bad arguments"); return BALM_ERR_INVALID; }
+  TRY(pose_priors_check(who, c->N, n_priors, pose, poses_hat12, lever3, H36, kind, scale));
+  CUDA_TRY(cudaSetDevice(c->device));
+  PriorSet *pr = nullptr;
+  std::vector<int> status;
+  if (n_priors > 0)  // 0 detaches the prior set
+    TRY(prior_set_build(c->stream, n_priors, pose, poses_hat12, lever3, H36, kind, scale, &status, &pr));
+  std::unique_ptr<PriorSet, void (*)(PriorSet *)> pr_own(pr, prior_set_free);
+  if (pr && c->prec == BALM_PREC_BLOCKS && c->bh) TRY(prior_set_map(pr, c->stream, blocks_pairs(c->bh)));
+  if (status_out) std::copy(status.begin(), status.end(), status_out);
+  prior_set_free(c->pr);
+  c->pr = pr_own.release();
+  return BALM_OK;
+}
+
+extern "C" int balm_prior_residuals(balm_ctx *c, const double *poses12, double *s, double *w) {
+  if (!c || !poses12) { balm_set_error("balm_prior_residuals: bad arguments"); return BALM_ERR_INVALID; }
+  if (!c->pr) { balm_set_error("balm_prior_residuals: no pose priors registered"); return BALM_ERR_INVALID; }
+  CUDA_TRY(cudaSetDevice(c->device));
+  CUDA_TRY(cudaMemcpyAsync(c->poses, poses12, sizeof(double) * 12 * c->N, cudaMemcpyHostToDevice, c->stream));
+  return prior_residuals(c->pr, c->stream, c->poses, s, w, &c->launches);
+}
+
+extern "C" int balm_spg_set_pose_priors(balm_spg *s, int n_priors, const int32_t *pose, const double *poses_hat12,
+                                        const double *lever3, const double *H36, const int32_t *kind,
+                                        const double *scale, int32_t *status_out) {
+  const char *who = "balm_spg_set_pose_priors";
+  if (!s) { balm_set_error(std::string(who) + ": bad arguments"); return BALM_ERR_INVALID; }
+  TRY(pose_priors_check(who, s->N, n_priors, pose, poses_hat12, lever3, H36, kind, scale));
+  CUDA_TRY(cudaSetDevice(s->device));
+  PriorSet *pr = nullptr;
+  std::vector<int> status;
+  if (n_priors > 0)  // 0 detaches the prior set
+    TRY(prior_set_build(s->stream, n_priors, pose, poses_hat12, lever3, H36, kind, scale, &status, &pr));
+  std::unique_ptr<PriorSet, void (*)(PriorSet *)> pr_own(pr, prior_set_free);
+  if (s->pg) {  // the pattern is rebuilt only when its union with the priors' diagonal pairs changes
+    std::vector<int2> up;
+    std::vector<int> fmap;
+    const bool grown = spg_union(s->pg, pr, &up, &fmap);
+    const bool same = grown ? (s->fmap && up.size() == s->upairs.size() &&
+                               std::equal(up.begin(), up.end(), s->upairs.begin(),
+                                          [](const int2 &a, const int2 &b) { return a.x == b.x && a.y == b.y; }))
+                            : !s->fmap;
+    SpgPattern pat;
+    if (!same) TRY(spg_pattern(s, s->pg, pr, who, &pat));
+    if (pr) TRY(prior_set_map(pr, s->stream, same ? spg_pairs(s) : pat.pairs(s->pg)));
+    if (!same) pat.commit(s);
+  }
+  if (status_out) std::copy(status.begin(), status.end(), status_out);
+  prior_set_free(s->pr);
+  s->pr = pr_own.release();
+  return BALM_OK;
+}
+
+extern "C" int balm_spg_prior_residuals(balm_spg *s, const double *poses12, double *sp, double *w) {
+  if (!s || !poses12) { balm_set_error("balm_spg_prior_residuals: bad arguments"); return BALM_ERR_INVALID; }
+  if (!s->pr) { balm_set_error("balm_spg_prior_residuals: no pose priors registered"); return BALM_ERR_INVALID; }
+  CUDA_TRY(cudaSetDevice(s->device));
+  CUDA_TRY(cudaMemcpyAsync(s->poses, poses12, sizeof(double) * 12 * s->N, cudaMemcpyHostToDevice, s->stream));
+  return prior_residuals(s->pr, s->stream, s->poses, sp, w, &s->launches);
 }
 
 // ---------------- sliding window on the registered voxel set (assoc.cu) ----------------
@@ -1594,7 +1789,7 @@ extern "C" int balm_block_structure(balm_ctx *c, int64_t stats[4], int32_t *pair
                      (size_t)(c->obs_chunks + 2) * BALM_ACC * c->Np + 24 * N + 3 * n + 8 + 32 + c->res_blocks;
   const size_t ints = K + (M + 1) * 2 + 2 * N + 8 + (c->csc_ptr ? 2 * K + 3 * N + 1 : 0);
   stats[3] = blocks_bytes(c->bh, &stats[1], &stats[2]) + (int64_t)(sizeof(double) * dbl + sizeof(int) * ints) +
-             (c->pg ? pose_graph_bytes(c->pg) : 0);
+             (c->pg ? pose_graph_bytes(c->pg) : 0) + (c->pr ? prior_set_bytes(c->pr) : 0);
   if (pairs)
     for (size_t p = 0; p < pr.size(); p++) { pairs[2 * p] = pr[p].x; pairs[2 * p + 1] = pr[p].y; }
   return BALM_OK;

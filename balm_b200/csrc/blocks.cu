@@ -13,6 +13,8 @@
 //   the voxel pairs, the active factors' pairs and the diagonal (block_pattern_build, rebuilt without re-sorting the
 //   voxel terms when only the factors change); a full-range evaluation adds the factor sums of pose_graph.cu onto the
 //   voxel blocks, g and residual, each entry once, in that order.
+//   Absolute pose priors (balm_set_pose_priors, DESIGN.md "Absolute pose priors"): they touch only diagonal blocks, which
+//   the union always holds, so they change no pattern; a full-range evaluation adds their sums after the factors'.
 #include <cub/cub.cuh>
 #include <algorithm>
 #include <memory>
@@ -265,6 +267,7 @@ int block_hessian_build(balm_ctx *c, const char *who) {
     pool.release(bh->term);
   }
   TRY(block_pattern_build(c, *bh, c->pg, who, &bh->pat));
+  if (c->pr) TRY(prior_set_map(c->pr, st, bh->pat->pairs));
   block_hessian_free(c->bh);
   c->bh = bh.release();
   return BALM_OK;
@@ -273,8 +276,18 @@ int block_hessian_build(balm_ctx *c, const char *who) {
 int blocks_repattern(balm_ctx *c, const PoseGraph *pg, const char *who) {
   std::unique_ptr<BlockPattern> pat;
   TRY(block_pattern_build(c, *c->bh, pg, who, &pat));
+  if (c->pr) TRY(prior_set_map(c->pr, c->stream, pat->pairs));
   c->bh->pat = std::move(pat);
   return BALM_OK;
+}
+
+int blocks_map_priors(balm_ctx *c) {
+  if (!c->pr || !c->bh) return BALM_OK;
+  return prior_set_map(c->pr, c->stream, c->bh->pat->pairs);
+}
+
+int blocks_add_priors(balm_ctx *c, const double *poses) {
+  return prior_add_blocks(c->pr, c->stream, poses, c->bh->pat->blocks, c->g, c->g + c->n, &c->launches);
 }
 
 int launch_blocks(balm_ctx *c, int64_t head, int64_t end) {
@@ -292,7 +305,7 @@ int launch_blocks(balm_ctx *c, int64_t head, int64_t end) {
 
 int blocks_add_factors(balm_ctx *c, const double *poses) {
   const BlockPattern &u = *c->bh->pat;
-  TRY(pose_graph_add_blocks(c->pg, c->stream, poses, u.blocks, u.fmap, u.fgc, &c->launches));
+  TRY(pose_graph_add_blocks(c->pg, c->stream, poses, u.blocks, u.fmap, u.fgc, u.fgc + c->n, &c->launches));
   add_kernel<<<(unsigned)((c->n + 1 + 255) / 256), 256, 0, c->stream>>>(u.fgc, c->n + 1, c->g);  // g, then r = g[n]
   c->launches += 1;
   CUDA_TRY(cudaGetLastError());

@@ -34,6 +34,8 @@ struct PoseGraph;    // the registered window factors (pose_graph.cu)
 void pose_graph_free(PoseGraph *p);
 struct BlockHessian;  // the block pattern of a BALM_PREC_BLOCKS context (blocks.cu)
 void block_hessian_free(BlockHessian *b);
+struct PriorSet;      // the registered absolute pose priors (pose_graph.cu)
+void prior_set_free(PriorSet *p);
 
 #define CUDA_TRY(expr)                                                                        \
   do {                                                                                        \
@@ -119,6 +121,8 @@ struct balm_ctx {
   PoseGraph *pg = nullptr;        // balm_set_pose_factors' window factors (independent of the registered voxel set);
                                   // BALM_PREC_BLOCKS: balm_block_set_factors' factors, part of the cost
   BlockHessian *bh = nullptr;     // BALM_PREC_BLOCKS: the registered set's block pattern, terms, blocks and solver
+  PriorSet *pr = nullptr;         // balm_set_pose_priors' priors (independent of the factor and the voxel set): part of
+                                  // the pose-graph cost, and on BALM_PREC_BLOCKS of every full-range evaluation
 
   // ---- optimiser state (device) ----
   double *poses = nullptr, *poses_trial = nullptr;  // [12N]
@@ -767,10 +771,10 @@ int pose_graph_eval(balm_ctx *c, const double *poses);
 // the same sums with one 6x6 block per pair (column-major, in pose_graph_pairs order) instead of dense H (enqueued)
 int pose_graph_eval_blocks(const PoseGraph *p, cudaStream_t st, const double *poses, double *blocks, double *g,
                            double *cost, long long *launches);
-// A blocks context's factor term (enqueued): pair p's sum added onto blocks[map[p]], the factor g into g_cost[0 .. 6P)
-// and the cost into g_cost[6P]
+// The factor term on a larger block pattern (enqueued): pair p's sum added onto blocks[map[p]], the factor g into
+// g [6P] and the cost into *cost
 int pose_graph_add_blocks(const PoseGraph *p, cudaStream_t st, const double *poses, double *blocks, const int *map,
-                          double *g_cost, long long *launches);
+                          double *g, double *cost, long long *launches);
 // the cost at the device poses into the device scalar *out (enqueued, no wait)
 int pose_graph_cost(const PoseGraph *p, cudaStream_t st, const double *poses, double *out, long long *launches);
 // the (i, j), i <= j, of every nonzero 6x6 block pair of H, ascending in (i, j)
@@ -784,6 +788,32 @@ int pose_graph_set_loss(PoseGraph *p, cudaStream_t st, const int32_t *kind, cons
 // arrays s and w [F] (either may be null); enqueues the cost pass and waits once
 int pose_graph_residuals(const PoseGraph *p, cudaStream_t st, const double *poses, double *s, double *w,
                          long long *launches);
+
+// ---------------- absolute pose priors (pose_graph.cu) ----------------
+// After the argument checks: uploads n priors (pose [n], hat12 [12n], lever3 [3n] or null, H36 [36n] column-major,
+// kind [n] or null, scale [n]), decides each prior's status (BALM_OK, or BALM_ERR_NOT_PD when H has an eigenvalue below
+// -1e-12 lambda_max or is zero; such a prior is in no sum) and builds the assembly tables -> a new set in *out (waits)
+int prior_set_build(cudaStream_t st, int n, const int32_t *pose, const double *hat12, const double *lever3,
+                    const double *H36, const int32_t *kind, const double *scale, std::vector<int> *status,
+                    PriorSet **out);
+// the index in `pairs` (ascending (i, j)) of the diagonal block of every pose with an active prior (waits)
+int prior_set_map(PriorSet *p, cudaStream_t st, const std::vector<int2> &pairs);
+// an active prior exists (p may be null)
+bool prior_set_active(const PriorSet *p);
+// the poses with active priors, ascending
+const std::vector<int> &prior_set_poses(const PriorSet *p);
+long long prior_set_bytes(const PriorSet *p);
+// the priors' H and g at the device poses added onto the dense H (n x n) / onto the diagonal blocks of the mapped
+// pattern, and onto g; their cost added onto *cost (enqueued)
+int prior_add_dense(const PriorSet *p, cudaStream_t st, const double *poses, double *H, size_t n, double *g,
+                    double *cost, long long *launches);
+int prior_add_blocks(const PriorSet *p, cudaStream_t st, const double *poses, double *blocks, double *g, double *cost,
+                     long long *launches);
+// the priors' cost at the device poses added onto the device scalar *cost (enqueued)
+int prior_add_cost(const PriorSet *p, cudaStream_t st, const double *poses, double *cost, long long *launches);
+// balm_prior_residuals: s and rho'(s) of every prior (0 for NOT_PD ones) into the host arrays s, w [n] (either may be
+// null); waits once
+int prior_residuals(const PriorSet *p, cudaStream_t st, const double *poses, double *s, double *w, long long *launches);
 
 // ---------------- sparse pose graph (pose_graph_sparse.cu) ----------------
 struct SparseSolver;  // nested-dissection ordering, symbolic factorisation and the per-solve CUDA graph
@@ -821,6 +851,11 @@ int blocks_repattern(balm_ctx *c, const PoseGraph *pg, const char *who);
 int blocks_add_factors(balm_ctx *c, const double *poses);
 // c->pg's cost at poses added onto the device scalar *r (enqueued)
 int blocks_add_factor_cost(balm_ctx *c, const double *poses, double *r);
+// c->pr's blocks, g and cost at poses added onto the evaluated blocks (after the factors'), c->g and the residual
+// c->g[n] (enqueued)
+int blocks_add_priors(balm_ctx *c, const double *poses);
+// points c->pr's diagonal table at the current pattern (no-op without priors or without a pattern)
+int blocks_map_priors(balm_ctx *c);
 // the blocks of voxels [head, end) from c->G (the per-observation store) and the accumulators, g from the accumulators
 int launch_blocks(balm_ctx *c, int64_t head, int64_t end);
 int blocks_zero(balm_ctx *c);

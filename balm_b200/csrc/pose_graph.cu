@@ -15,6 +15,9 @@
 // rho'(s_f) b and its M rho'(s_f) M (IRLS). The <FactorLoss> instantiations of pg_cost_kernel (writes s_f and
 // w_f = rho'(s_f)) and pg_linearise_kernel (scales M and b by w_f) run only when an active factor has a non-trivial loss;
 // the <NoLoss> ones are the kernels without a loss.
+// Absolute pose priors (DESIGN.md "Absolute pose priors"; PriorSet, balm_set_pose_priors): prior_cost_kernel and
+// prior_linearise_kernel per active prior, prior_assemble_kernel per (pose with priors, entry) adding the pose's sums onto
+// the diagonal block and g after the factors; run only while a prior is active.
 #include <math.h>
 #include <type_traits>
 #include <algorithm>
@@ -352,6 +355,163 @@ __global__ void __launch_bounds__(PG_THREADS) pg_sum_kernel(const double *part, 
   }
 }
 
+// ---- absolute pose priors (DESIGN.md "Absolute pose priors"): prior q on pose i with measured pose T^ = (R^, p^),
+// body-frame lever arm l and 6x6 H_q (column-major, (rotation, translation) order):
+//   e = (Log(R R^^T), R l + p - p^),   s_q = e^T H_q e,   cost_q = 1/2 rho(s_q),
+//   J = de/d(delta) = [[Jl^-1(e_rot), 0], [-hat(R l + p), I]] under the left update,   M_q = w J^T H_q J, b_q = w J^T H_q e
+// with w = rho'(s_q) (1 without a loss). One thread per active prior; the active priors are held sorted by pose, prior
+// order within a pose, so that prior_assemble_kernel sums a contiguous range. ----
+
+// e (6) and, when J is not null, J (row-major 6 x 6). Not inlined, so that the cost and the linearisation compute
+// bitwise the same e.
+__device__ __noinline__ void prior_residual(const double *T, const double *hat, const double *lever, double *e,
+                                            double *J) {
+  double r[9], p[3], rh[9], ph[3], D[9], x[3];
+  load_pose(T, r, p);
+  load_pose(hat, rh, ph);
+  for (int a = 0; a < 3; a++)
+    for (int b = 0; b < 3; b++) D[a * 3 + b] = r[a * 3] * rh[b * 3] + r[a * 3 + 1] * rh[b * 3 + 1] + r[a * 3 + 2] * rh[b * 3 + 2];
+  log_so3(D, e);
+  for (int a = 0; a < 3; a++) {
+    x[a] = r[a * 3] * lever[0] + r[a * 3 + 1] * lever[1] + r[a * 3 + 2] * lever[2] + p[a];  // R l + p
+    e[3 + a] = x[a] - ph[a];
+  }
+  if (!J) return;
+  // Jl^-1(phi) = I - 1/2 hat(phi) + c2 hat(phi)^2, c2 = (1 - (th/2) cot(th/2)) / th^2 (series below th = 0.1)
+  const double t2 = e[0] * e[0] + e[1] * e[1] + e[2] * e[2], th = sqrt(t2);
+  double c2;
+  if (th < 0.1) {
+    c2 = 1.0 / 12 + t2 * (1.0 / 720 + t2 * (1.0 / 30240 + t2 / 1209600));
+  } else {
+    const double h = 0.5 * th;
+    c2 = (1.0 - h * cos(h) / sin(h)) / t2;
+  }
+  const double K[9] = {0, -e[2], e[1], e[2], 0, -e[0], -e[1], e[0], 0};
+  const double W[9] = {0, -x[2], x[1], x[2], 0, -x[0], -x[1], x[0], 0};
+  for (int a = 0; a < 3; a++)
+    for (int b = 0; b < 3; b++) {
+      J[a * 6 + b] = (a == b ? 1.0 : 0.0) - 0.5 * K[a * 3 + b] + c2 * (e[a] * e[b] - (a == b ? t2 : 0.0));
+      J[a * 6 + 3 + b] = 0.0;
+      J[(3 + a) * 6 + b] = -W[a * 3 + b];
+      J[(3 + a) * 6 + 3 + b] = a == b ? 1.0 : 0.0;
+    }
+}
+
+struct PriorView {  // the prior set as the per-prior kernels read it
+  const int *pose;      // [n] pose of every prior
+  const double *hat;    // [n][12] T^
+  const double *lever;  // [n][3] l
+  const double *H;      // [n][36] column-major
+};
+
+// ---- per active prior k (act[k] = prior q): cost_part[k] = 1/2 rho(s_q); with FactorLoss s_q, w_q to its outputs ----
+template <typename Loss>
+__global__ void __launch_bounds__(PG_THREADS) prior_cost_kernel(PriorView pv, const int *act, int n_act,
+                                                                const double *poses, double *cost_part, Loss loss) {
+  const int k = blockIdx.x * PG_THREADS + threadIdx.x;
+  if (k >= n_act) return;
+  const int q = act[k];
+  double e[6];
+  prior_residual(poses + 12 * (size_t)pv.pose[q], pv.hat + 12 * (size_t)q, pv.lever + 3 * (size_t)q, e, nullptr);
+  const double *Hq = pv.H + 36 * (size_t)q;
+  double s = 0.0;
+  for (int r = 0; r < 6; r++) {
+    double t = 0.0;
+    for (int c = 0; c < 6; c++) t += Hq[6 * c + r] * e[c];
+    s += e[r] * t;
+  }
+  if constexpr (std::is_same<Loss, FactorLoss>::value) {
+    double rho, drho;
+    loss_rho(loss.kind ? loss.kind[q] : BALM_LOSS_TRIVIAL, loss.kind ? loss.scale[q] : 1.0, s, &rho, &drho);
+    loss.s[q] = s;
+    loss.w[q] = drho;
+    s = rho;
+  }
+  cost_part[k] = 0.5 * s;
+}
+
+// ---- per active prior k: M[k] = w J^T H J (36, column-major) and b[k] = w J^T H e; with FactorLoss w is the w_q that
+// the cost pass before has written ----
+template <typename Loss>
+__global__ void __launch_bounds__(PG_THREADS) prior_linearise_kernel(PriorView pv, const int *act, int n_act,
+                                                                     const double *poses, double *M, double *b,
+                                                                     Loss loss) {
+  const int k = blockIdx.x * PG_THREADS + threadIdx.x;
+  if (k >= n_act) return;
+  const int q = act[k];
+  double e[6], J[36];
+  prior_residual(poses + 12 * (size_t)pv.pose[q], pv.hat + 12 * (size_t)q, pv.lever + 3 * (size_t)q, e, J);
+  double w = 1.0;
+  if constexpr (std::is_same<Loss, FactorLoss>::value) w = loss.w[q];
+  const double *Hq = pv.H + 36 * (size_t)q;
+  double *Mk = M + 36 * (size_t)k, *bk = b + 6 * (size_t)k;
+  double He[6];
+  for (int r = 0; r < 6; r++) {
+    double t = 0.0;
+    for (int c = 0; c < 6; c++) t += Hq[6 * c + r] * e[c];
+    He[r] = t;
+  }
+  for (int a = 0; a < 6; a++) {
+    double t = 0.0;
+    for (int r = 0; r < 6; r++) t += J[r * 6 + a] * He[r];
+    bk[a] = w * t;
+  }
+  for (int d = 0; d < 6; d++) {  // column d: (H J)[:, d], then M[:, d] = J^T (H J)[:, d]
+    double HJ[6];
+    for (int r = 0; r < 6; r++) {
+      double t = 0.0;
+      for (int c = 0; c < 6; c++) t += Hq[6 * c + r] * J[c * 6 + d];
+      HJ[r] = t;
+    }
+    for (int a = 0; a < 6; a++) {
+      double t = 0.0;
+      for (int r = 0; r < 6; r++) t += J[r * 6 + a] * HJ[r];
+      Mk[6 * d + a] = w * t;
+    }
+  }
+}
+
+// Where a pose's prior sum goes: onto the dense H of a context's pose graph, or onto the pose's diagonal block of a
+// block pattern (the sparse pose graph's pairs or a BALM_PREC_BLOCKS context's union), diag[u] its index there.
+struct DenseAdd {
+  double *H;
+  size_t n;
+  __device__ __forceinline__ void operator()(int u, int i, int a, int c6, double s) const {
+    H[(6 * (size_t)i + c6) * n + 6 * (size_t)i + a] += s;
+  }
+};
+struct DiagAdd {
+  double *B;
+  const int *diag;
+  __device__ __forceinline__ void operator()(int u, int, int a, int c6, double s) const {
+    B[36 * (size_t)diag[u] + 6 * c6 + a] += s;
+  }
+};
+
+// ---- per (pose u with priors, entry): the sum of its priors' M (36 entries) or b (6 entries), in their order, added
+// once onto the block and g that the factor and voxel assembly wrote. Like pg_assemble_kernel on a diagonal pair, both
+// (a, c6) and (c6, a) read the lower entry, so the block stays exactly symmetric. ----
+template <typename Out>
+__global__ void __launch_bounds__(PG_THREADS) prior_assemble_kernel(const int *upose, const int *uptr, int n_u,
+                                                                    const double *M, const double *b, Out out,
+                                                                    double *g) {
+  const long long t = (long long)blockIdx.x * PG_THREADS + threadIdx.x;
+  if (t >= 42LL * n_u) return;
+  const int u = (int)(t / 42), e = (int)(t % 42), i = upose[u];
+  double s = 0.0;
+  if (e < 36) {
+    const int a = e % 6, c6 = e / 6, ra = max(a, c6), rc = min(a, c6);
+    for (int k = uptr[u]; k < uptr[u + 1]; k++) s += M[36 * (size_t)k + 6 * rc + ra];
+    out(u, i, a, c6, s);
+  } else {
+    const int a = e - 36;
+    for (int k = uptr[u]; k < uptr[u + 1]; k++) s += b[6 * (size_t)k + a];
+    g[6 * (size_t)i + a] += s;
+  }
+}
+
+__global__ void prior_add_cost_kernel(const double *x, double *y) { *y += *x; }
+
 }  // namespace
 
 // The registered factor set (device). Factor f owns slots [fptr[f], fptr[f+1]) and the (6N_f)^2 doubles at hoff[f] of
@@ -606,7 +766,9 @@ static int pose_graph_assemble(const PoseGraph &p, cudaStream_t st, const double
 int pose_graph_eval(balm_ctx *c, const double *poses) {
   const size_t n = c->n;
   CUDA_TRY(cudaMemsetAsync(c->H, 0, sizeof(double) * n * n, c->stream));
-  return pose_graph_assemble(*c->pg, c->stream, poses, DenseH{c->H}, c->g, c->scal, &c->launches);
+  TRY(pose_graph_assemble(*c->pg, c->stream, poses, DenseH{c->H}, c->g, c->scal, &c->launches));
+  if (c->pr) TRY(prior_add_dense(c->pr, c->stream, poses, c->H, n, c->g, c->scal, &c->launches));
+  return BALM_OK;
 }
 
 int pose_graph_eval_blocks(const PoseGraph *p, cudaStream_t st, const double *poses, double *blocks, double *g,
@@ -615,6 +777,222 @@ int pose_graph_eval_blocks(const PoseGraph *p, cudaStream_t st, const double *po
 }
 
 int pose_graph_add_blocks(const PoseGraph *p, cudaStream_t st, const double *poses, double *blocks, const int *map,
-                          double *g_cost, long long *launches) {
-  return pose_graph_assemble(*p, st, poses, AddBlocks{blocks, map}, g_cost, g_cost + 6 * (size_t)p->P, launches);
+                          double *g, double *cost, long long *launches) {
+  return pose_graph_assemble(*p, st, poses, AddBlocks{blocks, map}, g, cost, launches);
+}
+
+// ---------------- absolute pose priors ----------------
+// The registered prior set (device). Prior q's pose, T^, l and H at index q; the active priors (status BALM_OK) in
+// `act`, sorted by pose and in prior order within a pose; the poses with active priors (upose) and their ranges of `act`
+// (uptr). M and b are the linearisation's staging per active prior. diag[u]: upose[u]'s diagonal block in the handle's
+// block pattern (prior_set_map; absent on a dense context).
+struct PriorSet {
+  int n = 0, n_act = 0, n_u = 0;
+  int *pose = nullptr, *act = nullptr, *upose = nullptr, *uptr = nullptr, *diag = nullptr;
+  double *hat = nullptr, *lever = nullptr, *H = nullptr, *M = nullptr, *b = nullptr, *cost_part = nullptr,
+         *cost = nullptr;
+  // [n] kind, scale, s, w; allocated only while some prior's kind is non-trivial
+  int *loss_kind = nullptr;
+  double *loss_scale = nullptr, *loss_s = nullptr, *loss_w = nullptr;
+  bool robust = false;  // an active prior has a non-trivial kind
+  std::vector<int> upose_h;
+  long long bytes = 0, diag_bytes = 0;
+  ~PriorSet() {
+    cudaFree(pose); cudaFree(act); cudaFree(upose); cudaFree(uptr); cudaFree(diag); cudaFree(hat); cudaFree(lever);
+    cudaFree(H); cudaFree(M); cudaFree(b); cudaFree(cost_part); cudaFree(cost);
+    cudaFree(loss_kind); cudaFree(loss_scale); cudaFree(loss_s); cudaFree(loss_w);
+  }
+  PriorView view() const { return PriorView{pose, hat, lever, H}; }
+  FactorLoss loss() const { return FactorLoss{loss_kind, loss_scale, loss_s, loss_w}; }
+};
+
+void prior_set_free(PriorSet *p) { delete p; }
+long long prior_set_bytes(const PriorSet *p) { return p->bytes + p->diag_bytes; }
+bool prior_set_active(const PriorSet *p) { return p && p->n_act > 0; }
+const std::vector<int> &prior_set_poses(const PriorSet *p) { return p->upose_h; }
+
+// Eigenvalues of a symmetric 6 x 6 matrix (cyclic Jacobi, host)
+static void sym6_eigenvalues(const double *H, double *lam) {
+  double A[36];
+  std::copy(H, H + 36, A);
+  for (int sweep = 0; sweep < 50; sweep++) {
+    double off = 0.0, tot = 0.0;
+    for (int i = 0; i < 36; i++) { tot += A[i] * A[i]; if (i % 7) off += A[i] * A[i]; }
+    if (off <= 1e-300 || off <= 1e-32 * tot) break;
+    for (int p = 0; p < 5; p++)
+      for (int q = p + 1; q < 6; q++) {
+        const double apq = A[6 * q + p];
+        if (apq == 0.0) continue;
+        const double th = (A[6 * q + q] - A[6 * p + p]) / (2.0 * apq);
+        const double t = (th >= 0 ? 1.0 : -1.0) / (fabs(th) + sqrt(th * th + 1.0));
+        const double c = 1.0 / sqrt(t * t + 1.0), s = t * c;
+        for (int k = 0; k < 6; k++) {  // columns p, q
+          const double akp = A[6 * p + k], akq = A[6 * q + k];
+          A[6 * p + k] = c * akp - s * akq;
+          A[6 * q + k] = s * akp + c * akq;
+        }
+        for (int k = 0; k < 6; k++) {  // rows p, q
+          const double apk = A[6 * k + p], aqk = A[6 * k + q];
+          A[6 * k + p] = c * apk - s * aqk;
+          A[6 * k + q] = s * apk + c * aqk;
+        }
+      }
+  }
+  for (int i = 0; i < 6; i++) lam[i] = A[7 * i];
+}
+
+int prior_set_build(cudaStream_t st, int n, const int32_t *pose, const double *hat12, const double *lever3,
+                    const double *H36, const int32_t *kind, const double *scale, std::vector<int> *status_out,
+                    PriorSet **out) {
+  std::unique_ptr<PriorSet> p(new PriorSet());
+  p->n = n;
+  std::vector<int> status(n), act;
+  for (int q = 0; q < n; q++) {  // PSD and nonzero: min eigenvalue >= -1e-12 max eigenvalue > 0
+    double lam[6];
+    sym6_eigenvalues(H36 + 36 * (size_t)q, lam);
+    const double lmin = *std::min_element(lam, lam + 6), lmax = *std::max_element(lam, lam + 6);
+    status[q] = lmax > 0.0 && lmin >= -1e-12 * lmax ? BALM_OK : BALM_ERR_NOT_PD;
+    if (status[q] == BALM_OK) act.push_back(q);
+  }
+  std::stable_sort(act.begin(), act.end(), [&](int a, int b) { return pose[a] < pose[b]; });
+  std::vector<int> uptr;
+  for (size_t k = 0; k < act.size(); k++)
+    if (k == 0 || pose[act[k]] != pose[act[k - 1]]) { p->upose_h.push_back(pose[act[k]]); uptr.push_back((int)k); }
+  uptr.push_back((int)act.size());
+  p->n_act = (int)act.size();
+  p->n_u = (int)p->upose_h.size();
+  std::vector<double> lever(3 * (size_t)n, 0.0);
+  if (lever3) std::copy(lever3, lever3 + 3 * (size_t)n, lever.begin());
+  TRY(upload(&p->pose, pose, (size_t)n, st));
+  TRY(upload(&p->hat, hat12, 12 * (size_t)n, st));
+  TRY(upload(&p->lever, lever.data(), lever.size(), st));
+  TRY(upload(&p->H, H36, 36 * (size_t)n, st));
+  TRY(upload(&p->act, act.data(), act.size(), st));
+  TRY(upload(&p->upose, p->upose_h.data(), p->upose_h.size(), st));
+  TRY(upload(&p->uptr, uptr.data(), uptr.size(), st));
+  TRY(dev_alloc(&p->M, 36 * act.size()));
+  TRY(dev_alloc(&p->b, 6 * act.size()));
+  TRY(dev_alloc(&p->cost_part, std::max<size_t>(1, act.size())));
+  TRY(dev_alloc(&p->cost, 1));
+  const auto nz = [](size_t k) { return std::max<size_t>(1, k); };
+  p->bytes = (long long)(sizeof(int) * (nz(n) + nz(act.size()) + nz(p->upose_h.size()) + uptr.size()) +
+                         sizeof(double) * (nz(12 * (size_t)n) + nz(3 * (size_t)n) + nz(36 * (size_t)n) +
+                                           nz(36 * act.size()) + nz(6 * act.size()) + nz(act.size()) + 1));
+  const bool any = kind && std::any_of(kind, kind + n, [](int32_t k) { return k != BALM_LOSS_TRIVIAL; });
+  if (any) {
+    std::vector<double> c(n);
+    for (int q = 0; q < n; q++) c[q] = kind[q] == BALM_LOSS_TRIVIAL ? 1.0 : scale[q];  // a trivial prior's scale is unused
+    for (int q : act) p->robust = p->robust || kind[q] != BALM_LOSS_TRIVIAL;
+    TRY(upload(&p->loss_kind, kind, (size_t)n, st));
+    TRY(upload(&p->loss_scale, c.data(), (size_t)n, st));
+    TRY(dev_alloc(&p->loss_s, (size_t)n));
+    TRY(dev_alloc(&p->loss_w, (size_t)n));
+    CUDA_TRY(cudaMemsetAsync(p->loss_s, 0, sizeof(double) * n, st));  // inactive priors keep s = w = 0
+    CUDA_TRY(cudaMemsetAsync(p->loss_w, 0, sizeof(double) * n, st));
+    p->bytes += LOSS_BYTES_PER_FACTOR * n;
+  }
+  CUDA_TRY(cudaStreamSynchronize(st));
+  *status_out = std::move(status);
+  *out = p.release();
+  return BALM_OK;
+}
+
+int prior_set_map(PriorSet *p, cudaStream_t st, const std::vector<int2> &pairs) {
+  std::vector<int> diag(p->upose_h.size());
+  for (size_t u = 0; u < diag.size(); u++) {
+    const int2 key = make_int2(p->upose_h[u], p->upose_h[u]);
+    const auto it = std::lower_bound(pairs.begin(), pairs.end(), key, [](const int2 &a, const int2 &b) {
+      return a.x < b.x || (a.x == b.x && a.y < b.y);
+    });
+    if (it == pairs.end() || it->x != key.x || it->y != key.y) {
+      balm_set_error("prior_set_map: a prior's pose has no diagonal block in the pattern");
+      return BALM_ERR_INVALID;
+    }
+    diag[u] = (int)(it - pairs.begin());
+  }
+  cudaFree(p->diag);
+  p->diag = nullptr;
+  TRY(upload(&p->diag, diag.data(), diag.size(), st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  p->diag_bytes = (long long)(sizeof(int) * std::max<size_t>(1, diag.size()));
+  return BALM_OK;
+}
+
+static int prior_cost_pass(const PriorSet &p, cudaStream_t st, const double *poses, const FactorLoss *loss,
+                           long long *launches) {
+  if (!p.n_act) return BALM_OK;
+  const unsigned grid = (unsigned)((p.n_act + PG_THREADS - 1) / PG_THREADS);
+  if (loss) prior_cost_kernel<<<grid, PG_THREADS, 0, st>>>(p.view(), p.act, p.n_act, poses, p.cost_part, *loss);
+  else prior_cost_kernel<<<grid, PG_THREADS, 0, st>>>(p.view(), p.act, p.n_act, poses, p.cost_part, NoLoss{});
+  *launches += 1;
+  CUDA_TRY(cudaGetLastError());
+  return BALM_OK;
+}
+
+// the priors' cost summed and added onto *cost (after whatever the factors and voxels wrote there)
+static int prior_sum_add(const PriorSet &p, cudaStream_t st, double *cost, long long *launches) {
+  pg_sum_kernel<<<1, PG_THREADS, 0, st>>>(p.cost_part, p.n_act, p.cost);
+  prior_add_cost_kernel<<<1, 1, 0, st>>>(p.cost, cost);
+  *launches += 2;
+  CUDA_TRY(cudaGetLastError());
+  return BALM_OK;
+}
+
+int prior_add_cost(const PriorSet *pr, cudaStream_t st, const double *poses, double *cost, long long *launches) {
+  const PriorSet &p = *pr;
+  if (!p.n_act) return BALM_OK;
+  const FactorLoss l = p.loss();
+  TRY(prior_cost_pass(p, st, poses, p.robust ? &l : nullptr, launches));
+  return prior_sum_add(p, st, cost, launches);
+}
+
+int prior_residuals(const PriorSet *pr, cudaStream_t st, const double *poses, double *s, double *w,
+                    long long *launches) {
+  const PriorSet &p = *pr;
+  const size_t n = (size_t)p.n;
+  double *tmp = nullptr;  // without a loss: s and w of one call
+  if (!p.loss_kind) {
+    TRY(dev_alloc(&tmp, 2 * n));
+    CUDA_TRY(cudaMemsetAsync(tmp, 0, sizeof(double) * 2 * n, st));
+  }
+  std::unique_ptr<double, cudaError_t (*)(void *)> tmp_own(tmp, cudaFree);
+  const FactorLoss loss = tmp ? FactorLoss{nullptr, nullptr, tmp, tmp + n} : p.loss();
+  TRY(prior_cost_pass(p, st, poses, &loss, launches));
+  if (s && n) CUDA_TRY(cudaMemcpyAsync(s, loss.s, sizeof(double) * n, cudaMemcpyDeviceToHost, st));
+  if (w && n) CUDA_TRY(cudaMemcpyAsync(w, loss.w, sizeof(double) * n, cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  return BALM_OK;
+}
+
+// the priors' M and b onto H (through `out`) and g, their cost onto *cost; with a loss the cost pass runs first so that
+// the linearisation can weight M and b
+template <typename Out>
+static int prior_assemble(const PriorSet &p, cudaStream_t st, const double *poses, Out out, double *g, double *cost,
+                          long long *launches) {
+  if (!p.n_act) return BALM_OK;
+  const unsigned grid = (unsigned)((p.n_act + PG_THREADS - 1) / PG_THREADS);
+  if (p.robust) {
+    const FactorLoss l = p.loss();
+    TRY(prior_cost_pass(p, st, poses, &l, launches));
+    prior_linearise_kernel<<<grid, PG_THREADS, 0, st>>>(p.view(), p.act, p.n_act, poses, p.M, p.b, l);
+  } else {
+    prior_linearise_kernel<<<grid, PG_THREADS, 0, st>>>(p.view(), p.act, p.n_act, poses, p.M, p.b, NoLoss{});
+  }
+  const long long threads = 42LL * p.n_u;
+  prior_assemble_kernel<<<(unsigned)((threads + PG_THREADS - 1) / PG_THREADS), PG_THREADS, 0, st>>>(
+      p.upose, p.uptr, p.n_u, p.M, p.b, out, g);
+  *launches += 2;
+  CUDA_TRY(cudaGetLastError());
+  if (!p.robust) TRY(prior_cost_pass(p, st, poses, nullptr, launches));
+  return prior_sum_add(p, st, cost, launches);
+}
+
+int prior_add_dense(const PriorSet *p, cudaStream_t st, const double *poses, double *H, size_t n, double *g,
+                    double *cost, long long *launches) {
+  return prior_assemble(*p, st, poses, DenseAdd{H, n}, g, cost, launches);
+}
+
+int prior_add_blocks(const PriorSet *p, cudaStream_t st, const double *poses, double *blocks, double *g, double *cost,
+                     long long *launches) {
+  return prior_assemble(*p, st, poses, DiagAdd{blocks, p->diag}, g, cost, launches);
 }

@@ -83,23 +83,30 @@ def propagate(layers):
     return np.array(F)
 
 
-def fuse_windows(poses_in, poses0, factors, device=0):
+def fuse_windows(poses_in, poses0, factors, device=0, priors=None):
     """The pose graph's LM (gauge_mode 2) over all scans from poses0, then re-anchored so that scan 0 keeps its input
     pose poses_in[0] -> (poses, dict(status, trace, n_factors, ms)). From PG_SPARSE_MIN_POSES scans on it runs on the
-    sparse solve (PoseGraph), below on the context's dense one."""
+    sparse solve (PoseGraph), below on the context's dense one. priors (set_pose_priors' dicts, by scan index) join the
+    pose graph; with any, the result is already in the priors' frame and is not re-anchored (the dict also holds
+    prior_status)."""
     t0 = time.perf_counter()
     c = PoseGraph(len(poses0), device) if len(poses0) >= PG_SPARSE_MIN_POSES else Context(len(poses0), device)
     try:
         status = c.set_pose_factors(factors)
+        prior_status = c.set_pose_priors(priors) if priors else []
         x, trace = c.pose_graph_iter(poses0, gauge_mode=2)
     finally:
         c.close()
-    x = np.array([relative_chain(poses_in[0], x[0], p) for p in x])
-    return x, dict(status=status, trace=trace, n_factors=len(factors), ms=1e3 * (time.perf_counter() - t0))
+    if not priors:
+        x = np.array([relative_chain(poses_in[0], x[0], p) for p in x])
+    info = dict(status=status, trace=trace, n_factors=len(factors), ms=1e3 * (time.perf_counter() - t0))
+    if priors:
+        info["prior_status"] = prior_status
+    return x, info
 
 
 def hba(scans, poses12, length=10, stride=5, downsample=0.1, assoc=None, device=0, top_size=MAX_POSES,
-        pose_graph=False, **lm_opts):
+        pose_graph=False, priors=None, **lm_opts):
     """scans: list of (n_s x 3) body-frame points; poses12: P x 12 initial poses. downsample: the keyframes' voxel edge
     (< 0.001: keyframes keep every point); assoc: cut_scans options (DEFAULT_ASSOC when None); lm_opts: damping_iter
     options of every window. Layers are built while more than top_size (<= 32) items remain.
@@ -107,7 +114,11 @@ def hba(scans, poses12, length=10, stride=5, downsample=0.1, assoc=None, device=
     n_voxels, poses_in (the items' input poses), poses (per window the poses carried down), kf_sizes (None at the top)
     and ms (wall times of cut, lm and merge)). pose_graph: the final poses come from the pose graph over every converged
     window with at least 2 items, started from the propagated ones; the result then also holds pose_graph = dict(status
-    per factor, trace, n_factors, ms)."""
+    per factor, trace, n_factors, ms). priors (pose_graph only): absolute pose priors by scan index, in
+    Context.set_pose_priors' format (e.g. position_priors of GNSS fixes); they join that pose graph, and the final poses
+    are then in the priors' frame rather than re-anchored to scan 0."""
+    if priors and not pose_graph:
+        raise ValueError("hba: priors join the top pose graph: pass pose_graph=True")
     if not (2 <= length <= MAX_POSES and 1 <= stride <= length and 1 <= top_size <= MAX_POSES):
         raise ValueError("hba: needs 2 <= length <= 32, 1 <= stride <= length and 1 <= top_size <= 32")
     poses12 = np.asarray(poses12, dtype=np.float64).reshape(-1, 12)
@@ -149,7 +160,7 @@ def hba(scans, poses12, length=10, stride=5, downsample=0.1, assoc=None, device=
     res = dict(poses=propagate(layers), layers=layers)
     if pose_graph:
         if factors:
-            res["poses"], res["pose_graph"] = fuse_windows(poses12, res["poses"], factors, device)
+            res["poses"], res["pose_graph"] = fuse_windows(poses12, res["poses"], factors, device, priors)
         else:
             res["pose_graph"] = dict(status=[], trace=[], n_factors=0, ms=0.0)
     return res

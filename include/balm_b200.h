@@ -131,7 +131,9 @@ int balm_residual(balm_ctx *ctx, const double *poses12, double *residual);
 int balm_solve(balm_ctx *ctx, double u, double *dx, double *q1, int *not_pd);
 /* BALM2::damping_iter(x_stats, voxhess) (bavoxel.hpp:1069-1166). poses12 updated in place.
  * trace: room for opts->max_iter entries (may be NULL). poses_per_iter: max_iter*N*12 doubles or NULL,
- * receives the accepted pose set after every iteration (before the gauge step) for parity checks. */
+ * receives the accepted pose set after every iteration (before the gauge step) for parity checks.
+ * On a BALM_PREC_BLOCKS context with an active pose prior (balm_set_pose_priors) gauge_mode 0 and 1 are BALM_ERR_INVALID:
+ * the priors fix the frame, and re-anchoring to pose 0 would move the result off them; pass 2. */
 int balm_damping_iter(balm_ctx *ctx, double *poses12, const balm_lm_opts *opts, balm_trace *trace, int *n_iters,
                       double *poses_per_iter);
 void balm_default_lm_opts(balm_lm_opts *opts);
@@ -419,7 +421,8 @@ int balm_pose_graph_evaluate(balm_ctx *ctx, const double *poses12, double *H, do
 /* balm_damping_iter on the pose-graph cost: the same LM rule (u0, v0, q / q1, rel_tol, max_iter, force_hess, verbose),
  * solve, refinement, pose update and gauge_mode, with the factor evaluation in place of the voxel evaluation.
  * min_planes_per_pose and hess_includes_fix have no meaning here and are ignored. BALM_ERR_INVALID with a communicator
- * attached (single GPU only) or without registered factors. */
+ * attached (single GPU only) or without registered factors, and for gauge_mode 0 or 1 while a pose prior is active
+ * (balm_set_pose_priors: the priors fix the frame; pass 2). */
 int balm_pose_graph_iter(balm_ctx *ctx, double *poses12, const balm_lm_opts *opts, balm_trace *trace, int *n_iters,
                          double *poses_per_iter);
 
@@ -445,7 +448,7 @@ int balm_spg_structure(balm_spg *spg, int64_t stats[4], int32_t *pairs);
  * column-major) in balm_spg_structure's order, bitwise the context's dense entries. blocks and g may be NULL. */
 int balm_spg_evaluate(balm_spg *spg, const double *poses12, double *blocks, double *g, double *cost);
 /* balm_pose_graph_iter's contract (LM rule, force_hess, rel_tol, gauge_mode, trace records, refinement and not_pd
- * rules) on the sparse solve. */
+ * rules, gauge_mode 0 / 1 refused while a pose prior is active) on the sparse solve. */
 int balm_spg_iter(balm_spg *spg, double *poses12, const balm_lm_opts *opts, balm_trace *trace, int *n_iters,
                   double *poses_per_iter);
 /* Marginal pose covariances (DESIGN.md "Marginal covariances"): H evaluated undamped at poses12, the 6 rows and columns
@@ -527,6 +530,44 @@ int balm_set_factor_loss(balm_ctx *ctx, int n_factors, const int32_t *kind, cons
  * chi-square gating of candidate closures. Enqueues the cost pass only and waits once. BALM_ERR_INVALID for a null ctx
  * or poses12, or no registered factor set. */
 int balm_factor_residuals(balm_ctx *ctx, const double *poses12, double *s, double *w);
+
+/* Absolute pose priors (DESIGN.md "Absolute pose priors"): GNSS positions, surveyed control points, full-pose anchors.
+ * Prior q names a pose slot pose[q] and holds a measured pose T^ = (R^, p^) (poses_hat12, 12 doubles each), a body-frame
+ * lever arm l (lever3, 3 doubles each; NULL: all 0), a 6 x 6 symmetric positive semi-definite H_q (H36, 36 doubles each,
+ * column-major, (rotation, translation) order, in the units of the cost it joins) and a loss kind[q] / scale[q] as
+ * balm_set_factor_loss's (kind NULL: all trivial). With T = (R, p) of the pose:
+ *   e = (Log(R R^^T), R l + p - p^),   s_q = e^T H_q e,   cost_q = 1/2 rho(s_q),
+ * gradient w J^T H_q e and Hessian w J^T H_q J with w = rho'(s_q), J = [[Jl^-1(e_rot), 0], [-hat(R l + p), I]] under the
+ * library's left update. A position-only (GNSS) prior is H_q = blockdiag(0, Omega_p), its R^ unused; a full-pose
+ * anchor is any positive definite H_q with l = 0. The priors join the pose-graph cost (balm_pose_graph_evaluate /
+ * _iter) on FP64 / TENSOR contexts, and on a BALM_PREC_BLOCKS context every evaluation over the whole voxel range, as
+ * balm_block_set_factors' factors do (balm_evaluate, balm_residual, balm_damping_iter, balm_solve, balm_download_blocks,
+ * balm_block_covariance); every sum adds voxels, then factors, then priors. A prior touches only its pose's diagonal
+ * block, so a blocks context's pattern does not change.
+ * n_priors == 0 (the arrays may be NULL) detaches the set; several priors may name the same pose. The set belongs to the
+ * context, independent of the factor set, its loss and the voxel registration; it survives all of them. The pose
+ * graph calls still need a registered factor set.
+ * status_out (n_priors, may be NULL): BALM_OK, or BALM_ERR_NOT_PD when H_q has an eigenvalue below -1e-12 lambda_max or
+ * is zero; such a prior is left out of every sum. BALM_ERR_INVALID, the previous set kept, for a pose outside [0, N), a
+ * non-finite T^, l, H or scale, an H not symmetric to 1e-12 of its max |entry|, a kind outside BALM_LOSS_*, or a
+ * non-trivial kind without a finite scale > 0.
+ * Gauge: with an active prior the cost has no gauge null space, so balm_damping_iter (blocks), balm_pose_graph_iter and
+ * balm_spg_iter refuse gauge_mode 0 and 1 (BALM_ERR_INVALID: pass 2), and anchor = -1 is the natural covariance call.
+ * balm_block_structure's / balm_spg_structure's stats[3] count the set's device bytes. */
+int balm_set_pose_priors(balm_ctx *ctx, int n_priors, const int32_t *pose, const double *poses_hat12,
+                         const double *lever3, const double *H36, const int32_t *kind, const double *scale,
+                         int32_t *status_out);
+/* s_q and w_q = rho'(s_q) of every prior at poses12 into s and w (n_priors each; either may be NULL); NOT_PD priors
+ * report 0, 0. Waits once. BALM_ERR_INVALID without a registered prior set. */
+int balm_prior_residuals(balm_ctx *ctx, const double *poses12, double *s, double *w);
+/* balm_set_pose_priors and balm_prior_residuals on a sparse pose graph: same arguments, checks, meaning (balm_spg_evaluate,
+ * _iter and _covariance) and lifetime (the set survives balm_spg_set_factors). A prior on a pose that no active factor
+ * covers adds that pose's diagonal pair to the pattern, which is then re-ordered and re-captured; only such a change
+ * does that. */
+int balm_spg_set_pose_priors(balm_spg *spg, int n_priors, const int32_t *pose, const double *poses_hat12,
+                             const double *lever3, const double *H36, const int32_t *kind, const double *scale,
+                             int32_t *status_out);
+int balm_spg_prior_residuals(balm_spg *spg, const double *poses12, double *s, double *w);
 
 /* Multi-GPU: voxels are sharded across ranks by the caller (each rank registers its own shard); the library
  * all-reduces [H | g | r] with NCCL after every evaluation and the scalar after every residual pass.
