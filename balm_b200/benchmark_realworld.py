@@ -21,10 +21,12 @@ def main(argv=None):
     ap.add_argument("--out", default=None, help="write the refined poses in alidarPose.csv format")
     ap.add_argument("--cloud_out", default=None, help="write the refined map (what the reference publishes on /map_show) as .pcd")
     ap.add_argument("--path_out", default=None, help="write the refined trajectory (/map_path) as .pcd")
+    drivers.add_voxel_loss_args(ap)
     a = ap.parse_args(argv)
     res = drivers.benchmark_realworld(a.file_path, a.voxel_size, a.device,
                                       L.PREC_TENSOR if a.precision == "tensor" else L.PREC_FP64, a.max_scans,
-                                      keep_scans=bool(a.cloud_out or a.path_out))
+                                      keep_scans=bool(a.cloud_out or a.path_out),
+                                      voxel_loss=drivers.voxel_loss_arg(ap, a))
     if res is None:
         return 0  # the reference exits with status 0 when the plane guard fires (:208, bavoxel.hpp:1084)
     if a.out:

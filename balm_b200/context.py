@@ -54,6 +54,14 @@ def _set_factor_loss(fn, handle, n_factors, kind, scale):
     L.check(fn(handle, len(k), _p(k), _p(sc)))
 
 
+def _set_voxel_loss(fn, handle, kind, scale):
+    """balm_set_voxel_loss / balm_batch_set_voxel_loss: kind a loss name as set_factor_loss', scale c in metres (a
+    plane thickness; unused for "trivial")."""
+    if kind not in _LOSS:
+        raise ValueError(f"set_voxel_loss: kind must be in {sorted(_LOSS)}, got {kind!r}")
+    L.check(fn(handle, _LOSS[kind], 0.0 if scale is None else float(scale)))
+
+
 def _factor_residuals(fn, handle, n_factors, poses12):
     """balm_factor_residuals / balm_spg_factor_residuals -> (s, w), one entry per factor of the registered set."""
     poses12 = np.ascontiguousarray(poses12, dtype=np.float64)
@@ -206,6 +214,22 @@ class Context:
         r = C.c_double()
         L.check(L.lib().balm_residual(self._h, _p(poses12), C.byref(r)))
         return r.value
+
+    def set_voxel_loss(self, kind, scale=None):
+        """Robust loss of every voxel (include/balm_b200.h, balm_set_voxel_loss): kind "trivial", "huber" or "cauchy" of
+        s_v = lambda_min (m^2) at scale c in metres. Voxel v then costs coe_v rho(s_v) and its H and g are weighted by
+        w_v = rho'(s_v) in every evaluation, LM and covariance. Useful c: 1.5 - 3 point-noise sigmas. "trivial" resets;
+        the loss survives every voxel registration."""
+        _set_voxel_loss(L.lib().balm_set_voxel_loss, self._h, kind, scale)
+
+    def voxel_residuals(self, poses12, head=0, end=None, include_fix=False):
+        """-> (lam, w): lambda_min and its weight rho'(lambda_min) of voxels [head, end) at poses12 (w = 1 without a
+        loss); w is bitwise the weight an evaluation at these poses applies."""
+        poses12 = np.ascontiguousarray(poses12, dtype=np.float64)
+        end = self.M if end is None else end
+        lam, w = np.zeros(max(0, end - head)), np.zeros(max(0, end - head))
+        L.check(L.lib().balm_voxel_residuals(self._h, _p(poses12), int(head), int(end), int(include_fix), _p(lam), _p(w)))
+        return lam, w
 
     def block_structure(self, want_pairs=False):
         """PREC_BLOCKS contexts: -> dict(pairs, l_blocks, levels, device_bytes): block pairs (i <= j) of H, blocks of the
@@ -651,6 +675,23 @@ class Batch:
             out.append((H[ho:ho + n * n].reshape(n, n, order="F"), g[g0:g0 + n].copy(), float(r[b])))
             ho += n * n
         return out
+
+    def set_voxel_loss(self, kind, scale=None):
+        """Context.set_voxel_loss for every voxel of every problem (evaluate, damping_iter, pose_covariance); the loss
+        belongs to the batch and survives every registration."""
+        _set_voxel_loss(L.lib().balm_batch_set_voxel_loss, self._h, kind, scale)
+
+    def voxel_residuals(self, poses_list, include_fix=False):
+        """Context.voxel_residuals per problem -> list of (lam, w), each over the problem's voxels in registration order."""
+        poses = self._concat(poses_list)
+        B, M = C.c_int(), C.c_int64()
+        L.check(L.lib().balm_batch_sizes(self._h, C.byref(B), None, C.byref(M), None))
+        lam, w = np.zeros(M.value), np.zeros(M.value)
+        L.check(L.lib().balm_batch_voxel_residuals(self._h, _p(poses), int(include_fix), _p(lam), _p(w)))
+        voxel_ptr = np.zeros(B.value + 1, dtype=np.int64)
+        L.check(L.lib().balm_batch_download_voxels(self._h, _p(voxel_ptr), None, None, None, None, None, None))
+        return [(lam[voxel_ptr[b]:voxel_ptr[b + 1]].copy(), w[voxel_ptr[b]:voxel_ptr[b + 1]].copy())
+                for b in range(B.value)]
 
     def damping_iter(self, poses_list, max_iter=10, u0=0.01, v0=2.0, rel_tol=1e-6, hess_includes_fix=False,
                      gauge_mode=0, min_planes_per_pose=20, verbose=False, want_per_iter=False, force_hess=False):

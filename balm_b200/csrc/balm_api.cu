@@ -736,6 +736,38 @@ extern "C" int balm_residual(balm_ctx *c, const double *poses12, double *residua
   return residual_dev(c, c->poses_trial, residual);
 }
 
+extern "C" int balm_set_voxel_loss(balm_ctx *c, int kind, double scale) {
+  if (!c) { balm_set_error("balm_set_voxel_loss: bad arguments"); return BALM_ERR_INVALID; }
+  TRY(check_voxel_loss("balm_set_voxel_loss", kind, scale));
+  c->vloss_kind = kind;
+  c->vloss_scale = kind == BALM_LOSS_TRIVIAL ? 1.0 : scale;  // a trivial loss's scale is unused
+  return BALM_OK;
+}
+
+extern "C" int balm_voxel_residuals(balm_ctx *c, const double *poses12, int64_t head, int64_t end, int include_fix,
+                                    double *lam, double *w) {
+  if (!c || !poses12) { balm_set_error("balm_voxel_residuals: bad arguments"); return BALM_ERR_INVALID; }
+  if (!c->registered) { balm_set_error("no voxels registered"); return BALM_ERR_INVALID; }
+  if (head < 0 || end > c->M || head > end) { balm_set_error("balm_voxel_residuals: bad voxel range"); return BALM_ERR_INVALID; }
+  CUDA_TRY(cudaSetDevice(c->device));
+  const int64_t nv = end - head;
+  ScratchPool pool;
+  double *d_out = nullptr;
+  TRY(pool.get(&d_out, 2 * (size_t)nv + 1));  // lam | w | the residual the stats pass also sums
+  CUDA_TRY(cudaMemcpyAsync(c->poses, poses12, sizeof(double) * 12 * c->N, cudaMemcpyHostToDevice, c->stream));
+  CUDA_TRY(cudaMemsetAsync(d_out + 2 * nv, 0, sizeof(double), c->stream));
+  // the evaluation's own stats instantiation (into c->stats), so that w is bitwise the weight an evaluation applies
+  for (int64_t v0 = head; v0 < end; v0 += c->VB) {
+    const int64_t v1 = std::min(end, v0 + c->VB);
+    TRY(launch_voxel_stats(c, c->poses, v0, v1, c->stats, include_fix != 0, d_out + 2 * nv, d_out + (v0 - head),
+                           d_out + nv + (v0 - head)));
+  }
+  if (lam && nv) CUDA_TRY(cudaMemcpyAsync(lam, d_out, sizeof(double) * nv, cudaMemcpyDeviceToHost, c->stream));
+  if (w && nv) CUDA_TRY(cudaMemcpyAsync(w, d_out + nv, sizeof(double) * nv, cudaMemcpyDeviceToHost, c->stream));
+  CUDA_TRY(cudaStreamSynchronize(c->stream));
+  return BALM_OK;
+}
+
 static int collect_solve(balm_ctx *c, double *q1, int *not_pd) {
   float ms;
   cudaEventElapsedTime(&ms, c->ev[9], c->ev[10]);

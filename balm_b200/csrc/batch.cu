@@ -29,6 +29,7 @@
 #include <math.h>
 #include <string.h>
 #include <algorithm>
+#include <type_traits>
 #include <vector>
 #include "internal.cuh"
 
@@ -62,10 +63,14 @@ struct Dev {  // what the kernels read
   int64_t M, K;
 };
 
-// ---- per voxel: the world-frame cluster sum over its observations (+ fix), eig, residual term, stats row ----
-template <bool STORE>
+struct NoLoss {};  // the pure quadratic: the kernel exactly as without a voxel loss
+
+// ---- per voxel: the world-frame cluster sum over its observations (+ fix), eig, residual term, stats row; with
+// VoxelLoss the residual term coe rho(lambda_0) and coe w in the stats row (voxel_eig_kernel's rule) ----
+template <bool STORE, typename Loss>
 __global__ void __launch_bounds__(256) batch_stats_kernel(Dev d, const double *poses, const int *mask, int use_fix,
-                                                          double *stats, double *res_v) {
+                                                          double *stats, double *res_v, Loss loss) {
+  constexpr bool robust = std::is_same<Loss, VoxelLoss>::value;
   const int lane = threadIdx.x & 31;
   const int64_t nw = (int64_t)gridDim.x * 8;
   for (int64_t v = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5); v < d.M; v += nw) {
@@ -97,8 +102,16 @@ __global__ void __launch_bounds__(256) batch_stats_kernel(Dev d, const double *p
       eig3_jacobi(acc[0] * inv - vb0 * vb0, acc[1] * inv - vb0 * vb1, acc[2] * inv - vb0 * vb2,
                   acc[3] * inv - vb1 * vb1, acc[4] * inv - vb1 * vb2, acc[5] * inv - vb2 * vb2, lam, u0, u1, u2);
       const double coe = d.coe[v];
-      res_v[v] = coe * lam[0];
-      if (STORE) store_stats_row(stats + (size_t)v * BALM_STATS_STRIDE, vb0, vb1, vb2, u0, u1, u2, inv, coe, lam);
+      if constexpr (robust) {
+        double rho, w;
+        loss_rho(loss.kind, loss.scale, lam[0], &rho, &w);
+        res_v[v] = coe * rho;
+        if (loss.lam) { loss.lam[v] = lam[0]; loss.w[v] = w; }
+        if (STORE) store_stats_row(stats + (size_t)v * BALM_STATS_STRIDE, vb0, vb1, vb2, u0, u1, u2, inv, coe * w, lam);
+      } else {
+        res_v[v] = coe * lam[0];
+        if (STORE) store_stats_row(stats + (size_t)v * BALM_STATS_STRIDE, vb0, vb1, vb2, u0, u1, u2, inv, coe, lam);
+      }
     }
   }
 }
@@ -697,6 +710,8 @@ struct balm_batch {
   BatchReg *reg = nullptr;
   WindowState *win = nullptr;  // balm_batch_window_* maps (independent of the registration)
   int *h_count = nullptr;  // pinned: problems still active after an iteration
+  int vloss_kind = BALM_LOSS_TRIVIAL;  // balm_batch_set_voxel_loss: every voxel's loss (independent of the registration)
+  double vloss_scale = 1.0;
 };
 
 namespace {
@@ -740,15 +755,24 @@ void syrk_items(const std::vector<Prob> &hprob, int rpv, std::vector<int4> &item
   }
 }
 
-// batch_stats_kernel at poses for every problem with mask[b] != 0: the residual terms, and with stats non-null the
-// stats rows.
-void enqueue_stats(balm_batch *bt, BatchReg *r, const double *poses, const int *mask, bool use_fix, double *stats) {
+// batch_stats_kernel at poses for every problem with mask[b] != 0 under the batch's voxel loss: the residual terms, and
+// with stats non-null the stats rows; lam / w (both or neither; need stats): the per-voxel readout of
+// balm_batch_voxel_residuals.
+void enqueue_stats(balm_batch *bt, BatchReg *r, const double *poses, const int *mask, bool use_fix, double *stats,
+                   double *lam = nullptr, double *w = nullptr) {
   if (r->M == 0) return;
   const int blocks = (int)std::min<int64_t>((r->M + 7) / 8, (int64_t)bt->sm_count * 8);
-  if (stats)
-    batch_stats_kernel<true><<<blocks, 256, 0, bt->stream>>>(r->dev(), poses, mask, use_fix ? 1 : 0, stats, r->res_v);
-  else
-    batch_stats_kernel<false><<<blocks, 256, 0, bt->stream>>>(r->dev(), poses, mask, use_fix ? 1 : 0, nullptr, r->res_v);
+  const int fx = use_fix ? 1 : 0;
+  // without a loss (and outside the readout) the NoLoss kernels, the only ones that run
+  if (bt->vloss_kind != BALM_LOSS_TRIVIAL || lam) {
+    const VoxelLoss loss{bt->vloss_kind, bt->vloss_scale, lam, w};
+    if (stats) batch_stats_kernel<true><<<blocks, 256, 0, bt->stream>>>(r->dev(), poses, mask, fx, stats, r->res_v, loss);
+    else batch_stats_kernel<false><<<blocks, 256, 0, bt->stream>>>(r->dev(), poses, mask, fx, nullptr, r->res_v, loss);
+  } else if (stats) {
+    batch_stats_kernel<true><<<blocks, 256, 0, bt->stream>>>(r->dev(), poses, mask, fx, stats, r->res_v, NoLoss{});
+  } else {
+    batch_stats_kernel<false><<<blocks, 256, 0, bt->stream>>>(r->dev(), poses, mask, fx, nullptr, r->res_v, NoLoss{});
+  }
 }
 
 // The evaluation of every problem with mask[b] != 0 at r->poses: r_eval, H, g.
@@ -1447,5 +1471,32 @@ extern "C" int balm_batch_pose_covariance(balm_batch *bt, const double *poses12,
   CUDA_TRY(cudaStreamSynchronize(st));
   if (!Rcov && status)
     for (int b = 0; b < B; b++) status[b] = BALM_OK;
+  return BALM_OK;
+}
+
+extern "C" int balm_batch_set_voxel_loss(balm_batch *bt, int kind, double scale) {
+  if (!bt) return invalid("balm_batch_set_voxel_loss: bad arguments");
+  TRY(check_voxel_loss("balm_batch_set_voxel_loss", kind, scale));
+  bt->vloss_kind = kind;
+  bt->vloss_scale = kind == BALM_LOSS_TRIVIAL ? 1.0 : scale;  // a trivial loss's scale is unused
+  return BALM_OK;
+}
+
+extern "C" int balm_batch_voxel_residuals(balm_batch *bt, const double *poses12, int include_fix, double *lam, double *w) {
+  if (!bt || !poses12) return invalid("balm_batch_voxel_residuals: bad arguments");
+  BatchReg *r = bt->reg;
+  if (!r) return invalid("balm_batch_voxel_residuals: no problems registered");
+  CUDA_TRY(cudaSetDevice(bt->device));
+  cudaStream_t st = bt->stream;
+  ScratchPool pool;
+  double *d_out = nullptr;
+  TRY(pool.get(&d_out, 2 * (size_t)r->M));
+  CUDA_TRY(cudaMemcpyAsync(r->poses, poses12, sizeof(double) * 12 * r->P, cudaMemcpyHostToDevice, st));
+  // the evaluation's own stats instantiation, so that w is bitwise the weight an evaluation at these poses applies
+  enqueue_stats(bt, r, r->poses, r->ones(), include_fix != 0, r->stats, d_out, d_out + r->M);
+  CUDA_TRY(cudaGetLastError());
+  if (lam && r->M) CUDA_TRY(cudaMemcpyAsync(lam, d_out, sizeof(double) * r->M, cudaMemcpyDeviceToHost, st));
+  if (w && r->M) CUDA_TRY(cudaMemcpyAsync(w, d_out + r->M, sizeof(double) * r->M, cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
   return BALM_OK;
 }

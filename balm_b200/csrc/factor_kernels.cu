@@ -13,6 +13,7 @@
 // Layouts: observations SoA obs[c][s] (c<10, s in CSR order), so a warp reading 32 consecutive slots of one
 // voxel issues ten fully coalesced 256-byte requests; the stats table is AoS (20 doubles per voxel) because
 // the observation pass reads it warp-uniformly (one broadcast transaction per 16 bytes).
+#include <type_traits>
 #include "internal.cuh"
 
 namespace {
@@ -89,9 +90,14 @@ __global__ void __launch_bounds__(STATS_THREADS, 3) voxel_sums_kernel(StatsArgs 
   }
 }
 
-template <bool STORE>
+struct NoLoss {};  // the pure quadratic: the kernel exactly as without a voxel loss
+
+// With VoxelLoss, rho and w = rho'(lambda_0) once per voxel: the residual term is coe rho(lambda_0) and the stats row
+// gets coe w in place of coe, which every Hessian, gradient and covariance term downstream is linear in.
+template <bool STORE, typename Loss>
 __global__ void __launch_bounds__(128) voxel_eig_kernel(const double *sums, const double *coe_all, int64_t v0, int64_t v1,
-                                                        double *stats, double *res_part) {
+                                                        double *stats, double *res_part, Loss loss) {
+  constexpr bool robust = std::is_same<Loss, VoxelLoss>::value;
   __shared__ double red[4];
   double res_acc = 0.0;
   for (int64_t v = v0 + (int64_t)blockIdx.x * 128 + threadIdx.x; v < v1; v += (int64_t)gridDim.x * 128) {
@@ -109,8 +115,16 @@ __global__ void __launch_bounds__(128) voxel_eig_kernel(const double *sums, cons
     eig3_jacobi(acc[0] * inv - vb0 * vb0, acc[1] * inv - vb0 * vb1, acc[2] * inv - vb0 * vb2,
                 acc[3] * inv - vb1 * vb1, acc[4] * inv - vb1 * vb2, acc[5] * inv - vb2 * vb2, lam, u0, u1, u2);
     const double coe = __ldg(coe_all + v);
-    res_acc += coe * lam[0];
-    if (STORE) store_stats_row(stats + (v - v0) * BALM_STATS_STRIDE, vb0, vb1, vb2, u0, u1, u2, inv, coe, lam);
+    if constexpr (robust) {
+      double rho, w;
+      loss_rho(loss.kind, loss.scale, lam[0], &rho, &w);
+      res_acc += coe * rho;
+      if (loss.lam) { loss.lam[v - v0] = lam[0]; loss.w[v - v0] = w; }
+      if (STORE) store_stats_row(stats + (v - v0) * BALM_STATS_STRIDE, vb0, vb1, vb2, u0, u1, u2, inv, coe * w, lam);
+    } else {
+      res_acc += coe * lam[0];
+      if (STORE) store_stats_row(stats + (v - v0) * BALM_STATS_STRIDE, vb0, vb1, vb2, u0, u1, u2, inv, coe, lam);
+    }
   }
   res_acc = warp_sum(res_acc);
   if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = res_acc;
@@ -356,7 +370,7 @@ __global__ void obs_reduce_kernel(const double *part, int chunks, int total, dou
 }  // namespace
 
 int launch_voxel_stats(balm_ctx *c, const double *poses, int64_t v0, int64_t v1, double *stats_out, bool use_fix,
-                       double *residual_out_dev) {
+                       double *residual_out_dev, double *lam_out, double *w_out) {
   const bool store_stats = stats_out != nullptr;
   // residual_out_dev: accumulated (+=) when it is not the first batch -> caller zeroes it first
   const int64_t nv = v1 - v0;
@@ -371,8 +385,16 @@ int launch_voxel_stats(balm_ctx *c, const double *poses, int64_t v0, int64_t v1,
   else voxel_sums_kernel<false><<<blocks, STATS_THREADS, 0, c->stream>>>(a, c->vsums);
   const int64_t wantb = (nv + 127) / 128;
   const int eb = (int)(wantb < (int64_t)c->res_blocks ? wantb : c->res_blocks);
-  if (store_stats) voxel_eig_kernel<true><<<eb, 128, 0, c->stream>>>(c->vsums, c->coe, v0, v1, stats_out, c->res_part);
-  else voxel_eig_kernel<false><<<eb, 128, 0, c->stream>>>(c->vsums, c->coe, v0, v1, nullptr, c->res_part);
+  // without a loss (and outside the readout) the NoLoss kernels, the only ones that run
+  if (c->vloss_kind != BALM_LOSS_TRIVIAL || lam_out) {
+    const VoxelLoss loss{c->vloss_kind, c->vloss_scale, lam_out, w_out};
+    if (store_stats) voxel_eig_kernel<true><<<eb, 128, 0, c->stream>>>(c->vsums, c->coe, v0, v1, stats_out, c->res_part, loss);
+    else voxel_eig_kernel<false><<<eb, 128, 0, c->stream>>>(c->vsums, c->coe, v0, v1, nullptr, c->res_part, loss);
+  } else if (store_stats) {
+    voxel_eig_kernel<true><<<eb, 128, 0, c->stream>>>(c->vsums, c->coe, v0, v1, stats_out, c->res_part, NoLoss{});
+  } else {
+    voxel_eig_kernel<false><<<eb, 128, 0, c->stream>>>(c->vsums, c->coe, v0, v1, nullptr, c->res_part, NoLoss{});
+  }
   residual_reduce_kernel<<<1, 32, 0, c->stream>>>(c->res_part, eb, residual_out_dev, 1);
   c->launches += 3;
   CUDA_TRY(cudaGetLastError());

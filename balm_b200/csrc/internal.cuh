@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
+#include <cmath>
 #include <functional>
 #include <string>
 #include <vector>
@@ -123,6 +124,8 @@ struct balm_ctx {
   BlockHessian *bh = nullptr;     // BALM_PREC_BLOCKS: the registered set's block pattern, terms, blocks and solver
   PriorSet *pr = nullptr;         // balm_set_pose_priors' priors (independent of the factor and the voxel set): part of
                                   // the pose-graph cost, and on BALM_PREC_BLOCKS of every full-range evaluation
+  int vloss_kind = BALM_LOSS_TRIVIAL;  // balm_set_voxel_loss: the loss of every voxel (independent of the voxel set)
+  double vloss_scale = 1.0;
 
   // ---- optimiser state (device) ----
   double *poses = nullptr, *poses_trial = nullptr;  // [12N]
@@ -188,8 +191,47 @@ inline int refuse_blocks(const balm_ctx *c, const char *who) {
   return BALM_ERR_UNSUPPORTED;
 }
 
+// balm_set_voxel_loss / balm_batch_set_voxel_loss arguments: a kind of balm_loss, a finite scale > 0 unless trivial
+inline int check_voxel_loss(const char *who, int kind, double scale) {
+  if (kind != BALM_LOSS_TRIVIAL && kind != BALM_LOSS_HUBER && kind != BALM_LOSS_CAUCHY) {
+    balm_set_error(std::string(who) + ": loss kind " + std::to_string(kind) + " (0, 1, 2 allowed)");
+    return BALM_ERR_INVALID;
+  }
+  if (kind != BALM_LOSS_TRIVIAL && !(std::isfinite(scale) && scale > 0.0)) {
+    balm_set_error(std::string(who) + ": a robust loss needs a finite scale > 0");
+    return BALM_ERR_INVALID;
+  }
+  return BALM_OK;
+}
+
+// The voxel loss as the stats kernels take it (voxel_eig_kernel, batch_stats_kernel): kind / scale of
+// balm_set_voxel_loss, and with lam non-null the per-voxel readout lam[i] = lambda_min, w[i] = rho'(lambda_min)
+// (i: the voxel's index from the start of the launch's range).
+struct VoxelLoss {
+  int kind;
+  double scale;
+  double *lam, *w;
+};
+
 // ---------------- device math ----------------
 #ifdef __CUDACC__
+
+// rho(s) and rho'(s) of BALM_LOSS_HUBER / BALM_LOSS_CAUCHY at scale c; BALM_LOSS_TRIVIAL: s and 1. Shared by the pose
+// factors and priors (pose_graph.cu) and the voxels (factor_kernels.cu, batch.cu).
+__device__ __forceinline__ void loss_rho(int kind, double c, double s, double *rho, double *drho) {
+  const double c2 = c * c;
+  if (kind == BALM_LOSS_HUBER && s > c2) {
+    const double r = sqrt(s);
+    *rho = 2.0 * c * r - c2;
+    *drho = c / r;
+  } else if (kind == BALM_LOSS_CAUCHY) {
+    *rho = c2 * log1p(s / c2);
+    *drho = 1.0 / (1.0 + s / c2);
+  } else {
+    *rho = s;
+    *drho = 1.0;
+  }
+}
 
 struct WC {  // world-frame cluster
   double p00, p01, p02, p11, p12, p22, v0, v1, v2, n;
@@ -718,8 +760,10 @@ __device__ __forceinline__ void dmma_8x8x4(double &c0, double &c1, double a, dou
 #endif  // __CUDACC__
 
 // ---------------- kernel launchers (defined in the .cu files) ----------------
+// The stats pass of voxels [v0, v1) under the context's voxel loss; lam_out / w_out (both or neither; need stats_out):
+// the per-voxel readout of balm_voxel_residuals, index v - v0.
 int launch_voxel_stats(balm_ctx *c, const double *poses, int64_t v0, int64_t v1, double *stats_out, bool use_fix,
-                       double *residual_out_dev);
+                       double *residual_out_dev, double *lam_out = nullptr, double *w_out = nullptr);
 int launch_obs_pass(balm_ctx *c, const double *poses, int64_t v0, int64_t v1, bool first_batch);
 int launch_obs_colmax(balm_ctx *c, const double *poses, int64_t v0, int64_t v1, bool first_batch);
 int launch_obs_int8(balm_ctx *c, const double *poses, int64_t v0, int64_t v1, bool first_batch, const double *sc,

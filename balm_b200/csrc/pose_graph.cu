@@ -288,22 +288,6 @@ __global__ void __launch_bounds__(PG_THREADS) pg_assemble_kernel(const long long
   }
 }
 
-// rho(s) and rho'(s) of BALM_LOSS_HUBER / BALM_LOSS_CAUCHY at scale c; BALM_LOSS_TRIVIAL: s and 1
-__device__ __forceinline__ void loss_rho(int kind, double c, double s, double *rho, double *drho) {
-  const double c2 = c * c;
-  if (kind == BALM_LOSS_HUBER && s > c2) {
-    const double r = sqrt(s);
-    *rho = 2.0 * c * r - c2;
-    *drho = c / r;
-  } else if (kind == BALM_LOSS_CAUCHY) {
-    *rho = c2 * log1p(s / c2);
-    *drho = 1.0 / (1.0 + s / c2);
-  } else {
-    *rho = s;
-    *drho = 1.0;
-  }
-}
-
 // ---- per active factor: cost_f = 1/2 e~^T H~ e~, thread r owning row 6 + r of H~; with FactorLoss s_f = e~^T H~ e~,
 // cost_f = 1/2 rho(s_f) and s_f, w_f = rho'(s_f) to the loss's outputs ----
 template <typename Loss>

@@ -88,6 +88,23 @@ def data_show(poses12, scans, voxel_size=0.05):
     return cloud, p.astype(np.float32)
 
 
+def add_voxel_loss_args(ap):
+    """--voxel_loss {huber,cauchy} --voxel_loss_scale C on an argparse parser (default: no loss)."""
+    ap.add_argument("--voxel_loss", choices=["huber", "cauchy"], default=None,
+                    help="robust voxel cost (Context.set_voxel_loss); default: none")
+    ap.add_argument("--voxel_loss_scale", type=float, default=None,
+                    help="its scale in metres, a plane thickness (about 1.5 - 3 point-noise sigmas)")
+
+
+def voxel_loss_arg(ap, a):
+    """The (kind, scale) of add_voxel_loss_args' options, or None."""
+    if a.voxel_loss is None:
+        return None
+    if a.voxel_loss_scale is None:
+        ap.error("--voxel_loss needs --voxel_loss_scale")
+    return a.voxel_loss, a.voxel_loss_scale
+
+
 def _print_trace(trace):
     for i, t in enumerate(trace):  # the line of bavoxel.hpp:1132 / benchmark_virtual.cpp:432
         rho = t["q"] / t["q1"] if t["q1"] != 0 else float("nan")
@@ -95,9 +112,10 @@ def _print_trace(trace):
 
 
 def benchmark_realworld(file_path, voxel_size=2.0, device=0, precision=L.PREC_TENSOR, max_scans=None, quiet=False,
-                        keep_scans=False):
+                        keep_scans=False, voxel_loss=None):
     """file_path: the directory holding alidarPose.csv and full<i>.pcd (the reference appends
-    "/datas/benchmark_realworld/" to its package path, benchmark_realworld.cpp:77).
+    "/datas/benchmark_realworld/" to its package path, benchmark_realworld.cpp:77). voxel_loss: None, or (kind, scale)
+    as Context.set_voxel_loss takes them (a robust voxel cost; the reference has none).
     Returns dict(poses_init, poses, trace, n_voxels, n_obs, seconds) or None when the plane guard fires."""
     say = (lambda *a: None) if quiet else print
     t0 = time.perf_counter()
@@ -114,6 +132,8 @@ def benchmark_realworld(file_path, voxel_size=2.0, device=0, precision=L.PREC_TE
     frame = np.concatenate([np.full(len(s), i, dtype=np.int32) for i, s in enumerate(scans)])
     t_read = time.perf_counter()
     ctx = Context(win_size, device, L.PREC_BLOCKS if win_size >= BLOCKS_MIN_POSES else precision)
+    if voxel_loss is not None:
+        ctx.set_voxel_loss(*voxel_loss)
     try:
         n_vox, n_obs = ctx.cut_voxels(xyz, frame, poses_init, voxel_size=voxel_size, layer_limit=2, min_ps=15,
                                       eigen_value_array=(1.0 / 16, 1.0 / 16, 1.0 / 9))  # :183-185, bavoxel.hpp:8-19

@@ -106,7 +106,7 @@ def fuse_windows(poses_in, poses0, factors, device=0, priors=None):
 
 
 def hba(scans, poses12, length=10, stride=5, downsample=0.1, assoc=None, device=0, top_size=MAX_POSES,
-        pose_graph=False, priors=None, **lm_opts):
+        pose_graph=False, priors=None, voxel_loss=None, **lm_opts):
     """scans: list of (n_s x 3) body-frame points; poses12: P x 12 initial poses. downsample: the keyframes' voxel edge
     (< 0.001: keyframes keep every point); assoc: cut_scans options (DEFAULT_ASSOC when None); lm_opts: damping_iter
     options of every window. Layers are built while more than top_size (<= 32) items remain.
@@ -116,7 +116,9 @@ def hba(scans, poses12, length=10, stride=5, downsample=0.1, assoc=None, device=
     window with at least 2 items, started from the propagated ones; the result then also holds pose_graph = dict(status
     per factor, trace, n_factors, ms). priors (pose_graph only): absolute pose priors by scan index, in
     Context.set_pose_priors' format (e.g. position_priors of GNSS fixes); they join that pose graph, and the final poses
-    are then in the priors' frame rather than re-anchored to scan 0."""
+    are then in the priors' frame rather than re-anchored to scan 0. voxel_loss: None, or (kind, scale) as
+    Batch.set_voxel_loss takes them: a robust voxel cost in every layer's BA, whose weighted H the pose graph's window
+    factors then carry."""
     if priors and not pose_graph:
         raise ValueError("hba: priors join the top pose graph: pass pose_graph=True")
     if not (2 <= length <= MAX_POSES and 1 <= stride <= length and 1 <= top_size <= MAX_POSES):
@@ -130,6 +132,8 @@ def hba(scans, poses12, length=10, stride=5, downsample=0.1, assoc=None, device=
     layers, factors = [], []
     b = Batch(device)
     try:
+        if voxel_loss is not None:
+            b.set_voxel_loss(*voxel_loss)
         while True:
             top = len(items) <= top_size
             windows = [list(range(len(items)))] if top else layer_windows(len(items), length, stride)
@@ -178,6 +182,7 @@ def main(argv=None):
     ap.add_argument("--max_scans", type=int, default=None, help="use only the first scans")
     ap.add_argument("--out", default=None, help="write the refined poses in alidarPose.csv format")
     ap.add_argument("--pose_graph", action="store_true", help="fuse every window's relative poses in a pose graph")
+    drivers.add_voxel_loss_args(ap)
     a = ap.parse_args(argv)
     R, p, _, scans = io.read_realworld_dir(a.file_path, a.max_scans)
     if len(R) == 0:
@@ -188,7 +193,7 @@ def main(argv=None):
     print("The size of poses: %d" % len(R))
     assoc = dict(DEFAULT_ASSOC, voxel_size=a.voxel_size)
     res = hba(scans, drivers.pack_poses(R, p), a.length, a.stride, a.downsample, assoc, a.device, a.top_size,
-              pose_graph=a.pose_graph)
+              pose_graph=a.pose_graph, voxel_loss=drivers.voxel_loss_arg(ap, a))
     for li, lay in enumerate(res["layers"]):
         guard = sum(st == L.ERR_TOO_FEW_PLANES for st in lay["status"])
         print("layer %d: %d windows, %d iterations, voxels %d, keyframe points %s, cut %.1f ms, LM %.1f ms, merge %.1f ms"

@@ -59,7 +59,8 @@ typedef enum {
                            join the voxel cost through balm_block_set_factors. */
 } balm_precision;
 
-/* Robust losses of pose factors (balm_set_factor_loss), rho of s = e~^T H~ e~ at scale c > 0 (units of sqrt(s)). */
+/* Robust losses of pose factors (balm_set_factor_loss), rho of s = e~^T H~ e~ at scale c > 0 (units of sqrt(s)), and of
+ * voxels (balm_set_voxel_loss), rho of s = lambda_min at a scale c in metres. */
 typedef enum {
   BALM_LOSS_TRIVIAL = 0, /* rho = s */
   BALM_LOSS_HUBER = 1,   /* rho = s for s <= c^2, else 2 c sqrt(s) - c^2 */
@@ -137,6 +138,28 @@ int balm_solve(balm_ctx *ctx, double u, double *dx, double *q1, int *not_pd);
 int balm_damping_iter(balm_ctx *ctx, double *poses12, const balm_lm_opts *opts, balm_trace *trace, int *n_iters,
                       double *poses_per_iter);
 void balm_default_lm_opts(balm_lm_opts *opts);
+
+/* Robust voxel cost (DESIGN.md "Robust voxels"): one loss kind (balm_loss) and scale c > 0 in metres -- a plane
+ * thickness -- for every voxel of the context. With s_v = lambda_min(C_v) (m^2) of the cluster the pass builds (its
+ * observations at the given poses, plus the fix cluster exactly where that pass adds it) and w_v = rho'(s_v), voxel v
+ * contributes cost coe_v rho(s_v) (no 1/2: a trivial loss is the plain cost), gradient w_v coe_v grad(lambda_min) and
+ * Hessian w_v times the voxel's Hessian without a loss (iteratively reweighted; the rho'' term is left out). Every H, g
+ * and covariance therefore equals that of a trivial-loss context registered with coe_v w_v, the weights frozen at the
+ * given poses. The loss applies to every call that evaluates voxels: balm_evaluate (any range), balm_residual,
+ * balm_damping_iter, balm_solve, balm_download_blocks, balm_pose_covariance and balm_block_covariance. Useful scales:
+ * inliers with point noise sigma_p have sqrt(lambda_min) slightly below sigma_p, so c = 1.5 - 3 sigma_p.
+ * BALM_LOSS_TRIVIAL resets (scale ignored); a trivial loss's outputs are bitwise those without one. BALM_ERR_INVALID, the
+ * previous loss kept, for a kind outside BALM_LOSS_* or a non-trivial kind without a finite scale > 0. Works on every
+ * precision; the loss belongs to the context and survives every voxel registration (balm_set_voxels, _dev,
+ * balm_cut_voxels, balm_marginalize, balm_append_scan, balm_window_push, balm_synth_virtual, the empty set). With a
+ * communicator attached every rank must set the same loss (it is not checked). */
+int balm_set_voxel_loss(balm_ctx *ctx, int kind, double scale);
+/* s_v = lambda_min and w_v = rho'(s_v) of the voxels [head, end) of this rank at poses12, into lam and w (end - head
+ * each; either may be NULL), with the fix clusters when include_fix. w is bitwise the weight an evaluation at these
+ * poses applies (1 without a loss). Waits once. BALM_ERR_INVALID for a null ctx or poses12, no registered voxels or a
+ * bad range. */
+int balm_voxel_residuals(balm_ctx *ctx, const double *poses12, int64_t head, int64_t end, int include_fix, double *lam,
+                         double *w);
 
 /* Association on the GPU (SURVEY.md section 8f, row N1): raw scans + initial poses -> plane voxels, registered in the
  * ctx exactly as balm_set_voxels would. Replaces the loop  cut_voxel(surf_map, *pl_fulls[i], x_buf[i], i)  over all scans
@@ -237,6 +260,12 @@ int balm_batch_set_voxels(balm_batch *b, int n_problems, const int64_t *pose_ptr
 /* left_evaluate_acc2 per problem, at poses12 (P x 12, P = pose_ptr[B]). H: the problems' full column-major (6N_p)^2
  * blocks one after the other, g: 6P, residual: B. H, g may be NULL. */
 int balm_batch_evaluate(balm_batch *b, const double *poses12, int include_fix, double *H, double *g, double *residual);
+/* balm_set_voxel_loss for a batch: one loss for every voxel of every problem, used by balm_batch_evaluate,
+ * balm_batch_damping_iter and balm_batch_pose_covariance. Same refusals; it belongs to the batch and survives every
+ * registration (set_voxels, cut_voxels, marginalize, append_scan, window_push), whatever the problem count. */
+int balm_batch_set_voxel_loss(balm_batch *b, int kind, double scale);
+/* balm_voxel_residuals over all voxels of the registration, in registration order (voxel_ptr[B] each). */
+int balm_batch_voxel_residuals(balm_batch *b, const double *poses12, int include_fix, double *lam, double *w);
 /* balm_damping_iter per problem, all problems advanced together: each problem's iterations are exactly those of
  * balm_damping_iter on a BALM_PREC_FP64 context holding only that problem (precheck, u0 / v0, accept rule, reused H after a
  * rejected step unless force_hess, rel_tol exit, hess_includes_fix, gauge_mode on the problem's own pose 0). A converged
