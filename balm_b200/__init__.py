@@ -8,6 +8,7 @@ from . import _lib
 from ._lib import PREC_BLOCKS, PREC_FP64, PREC_TENSOR, BalmError
 from .context import Batch, Context, PoseGraph
 from .factors import odometry_factors, pose_priors, position_priors
+from .rig import calibrate_rig, rig_poses
 from . import bavoxel
 from . import shard
 from . import io
@@ -15,5 +16,5 @@ from . import drivers
 from .bavoxel import BALM2, IMUST, VOX_HESS, PointCluster
 
 __all__ = ["Context", "Batch", "PoseGraph", "BALM2", "VOX_HESS", "IMUST", "PointCluster", "PREC_FP64", "PREC_TENSOR", "PREC_BLOCKS",
-           "BalmError", "odometry_factors", "pose_priors", "position_priors",
+           "BalmError", "odometry_factors", "pose_priors", "position_priors", "calibrate_rig", "rig_poses",
            "bavoxel", "shard", "io", "drivers"]

@@ -61,7 +61,8 @@ SYMBOLS = ["balm_last_error", "balm_version", "balm_create", "balm_destroy", "ba
            "balm_block_covariance", "balm_block_set_factors", "balm_set_factor_loss", "balm_factor_residuals",
            "balm_spg_set_factor_loss", "balm_spg_factor_residuals", "balm_set_pose_priors", "balm_prior_residuals",
            "balm_spg_set_pose_priors", "balm_spg_prior_residuals", "balm_set_voxel_loss", "balm_voxel_residuals",
-           "balm_batch_set_voxel_loss", "balm_batch_voxel_residuals"]
+           "balm_batch_set_voxel_loss", "balm_batch_voxel_residuals",
+           "balm_set_rig", "balm_rig_evaluate", "balm_rig_damping_iter"]
 
 
 def lib():
@@ -168,6 +169,11 @@ def lib():
         L.balm_voxel_residuals.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_void_p, C.c_void_p]
         L.balm_batch_set_voxel_loss.argtypes = [C.c_void_p, C.c_int, C.c_double]
         L.balm_batch_voxel_residuals.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
+        L.balm_set_rig.argtypes = [C.c_void_p, C.c_int, C.c_int] + [C.c_void_p] * 4 + [C.POINTER(C.c_int)]
+        L.balm_rig_evaluate.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
+                                        C.POINTER(C.c_double)]
+        L.balm_rig_damping_iter.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(LmOpts), C.c_void_p,
+                                            C.POINTER(C.c_int), C.c_void_p]
         _lib = L
     return _lib
 

@@ -134,6 +134,7 @@ class Context:
         self.n = 6 * self.N
         self._n_factors = 0  # the registered pose factor set's size
         self._n_priors = 0   # the registered pose prior set's size
+        self._rig = None     # (n_base, n_lidar, n_rig) of the rig set by set_rig
         L.check(L.lib().balm_create(C.byref(self._h), self.N, int(device), int(precision)))
 
     def close(self):
@@ -320,6 +321,72 @@ class Context:
         per_iter = np.zeros((max_iter, self.N, 12)) if want_per_iter else None
         L.check(L.lib().balm_damping_iter(self._h, _p(poses), C.byref(opts), trace, C.byref(n_it), _p(per_iter)))
         return poses, _trace_dicts(trace[:n_it.value]), (per_iter[:n_it.value] if want_per_iter else None)
+
+    # ---- rig calibration ----
+    def set_rig(self, base_of, lidar_of, fixed_bases=(), fixed_lidars=(0,)):
+        """Drive the N scan slots by base poses and LiDAR extrinsics (include/balm_b200.h, balm_set_rig): slot s is
+        scanned at T_{base_of[s]} E_{lidar_of[s]}. fixed_bases / fixed_lidars list the unknowns held fixed; the default
+        fixes LiDAR 0 as the reference (the extrinsics' gauge). base_of=None detaches the rig. -> n_rig, 6 x the free
+        unknowns."""
+        n_rig = C.c_int()
+        if base_of is None:
+            L.check(L.lib().balm_set_rig(self._h, 0, 0, None, None, None, None, C.byref(n_rig)))
+            self._rig = None
+            return 0
+        base_of = np.ascontiguousarray(base_of, dtype=np.int32)
+        lidar_of = np.ascontiguousarray(lidar_of, dtype=np.int32)
+        if base_of.shape != (self.N,) or lidar_of.shape != (self.N,):
+            raise ValueError(f"set_rig: base_of and lidar_of need one entry per slot ({self.N})")
+        B = int(base_of.max()) + 1 if self.N else 0
+        nl = int(lidar_of.max()) + 1 if self.N else 0
+        bf = np.zeros(B, dtype=np.uint8)
+        lf = np.zeros(nl, dtype=np.uint8)
+        for name, idx, arr in (("fixed_bases", fixed_bases, bf), ("fixed_lidars", fixed_lidars, lf)):
+            for i in idx:
+                if not 0 <= int(i) < len(arr):
+                    raise ValueError(f"set_rig: {name} entry {i} outside [0, {len(arr)})")
+                arr[int(i)] = 1
+        L.check(L.lib().balm_set_rig(self._h, B, nl, _p(base_of), _p(lidar_of), _p(bf), _p(lf), C.byref(n_rig)))
+        self._rig = (B, nl, n_rig.value)
+        return n_rig.value
+
+    def _rig_shapes(self, base12, ext12):
+        if getattr(self, "_rig", None) is None:
+            raise L.BalmError(L.ERR_INVALID, "no rig set (set_rig)")
+        B, nl, n_rig = self._rig
+        base12 = np.array(base12, dtype=np.float64, order="C", copy=True).reshape(B, 12)
+        ext12 = np.array(ext12, dtype=np.float64, order="C", copy=True).reshape(nl, 12)
+        return base12, ext12, n_rig
+
+    def rig_evaluate(self, base12, ext12, include_fix=False):
+        """-> (H_rig, g_rig, residual) at base poses base12 (B x 12) and extrinsics ext12 (L x 12), the unknowns in
+        set_rig's order: free base poses ascending, then free extrinsics ascending, 6 each."""
+        base12, ext12, n_rig = self._rig_shapes(base12, ext12)
+        H = np.zeros((n_rig, n_rig), order="F")
+        g = np.zeros(n_rig)
+        r = C.c_double()
+        L.check(L.lib().balm_rig_evaluate(self._h, _p(base12), _p(ext12), int(include_fix), _p(H), _p(g), C.byref(r)))
+        return H, g, r.value
+
+    def rig_damping_iter(self, base12, ext12, max_iter=10, u0=0.01, v0=2.0, rel_tol=1e-6, hess_includes_fix=False,
+                         gauge_mode=0, min_planes_per_pose=20, verbose=False, want_per_iter=False, force_hess=False):
+        """damping_iter's LM on the rig's unknowns -> (base12, ext12, trace) and, with want_per_iter, the accepted
+        (base12, ext12) after every iteration as a fourth item. gauge_mode 0 / 1 re-anchor the base poses to base 0
+        (refused while a base pose is fixed: pass 2)."""
+        base12, ext12, _ = self._rig_shapes(base12, ext12)
+        B, nl = len(base12), len(ext12)
+        opts = L.LmOpts(max_iter, u0, v0, rel_tol, int(hess_includes_fix), gauge_mode, min_planes_per_pose,
+                        int(verbose), int(force_hess))
+        trace = (L.Trace * max(1, max_iter))()
+        n_it = C.c_int()
+        per_iter = np.zeros((max_iter, B + nl, 12)) if want_per_iter else None
+        L.check(L.lib().balm_rig_damping_iter(self._h, _p(base12), _p(ext12), C.byref(opts), trace, C.byref(n_it),
+                                              _p(per_iter)))
+        tr = _trace_dicts(trace[:n_it.value])
+        if not want_per_iter:
+            return base12, ext12, tr
+        per = [(p[:B].copy(), p[B:].copy()) for p in per_iter[:n_it.value]]
+        return base12, ext12, tr, per
 
     def marginalize(self, mg_size, poses12, min_ps=15):
         """OCTO_TREE_ROOT::marginalize on the registered voxel set (bavoxel.hpp:948-963, 778-816) -> (n_voxels, n_obs)."""

@@ -237,12 +237,14 @@ extern "C" int balm_destroy(balm_ctx *c) {
   window_free(c->win);
   pose_graph_free(c->pg);
   prior_set_free(c->pr);
+  rig_free(c->rig);
   if (c->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(c->comm);
   if (c->prec == BALM_PREC_BLOCKS) cudaFree(c->g);
   cudaFree(c->poses); cudaFree(c->poses_trial); cudaFree(c->H); cudaFree(c->A);
   cudaFree(c->dx); cudaFree(c->dvec); cudaFree(c->scal); cudaFree(c->flags); cudaFree(c->accum); cudaFree(c->accum_batch);
-  cudaFree(c->vox_key); cudaFree(c->vox_layer); cudaFree(c->res_part); cudaFree(c->planes); cudaFree(c->Xinv); cudaFree(c->dinv); cudaFree(c->sol); cudaFree(c->ysol);
-  cudaFree(c->Hpack); cudaFree(c->dval); cudaFree(c->rres); cudaFree(c->rdelta); cudaFree(c->dag_flags);
+  cudaFree(c->vox_key); cudaFree(c->vox_layer); cudaFree(c->res_part); cudaFree(c->planes);
+  ldlt_work_free(&c->lw);
+  cudaFree(c->Hpack);
   cudaFree(c->tc_trace);
   cudaFreeHost(c->h_scal); cudaFreeHost(c->h_flags);
   for (auto &e : c->ev) if (e) cudaEventDestroy(e);
@@ -778,25 +780,26 @@ static int collect_solve(balm_ctx *c, double *q1, int *not_pd) {
   return BALM_OK;
 }
 
-// The backward-error check of the last solve failed (flags[4]: an indefinite H + uD factored without pivoting lost
-// digits): refine dx in fp64 with the same factors; if that does not bring the error down, the step counts as not_pd.
-// Returns 1 in *refined when dx changed (the caller re-applies the pose update).
-static int maybe_refine(balm_ctx *c, double *q1, int *not_pd, int *refined) {
+// The backward-error check of the last solve of sys failed (flags[4]: an indefinite H + uD factored without pivoting
+// lost digits): refine dx in fp64 with the same factors; if that does not bring the error down, the step counts as
+// not_pd. Returns 1 in *refined when dx changed (the caller re-applies the pose update).
+static int maybe_refine(balm_ctx *c, const DenseSystem &sys, double *q1, int *not_pd, int *refined) {
   *refined = 0;
   if (c->h_flags[4] == 0 || *not_pd) return BALM_OK;
   int still_bad = 0;
   if (c->prec == BALM_PREC_BLOCKS) TRY(blocks_refine(c, &still_bad));
-  else TRY(refine_solution(c, &still_bad));
+  else TRY(refine_solution(c, sys, &still_bad));
   *q1 = c->h_scal[1];
   *refined = 1;
   if (still_bad || !std::isfinite(*q1)) *not_pd = 1;
   return BALM_OK;
 }
 
-static int solve_dev(balm_ctx *c, double u, double *q1, int *not_pd) {
+// The damped solve of sys (the context's own system, or a rig's; a blocks context solves its blocks instead)
+static int solve_dev(balm_ctx *c, const DenseSystem &sys, double u, double *q1, int *not_pd) {
   CUDA_TRY(cudaEventRecord(c->ev[9], c->stream));
   if (c->prec == BALM_PREC_BLOCKS) TRY(blocks_solve(c, u));
-  else TRY(launch_ldlt_solve(c, u));
+  else TRY(launch_ldlt_solve(c, sys, u));
   CUDA_TRY(cudaEventRecord(c->ev[10], c->stream));
   CUDA_TRY(cudaMemcpyAsync(c->h_scal + 1, c->scal + 1, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
   CUDA_TRY(cudaMemcpyAsync(c->h_flags, c->flags, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
@@ -805,7 +808,7 @@ static int solve_dev(balm_ctx *c, double u, double *q1, int *not_pd) {
   CUDA_TRY(cudaStreamSynchronize(c->stream));
   TRY(collect_solve(c, q1, not_pd));
   int refined = 0;
-  return maybe_refine(c, q1, not_pd, &refined);
+  return maybe_refine(c, sys, q1, not_pd, &refined);
 }
 
 extern "C" int balm_solve(balm_ctx *c, double u, double *dx, double *q1, int *not_pd) {
@@ -813,7 +816,7 @@ extern "C" int balm_solve(balm_ctx *c, double u, double *dx, double *q1, int *no
   CUDA_TRY(cudaSetDevice(c->device));
   double q = 0;
   int bad = 0;
-  TRY(solve_dev(c, u, &q, &bad));
+  TRY(solve_dev(c, ctx_system(c), u, &q, &bad));
   if (dx) CUDA_TRY(cudaMemcpy(dx, c->dx, sizeof(double) * c->n, cudaMemcpyDeviceToHost));
   if (q1) *q1 = q;
   if (not_pd) *not_pd = bad;
@@ -914,7 +917,7 @@ extern "C" int balm_damping_iter(balm_ctx *c, double *poses12, const balm_lm_opt
     }
     double q1 = 0;
     int not_pd = 0;
-    if (rc == BALM_OK) rc = solve_dev(c, u, &q1, &not_pd);
+    if (rc == BALM_OK) rc = solve_dev(c, ctx_system(c), u, &q1, &not_pd);
     if (rc == BALM_OK) rc = launch_pose_update(c, c->poses, c->dx, c->poses_trial);
     if (rc == BALM_OK) rc = residual_dev(c, c->poses_trial, &r2, hand_over);  // synchronises the stream
     const bool was_deferred = c->defer;
@@ -924,7 +927,7 @@ extern "C" int balm_damping_iter(balm_ctx *c, double *poses12, const balm_lm_opt
       TRY(collect_eval(c));
       TRY(collect_solve(c, &q1, &not_pd));
       int refined = 0;
-      TRY(maybe_refine(c, &q1, &not_pd, &refined));
+      TRY(maybe_refine(c, ctx_system(c), &q1, &not_pd, &refined));
       if (refined && !not_pd) {  // dx changed: the trial poses and their residual are recomputed (rare path, synchronous)
         TRY(launch_pose_update(c, c->poses, c->dx, c->poses_trial));
         TRY(residual_dev(c, c->poses_trial, &r2, hand_over));
@@ -1179,15 +1182,184 @@ extern "C" int balm_pose_graph_iter(balm_ctx *c, double *poses12, const balm_lm_
     double q1 = 0;
     int not_pd = 0;
     c->defer = true;
-    const int rc = solve_dev(c, u, &q1, &not_pd);
+    const int rc = solve_dev(c, ctx_system(c), u, &q1, &not_pd);
     c->defer = false;
     return rc;
   };
   s.finish = [c](double *q1, int *not_pd, int *refined) -> int {
     TRY(collect_solve(c, q1, not_pd));
-    return maybe_refine(c, q1, not_pd, refined);
+    return maybe_refine(c, ctx_system(c), q1, not_pd, refined);
   };
   return pose_graph_lm(s, poses12, o, trace, n_iters, poses_per_iter);
+}
+
+// ---------------- rig calibration (rig.cu) ----------------
+extern "C" int balm_set_rig(balm_ctx *c, int n_base, int n_lidar, const int32_t *base_of, const int32_t *lidar_of,
+                            const uint8_t *base_fixed, const uint8_t *lidar_fixed, int *n_rig_out) {
+  const std::string w = "balm_set_rig: ";
+  if (!c) { balm_set_error(w + "bad arguments"); return BALM_ERR_INVALID; }
+  if (c->prec == BALM_PREC_BLOCKS) {
+    balm_set_error(w + "not available on a BALM_PREC_BLOCKS context (it holds no dense H)");
+    return BALM_ERR_UNSUPPORTED;
+  }
+  if (c->world > 1 || c->comm) { balm_set_error(w + "single-GPU contexts only"); return BALM_ERR_INVALID; }
+  CUDA_TRY(cudaSetDevice(c->device));
+  if (n_base == 0) {  // detach
+    rig_free(c->rig);
+    c->rig = nullptr;
+    if (n_rig_out) *n_rig_out = 0;
+    return BALM_OK;
+  }
+  if (n_base < 0 || n_lidar < 1 || !base_of || !lidar_of) { balm_set_error(w + "bad arguments"); return BALM_ERR_INVALID; }
+  std::vector<char> base_used((size_t)n_base, 0), lidar_used((size_t)n_lidar, 0);
+  for (int s = 0; s < c->N; s++) {
+    if (base_of[s] < 0 || base_of[s] >= n_base || lidar_of[s] < 0 || lidar_of[s] >= n_lidar) {
+      balm_set_error(w + "slot " + std::to_string(s) + " has base " + std::to_string(base_of[s]) + " / lidar " +
+                     std::to_string(lidar_of[s]) + " outside [0, n_base) / [0, n_lidar)");
+      return BALM_ERR_INVALID;
+    }
+    base_used[base_of[s]] = 1;
+    lidar_used[lidar_of[s]] = 1;
+  }
+  for (int b = 0; b < n_base; b++)
+    if (!base_used[b]) { balm_set_error(w + "no slot uses base " + std::to_string(b)); return BALM_ERR_INVALID; }
+  for (int l = 0; l < n_lidar; l++)
+    if (!lidar_used[l]) { balm_set_error(w + "no slot uses lidar " + std::to_string(l)); return BALM_ERR_INVALID; }
+  int n_free = 0;
+  for (int b = 0; b < n_base; b++) n_free += !(base_fixed && base_fixed[b]);
+  for (int l = 0; l < n_lidar; l++) n_free += !(lidar_fixed && lidar_fixed[l]);
+  if (n_free == 0) { balm_set_error(w + "every base pose and extrinsic is fixed"); return BALM_ERR_INVALID; }
+  Rig *r = nullptr;
+  const int rc = rig_build(c->stream, c->N, n_base, n_lidar, base_of, lidar_of, base_fixed, lidar_fixed, &r);
+  if (rc != BALM_OK) {
+    cudaGetLastError();  // an out-of-memory allocation must not fail the next launch check; the previous rig stays
+    return rc;
+  }
+  rig_free(c->rig);
+  c->rig = r;
+  if (n_rig_out) *n_rig_out = rig_n(r);
+  return BALM_OK;
+}
+
+// uploads base12 / ext12 into the rig's current state
+static int rig_upload(balm_ctx *c, const double *base12, const double *ext12) {
+  Rig *r = c->rig;
+  double *st = rig_state(r, false);
+  const int B = rig_bases(r), L = rig_lidars(r);
+  CUDA_TRY(cudaMemcpyAsync(st, base12, sizeof(double) * 12 * B, cudaMemcpyHostToDevice, c->stream));
+  CUDA_TRY(cudaMemcpyAsync(st + 12 * (size_t)B, ext12, sizeof(double) * 12 * L, cudaMemcpyHostToDevice, c->stream));
+  return BALM_OK;
+}
+
+// compose, evaluate every voxel and reduce to H_rig | g_rig at the rig's current state; the residual in c->scal[0].
+// The reduction's time joins ms_assemble.
+static int rig_evaluate_dev(balm_ctx *c, bool include_fix) {
+  Rig *r = c->rig;
+  const double *st = rig_state(r, false);
+  TRY(rig_compose(r, c->stream, st, c->poses, &c->launches));
+  TRY(evaluate_dev(c, c->poses, 0, c->M, include_fix));
+  CUDA_TRY(cudaEventRecord(c->ev[13], c->stream));
+  TRY(rig_reduce(r, c->stream, st, c->H, c->g, &c->launches));
+  CUDA_TRY(cudaEventRecord(c->ev[14], c->stream));
+  return BALM_OK;
+}
+
+static int rig_collect_reduce(balm_ctx *c) {
+  float ms;
+  CUDA_TRY(cudaEventElapsedTime(&ms, c->ev[13], c->ev[14]));
+  c->tm.ms_assemble += ms;
+  return BALM_OK;
+}
+
+static int rig_check(balm_ctx *c, const char *who) {
+  if (!c->rig) { balm_set_error(std::string(who) + ": no rig set (balm_set_rig)"); return BALM_ERR_INVALID; }
+  // balm_comm_init may attach a communicator after balm_set_rig: the rig calls stay single-GPU
+  if (c->world > 1 || c->comm) { balm_set_error(std::string(who) + ": single-GPU contexts only"); return BALM_ERR_INVALID; }
+  if (!c->registered) { balm_set_error("no voxels registered"); return BALM_ERR_INVALID; }
+  return BALM_OK;
+}
+
+extern "C" int balm_rig_evaluate(balm_ctx *c, const double *base12, const double *ext12, int include_fix, double *H,
+                                 double *g, double *residual) {
+  if (!c || !base12 || !ext12) { balm_set_error("balm_rig_evaluate: bad arguments"); return BALM_ERR_INVALID; }
+  TRY(rig_check(c, "balm_rig_evaluate"));
+  CUDA_TRY(cudaSetDevice(c->device));
+  TRY(rig_upload(c, base12, ext12));
+  TRY(rig_evaluate_dev(c, include_fix != 0));
+  const DenseSystem sys = rig_system(c->rig);
+  const size_t nr = sys.n;
+  if (H) CUDA_TRY(cudaMemcpyAsync(H, sys.H, sizeof(double) * nr * nr, cudaMemcpyDeviceToHost, c->stream));
+  if (g) CUDA_TRY(cudaMemcpyAsync(g, sys.g, sizeof(double) * nr, cudaMemcpyDeviceToHost, c->stream));
+  CUDA_TRY(cudaMemcpyAsync(c->h_scal, c->scal, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+  CUDA_TRY(cudaStreamSynchronize(c->stream));
+  TRY(rig_collect_reduce(c));
+  if (residual) *residual = c->h_scal[0];
+  return BALM_OK;
+}
+
+// balm_damping_iter's rule on the rig cost: per iteration compose -> evaluate -> reduce -> solve -> rig update ->
+// compose the trial state -> trial residual; H_rig is reused after a rejected step unless force_hess.
+extern "C" int balm_rig_damping_iter(balm_ctx *c, double *base12, double *ext12, const balm_lm_opts *o,
+                                     balm_trace *trace, int *n_iters, double *rig_per_iter) {
+  const char *who = "balm_rig_damping_iter";
+  if (!c || !base12 || !ext12 || !o) { balm_set_error(std::string(who) + ": bad arguments"); return BALM_ERR_INVALID; }
+  if (n_iters) *n_iters = 0;
+  TRY(rig_check(c, who));
+  Rig *rg = c->rig;
+  if ((o->gauge_mode == 0 || o->gauge_mode == 1) && rig_any_base_fixed(rg)) {
+    balm_set_error(std::string(who) + ": gauge_mode " + std::to_string(o->gauge_mode) +
+                   " re-anchors to base pose 0, which moves the result off the fixed base poses; pass gauge_mode 2");
+    return BALM_ERR_INVALID;
+  }
+  if (o->min_planes_per_pose > 0 && c->min_planes < o->min_planes_per_pose) {  // per scan slot, as balm_damping_iter
+    balm_set_error("Initial error too large. Please loose plane determination criteria for more planes.");
+    return BALM_ERR_TOO_FEW_PLANES;
+  }
+  CUDA_TRY(cudaSetDevice(c->device));
+  TRY(rig_upload(c, base12, ext12));
+  const int B = rig_bases(rg), U = B + rig_lidars(rg);
+  const size_t sbytes = sizeof(double) * 12 * U;
+  const DenseSystem sys = rig_system(rg);
+  double u = o->u0, v = o->v0, r1 = 0, r2 = 0;
+  bool calc_hess = true;
+  for (int it = 0; it < o->max_iter; it++) {
+    if (calc_hess) {
+      TRY(rig_evaluate_dev(c, o->hess_includes_fix != 0));
+      CUDA_TRY(cudaMemcpyAsync(c->h_scal, c->scal, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+    }
+    double q1 = 0;
+    int not_pd = 0;
+    TRY(solve_dev(c, sys, u, &q1, &not_pd));  // waits, and refines dx when the backward-error check asks for it
+    if (calc_hess) {
+      TRY(rig_collect_reduce(c));
+      r1 = c->h_scal[0];
+    }
+    TRY(rig_update(rg, c->stream, rig_state(rg, false), rig_state(rg, true), &c->launches));
+    TRY(rig_compose(rg, c->stream, rig_state(rg, true), c->poses_trial, &c->launches));
+    TRY(residual_dev(c, c->poses_trial, &r2));
+    balm_trace t;
+    if (lm_rule(o, it, r1, r2, q1, not_pd, calc_hess, &u, &v, &t)) {
+      rig_swap_states(rg);
+      calc_hess = true;
+    } else {
+      calc_hess = o->force_hess != 0;  // H_rig and g_rig of the current state are still in place
+    }
+    if (trace) trace[it] = t;
+    if (rig_per_iter)
+      CUDA_TRY(cudaMemcpyAsync(rig_per_iter + (size_t)it * 12 * U, rig_state(rg, false), sbytes, cudaMemcpyDeviceToHost,
+                               c->stream));
+    if (n_iters) *n_iters = it + 1;
+    if (o->rel_tol >= 0 && fabs(r1 - r2) / r1 < o->rel_tol) break;
+  }
+  if (o->gauge_mode == 0 || o->gauge_mode == 1) {  // base poses re-anchored to base 0; extrinsics are body-frame
+    c->launches += 1;
+    TRY(launch_gauge(c->stream, B, rig_state(rg, false), c->scal + 4, o->gauge_mode));
+  }
+  const double *st = rig_state(rg, false);
+  CUDA_TRY(cudaMemcpyAsync(base12, st, sizeof(double) * 12 * B, cudaMemcpyDeviceToHost, c->stream));
+  CUDA_TRY(cudaMemcpyAsync(ext12, st + 12 * (size_t)B, sizeof(double) * 12 * (U - B), cudaMemcpyDeviceToHost, c->stream));
+  CUDA_TRY(cudaStreamSynchronize(c->stream));
+  return BALM_OK;
 }
 
 // ---------------- sparse pose graph (pose_graph.cu, pose_graph_sparse.cu) ----------------
@@ -1792,10 +1964,10 @@ extern "C" int balm_timer_end(balm_ctx *c, float *ms) {
 // Debug aid (BALM_DAG_TRACE=1): timestamps of the last tile-DAG factorisation. out: 4*nt chain entries (step start,
 // mini-panel inputs ready, diagonal block ready, step published; ns) followed by 3 per CTA (start, end, tasks).
 extern "C" int balm_debug_dag_trace(balm_ctx *c, unsigned long long *out, int max_entries) {
-  if (!c || !out || !c->dag_trace) return BALM_ERR_INVALID;
+  if (!c || !out || !c->lw.dag_trace) return BALM_ERR_INVALID;
   const int nt = (c->n + BALM_NB - 1) / BALM_NB;
   const int total = std::min(max_entries, 4 * nt + 8 * 1024);
-  CUDA_TRY(cudaMemcpy(out, c->dag_trace, sizeof(unsigned long long) * total, cudaMemcpyDeviceToHost));
+  CUDA_TRY(cudaMemcpy(out, c->lw.dag_trace, sizeof(unsigned long long) * total, cudaMemcpyDeviceToHost));
   return BALM_OK;
 }
 

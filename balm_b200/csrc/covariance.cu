@@ -216,17 +216,17 @@ int solve_many(balm_ctx *c, double *B) {
   int launches = 0;
   for (int j0 = 0, pi = 0; j0 < n; j0 += NB, pi++) {
     const int nbw = std::min(NB, n - j0), m = n - j0 - nbw;
-    mrhs_diag_kernel<0><<<ct, 256, MRHS_SMEM, st>>>(c->Xinv + (size_t)pi * NB * NB, B, n, j0, nbw, nullptr);
+    mrhs_diag_kernel<0><<<ct, 256, MRHS_SMEM, st>>>(c->lw.Xinv + (size_t)pi * NB * NB, B, n, j0, nbw, nullptr);
     if (m > 0) mrhs_fwd_update_kernel<<<dim3((m + NB - 1) / NB, ct), 256, MRHS_SMEM, st>>>(c->A, B, n, j0, nbw);
     launches += 2;
   }
-  scale_rows_kernel<<<dim3((n + 255) / 256, n), 256, 0, st>>>(B, c->dinv, n);
+  scale_rows_kernel<<<dim3((n + 255) / 256, n), 256, 0, st>>>(B, c->lw.dinv, n);
   launches++;
   const int npan = (n + NB - 1) / NB;
   for (int pi = npan - 1; pi >= 0; pi--) {
     const int j0 = pi * NB, nbw = std::min(NB, n - j0);
     if (j0 + nbw < n) mrhs_bwd_update_kernel<<<ct, 256, MRHS_SMEM, st>>>(c->A, B, n, j0, nbw);
-    mrhs_diag_kernel<1><<<ct, 256, MRHS_SMEM, st>>>(c->Xinv + (size_t)pi * NB * NB, B, n, j0, nbw, nullptr);
+    mrhs_diag_kernel<1><<<ct, 256, MRHS_SMEM, st>>>(c->lw.Xinv + (size_t)pi * NB * NB, B, n, j0, nbw, nullptr);
     launches += 2;
   }
   c->launches += launches;
@@ -294,13 +294,13 @@ int pose_covariance_dev(balm_ctx *c, const double *poses_dev, const double *ccov
   if (Rcov_host) {
     // H at these poses (divide_thread, BAs_left.hpp:1091), factored without damping, then H^-1 R H^-T
     TRY(balm_cov_evaluate_hessian(c, poses_dev, include_fix));
-    TRY(launch_ldlt_solve(c, 0.0));
+    TRY(launch_ldlt_solve(c, ctx_system(c), 0.0));
     CUDA_TRY(cudaMemcpyAsync(c->h_flags, c->flags, sizeof(int), cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
     // a singular H (free gauge: no fix clusters in it) does not produce an exact zero pivot in floating point but
     // pivots at rounding level relative to the others: refuse instead of returning 1e16-sized garbage
     std::vector<double> dinv_h((size_t)n);
-    CUDA_TRY(cudaMemcpy(dinv_h.data(), c->dinv, sizeof(double) * n, cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(dinv_h.data(), c->lw.dinv, sizeof(double) * n, cudaMemcpyDeviceToHost));
     double dmin = 1e300, dmax = 0.0;
     for (int i = 0; i < n; i++) { const double d = fabs(1.0 / dinv_h[i]); dmin = std::min(dmin, d); dmax = std::max(dmax, d); }
     if (c->h_flags[0] || !(dmin > 1e-11 * dmax)) {

@@ -37,6 +37,8 @@ struct BlockHessian;  // the block pattern of a BALM_PREC_BLOCKS context (blocks
 void block_hessian_free(BlockHessian *b);
 struct PriorSet;      // the registered absolute pose priors (pose_graph.cu)
 void prior_set_free(PriorSet *p);
+struct Rig;           // balm_set_rig's slot assignment, unknowns and reduced system (rig.cu)
+void rig_free(Rig *r);
 
 #define CUDA_TRY(expr)                                                                        \
   do {                                                                                        \
@@ -85,10 +87,32 @@ struct ScratchPool {
   }
 };
 
+// The workspaces of the dense LDL^T solve of one system of order n (ldlt.cu allocates them on the system's first solve).
+struct LdltWork {
+  double *Xinv = nullptr;                   // [panels][64*64] inverses of the unit-lower diagonal blocks
+  double *dinv = nullptr;                   // [n] 1/d
+  double *dval = nullptr;                   // [n] d (the tile-DAG factorisation scales its operands with it)
+  double *sol = nullptr;                    // [n] right-hand side / forward-substitution vector
+  double *ysol = nullptr;                   // [n] forward-substitution result y (kept apart from the running rhs `sol`)
+  double *rres = nullptr;                   // [n] residual b - A x of the last solve (backward-error check)
+  double *rdelta = nullptr;                 // [n] refinement correction
+  int *dag_flags = nullptr;                 // tile-DAG dependency counters: upd | pdone [nt*nt], xdone | rhs_cnt [nt]
+  unsigned long long *dag_trace = nullptr;  // BALM_DAG_TRACE: device timestamps of the last factorisation
+};
+void ldlt_work_free(LdltWork *w);
+
+// One damped system (H + u diag(H)) dx = -g of order n (H column-major n x n): the context's own, or a rig's reduced
+// one. The solve factors into A [n*n] and w, writes dvec = diag(H) and dx, and uses the context's scal / flags.
+struct DenseSystem {
+  int n;
+  const double *H, *g;
+  double *dx, *dvec, *A;
+  LdltWork *w;
+};
+
 struct balm_ctx {
   int N = 0, n = 0, ldg = 0, Np = 0, device = 0, prec = 0;
   cudaStream_t stream = nullptr;
-  double *ysol = nullptr;          // [n] forward-substitution result y (kept apart from the running rhs `sol`)
   bool lm_active = false;     // inside balm_damping_iter (scale speculation and stats hand-over are loop-local)
   bool reuse_ws = false;      // the registration in progress has the shape of the previous one: buffers are kept
   bool defer = false;         // inside balm_damping_iter: phases are enqueued back to back, one host sync per iteration
@@ -126,6 +150,7 @@ struct balm_ctx {
                                   // the pose-graph cost, and on BALM_PREC_BLOCKS of every full-range evaluation
   int vloss_kind = BALM_LOSS_TRIVIAL;  // balm_set_voxel_loss: the loss of every voxel (independent of the voxel set)
   double vloss_scale = 1.0;
+  Rig *rig = nullptr;             // balm_set_rig's rig (independent of the voxel set: N is fixed at creation)
 
   // ---- optimiser state (device) ----
   double *poses = nullptr, *poses_trial = nullptr;  // [12N]
@@ -134,14 +159,7 @@ struct balm_ctx {
   double *A = nullptr;                              // [n*n] factor workspace (none in BALM_PREC_BLOCKS)
   double *dx = nullptr;                             // [n]
   double *dvec = nullptr;                           // [n] diag(H)
-  double *Xinv = nullptr;                           // [panels][64*64] inverses of the unit-lower diagonal blocks
-  double *dinv = nullptr;                           // [n] 1/d
-  double *sol = nullptr;                            // [n] right-hand side / forward-substitution vector
-  double *dval = nullptr;                           // [n] d (the tile-DAG factorisation scales its operands with it)
-  double *rres = nullptr;                           // [n] residual b - A x of the last solve (backward-error check)
-  double *rdelta = nullptr;                         // [n] refinement correction
-  int *dag_flags = nullptr;                         // tile-DAG dependency counters: upd | pdone [nt*nt], xdone | rhs_cnt [nt]
-  unsigned long long *dag_trace = nullptr;          // BALM_DAG_TRACE: device timestamps of the last factorisation
+  LdltWork lw;                                      // the factor workspaces of the solve of H
   unsigned long long *tc_trace = nullptr;           // BALM_TC_TRACE: per-CTA clocks of the last tensor SYRK launch
   double *scal = nullptr;                           // device scalars [32]: 0 r(eval) 1 q1 2 r(residual) 3 u 4..15 gauge
                                                     // snapshot, 16/17 this rank's residual at the current / trial poses
@@ -777,8 +795,13 @@ int launch_syrk_f64(balm_ctx *c, int64_t rows, bool first_batch);
 int launch_assemble(balm_ctx *c, const double *Dacc = nullptr, double *R = nullptr);
 int build_pose_major_lists(balm_ctx *c, const int *planes_host);
 int launch_csc_batch(balm_ctx *c, int64_t v0, int64_t v1);
-int launch_ldlt_solve(balm_ctx *c, double u);
-int refine_solution(balm_ctx *c, int *still_bad);
+// the context's own system: c->n, c->H, c->g, c->dx, c->dvec, c->A, c->lw
+inline DenseSystem ctx_system(balm_ctx *c) { return DenseSystem{c->n, c->H, c->g, c->dx, c->dvec, c->A, &c->lw}; }
+// (H + u diag(H)) dx = -g of s with u into scal[3], q1 into scal[1], flags[0] bad pivot, flags[4] backward-error check
+// failed (enqueued; allocates s.w on its first call)
+int launch_ldlt_solve(balm_ctx *c, const DenseSystem &s, double u);
+// fp64 iterative refinement of s.dx with the factors of the last launch_ldlt_solve of s (waits)
+int refine_solution(balm_ctx *c, const DenseSystem &s, int *still_bad);
 int launch_pose_update(balm_ctx *c, const double *poses_in, const double *dx, double *poses_out);
 int launch_pose_update(cudaStream_t st, int N, const double *poses_in, const double *dx, double *poses_out);
 int launch_gauge(balm_ctx *c, double *poses, int mode);
@@ -858,6 +881,29 @@ int prior_add_cost(const PriorSet *p, cudaStream_t st, const double *poses, doub
 // balm_prior_residuals: s and rho'(s) of every prior (0 for NOT_PD ones) into the host arrays s, w [n] (either may be
 // null); waits once
 int prior_residuals(const PriorSet *p, cudaStream_t st, const double *poses, double *s, double *w, long long *launches);
+
+// ---------------- rig (rig.cu) ----------------
+// After the argument checks: the rig of N slots (base_of / lidar_of [N] host, base_fixed [B] / lidar_fixed [L] host or
+// null: none fixed), its slot tables and the buffers of its reduced system -> a new rig in *out (waits)
+int rig_build(cudaStream_t st, int N, int B, int L, const int32_t *base_of, const int32_t *lidar_of,
+              const uint8_t *base_fixed, const uint8_t *lidar_fixed, Rig **out);
+int rig_n(const Rig *r);  // n_rig = 6 x free unknowns
+int rig_bases(const Rig *r);
+int rig_lidars(const Rig *r);
+bool rig_any_base_fixed(const Rig *r);
+// the reduced system H_rig | g_rig, dx, and the rig's own factor workspaces
+DenseSystem rig_system(Rig *r);
+// device [12 (B + L)] base poses then extrinsics: the current state, or the trial one; rig_swap_states exchanges them
+double *rig_state(Rig *r, bool trial);
+void rig_swap_states(Rig *r);
+// the scan poses X_s = T_base_of[s] E_lidar_of[s] of every slot into poses [12N] (enqueued)
+int rig_compose(const Rig *r, cudaStream_t st, const double *state, double *poses, long long *launches);
+// H_rig and g_rig at state from the context's H [6N x 6N] and g [6N] (enqueued): K = H J, then J^T K on the lower
+// blocks plus the second-order correction, each sum in ascending slot order, mirrored; no atomics
+int rig_reduce(const Rig *r, cudaStream_t st, const double *state, const double *H, const double *g,
+               long long *launches);
+// state_out = the left step of the rig's dx on every free unknown of state, fixed ones copied (enqueued)
+int rig_update(const Rig *r, cudaStream_t st, const double *state, double *state_out, long long *launches);
 
 // ---------------- sparse pose graph (pose_graph_sparse.cu) ----------------
 struct SparseSolver;  // nested-dissection ordering, symbolic factorisation and the per-solve CUDA graph

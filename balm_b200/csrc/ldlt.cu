@@ -735,42 +735,43 @@ __global__ void gauge_kernel(double *poses, const double *pose0_snapshot, int N,
 
 }  // namespace
 
-// omega of the current c->dx (+ the residual vector in c->rres); flags[4] raised when omega > tol. scal[20] = omega.
-static int enqueue_solve_check(balm_ctx *c) {
-  const int n = c->n;
+// omega of the current s.dx (+ the residual vector in s.w->rres); flags[4] raised when omega > tol. scal[20] = omega.
+static int enqueue_solve_check(balm_ctx *c, const DenseSystem &s) {
+  const int n = s.n;
   CUDA_TRY(cudaMemsetAsync(c->scal + 20, 0, sizeof(double), c->stream));
-  solve_residual_kernel<<<(n + 7) / 8, 256, 0, c->stream>>>(c->H, c->g, c->dx, n, c->scal + 3, SOLVE_OMEGA_TOL, c->rres,
+  solve_residual_kernel<<<(n + 7) / 8, 256, 0, c->stream>>>(s.H, s.g, s.dx, n, c->scal + 3, SOLVE_OMEGA_TOL, s.w->rres,
                                                             c->flags, c->scal + 20);
   c->launches += 1;
   return BALM_OK;
 }
 
-static int enqueue_back_substitution(balm_ctx *c, const double *rhs_g, double *x_out, bool with_q1);
+static int enqueue_back_substitution(balm_ctx *c, const DenseSystem &s, const double *rhs_g, double *x_out, bool with_q1);
 
-// fp64 iterative refinement of c->dx with the factors left in c->A / c->Xinv / c->dinv (host-driven, rare path: the
+// fp64 iterative refinement of s.dx with the factors left in s.A / s.w->Xinv / s.w->dinv (host-driven, rare path: the
 // backward-error check of the last solve raised flags[4]). Returns via *still_bad whether omega stayed above the tolerance.
-int refine_solution(balm_ctx *c, int *still_bad) {
-  const int n = c->n;
+int refine_solution(balm_ctx *c, const DenseSystem &s, int *still_bad) {
+  const int n = s.n;
+  LdltWork &w = *s.w;
   cudaStream_t st = c->stream;
   *still_bad = 1;
   for (int round = 0; round < 3; round++) {
     // solve A delta = r with the existing factors: forward (block by block), scale, backward
-    copy_kernel<<<(n + 255) / 256, 256, 0, st>>>(c->sol, c->rres, n);
+    copy_kernel<<<(n + 255) / 256, 256, 0, st>>>(w.sol, w.rres, n);
     int launches = 1;
     for (int j0 = 0, pi = 0; j0 < n; j0 += NB, pi++) {
       const int nbw = (n - j0 < NB) ? n - j0 : NB;
       const int m = n - j0 - nbw;
-      ldl_fwd_block_kernel<<<m > 0 ? (m + 255) / 256 : 1, 256, 0, st>>>(c->A, n, j0, nbw, c->Xinv + (size_t)pi * NB * NB,
-                                                                        c->sol, c->ysol);
+      ldl_fwd_block_kernel<<<m > 0 ? (m + 255) / 256 : 1, 256, 0, st>>>(s.A, n, j0, nbw, w.Xinv + (size_t)pi * NB * NB,
+                                                                        w.sol, w.ysol);
       launches++;
     }
     c->launches += launches;
-    TRY(enqueue_back_substitution(c, c->g, c->rdelta, false));
-    axpy_kernel<<<(n + 255) / 256, 256, 0, st>>>(c->dx, c->rdelta, n);
-    q1_kernel<<<1, 1024, 0, st>>>(c->dx, c->g, c->dvec, n, c->scal + 3, c->scal);
+    TRY(enqueue_back_substitution(c, s, s.g, w.rdelta, false));
+    axpy_kernel<<<(n + 255) / 256, 256, 0, st>>>(s.dx, w.rdelta, n);
+    q1_kernel<<<1, 1024, 0, st>>>(s.dx, s.g, s.dvec, n, c->scal + 3, c->scal);
     c->launches += 2;
     CUDA_TRY(cudaMemsetAsync(c->flags + 4, 0, sizeof(int), st));
-    TRY(enqueue_solve_check(c));
+    TRY(enqueue_solve_check(c, s));
     CUDA_TRY(cudaMemcpyAsync(c->h_flags + 4, c->flags + 4, sizeof(int), cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaMemcpyAsync(c->h_scal + 1, c->scal + 1, sizeof(double), cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
@@ -781,10 +782,11 @@ int refine_solution(balm_ctx *c, int *still_bad) {
 }
 
 // Everything of the solve that follows the factorisation: w = d^-1 y, grouped backward substitution, q1.
-static int enqueue_back_substitution(balm_ctx *c, const double *rhs_g, double *x_out, bool with_q1) {
-  const int n = c->n;
+static int enqueue_back_substitution(balm_ctx *c, const DenseSystem &s, const double *rhs_g, double *x_out, bool with_q1) {
+  const int n = s.n;
+  const LdltWork &w = *s.w;
   cudaStream_t st = c->stream;
-  scale_rhs_kernel<<<(n + 255) / 256, 256, 0, st>>>(c->sol, c->ysol, c->dinv, n);
+  scale_rhs_kernel<<<(n + 255) / 256, 256, 0, st>>>(w.sol, w.ysol, w.dinv, n);
   int launches = 1;
   const int npan = (n + NB - 1) / NB;
   for (int hi = npan - 1; hi >= 0; hi -= BACK_GROUP) {
@@ -792,11 +794,11 @@ static int enqueue_back_substitution(balm_ctx *c, const double *rhs_g, double *x
     const int g_lo = lo * NB;
     const int g_hi = (hi + 1) * NB < n ? (hi + 1) * NB : n;
     const int blocks = g_lo > 0 ? (g_lo + 31) / 32 : 1;
-    ldl_back_kernel<<<blocks, 256, 0, st>>>(c->A, n, g_lo, g_hi - g_lo, c->Xinv + (size_t)lo * NB * NB, c->sol, x_out);
+    ldl_back_kernel<<<blocks, 256, 0, st>>>(s.A, n, g_lo, g_hi - g_lo, w.Xinv + (size_t)lo * NB * NB, w.sol, x_out);
     launches++;
   }
   if (with_q1) {
-    q1_kernel<<<1, 1024, 0, st>>>(x_out, rhs_g, c->dvec, n, c->scal + 3, c->scal);
+    q1_kernel<<<1, 1024, 0, st>>>(x_out, rhs_g, s.dvec, n, c->scal + 3, c->scal);
     launches++;
   }
   c->launches += launches;
@@ -805,51 +807,59 @@ static int enqueue_back_substitution(balm_ctx *c, const double *rhs_g, double *x
 
 // The damped solve: damp/copy + rhs, ONE cooperative launch for the factorisation and forward substitution,
 // then the grouped backward substitution, q1 and the backward-error check.
-static int enqueue_solve_dag(balm_ctx *c) {
-  const int n = c->n, nt = (n + NB - 1) / NB;
+static int enqueue_solve_dag(balm_ctx *c, const DenseSystem &s) {
+  const int n = s.n, nt = (n + NB - 1) / NB;
+  const LdltWork &w = *s.w;
   cudaStream_t st = c->stream;
   dim3 g1((n + 255) / 256, n);
-  damp_copy_kernel<<<g1, 256, 0, st>>>(c->H, c->A, c->dvec, n, c->scal + 3);
-  rhs_init_kernel<<<(n + 255) / 256, 256, 0, st>>>(c->g, c->sol, n);
-  CUDA_TRY(cudaMemsetAsync(c->dag_flags, 0, sizeof(int) * (2 * (size_t)nt * nt + 2 * nt), st));
+  damp_copy_kernel<<<g1, 256, 0, st>>>(s.H, s.A, s.dvec, n, c->scal + 3);
+  rhs_init_kernel<<<(n + 255) / 256, 256, 0, st>>>(s.g, w.sol, n);
+  CUDA_TRY(cudaMemsetAsync(w.dag_flags, 0, sizeof(int) * (2 * (size_t)nt * nt + 2 * nt), st));
   dag::Args a;
-  a.A = c->A; a.n = n; a.nt = nt; a.Xinv = c->Xinv; a.dinv = c->dinv; a.dval = c->dval; a.sol = c->sol; a.ysol = c->ysol;
-  a.flags = c->flags; a.upd = c->dag_flags; a.pdone = c->dag_flags + (size_t)nt * nt;
-  a.xdone = c->dag_flags + 2 * (size_t)nt * nt; a.rhs_cnt = a.xdone + nt;
+  a.A = s.A; a.n = n; a.nt = nt; a.Xinv = w.Xinv; a.dinv = w.dinv; a.dval = w.dval; a.sol = w.sol; a.ysol = w.ysol;
+  a.flags = c->flags; a.upd = w.dag_flags; a.pdone = w.dag_flags + (size_t)nt * nt;
+  a.xdone = w.dag_flags + 2 * (size_t)nt * nt; a.rhs_cnt = a.xdone + nt;
   // one CTA per SM (216 KB of shared memory each); a grid that cannot be co-resident makes the cooperative launch fail
   const int grid = nt < 2 ? 1 : c->sm_count;
   const int workers = grid - 1;
   a.near_ctas = workers >= 16 ? 8 : 0;
-  a.trace = c->dag_trace;
+  a.trace = w.dag_trace;
   void *params[] = {&a};
   CUDA_TRY(cudaLaunchCooperativeKernel((const void *)dag::ldl_dag_kernel, dim3(grid), dim3(256), params,
                                        dag::SMEM_DOUBLES * sizeof(double), st));
   c->launches += 3;
-  return enqueue_back_substitution(c, c->g, c->dx, true);
+  return enqueue_back_substitution(c, s, s.g, s.dx, true);
 }
 
-int launch_ldlt_solve(balm_ctx *c, double u) {
-  const int n = c->n;
-  if (!c->Xinv) {
+void ldlt_work_free(LdltWork *w) {
+  cudaFree(w->Xinv); cudaFree(w->dinv); cudaFree(w->dval); cudaFree(w->sol); cudaFree(w->ysol); cudaFree(w->rres);
+  cudaFree(w->rdelta); cudaFree(w->dag_flags); cudaFree(w->dag_trace);
+  *w = LdltWork{};
+}
+
+int launch_ldlt_solve(balm_ctx *c, const DenseSystem &s, double u) {
+  const int n = s.n;
+  LdltWork &w = *s.w;
+  if (!w.Xinv) {
     const int npan = (n + NB - 1) / NB;
-    CUDA_TRY(cudaMalloc((void **)&c->Xinv, sizeof(double) * (size_t)npan * NB * NB));
-    CUDA_TRY(cudaMalloc((void **)&c->dinv, sizeof(double) * n));
-    CUDA_TRY(cudaMalloc((void **)&c->dval, sizeof(double) * n));
-    CUDA_TRY(cudaMalloc((void **)&c->sol, sizeof(double) * n));
-    CUDA_TRY(cudaMalloc((void **)&c->ysol, sizeof(double) * n));
-    CUDA_TRY(cudaMalloc((void **)&c->rres, sizeof(double) * n));
-    CUDA_TRY(cudaMalloc((void **)&c->rdelta, sizeof(double) * n));
-    CUDA_TRY(cudaMalloc((void **)&c->dag_flags, sizeof(int) * (2 * (size_t)npan * npan + 2 * npan)));
+    CUDA_TRY(cudaMalloc((void **)&w.Xinv, sizeof(double) * (size_t)npan * NB * NB));
+    CUDA_TRY(cudaMalloc((void **)&w.dinv, sizeof(double) * n));
+    CUDA_TRY(cudaMalloc((void **)&w.dval, sizeof(double) * n));
+    CUDA_TRY(cudaMalloc((void **)&w.sol, sizeof(double) * n));
+    CUDA_TRY(cudaMalloc((void **)&w.ysol, sizeof(double) * n));
+    CUDA_TRY(cudaMalloc((void **)&w.rres, sizeof(double) * n));
+    CUDA_TRY(cudaMalloc((void **)&w.rdelta, sizeof(double) * n));
+    CUDA_TRY(cudaMalloc((void **)&w.dag_flags, sizeof(int) * (2 * (size_t)npan * npan + 2 * npan)));
     if (getenv("BALM_DAG_TRACE")) {
-      CUDA_TRY(cudaMalloc((void **)&c->dag_trace, sizeof(unsigned long long) * (4 * (size_t)npan + 8 * 1024)));
-      CUDA_TRY(cudaMemset(c->dag_trace, 0, sizeof(unsigned long long) * (4 * (size_t)npan + 8 * 1024)));
+      CUDA_TRY(cudaMalloc((void **)&w.dag_trace, sizeof(unsigned long long) * (4 * (size_t)npan + 8 * 1024)));
+      CUDA_TRY(cudaMemset(w.dag_trace, 0, sizeof(unsigned long long) * (4 * (size_t)npan + 8 * 1024)));
     }
   }
   c->h_scal[3] = u;  // pinned; the kernels read the damping factor from device memory
   CUDA_TRY(cudaMemcpyAsync(c->scal + 3, c->h_scal + 3, sizeof(double), cudaMemcpyHostToDevice, c->stream));
   CUDA_TRY(cudaMemsetAsync(c->flags, 0, sizeof(int) * 8, c->stream));
-  TRY(enqueue_solve_dag(c));
-  TRY(enqueue_solve_check(c));
+  TRY(enqueue_solve_dag(c, s));
+  TRY(enqueue_solve_check(c, s));
   CUDA_TRY(cudaGetLastError());
   return BALM_OK;
 }

@@ -455,6 +455,39 @@ int balm_pose_graph_evaluate(balm_ctx *ctx, const double *poses12, double *H, do
 int balm_pose_graph_iter(balm_ctx *ctx, double *poses12, const balm_lm_opts *opts, balm_trace *trace, int *n_iters,
                          double *poses_per_iter);
 
+/* Rig calibration (DESIGN.md "Rig calibration"): the ctx's N scan slots driven by n_base base poses T_b and n_lidar
+ * extrinsics E_l (body-frame poses of the LiDARs): slot s is scanned at X_s = T_b E_l with b = base_of[s] and
+ * l = lidar_of[s] (R = R_T R_E, p = R_T p_E + p_T). The cost is the ctx's voxel cost, voxel loss included, at those X_s.
+ * Unknowns are the base poses and extrinsics not fixed by base_fixed / lidar_fixed (nonzero = fixed; NULL: none), free
+ * base poses ascending then free extrinsics ascending, 6 each (phi, t), updated by the left rule of balm_damping_iter;
+ * *n_rig_out = 6 x the free count. With every extrinsic free the cost has a second gauge (T_b Q, Q^-1 E_l): fix one
+ * reference LiDAR, as MLCC does. The rig belongs to the ctx: every voxel registration keeps it, and balm_evaluate,
+ * balm_damping_iter, the pose-graph and covariance calls ignore it. n_base == 0 detaches it. Refused, with the previous
+ * rig kept: BALM_ERR_UNSUPPORTED on a BALM_PREC_BLOCKS ctx; BALM_ERR_INVALID with a communicator attached, for a base or
+ * LiDAR index out of range, a base or LiDAR no slot uses, or when every unknown is fixed. Device memory: the rig holds
+ * K = H J (n_rig x 6N doubles), H_rig and its factor (2 n_rig^2) on top of the ctx's H and factor (2 (6N)^2); a rig with
+ * about one free unknown per slot (n_rig ~ 6N) therefore needs about twice the ctx's dense memory, and balm_set_rig
+ * returns BALM_ERR_CUDA (out of memory), the previous rig kept, when that does not fit. balm_rig_evaluate and
+ * balm_rig_damping_iter are refused (BALM_ERR_INVALID) once a communicator is attached. */
+int balm_set_rig(balm_ctx *ctx, int n_base, int n_lidar, const int32_t *base_of, const int32_t *lidar_of,
+                 const uint8_t *base_fixed, const uint8_t *lidar_fixed, int *n_rig_out);
+/* H_rig (n_rig x n_rig, column-major, exactly symmetric), g_rig (n_rig) and the residual at base12 (n_base x 12) and
+ * ext12 (n_lidar x 12); the voxels' H and g without (include_fix 0) or with the fix clusters, as balm_evaluate over all
+ * voxels. With H_st, g_s the ctx's H and g at the scan poses and J_s = [I on base b | Ad(T_b) on lidar l]:
+ * H_rig = sum J_s^T H_st J_t + the second-order part of the composition contracted with g_s, the exact Hessian in these
+ * coordinates; g_rig = sum J_s^T g_s. Fixed order, no atomics: two calls give the same bits. H and g may be NULL.
+ * BALM_ERR_INVALID without a rig or registered voxels. */
+int balm_rig_evaluate(balm_ctx *ctx, const double *base12, const double *ext12, int include_fix, double *H, double *g,
+                      double *residual);
+/* balm_damping_iter's LM on the rig cost: the same opts (u0, v0, rel_tol, max_iter, hess_includes_fix, force_hess,
+ * verbose; min_planes_per_pose counts voxels per scan slot), accept rule and refinement, with the solve on H_rig.
+ * base12 / ext12 are updated in place. rig_per_iter: max_iter x (n_base + n_lidar) x 12 (base poses, then extrinsics,
+ * after every iteration, before the gauge step) or NULL. gauge_mode 0 / 1 re-anchors the base poses to base 0
+ * (extrinsics are body-frame and stay); BALM_ERR_INVALID for gauge_mode 0 or 1 while a base pose is fixed (the fixed
+ * poses set the frame; pass 2), and without a rig or registered voxels. */
+int balm_rig_damping_iter(balm_ctx *ctx, double *base12, double *ext12, const balm_lm_opts *opts, balm_trace *trace,
+                          int *n_iters, double *rig_per_iter);
+
 /* Sparse pose graph (DESIGN.md "Pose graph", "Sparse solve"): the same factors, cost and LM as balm_set_pose_factors /
  * balm_pose_graph_iter, with H held as its nonzero 6x6 blocks and the damped system solved by a block LDL^T in a
  * nested-dissection order. Device memory grows with the number of blocks, not with (6P)^2, so trajectories of any
