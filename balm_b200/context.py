@@ -102,15 +102,21 @@ def _set_pose_priors(fn, handle, N, priors, kind, scale):
     return [int(s) for s in status]
 
 
+def _lm_args(rows, want_per_iter, max_iter, u0, v0, rel_tol, *flags, problems=1):
+    """An LM call's LmOpts (flags: hess_includes_fix, gauge_mode, min_planes_per_pose, verbose, force_hess), room for
+    max(1, max_iter) trace records and an iteration count per problem, and with want_per_iter the state after every
+    iteration (max_iter x rows x 12)."""
+    return (L.LmOpts(max_iter, u0, v0, rel_tol, *map(int, flags)), (L.Trace * (problems * max(1, max_iter)))(),
+            (C.c_int * problems)(), np.zeros((max_iter, rows, 12)) if want_per_iter else None)
+
+
 def _pose_graph_iter(fn, handle, N, poses12, max_iter, u0, v0, rel_tol, gauge_mode, verbose, want_per_iter, force_hess):
     """balm_pose_graph_iter / balm_spg_iter -> (poses, trace dicts)."""
     poses = np.array(poses12, dtype=np.float64, order="C", copy=True)
-    opts = L.LmOpts(max_iter, u0, v0, rel_tol, 0, gauge_mode, 0, int(verbose), int(force_hess))
-    trace = (L.Trace * max(1, max_iter))()
-    n_it = C.c_int()
-    per_iter = np.zeros((max_iter, N, 12)) if want_per_iter else None
-    L.check(fn(handle, _p(poses), C.byref(opts), trace, C.byref(n_it), _p(per_iter)))
-    tr = _trace_dicts(trace[:n_it.value])
+    opts, trace, n_it, per_iter = _lm_args(N, want_per_iter, max_iter, u0, v0, rel_tol, 0, gauge_mode, 0, verbose,
+                                           force_hess)
+    L.check(fn(handle, _p(poses), C.byref(opts), trace, n_it, _p(per_iter)))
+    tr = _trace_dicts(trace[:n_it[0]])
     if want_per_iter:
         for t, p in zip(tr, per_iter):
             t["poses"] = p
@@ -314,13 +320,10 @@ class Context:
     def damping_iter(self, poses12, max_iter=10, u0=0.01, v0=2.0, rel_tol=1e-6, hess_includes_fix=False,
                      gauge_mode=0, min_planes_per_pose=20, verbose=False, want_per_iter=False, force_hess=False):
         poses = np.array(poses12, dtype=np.float64, order="C", copy=True)
-        opts = L.LmOpts(max_iter, u0, v0, rel_tol, int(hess_includes_fix), gauge_mode, min_planes_per_pose,
-                        int(verbose), int(force_hess))
-        trace = (L.Trace * max_iter)()
-        n_it = C.c_int()
-        per_iter = np.zeros((max_iter, self.N, 12)) if want_per_iter else None
-        L.check(L.lib().balm_damping_iter(self._h, _p(poses), C.byref(opts), trace, C.byref(n_it), _p(per_iter)))
-        return poses, _trace_dicts(trace[:n_it.value]), (per_iter[:n_it.value] if want_per_iter else None)
+        opts, trace, n_it, per_iter = _lm_args(self.N, want_per_iter, max_iter, u0, v0, rel_tol, hess_includes_fix,
+                                               gauge_mode, min_planes_per_pose, verbose, force_hess)
+        L.check(L.lib().balm_damping_iter(self._h, _p(poses), C.byref(opts), trace, n_it, _p(per_iter)))
+        return poses, _trace_dicts(trace[:n_it[0]]), (per_iter[:n_it[0]] if want_per_iter else None)
 
     # ---- rig calibration ----
     def set_rig(self, base_of, lidar_of, fixed_bases=(), fixed_lidars=(0,)):
@@ -375,17 +378,14 @@ class Context:
         (refused while a base pose is fixed: pass 2)."""
         base12, ext12, _ = self._rig_shapes(base12, ext12)
         B, nl = len(base12), len(ext12)
-        opts = L.LmOpts(max_iter, u0, v0, rel_tol, int(hess_includes_fix), gauge_mode, min_planes_per_pose,
-                        int(verbose), int(force_hess))
-        trace = (L.Trace * max(1, max_iter))()
-        n_it = C.c_int()
-        per_iter = np.zeros((max_iter, B + nl, 12)) if want_per_iter else None
-        L.check(L.lib().balm_rig_damping_iter(self._h, _p(base12), _p(ext12), C.byref(opts), trace, C.byref(n_it),
+        opts, trace, n_it, per_iter = _lm_args(B + nl, want_per_iter, max_iter, u0, v0, rel_tol, hess_includes_fix,
+                                               gauge_mode, min_planes_per_pose, verbose, force_hess)
+        L.check(L.lib().balm_rig_damping_iter(self._h, _p(base12), _p(ext12), C.byref(opts), trace, n_it,
                                               _p(per_iter)))
-        tr = _trace_dicts(trace[:n_it.value])
+        tr = _trace_dicts(trace[:n_it[0]])
         if not want_per_iter:
             return base12, ext12, tr
-        per = [(p[:B].copy(), p[B:].copy()) for p in per_iter[:n_it.value]]
+        per = [(p[:B].copy(), p[B:].copy()) for p in per_iter[:n_it[0]]]
         return base12, ext12, tr, per
 
     def marginalize(self, mg_size, poses12, min_ps=15):
@@ -765,20 +765,17 @@ class Batch:
         """damping_iter per problem, all advanced together -> list of (status, poses, trace, per_iter)."""
         poses = self._concat(poses_list)
         B, P = len(self.n_poses), len(poses)
-        opts = L.LmOpts(max_iter, u0, v0, rel_tol, int(hess_includes_fix), gauge_mode, min_planes_per_pose,
-                        int(verbose), int(force_hess))
+        opts, trace, n_it, per_iter = _lm_args(P, want_per_iter, max_iter, u0, v0, rel_tol, hess_includes_fix,
+                                               gauge_mode, min_planes_per_pose, verbose, force_hess, problems=B)
         status = np.zeros(B, dtype=np.int32)
-        n_it = np.zeros(B, dtype=np.int32)
-        trace = (L.Trace * (B * max(1, max_iter)))()
-        per_iter = np.zeros((max_iter, P, 12)) if want_per_iter else None
-        L.check(L.lib().balm_batch_damping_iter(self._h, _p(poses), C.byref(opts), _p(status), _p(n_it), trace,
+        L.check(L.lib().balm_batch_damping_iter(self._h, _p(poses), C.byref(opts), _p(status), n_it, trace,
                                                 _p(per_iter)))
         out = []
         for b in range(B):
             p0, p1 = int(self._pose_ptr[b]), int(self._pose_ptr[b + 1])
-            tr = _trace_dicts(trace[b * max_iter:b * max_iter + int(n_it[b])])
+            tr = _trace_dicts(trace[b * max_iter:b * max_iter + n_it[b]])
             out.append((int(status[b]), poses[p0:p1].copy(), tr,
-                        per_iter[:int(n_it[b]), p0:p1].copy() if want_per_iter else None))
+                        per_iter[:n_it[b], p0:p1].copy() if want_per_iter else None))
         return out
 
     def pose_covariance(self, poses_list, point_noise=0.0, c_cov=None, include_fix=False, want_raw=True, want_cov=True):

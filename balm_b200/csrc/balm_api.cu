@@ -770,33 +770,40 @@ extern "C" int balm_voxel_residuals(balm_ctx *c, const double *poses12, int64_t 
   return BALM_OK;
 }
 
-static int collect_solve(balm_ctx *c, double *q1, int *not_pd) {
-  float ms;
-  cudaEventElapsedTime(&ms, c->ev[9], c->ev[10]);
-  c->tm.ms_solve += ms;
-  c->tm.n_solve += 1;
-  *q1 = c->h_scal[1];
-  *not_pd = c->h_flags[0] != 0 || !std::isfinite(*q1);
-  return BALM_OK;
-}
-
-// The backward-error check of the last solve of sys failed (flags[4]: an indefinite H + uD factored without pivoting
-// lost digits): refine dx in fp64 with the same factors; if that does not bring the error down, the step counts as
-// not_pd. Returns 1 in *refined when dx changed (the caller re-applies the pose update).
-static int maybe_refine(balm_ctx *c, const DenseSystem &sys, double *q1, int *not_pd, int *refined) {
+// The outcome of a damped solve once its stream has been waited for, from the owner's pinned mirrors of scal / flags
+// (balm_ctx's layout, which balm_spg shares): q1 = h_scal[1], not_pd on a bad pivot (h_flags[0]) or a non-finite q1.
+// When the backward-error check failed (h_flags[4]: an indefinite H + uD factored without pivoting lost digits),
+// `refine` refines dx in fp64 with the same factors and leaves the new q1 in h_scal[1]; if that does not bring the
+// error down (*still_bad), the step counts as not_pd. Returns 1 in *refined when dx changed (the caller re-applies
+// the update).
+static int solve_outcome(const double *h_scal, const int *h_flags, const std::function<int(int *still_bad)> &refine,
+                         double *q1, int *not_pd, int *refined) {
+  *q1 = h_scal[1];
+  *not_pd = h_flags[0] != 0 || !std::isfinite(*q1);
   *refined = 0;
-  if (c->h_flags[4] == 0 || *not_pd) return BALM_OK;
+  if (h_flags[4] == 0 || *not_pd) return BALM_OK;
   int still_bad = 0;
-  if (c->prec == BALM_PREC_BLOCKS) TRY(blocks_refine(c, &still_bad));
-  else TRY(refine_solution(c, sys, &still_bad));
-  *q1 = c->h_scal[1];
+  TRY(refine(&still_bad));
+  *q1 = h_scal[1];
   *refined = 1;
   if (still_bad || !std::isfinite(*q1)) *not_pd = 1;
   return BALM_OK;
 }
 
-// The damped solve of sys (the context's own system, or a rig's; a blocks context solves its blocks instead)
-static int solve_dev(balm_ctx *c, const DenseSystem &sys, double u, double *q1, int *not_pd) {
+// The context's solve of sys after the wait: its time, then its outcome (solve_outcome)
+static int collect_solve(balm_ctx *c, const DenseSystem &sys, double *q1, int *not_pd, int *refined) {
+  float ms;
+  cudaEventElapsedTime(&ms, c->ev[9], c->ev[10]);
+  c->tm.ms_solve += ms;
+  c->tm.n_solve += 1;
+  return solve_outcome(c->h_scal, c->h_flags, [c, &sys](int *still_bad) {
+    return c->prec == BALM_PREC_BLOCKS ? blocks_refine(c, still_bad) : refine_solution(c, sys, still_bad);
+  }, q1, not_pd, refined);
+}
+
+// The damped solve of sys (the context's own system, or a rig's; a blocks context solves its blocks instead),
+// enqueued; collect_solve() reads it after the stream has been waited for
+static int solve_dev(balm_ctx *c, const DenseSystem &sys, double u) {
   CUDA_TRY(cudaEventRecord(c->ev[9], c->stream));
   if (c->prec == BALM_PREC_BLOCKS) TRY(blocks_solve(c, u));
   else TRY(launch_ldlt_solve(c, sys, u));
@@ -804,19 +811,18 @@ static int solve_dev(balm_ctx *c, const DenseSystem &sys, double u, double *q1, 
   CUDA_TRY(cudaMemcpyAsync(c->h_scal + 1, c->scal + 1, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
   CUDA_TRY(cudaMemcpyAsync(c->h_flags, c->flags, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
   CUDA_TRY(cudaMemcpyAsync(c->h_flags + 4, c->flags + 4, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-  if (c->defer) return BALM_OK;  // collect_solve() / maybe_refine() after the iteration's synchronisation
-  CUDA_TRY(cudaStreamSynchronize(c->stream));
-  TRY(collect_solve(c, q1, not_pd));
-  int refined = 0;
-  return maybe_refine(c, sys, q1, not_pd, &refined);
+  return BALM_OK;
 }
 
 extern "C" int balm_solve(balm_ctx *c, double u, double *dx, double *q1, int *not_pd) {
   if (!c) { balm_set_error("balm_solve: bad arguments"); return BALM_ERR_INVALID; }
   CUDA_TRY(cudaSetDevice(c->device));
+  const DenseSystem sys = ctx_system(c);
   double q = 0;
-  int bad = 0;
-  TRY(solve_dev(c, ctx_system(c), u, &q, &bad));
+  int bad = 0, refined = 0;
+  TRY(solve_dev(c, sys, u));
+  CUDA_TRY(cudaStreamSynchronize(c->stream));
+  TRY(collect_solve(c, sys, &q, &bad, &refined));
   if (dx) CUDA_TRY(cudaMemcpy(dx, c->dx, sizeof(double) * c->n, cudaMemcpyDeviceToHost));
   if (q1) *q1 = q;
   if (not_pd) *not_pd = bad;
@@ -828,30 +834,6 @@ extern "C" void balm_default_lm_opts(balm_lm_opts *o) {
   o->min_planes_per_pose = 20; o->verbose = 0; o->force_hess = 0;
 }
 
-// The accept rule of BALM2::damping_iter (bavoxel.hpp:1127-1149), shared by balm_damping_iter and balm_pose_graph_iter:
-// q = r1 - r2 (-1 for an unusable step, which is then rejected), the reference's trace line, and u, v updated: on
-// acceptance (q > 0) u *= max(1/3, 1 - (2 rho - 1)^3) with rho = q / q1 and v = 2, else u *= v and v *= 2.
-// *t receives the iteration's trace record; returns whether the step is accepted.
-static bool lm_rule(const balm_lm_opts *o, int it, double r1, double r2, double q1, int not_pd, bool calc_hess, double *u,
-                    double *v, balm_trace *t) {
-  double q = r1 - r2;
-  if (not_pd || !std::isfinite(r2)) q = -1.0;
-  if (o->verbose)  // the reference's trace line (bavoxel.hpp:1132)
-    printf("iter%d: (%lf %lf) u: %lf v: %.1lf q: %.3lf %lf %lf\n", it, r1, r2, *u, *v, q / q1, q1, q);
-  *t = balm_trace{r1, r2, *u, *v, q, q1, 0, calc_hess ? 1 : 0, not_pd};
-  if (q > 0) {  // bavoxel.hpp:1134-1143
-    const double rho = q / q1;
-    *v = 2;
-    const double f = 1 - pow(2 * rho - 1, 3);
-    *u *= (f < (1.0 / 3.0) ? (1.0 / 3.0) : f);
-    t->accepted = 1;
-    return true;
-  }
-  *u = *u * *v;  // bavoxel.hpp:1144-1149
-  *v = 2 * *v;
-  return false;
-}
-
 // With an active absolute pose prior the cost has no gauge freedom: re-anchoring to pose 0 would move the result off
 // the priors.
 static int refuse_gauge_with_priors(const char *who, const PriorSet *pr, const balm_lm_opts *o) {
@@ -860,6 +842,63 @@ static int refuse_gauge_with_priors(const char *who, const PriorSet *pr, const b
                  " re-anchors to pose 0, which moves the result off the pose priors; pass gauge_mode 2");
   return BALM_ERR_INVALID;
 }
+
+// One LM loop's steps, supplied by its owner (balm_damping_iter, balm_rig_damping_iter, balm_pose_graph_iter,
+// balm_spg_iter). Each returns a BALM_* status.
+struct LmSteps {
+  cudaStream_t st;
+  const double *scal;  // the owner's device scalars: eval leaves r1 in scal[0]
+  double *h_scal;      // their pinned host mirror
+  std::function<int()> eval;                                         // H, g and r1 at the current state, enqueued
+  std::function<int(double u)> solve;                                // the damped solve for dx, enqueued
+  std::function<int()> trial;                                        // the trial state from dx, enqueued
+  std::function<int(double *r2)> trial_cost;                         // its cost; ends in the iteration's one wait
+  std::function<int(double *q1, int *not_pd, int *refined)> finish;  // the solve's outcome (solve_outcome)
+  std::function<int(bool accepted)> step;                            // accept / reject bookkeeping
+  std::function<int(int it)> snapshot;                               // the state after iteration it
+};
+
+// BALM2::damping_iter's loop (bavoxel.hpp:1127-1155): per iteration evaluation (when H is stale), solve, trial state and
+// trial cost are enqueued back to back and the host waits once; a refined dx redoes the trial state and its cost.
+static int lm_run(const LmSteps &s, const balm_lm_opts *o, balm_trace *trace, int *n_iters) {
+  double u = o->u0, v = o->v0, r1 = 0, r2 = 0;
+  bool calc_hess = true;
+  for (int it = 0; it < o->max_iter; it++) {
+    if (calc_hess) {
+      TRY(s.eval());
+      CUDA_TRY(cudaMemcpyAsync(s.h_scal, s.scal, sizeof(double), cudaMemcpyDeviceToHost, s.st));
+    }
+    TRY(s.solve(u));
+    TRY(s.trial());
+    TRY(s.trial_cost(&r2));
+    double q1 = 0;
+    int not_pd = 0, refined = 0;
+    TRY(s.finish(&q1, &not_pd, &refined));
+    if (refined && !not_pd) {  // dx changed: the trial state and its cost again (rare path)
+      TRY(s.trial());
+      TRY(s.trial_cost(&r2));
+    }
+    if (calc_hess) r1 = s.h_scal[0];
+    balm_trace t;
+    bool stop;
+    const bool accepted = lm_rule(r1, r2, q1, not_pd, calc_hess, o->rel_tol, &u, &v, &t, &stop);
+    if (o->verbose)  // the reference's trace line (bavoxel.hpp:1132)
+      printf("iter%d: (%lf %lf) u: %lf v: %.1lf q: %.3lf %lf %lf\n", it, r1, r2, t.u, t.v, t.q / q1, q1, t.q);
+    TRY(s.step(accepted));
+    calc_hess = accepted || o->force_hess != 0;  // after a rejection H and g of the current state are still in place
+    if (trace) trace[it] = t;
+    TRY(s.snapshot(it));
+    if (n_iters) *n_iters = it + 1;
+    if (stop) break;
+  }
+  return BALM_OK;
+}
+
+// Clears the context's LM flags (set by balm_damping_iter and balm_rig_damping_iter) on every exit path
+struct LmScope {
+  balm_ctx *c;
+  ~LmScope() { c->lm_active = false; c->defer = false; c->pending_eval = false; c->eval_same_poses = false; }
+};
 
 extern "C" int balm_damping_iter(balm_ctx *c, double *poses12, const balm_lm_opts *o, balm_trace *trace, int *n_iters,
                                  double *poses_per_iter) {
@@ -889,72 +928,56 @@ extern "C" int balm_damping_iter(balm_ctx *c, double *poses12, const balm_lm_opt
   }
   const size_t pbytes = sizeof(double) * 12 * c->N;
   CUDA_TRY(cudaMemcpyAsync(c->poses, poses12, pbytes, cudaMemcpyHostToDevice, c->stream));
-  double u = o->u0, v = o->v0, r1 = 0, r2 = 0;
-  bool calc_hess = true;
   // The residual pass at the trial poses computes the same per-voxel eigen data the next evaluation starts with:
   // when the step is accepted they are handed over (same kernel, same inputs -> identical values). Needs the whole
   // problem in one batch and the same treatment of the fix cluster in both passes.
   const bool hand_over = c->stats_trial != nullptr && (c->fix == nullptr || o->hess_includes_fix != 0);
   bool stats_cached = false;
-  tensor_syrk_new_problem(c);  // nothing speculative is carried over from earlier calls
-  struct LmScope {             // lm_active / defer are cleared on every exit path
-    balm_ctx *c;
-    ~LmScope() { c->lm_active = false; c->defer = false; c->pending_eval = false; c->eval_same_poses = false; }
-  } lm_scope{c};
-  c->lm_active = true;
   bool same_poses = false;  // the last step was rejected: c->poses are those of the previous evaluation
-  for (int it = 0; it < o->max_iter; it++) {
-    // evaluation -> solve -> pose update -> trial residual are enqueued back to back; the host waits once, at the
-    // end of residual_dev, and then reads r1, q1, the pivot flag and the phase timers
-    c->defer = !getenv("BALM_SYNC_PHASES");
-    int rc = BALM_OK;
-    if (calc_hess) {
-      c->eval_same_poses = same_poses;
-      rc = evaluate_dev(c, c->poses, 0, c->M, o->hess_includes_fix != 0, stats_cached);
-      c->eval_same_poses = false;
-      if (rc == BALM_OK && cudaMemcpyAsync(c->h_scal, c->scal, sizeof(double), cudaMemcpyDeviceToHost, c->stream) != cudaSuccess)
-        rc = BALM_ERR_CUDA;
-    }
-    double q1 = 0;
-    int not_pd = 0;
-    if (rc == BALM_OK) rc = solve_dev(c, ctx_system(c), u, &q1, &not_pd);
-    if (rc == BALM_OK) rc = launch_pose_update(c, c->poses, c->dx, c->poses_trial);
-    if (rc == BALM_OK) rc = residual_dev(c, c->poses_trial, &r2, hand_over);  // synchronises the stream
-    const bool was_deferred = c->defer;
-    c->defer = false;
-    if (rc != BALM_OK) { c->pending_eval = false; return rc; }
-    if (was_deferred) {
-      TRY(collect_eval(c));
-      TRY(collect_solve(c, &q1, &not_pd));
-      int refined = 0;
-      TRY(maybe_refine(c, ctx_system(c), &q1, &not_pd, &refined));
-      if (refined && !not_pd) {  // dx changed: the trial poses and their residual are recomputed (rare path, synchronous)
-        TRY(launch_pose_update(c, c->poses, c->dx, c->poses_trial));
-        TRY(residual_dev(c, c->poses_trial, &r2, hand_over));
-      }
-    }
-    if (calc_hess) r1 = c->h_scal[0];
-    balm_trace t;
-    if (lm_rule(o, it, r1, r2, q1, not_pd, calc_hess, &u, &v, &t)) {
+  tensor_syrk_new_problem(c);  // nothing speculative is carried over from earlier calls
+  LmScope lm_scope{c};
+  c->lm_active = true;
+  // the evaluation's events and flags are read after the iteration's wait; BALM_SYNC_PHASES waits after every phase
+  c->defer = !getenv("BALM_SYNC_PHASES");
+  const DenseSystem sys = ctx_system(c);
+  LmSteps s{c->stream, c->scal, c->h_scal};
+  s.eval = [&]() -> int {
+    c->eval_same_poses = same_poses;
+    const int rc = evaluate_dev(c, c->poses, 0, c->M, o->hess_includes_fix != 0, stats_cached);
+    c->eval_same_poses = false;
+    return rc;
+  };
+  s.solve = [&](double u) -> int {
+    TRY(solve_dev(c, sys, u));
+    if (!c->defer) CUDA_TRY(cudaStreamSynchronize(c->stream));
+    return BALM_OK;
+  };
+  s.trial = [c]() { return launch_pose_update(c, c->poses, c->dx, c->poses_trial); };
+  s.trial_cost = [&](double *r2) { return residual_dev(c, c->poses_trial, r2, hand_over); };
+  s.finish = [&](double *q1, int *not_pd, int *refined) -> int {
+    TRY(collect_eval(c));
+    return collect_solve(c, sys, q1, not_pd, refined);
+  };
+  s.step = [&](bool accepted) -> int {
+    if (accepted) {
       std::swap(c->poses, c->poses_trial);
       if (hand_over) {
         std::swap(c->stats, c->stats_trial);
         CUDA_TRY(cudaMemcpyAsync(c->scal + BALM_SCAL_RCUR, c->scal + BALM_SCAL_RTRIAL, sizeof(double), cudaMemcpyDeviceToDevice, c->stream));
       }
       stats_cached = hand_over;
-      calc_hess = true;
-      same_poses = false;
     } else {
-      calc_hess = o->force_hess != 0;
       stats_cached = c->stats_trial != nullptr;  // c->stats still describes c->poses (single batch)
-      same_poses = true;
     }
-    if (trace) trace[it] = t;
+    same_poses = !accepted;
+    return BALM_OK;
+  };
+  s.snapshot = [&](int it) -> int {
     if (poses_per_iter)
       CUDA_TRY(cudaMemcpyAsync(poses_per_iter + (size_t)it * 12 * c->N, c->poses, pbytes, cudaMemcpyDeviceToHost, c->stream));
-    if (n_iters) *n_iters = it + 1;
-    if (o->rel_tol >= 0 && fabs(r1 - r2) / r1 < o->rel_tol) break;  // bavoxel.hpp:1155
-  }
+    return BALM_OK;
+  };
+  TRY(lm_run(s, o, trace, n_iters));
   if (o->gauge_mode == 0 || o->gauge_mode == 1) TRY(launch_gauge(c, c->poses, o->gauge_mode));
   CUDA_TRY(cudaMemcpyAsync(poses12, c->poses, pbytes, cudaMemcpyDeviceToHost, c->stream));
   CUDA_TRY(cudaStreamSynchronize(c->stream));
@@ -1085,87 +1108,6 @@ extern "C" int balm_pose_graph_evaluate(balm_ctx *c, const double *poses12, doub
   return BALM_OK;
 }
 
-// The LM loop of balm_pose_graph_iter and balm_spg_iter: damping_iter's rule on the pose-graph cost. The two hold and
-// solve H differently: `eval` leaves H, g and the cost (scal[0]) at the given poses, `solve` dx, q1 (scal[1]) and the
-// flags for the damping u, both enqueued; `finish` reads q1 and not_pd after the iteration's wait and refines dx when
-// the backward-error check failed (*refined = 1: dx changed).
-struct PoseGraphLm {
-  cudaStream_t st;
-  int N;
-  const PoseGraph *pg;
-  double **poses, **poses_trial;  // the owner's [12N] buffers, swapped on acceptance
-  double *dx, *scal, *h_scal;     // scal: device [32] (3 u, 4..15 gauge snapshot), h_scal: pinned host [16]
-  long long *launches;
-  const PriorSet *pr = nullptr;   // the owner's pose priors (their cost joins the trial cost)
-  std::function<int(const double *poses)> eval;
-  std::function<int(double u)> solve;
-  std::function<int(double *q1, int *not_pd, int *refined)> finish;
-};
-
-// the pose-graph cost at the trial poses -> *r2 (waits for the stream)
-static int pose_graph_trial_cost(const PoseGraphLm &s, double *r2) {
-  TRY(pose_graph_cost(s.pg, s.st, *s.poses_trial, s.scal + 2, s.launches));
-  if (s.pr) TRY(prior_add_cost(s.pr, s.st, *s.poses_trial, s.scal + 2, s.launches));
-  CUDA_TRY(cudaMemcpyAsync(s.h_scal + 2, s.scal + 2, sizeof(double), cudaMemcpyDeviceToHost, s.st));
-  CUDA_TRY(cudaStreamSynchronize(s.st));
-  *r2 = s.h_scal[2];
-  return BALM_OK;
-}
-
-static int trial_poses(const PoseGraphLm &s) {
-  *s.launches += 1;
-  return launch_pose_update(s.st, s.N, *s.poses, s.dx, *s.poses_trial);
-}
-
-static int pose_graph_lm(const PoseGraphLm &s, double *poses12, const balm_lm_opts *o, balm_trace *trace, int *n_iters,
-                         double *poses_per_iter) {
-  const size_t pbytes = sizeof(double) * 12 * s.N;
-  CUDA_TRY(cudaMemcpyAsync(*s.poses, poses12, pbytes, cudaMemcpyHostToDevice, s.st));
-  double u = o->u0, v = o->v0, r1 = 0, r2 = 0;
-  bool calc_hess = true;
-  for (int it = 0; it < o->max_iter; it++) {
-    // evaluation -> solve -> pose update -> trial cost enqueued back to back, one wait at the end
-    int rc = BALM_OK;
-    if (calc_hess) {
-      rc = s.eval(*s.poses);
-      if (rc == BALM_OK && cudaMemcpyAsync(s.h_scal, s.scal, sizeof(double), cudaMemcpyDeviceToHost, s.st) != cudaSuccess)
-        rc = BALM_ERR_CUDA;
-    }
-    double q1 = 0;
-    int not_pd = 0;
-    if (rc == BALM_OK) rc = s.solve(u);
-    if (rc == BALM_OK) rc = trial_poses(s);
-    if (rc == BALM_OK) rc = pose_graph_trial_cost(s, &r2);
-    if (rc != BALM_OK) return rc;
-    int refined = 0;
-    TRY(s.finish(&q1, &not_pd, &refined));
-    if (refined && !not_pd) {  // dx changed: the trial poses and their cost again
-      TRY(trial_poses(s));
-      TRY(pose_graph_trial_cost(s, &r2));
-    }
-    if (calc_hess) r1 = s.h_scal[0];
-    balm_trace t;
-    if (lm_rule(o, it, r1, r2, q1, not_pd, calc_hess, &u, &v, &t)) {
-      std::swap(*s.poses, *s.poses_trial);
-      calc_hess = true;
-    } else {
-      calc_hess = o->force_hess != 0;  // H and g at the current poses are still in place
-    }
-    if (trace) trace[it] = t;
-    if (poses_per_iter)
-      CUDA_TRY(cudaMemcpyAsync(poses_per_iter + (size_t)it * 12 * s.N, *s.poses, pbytes, cudaMemcpyDeviceToHost, s.st));
-    if (n_iters) *n_iters = it + 1;
-    if (o->rel_tol >= 0 && fabs(r1 - r2) / r1 < o->rel_tol) break;
-  }
-  if (o->gauge_mode == 0 || o->gauge_mode == 1) {
-    *s.launches += 1;
-    TRY(launch_gauge(s.st, s.N, *s.poses, s.scal + 4, o->gauge_mode));
-  }
-  CUDA_TRY(cudaMemcpyAsync(poses12, *s.poses, pbytes, cudaMemcpyDeviceToHost, s.st));
-  CUDA_TRY(cudaStreamSynchronize(s.st));
-  return BALM_OK;
-}
-
 extern "C" int balm_pose_graph_iter(balm_ctx *c, double *poses12, const balm_lm_opts *o, balm_trace *trace, int *n_iters,
                                     double *poses_per_iter) {
   if (!c || !poses12 || !o) { balm_set_error("balm_pose_graph_iter: bad arguments"); return BALM_ERR_INVALID; }
@@ -1175,22 +1117,36 @@ extern "C" int balm_pose_graph_iter(balm_ctx *c, double *poses12, const balm_lm_
   if (!c->pg) { balm_set_error("balm_pose_graph_iter: no pose factors registered"); return BALM_ERR_INVALID; }
   TRY(refuse_gauge_with_priors("balm_pose_graph_iter", c->pr, o));
   CUDA_TRY(cudaSetDevice(c->device));
-  PoseGraphLm s{c->stream, c->N, c->pg, &c->poses, &c->poses_trial, c->dx, c->scal, c->h_scal, &c->launches};
-  s.pr = c->pr;
-  s.eval = [c](const double *poses) -> int { return pose_graph_eval(c, poses); };
-  s.solve = [c](double u) -> int {  // deferred: q1 and the flags are read by finish()
-    double q1 = 0;
-    int not_pd = 0;
-    c->defer = true;
-    const int rc = solve_dev(c, ctx_system(c), u, &q1, &not_pd);
-    c->defer = false;
-    return rc;
+  const size_t pbytes = sizeof(double) * 12 * c->N;
+  CUDA_TRY(cudaMemcpyAsync(c->poses, poses12, pbytes, cudaMemcpyHostToDevice, c->stream));
+  const DenseSystem sys = ctx_system(c);
+  LmSteps s{c->stream, c->scal, c->h_scal};
+  s.eval = [c]() { return pose_graph_eval(c, c->poses); };
+  s.solve = [c, &sys](double u) { return solve_dev(c, sys, u); };
+  s.trial = [c]() { return launch_pose_update(c, c->poses, c->dx, c->poses_trial); };
+  s.trial_cost = [c](double *r2) -> int {  // the factors', then the priors' cost -> scal[2]
+    TRY(pose_graph_cost(c->pg, c->stream, c->poses_trial, c->scal + 2, &c->launches));
+    if (c->pr) TRY(prior_add_cost(c->pr, c->stream, c->poses_trial, c->scal + 2, &c->launches));
+    CUDA_TRY(cudaMemcpyAsync(c->h_scal + 2, c->scal + 2, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+    CUDA_TRY(cudaStreamSynchronize(c->stream));
+    *r2 = c->h_scal[2];
+    return BALM_OK;
   };
-  s.finish = [c](double *q1, int *not_pd, int *refined) -> int {
-    TRY(collect_solve(c, q1, not_pd));
-    return maybe_refine(c, ctx_system(c), q1, not_pd, refined);
+  s.finish = [c, &sys](double *q1, int *not_pd, int *refined) { return collect_solve(c, sys, q1, not_pd, refined); };
+  s.step = [c](bool accepted) {
+    if (accepted) std::swap(c->poses, c->poses_trial);
+    return BALM_OK;
   };
-  return pose_graph_lm(s, poses12, o, trace, n_iters, poses_per_iter);
+  s.snapshot = [&](int it) -> int {
+    if (poses_per_iter)
+      CUDA_TRY(cudaMemcpyAsync(poses_per_iter + (size_t)it * 12 * c->N, c->poses, pbytes, cudaMemcpyDeviceToHost, c->stream));
+    return BALM_OK;
+  };
+  TRY(lm_run(s, o, trace, n_iters));
+  if (o->gauge_mode == 0 || o->gauge_mode == 1) TRY(launch_gauge(c, c->poses, o->gauge_mode));
+  CUDA_TRY(cudaMemcpyAsync(poses12, c->poses, pbytes, cudaMemcpyDeviceToHost, c->stream));
+  CUDA_TRY(cudaStreamSynchronize(c->stream));
+  return BALM_OK;
 }
 
 // ---------------- rig calibration (rig.cu) ----------------
@@ -1297,8 +1253,9 @@ extern "C" int balm_rig_evaluate(balm_ctx *c, const double *base12, const double
   return BALM_OK;
 }
 
-// balm_damping_iter's rule on the rig cost: per iteration compose -> evaluate -> reduce -> solve -> rig update ->
-// compose the trial state -> trial residual; H_rig is reused after a rejected step unless force_hess.
+// balm_damping_iter's loop on the rig cost: per iteration compose -> evaluate -> reduce -> solve -> rig update ->
+// compose the trial state -> trial residual, then the one wait. No hand-over and no speculation: every evaluation is
+// the pure function balm_evaluate is.
 extern "C" int balm_rig_damping_iter(balm_ctx *c, double *base12, double *ext12, const balm_lm_opts *o,
                                      balm_trace *trace, int *n_iters, double *rig_per_iter) {
   const char *who = "balm_rig_damping_iter";
@@ -1320,37 +1277,37 @@ extern "C" int balm_rig_damping_iter(balm_ctx *c, double *base12, double *ext12,
   const int B = rig_bases(rg), U = B + rig_lidars(rg);
   const size_t sbytes = sizeof(double) * 12 * U;
   const DenseSystem sys = rig_system(rg);
-  double u = o->u0, v = o->v0, r1 = 0, r2 = 0;
-  bool calc_hess = true;
-  for (int it = 0; it < o->max_iter; it++) {
-    if (calc_hess) {
-      TRY(rig_evaluate_dev(c, o->hess_includes_fix != 0));
-      CUDA_TRY(cudaMemcpyAsync(c->h_scal, c->scal, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
-    }
-    double q1 = 0;
-    int not_pd = 0;
-    TRY(solve_dev(c, sys, u, &q1, &not_pd));  // waits, and refines dx when the backward-error check asks for it
-    if (calc_hess) {
-      TRY(rig_collect_reduce(c));
-      r1 = c->h_scal[0];
-    }
+  LmScope lm_scope{c};
+  c->defer = true;  // the evaluation's events and flags are read after the iteration's wait
+  bool reduced = false;  // this iteration evaluated: the reduction's events are to be read
+  LmSteps s{c->stream, c->scal, c->h_scal};
+  s.eval = [&]() {
+    reduced = true;
+    return rig_evaluate_dev(c, o->hess_includes_fix != 0);
+  };
+  s.solve = [c, &sys](double u) { return solve_dev(c, sys, u); };
+  s.trial = [c, rg]() -> int {
     TRY(rig_update(rg, c->stream, rig_state(rg, false), rig_state(rg, true), &c->launches));
-    TRY(rig_compose(rg, c->stream, rig_state(rg, true), c->poses_trial, &c->launches));
-    TRY(residual_dev(c, c->poses_trial, &r2));
-    balm_trace t;
-    if (lm_rule(o, it, r1, r2, q1, not_pd, calc_hess, &u, &v, &t)) {
-      rig_swap_states(rg);
-      calc_hess = true;
-    } else {
-      calc_hess = o->force_hess != 0;  // H_rig and g_rig of the current state are still in place
-    }
-    if (trace) trace[it] = t;
+    return rig_compose(rg, c->stream, rig_state(rg, true), c->poses_trial, &c->launches);
+  };
+  s.trial_cost = [c](double *r2) { return residual_dev(c, c->poses_trial, r2); };
+  s.finish = [&](double *q1, int *not_pd, int *refined) -> int {
+    TRY(collect_eval(c));
+    if (reduced) TRY(rig_collect_reduce(c));
+    reduced = false;
+    return collect_solve(c, sys, q1, not_pd, refined);
+  };
+  s.step = [rg](bool accepted) {
+    if (accepted) rig_swap_states(rg);
+    return BALM_OK;
+  };
+  s.snapshot = [&](int it) -> int {
     if (rig_per_iter)
       CUDA_TRY(cudaMemcpyAsync(rig_per_iter + (size_t)it * 12 * U, rig_state(rg, false), sbytes, cudaMemcpyDeviceToHost,
                                c->stream));
-    if (n_iters) *n_iters = it + 1;
-    if (o->rel_tol >= 0 && fabs(r1 - r2) / r1 < o->rel_tol) break;
-  }
+    return BALM_OK;
+  };
+  TRY(lm_run(s, o, trace, n_iters));
   if (o->gauge_mode == 0 || o->gauge_mode == 1) {  // base poses re-anchored to base 0; extrinsics are body-frame
     c->launches += 1;
     TRY(launch_gauge(c->stream, B, rig_state(rg, false), c->scal + 4, o->gauge_mode));
@@ -1557,9 +1514,10 @@ extern "C" int balm_spg_iter(balm_spg *sp, double *poses12, const balm_lm_opts *
   if (!sp->pg) { balm_set_error("balm_spg_iter: no pose factors registered"); return BALM_ERR_INVALID; }
   TRY(refuse_gauge_with_priors("balm_spg_iter", sp->pr, o));
   CUDA_TRY(cudaSetDevice(sp->device));
-  PoseGraphLm s{sp->stream, sp->N, sp->pg, &sp->poses, &sp->poses_trial, sp->dx, sp->scal, sp->h_scal, &sp->launches};
-  s.pr = sp->pr;
-  s.eval = [sp](const double *poses) -> int { return spg_eval(sp, poses); };
+  const size_t pbytes = sizeof(double) * 12 * sp->N;
+  CUDA_TRY(cudaMemcpyAsync(sp->poses, poses12, pbytes, cudaMemcpyHostToDevice, sp->stream));
+  LmSteps s{sp->stream, sp->scal, sp->h_scal};
+  s.eval = [sp]() { return spg_eval(sp, sp->poses); };
   s.solve = [sp](double u) -> int {
     sp->h_scal[3] = u;  // pinned; the kernels read the damping factor from device memory
     CUDA_TRY(cudaMemcpyAsync(sp->scal + 3, sp->h_scal + 3, sizeof(double), cudaMemcpyHostToDevice, sp->stream));
@@ -1569,19 +1527,41 @@ extern "C" int balm_spg_iter(balm_spg *sp, double *poses12, const balm_lm_opts *
     CUDA_TRY(cudaMemcpyAsync(sp->h_flags, sp->flags, sizeof(int) * 8, cudaMemcpyDeviceToHost, sp->stream));
     return BALM_OK;
   };
-  s.finish = [sp](double *q1, int *not_pd, int *refined) -> int {  // collect_solve and maybe_refine of the context
-    *q1 = sp->h_scal[1];
-    *not_pd = sp->h_flags[0] != 0 || !std::isfinite(*q1);
-    *refined = 0;
-    if (sp->h_flags[4] == 0 || *not_pd) return BALM_OK;
-    int still_bad = 0;
-    TRY(sparse_refine(sp->solver, sp->stream, sp->h_flags, sp->h_scal, &still_bad));
-    *q1 = sp->h_scal[1];
-    *refined = 1;
-    if (still_bad || !std::isfinite(*q1)) *not_pd = 1;
+  s.trial = [sp]() {
+    sp->launches += 1;
+    return launch_pose_update(sp->stream, sp->N, sp->poses, sp->dx, sp->poses_trial);
+  };
+  s.trial_cost = [sp](double *r2) -> int {  // the factors', then the priors' cost -> scal[2]
+    TRY(pose_graph_cost(sp->pg, sp->stream, sp->poses_trial, sp->scal + 2, &sp->launches));
+    if (sp->pr) TRY(prior_add_cost(sp->pr, sp->stream, sp->poses_trial, sp->scal + 2, &sp->launches));
+    CUDA_TRY(cudaMemcpyAsync(sp->h_scal + 2, sp->scal + 2, sizeof(double), cudaMemcpyDeviceToHost, sp->stream));
+    CUDA_TRY(cudaStreamSynchronize(sp->stream));
+    *r2 = sp->h_scal[2];
     return BALM_OK;
   };
-  return pose_graph_lm(s, poses12, o, trace, n_iters, poses_per_iter);
+  s.finish = [sp](double *q1, int *not_pd, int *refined) {
+    return solve_outcome(sp->h_scal, sp->h_flags, [sp](int *still_bad) {
+      return sparse_refine(sp->solver, sp->stream, sp->h_flags, sp->h_scal, still_bad);
+    }, q1, not_pd, refined);
+  };
+  s.step = [sp](bool accepted) {
+    if (accepted) std::swap(sp->poses, sp->poses_trial);
+    return BALM_OK;
+  };
+  s.snapshot = [&](int it) -> int {
+    if (poses_per_iter)
+      CUDA_TRY(cudaMemcpyAsync(poses_per_iter + (size_t)it * 12 * sp->N, sp->poses, pbytes, cudaMemcpyDeviceToHost,
+                               sp->stream));
+    return BALM_OK;
+  };
+  TRY(lm_run(s, o, trace, n_iters));
+  if (o->gauge_mode == 0 || o->gauge_mode == 1) {
+    sp->launches += 1;
+    TRY(launch_gauge(sp->stream, sp->N, sp->poses, sp->scal + 4, o->gauge_mode));
+  }
+  CUDA_TRY(cudaMemcpyAsync(poses12, sp->poses, pbytes, cudaMemcpyDeviceToHost, sp->stream));
+  CUDA_TRY(cudaStreamSynchronize(sp->stream));
+  return BALM_OK;
 }
 
 extern "C" int balm_spg_covariance(balm_spg *s, const double *poses12, int anchor, double *cov) {

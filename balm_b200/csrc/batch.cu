@@ -439,34 +439,23 @@ __global__ void batch_lm_kernel(LmArgs a) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= a.B || !a.active[b]) return;
   const int calc = a.calc[b];
-  const double r1 = calc ? a.r_eval[b] : a.r1[b], r2 = a.r2[b], q1 = a.q1[b];
-  const int not_pd = a.notpd[b];
+  const double r1 = calc ? a.r_eval[b] : a.r1[b];
   double u = a.u[b], v = a.v[b];
-  double q = r1 - r2;
-  if (not_pd || !isfinite(r2)) q = -1.0;  // unusable step -> rejected, u *= v
-  balm_trace t{r1, r2, u, v, q, q1, 0, calc, not_pd};
-  int next_calc;
-  if (q > 0) {  // bavoxel.hpp:1134-1143
+  balm_trace t;
+  bool stop;
+  const bool accepted = lm_rule(r1, a.r2[b], a.q1[b], a.notpd[b], calc, a.rel_tol, &u, &v, &t, &stop);
+  if (accepted) {
     const Prob pr = a.prob[b];
     for (int e = 0; e < 12 * pr.np; e++) a.poses[12 * (size_t)pr.pose_base + e] = a.trial[12 * (size_t)pr.pose_base + e];
-    const double rho = q / q1;
-    v = 2;
-    const double f = 1 - pow(2 * rho - 1, 3.0);
-    u *= (f < (1.0 / 3.0) ? (1.0 / 3.0) : f);
-    next_calc = 1;
-    t.accepted = 1;
-  } else {  // bavoxel.hpp:1144-1149
-    u = u * v;
-    v = 2 * v;
-    next_calc = a.force_hess;
   }
+  const int next_calc = accepted ? 1 : a.force_hess;
   a.trace[(size_t)b * a.max_iter + a.it] = t;
   a.n_iters[b] = a.it + 1;
   a.r1[b] = r1;
   a.u[b] = u;
   a.v[b] = v;
   a.calc[b] = next_calc;
-  const bool stop = (a.rel_tol >= 0 && fabs(r1 - r2) / r1 < a.rel_tol) || a.it + 1 >= a.max_iter;  // bavoxel.hpp:1155
+  stop = stop || a.it + 1 >= a.max_iter;
   a.evalm[b] = stop ? 0 : next_calc;
   if (stop) a.active[b] = 0;
   else atomicAdd(a.n_active, 1);

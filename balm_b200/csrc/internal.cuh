@@ -251,6 +251,30 @@ __device__ __forceinline__ void loss_rho(int kind, double c, double s, double *r
   }
 }
 
+// The accept rule of BALM2::damping_iter (bavoxel.hpp:1127-1155), on the host (lm_run, balm_api.cu) and per problem on
+// the device (batch_lm_kernel): q = r1 - r2 (-1 for an unusable step, not_pd or a non-finite r2, which is then
+// rejected); on acceptance (q > 0) u *= max(1/3, 1 - (2 rho - 1)^3) with rho = q / q1 and v = 2, else u *= v and
+// v *= 2. *t receives the iteration's trace record and *stop the rel_tol exit; returns whether the step is accepted.
+// pow is the C library's on the host and CUDA's on the device, as in the reference and the batch respectively.
+__host__ __device__ inline bool lm_rule(double r1, double r2, double q1, int not_pd, int calc_hess, double rel_tol,
+                                        double *u, double *v, balm_trace *t, bool *stop) {
+  double q = r1 - r2;
+  if (not_pd || !isfinite(r2)) q = -1.0;
+  *t = balm_trace{r1, r2, *u, *v, q, q1, 0, calc_hess, not_pd};
+  *stop = rel_tol >= 0 && fabs(r1 - r2) / r1 < rel_tol;  // bavoxel.hpp:1155
+  if (q > 0) {  // bavoxel.hpp:1134-1143
+    const double rho = q / q1;
+    *v = 2;
+    const double f = 1 - pow(2 * rho - 1, 3.0);
+    *u *= (f < (1.0 / 3.0) ? (1.0 / 3.0) : f);
+    t->accepted = 1;
+    return true;
+  }
+  *u = *u * *v;  // bavoxel.hpp:1144-1149
+  *v = 2 * *v;
+  return false;
+}
+
 struct WC {  // world-frame cluster
   double p00, p01, p02, p11, p12, p22, v0, v1, v2, n;
 };
