@@ -62,7 +62,7 @@ SYMBOLS = ["balm_last_error", "balm_version", "balm_create", "balm_destroy", "ba
            "balm_spg_set_factor_loss", "balm_spg_factor_residuals", "balm_set_pose_priors", "balm_prior_residuals",
            "balm_spg_set_pose_priors", "balm_spg_prior_residuals", "balm_set_voxel_loss", "balm_voxel_residuals",
            "balm_batch_set_voxel_loss", "balm_batch_voxel_residuals",
-           "balm_set_rig", "balm_rig_evaluate", "balm_rig_damping_iter"]
+           "balm_set_rig", "balm_rig_evaluate", "balm_rig_damping_iter", "balm_rig_covariance"]
 
 
 def lib():
@@ -174,6 +174,8 @@ def lib():
                                         C.POINTER(C.c_double)]
         L.balm_rig_damping_iter.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(LmOpts), C.c_void_p,
                                             C.POINTER(C.c_int), C.c_void_p]
+        L.balm_rig_covariance.argtypes = [C.c_void_p] + [C.c_void_p] * 3 + [C.c_double, C.c_int, C.c_int, C.c_void_p,
+                                                                              C.c_void_p]
         _lib = L
     return _lib
 

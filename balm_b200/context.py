@@ -388,6 +388,20 @@ class Context:
         per = [(p[:B].copy(), p[B:].copy()) for p in per_iter[:n_it[0]]]
         return base12, ext12, tr, per
 
+    def rig_covariance(self, base12, ext12, point_noise=0.0, c_cov=None, include_fix=False, anchor=-1, want_raw=True,
+                       want_cov=True):
+        """pose_covariance on the rig's unknowns (include/balm_b200.h, balm_rig_covariance) -> (raw, cov), n_rig x n_rig
+        in set_rig's order: raw = J^T Rcov_raw J at the composed scan poses, cov = H_rig^-1 raw H_rig^-T. anchor: -1 or
+        the free index of a free base pose, deleted from both (its rows and columns 0); pass a base anchor when the base
+        poses' gauge is free (no fixed base and no fix clusters in H), -1 when every base pose is fixed."""
+        base12, ext12, n_rig = self._rig_shapes(base12, ext12)
+        cc = None if c_cov is None else np.ascontiguousarray(c_cov, dtype=np.float64).reshape(-1, 81)
+        raw = np.zeros((n_rig, n_rig), order="F") if want_raw else None
+        cov = np.zeros((n_rig, n_rig), order="F") if want_cov else None
+        L.check(L.lib().balm_rig_covariance(self._h, _p(base12), _p(ext12), _p(cc), float(point_noise), int(include_fix),
+                                            int(anchor), _p(raw), _p(cov)))
+        return raw, cov
+
     def marginalize(self, mg_size, poses12, min_ps=15):
         """OCTO_TREE_ROOT::marginalize on the registered voxel set (bavoxel.hpp:948-963, 778-816) -> (n_voxels, n_obs)."""
         poses12 = np.ascontiguousarray(poses12, dtype=np.float64)

@@ -1253,6 +1253,62 @@ extern "C" int balm_rig_evaluate(balm_ctx *c, const double *base12, const double
   return BALM_OK;
 }
 
+// raw_rig = J^T R J with R balm_pose_covariance's Rcov_raw at the composed poses, and H_rig^-1 raw_rig H_rig^-T with
+// balm_rig_evaluate's H_rig, both with the anchor's rows and columns deleted. Waits for the pivot test and at the end.
+extern "C" int balm_rig_covariance(balm_ctx *c, const double *base12, const double *ext12, const double *c_cov81,
+                                   double point_noise, int include_fix, int anchor, double *raw, double *cov) {
+  const char *who = "balm_rig_covariance";
+  if (!c || !base12 || !ext12 || (!raw && !cov)) { balm_set_error(std::string(who) + ": bad arguments"); return BALM_ERR_INVALID; }
+  TRY(rig_check(c, who));
+  if (c->M < 1) { balm_set_error(std::string(who) + ": no voxels registered"); return BALM_ERR_INVALID; }
+  Rig *rg = c->rig;
+  const int nr = rig_n(rg);
+  if (anchor < -1 || anchor >= rig_free_bases(rg)) {
+    balm_set_error(std::string(who) + ": anchor " + std::to_string(anchor) + " is neither -1 nor a free base index in [0, " +
+                   std::to_string(rig_free_bases(rg)) + ")");
+    return BALM_ERR_INVALID;
+  }
+  const int a0 = anchor < 0 ? -1 : 6 * anchor;
+  CUDA_TRY(cudaSetDevice(c->device));
+  TRY(rig_upload(c, base12, ext12));
+  const double *st = rig_state(rg, false);
+  ScratchPool pool;
+  double *R = nullptr, *raw_rig = nullptr;
+  TRY(pool.get(&raw_rig, (size_t)nr * nr));
+  TRY(rig_compose(rg, c->stream, st, c->poses, &c->launches));
+  TRY(cov_raw_dev(c, pool, c->poses, c_cov81, point_noise, include_fix != 0, &R));
+  TRY(rig_reduce_raw(rg, c->stream, st, R, raw_rig, &c->launches));
+  if (a0 >= 0) TRY(cov_delete_block(c, raw_rig, nr, a0, 0.0));
+  const DenseSystem sys = rig_system(rg);
+  if (cov) {
+    // H_rig at the same state (the evaluation deferred: its events are read after cov_factor's wait), the anchor
+    // deleted with 1 on its diagonal, factored undamped
+    c->defer = true;
+    int rc = rig_evaluate_dev(c, include_fix != 0);
+    c->defer = false;
+    // the rig owns H_rig: the deletion edits it in place, and the next evaluation rewrites it
+    if (rc == BALM_OK && a0 >= 0) rc = cov_delete_block(c, const_cast<double *>(sys.H), nr, a0, 1.0);
+    if (rc == BALM_OK)
+      rc = cov_factor(c, sys, a0, "balm_rig_covariance: H_rig is singular (a gauge or an unobservable direction of the "
+                                  "rig is not fixed: fix clusters, fixed unknowns or an anchor)");
+    if (rc == BALM_OK || rc == BALM_ERR_NOT_PD) {  // the stream has been synchronised
+      const int rc2 = collect_eval(c);
+      if (rc2 != BALM_OK) rc = rc2;
+      else TRY(rig_collect_reduce(c));
+    }
+    c->pending_eval = false;
+    TRY(rc);
+  }
+  if (raw) CUDA_TRY(cudaMemcpyAsync(raw, raw_rig, sizeof(double) * nr * nr, cudaMemcpyDeviceToHost, c->stream));
+  if (cov) {
+    TRY(cov_sandwich(c, sys, raw_rig));
+    if (a0 >= 0) TRY(cov_delete_block(c, raw_rig, nr, a0, 0.0));
+    CUDA_TRY(cudaMemcpyAsync(cov, raw_rig, sizeof(double) * nr * nr, cudaMemcpyDeviceToHost, c->stream));
+  }
+  CUDA_TRY(cudaStreamSynchronize(c->stream));
+  return BALM_OK;
+}
+
 // balm_damping_iter's loop on the rig cost: per iteration compose -> evaluate -> reduce -> solve -> rig update ->
 // compose the trial state -> trial residual, then the one wait. No hand-over and no speculation: every evaluation is
 // the pure function balm_evaluate is.

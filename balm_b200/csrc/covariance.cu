@@ -208,30 +208,39 @@ __global__ void scale_rows_kernel(double *B, const double *dinv, int n) {
   if (i < n) B[(size_t)j * n + i] *= dinv[i];
 }
 
-// B <- (L D L^T)^-1 B for all n columns: forward sweep (B_j <- X_j B_j, rows below -= L21 B_j), rows scaled by 1/d,
-// backward sweep (B_j <- X_j^T (B_j - sum_{r>j} L_rj^T B_r))
-int solve_many(balm_ctx *c, double *B) {
-  const int n = c->n, ct = (n + NB - 1) / NB;
+// B <- (L D L^T)^-1 B for all n columns of s's last factor: forward sweep (B_j <- X_j B_j, rows below -= L21 B_j),
+// rows scaled by 1/d, backward sweep (B_j <- X_j^T (B_j - sum_{r>j} L_rj^T B_r))
+int solve_many(balm_ctx *c, const DenseSystem &s, double *B) {
+  const int n = s.n, ct = (n + NB - 1) / NB;
   cudaStream_t st = c->stream;
   int launches = 0;
   for (int j0 = 0, pi = 0; j0 < n; j0 += NB, pi++) {
     const int nbw = std::min(NB, n - j0), m = n - j0 - nbw;
-    mrhs_diag_kernel<0><<<ct, 256, MRHS_SMEM, st>>>(c->lw.Xinv + (size_t)pi * NB * NB, B, n, j0, nbw, nullptr);
-    if (m > 0) mrhs_fwd_update_kernel<<<dim3((m + NB - 1) / NB, ct), 256, MRHS_SMEM, st>>>(c->A, B, n, j0, nbw);
+    mrhs_diag_kernel<0><<<ct, 256, MRHS_SMEM, st>>>(s.w->Xinv + (size_t)pi * NB * NB, B, n, j0, nbw, nullptr);
+    if (m > 0) mrhs_fwd_update_kernel<<<dim3((m + NB - 1) / NB, ct), 256, MRHS_SMEM, st>>>(s.A, B, n, j0, nbw);
     launches += 2;
   }
-  scale_rows_kernel<<<dim3((n + 255) / 256, n), 256, 0, st>>>(B, c->lw.dinv, n);
+  scale_rows_kernel<<<dim3((n + 255) / 256, n), 256, 0, st>>>(B, s.w->dinv, n);
   launches++;
   const int npan = (n + NB - 1) / NB;
   for (int pi = npan - 1; pi >= 0; pi--) {
     const int j0 = pi * NB, nbw = std::min(NB, n - j0);
-    if (j0 + nbw < n) mrhs_bwd_update_kernel<<<ct, 256, MRHS_SMEM, st>>>(c->A, B, n, j0, nbw);
-    mrhs_diag_kernel<1><<<ct, 256, MRHS_SMEM, st>>>(c->lw.Xinv + (size_t)pi * NB * NB, B, n, j0, nbw, nullptr);
+    if (j0 + nbw < n) mrhs_bwd_update_kernel<<<ct, 256, MRHS_SMEM, st>>>(s.A, B, n, j0, nbw);
+    mrhs_diag_kernel<1><<<ct, 256, MRHS_SMEM, st>>>(s.w->Xinv + (size_t)pi * NB * NB, B, n, j0, nbw, nullptr);
     launches += 2;
   }
   c->launches += launches;
   CUDA_TRY(cudaGetLastError());
   return BALM_OK;
+}
+
+// rows and columns [a0, a0 + 6) of the n x n matrix A set to 0, diagonal to diag
+__global__ void delete_block_kernel(double *A, int n, int a0, double diag) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x, k = blockIdx.y;
+  if (i >= n) return;
+  const double v = i == a0 + k ? diag : 0.0;
+  A[(size_t)(a0 + k) * n + i] = v;  // column a0 + k
+  A[(size_t)i * n + a0 + k] = v;    // row a0 + k
 }
 
 }  // namespace
@@ -247,13 +256,11 @@ int covariance_setup() {
 // Defined in balm_api.cu
 int balm_cov_evaluate_hessian(balm_ctx *c, const double *poses_dev, bool include_fix);
 
-int pose_covariance_dev(balm_ctx *c, const double *poses_dev, const double *ccov_host, double point_noise, bool include_fix,
-                        double *Rraw_host, double *Rcov_host) {
+int cov_raw_dev(balm_ctx *c, ScratchPool &pool, const double *poses_dev, const double *ccov_host, double point_noise,
+                bool include_fix, double **R_out) {
   const int n = c->n, N = c->N;
   const int64_t M = c->M, K = c->K;
   cudaStream_t st = c->stream;
-  if (M < 1) { balm_set_error("balm_pose_covariance: no voxels registered"); return BALM_ERR_INVALID; }
-  ScratchPool pool;
   // voxels per batch: the stats table holds VB voxels; the row buffer gets its own budget
   size_t budget = (size_t)4 << 30;
   if (const char *e = getenv("BALM_COV_BUDGET_MB")) budget = (size_t)atoll(e) << 20;
@@ -290,27 +297,70 @@ int pose_covariance_dev(balm_ctx *c, const double *poses_dev, const double *ccov
   }
   TRY(launch_csc_batch(c, 0, M));
   TRY(launch_assemble(c, Dacc, R));
+  *R_out = R;
+  return BALM_OK;
+}
+
+int cov_factor(balm_ctx *c, const DenseSystem &s, int skip, const char *singular_msg) {
+  const int n = s.n;
+  cudaStream_t st = c->stream;
+  TRY(launch_ldlt_solve(c, s, 0.0));
+  CUDA_TRY(cudaMemcpyAsync(c->h_flags, c->flags, sizeof(int), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  // a singular H (free gauge: no fix clusters in it) does not produce an exact zero pivot in floating point but
+  // pivots at rounding level relative to the others: refuse instead of returning 1e16-sized garbage
+  std::vector<double> dinv_h((size_t)n);
+  CUDA_TRY(cudaMemcpy(dinv_h.data(), s.w->dinv, sizeof(double) * n, cudaMemcpyDeviceToHost));
+  double dmin = 1e300, dmax = 0.0;
+  for (int i = 0; i < n; i++) {
+    if (skip >= 0 && i >= skip && i < skip + 6) continue;
+    const double d = fabs(1.0 / dinv_h[i]);
+    dmin = std::min(dmin, d);
+    dmax = std::max(dmax, d);
+  }
+  if (c->h_flags[0] || !(dmin > 1e-11 * dmax)) {
+    balm_set_error(singular_msg);
+    return BALM_ERR_NOT_PD;
+  }
+  return BALM_OK;
+}
+
+int cov_sandwich(balm_ctx *c, const DenseSystem &s, double *B) {
+  const int n = s.n;
+  TRY(solve_many(c, s, B));                                   // H^-1 B
+  transpose_inplace_kernel<<<dim3((n + 31) / 32, (n + 31) / 32), dim3(32, 32), 0, c->stream>>>(B, n);
+  TRY(solve_many(c, s, B));                                   // H^-1 (H^-1 B)^T = H^-1 B H^-T
+  c->launches += 1;
+  CUDA_TRY(cudaGetLastError());
+  return BALM_OK;
+}
+
+int cov_delete_block(balm_ctx *c, double *A, int n, int a0, double diag) {
+  delete_block_kernel<<<dim3((n + 127) / 128, 6), 128, 0, c->stream>>>(A, n, a0, diag);
+  c->launches += 1;
+  CUDA_TRY(cudaGetLastError());
+  return BALM_OK;
+}
+
+// Defined in balm_api.cu
+int balm_cov_evaluate_hessian(balm_ctx *c, const double *poses_dev, bool include_fix);
+
+int pose_covariance_dev(balm_ctx *c, const double *poses_dev, const double *ccov_host, double point_noise, bool include_fix,
+                        double *Rraw_host, double *Rcov_host) {
+  const int n = c->n;
+  cudaStream_t st = c->stream;
+  if (c->M < 1) { balm_set_error("balm_pose_covariance: no voxels registered"); return BALM_ERR_INVALID; }
+  ScratchPool pool;
+  double *R = nullptr;
+  TRY(cov_raw_dev(c, pool, poses_dev, ccov_host, point_noise, include_fix, &R));
   if (Rraw_host) CUDA_TRY(cudaMemcpyAsync(Rraw_host, R, sizeof(double) * (size_t)n * n, cudaMemcpyDeviceToHost, st));
   if (Rcov_host) {
     // H at these poses (divide_thread, BAs_left.hpp:1091), factored without damping, then H^-1 R H^-T
     TRY(balm_cov_evaluate_hessian(c, poses_dev, include_fix));
-    TRY(launch_ldlt_solve(c, ctx_system(c), 0.0));
-    CUDA_TRY(cudaMemcpyAsync(c->h_flags, c->flags, sizeof(int), cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
-    // a singular H (free gauge: no fix clusters in it) does not produce an exact zero pivot in floating point but
-    // pivots at rounding level relative to the others: refuse instead of returning 1e16-sized garbage
-    std::vector<double> dinv_h((size_t)n);
-    CUDA_TRY(cudaMemcpy(dinv_h.data(), c->lw.dinv, sizeof(double) * n, cudaMemcpyDeviceToHost));
-    double dmin = 1e300, dmax = 0.0;
-    for (int i = 0; i < n; i++) { const double d = fabs(1.0 / dinv_h[i]); dmin = std::min(dmin, d); dmax = std::max(dmax, d); }
-    if (c->h_flags[0] || !(dmin > 1e-11 * dmax)) {
-      balm_set_error("balm_pose_covariance: H is singular (gauge freedom not fixed: no fix clusters in the Hessian)");
-      return BALM_ERR_NOT_PD;
-    }
-    TRY(solve_many(c, R));                                   // H^-1 R
-    transpose_inplace_kernel<<<dim3((n + 31) / 32, (n + 31) / 32), dim3(32, 32), 0, st>>>(R, n);
-    TRY(solve_many(c, R));                                   // H^-1 (H^-1 R)^T = H^-1 R H^-T
-    c->launches += 1;
+    const DenseSystem sys = ctx_system(c);
+    TRY(cov_factor(c, sys, -1,
+                   "balm_pose_covariance: H is singular (gauge freedom not fixed: no fix clusters in the Hessian)"));
+    TRY(cov_sandwich(c, sys, R));
     CUDA_TRY(cudaMemcpyAsync(Rcov_host, R, sizeof(double) * (size_t)n * n, cudaMemcpyDeviceToHost, st));
   }
   CUDA_TRY(cudaStreamSynchronize(st));

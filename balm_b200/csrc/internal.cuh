@@ -826,6 +826,18 @@ inline DenseSystem ctx_system(balm_ctx *c) { return DenseSystem{c->n, c->H, c->g
 int launch_ldlt_solve(balm_ctx *c, const DenseSystem &s, double u);
 // fp64 iterative refinement of s.dx with the factors of the last launch_ldlt_solve of s (waits)
 int refine_solution(balm_ctx *c, const DenseSystem &s, int *still_bad);
+// ---- pose-covariance pieces (covariance.cu) ----
+// Rcov_raw at the device poses into a new n x n buffer of pool, *R_out (enqueued; the voxel statistics, G rows, SYRK
+// partials and the assembly of balm_pose_covariance)
+int cov_raw_dev(balm_ctx *c, ScratchPool &pool, const double *poses_dev, const double *ccov_host, double point_noise,
+                bool include_fix, double **R_out);
+// undamped LDL^T of s (launch_ldlt_solve with u = 0), then one wait: BALM_ERR_NOT_PD with singular_msg for a bad pivot
+// or min |d| not above 1e-11 max |d|, pivots [skip, skip + 6) left out of both (skip -1: none)
+int cov_factor(balm_ctx *c, const DenseSystem &s, int skip, const char *singular_msg);
+// B <- H^-1 B H^-T with the factors of the last cov_factor of s (enqueued)
+int cov_sandwich(balm_ctx *c, const DenseSystem &s, double *B);
+// rows and columns [a0, a0 + 6) of the n x n matrix A set to 0, its diagonal there to diag (enqueued)
+int cov_delete_block(balm_ctx *c, double *A, int n, int a0, double diag);
 int launch_pose_update(balm_ctx *c, const double *poses_in, const double *dx, double *poses_out);
 int launch_pose_update(cudaStream_t st, int N, const double *poses_in, const double *dx, double *poses_out);
 int launch_gauge(balm_ctx *c, double *poses, int mode);
@@ -915,6 +927,7 @@ int rig_n(const Rig *r);  // n_rig = 6 x free unknowns
 int rig_bases(const Rig *r);
 int rig_lidars(const Rig *r);
 bool rig_any_base_fixed(const Rig *r);
+int rig_free_bases(const Rig *r);  // free base poses: free indices [0, rig_free_bases) are base poses
 // the reduced system H_rig | g_rig, dx, and the rig's own factor workspaces
 DenseSystem rig_system(Rig *r);
 // device [12 (B + L)] base poses then extrinsics: the current state, or the trial one; rig_swap_states exchanges them
@@ -926,6 +939,10 @@ int rig_compose(const Rig *r, cudaStream_t st, const double *state, double *pose
 // blocks plus the second-order correction, each sum in ascending slot order, mirrored; no atomics
 int rig_reduce(const Rig *r, cudaStream_t st, const double *state, const double *H, const double *g,
                long long *launches);
+// raw_rig = J^T R J at state for any symmetric R [6N x 6N] (enqueued): rig_reduce's sums without the correction and
+// without g, through the rig's K, into out [n_rig x n_rig] (column-major, mirrored)
+int rig_reduce_raw(const Rig *r, cudaStream_t st, const double *state, const double *R, double *out,
+                   long long *launches);
 // state_out = the left step of the rig's dx on every free unknown of state, fixed ones copied (enqueued)
 int rig_update(const Rig *r, cudaStream_t st, const double *state, double *state_out, long long *launches);
 

@@ -16,6 +16,7 @@
 
 struct Rig {
   int N = 0, B = 0, L = 0, F = 0;  // slots, bases, extrinsics, free unknowns (n_rig = 6F)
+  int FB = 0;                      // free base poses (the first FB free unknowns)
   int *base_of = nullptr;          // [N]
   int *var_of = nullptr;           // [B + L] free index of every unknown, -1 when fixed
   int *var_unknown = nullptr;      // [F] the unknown of every free index (< B: a base pose, else extrinsic - B)
@@ -133,9 +134,10 @@ __device__ __forceinline__ double rig_correction(const double *r, const double *
   return (a == k ? gtp : 0.0) - 0.5 * (rag * rkp + rap * rkg);
 }
 
-// H_rig[r, c] = sum over the slots s of r's unknown u, ascending, of J_s[:, a]^T K[6s .. 6s+5, c], then the
-// correction over the same slots, ascending; lower triangle only, mirrored into the upper one. Column c = n_rig is g:
-// g_rig[r] = sum_s J_s[:, a]^T g_s. One thread per row r, one grid row per column c.
+// H_rig[r, c] = sum over the slots s of r's unknown u, ascending, of J_s[:, a]^T K[6s .. 6s+5, c], then (CORRECTION)
+// the correction over the same slots, ascending; lower triangle only, mirrored into the upper one. Column c = n_rig is
+// g: g_rig[r] = sum_s J_s[:, a]^T g_s. One thread per row r, one grid row per column c.
+template <bool CORRECTION>
 __global__ void __launch_bounds__(128) rig_jtk_kernel(const double *__restrict__ K, const double *__restrict__ g, int n,
                                                       int nr, const double *state, const int *base_of,
                                                       const int *var_unknown, const int *var_ptr, const int *var_slot,
@@ -160,7 +162,7 @@ __global__ void __launch_bounds__(128) rig_jtk_kernel(const double *__restrict__
     load_pose(state + 12 * (size_t)base_of[s], r, p);
     acc += ad_column_dot(r, p, a, x + 6 * s);
   }
-  if (!grad && lidar) {
+  if (CORRECTION && !grad && lidar) {
     const int kv = var_unknown[col / 6], k = col % 6;
     if (kv == ku || kv < B) {
       for (int q = var_ptr[u]; q < var_ptr[u + 1]; q++) {
@@ -205,6 +207,7 @@ int rig_build(cudaStream_t st, int N, int B, int L, const int32_t *base_of, cons
     const bool fixed = j < B ? (base_fixed && base_fixed[j]) : (lidar_fixed && lidar_fixed[j - B]);
     if (j < B && fixed) r->any_base_fixed = true;
     if (fixed) continue;
+    if (j < B) r->FB++;
     var_of[j] = (int)var_unknown.size();
     var_unknown.push_back(j);
   }
@@ -245,6 +248,7 @@ int rig_n(const Rig *r) { return 6 * r->F; }
 int rig_bases(const Rig *r) { return r->B; }
 int rig_lidars(const Rig *r) { return r->L; }
 bool rig_any_base_fixed(const Rig *r) { return r->any_base_fixed; }
+int rig_free_bases(const Rig *r) { return r->FB; }
 DenseSystem rig_system(Rig *r) {
   const int nr = 6 * r->F;
   return DenseSystem{nr, r->H, r->H + (size_t)nr * nr, r->dx, r->dvec, r->A, &r->lw};
@@ -264,9 +268,22 @@ int rig_reduce(const Rig *r, cudaStream_t st, const double *state, const double 
   const int n = 6 * r->N, nr = 6 * r->F;
   rig_k_kernel<<<dim3((n + 127) / 128, r->F), 128, 0, st>>>(H, n, state, r->base_of, r->var_unknown, r->var_ptr,
                                                             r->var_slot, r->B, r->K);
-  rig_jtk_kernel<<<dim3((nr + 127) / 128, nr + 1), 128, 0, st>>>(r->K, g, n, nr, state, r->base_of, r->var_unknown,
-                                                                 r->var_ptr, r->var_slot, r->B, r->H,
-                                                                 r->H + (size_t)nr * nr);
+  rig_jtk_kernel<true><<<dim3((nr + 127) / 128, nr + 1), 128, 0, st>>>(r->K, g, n, nr, state, r->base_of,
+                                                                       r->var_unknown, r->var_ptr, r->var_slot, r->B,
+                                                                       r->H, r->H + (size_t)nr * nr);
+  *launches += 2;
+  CUDA_TRY(cudaGetLastError());
+  return BALM_OK;
+}
+
+int rig_reduce_raw(const Rig *r, cudaStream_t st, const double *state, const double *R, double *out,
+                   long long *launches) {
+  const int n = 6 * r->N, nr = 6 * r->F;
+  rig_k_kernel<<<dim3((n + 127) / 128, r->F), 128, 0, st>>>(R, n, state, r->base_of, r->var_unknown, r->var_ptr,
+                                                            r->var_slot, r->B, r->K);
+  rig_jtk_kernel<false><<<dim3((nr + 127) / 128, nr), 128, 0, st>>>(r->K, nullptr, n, nr, state, r->base_of,
+                                                                    r->var_unknown, r->var_ptr, r->var_slot, r->B,
+                                                                    out, nullptr);
   *launches += 2;
   CUDA_TRY(cudaGetLastError());
   return BALM_OK;

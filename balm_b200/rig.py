@@ -32,6 +32,14 @@ def rig_poses(base12, ext12, base_of, lidar_of):
     return out
 
 
+def extrinsic_sigmas(cov, n_free_bases):
+    """1-sigma rotation (rad) and translation (m) of every free extrinsic from a rig covariance (Context.rig_covariance's
+    cov; the free extrinsics follow the n_free_bases free base poses, 6 each as (phi, t)) -> (rot, trans), each
+    (free extrinsics x 3), the square roots of the 6 x 6 blocks' diagonals."""
+    d = np.sqrt(np.diag(np.asarray(cov, dtype=np.float64))[6 * n_free_bases:]).reshape(-1, 6)
+    return d[:, :3], d[:, 3:]
+
+
 def calibrate_rig(xyz, scan, base_of, lidar_of, base12, ext12, voxel_size=2.0, rounds=3, fixed_bases=(),
                   fixed_lidars=(0,), precision=L.PREC_TENSOR, device=0, layer_limit=2, min_ps=15,
                   eigen_value_array=(1.0 / 16, 1.0 / 16, 1.0 / 9), max_iter=10, gauge_mode=2, min_planes_per_pose=0,

@@ -479,6 +479,23 @@ int balm_set_rig(balm_ctx *ctx, int n_base, int n_lidar, const int32_t *base_of,
  * BALM_ERR_INVALID without a rig or registered voxels. */
 int balm_rig_evaluate(balm_ctx *ctx, const double *base12, const double *ext12, int include_fix, double *H, double *g,
                       double *residual);
+/* Point noise propagated to the rig's unknowns (DESIGN.md "Rig covariance"), at base12 / ext12 (normally the output of
+ * balm_rig_damping_iter). With X_s the composed scan poses, R balm_pose_covariance's Rcov_raw at them (c_cov81,
+ * point_noise and include_fix as there) and J the rig's first-order Jacobian of balm_rig_evaluate:
+ *   raw = J^T R J,   cov = H~^-1 raw~ H~^-T,
+ * H balm_rig_evaluate's H_rig at the same state and include_fix, factored without damping. anchor: -1, or the free
+ * index of a free base pose (in [0, free bases)), whose 6 rows and columns are deleted from H_rig and raw (as the
+ * anchor of balm_block_covariance); its entries are exactly 0 in both outputs. With free base poses and no fix clusters
+ * the cost keeps the base poses' left gauge: pass a base anchor; the extrinsic block of cov does not depend on which.
+ * LiDAR-to-INS (every base pose fixed) uses -1. Both outputs are n_rig x n_rig, column-major, in balm_set_rig's order;
+ * either may be NULL (not both), and without cov no H_rig is evaluated. BALM_ERR_INVALID, nothing written, without a
+ * rig, with a communicator attached, without registered voxels, for a NULL state, or for an anchor that is neither -1
+ * nor a free base index (an extrinsic cannot be the anchor). BALM_ERR_NOT_PD, nothing written, when H~ is singular
+ * (balm_pose_covariance's pivot test over the pivots outside the anchor). The rig's state, the poses and the next
+ * balm_rig_damping_iter are unaffected. Device memory on top of the rig's: R ((6N)^2 doubles) and the scratch of
+ * balm_pose_covariance's raw term, and raw (n_rig^2); the rig's K, H_rig and factor are reused. */
+int balm_rig_covariance(balm_ctx *ctx, const double *base12, const double *ext12, const double *c_cov81,
+                        double point_noise, int include_fix, int anchor, double *raw, double *cov);
 /* balm_damping_iter's LM on the rig cost: the same opts (u0, v0, rel_tol, max_iter, hess_includes_fix, force_hess,
  * verbose; min_planes_per_pose counts voxels per scan slot), accept rule and refinement, with the solve on H_rig.
  * base12 / ext12 are updated in place. rig_per_iter: max_iter x (n_base + n_lidar) x 12 (base poses, then extrinsics,
