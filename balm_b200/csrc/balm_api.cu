@@ -171,6 +171,9 @@ static int alloc_workspaces(balm_ctx *c) {
 }
 
 // ---------------- ctx ----------------
+// balm_create after its argument checks: c's streams, buffers and events (balm_destroy frees a partial c)
+static int ctx_init(balm_ctx *c, int n_poses, int device, int precision);
+
 extern "C" int balm_create(balm_ctx **out, int n_poses, int device, int precision) {
   if (!out || n_poses < 1) { balm_set_error("balm_create: bad arguments"); return BALM_ERR_INVALID; }
   if (precision != BALM_PREC_FP64 && precision != BALM_PREC_TENSOR && precision != BALM_PREC_BLOCKS) {
@@ -182,6 +185,16 @@ extern "C" int balm_create(balm_ctx **out, int n_poses, int device, int precisio
   if (device < 0 || device >= ndev) { balm_set_error("balm_create: no such CUDA device"); return BALM_ERR_CUDA; }
   CUDA_TRY(cudaSetDevice(device));
   balm_ctx *c = new balm_ctx();
+  const int rc = ctx_init(c, n_poses, device, precision);
+  if (rc != BALM_OK) {
+    balm_destroy(c);
+    return rc;
+  }
+  *out = c;
+  return BALM_OK;
+}
+
+static int ctx_init(balm_ctx *c, int n_poses, int device, int precision) {
   c->N = n_poses; c->n = 6 * n_poses; c->device = device; c->prec = precision;
   c->ldg = (c->n + BALM_SYRK_TILE - 1) / BALM_SYRK_TILE * BALM_SYRK_TILE;
   c->Np = (n_poses + 31) / 32 * 32;
@@ -225,14 +238,13 @@ extern "C" int balm_create(balm_ctx **out, int n_poses, int device, int precisio
   CUDA_TRY(cudaMallocHost((void **)&c->h_flags, 8 * sizeof(int)));
   memset(c->h_flags, 0, 8 * sizeof(int));
   for (auto &e : c->ev) CUDA_TRY(cudaEventCreate(&e));
-  *out = c;
   return BALM_OK;
 }
 
 extern "C" int balm_destroy(balm_ctx *c) {
   if (!c) return BALM_OK;
   cudaSetDevice(c->device);
-  cudaStreamSynchronize(c->stream);
+  if (c->stream) cudaStreamSynchronize(c->stream);
   free_problem(c);
   window_free(c->win);
   pose_graph_free(c->pg);
@@ -248,7 +260,7 @@ extern "C" int balm_destroy(balm_ctx *c) {
   cudaFree(c->tc_trace);
   cudaFreeHost(c->h_scal); cudaFreeHost(c->h_flags);
   for (auto &e : c->ev) if (e) cudaEventDestroy(e);
-  cudaStreamDestroy(c->stream);
+  if (c->stream) cudaStreamDestroy(c->stream);
   delete c;
   return BALM_OK;
 }
@@ -351,11 +363,11 @@ static int upload_aos(balm_ctx *c, const double *aos, bool aos_on_device, double
 }
 
 // An empty voxel set: evaluations give H = 0, g = 0, r = 0 (and still take part in the all-reduce).
-static int register_empty(balm_ctx *c) {
+static int register_empty(balm_ctx *c, const char *who = "blocks registration") {
   free_problem(c);
   CUDA_TRY(cudaMemsetAsync(c->planes, 0, sizeof(int) * c->N, c->stream));
   c->dense = true; c->max_k = 0; c->min_planes = 0; c->VB = 0;
-  if (c->prec == BALM_PREC_BLOCKS) TRY(block_hessian_build(c, "blocks registration"));  // every diagonal pair, no term
+  if (c->prec == BALM_PREC_BLOCKS) TRY(block_hessian_build(c, who));  // no term
   c->registered = true;
   return BALM_OK;
 }
@@ -579,12 +591,13 @@ static int evaluate_dev(balm_ctx *c, const double *poses, int64_t head, int64_t 
   if (!c->registered) { balm_set_error("no voxels registered"); return BALM_ERR_INVALID; }
   if (head < 0 || end > c->M || head > end) { balm_set_error("evaluate: bad voxel range"); return BALM_ERR_INVALID; }
   double *r_dev = c->g + c->n;  // contiguous with H and g -> one all-reduce
-  CUDA_TRY(cudaMemsetAsync(r_dev, 0, sizeof(double), c->stream));
   float ms;
   bool first = true;
   // defer mode (LM loop, whole problem in one batch): nothing is waited for here; collect_eval() reads the events and
-  // the tensor path's flags after the iteration's single synchronisation
-  const bool deferred = c->defer && head == 0 && end == c->M && c->VB >= c->M && end > head;
+  // the tensor path's flags after the iteration's single synchronisation. A blocks context without voxels (the sparse
+  // pose graph) defers too: its full range is the factors and priors.
+  const bool deferred = c->defer && head == 0 && end == c->M && c->VB >= c->M &&
+                        (end > head || c->prec == BALM_PREC_BLOCKS);
   // a blocks context's pose factors are part of every full-range evaluation (sub-ranges stay voxels only)
   const bool factors = c->prec == BALM_PREC_BLOCKS && c->pg && head == 0 && end == c->M;
   const bool priors = c->prec == BALM_PREC_BLOCKS && c->pr && head == 0 && end == c->M;  // so are its pose priors
@@ -593,11 +606,11 @@ static int evaluate_dev(balm_ctx *c, const double *poses, int64_t head, int64_t 
     // the all-reduce below, which the other ranks of a multi-GPU job are waiting in
     if (c->prec == BALM_PREC_BLOCKS) {
       TRY(blocks_zero(c));
-      CUDA_TRY(cudaMemsetAsync(c->g, 0, sizeof(double) * ((size_t)c->n + 1), c->stream));
     } else {
       CUDA_TRY(cudaMemsetAsync(c->H, 0, sizeof(double) * ((size_t)c->n * c->n + c->n + 1), c->stream));
     }
-    for (int e = 0; e <= 5; e++) CUDA_TRY(cudaEventRecord(c->ev[e], c->stream));
+  } else {
+    CUDA_TRY(cudaMemsetAsync(r_dev, 0, sizeof(double), c->stream));
   }
   for (int64_t v0 = head; v0 < end; v0 += c->VB) {
     const int64_t v1 = std::min(end, v0 + c->VB);
@@ -627,14 +640,15 @@ static int evaluate_dev(balm_ctx *c, const double *poses, int64_t head, int64_t 
     }
     first = false;
   }
-  CUDA_TRY(cudaMemcpyAsync(c->scal + BALM_SCAL_RCUR, r_dev, sizeof(double), cudaMemcpyDeviceToDevice, c->stream));  // local, pre all-reduce
+  if (end > head)  // local, pre all-reduce; the hand-over needs every voxel, so an empty range hands nothing over
+    CUDA_TRY(cudaMemcpyAsync(c->scal + BALM_SCAL_RCUR, r_dev, sizeof(double), cudaMemcpyDeviceToDevice, c->stream));
+  CUDA_TRY(cudaEventRecord(c->ev[4], c->stream));
   if (end > head || factors || priors) {
-    CUDA_TRY(cudaEventRecord(c->ev[4], c->stream));
     if (c->prec != BALM_PREC_BLOCKS) TRY(launch_assemble(c));
     if (factors) TRY(blocks_add_factors(c, poses));  // after the RCUR copy above: the hand-over caches voxels only
     if (priors) TRY(blocks_add_priors(c, poses));
-    CUDA_TRY(cudaEventRecord(c->ev[5], c->stream));
   }
+  CUDA_TRY(cudaEventRecord(c->ev[5], c->stream));
   if (c->world > 1 && c->comm) {  // the assembly wrote the lower triangle | g into c->Hpack (an empty range: zeros)
     const int n = c->n;
     const size_t tri = (size_t)n * (n + 1) / 2, cnt = tri + n + 1;
@@ -663,10 +677,12 @@ static int collect_eval(balm_ctx *c) {
   if (!c->pending_eval) return BALM_OK;
   c->pending_eval = false;
   float ms;
-  cudaEventElapsedTime(&ms, c->ev[0], c->ev[1]);
-  if (!c->pending_stats_cached) { c->tm.ms_stats += ms; c->tm.n_stats += 1; }
-  cudaEventElapsedTime(&ms, c->ev[1], c->ev[2]); c->tm.ms_obs += ms;
-  cudaEventElapsedTime(&ms, c->ev[2], c->ev[3]); c->tm.ms_syrk += ms;
+  if (c->M > 0) {  // deferred evaluations are full-range: the voxel phases ran (a voxel-free blocks context has none)
+    cudaEventElapsedTime(&ms, c->ev[0], c->ev[1]);
+    if (!c->pending_stats_cached) { c->tm.ms_stats += ms; c->tm.n_stats += 1; }
+    cudaEventElapsedTime(&ms, c->ev[1], c->ev[2]); c->tm.ms_obs += ms;
+    cudaEventElapsedTime(&ms, c->ev[2], c->ev[3]); c->tm.ms_syrk += ms;
+  }
   cudaEventElapsedTime(&ms, c->ev[4], c->ev[5]);
   if (c->prec != BALM_PREC_BLOCKS || c->pg || c->pr) c->tm.ms_assemble += ms;  // deferred: always full range
   cudaEventElapsedTime(&ms, c->ev[5], c->ev[6]); c->tm.ms_allreduce += ms;
@@ -770,35 +786,26 @@ extern "C" int balm_voxel_residuals(balm_ctx *c, const double *poses12, int64_t 
   return BALM_OK;
 }
 
-// The outcome of a damped solve once its stream has been waited for, from the owner's pinned mirrors of scal / flags
-// (balm_ctx's layout, which balm_spg shares): q1 = h_scal[1], not_pd on a bad pivot (h_flags[0]) or a non-finite q1.
-// When the backward-error check failed (h_flags[4]: an indefinite H + uD factored without pivoting lost digits),
-// `refine` refines dx in fp64 with the same factors and leaves the new q1 in h_scal[1]; if that does not bring the
-// error down (*still_bad), the step counts as not_pd. Returns 1 in *refined when dx changed (the caller re-applies
-// the update).
-static int solve_outcome(const double *h_scal, const int *h_flags, const std::function<int(int *still_bad)> &refine,
-                         double *q1, int *not_pd, int *refined) {
-  *q1 = h_scal[1];
-  *not_pd = h_flags[0] != 0 || !std::isfinite(*q1);
-  *refined = 0;
-  if (h_flags[4] == 0 || *not_pd) return BALM_OK;
-  int still_bad = 0;
-  TRY(refine(&still_bad));
-  *q1 = h_scal[1];
-  *refined = 1;
-  if (still_bad || !std::isfinite(*q1)) *not_pd = 1;
-  return BALM_OK;
-}
-
-// The context's solve of sys after the wait: its time, then its outcome (solve_outcome)
+// The context's solve of sys once its stream has been waited for: its time, then its outcome from the pinned mirrors of
+// scal / flags: q1 = h_scal[1], not_pd on a bad pivot (h_flags[0]) or a non-finite q1. When the backward-error check
+// failed (h_flags[4]: an indefinite H + uD factored without pivoting lost digits), dx is refined in fp64 with the same
+// factors, which leaves the new q1 in h_scal[1]; if that does not bring the error down, the step counts as not_pd.
+// Returns 1 in *refined when dx changed (the caller re-applies the update).
 static int collect_solve(balm_ctx *c, const DenseSystem &sys, double *q1, int *not_pd, int *refined) {
   float ms;
   cudaEventElapsedTime(&ms, c->ev[9], c->ev[10]);
   c->tm.ms_solve += ms;
   c->tm.n_solve += 1;
-  return solve_outcome(c->h_scal, c->h_flags, [c, &sys](int *still_bad) {
-    return c->prec == BALM_PREC_BLOCKS ? blocks_refine(c, still_bad) : refine_solution(c, sys, still_bad);
-  }, q1, not_pd, refined);
+  *q1 = c->h_scal[1];
+  *not_pd = c->h_flags[0] != 0 || !std::isfinite(*q1);
+  *refined = 0;
+  if (c->h_flags[4] == 0 || *not_pd) return BALM_OK;
+  int still_bad = 0;
+  TRY(c->prec == BALM_PREC_BLOCKS ? blocks_refine(c, &still_bad) : refine_solution(c, sys, &still_bad));
+  *q1 = c->h_scal[1];
+  *refined = 1;
+  if (still_bad || !std::isfinite(*q1)) *not_pd = 1;
+  return BALM_OK;
 }
 
 // The damped solve of sys (the context's own system, or a rig's; a blocks context solves its blocks instead),
@@ -809,8 +816,12 @@ static int solve_dev(balm_ctx *c, const DenseSystem &sys, double u) {
   else TRY(launch_ldlt_solve(c, sys, u));
   CUDA_TRY(cudaEventRecord(c->ev[10], c->stream));
   CUDA_TRY(cudaMemcpyAsync(c->h_scal + 1, c->scal + 1, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
-  CUDA_TRY(cudaMemcpyAsync(c->h_flags, c->flags, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-  CUDA_TRY(cudaMemcpyAsync(c->h_flags + 4, c->flags + 4, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+  if (c->prec == BALM_PREC_BLOCKS) {  // no tensor-path flags in 1..3 to keep: flags 0..4 in one copy
+    CUDA_TRY(cudaMemcpyAsync(c->h_flags, c->flags, sizeof(int) * 5, cudaMemcpyDeviceToHost, c->stream));
+  } else {
+    CUDA_TRY(cudaMemcpyAsync(c->h_flags, c->flags, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+    CUDA_TRY(cudaMemcpyAsync(c->h_flags + 4, c->flags + 4, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+  }
   return BALM_OK;
 }
 
@@ -843,8 +854,8 @@ static int refuse_gauge_with_priors(const char *who, const PriorSet *pr, const b
   return BALM_ERR_INVALID;
 }
 
-// One LM loop's steps, supplied by its owner (balm_damping_iter, balm_rig_damping_iter, balm_pose_graph_iter,
-// balm_spg_iter). Each returns a BALM_* status.
+// One LM loop's steps, supplied by its owner (balm_damping_iter, balm_rig_damping_iter, balm_pose_graph_iter). Each
+// returns a BALM_* status.
 struct LmSteps {
   cudaStream_t st;
   const double *scal;  // the owner's device scalars: eval leaves r1 in scal[0]
@@ -853,7 +864,7 @@ struct LmSteps {
   std::function<int(double u)> solve;                                // the damped solve for dx, enqueued
   std::function<int()> trial;                                        // the trial state from dx, enqueued
   std::function<int(double *r2)> trial_cost;                         // its cost; ends in the iteration's one wait
-  std::function<int(double *q1, int *not_pd, int *refined)> finish;  // the solve's outcome (solve_outcome)
+  std::function<int(double *q1, int *not_pd, int *refined)> finish;  // the solve's outcome (collect_solve)
   std::function<int(bool accepted)> step;                            // accept / reject bookkeeping
   std::function<int(int it)> snapshot;                               // the state after iteration it
 };
@@ -1033,15 +1044,9 @@ extern "C" int balm_set_pose_factors(balm_ctx *c, int n_factors, const int64_t *
   return pose_graph_set(c, n_factors, factor_ptr, factor_pose, poses_hat12, H, status_out);
 }
 
-extern "C" int balm_block_set_factors(balm_ctx *c, int n_factors, const int64_t *factor_ptr, const int32_t *factor_pose,
-                                      const double *poses_hat12, const double *H, int32_t *status_out) {
-  const char *who = "balm_block_set_factors";
-  if (!c) { balm_set_error(std::string(who) + ": bad arguments"); return BALM_ERR_INVALID; }
-  if (c->prec != BALM_PREC_BLOCKS) {
-    balm_set_error(std::string(who) + ": BALM_PREC_BLOCKS contexts only (the dense ones take balm_set_pose_factors)");
-    return BALM_ERR_INVALID;
-  }
-  if (n_factors != 0) TRY(pose_factors_check(who, c->N, n_factors, factor_ptr, factor_pose, poses_hat12, H));
+// balm_block_set_factors and balm_spg_set_factors after their argument checks
+static int block_set_factors(balm_ctx *c, const char *who, int n_factors, const int64_t *factor_ptr,
+                             const int32_t *factor_pose, const double *poses_hat12, const double *H, int32_t *status_out) {
   CUDA_TRY(cudaSetDevice(c->device));
   PoseGraph *pg = nullptr;
   std::vector<int> status;
@@ -1053,6 +1058,18 @@ extern "C" int balm_block_set_factors(balm_ctx *c, int n_factors, const int64_t 
   pose_graph_free(c->pg);
   c->pg = pg_own.release();
   return BALM_OK;
+}
+
+extern "C" int balm_block_set_factors(balm_ctx *c, int n_factors, const int64_t *factor_ptr, const int32_t *factor_pose,
+                                      const double *poses_hat12, const double *H, int32_t *status_out) {
+  const char *who = "balm_block_set_factors";
+  if (!c) { balm_set_error(std::string(who) + ": bad arguments"); return BALM_ERR_INVALID; }
+  if (c->prec != BALM_PREC_BLOCKS) {
+    balm_set_error(std::string(who) + ": BALM_PREC_BLOCKS contexts only (the dense ones take balm_set_pose_factors)");
+    return BALM_ERR_INVALID;
+  }
+  if (n_factors != 0) TRY(pose_factors_check(who, c->N, n_factors, factor_ptr, factor_pose, poses_hat12, H));
+  return block_set_factors(c, who, n_factors, factor_ptr, factor_pose, poses_hat12, H, status_out);
 }
 
 // balm_set_factor_loss / balm_spg_set_factor_loss on the factor set pg (null: none registered)
@@ -1375,276 +1392,6 @@ extern "C" int balm_rig_damping_iter(balm_ctx *c, double *base12, double *ext12,
   return BALM_OK;
 }
 
-// ---------------- sparse pose graph (pose_graph.cu, pose_graph_sparse.cu) ----------------
-struct balm_spg {
-  int N = 0, device = 0;
-  cudaStream_t stream = nullptr;
-  PoseGraph *pg = nullptr;          // the registered factors (null before the first registration)
-  PriorSet *pr = nullptr;           // the registered pose priors (null: none)
-  SparseSolver *solver = nullptr;   // their ordering, symbolic factorisation and captured solve
-  double *blocks = nullptr;         // [pairs][36] H
-  // Only while a prior sits on a pose that no active factor covers: the pattern is the factor pairs united with those
-  // poses' diagonal pairs (upairs), and the factor sums go to blocks[fmap[p]]; otherwise the pattern is the factors'.
-  std::vector<int2> upairs;
-  int *fmap = nullptr;
-  double *poses = nullptr, *poses_trial = nullptr;  // [12N]
-  double *g = nullptr, *dx = nullptr, *dvec = nullptr;  // [6N]
-  double *scal = nullptr;           // device scalars [32], laid out as balm_ctx::scal
-  int *flags = nullptr;             // device flags [8] (0: bad pivot, 4: backward-error check failed)
-  double *h_scal = nullptr;         // pinned [16]
-  int *h_flags = nullptr;           // pinned [8]
-  long long launches = 0;
-  ~balm_spg() {
-    sparse_solver_free(solver);
-    pose_graph_free(pg);
-    prior_set_free(pr);
-    cudaFree(fmap);
-    cudaFree(blocks); cudaFree(poses); cudaFree(poses_trial); cudaFree(g); cudaFree(dx); cudaFree(dvec); cudaFree(scal);
-    cudaFree(flags);
-    cudaFreeHost(h_scal);
-    cudaFreeHost(h_flags);
-    if (stream) cudaStreamDestroy(stream);
-  }
-};
-
-extern "C" int balm_spg_create(balm_spg **out, int n_poses, int device) {
-  if (!out || n_poses < 1 || n_poses > (INT_MAX / 6 - 1)) { balm_set_error("balm_spg_create: bad arguments"); return BALM_ERR_INVALID; }
-  *out = nullptr;
-  CUDA_TRY(cudaSetDevice(device));
-  TRY(pose_graph_setup());
-  std::unique_ptr<balm_spg> s(new balm_spg());
-  s->N = n_poses;
-  s->device = device;
-  const size_t n = 6 * (size_t)n_poses;
-  CUDA_TRY(cudaStreamCreateWithFlags(&s->stream, cudaStreamNonBlocking));
-  TRY(dev_alloc(&s->poses, 12 * (size_t)n_poses));
-  TRY(dev_alloc(&s->poses_trial, 12 * (size_t)n_poses));
-  TRY(dev_alloc(&s->g, n));
-  TRY(dev_alloc(&s->dx, n));
-  TRY(dev_alloc(&s->dvec, n));
-  TRY(dev_alloc(&s->scal, 32));
-  TRY(dev_alloc(&s->flags, 8));
-  CUDA_TRY(cudaMallocHost((void **)&s->h_scal, sizeof(double) * 16));
-  CUDA_TRY(cudaMallocHost((void **)&s->h_flags, sizeof(int) * 8));
-  CUDA_TRY(cudaMemset(s->scal, 0, sizeof(double) * 32));
-  CUDA_TRY(cudaMemset(s->flags, 0, sizeof(int) * 8));
-  *out = s.release();
-  return BALM_OK;
-}
-
-extern "C" void balm_spg_destroy(balm_spg *s) {
-  if (!s) return;
-  cudaSetDevice(s->device);
-  cudaStreamSynchronize(s->stream);
-  delete s;
-}
-
-// A sparse pose graph's block pattern for the factor set pg and the priors pr (either may hold nothing active): the
-// factor pairs, united with the diagonal pair of every pose with an active prior that no factor pair covers. Only such
-// a pose makes the union differ from the factor pattern (grown). Blocks and solver are built here; commit() hands them
-// to the handle.
-struct SpgPattern {
-  bool grown = false;
-  std::vector<int2> upairs;
-  int *fmap = nullptr;
-  double *blocks = nullptr;
-  SparseSolver *solver = nullptr;
-  ~SpgPattern() { sparse_solver_free(solver); cudaFree(fmap); cudaFree(blocks); }
-  const std::vector<int2> &pairs(const PoseGraph *pg) const { return grown ? upairs : pose_graph_pairs(pg); }
-  void commit(balm_spg *s) {
-    sparse_solver_free(s->solver);
-    cudaFree(s->fmap);
-    cudaFree(s->blocks);
-    s->solver = solver;
-    s->fmap = fmap;
-    s->blocks = blocks;
-    s->upairs = std::move(upairs);
-    solver = nullptr;
-    fmap = nullptr;
-    blocks = nullptr;
-  }
-};
-
-static bool pair_less(const int2 &a, const int2 &b) { return a.x < b.x || (a.x == b.x && a.y < b.y); }
-
-// the union's pairs only (no device work): false when the factor pattern already holds every prior pose's diagonal
-static bool spg_union(const PoseGraph *pg, const PriorSet *pr, std::vector<int2> *up, std::vector<int> *fmap) {
-  const std::vector<int2> &fp = pose_graph_pairs(pg);
-  std::vector<int2> extra;
-  if (prior_set_active(pr))
-    for (int i : prior_set_poses(pr))
-      if (!std::binary_search(fp.begin(), fp.end(), make_int2(i, i), pair_less)) extra.push_back(make_int2(i, i));
-  if (extra.empty()) return false;
-  up->resize(fp.size() + extra.size());
-  std::merge(fp.begin(), fp.end(), extra.begin(), extra.end(), up->begin(), pair_less);
-  fmap->resize(fp.size());
-  for (size_t p = 0, q = 0; p < fp.size(); p++) {
-    while ((*up)[q].x != fp[p].x || (*up)[q].y != fp[p].y) q++;
-    (*fmap)[p] = (int)q++;
-  }
-  return true;
-}
-
-static int spg_pattern(balm_spg *s, const PoseGraph *pg, const PriorSet *pr, const char *who, SpgPattern *out) {
-  std::vector<int> fmap;
-  out->grown = spg_union(pg, pr, &out->upairs, &fmap);
-  const std::vector<int2> &pairs = out->pairs(pg);
-  TRY(dev_alloc(&out->blocks, 36 * pairs.size()));
-  if (out->grown) {
-    TRY(dev_alloc(&out->fmap, fmap.size()));
-    CUDA_TRY(cudaMemcpyAsync(out->fmap, fmap.data(), sizeof(int) * fmap.size(), cudaMemcpyHostToDevice, s->stream));
-  }
-  TRY(sparse_solver_build(s->stream, s->N, pairs, out->blocks, s->g, s->dvec, s->dx, s->scal, s->flags, who,
-                          &out->solver));
-  CUDA_TRY(cudaStreamSynchronize(s->stream));
-  return BALM_OK;
-}
-
-extern "C" int balm_spg_set_factors(balm_spg *s, int n_factors, const int64_t *factor_ptr, const int32_t *factor_pose,
-                                    const double *poses_hat12, const double *H, int32_t *status_out) {
-  if (!s) { balm_set_error("balm_spg_set_factors: bad arguments"); return BALM_ERR_INVALID; }
-  TRY(pose_factors_check("balm_spg_set_factors", s->N, n_factors, factor_ptr, factor_pose, poses_hat12, H));
-  CUDA_TRY(cudaSetDevice(s->device));
-  PoseGraph *pg = nullptr;
-  std::vector<int> status;
-  TRY(pose_graph_build(s->stream, s->N, n_factors, factor_ptr, factor_pose, poses_hat12, H, &status, &pg, &s->launches));
-  std::unique_ptr<PoseGraph, void (*)(PoseGraph *)> pg_own(pg, pose_graph_free);
-  SpgPattern pat;
-  TRY(spg_pattern(s, pg, s->pr, "balm_spg_set_factors", &pat));
-  if (s->pr) TRY(prior_set_map(s->pr, s->stream, pat.pairs(pg)));
-  if (status_out) std::copy(status.begin(), status.end(), status_out);
-  pat.commit(s);
-  pose_graph_free(s->pg);
-  s->pg = pg_own.release();
-  return BALM_OK;
-}
-
-// H, g and the cost of the factors and then the priors at the device poses into s->blocks, s->g, s->scal[0] (enqueued)
-static int spg_eval(balm_spg *s, const double *poses) {
-  if (s->fmap) {
-    CUDA_TRY(cudaMemsetAsync(s->blocks, 0, sizeof(double) * 36 * s->upairs.size(), s->stream));
-    TRY(pose_graph_add_blocks(s->pg, s->stream, poses, s->blocks, s->fmap, s->g, s->scal, &s->launches));
-  } else {
-    TRY(pose_graph_eval_blocks(s->pg, s->stream, poses, s->blocks, s->g, s->scal, &s->launches));
-  }
-  if (s->pr) TRY(prior_add_blocks(s->pr, s->stream, poses, s->blocks, s->g, s->scal, &s->launches));
-  return BALM_OK;
-}
-
-static const std::vector<int2> &spg_pairs(const balm_spg *s) { return s->fmap ? s->upairs : pose_graph_pairs(s->pg); }
-
-extern "C" int balm_spg_structure(balm_spg *s, int64_t stats[4], int32_t *pairs) {
-  if (!s || !stats) { balm_set_error("balm_spg_structure: bad arguments"); return BALM_ERR_INVALID; }
-  if (!s->pg) { balm_set_error("balm_spg_structure: no pose factors registered"); return BALM_ERR_INVALID; }
-  const std::vector<int2> &pr = spg_pairs(s);
-  stats[0] = (int64_t)pr.size();
-  sparse_solver_stats(s->solver, &stats[1], &stats[2], &stats[3]);
-  stats[3] += (int64_t)(sizeof(double) * (36 * pr.size() + 2 * 12 * (size_t)s->N + 3 * 6 * (size_t)s->N + 32) +
-                        sizeof(int) * 8) + pose_graph_bytes(s->pg);
-  if (s->fmap) stats[3] += (int64_t)(sizeof(int) * pose_graph_pairs(s->pg).size());
-  if (s->pr) stats[3] += prior_set_bytes(s->pr);
-  if (pairs)
-    for (size_t p = 0; p < pr.size(); p++) { pairs[2 * p] = pr[p].x; pairs[2 * p + 1] = pr[p].y; }
-  return BALM_OK;
-}
-
-extern "C" int balm_spg_evaluate(balm_spg *s, const double *poses12, double *blocks, double *g, double *cost) {
-  if (!s || !poses12) { balm_set_error("balm_spg_evaluate: bad arguments"); return BALM_ERR_INVALID; }
-  if (!s->pg) { balm_set_error("balm_spg_evaluate: no pose factors registered"); return BALM_ERR_INVALID; }
-  CUDA_TRY(cudaSetDevice(s->device));
-  CUDA_TRY(cudaMemcpyAsync(s->poses, poses12, sizeof(double) * 12 * s->N, cudaMemcpyHostToDevice, s->stream));
-  TRY(spg_eval(s, s->poses));
-  const size_t nbl = 36 * spg_pairs(s).size();
-  if (blocks && nbl) CUDA_TRY(cudaMemcpyAsync(blocks, s->blocks, sizeof(double) * nbl, cudaMemcpyDeviceToHost, s->stream));
-  if (g) CUDA_TRY(cudaMemcpyAsync(g, s->g, sizeof(double) * 6 * s->N, cudaMemcpyDeviceToHost, s->stream));
-  CUDA_TRY(cudaMemcpyAsync(s->h_scal, s->scal, sizeof(double), cudaMemcpyDeviceToHost, s->stream));
-  CUDA_TRY(cudaStreamSynchronize(s->stream));
-  if (cost) *cost = s->h_scal[0];
-  return BALM_OK;
-}
-
-extern "C" int balm_spg_iter(balm_spg *sp, double *poses12, const balm_lm_opts *o, balm_trace *trace, int *n_iters,
-                             double *poses_per_iter) {
-  if (!sp || !poses12 || !o) { balm_set_error("balm_spg_iter: bad arguments"); return BALM_ERR_INVALID; }
-  if (n_iters) *n_iters = 0;
-  if (!sp->pg) { balm_set_error("balm_spg_iter: no pose factors registered"); return BALM_ERR_INVALID; }
-  TRY(refuse_gauge_with_priors("balm_spg_iter", sp->pr, o));
-  CUDA_TRY(cudaSetDevice(sp->device));
-  const size_t pbytes = sizeof(double) * 12 * sp->N;
-  CUDA_TRY(cudaMemcpyAsync(sp->poses, poses12, pbytes, cudaMemcpyHostToDevice, sp->stream));
-  LmSteps s{sp->stream, sp->scal, sp->h_scal};
-  s.eval = [sp]() { return spg_eval(sp, sp->poses); };
-  s.solve = [sp](double u) -> int {
-    sp->h_scal[3] = u;  // pinned; the kernels read the damping factor from device memory
-    CUDA_TRY(cudaMemcpyAsync(sp->scal + 3, sp->h_scal + 3, sizeof(double), cudaMemcpyHostToDevice, sp->stream));
-    TRY(sparse_solve(sp->solver, sp->stream));
-    sp->launches += 1;
-    CUDA_TRY(cudaMemcpyAsync(sp->h_scal + 1, sp->scal + 1, sizeof(double), cudaMemcpyDeviceToHost, sp->stream));
-    CUDA_TRY(cudaMemcpyAsync(sp->h_flags, sp->flags, sizeof(int) * 8, cudaMemcpyDeviceToHost, sp->stream));
-    return BALM_OK;
-  };
-  s.trial = [sp]() {
-    sp->launches += 1;
-    return launch_pose_update(sp->stream, sp->N, sp->poses, sp->dx, sp->poses_trial);
-  };
-  s.trial_cost = [sp](double *r2) -> int {  // the factors', then the priors' cost -> scal[2]
-    TRY(pose_graph_cost(sp->pg, sp->stream, sp->poses_trial, sp->scal + 2, &sp->launches));
-    if (sp->pr) TRY(prior_add_cost(sp->pr, sp->stream, sp->poses_trial, sp->scal + 2, &sp->launches));
-    CUDA_TRY(cudaMemcpyAsync(sp->h_scal + 2, sp->scal + 2, sizeof(double), cudaMemcpyDeviceToHost, sp->stream));
-    CUDA_TRY(cudaStreamSynchronize(sp->stream));
-    *r2 = sp->h_scal[2];
-    return BALM_OK;
-  };
-  s.finish = [sp](double *q1, int *not_pd, int *refined) {
-    return solve_outcome(sp->h_scal, sp->h_flags, [sp](int *still_bad) {
-      return sparse_refine(sp->solver, sp->stream, sp->h_flags, sp->h_scal, still_bad);
-    }, q1, not_pd, refined);
-  };
-  s.step = [sp](bool accepted) {
-    if (accepted) std::swap(sp->poses, sp->poses_trial);
-    return BALM_OK;
-  };
-  s.snapshot = [&](int it) -> int {
-    if (poses_per_iter)
-      CUDA_TRY(cudaMemcpyAsync(poses_per_iter + (size_t)it * 12 * sp->N, sp->poses, pbytes, cudaMemcpyDeviceToHost,
-                               sp->stream));
-    return BALM_OK;
-  };
-  TRY(lm_run(s, o, trace, n_iters));
-  if (o->gauge_mode == 0 || o->gauge_mode == 1) {
-    sp->launches += 1;
-    TRY(launch_gauge(sp->stream, sp->N, sp->poses, sp->scal + 4, o->gauge_mode));
-  }
-  CUDA_TRY(cudaMemcpyAsync(poses12, sp->poses, pbytes, cudaMemcpyDeviceToHost, sp->stream));
-  CUDA_TRY(cudaStreamSynchronize(sp->stream));
-  return BALM_OK;
-}
-
-extern "C" int balm_spg_covariance(balm_spg *s, const double *poses12, int anchor, double *cov) {
-  if (!s || !poses12 || !cov) { balm_set_error("balm_spg_covariance: bad arguments"); return BALM_ERR_INVALID; }
-  if (!s->pg) { balm_set_error("balm_spg_covariance: no pose factors registered"); return BALM_ERR_INVALID; }
-  if (anchor < -1 || anchor >= s->N) { balm_set_error("balm_spg_covariance: anchor outside [-1, N)"); return BALM_ERR_INVALID; }
-  CUDA_TRY(cudaSetDevice(s->device));
-  return sparse_covariance(s->solver, s->stream, anchor, [&]() -> int {
-    CUDA_TRY(cudaMemcpyAsync(s->poses, poses12, sizeof(double) * 12 * s->N, cudaMemcpyHostToDevice, s->stream));
-    return spg_eval(s, s->poses);
-  }, "balm_spg_covariance", cov, &s->launches);
-}
-
-extern "C" int balm_spg_set_factor_loss(balm_spg *s, int n_factors, const int32_t *kind, const double *scale) {
-  if (!s) { balm_set_error("balm_spg_set_factor_loss: bad arguments"); return BALM_ERR_INVALID; }
-  CUDA_TRY(cudaSetDevice(s->device));
-  return set_factor_loss("balm_spg_set_factor_loss", s->pg, s->stream, n_factors, kind, scale);
-}
-
-extern "C" int balm_spg_factor_residuals(balm_spg *s, const double *poses12, double *sf, double *w) {
-  if (!s || !poses12) { balm_set_error("balm_spg_factor_residuals: bad arguments"); return BALM_ERR_INVALID; }
-  if (!s->pg) { balm_set_error("balm_spg_factor_residuals: no pose factors registered"); return BALM_ERR_INVALID; }
-  CUDA_TRY(cudaSetDevice(s->device));
-  CUDA_TRY(cudaMemcpyAsync(s->poses, poses12, sizeof(double) * 12 * s->N, cudaMemcpyHostToDevice, s->stream));
-  return pose_graph_residuals(s->pg, s->stream, s->poses, sf, w, &s->launches);
-}
-
 // ---------------- absolute pose priors (pose_graph.cu) ----------------
 // The argument checks of balm_set_pose_priors and balm_spg_set_pose_priors over P poses (n_priors >= 1)
 static int pose_priors_check(const char *who, int P, int n, const int32_t *pose, const double *hat12,
@@ -1679,11 +1426,10 @@ static int pose_priors_check(const char *who, int P, int n, const int32_t *pose,
   return BALM_OK;
 }
 
-extern "C" int balm_set_pose_priors(balm_ctx *c, int n_priors, const int32_t *pose, const double *poses_hat12,
-                                    const double *lever3, const double *H36, const int32_t *kind, const double *scale,
-                                    int32_t *status_out) {
-  const char *who = "balm_set_pose_priors";
-  if (!c) { balm_set_error(std::string(who) + ": bad arguments"); return BALM_ERR_INVALID; }
+// balm_set_pose_priors and balm_spg_set_pose_priors; `who` prefixes the messages
+static int set_pose_priors(balm_ctx *c, const char *who, int n_priors, const int32_t *pose, const double *poses_hat12,
+                           const double *lever3, const double *H36, const int32_t *kind, const double *scale,
+                           int32_t *status_out) {
   TRY(pose_priors_check(who, c->N, n_priors, pose, poses_hat12, lever3, H36, kind, scale));
   CUDA_TRY(cudaSetDevice(c->device));
   PriorSet *pr = nullptr;
@@ -1691,11 +1437,18 @@ extern "C" int balm_set_pose_priors(balm_ctx *c, int n_priors, const int32_t *po
   if (n_priors > 0)  // 0 detaches the prior set
     TRY(prior_set_build(c->stream, n_priors, pose, poses_hat12, lever3, H36, kind, scale, &status, &pr));
   std::unique_ptr<PriorSet, void (*)(PriorSet *)> pr_own(pr, prior_set_free);
-  if (pr && c->prec == BALM_PREC_BLOCKS && c->bh) TRY(prior_set_map(pr, c->stream, blocks_pairs(c->bh)));
+  if (c->prec == BALM_PREC_BLOCKS && c->bh) TRY(blocks_set_priors(c, pr, who));
   if (status_out) std::copy(status.begin(), status.end(), status_out);
   prior_set_free(c->pr);
   c->pr = pr_own.release();
   return BALM_OK;
+}
+
+extern "C" int balm_set_pose_priors(balm_ctx *c, int n_priors, const int32_t *pose, const double *poses_hat12,
+                                    const double *lever3, const double *H36, const int32_t *kind, const double *scale,
+                                    int32_t *status_out) {
+  if (!c) { balm_set_error("balm_set_pose_priors: bad arguments"); return BALM_ERR_INVALID; }
+  return set_pose_priors(c, "balm_set_pose_priors", n_priors, pose, poses_hat12, lever3, H36, kind, scale, status_out);
 }
 
 extern "C" int balm_prior_residuals(balm_ctx *c, const double *poses12, double *s, double *w) {
@@ -1704,45 +1457,6 @@ extern "C" int balm_prior_residuals(balm_ctx *c, const double *poses12, double *
   CUDA_TRY(cudaSetDevice(c->device));
   CUDA_TRY(cudaMemcpyAsync(c->poses, poses12, sizeof(double) * 12 * c->N, cudaMemcpyHostToDevice, c->stream));
   return prior_residuals(c->pr, c->stream, c->poses, s, w, &c->launches);
-}
-
-extern "C" int balm_spg_set_pose_priors(balm_spg *s, int n_priors, const int32_t *pose, const double *poses_hat12,
-                                        const double *lever3, const double *H36, const int32_t *kind,
-                                        const double *scale, int32_t *status_out) {
-  const char *who = "balm_spg_set_pose_priors";
-  if (!s) { balm_set_error(std::string(who) + ": bad arguments"); return BALM_ERR_INVALID; }
-  TRY(pose_priors_check(who, s->N, n_priors, pose, poses_hat12, lever3, H36, kind, scale));
-  CUDA_TRY(cudaSetDevice(s->device));
-  PriorSet *pr = nullptr;
-  std::vector<int> status;
-  if (n_priors > 0)  // 0 detaches the prior set
-    TRY(prior_set_build(s->stream, n_priors, pose, poses_hat12, lever3, H36, kind, scale, &status, &pr));
-  std::unique_ptr<PriorSet, void (*)(PriorSet *)> pr_own(pr, prior_set_free);
-  if (s->pg) {  // the pattern is rebuilt only when its union with the priors' diagonal pairs changes
-    std::vector<int2> up;
-    std::vector<int> fmap;
-    const bool grown = spg_union(s->pg, pr, &up, &fmap);
-    const bool same = grown ? (s->fmap && up.size() == s->upairs.size() &&
-                               std::equal(up.begin(), up.end(), s->upairs.begin(),
-                                          [](const int2 &a, const int2 &b) { return a.x == b.x && a.y == b.y; }))
-                            : !s->fmap;
-    SpgPattern pat;
-    if (!same) TRY(spg_pattern(s, s->pg, pr, who, &pat));
-    if (pr) TRY(prior_set_map(pr, s->stream, same ? spg_pairs(s) : pat.pairs(s->pg)));
-    if (!same) pat.commit(s);
-  }
-  if (status_out) std::copy(status.begin(), status.end(), status_out);
-  prior_set_free(s->pr);
-  s->pr = pr_own.release();
-  return BALM_OK;
-}
-
-extern "C" int balm_spg_prior_residuals(balm_spg *s, const double *poses12, double *sp, double *w) {
-  if (!s || !poses12) { balm_set_error("balm_spg_prior_residuals: bad arguments"); return BALM_ERR_INVALID; }
-  if (!s->pr) { balm_set_error("balm_spg_prior_residuals: no pose priors registered"); return BALM_ERR_INVALID; }
-  CUDA_TRY(cudaSetDevice(s->device));
-  CUDA_TRY(cudaMemcpyAsync(s->poses, poses12, sizeof(double) * 12 * s->N, cudaMemcpyHostToDevice, s->stream));
-  return prior_residuals(s->pr, s->stream, s->poses, sp, w, &s->launches);
 }
 
 // ---------------- sliding window on the registered voxel set (assoc.cu) ----------------
@@ -2048,6 +1762,23 @@ extern "C" int balm_download_blocks(balm_ctx *c, double *blocks) {
   return BALM_OK;
 }
 
+// balm_block_covariance and balm_spg_covariance after their argument checks; `who` prefixes the messages
+static int block_covariance(balm_ctx *c, const char *who, const double *poses12, bool include_fix, int anchor,
+                            double *cov) {
+  CUDA_TRY(cudaSetDevice(c->device));
+  // the evaluation is deferred (its events are read after sparse_covariance's waits), so the call waits twice
+  const int rc = sparse_covariance(blocks_solver(c->bh), c->stream, anchor, [&]() -> int {
+    CUDA_TRY(cudaMemcpyAsync(c->poses, poses12, sizeof(double) * 12 * c->N, cudaMemcpyHostToDevice, c->stream));
+    c->defer = true;
+    const int e = balm_cov_evaluate_hessian(c, c->poses, include_fix);
+    c->defer = false;
+    return e;
+  }, who, cov, &c->launches);
+  if (rc == BALM_OK || rc == BALM_ERR_NOT_PD) TRY(collect_eval(c));  // the stream has been synchronised
+  c->pending_eval = false;
+  return rc;
+}
+
 extern "C" int balm_block_covariance(balm_ctx *c, const double *poses12, int include_fix, int anchor, double *cov) {
   if (!c || !poses12 || !cov) { balm_set_error("balm_block_covariance: bad arguments"); return BALM_ERR_INVALID; }
   if (c->prec != BALM_PREC_BLOCKS || !c->bh || !c->registered) {
@@ -2055,16 +1786,119 @@ extern "C" int balm_block_covariance(balm_ctx *c, const double *poses12, int inc
     return BALM_ERR_INVALID;
   }
   if (anchor < -1 || anchor >= c->N) { balm_set_error("balm_block_covariance: anchor outside [-1, N)"); return BALM_ERR_INVALID; }
+  return block_covariance(c, "balm_block_covariance", poses12, include_fix != 0, anchor, cov);
+}
+
+// ---------------- sparse pose graph (pose_graph.cu, pose_graph_sparse.cu, blocks.cu) ----------------
+// A BALM_PREC_BLOCKS context without voxels whose pattern holds the factor pairs and the diagonal pair of every pose
+// with an active prior, and no other diagonal pair. Each entry point makes its own checks, then runs the context's
+// code.
+struct balm_spg {
+  balm_ctx *c = nullptr;
+  ~balm_spg() { balm_destroy(c); }
+};
+
+// `who`'s refusal before the handle's first successful balm_spg_set_factors
+static int spg_registered(const balm_spg *s, const char *who) {
+  if (s->c->registered) return BALM_OK;
+  balm_set_error(std::string(who) + ": no pose factors registered");
+  return BALM_ERR_INVALID;
+}
+
+extern "C" int balm_spg_create(balm_spg **out, int n_poses, int device) {
+  if (!out || n_poses < 1 || n_poses > (INT_MAX / 6 - 1)) { balm_set_error("balm_spg_create: bad arguments"); return BALM_ERR_INVALID; }
+  *out = nullptr;
+  std::unique_ptr<balm_spg> s(new balm_spg());
+  const int rc = balm_create(&s->c, n_poses, device, BALM_PREC_BLOCKS);
+  if (rc != BALM_OK) {
+    balm_set_error("balm_spg_create: " + g_err);
+    return rc;
+  }
+  s->c->every_diagonal = false;
+  *out = s.release();
+  return BALM_OK;
+}
+
+extern "C" void balm_spg_destroy(balm_spg *s) { delete s; }
+
+extern "C" int balm_spg_set_factors(balm_spg *s, int n_factors, const int64_t *factor_ptr, const int32_t *factor_pose,
+                                    const double *poses_hat12, const double *H, int32_t *status_out) {
+  const char *who = "balm_spg_set_factors";
+  if (!s) { balm_set_error(std::string(who) + ": bad arguments"); return BALM_ERR_INVALID; }
+  TRY(pose_factors_check(who, s->c->N, n_factors, factor_ptr, factor_pose, poses_hat12, H));
+  const bool first = !s->c->registered;  // the empty voxel set is registered after the factors: one pattern per call
+  TRY(block_set_factors(s->c, who, n_factors, factor_ptr, factor_pose, poses_hat12, H, status_out));
+  return first ? register_empty(s->c, who) : BALM_OK;
+}
+
+extern "C" int balm_spg_structure(balm_spg *s, int64_t stats[4], int32_t *pairs) {
+  if (!s || !stats) { balm_set_error("balm_spg_structure: bad arguments"); return BALM_ERR_INVALID; }
+  TRY(spg_registered(s, "balm_spg_structure"));
+  return balm_block_structure(s->c, stats, pairs);
+}
+
+extern "C" int balm_spg_evaluate(balm_spg *s, const double *poses12, double *blocks, double *g, double *cost) {
+  if (!s || !poses12) { balm_set_error("balm_spg_evaluate: bad arguments"); return BALM_ERR_INVALID; }
+  TRY(spg_registered(s, "balm_spg_evaluate"));
+  balm_ctx *c = s->c;
   CUDA_TRY(cudaSetDevice(c->device));
-  // the evaluation is deferred (its events are read after sparse_covariance's waits), so the call waits twice
-  const int rc = sparse_covariance(blocks_solver(c->bh), c->stream, anchor, [&]() -> int {
-    CUDA_TRY(cudaMemcpyAsync(c->poses, poses12, sizeof(double) * 12 * c->N, cudaMemcpyHostToDevice, c->stream));
-    c->defer = true;
-    const int e = balm_cov_evaluate_hessian(c, c->poses, include_fix != 0);
-    c->defer = false;
-    return e;
-  }, "balm_block_covariance", cov, &c->launches);
-  if (rc == BALM_OK || rc == BALM_ERR_NOT_PD) TRY(collect_eval(c));  // the stream has been synchronised
-  c->pending_eval = false;
-  return rc;
+  CUDA_TRY(cudaMemcpyAsync(c->poses, poses12, sizeof(double) * 12 * c->N, cudaMemcpyHostToDevice, c->stream));
+  c->defer = true;  // one wait: the evaluation's events are read after the copy-out's
+  const int rc = evaluate_dev(c, c->poses, 0, 0, false);
+  c->defer = false;
+  TRY(rc);
+  if (blocks) CUDA_TRY(cudaMemcpyAsync(blocks, blocks_device(c->bh), sizeof(double) * 36 * blocks_pairs(c->bh).size(),
+                                       cudaMemcpyDeviceToHost, c->stream));
+  if (g) CUDA_TRY(cudaMemcpyAsync(g, c->g, sizeof(double) * c->n, cudaMemcpyDeviceToHost, c->stream));
+  CUDA_TRY(cudaMemcpyAsync(c->h_scal, c->scal, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+  CUDA_TRY(cudaStreamSynchronize(c->stream));
+  TRY(collect_eval(c));
+  if (cost) *cost = c->h_scal[0];
+  return BALM_OK;
+}
+
+extern "C" int balm_spg_iter(balm_spg *s, double *poses12, const balm_lm_opts *o, balm_trace *trace, int *n_iters,
+                             double *poses_per_iter) {
+  if (!s || !poses12 || !o) { balm_set_error("balm_spg_iter: bad arguments"); return BALM_ERR_INVALID; }
+  if (n_iters) *n_iters = 0;
+  TRY(spg_registered(s, "balm_spg_iter"));
+  TRY(refuse_gauge_with_priors("balm_spg_iter", s->c->pr, o));
+  balm_lm_opts lo = *o;
+  lo.min_planes_per_pose = 0;  // no voxels
+  lo.hess_includes_fix = 0;
+  return balm_damping_iter(s->c, poses12, &lo, trace, n_iters, poses_per_iter);
+}
+
+extern "C" int balm_spg_covariance(balm_spg *s, const double *poses12, int anchor, double *cov) {
+  if (!s || !poses12 || !cov) { balm_set_error("balm_spg_covariance: bad arguments"); return BALM_ERR_INVALID; }
+  TRY(spg_registered(s, "balm_spg_covariance"));
+  if (anchor < -1 || anchor >= s->c->N) { balm_set_error("balm_spg_covariance: anchor outside [-1, N)"); return BALM_ERR_INVALID; }
+  return block_covariance(s->c, "balm_spg_covariance", poses12, false, anchor, cov);
+}
+
+extern "C" int balm_spg_set_factor_loss(balm_spg *s, int n_factors, const int32_t *kind, const double *scale) {
+  if (!s) { balm_set_error("balm_spg_set_factor_loss: bad arguments"); return BALM_ERR_INVALID; }
+  TRY(spg_registered(s, "balm_spg_set_factor_loss"));
+  CUDA_TRY(cudaSetDevice(s->c->device));
+  return set_factor_loss("balm_spg_set_factor_loss", s->c->pg, s->c->stream, n_factors, kind, scale);
+}
+
+extern "C" int balm_spg_factor_residuals(balm_spg *s, const double *poses12, double *sf, double *w) {
+  if (!s || !poses12) { balm_set_error("balm_spg_factor_residuals: bad arguments"); return BALM_ERR_INVALID; }
+  TRY(spg_registered(s, "balm_spg_factor_residuals"));
+  return balm_factor_residuals(s->c, poses12, sf, w);
+}
+
+extern "C" int balm_spg_set_pose_priors(balm_spg *s, int n_priors, const int32_t *pose, const double *poses_hat12,
+                                        const double *lever3, const double *H36, const int32_t *kind,
+                                        const double *scale, int32_t *status_out) {
+  const char *who = "balm_spg_set_pose_priors";
+  if (!s) { balm_set_error(std::string(who) + ": bad arguments"); return BALM_ERR_INVALID; }
+  return set_pose_priors(s->c, who, n_priors, pose, poses_hat12, lever3, H36, kind, scale, status_out);
+}
+
+extern "C" int balm_spg_prior_residuals(balm_spg *s, const double *poses12, double *sp, double *w) {
+  if (!s || !poses12) { balm_set_error("balm_spg_prior_residuals: bad arguments"); return BALM_ERR_INVALID; }
+  if (!s->c->pr) { balm_set_error("balm_spg_prior_residuals: no pose priors registered"); return BALM_ERR_INVALID; }
+  return balm_prior_residuals(s->c, poses12, sp, w);
 }

@@ -10,11 +10,13 @@
 //   lane l taking the terms l, l + 32, ... and the lanes' sums meeting in warp_sum's fixed butterfly. The block is minus
 //   that sum, plus the observation sweep's diagonal block on a diagonal pair. fp64 throughout, no floating-point atomics.
 //   Pose factors (balm_block_set_factors, DESIGN.md "Voxels and pose factors in one cost"): the pattern is the union of
-//   the voxel pairs, the active factors' pairs and the diagonal (block_pattern_build, rebuilt without re-sorting the
-//   voxel terms when only the factors change); a full-range evaluation adds the factor sums of pose_graph.cu onto the
-//   voxel blocks, g and residual, each entry once, in that order.
-//   Absolute pose priors (balm_set_pose_priors, DESIGN.md "Absolute pose priors"): they touch only diagonal blocks, which
-//   the union always holds, so they change no pattern; a full-range evaluation adds their sums after the factors'.
+//   the voxel pairs, the active factors' pairs, the diagonal pairs of the poses with an active prior and, on a context
+//   of balm_create, every diagonal pair (block_pattern_build, rebuilt without re-sorting the voxel terms when only the
+//   factors or the priors change); a full-range evaluation adds the factor sums of pose_graph.cu onto the voxel blocks,
+//   g and residual, each entry once, in that order.
+//   Absolute pose priors (balm_set_pose_priors, DESIGN.md "Absolute pose priors"): they touch only diagonal blocks; a
+//   full-range evaluation adds their sums after the factors'. The sparse pose graph (balm_spg_*) is a context of this
+//   kind without voxels whose pattern leaves out the other diagonal pairs.
 #include <cub/cub.cuh>
 #include <algorithm>
 #include <memory>
@@ -26,11 +28,14 @@
 struct BlockPattern {
   std::vector<int2> pairs;           // host: (i, j), i <= j, ascending
   long long bytes = 0;
-  int2 *pair_dev = nullptr;          // [pairs]
-  long long *tptr = nullptr;         // [pairs + 1] terms of pair p: term[tptr[p] .. tptr[p+1])
+  int2 *pair_dev = nullptr;          // [pairs] (with voxel pairs only: blocks_kernel reads them)
+  long long *tptr = nullptr;         // [pairs + 1] terms of pair p: term[tptr[p] .. tptr[p+1]) (same)
   double *blocks = nullptr;          // [pairs][36] column-major, rows of pose i
+  // No voxel pair and every pair a factor pair (the sparse pose graph's usual pattern): the factor pass stores the
+  // blocks, g and the cost, as nothing precedes it; otherwise it adds them through fmap and fgc.
+  bool factors_only = false;
   int *fmap = nullptr;               // [factor pairs] index in `pairs` of each of pose_graph_pairs (with factors only)
-  double *fgc = nullptr;             // [n + 1] the factors' g and cost before they are added (with factors only)
+  double *fgc = nullptr;             // [n + 1] the factors' g and cost before they are added (same)
   SparseSolver *solver = nullptr;
   ~BlockPattern() {
     sparse_solver_free(solver);
@@ -146,27 +151,33 @@ __global__ void add_kernel(const double *x, int n, double *y) {
 
 }  // namespace
 
-// The union of bh's voxel pairs, pg's pairs (pg may be null) and every diagonal pair, in ascending (i, j): a pair no
-// voxel gives gets an empty term range (a pose in no voxel and no factor gets a zero block, hence a zero pivot). Then
-// the blocks, the factor map and the symbolic factorisation -> *out.
-static int block_pattern_build(balm_ctx *c, const BlockHessian &bh, const PoseGraph *pg, const char *who,
-                               std::unique_ptr<BlockPattern> *out) {
+// The union of bh's voxel pairs, pg's pairs (pg may be null), the diagonal pair of every pose with an active prior of pr
+// (pr may be null) and, when c->every_diagonal, every diagonal pair, in ascending (i, j): a pair no voxel gives gets an
+// empty term range (with every diagonal pair, a pose in no voxel and no factor gets a zero block, hence a zero pivot).
+// When `same` (may be null) already has the union's pairs, *out is left empty; otherwise the blocks, the factor map and
+// the symbolic factorisation -> *out.
+static int block_pattern_build(balm_ctx *c, const BlockHessian &bh, const PoseGraph *pg, const PriorSet *pr,
+                               const BlockPattern *same, const char *who, std::unique_ptr<BlockPattern> *out) {
   const int N = c->N;
   cudaStream_t st = c->stream;
   std::unique_ptr<BlockPattern> u(new BlockPattern());
   static const std::vector<int2> none;
+  static const std::vector<int> no_pose;
   const std::vector<int2> &fp = pg ? pose_graph_pairs(pg) : none;
+  const std::vector<int> &pp = prior_set_active(pr) ? prior_set_poses(pr) : no_pose;
   std::vector<long long> tptr;
   std::vector<int> fmap;
   u->pairs.reserve(bh.vkey.size() + N);
   tptr.reserve(bh.vkey.size() + N + 1);
   fmap.reserve(fp.size());
   tptr.push_back(0);
-  size_t q = 0, r = 0;  // cursors into the voxel and the factor pairs
+  size_t q = 0, r = 0, s = 0;  // cursors into the voxel pairs, the factor pairs and the prior poses
   const unsigned long long none_left = ~0ull;
   for (int i = 0; i < N; i++) {
     const unsigned long long row_end = (unsigned long long)(i + 1) * N;
-    bool diag = true;  // the diagonal pair is the smallest key of row i
+    const bool prior = s < pp.size() && pp[s] == i;
+    s += prior;
+    bool diag = c->every_diagonal || prior;  // the diagonal pair is the smallest key of row i
     for (;;) {
       const unsigned long long kv = q < bh.vkey.size() && bh.vkey[q] < row_end ? bh.vkey[q] : none_left;
       const unsigned long long kf = r < fp.size() && fp[r].x == i ? (unsigned long long)i * N + fp[r].y : none_left;
@@ -179,18 +190,26 @@ static int block_pattern_build(balm_ctx *c, const BlockHessian &bh, const PoseGr
     }
   }
   const size_t np = u->pairs.size();
+  if (same && same->pairs.size() == np &&
+      std::equal(u->pairs.begin(), u->pairs.end(), same->pairs.begin(),
+                 [](const int2 &a, const int2 &b) { return a.x == b.x && a.y == b.y; }))
+    return BALM_OK;
   if (np >= ((size_t)1 << 30)) {
     balm_set_error(std::string(who) + ": 2^30 or more block pairs");
     return BALM_ERR_UNSUPPORTED;
   }
-  TRY(dev_alloc(&u->pair_dev, np));
-  TRY(dev_alloc(&u->tptr, np + 1));
   TRY(dev_alloc(&u->blocks, 36 * np));
-  CUDA_TRY(cudaMemcpyAsync(u->pair_dev, u->pairs.data(), sizeof(int2) * np, cudaMemcpyHostToDevice, st));
-  CUDA_TRY(cudaMemcpyAsync(u->tptr, tptr.data(), sizeof(long long) * (np + 1), cudaMemcpyHostToDevice, st));
   CUDA_TRY(cudaMemsetAsync(u->blocks, 0, sizeof(double) * 36 * np, st));
-  u->bytes = (long long)(np * (sizeof(int2) + sizeof(long long) + 36 * sizeof(double)) + sizeof(long long));
-  if (pg) {
+  u->bytes = (long long)(np * 36 * sizeof(double));
+  if (!bh.vkey.empty()) {
+    TRY(dev_alloc(&u->pair_dev, np));
+    TRY(dev_alloc(&u->tptr, np + 1));
+    CUDA_TRY(cudaMemcpyAsync(u->pair_dev, u->pairs.data(), sizeof(int2) * np, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(u->tptr, tptr.data(), sizeof(long long) * (np + 1), cudaMemcpyHostToDevice, st));
+    u->bytes += (long long)(np * (sizeof(int2) + sizeof(long long)) + sizeof(long long));
+  }
+  u->factors_only = pg && bh.vkey.empty() && fmap.size() == np;
+  if (pg && !u->factors_only) {
     TRY(dev_alloc(&u->fmap, fmap.size()));
     TRY(dev_alloc(&u->fgc, (size_t)c->n + 1));
     if (!fmap.empty())
@@ -266,7 +285,7 @@ int block_hessian_build(balm_ctx *c, const char *who) {
     bh->term = dv.Current();
     pool.release(bh->term);
   }
-  TRY(block_pattern_build(c, *bh, c->pg, who, &bh->pat));
+  TRY(block_pattern_build(c, *bh, c->pg, c->pr, nullptr, who, &bh->pat));
   if (c->pr) TRY(prior_set_map(c->pr, st, bh->pat->pairs));
   block_hessian_free(c->bh);
   c->bh = bh.release();
@@ -275,15 +294,18 @@ int block_hessian_build(balm_ctx *c, const char *who) {
 
 int blocks_repattern(balm_ctx *c, const PoseGraph *pg, const char *who) {
   std::unique_ptr<BlockPattern> pat;
-  TRY(block_pattern_build(c, *c->bh, pg, who, &pat));
+  TRY(block_pattern_build(c, *c->bh, pg, c->pr, nullptr, who, &pat));
   if (c->pr) TRY(prior_set_map(c->pr, c->stream, pat->pairs));
   c->bh->pat = std::move(pat);
   return BALM_OK;
 }
 
-int blocks_map_priors(balm_ctx *c) {
-  if (!c->pr || !c->bh) return BALM_OK;
-  return prior_set_map(c->pr, c->stream, c->bh->pat->pairs);
+int blocks_set_priors(balm_ctx *c, PriorSet *pr, const char *who) {
+  std::unique_ptr<BlockPattern> pat;  // stays empty while the union keeps its pairs
+  if (!c->every_diagonal) TRY(block_pattern_build(c, *c->bh, c->pg, pr, c->bh->pat.get(), who, &pat));
+  if (pr) TRY(prior_set_map(pr, c->stream, (pat ? pat : c->bh->pat)->pairs));
+  if (pat) c->bh->pat = std::move(pat);
+  return BALM_OK;
 }
 
 int blocks_add_priors(balm_ctx *c, const double *poses) {
@@ -305,6 +327,7 @@ int launch_blocks(balm_ctx *c, int64_t head, int64_t end) {
 
 int blocks_add_factors(balm_ctx *c, const double *poses) {
   const BlockPattern &u = *c->bh->pat;
+  if (u.factors_only) return pose_graph_eval_blocks(c->pg, c->stream, poses, u.blocks, c->g, c->g + c->n, &c->launches);
   TRY(pose_graph_add_blocks(c->pg, c->stream, poses, u.blocks, u.fmap, u.fgc, u.fgc + c->n, &c->launches));
   add_kernel<<<(unsigned)((c->n + 1 + 255) / 256), 256, 0, c->stream>>>(u.fgc, c->n + 1, c->g);  // g, then r = g[n]
   c->launches += 1;
@@ -314,6 +337,7 @@ int blocks_add_factors(balm_ctx *c, const double *poses) {
 
 int blocks_add_factor_cost(balm_ctx *c, const double *poses, double *r) {
   const BlockPattern &u = *c->bh->pat;
+  if (u.factors_only) return pose_graph_cost(c->pg, c->stream, poses, r, &c->launches);  // *r holds no voxel cost
   TRY(pose_graph_cost(c->pg, c->stream, poses, u.fgc + c->n, &c->launches));
   add_kernel<<<1, 32, 0, c->stream>>>(u.fgc + c->n, 1, r);
   c->launches += 1;
@@ -322,7 +346,10 @@ int blocks_add_factor_cost(balm_ctx *c, const double *poses, double *r) {
 }
 
 int blocks_zero(balm_ctx *c) {
-  CUDA_TRY(cudaMemsetAsync(c->bh->pat->blocks, 0, sizeof(double) * 36 * c->bh->pat->pairs.size(), c->stream));
+  const BlockPattern &u = *c->bh->pat;
+  if (u.factors_only) return BALM_OK;  // blocks_add_factors writes every block, g and r
+  CUDA_TRY(cudaMemsetAsync(u.blocks, 0, sizeof(double) * 36 * u.pairs.size(), c->stream));
+  CUDA_TRY(cudaMemsetAsync(c->g, 0, sizeof(double) * ((size_t)c->n + 1), c->stream));
   return BALM_OK;
 }
 

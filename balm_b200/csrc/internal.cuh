@@ -146,6 +146,8 @@ struct balm_ctx {
   PoseGraph *pg = nullptr;        // balm_set_pose_factors' window factors (independent of the registered voxel set);
                                   // BALM_PREC_BLOCKS: balm_block_set_factors' factors, part of the cost
   BlockHessian *bh = nullptr;     // BALM_PREC_BLOCKS: the registered set's block pattern, terms, blocks and solver
+  bool every_diagonal = true;     // BALM_PREC_BLOCKS: the pattern holds every diagonal pair; false for a balm_spg's
+                                  // context, whose pattern holds only those of its factors and priors
   PriorSet *pr = nullptr;         // balm_set_pose_priors' priors (independent of the factor and the voxel set): part of
                                   // the pose-graph cost, and on BALM_PREC_BLOCKS of every full-range evaluation
   int vloss_kind = BALM_LOSS_TRIVIAL;  // balm_set_voxel_loss: the loss of every voxel (independent of the voxel set)
@@ -839,7 +841,6 @@ int cov_sandwich(balm_ctx *c, const DenseSystem &s, double *B);
 // rows and columns [a0, a0 + 6) of the n x n matrix A set to 0, its diagonal there to diag (enqueued)
 int cov_delete_block(balm_ctx *c, double *A, int n, int a0, double diag);
 int launch_pose_update(balm_ctx *c, const double *poses_in, const double *dx, double *poses_out);
-int launch_pose_update(cudaStream_t st, int N, const double *poses_in, const double *dx, double *poses_out);
 int launch_gauge(balm_ctx *c, double *poses, int mode);
 // snap: 12 doubles of device scratch for pose 0
 int launch_gauge(cudaStream_t st, int N, double *poses, double *snap, int mode);
@@ -971,24 +972,29 @@ int sparse_covariance(SparseSolver *s, cudaStream_t st, int anchor, const std::f
                       double *cov, long long *launches);
 
 // ---------------- block-sparse Hessian of a BALM_PREC_BLOCKS context (blocks.cu) ----------------
-// The registered voxels' pair pattern and update terms, then the union pattern with c->pg's factor pairs and its
-// symbolic factorisation -> c->bh (replacing the previous one). BALM_ERR_UNSUPPORTED (message prefixed with who) when
-// the terms or pairs are too many to index; c->bh is then kept.
+// The registered voxels' pair pattern and update terms, then the union pattern with c->pg's factor pairs and c->pr's
+// diagonal pairs and its symbolic factorisation -> c->bh (replacing the previous one). BALM_ERR_UNSUPPORTED (message
+// prefixed with who) when the terms or pairs are too many to index; c->bh is then kept.
 int block_hessian_build(balm_ctx *c, const char *who);
-// The union pattern of c->bh's voxel pairs and pg's pairs (pg may be null) replaces c->bh's, the voxel terms kept; on an
-// error c->bh is unchanged.
+// The union pattern of c->bh's voxel pairs, pg's pairs (pg may be null) and c->pr's diagonal pairs replaces c->bh's, the
+// voxel terms kept; on an error c->bh is unchanged.
 int blocks_repattern(balm_ctx *c, const PoseGraph *pg, const char *who);
-// c->pg's factor blocks, g and cost at poses added onto the evaluated blocks, c->g and the residual c->g[n] (enqueued)
+// The prior set pr (may be null) in place of c->pr: c->bh's pattern is rebuilt only when its union with pr's diagonal
+// pairs differs from the current one (never when it holds every diagonal pair), and pr's diagonal table points into
+// it; on an error c->bh is unchanged.
+int blocks_set_priors(balm_ctx *c, PriorSet *pr, const char *who);
+// c->pg's factor blocks, g and cost at poses added onto the evaluated blocks, c->g and the residual c->g[n] (enqueued);
+// stored there when the pattern is the factor pairs alone and there is no voxel term
 int blocks_add_factors(balm_ctx *c, const double *poses);
-// c->pg's cost at poses added onto the device scalar *r (enqueued)
+// c->pg's cost at poses added onto the device scalar *r (enqueued; stored when there is no voxel term, as above)
 int blocks_add_factor_cost(balm_ctx *c, const double *poses, double *r);
 // c->pr's blocks, g and cost at poses added onto the evaluated blocks (after the factors'), c->g and the residual
 // c->g[n] (enqueued)
 int blocks_add_priors(balm_ctx *c, const double *poses);
-// points c->pr's diagonal table at the current pattern (no-op without priors or without a pattern)
-int blocks_map_priors(balm_ctx *c);
 // the blocks of voxels [head, end) from c->G (the per-observation store) and the accumulators, g from the accumulators
 int launch_blocks(balm_ctx *c, int64_t head, int64_t end);
+// the blocks and c->g | r zeroed before an evaluation without voxel term (nothing when the pattern is the factor pairs
+// alone: blocks_add_factors then stores every block, g and r)
 int blocks_zero(balm_ctx *c);
 // the damped solve (u into scal[3]) and its refinement: launch_ldlt_solve / refine_solution of a blocks context
 int blocks_solve(balm_ctx *c, double u);

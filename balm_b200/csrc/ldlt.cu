@@ -864,15 +864,11 @@ int launch_ldlt_solve(balm_ctx *c, const DenseSystem &s, double u) {
   return BALM_OK;
 }
 
-int launch_pose_update(cudaStream_t st, int N, const double *poses_in, const double *dx, double *poses_out) {
-  pose_update_kernel<<<(N + 127) / 128, 128, 0, st>>>(poses_in, dx, poses_out, N);
+int launch_pose_update(balm_ctx *c, const double *poses_in, const double *dx, double *poses_out) {
+  pose_update_kernel<<<(c->N + 127) / 128, 128, 0, c->stream>>>(poses_in, dx, poses_out, c->N);
+  c->launches += 1;
   CUDA_TRY(cudaGetLastError());
   return BALM_OK;
-}
-
-int launch_pose_update(balm_ctx *c, const double *poses_in, const double *dx, double *poses_out) {
-  c->launches += 1;
-  return launch_pose_update(c->stream, c->N, poses_in, dx, poses_out);
 }
 
 int launch_gauge(cudaStream_t st, int N, double *poses, double *snap, int mode) {

@@ -8,7 +8,7 @@
 //   pg_linearise_kernel  per active factor, one CTA: e_k, J_k (shared), M = E^T H~ E and b = E^T H~ e -> staging
 //   pg_assemble_kernel   per (global 6x6 block pair i <= j, entry): the pair's (factor, slot, slot) terms in factor order
 //                        -> H (i, j) and (j, i) from one sum; per gradient entry: the pose's slots in factor order -> g
-//                        (outputs: dense H, the sparse pose graph's blocks, or added onto a blocks context's blocks)
+//                        (outputs: dense H, or a blocks context's blocks: stored, or added onto its voxel blocks)
 //   pg_cost_kernel       per active factor, one CTA: cost_f
 //   pg_sum_kernel        one CTA: the factors' costs in factor order -> a device scalar
 // Robust losses (DESIGN.md "Robust pose factors"): with s_f = e~^T H~ e~ the factor's cost becomes 1/2 rho(s_f), its b
@@ -235,8 +235,9 @@ __global__ void __launch_bounds__(PG_THREADS) pg_linearise_kernel(FactorView fv,
 }
 
 // ---- H and g: one thread per (block pair, entry), then one per gradient entry. The pair sums go to `out`: dense H
-// (zeroed beforehand) for the context, one 6x6 block per pair for the sparse pose graph, or added onto the voxel blocks of
-// a BALM_PREC_BLOCKS context (DESIGN.md "Voxels and pose factors in one cost"). ----
+// (zeroed beforehand) for the context; on a BALM_PREC_BLOCKS context one 6x6 block per pair when the factor pairs are
+// its whole pattern (the sparse pose graph's usual case), else added onto its union pattern's blocks (DESIGN.md "Voxels
+// and pose factors in one cost"). ----
 struct DenseH {  // H (6P)^2 column-major: entry (a, c6) of pair (i, j) at (6i + a, 6j + c6) and its transpose
   double *H;
   __device__ __forceinline__ void operator()(size_t n, long long p, int2 ij, int a, int c6, double s) const {
@@ -456,7 +457,7 @@ __global__ void __launch_bounds__(PG_THREADS) prior_linearise_kernel(PriorView p
 }
 
 // Where a pose's prior sum goes: onto the dense H of a context's pose graph, or onto the pose's diagonal block of a
-// block pattern (the sparse pose graph's pairs or a BALM_PREC_BLOCKS context's union), diag[u] its index there.
+// BALM_PREC_BLOCKS context's pattern (the sparse pose graph's included), diag[u] its index there.
 struct DenseAdd {
   double *H;
   size_t n;

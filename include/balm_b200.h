@@ -508,8 +508,10 @@ int balm_rig_damping_iter(balm_ctx *ctx, double *base12, double *ext12, const ba
 /* Sparse pose graph (DESIGN.md "Pose graph", "Sparse solve"): the same factors, cost and LM as balm_set_pose_factors /
  * balm_pose_graph_iter, with H held as its nonzero 6x6 blocks and the damped system solved by a block LDL^T in a
  * nested-dissection order. Device memory grows with the number of blocks, not with (6P)^2, so trajectories of any
- * length fit; the context's dense pose graph is the faster choice for short ones. A balm_spg is a handle of its own:
- * it holds no voxels and takes no balm_ctx call.
+ * length fit; the context's dense pose graph is the faster choice for short ones. A balm_spg is a handle of its own
+ * (it takes no balm_ctx call) that owns a BALM_PREC_BLOCKS context without voxels, whose block pattern holds the factor
+ * pairs and the diagonal pairs of the prior poses only; each balm_spg_* call runs that context's code after its own
+ * checks (balm_block_set_factors, balm_block_structure, balm_evaluate, balm_damping_iter, balm_block_covariance, ...).
  * balm_spg_create: n_poses >= 1 poses on `device`; allocates O(n_poses) device memory only. */
 typedef struct balm_spg balm_spg;
 int balm_spg_create(balm_spg **out, int n_poses, int device);
@@ -520,7 +522,7 @@ void balm_spg_destroy(balm_spg *spg);
 int balm_spg_set_factors(balm_spg *spg, int n_factors, const int64_t *factor_ptr, const int32_t *factor_pose,
                          const double *poses_hat12, const double *H, int32_t *status_out);
 /* stats: [0] nonzero block pairs (i <= j) of H, [1] blocks of L, [2] elimination-tree levels, [3] device bytes the
- * handle holds (factors and their staging, tables, L, vectors).
+ * handle holds (factors and their staging, tables, L, vectors), as balm_block_structure counts them.
  * pairs (may be NULL, so that a first call can size it): 2 int32 (i, j) per block pair, ascending in (i, j). */
 int balm_spg_structure(balm_spg *spg, int64_t stats[4], int32_t *pairs);
 /* balm_pose_graph_evaluate with H as blocks: 36 doubles per block pair (rows of pose i, columns of pose j,
@@ -641,8 +643,8 @@ int balm_set_pose_priors(balm_ctx *ctx, int n_priors, const int32_t *pose, const
 int balm_prior_residuals(balm_ctx *ctx, const double *poses12, double *s, double *w);
 /* balm_set_pose_priors and balm_prior_residuals on a sparse pose graph: same arguments, checks, meaning (balm_spg_evaluate,
  * _iter and _covariance) and lifetime (the set survives balm_spg_set_factors). A prior on a pose that no active factor
- * covers adds that pose's diagonal pair to the pattern, which is then re-ordered and re-captured; only such a change
- * does that. */
+ * covers adds that pose's diagonal pair to the pattern, which is then re-ordered and re-captured; only a change of the
+ * pattern's pairs does that. */
 int balm_spg_set_pose_priors(balm_spg *spg, int n_priors, const int32_t *pose, const double *poses_hat12,
                              const double *lever3, const double *H36, const int32_t *kind, const double *scale,
                              int32_t *status_out);
