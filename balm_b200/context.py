@@ -331,15 +331,24 @@ class Context:
         scanned at T_{base_of[s]} E_{lidar_of[s]}. fixed_bases / fixed_lidars list the unknowns held fixed; the default
         fixes LiDAR 0 as the reference (the extrinsics' gauge). base_of=None detaches the rig. -> n_rig, 6 x the free
         unknowns."""
+        return self._set_rig(L.lib().balm_set_rig, "set_rig", base_of, lidar_of, fixed_bases, fixed_lidars)
+
+    def set_block_rig(self, base_of, lidar_of, fixed_bases=(), fixed_lidars=(0,)):
+        """set_rig on a PREC_BLOCKS context (include/balm_b200.h, balm_block_set_rig): H_rig held as 6x6 blocks and
+        solved sparse, the context's pose factors and priors part of the rig cost. rig_evaluate, rig_damping_iter,
+        rig_block_structure and rig_block_covariance then take the rig."""
+        return self._set_rig(L.lib().balm_block_set_rig, "set_block_rig", base_of, lidar_of, fixed_bases, fixed_lidars)
+
+    def _set_rig(self, fn, who, base_of, lidar_of, fixed_bases, fixed_lidars):
         n_rig = C.c_int()
         if base_of is None:
-            L.check(L.lib().balm_set_rig(self._h, 0, 0, None, None, None, None, C.byref(n_rig)))
+            L.check(fn(self._h, 0, 0, None, None, None, None, C.byref(n_rig)))
             self._rig = None
             return 0
         base_of = np.ascontiguousarray(base_of, dtype=np.int32)
         lidar_of = np.ascontiguousarray(lidar_of, dtype=np.int32)
         if base_of.shape != (self.N,) or lidar_of.shape != (self.N,):
-            raise ValueError(f"set_rig: base_of and lidar_of need one entry per slot ({self.N})")
+            raise ValueError(f"{who}: base_of and lidar_of need one entry per slot ({self.N})")
         B = int(base_of.max()) + 1 if self.N else 0
         nl = int(lidar_of.max()) + 1 if self.N else 0
         bf = np.zeros(B, dtype=np.uint8)
@@ -347,11 +356,34 @@ class Context:
         for name, idx, arr in (("fixed_bases", fixed_bases, bf), ("fixed_lidars", fixed_lidars, lf)):
             for i in idx:
                 if not 0 <= int(i) < len(arr):
-                    raise ValueError(f"set_rig: {name} entry {i} outside [0, {len(arr)})")
+                    raise ValueError(f"{who}: {name} entry {i} outside [0, {len(arr)})")
                 arr[int(i)] = 1
-        L.check(L.lib().balm_set_rig(self._h, B, nl, _p(base_of), _p(lidar_of), _p(bf), _p(lf), C.byref(n_rig)))
+        L.check(fn(self._h, B, nl, _p(base_of), _p(lidar_of), _p(bf), _p(lf), C.byref(n_rig)))
         self._rig = (B, nl, n_rig.value)
         return n_rig.value
+
+    def rig_block_structure(self, want_pairs=False):
+        """set_block_rig's rig: -> dict(pairs, l_blocks, levels, device_bytes) as block_structure, over the rig's free
+        unknowns (set_rig's order); with want_pairs also "pair_list", the (pairs, 2) int32 array of (u, v), u <= v."""
+        st = np.zeros(4, dtype=np.int64)
+        L.check(L.lib().balm_rig_block_structure(self._h, _p(st), None))
+        out = dict(pairs=int(st[0]), l_blocks=int(st[1]), levels=int(st[2]), device_bytes=int(st[3]))
+        if want_pairs:
+            pr = np.zeros((out["pairs"], 2), dtype=np.int32)
+            L.check(L.lib().balm_rig_block_structure(self._h, _p(st), _p(pr)))
+            out["pair_list"] = pr
+        return out
+
+    def rig_block_covariance(self, base12, ext12, include_fix=False, anchor=-1):
+        """set_block_rig's rig: Sigma = (H_rig without free base anchor's rows and columns)^-1 on the rig's block
+        pattern, H_rig as rig_evaluate returns it (anchor=-1: nothing deleted). -> (pairs [n_pairs, 2] (u <= v),
+        cov [n_pairs, 6, 6]) with cov[p, a, c] = Sigma[6 u + a, 6 v + c]."""
+        base12, ext12, _ = self._rig_shapes(base12, ext12)
+        pairs = self.rig_block_structure(want_pairs=True)["pair_list"]
+        cov = np.zeros((len(pairs), 36))
+        L.check(L.lib().balm_rig_block_covariance(self._h, _p(base12), _p(ext12), int(include_fix), int(anchor),
+                                                  _p(cov)))
+        return pairs, cov.reshape(-1, 6, 6).transpose(0, 2, 1)
 
     def _rig_shapes(self, base12, ext12):
         if getattr(self, "_rig", None) is None:

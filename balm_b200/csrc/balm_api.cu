@@ -786,12 +786,12 @@ extern "C" int balm_voxel_residuals(balm_ctx *c, const double *poses12, int64_t 
   return BALM_OK;
 }
 
-// The context's solve of sys once its stream has been waited for: its time, then its outcome from the pinned mirrors of
-// scal / flags: q1 = h_scal[1], not_pd on a bad pivot (h_flags[0]) or a non-finite q1. When the backward-error check
-// failed (h_flags[4]: an indefinite H + uD factored without pivoting lost digits), dx is refined in fp64 with the same
-// factors, which leaves the new q1 in h_scal[1]; if that does not bring the error down, the step counts as not_pd.
-// Returns 1 in *refined when dx changed (the caller re-applies the update).
-static int collect_solve(balm_ctx *c, const DenseSystem &sys, double *q1, int *not_pd, int *refined) {
+// The context's solve of sys (sp null) or of the sparse solver sp once its stream has been waited for: its time, then
+// its outcome from the pinned mirrors of scal / flags: q1 = h_scal[1], not_pd on a bad pivot (h_flags[0]) or a
+// non-finite q1. When the backward-error check failed (h_flags[4]: an indefinite H + uD factored without pivoting lost
+// digits), dx is refined in fp64 with the same factors, which leaves the new q1 in h_scal[1]; if that does not bring the
+// error down, the step counts as not_pd. Returns 1 in *refined when dx changed (the caller re-applies the update).
+static int collect_solve(balm_ctx *c, const DenseSystem &sys, SparseSolver *sp, double *q1, int *not_pd, int *refined) {
   float ms;
   cudaEventElapsedTime(&ms, c->ev[9], c->ev[10]);
   c->tm.ms_solve += ms;
@@ -801,22 +801,34 @@ static int collect_solve(balm_ctx *c, const DenseSystem &sys, double *q1, int *n
   *refined = 0;
   if (c->h_flags[4] == 0 || *not_pd) return BALM_OK;
   int still_bad = 0;
-  TRY(c->prec == BALM_PREC_BLOCKS ? blocks_refine(c, &still_bad) : refine_solution(c, sys, &still_bad));
+  if (sp) {
+    TRY(sparse_refine(sp, c->stream, c->h_flags, c->h_scal, &still_bad));
+    c->tm.refinements += 1;
+  } else {
+    TRY(refine_solution(c, sys, &still_bad));
+  }
   *q1 = c->h_scal[1];
   *refined = 1;
   if (still_bad || !std::isfinite(*q1)) *not_pd = 1;
   return BALM_OK;
 }
 
-// The damped solve of sys (the context's own system, or a rig's; a blocks context solves its blocks instead),
-// enqueued; collect_solve() reads it after the stream has been waited for
-static int solve_dev(balm_ctx *c, const DenseSystem &sys, double u) {
+// The damped solve of sys (the context's own system, or a rig's), or of the sparse solver sp when it is not null (a
+// blocks context's blocks, or a block-sparse rig's), enqueued; collect_solve() reads it after the stream has been waited
+// for
+static int solve_dev(balm_ctx *c, const DenseSystem &sys, SparseSolver *sp, double u) {
   CUDA_TRY(cudaEventRecord(c->ev[9], c->stream));
-  if (c->prec == BALM_PREC_BLOCKS) TRY(blocks_solve(c, u));
-  else TRY(launch_ldlt_solve(c, sys, u));
+  if (sp) {
+    c->h_scal[3] = u;  // pinned; the kernels read the damping factor from device memory
+    CUDA_TRY(cudaMemcpyAsync(c->scal + 3, c->h_scal + 3, sizeof(double), cudaMemcpyHostToDevice, c->stream));
+    TRY(sparse_solve(sp, c->stream));
+    c->launches += 1;
+  } else {
+    TRY(launch_ldlt_solve(c, sys, u));
+  }
   CUDA_TRY(cudaEventRecord(c->ev[10], c->stream));
   CUDA_TRY(cudaMemcpyAsync(c->h_scal + 1, c->scal + 1, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
-  if (c->prec == BALM_PREC_BLOCKS) {  // no tensor-path flags in 1..3 to keep: flags 0..4 in one copy
+  if (sp) {  // no tensor-path flags in 1..3 to keep: flags 0..4 in one copy
     CUDA_TRY(cudaMemcpyAsync(c->h_flags, c->flags, sizeof(int) * 5, cudaMemcpyDeviceToHost, c->stream));
   } else {
     CUDA_TRY(cudaMemcpyAsync(c->h_flags, c->flags, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
@@ -825,15 +837,19 @@ static int solve_dev(balm_ctx *c, const DenseSystem &sys, double u) {
   return BALM_OK;
 }
 
+// the context's own sparse solver: a blocks context's, else null (the dense solve of ctx_system)
+static SparseSolver *ctx_solver(balm_ctx *c) { return c->prec == BALM_PREC_BLOCKS ? blocks_solver(c->bh) : nullptr; }
+
 extern "C" int balm_solve(balm_ctx *c, double u, double *dx, double *q1, int *not_pd) {
   if (!c) { balm_set_error("balm_solve: bad arguments"); return BALM_ERR_INVALID; }
   CUDA_TRY(cudaSetDevice(c->device));
   const DenseSystem sys = ctx_system(c);
+  SparseSolver *sp = ctx_solver(c);
   double q = 0;
   int bad = 0, refined = 0;
-  TRY(solve_dev(c, sys, u));
+  TRY(solve_dev(c, sys, sp, u));
   CUDA_TRY(cudaStreamSynchronize(c->stream));
-  TRY(collect_solve(c, sys, &q, &bad, &refined));
+  TRY(collect_solve(c, sys, sp, &q, &bad, &refined));
   if (dx) CUDA_TRY(cudaMemcpy(dx, c->dx, sizeof(double) * c->n, cudaMemcpyDeviceToHost));
   if (q1) *q1 = q;
   if (not_pd) *not_pd = bad;
@@ -951,6 +967,7 @@ extern "C" int balm_damping_iter(balm_ctx *c, double *poses12, const balm_lm_opt
   // the evaluation's events and flags are read after the iteration's wait; BALM_SYNC_PHASES waits after every phase
   c->defer = !getenv("BALM_SYNC_PHASES");
   const DenseSystem sys = ctx_system(c);
+  SparseSolver *sp = ctx_solver(c);
   LmSteps s{c->stream, c->scal, c->h_scal};
   s.eval = [&]() -> int {
     c->eval_same_poses = same_poses;
@@ -959,7 +976,7 @@ extern "C" int balm_damping_iter(balm_ctx *c, double *poses12, const balm_lm_opt
     return rc;
   };
   s.solve = [&](double u) -> int {
-    TRY(solve_dev(c, sys, u));
+    TRY(solve_dev(c, sys, sp, u));
     if (!c->defer) CUDA_TRY(cudaStreamSynchronize(c->stream));
     return BALM_OK;
   };
@@ -967,7 +984,7 @@ extern "C" int balm_damping_iter(balm_ctx *c, double *poses12, const balm_lm_opt
   s.trial_cost = [&](double *r2) { return residual_dev(c, c->poses_trial, r2, hand_over); };
   s.finish = [&](double *q1, int *not_pd, int *refined) -> int {
     TRY(collect_eval(c));
-    return collect_solve(c, sys, q1, not_pd, refined);
+    return collect_solve(c, sys, sp, q1, not_pd, refined);
   };
   s.step = [&](bool accepted) -> int {
     if (accepted) {
@@ -1139,7 +1156,7 @@ extern "C" int balm_pose_graph_iter(balm_ctx *c, double *poses12, const balm_lm_
   const DenseSystem sys = ctx_system(c);
   LmSteps s{c->stream, c->scal, c->h_scal};
   s.eval = [c]() { return pose_graph_eval(c, c->poses); };
-  s.solve = [c, &sys](double u) { return solve_dev(c, sys, u); };
+  s.solve = [c, &sys](double u) { return solve_dev(c, sys, nullptr, u); };
   s.trial = [c]() { return launch_pose_update(c, c->poses, c->dx, c->poses_trial); };
   s.trial_cost = [c](double *r2) -> int {  // the factors', then the priors' cost -> scal[2]
     TRY(pose_graph_cost(c->pg, c->stream, c->poses_trial, c->scal + 2, &c->launches));
@@ -1149,7 +1166,9 @@ extern "C" int balm_pose_graph_iter(balm_ctx *c, double *poses12, const balm_lm_
     *r2 = c->h_scal[2];
     return BALM_OK;
   };
-  s.finish = [c, &sys](double *q1, int *not_pd, int *refined) { return collect_solve(c, sys, q1, not_pd, refined); };
+  s.finish = [c, &sys](double *q1, int *not_pd, int *refined) {
+    return collect_solve(c, sys, nullptr, q1, not_pd, refined);
+  };
   s.step = [c](bool accepted) {
     if (accepted) std::swap(c->poses, c->poses_trial);
     return BALM_OK;
@@ -1167,14 +1186,11 @@ extern "C" int balm_pose_graph_iter(balm_ctx *c, double *poses12, const balm_lm_
 }
 
 // ---------------- rig calibration (rig.cu) ----------------
-extern "C" int balm_set_rig(balm_ctx *c, int n_base, int n_lidar, const int32_t *base_of, const int32_t *lidar_of,
-                            const uint8_t *base_fixed, const uint8_t *lidar_fixed, int *n_rig_out) {
-  const std::string w = "balm_set_rig: ";
-  if (!c) { balm_set_error(w + "bad arguments"); return BALM_ERR_INVALID; }
-  if (c->prec == BALM_PREC_BLOCKS) {
-    balm_set_error(w + "not available on a BALM_PREC_BLOCKS context (it holds no dense H)");
-    return BALM_ERR_UNSUPPORTED;
-  }
+// balm_set_rig's and balm_block_set_rig's checks and attach (`who` prefixes the messages): detach on n_base 0, else the
+// arguments checked and a new rig built; on a refusal the previous rig stays
+static int set_rig(balm_ctx *c, const char *who, bool sparse, int n_base, int n_lidar, const int32_t *base_of,
+                   const int32_t *lidar_of, const uint8_t *base_fixed, const uint8_t *lidar_fixed, int *n_rig_out) {
+  const std::string w = std::string(who) + ": ";
   if (c->world > 1 || c->comm) { balm_set_error(w + "single-GPU contexts only"); return BALM_ERR_INVALID; }
   CUDA_TRY(cudaSetDevice(c->device));
   if (n_base == 0) {  // detach
@@ -1203,7 +1219,7 @@ extern "C" int balm_set_rig(balm_ctx *c, int n_base, int n_lidar, const int32_t 
   for (int l = 0; l < n_lidar; l++) n_free += !(lidar_fixed && lidar_fixed[l]);
   if (n_free == 0) { balm_set_error(w + "every base pose and extrinsic is fixed"); return BALM_ERR_INVALID; }
   Rig *r = nullptr;
-  const int rc = rig_build(c->stream, c->N, n_base, n_lidar, base_of, lidar_of, base_fixed, lidar_fixed, &r);
+  const int rc = rig_build(c->stream, c->N, n_base, n_lidar, base_of, lidar_of, base_fixed, lidar_fixed, sparse, &r);
   if (rc != BALM_OK) {
     cudaGetLastError();  // an out-of-memory allocation must not fail the next launch check; the previous rig stays
     return rc;
@@ -1212,6 +1228,29 @@ extern "C" int balm_set_rig(balm_ctx *c, int n_base, int n_lidar, const int32_t 
   c->rig = r;
   if (n_rig_out) *n_rig_out = rig_n(r);
   return BALM_OK;
+}
+
+extern "C" int balm_set_rig(balm_ctx *c, int n_base, int n_lidar, const int32_t *base_of, const int32_t *lidar_of,
+                            const uint8_t *base_fixed, const uint8_t *lidar_fixed, int *n_rig_out) {
+  if (!c) { balm_set_error("balm_set_rig: bad arguments"); return BALM_ERR_INVALID; }
+  if (c->prec == BALM_PREC_BLOCKS) {
+    balm_set_error("balm_set_rig: not available on a BALM_PREC_BLOCKS context (it holds no dense H); use "
+                   "balm_block_set_rig");
+    return BALM_ERR_UNSUPPORTED;
+  }
+  return set_rig(c, "balm_set_rig", false, n_base, n_lidar, base_of, lidar_of, base_fixed, lidar_fixed, n_rig_out);
+}
+
+extern "C" int balm_block_set_rig(balm_ctx *c, int n_base, int n_lidar, const int32_t *base_of,
+                                  const int32_t *lidar_of, const uint8_t *base_fixed, const uint8_t *lidar_fixed,
+                                  int *n_rig_out) {
+  if (!c) { balm_set_error("balm_block_set_rig: bad arguments"); return BALM_ERR_INVALID; }
+  if (c->prec != BALM_PREC_BLOCKS) {
+    balm_set_error("balm_block_set_rig: BALM_PREC_BLOCKS contexts only (the dense ones take balm_set_rig)");
+    return BALM_ERR_INVALID;
+  }
+  return set_rig(c, "balm_block_set_rig", true, n_base, n_lidar, base_of, lidar_of, base_fixed, lidar_fixed,
+                 n_rig_out);
 }
 
 // uploads base12 / ext12 into the rig's current state
@@ -1230,9 +1269,10 @@ static int rig_evaluate_dev(balm_ctx *c, bool include_fix) {
   Rig *r = c->rig;
   const double *st = rig_state(r, false);
   TRY(rig_compose(r, c->stream, st, c->poses, &c->launches));
-  TRY(evaluate_dev(c, c->poses, 0, c->M, include_fix));
+  TRY(evaluate_dev(c, c->poses, 0, c->M, include_fix));  // a blocks context: the slot blocks, factors, then priors
   CUDA_TRY(cudaEventRecord(c->ev[13], c->stream));
-  TRY(rig_reduce(r, c->stream, st, c->H, c->g, &c->launches));
+  if (rig_sparse(r)) TRY(rig_reduce_blocks(r, c->stream, st, blocks_device(c->bh), c->g, &c->launches));
+  else TRY(rig_reduce(r, c->stream, st, c->H, c->g, &c->launches));
   CUDA_TRY(cudaEventRecord(c->ev[14], c->stream));
   return BALM_OK;
 }
@@ -1244,11 +1284,40 @@ static int rig_collect_reduce(balm_ctx *c) {
   return BALM_OK;
 }
 
+// A block-sparse rig's pattern follows the slot pattern: rebuilt here when that has changed (BALM_ERR_UNSUPPORTED when
+// too large to index)
 static int rig_check(balm_ctx *c, const char *who) {
   if (!c->rig) { balm_set_error(std::string(who) + ": no rig set (balm_set_rig)"); return BALM_ERR_INVALID; }
   // balm_comm_init may attach a communicator after balm_set_rig: the rig calls stay single-GPU
   if (c->world > 1 || c->comm) { balm_set_error(std::string(who) + ": single-GPU contexts only"); return BALM_ERR_INVALID; }
   if (!c->registered) { balm_set_error("no voxels registered"); return BALM_ERR_INVALID; }
+  if (rig_sparse(c->rig)) {
+    CUDA_TRY(cudaSetDevice(c->device));
+    const int rc = rig_blocks_sync(c->rig, c->stream, blocks_pairs(c->bh), blocks_generation(c->bh), c->scal, c->flags,
+                                   who);
+    if (rc != BALM_OK) cudaGetLastError();  // as balm_set_rig: an out-of-memory build leaves no launch error behind
+    TRY(rc);
+  }
+  return BALM_OK;
+}
+
+// A block-sparse rig's H_rig as the dense column-major n_rig x n_rig matrix of its blocks (zeros elsewhere), on the
+// host (waits), as blocks_to_dense
+static int rig_blocks_to_dense(balm_ctx *c, double *H) {
+  const std::vector<int2> &pr = rig_pairs(c->rig);
+  std::vector<double> b(36 * pr.size());
+  CUDA_TRY(cudaMemcpyAsync(b.data(), rig_blocks(c->rig), sizeof(double) * b.size(), cudaMemcpyDeviceToHost, c->stream));
+  CUDA_TRY(cudaStreamSynchronize(c->stream));
+  const size_t n = rig_n(c->rig);
+  std::fill(H, H + n * n, 0.0);
+  for (size_t p = 0; p < pr.size(); p++)
+    for (int col = 0; col < 6; col++)
+      for (int row = 0; row < 6; row++) {
+        const double h = b[36 * p + 6 * col + row];
+        const size_t r = 6 * (size_t)pr[p].x + row, cc = 6 * (size_t)pr[p].y + col;
+        H[cc * n + r] = h;
+        H[r * n + cc] = h;
+      }
   return BALM_OK;
 }
 
@@ -1261,7 +1330,8 @@ extern "C" int balm_rig_evaluate(balm_ctx *c, const double *base12, const double
   TRY(rig_evaluate_dev(c, include_fix != 0));
   const DenseSystem sys = rig_system(c->rig);
   const size_t nr = sys.n;
-  if (H) CUDA_TRY(cudaMemcpyAsync(H, sys.H, sizeof(double) * nr * nr, cudaMemcpyDeviceToHost, c->stream));
+  if (H && rig_sparse(c->rig)) TRY(rig_blocks_to_dense(c, H));
+  else if (H) CUDA_TRY(cudaMemcpyAsync(H, sys.H, sizeof(double) * nr * nr, cudaMemcpyDeviceToHost, c->stream));
   if (g) CUDA_TRY(cudaMemcpyAsync(g, sys.g, sizeof(double) * nr, cudaMemcpyDeviceToHost, c->stream));
   CUDA_TRY(cudaMemcpyAsync(c->h_scal, c->scal, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
   CUDA_TRY(cudaStreamSynchronize(c->stream));
@@ -1276,6 +1346,11 @@ extern "C" int balm_rig_covariance(balm_ctx *c, const double *base12, const doub
                                    double point_noise, int include_fix, int anchor, double *raw, double *cov) {
   const char *who = "balm_rig_covariance";
   if (!c || !base12 || !ext12 || (!raw && !cov)) { balm_set_error(std::string(who) + ": bad arguments"); return BALM_ERR_INVALID; }
+  if (c->rig && rig_sparse(c->rig)) {
+    balm_set_error(std::string(who) + ": not available for a BALM_PREC_BLOCKS context's rig (it needs the dense 6N x 6N "
+                   "raw term); balm_rig_block_covariance gives H_rig^-1");
+    return BALM_ERR_UNSUPPORTED;
+  }
   TRY(rig_check(c, who));
   if (c->M < 1) { balm_set_error(std::string(who) + ": no voxels registered"); return BALM_ERR_INVALID; }
   Rig *rg = c->rig;
@@ -1341,6 +1416,7 @@ extern "C" int balm_rig_damping_iter(balm_ctx *c, double *base12, double *ext12,
                    " re-anchors to base pose 0, which moves the result off the fixed base poses; pass gauge_mode 2");
     return BALM_ERR_INVALID;
   }
+  if (c->prec == BALM_PREC_BLOCKS) TRY(refuse_gauge_with_priors(who, c->pr, o));
   if (o->min_planes_per_pose > 0 && c->min_planes < o->min_planes_per_pose) {  // per scan slot, as balm_damping_iter
     balm_set_error("Initial error too large. Please loose plane determination criteria for more planes.");
     return BALM_ERR_TOO_FEW_PLANES;
@@ -1350,6 +1426,7 @@ extern "C" int balm_rig_damping_iter(balm_ctx *c, double *base12, double *ext12,
   const int B = rig_bases(rg), U = B + rig_lidars(rg);
   const size_t sbytes = sizeof(double) * 12 * U;
   const DenseSystem sys = rig_system(rg);
+  SparseSolver *sp = rig_sparse(rg) ? rig_solver(rg) : nullptr;
   LmScope lm_scope{c};
   c->defer = true;  // the evaluation's events and flags are read after the iteration's wait
   bool reduced = false;  // this iteration evaluated: the reduction's events are to be read
@@ -1358,7 +1435,7 @@ extern "C" int balm_rig_damping_iter(balm_ctx *c, double *base12, double *ext12,
     reduced = true;
     return rig_evaluate_dev(c, o->hess_includes_fix != 0);
   };
-  s.solve = [c, &sys](double u) { return solve_dev(c, sys, u); };
+  s.solve = [c, &sys, sp](double u) { return solve_dev(c, sys, sp, u); };
   s.trial = [c, rg]() -> int {
     TRY(rig_update(rg, c->stream, rig_state(rg, false), rig_state(rg, true), &c->launches));
     return rig_compose(rg, c->stream, rig_state(rg, true), c->poses_trial, &c->launches);
@@ -1368,7 +1445,7 @@ extern "C" int balm_rig_damping_iter(balm_ctx *c, double *base12, double *ext12,
     TRY(collect_eval(c));
     if (reduced) TRY(rig_collect_reduce(c));
     reduced = false;
-    return collect_solve(c, sys, q1, not_pd, refined);
+    return collect_solve(c, sys, sp, q1, not_pd, refined);
   };
   s.step = [rg](bool accepted) {
     if (accepted) rig_swap_states(rg);
@@ -1390,6 +1467,59 @@ extern "C" int balm_rig_damping_iter(balm_ctx *c, double *base12, double *ext12,
   CUDA_TRY(cudaMemcpyAsync(ext12, st + 12 * (size_t)B, sizeof(double) * 12 * (U - B), cudaMemcpyDeviceToHost, c->stream));
   CUDA_TRY(cudaStreamSynchronize(c->stream));
   return BALM_OK;
+}
+
+// the block-sparse rig's calls: a rig set by balm_block_set_rig, its pattern in step with the slot pattern
+static int block_rig_check(balm_ctx *c, const char *who) {
+  if (c->rig && !rig_sparse(c->rig)) {
+    balm_set_error(std::string(who) + ": the rig was set by balm_set_rig (a dense context's)");
+    return BALM_ERR_INVALID;
+  }
+  if (!c->rig) { balm_set_error(std::string(who) + ": no rig set (balm_block_set_rig)"); return BALM_ERR_INVALID; }
+  return rig_check(c, who);
+}
+
+extern "C" int balm_rig_block_structure(balm_ctx *c, int64_t stats[4], int32_t *pairs) {
+  const char *who = "balm_rig_block_structure";
+  if (!c || !stats) { balm_set_error(std::string(who) + ": bad arguments"); return BALM_ERR_INVALID; }
+  TRY(block_rig_check(c, who));
+  const std::vector<int2> &pr = rig_pairs(c->rig);
+  stats[0] = (int64_t)pr.size();
+  stats[3] = rig_blocks_bytes(c->rig, &stats[1], &stats[2]);
+  if (pairs)
+    for (size_t p = 0; p < pr.size(); p++) { pairs[2 * p] = pr[p].x; pairs[2 * p + 1] = pr[p].y; }
+  return BALM_OK;
+}
+
+extern "C" int balm_rig_block_covariance(balm_ctx *c, const double *base12, const double *ext12, int include_fix,
+                                         int anchor, double *cov) {
+  const char *who = "balm_rig_block_covariance";
+  if (!c || !base12 || !ext12 || !cov) { balm_set_error(std::string(who) + ": bad arguments"); return BALM_ERR_INVALID; }
+  TRY(block_rig_check(c, who));
+  Rig *rg = c->rig;
+  if (anchor < -1 || anchor >= rig_free_bases(rg)) {
+    balm_set_error(std::string(who) + ": anchor " + std::to_string(anchor) + " is neither -1 nor a free base index in [0, " +
+                   std::to_string(rig_free_bases(rg)) + ")");
+    return BALM_ERR_INVALID;
+  }
+  CUDA_TRY(cudaSetDevice(c->device));
+  // H_rig at base12 / ext12 left in the rig's blocks, the evaluation deferred (its events are read after
+  // sparse_covariance's waits)
+  bool evaluated = false;
+  const int rc = sparse_covariance(rig_solver(rg), c->stream, anchor, [&]() -> int {
+    TRY(rig_upload(c, base12, ext12));
+    evaluated = true;
+    c->defer = true;
+    const int e = rig_evaluate_dev(c, include_fix != 0);
+    c->defer = false;
+    return e;
+  }, who, cov, &c->launches);
+  if (evaluated && (rc == BALM_OK || rc == BALM_ERR_NOT_PD)) {  // the stream has been synchronised
+    TRY(collect_eval(c));
+    TRY(rig_collect_reduce(c));
+  }
+  c->pending_eval = false;
+  return rc;
 }
 
 // ---------------- absolute pose priors (pose_graph.cu) ----------------

@@ -37,6 +37,7 @@ struct BlockPattern {
   int *fmap = nullptr;               // [factor pairs] index in `pairs` of each of pose_graph_pairs (with factors only)
   double *fgc = nullptr;             // [n + 1] the factors' g and cost before they are added (same)
   SparseSolver *solver = nullptr;
+  long long gen = 0;                 // blocks_generation: unique to this pattern
   ~BlockPattern() {
     sparse_solver_free(solver);
     cudaFree(pair_dev); cudaFree(tptr); cudaFree(blocks); cudaFree(fmap); cudaFree(fgc);
@@ -218,6 +219,8 @@ static int block_pattern_build(balm_ctx *c, const BlockHessian &bh, const PoseGr
   }
   TRY(sparse_solver_build(st, N, u->pairs, u->blocks, c->g, c->dvec, c->dx, c->scal, c->flags, who, &u->solver));
   CUDA_TRY(cudaStreamSynchronize(st));  // the host tables above are freed on return
+  static long long generations = 0;
+  u->gen = ++generations;
   *out = std::move(u);
   return BALM_OK;
 }
@@ -353,23 +356,10 @@ int blocks_zero(balm_ctx *c) {
   return BALM_OK;
 }
 
-int blocks_solve(balm_ctx *c, double u) {
-  c->h_scal[3] = u;  // pinned; the kernels read the damping factor from device memory
-  CUDA_TRY(cudaMemcpyAsync(c->scal + 3, c->h_scal + 3, sizeof(double), cudaMemcpyHostToDevice, c->stream));
-  TRY(sparse_solve(c->bh->pat->solver, c->stream));
-  c->launches += 1;
-  return BALM_OK;
-}
-
-int blocks_refine(balm_ctx *c, int *still_bad) {
-  TRY(sparse_refine(c->bh->pat->solver, c->stream, c->h_flags, c->h_scal, still_bad));
-  c->tm.refinements += 1;
-  return BALM_OK;
-}
-
 const std::vector<int2> &blocks_pairs(const BlockHessian *b) { return b->pat->pairs; }
 const double *blocks_device(const BlockHessian *b) { return b->pat->blocks; }
 SparseSolver *blocks_solver(const BlockHessian *b) { return b->pat->solver; }
+long long blocks_generation(const BlockHessian *b) { return b->pat->gen; }
 
 long long blocks_bytes(const BlockHessian *b, int64_t *l_blocks, int64_t *levels) {
   int64_t sb = 0;

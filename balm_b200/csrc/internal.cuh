@@ -39,6 +39,7 @@ struct PriorSet;      // the registered absolute pose priors (pose_graph.cu)
 void prior_set_free(PriorSet *p);
 struct Rig;           // balm_set_rig's slot assignment, unknowns and reduced system (rig.cu)
 void rig_free(Rig *r);
+struct SparseSolver;  // nested-dissection ordering, symbolic factorisation and the per-solve CUDA graph
 
 #define CUDA_TRY(expr)                                                                        \
   do {                                                                                        \
@@ -921,9 +922,10 @@ int prior_residuals(const PriorSet *p, cudaStream_t st, const double *poses, dou
 
 // ---------------- rig (rig.cu) ----------------
 // After the argument checks: the rig of N slots (base_of / lidar_of [N] host, base_fixed [B] / lidar_fixed [L] host or
-// null: none fixed), its slot tables and the buffers of its reduced system -> a new rig in *out (waits)
+// null: none fixed), its slot tables and the buffers of its reduced system -> a new rig in *out (waits). sparse: the
+// block-sparse rig of a BALM_PREC_BLOCKS context (no dense H_rig, K or factor; its pattern comes with rig_blocks_sync)
 int rig_build(cudaStream_t st, int N, int B, int L, const int32_t *base_of, const int32_t *lidar_of,
-              const uint8_t *base_fixed, const uint8_t *lidar_fixed, Rig **out);
+              const uint8_t *base_fixed, const uint8_t *lidar_fixed, bool sparse, Rig **out);
 int rig_n(const Rig *r);  // n_rig = 6 x free unknowns
 int rig_bases(const Rig *r);
 int rig_lidars(const Rig *r);
@@ -944,11 +946,26 @@ int rig_reduce(const Rig *r, cudaStream_t st, const double *state, const double 
 // without g, through the rig's K, into out [n_rig x n_rig] (column-major, mirrored)
 int rig_reduce_raw(const Rig *r, cudaStream_t st, const double *state, const double *R, double *out,
                    long long *launches);
+// ---- block-sparse rig (rig_sparse) ----
+bool rig_sparse(const Rig *r);
+// The rig's block pattern, K tables, blocks and SparseSolver (on scal / flags) from the slot pattern slot_pairs of
+// generation gen, unless it was derived from that generation already (waits when it builds). BALM_ERR_UNSUPPORTED
+// (message prefixed with who) when too large to index; the rig then keeps its previous pattern.
+int rig_blocks_sync(Rig *r, cudaStream_t st, const std::vector<int2> &slot_pairs, long long gen, double *scal,
+                    int *flags, const char *who);
+// H_rig's blocks and g_rig at state from the slot blocks Hb and g [6N] (enqueued): K_sv = sum_t H_st J_t, then
+// J^T K plus the correction per rig pair, every sum in ascending slot order; no atomics
+int rig_reduce_blocks(const Rig *r, cudaStream_t st, const double *state, const double *Hb, const double *g,
+                      long long *launches);
+const std::vector<int2> &rig_pairs(const Rig *r);  // (u, v), u <= v, ascending over the free unknowns
+const double *rig_blocks(const Rig *r);            // device [pairs][36], column-major, rows of u
+SparseSolver *rig_solver(const Rig *r);
+// device bytes the rig holds (tables, states, vectors, pattern, blocks and solver); l_blocks / levels of its L
+long long rig_blocks_bytes(const Rig *r, int64_t *l_blocks, int64_t *levels);
 // state_out = the left step of the rig's dx on every free unknown of state, fixed ones copied (enqueued)
 int rig_update(const Rig *r, cudaStream_t st, const double *state, double *state_out, long long *launches);
 
 // ---------------- sparse pose graph (pose_graph_sparse.cu) ----------------
-struct SparseSolver;  // nested-dissection ordering, symbolic factorisation and the per-solve CUDA graph
 void sparse_solver_free(SparseSolver *s);
 // Symbolic factorisation of the pairs' block pattern over P poses (host), device tables and the captured solve on st.
 // dvec, dx, scal and flags are the handle's buffers the solve reads and writes (as the context's launch_ldlt_solve).
@@ -996,12 +1013,11 @@ int launch_blocks(balm_ctx *c, int64_t head, int64_t end);
 // the blocks and c->g | r zeroed before an evaluation without voxel term (nothing when the pattern is the factor pairs
 // alone: blocks_add_factors then stores every block, g and r)
 int blocks_zero(balm_ctx *c);
-// the damped solve (u into scal[3]) and its refinement: launch_ldlt_solve / refine_solution of a blocks context
-int blocks_solve(balm_ctx *c, double u);
-int blocks_refine(balm_ctx *c, int *still_bad);
 const std::vector<int2> &blocks_pairs(const BlockHessian *b);
 const double *blocks_device(const BlockHessian *b);
 SparseSolver *blocks_solver(const BlockHessian *b);
+// the slot pattern's generation: it changes whenever blocks.cu builds a new pattern
+long long blocks_generation(const BlockHessian *b);
 // device bytes of the pattern, terms, blocks and solver; l_blocks / levels of the factorisation
 long long blocks_bytes(const BlockHessian *b, int64_t *l_blocks, int64_t *levels);
 

@@ -9,6 +9,16 @@
 //   delta_s^(2) = ( 1/2 a_phi x c ;  a_phi x (R e_t + p x c) - 1/2 c x (c x p) ),  c = R e_phi.
 // So g_rig = sum_s J_s^T g_s and H_rig = sum_{s,t} J_s^T H_st J_t + sum_s d2(g_s . delta_s^(2)): the exact Hessian of
 // the rig cost in these coordinates. The correction touches only the (lidar, base) and (lidar, lidar) blocks.
+//
+// On a BALM_PREC_BLOCKS context (balm_block_set_rig, DESIGN.md "Rig calibration on block-sparse voxel BA") nothing of
+// size n_rig x 6N or n_rig^2 exists: H_rig is held as the 6x6 blocks of the rig pairs (u, v), u <= v, for which a slot
+// of u and a slot of v form a pair of the context's slot pattern (plus every diagonal pair), derived from that pattern
+// whenever its generation moves, and solved with the nested-dissection block LDL^T of pose_graph_sparse.cu. The
+// reduction runs in two passes, the sparse form of rig_k_kernel / rig_jtk_kernel<true>:
+//   rig_k_blocks_kernel    per (K block (s, v), row): K_sv = sum_{t in v, ascending} H_st J_t from the slot blocks
+//   rig_jtk_blocks_kernel  per rig pair, one warp: sum_{s in u, ascending} J_s^T K_sv plus the correction of s, lane l
+//                          taking the slots l, l + 32, ..., the lanes' sums meeting in warp_sum's fixed butterfly;
+//                          a diagonal pair also sums g_rig(u) = sum_{s in u} J_s^T g_s the same way
 #include <algorithm>
 #include <memory>
 #include <vector>
@@ -29,16 +39,44 @@ struct Rig {
   double *K = nullptr;             // [n_rig][6N] K = H J, column-major
   LdltWork lw;
   bool any_base_fixed = false;
+  // block-sparse rig (balm_block_set_rig): no H, A, K or lw; g_rig in gb and the pattern derived from the slot pattern
+  bool sparse = false;
+  double *gb = nullptr;            // [n_rig] g_rig
+  long long bytes = 0;             // device bytes of the tables, states and vectors above
+  std::vector<int> h_base_of, h_lidar_of, h_var_of;  // host copies for the pattern
+  std::unique_ptr<struct RigPattern> pat;
+  ~Rig();
 };
 
-void rig_free(Rig *r) {
-  if (!r) return;
-  cudaFree(r->base_of); cudaFree(r->lidar_of); cudaFree(r->var_of); cudaFree(r->var_unknown); cudaFree(r->var_ptr);
-  cudaFree(r->var_slot); cudaFree(r->state); cudaFree(r->state_trial); cudaFree(r->H); cudaFree(r->dx);
-  cudaFree(r->dvec); cudaFree(r->A); cudaFree(r->K);
-  ldlt_work_free(&r->lw);
-  delete r;
+// The rig's block pattern (host-derived from one generation of the slot pattern) and its device tables.
+struct RigPattern {
+  long long gen = -1;        // the slot pattern's generation it was derived from
+  std::vector<int2> pairs;   // host: rig pairs (u, v), u <= v, ascending
+  long long nk = 0, bytes = 0;
+  int2 *kkey = nullptr;      // [nk] (slot s, free unknown v) of every K block, s-major, v ascending
+  long long *kptr = nullptr; // [nk + 1] K block k's terms kterm[kptr[k] .. kptr[k+1])
+  int2 *kterm = nullptr;     // (2 x slot pair + (s > t: H_st read transposed), slot t), t ascending
+  int2 *pair_dev = nullptr;  // [pairs]
+  long long *jptr = nullptr; // [pairs + 1] rig pair p's terms jterm[jptr[p] .. jptr[p+1])
+  int2 *jterm = nullptr;     // (slot s of u, its K block (s, v)), s ascending
+  double *K = nullptr;       // [nk][36] column-major, rows of slot s
+  double *blocks = nullptr;  // [pairs][36] column-major, rows of unknown u
+  SparseSolver *solver = nullptr;
+  ~RigPattern() {
+    sparse_solver_free(solver);
+    cudaFree(kkey); cudaFree(kptr); cudaFree(kterm); cudaFree(pair_dev); cudaFree(jptr); cudaFree(jterm); cudaFree(K);
+    cudaFree(blocks);
+  }
+};
+
+Rig::~Rig() {
+  cudaFree(base_of); cudaFree(lidar_of); cudaFree(var_of); cudaFree(var_unknown); cudaFree(var_ptr);
+  cudaFree(var_slot); cudaFree(state); cudaFree(state_trial); cudaFree(H); cudaFree(dx);
+  cudaFree(dvec); cudaFree(A); cudaFree(K); cudaFree(gb);
+  ldlt_work_free(&lw);
 }
+
+void rig_free(Rig *r) { delete r; }
 
 namespace {
 
@@ -182,6 +220,110 @@ __global__ void __launch_bounds__(128) rig_jtk_kernel(const double *__restrict__
   }
 }
 
+// K block k = (s, v): K_sv[m, c] = sum over its terms (slot t of v, ascending) of J_t[:, c]^T H_st[m, :], H_st read
+// from the slot blocks Hb (transposed when s > t). One thread per row m; the sums start at -0.0.
+__global__ void __launch_bounds__(128) rig_k_blocks_kernel(const int2 *__restrict__ kkey, const long long *kptr,
+                                                           const int2 *__restrict__ kterm, long long nk,
+                                                           const double *__restrict__ Hb, const double *state,
+                                                           const int *base_of, const int *var_unknown, int B,
+                                                           double *__restrict__ K) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= 6 * nk) return;
+  const long long k = i / 6;
+  const int m = (int)(i % 6);
+  const bool lidar = var_unknown[kkey[k].y] >= B;
+  double acc[6];
+#pragma unroll
+  for (int c = 0; c < 6; c++) acc[c] = -0.0;
+  for (long long q = kptr[k]; q < kptr[k + 1]; q++) {
+    const int2 w = kterm[q];
+    const double *hb = Hb + 36 * (size_t)(w.x >> 1);
+    double h[6];  // row m of H_st
+#pragma unroll
+    for (int n = 0; n < 6; n++) h[n] = (w.x & 1) ? hb[6 * m + n] : hb[6 * n + m];
+    if (!lidar) {
+#pragma unroll
+      for (int c = 0; c < 6; c++) acc[c] += h[c];
+      continue;
+    }
+    double r[9], p[3];
+    load_pose(state + 12 * (size_t)base_of[w.y], r, p);
+#pragma unroll
+    for (int c = 0; c < 6; c++) acc[c] += ad_column_dot(r, p, c, h);
+  }
+#pragma unroll
+  for (int c = 0; c < 6; c++) K[36 * (size_t)k + 6 * c + m] = acc[c];
+}
+
+// One warp per rig pair p = (u, v), u <= v: block[r, c] = sum over its terms (slot s of u with K block (s, v),
+// ascending) of J_s[:, r]^T K_sv[:, c], each slot's correction added after its term: on a (base, lidar) pair for the
+// slots of u on that lidar (rig_correction with the roles of r and c swapped: the dense kernel's (lidar, base) entry),
+// on a (lidar, same lidar) pair for every slot. Lane l takes the terms l, l + 32, ... from -0.0; the lanes' sums meet
+// in warp_sum. A diagonal pair keeps its lower triangle, mirrored, and sums g_rig(u) over the same terms.
+__global__ void __launch_bounds__(128) rig_jtk_blocks_kernel(const int2 *__restrict__ pairs, const long long *jptr,
+                                                             const int2 *__restrict__ jterm, long long np,
+                                                             const double *__restrict__ K, const double *g,
+                                                             const double *state, const int *base_of,
+                                                             const int *lidar_of, const int *var_unknown, int B,
+                                                             double *__restrict__ blocks, double *__restrict__ gr) {
+  const long long p = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (p >= np) return;
+  const int2 pr = pairs[p];
+  const int ku = var_unknown[pr.x], kv = var_unknown[pr.y];
+  const bool lidar = ku >= B, diag = pr.x == pr.y;
+  const bool corr = kv >= B && (diag || !lidar);  // (lidar, same lidar) or (base, lidar)
+  double acc[36], ga[6];
+#pragma unroll
+  for (int e = 0; e < 36; e++) acc[e] = -0.0;
+#pragma unroll
+  for (int a = 0; a < 6; a++) ga[a] = -0.0;
+  for (long long t = jptr[p] + lane; t < jptr[p + 1]; t += 32) {
+    const int2 w = jterm[t];
+    const int s = w.x;
+    const double *k = K + 36 * (size_t)w.y;
+    double r[9], q[3];
+    if (lidar || corr) load_pose(state + 12 * (size_t)base_of[s], r, q);
+#pragma unroll
+    for (int c = 0; c < 6; c++)
+#pragma unroll
+      for (int a = 0; a < 6; a++) acc[6 * c + a] += lidar ? ad_column_dot(r, q, a, k + 6 * c) : k[6 * c + a];
+    if (corr && (diag || lidar_of[s] == kv - B)) {
+      const double *gs = g + 6 * (size_t)s;
+#pragma unroll
+      for (int c = 0; c < 6; c++)
+#pragma unroll
+        for (int a = 0; a < 6; a++)
+          acc[6 * c + a] += diag ? rig_correction(r, q, gs, a, c, false) : rig_correction(r, q, gs, c, a, true);
+    }
+    if (diag) {
+#pragma unroll
+      for (int a = 0; a < 6; a++) ga[a] += lidar ? ad_column_dot(r, q, a, g + 6 * (size_t)s) : g[6 * (size_t)s + a];
+    }
+  }
+  double *out = blocks + 36 * (size_t)p;
+#pragma unroll
+  for (int e = 0; e < 36; e++) {
+    const double h = warp_sum(acc[e]);
+    const int a = e % 6, c = e / 6;
+    if (lane == (e & 31)) {
+      if (!diag) {
+        out[e] = h;
+      } else if (a >= c) {
+        out[e] = h;
+        out[6 * a + c] = h;
+      }
+    }
+  }
+  if (diag) {
+#pragma unroll
+    for (int a = 0; a < 6; a++) {
+      const double h = warp_sum(ga[a]);
+      if (lane == a) gr[6 * (size_t)pr.x + a] = h;
+    }
+  }
+}
+
 // Free unknowns take the left step of their slice of dx; fixed ones are copied.
 __global__ void rig_update_kernel(const double *state, const double *dx, const int *var_of, int U, double *out) {
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
@@ -198,9 +340,10 @@ __global__ void rig_update_kernel(const double *state, const double *dx, const i
 }  // namespace
 
 int rig_build(cudaStream_t st, int N, int B, int L, const int32_t *base_of, const int32_t *lidar_of,
-              const uint8_t *base_fixed, const uint8_t *lidar_fixed, Rig **out) {
-  std::unique_ptr<Rig, void (*)(Rig *)> r(new Rig(), rig_free);
+              const uint8_t *base_fixed, const uint8_t *lidar_fixed, bool sparse, Rig **out) {
+  std::unique_ptr<Rig> r(new Rig());
   r->N = N; r->B = B; r->L = L;
+  r->sparse = sparse;
   const int U = B + L;
   std::vector<int> var_of(U, -1), var_unknown;
   for (int j = 0; j < U; j++) {
@@ -228,11 +371,20 @@ int rig_build(cudaStream_t st, int N, int B, int L, const int32_t *base_of, cons
   TRY(dev_alloc(&r->var_slot, var_slot.size()));
   TRY(dev_alloc(&r->state, 12 * (size_t)U));
   TRY(dev_alloc(&r->state_trial, 12 * (size_t)U));
-  TRY(dev_alloc(&r->H, nr * nr + nr));
   TRY(dev_alloc(&r->dx, nr));
   TRY(dev_alloc(&r->dvec, nr));
-  TRY(dev_alloc(&r->A, nr * nr));
-  TRY(dev_alloc(&r->K, nr * n));
+  if (sparse) {
+    TRY(dev_alloc(&r->gb, nr));
+    r->h_base_of.assign(base_of, base_of + N);
+    r->h_lidar_of.assign(lidar_of, lidar_of + N);
+    r->h_var_of = var_of;
+    r->bytes = (long long)(sizeof(int) * (2 * (size_t)N + U + r->F + r->F + 1 + std::max<size_t>(1, var_slot.size())) +
+                           sizeof(double) * (24 * (size_t)U + 3 * nr));
+  } else {
+    TRY(dev_alloc(&r->H, nr * nr + nr));
+    TRY(dev_alloc(&r->A, nr * nr));
+    TRY(dev_alloc(&r->K, nr * n));
+  }
   CUDA_TRY(cudaMemcpyAsync(r->base_of, base_of, sizeof(int) * N, cudaMemcpyHostToDevice, st));
   CUDA_TRY(cudaMemcpyAsync(r->lidar_of, lidar_of, sizeof(int) * N, cudaMemcpyHostToDevice, st));
   CUDA_TRY(cudaMemcpyAsync(r->var_of, var_of.data(), sizeof(int) * U, cudaMemcpyHostToDevice, st));
@@ -244,6 +396,153 @@ int rig_build(cudaStream_t st, int N, int B, int L, const int32_t *base_of, cons
   return BALM_OK;
 }
 
+int rig_blocks_sync(Rig *r, cudaStream_t st, const std::vector<int2> &slot_pairs, long long gen, double *scal,
+                    int *flags, const char *who) {
+  if (r->pat && r->pat->gen == gen) return BALM_OK;
+  const int N = r->N, B = r->B, F = r->F;
+  auto refuse = [&](const char *what) {
+    balm_set_error(std::string(who) + ": " + what);
+    return (int)BALM_ERR_UNSUPPORTED;
+  };
+  // the free unknowns of every slot, ascending (its base pose's before its extrinsic's)
+  auto free_of = [&](int s, int *u) {
+    int n = 0;
+    const int a = r->h_var_of[r->h_base_of[s]], b = r->h_var_of[B + r->h_lidar_of[s]];
+    if (a >= 0) u[n++] = a;
+    if (b >= 0) u[n++] = b;
+    return n;
+  };
+  // every slot's neighbours t in the slot pattern, ascending, with 2 x pair + (s > t)
+  std::vector<long long> aptr((size_t)N + 1, 0);
+  for (const int2 &q : slot_pairs) {
+    aptr[q.x + 1]++;
+    if (q.x != q.y) aptr[q.y + 1]++;
+  }
+  for (int s = 0; s < N; s++) aptr[s + 1] += aptr[s];
+  std::vector<int2> adj(aptr[N]);  // (t, source); the ascending pairs fill every list in ascending t
+  {
+    std::vector<long long> fill(aptr.begin(), aptr.end() - 1);
+    for (size_t p = 0; p < slot_pairs.size(); p++) {
+      const int2 q = slot_pairs[p];
+      adj[fill[q.x]++] = make_int2(q.y, (int)(2 * p));
+      if (q.x != q.y) adj[fill[q.y]++] = make_int2(q.x, (int)(2 * p + 1));
+    }
+  }
+  // K blocks (s, v) for v >= the first free unknown of s, with their terms (t ascending); every slot gets the K blocks
+  // of its own free unknowns even without a diagonal slot pair
+  std::vector<int2> kkey, kterm;
+  std::vector<long long> kptr;
+  {
+    std::vector<int3> cand;  // (v, t, source); t = -1: a block without this term
+    for (int s = 0; s < N; s++) {
+      int us[2], ut[2];
+      const int ns = free_of(s, us);
+      if (!ns) continue;
+      cand.clear();
+      for (int a = 0; a < ns; a++) cand.push_back(make_int3(us[a], -1, -1));
+      for (long long q = aptr[s]; q < aptr[s + 1]; q++) {
+        const int nt = free_of(adj[q].x, ut);
+        for (int b = 0; b < nt; b++)
+          if (ut[b] >= us[0]) cand.push_back(make_int3(ut[b], adj[q].x, adj[q].y));
+      }
+      std::stable_sort(cand.begin(), cand.end(), [](const int3 &x, const int3 &y) { return x.x < y.x; });
+      for (size_t q = 0; q < cand.size(); q++) {
+        if (q == 0 || cand[q].x != cand[q - 1].x) {
+          kptr.push_back((long long)kterm.size());
+          kkey.push_back(make_int2(s, cand[q].x));
+        }
+        if (cand[q].y >= 0) kterm.push_back(make_int2(cand[q].z, cand[q].y));
+      }
+    }
+    kptr.push_back((long long)kterm.size());
+  }
+  const long long nk = (long long)kkey.size();
+  if (nk >= (1LL << 31)) return refuse("2^31 or more rig K blocks");
+  // rig pairs (u, v), u <= v: one term (s, k) for every K block k = (s, v) and free unknown u <= v of s, in ascending k,
+  // hence ascending s within a pair
+  std::vector<unsigned long long> key;
+  key.reserve(2 * nk);
+  for (long long k = 0; k < nk; k++) {
+    int us[2];
+    const int ns = free_of(kkey[k].x, us);
+    for (int a = 0; a < ns; a++)
+      if (us[a] <= kkey[k].y) key.push_back((unsigned long long)us[a] * F + kkey[k].y);
+  }
+  std::vector<unsigned long long> ukey(key);
+  std::sort(ukey.begin(), ukey.end());
+  ukey.erase(std::unique(ukey.begin(), ukey.end()), ukey.end());
+  if (ukey.size() >= ((size_t)1 << 30)) return refuse("2^30 or more rig block pairs");
+  std::unique_ptr<RigPattern> pat(new RigPattern());
+  const size_t np = ukey.size();
+  pat->gen = gen;
+  pat->nk = nk;
+  pat->pairs.resize(np);
+  for (size_t p = 0; p < np; p++) pat->pairs[p] = make_int2((int)(ukey[p] / F), (int)(ukey[p] % F));
+  std::vector<long long> jptr(np + 1, 0);
+  std::vector<int> jpair(key.size());
+  for (size_t q = 0; q < key.size(); q++) {
+    jpair[q] = (int)(std::lower_bound(ukey.begin(), ukey.end(), key[q]) - ukey.begin());
+    jptr[jpair[q] + 1]++;
+  }
+  for (size_t p = 0; p < np; p++) jptr[p + 1] += jptr[p];
+  std::vector<int2> jterm(key.size());
+  {
+    std::vector<long long> fill(jptr.begin(), jptr.end() - 1);
+    size_t q = 0;
+    for (long long k = 0; k < nk; k++) {
+      int us[2];
+      const int ns = free_of(kkey[k].x, us);
+      for (int a = 0; a < ns; a++)
+        if (us[a] <= kkey[k].y) jterm[fill[jpair[q++]]++] = make_int2(kkey[k].x, (int)k);
+    }
+  }
+  auto put = [&](auto **d, const auto &h) -> int {  // pat frees whatever it holds when a step fails
+    TRY(dev_alloc(d, h.size()));
+    pat->bytes += (long long)(sizeof(**d) * std::max<size_t>(1, h.size()));
+    if (!h.empty()) CUDA_TRY(cudaMemcpyAsync(*d, h.data(), sizeof(**d) * h.size(), cudaMemcpyHostToDevice, st));
+    return BALM_OK;
+  };
+  TRY(put(&pat->kkey, kkey));
+  TRY(put(&pat->kptr, kptr));
+  TRY(put(&pat->kterm, kterm));
+  TRY(put(&pat->pair_dev, pat->pairs));
+  TRY(put(&pat->jptr, jptr));
+  TRY(put(&pat->jterm, jterm));
+  TRY(dev_alloc(&pat->K, 36 * (size_t)nk));
+  TRY(dev_alloc(&pat->blocks, 36 * np));
+  pat->bytes += (long long)(sizeof(double) * 36 * (std::max<size_t>(1, (size_t)nk) + np));
+  TRY(sparse_solver_build(st, F, pat->pairs, pat->blocks, r->gb, r->dvec, r->dx, scal, flags, who, &pat->solver));
+  CUDA_TRY(cudaStreamSynchronize(st));  // the host tables above are freed on return
+  r->pat = std::move(pat);
+  return BALM_OK;
+}
+
+int rig_reduce_blocks(const Rig *r, cudaStream_t st, const double *state, const double *Hb, const double *g,
+                      long long *launches) {
+  const RigPattern &u = *r->pat;
+  const long long np = (long long)u.pairs.size();
+  if (u.nk)
+    rig_k_blocks_kernel<<<(unsigned)((6 * u.nk + 127) / 128), 128, 0, st>>>(u.kkey, u.kptr, u.kterm, u.nk, Hb, state,
+                                                                            r->base_of, r->var_unknown, r->B, u.K);
+  rig_jtk_blocks_kernel<<<(unsigned)((32 * np + 127) / 128), 128, 0, st>>>(u.pair_dev, u.jptr, u.jterm, np, u.K, g,
+                                                                           state, r->base_of, r->lidar_of,
+                                                                           r->var_unknown, r->B, u.blocks, r->gb);
+  *launches += 2;
+  CUDA_TRY(cudaGetLastError());
+  return BALM_OK;
+}
+
+bool rig_sparse(const Rig *r) { return r->sparse; }
+const std::vector<int2> &rig_pairs(const Rig *r) { return r->pat->pairs; }
+const double *rig_blocks(const Rig *r) { return r->pat->blocks; }
+SparseSolver *rig_solver(const Rig *r) { return r->pat->solver; }
+
+long long rig_blocks_bytes(const Rig *r, int64_t *l_blocks, int64_t *levels) {
+  int64_t sb = 0;
+  sparse_solver_stats(r->pat->solver, l_blocks, levels, &sb);
+  return r->bytes + r->pat->bytes + sb;
+}
+
 int rig_n(const Rig *r) { return 6 * r->F; }
 int rig_bases(const Rig *r) { return r->B; }
 int rig_lidars(const Rig *r) { return r->L; }
@@ -251,6 +550,7 @@ bool rig_any_base_fixed(const Rig *r) { return r->any_base_fixed; }
 int rig_free_bases(const Rig *r) { return r->FB; }
 DenseSystem rig_system(Rig *r) {
   const int nr = 6 * r->F;
+  if (r->sparse) return DenseSystem{nr, nullptr, r->gb, r->dx, r->dvec, nullptr, &r->lw};
   return DenseSystem{nr, r->H, r->H + (size_t)nr * nr, r->dx, r->dvec, r->A, &r->lw};
 }
 double *rig_state(Rig *r, bool trial) { return trial ? r->state_trial : r->state; }

@@ -49,14 +49,16 @@ def calibrate_rig(xyz, scan, base_of, lidar_of, base12, ext12, voxel_size=2.0, r
     poses and extrinsics. Each of the `rounds` rounds cuts plane voxels (Context.cut_voxels with voxel_size, layer_limit,
     min_ps, eigen_value_array) at the composed scan poses and runs rig_damping_iter (max_iter, gauge_mode,
     min_planes_per_pose and any other damping_iter keyword in lm). gauge_mode defaults to 2, which keeps the input's
-    frame. -> (base12, ext12, traces), traces one LM trace per round."""
+    frame. precision=PREC_BLOCKS runs the block-sparse rig (Context.set_block_rig), for long drives. -> (base12, ext12,
+    traces), traces one LM trace per round."""
     base_of = np.asarray(base_of, dtype=np.int32)
     lidar_of = np.asarray(lidar_of, dtype=np.int32)
     base = np.array(base12, dtype=np.float64, copy=True).reshape(-1, 12)
     ext = np.array(ext12, dtype=np.float64, copy=True).reshape(-1, 12)
     ctx = Context(len(base_of), device, precision)
     try:
-        ctx.set_rig(base_of, lidar_of, fixed_bases=fixed_bases, fixed_lidars=fixed_lidars)
+        set_rig = ctx.set_block_rig if precision == L.PREC_BLOCKS else ctx.set_rig
+        set_rig(base_of, lidar_of, fixed_bases=fixed_bases, fixed_lidars=fixed_lidars)
         traces = []
         for _ in range(rounds):
             ctx.cut_voxels(xyz, scan, rig_poses(base, ext, base_of, lidar_of), voxel_size=voxel_size,

@@ -463,7 +463,7 @@ int balm_pose_graph_iter(balm_ctx *ctx, double *poses12, const balm_lm_opts *opt
  * *n_rig_out = 6 x the free count. With every extrinsic free the cost has a second gauge (T_b Q, Q^-1 E_l): fix one
  * reference LiDAR, as MLCC does. The rig belongs to the ctx: every voxel registration keeps it, and balm_evaluate,
  * balm_damping_iter, the pose-graph and covariance calls ignore it. n_base == 0 detaches it. Refused, with the previous
- * rig kept: BALM_ERR_UNSUPPORTED on a BALM_PREC_BLOCKS ctx; BALM_ERR_INVALID with a communicator attached, for a base or
+ * rig kept: BALM_ERR_UNSUPPORTED on a BALM_PREC_BLOCKS ctx (it takes balm_block_set_rig); BALM_ERR_INVALID with a communicator attached, for a base or
  * LiDAR index out of range, a base or LiDAR no slot uses, or when every unknown is fixed. Device memory: the rig holds
  * K = H J (n_rig x 6N doubles), H_rig and its factor (2 n_rig^2) on top of the ctx's H and factor (2 (6N)^2); a rig with
  * about one free unknown per slot (n_rig ~ 6N) therefore needs about twice the ctx's dense memory, and balm_set_rig
@@ -504,6 +504,35 @@ int balm_rig_covariance(balm_ctx *ctx, const double *base12, const double *ext12
  * poses set the frame; pass 2), and without a rig or registered voxels. */
 int balm_rig_damping_iter(balm_ctx *ctx, double *base12, double *ext12, const balm_lm_opts *opts, balm_trace *trace,
                           int *n_iters, double *rig_per_iter);
+
+/* Rig calibration on a BALM_PREC_BLOCKS ctx (DESIGN.md "Rig calibration on block-sparse voxel BA"): balm_set_rig's
+ * arguments, checks, error codes and lifetime (n_base == 0 detaches; a refused call keeps the previous rig);
+ * BALM_ERR_INVALID on any other precision. Nothing of size n_rig x 6N or n_rig^2 is held: H_rig is kept as the 6x6
+ * blocks of the rig pairs (u, v), u <= v over the free unknowns, for which some slot of u and some slot of v form a
+ * block pair of the ctx (balm_block_structure's pattern, pose factors and priors included), plus every diagonal pair,
+ * and solved by the nested-dissection block LDL^T of the ctx. The rig's pattern follows the ctx's: every rig call after
+ * a voxel registration, balm_block_set_factors or balm_set_pose_priors rebuilds it (BALM_ERR_UNSUPPORTED from that call
+ * when it is too large to index). balm_rig_evaluate (H expanded on the host from the blocks) and balm_rig_damping_iter
+ * take such a rig with their usual arguments and meaning; the cost is the ctx's full cost: voxels, then pose factors,
+ * then priors, all at the composed scan poses (with an active prior gauge_mode 0 and 1 are BALM_ERR_INVALID, as for
+ * balm_damping_iter). balm_rig_covariance is BALM_ERR_UNSUPPORTED for it. */
+int balm_block_set_rig(balm_ctx *ctx, int n_base, int n_lidar, const int32_t *base_of, const int32_t *lidar_of,
+                       const uint8_t *base_fixed, const uint8_t *lidar_fixed, int *n_rig_out);
+/* The block-sparse rig's pattern, as balm_block_structure: stats[0] rig block pairs, stats[1] blocks of its L,
+ * stats[2] elimination-tree levels, stats[3] device bytes the rig holds (tables, states, K blocks, blocks, solver);
+ * pairs (may be NULL): 2 x stats[0] int32, the (u, v), u <= v, in balm_set_rig's unknown order, ascending.
+ * BALM_ERR_INVALID without a balm_block_set_rig rig or registered voxels. */
+int balm_rig_block_structure(balm_ctx *ctx, int64_t stats[4], int32_t *pairs);
+/* Sigma = H~_rig^-1 on the rig's block pattern (balm_rig_block_structure's order, [pairs][36] column-major, rows of u),
+ * H~_rig balm_rig_evaluate's H_rig at base12 / ext12 and include_fix without the anchor's rows and columns: the
+ * Laplace form balm_block_covariance gives for scan poses. anchor: -1 or the free index of a free base pose (as
+ * balm_rig_covariance); its blocks are 0. H_rig holds the composition's second-order term, so away from the optimum it
+ * can be indefinite: pass balm_rig_damping_iter's result. BALM_ERR_NOT_PD when H~_rig is singular or indefinite
+ * (balm_block_covariance's test),
+ * BALM_ERR_INVALID without a balm_block_set_rig rig or registered voxels, for a NULL argument or a bad anchor. The next
+ * balm_rig_damping_iter is unaffected. */
+int balm_rig_block_covariance(balm_ctx *ctx, const double *base12, const double *ext12, int include_fix, int anchor,
+                              double *cov);
 
 /* Sparse pose graph (DESIGN.md "Pose graph", "Sparse solve"): the same factors, cost and LM as balm_set_pose_factors /
  * balm_pose_graph_iter, with H held as its nonzero 6x6 blocks and the damped system solved by a block LDL^T in a
