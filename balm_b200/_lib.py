@@ -63,7 +63,8 @@ SYMBOLS = ["balm_last_error", "balm_version", "balm_create", "balm_destroy", "ba
            "balm_spg_set_pose_priors", "balm_spg_prior_residuals", "balm_set_voxel_loss", "balm_voxel_residuals",
            "balm_batch_set_voxel_loss", "balm_batch_voxel_residuals",
            "balm_set_rig", "balm_rig_evaluate", "balm_rig_damping_iter", "balm_rig_covariance",
-           "balm_block_set_rig", "balm_rig_block_structure", "balm_rig_block_covariance"]
+           "balm_block_set_rig", "balm_rig_block_structure", "balm_rig_block_covariance",
+           "balm_block_point_covariance", "balm_rig_block_point_covariance"]
 
 
 def lib():
@@ -180,6 +181,10 @@ def lib():
         L.balm_block_set_rig.argtypes = L.balm_set_rig.argtypes
         L.balm_rig_block_structure.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
         L.balm_rig_block_covariance.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]
+        L.balm_block_point_covariance.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_double, C.c_int, C.c_int,
+                                                  C.c_int] + [C.c_void_p] * 4
+        L.balm_rig_block_point_covariance.argtypes = [C.c_void_p] + [C.c_void_p] * 3 + [C.c_double, C.c_int, C.c_int,
+                                                                                          C.c_int] + [C.c_void_p] * 3
         _lib = L
     return _lib
 

@@ -267,6 +267,28 @@ class Context:
         return pairs, _covariance(L.lib().balm_block_covariance, self._h, poses12, len(pairs), int(include_fix),
                                   int(anchor))
 
+    def block_point_covariance(self, poses12, sel, point_noise=0.0, c_cov=None, include_fix=False, anchor=0, joint=True,
+                               want_raw=False):
+        """PREC_BLOCKS contexts: pose_covariance's Rcov restricted to the poses sel, without a 6N x 6N matrix
+        (include/balm_b200.h, balm_block_point_covariance): Sigma = Y^T R Y, Y = H~^-1 E, H~ as block_covariance's (anchor
+        -1 or a pose, deleted; its entries 0), R the raw term. -> the joint (6 s x 6 s) Sigma in sel's order, or with
+        joint=False the (s, 6, 6) marginals (all poses of a long drive fit one call); with want_raw also (pairs [n_pairs, 2],
+        raw [n_pairs, 6, 6]) with raw[p, a, c] = R[6 i + a, 6 j + c]. c_cov: K x 9 x 9 or None (isotropic point_noise)."""
+        poses12 = np.ascontiguousarray(poses12, dtype=np.float64)
+        sel = np.ascontiguousarray(sel, dtype=np.int32).reshape(-1)
+        cc = None if c_cov is None else np.ascontiguousarray(c_cov, dtype=np.float64).reshape(-1, 81)
+        s = len(sel)
+        cov = np.zeros((6 * s, 6 * s), order="F") if joint else None
+        marg = None if joint else np.zeros((s, 36))
+        pairs = self.block_structure(want_pairs=True)["pair_list"] if want_raw else None
+        raw = np.zeros((len(pairs), 36)) if want_raw else None
+        L.check(L.lib().balm_block_point_covariance(self._h, _p(poses12), _p(cc), float(point_noise), int(include_fix),
+                                                    int(anchor), s, _p(sel), _p(raw), _p(cov), _p(marg)))
+        out = cov if joint else marg.reshape(s, 6, 6).transpose(0, 2, 1).copy()
+        if want_raw:
+            return out, (pairs, raw.reshape(-1, 6, 6).transpose(0, 2, 1).copy())
+        return out
+
     def set_block_factors(self, factors):
         """PREC_BLOCKS contexts: pose factors (set_pose_factors' dicts, e.g. from odometry_factors) in the cost, added to
         the voxel cost in every evaluation over all voxels, damping_iter, block_covariance (include/balm_b200.h,
@@ -384,6 +406,22 @@ class Context:
         L.check(L.lib().balm_rig_block_covariance(self._h, _p(base12), _p(ext12), int(include_fix), int(anchor),
                                                   _p(cov)))
         return pairs, cov.reshape(-1, 6, 6).transpose(0, 2, 1)
+
+    def rig_block_point_covariance(self, base12, ext12, sel, point_noise=0.0, c_cov=None, include_fix=False, anchor=-1,
+                                   joint=True):
+        """set_block_rig's rig: rig_covariance's cov restricted to the free unknowns sel (set_rig's order), without an
+        n_rig x n_rig or 6N x 6N matrix (include/balm_b200.h, balm_rig_block_point_covariance). anchor as
+        rig_block_covariance. -> the joint (6 s x 6 s) Sigma in sel's order, or with joint=False the (s, 6, 6) marginals.
+        balm_b200.rig.extrinsic_sigmas(cov, 0) reads it when sel lists the free extrinsics."""
+        base12, ext12, _ = self._rig_shapes(base12, ext12)
+        sel = np.ascontiguousarray(sel, dtype=np.int32).reshape(-1)
+        cc = None if c_cov is None else np.ascontiguousarray(c_cov, dtype=np.float64).reshape(-1, 81)
+        s = len(sel)
+        cov = np.zeros((6 * s, 6 * s), order="F") if joint else None
+        marg = None if joint else np.zeros((s, 36))
+        L.check(L.lib().balm_rig_block_point_covariance(self._h, _p(base12), _p(ext12), _p(cc), float(point_noise),
+                                                        int(include_fix), int(anchor), s, _p(sel), _p(cov), _p(marg)))
+        return cov if joint else marg.reshape(s, 6, 6).transpose(0, 2, 1).copy()
 
     def _rig_shapes(self, base12, ext12):
         if getattr(self, "_rig", None) is None:

@@ -1522,6 +1522,86 @@ extern "C" int balm_rig_block_covariance(balm_ctx *c, const double *base12, cons
   return rc;
 }
 
+// ---------------- point-noise covariance on blocks contexts (covariance.cu) ----------------
+// sel [n_sel]: distinct indices in [0, n) (`what` names them in the message)
+static int point_cov_sel_check(const char *who, int n_sel, const int32_t *sel, int n, const char *what) {
+  const std::string w = std::string(who) + ": ";
+  if (n_sel < 1 || !sel) { balm_set_error(w + "n_sel must be at least 1 with a selection"); return BALM_ERR_INVALID; }
+  std::vector<char> seen((size_t)n, 0);
+  for (int u = 0; u < n_sel; u++) {
+    if (sel[u] < 0 || sel[u] >= n) {
+      balm_set_error(w + "sel[" + std::to_string(u) + "] = " + std::to_string(sel[u]) + " is not a " + what + " in [0, " +
+                     std::to_string(n) + ")");
+      return BALM_ERR_INVALID;
+    }
+    if (seen[sel[u]]) {
+      balm_set_error(w + "sel[" + std::to_string(u) + "] = " + std::to_string(sel[u]) + " is selected twice");
+      return BALM_ERR_INVALID;
+    }
+    seen[sel[u]] = 1;
+  }
+  return BALM_OK;
+}
+
+// The budget refusal of the joint covariance (before anything is enqueued)
+static int point_cov_budget_check(const char *who, int P, int N, int n_sel, bool joint) {
+  if (block_point_cov_fits(P, N, n_sel, joint)) return BALM_OK;
+  balm_set_error(std::string(who) + (joint ? ": the joint covariance's Y, W and Z (8 (6P + 12N) 6 n_sel bytes and its "
+                                             "partial sums) exceed BALM_COV_BUDGET_MB; ask for the marginals alone"
+                                           : ": one unknown's right-hand sides exceed BALM_COV_BUDGET_MB"));
+  return BALM_ERR_UNSUPPORTED;
+}
+
+// The eval of H (or H_rig) at the caller's state, deferred, then the anchored undamped factorisation; the evaluation's
+// events are read after the factorisation's wait (as block_covariance)
+static int point_cov_factor(balm_ctx *c, SparseSolver *sp, int anchor, const char *who,
+                            const std::function<int()> &eval, bool rig) {
+  c->defer = true;
+  int rc = eval();
+  c->defer = false;
+  const bool evaluated = rc == BALM_OK;
+  if (rc == BALM_OK) rc = sparse_factor_undamped(sp, c->stream, anchor, who, &c->launches);
+  if (evaluated && (rc == BALM_OK || rc == BALM_ERR_NOT_PD)) {  // the stream has been synchronised
+    TRY(collect_eval(c));
+    if (rig) TRY(rig_collect_reduce(c));
+  }
+  c->pending_eval = false;
+  return rc;
+}
+
+extern "C" int balm_rig_block_point_covariance(balm_ctx *c, const double *base12, const double *ext12,
+                                               const double *c_cov81, double point_noise, int include_fix, int anchor,
+                                               int n_sel, const int32_t *sel, double *cov, double *marg) {
+  const char *who = "balm_rig_block_point_covariance";
+  if (!c || !base12 || !ext12 || (!cov && !marg)) { balm_set_error(std::string(who) + ": bad arguments"); return BALM_ERR_INVALID; }
+  if (c->prec != BALM_PREC_BLOCKS) {
+    balm_set_error(std::string(who) + ": BALM_PREC_BLOCKS contexts only (the dense ones take balm_rig_covariance)");
+    return BALM_ERR_INVALID;
+  }
+  TRY(block_rig_check(c, who));
+  if (c->M < 1) { balm_set_error(std::string(who) + ": no voxels registered"); return BALM_ERR_INVALID; }
+  Rig *rg = c->rig;
+  const int F = rig_n(rg) / 6;
+  if (anchor < -1 || anchor >= rig_free_bases(rg)) {
+    balm_set_error(std::string(who) + ": anchor " + std::to_string(anchor) + " is neither -1 nor a free base index in [0, " +
+                   std::to_string(rig_free_bases(rg)) + ")");
+    return BALM_ERR_INVALID;
+  }
+  TRY(point_cov_sel_check(who, n_sel, sel, F, "free unknown"));
+  TRY(point_cov_budget_check(who, F, c->N, n_sel, cov != nullptr));
+  CUDA_TRY(cudaSetDevice(c->device));
+  SparseSolver *sp = rig_solver(rg);
+  TRY(point_cov_factor(c, sp, anchor, who, [&]() -> int {
+    TRY(rig_upload(c, base12, ext12));
+    return rig_evaluate_dev(c, include_fix != 0);  // composes the slot poses into c->poses
+  }, true));
+  ScratchPool pool;
+  double *raw = nullptr;
+  TRY(pool.get(&raw, 36 * blocks_pairs(c->bh).size()));
+  TRY(cov_raw_blocks_dev(c, pool, c->poses, c_cov81, point_noise, include_fix != 0, raw));
+  return block_point_cov_dev(c, sp, rg, rig_state(rg, false), anchor, n_sel, sel, raw, cov, marg);
+}
+
 // ---------------- absolute pose priors (pose_graph.cu) ----------------
 // The argument checks of balm_set_pose_priors and balm_spg_set_pose_priors over P poses (n_priors >= 1)
 static int pose_priors_check(const char *who, int P, int n, const int32_t *pose, const double *hat12,
@@ -1917,6 +1997,42 @@ extern "C" int balm_block_covariance(balm_ctx *c, const double *poses12, int inc
   }
   if (anchor < -1 || anchor >= c->N) { balm_set_error("balm_block_covariance: anchor outside [-1, N)"); return BALM_ERR_INVALID; }
   return block_covariance(c, "balm_block_covariance", poses12, include_fix != 0, anchor, cov);
+}
+
+extern "C" int balm_block_point_covariance(balm_ctx *c, const double *poses12, const double *c_cov81, double point_noise,
+                                           int include_fix, int anchor, int n_sel, const int32_t *sel,
+                                           double *raw_blocks, double *cov, double *marg) {
+  const char *who = "balm_block_point_covariance";
+  if (!c || !poses12 || (!raw_blocks && !cov && !marg)) {
+    balm_set_error(std::string(who) + ": bad arguments");
+    return BALM_ERR_INVALID;
+  }
+  if (c->prec != BALM_PREC_BLOCKS || !c->bh || !c->registered || c->M < 1) {
+    balm_set_error(std::string(who) + ": no voxels registered on a BALM_PREC_BLOCKS context");
+    return BALM_ERR_INVALID;
+  }
+  if (c->world > 1 || c->comm) { balm_set_error(std::string(who) + ": single-GPU contexts only"); return BALM_ERR_INVALID; }
+  if (anchor < -1 || anchor >= c->N) { balm_set_error(std::string(who) + ": anchor outside [-1, N)"); return BALM_ERR_INVALID; }
+  const bool sigma = cov || marg;
+  if (sigma) {
+    TRY(point_cov_sel_check(who, n_sel, sel, c->N, "pose"));
+    TRY(point_cov_budget_check(who, c->N, c->N, n_sel, cov != nullptr));
+  }
+  CUDA_TRY(cudaSetDevice(c->device));
+  SparseSolver *sp = blocks_solver(c->bh);
+  CUDA_TRY(cudaMemcpyAsync(c->poses, poses12, sizeof(double) * 12 * c->N, cudaMemcpyHostToDevice, c->stream));
+  if (sigma)
+    TRY(point_cov_factor(c, sp, anchor, who, [&]() { return balm_cov_evaluate_hessian(c, c->poses, include_fix != 0); },
+                         false));
+  ScratchPool pool;
+  double *raw = nullptr;
+  const size_t nraw = 36 * blocks_pairs(c->bh).size();
+  TRY(pool.get(&raw, nraw));
+  TRY(cov_raw_blocks_dev(c, pool, c->poses, c_cov81, point_noise, include_fix != 0, raw));
+  if (sigma) TRY(block_point_cov_dev(c, sp, nullptr, nullptr, anchor, n_sel, sel, raw, cov, marg));
+  if (raw_blocks) CUDA_TRY(cudaMemcpyAsync(raw_blocks, raw, sizeof(double) * nraw, cudaMemcpyDeviceToHost, c->stream));
+  CUDA_TRY(cudaStreamSynchronize(c->stream));
+  return BALM_OK;
 }
 
 // ---------------- sparse pose graph (pose_graph.cu, pose_graph_sparse.cu, blocks.cu) ----------------

@@ -144,6 +144,64 @@ __global__ void __launch_bounds__(256) blocks_kernel(const int2 *pairs, const lo
   }
 }
 
+// The point-noise raw term in blocks_kernel's shape (one warp per pair, the same term ranges and butterfly): per term
+// (s_i, s_j) the partner-row product sum_m rows[s_i][m] rows[s_j][m ^ 4]^T of covariance.cu's eight rows, rows of
+// observation s at rows + 48 (s - row_ptr[v0]); Dacc (the diagonal blocks c2^2 D, [21][N], upper triangle) added on a
+// diagonal pair when not null. A pair without voxel terms in the batch gets a zero sum.
+__global__ void __launch_bounds__(256) raw_blocks_kernel(const int2 *pairs, const long long *tptr,
+                                                         const unsigned long long *term, long long npairs,
+                                                         const double *rows, const long long *row_ptr, int64_t v0,
+                                                         int64_t v1, const double *Dacc, int N, int add, double *raw) {
+  const long long p = ((long long)blockIdx.x * 256 + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (p >= npairs) return;
+  const unsigned lo = (unsigned)row_ptr[v0], hi = (unsigned)row_ptr[v1];
+  long long t0 = tptr[p], t1 = tptr[p + 1];
+  {
+    long long l = t0, h = t1;
+    while (l < h) { const long long m = (l + h) >> 1; if ((unsigned)term[m] < lo) l = m + 1; else h = m; }
+    t0 = l;
+    h = t1;
+    while (l < h) { const long long m = (l + h) >> 1; if ((unsigned)term[m] < hi) l = m + 1; else h = m; }
+    t1 = l;
+  }
+  double acc[36];
+#pragma unroll
+  for (int e = 0; e < 36; e++) acc[e] = 0.0;
+  for (long long t = t0 + lane; t < t1; t += 32) {
+    const unsigned long long w = term[t];
+    const double *gi = rows + 48 * (size_t)((unsigned)w - lo), *gj = rows + 48 * (size_t)((unsigned)(w >> 32) - lo);
+#pragma unroll
+    for (int m = 0; m < 8; m++) {
+      double a[6], b[6];
+#pragma unroll
+      for (int r = 0; r < 6; r++) {
+        a[r] = __ldg(gi + 6 * m + r);
+        b[r] = __ldg(gj + 6 * (m ^ 4) + r);
+      }
+#pragma unroll
+      for (int c = 0; c < 6; c++)
+#pragma unroll
+        for (int r = 0; r < 6; r++) acc[6 * c + r] = fma(a[r], b[c], acc[6 * c + r]);
+    }
+  }
+  const int2 pr = pairs[p];
+  double *B = raw + 36 * (size_t)p;
+#pragma unroll
+  for (int e = 0; e < 36; e++) {
+    double h = warp_sum(acc[e]);
+    if (lane == (e & 31)) {
+      if (add) h = B[e] + h;
+      if (Dacc && pr.x == pr.y) {
+        const int r = e % 6, c = e / 6, r6 = r < c ? r : c, c6 = r < c ? c : r;
+        const int q = r6 * 6 - r6 * (r6 - 1) / 2 + (c6 - r6);
+        h += Dacc[(size_t)q * N + pr.x];
+      }
+      B[e] = h;
+    }
+  }
+}
+
 // y[t] += x[t]: a blocks context's factor g and cost added onto the voxel ones (one add per entry, fixed order)
 __global__ void add_kernel(const double *x, int n, double *y) {
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
@@ -353,6 +411,19 @@ int blocks_zero(balm_ctx *c) {
   if (u.factors_only) return BALM_OK;  // blocks_add_factors writes every block, g and r
   CUDA_TRY(cudaMemsetAsync(u.blocks, 0, sizeof(double) * 36 * u.pairs.size(), c->stream));
   CUDA_TRY(cudaMemsetAsync(c->g, 0, sizeof(double) * ((size_t)c->n + 1), c->stream));
+  return BALM_OK;
+}
+
+int launch_raw_blocks(balm_ctx *c, const double *rows, int64_t v0, int64_t v1, const double *Dacc, bool add, double *raw) {
+  const BlockHessian *b = c->bh;
+  const BlockPattern &u = *b->pat;
+  if (!u.pair_dev) { balm_set_error("raw blocks: the pattern has no voxel pairs"); return BALM_ERR_INVALID; }
+  const long long np = (long long)u.pairs.size();
+  raw_blocks_kernel<<<(unsigned)((32 * np + 255) / 256), 256, 0, c->stream>>>(u.pair_dev, u.tptr, b->term, np, rows,
+                                                                              c->row_ptr, v0, v1, Dacc, c->N, add ? 1 : 0,
+                                                                              raw);
+  c->launches += 1;
+  CUDA_TRY(cudaGetLastError());
   return BALM_OK;
 }
 

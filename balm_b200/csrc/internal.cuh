@@ -834,6 +834,18 @@ int refine_solution(balm_ctx *c, const DenseSystem &s, int *still_bad);
 // partials and the assembly of balm_pose_covariance)
 int cov_raw_dev(balm_ctx *c, ScratchPool &pool, const double *poses_dev, const double *ccov_host, double point_noise,
                 bool include_fix, double **R_out);
+// A BALM_PREC_BLOCKS context's raw term at the device poses into raw [pairs][36] on its slot pattern (enqueued; voxel
+// batches under BALM_COV_BUDGET_MB with cov_raw_dev's stats and rows, each observation's rows stored on their own)
+int cov_raw_blocks_dev(balm_ctx *c, ScratchPool &pool, const double *poses_dev, const double *ccov_host,
+                       double point_noise, bool include_fix, double *raw);
+// The joint (n_sel x 6)^2 covariance of the selection, or its marginals alone, fit BALM_COV_BUDGET_MB (P: the solver's
+// unknowns, N: slots)
+bool block_point_cov_fits(int P, int N, int n_sel, bool joint);
+// Sigma_sel = W^T R W, W = J Y, Y = A^-1 E after sparse_factor_undamped(sp, anchor): rig null for the context's own
+// unknowns (J = I), else the rig at state; sel [n_sel] distinct unknowns; raw the device raw term on the slot pattern.
+// cov_host (6 n_sel)^2 column-major or null (then the marginals in chunks), marg_host [n_sel][36] or null. Waits.
+int block_point_cov_dev(balm_ctx *c, SparseSolver *sp, const Rig *rig, const double *state, int anchor, int n_sel,
+                        const int32_t *sel, const double *raw, double *cov_host, double *marg_host);
 // undamped LDL^T of s (launch_ldlt_solve with u = 0), then one wait: BALM_ERR_NOT_PD with singular_msg for a bad pivot
 // or min |d| not above 1e-11 max |d|, pivots [skip, skip + 6) left out of both (skip -1: none)
 int cov_factor(balm_ctx *c, const DenseSystem &s, int skip, const char *singular_msg);
@@ -962,6 +974,10 @@ const double *rig_blocks(const Rig *r);            // device [pairs][36], column
 SparseSolver *rig_solver(const Rig *r);
 // device bytes the rig holds (tables, states, vectors, pattern, blocks and solver); l_blocks / levels of its L
 long long rig_blocks_bytes(const Rig *r, int64_t *l_blocks, int64_t *levels);
+// W = J Y at state (enqueued): Y [6 x free unknowns][ld] row-major with unknown u's rows at 6 col[u] (device col),
+// W [6N][ld], the first ncols columns
+int rig_apply_j(const Rig *r, cudaStream_t st, const double *state, const int *col, const double *Y, int ld, int ncols,
+                double *W, long long *launches);
 // state_out = the left step of the rig's dx on every free unknown of state, fixed ones copied (enqueued)
 int rig_update(const Rig *r, cudaStream_t st, const double *state, double *state_out, long long *launches);
 
@@ -987,6 +1003,18 @@ int sparse_refine(SparseSolver *s, cudaStream_t st, int *h_flags, double *h_scal
 // Waits twice (pivot test, copy-out), and once more on the first call while it builds the tables.
 int sparse_covariance(SparseSolver *s, cudaStream_t st, int anchor, const std::function<int()> &eval, const char *who,
                       double *cov, long long *launches);
+// The undamped factorisation of the solver's blocks with pose anchor's rows and columns replaced by I (anchor -1: none)
+// and the singularity test of sparse_covariance, which runs it after eval: BALM_ERR_NOT_PD (message prefixed with who)
+// when singular. Overwrites L, D, dvec and scal[3]; waits once.
+int sparse_factor_undamped(SparseSolver *s, cudaStream_t st, int anchor, const char *who, long long *launches);
+// Y <- A^-1 Y for the last sparse_factor_undamped's A: Y [6P][ld] row-major, rows in column (elimination) order, the
+// first ncols columns (enqueued). A column's result does not depend on the other columns.
+int sparse_solve_many(SparseSolver *s, cudaStream_t st, double *Y, int ld, int ncols, long long *launches);
+// the column of every pose (host; filled by sparse_factor_undamped), the number of poses, and every pose's pairs (device
+// pp_ptr [P + 1], pp: (2 pair + transposed, other pose), ascending in the other pose)
+const std::vector<int> &sparse_solver_columns(SparseSolver *s);
+int sparse_solver_size(const SparseSolver *s);
+void sparse_solver_pose_pairs(const SparseSolver *s, const int **pp_ptr, const int2 **pp);
 
 // ---------------- block-sparse Hessian of a BALM_PREC_BLOCKS context (blocks.cu) ----------------
 // The registered voxels' pair pattern and update terms, then the union pattern with c->pg's factor pairs and c->pr's
@@ -1020,6 +1048,11 @@ SparseSolver *blocks_solver(const BlockHessian *b);
 long long blocks_generation(const BlockHessian *b);
 // device bytes of the pattern, terms, blocks and solver; l_blocks / levels of the factorisation
 long long blocks_bytes(const BlockHessian *b, int64_t *l_blocks, int64_t *levels);
+// The point-noise raw term R on the pattern (covariance.cu has its terms), one voxel batch [v0, v1): raw [pairs][36]
+// = (add ? raw : 0) + sum over the batch's update terms of the partner-row products of rows [obs - row_ptr[v0]][8][6]
+// (c2 Q^T | c2 V^T of covariance.cu), plus Dacc [21][N] on the diagonal pairs when Dacc is not null (enqueued).
+// BALM_ERR_INVALID without voxel pairs.
+int launch_raw_blocks(balm_ctx *c, const double *rows, int64_t v0, int64_t v1, const double *Dacc, bool add, double *raw);
 
 // ---------------- association (assoc.cu) ----------------
 // The plane voxels of one or more problems cut from raw scans. Host arrays; xyz (n_points x 3 float32, body frame) and

@@ -20,6 +20,10 @@
 //   spg_selinv_kernel    per column of one level, top level first, one CTA: L^ = L L_jj^-1 in place, the column's Z
 //                        blocks from its ancestors' (a warp per block), then its diagonal block
 //   spg_cov_gather_kernel  per (pair, entry): Z's block of every pair of H
+// Point-noise covariance on blocks contexts (sparse_solve_many; DESIGN.md "Point-noise covariance on blocks contexts"):
+// the same undamped, anchored factorisation (sparse_factor_undamped), then many right-hand sides at once.
+//   spg_fwd_many_kernel / spg_back_many_kernel  per (column of one level, tile of right-hand sides), one CTA: the
+//                        forward / backward substitution of spg_factor_kernel<false> / spg_back_kernel, in place
 #include <math.h>
 #include <algorithm>
 #include <memory>
@@ -335,6 +339,65 @@ __global__ void __launch_bounds__(SEL_THREADS) spg_selinv_kernel(SpView v, const
     double e = 0.0;
     for (int r = hi; r < 6; r++) e += Minv[6 * hi + r] * Minv[6 * lo + r] / v.D[6 * (size_t)j + r];
     Z[36 * (size_t)b0 + tid] = e - S[6 * lo + hi];
+  }
+}
+
+// Many right-hand sides (sparse_solve_many): Y [6P rows in column order][ld], row-major, one CTA per (column j of a
+// level, tile of MANY_TILE right-hand sides), thread (row a of the column, right-hand side c). Every right-hand side is
+// summed in the single-RHS kernels' order, independently of the tile it lands in.
+constexpr int MANY_TILE = 32;
+//   forward: y_j = L_jj^-1 (y_j - sum_k L_jk y_k) over row j's off-diagonal blocks in ascending column
+__global__ void __launch_bounds__(6 * MANY_TILE) spg_fwd_many_kernel(SpView v, const int *cols, double *Y, int ld,
+                                                                     int ncols) {
+  __shared__ double sy[6][MANY_TILE];
+  const int j = cols[blockIdx.x], a = threadIdx.x / MANY_TILE, ci = threadIdx.x % MANY_TILE;
+  const int c = blockIdx.y * MANY_TILE + ci;
+  if (c < ncols) {
+    double s = Y[(6 * (size_t)j + a) * ld + c];
+    for (int q = v.rptr[j]; q < v.rptr[j + 1]; q++) {
+      const int p = v.rpos[q];
+      const double *B = v.Lx + 36 * (size_t)p, *yk = Y + 6 * (size_t)v.lcol[p] * ld + c;
+      for (int m = 0; m < 6; m++) s -= B[6 * m + a] * yk[(size_t)m * ld];
+    }
+    sy[a][ci] = s;
+  }
+  __syncthreads();
+  if (a == 0 && c < ncols) {
+    const double *Ljj = v.Lx + 36 * (size_t)v.colptr[j];
+    double y[6];
+    for (int m = 0; m < 6; m++) {
+      double s = sy[m][ci];
+      for (int p = 0; p < m; p++) s -= Ljj[6 * p + m] * y[p];
+      y[m] = s;
+      Y[(6 * (size_t)j + m) * ld + c] = s;
+    }
+  }
+}
+//   backward: x_j = L_jj^-T (D_j^-1 y_j - sum_i L_ij^T x_i) over the column's off-diagonal blocks in ascending row
+__global__ void __launch_bounds__(6 * MANY_TILE) spg_back_many_kernel(SpView v, const int *cols, double *Y, int ld,
+                                                                      int ncols) {
+  __shared__ double sz[6][MANY_TILE];
+  const int j = cols[blockIdx.x], a = threadIdx.x / MANY_TILE, ci = threadIdx.x % MANY_TILE;
+  const int c = blockIdx.y * MANY_TILE + ci;
+  const int b0 = v.colptr[j], b1 = v.colptr[j + 1];
+  if (c < ncols) {
+    double s = Y[(6 * (size_t)j + a) * ld + c] / v.D[6 * (size_t)j + a];
+    for (int b = b0 + 1; b < b1; b++) {
+      const double *B = v.Lx + 36 * (size_t)b, *xi = Y + 6 * (size_t)v.rowidx[b] * ld + c;
+      for (int cc = 0; cc < 6; cc++) s -= B[6 * a + cc] * xi[(size_t)cc * ld];
+    }
+    sz[a][ci] = s;
+  }
+  __syncthreads();
+  if (a == 0 && c < ncols) {
+    const double *Ljj = v.Lx + 36 * (size_t)b0;
+    double z[6];
+    for (int m = 5; m >= 0; m--) {
+      double s = sz[m][ci];
+      for (int p = m + 1; p < 6; p++) s -= Ljj[6 * m + p] * z[p];
+      z[m] = s;
+      Y[(6 * (size_t)j + m) * ld + c] = s;
+    }
   }
 }
 
@@ -731,10 +794,19 @@ static int selinv_build(SparseSolver &s, cudaStream_t st, const char *who) {
   return BALM_OK;
 }
 
-int sparse_covariance(SparseSolver *s, cudaStream_t st, int anchor, const std::function<int()> &eval, const char *who,
-                      double *cov, long long *launches) {
-  if (!s->Z) TRY(selinv_build(*s, st, who));
-  TRY(eval());
+// The column of every pose, on the host (once)
+static int col_of_build(SparseSolver &s, cudaStream_t st) {
+  if ((int)s.col_of.size() == s.P) return BALM_OK;
+  std::vector<int> perm(s.P);
+  CUDA_TRY(cudaMemcpyAsync(perm.data(), s.perm, sizeof(int) * s.P, cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  s.col_of.assign(s.P, 0);
+  for (int j = 0; j < s.P; j++) s.col_of[perm[j]] = j;
+  return BALM_OK;
+}
+
+int sparse_factor_undamped(SparseSolver *s, cudaStream_t st, int anchor, const char *who, long long *launches) {
+  TRY(col_of_build(*s, st));
   const SpView v = s->view();
   const int P = s->P, nlev = (int)s->lev_ptr.size() - 1, ac = anchor >= 0 ? s->col_of[anchor] : -1;
   // the undamped copy (u = 0 in scal[3]; the next solve writes its own), the anchor's blocks, the factorisation (its
@@ -767,6 +839,16 @@ int sparse_covariance(SparseSolver *s, cudaStream_t st, int anchor, const std::f
     balm_set_error(std::string(who) + ": H with the anchor's rows and columns deleted is singular");
     return BALM_ERR_NOT_PD;
   }
+  return BALM_OK;
+}
+
+int sparse_covariance(SparseSolver *s, cudaStream_t st, int anchor, const std::function<int()> &eval, const char *who,
+                      double *cov, long long *launches) {
+  if (!s->Z) TRY(selinv_build(*s, st, who));
+  TRY(eval());
+  TRY(sparse_factor_undamped(s, st, anchor, who, launches));
+  const SpView v = s->view();
+  const int nlev = (int)s->lev_ptr.size() - 1, ac = anchor >= 0 ? s->col_of[anchor] : -1;
   // Z top level first, then cov gathered into L's storage (no longer needed) and copied out
   for (int l = nlev - 1; l >= 0; l--)
     spg_selinv_kernel<<<s->lev_ptr[l + 1] - s->lev_ptr[l], SEL_THREADS, 0, st>>>(v, s->levcols + s->lev_ptr[l], s->sptr,
@@ -778,4 +860,27 @@ int sparse_covariance(SparseSolver *s, cudaStream_t st, int anchor, const std::f
   CUDA_TRY(cudaMemcpyAsync(cov, s->Lx, sizeof(double) * 36 * s->npairs, cudaMemcpyDeviceToHost, st));
   CUDA_TRY(cudaStreamSynchronize(st));
   return BALM_OK;
+}
+
+int sparse_solve_many(SparseSolver *s, cudaStream_t st, double *Y, int ld, int ncols, long long *launches) {
+  const SpView v = s->view();
+  const int nlev = (int)s->lev_ptr.size() - 1;
+  const unsigned tiles = (unsigned)((ncols + MANY_TILE - 1) / MANY_TILE);
+  if (ncols < 1) return BALM_OK;
+  for (int l = 0; l < nlev; l++)
+    spg_fwd_many_kernel<<<dim3(s->lev_ptr[l + 1] - s->lev_ptr[l], tiles), 6 * MANY_TILE, 0, st>>>(
+        v, s->levcols + s->lev_ptr[l], Y, ld, ncols);
+  for (int l = nlev - 1; l >= 0; l--)
+    spg_back_many_kernel<<<dim3(s->lev_ptr[l + 1] - s->lev_ptr[l], tiles), 6 * MANY_TILE, 0, st>>>(
+        v, s->levcols + s->lev_ptr[l], Y, ld, ncols);
+  CUDA_TRY(cudaGetLastError());
+  *launches += 2 * nlev;
+  return BALM_OK;
+}
+
+const std::vector<int> &sparse_solver_columns(SparseSolver *s) { return s->col_of; }
+int sparse_solver_size(const SparseSolver *s) { return s->P; }
+void sparse_solver_pose_pairs(const SparseSolver *s, const int **pp_ptr, const int2 **pp) {
+  *pp_ptr = s->pp_ptr;
+  *pp = s->pp;
 }

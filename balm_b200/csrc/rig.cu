@@ -111,6 +111,40 @@ __device__ __forceinline__ double ad_column_dot(const double *r, const double *p
   return c[0] * x[0] + c[1] * x[1] + c[2] * x[2] + pc[0] * x[3] + pc[1] * x[4] + pc[2] * x[5];
 }
 
+// W[6 s + r][c] = (J Y)[6 s + r][c] for every slot s (one thread per (slot, column)): Y's rows of s's free base plus
+// Ad(T_b) = [[R, 0], [p^ R, R]] times the rows of its free extrinsic (the transpose of ad_column_dot); a fixed unknown
+// adds nothing. Y [6F rows in the solver's column order col[u]][ld], W [6N][ld], row-major.
+__global__ void __launch_bounds__(128) rig_j_apply_kernel(const double *state, const int *base_of, const int *lidar_of,
+                                                          const int *var_of, int B, const int *col, const double *Y,
+                                                          int ld, int ncols, double *W) {
+  const int s = blockIdx.y, c = blockIdx.x * 128 + threadIdx.x;
+  if (c >= ncols) return;
+  const int vb = var_of[base_of[s]], vl = var_of[B + lidar_of[s]];
+  double w[6];
+#pragma unroll
+  for (int k = 0; k < 6; k++) w[k] = vb >= 0 ? Y[(6 * (size_t)col[vb] + k) * ld + c] : 0.0;
+  if (vl >= 0) {
+    double r[9], p[3], x[6];
+    load_pose(state + 12 * (size_t)base_of[s], r, p);
+#pragma unroll
+    for (int k = 0; k < 6; k++) x[k] = Y[(6 * (size_t)col[vl] + k) * ld + c];
+    double rp[3], rt[3], pc[3];
+#pragma unroll
+    for (int a = 0; a < 3; a++) {
+      rp[a] = r[3 * a] * x[0] + r[3 * a + 1] * x[1] + r[3 * a + 2] * x[2];
+      rt[a] = r[3 * a] * x[3] + r[3 * a + 1] * x[4] + r[3 * a + 2] * x[5];
+    }
+    cross3(p, rp, pc);
+#pragma unroll
+    for (int a = 0; a < 3; a++) {
+      w[a] += rp[a];
+      w[3 + a] += pc[a] + rt[a];
+    }
+  }
+#pragma unroll
+  for (int k = 0; k < 6; k++) W[(6 * (size_t)s + k) * ld + c] = w[k];
+}
+
 // K[:, 6u + k] = sum over the slots s of free unknown u, ascending, of H[:, 6s .. 6s+5] J_s (column block u).
 // One thread per row i of H; H is symmetric, so row i of column block s is read down the columns (coalesced in i).
 // The sums start at -0.0 so that a one-term sum is bitwise its term (a base with one slot copies H's columns).
@@ -592,6 +626,15 @@ int rig_reduce_raw(const Rig *r, cudaStream_t st, const double *state, const dou
 int rig_update(const Rig *r, cudaStream_t st, const double *state, double *state_out, long long *launches) {
   const int U = r->B + r->L;
   rig_update_kernel<<<(U + 127) / 128, 128, 0, st>>>(state, r->dx, r->var_of, U, state_out);
+  *launches += 1;
+  CUDA_TRY(cudaGetLastError());
+  return BALM_OK;
+}
+
+int rig_apply_j(const Rig *r, cudaStream_t st, const double *state, const int *col, const double *Y, int ld, int ncols,
+                double *W, long long *launches) {
+  rig_j_apply_kernel<<<dim3((ncols + 127) / 128, r->N), 128, 0, st>>>(state, r->base_of, r->lidar_of, r->var_of, r->B, col,
+                                                                      Y, ld, ncols, W);
   *launches += 1;
   CUDA_TRY(cudaGetLastError());
   return BALM_OK;

@@ -533,6 +533,27 @@ int balm_rig_block_structure(balm_ctx *ctx, int64_t stats[4], int32_t *pairs);
  * balm_rig_damping_iter is unaffected. */
 int balm_rig_block_covariance(balm_ctx *ctx, const double *base12, const double *ext12, int include_fix, int anchor,
                               double *cov);
+/* balm_rig_covariance's point-noise covariance on a balm_block_set_rig rig (DESIGN.md "Point-noise covariance on blocks
+ * contexts"), restricted to the n_sel distinct free unknowns sel (free indices in balm_set_rig's order, in [0, n_rig / 6)):
+ *   Sigma_sel = W^T R W,   W = J Y,   Y = H~_rig^-1 E,
+ * E the unit columns of the selection, H~_rig balm_rig_block_covariance's undamped H_rig without the anchor's rows and
+ * columns, J the rig's first-order Jacobian and R balm_block_point_covariance's raw term at the composed scan poses
+ * (c_cov81, point_noise and include_fix as in balm_pose_covariance). This is balm_rig_covariance's cov restricted to the
+ * selection; nothing of size n_rig^2 or (6N)^2 is formed. cov: (6 n_sel)^2 doubles, column-major, exactly symmetric, in
+ * sel's order, or NULL; marg: n_sel x 36 doubles (unknown u's 6x6 block, column-major), bitwise the diagonal blocks of
+ * cov, or NULL (not both). anchor: as balm_rig_block_covariance; its entries are exactly 0. BALM_ERR_INVALID, nothing
+ * written, on any other kind of ctx, without a balm_block_set_rig rig or registered voxels, with a communicator attached,
+ * for a NULL state, a bad anchor, n_sel < 1 or a sel entry repeated or out of range. BALM_ERR_NOT_PD, nothing written,
+ * under balm_block_covariance's pivot test. BALM_ERR_UNSUPPORTED, nothing written, when cov's buffers exceed the budget
+ * below. The rig, the ctx and the next balm_rig_damping_iter are as without the call. Device memory, freed by the call,
+ * in doubles: balm_block_point_covariance's raw-term scratch, and with F free unknowns, C right-hand sides per chunk
+ * (6 n_sel for cov; marg alone: as many whole unknowns as fit) and S = ceil(6N / 384):
+ *   C (6F + 12N) (Y, W, Z) + 36 S pairs (partial sums; pairs = n_sel (n_sel + 1) / 2 with cov, else C / 6)
+ *   + 36 n_sel^2 with cov, else 36 n_sel (outputs), plus 4 (F + n_sel) bytes.
+ * BALM_COV_BUDGET_MB (default 4096) bounds the first two terms and the outputs. */
+int balm_rig_block_point_covariance(balm_ctx *ctx, const double *base12, const double *ext12, const double *c_cov81,
+                                    double point_noise, int include_fix, int anchor, int n_sel, const int32_t *sel,
+                                    double *cov, double *marg);
 
 /* Sparse pose graph (DESIGN.md "Pose graph", "Sparse solve"): the same factors, cost and LM as balm_set_pose_factors /
  * balm_pose_graph_iter, with H held as its nonzero 6x6 blocks and the damped system solved by a block LDL^T in a
@@ -601,6 +622,31 @@ int balm_download_blocks(balm_ctx *ctx, double *blocks);
  * registration. Tables, errors and side effects as balm_spg_covariance's: afterwards balm_download_blocks returns H at
  * poses12, and the next balm_damping_iter is bitwise what it would have been without this call. */
 int balm_block_covariance(balm_ctx *ctx, const double *poses12, int include_fix, int anchor, double *cov);
+/* Point noise propagated to selected poses of a BALM_PREC_BLOCKS context (DESIGN.md "Point-noise covariance on blocks
+ * contexts"): balm_pose_covariance's Rcov restricted to the n_sel distinct poses sel (in [0, N)), without any 6N x 6N
+ * matrix:
+ *   Sigma_sel = Y^T R Y,   Y = H~^-1 E,
+ * E the unit columns of the selection, H~ balm_block_covariance's undamped H at poses12 (include_fix as there) with the
+ * anchor's rows and columns replaced by I, and R balm_pose_covariance's Rcov_raw (c_cov81, point_noise, include_fix as
+ * there). R couples exactly the poses that share a voxel, so it lives on the block pattern: raw_blocks (NULL or
+ * 36 doubles per pair in balm_block_structure's order, rows of pose i, column-major) receives it; pairs that only a pose
+ * factor or a prior gives are 0. Pose factors and priors shape H only: their information matrices are cost weights, not a
+ * noise model, so they add nothing to R. cov: (6 n_sel)^2 doubles, column-major, exactly symmetric, in sel's order;
+ * marg: n_sel x 36 doubles (pose sel[u]'s block, column-major), bitwise the diagonal blocks of cov. anchor: -1 or a
+ * pose, as balm_block_covariance; its entries are exactly 0. Any of the three outputs may be NULL, not all; with cov and
+ * marg NULL nothing is factored and sel is not read. With cov NULL the marginals go in chunks that fit the budget, so
+ * every pose of a long drive can be asked for in one call. Errors, each writing nothing: BALM_ERR_INVALID on any other
+ * kind of ctx, before a registration or without voxels, with a communicator attached, for a NULL poses12, a bad anchor,
+ * n_sel < 1 or a sel entry repeated or out of range (when cov or marg is asked for); BALM_ERR_NOT_PD under
+ * balm_block_covariance's pivot test; BALM_ERR_UNSUPPORTED when cov's buffers exceed the budget. The ctx and the next
+ * balm_damping_iter are as without the call (balm_download_blocks then returns H at poses12, as after
+ * balm_block_covariance). Device memory, freed by the call, in doubles: the raw term's 36 pairs + 21 K + 21 N + 10 M
+ * + 48 x (observations of its largest voxel batch; batches are cut to fit the budget) + 81 K with c_cov81, and for Sigma
+ * balm_rig_block_point_covariance's terms with F = N. BALM_COV_BUDGET_MB (default 4096) bounds the batches and Sigma's
+ * buffers. */
+int balm_block_point_covariance(balm_ctx *ctx, const double *poses12, const double *c_cov81, double point_noise,
+                                int include_fix, int anchor, int n_sel, const int32_t *sel, double *raw_blocks,
+                                double *cov, double *marg);
 /* Pose factors in the cost of a BALM_PREC_BLOCKS context (DESIGN.md "Voxels and pose factors in one cost"): odometry
  * between consecutive scans, loop closures, HBA window factors. Arguments, checks, error messages, per-factor status
  * (BALM_ERR_NOT_PD factors are left out of the pattern and every sum) and factor cost are balm_set_pose_factors'; H_f must
