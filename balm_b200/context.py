@@ -123,12 +123,40 @@ def _pose_graph_iter(fn, handle, N, poses12, max_iter, u0, v0, rel_tol, gauge_mo
     return poses, tr
 
 
-def _covariance(fn, handle, poses12, n_pairs, *args):
-    """balm_spg_covariance / balm_block_covariance -> [n_pairs, 6, 6] blocks (rows of pose i, columns of pose j)."""
-    poses12 = np.ascontiguousarray(poses12, dtype=np.float64)
+def _block_structure(fn, handle, want_pairs):
+    """balm_block_structure / balm_rig_block_structure / balm_spg_structure -> dict(pairs, l_blocks, levels,
+    device_bytes), with want_pairs also "pair_list", the (pairs, 2) int32 array of (i, j), i <= j, ascending."""
+    st = np.zeros(4, dtype=np.int64)
+    L.check(fn(handle, _p(st), None))
+    out = dict(pairs=int(st[0]), l_blocks=int(st[1]), levels=int(st[2]), device_bytes=int(st[3]))
+    if want_pairs:
+        pr = np.zeros((out["pairs"], 2), dtype=np.int32)
+        L.check(fn(handle, _p(st), _p(pr)))
+        out["pair_list"] = pr
+    return out
+
+
+def _covariance(fn, handle, state, n_pairs, *args):
+    """balm_spg_covariance / balm_block_covariance / balm_rig_block_covariance at state (poses12, or base12 and ext12)
+    -> [n_pairs, 6, 6] blocks (rows of unknown i, columns of unknown j)."""
+    state = [np.ascontiguousarray(x, dtype=np.float64) for x in state]
     cov = np.zeros((n_pairs, 36))
-    L.check(fn(handle, _p(poses12), *args, _p(cov)))
+    L.check(fn(handle, *map(_p, state), *args, _p(cov)))
     return cov.reshape(-1, 6, 6).transpose(0, 2, 1)
+
+
+def _block_point_covariance(fn, handle, state, sel, point_noise, c_cov, include_fix, anchor, joint, *raw):
+    """balm_block_point_covariance / balm_rig_block_point_covariance at state (poses12, or base12 and ext12); raw: the
+    plain call's raw_blocks pointer -> the joint (6 s x 6 s) Sigma in sel's order, or the (s, 6, 6) marginals."""
+    state = [np.ascontiguousarray(x, dtype=np.float64) for x in state]
+    sel = np.ascontiguousarray(sel, dtype=np.int32).reshape(-1)
+    cc = None if c_cov is None else np.ascontiguousarray(c_cov, dtype=np.float64).reshape(-1, 81)
+    s = len(sel)
+    cov = np.zeros((6 * s, 6 * s), order="F") if joint else None
+    marg = None if joint else np.zeros((s, 36))
+    L.check(fn(handle, *map(_p, state), _p(cc), float(point_noise), int(include_fix), int(anchor), s, _p(sel), *raw,
+               _p(cov), _p(marg)))
+    return cov if joint else marg.reshape(s, 6, 6).transpose(0, 2, 1).copy()
 
 
 class Context:
@@ -242,14 +270,7 @@ class Context:
         """PREC_BLOCKS contexts: -> dict(pairs, l_blocks, levels, device_bytes): block pairs (i <= j) of H, blocks of the
         factor L, levels of its elimination tree and the device memory the context holds; with want_pairs also
         "pair_list", the (pairs, 2) int32 array of (i, j), ascending."""
-        st = np.zeros(4, dtype=np.int64)
-        L.check(L.lib().balm_block_structure(self._h, _p(st), None))
-        out = dict(pairs=int(st[0]), l_blocks=int(st[1]), levels=int(st[2]), device_bytes=int(st[3]))
-        if want_pairs:
-            pr = np.zeros((out["pairs"], 2), dtype=np.int32)
-            L.check(L.lib().balm_block_structure(self._h, _p(st), _p(pr)))
-            out["pair_list"] = pr
-        return out
+        return _block_structure(L.lib().balm_block_structure, self._h, want_pairs)
 
     def download_blocks(self):
         """PREC_BLOCKS contexts: the last evaluation's blocks, (pairs, 6, 6) with [p, a, c] = H[6 i + a, 6 j + c] of
@@ -264,7 +285,7 @@ class Context:
         evaluate(poses12, include_fix=include_fix) returns it (anchor=-1: nothing deleted; fix clusters must then fix the
         gauge). -> (pairs [n_pairs, 2] (i <= j), cov [n_pairs, 6, 6]) with cov[p, a, c] = Sigma[6 i + a, 6 j + c]."""
         pairs = self.block_structure(want_pairs=True)["pair_list"]
-        return pairs, _covariance(L.lib().balm_block_covariance, self._h, poses12, len(pairs), int(include_fix),
+        return pairs, _covariance(L.lib().balm_block_covariance, self._h, (poses12,), len(pairs), int(include_fix),
                                   int(anchor))
 
     def block_point_covariance(self, poses12, sel, point_noise=0.0, c_cov=None, include_fix=False, anchor=0, joint=True,
@@ -274,17 +295,10 @@ class Context:
         -1 or a pose, deleted; its entries 0), R the raw term. -> the joint (6 s x 6 s) Sigma in sel's order, or with
         joint=False the (s, 6, 6) marginals (all poses of a long drive fit one call); with want_raw also (pairs [n_pairs, 2],
         raw [n_pairs, 6, 6]) with raw[p, a, c] = R[6 i + a, 6 j + c]. c_cov: K x 9 x 9 or None (isotropic point_noise)."""
-        poses12 = np.ascontiguousarray(poses12, dtype=np.float64)
-        sel = np.ascontiguousarray(sel, dtype=np.int32).reshape(-1)
-        cc = None if c_cov is None else np.ascontiguousarray(c_cov, dtype=np.float64).reshape(-1, 81)
-        s = len(sel)
-        cov = np.zeros((6 * s, 6 * s), order="F") if joint else None
-        marg = None if joint else np.zeros((s, 36))
         pairs = self.block_structure(want_pairs=True)["pair_list"] if want_raw else None
         raw = np.zeros((len(pairs), 36)) if want_raw else None
-        L.check(L.lib().balm_block_point_covariance(self._h, _p(poses12), _p(cc), float(point_noise), int(include_fix),
-                                                    int(anchor), s, _p(sel), _p(raw), _p(cov), _p(marg)))
-        out = cov if joint else marg.reshape(s, 6, 6).transpose(0, 2, 1).copy()
+        out = _block_point_covariance(L.lib().balm_block_point_covariance, self._h, (poses12,), sel, point_noise, c_cov,
+                                      include_fix, anchor, joint, _p(raw))
         if want_raw:
             return out, (pairs, raw.reshape(-1, 6, 6).transpose(0, 2, 1).copy())
         return out
@@ -387,14 +401,7 @@ class Context:
     def rig_block_structure(self, want_pairs=False):
         """set_block_rig's rig: -> dict(pairs, l_blocks, levels, device_bytes) as block_structure, over the rig's free
         unknowns (set_rig's order); with want_pairs also "pair_list", the (pairs, 2) int32 array of (u, v), u <= v."""
-        st = np.zeros(4, dtype=np.int64)
-        L.check(L.lib().balm_rig_block_structure(self._h, _p(st), None))
-        out = dict(pairs=int(st[0]), l_blocks=int(st[1]), levels=int(st[2]), device_bytes=int(st[3]))
-        if want_pairs:
-            pr = np.zeros((out["pairs"], 2), dtype=np.int32)
-            L.check(L.lib().balm_rig_block_structure(self._h, _p(st), _p(pr)))
-            out["pair_list"] = pr
-        return out
+        return _block_structure(L.lib().balm_rig_block_structure, self._h, want_pairs)
 
     def rig_block_covariance(self, base12, ext12, include_fix=False, anchor=-1):
         """set_block_rig's rig: Sigma = (H_rig without free base anchor's rows and columns)^-1 on the rig's block
@@ -402,10 +409,8 @@ class Context:
         cov [n_pairs, 6, 6]) with cov[p, a, c] = Sigma[6 u + a, 6 v + c]."""
         base12, ext12, _ = self._rig_shapes(base12, ext12)
         pairs = self.rig_block_structure(want_pairs=True)["pair_list"]
-        cov = np.zeros((len(pairs), 36))
-        L.check(L.lib().balm_rig_block_covariance(self._h, _p(base12), _p(ext12), int(include_fix), int(anchor),
-                                                  _p(cov)))
-        return pairs, cov.reshape(-1, 6, 6).transpose(0, 2, 1)
+        return pairs, _covariance(L.lib().balm_rig_block_covariance, self._h, (base12, ext12), len(pairs),
+                                  int(include_fix), int(anchor))
 
     def rig_block_point_covariance(self, base12, ext12, sel, point_noise=0.0, c_cov=None, include_fix=False, anchor=-1,
                                    joint=True):
@@ -414,14 +419,8 @@ class Context:
         rig_block_covariance. -> the joint (6 s x 6 s) Sigma in sel's order, or with joint=False the (s, 6, 6) marginals.
         balm_b200.rig.extrinsic_sigmas(cov, 0) reads it when sel lists the free extrinsics."""
         base12, ext12, _ = self._rig_shapes(base12, ext12)
-        sel = np.ascontiguousarray(sel, dtype=np.int32).reshape(-1)
-        cc = None if c_cov is None else np.ascontiguousarray(c_cov, dtype=np.float64).reshape(-1, 81)
-        s = len(sel)
-        cov = np.zeros((6 * s, 6 * s), order="F") if joint else None
-        marg = None if joint else np.zeros((s, 36))
-        L.check(L.lib().balm_rig_block_point_covariance(self._h, _p(base12), _p(ext12), _p(cc), float(point_noise),
-                                                        int(include_fix), int(anchor), s, _p(sel), _p(cov), _p(marg)))
-        return cov if joint else marg.reshape(s, 6, 6).transpose(0, 2, 1).copy()
+        return _block_point_covariance(L.lib().balm_rig_block_point_covariance, self._h, (base12, ext12), sel,
+                                       point_noise, c_cov, include_fix, anchor, joint)
 
     def _rig_shapes(self, base12, ext12):
         if getattr(self, "_rig", None) is None:
@@ -943,17 +942,12 @@ class PoseGraph:
     def structure(self):
         """-> dict(pairs, l_blocks, levels, device_bytes): nonzero block pairs of H, blocks of the factor L, levels of
         its elimination tree and the device memory the handle holds."""
-        st = np.zeros(4, dtype=np.int64)
-        L.check(L.lib().balm_spg_structure(self._h, _p(st), None))
-        return dict(pairs=int(st[0]), l_blocks=int(st[1]), levels=int(st[2]), device_bytes=int(st[3]))
+        return _block_structure(L.lib().balm_spg_structure, self._h, False)
 
     def pose_graph_evaluate(self, poses12):
         """-> (pairs [n_pairs, 2] (i <= j), blocks [n_pairs, 6, 6] (H rows of pose i, columns of pose j), g, cost)."""
         poses12 = np.ascontiguousarray(poses12, dtype=np.float64)
-        st = np.zeros(4, dtype=np.int64)
-        L.check(L.lib().balm_spg_structure(self._h, _p(st), None))
-        pairs = np.zeros((int(st[0]), 2), dtype=np.int32)
-        L.check(L.lib().balm_spg_structure(self._h, _p(st), _p(pairs)))
+        pairs = _block_structure(L.lib().balm_spg_structure, self._h, True)["pair_list"]
         blocks = np.zeros((len(pairs), 36))
         g = np.zeros(self.n)
         r = C.c_double()
@@ -964,11 +958,8 @@ class PoseGraph:
         """Marginal covariances: Sigma = (H without pose anchor's rows and columns)^-1 on H's block pattern, H the
         Gauss-Newton Hessian at poses12 (anchor=-1: nothing deleted, which leaves the gauge free: ERR_NOT_PD).
         -> (pairs [n_pairs, 2] (i <= j), cov [n_pairs, 6, 6]) with cov[p, a, c] = Sigma[6 i + a, 6 j + c]."""
-        st = np.zeros(4, dtype=np.int64)
-        L.check(L.lib().balm_spg_structure(self._h, _p(st), None))
-        pairs = np.zeros((int(st[0]), 2), dtype=np.int32)
-        L.check(L.lib().balm_spg_structure(self._h, _p(st), _p(pairs)))
-        return pairs, _covariance(L.lib().balm_spg_covariance, self._h, poses12, len(pairs), int(anchor))
+        pairs = _block_structure(L.lib().balm_spg_structure, self._h, True)["pair_list"]
+        return pairs, _covariance(L.lib().balm_spg_covariance, self._h, (poses12,), len(pairs), int(anchor))
 
     def pose_graph_iter(self, poses12, max_iter=10, u0=0.01, v0=2.0, rel_tol=1e-6, gauge_mode=0, verbose=False,
                         want_per_iter=False, force_hess=False):

@@ -712,13 +712,110 @@ static int residual_dev(balm_ctx *c, const double *poses, double *host_out, bool
   return BALM_OK;
 }
 
-// A blocks context's H as the dense column-major n x n matrix of its blocks (zeros elsewhere), on the host (waits).
-static int blocks_to_dense(balm_ctx *c, double *H) {
-  const std::vector<int2> &pr = blocks_pairs(c->bh);
+// ---------------- the unknowns of a call ----------------
+// What an evaluation, LM loop or covariance solves for: the context's N slot poses (rig null), or a rig's free base
+// poses and extrinsics, composed to slot poses before every evaluation, with H and g reduced to H_rig and g_rig after
+// it. Everything else (the dense or sparse solve, the LM rule, the undamped factor, the covariance algebra) is the same
+// for both, so these functions are the only code that tells them apart.
+struct Unknowns {
+  balm_ctx *c;
+  Rig *rig;
+
+  bool sparse() const { return rig ? rig_sparse(rig) : c->prec == BALM_PREC_BLOCKS; }
+  DenseSystem system() const { return rig ? rig_system(rig) : ctx_system(c); }
+  // the sparse solver of a blocks context or a block-sparse rig, else null (the dense solve of system())
+  SparseSolver *solver() const {
+    if (!sparse()) return nullptr;
+    return rig ? rig_solver(rig) : blocks_solver(c->bh);
+  }
+  // a sparse one's block pairs and their device blocks
+  const std::vector<int2> &pairs() const { return rig ? rig_pairs(rig) : blocks_pairs(c->bh); }
+  const double *blocks() const { return rig ? rig_blocks(rig) : blocks_device(c->bh); }
+  // the current state: the slot poses, or the base poses then the extrinsics; 12 doubles per pose
+  double *state() const { return rig ? rig_state(rig, false) : c->poses; }
+  int n_state() const { return rig ? rig_bases(rig) + rig_lidars(rig) : c->N; }
+  // a covariance's anchor: -1, or a pose, or a free base pose (`who` prefixes the message)
+  int check_anchor(const char *who, int anchor) const {
+    if (anchor >= -1 && anchor < (rig ? rig_free_bases(rig) : c->N)) return BALM_OK;
+    if (rig)
+      balm_set_error(std::string(who) + ": anchor " + std::to_string(anchor) + " is neither -1 nor a free base index in [0, " +
+                     std::to_string(rig_free_bases(rig)) + ")");
+    else
+      balm_set_error(std::string(who) + ": anchor outside [-1, N)");
+    return BALM_ERR_INVALID;
+  }
+
+  // x12 (the slot poses, or a rig's base poses) and ext12 (a rig's extrinsics) in or out of the current state
+  int upload(const double *x12, const double *ext12) const {
+    const size_t nx = 12 * (size_t)(rig ? rig_bases(rig) : c->N);
+    CUDA_TRY(cudaMemcpyAsync(state(), x12, sizeof(double) * nx, cudaMemcpyHostToDevice, c->stream));
+    if (rig)
+      CUDA_TRY(cudaMemcpyAsync(state() + nx, ext12, sizeof(double) * 12 * rig_lidars(rig), cudaMemcpyHostToDevice, c->stream));
+    return BALM_OK;
+  }
+  int download(double *x12, double *ext12) const {
+    const size_t nx = 12 * (size_t)(rig ? rig_bases(rig) : c->N);
+    CUDA_TRY(cudaMemcpyAsync(x12, state(), sizeof(double) * nx, cudaMemcpyDeviceToHost, c->stream));
+    if (rig)
+      CUDA_TRY(cudaMemcpyAsync(ext12, state() + nx, sizeof(double) * 12 * rig_lidars(rig), cudaMemcpyDeviceToHost, c->stream));
+    return BALM_OK;
+  }
+  // the slot poses of the current state in c->poses
+  int compose() const { return rig ? rig_compose(rig, c->stream, state(), c->poses, &c->launches) : BALM_OK; }
+  // evaluate_dev at the current state: H, g and the residual in c->scal[0], then a rig's H_rig and g_rig (the
+  // reduction timed by ev[13] and ev[14]); with a blocks context, its slot blocks, factors and priors first
+  int eval(bool include_fix, int64_t head, int64_t end, bool stats_cached = false) const {
+    TRY(compose());
+    TRY(evaluate_dev(c, c->poses, head, end, include_fix, stats_cached));
+    if (!rig) return BALM_OK;
+    CUDA_TRY(cudaEventRecord(c->ev[13], c->stream));
+    if (rig_sparse(rig)) TRY(rig_reduce_blocks(rig, c->stream, state(), blocks_device(c->bh), c->g, &c->launches));
+    else TRY(rig_reduce(rig, c->stream, state(), c->H, c->g, &c->launches));
+    CUDA_TRY(cudaEventRecord(c->ev[14], c->stream));
+    return BALM_OK;
+  }
+  // after an eval, once the stream has been waited for: its accounting (collect_eval), a rig's reduction in ms_assemble
+  int collect() const {
+    TRY(collect_eval(c));
+    if (rig) {
+      float ms;
+      CUDA_TRY(cudaEventElapsedTime(&ms, c->ev[13], c->ev[14]));
+      c->tm.ms_assemble += ms;
+    }
+    return BALM_OK;
+  }
+  // the raw term R (6N x 6N, at the slot poses) in these unknowns: R itself, or a rig's J^T R J (taken from pool)
+  int reduce_raw(ScratchPool &pool, double **R) const {
+    if (!rig) return BALM_OK;
+    double *out = nullptr;
+    TRY(pool.get(&out, (size_t)rig_n(rig) * rig_n(rig)));
+    TRY(rig_reduce_raw(rig, c->stream, state(), *R, out, &c->launches));
+    *R = out;
+    return BALM_OK;
+  }
+  // the LM trial state from system()'s dx, its slot poses in c->poses_trial; accept() makes it the current state
+  int trial() const {
+    if (!rig) return launch_pose_update(c, c->poses, c->dx, c->poses_trial);
+    TRY(rig_update(rig, c->stream, state(), rig_state(rig, true), &c->launches));
+    return rig_compose(rig, c->stream, rig_state(rig, true), c->poses_trial, &c->launches);
+  }
+  void accept() const {
+    if (rig) rig_swap_states(rig);
+    else std::swap(c->poses, c->poses_trial);
+  }
+  // gauge modes 0 and 1: the poses re-anchored to pose 0, or a rig's base poses to base 0 (extrinsics are body-frame)
+  int gauge(int mode) const {
+    c->launches += 1;
+    return launch_gauge(c->stream, rig ? rig_bases(rig) : c->N, state(), c->scal + 4, mode);  // pose 0 into scal[4..15]
+  }
+};
+
+// The n x n matrix of a block-sparse H (or H_rig), column-major, from its pairs and device blocks, zeros elsewhere, on
+// the host (waits).
+static int blocks_to_dense(balm_ctx *c, const std::vector<int2> &pr, const double *blocks, size_t n, double *H) {
   std::vector<double> b(36 * pr.size());
-  CUDA_TRY(cudaMemcpyAsync(b.data(), blocks_device(c->bh), sizeof(double) * b.size(), cudaMemcpyDeviceToHost, c->stream));
+  CUDA_TRY(cudaMemcpyAsync(b.data(), blocks, sizeof(double) * b.size(), cudaMemcpyDeviceToHost, c->stream));
   CUDA_TRY(cudaStreamSynchronize(c->stream));
-  const size_t n = c->n;
   std::fill(H, H + n * n, 0.0);
   for (size_t p = 0; p < pr.size(); p++)
     for (int col = 0; col < 6; col++)
@@ -731,20 +828,30 @@ static int blocks_to_dense(balm_ctx *c, double *H) {
   return BALM_OK;
 }
 
+// balm_evaluate and balm_rig_evaluate after their checks: H (dense, expanded from blocks), g and the residual of voxels
+// [head, end) at x12 / ext12
+static int evaluate(const Unknowns &u, const double *x12, const double *ext12, int64_t head, int64_t end,
+                    bool include_fix, double *H, double *g, double *residual) {
+  balm_ctx *c = u.c;
+  CUDA_TRY(cudaSetDevice(c->device));
+  TRY(u.upload(x12, ext12));
+  TRY(u.eval(include_fix, head, end));
+  const DenseSystem sys = u.system();
+  const size_t n = sys.n;
+  if (H && u.sparse()) TRY(blocks_to_dense(c, u.pairs(), u.blocks(), n, H));
+  else if (H) CUDA_TRY(cudaMemcpyAsync(H, sys.H, sizeof(double) * n * n, cudaMemcpyDeviceToHost, c->stream));
+  if (g) CUDA_TRY(cudaMemcpyAsync(g, sys.g, sizeof(double) * n, cudaMemcpyDeviceToHost, c->stream));
+  CUDA_TRY(cudaMemcpyAsync(c->h_scal, c->scal, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+  CUDA_TRY(cudaStreamSynchronize(c->stream));
+  TRY(u.collect());
+  if (residual) *residual = c->h_scal[0];
+  return BALM_OK;
+}
+
 extern "C" int balm_evaluate(balm_ctx *c, const double *poses12, int64_t head, int64_t end, int include_fix,
                              double *H, double *g, double *residual) {
   if (!c || !poses12) { balm_set_error("balm_evaluate: bad arguments"); return BALM_ERR_INVALID; }
-  CUDA_TRY(cudaSetDevice(c->device));
-  CUDA_TRY(cudaMemcpyAsync(c->poses, poses12, sizeof(double) * 12 * c->N, cudaMemcpyHostToDevice, c->stream));
-  TRY(evaluate_dev(c, c->poses, head, end, include_fix != 0));
-  const size_t n = c->n;
-  if (H && c->prec == BALM_PREC_BLOCKS) TRY(blocks_to_dense(c, H));
-  else if (H) CUDA_TRY(cudaMemcpyAsync(H, c->H, sizeof(double) * n * n, cudaMemcpyDeviceToHost, c->stream));
-  if (g) CUDA_TRY(cudaMemcpyAsync(g, c->g, sizeof(double) * n, cudaMemcpyDeviceToHost, c->stream));
-  CUDA_TRY(cudaMemcpyAsync(c->h_scal, c->scal, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
-  CUDA_TRY(cudaStreamSynchronize(c->stream));
-  if (residual) *residual = c->h_scal[0];
-  return BALM_OK;
+  return evaluate(Unknowns{c, nullptr}, poses12, nullptr, head, end, include_fix != 0, H, g, residual);
 }
 
 extern "C" int balm_residual(balm_ctx *c, const double *poses12, double *residual) {
@@ -837,14 +944,11 @@ static int solve_dev(balm_ctx *c, const DenseSystem &sys, SparseSolver *sp, doub
   return BALM_OK;
 }
 
-// the context's own sparse solver: a blocks context's, else null (the dense solve of ctx_system)
-static SparseSolver *ctx_solver(balm_ctx *c) { return c->prec == BALM_PREC_BLOCKS ? blocks_solver(c->bh) : nullptr; }
-
 extern "C" int balm_solve(balm_ctx *c, double u, double *dx, double *q1, int *not_pd) {
   if (!c) { balm_set_error("balm_solve: bad arguments"); return BALM_ERR_INVALID; }
   CUDA_TRY(cudaSetDevice(c->device));
   const DenseSystem sys = ctx_system(c);
-  SparseSolver *sp = ctx_solver(c);
+  SparseSolver *sp = Unknowns{c, nullptr}.solver();
   double q = 0;
   int bad = 0, refined = 0;
   TRY(solve_dev(c, sys, sp, u));
@@ -870,7 +974,7 @@ static int refuse_gauge_with_priors(const char *who, const PriorSet *pr, const b
   return BALM_ERR_INVALID;
 }
 
-// One LM loop's steps, supplied by its owner (balm_damping_iter, balm_rig_damping_iter, balm_pose_graph_iter). Each
+// One LM loop's steps, supplied by its owner (damping_iter for the voxel and rig costs, balm_pose_graph_iter). Each
 // returns a BALM_* status.
 struct LmSteps {
   cudaStream_t st;
@@ -921,20 +1025,29 @@ static int lm_run(const LmSteps &s, const balm_lm_opts *o, balm_trace *trace, in
   return BALM_OK;
 }
 
-// Clears the context's LM flags (set by balm_damping_iter and balm_rig_damping_iter) on every exit path
+// Clears the context's LM flags (set by damping_iter) on every exit path
 struct LmScope {
   balm_ctx *c;
   ~LmScope() { c->lm_active = false; c->defer = false; c->pending_eval = false; c->eval_same_poses = false; }
 };
 
-extern "C" int balm_damping_iter(balm_ctx *c, double *poses12, const balm_lm_opts *o, balm_trace *trace, int *n_iters,
-                                 double *poses_per_iter) {
-  if (!c || !poses12 || !o) { balm_set_error("balm_damping_iter: bad arguments"); return BALM_ERR_INVALID; }
-  CUDA_TRY(cudaSetDevice(c->device));
-  if (n_iters) *n_iters = 0;
-  if (!c->registered) { balm_set_error("no voxels registered"); return BALM_ERR_INVALID; }
-  if (c->prec == BALM_PREC_BLOCKS) TRY(refuse_gauge_with_priors("balm_damping_iter", c->pr, o));
-  if (o->min_planes_per_pose > 0) {  // bavoxel.hpp:1071-1085 (the shim reproduces the printf + exit(0))
+// balm_damping_iter and balm_rig_damping_iter after their checks (`who` prefixes the messages): LM from x12 / ext12,
+// the result written back to them, the state after every iteration to per_iter
+static int damping_iter(const Unknowns &u, const char *who, double *x12, double *ext12, const balm_lm_opts *o,
+                        balm_trace *trace, int *n_iters, double *per_iter) {
+  balm_ctx *c = u.c;
+  // A rig's evaluations stay the pure function balm_rig_evaluate is: no per-voxel stats handed over from the trial
+  // residual pass and no tensor scale speculation (lm_active and eval_same_poses stay false).
+  const bool carry_over = !u.rig;
+  // Re-anchoring a rig to base pose 0 would move the result off its fixed base poses.
+  const bool bases_fixed = u.rig && rig_any_base_fixed(u.rig);
+  if ((o->gauge_mode == 0 || o->gauge_mode == 1) && bases_fixed) {
+    balm_set_error(std::string(who) + ": gauge_mode " + std::to_string(o->gauge_mode) +
+                   " re-anchors to base pose 0, which moves the result off the fixed base poses; pass gauge_mode 2");
+    return BALM_ERR_INVALID;
+  }
+  if (c->prec == BALM_PREC_BLOCKS) TRY(refuse_gauge_with_priors(who, c->pr, o));
+  if (o->min_planes_per_pose > 0) {  // bavoxel.hpp:1071-1085 (the shim reproduces the printf + exit(0)); per scan slot
     // The guard is on the GLOBAL count of voxels seeing each pose. With several ranks every rank all-reduces the
     // per-pose histogram of its shard first, so all ranks take the same branch (a rank returning alone would leave
     // the others waiting in the next collective).
@@ -953,63 +1066,76 @@ extern "C" int balm_damping_iter(balm_ctx *c, double *poses12, const balm_lm_opt
       return BALM_ERR_TOO_FEW_PLANES;
     }
   }
-  const size_t pbytes = sizeof(double) * 12 * c->N;
-  CUDA_TRY(cudaMemcpyAsync(c->poses, poses12, pbytes, cudaMemcpyHostToDevice, c->stream));
+  TRY(u.upload(x12, ext12));
   // The residual pass at the trial poses computes the same per-voxel eigen data the next evaluation starts with:
   // when the step is accepted they are handed over (same kernel, same inputs -> identical values). Needs the whole
   // problem in one batch and the same treatment of the fix cluster in both passes.
-  const bool hand_over = c->stats_trial != nullptr && (c->fix == nullptr || o->hess_includes_fix != 0);
+  const bool hand_over = carry_over && c->stats_trial != nullptr && (c->fix == nullptr || o->hess_includes_fix != 0);
   bool stats_cached = false;
   bool same_poses = false;  // the last step was rejected: c->poses are those of the previous evaluation
-  tensor_syrk_new_problem(c);  // nothing speculative is carried over from earlier calls
+  bool evaluated = false;   // this iteration evaluated: its events are to be read
+  if (carry_over) tensor_syrk_new_problem(c);  // nothing speculative is carried over from earlier calls
   LmScope lm_scope{c};
-  c->lm_active = true;
+  c->lm_active = carry_over;
   // the evaluation's events and flags are read after the iteration's wait; BALM_SYNC_PHASES waits after every phase
   c->defer = !getenv("BALM_SYNC_PHASES");
-  const DenseSystem sys = ctx_system(c);
-  SparseSolver *sp = ctx_solver(c);
+  const DenseSystem sys = u.system();
+  SparseSolver *sp = u.solver();
+  const int ns = u.n_state();
   LmSteps s{c->stream, c->scal, c->h_scal};
   s.eval = [&]() -> int {
-    c->eval_same_poses = same_poses;
-    const int rc = evaluate_dev(c, c->poses, 0, c->M, o->hess_includes_fix != 0, stats_cached);
+    evaluated = true;
+    c->eval_same_poses = carry_over && same_poses;
+    const int rc = u.eval(o->hess_includes_fix != 0, 0, c->M, stats_cached);
     c->eval_same_poses = false;
     return rc;
   };
-  s.solve = [&](double u) -> int {
-    TRY(solve_dev(c, sys, sp, u));
+  s.solve = [&](double uu) -> int {
+    TRY(solve_dev(c, sys, sp, uu));
     if (!c->defer) CUDA_TRY(cudaStreamSynchronize(c->stream));
     return BALM_OK;
   };
-  s.trial = [c]() { return launch_pose_update(c, c->poses, c->dx, c->poses_trial); };
+  s.trial = [&u]() { return u.trial(); };
   s.trial_cost = [&](double *r2) { return residual_dev(c, c->poses_trial, r2, hand_over); };
   s.finish = [&](double *q1, int *not_pd, int *refined) -> int {
-    TRY(collect_eval(c));
+    if (evaluated) TRY(u.collect());
+    evaluated = false;
     return collect_solve(c, sys, sp, q1, not_pd, refined);
   };
   s.step = [&](bool accepted) -> int {
     if (accepted) {
-      std::swap(c->poses, c->poses_trial);
+      u.accept();
       if (hand_over) {
         std::swap(c->stats, c->stats_trial);
         CUDA_TRY(cudaMemcpyAsync(c->scal + BALM_SCAL_RCUR, c->scal + BALM_SCAL_RTRIAL, sizeof(double), cudaMemcpyDeviceToDevice, c->stream));
       }
       stats_cached = hand_over;
     } else {
-      stats_cached = c->stats_trial != nullptr;  // c->stats still describes c->poses (single batch)
+      stats_cached = carry_over && c->stats_trial != nullptr;  // c->stats still describes c->poses (single batch)
     }
     same_poses = !accepted;
     return BALM_OK;
   };
   s.snapshot = [&](int it) -> int {
-    if (poses_per_iter)
-      CUDA_TRY(cudaMemcpyAsync(poses_per_iter + (size_t)it * 12 * c->N, c->poses, pbytes, cudaMemcpyDeviceToHost, c->stream));
+    if (per_iter)
+      CUDA_TRY(cudaMemcpyAsync(per_iter + (size_t)it * 12 * ns, u.state(), sizeof(double) * 12 * ns,
+                               cudaMemcpyDeviceToHost, c->stream));
     return BALM_OK;
   };
   TRY(lm_run(s, o, trace, n_iters));
-  if (o->gauge_mode == 0 || o->gauge_mode == 1) TRY(launch_gauge(c, c->poses, o->gauge_mode));
-  CUDA_TRY(cudaMemcpyAsync(poses12, c->poses, pbytes, cudaMemcpyDeviceToHost, c->stream));
+  if (o->gauge_mode == 0 || o->gauge_mode == 1) TRY(u.gauge(o->gauge_mode));
+  TRY(u.download(x12, ext12));
   CUDA_TRY(cudaStreamSynchronize(c->stream));
   return BALM_OK;
+}
+
+extern "C" int balm_damping_iter(balm_ctx *c, double *poses12, const balm_lm_opts *o, balm_trace *trace, int *n_iters,
+                                 double *poses_per_iter) {
+  if (!c || !poses12 || !o) { balm_set_error("balm_damping_iter: bad arguments"); return BALM_ERR_INVALID; }
+  CUDA_TRY(cudaSetDevice(c->device));
+  if (n_iters) *n_iters = 0;
+  if (!c->registered) { balm_set_error("no voxels registered"); return BALM_ERR_INVALID; }
+  return damping_iter(Unknowns{c, nullptr}, "balm_damping_iter", poses12, nullptr, o, trace, n_iters, poses_per_iter);
 }
 
 // ---------------- pose graph (pose_graph.cu, pose_graph_sparse.cu) ----------------
@@ -1185,6 +1311,100 @@ extern "C" int balm_pose_graph_iter(balm_ctx *c, double *poses12, const balm_lm_
   return BALM_OK;
 }
 
+// ---------------- covariances at a state (covariance.cu, pose_graph_sparse.cu) ----------------
+// The undamped factorisation of H (or H_rig) at the unknowns' current state: `factor` runs `eval`, the evaluation
+// deferred, then a factorisation that waits for the stream; the evaluation's events are read after that wait.
+using FactorStep = std::function<int(const std::function<int()> &eval)>;
+static int factor_at_state(const Unknowns &u, bool include_fix, const FactorStep &factor) {
+  balm_ctx *c = u.c;
+  const int rc = factor([&]() -> int {
+    c->defer = true;
+    const int e = u.eval(include_fix, 0, c->M);
+    c->defer = false;
+    return e;
+  });
+  if (rc == BALM_OK || rc == BALM_ERR_NOT_PD) TRY(u.collect());  // the stream has been synchronised
+  c->pending_eval = false;
+  return rc;
+}
+
+// balm_pose_covariance and balm_rig_covariance after their checks: raw = the raw term R (cov_raw_dev) at the slot
+// poses of x12 / ext12 in the unknowns (J^T R J for a rig), cov = H~^-1 raw H~^-T with H (or H_rig) at the same state
+// factored undamped. The anchor's rows and columns (none for -1) are deleted from both, with 1 on H~'s diagonal. Waits
+// for the pivot test and at the end.
+static int covariance(const Unknowns &u, const double *x12, const double *ext12, const double *c_cov81,
+                      double point_noise, bool include_fix, int anchor, const char *singular_msg, double *raw,
+                      double *cov) {
+  balm_ctx *c = u.c;
+  const DenseSystem sys = u.system();
+  const int n = sys.n, a0 = anchor < 0 ? -1 : 6 * anchor;
+  CUDA_TRY(cudaSetDevice(c->device));
+  TRY(u.upload(x12, ext12));
+  TRY(u.compose());
+  ScratchPool pool;
+  double *R = nullptr;
+  TRY(cov_raw_dev(c, pool, c->poses, c_cov81, point_noise, include_fix, &R));
+  TRY(u.reduce_raw(pool, &R));
+  if (a0 >= 0) TRY(cov_delete_block(c, R, n, a0, 0.0));
+  if (cov)  // H at these poses (divide_thread, BAs_left.hpp:1091)
+    TRY(factor_at_state(u, include_fix, [&](const std::function<int()> &eval) -> int {
+      TRY(eval());
+      // the context or the rig owns H: the deletion edits it in place, and the next evaluation rewrites it
+      if (a0 >= 0) TRY(cov_delete_block(c, const_cast<double *>(sys.H), n, a0, 1.0));
+      return cov_factor(c, sys, a0, singular_msg);
+    }));
+  if (raw) CUDA_TRY(cudaMemcpyAsync(raw, R, sizeof(double) * n * n, cudaMemcpyDeviceToHost, c->stream));
+  if (cov) {
+    TRY(cov_sandwich(c, sys, R));
+    if (a0 >= 0) TRY(cov_delete_block(c, R, n, a0, 0.0));
+    CUDA_TRY(cudaMemcpyAsync(cov, R, sizeof(double) * n * n, cudaMemcpyDeviceToHost, c->stream));
+  }
+  CUDA_TRY(cudaStreamSynchronize(c->stream));
+  return BALM_OK;
+}
+
+// balm_block_covariance, balm_spg_covariance and balm_rig_block_covariance after their checks (`who` prefixes the
+// messages): H~^-1 on the block pattern at x12 / ext12 (sparse_covariance), so the call waits twice
+static int block_covariance(const Unknowns &u, const char *who, const double *x12, const double *ext12,
+                            bool include_fix, int anchor, double *cov) {
+  CUDA_TRY(cudaSetDevice(u.c->device));
+  return factor_at_state(u, include_fix, [&](const std::function<int()> &eval) {
+    return sparse_covariance(u.solver(), u.c->stream, anchor, [&]() -> int {
+      TRY(u.upload(x12, ext12));
+      return eval();
+    }, who, cov, &u.c->launches);
+  });
+}
+
+// balm_block_point_covariance and balm_rig_block_point_covariance after their checks (`who` prefixes the messages): the
+// raw term on the slot pattern at x12 / ext12 into raw_blocks, and with cov or marg Sigma_sel (block_point_cov_dev)
+// after the anchored undamped factorisation at the same state
+static int block_point_covariance(const Unknowns &u, const char *who, const double *x12, const double *ext12,
+                                  const double *c_cov81, double point_noise, bool include_fix, int anchor, int n_sel,
+                                  const int32_t *sel, double *raw_blocks, double *cov, double *marg) {
+  balm_ctx *c = u.c;
+  const bool sigma = cov || marg;
+  SparseSolver *sp = u.solver();
+  CUDA_TRY(cudaSetDevice(c->device));
+  TRY(u.upload(x12, ext12));
+  if (sigma)  // the evaluation composes the slot poses
+    TRY(factor_at_state(u, include_fix, [&](const std::function<int()> &eval) -> int {
+      TRY(eval());
+      return sparse_factor_undamped(sp, c->stream, anchor, who, &c->launches);
+    }));
+  else
+    TRY(u.compose());
+  ScratchPool pool;
+  double *raw = nullptr;
+  const size_t nraw = 36 * blocks_pairs(c->bh).size();
+  TRY(pool.get(&raw, nraw));
+  TRY(cov_raw_blocks_dev(c, pool, c->poses, c_cov81, point_noise, include_fix, raw));
+  if (sigma) TRY(block_point_cov_dev(c, sp, u.rig, u.state(), anchor, n_sel, sel, raw, cov, marg));
+  if (raw_blocks) CUDA_TRY(cudaMemcpyAsync(raw_blocks, raw, sizeof(double) * nraw, cudaMemcpyDeviceToHost, c->stream));
+  CUDA_TRY(cudaStreamSynchronize(c->stream));
+  return BALM_OK;
+}
+
 // ---------------- rig calibration (rig.cu) ----------------
 // balm_set_rig's and balm_block_set_rig's checks and attach (`who` prefixes the messages): detach on n_base 0, else the
 // arguments checked and a new rig built; on a refusal the previous rig stays
@@ -1253,37 +1473,6 @@ extern "C" int balm_block_set_rig(balm_ctx *c, int n_base, int n_lidar, const in
                  n_rig_out);
 }
 
-// uploads base12 / ext12 into the rig's current state
-static int rig_upload(balm_ctx *c, const double *base12, const double *ext12) {
-  Rig *r = c->rig;
-  double *st = rig_state(r, false);
-  const int B = rig_bases(r), L = rig_lidars(r);
-  CUDA_TRY(cudaMemcpyAsync(st, base12, sizeof(double) * 12 * B, cudaMemcpyHostToDevice, c->stream));
-  CUDA_TRY(cudaMemcpyAsync(st + 12 * (size_t)B, ext12, sizeof(double) * 12 * L, cudaMemcpyHostToDevice, c->stream));
-  return BALM_OK;
-}
-
-// compose, evaluate every voxel and reduce to H_rig | g_rig at the rig's current state; the residual in c->scal[0].
-// The reduction's time joins ms_assemble.
-static int rig_evaluate_dev(balm_ctx *c, bool include_fix) {
-  Rig *r = c->rig;
-  const double *st = rig_state(r, false);
-  TRY(rig_compose(r, c->stream, st, c->poses, &c->launches));
-  TRY(evaluate_dev(c, c->poses, 0, c->M, include_fix));  // a blocks context: the slot blocks, factors, then priors
-  CUDA_TRY(cudaEventRecord(c->ev[13], c->stream));
-  if (rig_sparse(r)) TRY(rig_reduce_blocks(r, c->stream, st, blocks_device(c->bh), c->g, &c->launches));
-  else TRY(rig_reduce(r, c->stream, st, c->H, c->g, &c->launches));
-  CUDA_TRY(cudaEventRecord(c->ev[14], c->stream));
-  return BALM_OK;
-}
-
-static int rig_collect_reduce(balm_ctx *c) {
-  float ms;
-  CUDA_TRY(cudaEventElapsedTime(&ms, c->ev[13], c->ev[14]));
-  c->tm.ms_assemble += ms;
-  return BALM_OK;
-}
-
 // A block-sparse rig's pattern follows the slot pattern: rebuilt here when that has changed (BALM_ERR_UNSUPPORTED when
 // too large to index)
 static int rig_check(balm_ctx *c, const char *who) {
@@ -1301,47 +1490,13 @@ static int rig_check(balm_ctx *c, const char *who) {
   return BALM_OK;
 }
 
-// A block-sparse rig's H_rig as the dense column-major n_rig x n_rig matrix of its blocks (zeros elsewhere), on the
-// host (waits), as blocks_to_dense
-static int rig_blocks_to_dense(balm_ctx *c, double *H) {
-  const std::vector<int2> &pr = rig_pairs(c->rig);
-  std::vector<double> b(36 * pr.size());
-  CUDA_TRY(cudaMemcpyAsync(b.data(), rig_blocks(c->rig), sizeof(double) * b.size(), cudaMemcpyDeviceToHost, c->stream));
-  CUDA_TRY(cudaStreamSynchronize(c->stream));
-  const size_t n = rig_n(c->rig);
-  std::fill(H, H + n * n, 0.0);
-  for (size_t p = 0; p < pr.size(); p++)
-    for (int col = 0; col < 6; col++)
-      for (int row = 0; row < 6; row++) {
-        const double h = b[36 * p + 6 * col + row];
-        const size_t r = 6 * (size_t)pr[p].x + row, cc = 6 * (size_t)pr[p].y + col;
-        H[cc * n + r] = h;
-        H[r * n + cc] = h;
-      }
-  return BALM_OK;
-}
-
 extern "C" int balm_rig_evaluate(balm_ctx *c, const double *base12, const double *ext12, int include_fix, double *H,
                                  double *g, double *residual) {
   if (!c || !base12 || !ext12) { balm_set_error("balm_rig_evaluate: bad arguments"); return BALM_ERR_INVALID; }
   TRY(rig_check(c, "balm_rig_evaluate"));
-  CUDA_TRY(cudaSetDevice(c->device));
-  TRY(rig_upload(c, base12, ext12));
-  TRY(rig_evaluate_dev(c, include_fix != 0));
-  const DenseSystem sys = rig_system(c->rig);
-  const size_t nr = sys.n;
-  if (H && rig_sparse(c->rig)) TRY(rig_blocks_to_dense(c, H));
-  else if (H) CUDA_TRY(cudaMemcpyAsync(H, sys.H, sizeof(double) * nr * nr, cudaMemcpyDeviceToHost, c->stream));
-  if (g) CUDA_TRY(cudaMemcpyAsync(g, sys.g, sizeof(double) * nr, cudaMemcpyDeviceToHost, c->stream));
-  CUDA_TRY(cudaMemcpyAsync(c->h_scal, c->scal, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
-  CUDA_TRY(cudaStreamSynchronize(c->stream));
-  TRY(rig_collect_reduce(c));
-  if (residual) *residual = c->h_scal[0];
-  return BALM_OK;
+  return evaluate(Unknowns{c, c->rig}, base12, ext12, 0, c->M, include_fix != 0, H, g, residual);
 }
 
-// raw_rig = J^T R J with R balm_pose_covariance's Rcov_raw at the composed poses, and H_rig^-1 raw_rig H_rig^-T with
-// balm_rig_evaluate's H_rig, both with the anchor's rows and columns deleted. Waits for the pivot test and at the end.
 extern "C" int balm_rig_covariance(balm_ctx *c, const double *base12, const double *ext12, const double *c_cov81,
                                    double point_noise, int include_fix, int anchor, double *raw, double *cov) {
   const char *who = "balm_rig_covariance";
@@ -1353,120 +1508,22 @@ extern "C" int balm_rig_covariance(balm_ctx *c, const double *base12, const doub
   }
   TRY(rig_check(c, who));
   if (c->M < 1) { balm_set_error(std::string(who) + ": no voxels registered"); return BALM_ERR_INVALID; }
-  Rig *rg = c->rig;
-  const int nr = rig_n(rg);
-  if (anchor < -1 || anchor >= rig_free_bases(rg)) {
-    balm_set_error(std::string(who) + ": anchor " + std::to_string(anchor) + " is neither -1 nor a free base index in [0, " +
-                   std::to_string(rig_free_bases(rg)) + ")");
-    return BALM_ERR_INVALID;
-  }
-  const int a0 = anchor < 0 ? -1 : 6 * anchor;
-  CUDA_TRY(cudaSetDevice(c->device));
-  TRY(rig_upload(c, base12, ext12));
-  const double *st = rig_state(rg, false);
-  ScratchPool pool;
-  double *R = nullptr, *raw_rig = nullptr;
-  TRY(pool.get(&raw_rig, (size_t)nr * nr));
-  TRY(rig_compose(rg, c->stream, st, c->poses, &c->launches));
-  TRY(cov_raw_dev(c, pool, c->poses, c_cov81, point_noise, include_fix != 0, &R));
-  TRY(rig_reduce_raw(rg, c->stream, st, R, raw_rig, &c->launches));
-  if (a0 >= 0) TRY(cov_delete_block(c, raw_rig, nr, a0, 0.0));
-  const DenseSystem sys = rig_system(rg);
-  if (cov) {
-    // H_rig at the same state (the evaluation deferred: its events are read after cov_factor's wait), the anchor
-    // deleted with 1 on its diagonal, factored undamped
-    c->defer = true;
-    int rc = rig_evaluate_dev(c, include_fix != 0);
-    c->defer = false;
-    // the rig owns H_rig: the deletion edits it in place, and the next evaluation rewrites it
-    if (rc == BALM_OK && a0 >= 0) rc = cov_delete_block(c, const_cast<double *>(sys.H), nr, a0, 1.0);
-    if (rc == BALM_OK)
-      rc = cov_factor(c, sys, a0, "balm_rig_covariance: H_rig is singular (a gauge or an unobservable direction of the "
-                                  "rig is not fixed: fix clusters, fixed unknowns or an anchor)");
-    if (rc == BALM_OK || rc == BALM_ERR_NOT_PD) {  // the stream has been synchronised
-      const int rc2 = collect_eval(c);
-      if (rc2 != BALM_OK) rc = rc2;
-      else TRY(rig_collect_reduce(c));
-    }
-    c->pending_eval = false;
-    TRY(rc);
-  }
-  if (raw) CUDA_TRY(cudaMemcpyAsync(raw, raw_rig, sizeof(double) * nr * nr, cudaMemcpyDeviceToHost, c->stream));
-  if (cov) {
-    TRY(cov_sandwich(c, sys, raw_rig));
-    if (a0 >= 0) TRY(cov_delete_block(c, raw_rig, nr, a0, 0.0));
-    CUDA_TRY(cudaMemcpyAsync(cov, raw_rig, sizeof(double) * nr * nr, cudaMemcpyDeviceToHost, c->stream));
-  }
-  CUDA_TRY(cudaStreamSynchronize(c->stream));
-  return BALM_OK;
+  const Unknowns u{c, c->rig};
+  TRY(u.check_anchor(who, anchor));
+  return covariance(u, base12, ext12, c_cov81, point_noise, include_fix != 0, anchor,
+                    "balm_rig_covariance: H_rig is singular (a gauge or an unobservable direction of the rig is not "
+                    "fixed: fix clusters, fixed unknowns or an anchor)",
+                    raw, cov);
 }
 
-// balm_damping_iter's loop on the rig cost: per iteration compose -> evaluate -> reduce -> solve -> rig update ->
-// compose the trial state -> trial residual, then the one wait. No hand-over and no speculation: every evaluation is
-// the pure function balm_evaluate is.
 extern "C" int balm_rig_damping_iter(balm_ctx *c, double *base12, double *ext12, const balm_lm_opts *o,
                                      balm_trace *trace, int *n_iters, double *rig_per_iter) {
   const char *who = "balm_rig_damping_iter";
   if (!c || !base12 || !ext12 || !o) { balm_set_error(std::string(who) + ": bad arguments"); return BALM_ERR_INVALID; }
   if (n_iters) *n_iters = 0;
   TRY(rig_check(c, who));
-  Rig *rg = c->rig;
-  if ((o->gauge_mode == 0 || o->gauge_mode == 1) && rig_any_base_fixed(rg)) {
-    balm_set_error(std::string(who) + ": gauge_mode " + std::to_string(o->gauge_mode) +
-                   " re-anchors to base pose 0, which moves the result off the fixed base poses; pass gauge_mode 2");
-    return BALM_ERR_INVALID;
-  }
-  if (c->prec == BALM_PREC_BLOCKS) TRY(refuse_gauge_with_priors(who, c->pr, o));
-  if (o->min_planes_per_pose > 0 && c->min_planes < o->min_planes_per_pose) {  // per scan slot, as balm_damping_iter
-    balm_set_error("Initial error too large. Please loose plane determination criteria for more planes.");
-    return BALM_ERR_TOO_FEW_PLANES;
-  }
   CUDA_TRY(cudaSetDevice(c->device));
-  TRY(rig_upload(c, base12, ext12));
-  const int B = rig_bases(rg), U = B + rig_lidars(rg);
-  const size_t sbytes = sizeof(double) * 12 * U;
-  const DenseSystem sys = rig_system(rg);
-  SparseSolver *sp = rig_sparse(rg) ? rig_solver(rg) : nullptr;
-  LmScope lm_scope{c};
-  c->defer = true;  // the evaluation's events and flags are read after the iteration's wait
-  bool reduced = false;  // this iteration evaluated: the reduction's events are to be read
-  LmSteps s{c->stream, c->scal, c->h_scal};
-  s.eval = [&]() {
-    reduced = true;
-    return rig_evaluate_dev(c, o->hess_includes_fix != 0);
-  };
-  s.solve = [c, &sys, sp](double u) { return solve_dev(c, sys, sp, u); };
-  s.trial = [c, rg]() -> int {
-    TRY(rig_update(rg, c->stream, rig_state(rg, false), rig_state(rg, true), &c->launches));
-    return rig_compose(rg, c->stream, rig_state(rg, true), c->poses_trial, &c->launches);
-  };
-  s.trial_cost = [c](double *r2) { return residual_dev(c, c->poses_trial, r2); };
-  s.finish = [&](double *q1, int *not_pd, int *refined) -> int {
-    TRY(collect_eval(c));
-    if (reduced) TRY(rig_collect_reduce(c));
-    reduced = false;
-    return collect_solve(c, sys, sp, q1, not_pd, refined);
-  };
-  s.step = [rg](bool accepted) {
-    if (accepted) rig_swap_states(rg);
-    return BALM_OK;
-  };
-  s.snapshot = [&](int it) -> int {
-    if (rig_per_iter)
-      CUDA_TRY(cudaMemcpyAsync(rig_per_iter + (size_t)it * 12 * U, rig_state(rg, false), sbytes, cudaMemcpyDeviceToHost,
-                               c->stream));
-    return BALM_OK;
-  };
-  TRY(lm_run(s, o, trace, n_iters));
-  if (o->gauge_mode == 0 || o->gauge_mode == 1) {  // base poses re-anchored to base 0; extrinsics are body-frame
-    c->launches += 1;
-    TRY(launch_gauge(c->stream, B, rig_state(rg, false), c->scal + 4, o->gauge_mode));
-  }
-  const double *st = rig_state(rg, false);
-  CUDA_TRY(cudaMemcpyAsync(base12, st, sizeof(double) * 12 * B, cudaMemcpyDeviceToHost, c->stream));
-  CUDA_TRY(cudaMemcpyAsync(ext12, st + 12 * (size_t)B, sizeof(double) * 12 * (U - B), cudaMemcpyDeviceToHost, c->stream));
-  CUDA_TRY(cudaStreamSynchronize(c->stream));
-  return BALM_OK;
+  return damping_iter(Unknowns{c, c->rig}, who, base12, ext12, o, trace, n_iters, rig_per_iter);
 }
 
 // the block-sparse rig's calls: a rig set by balm_block_set_rig, its pattern in step with the slot pattern
@@ -1496,30 +1553,9 @@ extern "C" int balm_rig_block_covariance(balm_ctx *c, const double *base12, cons
   const char *who = "balm_rig_block_covariance";
   if (!c || !base12 || !ext12 || !cov) { balm_set_error(std::string(who) + ": bad arguments"); return BALM_ERR_INVALID; }
   TRY(block_rig_check(c, who));
-  Rig *rg = c->rig;
-  if (anchor < -1 || anchor >= rig_free_bases(rg)) {
-    balm_set_error(std::string(who) + ": anchor " + std::to_string(anchor) + " is neither -1 nor a free base index in [0, " +
-                   std::to_string(rig_free_bases(rg)) + ")");
-    return BALM_ERR_INVALID;
-  }
-  CUDA_TRY(cudaSetDevice(c->device));
-  // H_rig at base12 / ext12 left in the rig's blocks, the evaluation deferred (its events are read after
-  // sparse_covariance's waits)
-  bool evaluated = false;
-  const int rc = sparse_covariance(rig_solver(rg), c->stream, anchor, [&]() -> int {
-    TRY(rig_upload(c, base12, ext12));
-    evaluated = true;
-    c->defer = true;
-    const int e = rig_evaluate_dev(c, include_fix != 0);
-    c->defer = false;
-    return e;
-  }, who, cov, &c->launches);
-  if (evaluated && (rc == BALM_OK || rc == BALM_ERR_NOT_PD)) {  // the stream has been synchronised
-    TRY(collect_eval(c));
-    TRY(rig_collect_reduce(c));
-  }
-  c->pending_eval = false;
-  return rc;
+  const Unknowns u{c, c->rig};
+  TRY(u.check_anchor(who, anchor));
+  return block_covariance(u, who, base12, ext12, include_fix != 0, anchor, cov);
 }
 
 // ---------------- point-noise covariance on blocks contexts (covariance.cu) ----------------
@@ -1552,23 +1588,6 @@ static int point_cov_budget_check(const char *who, int P, int N, int n_sel, bool
   return BALM_ERR_UNSUPPORTED;
 }
 
-// The eval of H (or H_rig) at the caller's state, deferred, then the anchored undamped factorisation; the evaluation's
-// events are read after the factorisation's wait (as block_covariance)
-static int point_cov_factor(balm_ctx *c, SparseSolver *sp, int anchor, const char *who,
-                            const std::function<int()> &eval, bool rig) {
-  c->defer = true;
-  int rc = eval();
-  c->defer = false;
-  const bool evaluated = rc == BALM_OK;
-  if (rc == BALM_OK) rc = sparse_factor_undamped(sp, c->stream, anchor, who, &c->launches);
-  if (evaluated && (rc == BALM_OK || rc == BALM_ERR_NOT_PD)) {  // the stream has been synchronised
-    TRY(collect_eval(c));
-    if (rig) TRY(rig_collect_reduce(c));
-  }
-  c->pending_eval = false;
-  return rc;
-}
-
 extern "C" int balm_rig_block_point_covariance(balm_ctx *c, const double *base12, const double *ext12,
                                                const double *c_cov81, double point_noise, int include_fix, int anchor,
                                                int n_sel, const int32_t *sel, double *cov, double *marg) {
@@ -1580,26 +1599,13 @@ extern "C" int balm_rig_block_point_covariance(balm_ctx *c, const double *base12
   }
   TRY(block_rig_check(c, who));
   if (c->M < 1) { balm_set_error(std::string(who) + ": no voxels registered"); return BALM_ERR_INVALID; }
-  Rig *rg = c->rig;
-  const int F = rig_n(rg) / 6;
-  if (anchor < -1 || anchor >= rig_free_bases(rg)) {
-    balm_set_error(std::string(who) + ": anchor " + std::to_string(anchor) + " is neither -1 nor a free base index in [0, " +
-                   std::to_string(rig_free_bases(rg)) + ")");
-    return BALM_ERR_INVALID;
-  }
+  const Unknowns u{c, c->rig};
+  const int F = rig_n(u.rig) / 6;
+  TRY(u.check_anchor(who, anchor));
   TRY(point_cov_sel_check(who, n_sel, sel, F, "free unknown"));
   TRY(point_cov_budget_check(who, F, c->N, n_sel, cov != nullptr));
-  CUDA_TRY(cudaSetDevice(c->device));
-  SparseSolver *sp = rig_solver(rg);
-  TRY(point_cov_factor(c, sp, anchor, who, [&]() -> int {
-    TRY(rig_upload(c, base12, ext12));
-    return rig_evaluate_dev(c, include_fix != 0);  // composes the slot poses into c->poses
-  }, true));
-  ScratchPool pool;
-  double *raw = nullptr;
-  TRY(pool.get(&raw, 36 * blocks_pairs(c->bh).size()));
-  TRY(cov_raw_blocks_dev(c, pool, c->poses, c_cov81, point_noise, include_fix != 0, raw));
-  return block_point_cov_dev(c, sp, rg, rig_state(rg, false), anchor, n_sel, sel, raw, cov, marg);
+  return block_point_covariance(u, who, base12, ext12, c_cov81, point_noise, include_fix != 0, anchor, n_sel, sel,
+                                nullptr, cov, marg);
 }
 
 // ---------------- absolute pose priors (pose_graph.cu) ----------------
@@ -1833,20 +1839,15 @@ extern "C" int balm_window_push(balm_ctx *c, int win_count, int64_t *n_voxels_ou
 }
 
 // ---------------- pose covariance (covariance.cu) ----------------
-int pose_covariance_dev(balm_ctx *c, const double *poses_dev, const double *ccov_host, double point_noise, bool include_fix,
-                        double *Rraw_host, double *Rcov_host);
-int balm_cov_evaluate_hessian(balm_ctx *c, const double *poses_dev, bool include_fix) {
-  return evaluate_dev(c, poses_dev, 0, c->M, include_fix);
-}
 extern "C" int balm_pose_covariance(balm_ctx *c, const double *poses12, const double *c_cov81, double point_noise,
                                     int include_fix, double *Rcov_raw, double *Rcov) {
   if (!c || !poses12 || (!Rcov_raw && !Rcov)) { balm_set_error("balm_pose_covariance: bad arguments"); return BALM_ERR_INVALID; }
   TRY(refuse_blocks(c, "balm_pose_covariance"));
   if (!c->registered || c->M < 1) { balm_set_error("balm_pose_covariance: no voxels registered"); return BALM_ERR_INVALID; }
   if (c->world > 1) { balm_set_error("balm_pose_covariance: single-GPU contexts only"); return BALM_ERR_UNSUPPORTED; }
-  CUDA_TRY(cudaSetDevice(c->device));
-  CUDA_TRY(cudaMemcpyAsync(c->poses, poses12, sizeof(double) * 12 * c->N, cudaMemcpyHostToDevice, c->stream));
-  return pose_covariance_dev(c, c->poses, c_cov81, point_noise, include_fix != 0, Rcov_raw, Rcov);
+  return covariance(Unknowns{c, nullptr}, poses12, nullptr, c_cov81, point_noise, include_fix != 0, -1,
+                    "balm_pose_covariance: H is singular (gauge freedom not fixed: no fix clusters in the Hessian)",
+                    Rcov_raw, Rcov);
 }
 
 // ---------------- multi-GPU ----------------
@@ -1972,31 +1973,15 @@ extern "C" int balm_download_blocks(balm_ctx *c, double *blocks) {
   return BALM_OK;
 }
 
-// balm_block_covariance and balm_spg_covariance after their argument checks; `who` prefixes the messages
-static int block_covariance(balm_ctx *c, const char *who, const double *poses12, bool include_fix, int anchor,
-                            double *cov) {
-  CUDA_TRY(cudaSetDevice(c->device));
-  // the evaluation is deferred (its events are read after sparse_covariance's waits), so the call waits twice
-  const int rc = sparse_covariance(blocks_solver(c->bh), c->stream, anchor, [&]() -> int {
-    CUDA_TRY(cudaMemcpyAsync(c->poses, poses12, sizeof(double) * 12 * c->N, cudaMemcpyHostToDevice, c->stream));
-    c->defer = true;
-    const int e = balm_cov_evaluate_hessian(c, c->poses, include_fix);
-    c->defer = false;
-    return e;
-  }, who, cov, &c->launches);
-  if (rc == BALM_OK || rc == BALM_ERR_NOT_PD) TRY(collect_eval(c));  // the stream has been synchronised
-  c->pending_eval = false;
-  return rc;
-}
-
 extern "C" int balm_block_covariance(balm_ctx *c, const double *poses12, int include_fix, int anchor, double *cov) {
   if (!c || !poses12 || !cov) { balm_set_error("balm_block_covariance: bad arguments"); return BALM_ERR_INVALID; }
   if (c->prec != BALM_PREC_BLOCKS || !c->bh || !c->registered) {
     balm_set_error("balm_block_covariance: no voxels registered on a BALM_PREC_BLOCKS context");
     return BALM_ERR_INVALID;
   }
-  if (anchor < -1 || anchor >= c->N) { balm_set_error("balm_block_covariance: anchor outside [-1, N)"); return BALM_ERR_INVALID; }
-  return block_covariance(c, "balm_block_covariance", poses12, include_fix != 0, anchor, cov);
+  const Unknowns u{c, nullptr};
+  TRY(u.check_anchor("balm_block_covariance", anchor));
+  return block_covariance(u, "balm_block_covariance", poses12, nullptr, include_fix != 0, anchor, cov);
 }
 
 extern "C" int balm_block_point_covariance(balm_ctx *c, const double *poses12, const double *c_cov81, double point_noise,
@@ -2012,27 +1997,14 @@ extern "C" int balm_block_point_covariance(balm_ctx *c, const double *poses12, c
     return BALM_ERR_INVALID;
   }
   if (c->world > 1 || c->comm) { balm_set_error(std::string(who) + ": single-GPU contexts only"); return BALM_ERR_INVALID; }
-  if (anchor < -1 || anchor >= c->N) { balm_set_error(std::string(who) + ": anchor outside [-1, N)"); return BALM_ERR_INVALID; }
-  const bool sigma = cov || marg;
-  if (sigma) {
+  const Unknowns u{c, nullptr};
+  TRY(u.check_anchor(who, anchor));
+  if (cov || marg) {
     TRY(point_cov_sel_check(who, n_sel, sel, c->N, "pose"));
     TRY(point_cov_budget_check(who, c->N, c->N, n_sel, cov != nullptr));
   }
-  CUDA_TRY(cudaSetDevice(c->device));
-  SparseSolver *sp = blocks_solver(c->bh);
-  CUDA_TRY(cudaMemcpyAsync(c->poses, poses12, sizeof(double) * 12 * c->N, cudaMemcpyHostToDevice, c->stream));
-  if (sigma)
-    TRY(point_cov_factor(c, sp, anchor, who, [&]() { return balm_cov_evaluate_hessian(c, c->poses, include_fix != 0); },
-                         false));
-  ScratchPool pool;
-  double *raw = nullptr;
-  const size_t nraw = 36 * blocks_pairs(c->bh).size();
-  TRY(pool.get(&raw, nraw));
-  TRY(cov_raw_blocks_dev(c, pool, c->poses, c_cov81, point_noise, include_fix != 0, raw));
-  if (sigma) TRY(block_point_cov_dev(c, sp, nullptr, nullptr, anchor, n_sel, sel, raw, cov, marg));
-  if (raw_blocks) CUDA_TRY(cudaMemcpyAsync(raw_blocks, raw, sizeof(double) * nraw, cudaMemcpyDeviceToHost, c->stream));
-  CUDA_TRY(cudaStreamSynchronize(c->stream));
-  return BALM_OK;
+  return block_point_covariance(u, who, poses12, nullptr, c_cov81, point_noise, include_fix != 0, anchor, n_sel, sel,
+                                raw_blocks, cov, marg);
 }
 
 // ---------------- sparse pose graph (pose_graph.cu, pose_graph_sparse.cu, blocks.cu) ----------------
@@ -2118,8 +2090,9 @@ extern "C" int balm_spg_iter(balm_spg *s, double *poses12, const balm_lm_opts *o
 extern "C" int balm_spg_covariance(balm_spg *s, const double *poses12, int anchor, double *cov) {
   if (!s || !poses12 || !cov) { balm_set_error("balm_spg_covariance: bad arguments"); return BALM_ERR_INVALID; }
   TRY(spg_registered(s, "balm_spg_covariance"));
-  if (anchor < -1 || anchor >= s->c->N) { balm_set_error("balm_spg_covariance: anchor outside [-1, N)"); return BALM_ERR_INVALID; }
-  return block_covariance(s->c, "balm_spg_covariance", poses12, false, anchor, cov);
+  const Unknowns u{s->c, nullptr};
+  TRY(u.check_anchor("balm_spg_covariance", anchor));
+  return block_covariance(u, "balm_spg_covariance", poses12, nullptr, false, anchor, cov);
 }
 
 extern "C" int balm_spg_set_factor_loss(balm_spg *s, int n_factors, const int32_t *kind, const double *scale) {

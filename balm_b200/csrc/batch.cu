@@ -577,7 +577,7 @@ __global__ void __launch_bounds__(128) batch_cov_diag_kernel(Dev d, const int *o
   }
 }
 
-// ---- per problem, one CTA: undamped LDL^T of H in shared memory, the singularity test of pose_covariance_dev, then
+// ---- per problem, one CTA: undamped LDL^T of H in shared memory, the singularity test of cov_factor, then
 // Rcov = H^-1 R H^-1 as two sweeps over n right-hand sides, thread t owning right-hand side t (R and the result in
 // global memory, n^2 doubles being too many for shared memory; every access below is coalesced across threads).
 // The result is made exactly symmetric by copying its upper triangle to the lower one. ----

@@ -257,9 +257,6 @@ int covariance_setup() {
   return BALM_OK;
 }
 
-// Defined in balm_api.cu
-int balm_cov_evaluate_hessian(balm_ctx *c, const double *poses_dev, bool include_fix);
-
 // bytes of device scratch a covariance call's batched buffers may take
 static size_t cov_budget() {
   size_t budget = (size_t)4 << 30;
@@ -349,31 +346,6 @@ int cov_delete_block(balm_ctx *c, double *A, int n, int a0, double diag) {
   delete_block_kernel<<<dim3((n + 127) / 128, 6), 128, 0, c->stream>>>(A, n, a0, diag);
   c->launches += 1;
   CUDA_TRY(cudaGetLastError());
-  return BALM_OK;
-}
-
-// Defined in balm_api.cu
-int balm_cov_evaluate_hessian(balm_ctx *c, const double *poses_dev, bool include_fix);
-
-int pose_covariance_dev(balm_ctx *c, const double *poses_dev, const double *ccov_host, double point_noise, bool include_fix,
-                        double *Rraw_host, double *Rcov_host) {
-  const int n = c->n;
-  cudaStream_t st = c->stream;
-  if (c->M < 1) { balm_set_error("balm_pose_covariance: no voxels registered"); return BALM_ERR_INVALID; }
-  ScratchPool pool;
-  double *R = nullptr;
-  TRY(cov_raw_dev(c, pool, poses_dev, ccov_host, point_noise, include_fix, &R));
-  if (Rraw_host) CUDA_TRY(cudaMemcpyAsync(Rraw_host, R, sizeof(double) * (size_t)n * n, cudaMemcpyDeviceToHost, st));
-  if (Rcov_host) {
-    // H at these poses (divide_thread, BAs_left.hpp:1091), factored without damping, then H^-1 R H^-T
-    TRY(balm_cov_evaluate_hessian(c, poses_dev, include_fix));
-    const DenseSystem sys = ctx_system(c);
-    TRY(cov_factor(c, sys, -1,
-                   "balm_pose_covariance: H is singular (gauge freedom not fixed: no fix clusters in the Hessian)"));
-    TRY(cov_sandwich(c, sys, R));
-    CUDA_TRY(cudaMemcpyAsync(Rcov_host, R, sizeof(double) * (size_t)n * n, cudaMemcpyDeviceToHost, st));
-  }
-  CUDA_TRY(cudaStreamSynchronize(st));
   return BALM_OK;
 }
 
