@@ -39,18 +39,23 @@ def _set_pose_factors(fn, handle, factors):
 _LOSS = {"trivial": L.LOSS_TRIVIAL, "huber": L.LOSS_HUBER, "cauchy": L.LOSS_CAUCHY}
 
 
+def _loss_arrays(who, kinds, scale):
+    """Loss names, one per term, and scale a scalar or one per term (unused for trivial terms) -> the int32 kind and
+    float64 scale arrays of balm_set_factor_loss / balm_set_pose_priors (scale None: None); `who` prefixes errors."""
+    if any(k not in _LOSS for k in kinds):
+        raise ValueError(f"{who}: kinds must be in {sorted(_LOSS)}, got {sorted(set(kinds) - set(_LOSS))}")
+    k = np.array([_LOSS[x] for x in kinds], dtype=np.int32)
+    sc = None if scale is None else np.ascontiguousarray(np.broadcast_to(np.asarray(scale, dtype=np.float64), k.shape))
+    return k, sc
+
+
 def _set_factor_loss(fn, handle, n_factors, kind, scale):
     """balm_set_factor_loss / balm_spg_set_factor_loss: kind a loss name or one per factor, scale a scalar or one per
     factor (ignored for trivial factors); kind="trivial" resets every factor."""
-    if isinstance(kind, str):
-        if kind == "trivial":
-            L.check(fn(handle, n_factors, None, None))
-            return
-        kind = [kind] * n_factors
-    if any(k not in _LOSS for k in kind):
-        raise ValueError(f"set_factor_loss: kinds must be in {sorted(_LOSS)}, got {sorted(set(kind) - set(_LOSS))}")
-    k = np.array([_LOSS[x] for x in kind], dtype=np.int32)
-    sc = None if scale is None else np.ascontiguousarray(np.broadcast_to(np.asarray(scale, dtype=np.float64), k.shape))
+    if isinstance(kind, str) and kind == "trivial":
+        L.check(fn(handle, n_factors, None, None))
+        return
+    k, sc = _loss_arrays("set_factor_loss", [kind] * n_factors if isinstance(kind, str) else kind, scale)
     L.check(fn(handle, len(k), _p(k), _p(sc)))
 
 
@@ -92,11 +97,7 @@ def _set_pose_priors(fn, handle, N, priors, kind, scale):
         lever = np.ascontiguousarray([np.zeros(3) if p.get("lever_arm") is None else
                                       np.asarray(p["lever_arm"], dtype=np.float64).reshape(3) for p in priors])
     kinds = [kind] * n if isinstance(kind, str) else list(kind)
-    if any(k not in _LOSS for k in kinds):
-        raise ValueError(f"set_pose_priors: kinds must be in {sorted(_LOSS)}, got {sorted(set(kinds) - set(_LOSS))}")
-    k = None if all(x == "trivial" for x in kinds) else np.array([_LOSS[x] for x in kinds], dtype=np.int32)
-    sc = None if k is None or scale is None else \
-        np.ascontiguousarray(np.broadcast_to(np.asarray(scale, dtype=np.float64), (n,)))
+    k, sc = (None, None) if all(x == "trivial" for x in kinds) else _loss_arrays("set_pose_priors", kinds, scale)
     status = np.zeros(n, dtype=np.int32)
     L.check(fn(handle, n, _p(pose), _p(hat), _p(lever), _p(H), _p(k), _p(sc), _p(status)))
     return [int(s) for s in status]

@@ -1178,16 +1178,7 @@ static int pose_factors_check(const char *who, int P, int n_factors, const int64
   return BALM_OK;
 }
 
-extern "C" int balm_set_pose_factors(balm_ctx *c, int n_factors, const int64_t *factor_ptr, const int32_t *factor_pose,
-                                     const double *poses_hat12, const double *H, int32_t *status_out) {
-  if (!c) { balm_set_error("balm_set_pose_factors: bad arguments"); return BALM_ERR_INVALID; }
-  TRY(refuse_blocks(c, "balm_set_pose_factors"));
-  TRY(pose_factors_check("balm_set_pose_factors", c->N, n_factors, factor_ptr, factor_pose, poses_hat12, H));
-  CUDA_TRY(cudaSetDevice(c->device));
-  return pose_graph_set(c, n_factors, factor_ptr, factor_pose, poses_hat12, H, status_out);
-}
-
-// balm_block_set_factors and balm_spg_set_factors after their argument checks
+// balm_set_pose_factors, balm_block_set_factors and balm_spg_set_factors after their argument checks
 static int block_set_factors(balm_ctx *c, const char *who, int n_factors, const int64_t *factor_ptr,
                              const int32_t *factor_pose, const double *poses_hat12, const double *H, int32_t *status_out) {
   CUDA_TRY(cudaSetDevice(c->device));
@@ -1215,6 +1206,29 @@ extern "C" int balm_block_set_factors(balm_ctx *c, int n_factors, const int64_t 
   return block_set_factors(c, who, n_factors, factor_ptr, factor_pose, poses_hat12, H, status_out);
 }
 
+extern "C" int balm_set_pose_factors(balm_ctx *c, int n_factors, const int64_t *factor_ptr, const int32_t *factor_pose,
+                                     const double *poses_hat12, const double *H, int32_t *status_out) {
+  const char *who = "balm_set_pose_factors";
+  if (!c) { balm_set_error(std::string(who) + ": bad arguments"); return BALM_ERR_INVALID; }
+  TRY(refuse_blocks(c, who));
+  TRY(pose_factors_check(who, c->N, n_factors, factor_ptr, factor_pose, poses_hat12, H));
+  return block_set_factors(c, who, n_factors, factor_ptr, factor_pose, poses_hat12, H, status_out);
+}
+
+// The loss arguments of one factor or prior: kind one of balm_loss, and a finite scale > 0 unless trivial. `item`
+// ("<who>: factor f" / "<who>: prior q") prefixes the messages.
+static int term_loss_check(const std::string &item, int32_t kind, const double *scale) {
+  if (kind != BALM_LOSS_TRIVIAL && kind != BALM_LOSS_HUBER && kind != BALM_LOSS_CAUCHY) {
+    balm_set_error(item + " has loss kind " + std::to_string(kind) + " (0, 1, 2 allowed)");
+    return BALM_ERR_INVALID;
+  }
+  if (kind != BALM_LOSS_TRIVIAL && !(scale && std::isfinite(*scale) && *scale > 0.0)) {
+    balm_set_error(item + " needs a finite scale > 0");
+    return BALM_ERR_INVALID;
+  }
+  return BALM_OK;
+}
+
 // balm_set_factor_loss / balm_spg_set_factor_loss on the factor set pg (null: none registered)
 static int set_factor_loss(const char *who, PoseGraph *pg, cudaStream_t st, int n_factors, const int32_t *kind,
                            const double *scale) {
@@ -1225,16 +1239,8 @@ static int set_factor_loss(const char *who, PoseGraph *pg, cudaStream_t st, int 
                    std::to_string(pose_graph_n_factors(pg)));
     return BALM_ERR_INVALID;
   }
-  for (int f = 0; kind && f < n_factors; f++) {
-    if (kind[f] != BALM_LOSS_TRIVIAL && kind[f] != BALM_LOSS_HUBER && kind[f] != BALM_LOSS_CAUCHY) {
-      balm_set_error(w + "factor " + std::to_string(f) + " has loss kind " + std::to_string(kind[f]) + " (0, 1, 2 allowed)");
-      return BALM_ERR_INVALID;
-    }
-    if (kind[f] != BALM_LOSS_TRIVIAL && !(scale && std::isfinite(scale[f]) && scale[f] > 0.0)) {
-      balm_set_error(w + "factor " + std::to_string(f) + " needs a finite scale > 0");
-      return BALM_ERR_INVALID;
-    }
-  }
+  for (int f = 0; kind && f < n_factors; f++)
+    TRY(term_loss_check(w + "factor " + std::to_string(f), kind[f], scale ? scale + f : nullptr));
   return pose_graph_set_loss(pg, st, kind, scale);
 }
 
@@ -1244,12 +1250,20 @@ extern "C" int balm_set_factor_loss(balm_ctx *c, int n_factors, const int32_t *k
   return set_factor_loss("balm_set_factor_loss", c->pg, c->stream, n_factors, kind, scale);
 }
 
-extern "C" int balm_factor_residuals(balm_ctx *c, const double *poses12, double *s, double *w) {
-  if (!c || !poses12) { balm_set_error("balm_factor_residuals: bad arguments"); return BALM_ERR_INVALID; }
-  if (!c->pg) { balm_set_error("balm_factor_residuals: no pose factors registered"); return BALM_ERR_INVALID; }
+// balm_factor_residuals / balm_prior_residuals: the readout of the context's term set `set` (c->pg or c->pr), named
+// `what` in the refusal when none is registered
+template <typename Set>
+static int set_residuals(balm_ctx *c, Set *balm_ctx::*set, const char *who, const char *what, const double *poses12,
+                         double *s, double *w) {
+  if (!c || !poses12) { balm_set_error(std::string(who) + ": bad arguments"); return BALM_ERR_INVALID; }
+  if (!(c->*set)) { balm_set_error(std::string(who) + ": no " + what + " registered"); return BALM_ERR_INVALID; }
   CUDA_TRY(cudaSetDevice(c->device));
   CUDA_TRY(cudaMemcpyAsync(c->poses, poses12, sizeof(double) * 12 * c->N, cudaMemcpyHostToDevice, c->stream));
-  return pose_graph_residuals(c->pg, c->stream, c->poses, s, w, &c->launches);
+  return term_residuals(c->*set, c->stream, c->poses, s, w, &c->launches);
+}
+
+extern "C" int balm_factor_residuals(balm_ctx *c, const double *poses12, double *s, double *w) {
+  return set_residuals(c, &balm_ctx::pg, "balm_factor_residuals", "pose factors", poses12, s, w);
 }
 
 extern "C" int balm_pose_graph_evaluate(balm_ctx *c, const double *poses12, double *H, double *g, double *cost) {
@@ -1630,14 +1644,7 @@ static int pose_priors_check(const char *who, int P, int n, const int32_t *pose,
           balm_set_error(pq + " has an H that is not symmetric");
           return BALM_ERR_INVALID;
         }
-    if (kind && kind[q] != BALM_LOSS_TRIVIAL && kind[q] != BALM_LOSS_HUBER && kind[q] != BALM_LOSS_CAUCHY) {
-      balm_set_error(pq + " has loss kind " + std::to_string(kind[q]) + " (0, 1, 2 allowed)");
-      return BALM_ERR_INVALID;
-    }
-    if (kind && kind[q] != BALM_LOSS_TRIVIAL && !(scale && std::isfinite(scale[q]) && scale[q] > 0.0)) {
-      balm_set_error(pq + " needs a finite scale > 0");
-      return BALM_ERR_INVALID;
-    }
+    if (kind) TRY(term_loss_check(pq, kind[q], scale ? scale + q : nullptr));
   }
   return BALM_OK;
 }
@@ -1668,11 +1675,7 @@ extern "C" int balm_set_pose_priors(balm_ctx *c, int n_priors, const int32_t *po
 }
 
 extern "C" int balm_prior_residuals(balm_ctx *c, const double *poses12, double *s, double *w) {
-  if (!c || !poses12) { balm_set_error("balm_prior_residuals: bad arguments"); return BALM_ERR_INVALID; }
-  if (!c->pr) { balm_set_error("balm_prior_residuals: no pose priors registered"); return BALM_ERR_INVALID; }
-  CUDA_TRY(cudaSetDevice(c->device));
-  CUDA_TRY(cudaMemcpyAsync(c->poses, poses12, sizeof(double) * 12 * c->N, cudaMemcpyHostToDevice, c->stream));
-  return prior_residuals(c->pr, c->stream, c->poses, s, w, &c->launches);
+  return set_residuals(c, &balm_ctx::pr, "balm_prior_residuals", "pose priors", poses12, s, w);
 }
 
 // ---------------- sliding window on the registered voxel set (assoc.cu) ----------------

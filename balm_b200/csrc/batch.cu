@@ -63,8 +63,6 @@ struct Dev {  // what the kernels read
   int64_t M, K;
 };
 
-struct NoLoss {};  // the pure quadratic: the kernel exactly as without a voxel loss
-
 // ---- per voxel: the world-frame cluster sum over its observations (+ fix), eig, residual term, stats row; with
 // VoxelLoss the residual term coe rho(lambda_0) and coe w in the stats row (voxel_eig_kernel's rule) ----
 template <bool STORE, typename Loss>

@@ -90,8 +90,6 @@ __global__ void __launch_bounds__(STATS_THREADS, 3) voxel_sums_kernel(StatsArgs 
   }
 }
 
-struct NoLoss {};  // the pure quadratic: the kernel exactly as without a voxel loss
-
 // With VoxelLoss, rho and w = rho'(lambda_0) once per voxel: the residual term is coe rho(lambda_0) and the stats row
 // gets coe w in place of coe, which every Hessian, gradient and covariance term downstream is linear in.
 template <bool STORE, typename Loss>

@@ -225,6 +225,10 @@ inline int check_voxel_loss(const char *who, int kind, double scale) {
   return BALM_OK;
 }
 
+// The pure quadratic as a loss argument: the NoLoss instantiation of a kernel templated on its loss is that kernel as
+// without robust losses (the voxel stats kernels, the pose factors' and priors' cost and linearisation kernels)
+struct NoLoss {};
+
 // The voxel loss as the stats kernels take it (voxel_eig_kernel, batch_stats_kernel): kind / scale of
 // balm_set_voxel_loss, and with lam non-null the per-voxel readout lam[i] = lambda_min, w[i] = rho'(lambda_min)
 // (i: the voxel's index from the start of the launch's range).
@@ -880,9 +884,6 @@ void tensor_syrk_new_problem(balm_ctx *c);
 int pose_graph_build(cudaStream_t st, int P, int n_factors, const int64_t *factor_ptr, const int32_t *factor_pose,
                      const double *poses_hat12, const double *H, std::vector<int> *status, PoseGraph **out,
                      long long *launches);
-// balm_set_pose_factors after its argument checks: pose_graph_build, status_out [n_factors]; replaces c->pg on success.
-int pose_graph_set(balm_ctx *c, int n_factors, const int64_t *factor_ptr, const int32_t *factor_pose,
-                   const double *poses_hat12, const double *H, int32_t *status_out);
 // H | g | scal[0] of the registered factors at the device poses (enqueued, no wait)
 int pose_graph_eval(balm_ctx *c, const double *poses);
 // the same sums with one 6x6 block per pair (column-major, in pose_graph_pairs order) instead of dense H (enqueued)
@@ -903,8 +904,7 @@ int pose_graph_n_factors(const PoseGraph *p);
 int pose_graph_set_loss(PoseGraph *p, cudaStream_t st, const int32_t *kind, const double *scale);
 // balm_factor_residuals: s_f and rho'(s_f) of every factor at the device poses (0 for inactive factors) into the host
 // arrays s and w [F] (either may be null); enqueues the cost pass and waits once
-int pose_graph_residuals(const PoseGraph *p, cudaStream_t st, const double *poses, double *s, double *w,
-                         long long *launches);
+int term_residuals(const PoseGraph *p, cudaStream_t st, const double *poses, double *s, double *w, long long *launches);
 
 // ---------------- absolute pose priors (pose_graph.cu) ----------------
 // After the argument checks: uploads n priors (pose [n], hat12 [12n], lever3 [3n] or null, H36 [36n] column-major,
@@ -930,7 +930,7 @@ int prior_add_blocks(const PriorSet *p, cudaStream_t st, const double *poses, do
 int prior_add_cost(const PriorSet *p, cudaStream_t st, const double *poses, double *cost, long long *launches);
 // balm_prior_residuals: s and rho'(s) of every prior (0 for NOT_PD ones) into the host arrays s, w [n] (either may be
 // null); waits once
-int prior_residuals(const PriorSet *p, cudaStream_t st, const double *poses, double *s, double *w, long long *launches);
+int term_residuals(const PriorSet *p, cudaStream_t st, const double *poses, double *s, double *w, long long *launches);
 
 // ---------------- rig (rig.cu) ----------------
 // After the argument checks: the rig of N slots (base_of / lidar_of [N] host, base_fixed [B] / lidar_fixed [L] host or

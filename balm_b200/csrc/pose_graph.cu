@@ -11,13 +11,14 @@
 //                        (outputs: dense H, or a blocks context's blocks: stored, or added onto its voxel blocks)
 //   pg_cost_kernel       per active factor, one CTA: cost_f
 //   pg_sum_kernel        one CTA: the factors' costs in factor order -> a device scalar
-// Robust losses (DESIGN.md "Robust pose factors"): with s_f = e~^T H~ e~ the factor's cost becomes 1/2 rho(s_f), its b
-// rho'(s_f) b and its M rho'(s_f) M (IRLS). The <FactorLoss> instantiations of pg_cost_kernel (writes s_f and
-// w_f = rho'(s_f)) and pg_linearise_kernel (scales M and b by w_f) run only when an active factor has a non-trivial loss;
-// the <NoLoss> ones are the kernels without a loss.
 // Absolute pose priors (DESIGN.md "Absolute pose priors"; PriorSet, balm_set_pose_priors): prior_cost_kernel and
 // prior_linearise_kernel per active prior, prior_assemble_kernel per (pose with priors, entry) adding the pose's sums onto
 // the diagonal block and g after the factors; run only while a prior is active.
+// Robust losses (DESIGN.md "Robust pose factors"): with s = e~^T H~ e~ a term's cost becomes 1/2 rho(s), its b rho'(s) b
+// and its M rho'(s) M (IRLS). Factors and priors each own one TermLoss, the loss core: the per-term arrays, the robust
+// flag, their bytes, the readout and the evaluation order. The <FactorLoss> instantiations of the cost kernels (write s
+// and w = rho'(s)) and the linearisations (scale M and b by w) run only when an active term has a non-trivial loss; the
+// <NoLoss> ones are the kernels without a loss.
 #include <math.h>
 #include <type_traits>
 #include <algorithm>
@@ -156,12 +157,24 @@ __device__ __forceinline__ void factor_residuals(const FactorView &fv, int f, co
   __syncthreads();
 }
 
-struct NoLoss {};      // the pure quadratic: kernels exactly as without robust losses
-struct FactorLoss {   // per factor: kind (BALM_LOSS_*), scale c, outputs s_f and w_f = rho'(s_f)
-  const int *kind;    // null: every factor trivial
-  const double *scale;
-  double *s, *w;
+struct FactorLoss {   // per term (factor or prior): kind (BALM_LOSS_*), scale c, outputs s and w = rho'(s)
+  int *kind;          // null: every term trivial
+  double *scale, *s, *w;
 };
+
+// A term's cost from its s, index q of the loss arrays: with FactorLoss 1/2 rho(s), and s, w = rho'(s) to the loss's
+// outputs; with NoLoss 1/2 s
+template <typename Loss>
+__device__ __forceinline__ double term_cost(const Loss &loss, int q, double s) {
+  if constexpr (std::is_same<Loss, FactorLoss>::value) {
+    double rho, drho;
+    loss_rho(loss.kind ? loss.kind[q] : BALM_LOSS_TRIVIAL, loss.kind ? loss.scale[q] : 1.0, s, &rho, &drho);
+    loss.s[q] = s;
+    loss.w[q] = drho;
+    s = rho;
+  }
+  return 0.5 * s;
+}
 
 // ---- per active factor: M (6N x 6N, column-major, at the factor's H offset) and b (6 per slot); with FactorLoss both
 // scaled by w_f, which the cost pass before has written ----
@@ -314,14 +327,7 @@ __global__ void __launch_bounds__(PG_THREADS) pg_cost_kernel(FactorView fv, cons
   if (tid == 0) {
     double s = 0.0;
     for (int q = 0; q < PG_THREADS / 32; q++) s += red[q];
-    if constexpr (std::is_same<Loss, FactorLoss>::value) {
-      double rho, drho;
-      loss_rho(loss.kind ? loss.kind[f] : BALM_LOSS_TRIVIAL, loss.kind ? loss.scale[f] : 1.0, s, &rho, &drho);
-      loss.s[f] = s;
-      loss.w[f] = drho;
-      s = rho;
-    }
-    cost_part[blockIdx.x] = 0.5 * s;
+    cost_part[blockIdx.x] = term_cost(loss, f, s);
   }
 }
 
@@ -405,14 +411,7 @@ __global__ void __launch_bounds__(PG_THREADS) prior_cost_kernel(PriorView pv, co
     for (int c = 0; c < 6; c++) t += Hq[6 * c + r] * e[c];
     s += e[r] * t;
   }
-  if constexpr (std::is_same<Loss, FactorLoss>::value) {
-    double rho, drho;
-    loss_rho(loss.kind ? loss.kind[q] : BALM_LOSS_TRIVIAL, loss.kind ? loss.scale[q] : 1.0, s, &rho, &drho);
-    loss.s[q] = s;
-    loss.w[q] = drho;
-    s = rho;
-  }
-  cost_part[k] = 0.5 * s;
+  cost_part[k] = term_cost(loss, q, s);
 }
 
 // ---- per active prior k: M[k] = w J^T H J (36, column-major) and b[k] = w J^T H e; with FactorLoss w is the w_q that
@@ -499,6 +498,82 @@ __global__ void prior_add_cost_kernel(const double *x, double *y) { *y += *x; }
 
 }  // namespace
 
+constexpr long long LOSS_BYTES_PER_FACTOR = sizeof(int) + 3 * sizeof(double);
+
+// Launches `launch` with the loss argument of a cost pass or a linearisation: *l (robust mode, or a readout), or NoLoss
+// when l is null.
+template <typename Launch>
+static void with_loss(const FactorLoss *l, Launch launch) {
+  if (l) launch(*l);
+  else launch(NoLoss{});
+}
+
+// The loss core of a term set (balm_set_factor_loss's factors, balm_set_pose_priors' priors; DESIGN.md "Robust pose
+// factors"): kind, scale, s and w per term on the device, allocated only while some term's kind is non-trivial.
+struct TermLoss {
+  FactorLoss arr{};     // all null without arrays: every term trivial
+  bool robust = false;  // an active term has a non-trivial kind
+  long long bytes = 0;  // device memory the arrays hold: LOSS_BYTES_PER_FACTOR per term
+  ~TermLoss() { release(); }
+  void release() {
+    cudaFree(arr.kind); cudaFree(arr.scale); cudaFree(arr.s); cudaFree(arr.w);
+    arr = FactorLoss{};
+    robust = false;
+    bytes = 0;
+  }
+  // The loss argument of the cost pass and the linearisation: the arrays in robust mode, else null (NoLoss). With
+  // arrays an evaluation runs the cost pass first, so that the linearisation can weight M and b with its w and the
+  // evaluation's cost is its sum; without, the cost pass runs after the assembly.
+  const FactorLoss *active() const { return robust ? &arr : nullptr; }
+
+  // kind [n] (null: every term trivial) and scale [n] of the n terms, `act` the active ones. Every term trivial frees
+  // the arrays; else they are allocated when absent (a failed allocation leaves every term trivial) and uploaded with
+  // s = w = 0. Waits for the upload.
+  int set(cudaStream_t st, int n, const int32_t *kind, const double *scale, const std::vector<int> &act) {
+    if (!kind || std::all_of(kind, kind + n, [](int32_t k) { return k == BALM_LOSS_TRIVIAL; })) {
+      release();  // no arrays: the kernels without a loss
+      return BALM_OK;
+    }
+    if (!arr.kind) {
+      if (dev_alloc(&arr.kind, n) != BALM_OK || dev_alloc(&arr.scale, n) != BALM_OK ||
+          dev_alloc(&arr.s, n) != BALM_OK || dev_alloc(&arr.w, n) != BALM_OK) {
+        release();
+        return BALM_ERR_CUDA;
+      }
+      bytes = LOSS_BYTES_PER_FACTOR * n;
+    }
+    std::vector<double> c(n);
+    bool any_active = false;
+    for (int q = 0; q < n; q++) c[q] = kind[q] == BALM_LOSS_TRIVIAL ? 1.0 : scale[q];  // a trivial term's c is unused
+    for (int q : act) any_active = any_active || kind[q] != BALM_LOSS_TRIVIAL;
+    CUDA_TRY(cudaMemcpyAsync(arr.kind, kind, sizeof(int) * n, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(arr.scale, c.data(), sizeof(double) * n, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemsetAsync(arr.s, 0, sizeof(double) * n, st));  // inactive terms keep s = w = 0
+    CUDA_TRY(cudaMemsetAsync(arr.w, 0, sizeof(double) * n, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    robust = any_active;
+    return BALM_OK;
+  }
+
+  // balm_factor_residuals / balm_prior_residuals over n terms: `cost_pass` with the arrays, or with temporary s and w
+  // when no loss is set (every term trivial), then s and w to the host arrays (either may be null); waits once
+  template <typename Pass>
+  int readout(size_t n, cudaStream_t st, double *s, double *w, Pass cost_pass) const {
+    double *tmp = nullptr;
+    if (!arr.kind) {
+      TRY(dev_alloc(&tmp, 2 * n));
+      CUDA_TRY(cudaMemsetAsync(tmp, 0, sizeof(double) * 2 * n, st));
+    }
+    std::unique_ptr<double, cudaError_t (*)(void *)> tmp_own(tmp, cudaFree);
+    const FactorLoss loss = tmp ? FactorLoss{nullptr, nullptr, tmp, tmp + n} : arr;
+    TRY(cost_pass(&loss));
+    if (s) CUDA_TRY(cudaMemcpyAsync(s, loss.s, sizeof(double) * n, cudaMemcpyDeviceToHost, st));
+    if (w) CUDA_TRY(cudaMemcpyAsync(w, loss.w, sizeof(double) * n, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    return BALM_OK;
+  }
+};
+
 // The registered factor set (device). Factor f owns slots [fptr[f], fptr[f+1]) and the (6N_f)^2 doubles at hoff[f] of
 // H and of the staging M.
 struct PoseGraph {
@@ -509,29 +584,17 @@ struct PoseGraph {
   int2 *pair = nullptr;
   int3 *term = nullptr;
   double *hat = nullptr, *H = nullptr, *M = nullptr, *b = nullptr, *cost_part = nullptr;
-  // balm_set_factor_loss: [F] kind, scale, s, w; allocated only while some factor's kind is non-trivial
-  int *loss_kind = nullptr;
-  double *loss_scale = nullptr, *loss_s = nullptr, *loss_w = nullptr;
-  bool robust = false;       // an active factor has a non-trivial kind
+  TermLoss loss;             // balm_set_factor_loss
   std::vector<int2> pair_h;  // host copy of `pair`
   std::vector<int> act_h;    // host copy of `act`
-  long long bytes = 0;       // device memory held
+  long long bytes = 0;       // device memory held, the loss arrays' aside
   ~PoseGraph() {
     cudaFree(fptr); cudaFree(hoff); cudaFree(gp_slot); cudaFree(pose); cudaFree(act); cudaFree(pair_ptr);
     cudaFree(gp_ptr); cudaFree(status); cudaFree(pair); cudaFree(term); cudaFree(hat); cudaFree(H); cudaFree(M);
     cudaFree(b); cudaFree(cost_part);
-    free_loss();
-  }
-  void free_loss() {
-    cudaFree(loss_kind); cudaFree(loss_scale); cudaFree(loss_s); cudaFree(loss_w);
-    loss_kind = nullptr;
-    loss_scale = loss_s = loss_w = nullptr;
   }
   FactorView view() const { return FactorView{fptr, hoff, pose, hat, H}; }
-  FactorLoss loss() const { return FactorLoss{loss_kind, loss_scale, loss_s, loss_w}; }
 };
-
-constexpr long long LOSS_BYTES_PER_FACTOR = sizeof(int) + 3 * sizeof(double);
 
 void pose_graph_free(PoseGraph *p) { delete p; }
 
@@ -635,56 +698,21 @@ int pose_graph_build(cudaStream_t st, int P, int n_factors, const int64_t *facto
   return BALM_OK;
 }
 
-int pose_graph_set(balm_ctx *c, int n_factors, const int64_t *factor_ptr, const int32_t *factor_pose,
-                   const double *poses_hat12, const double *H, int32_t *status_out) {
-  PoseGraph *p = nullptr;
-  std::vector<int> status;
-  TRY(pose_graph_build(c->stream, c->N, n_factors, factor_ptr, factor_pose, poses_hat12, H, &status, &p, &c->launches));
-  if (status_out) std::copy(status.begin(), status.end(), status_out);
-  pose_graph_free(c->pg);
-  c->pg = p;
-  return BALM_OK;
-}
-
 const std::vector<int2> &pose_graph_pairs(const PoseGraph *p) { return p->pair_h; }
-long long pose_graph_bytes(const PoseGraph *p) { return p->bytes; }
+long long pose_graph_bytes(const PoseGraph *p) { return p->bytes + p->loss.bytes; }
 int pose_graph_n_factors(const PoseGraph *p) { return p->F; }
 
 int pose_graph_set_loss(PoseGraph *p, cudaStream_t st, const int32_t *kind, const double *scale) {
-  const int F = p->F;
-  const bool any = kind && std::any_of(kind, kind + F, [](int32_t k) { return k != BALM_LOSS_TRIVIAL; });
-  if (!any) {  // every factor trivial: no arrays, the kernels without a loss
-    if (p->loss_kind) p->bytes -= LOSS_BYTES_PER_FACTOR * F;
-    p->free_loss();
-    p->robust = false;
-    return BALM_OK;
-  }
-  if (!p->loss_kind) {
-    if (dev_alloc(&p->loss_kind, F) != BALM_OK || dev_alloc(&p->loss_scale, F) != BALM_OK ||
-        dev_alloc(&p->loss_s, F) != BALM_OK || dev_alloc(&p->loss_w, F) != BALM_OK) {
-      p->free_loss();  // still no loss: every factor trivial
-      return BALM_ERR_CUDA;
-    }
-    p->bytes += LOSS_BYTES_PER_FACTOR * F;
-  }
-  std::vector<double> c(F);
-  bool robust = false;
-  for (int f = 0; f < F; f++) c[f] = kind[f] == BALM_LOSS_TRIVIAL ? 1.0 : scale[f];  // a trivial factor's scale is unused
-  for (int f : p->act_h) robust = robust || kind[f] != BALM_LOSS_TRIVIAL;
-  CUDA_TRY(cudaMemcpyAsync(p->loss_kind, kind, sizeof(int) * F, cudaMemcpyHostToDevice, st));
-  CUDA_TRY(cudaMemcpyAsync(p->loss_scale, c.data(), sizeof(double) * F, cudaMemcpyHostToDevice, st));
-  CUDA_TRY(cudaMemsetAsync(p->loss_s, 0, sizeof(double) * F, st));  // inactive factors keep s = w = 0
-  CUDA_TRY(cudaMemsetAsync(p->loss_w, 0, sizeof(double) * F, st));
-  CUDA_TRY(cudaStreamSynchronize(st));
-  p->robust = robust;
-  return BALM_OK;
+  return p->loss.set(st, p->F, kind, scale, p->act_h);
 }
 
-// the robust cost pass into cost_part and the loss outputs
-static int robust_cost_pass(const PoseGraph &p, cudaStream_t st, const double *poses, const FactorLoss &loss,
-                            long long *launches) {
+// the cost pass into cost_part, and with a loss argument into its s and w
+static int pg_cost_pass(const PoseGraph &p, cudaStream_t st, const double *poses, const FactorLoss *l,
+                        long long *launches) {
   if (!p.n_act) return BALM_OK;
-  pg_cost_kernel<<<p.n_act, PG_THREADS, 0, st>>>(p.view(), p.act, poses, p.cost_part, loss);
+  with_loss(l, [&](auto loss) {
+    pg_cost_kernel<<<p.n_act, PG_THREADS, 0, st>>>(p.view(), p.act, poses, p.cost_part, loss);
+  });
   *launches += 1;
   CUDA_TRY(cudaGetLastError());
   return BALM_OK;
@@ -698,54 +726,33 @@ static int sum_pass(const PoseGraph &p, cudaStream_t st, double *out, long long 
 }
 
 int pose_graph_cost(const PoseGraph *pg, cudaStream_t st, const double *poses, double *out, long long *launches) {
-  const PoseGraph &p = *pg;
-  if (p.robust) {
-    TRY(robust_cost_pass(p, st, poses, p.loss(), launches));
-    return sum_pass(p, st, out, launches);
-  }
-  if (p.n_act) pg_cost_kernel<<<p.n_act, PG_THREADS, 0, st>>>(p.view(), p.act, poses, p.cost_part, NoLoss{});
-  pg_sum_kernel<<<1, PG_THREADS, 0, st>>>(p.cost_part, p.n_act, out);
-  *launches += p.n_act ? 2 : 1;
-  CUDA_TRY(cudaGetLastError());
-  return BALM_OK;
+  TRY(pg_cost_pass(*pg, st, poses, pg->loss.active(), launches));
+  return sum_pass(*pg, st, out, launches);
 }
 
-int pose_graph_residuals(const PoseGraph *pg, cudaStream_t st, const double *poses, double *s, double *w,
-                         long long *launches) {
-  const PoseGraph &p = *pg;
-  const size_t F = (size_t)p.F;
-  double *tmp = nullptr;  // without a loss: s and w of one call
-  if (!p.loss_kind) {
-    TRY(dev_alloc(&tmp, 2 * F));
-    CUDA_TRY(cudaMemsetAsync(tmp, 0, sizeof(double) * 2 * F, st));
-  }
-  std::unique_ptr<double, cudaError_t (*)(void *)> tmp_own(tmp, cudaFree);
-  const FactorLoss loss = tmp ? FactorLoss{nullptr, nullptr, tmp, tmp + F} : p.loss();
-  TRY(robust_cost_pass(p, st, poses, loss, launches));
-  if (s) CUDA_TRY(cudaMemcpyAsync(s, loss.s, sizeof(double) * F, cudaMemcpyDeviceToHost, st));
-  if (w) CUDA_TRY(cudaMemcpyAsync(w, loss.w, sizeof(double) * F, cudaMemcpyDeviceToHost, st));
-  CUDA_TRY(cudaStreamSynchronize(st));
-  return BALM_OK;
+int term_residuals(const PoseGraph *p, cudaStream_t st, const double *poses, double *s, double *w,
+                   long long *launches) {
+  return p->loss.readout((size_t)p->F, st, s, w,
+                         [&](const FactorLoss *l) { return pg_cost_pass(*p, st, poses, l, launches); });
 }
 
-// H (through `out`), g and the cost at poses. With a loss the cost pass runs first, so that the linearisation can weight
-// M and b, and the evaluation's cost is its sum; without one, today's order.
+// H (through `out`), g and the cost at poses, the cost pass placed by TermLoss::active
 template <typename Out>
 static int pose_graph_assemble(const PoseGraph &p, cudaStream_t st, const double *poses, Out out, double *g,
                                double *cost, long long *launches) {
-  if (p.robust) {
-    TRY(robust_cost_pass(p, st, poses, p.loss(), launches));
-    if (p.n_act) pg_linearise_kernel<<<p.n_act, PG_THREADS, 0, st>>>(p.view(), p.act, poses, p.M, p.b, p.loss());
-  } else if (p.n_act) {
-    pg_linearise_kernel<<<p.n_act, PG_THREADS, 0, st>>>(p.view(), p.act, poses, p.M, p.b, NoLoss{});
-  }
+  const FactorLoss *l = p.loss.active();
+  if (l) TRY(pg_cost_pass(p, st, poses, l, launches));
+  if (p.n_act)
+    with_loss(l, [&](auto loss) {
+      pg_linearise_kernel<<<p.n_act, PG_THREADS, 0, st>>>(p.view(), p.act, poses, p.M, p.b, loss);
+    });
   const long long threads = 36 * p.n_pairs + 6 * (long long)p.P;
   pg_assemble_kernel<<<(unsigned)((threads + PG_THREADS - 1) / PG_THREADS), PG_THREADS, 0, st>>>(
       p.fptr, p.hoff, p.pair, p.pair_ptr, p.term, p.n_pairs, p.M, p.gp_ptr, p.gp_slot, p.b, p.P, out, g);
   *launches += p.n_act ? 2 : 1;
   CUDA_TRY(cudaGetLastError());
-  if (p.robust) return sum_pass(p, st, cost, launches);
-  return pose_graph_cost(&p, st, poses, cost, launches);
+  if (!l) TRY(pg_cost_pass(p, st, poses, l, launches));
+  return sum_pass(p, st, cost, launches);
 }
 
 int pose_graph_eval(balm_ctx *c, const double *poses) {
@@ -776,23 +783,18 @@ struct PriorSet {
   int *pose = nullptr, *act = nullptr, *upose = nullptr, *uptr = nullptr, *diag = nullptr;
   double *hat = nullptr, *lever = nullptr, *H = nullptr, *M = nullptr, *b = nullptr, *cost_part = nullptr,
          *cost = nullptr;
-  // [n] kind, scale, s, w; allocated only while some prior's kind is non-trivial
-  int *loss_kind = nullptr;
-  double *loss_scale = nullptr, *loss_s = nullptr, *loss_w = nullptr;
-  bool robust = false;  // an active prior has a non-trivial kind
+  TermLoss loss;  // the priors' kind and scale
   std::vector<int> upose_h;
   long long bytes = 0, diag_bytes = 0;
   ~PriorSet() {
     cudaFree(pose); cudaFree(act); cudaFree(upose); cudaFree(uptr); cudaFree(diag); cudaFree(hat); cudaFree(lever);
     cudaFree(H); cudaFree(M); cudaFree(b); cudaFree(cost_part); cudaFree(cost);
-    cudaFree(loss_kind); cudaFree(loss_scale); cudaFree(loss_s); cudaFree(loss_w);
   }
   PriorView view() const { return PriorView{pose, hat, lever, H}; }
-  FactorLoss loss() const { return FactorLoss{loss_kind, loss_scale, loss_s, loss_w}; }
 };
 
 void prior_set_free(PriorSet *p) { delete p; }
-long long prior_set_bytes(const PriorSet *p) { return p->bytes + p->diag_bytes; }
+long long prior_set_bytes(const PriorSet *p) { return p->bytes + p->diag_bytes + p->loss.bytes; }
 bool prior_set_active(const PriorSet *p) { return p && p->n_act > 0; }
 const std::vector<int> &prior_set_poses(const PriorSet *p) { return p->upose_h; }
 
@@ -863,19 +865,7 @@ int prior_set_build(cudaStream_t st, int n, const int32_t *pose, const double *h
   p->bytes = (long long)(sizeof(int) * (nz(n) + nz(act.size()) + nz(p->upose_h.size()) + uptr.size()) +
                          sizeof(double) * (nz(12 * (size_t)n) + nz(3 * (size_t)n) + nz(36 * (size_t)n) +
                                            nz(36 * act.size()) + nz(6 * act.size()) + nz(act.size()) + 1));
-  const bool any = kind && std::any_of(kind, kind + n, [](int32_t k) { return k != BALM_LOSS_TRIVIAL; });
-  if (any) {
-    std::vector<double> c(n);
-    for (int q = 0; q < n; q++) c[q] = kind[q] == BALM_LOSS_TRIVIAL ? 1.0 : scale[q];  // a trivial prior's scale is unused
-    for (int q : act) p->robust = p->robust || kind[q] != BALM_LOSS_TRIVIAL;
-    TRY(upload(&p->loss_kind, kind, (size_t)n, st));
-    TRY(upload(&p->loss_scale, c.data(), (size_t)n, st));
-    TRY(dev_alloc(&p->loss_s, (size_t)n));
-    TRY(dev_alloc(&p->loss_w, (size_t)n));
-    CUDA_TRY(cudaMemsetAsync(p->loss_s, 0, sizeof(double) * n, st));  // inactive priors keep s = w = 0
-    CUDA_TRY(cudaMemsetAsync(p->loss_w, 0, sizeof(double) * n, st));
-    p->bytes += LOSS_BYTES_PER_FACTOR * n;
-  }
+  TRY(p->loss.set(st, n, kind, scale, act));
   CUDA_TRY(cudaStreamSynchronize(st));
   *status_out = std::move(status);
   *out = p.release();
@@ -903,12 +893,14 @@ int prior_set_map(PriorSet *p, cudaStream_t st, const std::vector<int2> &pairs) 
   return BALM_OK;
 }
 
-static int prior_cost_pass(const PriorSet &p, cudaStream_t st, const double *poses, const FactorLoss *loss,
+// the priors' cost pass into cost_part, and with a loss argument into its s and w
+static int prior_cost_pass(const PriorSet &p, cudaStream_t st, const double *poses, const FactorLoss *l,
                            long long *launches) {
   if (!p.n_act) return BALM_OK;
   const unsigned grid = (unsigned)((p.n_act + PG_THREADS - 1) / PG_THREADS);
-  if (loss) prior_cost_kernel<<<grid, PG_THREADS, 0, st>>>(p.view(), p.act, p.n_act, poses, p.cost_part, *loss);
-  else prior_cost_kernel<<<grid, PG_THREADS, 0, st>>>(p.view(), p.act, p.n_act, poses, p.cost_part, NoLoss{});
+  with_loss(l, [&](auto loss) {
+    prior_cost_kernel<<<grid, PG_THREADS, 0, st>>>(p.view(), p.act, p.n_act, poses, p.cost_part, loss);
+  });
   *launches += 1;
   CUDA_TRY(cudaGetLastError());
   return BALM_OK;
@@ -923,52 +915,35 @@ static int prior_sum_add(const PriorSet &p, cudaStream_t st, double *cost, long 
   return BALM_OK;
 }
 
-int prior_add_cost(const PriorSet *pr, cudaStream_t st, const double *poses, double *cost, long long *launches) {
-  const PriorSet &p = *pr;
-  if (!p.n_act) return BALM_OK;
-  const FactorLoss l = p.loss();
-  TRY(prior_cost_pass(p, st, poses, p.robust ? &l : nullptr, launches));
-  return prior_sum_add(p, st, cost, launches);
+int prior_add_cost(const PriorSet *p, cudaStream_t st, const double *poses, double *cost, long long *launches) {
+  if (!p->n_act) return BALM_OK;
+  TRY(prior_cost_pass(*p, st, poses, p->loss.active(), launches));
+  return prior_sum_add(*p, st, cost, launches);
 }
 
-int prior_residuals(const PriorSet *pr, cudaStream_t st, const double *poses, double *s, double *w,
-                    long long *launches) {
-  const PriorSet &p = *pr;
-  const size_t n = (size_t)p.n;
-  double *tmp = nullptr;  // without a loss: s and w of one call
-  if (!p.loss_kind) {
-    TRY(dev_alloc(&tmp, 2 * n));
-    CUDA_TRY(cudaMemsetAsync(tmp, 0, sizeof(double) * 2 * n, st));
-  }
-  std::unique_ptr<double, cudaError_t (*)(void *)> tmp_own(tmp, cudaFree);
-  const FactorLoss loss = tmp ? FactorLoss{nullptr, nullptr, tmp, tmp + n} : p.loss();
-  TRY(prior_cost_pass(p, st, poses, &loss, launches));
-  if (s && n) CUDA_TRY(cudaMemcpyAsync(s, loss.s, sizeof(double) * n, cudaMemcpyDeviceToHost, st));
-  if (w && n) CUDA_TRY(cudaMemcpyAsync(w, loss.w, sizeof(double) * n, cudaMemcpyDeviceToHost, st));
-  CUDA_TRY(cudaStreamSynchronize(st));
-  return BALM_OK;
+int term_residuals(const PriorSet *p, cudaStream_t st, const double *poses, double *s, double *w,
+                   long long *launches) {
+  return p->loss.readout((size_t)p->n, st, s, w,
+                         [&](const FactorLoss *l) { return prior_cost_pass(*p, st, poses, l, launches); });
 }
 
-// the priors' M and b onto H (through `out`) and g, their cost onto *cost; with a loss the cost pass runs first so that
-// the linearisation can weight M and b
+// the priors' M and b onto H (through `out`) and g, their cost onto *cost, the cost pass placed by TermLoss::active
 template <typename Out>
 static int prior_assemble(const PriorSet &p, cudaStream_t st, const double *poses, Out out, double *g, double *cost,
                           long long *launches) {
   if (!p.n_act) return BALM_OK;
+  const FactorLoss *l = p.loss.active();
+  if (l) TRY(prior_cost_pass(p, st, poses, l, launches));
   const unsigned grid = (unsigned)((p.n_act + PG_THREADS - 1) / PG_THREADS);
-  if (p.robust) {
-    const FactorLoss l = p.loss();
-    TRY(prior_cost_pass(p, st, poses, &l, launches));
-    prior_linearise_kernel<<<grid, PG_THREADS, 0, st>>>(p.view(), p.act, p.n_act, poses, p.M, p.b, l);
-  } else {
-    prior_linearise_kernel<<<grid, PG_THREADS, 0, st>>>(p.view(), p.act, p.n_act, poses, p.M, p.b, NoLoss{});
-  }
+  with_loss(l, [&](auto loss) {
+    prior_linearise_kernel<<<grid, PG_THREADS, 0, st>>>(p.view(), p.act, p.n_act, poses, p.M, p.b, loss);
+  });
   const long long threads = 42LL * p.n_u;
   prior_assemble_kernel<<<(unsigned)((threads + PG_THREADS - 1) / PG_THREADS), PG_THREADS, 0, st>>>(
       p.upose, p.uptr, p.n_u, p.M, p.b, out, g);
   *launches += 2;
   CUDA_TRY(cudaGetLastError());
-  if (!p.robust) TRY(prior_cost_pass(p, st, poses, nullptr, launches));
+  if (!l) TRY(prior_cost_pass(p, st, poses, l, launches));
   return prior_sum_add(p, st, cost, launches);
 }
 
