@@ -908,12 +908,9 @@ static int collect_solve(balm_ctx *c, const DenseSystem &sys, SparseSolver *sp, 
   *refined = 0;
   if (c->h_flags[4] == 0 || *not_pd) return BALM_OK;
   int still_bad = 0;
-  if (sp) {
-    TRY(sparse_refine(sp, c->stream, c->h_flags, c->h_scal, &still_bad));
-    c->tm.refinements += 1;
-  } else {
-    TRY(refine_solution(c, sys, &still_bad));
-  }
+  if (sp) TRY(sparse_refine(sp, c->stream, c->h_flags, c->h_scal, &still_bad));
+  else TRY(refine_solution(c, sys, &still_bad));
+  c->tm.refinements += 1;  // once per refined solve, however many rounds it took
   *q1 = c->h_scal[1];
   *refined = 1;
   if (still_bad || !std::isfinite(*q1)) *not_pd = 1;
@@ -955,6 +952,47 @@ extern "C" int balm_solve(balm_ctx *c, double u, double *dx, double *q1, int *no
   CUDA_TRY(cudaStreamSynchronize(c->stream));
   TRY(collect_solve(c, sys, sp, &q, &bad, &refined));
   if (dx) CUDA_TRY(cudaMemcpy(dx, c->dx, sizeof(double) * c->n, cudaMemcpyDeviceToHost));
+  if (q1) *q1 = q;
+  if (not_pd) *not_pd = bad;
+  return BALM_OK;
+}
+
+// Debug aid (include/balm_b200.h): balm_solve's path on a caller-supplied H and g, in scratch buffers of its own
+extern "C" int balm_debug_ldlt(balm_ctx *c, const double *H, const double *g, double u, double *dx, double *q1,
+                               int *not_pd, double *LD, double *omega) {
+  if (!c || !H || !g) { balm_set_error("balm_debug_ldlt: bad arguments"); return BALM_ERR_INVALID; }
+  if (c->prec == BALM_PREC_BLOCKS) {
+    balm_set_error("balm_debug_ldlt: not available on a BALM_PREC_BLOCKS context (its solve is the sparse one)");
+    return BALM_ERR_INVALID;
+  }
+  CUDA_TRY(cudaSetDevice(c->device));
+  const int n = c->n;
+  const size_t nn = (size_t)n * n;
+  ScratchPool pool;
+  struct WorkGuard {
+    LdltWork w;
+    ~WorkGuard() { ldlt_work_free(&w); }
+  } wg;
+  double *d_H, *d_g, *d_dx, *d_dvec, *d_A;
+  TRY(pool.get(&d_H, nn));
+  TRY(pool.get(&d_g, (size_t)n));
+  TRY(pool.get(&d_dx, (size_t)n));
+  TRY(pool.get(&d_dvec, (size_t)n));
+  TRY(pool.get(&d_A, nn));
+  const DenseSystem sys{n, d_H, d_g, d_dx, d_dvec, d_A, &wg.w};
+  CUDA_TRY(cudaMemcpyAsync(d_H, H, sizeof(double) * nn, cudaMemcpyHostToDevice, c->stream));
+  CUDA_TRY(cudaMemcpyAsync(d_g, g, sizeof(double) * n, cudaMemcpyHostToDevice, c->stream));
+  double q = 0;
+  int bad = 0, refined = 0;
+  TRY(solve_dev(c, sys, nullptr, u));
+  CUDA_TRY(cudaStreamSynchronize(c->stream));
+  TRY(collect_solve(c, sys, nullptr, &q, &bad, &refined));
+  if (dx) CUDA_TRY(cudaMemcpy(dx, d_dx, sizeof(double) * n, cudaMemcpyDeviceToHost));
+  if (omega) CUDA_TRY(cudaMemcpy(omega, c->scal + 20, sizeof(double), cudaMemcpyDeviceToHost));
+  if (LD) {  // the factorisation writes the lower triangle only: the upper one still holds H + u diag(H)
+    CUDA_TRY(cudaMemcpy(LD, d_A, sizeof(double) * nn, cudaMemcpyDeviceToHost));
+    for (int j = 1; j < n; j++) memset(LD + (size_t)j * n, 0, sizeof(double) * j);
+  }
   if (q1) *q1 = q;
   if (not_pd) *not_pd = bad;
   return BALM_OK;

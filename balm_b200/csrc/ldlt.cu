@@ -775,7 +775,6 @@ int refine_solution(balm_ctx *c, const DenseSystem &s, int *still_bad) {
     CUDA_TRY(cudaMemcpyAsync(c->h_flags + 4, c->flags + 4, sizeof(int), cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaMemcpyAsync(c->h_scal + 1, c->scal + 1, sizeof(double), cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
-    c->tm.refinements += 1;
     if (c->h_flags[4] == 0) { *still_bad = 0; break; }
   }
   return BALM_OK;

@@ -745,6 +745,16 @@ int balm_timer_end(balm_ctx *ctx, float *ms);
 /* Debug aid: with BALM_DAG_TRACE=1 in the environment, device timestamps (ns) of the last factorisation: 4 per 64-column
  * step of the chain, then 3 per CTA (start, end, tasks executed). */
 int balm_debug_dag_trace(balm_ctx *ctx, unsigned long long *out, int max_entries);
+/* Debug aid: the dense damped solve of balm_solve(u) -- tile-DAG LDL^T, backward substitution, q1, the backward-error
+ * check, fp64 refinement, the not_pd rule and the timings counters -- on a caller-supplied system, so that it can be
+ * compared bit for bit with an exact reference. H is n x n column-major and symmetric and g has length n, n = 6N of
+ * ctx; both are copied to scratch buffers, which (with the factor workspaces) the call allocates and frees. It neither
+ * needs nor touches a registration, an evaluation or the context's H, g and factors. dx, q1 and not_pd mean what they
+ * mean in balm_solve. LD (may be NULL) receives the n x n column-major factor: L strictly below the diagonal, d on it,
+ * zeros above. omega (may be NULL) receives the componentwise backward error of the final check. BALM_ERR_INVALID on a
+ * BALM_PREC_BLOCKS context or for a NULL H or g. */
+int balm_debug_ldlt(balm_ctx *ctx, const double *H, const double *g, double u, double *dx, double *q1, int *not_pd,
+                    double *LD, double *omega);
 /* Debug aid: with BALM_TC_TRACE=1 in the environment when a tensor-precision ctx is created, the last tensor SYRK launch
  * (of an evaluation or of balm_debug_syrk_tc) records clock64 sums per role, 18 words per CTA, CTA b at 18 b (CTAs
  * beyond the launch's grid hold zeros):
