@@ -49,7 +49,7 @@ SYMBOLS = ["balm_last_error", "balm_version", "balm_create", "balm_destroy", "ba
            "balm_default_lm_opts", "balm_comm_unique_id", "balm_comm_init", "balm_get_timings", "balm_get_reused_sweeps",
            "balm_reset_counters", "balm_sync", "balm_timer_begin", "balm_timer_end", "balm_device_views", "balm_debug_dag_trace",
            "balm_debug_ldlt", "balm_debug_syrk_tc", "balm_debug_tc_planes", "balm_debug_tc_trace", "balm_debug_tc_copy_trace", "balm_synth_virtual",
-           "balm_download_voxels", "balm_download_voxel_range", "balm_num_obs", "balm_default_assoc_opts", "balm_cut_voxels", "balm_pose_covariance", "balm_marginalize", "balm_download_fix", "balm_append_scan",
+           "balm_download_voxels", "balm_download_voxel_range", "balm_num_obs", "balm_default_assoc_opts", "balm_cut_voxels", "balm_cut_voxels_stats", "balm_pose_covariance", "balm_marginalize", "balm_download_fix", "balm_append_scan",
            "balm_download_keys", "balm_window_reset", "balm_window_cut", "balm_window_recut", "balm_window_marginalize",
            "balm_window_push", "balm_batch_create", "balm_batch_destroy", "balm_batch_set_voxels", "balm_batch_evaluate",
            "balm_batch_damping_iter", "balm_batch_cut_voxels", "balm_batch_sizes", "balm_batch_download_voxels",
@@ -112,6 +112,7 @@ def lib():
         L.balm_default_assoc_opts.argtypes = [C.POINTER(AssocOpts)]
         L.balm_cut_voxels.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(AssocOpts),
                                       C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
+        L.balm_cut_voxels_stats.argtypes = [C.c_void_p, C.c_void_p]
         L.balm_pose_covariance.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_double, C.c_int, C.c_void_p, C.c_void_p]
         L.balm_marginalize.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
         L.balm_download_fix.argtypes = [C.c_void_p, C.c_void_p]

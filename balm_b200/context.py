@@ -214,6 +214,18 @@ class Context:
         self.M = M.value
         return M.value, K.value
 
+    def cut_stats(self):
+        """The last successful cut_voxels: slabs (1 in one pass), the points of the largest slab, root voxels, peak
+        device scratch bytes, host-to-device bytes, the scratch bound's bytes per point and fixed bytes, and the wall
+        times (ms) of the root-count pass, the slab selection, the cuts and the registration."""
+        st = np.zeros(11, dtype=np.int64)
+        L.check(L.lib().balm_cut_voxels_stats(self._h, _p(st)))
+        keys = ("slabs", "max_slab_points", "roots", "peak_scratch_bytes", "h2d_bytes", "scratch_per_point",
+                "scratch_fixed")
+        out = {k: int(v) for k, v in zip(keys, st)}
+        out.update({k: st[7 + i] / 1e3 for i, k in enumerate(("ms_roots", "ms_select", "ms_cut", "ms_register"))})
+        return out
+
     def download_voxels(self):
         K = L.lib().balm_num_obs(self._h)
         row_ptr = np.zeros(self.M + 1, dtype=np.int64)

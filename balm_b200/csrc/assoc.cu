@@ -21,7 +21,9 @@
 // slot) segment is summed in the order a context holding only that problem would sum it, so each problem's voxels are
 // bitwise those of balm_cut_voxels on its own points. One problem with rows = frames is balm_cut_voxels itself.
 #include <cub/cub.cuh>
+#include <string.h>
 #include <algorithm>
+#include <chrono>
 #include <vector>
 #include "internal.cuh"
 
@@ -298,6 +300,13 @@ __global__ void emit_kernel(const int *ref, const int *obs_start, int nleaf, Emi
   }
 }
 
+// bad: bit 2 = a frame index outside [0, n_rows), bit 1 = a point outside the root range (item_key_kernel)
+int bad_points_error(const char *who, int bad) {
+  balm_set_error(std::string(who) + (bad & 2 ? ": frame index outside [0, n_poses)"
+                                             : ": a point lies outside the +-2^18 root-voxel range"));
+  return BALM_ERR_INVALID;
+}
+
 }  // namespace
 
 int assoc_cut(cudaStream_t st, const AssocInput &in, const balm_assoc_opts &o, const AssocRegister &reg,
@@ -305,12 +314,14 @@ int assoc_cut(cudaStream_t st, const AssocInput &in, const balm_assoc_opts &o, c
   const bool one = in.frame != nullptr;  // balm_cut_voxels: one problem, rows = frames
   const int B = one ? 1 : in.n_problems, n_rows = one ? in.n_rows : (int)in.pose_ptr[in.n_problems];
   const int64_t n = one ? in.n_points : in.n_items;
-  ScratchPool pool;
+  ScratchPool pool(in.outer);
   AssocParams P{o.voxel_size, o.layer_limit, o.min_ps, {o.eigen_value_array[0], o.eigen_value_array[1], o.eigen_value_array[2]}};
-  float *xyz = nullptr;
+  const float *xyz = in.xyz;
+  float *dxyz = nullptr;
   double *poses = nullptr;
   int *src = nullptr, *row = nullptr, *row_slot = nullptr, *row_prob = nullptr, *bad = nullptr;
-  TRY(pool.get(&xyz, (size_t)3 * in.n_points)); TRY(pool.get(&poses, (size_t)12 * n_rows));
+  if (!in.on_device) { TRY(pool.get(&dxyz, (size_t)3 * in.n_points)); xyz = dxyz; }
+  TRY(pool.get(&poses, (size_t)12 * n_rows));
   TRY(pool.get(&src, (size_t)n)); TRY(pool.get(&row, (size_t)n)); TRY(pool.get(&bad, 1));
   TRY(pool.get(&row_slot, (size_t)2 * n_rows));
   row_prob = row_slot + n_rows;
@@ -320,9 +331,13 @@ int assoc_cut(cudaStream_t st, const AssocInput &in, const balm_assoc_opts &o, c
       hrow[j] = one ? j : j - (int)in.pose_ptr[p];
       hrow[(size_t)n_rows + j] = p;
     }
-  if (in.n_points) CUDA_TRY(cudaMemcpyAsync(xyz, in.xyz, sizeof(float) * 3 * in.n_points, cudaMemcpyHostToDevice, st));
+  if (in.n_points && !in.on_device)
+    CUDA_TRY(cudaMemcpyAsync(dxyz, in.xyz, sizeof(float) * 3 * in.n_points, cudaMemcpyHostToDevice, st));
   CUDA_TRY(cudaMemcpyAsync(poses, in.poses12, sizeof(double) * 12 * n_rows, cudaMemcpyHostToDevice, st));
   CUDA_TRY(cudaMemcpyAsync(row_slot, hrow.data(), sizeof(int) * 2 * n_rows, cudaMemcpyHostToDevice, st));
+  if (in.stats)
+    in.stats->h2d_bytes += (in.on_device ? 0 : (int64_t)(sizeof(float) * 3 + (one ? sizeof(int) : 0)) * in.n_points) +
+                           (int64_t)(sizeof(double) * 12 + sizeof(int) * 2) * n_rows;
   CUDA_TRY(cudaMemsetAsync(bad, 0, sizeof(int), st));
   int *flag = nullptr, *scan = nullptr, *seg_start = nullptr, *idx = nullptr, *work = nullptr, *work2 = nullptr;
   unsigned *pk = nullptr, *pk2 = nullptr;
@@ -346,7 +361,8 @@ int assoc_cut(cudaStream_t st, const AssocInput &in, const balm_assoc_opts &o, c
     if (one) {
       // items = the points in a stable order by frame, so that every later stable sort keeps the frames ascending
       // inside a node
-      CUDA_TRY(cudaMemcpyAsync(pk, in.frame, sizeof(int) * n, cudaMemcpyHostToDevice, st));
+      CUDA_TRY(cudaMemcpyAsync(pk, in.frame, sizeof(int) * n,
+                               in.on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
       iota_kernel<<<gb, 256, 0, st>>>(idx, n);
       CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, pk, reinterpret_cast<unsigned *>(row), idx, src, (int)n,
                                                0, 32, st));
@@ -423,11 +439,8 @@ int assoc_cut(cudaStream_t st, const AssocInput &in, const balm_assoc_opts &o, c
   }
   int h_bad = 0;
   CUDA_TRY(cudaMemcpy(&h_bad, bad, sizeof(int), cudaMemcpyDeviceToHost));
-  if (h_bad) {
-    balm_set_error(std::string(in.who) + (h_bad & 2 ? ": frame index outside [0, n_poses)"
-                                                    : ": a point lies outside the +-2^18 root-voxel range"));
-    return BALM_ERR_INVALID;
-  }
+  if (h_bad) return bad_points_error(in.who, h_bad);
+  if (in.stats) in.stats->roots += T[0].nnode;  // layer-0 nodes of one problem: its root voxels
 
   // ---- leaves of every layer, merged in (problem, key) order ----
   int nleaf_L[3] = {0, 0, 0};
@@ -506,6 +519,346 @@ int assoc_cut(cudaStream_t st, const AssocInput &in, const balm_assoc_opts &o, c
   CUDA_TRY(cudaStreamSynchronize(st));
   CUDA_TRY(cudaGetLastError());
   // the pool's destructor frees every scratch buffer (level tables included)
+  return BALM_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// balm_cut_voxels on inputs larger than BALM_ASSOC_BUDGET_MB: root-key slabs. Every decision about a plane voxel (its
+// (node, frame) segment sums, the node judge, the ancestor lookups of leaf_decide_kernel, min_ps and the two-frame rule)
+// depends only on the points of its root voxel, and the output is ordered by the key, whose top 57 bits are the root. So
+// the points of a contiguous range of roots, kept in their input order, are cut on their own: the stable frame sort
+// gives them the subsequence the full sort gives, every segment is summed over the same points in the same order, and
+// the slabs' voxels, concatenated in root order, are the one-pass registration bit for bit (DESIGN.md section 7).
+// A root-count pass streams the host points once and counts the points of every root; the plan closes a slab before the
+// root that would take it over the cap; a selection pass per slab re-streams only the chunks whose root range overlaps
+// the slab and compacts the slab's points, in input order, into device buffers that assoc_cut takes as they are.
+namespace {
+
+struct Float3 {
+  float x, y, z;
+};
+
+__global__ void root_of_kernel(unsigned long long *key, int64_t n) {  // key -> its root voxel (the top 57 bits)
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) key[i] >>= 6;
+}
+__global__ void in_slab_kernel(const unsigned long long *key, int64_t n, unsigned long long lo, unsigned long long hi,
+                               char *flag) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const unsigned long long r = key[i] >> 6;
+  flag[i] = (r >= lo && r <= hi) ? 1 : 0;
+}
+
+// The host points in chunks of `chunk` points: stage(c, b) copies chunk c into pinned buffer b once the upload that
+// read it last is done, upload(c, b) enqueues its copy into the device chunk. Two pinned buffers let the host copy of
+// the next chunk run while the device works on this one.
+struct PointRing {
+  const AssocInput &in;
+  int64_t chunk;
+  float *hx[2] = {nullptr, nullptr};
+  int *hf[2] = {nullptr, nullptr};
+  cudaEvent_t ev[2] = {nullptr, nullptr};
+  float *dx = nullptr;
+  int *df = nullptr;
+  PointRing(const AssocInput &i, int64_t c) : in(i), chunk(c) {}
+  ~PointRing() {
+    for (int b = 0; b < 2; b++) {
+      if (ev[b]) cudaEventSynchronize(ev[b]);
+      cudaFreeHost(hx[b]);
+      cudaFreeHost(hf[b]);
+      if (ev[b]) cudaEventDestroy(ev[b]);
+    }
+  }
+  int init(ScratchPool &pool) {
+    for (int b = 0; b < 2; b++) {
+      CUDA_TRY(cudaHostAlloc((void **)&hx[b], sizeof(float) * 3 * chunk, cudaHostAllocDefault));
+      CUDA_TRY(cudaHostAlloc((void **)&hf[b], sizeof(int) * chunk, cudaHostAllocDefault));
+      CUDA_TRY(cudaEventCreateWithFlags(&ev[b], cudaEventDisableTiming));
+    }
+    TRY(pool.get(&dx, (size_t)3 * chunk));
+    TRY(pool.get(&df, (size_t)chunk));
+    return BALM_OK;
+  }
+  int64_t size(int64_t c) const { return std::min(chunk, in.n_points - c * chunk); }
+  int stage(int64_t c, int b) {
+    CUDA_TRY(cudaEventSynchronize(ev[b]));
+    memcpy(hx[b], in.xyz + 3 * c * chunk, sizeof(float) * 3 * size(c));
+    memcpy(hf[b], in.frame + c * chunk, sizeof(int) * size(c));
+    return BALM_OK;
+  }
+  int upload(cudaStream_t st, int64_t c, int b, int64_t *h2d) {
+    CUDA_TRY(cudaMemcpyAsync(dx, hx[b], sizeof(float) * 3 * size(c), cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(df, hf[b], sizeof(int) * size(c), cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaEventRecord(ev[b], st));
+    *h2d += (int64_t)(sizeof(float) * 3 + sizeof(int)) * size(c);
+    return BALM_OK;
+  }
+};
+
+double now_ms() {
+  return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count();
+}
+
+// cub scratch that grows on demand (pool-owned)
+struct Tmp {
+  ScratchPool &pool;
+  char *p = nullptr;
+  size_t bytes = 0;
+  int need(size_t b) {
+    if (b <= bytes) return BALM_OK;
+    pool.drop(p);
+    p = nullptr;
+    bytes = b;
+    return pool.get(&p, bytes);
+  }
+  void free() {
+    pool.drop(p);
+    p = nullptr;
+    bytes = 0;
+  }
+};
+
+}  // namespace
+
+int64_t assoc_bytes_per_point(int layer_limit) {
+  return 16                         // the slab's points and frames (xyz, frame)
+         + 64                       // items: src row flag scan seg_start idx work work2 pk pk2 (4 B), key keyL keyL2 (8 B)
+         + 16                       // radix sort scratch (alternate keys and values, digit histograms, look-back)
+         + 120 * (layer_limit + 1)  // one segment per point per layer, kept to the emission: segB 80 + seg_row 4, node
+                                    // tables 32 (start key prob size planar nframes leaf) + leaf scan 4
+         + 96                       // one layer's transient segment tables: segW 80 + seg_key 8 + nflag 4 + nscan 4
+         + 32                       // leaves: lkey lkey2 (8 B), lref lref2 lcnt lobs (4 B)
+         + 112                      // the slab's emitted voxels: obs 80 + pose_idx 4 + row_ptr 8 + coe 8 + key 8 + layer 4
+         + 9;                       // the slab path's chunk staging (cap / 8 points, at least 4096, at about 50 B
+                                    // each) and the slab buffers' one chunk of room (16 B per chunk point)
+}
+int64_t assoc_bytes_fixed(int n_rows) {
+  // poses twice (root pass and cut, 96 B per row each) and the row tables (8 B per row), plus 1 MiB for cub's tile
+  // state, the small tables and the one-element minimum of every allocation
+  return (int64_t)200 * n_rows + (1 << 20);
+}
+
+int assoc_cut_slabs(cudaStream_t st, const AssocInput &in, const balm_assoc_opts &o, size_t budget, int64_t cap,
+                    ScratchPool &outer, SlabVoxels *out, CutSlabStats *stats, long long *launches) {
+  const int n_rows = in.n_rows;
+  const int64_t n = in.n_points;
+  const AssocParams P{o.voxel_size, o.layer_limit, o.min_ps, {o.eigen_value_array[0], o.eigen_value_array[1], o.eigen_value_array[2]}};
+  const int64_t chunk = std::min(n, std::max<int64_t>(4096, std::min<int64_t>(cap / 8, 1 << 23)));
+  const int64_t n_chunks = (n + chunk - 1) / chunk;
+  CutSlabStats S;
+  const double t0 = now_ms();
+  PointRing ring(in, chunk);
+  TRY(ring.init(outer));
+  double *poses = nullptr;
+  int *iota = nullptr, *bad = nullptr, *d_num = nullptr;
+  unsigned long long *key = nullptr, *key2 = nullptr;
+  TRY(outer.get(&poses, (size_t)12 * n_rows)); TRY(outer.get(&iota, (size_t)ring.chunk)); TRY(outer.get(&bad, 1));
+  TRY(outer.get(&d_num, 2)); TRY(outer.get(&key, (size_t)ring.chunk)); TRY(outer.get(&key2, (size_t)ring.chunk));
+  CUDA_TRY(cudaMemcpyAsync(poses, in.poses12, sizeof(double) * 12 * n_rows, cudaMemcpyHostToDevice, st));
+  CUDA_TRY(cudaMemsetAsync(bad, 0, sizeof(int), st));
+  S.h2d_bytes += (int64_t)sizeof(double) * 12 * n_rows;
+  iota_kernel<<<(unsigned)((ring.chunk + 255) / 256), 256, 0, st>>>(iota, ring.chunk);
+  *launches += 1;
+  Tmp tmp{outer};
+
+  // ---- root-count pass: (root, count) runs of every chunk merged into one table, sorted by root ----
+  int64_t T = 0, tcap = 0;  // table entries and capacity (room for a chunk's runs after the table)
+  unsigned long long *tk = nullptr, *sk = nullptr;
+  long long *tc = nullptr, *sc = nullptr;
+  std::vector<unsigned long long> cmin((size_t)n_chunks), cmax((size_t)n_chunks);
+  int h_bad = 0;
+  TRY(ring.stage(0, 0));
+  for (int64_t c = 0; c < n_chunks; c++) {
+    const int b = (int)(c & 1);
+    const int64_t m = ring.size(c);
+    const unsigned gm = (unsigned)((m + 255) / 256);
+    TRY(ring.upload(st, c, b, &S.h2d_bytes));
+    item_key_kernel<<<gm, 256, 0, st>>>(ring.dx, iota, ring.df, poses, n_rows, m, P, key, bad);
+    *launches += 1;
+    if (!h_bad) {  // once a point is bad the call fails: the rest of the pass only looks for a bad frame
+      if (T + m > tcap) {  // grow the table (and its sort buffers) to hold this chunk's runs after it
+        const int64_t ncap = std::max(2 * tcap, T + m);
+        unsigned long long *nk = nullptr, *nsk = nullptr;
+        long long *nc = nullptr, *nsc = nullptr;
+        TRY(outer.get(&nk, (size_t)ncap)); TRY(outer.get(&nc, (size_t)ncap));
+        TRY(outer.get(&nsk, (size_t)ncap)); TRY(outer.get(&nsc, (size_t)ncap));
+        if (T) {
+          CUDA_TRY(cudaMemcpyAsync(nk, tk, sizeof(unsigned long long) * T, cudaMemcpyDeviceToDevice, st));
+          CUDA_TRY(cudaMemcpyAsync(nc, tc, sizeof(long long) * T, cudaMemcpyDeviceToDevice, st));
+        }
+        CUDA_TRY(cudaStreamSynchronize(st));
+        outer.drop(tk); outer.drop(tc); outer.drop(sk); outer.drop(sc);
+        tk = nk; tc = nc; sk = nsk; sc = nsc; tcap = ncap;
+      }
+      root_of_kernel<<<gm, 256, 0, st>>>(key, m);
+      size_t b1 = 0, b2 = 0, b3 = 0, b4 = 0;
+      cub::DeviceRadixSort::SortKeys(nullptr, b1, key, key2, (int)m, 0, 57, st);
+      cub::DeviceRunLengthEncode::Encode(nullptr, b2, key2, tk + T, tc + T, d_num, (int)m, st);
+      cub::DeviceRadixSort::SortPairs(nullptr, b3, tk, sk, tc, sc, (int)(T + m), 0, 57, st);
+      cub::DeviceReduce::ReduceByKey(nullptr, b4, sk, tk, sc, tc, d_num + 1, cub::Sum(), (int)(T + m), st);
+      TRY(tmp.need(std::max(std::max(b1, b2), std::max(b3, b4))));
+      if (outer.bytes > budget) {
+        balm_set_error(std::string(in.who) + ": the root table (" + std::to_string(T) +
+                       " roots so far) does not fit BALM_ASSOC_BUDGET_MB (" + std::to_string(budget) + " bytes)");
+        return BALM_ERR_UNSUPPORTED;
+      }
+      CUDA_TRY(cub::DeviceRadixSort::SortKeys(tmp.p, tmp.bytes, key, key2, (int)m, 0, 57, st));
+      CUDA_TRY(cub::DeviceRunLengthEncode::Encode(tmp.p, tmp.bytes, key2, tk + T, tc + T, d_num, (int)m, st));
+      int r = 0;
+      CUDA_TRY(cudaMemcpyAsync(&r, d_num, sizeof(int), cudaMemcpyDeviceToHost, st));
+      if (c + 1 < n_chunks) TRY(ring.stage(c + 1, b ^ 1));  // the host copy of the next chunk overlaps this one's work
+      CUDA_TRY(cudaStreamSynchronize(st));
+      CUDA_TRY(cudaMemcpy(&cmin[c], tk + T, sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+      CUDA_TRY(cudaMemcpy(&cmax[c], tk + T + r - 1, sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+      if (T > 0) {  // merge: sort table + runs by root, add the counts of equal roots
+        CUDA_TRY(cub::DeviceRadixSort::SortPairs(tmp.p, tmp.bytes, tk, sk, tc, sc, (int)(T + r), 0, 57, st));
+        CUDA_TRY(cub::DeviceReduce::ReduceByKey(tmp.p, tmp.bytes, sk, tk, sc, tc, d_num + 1, cub::Sum(), (int)(T + r), st));
+        int t = 0;
+        CUDA_TRY(cudaMemcpyAsync(&t, d_num + 1, sizeof(int), cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaStreamSynchronize(st));
+        T = t;
+        *launches += 2;
+      } else {
+        T = r;
+      }
+      *launches += 3;
+    } else if (c + 1 < n_chunks) {
+      TRY(ring.stage(c + 1, b ^ 1));
+    }
+    CUDA_TRY(cudaMemcpyAsync(&h_bad, bad, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+  }
+  if (h_bad) return bad_points_error(in.who, h_bad);
+  std::vector<unsigned long long> rkey((size_t)T);
+  std::vector<long long> rcnt((size_t)T);
+  CUDA_TRY(cudaMemcpy(rkey.data(), tk, sizeof(unsigned long long) * T, cudaMemcpyDeviceToHost));
+  CUDA_TRY(cudaMemcpy(rcnt.data(), tc, sizeof(long long) * T, cudaMemcpyDeviceToHost));
+  outer.drop(tk); outer.drop(tc); outer.drop(sk); outer.drop(sc);
+  tmp.free();
+  S.roots = T;
+  S.ms_roots = now_ms() - t0;
+
+  // ---- slab plan: roots in ascending order, a slab closed before the root that would take it over the cap ----
+  std::vector<int64_t> slab_root{0};  // slab s holds the roots [slab_root[s], slab_root[s + 1])
+  std::vector<int64_t> slab_pts;
+  int64_t cur = 0;
+  for (int64_t r = 0; r < T; r++) {
+    if (rcnt[r] > cap) {
+      balm_set_error(std::string(in.who) + ": a root voxel holds " + std::to_string(rcnt[r]) +
+                     " points, more than the " + std::to_string(cap) + " points per slab BALM_ASSOC_BUDGET_MB allows");
+      return BALM_ERR_UNSUPPORTED;
+    }
+    if (cur + rcnt[r] > cap) {
+      slab_root.push_back(r);
+      slab_pts.push_back(cur);
+      cur = 0;
+    }
+    cur += rcnt[r];
+  }
+  slab_root.push_back(T);
+  slab_pts.push_back(cur);
+  S.slabs = (int64_t)slab_pts.size();
+  S.max_slab = *std::max_element(slab_pts.begin(), slab_pts.end());
+
+  // ---- per slab: select its points in input order, cut them, stage its voxels on the host ----
+  char *flag = nullptr;
+  TRY(outer.get(&flag, (size_t)ring.chunk));
+  {
+    size_t b1 = 0, b2 = 0;
+    cub::DeviceSelect::Flagged(nullptr, b1, (const Float3 *)ring.dx, flag, (Float3 *)nullptr, d_num, (int)ring.chunk, st);
+    cub::DeviceSelect::Flagged(nullptr, b2, ring.df, flag, (int *)nullptr, d_num + 1, (int)ring.chunk, st);
+    TRY(tmp.need(std::max(b1, b2)));
+  }
+  SlabVoxels V;
+  V.row_ptr.push_back(0);
+  AssocStats ast;
+  for (int64_t s = 0; s < S.slabs; s++) {
+    const double ts = now_ms();
+    const unsigned long long lo = rkey[slab_root[s]], hi = rkey[slab_root[s + 1] - 1];
+    const int64_t pts = slab_pts[s];
+    std::vector<int64_t> cs;
+    for (int64_t c = 0; c < n_chunks; c++)
+      if (cmax[c] >= lo && cmin[c] <= hi) cs.push_back(c);
+    ScratchPool sp(&outer);
+    float *sx = nullptr;
+    int *sf = nullptr;
+    // one chunk of room past the slab's count: a selection that disagreed with the root counts could not write out of
+    // bounds before the check below catches it
+    TRY(sp.get(&sx, (size_t)3 * (pts + ring.chunk))); TRY(sp.get(&sf, (size_t)(pts + ring.chunk)));
+    int64_t filled = 0;
+    TRY(ring.stage(cs[0], 0));
+    for (size_t q = 0; q < cs.size(); q++) {
+      const int b = (int)(q & 1);
+      const int64_t m = ring.size(cs[q]);
+      const unsigned gm = (unsigned)((m + 255) / 256);
+      TRY(ring.upload(st, cs[q], b, &S.h2d_bytes));
+      item_key_kernel<<<gm, 256, 0, st>>>(ring.dx, iota, ring.df, poses, n_rows, m, P, key, bad);
+      in_slab_kernel<<<gm, 256, 0, st>>>(key, m, lo, hi, flag);
+      CUDA_TRY(cub::DeviceSelect::Flagged(tmp.p, tmp.bytes, (const Float3 *)ring.dx, flag, (Float3 *)(sx + 3 * filled),
+                                          d_num, (int)m, st));
+      CUDA_TRY(cub::DeviceSelect::Flagged(tmp.p, tmp.bytes, ring.df, flag, sf + filled, d_num + 1, (int)m, st));
+      *launches += 4;
+      int got = 0;
+      CUDA_TRY(cudaMemcpyAsync(&got, d_num, sizeof(int), cudaMemcpyDeviceToHost, st));
+      if (q + 1 < cs.size()) TRY(ring.stage(cs[q + 1], b ^ 1));
+      CUDA_TRY(cudaStreamSynchronize(st));
+      filled += got;
+      if (filled > pts) break;
+    }
+    if (filled != pts) {
+      balm_set_error(std::string(in.who) + ": internal error: a slab's selection disagrees with its root counts");
+      return BALM_ERR_CUDA;
+    }
+    const double tc0 = now_ms();
+    S.ms_select += tc0 - ts;
+    AssocInput sin = in;
+    sin.n_points = sin.n_items = pts;
+    sin.xyz = sx;
+    sin.frame = sf;
+    sin.on_device = true;
+    sin.outer = &sp;
+    sin.stats = &ast;
+    // the slab's voxels land in slab-local device arrays (SoA observations, stride = the slab's K)
+    double *eobs = nullptr, *ecoe = nullptr;
+    int *epose = nullptr, *elayer = nullptr;
+    long long *erow = nullptr;
+    unsigned long long *ekey = nullptr;
+    int64_t Ms = 0, Ks = 0;
+    const AssocRegister reg = [&](int64_t M, int64_t K, const int64_t *, const int64_t *, AssocEmit *e) {
+      Ms = M; Ks = K;
+      TRY(sp.get(&eobs, (size_t)10 * K)); TRY(sp.get(&epose, (size_t)K)); TRY(sp.get(&erow, (size_t)M + 1));
+      TRY(sp.get(&ecoe, (size_t)M)); TRY(sp.get(&ekey, (size_t)M)); TRY(sp.get(&elayer, (size_t)M));
+      *e = AssocEmit{eobs, K, 1, epose, erow, ecoe, ekey, elayer};
+      return (int)BALM_OK;
+    };
+    TRY(assoc_cut(st, sin, o, reg, launches));
+    const int64_t M0 = V.M, K0 = V.K;
+    V.M += Ms;
+    V.K += Ks;
+    V.row_ptr.resize((size_t)V.M + 1);
+    V.pose_idx.resize((size_t)V.K);
+    V.coe.resize((size_t)V.M);
+    V.key.resize((size_t)V.M);
+    V.layer.resize((size_t)V.M);
+    for (int c = 0; c < 10; c++) V.obs[c].resize((size_t)V.K);
+    CUDA_TRY(cudaMemcpy(V.row_ptr.data() + M0, erow, sizeof(long long) * (Ms + 1), cudaMemcpyDeviceToHost));
+    for (int64_t v = M0; v <= V.M; v++) V.row_ptr[v] += K0;
+    if (Ks) {
+      CUDA_TRY(cudaMemcpy(V.pose_idx.data() + K0, epose, sizeof(int) * Ks, cudaMemcpyDeviceToHost));
+      for (int c = 0; c < 10; c++)
+        CUDA_TRY(cudaMemcpy(V.obs[c].data() + K0, eobs + (size_t)c * Ks, sizeof(double) * Ks, cudaMemcpyDeviceToHost));
+    }
+    if (Ms) {
+      CUDA_TRY(cudaMemcpy(V.coe.data() + M0, ecoe, sizeof(double) * Ms, cudaMemcpyDeviceToHost));
+      CUDA_TRY(cudaMemcpy(V.key.data() + M0, ekey, sizeof(unsigned long long) * Ms, cudaMemcpyDeviceToHost));
+      CUDA_TRY(cudaMemcpy(V.layer.data() + M0, elayer, sizeof(int) * Ms, cudaMemcpyDeviceToHost));
+    }
+    S.ms_cut += now_ms() - tc0;
+  }
+  S.h2d_bytes += ast.h2d_bytes;
+  *out = std::move(V);
+  *stats = S;
   return BALM_OK;
 }
 

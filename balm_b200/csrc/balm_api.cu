@@ -454,34 +454,99 @@ balm_assoc_opts resolve_assoc_opts(const balm_assoc_opts *opts) {
   return o;
 }
 
+// BALM_ASSOC_BUDGET_MB (read at every call, default 16 GB): the association's device scratch
+static size_t assoc_budget() {
+  size_t budget = (size_t)16 << 30;
+  if (const char *e = getenv("BALM_ASSOC_BUDGET_MB")) budget = (size_t)llround(std::max(0.0, atof(e)) * 1048576.0);
+  return budget;
+}
+
+// The slab path's voxels, staged on the host, registered like the one-pass call's register step does it
+static int register_slabs(balm_ctx *c, const SlabVoxels &V) {
+  TRY(alloc_problem_arrays(c, V.M, V.K, false));
+  drop_keys(c);
+  TRY(dev_alloc(&c->vox_key, (size_t)V.M));
+  TRY(dev_alloc(&c->vox_layer, (size_t)V.M));
+  CUDA_TRY(cudaMemcpyAsync(c->row_ptr, V.row_ptr.data(), sizeof(long long) * (V.M + 1), cudaMemcpyHostToDevice, c->stream));
+  CUDA_TRY(cudaMemcpyAsync(c->pose_idx, V.pose_idx.data(), sizeof(int) * V.K, cudaMemcpyHostToDevice, c->stream));
+  for (int col = 0; col < 10; col++)
+    CUDA_TRY(cudaMemcpyAsync(c->obs + (size_t)col * c->Kp, V.obs[col].data(), sizeof(double) * V.K,
+                             cudaMemcpyHostToDevice, c->stream));
+  CUDA_TRY(cudaMemcpyAsync(c->coe, V.coe.data(), sizeof(double) * V.M, cudaMemcpyHostToDevice, c->stream));
+  CUDA_TRY(cudaMemcpyAsync(c->vox_key, V.key.data(), sizeof(unsigned long long) * V.M, cudaMemcpyHostToDevice, c->stream));
+  CUDA_TRY(cudaMemcpyAsync(c->vox_layer, V.layer.data(), sizeof(int) * V.M, cudaMemcpyHostToDevice, c->stream));
+  CUDA_TRY(cudaStreamSynchronize(c->stream));
+  return BALM_OK;
+}
+
 extern "C" int balm_cut_voxels(balm_ctx *c, int64_t n_points, const float *xyz, const int32_t *frame,
                                const double *poses12, const balm_assoc_opts *opts, int64_t *n_voxels_out,
                                int64_t *n_obs_out) {
   if (!c || !xyz || !frame || !poses12) { balm_set_error("balm_cut_voxels: bad arguments"); return BALM_ERR_INVALID; }
   const balm_assoc_opts o = resolve_assoc_opts(opts);
-  if (n_points < 1 || n_points >= (1ll << 31) || o.layer_limit < 0 || o.layer_limit > 2) {
-    balm_set_error("balm_cut_voxels: bad arguments (n < 2^31, layer_limit in 0..2)");
+  if (n_points < 1 || o.layer_limit < 0 || o.layer_limit > 2) {
+    balm_set_error("balm_cut_voxels: bad arguments (n >= 1, layer_limit in 0..2)");
     return BALM_ERR_INVALID;
   }
   CUDA_TRY(cudaSetDevice(c->device));
+  const double t0 = host_ms();
+  const size_t budget = assoc_budget();
+  const int64_t per_point = assoc_bytes_per_point(o.layer_limit), fixed = assoc_bytes_fixed(c->N);
+  ScratchPool acct;  // counts the scratch of the whole call
+  AssocStats ast;
   AssocInput in{"balm_cut_voxels", n_points, xyz, c->N, poses12, frame, 1, nullptr, nullptr, nullptr, n_points};
-  // register: allocate the problem arrays of the context and the voxel keys, which stay with it (balm_append_scan /
-  // balm_marginalize need them)
-  const AssocRegister reg = [c](int64_t M, int64_t K, const int64_t *, const int64_t *, AssocEmit *out) {
-    if (M < 1) { balm_set_error("balm_cut_voxels: no plane voxels found"); return (int)BALM_ERR_INVALID; }
-    TRY(alloc_problem_arrays(c, M, K, false));
-    drop_keys(c);
-    TRY(dev_alloc(&c->vox_key, (size_t)M));
-    TRY(dev_alloc(&c->vox_layer, (size_t)M));
-    *out = AssocEmit{c->obs, c->Kp, 1, c->pose_idx, c->row_ptr, c->coe, c->vox_key, c->vox_layer};
-    return (int)BALM_OK;
-  };
-  TRY(assoc_cut(c->stream, in, o, reg, &c->launches));
+  in.outer = &acct;
+  in.stats = &ast;
+  int64_t st[BALM_CUT_STATS] = {1, n_points, 0, 0, 0, per_point, fixed, 0, 0, 0, 0};
+  if (n_points < (1ll << 31) && (double)n_points * per_point + fixed <= (double)budget) {
+    // one pass: register: allocate the problem arrays of the context and the voxel keys, which stay with it
+    // (balm_append_scan / balm_marginalize need them)
+    const AssocRegister reg = [c](int64_t M, int64_t K, const int64_t *, const int64_t *, AssocEmit *out) {
+      if (M < 1) { balm_set_error("balm_cut_voxels: no plane voxels found"); return (int)BALM_ERR_INVALID; }
+      TRY(alloc_problem_arrays(c, M, K, false));
+      drop_keys(c);
+      TRY(dev_alloc(&c->vox_key, (size_t)M));
+      TRY(dev_alloc(&c->vox_layer, (size_t)M));
+      *out = AssocEmit{c->obs, c->Kp, 1, c->pose_idx, c->row_ptr, c->coe, c->vox_key, c->vox_layer};
+      return (int)BALM_OK;
+    };
+    TRY(assoc_cut(c->stream, in, o, reg, &c->launches));
+    st[2] = ast.roots;
+    st[4] = ast.h2d_bytes;
+    st[9] = (int64_t)(1e3 * (host_ms() - t0));
+  } else {
+    // root-key slabs of at most cap points, each within the budget
+    const int64_t cap = std::min<int64_t>(std::max<int64_t>(0, ((int64_t)budget - fixed) / per_point), INT_MAX);
+    SlabVoxels V;
+    CutSlabStats S;
+    TRY(assoc_cut_slabs(c->stream, in, o, budget, cap, acct, &V, &S, &c->launches));
+    if (V.M < 1) { balm_set_error("balm_cut_voxels: no plane voxels found"); return BALM_ERR_INVALID; }
+    if (V.K >= ((int64_t)1 << 31)) {
+      balm_set_error("balm_cut_voxels: more than 2^31 observations per GPU");
+      return BALM_ERR_UNSUPPORTED;
+    }
+    const double t1 = host_ms();
+    TRY(register_slabs(c, V));
+    st[0] = S.slabs; st[1] = S.max_slab; st[2] = S.roots; st[4] = S.h2d_bytes + V.K * 84 + V.M * 28 + 8;
+    st[7] = (int64_t)(1e3 * S.ms_roots); st[8] = (int64_t)(1e3 * S.ms_select); st[9] = (int64_t)(1e3 * S.ms_cut);
+    st[10] = (int64_t)(1e3 * (host_ms() - t1));
+  }
   c->has_keys = true;
   c->assoc = o;
   if (n_voxels_out) *n_voxels_out = c->M;
   if (n_obs_out) *n_obs_out = c->K;
-  return finish_registration(c);
+  st[3] = (int64_t)acct.peak;
+  const double t2 = host_ms();
+  const int rc = finish_registration(c);
+  st[10] += (int64_t)(1e3 * (host_ms() - t2));
+  if (rc == BALM_OK) memcpy(c->cut_stats, st, sizeof(st));
+  return rc;
+}
+
+extern "C" int balm_cut_voxels_stats(balm_ctx *c, int64_t *stats) {
+  if (!c || !stats) { balm_set_error("balm_cut_voxels_stats: bad arguments"); return BALM_ERR_INVALID; }
+  memcpy(stats, c->cut_stats, sizeof(c->cut_stats));
+  return BALM_OK;
 }
 
 extern "C" int balm_download_voxel_range(balm_ctx *c, int64_t head, int64_t end, int64_t *row_ptr, int32_t *pose_idx,

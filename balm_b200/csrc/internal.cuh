@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
+#include <algorithm>
 #include <cmath>
 #include <functional>
 #include <string>
@@ -68,13 +69,25 @@ int dev_alloc(T **p, size_t count) {  // count elements of T (at least one, so t
 
 // Device scratch of one call: every buffer taken from the pool is freed on ANY exit path (the early returns of TRY /
 // CUDA_TRY, a rejected registration, a bad frame index ...), so a failed call leaks nothing. drop frees one early.
+// bytes / peak count the bytes requested from the pool and from every pool nested in it (constructed with it as up), so
+// the outermost pool of a call sees the call's whole scratch.
 struct ScratchPool {
-  std::vector<void *> ptrs;
-  ~ScratchPool() { for (void *q : ptrs) cudaFree(q); }
+  std::vector<std::pair<void *, size_t>> ptrs;
+  ScratchPool *up = nullptr;
+  size_t bytes = 0, peak = 0;
+  ScratchPool() = default;
+  explicit ScratchPool(ScratchPool *outer) : up(outer) {}
+  ScratchPool(const ScratchPool &) = delete;
+  ScratchPool &operator=(const ScratchPool &) = delete;
+  ~ScratchPool() {
+    for (auto &q : ptrs) { cudaFree(q.first); count(-(long long)q.second); }
+  }
   template <typename T>
   int get(T **p, size_t n) {
     TRY(dev_alloc(p, n));
-    ptrs.push_back((void *)*p);
+    const size_t b = sizeof(T) * (n ? n : 1);
+    ptrs.push_back({(void *)*p, b});
+    count((long long)b);
     return BALM_OK;
   }
   void drop(void *q) {
@@ -84,7 +97,18 @@ struct ScratchPool {
   void release(void *q) {  // the caller keeps q: it is no longer freed on exit
     if (!q) return;
     for (size_t i = 0; i < ptrs.size(); i++)
-      if (ptrs[i] == q) { ptrs[i] = ptrs.back(); ptrs.pop_back(); break; }
+      if (ptrs[i].first == q) {
+        count(-(long long)ptrs[i].second);
+        ptrs[i] = ptrs.back();
+        ptrs.pop_back();
+        break;
+      }
+  }
+  void count(long long d) {
+    for (ScratchPool *s = this; s; s = s->up) {
+      s->bytes = (size_t)((long long)s->bytes + d);
+      s->peak = std::max(s->peak, s->bytes);
+    }
   }
 };
 
@@ -142,6 +166,7 @@ struct balm_ctx {
   int *vox_layer = nullptr;       // [M] octree layer of every voxel (a key digit 7 is BOTH octant 7 and "not split":
                                   // the layer says which)
   bool has_keys = false;
+  int64_t cut_stats[BALM_CUT_STATS] = {};  // balm_cut_voxels_stats: the last successful balm_cut_voxels
   balm_assoc_opts assoc{1.0, 2, 15, {1.0 / 16, 1.0 / 16, 1.0 / 16}};  // association options of that call
   WindowState *win = nullptr;     // balm_window_* state (independent of the registered voxel set)
   PoseGraph *pg = nullptr;        // balm_set_pose_factors' window factors (independent of the registered voxel set);
@@ -1059,7 +1084,12 @@ int launch_raw_blocks(balm_ctx *c, const double *rows, int64_t v0, int64_t v1, c
 // poses12 are uploaded once. Either frame != NULL: one problem whose pose rows are its frames (balm_cut_voxels; the
 // points of frame f are in slot f), or a problem table: problem p owns the rows [pose_ptr[p], pose_ptr[p+1]) and row j
 // is the scan pose_scan[j] = points [scan_ptr[s], scan_ptr[s+1]) in slot j - pose_ptr[p]; n_items = the sum of the
-// rows' point counts (< 2^31, checked by the caller).
+// rows' point counts (< 2^31, checked by the caller). With on_device (one problem only) xyz and frame are device arrays
+// that stay with the caller. outer: the pool the call's scratch is counted in (may be null); stats: the call's
+// host-to-device bytes and its root voxels are added to it (may be null).
+struct AssocStats {
+  int64_t h2d_bytes = 0, roots = 0;
+};
 struct AssocInput {
   const char *who;  // prefix of error messages
   int64_t n_points;
@@ -1072,6 +1102,26 @@ struct AssocInput {
   const int32_t *pose_scan;
   const int64_t *scan_ptr;
   int64_t n_items;
+  bool on_device = false;
+  ScratchPool *outer = nullptr;
+  AssocStats *stats = nullptr;
+};
+// Scratch bound of assoc_cut's one-problem mode, in bytes: n points x assoc_bytes_per_point(layer_limit) +
+// assoc_bytes_fixed(n_rows) covers every buffer the call (and balm_cut_voxels' slab path around it) takes at once.
+int64_t assoc_bytes_per_point(int layer_limit);
+int64_t assoc_bytes_fixed(int n_rows);
+// balm_cut_voxels' slab path (assoc.cu): the points of in (host arrays, one problem, any n_points) cut in root-key slabs
+// of at most `cap` points each, every slab's voxels staged on the host (the caller registers them).
+struct CutSlabStats {
+  int64_t slabs = 0, max_slab = 0, roots = 0, h2d_bytes = 0;
+  double ms_roots = 0, ms_select = 0, ms_cut = 0;
+};
+struct SlabVoxels {  // the staged registration: M voxels, K observations, host arrays
+  int64_t M = 0, K = 0;
+  std::vector<long long> row_ptr;
+  std::vector<int> pose_idx, layer;
+  std::vector<double> obs[10], coe;
+  std::vector<unsigned long long> key;
 };
 // Where the voxels are emitted (device arrays): observation o, column c at obs[c * obs_cstride + o * obs_ostride]
 // (SoA of a context or AoS of a batch), pose_idx = slot, row_ptr [M + 1], coe, key and layer [M].
@@ -1092,6 +1142,9 @@ balm_assoc_opts resolve_assoc_opts(const balm_assoc_opts *opts);  // opts or the
 // opts: from resolve_assoc_opts, layer_limit in 0..2 (checked by the caller)
 int assoc_cut(cudaStream_t st, const AssocInput &in, const balm_assoc_opts &opts, const AssocRegister &reg,
               long long *launches);
+// budget: device scratch bytes; cap: points per slab (< 2^31). Fills out on success; on any error nothing is staged.
+int assoc_cut_slabs(cudaStream_t st, const AssocInput &in, const balm_assoc_opts &opts, size_t budget, int64_t cap,
+                    ScratchPool &outer, SlabVoxels *out, CutSlabStats *stats, long long *launches);
 // Keyframes of a batch (balm_batch_merge_scans): the problem table and scan pool of AssocInput's batch form, checked by
 // the caller; n_items (< 2^31) = the rows' point counts summed. Writes kf_ptr [B + 1] and kf_xyz (host) only on success;
 // BALM_ERR_INVALID names the lowest problem with a voxel index outside +-2^20.

@@ -174,8 +174,29 @@ typedef struct {
   double eigen_value_array[3];/* bavoxel.hpp:11; benchmark_realworld.cpp:183-185 sets {1/16, 1/16, 1/9} */
 } balm_assoc_opts;
 void balm_default_assoc_opts(balm_assoc_opts *opts);
+/* Device memory: BALM_ASSOC_BUDGET_MB (read at every call, default 16384; fractions allowed) bounds the association's
+ * device scratch. The bound of the call is n_points x P + F bytes, P = 345 + 120 (layer_limit + 1) per point (one
+ * segment per point per layer, the worst case) and F = 200 N + 1 MiB; balm_cut_voxels_stats reports both. When it fits
+ * the budget (and n_points < 2^31) the points are cut in one pass. Otherwise they are cut in root-key slabs: a pass over
+ * the points counts every root voxel's points, the roots are grouped in ascending key order into slabs of at most
+ * cap = (budget - F) / P points (and < 2^31), and each slab's points are selected in their input order and cut on their
+ * own, then every slab's voxels are registered at once. The result is bitwise that of the one-pass cut (every decision
+ * about a voxel depends only on the points of its root voxel; DESIGN.md section 7), so n_points may be 2^31 or more.
+ * The device peak is the larger of the budget and the registration; the slabs' voxels are staged in host memory (84 B
+ * per observation, 28 B per voxel) on top of the caller's points (16 B per point: xyz and frame), and the slab path
+ * streams the points through two pinned buffers of at most 2^23 points. Errors, each leaving the registered voxel set
+ * as it was: BALM_ERR_INVALID for a frame outside [0, N), a point outside the +-2^18 root-voxel range, or no plane
+ * voxel; BALM_ERR_UNSUPPORTED (slab path) for a root voxel holding more than cap points (the message gives both), a
+ * table of the roots that does not fit the budget, or 2^31 or more observations. */
 int balm_cut_voxels(balm_ctx *ctx, int64_t n_points, const float *xyz, const int32_t *frame, const double *poses12,
                     const balm_assoc_opts *opts, int64_t *n_voxels_out, int64_t *n_obs_out);
+/* The last successful balm_cut_voxels, into stats[BALM_CUT_STATS]: [0] slabs (1 in one pass), [1] points in the largest
+ * slab, [2] root voxels, [3] peak device scratch bytes (as allocated by the call, counted by request), [4] host-to-device
+ * bytes (points, poses, and in the slab path every re-streamed chunk and the registration's upload), [5] P and [6] F of
+ * the scratch bound above, then wall times in microseconds: [7] root-count pass, [8] slab selection, [9] cuts (the whole
+ * cut in one pass), [10] registration. All zero before the first cut. */
+#define BALM_CUT_STATS 11
+int balm_cut_voxels_stats(balm_ctx *ctx, int64_t *stats);
 
 /* Sliding-window marginalisation of the registered voxel set (SURVEY.md section 8f, row N2) =
  * OCTO_TREE_ROOT::marginalize -> OCTO_TREE_NODE::to_margi on every plane leaf (bavoxel.hpp:948-963, 778-816) followed by
