@@ -781,10 +781,12 @@ static int residual_dev(balm_ctx *c, const double *poses, double *host_out, bool
 // What an evaluation, LM loop or covariance solves for: the context's N slot poses (rig null), or a rig's free base
 // poses and extrinsics, composed to slot poses before every evaluation, with H and g reduced to H_rig and g_rig after
 // it. Everything else (the dense or sparse solve, the LM rule, the undamped factor, the covariance algebra) is the same
-// for both, so these functions are the only code that tells them apart.
+// for both, so these functions are the only code that tells them apart. pose_terms (the dense pose-graph calls, rig
+// null) costs the slot poses by the context's pose factors and priors instead of its voxels.
 struct Unknowns {
   balm_ctx *c;
   Rig *rig;
+  bool pose_terms = false;
 
   bool sparse() const { return rig ? rig_sparse(rig) : c->prec == BALM_PREC_BLOCKS; }
   DenseSystem system() const { return rig ? rig_system(rig) : ctx_system(c); }
@@ -828,8 +830,10 @@ struct Unknowns {
   // the slot poses of the current state in c->poses
   int compose() const { return rig ? rig_compose(rig, c->stream, state(), c->poses, &c->launches) : BALM_OK; }
   // evaluate_dev at the current state: H, g and the residual in c->scal[0], then a rig's H_rig and g_rig (the
-  // reduction timed by ev[13] and ev[14]); with a blocks context, its slot blocks, factors and priors first
+  // reduction timed by ev[13] and ev[14]); with a blocks context, its slot blocks, factors and priors first. Pose terms:
+  // pose_graph_eval, the factors' and priors' H, g and cost, no voxels (the other arguments are unused)
   int eval(bool include_fix, int64_t head, int64_t end, bool stats_cached = false) const {
+    if (pose_terms) return pose_graph_eval(c, c->poses);
     TRY(compose());
     TRY(evaluate_dev(c, c->poses, head, end, include_fix, stats_cached));
     if (!rig) return BALM_OK;
@@ -864,6 +868,17 @@ struct Unknowns {
     TRY(rig_update(rig, c->stream, state(), rig_state(rig, true), &c->launches));
     return rig_compose(rig, c->stream, rig_state(rig, true), c->poses_trial, &c->launches);
   }
+  // the cost at c->poses_trial into *r2, once the stream has been waited for: residual_dev (keep_stats: its per-voxel
+  // stats kept for a hand-over), or the pose factors' then the priors' cost in scal[2]
+  int trial_cost(bool keep_stats, double *r2) const {
+    if (!pose_terms) return residual_dev(c, c->poses_trial, r2, keep_stats);
+    TRY(pose_graph_cost(c->pg, c->stream, c->poses_trial, c->scal + 2, &c->launches));
+    if (c->pr) TRY(prior_add_cost(c->pr, c->stream, c->poses_trial, c->scal + 2, &c->launches));
+    CUDA_TRY(cudaMemcpyAsync(c->h_scal + 2, c->scal + 2, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+    CUDA_TRY(cudaStreamSynchronize(c->stream));
+    *r2 = c->h_scal[2];
+    return BALM_OK;
+  }
   void accept() const {
     if (rig) rig_swap_states(rig);
     else std::swap(c->poses, c->poses_trial);
@@ -893,8 +908,8 @@ static int blocks_to_dense(balm_ctx *c, const std::vector<int2> &pr, const doubl
   return BALM_OK;
 }
 
-// balm_evaluate and balm_rig_evaluate after their checks: H (dense, expanded from blocks), g and the residual of voxels
-// [head, end) at x12 / ext12
+// balm_evaluate, balm_rig_evaluate and balm_pose_graph_evaluate after their checks: H (dense, expanded from blocks), g
+// and the residual of voxels [head, end) (or the pose terms' cost) at x12 / ext12
 static int evaluate(const Unknowns &u, const double *x12, const double *ext12, int64_t head, int64_t end,
                     bool include_fix, double *H, double *g, double *residual) {
   balm_ctx *c = u.c;
@@ -1077,71 +1092,21 @@ static int refuse_gauge_with_priors(const char *who, const PriorSet *pr, const b
   return BALM_ERR_INVALID;
 }
 
-// One LM loop's steps, supplied by its owner (damping_iter for the voxel and rig costs, balm_pose_graph_iter). Each
-// returns a BALM_* status.
-struct LmSteps {
-  cudaStream_t st;
-  const double *scal;  // the owner's device scalars: eval leaves r1 in scal[0]
-  double *h_scal;      // their pinned host mirror
-  std::function<int()> eval;                                         // H, g and r1 at the current state, enqueued
-  std::function<int(double u)> solve;                                // the damped solve for dx, enqueued
-  std::function<int()> trial;                                        // the trial state from dx, enqueued
-  std::function<int(double *r2)> trial_cost;                         // its cost; ends in the iteration's one wait
-  std::function<int(double *q1, int *not_pd, int *refined)> finish;  // the solve's outcome (collect_solve)
-  std::function<int(bool accepted)> step;                            // accept / reject bookkeeping
-  std::function<int(int it)> snapshot;                               // the state after iteration it
-};
-
-// BALM2::damping_iter's loop (bavoxel.hpp:1127-1155): per iteration evaluation (when H is stale), solve, trial state and
-// trial cost are enqueued back to back and the host waits once; a refined dx redoes the trial state and its cost.
-static int lm_run(const LmSteps &s, const balm_lm_opts *o, balm_trace *trace, int *n_iters) {
-  double u = o->u0, v = o->v0, r1 = 0, r2 = 0;
-  bool calc_hess = true;
-  for (int it = 0; it < o->max_iter; it++) {
-    if (calc_hess) {
-      TRY(s.eval());
-      CUDA_TRY(cudaMemcpyAsync(s.h_scal, s.scal, sizeof(double), cudaMemcpyDeviceToHost, s.st));
-    }
-    TRY(s.solve(u));
-    TRY(s.trial());
-    TRY(s.trial_cost(&r2));
-    double q1 = 0;
-    int not_pd = 0, refined = 0;
-    TRY(s.finish(&q1, &not_pd, &refined));
-    if (refined && !not_pd) {  // dx changed: the trial state and its cost again (rare path)
-      TRY(s.trial());
-      TRY(s.trial_cost(&r2));
-    }
-    if (calc_hess) r1 = s.h_scal[0];
-    balm_trace t;
-    bool stop;
-    const bool accepted = lm_rule(r1, r2, q1, not_pd, calc_hess, o->rel_tol, &u, &v, &t, &stop);
-    if (o->verbose)  // the reference's trace line (bavoxel.hpp:1132)
-      printf("iter%d: (%lf %lf) u: %lf v: %.1lf q: %.3lf %lf %lf\n", it, r1, r2, t.u, t.v, t.q / q1, q1, t.q);
-    TRY(s.step(accepted));
-    calc_hess = accepted || o->force_hess != 0;  // after a rejection H and g of the current state are still in place
-    if (trace) trace[it] = t;
-    TRY(s.snapshot(it));
-    if (n_iters) *n_iters = it + 1;
-    if (stop) break;
-  }
-  return BALM_OK;
-}
-
 // Clears the context's LM flags (set by damping_iter) on every exit path
 struct LmScope {
   balm_ctx *c;
   ~LmScope() { c->lm_active = false; c->defer = false; c->pending_eval = false; c->eval_same_poses = false; }
 };
 
-// balm_damping_iter and balm_rig_damping_iter after their checks (`who` prefixes the messages): LM from x12 / ext12,
-// the result written back to them, the state after every iteration to per_iter
+// balm_damping_iter, balm_rig_damping_iter and balm_pose_graph_iter after their checks (`who` prefixes the messages):
+// LM from x12 / ext12, the result written back to them, the state after every iteration to per_iter
 static int damping_iter(const Unknowns &u, const char *who, double *x12, double *ext12, const balm_lm_opts *o,
                         balm_trace *trace, int *n_iters, double *per_iter) {
   balm_ctx *c = u.c;
-  // A rig's evaluations stay the pure function balm_rig_evaluate is: no per-voxel stats handed over from the trial
-  // residual pass and no tensor scale speculation (lm_active and eval_same_poses stay false).
-  const bool carry_over = !u.rig;
+  // A rig's and the pose terms' evaluations stay the pure functions balm_rig_evaluate and balm_pose_graph_evaluate
+  // are: no per-voxel stats handed over from the trial residual pass and no tensor scale speculation (lm_active and
+  // eval_same_poses stay false).
+  const bool carry_over = !u.rig && !u.pose_terms;
   // Re-anchoring a rig to base pose 0 would move the result off its fixed base poses.
   const bool bases_fixed = u.rig && rig_any_base_fixed(u.rig);
   if ((o->gauge_mode == 0 || o->gauge_mode == 1) && bases_fixed) {
@@ -1176,7 +1141,6 @@ static int damping_iter(const Unknowns &u, const char *who, double *x12, double 
   const bool hand_over = carry_over && c->stats_trial != nullptr && (c->fix == nullptr || o->hess_includes_fix != 0);
   bool stats_cached = false;
   bool same_poses = false;  // the last step was rejected: c->poses are those of the previous evaluation
-  bool evaluated = false;   // this iteration evaluated: its events are to be read
   if (carry_over) tensor_syrk_new_problem(c);  // nothing speculative is carried over from earlier calls
   LmScope lm_scope{c};
   c->lm_active = carry_over;
@@ -1185,27 +1149,36 @@ static int damping_iter(const Unknowns &u, const char *who, double *x12, double 
   const DenseSystem sys = u.system();
   SparseSolver *sp = u.solver();
   const int ns = u.n_state();
-  LmSteps s{c->stream, c->scal, c->h_scal};
-  s.eval = [&]() -> int {
-    evaluated = true;
-    c->eval_same_poses = carry_over && same_poses;
-    const int rc = u.eval(o->hess_includes_fix != 0, 0, c->M, stats_cached);
-    c->eval_same_poses = false;
-    return rc;
-  };
-  s.solve = [&](double uu) -> int {
+  // BALM2::damping_iter's loop (bavoxel.hpp:1127-1155): per iteration evaluation (when H is stale), solve, trial state
+  // and trial cost are enqueued back to back and the host waits once; a refined dx redoes the trial state and its cost.
+  double uu = o->u0, v = o->v0, r1 = 0, r2 = 0;
+  bool calc_hess = true;
+  for (int it = 0; it < o->max_iter; it++) {
+    if (calc_hess) {
+      c->eval_same_poses = carry_over && same_poses;
+      const int rc = u.eval(o->hess_includes_fix != 0, 0, c->M, stats_cached);
+      c->eval_same_poses = false;
+      TRY(rc);
+      CUDA_TRY(cudaMemcpyAsync(c->h_scal, c->scal, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+    }
     TRY(solve_dev(c, sys, sp, uu));
     if (!c->defer) CUDA_TRY(cudaStreamSynchronize(c->stream));
-    return BALM_OK;
-  };
-  s.trial = [&u]() { return u.trial(); };
-  s.trial_cost = [&](double *r2) { return residual_dev(c, c->poses_trial, r2, hand_over); };
-  s.finish = [&](double *q1, int *not_pd, int *refined) -> int {
-    if (evaluated) TRY(u.collect());
-    evaluated = false;
-    return collect_solve(c, sys, sp, q1, not_pd, refined);
-  };
-  s.step = [&](bool accepted) -> int {
+    TRY(u.trial());
+    TRY(u.trial_cost(hand_over, &r2));
+    if (calc_hess) TRY(u.collect());  // the evaluation's events, read after the trial cost's wait
+    double q1 = 0;
+    int not_pd = 0, refined = 0;
+    TRY(collect_solve(c, sys, sp, &q1, &not_pd, &refined));
+    if (refined && !not_pd) {  // dx changed: the trial state and its cost again (rare path)
+      TRY(u.trial());
+      TRY(u.trial_cost(hand_over, &r2));
+    }
+    if (calc_hess) r1 = c->h_scal[0];
+    balm_trace t;
+    bool stop;
+    const bool accepted = lm_rule(r1, r2, q1, not_pd, calc_hess, o->rel_tol, &uu, &v, &t, &stop);
+    if (o->verbose)  // the reference's trace line (bavoxel.hpp:1132)
+      printf("iter%d: (%lf %lf) u: %lf v: %.1lf q: %.3lf %lf %lf\n", it, r1, r2, t.u, t.v, t.q / q1, q1, t.q);
     if (accepted) {
       u.accept();
       if (hand_over) {
@@ -1217,15 +1190,14 @@ static int damping_iter(const Unknowns &u, const char *who, double *x12, double 
       stats_cached = carry_over && c->stats_trial != nullptr;  // c->stats still describes c->poses (single batch)
     }
     same_poses = !accepted;
-    return BALM_OK;
-  };
-  s.snapshot = [&](int it) -> int {
+    calc_hess = accepted || o->force_hess != 0;  // after a rejection H and g of the current state are still in place
+    if (trace) trace[it] = t;
     if (per_iter)
       CUDA_TRY(cudaMemcpyAsync(per_iter + (size_t)it * 12 * ns, u.state(), sizeof(double) * 12 * ns,
                                cudaMemcpyDeviceToHost, c->stream));
-    return BALM_OK;
-  };
-  TRY(lm_run(s, o, trace, n_iters));
+    if (n_iters) *n_iters = it + 1;
+    if (stop) break;
+  }
   if (o->gauge_mode == 0 || o->gauge_mode == 1) TRY(u.gauge(o->gauge_mode));
   TRY(u.download(x12, ext12));
   CUDA_TRY(cudaStreamSynchronize(c->stream));
@@ -1373,16 +1345,7 @@ extern "C" int balm_pose_graph_evaluate(balm_ctx *c, const double *poses12, doub
   if (!c || !poses12) { balm_set_error("balm_pose_graph_evaluate: bad arguments"); return BALM_ERR_INVALID; }
   TRY(refuse_blocks(c, "balm_pose_graph_evaluate"));
   if (!c->pg) { balm_set_error("balm_pose_graph_evaluate: no pose factors registered"); return BALM_ERR_INVALID; }
-  CUDA_TRY(cudaSetDevice(c->device));
-  CUDA_TRY(cudaMemcpyAsync(c->poses, poses12, sizeof(double) * 12 * c->N, cudaMemcpyHostToDevice, c->stream));
-  TRY(pose_graph_eval(c, c->poses));
-  const size_t n = c->n;
-  if (H) CUDA_TRY(cudaMemcpyAsync(H, c->H, sizeof(double) * n * n, cudaMemcpyDeviceToHost, c->stream));
-  if (g) CUDA_TRY(cudaMemcpyAsync(g, c->g, sizeof(double) * n, cudaMemcpyDeviceToHost, c->stream));
-  CUDA_TRY(cudaMemcpyAsync(c->h_scal, c->scal, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
-  CUDA_TRY(cudaStreamSynchronize(c->stream));
-  if (cost) *cost = c->h_scal[0];
-  return BALM_OK;
+  return evaluate(Unknowns{c, nullptr, true}, poses12, nullptr, 0, 0, false, H, g, cost);
 }
 
 extern "C" int balm_pose_graph_iter(balm_ctx *c, double *poses12, const balm_lm_opts *o, balm_trace *trace, int *n_iters,
@@ -1394,38 +1357,11 @@ extern "C" int balm_pose_graph_iter(balm_ctx *c, double *poses12, const balm_lm_
   if (!c->pg) { balm_set_error("balm_pose_graph_iter: no pose factors registered"); return BALM_ERR_INVALID; }
   TRY(refuse_gauge_with_priors("balm_pose_graph_iter", c->pr, o));
   CUDA_TRY(cudaSetDevice(c->device));
-  const size_t pbytes = sizeof(double) * 12 * c->N;
-  CUDA_TRY(cudaMemcpyAsync(c->poses, poses12, pbytes, cudaMemcpyHostToDevice, c->stream));
-  const DenseSystem sys = ctx_system(c);
-  LmSteps s{c->stream, c->scal, c->h_scal};
-  s.eval = [c]() { return pose_graph_eval(c, c->poses); };
-  s.solve = [c, &sys](double u) { return solve_dev(c, sys, nullptr, u); };
-  s.trial = [c]() { return launch_pose_update(c, c->poses, c->dx, c->poses_trial); };
-  s.trial_cost = [c](double *r2) -> int {  // the factors', then the priors' cost -> scal[2]
-    TRY(pose_graph_cost(c->pg, c->stream, c->poses_trial, c->scal + 2, &c->launches));
-    if (c->pr) TRY(prior_add_cost(c->pr, c->stream, c->poses_trial, c->scal + 2, &c->launches));
-    CUDA_TRY(cudaMemcpyAsync(c->h_scal + 2, c->scal + 2, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
-    CUDA_TRY(cudaStreamSynchronize(c->stream));
-    *r2 = c->h_scal[2];
-    return BALM_OK;
-  };
-  s.finish = [c, &sys](double *q1, int *not_pd, int *refined) {
-    return collect_solve(c, sys, nullptr, q1, not_pd, refined);
-  };
-  s.step = [c](bool accepted) {
-    if (accepted) std::swap(c->poses, c->poses_trial);
-    return BALM_OK;
-  };
-  s.snapshot = [&](int it) -> int {
-    if (poses_per_iter)
-      CUDA_TRY(cudaMemcpyAsync(poses_per_iter + (size_t)it * 12 * c->N, c->poses, pbytes, cudaMemcpyDeviceToHost, c->stream));
-    return BALM_OK;
-  };
-  TRY(lm_run(s, o, trace, n_iters));
-  if (o->gauge_mode == 0 || o->gauge_mode == 1) TRY(launch_gauge(c, c->poses, o->gauge_mode));
-  CUDA_TRY(cudaMemcpyAsync(poses12, c->poses, pbytes, cudaMemcpyDeviceToHost, c->stream));
-  CUDA_TRY(cudaStreamSynchronize(c->stream));
-  return BALM_OK;
+  balm_lm_opts lo = *o;
+  lo.min_planes_per_pose = 0;  // no voxels
+  lo.hess_includes_fix = 0;
+  return damping_iter(Unknowns{c, nullptr, true}, "balm_pose_graph_iter", poses12, nullptr, &lo, trace, n_iters,
+                      poses_per_iter);
 }
 
 // ---------------- covariances at a state (covariance.cu, pose_graph_sparse.cu) ----------------

@@ -283,8 +283,8 @@ __device__ __forceinline__ void loss_rho(int kind, double c, double s, double *r
   }
 }
 
-// The accept rule of BALM2::damping_iter (bavoxel.hpp:1127-1155), on the host (lm_run, balm_api.cu) and per problem on
-// the device (batch_lm_kernel): q = r1 - r2 (-1 for an unusable step, not_pd or a non-finite r2, which is then
+// The accept rule of BALM2::damping_iter (bavoxel.hpp:1127-1155), on the host (damping_iter, balm_api.cu) and per
+// problem on the device (batch_lm_kernel): q = r1 - r2 (-1 for an unusable step, not_pd or a non-finite r2, which is then
 // rejected); on acceptance (q > 0) u *= max(1/3, 1 - (2 rho - 1)^3) with rho = q / q1 and v = 2, else u *= v and
 // v *= 2. *t receives the iteration's trace record and *stop the rel_tol exit; returns whether the step is accepted.
 // pow is the C library's on the host and CUDA's on the device, as in the reference and the batch respectively.
@@ -883,7 +883,6 @@ int cov_sandwich(balm_ctx *c, const DenseSystem &s, double *B);
 // rows and columns [a0, a0 + 6) of the n x n matrix A set to 0, its diagonal there to diag (enqueued)
 int cov_delete_block(balm_ctx *c, double *A, int n, int a0, double diag);
 int launch_pose_update(balm_ctx *c, const double *poses_in, const double *dx, double *poses_out);
-int launch_gauge(balm_ctx *c, double *poses, int mode);
 // snap: 12 doubles of device scratch for pose 0
 int launch_gauge(cudaStream_t st, int N, double *poses, double *snap, int mode);
 // q1 = 1/2 x.(u D x - g) -> scal[1], u = *u_dev

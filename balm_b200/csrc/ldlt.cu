@@ -877,11 +877,6 @@ int launch_gauge(cudaStream_t st, int N, double *poses, double *snap, int mode) 
   return BALM_OK;
 }
 
-int launch_gauge(balm_ctx *c, double *poses, int mode) {
-  c->launches += 1;
-  return launch_gauge(c->stream, c->N, poses, c->scal + 4, mode);  // snapshot pose 0 into scal[4..15]
-}
-
 int launch_q1(cudaStream_t st, const double *x, const double *g, const double *dvec, int n, const double *u_dev,
               double *scal) {
   q1_kernel<<<1, 1024, 0, st>>>(x, g, dvec, n, u_dev, scal);
