@@ -60,6 +60,7 @@ SYMBOLS = ["balm_last_error", "balm_version", "balm_create", "balm_destroy", "ba
            "balm_spg_evaluate", "balm_spg_iter", "balm_spg_covariance", "balm_block_structure", "balm_download_blocks",
            "balm_block_covariance", "balm_block_set_factors", "balm_set_factor_loss", "balm_factor_residuals",
            "balm_spg_set_factor_loss", "balm_spg_factor_residuals", "balm_set_pose_priors", "balm_prior_residuals",
+           "balm_set_joint_cost",
            "balm_spg_set_pose_priors", "balm_spg_prior_residuals", "balm_set_voxel_loss", "balm_voxel_residuals",
            "balm_batch_set_voxel_loss", "balm_batch_voxel_residuals",
            "balm_set_rig", "balm_rig_evaluate", "balm_rig_damping_iter", "balm_rig_covariance",
@@ -168,6 +169,7 @@ def lib():
         L.balm_spg_factor_residuals.argtypes = [C.c_void_p] + [C.c_void_p] * 3
         L.balm_set_pose_priors.argtypes = [C.c_void_p, C.c_int] + [C.c_void_p] * 7
         L.balm_prior_residuals.argtypes = [C.c_void_p] + [C.c_void_p] * 3
+        L.balm_set_joint_cost.argtypes = [C.c_void_p, C.c_int]
         L.balm_spg_set_pose_priors.argtypes = [C.c_void_p, C.c_int] + [C.c_void_p] * 7
         L.balm_spg_prior_residuals.argtypes = [C.c_void_p] + [C.c_void_p] * 3
         L.balm_set_voxel_loss.argtypes = [C.c_void_p, C.c_int, C.c_double]

@@ -347,10 +347,10 @@ class Context:
         """Absolute pose priors (include/balm_b200.h, balm_set_pose_priors): list of dict(pose, pose_hat (12), H (6 x 6,
         (rotation, translation) order, positive semi-definite), optional lever_arm (3, body frame)), e.g. from
         pose_priors / position_priors. Prior cost 1/2 rho(e^T H e) with e = (Log(R R^^T), R l + p - p^). They join the
-        pose-graph cost (pose_graph_evaluate / pose_graph_iter), and on PREC_BLOCKS contexts every evaluation over all
-        voxels, damping_iter and block_covariance. With an active prior pass gauge_mode=2 and use anchor=-1. kind / scale
-        as set_factor_loss'. [] detaches; the set survives factor and voxel registrations. -> per prior OK or ERR_NOT_PD
-        (left out of the cost)."""
+        pose-graph cost (pose_graph_evaluate / pose_graph_iter), and on PREC_BLOCKS contexts, or FP64 / TENSOR ones with
+        set_joint_cost on, every evaluation over all voxels, damping_iter, the rig calls and the covariances. With an
+        active prior pass gauge_mode=2 and use anchor=-1. kind / scale as set_factor_loss'. [] detaches; the set survives
+        factor and voxel registrations. -> per prior OK or ERR_NOT_PD (left out of the cost)."""
         status = _set_pose_priors(L.lib().balm_set_pose_priors, self._h, self.N, priors, kind, scale)
         self._n_priors = len(status)
         return status
@@ -358,6 +358,16 @@ class Context:
     def prior_residuals(self, poses12):
         """-> (s, w): s_q = e^T H_q e and w_q = rho'(s_q) of every registered prior at poses12 (0, 0 for NOT_PD ones)."""
         return _factor_residuals(L.lib().balm_prior_residuals, self._h, self._n_priors, poses12)
+
+    def set_joint_cost(self, on=True):
+        """FP64 / TENSOR contexts: with on, the registered pose factors (set_pose_factors, with set_factor_loss) and
+        priors (set_pose_priors) join every evaluation over all voxels, as on PREC_BLOCKS contexts (include/balm_b200.h,
+        balm_set_joint_cost): evaluate (head 0, end M), residual, damping_iter, the rig calls and pose_covariance (H only;
+        the raw term stays voxels only), summed as voxels, then factors, then priors. A sub-range evaluation stays voxels
+        only. Odometry then carries scans that see no plane (pass min_planes_per_pose=0), and GNSS priors fix the frame
+        (pass gauge_mode=2). The switch survives every registration of voxels, factors and priors; on=False restores the
+        voxel cost bitwise. Refused on PREC_BLOCKS contexts and with a communicator attached."""
+        L.check(L.lib().balm_set_joint_cost(self._h, int(bool(on))))
 
     def solve(self, u):
         dx = np.zeros(self.n)
@@ -368,6 +378,9 @@ class Context:
 
     def damping_iter(self, poses12, max_iter=10, u0=0.01, v0=2.0, rel_tol=1e-6, hess_includes_fix=False,
                      gauge_mode=0, min_planes_per_pose=20, verbose=False, want_per_iter=False, force_hess=False):
+        """LM from poses12 -> (poses, trace, per-iteration poses or None). On PREC_BLOCKS contexts, and on FP64 / TENSOR
+        ones with set_joint_cost on, the cost holds the pose factors and priors; with an active prior gauge_mode 0 and 1
+        are refused (pass 2). min_planes_per_pose counts voxels only: pass 0 when factors carry plane-poor scans."""
         poses = np.array(poses12, dtype=np.float64, order="C", copy=True)
         opts, trace, n_it, per_iter = _lm_args(self.N, want_per_iter, max_iter, u0, v0, rel_tol, hess_includes_fix,
                                                gauge_mode, min_planes_per_pose, verbose, force_hess)
@@ -457,7 +470,8 @@ class Context:
                          gauge_mode=0, min_planes_per_pose=20, verbose=False, want_per_iter=False, force_hess=False):
         """damping_iter's LM on the rig's unknowns -> (base12, ext12, trace) and, with want_per_iter, the accepted
         (base12, ext12) after every iteration as a fourth item. gauge_mode 0 / 1 re-anchor the base poses to base 0
-        (refused while a base pose is fixed: pass 2)."""
+        (refused while a base pose is fixed: pass 2). With set_joint_cost on (or a set_block_rig rig) the pose factors
+        and priors act at the composed scan poses, and an active prior also refuses gauge_mode 0 and 1."""
         base12, ext12, _ = self._rig_shapes(base12, ext12)
         B, nl = len(base12), len(ext12)
         opts, trace, n_it, per_iter = _lm_args(B + nl, want_per_iter, max_iter, u0, v0, rel_tol, hess_includes_fix,
@@ -543,7 +557,9 @@ class Context:
 
     def pose_covariance(self, poses12, point_noise=0.0, c_cov=None, include_fix=False, want_raw=True, want_cov=True):
         """left_jacobian_point / multi_second / H^-1 Rcov H^-T (BAs_left.hpp:342-473, 995-1023, 1089-1096).
-        -> (Rcov_raw, Rcov); c_cov: K x 9 x 9 per-observation cluster covariances, or None for isotropic point noise."""
+        -> (Rcov_raw, Rcov); c_cov: K x 9 x 9 per-observation cluster covariances, or None for isotropic point noise.
+        With set_joint_cost on, H is the joint H of voxels, pose factors and priors (priors can fix the gauge without fix
+        clusters); Rcov_raw stays the voxels' term."""
         poses12 = np.ascontiguousarray(poses12, dtype=np.float64)
         cc = None if c_cov is None else np.ascontiguousarray(c_cov, dtype=np.float64).reshape(-1, 81)
         raw = np.zeros((self.n, self.n), order="F") if want_raw else None
@@ -556,7 +572,9 @@ class Context:
     def set_pose_factors(self, factors):
         """Window factors (include/balm_b200.h, balm_set_pose_factors): list of dict(poses = N_f distinct global pose
         indices, poses_hat = N_f x 12 refined window poses, H = (6 N_f)^2 window BA Hessian). Replaces the previous factor
-        set; a rejected call keeps it. -> per factor OK or ERR_NOT_PD (left out of the cost)."""
+        set; a rejected call keeps it. They make the pose-graph cost, and with set_joint_cost on they also join the voxel
+        cost (H in its units: points x m^2, as odometry_factors gives). -> per factor OK or ERR_NOT_PD (left out of the
+        cost)."""
         status = _set_pose_factors(L.lib().balm_set_pose_factors, self._h, factors)
         self._n_factors = len(status)
         return status

@@ -257,6 +257,7 @@ extern "C" int balm_destroy(balm_ctx *c) {
   cudaFree(c->vox_key); cudaFree(c->vox_layer); cudaFree(c->res_part); cudaFree(c->planes);
   ldlt_work_free(&c->lw);
   cudaFree(c->Hpack);
+  cudaFree(c->joint_fg);
   cudaFree(c->tc_trace);
   cudaFreeHost(c->h_scal); cudaFreeHost(c->h_flags);
   for (auto &e : c->ev) if (e) cudaEventDestroy(e);
@@ -648,6 +649,10 @@ static int allreduce_sum(balm_ctx *c, double *buf, size_t count) {
   return BALM_OK;
 }
 
+// The registered pose factors and priors join the full-range voxel cost: always on a blocks context, on a dense one
+// while balm_set_joint_cost is on. The sum is voxels, then factors, then priors.
+static bool pose_terms_in_cost(const balm_ctx *c) { return c->prec == BALM_PREC_BLOCKS || c->joint_cost; }
+
 // H, g, r of voxels [head,end) at device poses `poses`; result in c->H | c->g | c->scal[0] (all-reduced).
 // stats_cached: c->stats already holds the per-voxel eigen data of exactly these poses (left there by the residual
 // pass of an accepted LM step, or by the evaluation before a rejected one) and c->scal[BALM_SCAL_RCUR] this rank's residual.
@@ -663,9 +668,10 @@ static int evaluate_dev(balm_ctx *c, const double *poses, int64_t head, int64_t 
   // pose graph) defers too: its full range is the factors and priors.
   const bool deferred = c->defer && head == 0 && end == c->M && c->VB >= c->M &&
                         (end > head || c->prec == BALM_PREC_BLOCKS);
-  // a blocks context's pose factors are part of every full-range evaluation (sub-ranges stay voxels only)
-  const bool factors = c->prec == BALM_PREC_BLOCKS && c->pg && head == 0 && end == c->M;
-  const bool priors = c->prec == BALM_PREC_BLOCKS && c->pr && head == 0 && end == c->M;  // so are its pose priors
+  // the pose factors of a blocks context, or of a dense one with the joint cost, are part of every full-range evaluation
+  // (sub-ranges stay voxels only)
+  const bool factors = pose_terms_in_cost(c) && c->pg && head == 0 && end == c->M;
+  const bool priors = pose_terms_in_cost(c) && c->pr && head == 0 && end == c->M;  // so are its pose priors
   c->pending_stats_cached = stats_cached;
   if (head == end) {  // empty range (or an empty shard): this rank contributes H = 0, g = 0, r = 0 -- and still enters
     // the all-reduce below, which the other ranks of a multi-GPU job are waiting in
@@ -708,10 +714,13 @@ static int evaluate_dev(balm_ctx *c, const double *poses, int64_t head, int64_t 
   if (end > head)  // local, pre all-reduce; the hand-over needs every voxel, so an empty range hands nothing over
     CUDA_TRY(cudaMemcpyAsync(c->scal + BALM_SCAL_RCUR, r_dev, sizeof(double), cudaMemcpyDeviceToDevice, c->stream));
   CUDA_TRY(cudaEventRecord(c->ev[4], c->stream));
-  if (end > head || factors || priors) {
-    if (c->prec != BALM_PREC_BLOCKS) TRY(launch_assemble(c));
-    if (factors) TRY(blocks_add_factors(c, poses));  // after the RCUR copy above: the hand-over caches voxels only
+  if (end > head && c->prec != BALM_PREC_BLOCKS) TRY(launch_assemble(c));
+  if (c->prec == BALM_PREC_BLOCKS) {  // after the RCUR copy above: the hand-over caches voxels only
+    if (factors) TRY(blocks_add_factors(c, poses));
     if (priors) TRY(blocks_add_priors(c, poses));
+  } else {
+    if (factors) TRY(joint_add_factors(c, poses));
+    if (priors) TRY(prior_add_dense(c->pr, c->stream, poses, c->H, c->n, c->g, r_dev, &c->launches));
   }
   CUDA_TRY(cudaEventRecord(c->ev[5], c->stream));
   if (c->world > 1 && c->comm) {  // the assembly wrote the lower triangle | g into c->Hpack (an empty range: zeros)
@@ -763,8 +772,11 @@ static int residual_dev(balm_ctx *c, const double *poses, double *host_out, bool
   CUDA_TRY(cudaMemsetAsync(r_dev, 0, sizeof(double), c->stream));
   TRY(launch_voxel_stats(c, poses, 0, c->M, keep_stats ? c->stats_trial : nullptr, true, r_dev));
   CUDA_TRY(cudaMemcpyAsync(c->scal + BALM_SCAL_RTRIAL, r_dev, sizeof(double), cudaMemcpyDeviceToDevice, c->stream));  // local, pre all-reduce
-  if (c->prec == BALM_PREC_BLOCKS && c->pg) TRY(blocks_add_factor_cost(c, poses, r_dev));  // after RTRIAL: voxels only
-  if (c->prec == BALM_PREC_BLOCKS && c->pr) TRY(prior_add_cost(c->pr, c->stream, poses, r_dev, &c->launches));
+  if (pose_terms_in_cost(c) && c->pg) {  // after RTRIAL: voxels only
+    if (c->prec == BALM_PREC_BLOCKS) TRY(blocks_add_factor_cost(c, poses, r_dev));
+    else TRY(joint_add_factor_cost(c, poses, r_dev));
+  }
+  if (pose_terms_in_cost(c) && c->pr) TRY(prior_add_cost(c->pr, c->stream, poses, r_dev, &c->launches));
   TRY(allreduce_sum(c, r_dev, 1));
   CUDA_TRY(cudaEventRecord(c->ev[8], c->stream));
   CUDA_TRY(cudaMemcpyAsync(c->h_scal + 2, r_dev, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
@@ -1105,7 +1117,8 @@ static int damping_iter(const Unknowns &u, const char *who, double *x12, double 
   balm_ctx *c = u.c;
   // A rig's and the pose terms' evaluations stay the pure functions balm_rig_evaluate and balm_pose_graph_evaluate
   // are: no per-voxel stats handed over from the trial residual pass and no tensor scale speculation (lm_active and
-  // eval_same_poses stay false).
+  // eval_same_poses stay false). A joint cost (balm_set_joint_cost) keeps them: its terms are added after the voxel sums
+  // and the RCUR / RTRIAL copies, and read no observation.
   const bool carry_over = !u.rig && !u.pose_terms;
   // Re-anchoring a rig to base pose 0 would move the result off its fixed base poses.
   const bool bases_fixed = u.rig && rig_any_base_fixed(u.rig);
@@ -1114,7 +1127,7 @@ static int damping_iter(const Unknowns &u, const char *who, double *x12, double 
                    " re-anchors to base pose 0, which moves the result off the fixed base poses; pass gauge_mode 2");
     return BALM_ERR_INVALID;
   }
-  if (c->prec == BALM_PREC_BLOCKS) TRY(refuse_gauge_with_priors(who, c->pr, o));
+  if (pose_terms_in_cost(c)) TRY(refuse_gauge_with_priors(who, c->pr, o));
   if (o->min_planes_per_pose > 0) {  // bavoxel.hpp:1071-1085 (the shim reproduces the printf + exit(0)); per scan slot
     // The guard is on the GLOBAL count of voxels seeing each pose. With several ranks every rank all-reduces the
     // per-pose histogram of its shard first, so all ranks take the same branch (a rank returning alone would leave
@@ -1717,6 +1730,22 @@ extern "C" int balm_prior_residuals(balm_ctx *c, const double *poses12, double *
   return set_residuals(c, &balm_ctx::pr, "balm_prior_residuals", "pose priors", poses12, s, w);
 }
 
+extern "C" int balm_set_joint_cost(balm_ctx *c, int on) {
+  const char *who = "balm_set_joint_cost";
+  if (!c) { balm_set_error(std::string(who) + ": bad arguments"); return BALM_ERR_INVALID; }
+  if (c->prec == BALM_PREC_BLOCKS) {
+    balm_set_error(std::string(who) + ": a BALM_PREC_BLOCKS context's voxel cost always holds its factors and priors");
+    return BALM_ERR_INVALID;
+  }
+  if (c->world > 1 || c->comm) { balm_set_error(std::string(who) + ": single-GPU contexts only"); return BALM_ERR_INVALID; }
+  if (on && !c->joint_fg) {
+    CUDA_TRY(cudaSetDevice(c->device));
+    TRY(dev_alloc(&c->joint_fg, (size_t)c->n + 1));
+  }
+  c->joint_cost = on != 0;
+  return BALM_OK;
+}
+
 // ---------------- sliding window on the registered voxel set (assoc.cu) ----------------
 // A sliding-window build of the batch (batch_marginalize_build, batch_append_build, window_push_build) run as its
 // one-problem case into scratch buffers, then registered as the context's voxel set, with fix clusters when `fix` and
@@ -1906,6 +1935,10 @@ extern "C" int balm_comm_unique_id(void *out128) {
 extern "C" int balm_comm_init(balm_ctx *c, int rank, int world, const void *unique_id128) {
   if (!c || world < 1 || rank < 0 || rank >= world) { balm_set_error("balm_comm_init: bad arguments"); return BALM_ERR_INVALID; }
   TRY(refuse_blocks(c, "balm_comm_init"));
+  if (world > 1 && c->joint_cost) {
+    balm_set_error("balm_comm_init: the joint cost (balm_set_joint_cost) is single-GPU only; switch it off first");
+    return BALM_ERR_INVALID;
+  }
   c->rank = rank; c->world = world;
   if (world == 1) return BALM_OK;
   if (!unique_id128) { balm_set_error("balm_comm_init: unique id required"); return BALM_ERR_INVALID; }

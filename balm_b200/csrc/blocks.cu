@@ -202,7 +202,8 @@ __global__ void __launch_bounds__(256) raw_blocks_kernel(const int2 *pairs, cons
   }
 }
 
-// y[t] += x[t]: a blocks context's factor g and cost added onto the voxel ones (one add per entry, fixed order)
+// y[t] += x[t]: a blocks context's or a joint cost's factor g and cost added onto the voxel ones (one add per entry,
+// fixed order)
 __global__ void add_kernel(const double *x, int n, double *y) {
   const int t = blockIdx.x * blockDim.x + threadIdx.x;
   if (t < n) y[t] += x[t];
@@ -401,6 +402,22 @@ int blocks_add_factor_cost(balm_ctx *c, const double *poses, double *r) {
   if (u.factors_only) return pose_graph_cost(c->pg, c->stream, poses, r, &c->launches);  // *r holds no voxel cost
   TRY(pose_graph_cost(c->pg, c->stream, poses, u.fgc + c->n, &c->launches));
   add_kernel<<<1, 32, 0, c->stream>>>(u.fgc + c->n, 1, r);
+  c->launches += 1;
+  CUDA_TRY(cudaGetLastError());
+  return BALM_OK;
+}
+
+int joint_add_factors(balm_ctx *c, const double *poses) {
+  TRY(pose_graph_add_dense(c->pg, c->stream, poses, c->H, c->joint_fg, c->joint_fg + c->n, &c->launches));
+  add_kernel<<<(unsigned)((c->n + 1 + 255) / 256), 256, 0, c->stream>>>(c->joint_fg, c->n + 1, c->g);  // g, r = g[n]
+  c->launches += 1;
+  CUDA_TRY(cudaGetLastError());
+  return BALM_OK;
+}
+
+int joint_add_factor_cost(balm_ctx *c, const double *poses, double *r) {
+  TRY(pose_graph_cost(c->pg, c->stream, poses, c->joint_fg + c->n, &c->launches));
+  add_kernel<<<1, 32, 0, c->stream>>>(c->joint_fg + c->n, 1, r);
   c->launches += 1;
   CUDA_TRY(cudaGetLastError());
   return BALM_OK;

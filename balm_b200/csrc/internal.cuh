@@ -176,6 +176,8 @@ struct balm_ctx {
                                   // context, whose pattern holds only those of its factors and priors
   PriorSet *pr = nullptr;         // balm_set_pose_priors' priors (independent of the factor and the voxel set): part of
                                   // the pose-graph cost, and on BALM_PREC_BLOCKS of every full-range evaluation
+  bool joint_cost = false;        // balm_set_joint_cost (FP64 / TENSOR): pg and pr join every full-range evaluation
+  double *joint_fg = nullptr;     // [n + 1] the joint cost's factor g | cost, before they are added onto c->g | r
   int vloss_kind = BALM_LOSS_TRIVIAL;  // balm_set_voxel_loss: the loss of every voxel (independent of the voxel set)
   double vloss_scale = 1.0;
   Rig *rig = nullptr;             // balm_set_rig's rig (independent of the voxel set: N is fixed at creation)
@@ -917,6 +919,10 @@ int pose_graph_eval_blocks(const PoseGraph *p, cudaStream_t st, const double *po
 // g [6P] and the cost into *cost
 int pose_graph_add_blocks(const PoseGraph *p, cudaStream_t st, const double *poses, double *blocks, const int *map,
                           double *g, double *cost, long long *launches);
+// The factor term on an evaluated dense H (6P x 6P, enqueued): pair (i, j)'s sum added onto H at (i, j) and at its
+// transpose, the factor g into g [6P] and the cost into *cost
+int pose_graph_add_dense(const PoseGraph *p, cudaStream_t st, const double *poses, double *H, double *g, double *cost,
+                         long long *launches);
 // the cost at the device poses into the device scalar *out (enqueued, no wait)
 int pose_graph_cost(const PoseGraph *p, cudaStream_t st, const double *poses, double *out, long long *launches);
 // the (i, j), i <= j, of every nonzero 6x6 block pair of H, ascending in (i, j)
@@ -1060,6 +1066,11 @@ int blocks_add_factor_cost(balm_ctx *c, const double *poses, double *r);
 // c->pr's blocks, g and cost at poses added onto the evaluated blocks (after the factors'), c->g and the residual
 // c->g[n] (enqueued)
 int blocks_add_priors(balm_ctx *c, const double *poses);
+// An FP64 / TENSOR context's joint cost (balm_set_joint_cost): c->pg's H added onto the evaluated dense c->H, its g and
+// cost through c->joint_fg onto c->g and the residual c->g[n] (enqueued)
+int joint_add_factors(balm_ctx *c, const double *poses);
+// c->pg's cost at poses through c->joint_fg onto the device scalar *r (enqueued)
+int joint_add_factor_cost(balm_ctx *c, const double *poses, double *r);
 // the blocks of voxels [head, end) from c->G (the per-observation store) and the accumulators, g from the accumulators
 int launch_blocks(balm_ctx *c, int64_t head, int64_t end);
 // the blocks and c->g | r zeroed before an evaluation without voxel term (nothing when the pattern is the factor pairs

@@ -8,7 +8,8 @@
 //   pg_linearise_kernel  per active factor, one CTA: e_k, J_k (shared), M = E^T H~ E and b = E^T H~ e -> staging
 //   pg_assemble_kernel   per (global 6x6 block pair i <= j, entry): the pair's (factor, slot, slot) terms in factor order
 //                        -> H (i, j) and (j, i) from one sum; per gradient entry: the pose's slots in factor order -> g
-//                        (outputs: dense H, or a blocks context's blocks: stored, or added onto its voxel blocks)
+//                        (outputs: dense H, stored or added onto the voxel H of a joint cost, or a blocks context's
+//                        blocks: stored, or added onto its voxel blocks)
 //   pg_cost_kernel       per active factor, one CTA: cost_f
 //   pg_sum_kernel        one CTA: the factors' costs in factor order -> a device scalar
 // Absolute pose priors (DESIGN.md "Absolute pose priors"; PriorSet, balm_set_pose_priors): prior_cost_kernel and
@@ -250,7 +251,8 @@ __global__ void __launch_bounds__(PG_THREADS) pg_linearise_kernel(FactorView fv,
 // ---- H and g: one thread per (block pair, entry), then one per gradient entry. The pair sums go to `out`: dense H
 // (zeroed beforehand) for the context; on a BALM_PREC_BLOCKS context one 6x6 block per pair when the factor pairs are
 // its whole pattern (the sparse pose graph's usual case), else added onto its union pattern's blocks (DESIGN.md "Voxels
-// and pose factors in one cost"). ----
+// and pose factors in one cost"); with an FP64 / TENSOR context's joint cost, added onto its voxel H (DESIGN.md "Voxels,
+// factors and priors in one cost on dense contexts"). ----
 struct DenseH {  // H (6P)^2 column-major: entry (a, c6) of pair (i, j) at (6i + a, 6j + c6) and its transpose
   double *H;
   __device__ __forceinline__ void operator()(size_t n, long long p, int2 ij, int a, int c6, double s) const {
@@ -269,6 +271,13 @@ struct AddBlocks {  // a BALM_PREC_BLOCKS context's union pattern: block map[p] 
   const int *map;
   __device__ __forceinline__ void operator()(size_t, long long p, int2, int a, int c6, double s) const {
     B[36 * (size_t)map[p] + 6 * c6 + a] += s;
+  }
+};
+struct AddDenseH {  // an FP64 / TENSOR context's joint cost: DenseH's entries added onto the voxel H, one add per entry
+  double *H;
+  __device__ __forceinline__ void operator()(size_t n, long long, int2 ij, int a, int c6, double s) const {
+    H[(6 * (size_t)ij.y + c6) * n + 6 * (size_t)ij.x + a] += s;
+    if (ij.x != ij.y) H[(6 * (size_t)ij.x + a) * n + 6 * (size_t)ij.y + c6] += s;
   }
 };
 
@@ -771,6 +780,11 @@ int pose_graph_eval_blocks(const PoseGraph *p, cudaStream_t st, const double *po
 int pose_graph_add_blocks(const PoseGraph *p, cudaStream_t st, const double *poses, double *blocks, const int *map,
                           double *g, double *cost, long long *launches) {
   return pose_graph_assemble(*p, st, poses, AddBlocks{blocks, map}, g, cost, launches);
+}
+
+int pose_graph_add_dense(const PoseGraph *p, cudaStream_t st, const double *poses, double *H, double *g, double *cost,
+                         long long *launches) {
+  return pose_graph_assemble(*p, st, poses, AddDenseH{H}, g, cost, launches);
 }
 
 // ---------------- absolute pose priors ----------------

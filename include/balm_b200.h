@@ -56,7 +56,8 @@ typedef enum {
                            balm_pose_covariance, balm_set_pose_factors, balm_pose_graph_*, balm_device_views and the
                            tensor debug aids return BALM_ERR_UNSUPPORTED on such a context and change nothing;
                            balm_evaluate's H (when not NULL) is the dense matrix expanded from the blocks. Pose factors
-                           join the voxel cost through balm_block_set_factors. */
+                           join the voxel cost through balm_block_set_factors (on FP64 / TENSOR contexts through
+                           balm_set_joint_cost). */
 } balm_precision;
 
 /* Robust losses of pose factors (balm_set_factor_loss), rho of s = e~^T H~ e~ at scale c > 0 (units of sqrt(s)), and of
@@ -133,8 +134,9 @@ int balm_solve(balm_ctx *ctx, double u, double *dx, double *q1, int *not_pd);
 /* BALM2::damping_iter(x_stats, voxhess) (bavoxel.hpp:1069-1166). poses12 updated in place.
  * trace: room for opts->max_iter entries (may be NULL). poses_per_iter: max_iter*N*12 doubles or NULL,
  * receives the accepted pose set after every iteration (before the gauge step) for parity checks.
- * On a BALM_PREC_BLOCKS context with an active pose prior (balm_set_pose_priors) gauge_mode 0 and 1 are BALM_ERR_INVALID:
- * the priors fix the frame, and re-anchoring to pose 0 would move the result off them; pass 2. */
+ * On a BALM_PREC_BLOCKS context, or a dense one with the joint cost on (balm_set_joint_cost), with an active pose prior
+ * (balm_set_pose_priors) gauge_mode 0 and 1 are BALM_ERR_INVALID: the priors fix the frame, and re-anchoring to pose 0
+ * would move the result off them; pass 2. */
 int balm_damping_iter(balm_ctx *ctx, double *poses12, const balm_lm_opts *opts, balm_trace *trace, int *n_iters,
                       double *poses_per_iter);
 void balm_default_lm_opts(balm_lm_opts *opts);
@@ -447,7 +449,10 @@ int balm_batch_pose_covariance(balm_batch *b, const double *poses12, const doubl
  * (src/simulation/toolss.hpp:288,341); NULL derives it from the cluster moments for isotropic point noise of standard
  * deviation point_noise, which is exactly what PointCluster::push accumulates (toolss.hpp:311-343). include_fix: the fix
  * clusters take part in the voxel statistics and in H (BAs_left.hpp:183-185); without them H is singular (gauge) and the
- * call fails with BALM_ERR_NOT_PD when Rcov is requested. Either output (n x n, column-major, symmetric) may be NULL. */
+ * call fails with BALM_ERR_NOT_PD when Rcov is requested. Either output (n x n, column-major, symmetric) may be NULL.
+ * With the joint cost on (balm_set_joint_cost) H is the joint H of voxels, pose factors and priors, so priors can fix
+ * the gauge without fix clusters; Rcov_raw stays the voxels' term (the terms' information matrices are cost weights,
+ * not a point-noise model). */
 int balm_pose_covariance(balm_ctx *ctx, const double *poses12, const double *c_cov81, double point_noise, int include_fix,
                          double *Rcov_raw, double *Rcov);
 
@@ -462,7 +467,8 @@ int balm_pose_covariance(balm_ctx *ctx, const double *poses12, const double *c_c
  * definite (pivot test of balm_batch_pose_covariance, or a non-positive pivot); such a factor is left out of every sum.
  * BALM_ERR_INVALID (nothing registered, the previous factor set kept) for n_factors < 1, factor_ptr[0] != 0, a factor
  * with fewer than 2 or more than BALM_BATCH_MAX_POSES poses, an index outside [0, N) or repeated within a factor, or a
- * non-finite T^ / H entry. The factor set is independent of the voxel registration; it is replaced by the next call. */
+ * non-finite T^ / H entry. The factor set is independent of the voxel registration; it is replaced by the next call.
+ * With balm_set_joint_cost on, the set (with its balm_set_factor_loss) also joins the context's voxel cost. */
 int balm_set_pose_factors(balm_ctx *ctx, int n_factors, const int64_t *factor_ptr, const int32_t *factor_pose,
                           const double *poses_hat12, const double *H, int32_t *status_out);
 /* balm_evaluate's analogue for the registered factors: dense H (n x n, column-major, exactly symmetric, 6-dimensional
@@ -717,7 +723,8 @@ int balm_factor_residuals(balm_ctx *ctx, const double *poses12, double *s, doubl
  * gradient w J^T H_q e and Hessian w J^T H_q J with w = rho'(s_q), J = [[Jl^-1(e_rot), 0], [-hat(R l + p), I]] under the
  * library's left update. A position-only (GNSS) prior is H_q = blockdiag(0, Omega_p), its R^ unused; a full-pose
  * anchor is any positive definite H_q with l = 0. The priors join the pose-graph cost (balm_pose_graph_evaluate /
- * _iter) on FP64 / TENSOR contexts, and on a BALM_PREC_BLOCKS context every evaluation over the whole voxel range, as
+ * _iter) on FP64 / TENSOR contexts, and the voxel cost there while balm_set_joint_cost is on; on a BALM_PREC_BLOCKS
+ * context they join every evaluation over the whole voxel range, as
  * balm_block_set_factors' factors do (balm_evaluate, balm_residual, balm_damping_iter, balm_solve, balm_download_blocks,
  * balm_block_covariance); every sum adds voxels, then factors, then priors. A prior touches only its pose's diagonal
  * block, so a blocks context's pattern does not change.
@@ -728,8 +735,9 @@ int balm_factor_residuals(balm_ctx *ctx, const double *poses12, double *s, doubl
  * is zero; such a prior is left out of every sum. BALM_ERR_INVALID, the previous set kept, for a pose outside [0, N), a
  * non-finite T^, l, H or scale, an H not symmetric to 1e-12 of its max |entry|, a kind outside BALM_LOSS_*, or a
  * non-trivial kind without a finite scale > 0.
- * Gauge: with an active prior the cost has no gauge null space, so balm_damping_iter (blocks), balm_pose_graph_iter and
- * balm_spg_iter refuse gauge_mode 0 and 1 (BALM_ERR_INVALID: pass 2), and anchor = -1 is the natural covariance call.
+ * Gauge: with an active prior the cost has no gauge null space, so balm_damping_iter (blocks, or joint cost),
+ * balm_rig_damping_iter (joint cost or blocks), balm_pose_graph_iter and balm_spg_iter refuse gauge_mode 0 and 1
+ * (BALM_ERR_INVALID: pass 2), and anchor = -1 is the natural covariance call.
  * balm_block_structure's / balm_spg_structure's stats[3] count the set's device bytes. */
 int balm_set_pose_priors(balm_ctx *ctx, int n_priors, const int32_t *pose, const double *poses_hat12,
                          const double *lever3, const double *H36, const int32_t *kind, const double *scale,
@@ -737,6 +745,22 @@ int balm_set_pose_priors(balm_ctx *ctx, int n_priors, const int32_t *pose, const
 /* s_q and w_q = rho'(s_q) of every prior at poses12 into s and w (n_priors each; either may be NULL); NOT_PD priors
  * report 0, 0. Waits once. BALM_ERR_INVALID without a registered prior set. */
 int balm_prior_residuals(balm_ctx *ctx, const double *poses12, double *s, double *w);
+/* Voxels, pose factors and priors in one cost on an FP64 / TENSOR context (DESIGN.md "Voxels, factors and priors in one
+ * cost on dense contexts"). on != 0: the registered factor set (balm_set_pose_factors, with its balm_set_factor_loss) and
+ * prior set (balm_set_pose_priors) join every evaluation over the whole voxel range (head == 0, end == M), summed as
+ * voxels, then factors, then priors, as on a BALM_PREC_BLOCKS context: balm_evaluate, balm_residual,
+ * balm_damping_iter, balm_solve (on the last evaluation), balm_rig_evaluate, balm_rig_damping_iter and
+ * balm_rig_covariance (the terms act at the composed scan poses, before the rig reduction) and balm_pose_covariance
+ * (the terms shape H only; Rcov_raw stays voxels only). A sub-range evaluation stays voxels only, bitwise;
+ * balm_voxel_residuals and the pose-graph calls are unchanged. With an active prior balm_damping_iter and
+ * balm_rig_damping_iter refuse gauge_mode 0 and 1. min_planes_per_pose still counts voxels: pass 0 when factors carry
+ * scans that see no plane. The tensor path keeps its once-per-step observation read (the trial pass's digit planes,
+ * sweep reuse after a rejected step, the stats hand-over): the terms read no observation. on == 0 (the default)
+ * restores the voxel cost, bitwise. The switch belongs to the context: it survives every voxel registration and every
+ * replacement or detachment of the factor and prior sets. The first call with on != 0 allocates 6N + 1 doubles.
+ * BALM_ERR_INVALID, nothing changed, for a null ctx, a BALM_PREC_BLOCKS context (whose voxel cost always holds its
+ * terms) or a communicator attached; balm_comm_init with world > 1 is refused while the switch is on. */
+int balm_set_joint_cost(balm_ctx *ctx, int on);
 /* balm_set_pose_priors and balm_prior_residuals on a sparse pose graph: same arguments, checks, meaning (balm_spg_evaluate,
  * _iter and _covariance) and lifetime (the set survives balm_spg_set_factors). A prior on a pose that no active factor
  * covers adds that pose's diagonal pair to the pattern, which is then re-ordered and re-captured; only a change of the
