@@ -571,8 +571,8 @@ class Context:
     # ---- pose graph ----
     def set_pose_factors(self, factors):
         """Window factors (include/balm_b200.h, balm_set_pose_factors): list of dict(poses = N_f distinct global pose
-        indices, poses_hat = N_f x 12 refined window poses, H = (6 N_f)^2 window BA Hessian). Replaces the previous factor
-        set; a rejected call keeps it. They make the pose-graph cost, and with set_joint_cost on they also join the voxel
+        indices, poses_hat = N_f x 12 refined window poses, H = (6 N_f)^2 window BA Hessian, symmetric to 1e-12 of its
+        max |entry|). Replaces the previous factor set; a rejected call keeps it. They make the pose-graph cost, and with set_joint_cost on they also join the voxel
         cost (H in its units: points x m^2, as odometry_factors gives). -> per factor OK or ERR_NOT_PD (left out of the
         cost)."""
         status = _set_pose_factors(L.lib().balm_set_pose_factors, self._h, factors)
@@ -946,7 +946,8 @@ class PoseGraph:
             pass
 
     def set_pose_factors(self, factors):
-        """Context.set_pose_factors' factors, checks and result; also orders the poses and factors the pattern."""
+        """Context.set_pose_factors' factors (H_f symmetric to 1e-12 of its max |entry|), checks and result; also orders
+        the poses and factors the pattern."""
         status = _set_pose_factors(L.lib().balm_spg_set_factors, self._h, factors)
         self._n_factors = len(status)
         return status

@@ -1263,6 +1263,21 @@ static int pose_factors_check(const char *who, int P, int n_factors, const int64
     if (!std::isfinite(poses_hat12[e])) { balm_set_error(w + "non-finite poses_hat12"); return BALM_ERR_INVALID; }
   for (int64_t e = 0; e < hsize; e++)
     if (!std::isfinite(H[e])) { balm_set_error(w + "non-finite H"); return BALM_ERR_INVALID; }
+  // H_f symmetric to 1e-12 of its largest entry: the cost reads e^T H_f e, the gradient H_f's rows as given and the
+  // assembly one triangle, which agree only when H_f is symmetric
+  const double *Hf = H;
+  for (int f = 0; f < n_factors; f++) {
+    const int64_t n6 = 6 * (factor_ptr[f + 1] - factor_ptr[f]);
+    double hmax = 0.0;
+    for (int64_t e = 0; e < n6 * n6; e++) hmax = std::max(hmax, fabs(Hf[e]));
+    for (int64_t a = 0; a < n6; a++)
+      for (int64_t c = 0; c < a; c++)
+        if (fabs(Hf[c * n6 + a] - Hf[a * n6 + c]) > 1e-12 * hmax) {
+          balm_set_error(w + "factor " + std::to_string(f) + " has an H that is not symmetric");
+          return BALM_ERR_INVALID;
+        }
+    Hf += n6 * n6;
+  }
   return BALM_OK;
 }
 

@@ -459,15 +459,16 @@ int balm_pose_covariance(balm_ctx *ctx, const double *poses12, const double *c_c
 /* Pose graph (hierarchical BA's top-down step, DESIGN.md "Pose graph"): window factors over the ctx's N poses, each from
  * one converged BA window. Factor f has the N_f = factor_ptr[f+1] - factor_ptr[f] (2 .. BALM_BATCH_MAX_POSES) distinct
  * global pose indices factor_pose[factor_ptr[f] ..], the window's refined poses T^_k (poses_hat12, 12 doubles per slot in
- * the same order) and its BA Hessian H_f ((6 N_f)^2 doubles, column-major, as balm_batch_evaluate returns it; the factors'
- * Hessians concatenated). With c(T, T^) = (Log(R R^^T), p - R R^^T p^) and A = T_idx[0] T^_0^-1:
+ * the same order) and its BA Hessian H_f ((6 N_f)^2 doubles, column-major, symmetric, as balm_batch_evaluate returns it;
+ * the factors' Hessians concatenated). With c(T, T^) = (Log(R R^^T), p - R R^^T p^) and A = T_idx[0] T^_0^-1:
  *   e_k = c(A^-1 T_idx[k], T^_k),   cost_f = 1/2 sum_{k,l >= 1} e_k^T H_f[k,l] e_l,
  * the second-order model of the window's BA cost with slot 0 pinned; the total is the sum over factors.
  * status_out (n_factors, may be NULL): BALM_OK, or BALM_ERR_NOT_PD when H_f restricted to slots >= 1 is not positive
  * definite (pivot test of balm_batch_pose_covariance, or a non-positive pivot); such a factor is left out of every sum.
  * BALM_ERR_INVALID (nothing registered, the previous factor set kept) for n_factors < 1, factor_ptr[0] != 0, a factor
- * with fewer than 2 or more than BALM_BATCH_MAX_POSES poses, an index outside [0, N) or repeated within a factor, or a
- * non-finite T^ / H entry. The factor set is independent of the voxel registration; it is replaced by the next call.
+ * with fewer than 2 or more than BALM_BATCH_MAX_POSES poses, an index outside [0, N) or repeated within a factor, a
+ * non-finite T^ / H entry, or an H_f not symmetric to 1e-12 of its max |entry| (the cost reads its symmetric part,
+ * the gradient its rows). The factor set is independent of the voxel registration; it is replaced by the next call.
  * With balm_set_joint_cost on, the set (with its balm_set_factor_loss) also joins the context's voxel cost. */
 int balm_set_pose_factors(balm_ctx *ctx, int n_factors, const int64_t *factor_ptr, const int32_t *factor_pose,
                           const double *poses_hat12, const double *H, int32_t *status_out);
